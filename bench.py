@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- pose-hypotheses/s of the NOPE hot path on B200.
+"""bench.py -- pose-hypotheses/s of the NOPE hot path on H100.
 
 A "step" = one pass of the hot path for one query: the pose-conditioned UNet over the
 whole pose grid + l2 scoring + top-5 (BASELINE.json configs[1]: 256x256, 642-pose
@@ -14,7 +14,11 @@ all-gather of per-shard (score, index) top-k.
   cpu_baseline  the oracle (CPU port of the reference) on the host cores, bounded sample
 
 `--impl reference` times the reference's own CPU implementation of the path (the real
-reference modules when /root/reference is mounted, else the oracle port of them).
+reference modules when the reference tree is available, else the oracle port of them).
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (scores and top-5
+indices) as DIR/<name>.npy, so that two builds can be compared output for output: the inputs are
+seeded and identical from run to run.
 """
 import argparse
 import json
@@ -45,7 +49,7 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--variant", default="default", choices=["default", "ldm"],
                     help="default: template_base UNet (BASELINE configs); ldm: the LDM-variant UNetModelPose "
-                         "sweep on latents (SURVEY.md 8 f2), an additional line for profiles/")
+                         "sweep on latents (SURVEY.md 8 f2), an additional bench line")
     ap.add_argument("--conv-impl", default=os.environ.get("NOPE_CONV_IMPL", "tcgen05_2cta"),
                     choices=["tcgen05", "tcgen05_2cta"])
     ap.add_argument("--precision", default=os.environ.get("NOPE_PRECISION", "fp16"),
@@ -57,12 +61,34 @@ def parse():
                          "GPUs (10248 = level-3 grid x 4 in-plane rotations); 0 = weak scaling, --poses per GPU")
     ap.add_argument("--no-extras", action="store_true",
                     help="skip the extra legs (other precision modes, eager-cuDNN baseline, LDM variant)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64)")
     return ap.parse_args()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes {name: tensor} as out_dir/<name>.npy: floating arrays as float32, integer ones (indices) as float64
+    (exact below 2^53).  An array that would take the total past 64 MB is replaced by a fixed, seeded sample of
+    its flattened elements (the same positions in every run with the same arguments)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        a = a.astype(np.float32) if np.issubdtype(a.dtype, np.floating) else a.astype(np.float64)
+        if total + a.nbytes > DUMP_LIMIT_BYTES:
+            keep = min(a.size, max(0, (DUMP_LIMIT_BYTES - total) // a.itemsize))
+            a = a.reshape(-1)[np.sort(np.random.default_rng(0).choice(a.size, size=keep, replace=False))]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        total += a.nbytes
 
 
 # ---------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -131,7 +157,7 @@ def measured_peaks():
         d = json.load(open(p))
         return (d.get("bf16_tflops_sustained", d.get("bf16_tflops")), d.get("hbm_gbs"), "measured",
                 d.get("bf16_tflops"))
-    return 1400.0, 6650.0, "fallback", 1590.0     # B200_PROFILING.md fallback (sustained, burst)
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3), not measured", 989.0
 
 
 # ---------------------------------------------------------------------------------------
@@ -183,7 +209,7 @@ def cpu_baseline(seconds=12.0, chunk=16):
 def eager_gpu_baseline(dev, chunks=(64, 128, 256, 642), reps=2):
     """SURVEY.md 8d: the reference ships no custom kernel, so the on-box GPU baseline is the same
     module in PyTorch eager (cuDNN/cuBLAS), fp16, channels_last activations AND weights.
-    /root/reference does not exist on the GPU box: the oracle's torch restatement of UNet.forward runs
+    the reference tree is not needed on the GPU machine: the oracle's torch restatement of UNet.forward runs
     on CUDA half tensors instead.  The number of hypotheses per forward is swept and the best is
     reported.  hyp/s (UNet + l2 score only, no encoder)."""
     import torch
@@ -262,17 +288,17 @@ def workload_config(args, world):
               f"{st} UNet (fp32 accumulate / statistics), l2 score + top-5")
     return {"workload": wl, "poses_per_gpu": per, "global_poses": n_global, "queries": args.queries,
             "chunk": args.chunk, "conv_impl": args.conv_impl,
-            # engine precision of the B200 arm (the reference arm always computes fp32; its `dtype` says so)
+            # engine precision of the GPU arm (the reference arm always computes fp32; its `dtype` says so)
             "precision": f"{args.precision}: {PRECISION_NOTES[args.precision]}",
             "weights": "seeded random init, reference state_dict schema (305.8 M params)",
             "l2": "not flushed: each step streams 0.61 GB of fp16 weights and ~1.4 GB of "
-                  "activations per chunk, >> 126 MB L2",
+                  "activations per chunk, >> 50 MB L2",
             "parallelism": f"pose grid sharded {world}-way, one all-gather of packed top-k records" if world > 1 else "1 GPU"}
 
 
 def run_reference(args):
     """--impl reference: the reference's own CPU implementation of the path on the host cores (its
-    unmodified modules when /root/reference is mounted, else the oracle port of them), on the same
+    unmodified modules when the reference tree is available, else the oracle port of them), on the same
     workload config as our arm.  One step = the two encoder calls + the UNet sweep over a BOUNDED
     SAMPLE of the grid + scoring; the sample is sized from a probe so that the whole
     --steps/--warmup run ends within a few minutes.  `value` is the throughput of the FULL grid that
@@ -447,6 +473,8 @@ def main_ldm(args):
         if world > 1:
             dist.barrier()
 
+    last = {}
+
     def timed(fn, steps, warmup):
         for _ in range(warmup):
             fn()
@@ -456,7 +484,7 @@ def main_ldm(args):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            fn()
+            last["out"] = fn()
         e1.record()
         torch.cuda.synchronize()
         barrier()
@@ -473,6 +501,8 @@ def main_ldm(args):
     ms = timed(step_resident, args.steps, max(args.warmup, 3))
     launches = m.last_launch_count
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"sim": last["out"]["sim"], "topi": last["out"]["topi"]})
     ms_e2e = timed(step_e2e, args.steps, max(args.warmup, 3))
     m.profile(True)
     step_resident()
@@ -504,7 +534,7 @@ def main_ldm(args):
             "weights": "seeded random init, reference state_dict schema (395.0 M params)",
             "gflop_per_hyp": fl["total"] / 1e9,
             "encoder": "none: the diffusers VAE of this variant is not in the reference tree; inputs are latents",
-            "l2": "not flushed: each step streams 0.79 GB of fp16 weights and > 5 GB of activations, >> 126 MB L2",
+            "l2": "not flushed: each step streams 0.79 GB of fp16 weights and > 5 GB of activations, >> 50 MB L2",
         },
         "clocks": clocks,
         "e2e": {"value": Q * n / (ms_e2e * 1e-3), "unit": "hyp/s", "ms_per_step": ms_e2e,
@@ -512,13 +542,13 @@ def main_ldm(args):
                 "api": "UNetModelPose.sweep (pinned host latents + poses -> sweep -> top-5 -> host)"},
         "gpu_launches": int(launches * args.steps),
         "roofline": {
-            "bound": "tensor", "kernel": "conv_tc2_kernel (tcgen05 implicit-GEMM conv / linear layers)",
+            "bound": "tensor", "kernel": "conv_tc2_kernel (wgmma implicit-GEMM conv / linear layers)",
             "achieved": gemm_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": gemm_tf / peak_tf if peak_tf else None,
-            "peak_source": f"{peak_src} (sustained bf16 cuBLAS)", "traffic": None,
+            "peak_source": f"{peak_src} (bf16)", "traffic": None,
             "launches_per_step": gm["launches"], "gemm_ms_per_step": gm["ms"],
             "gemm_share_of_step": gm["ms"] / ms if ms else None,
             "algorithmic_tflop_per_step": gm["flops"] / 1e12,
-            "attention": {"kernel": "ldm_attn_tc_kernel (tcgen05 QK^T / PV, softmax in registers)",
+            "attention": {"kernel": "ldm_attn_tc_kernel (wgmma QK^T / PV, softmax in registers)",
                           "achieved": attn_tf, "unit": "TFLOP/s", "ms_per_step": at["ms"],
                           "launches_per_step": at["launches"], "share_of_step": at["ms"] / ms if ms else None},
             "whole_step_tflops": value * fl["total"] / 1e12,
@@ -620,6 +650,8 @@ def main():
         if world > 1:
             dist.barrier()
 
+    last = {}
+
     def timed(fn, steps, warmup):
         for _ in range(warmup):
             fn()
@@ -629,7 +661,7 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            fn()
+            last["out"] = fn()
         e1.record()
         torch.cuda.synchronize()
         barrier()
@@ -646,6 +678,9 @@ def main():
     ms = timed(step_resident, args.steps, max(args.warmup, 3))
     launches_per_step = unet.last_launch_count
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        sim, topi, _ = last["out"]
+        dump_outputs(args.dump_outputs, {"sim": sim, "topi": topi})
     ms_e2e = timed(step_e2e, args.steps, max(args.warmup, 3))
 
     # ---- BASELINE configs[3] beside the weak-scaling headline: the FIXED 10 248-pose grid (level-3 icosphere x 4
@@ -660,7 +695,7 @@ def main():
                         "ms_per_step": ms_s, "scaling": "strong"}
         del poses_s
 
-    # ---- roofline of the dominant kernel (tcgen05 convolution), CUDA events per launch
+    # ---- roofline of the dominant kernel (wgmma convolution), CUDA events per launch
     def conv_profile(u, step):
         u.profile(True)
         step()
@@ -730,23 +765,21 @@ def main():
                 "api": "PoseConditional.predict_pose (pinned host images -> encoder x2 -> sweep -> top-5 -> host)"},
         "gpu_launches": int(launches_per_step * args.steps),
         "roofline": {
-            "bound": "tensor", "kernel": "conv_tc2_kernel (tcgen05 implicit-GEMM conv, CTA pairs; GroupNorm / SiLU / "
+            "bound": "tensor", "kernel": "conv_tc2_kernel (wgmma implicit-GEMM conv, clusters of 2; GroupNorm / SiLU / "
                                          "pose bias / residual in its epilogue)",
             "achieved": conv_tf, "peak": peak_tf, "unit": "TFLOP/s",
-            "frac": conv_tf / peak_tf if peak_tf else None, "peak_source": f"{peak_src} (sustained bf16 cuBLAS)",
+            "frac": conv_tf / peak_tf if peak_tf else None, "peak_source": f"{peak_src} (bf16)",
             "peak_burst": peak_burst, "frac_of_burst": conv_tf / peak_burst if peak_burst else None,
             "executed_tflops": conv_exec_tf,
             "traffic": ncu_traffic(), "traffic_source": "profiles/roofline_traffic.json (ncu --set full, "
-            "dram__bytes_read.sum + dram__bytes_write.sum per launch, sweep convolutions)",
+            "dram__bytes_read.sum + dram__bytes_write.sum per launch, sweep convolutions), when present",
             "launches_per_step": prof["conv_launches"],
             "conv_ms_per_step": prof["conv_ms"], "conv_share_of_step": prof["conv_ms"] / ms if ms else None,
             "algorithmic_tflop_per_step": prof["conv_alg_flops"] / 1e12,
             "best_single_launch_tflops": prof["max_launch_tflops"],
             "whole_step_tflops": value * GFLOP_PER_HYP / 1e3,
             "whole_step_frac": value * GFLOP_PER_HYP / 1e3 / peak_tf if peak_tf else None,
-            "note": "the convolution kernel also normalises / activates / adds pose bias and residual in its epilogue "
-                    "(round 1 ran those as separate HBM passes and reported frac 0.87-0.90 for the bare convolution): "
-                    "compare whole_step_frac, 0.71 in round 1",
+            "note": "the convolution kernel also normalises / activates / adds pose bias and residual in its epilogue",
         },
         "modes": modes,
         "cpu_baseline": cpu,

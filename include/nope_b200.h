@@ -1,4 +1,4 @@
-/* nope_b200 -- C ABI of the B200-native NOPE inference hot path.
+/* nope_b200 -- C ABI of the H100-native NOPE inference hot path.
  *
  * The reference (nv-nguyen/nope) is pure Python/PyTorch and has no FFI of its own;
  * each entry point below names the reference function it replaces (paths relative to
@@ -41,7 +41,7 @@ typedef struct nope_unet nope_unet_t;
 /* Thread-local message of the last failing call on this thread. */
 const char* nope_last_error(void);
 
-/* Library/ABI version and the SM architecture the kernels were built for ("sm_100a"). */
+/* Library/ABI version and the SM architecture the kernels were built for ("sm_90a"). */
 int nope_abi_version(void);
 const char* nope_build_arch(void);
 
@@ -68,8 +68,8 @@ int nope_unet_load_tensor(nope_unet_t* u, const char* key, const float* data,
 int nope_unet_finalize(nope_unet_t* u);
 
 /* Tunables: hypotheses per chunk (workspace = ~5.5 MB per hypothesis), and the
- * convolution implementation: 0 = tcgen05 tensor cores, 128-pixel tiles, 1 = SIMT debug
- * twin, 2 = tcgen05 with CTA pairs (cta_group::2, 256-pixel tiles; default). */
+ * convolution implementation: 0 = wgmma tensor cores, single-CTA kernel, 1 = SIMT debug
+ * twin, 2 = wgmma, clustered kernel with the fused epilogues (default). */
 int nope_unet_set_chunk(nope_unet_t* u, int hyps_per_chunk);
 int nope_unet_set_conv_impl(nope_unet_t* u, int impl);
 /* Named options:
@@ -85,7 +85,7 @@ int nope_unet_set_conv_impl(nope_unet_t* u, int impl);
  *       convolution (Block.forward / ResnetBlock.forward, model_utils.py:237-279); 0 = separate
  *       gn_apply pass (round-1 schedule; also what conv_impl 0 / 1 use);
  *   "conv_impl": as nope_unet_set_conv_impl;
- *   "attn_impl": LinearAttention core, 0 = tcgen05 kernel at 32x32 / 16x16 (CUDA cores below 128 tokens),
+ *   "attn_impl": LinearAttention core, 0 = wgmma kernel at 32x32 / 16x16 (CUDA cores below 128 tokens),
  *       1 = CUDA-core kernel everywhere. */
 int nope_unet_set_option(nope_unet_t* u, const char* name, int value);
 int nope_unet_get_option(const nope_unet_t* u, const char* name, int* value);
@@ -138,7 +138,7 @@ int nope_unet_profile_read(nope_unet_t* u, double* conv_ms, double* conv_flops, 
  * FeatureExtractor.encode_image (src/model/encoder/template.py:47-53): ResNet-50 without
  * max-pool and with layer4 at stride 1 (src/model/encoder/resnet.py:93-152), eval-mode
  * BatchNorm folded into the convolutions, projector ReLU-1x1-ReLU-1x1, normalize=False.
- * Runs on the tcgen05 convolution kernel with split-precision (fp16 hi+lo) operands, so the
+ * Runs on the wgmma convolution kernel with split-precision (fp16 hi+lo) operands, so the
  * latents match the reference's fp32 path to 5e-5 rel-L2 (measured; tests assert 1.5e-4;
  * cuDNN TF32 / fp16 are 2-3e-3 off).  Keys are the reference's
  * `backbone.*` / `projector.*` names (HOST fp32 pointers, shape-checked); 256x256 inputs. */
@@ -209,7 +209,7 @@ int nope_op_groupnorm(const float* x, const float* gamma, const float* beta, int
                       const float* chan_bias, const float* residual, float* out, int n_img,
                       int C, int H, int W, void* stream);
 /* LinearAttention core on qkv [n, 384, H, W] -> [n, 128, H, W] (model_utils.py:403-417).
- * impl 0: tcgen05 kernel (both contractions on tensor cores, H*W a multiple of 128), 1: CUDA cores. */
+ * impl 0: wgmma kernel (both contractions on tensor cores, H*W a multiple of 128), 1: CUDA cores. */
 int nope_op_linear_attention(int impl, const float* qkv, float* out, int n_img, int H, int W, void* stream);
 /* Attention core on qkv [n, 384, H, W] -> [n, 128, H, W], H*W <= 32 (model_utils.py:376-388) */
 int nope_op_attention(const float* qkv, float* out, int n_img, int H, int W, void* stream);
@@ -225,7 +225,7 @@ int nope_unet_debug_tap(nope_unet_t* u, const float* ref_feat, const float* pose
 /* ---- LDM variant (SURVEY.md 8 f2) ------------------------------------------------------
  * UNetModelPose (src/model/u_net/ldm/adapt_openaimodel.py:14-158 over ldm/openaimodel.py:428-760
  * and ldm/attention.py:149-277; configs/model/vae_cin_ldm.yaml): ResBlocks + SpatialTransformers
- * (self-attention on tcgen05, the one-token pose cross-attention folded to a per-hypothesis
+ * (self-attention on wgmma, the one-token pose cross-attention folded to a per-hypothesis
  * channel vector, GEGLU feed-forward), strided-conv down / nearest-x2+conv up, emb = 0.
  * Supported configuration: channel_mult (1, 2, 4), 2 ResBlocks per level, attention at every
  * level, num_head_channels 32, transformer_depth 1, injecting_condition_twice false,
@@ -243,8 +243,8 @@ int nope_ldm_load_tensor(nope_ldm_t* m, const char* key, const float* data, cons
                          int ndim);
 int nope_ldm_finalize(nope_ldm_t* m);
 int nope_ldm_set_chunk(nope_ldm_t* m, int hyps_per_chunk);       /* ~20.5 MB workspace / hypothesis */
-/* conv_impl: 2 = tcgen05 CTA pairs (default), 0 = tcgen05 1-CTA tiles;
- * attn_impl: 0 = tcgen05 attention (default), 1 = CUDA-core twin (bring-up). */
+/* conv_impl: 2 = clustered wgmma kernel (default), 0 = single-CTA wgmma kernel;
+ * attn_impl: 0 = wgmma attention (default), 1 = CUDA-core twin (bring-up). */
 int nope_ldm_set_impl(nope_ldm_t* m, int conv_impl, int attn_impl);
 /* Named switches (bring-up / A-B measurements): "fuse_geglu" (default 1: GEGLU runs in the
  * epilogue of its projection GEMM; 0: separate elementwise kernel), "hoist" (default 1: the

@@ -1,4 +1,4 @@
-"""nope_b200 -- B200-native implementation of the NOPE (nv-nguyen/nope) inference hot
+"""nope_b200 -- H100-native implementation of the NOPE (nv-nguyen/nope) inference hot
 path: pose-conditioned UNet sweep over a pose grid + template scoring + top-k."""
 from ._lib import NopeError, load as load_library  # noqa: F401
 

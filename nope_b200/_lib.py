@@ -96,7 +96,7 @@ def load():
     if LIB_PATH == _DEFAULT_LIB_PATH and not os.environ.get("NOPE_NO_AUTOBUILD"):
         # the library is built in-tree by `python -m nope_b200.build` / __graft_entry__.build();
         # on a fresh checkout, or when a source file is newer than the binary, compile it now
-        # (nvcc, sm_100a) -- still the CUDA path, never a fallback.  A box without nvcc keeps the
+        # (nvcc, sm_90a) -- still the CUDA path, never a fallback.  A box without nvcc keeps the
         # shipped binary (its ABI version is checked below).
         from . import build as _build
         if not os.path.exists(LIB_PATH) or (_build.is_stale() and _build.have_nvcc()):

@@ -1,4 +1,4 @@
-"""Build libnope_b200.so in-tree with nvcc for sm_100a (no torch extension machinery:
+"""Build libnope_b200.so in-tree with nvcc for sm_90a (no torch extension machinery:
 the library is a plain C-ABI shared object, bound from Python with ctypes)."""
 import os
 import shutil
@@ -53,7 +53,7 @@ def build(force=False, verbose=False):
         return OUT
     os.makedirs(OUT_DIR, exist_ok=True)
     tmp = f"{OUT}.{os.getpid()}.tmp"       # several ranks may build at once: private temp, atomic rename
-    cmd = [nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3",
+    cmd = [nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3",
            "-lineinfo", "-Xcompiler", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"),
            "-o", tmp, SRC]
     if verbose:

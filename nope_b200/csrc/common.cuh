@@ -1,5 +1,5 @@
-// nope_b200 -- shared device helpers: error plumbing, mbarrier / TMA / tcgen05
-// PTX wrappers for sm_100a.  Everything here is hand-written inline PTX; no
+// nope_b200 -- shared device helpers: error plumbing, mbarrier / TMA / wgmma
+// PTX wrappers for sm_90a.  Everything here is hand-written inline PTX; no
 // CUTLASS/CuTe types are used.
 #pragma once
 #include <cuda.h>
@@ -8,6 +8,8 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string>
+
+#include "wgmma.cuh"
 
 namespace nope {
 
@@ -84,17 +86,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Bounded wait: a protocol bug traps (surfaces as a CUDA error) instead of
-// hanging the GPU box.  ~4 s at 2 GHz.
+// hanging the GPU.  ~4 s at 2 GHz.  No printf: a function call anywhere in a kernel makes
+// ptxas retire every wgmma before issuing the next one, which serialises the mainloop.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 8000000000LL) {
-      printf("nope_b200: mbarrier wait timed out (block %d thread %d)\n", (int)blockIdx.x,
-             (int)threadIdx.x);
-      __trap();
-    }
-  }
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > 8000000000LL) __trap();
 }
 
 // ---- async proxy fences / TMA ------------------------------------------------
@@ -156,82 +154,6 @@ __device__ __forceinline__ void tma_store_wait_read1() {
 }
 __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-}
-
-// ---- tcgen05 / TMEM ------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers fp16 and bf16 inputs.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once every previously issued tcgen05.mma of this thread retires.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::
-                   "r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (lane = row).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-        "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]),
-        "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// K-major, 128-byte-swizzled shared-memory operand descriptor (tcgen05 matrix
-// descriptor): rows are 128 B (64 x 16-bit), 8-row groups are 1024 B apart.
-//   [0,14)  start address >> 4        [16,30) leading byte offset >> 4 (unused here)
-//   [32,46) stride byte offset >> 4   [46,48) descriptor version = 1 (sm_100)
-//   [49,52) base offset = 0           [61,64) layout type: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;             // LBO (ignored for swizzled K-major)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;     // SBO: 8 rows * 128 B
-  d |= static_cast<uint64_t>(1) << 46;             // version
-  d |= static_cast<uint64_t>(2) << 61;             // SWIZZLE_128B
-  return d;
-}
-// tcgen05 instruction descriptor, kind::f16, fp32 accumulate, both operands K-major.
-//   [4,6) D format (1 = f32)  [7,10) A format (0 = f16, 1 = bf16)  [10,13) B format
-//   [15] A major (0 = K)  [16] B major (0 = K)  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n, bool bf16) {
-  return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
 }
 
 // x * sigmoid(x) with the fast divide (MUFU.RCP + FMUL, <= 2 ulp): the IEEE '/' expands to a

@@ -1,4 +1,4 @@
-// nope_b200 -- implicit-GEMM convolution on tcgen05 tensor cores (sm_100a).
+// nope_b200 -- implicit-GEMM convolution on wgmma tensor cores (sm_90a).
 //
 // One kernel serves every GEMM-shaped op of the pose-conditioned UNet
 // (reference: src/model/u_net/denoising_diffusion_pytorch/model_utils.py:240
@@ -14,16 +14,15 @@
 // activation tensor, shifted by the tap offset (dy, dx); out-of-image rows and
 // columns are zero-filled by the TMA unit, which is exactly conv padding.  The
 // box lands in shared memory as a 128-row x 128-byte K-major SWIZZLE_128B tile,
-// the canonical tcgen05 operand layout.  Channel concatenation (skip
+// the canonical wgmma operand layout.  Channel concatenation (skip
 // connections, u_net.py:186-194) is two source tensor maps walked by the same K
 // loop; pixel-unshuffle + 1x1 (HardDownsample) is four stride-2 tensor maps.
 //
 // CTA = 12 warps, persistent over (m_tile, n_tile) work items:
 //   warp 0        : TMA producer      (smem ring, full/empty mbarriers; one elected lane issues)
-//   warp 1        : tcgen05.mma issuer (accumulator in TMEM, double buffered)
-//   warp 2        : TMEM allocator
-//   warps 4..11   : epilogue: tcgen05.ld -> +bias -> GroupNorm partial sums -> fp16 ->
-//                   swizzled smem -> TMA store (two warps per TMEM lane quarter)
+//   warps 4..11   : two warpgroups: wgmma mainloop (each warpgroup owns half of the tile's columns,
+//                   accumulator in registers), then the fp32 tile through shared memory (conv_mma_tile)
+//                   -> +bias -> GroupNorm partial sums -> fp16 -> swizzled smem -> TMA store
 #pragma once
 #include "common.cuh"
 #include <cudaTypedefs.h>
@@ -45,7 +44,7 @@ struct ConvSeg {
                     // (split precision re-reads the W_hi columns for the A_lo product)
 };
 
-// GroupNorm applied in the epilogue of the producing convolution (2-CTA kernel, EPI == 4 / 3):
+// GroupNorm applied in the epilogue of the producing convolution (clustered kernel, EPI == 4 / 3):
 //   y = [SiLU]((acc - mean) * rstd * gamma + beta) + pose_bias[img, c] + residual[pixel, c]
 // (Block.forward / ResnetBlock.forward, model_utils.py:237-253, 271-279; PreNorm / to_out[1] of
 // LinearAttention, model_utils.py:230, 401).  The statistics of an image are spread over the CTA
@@ -99,7 +98,7 @@ struct ConvParams {
   CUtensorMap amap[kMaxAMaps];
   int n_amaps;
   CUtensorMap bmap;
-  CUtensorMap bmap_half;  // box of BN/2 weight rows: the 2-CTA kernel (conv_tc2.cuh)
+  CUtensorMap bmap2;      // weight box of the clustered kernel's tile width (conv_tc2.cuh)
   CUtensorMap omap[4];  // one per output parity class when n_par == 4, else omap[0]
   CUtensorMap rmap;     // residual tensor (output geometry), EPI == 4 / 3 with gn.has_res
   GnFuse gn;            // EPI == 4 / 3
@@ -109,7 +108,7 @@ struct ConvParams {
   // (py, px) shifts every tap by (+py, +px), reads weight rows parity * n_per_par + ..., and
   // stores through omap[parity] (the stride-2 sub-lattice of the 2H x 2W output).
   int bf16;           // operands and the stored output are bf16 instead of fp16 (plain / GroupNorm-fused epilogues)
-  int l2_prefetch;    // 2-CTA kernel: the producer prefetches the next tile's activation rows into L2
+  int l2_prefetch;    // clustered kernel: the producer prefetches the next tile's activation rows into L2
   int n_par;          // 1 or 4
   int n_tiles_par;    // channel tiles per parity (== n_tiles when n_par == 1)
   int src_w, src_hw;  // n_par == 4: width / pixels of one SOURCE image (out_lo addressing)
@@ -121,7 +120,7 @@ struct ConvParams {
   const __half* res_lo;   // residual, low halves (nullptr: residual is a single fp16 tensor)
   __half* out_lo;         // low halves of the output (omap receives the high halves)
   float* out_f32;         // fp32 output instead of the fp16 TMA store
-  // GEGLU epilogue (ldm/attention.py:44-51; 2-CTA kernel, BN = 128 only): every 128-column tile
+  // GEGLU epilogue (ldm/attention.py:44-51; clustered kernel, BN = 128 only): every 128-column tile
   // holds 64 "x" channels followed by their 64 "gate" channels (rows permuted on the host);
   // the epilogue stores x * gelu(gate) as 64 fp16 channels at channel (n_tile * 64) of omap.
   int geglu;
@@ -150,6 +149,8 @@ struct ConvSmem {
   static constexpr int kBarOffset = STAGES * kStageBytes + kOutBytes;
   static constexpr int kBiasOffset = kBarOffset + 256;
   static constexpr int kTotal = kBiasOffset + BN * 4 + 1024;  // + alignment slack
+  static_assert(STAGES * kStageBytes >= kBM * (BN + 4) * 4, "the fp32 accumulator tile must fit in the operand ring");
+  static_assert(kTotal <= 227 * 1024, "shared memory per block");
 };
 
 __device__ __forceinline__ void conv_tile_coords(const ConvParams& p, int m_tile, int& b0,
@@ -163,9 +164,70 @@ __device__ __forceinline__ void conv_tile_coords(const ConvParams& p, int m_tile
   }
 }
 
-// constant bits of the K-major SWIZZLE_128B operand descriptor (see make_sw128_kmajor_desc)
-constexpr uint64_t kDescHi = (static_cast<uint64_t>(1) << 16) | (static_cast<uint64_t>(1024 >> 4) << 32) |
-                             (static_cast<uint64_t>(1) << 46) | (static_cast<uint64_t>(2) << 61);
+// Row stride (floats) of the fp32 accumulator tile in shared memory: 4 floats of padding keep the
+// row-per-lane 16-byte reads of the epilogue free of bank conflicts.
+__host__ __device__ constexpr int acc_ld(int BN) { return BN + 4; }
+
+// K loop of one tile for warpgroup wg: columns [wg NS, wg NS + NS) of all 128 rows, two m64 wgmmas (rows 0-63
+// and 64-127) per 16-deep K step, one wgmma group in flight while the previous stage is released.  The operand
+// type is a template parameter, so the loop is one straight wgmma pipeline.
+template <int NS, int STAGES, int kStageBytes, int kABytes, bool BF>
+__device__ __forceinline__ void conv_mma_loop(const ConvParams& p, const uint8_t* smem, uint64_t* full_bar,
+                                              uint64_t* empty_bar, int& stage, uint32_t& phase, int wg,
+                                              float (&d0)[NS / 2], float (&d1)[NS / 2]) {
+  const int lane = threadIdx.x & 31;
+  int prev = -1;
+  for (int ks = 0; ks < p.ksteps; ++ks) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint8_t* sa = smem + stage * kStageBytes;
+    const uint64_t adesc = wg_desc_k(sa);
+    const uint64_t bdesc = wg_desc_k(sa + kABytes + wg * NS * 128);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k) {
+      // advance 16 elements (32 B) along K inside the swizzle atom: +2 in the >>4 field; rows 64.. are 8 KB on
+      const uint32_t acc = (ks | k) != 0 ? 1u : 0u;
+      Wgmma<NS, BF>::mma(d0, adesc + 2 * k, bdesc + 2 * k, acc);
+      Wgmma<NS, BF>::mma(d1, adesc + 512 + 2 * k, bdesc + 2 * k, acc);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();            // the previous K-step's group has retired: its stage may be refilled
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+}
+
+// Mainloop of one 128 x BN tile, run by the NW warpgroups of threads [128, 128 + 128 NW).  Warpgroup w
+// accumulates columns [w BN / NW, (w + 1) BN / NW) of all 128 rows in registers, then the tile is written as
+// fp32 to s_acc, the front of the operand ring.  The ring is idle by then (every stage of this tile has been
+// consumed) and the producer refills it only after the epilogue has read the tile back (tempty barrier), so
+// accumulator and operands share the memory.
+template <int BN, int NW, int STAGES, int kStageBytes, int kABytes>
+__device__ __forceinline__ void conv_mma_tile(const ConvParams& p, uint8_t* smem, uint64_t* full_bar,
+                                              uint64_t* empty_bar, int& stage, uint32_t& phase, float* s_acc) {
+  constexpr int NS = BN / NW;
+  static_assert(NS % 32 == 0 && NS <= 128, "columns per warpgroup");
+  const int wg = (threadIdx.x >> 7) - 1;
+  float d0[NS / 2], d1[NS / 2];
+#pragma unroll
+  for (int i = 0; i < NS / 2; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+  if (p.bf16) conv_mma_loop<NS, STAGES, kStageBytes, kABytes, true>(p, smem, full_bar, empty_bar, stage, phase, wg, d0, d1);
+  else conv_mma_loop<NS, STAGES, kStageBytes, kABytes, false>(p, smem, full_bar, empty_bar, stage, phase, wg, d0, d1);
+  asm volatile("bar.sync 2, %0;" ::"n"(NW * 128) : "memory");      // no warpgroup still reads the ring
+  wg_store_acc<NS>(s_acc, acc_ld(BN), wg * NS, d0, d1);
+  asm volatile("bar.sync 2, %0;" ::"n"(NW * 128) : "memory");
+}
+
+// The epilogue has read the accumulator tile out of the ring: order its generic-proxy accesses before the
+// producer's next TMA writes, then release the ring (one arrive per epilogue warp).
+__device__ __forceinline__ void acc_release(uint64_t* tempty, int lane) {
+  fence_proxy_async_smem();
+  __syncwarp();
+  if (lane == 0) mbar_arrive(tempty);
+}
 
 // Transposing butterfly: every lane holds 8 partial values; afterwards v[0] of lane l is the
 // total over the kSeg lanes of its segment of value number `idx` (returned).  8+4+2(+1)
@@ -204,7 +266,7 @@ __device__ __forceinline__ int butterfly8(float (&v)[8], int lane) {
 }
 
 // Epilogue of one 128 x BN accumulator tile, executed by the 8 epilogue warps of a CTA.
-// Warp e reads TMEM lanes 32*(e&3).. (its pixel rows) and the 32-column half (e>>2) of every
+// Warp e reads accumulator rows 32*(e&3).. (its pixel rows) and the 32-column half (e>>2) of every
 // 64-column sub-tile: +bias (from smem) -> GroupNorm partial sums -> fp16 -> swizzled staging.
 // EXTRAS (compile time) enables ReLU / residual add / (hi, lo) split / fp32 output: the template
 // encoder's epilogue.  The sweep instantiates EXTRAS = false so its epilogue stays minimal (the
@@ -234,12 +296,12 @@ struct ResPrefetch {
 
 template <int BN, bool EXTRAS>
 __device__ __forceinline__ void conv_epilogue_tile(const ConvParams& p, uint8_t* out_stage,
-                                                   const float* s_bias, uint32_t t_acc, int m_tile,
+                                                   const float* s_bias, const float* s_acc, int m_tile,
                                                    int n_chan0, int e, int lane,
                                                    ResPrefetch<BN>* pre = nullptr, int par = 0) {
   const int q = e & 3, hh = e >> 2;
   const int row = q * 32 + lane;
-  const uint32_t t_row = t_acc + (static_cast<uint32_t>(q * 32) << 16) + hh * 32;
+  const float* a_row = s_acc + row * acc_ld(BN) + hh * 32;
   const int grow = m_tile * kBM + row;                                // linear pixel index
   const bool row_ok = grow < p.m_valid;
   size_t opix = (size_t)grow;                                         // output pixel (EXTRAS stores)
@@ -248,13 +310,10 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvParams& p, uint8_t*
     const int yy = r / p.src_w, xx = r - yy * p.src_w;
     opix = (size_t)img * 4 * p.src_hw + (size_t)(2 * yy + (par >> 1)) * (2 * p.src_w) + 2 * xx + (par & 1);
   }
-  uint32_t va[32], vb[32];
-  tmem_ld_32x32(t_row, va);
+  uint32_t v[32];
 #pragma unroll
   for (int cc = 0; cc < BN / 64; ++cc) {
-    tmem_ld_wait();
-    uint32_t(&v)[32] = (cc & 1) ? vb : va;
-    if (cc + 1 < BN / 64) tmem_ld_32x32(t_row + (cc + 1) * 64, (cc & 1) ? va : vb);
+    acc_ld_32(a_row + cc * 64, v);
     const float* bs = s_bias + cc * 64 + hh * 32;
     uint8_t* srow = out_stage + cc * (kBM * 128) + row * 128;
     // residual operands of this sub-tile: all loads issued before the math
@@ -361,15 +420,14 @@ __device__ __forceinline__ float gelu_erf_fast(float g) {
 // GEGLU epilogue of one 128 x 128 accumulator tile: columns 0..63 = x, 64..127 = gate.
 // Warp e owns pixel rows 32*(e&3).. and the 32-column half (e>>2) of BOTH halves, so
 // x * gelu(gate) needs no exchange.  erf-GELU (F.gelu's default) through gelu_erf_fast.
-__device__ __forceinline__ void conv_epilogue_geglu(uint8_t* out_stage, const float* s_bias, uint32_t t_acc,
+__device__ __forceinline__ void conv_epilogue_geglu(uint8_t* out_stage, const float* s_bias, const float* s_acc,
                                                     int e, int lane) {
   const int q = e & 3, hh = e >> 2;
   const int row = q * 32 + lane;
-  const uint32_t t_row = t_acc + (static_cast<uint32_t>(q * 32) << 16) + hh * 32;
+  const float* a_row = s_acc + row * acc_ld(128) + hh * 32;
   uint32_t vx[32], vg[32];
-  tmem_ld_32x32(t_row, vx);
-  tmem_ld_32x32(t_row + 64, vg);
-  tmem_ld_wait();
+  acc_ld_32(a_row, vx);
+  acc_ld_32(a_row + 64, vg);
   const float* bx = s_bias + hh * 32;
   const float* bg = s_bias + 64 + hh * 32;
   uint8_t* srow = out_stage + row * 128;
@@ -393,7 +451,6 @@ template <int BN, int STAGES, bool EXTRAS>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_tc_kernel(const __grid_constant__ ConvParams p) {
   using S = ConvSmem<BN, STAGES>;
-  constexpr int kTmemCols = (2 * BN <= 128) ? 128 : (2 * BN <= 256 ? 256 : 512);
   static_assert(BN % 64 == 0 && BN <= 256, "BN must be a multiple of 64");
 
   extern __shared__ uint8_t smem_raw[];
@@ -402,10 +459,9 @@ conv_tc_kernel(const __grid_constant__ ConvParams p) {
   uint8_t* out_stage = smem + STAGES * S::kStageBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint64_t* tempty_bar = empty_bar + STAGES;
   float* s_bias = reinterpret_cast<float*>(smem + S::kBiasOffset);
+  float* s_acc = reinterpret_cast<float*>(smem);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -419,34 +475,28 @@ conv_tc_kernel(const __grid_constant__ ConvParams p) {
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kEpiWarps);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], kEpiWarps);
-    }
+    mbar_init(tempty_bar, kEpiWarps);
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // The producer and MMA warps run their loops warp-converged and elect one lane only around
-  // the instruction issue: control flow and address arithmetic stay on the uniform datapath
-  // (a `lane == 0` branch around the whole loop cost ~120 SASS instructions per K-step).
+  // The producer runs its loop warp-converged and elects one lane only around the instruction issue:
+  // control flow and address arithmetic stay on the uniform datapath.
   if (warp == 0) {
     // ===================== TMA producer =====================
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int iter = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++iter) {
       const int m_tile = tile / p.n_tiles;
       const int n_tile = tile - m_tile * p.n_tiles;
       const int par = n_tile / p.n_tiles_par;          // 0 unless n_par == 4
       const int py = par >> 1, px = par & 1;
       int b0, y0;
       conv_tile_coords(p, m_tile, b0, y0);
+      if (iter > 0) mbar_wait(tempty_bar, (iter - 1) & 1);     // the previous accumulator tile left the ring
       int kcol = 0;
       for (int s = 0; s < p.nseg; ++s) {
         const ConvSeg sg = p.seg[s];
@@ -465,44 +515,12 @@ conv_tc_kernel(const __grid_constant__ ConvParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = make_idesc_f16(kBM, BN, false) | (p.bf16 ? ((1u << 7) | (1u << 10)) : 0u);
-    const uint32_t smem_base = smem_u32(smem);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int ks = 0; ks < p.ksteps; ++ks) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_lo = (smem_base + stage * S::kStageBytes) >> 4;
-          const uint64_t adesc = kDescHi | a_lo;
-          const uint64_t bdesc = kDescHi | (a_lo + (S::kABytes >> 4));
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            // advance 16 elements (32 B) along K inside the swizzle atom: +2 in the >>4 field
-            umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (ks | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (ks == p.ksteps - 1) umma_commit(&tfull_bar[acc]);
-        }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
   } else if (warp >= 4) {
-    // ===================== epilogue (8 warps) =====================
+    // ===================== mainloop + epilogue (8 warps) =====================
     const int e = warp - 4;
     const int etid = threadIdx.x - 128;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_tile = tile / p.n_tiles;
       const int n_tile = tile - m_tile * p.n_tiles;
@@ -514,13 +532,9 @@ conv_tc_kernel(const __grid_constant__ ConvParams p) {
       // staging buffer must have been fully read by the previous TMA store; bias visible
       if (etid == 0) tma_store_wait_read0();
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      conv_epilogue_tile<BN, EXTRAS>(p, out_stage, s_bias, tmem_base + acc * BN, m_tile, n_chan0, e, lane);
-      // accumulator fully read: hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+      conv_mma_tile<BN, 2, STAGES, S::kStageBytes, S::kABytes>(p, smem, full_bar, empty_bar, stage, phase, s_acc);
+      conv_epilogue_tile<BN, EXTRAS>(p, out_stage, s_bias, s_acc, m_tile, n_chan0, e, lane);
+      acc_release(tempty_bar, lane);
       // make the generic-proxy smem writes visible to the TMA (async proxy), then store
       fence_proxy_async_smem();
       asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -530,15 +544,9 @@ conv_tc_kernel(const __grid_constant__ ConvParams p) {
           tma_store_4d(&p.omap[par], out_stage + cc * (kBM * 128), n_chan0 + cc * 64, 0, y0, b0);
         tma_store_commit();
       }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
     if (etid == 0) tma_store_wait_all();
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<kTmemCols>(tmem_base);
 }
 
 // ----------------------------------------------------------------------------

@@ -1,33 +1,28 @@
-// nope_b200 -- 2-CTA (cta_group::2) variant of the implicit-GEMM convolution.
+// nope_b200 -- clustered variant of the implicit-GEMM convolution, with the fused epilogues.
 //
-// Same math, parameters and epilogue as conv_tc_kernel (conv_tc.cuh); the difference is
-// the tile: a CTA PAIR (thread-block cluster of 2, one TPC) owns a 256-pixel x BN tile.
-// Each CTA TMA-loads its own 128 pixel rows of A and only HALF of the weight tile
-// (BN/2 rows); one tcgen05.mma.cta_group::2 issued by the leader CTA multiplies both halves
-// of A against the full weight tile (each SM reads the peer's weight half over the pair
-// link), accumulating 128 x BN fp32 in each CTA's own TMEM.  Per K-step a CTA pulls
-// 16 KB + BN*64 B from L2 instead of 16 KB + BN*128 B: the L2->SM traffic that bounds the
-// 1-CTA kernel (77 FLOP/B at BN=192) drops by 30 % (110 FLOP/B), and the smaller stage
-// buys a 6-deep ring.
+// Same math, parameters and epilogue as conv_tc_kernel (conv_tc.cuh); CTAs are launched in
+// thread-block clusters of 2 that walk the tile list in PAIRS of 128-pixel M-tiles (tile
+// (m_pair, n_tile) -> M-tiles 2 m_pair and 2 m_pair + 1, one per CTA), so the two CTAs of a pair
+// read the same weight tile at the same time and the second read is served by L2.  Each CTA
+// TMA-loads its own 128 pixel rows of A and the whole BN-row weight tile, and its epilogue
+// warpgroups run the wgmma mainloop (conv_mma_tile): warpgroup w accumulates its share of the
+// tile's columns in registers, the fp32 tile then passes through shared memory to the epilogue.
 //
 // Tile widths: 192 (the default UNet: every width is a multiple of 192), 256 (the LDM variant:
-// multiples of 256; a 128-wide tile reads 16 KB of A + 8 KB of B per 64 tensor-core clocks,
-// exactly the 128 B/clk shared-memory limit, a 256-wide one 32 KB per 128), 128 / 64 (template
-// encoder, GEGLU).  Tiles of <= 128 columns double-buffer the output staging.  EPI selects the
-// epilogue at compile time: 0 plain (+ GroupNorm partial sums), 1 extras (ReLU, residual add,
-// (hi, lo) split, fp32 store: template encoder, LDM out conv), 2 GEGLU (conv_tc.cuh), 4 GroupNorm
-// fused (GnFuse, conv_tc.cuh) with the CTA split into math / statistics / store roles (conv_gn2_* below):
-// the default UNet's Block / ResnetBlock / to_qkv / to_out epilogues -- the normalised, activated tensor
-// is the only thing that reaches HBM.  3 is the same epilogue in lock step (all epilogue warps walk through
-// the tile together; kept behind NOPE_GN_EPI=3 as the A/B baseline the role split was measured against).
+// multiples of 256), 128 / 64 (template encoder, GEGLU).  Tiles of <= 128 columns double-buffer
+// the output staging.  EPI selects the epilogue at compile time: 0 plain (+ GroupNorm partial
+// sums), 1 extras (ReLU, residual add, (hi, lo) split, fp32 store: template encoder, LDM out conv),
+// 2 GEGLU (conv_tc.cuh), 4 GroupNorm fused (GnFuse, conv_tc.cuh) with the CTA split into math /
+// statistics / store roles (conv_gn2_* below): the default UNet's Block / ResnetBlock / to_qkv /
+// to_out epilogues -- the normalised, activated tensor is the only thing that reaches HBM.  3 is the
+// same epilogue in lock step (all epilogue warps walk through the tile together; kept behind
+// NOPE_GN_EPI=3 as the A/B baseline the role split was measured against).
 //
-// Protocol (per CTA unless noted; barriers live at identical smem offsets in both CTAs):
-//   full[s]   leader only, count 2: leader's arrive.expect_tx(bytes of BOTH CTAs) + the
-//             peer producer's remote arrive; both CTAs' TMA loads complete_tx on it
-//             (cta_group::2 loads with the peer bit of the barrier address cleared)
-//   empty[s]  count 1: tcgen05.commit multicast from the leader's MMA thread to both CTAs
-//   tfull[a]  count 1: same multicast commit after the last K-step of a tile
-//   tempty[a] leader only, count 8: the 4 epilogue warps of each CTA (peer: remote arrive)
+// Protocol (per CTA):
+//   full[s]   count 1: the producer's arrive.expect_tx; the stage's TMA loads complete_tx on it
+//   empty[s]  one arrive per epilogue (mainloop) warp once its wgmma reads of the stage retired
+//   tempty    one arrive per epilogue warp once the accumulator tile has been read out of the ring;
+//             the producer waits for it before it loads the next tile
 #pragma once
 #include "conv_tc.cuh"
 
@@ -52,34 +47,6 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the barrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}\n"
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
-}
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // address of the same offset in the pair's CTA 0
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar,
-                                                int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask),
-      "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar,
-                                                int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask),
-      "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
 // L2 prefetch of one activation box (no shared-memory destination, no barrier), issued by the producer one tile ahead.
 // Measured (ConvParams::l2_prefetch, NOPE_L2_PREFETCH=1): 3 % SLOWER over the sweep -- the ring's look-ahead already
 // covers the HBM latency and the extra requests only compete with it; off by default
@@ -88,38 +55,6 @@ __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* m, int c0, in
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void umma_f16_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives (once all prior MMAs of this thread retire) on the barrier at this offset in every
-// CTA of `mask`
-__device__ __forceinline__ void umma_commit_2cta_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64"
-      " [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
-
 // shared-memory map of the EPI == 4 epilogue (conv_gn2_* below), relative to Conv2Smem::kGnOffset
 template <int BN>
 struct Gn2Smem {
@@ -136,7 +71,7 @@ struct Gn2Smem {
 template <int BN, int STAGES, int EPI = 0>
 struct Conv2Smem {
   static constexpr int kABytes = kBM * kBK * 2;
-  static constexpr int kBBytes = (BN / 2) * kBK * 2;      // this CTA's half of the weight tile
+  static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kOutBytes = (BN / 64) * kBM * 128;
   // narrow tiles double-buffer the output staging: the TMA store of tile i drains while the
@@ -151,6 +86,8 @@ struct Conv2Smem {
   static constexpr int kGnBytes = EPI == 3 ? (2 * BN * 4 + 8 * BN * 2 + 8 * (BN / 8) * 8 + 64 * 8 + (BN / 8) * 4 + 32 * 8 + 256 * 4)
                                             : (EPI == 4 ? Gn2Smem<BN>::kBytes : 0);
   static constexpr int kTotal = kGnOffset + kGnBytes + 1024;
+  static_assert(STAGES * kStageBytes >= kBM * (BN + 4) * 4, "the fp32 accumulator tile must fit in the operand ring");
+  static_assert(kTotal <= 227 * 1024, "shared memory per block");
 };
 
 __device__ __forceinline__ unsigned long long global_ns() {
@@ -173,7 +110,7 @@ __device__ __forceinline__ void st_volatile_u2(uint2* p, uint2 v) {
 // Per tile, the 8 epilogue warps
 //   1. start the residual tile's TMA load into the output staging buffer (if any), stage
 //      bias / gamma / beta / pose-bias rows in shared memory;
-//   2. pull the accumulator out of TMEM into registers (+bias) and hand the TMEM buffer straight
+//   2. run the mainloop, pull the accumulator tile into registers (+bias) and hand the ring straight
 //      back to the MMA warp -- the mainloop of the next-but-one tile never waits for this epilogue;
 //   3. reduce per-(image, group) sums over the tile (butterfly over pixel rows, fixed order over
 //      row segments and channel octets), publish them and wait for the other tiles of the sync group
@@ -218,8 +155,8 @@ __host__ __device__ constexpr int gn_epi_warps(int BN) { return 4 * (BN / 64); }
 __host__ __device__ constexpr int gn_threads(int BN) { return 128 + 32 * gn_epi_warps(BN); }
 
 template <int BN, int STAGES>
-__device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8_t* smem, uint32_t tmem_base,
-                                                      uint64_t* tfull_bar, uint64_t* tempty_bar, uint64_t* res_bar,
+__device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8_t* smem, uint64_t* full_bar,
+                                                      uint64_t* empty_bar, uint64_t* tempty_bar, uint64_t* res_bar,
                                                       int tile0, int tile_step, int num_tiles, uint32_t rank) {
   using S = Conv2Smem<BN, STAGES, 3>;
   constexpr int kOct = BN / 8;
@@ -239,9 +176,8 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
   const GnFuse& g = p.gn;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int e = warp - 4, etid = threadIdx.x - 128;
-  const int q = e & 3, cc = e >> 2;                  // TMEM lane quarter, 64-column sub-tile of this warp
+  const int q = e & 3, cc = e >> 2;                  // row quarter, 64-column sub-tile of this warp
   const int row = q * 32 + lane;
-  const bool leader = rank == 0;
   const int hw = p.stats_hw;
   const bool small = hw < 32;                       // 4x4 images: 16-row segments, two per warp
   const int it = hw < kBM ? (row >> g.hw_shift) : 0;    // image of this thread's row inside the tile
@@ -255,9 +191,12 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
   if (etid < kOct) s_og[etid] = (g.G > 0 && g.cpg < BN) ? (etid * 8) / g.cpg : 0;
 #define NOPE_EPI_BAR() asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory")
 
-  int acc = 0, obuf = 0;
-  uint32_t acc_phase = 0, res_phase = 0;
+  int obuf = 0;
+  uint32_t res_phase = 0;
   int iter = 0;
+  int kstage = 0;
+  uint32_t kphase = 0;
+  float* s_acc = reinterpret_cast<float*>(smem);
   // The residual tile of tile t is TMA-loaded into the staging buffer tile t will be written to (same box /
   // swizzle as the store).  It is issued by the thread that issues the stores, as soon as the store that
   // last used the buffer has read it: right after tile t-1's store (or before the loop for the first
@@ -325,23 +264,16 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
     NOPE_EPI_BAR();
     NOPE_TS(1);
     if (!(g.dbg & 16)) fetch_pb(tile + tile_step);
-    mbar_wait(&tfull_bar[acc], acc_phase);
-    tc_fence_after();
+    conv_mma_tile<BN, BN / 64, STAGES, S::kStageBytes, S::kABytes>(p, smem, full_bar, empty_bar, kstage, kphase, s_acc);
     NOPE_TS(2);
 
-    // ---- pass 1: TMEM -> registers, free the accumulator, per-octet partial sums
+    // ---- pass 1: accumulator -> registers, free the ring, per-octet partial sums
     uint32_t a[64];
     {
-      const uint32_t t_row = tmem_base + acc * BN + (static_cast<uint32_t>(q * 32) << 16) + cc * 64;
-      tmem_ld_32x32(t_row, *reinterpret_cast<uint32_t(*)[32]>(&a[0]));
-      tmem_ld_32x32(t_row + 32, *reinterpret_cast<uint32_t(*)[32]>(&a[32]));
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(&tempty_bar[acc]);
-        else mbar_arrive_remote(&tempty_bar[acc], 0);
-      }
+      const float* a_row = s_acc + row * acc_ld(BN) + cc * 64;
+      acc_ld_32(a_row, *reinterpret_cast<uint32_t(*)[32]>(&a[0]));
+      acc_ld_32(a_row + 32, *reinterpret_cast<uint32_t(*)[32]>(&a[32]));
+      acc_release(tempty_bar, lane);
     }
     if (res_late && etid == 0 && (!live || g.G == 0 || g.expected == 1)) stage_residual(tile, obuf);
     if (live) {
@@ -407,10 +339,7 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
               const long long t0 = clock64();
               do {
                 u = ld_volatile_u2(xp + etid);
-                if (clock64() - t0 > 4000000000LL) {
-                  printf("nope_b200: GroupNorm tile sync timed out (block %d tile %d)\n", (int)blockIdx.x, tile);
-                  __trap();
-                }
+                if (clock64() - t0 > 4000000000LL) __trap();   // no printf: see mbar_wait
               } while (u.y != g.epoch);
             }
             s_x[etid] = __uint_as_float(u.x);
@@ -642,8 +571,6 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
     }
     if (etid == 0 && !res_late) stage_residual(tile + tile_step, obuf ^ (S::kOutBufs - 1));
     obuf ^= S::kOutBufs - 1;
-    acc ^= 1;
-    if (acc == 0) acc_phase ^= 1;
   }
   if (etid == 0) tma_store_wait_all();
 #undef NOPE_TS
@@ -656,11 +583,9 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
 //
 // EPI == 3 walks all epilogue warps through the tile in lock step: five to six block-wide barriers per tile,
 // the statistics exchange, the table build and the drain of the TMA store all sit on the critical path of the
-// warps that do the arithmetic (phase stamps, profiles/README.md: 10-11 us per tile against an 8.2 us mainloop
-// at K = 1728; the K = 192 pre-norm qkv tiles took 6.5 us because of a serial chain of eight L2 loads).
-// Here the two idle warps of the CTA take that work and talk to the math warps through mbarriers only:
+// warps that do the arithmetic.  Here warps 2 and 3 take that work and talk to the math warps through mbarriers only:
 //
-//   warps 4..   math: TMEM -> registers (+bias), release the accumulator, per-octet partial sums -> s_part,
+//   warps 4..   math: wgmma mainloop, accumulator -> registers (+bias), release the ring, per-octet partial sums -> s_part,
 //               arrive part_bar | wait stats_bar[b], res_bar | normalise / SiLU / pose bias / residual in place
 //               in the staging tile | arrive out_bar, tabfree_bar[b].   No block-wide barrier anywhere.
 //   warp 3      statistics: wait part_bar | per-(image, group) sums, publish {value, epoch} words, poll the peer
@@ -675,8 +600,9 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
 // are those of EPI == 3: results are bit-identical between the two.
 // ---------------------------------------------------------------------------------------------
 struct Gn2Bars {
-  uint64_t* tfull;      // [2]
-  uint64_t* tempty;     // [2]
+  uint64_t* full;       // [STAGES] operand stage landed (producer -> math warps)
+  uint64_t* empty;      // [STAGES] operand stage consumed (math warps -> producer)
+  uint64_t* tempty;     // accumulator tile read out of the ring (math warps -> producer)
   uint64_t* res[2];     // per staging buffer: residual landed / buffer free (store warp -> math warps)
   uint64_t* part;       // s_part written (math warps -> statistics warp)
   uint64_t* stats;      // [2] tables of tile parity b ready (statistics warp -> math warps)
@@ -774,7 +700,7 @@ __device__ __forceinline__ void gn2_pass2_octets(float* f, uint32_t a_sc, uint32
 
 
 template <int BN, int STAGES>
-__device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t* smem, uint8_t* gsm, uint32_t tmem_base,
+__device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t* smem, uint8_t* gsm,
                                                     const Gn2Bars& B, int tile0, int tile_step, int num_tiles,
                                                     uint32_t rank) {
   using S = Conv2Smem<BN, STAGES, 4>;
@@ -789,9 +715,8 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
   const GnFuse& g = p.gn;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int e = warp - 4;
-  const int q = e & 3, cc = e >> 2;                  // TMEM lane quarter, 64-column sub-tile of this warp
+  const int q = e & 3, cc = e >> 2;                  // row quarter, 64-column sub-tile of this warp
   const int row = q * 32 + lane;
-  const bool leader = rank == 0;
   const int hw = p.stats_hw;
   const bool small = hw < 32;                        // 4x4 images: 16-row segments, two per warp
   const int it = hw < kBM ? (row >> g.hw_shift) : 0; // image of this thread's row inside the tile
@@ -813,8 +738,9 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
   }
   if (g.dbg & 32) variant = -1;
 
-  int acc = 0;
-  uint32_t acc_phase = 0;
+  int kstage = 0;
+  uint32_t kphase = 0;
+  float* s_acc = reinterpret_cast<float*>(smem);
   int iter = 0;
 #define NOPE_TS(k) do { if (g.ts && e == 0 && lane == 0 && iter < 64) g.ts[((size_t)blockIdx.x * 64 + iter) * 16 + (k)] = global_ns(); } while (0)
   for (int tile = tile0; tile < num_tiles; tile += tile_step, ++iter) {
@@ -835,25 +761,16 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
     const __half* pb_row = g.pb + (size_t)(img_ok ? img0 + it : 0) * g.pb_stride + g.pb_off + n_chan0 + cc * 64;
     if (g.pb && live) asm volatile("prefetch.global.L1 [%0];" ::"l"(pb_row));
 
-    mbar_wait(&B.tfull[acc], acc_phase);
-    tc_fence_after();
+    conv_mma_tile<BN, BN / 64, STAGES, S::kStageBytes, S::kABytes>(p, smem, B.full, B.empty, kstage, kphase, s_acc);
     NOPE_TS(1);
-    // ---- pass 1: TMEM -> registers, free the accumulator, per-octet partial sums
+    // ---- pass 1: accumulator -> registers, free the ring, per-octet partial sums
     uint32_t a[64];
     {
-      const uint32_t t_row = tmem_base + acc * BN + (static_cast<uint32_t>(q * 32) << 16) + cc * 64;
-      tmem_ld_32x32(t_row, *reinterpret_cast<uint32_t(*)[32]>(&a[0]));
-      tmem_ld_32x32(t_row + 32, *reinterpret_cast<uint32_t(*)[32]>(&a[32]));
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(&B.tempty[acc]);
-        else mbar_arrive_remote(&B.tempty[acc], 0);
-      }
+      const float* a_row = s_acc + row * acc_ld(BN) + cc * 64;
+      acc_ld_32(a_row, *reinterpret_cast<uint32_t(*)[32]>(&a[0]));
+      acc_ld_32(a_row + 32, *reinterpret_cast<uint32_t(*)[32]>(&a[32]));
+      acc_release(B.tempty, lane);
     }
-    acc ^= 1;
-    if (acc == 0) acc_phase ^= 1;
     if (!live) continue;
 
     float* f = reinterpret_cast<float*>(a);
@@ -1155,10 +1072,7 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
           const long long t0 = clock64();
           do {
             u[k] = ld_volatile_u2(xp + w);
-            if (clock64() - t0 > 4000000000LL) {
-              printf("nope_b200: GroupNorm tile sync timed out (block %d tile %d)\n", (int)blockIdx.x, tile);
-              __trap();
-            }
+            if (clock64() - t0 > 4000000000LL) __trap();   // no printf: see mbar_wait
           } while (u[k].y != g.epoch);
         }
         tot += __uint_as_float(u[k].x);
@@ -1236,10 +1150,7 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
               const long long t0 = clock64();
               do {
                 u[k] = ld_volatile_u2(xp + w);
-                if (clock64() - t0 > 4000000000LL) {
-                  printf("nope_b200: GroupNorm tile sync timed out (block %d tile %d)\n", (int)blockIdx.x, tile);
-                  __trap();
-                }
+                if (clock64() - t0 > 4000000000LL) __trap();   // no printf: see mbar_wait
               } while (u[k].y != g.epoch);
             }
             s_x[w] = __uint_as_float(u[k].x);
@@ -1423,8 +1334,8 @@ template <int BN, int STAGES, int EPI>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(EPI >= 3 ? gn_threads(BN) : kConvThreads, 1)
 conv_tc2_kernel(const __grid_constant__ ConvParams p) {
   using S = Conv2Smem<BN, STAGES, EPI>;
-  constexpr int kTmemCols = (2 * BN <= 128) ? 128 : (2 * BN <= 256 ? 256 : 512);
   static_assert(BN % 64 == 0 && BN <= 256, "BN must be a multiple of 64");
+  constexpr int kMathWarps = EPI >= 3 ? gn_epi_warps(BN) : kEpiWarps;   // warps 4.. run mainloop + epilogue
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -1432,36 +1343,31 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
   uint8_t* out_stage = smem + STAGES * S::kStageBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  uint64_t* res_bar = reinterpret_cast<uint64_t*>(tmem_slot + 2);     // EPI >= 3: residual tile landed
+  uint64_t* tempty_bar = empty_bar + STAGES;
+  uint64_t* res_bar = tempty_bar + 1;                                 // EPI >= 3: residual tile landed
   uint64_t* gn2_bar = res_bar + 1;                                    // EPI == 4: part, stats[2], tabfree[2], out[2], res of buffer 1
-  static_assert((2 * STAGES + 4 + 2 + 8) * 8 <= 256, "barrier block overflow");
+  static_assert((2 * STAGES + 2 + 8) * 8 <= 256, "barrier block overflow");
   float* s_bias = reinterpret_cast<float*>(smem + S::kBiasOffset);
+  float* s_acc = reinterpret_cast<float*>(smem);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
   const int m_pairs = (p.m_tiles + 1) >> 1;
   const int num_tiles = m_pairs * p.n_tiles;          // pair tiles
   const int tile0 = cluster_id_x(), tile_step = num_clusters_x();
 
   if (warp == 0 && lane == 0) {
     for (int i = 0; i < p.n_amaps; ++i) prefetch_tmap(&p.amap[i]);
-    prefetch_tmap(&p.bmap_half);
+    prefetch_tmap(&p.bmap2);
     for (int i = 0; i < p.n_par; ++i) prefetch_tmap(&p.omap[i]);
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 2);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], kMathWarps);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], 2 * (EPI >= 3 ? gn_epi_warps(BN) : kEpiWarps));
-    }
+    mbar_init(tempty_bar, kMathWarps);
     mbar_init(res_bar, 1);
     if constexpr (EPI == 4) {
       mbar_init(&gn2_bar[0], gn_epi_warps(BN));                         // part
@@ -1475,21 +1381,18 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc_2cta<kTmemCols>(tmem_slot);
-  tc_fence_before();
-  cluster_sync_all();     // barriers of BOTH CTAs initialised before any remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation, descriptor prefetch) touched
-  // no global memory and may overlap the tail of the previous kernel in the stream; from here on the kernel reads
-  // what that kernel wrote.  The next kernel's CTAs may be scheduled as soon as this grid's CTAs retire.
+  __syncthreads();
+  // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) touched no global memory
+  // and may overlap the tail of the previous kernel in the stream; from here on the kernel reads what that kernel
+  // wrote.  The next kernel's CTAs may be scheduled as soon as this grid's CTAs retire.
   pdl_sync();
 
   if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
+    // ===================== TMA producer =====================
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+    int iter = 0;
+    for (int tile = tile0; tile < num_tiles; tile += tile_step, ++iter) {
       const int m_pair = tile / p.n_tiles;
       const int n_tile = tile - m_pair * p.n_tiles;
       const int m_tile = 2 * m_pair + (int)rank;       // may be one past the end: TMA zero-fills
@@ -1497,6 +1400,7 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
       const int py = par >> 1, px = par & 1;
       int b0, y0;
       conv_tile_coords(p, m_tile, b0, y0);
+      if (iter > 0) mbar_wait(tempty_bar, (iter - 1) & 1);     // the previous accumulator tile left the ring
       if (p.l2_prefetch && tile + tile_step < num_tiles) {
         // next tile of this CTA: the un-shifted tap of every source (the other taps re-read the same rows)
         const int nt = tile + tile_step;
@@ -1524,76 +1428,37 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           if (elect_one()) {
             uint8_t* sa = smem + stage * S::kStageBytes;
-            if (leader) mbar_expect_tx(&full_bar[stage], 2 * S::kStageBytes);
-            tma_load_4d_2sm(sa, am, &full_bar[stage], ch * kBK, sg.dx + px, y0 + sg.dy + py, b0);
-            tma_load_2d_2sm(sa + S::kABytes, &p.bmap_half, &full_bar[stage], kcol,
-                            n_tile * BN + (int)rank * (BN / 2));
-            if (!leader) mbar_arrive_remote(&full_bar[stage], 0);
+            mbar_expect_tx(&full_bar[stage], S::kStageBytes);
+            tma_load_4d(sa, am, &full_bar[stage], ch * kBK, sg.dx + px, y0 + sg.dy + py, b0);
+            tma_load_2d(sa + S::kABytes, &p.bmap2, &full_bar[stage], kcol, n_tile * BN);
           }
           kcol += kBK;
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1 && leader) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    const uint32_t idesc = make_idesc_f16(2 * kBM, BN, false) | (p.bf16 ? ((1u << 7) | (1u << 10)) : 0u);
-    const uint32_t smem_base = smem_u32(smem);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    int mma_iter = 0;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step, ++mma_iter) {
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      if constexpr (EPI == 4) {     // development: phase stamps 6 (accumulator granted) / 7 (last K-step issued)
-        if (p.gn.ts && lane == 0 && mma_iter < 64) p.gn.ts[((size_t)blockIdx.x * 64 + mma_iter) * 16 + 6] = global_ns();
-      }
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int ks = 0; ks < p.ksteps; ++ks) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_lo = (smem_base + stage * S::kStageBytes) >> 4;
-          const uint64_t adesc = kDescHi | a_lo;
-          const uint64_t bdesc = kDescHi | (a_lo + (S::kABytes >> 4));
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k)
-            umma_f16_2cta(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (ks | k) != 0 ? 1u : 0u);
-          umma_commit_2cta_mc(&empty_bar[stage], 3);
-          if (ks == p.ksteps - 1) umma_commit_2cta_mc(&tfull_bar[acc], 3);
-        }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if constexpr (EPI == 4) {
-        if (p.gn.ts && lane == 0 && mma_iter < 64) p.gn.ts[((size_t)blockIdx.x * 64 + mma_iter) * 16 + 7] = global_ns();
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
   } else if (EPI == 4 && warp >= 2) {
-    // ===================== epilogue with GroupNorm fused, bookkeeping on warps 2 / 3 =====================
+    // ===================== mainloop + epilogue with GroupNorm fused, bookkeeping on warps 2 / 3 =====================
     if constexpr (EPI == 4) {
       Gn2Bars B;
-      B.tfull = tfull_bar; B.tempty = tempty_bar; B.res[0] = res_bar; B.res[1] = &gn2_bar[7];
+      B.full = full_bar; B.empty = empty_bar; B.tempty = tempty_bar; B.res[0] = res_bar; B.res[1] = &gn2_bar[7];
       B.part = &gn2_bar[0]; B.stats = &gn2_bar[1]; B.tabfree = &gn2_bar[3]; B.out = &gn2_bar[5];
       uint8_t* gsm = smem + S::kGnOffset;
       if (warp == 2) conv_gn2_store_warp<BN, STAGES>(p, smem, gsm, B, tile0, tile_step, num_tiles, rank);
       else if (warp == 3) conv_gn2_stats_warp<BN, STAGES>(p, gsm, B, tile0, tile_step, num_tiles, rank);
-      else conv_gn2_math_warps<BN, STAGES>(p, smem, gsm, tmem_base, B, tile0, tile_step, num_tiles, rank);
+      else conv_gn2_math_warps<BN, STAGES>(p, smem, gsm, B, tile0, tile_step, num_tiles, rank);
     }
   } else if (warp >= 4 && EPI == 3) {
-    // ===================== epilogue with GroupNorm fused =====================
+    // ===================== mainloop + epilogue with GroupNorm fused =====================
     if constexpr (EPI == 3)
-      conv_gn_epilogue_loop<BN, STAGES>(p, smem, tmem_base, tfull_bar, tempty_bar, res_bar, tile0, tile_step,
+      conv_gn_epilogue_loop<BN, STAGES>(p, smem, full_bar, empty_bar, tempty_bar, res_bar, tile0, tile_step,
                                         num_tiles, rank);
   } else if (warp >= 4) {
-    // ===================== epilogue (both CTAs, own 128 rows, 8 warps) =====================
+    // ===================== mainloop + epilogue (own 128 rows, 8 warps) =====================
     const int e = warp - 4;
     const int etid = threadIdx.x - 128;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    int kstage = 0;
+    uint32_t kphase = 0;
     int obuf = 0;
     constexpr bool kPrefetchRes = EPI == 1 && BN <= 128;   // 32 registers; wider tiles load in place
     ResPrefetch<kPrefetchRes ? BN : 64> pre;
@@ -1624,23 +1489,16 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
         else tma_store_wait_read0();
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
+      conv_mma_tile<BN, 2, STAGES, S::kStageBytes, S::kABytes>(p, smem, full_bar, empty_bar, kstage, kphase, s_acc);
       if constexpr (EPI == 2)
-        conv_epilogue_geglu(ost, s_bias, tmem_base + acc * BN, e, lane);
+        conv_epilogue_geglu(ost, s_bias, s_acc, e, lane);
       else if constexpr (kPrefetchRes)
-        conv_epilogue_tile<BN, true>(p, ost, s_bias, tmem_base + acc * BN, m_tile, n_chan0, e, lane, &pre);
+        conv_epilogue_tile<BN, true>(p, ost, s_bias, s_acc, m_tile, n_chan0, e, lane, &pre);
       else if constexpr (EPI == 1)
-        conv_epilogue_tile<BN, true>(p, ost, s_bias, tmem_base + acc * BN, m_tile, n_chan0, e, lane, nullptr, par);
+        conv_epilogue_tile<BN, true>(p, ost, s_bias, s_acc, m_tile, n_chan0, e, lane, nullptr, par);
       else
-        conv_epilogue_tile<BN, false>(p, ost, s_bias, tmem_base + acc * BN, m_tile, n_chan0, e, lane);
-      // this CTA's accumulator half is drained: tell the leader's MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(&tempty_bar[acc]);
-        else mbar_arrive_remote(&tempty_bar[acc], 0);
-      }
+        conv_epilogue_tile<BN, false>(p, ost, s_bias, s_acc, m_tile, n_chan0, e, lane);
+      acc_release(tempty_bar, lane);
       fence_proxy_async_smem();
       asm volatile("bar.sync 1, 256;" ::: "memory");
       if (etid == 0) {
@@ -1654,15 +1512,9 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
         tma_store_commit();
       }
       obuf ^= S::kOutBufs - 1;
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
     if (etid == 0) tma_store_wait_all();
   }
-
-  tc_fence_before();
-  cluster_sync_all();      // neither CTA may exit (or free TMEM) while its peer still uses it
-  if (warp == 2) tmem_dealloc_2cta<kTmemCols>(tmem_base);
 }
 
 template <int BN, int STAGES, int EPI>
@@ -1727,22 +1579,18 @@ inline int launch_conv_gn(const ConvParams& p, int bn, int num_sms, cudaStream_t
     const char* e = getenv("NOPE_GN_EPI");
     return e && atoi(e) == 3 ? 3 : 4;
   }();
-  // NOPE_GN_SHORTK=k: layers of <= k K-steps per tile take the 4-deep ring + two staging buffers.  Measured (ncu launch
-  // list, to_qkv 192 -> 384 at 32x32, 3 K-steps per tile): 275 us against 203 us on the 6-deep ring with one staging
-  // buffer -- these layers are bound by load latency (two tiles in flight beat a free staging buffer): default off
-  static const int short_k = getenv("NOPE_GN_SHORTK") ? atoi(getenv("NOPE_GN_SHORTK")) : 0;
+  // ring depths: the deepest ring that fits 227 KB of shared memory beside the staging buffers
   if (epi == 3) {
     switch (bn) {
-      case 192: return launch_conv_tc2_t<192, 6, 3>(p, num_sms, stream);
-      case 128: return launch_conv_tc2_t<128, 6, 3>(p, num_sms, stream);
-      case 64: return launch_conv_tc2_t<64, 8, 3>(p, num_sms, stream);
+      case 192: return launch_conv_tc2_t<192, 4, 3>(p, num_sms, stream);
+      case 128: return launch_conv_tc2_t<128, 4, 3>(p, num_sms, stream);
+      case 64: return launch_conv_tc2_t<64, 6, 3>(p, num_sms, stream);
     }
   } else {
     switch (bn) {
-      case 192: return p.ksteps <= short_k ? launch_conv_tc2_t<192, 4, 4>(p, num_sms, stream)
-                                           : launch_conv_tc2_t<192, 6, 4>(p, num_sms, stream);
-      case 128: return launch_conv_tc2_t<128, 6, 4>(p, num_sms, stream);
-      case 64: return launch_conv_tc2_t<64, 8, 4>(p, num_sms, stream);
+      case 192: return launch_conv_tc2_t<192, 3, 4>(p, num_sms, stream);
+      case 128: return launch_conv_tc2_t<128, 4, 4>(p, num_sms, stream);
+      case 64: return launch_conv_tc2_t<64, 7, 4>(p, num_sms, stream);
     }
   }
   return fail("launch_conv_gn: unsupported BN");
@@ -1752,18 +1600,16 @@ inline int launch_conv_tc2(const ConvParams& p, int bn, int num_sms, cudaStream_
   const bool ex = conv_needs_extras(p);
   if (p.geglu) {
     if (bn != 128 || ex || p.stats || p.n_par != 1) return fail("launch_conv_tc2: GEGLU epilogue needs BN = 128, no extras");
-    return launch_conv_tc2_t<128, 6, 2>(p, num_sms, stream);
+    return launch_conv_tc2_t<128, 5, 2>(p, num_sms, stream);
   }
   switch (bn) {
-    // 256-wide tiles (LDM variant: every width is a multiple of 256): per K-step a CTA reads
-    // 16 KB of A + 16 KB of B for 128 tensor-core clocks, against 16 + 8 KB for 64 clocks at
-    // BN = 128, which sits exactly on the 128 B/clk shared-memory read limit
-    case 256: return ex ? launch_conv_tc2_t<256, 5, 1>(p, num_sms, stream)
-                        : launch_conv_tc2_t<256, 5, 0>(p, num_sms, stream);
-    case 192: return ex ? launch_conv_tc2_t<192, 6, 1>(p, num_sms, stream)
-                        : launch_conv_tc2_t<192, 6, 0>(p, num_sms, stream);
-    case 128: return ex ? launch_conv_tc2_t<128, 6, 1>(p, num_sms, stream)
-                        : launch_conv_tc2_t<128, 6, 0>(p, num_sms, stream);
+    // 256-wide tiles (LDM variant: every width is a multiple of 256): twice the MMA work per byte of A
+    case 256: return ex ? launch_conv_tc2_t<256, 3, 1>(p, num_sms, stream)
+                        : launch_conv_tc2_t<256, 3, 0>(p, num_sms, stream);
+    case 192: return ex ? launch_conv_tc2_t<192, 4, 1>(p, num_sms, stream)
+                        : launch_conv_tc2_t<192, 4, 0>(p, num_sms, stream);
+    case 128: return ex ? launch_conv_tc2_t<128, 5, 1>(p, num_sms, stream)
+                        : launch_conv_tc2_t<128, 5, 0>(p, num_sms, stream);
     case 64: return ex ? launch_conv_tc2_t<64, 8, 1>(p, num_sms, stream)
                        : launch_conv_tc2_t<64, 8, 0>(p, num_sms, stream);
   }

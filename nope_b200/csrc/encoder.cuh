@@ -1,4 +1,4 @@
-// nope_b200 -- template encoder on the tcgen05 convolution kernel, fp32-accurate.
+// nope_b200 -- template encoder on the wgmma convolution kernel, fp32-accurate.
 //
 // Reference: FeatureExtractor.encode_image (src/model/encoder/template.py:47-53) =
 // ResNet-50 without max-pool, layer4 at stride 1 (src/model/encoder/resnet.py:93-152),
@@ -8,7 +8,7 @@
 // better than fp16 (TF32 / fp16 cuDNN are 2-3e-3 off, measured).  fp32 accuracy on fp16 tensor
 // cores comes from split precision: every activation and weight is an fp16 pair
 // (hi = fp16(x), lo = fp16(x - hi), 22 significant bits) and each convolution accumulates the
-// three products A_hi W_hi + A_hi W_lo + A_lo W_hi in the fp32 TMEM accumulator -- for the
+// three products A_hi W_hi + A_hi W_lo + A_lo W_hi in the fp32 accumulator -- for the
 // implicit-GEMM kernel that is simply three K-segments per filter tap over two activation
 // tensor maps.  BatchNorm is folded into the weights / bias in double precision on the host;
 // ReLU, the bottleneck's residual add and the (hi, lo) split of the output run in the conv
@@ -72,7 +72,7 @@ struct EncConv {
   int cin = 0, cout = 0, cout_real = 0, k = 1, stride = 1, K = 0, bn = 0;
   __half* w = nullptr;   // [cout][taps][3][cin] fp16: (W_hi | W_lo | W_hi) per tap
   float* bias = nullptr;
-  CUtensorMap wmap_half;
+  CUtensorMap wmap;
 };
 
 struct ActPair {
@@ -83,7 +83,7 @@ struct ActPair {
 }  // namespace nope
 
 struct nope_encoder {
-  int D = 8, device = 0, num_sms = 148;
+  int D = 8, device = 0, num_sms = 132;
   bool finalized = false;
   std::map<std::string, std::pair<std::vector<int64_t>, std::vector<float>>> host;
   std::map<std::string, std::vector<int64_t>> expected;
@@ -174,7 +174,7 @@ struct nope_encoder {
     NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&L.bias), bias.size() * sizeof(float)));
     owned.push_back(L.bias);
     NOPE_CUDA(cudaMemcpy(L.bias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice));
-    if (make_weight_map(&L.wmap_half, L.w, L.cout, L.K, L.bn / 2)) return -1;
+    if (make_weight_map(&L.wmap, L.w, L.cout, L.K, L.bn)) return -1;
     convs[name] = L;
     return 0;
   }
@@ -302,7 +302,7 @@ struct nope_encoder {
         ksteps += 3 * nch;
       }
     NOPE_CHECK(nseg <= kMaxSeg && ksteps * 64 == L.K, "encoder conv: segment table");
-    p.bmap_half = L.wmap_half;
+    p.bmap2 = L.wmap;
     if (get_map(&m, out.hi, L.cout, g, -1)) return -1;
     for (int t = 0; t < 4; ++t) p.omap[t] = *m;
     p.bias = L.bias;

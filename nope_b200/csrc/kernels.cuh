@@ -1061,7 +1061,7 @@ topk_merge_kernel(const float* __restrict__ gathered, int world, long long pack,
 
 // ----------------------------------------------------------------------------
 // SIMT implicit-GEMM convolution: a slow, obviously-correct CUDA-core twin of the
-// tcgen05 kernel (same packed weights, same segment semantics).  Debug / bring-up
+// wgmma kernel (same packed weights, same segment semantics).  Debug / bring-up
 // only (NOPE_CONV_IMPL=simt); never the default path.
 // mode 0: 3x3 pad 1; mode 1: 1x1; mode 2: pixel-unshuffle(2) + 1x1 (input is 2H x 2W);
 // mode 3: parity-folded nearest-x2 upsample + 3x3 (input is H/2 x W/2, weights [4*Cout][4*Cin]).
@@ -1150,7 +1150,7 @@ __global__ void nhwc_f16_to_nchw_f32_kernel(const __half* __restrict__ x, float*
   }
 }
 
-inline int ew_grid(long long total, int threads = 256, int cap = 148 * 16) {
+inline int ew_grid(long long total, int threads = 256, int cap = 132 * 16) {
   long long g = (total + threads - 1) / threads;
   if (g < 1) g = 1;
   if (g > cap) g = cap;

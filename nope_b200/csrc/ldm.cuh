@@ -12,7 +12,7 @@
 //                     -> conv3x3 with the 1x1 skip_connection folded in as extra K segments
 //                        (or the identity skip added in the epilogue)
 //   SpatialTransformer GN32 (statistics from the ResBlock's last epilogue) -> proj_in -> LN ->
-//                     q|k|v GEMM -> tcgen05 attention -> to_out (+x) -> [+cross term, LN] ->
+//                     q|k|v GEMM -> wgmma attention -> to_out (+x) -> [+cross term, LN] ->
 //                     GEGLU feed-forward (+x) -> proj_out (+x_in)
 //   Downsample        conv3x3 stride 2 through the four stride-2 TMA lattices of its input
 //   Upsample          nearest-x2 + conv3x3 folded into four 2x2 parity kernels
@@ -36,14 +36,14 @@ namespace nope {
 struct LdmConv {
   int mode = 0;   // 0: 3x3 pad 1, 1: 1x1 / linear, 3: nearest-x2 + 3x3 (folded), 4: 3x3 stride 2 pad 1
   int cin = 0, cout = 0, K = 0;
-  int bn = 0;              // tile width of the 2-CTA kernel (up to 256)
+  int bn = 0;              // tile width of the clustered kernel (up to 256)
   int bn1 = 0;             // tile width of the 1-CTA kernel (up to 192)
   int skip_c = 0;          // channels of a folded 1x1 skip_connection / identity residual (extra K columns)
   int k_alg = 0;           // K without identity-residual columns (algorithmic FLOP count)
   bool geglu = false;      // rows permuted to (64 x | 64 gate) tiles; the epilogue emits x * gelu(gate)
   __half* w = nullptr;     // [rows][K] fp16
   float* bias = nullptr;
-  CUtensorMap wmap, wmap_half;
+  CUtensorMap wmap, wmap2;      // weight boxes of bn1 / bn rows
 };
 struct LdmNorm {
   float* gamma = nullptr;
@@ -65,16 +65,16 @@ __global__ void ldm_ref_of_kernel(int* r, int h0, int N, int n) {
 
 struct nope_ldm {
   using HostT = std::pair<std::vector<int64_t>, std::vector<float>>;
-  int mc = 256, ctx = 512, Cl = 4, S0 = 32, rot_dim = 6, device = 0, num_sms = 148;
+  int mc = 256, ctx = 512, Cl = 4, S0 = 32, rot_dim = 6, device = 0, num_sms = 132;
   int nres = 2;
   std::vector<int> mult{1, 2, 4};
   bool finalized = false;
-  int conv_impl = 2;   // 2: tcgen05 CTA pairs (default), 0: tcgen05 1-CTA tiles
-  int attn_impl = 0;   // 0: tcgen05 attention, 1: CUDA-core twin
+  int conv_impl = 2;   // 2: clustered wgmma kernel (default), 0: single-CTA wgmma kernel
+  int attn_impl = 0;   // 0: wgmma attention, 1: CUDA-core twin
   bool fold_residual = true;   // residual adds as identity K-segments of the GEMM (set before finalize)
-  bool wide_tiles = true;   // 256-channel tiles on the 2-CTA kernel where Cout % 256 == 0 (set before finalize)
+  bool wide_tiles = true;   // 256-channel tiles on the clustered kernel where Cout % 256 == 0 (set before finalize)
   bool hoist = true;        // pose-independent prefix once per reference (prestage)
-  bool fuse_geglu = true;   // GEGLU in the projection's epilogue (2-CTA kernel); false: separate kernel
+  bool fuse_geglu = true;   // GEGLU in the projection's epilogue (clustered kernel); false: separate kernel
   int precision = 0;        // 0: fp16 weights; 1: exact weights -- every packed row is [W_hi | W_lo] and the K loop
                             // walks its segment list twice (A W_hi + A W_lo), 2x the MMA work (set before finalize)
   int kp(int K) const { return precision ? 2 * K : K; }
@@ -306,7 +306,7 @@ struct nope_ldm {
     NOPE_CHECK(L.bn != 0 && L.K % 64 == 0, name + ": channel counts must be multiples of 64");
     if (!bias.empty() && upload(bias, &L.bias)) return -1;
     if (make_weight_map(&L.wmap, L.w, rows, kp(L.K), L.bn1)) return -1;
-    if (make_weight_map(&L.wmap_half, L.w, rows, kp(L.K), L.bn / 2)) return -1;
+    if (make_weight_map(&L.wmap2, L.w, rows, kp(L.K), L.bn)) return -1;
     convs[name] = L;
     return 0;
   }
@@ -414,7 +414,7 @@ struct nope_ldm {
     if (make_lin_res(p + ".proj_out", p + ".proj_out.weight", p + ".proj_out.bias")) return -1;
     if (make_lin_res(p + ".to_out", t + ".attn1.to_out.0.weight", t + ".attn1.to_out.0.bias")) return -1;
     if (make_conv(p + ".ff1", t + ".ff.net.0.proj.weight", t + ".ff.net.0.proj.bias", 1)) return -1;
-    {  // the same projection with GEGLU fused into the epilogue (2-CTA kernel): tile t of 128 rows =
+    {  // the same projection with GEGLU fused into the epilogue (clustered kernel): tile t of 128 rows =
        // x rows 64t..64t+63 followed by gate rows inner+64t..inner+64t+63
       const HostT& W = H(t + ".ff.net.0.proj.weight");
       const auto& b = H(t + ".ff.net.0.proj.bias").second;
@@ -670,7 +670,7 @@ struct nope_ldm {
     p.n_amaps = nmaps;
     for (int t = nmaps; t < kMaxAMaps; ++t) p.amap[t] = p.amap[0];
     p.bmap = L.wmap;
-    p.bmap_half = L.wmap_half;
+    p.bmap2 = L.wmap2;
     if (L.mode == 3) {
       for (int t = 0; t < 4; ++t) {
         if (get_map(&m, out, L.cout, g, t)) return -1;
@@ -855,7 +855,7 @@ struct nope_ldm {
   int st_post(const std::string& p, const __half* xs, const int* src_img, const __half* x_in, __half* out, int C,
               int S, int n, const float* cbp, cudaStream_t st) {
     if (ln(norms.at(p + ".ln3"), xs, PJ, cbp + cb_off.at(p), XN, C, S, n, st, src_img)) return -1;
-    // GEGLU: fused into the projection's epilogue on the 2-CTA kernel
+    // GEGLU: fused into the projection's epilogue on the clustered kernel
     if (conv_impl == 2 && fuse_geglu) {
       if (conv(convs.at(p + ".ff1g"), XN, GG, S, n, st)) return -1;
     } else {

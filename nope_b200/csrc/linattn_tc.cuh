@@ -1,4 +1,4 @@
-// nope_b200 -- LinearAttention core on tcgen05 (model_utils.py:403-417), heads = 4, dim_head = 32:
+// nope_b200 -- LinearAttention core on wgmma tensor cores (model_utils.py:403-417), heads = 4, dim_head = 32:
 //   q = softmax_d(q) * scale ; k = softmax_n(k) ; ctx[d,e] = sum_n k[d,n] v[e,n] ; out[e,n] = sum_d ctx[d,e] q[d,n]
 // qkv: [n_img, n_tok, 384] fp16 (q | k | v, each (head, 32)); out: [n_img, n_tok, 128] fp16; n_tok % 128 == 0.
 //
@@ -8,13 +8,14 @@
 //   ctx [128 d x 128 e] += ek^T [128 d x 128 tok] * v [128 tok x 128 e]          per 128-token tile
 //   out [128 tok x 128 e] = qs [128 tok x 128 d] * ctxm [128 d x 128 e]          ctxm = block-diagonal ctx / ksum
 // ek = exp(k - max_n k) and qs = softmax_d(q) * scale are written back IN PLACE over the TMA-loaded tiles
-// by the SIMT warps (fp16), so the token-major tiles serve directly as operands: token-major [tok][channel]
-// is the canonical MN-major SWIZZLE_128B layout for ek^T / v (M resp. N = channel is contiguous, K = token
-// runs over rows) and the canonical K-major layout for qs (K = channel).
+// (fp16), so the token-major tiles serve directly as operands: token-major [tok][channel] is the canonical
+// MN-major SWIZZLE_128B layout for ek^T / v (M resp. N = channel is contiguous, K = token runs over rows) and
+// the canonical K-major layout for qs (K = channel).
 //
 // One persistent CTA per SM; per image: pass 1 streams k (column max), pass 2 streams (k, v) (second read of
 // k comes from L2), pass 3 builds ctxm, pass 4 streams q and stores out.  Warp roles: 0 TMA producer,
-// 1 tcgen05.mma issuer, 2 TMEM allocator, 4..11 SIMT transforms + epilogues.
+// 4..11 (two warpgroups) SIMT transforms, wgmma and epilogues.  Warpgroup w owns rows [64 w, 64 w + 64) of
+// each GEMM: ctx stays in its registers across pass 2, the out tile is written from registers to staging.
 #pragma once
 #include "conv_tc.cuh"
 
@@ -41,13 +42,25 @@ struct LinAttnSmem {
   static constexpr int kTotal = kVecOff + (2 * 128 + 8 * 128) * 4 + 1024;
 };
 
-// MN-major SWIZZLE_128B operand descriptor: 64 MN-elements (128 B) contiguous, 8 K-rows per 1024-byte atom
+// MN-major SWIZZLE_128B wgmma descriptor: 64 MN-elements (128 B) contiguous, 8 K-rows per 1024-byte atom
 // (SBO), the next 64 MN-elements 16 KB further (LBO = the second 64-channel box).
-constexpr uint64_t kDescMN = (static_cast<uint64_t>(16384 >> 4) << 16) | (static_cast<uint64_t>(1024 >> 4) << 32) |
-                             (static_cast<uint64_t>(1) << 46) | (static_cast<uint64_t>(2) << 61);
-// instruction descriptor, kind::f16, fp32 accumulate, M = N = 128; bit 15 / 16: A / B MN-major
-constexpr uint32_t kIdescMN = make_idesc_f16(128, 128, false) | (1u << 15) | (1u << 16);
-constexpr uint32_t kIdescK = make_idesc_f16(128, 128, false);
+constexpr uint64_t kWgDescMN = (static_cast<uint64_t>(16384 >> 4) << 16) | (static_cast<uint64_t>(1024 >> 4) << 32) |
+                               (static_cast<uint64_t>(1) << 62);
+
+template <bool BF>
+__device__ __forceinline__ void linattn_ctx_mma(float (&c)[64], uint32_t a_lo, uint32_t b_lo, int t) {
+#pragma unroll
+  for (int k = 0; k < kBM / 16; ++k)        // 16 tokens = two 8-row atoms = 2048 B
+    Wgmma<128, BF, 1>::mma(c, kWgDescMN | (a_lo + k * 128), kWgDescMN | (b_lo + k * 128), (t | k) != 0 ? 1u : 0u);
+}
+template <bool BF>
+__device__ __forceinline__ void linattn_out_mma(float (&o)[64], uint32_t a_lo, uint32_t b_lo) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {             // K = 128 channels d: 4 steps of 16 per 64-channel box
+    const uint32_t off = (k >> 2) * ((kBM * 128) >> 4) + (k & 3) * 2;
+    Wgmma<128, BF>::mma(o, kWgDescK | (a_lo + off), kWgDescK | (b_lo + off), k != 0 ? 1u : 0u);
+  }
+}
 
 __global__ void __launch_bounds__(kLaThreads, 1) linattn_tc_kernel(const __grid_constant__ LinAttnParams p) {
   using S = LinAttnSmem;
@@ -57,12 +70,6 @@ __global__ void __launch_bounds__(kLaThreads, 1) linattn_tc_kernel(const __grid_
   uint8_t* s_out = smem + S::kOutOff;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + S::kBarOff);   // [slots] TMA landed
   uint64_t* empty = full + kLaSlots;                                 // [slots] slot may be refilled
-  uint64_t* ready = empty + kLaSlots;                                // [slots] transformed in place (SIMT -> MMA)
-  uint64_t* ctx_full = ready + kLaSlots;                             // ctx accumulated (MMA -> SIMT)
-  uint64_t* ctxm_ready = ctx_full + 1;                               // ctxm operand written (SIMT -> MMA)
-  uint64_t* d_full = ctxm_ready + 1;                                 // [2] out tile accumulated
-  uint64_t* d_empty = d_full + 2;                                    // [2] out tile drained
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d_empty + 2);
   float* s_kmax = reinterpret_cast<float*>(smem + S::kVecOff);
   float* s_ksum = s_kmax + 128;
   float* s_scr = s_ksum + 128;                                       // [8 warps][128]
@@ -78,29 +85,15 @@ __global__ void __launch_bounds__(kLaThreads, 1) linattn_tc_kernel(const __grid_
     for (int s = 0; s < kLaSlots; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 1);
-      mbar_init(&ready[s], 1);
-    }
-    mbar_init(ctx_full, 1);
-    mbar_init(ctxm_ready, 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&d_full[a], 1);
-      mbar_init(&d_empty[a], 1);
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_sync();       // the prologue above overlapped the previous kernel's tail; its output is read from here on
-  const uint32_t t_ctx = tmem_base;              // columns [0, 128)
-  const uint32_t t_d0 = tmem_base + 128;         // out-tile accumulators: columns [128, 256), [256, 384)
 
-  // Ring protocol: items are consumed in production order; item i lives in slot i % kLaSlots and EVERY
-  // item completes exactly one phase of full[s] (TMA), ready[s] (SIMT warps: operand usable by the MMA) and
-  // empty[s] (MMA commit, or the SIMT warps for pass-1 items), so all three flip with parity
-  // (i / kLaSlots) & 1.  Per image the item sequence is
+  // Ring protocol: items are consumed in production order; item i lives in slot i % kLaSlots and completes
+  // exactly one phase of full[s] (TMA) and of empty[s] (the compute warps, once done with the tile), so both
+  // flip with parity (i / kLaSlots) & 1.  Per image the item sequence is
   //   T x k (pass 1) | T x (k, v) (pass 2) | T x q (pass 4)
   if (warp == 0) {
     // ===================== TMA producer =====================
@@ -125,76 +118,20 @@ __global__ void __launch_bounds__(kLaThreads, 1) linattn_tc_kernel(const __grid_
       }
       for (int t = 0; t < T; ++t) load(0, t * kBM, img);                   // q
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t fmt = p.bf16 ? ((1u << 7) | (1u << 10)) : 0u;       // A / B format bits of the instruction descriptor
-    uint32_t item = 0, n_img_done = 0, dcount = 0;
-    for (int img = blockIdx.x; img < p.n_img; img += gridDim.x, ++n_img_done) {
-      // parity waits only work for a thread that observes EVERY phase of a barrier: this warp walks the
-      // pass-1 items too, and it (not the SIMT warps) hands their slots back, so the producer can never
-      // run a phase ahead of it
-      for (int t = 0; t < T; ++t, ++item) {
-        mbar_wait(&full[item % kLaSlots], (item / kLaSlots) & 1);
-        mbar_wait(&ready[item % kLaSlots], (item / kLaSlots) & 1);       // SIMT warps are done with the tile
-        if (elect_one()) mbar_arrive(&empty[item % kLaSlots]);
-        __syncwarp();
-      }
-      // ---- pass 2: ctx += ek^T v
-      for (int t = 0; t < T; ++t) {
-        const int sk = item % kLaSlots, sv = (item + 1) % kLaSlots;
-        mbar_wait(&full[sk], (item / kLaSlots) & 1);
-        mbar_wait(&ready[sk], (item / kLaSlots) & 1);                      // ek written in place
-        mbar_wait(&full[sv], ((item + 1) / kLaSlots) & 1);                 // v landed
-        mbar_wait(&ready[sv], ((item + 1) / kLaSlots) & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t adesc = kDescMN | ((smem_base + sk * kLaSlotBytes) >> 4);
-          const uint64_t bdesc = kDescMN | ((smem_base + sv * kLaSlotBytes) >> 4);
-#pragma unroll
-          for (int k = 0; k < kBM / 16; ++k)        // 16 tokens = two 8-row atoms = 2048 B
-            umma_f16(t_ctx, adesc + (uint64_t)(k * 128), bdesc + (uint64_t)(k * 128), kIdescMN | fmt, (t | k) != 0 ? 1u : 0u);
-          umma_commit(&empty[sk]);
-          umma_commit(&empty[sv]);
-          if (t == T - 1) umma_commit(ctx_full);
-        }
-        __syncwarp();
-        item += 2;
-      }
-      // ---- pass 4: out tile = qs ctxm
-      mbar_wait(ctxm_ready, n_img_done & 1);
-      for (int t = 0; t < T; ++t, ++dcount) {
-        const int sq = item % kLaSlots, db = dcount & 1;
-        mbar_wait(&full[sq], (item / kLaSlots) & 1);
-        mbar_wait(&ready[sq], (item / kLaSlots) & 1);                      // qs written in place
-        mbar_wait(&d_empty[db], ((dcount >> 1) & 1) ^ 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_lo = (smem_base + sq * kLaSlotBytes) >> 4;
-          const uint32_t b_lo = (smem_base + S::kCtxOff) >> 4;
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {             // K = 128 channels d: 4 steps of 16 per 64-channel box
-            const uint32_t off = (k >> 2) * ((kBM * 128) >> 4) + (k & 3) * 2;
-            umma_f16(t_d0 + db * 128, kDescHi | (a_lo + off), kDescHi | (b_lo + off), kIdescK | fmt, k != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[sq]);
-          umma_commit(&d_full[db]);
-        }
-        __syncwarp();
-        item += 1;
-      }
-    }
   } else if (warp >= 4) {
-    // ===================== SIMT transforms + epilogues (8 warps) =====================
+    // ===================== SIMT transforms, wgmma, epilogues (8 warps) =====================
     const int tid = threadIdx.x - 128, w8 = warp - 4;
     const int cx = tid & 15;                       // 16-byte chunk column: channels [8 cx, 8 cx + 8)
     const int r0 = tid >> 4;                       // token rows r0 + 16 i
     const int box = cx >> 3, cin = cx & 7;
-    const int q4 = w8 & 3, ch = w8 >> 2;           // TMEM lane quarter / 64-column half of this warp
+    const int wg = tid >> 7;                       // warpgroup: rows [64 wg, 64 wg + 64) of both GEMMs
+    const int fr = 64 * wg + 16 * (w8 & 3) + (lane >> 2);    // accumulator fragment rows fr, fr + 8
+    const int fc = 2 * (lane & 3);                           // fragment columns 8 i + fc, + 1
     const float scale = 0.17677669529663687f;      // 32^-0.5
     const bool bf = p.bf16 != 0;
-    uint32_t item = 0, n_img_done = 0, dcount = 0;
-    for (int img = blockIdx.x; img < p.n_img; img += gridDim.x, ++n_img_done) {
+    const uint32_t smem_base = smem_u32(smem);
+    uint32_t item = 0;
+    for (int img = blockIdx.x; img < p.n_img; img += gridDim.x) {
       // ---- pass 1: per-channel max of k over the image's tokens
       float mx[8];
 #pragma unroll
@@ -216,7 +153,7 @@ __global__ void __launch_bounds__(kLaThreads, 1) linattn_tc_kernel(const __grid_
           }
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (tid == 0) mbar_arrive(&ready[s]);        // the MMA warp returns the slot
+        if (tid == 0) mbar_arrive(&empty[s]);
       }
 #pragma unroll
       for (int i = 0; i < 8; ++i) mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 16));
@@ -234,9 +171,12 @@ __global__ void __launch_bounds__(kLaThreads, 1) linattn_tc_kernel(const __grid_
       float km[8], ks[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) { km[i] = s_kmax[cx * 8 + i]; ks[i] = 0.f; }
-      // ---- pass 2: ek = exp(k - max) in place; column sums of the stored values
+      // ---- pass 2: ek = exp(k - max) in place; column sums of the stored values; ctx += ek^T v
+      float c[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) c[i] = 0.f;
       for (int t = 0; t < T; ++t, item += 2) {
-        const int s = item % kLaSlots;
+        const int s = item % kLaSlots, sv = (item + 1) % kLaSlots;
         mbar_wait(&full[s], (item / kLaSlots) & 1);
         uint8_t* tile = smem + s * kLaSlotBytes + box * (kBM * 128);
 #pragma unroll
@@ -258,11 +198,18 @@ __global__ void __launch_bounds__(kLaThreads, 1) linattn_tc_kernel(const __grid_
         }
         fence_proxy_async_smem();
         asm volatile("bar.sync 1, 256;" ::: "memory");
+        mbar_wait(&full[sv], ((item + 1) / kLaSlots) & 1);              // v landed
+        const uint32_t a_lo = (smem_base + s * kLaSlotBytes + wg * (kBM * 128)) >> 4;
+        const uint32_t b_lo = (smem_base + sv * kLaSlotBytes) >> 4;
+        wgmma_fence();
+        if (bf) linattn_ctx_mma<true>(c, a_lo, b_lo, t);
+        else linattn_ctx_mma<false>(c, a_lo, b_lo, t);
+        wgmma_commit();
+        wgmma_wait<0>();
+        asm volatile("bar.sync 1, 256;" ::: "memory");
         if (tid == 0) {
-          mbar_arrive(&ready[s]);
-          const int sv = (item + 1) % kLaSlots;               // v needs no transform: usable as it lands
-          mbar_wait(&full[sv], ((item + 1) / kLaSlots) & 1);
-          mbar_arrive(&ready[sv]);
+          mbar_arrive(&empty[s]);
+          mbar_arrive(&empty[sv]);
         }
       }
 #pragma unroll
@@ -278,68 +225,26 @@ __global__ void __launch_bounds__(kLaThreads, 1) linattn_tc_kernel(const __grid_
         s_ksum[tid] = a;
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      // ---- pass 3: ctxm[e][d] = ctx[d][e] / ksum[d] inside a head, 0 across heads; fp16, K-major (K = d)
-      mbar_wait(ctx_full, n_img_done & 1);
-      tc_fence_after();
-      {
-        const int d = q4 * 32 + lane;                           // TMEM lane = ctx row d; head of d = q4
+      // ---- pass 3: ctxm[e][d] = ctx[d][e] / ksum[d] inside a head, 0 across heads; fp16, K-major (K = d).
+      // The previous image's out-tile MMAs have all retired, so the ctxm operand buffer is free to overwrite.
+#pragma unroll
+      for (int h8 = 0; h8 < 2; ++h8) {
+        const int d = fr + 8 * h8;
         const float inv = 1.0f / s_ksum[d];
-        uint32_t v[32];
-        // previous image's out-tile MMAs have retired before ctx_full of this image can complete, so the
-        // ctxm operand buffer is free to overwrite
+        uint8_t* cbox = s_ctx + (d >> 6) * (kBM * 128);
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int e0 = ch * 64 + half * 32;                   // 32 columns e0..e0+31 of ctx row d
-          tmem_ld_32x32(t_ctx + (static_cast<uint32_t>(q4 * 32) << 16) + e0, v);
-          tmem_ld_wait();
-          const bool same_head = (e0 >> 5) == q4;
-          uint8_t* cbox = s_ctx + (d >> 6) * (kBM * 128);
+        for (int i = 0; i < 16; ++i) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int e = e0 + j;                               // row of the operand
-            const float val = same_head ? __uint_as_float(v[j]) * inv : 0.f;
+          for (int j = 0; j < 2; ++j) {
+            const int e = 8 * i + fc + j;                       // row of the operand
+            const float val = (e >> 5) == (d >> 5) ? c[4 * i + 2 * h8 + j] * inv : 0.f;
             st16(reinterpret_cast<__half*>(cbox + e * 128 + ((((d & 63) >> 3) ^ (e & 7)) << 4) + (d & 7) * 2), val, bf);
           }
         }
       }
-      tc_fence_before();
       fence_proxy_async_smem();
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (tid == 0) mbar_arrive(ctxm_ready);
-      // ---- pass 4: qs = softmax_d(q) * scale in place; epilogue of the previous tile while the MMA runs
-      auto drain = [&](uint32_t dc, int tok0) {
-        const int db = dc & 1;
-        mbar_wait(&d_full[db], (dc >> 1) & 1);
-        tc_fence_after();
-        if (tid == 0) tma_store_wait_read0();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        const int row = q4 * 32 + lane;
-        uint32_t v[32];
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          tmem_ld_32x32(t_d0 + db * 128 + (static_cast<uint32_t>(q4 * 32) << 16) + ch * 64 + half * 32, v);
-          tmem_ld_wait();
-          uint8_t* srow = s_out + ch * (kBM * 128) + row * 128;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint4 w;
-            w.x = pack2(__uint_as_float(v[j * 8 + 0]), __uint_as_float(v[j * 8 + 1]), bf);
-            w.y = pack2(__uint_as_float(v[j * 8 + 2]), __uint_as_float(v[j * 8 + 3]), bf);
-            w.z = pack2(__uint_as_float(v[j * 8 + 4]), __uint_as_float(v[j * 8 + 5]), bf);
-            w.w = pack2(__uint_as_float(v[j * 8 + 6]), __uint_as_float(v[j * 8 + 7]), bf);
-            *reinterpret_cast<uint4*>(srow + (((half * 4 + j) ^ (row & 7)) << 4)) = w;
-          }
-        }
-        tc_fence_before();
-        fence_proxy_async_smem();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (tid == 0) {
-          mbar_arrive(&d_empty[db]);
-          tma_store_3d(&p.out, s_out, 0, tok0, img);
-          tma_store_3d(&p.out, s_out + kBM * 128, 64, tok0, img);
-          tma_store_commit();
-        }
-      };
+      // ---- pass 4: qs = softmax_d(q) * scale in place; out tile = qs ctxm -> staging -> TMA store
       for (int t = 0; t < T; ++t, ++item) {
         const int s = item % kLaSlots;
         mbar_wait(&full[s], (item / kLaSlots) & 1);
@@ -381,19 +286,39 @@ __global__ void __launch_bounds__(kLaThreads, 1) linattn_tc_kernel(const __grid_
           }
         }
         fence_proxy_async_smem();
+        if (tid == 0) tma_store_wait_read0();      // the previous tile's store has read the staging buffer
         asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (tid == 0) mbar_arrive(&ready[s]);
-        if (t > 0) { drain(dcount, (t - 1) * kBM); ++dcount; }
+        float o[64];
+        const uint32_t a_lo = (smem_base + s * kLaSlotBytes + wg * 64 * 128) >> 4;
+        const uint32_t b_lo = (smem_base + S::kCtxOff) >> 4;
+        wgmma_fence();
+        if (bf) linattn_out_mma<true>(o, a_lo, b_lo);
+        else linattn_out_mma<false>(o, a_lo, b_lo);
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int h8 = 0; h8 < 2; ++h8) {
+          const int row = fr + 8 * h8;
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const int e = 8 * i + fc;
+            *reinterpret_cast<uint32_t*>(s_out + (e >> 6) * (kBM * 128) + row * 128 +
+                                         ((((e & 63) >> 3) ^ (row & 7)) << 4) + (e & 7) * 2) =
+                pack2(o[4 * i + 2 * h8], o[4 * i + 2 * h8 + 1], bf);
+          }
+        }
+        fence_proxy_async_smem();
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (tid == 0) {
+          mbar_arrive(&empty[s]);
+          tma_store_3d(&p.out, s_out, 0, t * kBM, img);
+          tma_store_3d(&p.out, s_out + kBM * 128, 64, t * kBM, img);
+          tma_store_commit();
+        }
       }
-      drain(dcount, (T - 1) * kBM);
-      ++dcount;
     }
     if (tid == 0) tma_store_wait_all();
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<512>(tmem_base);
 }
 
 // fp16 3-D tensor map [n_img][n_tok][C], box {64, 128, 1}, 128-byte swizzle

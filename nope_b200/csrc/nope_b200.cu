@@ -43,7 +43,6 @@ struct ConvLayer {
   __half* w = nullptr;    // [rows][Kp] fp16
   float* bias = nullptr;  // [cout] fp32 or nullptr
   CUtensorMap wmap;
-  CUtensorMap wmap_half;  // BN/2-row box for the 2-CTA kernel
   bool has_map = false;
   // pre-norm folded into this (bias-free 1x1) layer: weights hold W diag(gamma); see GnFuse::pre_*
   float* pre_w1 = nullptr;
@@ -92,16 +91,16 @@ struct Bump {
 }  // namespace
 
 struct nope_unet {
-  int dim = 0, Cl = 0, S0 = 0, rot_dim = 6, cemb = 0, device = 0, num_sms = 148;
+  int dim = 0, Cl = 0, S0 = 0, rot_dim = 6, cemb = 0, device = 0, num_sms = 132;
   int dims[5] = {0, 0, 0, 0, 0};
   bool finalized = false;
-  int conv_impl = 2;   // 0: tcgen05 1-CTA tiles, 1: SIMT debug twin, 2: tcgen05 CTA pairs (default)
+  int conv_impl = 2;   // 0: wgmma single-CTA kernel, 1: SIMT debug twin, 2: clustered wgmma kernel (default)
   bool fuse_gn = true; // GroupNorm / SiLU / pose bias / residual in the conv epilogue (conv_impl 2 only)
   // 0: fp16 operands; 1: exact weights (W_hi + W_lo K-segments, 2x the MMA work); 2: split precision
   // (exact weights + activations carried as hi + lo: A_hi W_hi + A_hi W_lo + A_lo W_hi, 3x);
   // 3: bf16 operands and activations (8-bit mantissa: its own, looser tolerance)
   int precision = 0;
-  int attn_impl = 0;         // LinearAttention core: 0 tcgen05 (token counts >= 128), 1 CUDA cores
+  int attn_impl = 0;         // LinearAttention core: 0 wgmma (token counts >= 128), 1 CUDA cores
   int metric = 0;            // NOPE_METRIC_* of the fused scoring
   float occ_threshold = 0.2f;
   int chunk = 642;
@@ -297,7 +296,6 @@ struct nope_unet {
       if (upload_f32(bkey, &L.bias)) return -1;
     }
     if (make_weight_map(&L.wmap, L.w, rows, L.Kp, L.bn)) return -1;
-    if (make_weight_map(&L.wmap_half, L.w, rows, L.Kp, L.bn / 2)) return -1;
     L.has_map = true;
     convs[name] = L;
     return 0;
@@ -578,7 +576,7 @@ struct nope_unet {
       SimtConvArgs a;
       a.src0 = in0.hi; a.src1 = in1.hi; a.C0 = c0; a.C1 = c1; a.w = L.w; a.bias = L.bias; a.out = out.hi;
       a.n_img = n_img; a.H = So; a.W = So; a.Cout = L.cout; a.K = L.K; a.mode = L.mode;
-      conv_simt_kernel<<<ew_grid((long long)n_img * So * So * L.cout, 256, 148 * 32), 256, 0, st>>>(a);
+      conv_simt_kernel<<<ew_grid((long long)n_img * So * So * L.cout, 256, 132 * 32), 256, 0, st>>>(a);
       NOPE_CUDA(cudaGetLastError());
       if (stats) {
         // the SIMT twin has no fused statistics: produce them in the conv-epilogue format
@@ -663,7 +661,7 @@ struct nope_unet {
       if (alo1) add_seg(map_index(0, 1, 1), t, c1 / 64, wbase + c0);
     }
     p.bmap = L.wmap;
-    p.bmap_half = L.wmap_half;
+    p.bmap2 = L.wmap;
     p.bf16 = bf() ? 1 : 0;
     static const int l2pf = std::getenv("NOPE_L2_PREFETCH") ? std::atoi(std::getenv("NOPE_L2_PREFETCH")) : 0;   // measured 3 % slower when on
     p.l2_prefetch = l2pf;
@@ -1179,7 +1177,7 @@ extern "C" {
 
 const char* nope_last_error(void) { return last_error().c_str(); }
 int nope_abi_version(void) { return kAbiVersion; }
-const char* nope_build_arch(void) { return "sm_100a"; }
+const char* nope_build_arch(void) { return "sm_90a"; }
 
 int nope_unet_create(nope_unet_t** out, int u_net_dim, int latent_ch, int latent_hw, int device) {
   NOPE_CHECK(out != nullptr, "null out pointer");
@@ -1191,7 +1189,7 @@ int nope_unet_create(nope_unet_t** out, int u_net_dim, int latent_ch, int latent
   NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
   cudaDeviceProp prop;
   NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
-  NOPE_CHECK(prop.major == 10, "nope_b200 kernels are built for sm_100a only");
+  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
   auto u = std::make_unique<nope_unet>();
   u->dim = u_net_dim;
   u->Cl = latent_ch;
@@ -1239,7 +1237,7 @@ int nope_unet_set_chunk(nope_unet_t* u, int hyps) {
   return 0;
 }
 int nope_unet_set_conv_impl(nope_unet_t* u, int impl) {
-  NOPE_CHECK(u && impl >= 0 && impl <= 2, "impl must be 0 (tcgen05), 1 (simt) or 2 (tcgen05 2-CTA)");
+  NOPE_CHECK(u && impl >= 0 && impl <= 2, "impl must be 0 (tensor cores), 1 (simt) or 2 (tensor cores, clustered)");
   NOPE_CHECK(impl != 1 || u->precision == 0, "the SIMT debug convolution only runs fp16 weights");
   u->conv_impl = impl;
   return 0;
@@ -1260,7 +1258,7 @@ int nope_unet_set_option(nope_unet_t* u, const char* name, int value) {
   }
   if (std::strcmp(name, "conv_impl") == 0) return nope_unet_set_conv_impl(u, value);
   if (std::strcmp(name, "attn_impl") == 0) {
-    NOPE_CHECK(value == 0 || value == 1, "attn_impl must be 0 (tcgen05) or 1 (CUDA cores)");
+    NOPE_CHECK(value == 0 || value == 1, "attn_impl must be 0 (tensor cores) or 1 (CUDA cores)");
     u->attn_impl = value;
     return 0;
   }
@@ -1438,7 +1436,7 @@ int nope_encoder_create(nope_encoder_t** out, int descriptor_size, int device) {
   NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
   cudaDeviceProp prop;
   NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
-  NOPE_CHECK(prop.major == 10, "nope_b200 kernels are built for sm_100a only");
+  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
   auto e = std::make_unique<nope_encoder>();
   e->D = descriptor_size;
   e->device = device;
@@ -1541,8 +1539,7 @@ int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, i
     NOPE_CUDA(cudaMemcpyAsync(dbias, bias, Cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
   L.bias = dbias;
-  if (impl != 1 && (make_weight_map(&L.wmap, wp, rows, L.K, L.bn) ||
-                    make_weight_map(&L.wmap_half, wp, rows, L.K, L.bn / 2)))
+  if (impl != 1 && (make_weight_map(&L.wmap, wp, rows, L.K, L.bn)))
     return -1;
   if (eng.conv(L, Act(a0, C0), x1 ? Act(a1, C1) : Act(), Act(o, Cout), H, n_img, n_img, st)) return -1;
   if (to_nchw(o, out, n_img, Cout, H * W, st)) return -1;
@@ -1580,8 +1577,7 @@ int nope_op_conv_gn(int impl, int mode, const float* x0, int C0, const float* x1
   ConvLayer L;
   L.mode = mode; L.cin = cin; L.cout = Cout; L.K = cin * taps; L.Kp = L.K; L.bn = pick_bn(Cout); L.w = wp;
   L.bias = const_cast<float*>(bias);
-  if (impl != 1 && (make_weight_map(&L.wmap, wp, Cout, L.K, L.bn) ||
-                    make_weight_map(&L.wmap_half, wp, Cout, L.K, L.bn / 2)))
+  if (impl != 1 && (make_weight_map(&L.wmap, wp, Cout, L.K, L.bn)))
     return -1;
   const int parts = nope_unet::st_parts_of(H);
   float2* stats = nullptr;
@@ -1646,7 +1642,7 @@ int nope_op_conv_gn_fused(int mode, int precision, const float* x0, int C0, cons
   ConvLayer L;
   L.mode = mode; L.cin = cin; L.cout = Cout; L.K = K; L.Kp = Kp; L.bn = pick_bn(Cout); L.w = wp;
   L.bias = const_cast<float*>(bias);
-  if (make_weight_map(&L.wmap, wp, Cout, Kp, L.bn) || make_weight_map(&L.wmap_half, wp, Cout, Kp, L.bn / 2))
+  if (make_weight_map(&L.wmap, wp, Cout, Kp, L.bn))
     return -1;
   NormLayer N;
   N.C = Cout; N.G = std::max(G, 1);
@@ -1713,7 +1709,7 @@ int nope_op_groupnorm(const float* x, const float* gamma, const float* beta, int
 
 int nope_op_linear_attention(int impl, const float* qkv, float* out, int n_img, int H, int W, void* stream) {
   NOPE_CHECK(qkv && out, "null argument");
-  NOPE_CHECK(impl == 1 || (impl == 0 && (H * W) % kBM == 0), "impl 0 (tcgen05) needs H*W % 128 == 0; impl 1 = CUDA cores");
+  NOPE_CHECK(impl == 1 || (impl == 0 && (H * W) % kBM == 0), "impl 0 (tensor cores) needs H*W % 128 == 0; impl 1 = CUDA cores");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   Scratch s;
   __half *a = nullptr, *o = nullptr;
@@ -1798,7 +1794,7 @@ int nope_ldm_create(nope_ldm_t** out, int model_channels, int context_dim, int l
   NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
   cudaDeviceProp prop;
   NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
-  NOPE_CHECK(prop.major == 10, "nope_b200 kernels are built for sm_100a only");
+  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
   auto m = std::make_unique<nope_ldm>();
   m->mc = model_channels;
   m->ctx = context_dim;
@@ -1848,8 +1844,8 @@ int nope_ldm_set_chunk(nope_ldm_t* m, int hyps) {
   return 0;
 }
 int nope_ldm_set_impl(nope_ldm_t* m, int conv_impl, int attn_impl) {
-  NOPE_CHECK(m && (conv_impl == 0 || conv_impl == 2), "conv_impl must be 0 (tcgen05) or 2 (tcgen05 2-CTA)");
-  NOPE_CHECK(attn_impl == 0 || attn_impl == 1, "attn_impl must be 0 (tcgen05) or 1 (CUDA cores)");
+  NOPE_CHECK(m && (conv_impl == 0 || conv_impl == 2), "conv_impl must be 0 (tensor cores) or 2 (tensor cores, clustered)");
+  NOPE_CHECK(attn_impl == 0 || attn_impl == 1, "attn_impl must be 0 (tensor cores) or 1 (CUDA cores)");
   m->conv_impl = conv_impl;
   m->attn_impl = attn_impl;
   return 0;
@@ -2015,7 +2011,7 @@ int nope_ldm_run_block(nope_ldm_t* m, const char* name, const float* x0, int C0,
 int nope_op_mh_attention(int impl, const float* qkv, float* out, int n_img, int n_tok, int C, void* stream) {
   NOPE_CHECK(qkv && out && n_img >= 1 && n_tok >= 64 && n_tok % 64 == 0 && C % 64 == 0 && C >= 64,
              "bad arguments (n_tok and C must be multiples of 64)");
-  NOPE_CHECK(impl == 0 || impl == 1, "impl must be 0 (tcgen05) or 1 (CUDA cores)");
+  NOPE_CHECK(impl == 0 || impl == 1, "impl must be 0 (tensor cores) or 1 (CUDA cores)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   nope_ldm e;    // only the attention staging buffers are used; freed by the destructor
   e.attn_impl = impl;

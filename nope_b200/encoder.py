@@ -2,10 +2,10 @@
 
 Two backends behind the reference's `FeatureExtractor` surface:
   * "b200" (default on a CUDA device): the native engine in libnope_b200.so
-    (`nope_encoder_*`, csrc/encoder.cuh) -- the tcgen05 convolution kernel with
+    (`nope_encoder_*`, csrc/encoder.cuh) -- the wgmma convolution kernel with
     split-precision fp16 (hi, lo) operands, fp32-accurate (SURVEY.md section 8 row f1);
-  * "torch": the PyTorch/cuDNN module below in fp32 with TF32 off (row a3; 3.3x slower on
-    B200: cuDNN has no tensor-core path at fp32 accuracy).  Used for CPU tests and as a
+  * "torch": the PyTorch/cuDNN module below in fp32 with TF32 off (row a3; slower: cuDNN has
+    no tensor-core path at fp32 accuracy).  Used for CPU tests and as a
     cross-check; never picked silently on a GPU.
 
 Mirrors reference `FeatureExtractor` (src/model/encoder/template.py:24-53): ResNet-50

@@ -91,7 +91,7 @@ def groupnorm(x, gamma, beta, groups, silu=False, chan_bias=None, residual=None)
 
 
 def linear_attention(qkv, impl="simt"):
-    """impl 'tcgen05' (both contractions on tensor cores; H*W a multiple of 128) or 'simt'."""
+    """impl 'tcgen05' (both contractions on wgmma tensor cores; H*W a multiple of 128) or 'simt'."""
     lib = _lib.load()
     qkv = _f32(qkv)
     n, c, h, w = qkv.shape

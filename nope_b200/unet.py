@@ -179,7 +179,8 @@ class UNet:
         _lib.check(_lib.load().nope_unet_set_metric(self._handle(), _METRICS[metric], float(threshold)))
 
     def set_conv_impl(self, impl):
-        """'tcgen05_2cta' (CTA pairs, default), 'tcgen05' (1-CTA tiles) or 'simt' (debug twin)."""
+        """'tcgen05_2cta' (clustered kernel with the fused epilogues, default), 'tcgen05' (single-CTA
+        wgmma kernel) or 'simt' (debug twin); the names are kept from the first version of the engine."""
         _lib.check(_lib.load().nope_unet_set_conv_impl(
             self._handle(), {"tcgen05": 0, "simt": 1, "tcgen05_2cta": 2}[impl]))
 

@@ -19,7 +19,7 @@ def test_library_builds_and_loads():
     from nope_b200 import _lib
     lib = _lib.load()
     assert lib.nope_abi_version() == _lib.EXPECTED_ABI == 2
-    assert lib.nope_build_arch() == b"sm_100a"
+    assert lib.nope_build_arch() == b"sm_90a"
 
 
 def test_exports_match_header():

@@ -1,4 +1,4 @@
-"""GPU: the CTA-pair (cta_group::2, 256-pixel tile) variant of the tcgen05 convolution
+"""GPU: the clustered variant (conv_tc2.cuh, fused epilogues) of the wgmma convolution
 against the same oracle and cases as the 1-CTA kernel, including odd tile counts (the
 peer CTA of the last pair runs on a fully out-of-range tile) and fused GroupNorm statistics."""
 import pytest

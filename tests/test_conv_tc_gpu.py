@@ -1,4 +1,4 @@
-"""GPU: the tcgen05/TMA implicit-GEMM convolution against the oracle's torch-fp32
+"""GPU: the wgmma/TMA implicit-GEMM convolution against the oracle's torch-fp32
 F.conv2d on the same fp16-rounded operands, for every geometry the UNet uses: 32/16/8/4
 pixel sides (1, 1, 2 and 8 images per 128-row tile), two-source channel concatenation,
 1x1, pixel-unshuffle + 1x1, the 1x1-"image" linear layer, ragged last tiles, and all

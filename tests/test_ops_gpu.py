@@ -71,7 +71,7 @@ def test_linear_attention(dev, n, S):
 
 @pytest.mark.parametrize("n,S", [(3, 32), (5, 16), (150, 16), (1, 32)])
 def test_linear_attention_tcgen05(dev, n, S):
-    """The tensor-core LinearAttention core (csrc/linattn_tc.cuh): ek^T v and qs ctx as tcgen05 GEMMs over
+    """The tensor-core LinearAttention core (csrc/linattn_tc.cuh): ek^T v and qs ctx as wgmma GEMMs over
     token-major operands (MN-major descriptors), exp / softmax transforms in place.  fp16 operands (ek, qs,
     ctx) add ~3e-4 to the one output rounding of the CUDA-core kernel."""
     from nope_b200 import ops

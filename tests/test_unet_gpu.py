@@ -300,7 +300,7 @@ def test_full_size_grid_properties(gpu_model):
     of an oracle run (642 CPU forwards would take minutes):
       * determinism: the same sweep twice is bit-identical;
       * pose-permutation equivariance: permuting the grid permutes the scores, bit for bit
-        (every hypothesis is an independent forward, whatever tile / CTA pair it lands in);
+        (every hypothesis is an independent forward, whatever tile / cluster it lands in);
       * duplicated poses give identical scores and the top-k tie-break picks the lower index;
       * chunk-size invariance at a size with ragged last tiles (642 = 5*128 + 2)."""
     from nope_b200.poses import synthetic_pose_batch
@@ -366,7 +366,7 @@ def test_shard_size_invariance(gpu_model):
 
 
 def test_native_encoder_matches_oracle_and_torch(gpu_model, seeded_state_dict):
-    """template encoder on the tcgen05 kernel with split-precision operands (SURVEY 8 row f1)
+    """template encoder on the wgmma kernel with split-precision operands (SURVEY 8 row f1)
     vs the oracle's torch-CPU fp32 restatement and vs the cuDNN fp32 module: fp32-level parity
     (the latents feed the score directly; TF32 / fp16 would be 2-3e-3 off)."""
     from oracle import inputs, unet_oracle as orc
