@@ -20,9 +20,9 @@
 //
 // CTA = 12 warps, persistent over (m_tile, n_tile) work items:
 //   warp 0        : TMA producer      (smem ring, full/empty mbarriers; one elected lane issues)
-//   warps 4..11   : two warpgroups: wgmma mainloop (each warpgroup owns half of the tile's columns,
-//                   accumulator in registers), then the fp32 tile through shared memory (conv_mma_tile)
-//                   -> +bias -> GroupNorm partial sums -> fp16 -> swizzled smem -> TMA store
+//   warps 4..11   : two warpgroups: wgmma mainloop (warpgroup w owns rows 64 w .. 64 w + 63 and all of the
+//                   tile's columns, accumulator in registers), then the fp32 tile through shared memory
+//                   (conv_mma_tile) -> +bias -> GroupNorm partial sums -> fp16 -> swizzled smem -> TMA store
 #pragma once
 #include "common.cuh"
 #include <cudaTypedefs.h>
@@ -168,27 +168,31 @@ __device__ __forceinline__ void conv_tile_coords(const ConvParams& p, int m_tile
 // row-per-lane 16-byte reads of the epilogue free of bank conflicts.
 __host__ __device__ constexpr int acc_ld(int BN) { return BN + 4; }
 
-// K loop of one tile for warpgroup wg: columns [wg NS, wg NS + NS) of all 128 rows, two m64 wgmmas (rows 0-63
-// and 64-127) per 16-deep K step, one wgmma group in flight while the previous stage is released.  The operand
-// type is a template parameter, so the loop is one straight wgmma pipeline.
-template <int NS, int STAGES, int kStageBytes, int kABytes, bool BF>
+// Warps of a conv CTA that run the wgmma mainloop when NW warpgroups share a tile: two warpgroups split the tile by
+// rows, a single one takes both row halves.  With NW == 3 the third warpgroup only joins the epilogue.
+__host__ __device__ constexpr int conv_mma_warps(int NW) { return NW < 2 ? 4 * NW : 8; }
+
+// K loop of one tile for one warpgroup: per 16-deep K step, NH m64nNk16 wgmmas, one per 64-row block of A starting at
+// row block a_blk, each against the stage's whole N-row weight tile.  One wgmma group stays in flight while the
+// previous stage is released.  The operand type is a template parameter, so the loop is one straight wgmma pipeline.
+template <int N, int NH, int STAGES, int kStageBytes, int kABytes, bool BF>
 __device__ __forceinline__ void conv_mma_loop(const ConvParams& p, const uint8_t* smem, uint64_t* full_bar,
-                                              uint64_t* empty_bar, int& stage, uint32_t& phase, int wg,
-                                              float (&d0)[NS / 2], float (&d1)[NS / 2]) {
+                                              uint64_t* empty_bar, int& stage, uint32_t& phase, int a_blk,
+                                              float (&d)[NH][N / 2]) {
   const int lane = threadIdx.x & 31;
   int prev = -1;
   for (int ks = 0; ks < p.ksteps; ++ks) {
     mbar_wait(&full_bar[stage], phase);
     const uint8_t* sa = smem + stage * kStageBytes;
-    const uint64_t adesc = wg_desc_k(sa);
-    const uint64_t bdesc = wg_desc_k(sa + kABytes + wg * NS * 128);
+    const uint64_t adesc = wg_desc_k(sa + a_blk * (64 * 128));
+    const uint64_t bdesc = wg_desc_k(sa + kABytes);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < kBK / 16; ++k) {
-      // advance 16 elements (32 B) along K inside the swizzle atom: +2 in the >>4 field; rows 64.. are 8 KB on
+      // advance 16 elements (32 B) along K inside the swizzle atom: +2 in the >>4 field; the next 64 rows are 8 KB on
       const uint32_t acc = (ks | k) != 0 ? 1u : 0u;
-      Wgmma<NS, BF>::mma(d0, adesc + 2 * k, bdesc + 2 * k, acc);
-      Wgmma<NS, BF>::mma(d1, adesc + 512 + 2 * k, bdesc + 2 * k, acc);
+#pragma unroll
+      for (int h = 0; h < NH; ++h) Wgmma<N, BF>::mma(d[h], adesc + 512 * h + 2 * k, bdesc + 2 * k, acc);
     }
     wgmma_commit();
     wgmma_wait<1>();            // the previous K-step's group has retired: its stage may be refilled
@@ -200,25 +204,35 @@ __device__ __forceinline__ void conv_mma_loop(const ConvParams& p, const uint8_t
   if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 }
 
-// Mainloop of one 128 x BN tile, run by the NW warpgroups of threads [128, 128 + 128 NW).  Warpgroup w
-// accumulates columns [w BN / NW, (w + 1) BN / NW) of all 128 rows in registers, then the tile is written as
-// fp32 to s_acc, the front of the operand ring.  The ring is idle by then (every stage of this tile has been
-// consumed) and the producer refills it only after the epilogue has read the tile back (tempty barrier), so
-// accumulator and operands share the memory.
-template <int BN, int NW, int STAGES, int kStageBytes, int kABytes>
+// Mainloop of one 128 x BN tile, run by the NW warpgroups of threads [128, 128 + 128 NW).  With NW >= 2, warpgroup
+// w in {0, 1} accumulates rows [64 w, 64 w + 64) x all BN columns in registers, one m64nBNk16 wgmma per 16-deep K
+// step: per K step the tile's operands are read from shared memory once (A) and twice (B), where a split by
+// columns reads A once per warpgroup and B once per row half.  With NW == 1 the warpgroup takes both row halves.
+// The tile is then written as fp32 to s_acc, the front of the operand ring, in the [128][acc_ld(BN)] layout every
+// epilogue reads.  The ring is idle by then (every stage of this tile has been consumed) and the producer refills it
+// only after the epilogue has read the tile back (tempty barrier), so accumulator and operands share the memory.
+template <int BN, int NW, int STAGES, int kStageBytes, int kABytes, bool MMA = true>
 __device__ __forceinline__ void conv_mma_tile(const ConvParams& p, uint8_t* smem, uint64_t* full_bar,
                                               uint64_t* empty_bar, int& stage, uint32_t& phase, float* s_acc) {
-  constexpr int NS = BN / NW;
-  static_assert(NS % 32 == 0 && NS <= 128, "columns per warpgroup");
+  static_assert(NW >= 1 && NW <= 3 && BN % 64 == 0 && BN <= 256, "mainloop warpgroups / tile width");
+  constexpr int NH = NW >= 2 ? 1 : 2;       // 64-row blocks per mainloop warpgroup
   const int wg = (threadIdx.x >> 7) - 1;
-  float d0[NS / 2], d1[NS / 2];
+  static_assert(MMA || NW == 3, "only the third of three warpgroups skips the mainloop");
+  if constexpr (MMA) {                      // NW == 3: warpgroup 2 (MMA = false) waits for the tile at the barriers
+    float d[NH][BN / 2];
 #pragma unroll
-  for (int i = 0; i < NS / 2; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
-  if (p.bf16) conv_mma_loop<NS, STAGES, kStageBytes, kABytes, true>(p, smem, full_bar, empty_bar, stage, phase, wg, d0, d1);
-  else conv_mma_loop<NS, STAGES, kStageBytes, kABytes, false>(p, smem, full_bar, empty_bar, stage, phase, wg, d0, d1);
-  asm volatile("bar.sync 2, %0;" ::"n"(NW * 128) : "memory");      // no warpgroup still reads the ring
-  wg_store_acc<NS>(s_acc, acc_ld(BN), wg * NS, d0, d1);
-  asm volatile("bar.sync 2, %0;" ::"n"(NW * 128) : "memory");
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[h][i] = 0.f;
+    if (p.bf16) conv_mma_loop<BN, NH, STAGES, kStageBytes, kABytes, true>(p, smem, full_bar, empty_bar, stage, phase, wg, d);
+    else conv_mma_loop<BN, NH, STAGES, kStageBytes, kABytes, false>(p, smem, full_bar, empty_bar, stage, phase, wg, d);
+    asm volatile("barrier.sync 2, %0;" ::"n"(NW * 128) : "memory");    // no warpgroup still reads the ring
+#pragma unroll
+    for (int h = 0; h < NH; ++h) wg_store_acc64<BN>(s_acc, acc_ld(BN), 64 * (wg + h), d[h]);
+  } else {
+    asm volatile("barrier.sync 2, %0;" ::"n"(NW * 128) : "memory");
+  }
+  asm volatile("barrier.sync 2, %0;" ::"n"(NW * 128) : "memory");
 }
 
 // The epilogue has read the accumulator tile out of the ring: order its generic-proxy accesses before the
@@ -475,7 +489,7 @@ conv_tc_kernel(const __grid_constant__ ConvParams p) {
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kEpiWarps);
+      mbar_init(&empty_bar[s], conv_mma_warps(2));
     }
     mbar_init(tempty_bar, kEpiWarps);
     fence_mbar_init();

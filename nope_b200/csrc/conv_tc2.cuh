@@ -5,8 +5,10 @@
 // (m_pair, n_tile) -> M-tiles 2 m_pair and 2 m_pair + 1, one per CTA), so the two CTAs of a pair
 // read the same weight tile at the same time and the second read is served by L2.  Each CTA
 // TMA-loads its own 128 pixel rows of A and the whole BN-row weight tile, and its epilogue
-// warpgroups run the wgmma mainloop (conv_mma_tile): warpgroup w accumulates its share of the
-// tile's columns in registers, the fp32 tile then passes through shared memory to the epilogue.
+// warpgroups run the wgmma mainloop (conv_mma_tile): warpgroups 0 and 1 accumulate 64 rows x all
+// BN columns each in registers (a single warpgroup takes both row halves; a third one only joins the
+// epilogue), the fp32 tile then passes through shared memory to the epilogue.  setmaxnreg moves
+// registers from the control warpgroup (warps 0-3) to the math warpgroups (conv2_math_regs).
 //
 // Tile widths: 192 (the default UNet: every width is a multiple of 192), 256 (the LDM variant:
 // multiples of 256), 128 / 64 (template encoder, GEGLU).  Tiles of <= 128 columns double-buffer
@@ -20,7 +22,7 @@
 //
 // Protocol (per CTA):
 //   full[s]   count 1: the producer's arrive.expect_tx; the stage's TMA loads complete_tx on it
-//   empty[s]  one arrive per epilogue (mainloop) warp once its wgmma reads of the stage retired
+//   empty[s]  one arrive per mainloop warp (conv_mma_warps) once its wgmma reads of the stage retired
 //   tempty    one arrive per epilogue warp once the accumulator tile has been read out of the ring;
 //             the producer waits for it before it loads the next tile
 #pragma once
@@ -154,7 +156,7 @@ __device__ __forceinline__ float silu_ftz(float x) {
 __host__ __device__ constexpr int gn_epi_warps(int BN) { return 4 * (BN / 64); }           // one (lane quarter, 64-column sub-tile) each
 __host__ __device__ constexpr int gn_threads(int BN) { return 128 + 32 * gn_epi_warps(BN); }
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool MMA>
 __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8_t* smem, uint64_t* full_bar,
                                                       uint64_t* empty_bar, uint64_t* tempty_bar, uint64_t* res_bar,
                                                       int tile0, int tile_step, int num_tiles, uint32_t rank) {
@@ -264,7 +266,7 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
     NOPE_EPI_BAR();
     NOPE_TS(1);
     if (!(g.dbg & 16)) fetch_pb(tile + tile_step);
-    conv_mma_tile<BN, BN / 64, STAGES, S::kStageBytes, S::kABytes>(p, smem, full_bar, empty_bar, kstage, kphase, s_acc);
+    conv_mma_tile<BN, BN / 64, STAGES, S::kStageBytes, S::kABytes, MMA>(p, smem, full_bar, empty_bar, kstage, kphase, s_acc);
     NOPE_TS(2);
 
     // ---- pass 1: accumulator -> registers, free the ring, per-octet partial sums
@@ -699,7 +701,7 @@ __device__ __forceinline__ void gn2_pass2_octets(float* f, uint32_t a_sc, uint32
 }
 
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool MMA>
 __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t* smem, uint8_t* gsm,
                                                     const Gn2Bars& B, int tile0, int tile_step, int num_tiles,
                                                     uint32_t rank) {
@@ -761,7 +763,7 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
     const __half* pb_row = g.pb + (size_t)(img_ok ? img0 + it : 0) * g.pb_stride + g.pb_off + n_chan0 + cc * 64;
     if (g.pb && live) asm volatile("prefetch.global.L1 [%0];" ::"l"(pb_row));
 
-    conv_mma_tile<BN, BN / 64, STAGES, S::kStageBytes, S::kABytes>(p, smem, B.full, B.empty, kstage, kphase, s_acc);
+    conv_mma_tile<BN, BN / 64, STAGES, S::kStageBytes, S::kABytes, MMA>(p, smem, B.full, B.empty, kstage, kphase, s_acc);
     NOPE_TS(1);
     // ---- pass 1: accumulator -> registers, free the ring, per-octet partial sums
     uint32_t a[64];
@@ -1330,12 +1332,35 @@ __device__ __forceinline__ void conv_gn2_store_warp(const ConvParams& p, uint8_t
 }
 
 // EPI: 0 = plain epilogue (the sweep), 1 = extras (ReLU / residual / hi-lo / fp32), 2 = GEGLU
+// Register split (setmaxnreg) of the clustered kernel at 384 and 512 threads: the control warpgroup (warps 0-3: the
+// producer, and with EPI == 4 the store and statistics warps) drops to conv2_ctl_regs, the math warpgroups share the
+// rest of the 64 K register file evenly: 224 per thread at 384 threads (208 with EPI == 4), 144 at 512 threads
+// (BN = 192, EPI 3 / 4).  Blocks of 256 threads already allow 255 registers per thread and keep that limit.
+// Not every instantiation is spill-free (ptxas -v, spill store / load bytes): <192,3,4> 126 / 212 (148 / 236 with the
+// column split at 128 registers), spread over the statistics warp at 80 and the math warps at 144; at 512 threads
+// the four warpgroups average 128 registers, and moving registers between the roles moves the spills with them.
+// <128,4,4> 56 / 108 (statistics warp and epilogue), <128,4,3> 8 / 32, <192,4,3> 548 / 688 (the lock-step A/B
+// epilogue at 144), <256,3,1> 120 / 136 (the extras epilogue, not the K loop: the column split spills 232 / 232
+// there too, so the row split stays on for it).
+__host__ __device__ constexpr int conv2_threads(int BN, int EPI) { return EPI >= 3 ? gn_threads(BN) : kConvThreads; }
+__host__ __device__ constexpr int conv2_ctl_regs(int EPI) { return EPI == 4 ? 80 : 56; }
+__host__ __device__ constexpr int conv2_launch_regs(int threads) { return 65536 / threads / 8 * 8; }
+__host__ __device__ constexpr int conv2_math_regs(int threads, int EPI) {
+  return (conv2_launch_regs(threads) * (threads / 128) - conv2_ctl_regs(EPI)) / (threads / 128 - 1) / 8 * 8;
+}
+
 template <int BN, int STAGES, int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(EPI >= 3 ? gn_threads(BN) : kConvThreads, 1)
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(conv2_threads(BN, EPI), 1)
 conv_tc2_kernel(const __grid_constant__ ConvParams p) {
   using S = Conv2Smem<BN, STAGES, EPI>;
   static_assert(BN % 64 == 0 && BN <= 256, "BN must be a multiple of 64");
-  constexpr int kMathWarps = EPI >= 3 ? gn_epi_warps(BN) : kEpiWarps;   // warps 4.. run mainloop + epilogue
+  constexpr int kThreads = conv2_threads(BN, EPI);
+  constexpr int kMathWarps = kThreads / 32 - 4;                        // warps 4.. run mainloop + epilogue
+  constexpr bool kRegSplit = kThreads > 256;
+  constexpr int kCtlRegs = conv2_ctl_regs(EPI);
+  constexpr int kMathRegs = conv2_math_regs(kThreads, EPI);
+  static_assert(!kRegSplit || (kMathRegs <= 256 && kCtlRegs + (kThreads / 128 - 1) * kMathRegs <=
+                               conv2_launch_regs(kThreads) * (kThreads / 128)), "register split");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -1365,7 +1390,7 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kMathWarps);
+      mbar_init(&empty_bar[s], conv_mma_warps(kMathWarps / 4));
     }
     mbar_init(tempty_bar, kMathWarps);
     mbar_init(res_bar, 1);
@@ -1386,8 +1411,18 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
   // and may overlap the tail of the previous kernel in the stream; from here on the kernel reads what that kernel
   // wrote.  The next kernel's CTAs may be scheduled as soon as this grid's CTAs retire.
   pdl_sync();
+  auto gn2_bars = [&] {                                               // EPI == 4
+    Gn2Bars B;
+    B.full = full_bar; B.empty = empty_bar; B.tempty = tempty_bar; B.res[0] = res_bar; B.res[1] = &gn2_bar[7];
+    B.part = &gn2_bar[0]; B.stats = &gn2_bar[1]; B.tabfree = &gn2_bar[3]; B.out = &gn2_bar[5];
+    return B;
+  };
+  uint8_t* gsm = smem + S::kGnOffset;
 
-  if (warp == 0) {
+  // Each warpgroup sets its register limit once, before its warps take their roles (setmaxnreg is warpgroup-wide).
+  if (warp < 4) {
+    if constexpr (kRegSplit) setmaxnreg_dec<kCtlRegs>();
+    if (warp == 0) {
     // ===================== TMA producer =====================
     int stage = 0;
     uint32_t phase = 0;
@@ -1437,24 +1472,35 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
         }
       }
     }
-  } else if (EPI == 4 && warp >= 2) {
-    // ===================== mainloop + epilogue with GroupNorm fused, bookkeeping on warps 2 / 3 =====================
-    if constexpr (EPI == 4) {
-      Gn2Bars B;
-      B.full = full_bar; B.empty = empty_bar; B.tempty = tempty_bar; B.res[0] = res_bar; B.res[1] = &gn2_bar[7];
-      B.part = &gn2_bar[0]; B.stats = &gn2_bar[1]; B.tabfree = &gn2_bar[3]; B.out = &gn2_bar[5];
-      uint8_t* gsm = smem + S::kGnOffset;
+    } else if constexpr (EPI == 4) {
+      // ===================== GroupNorm-fused epilogue: store warp 2, statistics warp 3 =====================
+      const Gn2Bars B = gn2_bars();
       if (warp == 2) conv_gn2_store_warp<BN, STAGES>(p, smem, gsm, B, tile0, tile_step, num_tiles, rank);
       else if (warp == 3) conv_gn2_stats_warp<BN, STAGES>(p, gsm, B, tile0, tile_step, num_tiles, rank);
-      else conv_gn2_math_warps<BN, STAGES>(p, smem, gsm, B, tile0, tile_step, num_tiles, rank);
     }
-  } else if (warp >= 4 && EPI == 3) {
+  } else if constexpr (EPI == 4) {
+    // ===================== mainloop + epilogue with GroupNorm fused, bookkeeping on warps 2 / 3 =====================
+    if constexpr (kRegSplit) setmaxnreg_inc<kMathRegs>();
+    if (warp >= 12) {                       // BN = 192: the third math warpgroup runs the epilogue only
+      if constexpr (kMathWarps == 12) conv_gn2_math_warps<BN, STAGES, false>(p, smem, gsm, gn2_bars(), tile0, tile_step, num_tiles, rank);
+    } else {
+      conv_gn2_math_warps<BN, STAGES, true>(p, smem, gsm, gn2_bars(), tile0, tile_step, num_tiles, rank);
+    }
+  } else if constexpr (EPI == 3) {
     // ===================== mainloop + epilogue with GroupNorm fused =====================
-    if constexpr (EPI == 3)
-      conv_gn_epilogue_loop<BN, STAGES>(p, smem, full_bar, empty_bar, tempty_bar, res_bar, tile0, tile_step,
-                                        num_tiles, rank);
-  } else if (warp >= 4) {
+    if constexpr (kRegSplit) setmaxnreg_inc<kMathRegs>();
+    if (warp >= 12) {                       // BN = 192: the third math warpgroup runs the epilogue only
+      if constexpr (kMathWarps == 12)
+        conv_gn_epilogue_loop<BN, STAGES, false>(p, smem, full_bar, empty_bar, tempty_bar, res_bar, tile0, tile_step,
+                                                 num_tiles, rank);
+    } else {
+      conv_gn_epilogue_loop<BN, STAGES, true>(p, smem, full_bar, empty_bar, tempty_bar, res_bar, tile0, tile_step,
+                                              num_tiles, rank);
+    }
+  } else {
     // ===================== mainloop + epilogue (own 128 rows, 8 warps) =====================
+    static_assert(kRegSplit, "the plain epilogues run 384 threads");
+    setmaxnreg_inc<kMathRegs>();
     const int e = warp - 4;
     const int etid = threadIdx.x - 128;
     int kstage = 0;
@@ -1538,7 +1584,7 @@ inline int launch_conv_tc2_t(const ConvParams& p, int num_sms, cudaStream_t stre
       cudaLaunchConfig_t cfg;
       memset(&cfg, 0, sizeof cfg);
       cfg.gridDim = dim3(num_sms, 1, 1);
-      cfg.blockDim = dim3(EPI >= 3 ? gn_threads(BN) : kConvThreads, 1, 1);
+      cfg.blockDim = dim3(conv2_threads(BN, EPI), 1, 1);
       cfg.dynamicSmemBytes = S::kTotal;
       cudaLaunchAttribute at;
       at.id = cudaLaunchAttributeClusterDimension;
@@ -1558,7 +1604,7 @@ inline int launch_conv_tc2_t(const ConvParams& p, int num_sms, cudaStream_t stre
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.gridDim = dim3(2 * clusters, 1, 1);
-  cfg.blockDim = dim3(EPI >= 3 ? gn_threads(BN) : kConvThreads, 1, 1);
+  cfg.blockDim = dim3(conv2_threads(BN, EPI), 1, 1);
   cfg.dynamicSmemBytes = S::kTotal;
   cfg.stream = stream;
   cudaLaunchAttribute at;

@@ -810,9 +810,11 @@ struct nope_unet {
     // the split-precision modes execute 2x / 3x the K-steps of the fp16 mode
     prof_flops.push_back(2.0 * (double)n_img * So * So * (double)L.cout * (double)ksteps * 64.0);
     prof_alg.push_back(2.0 * (double)n_img * So * So * (double)L.cout * (double)L.K);
+    prof_shape.push_back(make_int4(So, L.mode, L.cout, L.K));
     return rc;
   }
   std::vector<double> prof_alg;     // algorithmic (fp16-mode) FLOPs of the same launches
+  std::vector<int4> prof_shape;     // (GEMM resolution, mode 0 3x3 / 1 1x1 / 2 unshuffle / 3 folded upsample, Cout, K)
 
   // pixel slabs per image for the GroupNorm kernels: as few as keep >= ~4 CTAs per SM in
   // flight (every CTA pays a fixed statistics prologue), at most 8, and >= 32 pixels each
@@ -1293,6 +1295,7 @@ int nope_unet_profile(nope_unet_t* u, int enable) {
   u->prof_ev.clear();
   u->prof_flops.clear();
   u->prof_alg.clear();
+  u->prof_shape.clear();
   u->profile = enable != 0;
   return 0;
 }
@@ -1312,11 +1315,13 @@ int nope_unet_profile_read(nope_unet_t* u, double* conv_ms, double* conv_flops, 
   }
   if (const char* path = std::getenv("NOPE_PROF_DUMP")) {     // development aid: per-launch table
     if (FILE* f = std::fopen(path, "a")) {
-      std::fprintf(f, "# launch,ms,executed_gflop,algorithmic_gflop\n");
+      std::fprintf(f, "# launch,ms,executed_gflop,algorithmic_gflop,res,mode,cout,k\n");
       for (size_t i = 0; i < u->prof_flops.size(); ++i) {
         float t = 0.f;
         cudaEventElapsedTime(&t, u->prof_ev[2 * i], u->prof_ev[2 * i + 1]);
-        std::fprintf(f, "%zu,%.4f,%.3f,%.3f\n", i, t, u->prof_flops[i] / 1e9, u->prof_alg[i] / 1e9);
+        const int4 sh = u->prof_shape[i];
+        std::fprintf(f, "%zu,%.4f,%.3f,%.3f,%d,%d,%d,%d\n", i, t, u->prof_flops[i] / 1e9, u->prof_alg[i] / 1e9, sh.x,
+                     sh.y, sh.z, sh.w);
       }
       std::fclose(f);
     }
