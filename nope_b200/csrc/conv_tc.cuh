@@ -90,8 +90,6 @@ struct GnFuse {
   float pre_inv_cnt;         // 1 / (H*W * Cin)
   const float* pre_w1;       // [n_total]
   const float* pre_wb;       // [n_total]
-  int dbg;               // development knobs (NOPE_GN_DBG): 1 skip the poll, 2 skip SiLU, 4 skip pass 2 math
-  unsigned long long* ts;  // development: per (CTA, tile iteration) phase timestamps [grid][64][8] (globaltimer, ns)
 };
 
 struct ConvParams {
@@ -108,7 +106,6 @@ struct ConvParams {
   // (py, px) shifts every tap by (+py, +px), reads weight rows parity * n_per_par + ..., and
   // stores through omap[parity] (the stride-2 sub-lattice of the 2H x 2W output).
   int bf16;           // operands and the stored output are bf16 instead of fp16 (plain / GroupNorm-fused epilogues)
-  int l2_prefetch;    // clustered kernel: the producer prefetches the next tile's activation rows into L2
   int n_par;          // 1 or 4
   int n_tiles_par;    // channel tiles per parity (== n_tiles when n_par == 1)
   int src_w, src_hw;  // n_par == 4: width / pixels of one SOURCE image (out_lo addressing)

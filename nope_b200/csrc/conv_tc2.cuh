@@ -49,14 +49,6 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// L2 prefetch of one activation box (no shared-memory destination, no barrier), issued by the producer one tile ahead.
-// Measured (ConvParams::l2_prefetch, NOPE_L2_PREFETCH=1): 3 % SLOWER over the sweep -- the ring's look-ahead already
-// covers the HBM latency and the extra requests only compete with it; off by default
-__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* m, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
 // shared-memory map of the EPI == 4 epilogue (conv_gn2_* below), relative to Conv2Smem::kGnOffset
 template <int BN>
 struct Gn2Smem {
@@ -92,11 +84,6 @@ struct Conv2Smem {
   static_assert(kTotal <= 227 * 1024, "shared memory per block");
 };
 
-__device__ __forceinline__ unsigned long long global_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
 // 8-byte {value, tag} words of the cross-CTA partial-sum exchange: single-copy atomic, L2-coherent
 __device__ __forceinline__ uint2 ld_volatile_u2(const uint2* p) {
   uint2 r;
@@ -195,7 +182,6 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
 
   int obuf = 0;
   uint32_t res_phase = 0;
-  int iter = 0;
   int kstage = 0;
   uint32_t kphase = 0;
   float* s_acc = reinterpret_cast<float*>(smem);
@@ -221,8 +207,7 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
         tma_load_4d(dst + c2 * (kBM * 128), &p.rmap, res_bar, nt * BN + c2 * 64, 0, yy, rb);
     }
   };
-  const bool res_late = (g.dbg & 8) != 0;      // development: issue the residual load inside the tile (after the publish)
-  if (etid == 0 && !res_late) stage_residual(tile0, 0);
+  if (etid == 0) stage_residual(tile0, 0);
   // pose-bias rows of the NEXT tile are fetched into a register while the current tile is normalised
   uint4 pb_next = make_uint4(0, 0, 0, 0);
   auto fetch_pb = [&](int t) {
@@ -238,9 +223,7 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
   };
   static_assert(8 * kOct <= kEpiThreads, "one thread per (image, octet) of the pose-bias rows");
   fetch_pb(tile0);
-#define NOPE_TS(k) do { if (g.ts && etid == 0 && iter < 64) g.ts[((size_t)blockIdx.x * 64 + iter) * 16 + (k)] = global_ns(); } while (0)
-  for (int tile = tile0; tile < num_tiles; tile += tile_step, ++iter) {
-    NOPE_TS(0);
+  for (int tile = tile0; tile < num_tiles; tile += tile_step) {
     const int m_pair = tile / p.n_tiles;
     const int n_tile = tile - m_pair * p.n_tiles;
     const int m_tile = 2 * m_pair + (int)rank;
@@ -260,14 +243,11 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
         s_beta[etid] = __ldg(g.pre_wb + n_chan0 + etid);
       }
     }
-    if (g.dbg & 16) fetch_pb(tile);
     if (g.pb && etid < g.ipt * kOct)
       *reinterpret_cast<uint4*>(s_pb + (etid / kOct) * BN + (etid % kOct) * 8) = pb_next;
     NOPE_EPI_BAR();
-    NOPE_TS(1);
-    if (!(g.dbg & 16)) fetch_pb(tile + tile_step);
+    fetch_pb(tile + tile_step);
     conv_mma_tile<BN, BN / 64, STAGES, S::kStageBytes, S::kABytes, MMA>(p, smem, full_bar, empty_bar, kstage, kphase, s_acc);
-    NOPE_TS(2);
 
     // ---- pass 1: accumulator -> registers, free the ring, per-octet partial sums
     uint32_t a[64];
@@ -277,7 +257,6 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
       acc_ld_32(a_row + 32, *reinterpret_cast<uint32_t(*)[32]>(&a[32]));
       acc_release(tempty_bar, lane);
     }
-    if (res_late && etid == 0 && (!live || g.G == 0 || g.expected == 1)) stage_residual(tile, obuf);
     if (live) {
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
@@ -310,7 +289,6 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
       }
       if (g.G > 0) {
         NOPE_EPI_BAR();
-        NOPE_TS(3);
         float Sx = 0.f, Qx = 0.f;
         if (etid < npairs) {
           const int ii = etid / g.gpt, gl = etid - ii * g.gpt;
@@ -334,10 +312,9 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
             st_volatile_u2(xp + ((size_t)slot * npairs + etid) * 2, make_uint2(__float_as_uint(Sx), g.epoch));
             st_volatile_u2(xp + ((size_t)slot * npairs + etid) * 2 + 1, make_uint2(__float_as_uint(Qx), g.epoch));
           }
-          if (res_late && etid == 0) stage_residual(tile, obuf);
           if (etid < g.expected * npairs * 2) {
             uint2 u = ld_volatile_u2(xp + etid);
-            if (u.y != g.epoch && !(g.dbg & 1)) {
+            if (u.y != g.epoch) {
               const long long t0 = clock64();
               do {
                 u = ld_volatile_u2(xp + etid);
@@ -347,7 +324,6 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
             s_x[etid] = __uint_as_float(u.x);
           }
           NOPE_EPI_BAR();
-          NOPE_TS(4);
           if (use_tab) {
             // one image per tile: per-channel scale / shift tables, y = x * sc[c] + sh[c]; every channel's
             // thread sums its group's partials itself (fixed slot order), no (mean, rstd) hand-over
@@ -410,7 +386,6 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
       }
 
       // ---- pass 2: normalise / activate / add, in place in the swizzled staging tile
-      NOPE_TS(5);
       if (g.has_res) mbar_wait(res_bar, res_phase);
       float e1 = 0.f, e2 = 0.f;
       const uint32_t tok = order_token(smem_u32(smem));          // tables below are read after the barrier above
@@ -427,8 +402,8 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
           ? (long long)((g.res_base + b0) / g.res_div) * hw + (m_tile % g.mt) * kBM + row
           : (long long)grow;
       uint8_t* srow = ost + cc * (kBM * 128) + row * 128;
-      const bool do_norm = g.G > 0 && !(g.dbg & 4);
-      const bool do_silu = g.silu && !(g.dbg & 2);
+      const bool do_norm = g.G > 0;
+      const bool do_silu = g.silu;
       const bool pre = g.pre_stats != nullptr;
       // Every step below runs over all 64 values of the thread with its (launch-uniform) condition tested
       // OUTSIDE the unrolled loop: one long basic block per step, so the scheduler can keep tens of
@@ -563,7 +538,6 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
       }
       fence_proxy_async_smem();
       NOPE_EPI_BAR();
-      NOPE_TS(6);
       if (etid == 0) {
 #pragma unroll 1
         for (int c2 = 0; c2 < kNS; ++c2)
@@ -571,11 +545,10 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
         tma_store_commit();
       }
     }
-    if (etid == 0 && !res_late) stage_residual(tile + tile_step, obuf ^ (S::kOutBufs - 1));
+    if (etid == 0) stage_residual(tile + tile_step, obuf ^ (S::kOutBufs - 1));
     obuf ^= S::kOutBufs - 1;
   }
   if (etid == 0) tma_store_wait_all();
-#undef NOPE_TS
 #undef NOPE_EPI_BAR
 }
 
@@ -598,8 +571,8 @@ __device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8
 //               read the staging buffer: TMA load of the NEXT tile's residual into it (or a plain arrive), res_bar.
 //
 // Per-channel parameters (bias, gamma, beta, pose-bias rows) are read through the read-only L1 path instead of
-// being staged in shared memory per tile, which removes the staging barrier.  Arithmetic and summation orders
-// are those of EPI == 3: results are bit-identical between the two.
+// being staged in shared memory per tile, which removes the staging barrier.  Results agree with EPI == 3 up to
+// the summation order of the statistics; the two are not bit-identical.
 // ---------------------------------------------------------------------------------------------
 struct Gn2Bars {
   uint64_t* full;       // [STAGES] operand stage landed (producer -> math warps)
@@ -729,7 +702,7 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
   const uint32_t gsm_off = (uint32_t)(gsm - smem);
   // pass-2 variant: the hot epilogue shapes run gn2_pass2_octets, everything else the phase-per-step code
   int variant = -1;
-  if (!(g.out_lo || g.res_lo || (g.dbg & 6))) {
+  if (!(g.out_lo || g.res_lo)) {
     if (g.G > 0 && g.silu) {
       const int nm2 = use_tab ? 0 : 1;
       if (g.pb && !g.has_res && !g.emit) variant = nm2;                                   // Block 1: + pose bias
@@ -738,15 +711,12 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
       variant = g.ipt > 1 ? 7 : 6;                                                        // folded pre-norm (to_qkv)
     }
   }
-  if (g.dbg & 32) variant = -1;
 
   int kstage = 0;
   uint32_t kphase = 0;
   float* s_acc = reinterpret_cast<float*>(smem);
   int iter = 0;
-#define NOPE_TS(k) do { if (g.ts && e == 0 && lane == 0 && iter < 64) g.ts[((size_t)blockIdx.x * 64 + iter) * 16 + (k)] = global_ns(); } while (0)
   for (int tile = tile0; tile < num_tiles; tile += tile_step, ++iter) {
-    NOPE_TS(0);
     const int b = iter & 1;
     const int ob = kNB == 2 ? (iter & 1) : 0;
     uint8_t* ost = ost0 + ob * S::kOutBytes;
@@ -764,7 +734,6 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
     if (g.pb && live) asm volatile("prefetch.global.L1 [%0];" ::"l"(pb_row));
 
     conv_mma_tile<BN, BN / 64, STAGES, S::kStageBytes, S::kABytes, MMA>(p, smem, B.full, B.empty, kstage, kphase, s_acc);
-    NOPE_TS(1);
     // ---- pass 1: accumulator -> registers, free the ring, per-octet partial sums
     uint32_t a[64];
     {
@@ -809,11 +778,8 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
       __syncwarp();
       if (lane == 0) mbar_arrive(B.part);
     }
-    NOPE_TS(2);
     if (wait_stats) mbar_wait(&B.stats[b], (iter >> 1) & 1);
-    NOPE_TS(3);
     mbar_wait(B.res[ob], (iter / kNB) & 1);      // residual tile landed in the staging buffer / the buffer is free
-    NOPE_TS(4);
 
     // ---- pass 2: normalise / activate / add, in place in the swizzled staging tile
     float e1 = 0.f, e2 = 0.f;
@@ -827,8 +793,8 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
         ? (long long)((g.res_base + b0) / g.res_div) * hw + (m_tile % g.mt) * kBM + row
         : (long long)grow;
     uint8_t* srow = ost + cc * (kBM * 128) + row * 128;
-    const bool do_norm = g.G > 0 && !(g.dbg & 4);
-    const bool do_silu = g.silu && !(g.dbg & 2);
+    const bool do_norm = g.G > 0;
+    const bool do_silu = g.silu;
     const bool want_emit = g.emit != nullptr;
     if (variant >= 0) {
       const uint32_t a_srow = tok + (uint32_t)(srow - smem);
@@ -974,9 +940,7 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
       mbar_arrive(&B.out[ob]);
       if (wait_stats) mbar_arrive(&B.tabfree[b]);
     }
-    NOPE_TS(5);
   }
-#undef NOPE_TS
 }
 
 // statistics warp (warp 3) of the EPI == 4 epilogue
@@ -1021,8 +985,6 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
     float* t_sh = t_sc + BN;
     float2* mr = s_mr + b * 64;
     if (iter >= 2) mbar_wait(&B.tabfree[b], ((iter >> 1) - 1) & 1);   // tile iter-2 has read buffer b
-#define NOPE_TS2(k) do { if (g.ts && lane == 0 && iter < 64) g.ts[((size_t)blockIdx.x * 64 + iter) * 16 + (k)] = global_ns(); } while (0)
-    NOPE_TS2(8);
     if (fast) {
       // ---- one image per tile, groups aligned to the lanes' octet blocks: the whole exchange in registers.
       // lane -> (octet block lane >> 2 of kOct / 8 octets, row segment lane & 3); xor tree over the lanes of a group
@@ -1035,7 +997,6 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
         }
       }
       mbar_wait(B.part, iter & 1);
-      NOPE_TS2(9);
       float ax = 0.f, aq = 0.f;
 #pragma unroll
       for (int k = 0; k < kOpl; ++k) {
@@ -1055,7 +1016,6 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
         st_volatile_u2(xp + ((size_t)slot * npairs + pr) * 2, make_uint2(__float_as_uint(ax), g.epoch));
         st_volatile_u2(xp + ((size_t)slot * npairs + pr) * 2 + 1, make_uint2(__float_as_uint(aq), g.epoch));
       }
-      NOPE_TS2(10);
       // word w = (slot * npairs + pair) * 2 + stat; 2 * npairs divides 32, so every word of lane l (w = l + 32 k)
       // belongs to (pair, stat) = l mod (2 npairs): sum over k in registers, then over the lanes of that class
       const int nw = g.expected * npairs * 2;        // <= 256 (host check)
@@ -1070,7 +1030,7 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
         const int w = lane + 32 * k;
-        if (w < nw && u[k].y != g.epoch && !(g.dbg & 1)) {
+        if (w < nw && u[k].y != g.epoch) {
           const long long t0 = clock64();
           do {
             u[k] = ld_volatile_u2(xp + w);
@@ -1080,7 +1040,6 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
         tot += __uint_as_float(u[k].x);
       }
       for (int off = 2 * npairs; off < 32; off <<= 1) tot += __shfl_xor_sync(0xffffffffu, tot, off);
-      NOPE_TS2(11);
       const float o1 = __shfl_sync(0xffffffffu, tot, lane & ~1), o2 = __shfl_sync(0xffffffffu, tot, lane | 1);
       const float mean_l = o1 * g.inv_cnt;                                  // lane l: group (l mod 2 npairs) >> 1
       const float rstd_l = rsqrtf(fmaxf(o2 * g.inv_cnt - mean_l * mean_l, 0.f) + g.eps);
@@ -1097,7 +1056,6 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
     } else
     if (g.G > 0) {
       mbar_wait(B.part, iter & 1);
-      NOPE_TS2(9);
       // sums of this tile per (image, group) pair: fixed order over row segments and channel octets
       float Sx[2], Qx[2];
 #pragma unroll
@@ -1135,7 +1093,6 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
             st_volatile_u2(xp + ((size_t)slot * npairs + pr) * 2 + 1, make_uint2(__float_as_uint(Qx[k]), g.epoch));
           }
         }
-        NOPE_TS2(10);
         const int nw = g.expected * npairs * 2;        // <= 256 (host check)
         uint2 u[8];
 #pragma unroll
@@ -1148,7 +1105,7 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
         for (int k = 0; k < 8; ++k) {
           const int w = lane + 32 * k;
           if (w < nw) {
-            if (u[k].y != g.epoch && !(g.dbg & 1)) {
+            if (u[k].y != g.epoch) {
               const long long t0 = clock64();
               do {
                 u[k] = ld_volatile_u2(xp + w);
@@ -1159,7 +1116,6 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
           }
         }
         __syncwarp();
-        NOPE_TS2(11);
         if (use_tab) {
           // one image per tile: totals per (group, statistic) in slot order, then per-channel scale / shift
           float tot = 0.f;
@@ -1245,9 +1201,7 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&B.stats[b]);
-    NOPE_TS2(12);
   }
-#undef NOPE_TS2
 }
 
 // store warp (warp 2) of the EPI == 4 epilogue
@@ -1298,7 +1252,6 @@ __device__ __forceinline__ void conv_gn2_store_warp(const ConvParams& p, uint8_t
     conv_tile_coords(p, m_tile, b0, y0);
     const int img0 = p.tiles_per_img > 0 ? m_tile / g.mt : m_tile * g.ipt;
     mbar_wait(&B.out[ob], (iter / kNB) & 1);
-    if (g.ts && lane == 0 && iter < 64) g.ts[((size_t)blockIdx.x * 64 + iter) * 16 + 13] = global_ns();
     if (g.emit && lane < g.ipt && img0 + lane < g.n_img) {
       const float2* s_em = s_em0 + ob * 32;
       const int r16 = hw >= kBM ? 8 : (hw >> 4);
@@ -1322,7 +1275,6 @@ __device__ __forceinline__ void conv_gn2_store_warp(const ConvParams& p, uint8_t
       const int nt = tile + kNB * tile_step;
       if (nt < num_tiles) {
         tma_store_wait_read0();
-        if (g.ts && iter < 64) g.ts[((size_t)blockIdx.x * 64 + iter) * 16 + 14] = global_ns();
         stage(nt, ob);
       }
     }
@@ -1436,24 +1388,6 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
       int b0, y0;
       conv_tile_coords(p, m_tile, b0, y0);
       if (iter > 0) mbar_wait(tempty_bar, (iter - 1) & 1);     // the previous accumulator tile left the ring
-      if (p.l2_prefetch && tile + tile_step < num_tiles) {
-        // next tile of this CTA: the un-shifted tap of every source (the other taps re-read the same rows)
-        const int nt = tile + tile_step;
-        const int nmp = nt / p.n_tiles;
-        if (nmp != m_pair) {
-          const int nmt = 2 * nmp + (int)rank;
-          int nb0, ny0;
-          conv_tile_coords(p, nmt, nb0, ny0);
-          if (nmt < p.m_tiles && elect_one()) {
-            for (int s = 0; s < p.nseg; ++s) {
-              const ConvSeg sg = p.seg[s];
-              if (sg.dy != 0 || sg.dx != 0) continue;
-              for (int ch = 0; ch < sg.nchunks; ++ch) tma_prefetch_4d(&p.amap[sg.map], ch * kBK, 0, ny0, nb0);
-            }
-          }
-          __syncwarp();
-        }
-      }
       int kcol = 0;
       for (int s = 0; s < p.nseg; ++s) {
         const ConvSeg sg = p.seg[s];

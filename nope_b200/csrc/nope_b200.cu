@@ -663,8 +663,6 @@ struct nope_unet {
     p.bmap = L.wmap;
     p.bmap2 = L.wmap;
     p.bf16 = bf() ? 1 : 0;
-    static const int l2pf = std::getenv("NOPE_L2_PREFETCH") ? std::atoi(std::getenv("NOPE_L2_PREFETCH")) : 0;   // measured 3 % slower when on
-    p.l2_prefetch = l2pf;
     if (L.mode == 3) {
       for (int t = 0; t < 4; ++t) {
         if (get_map(&m, out.hi, cap_img, L.cout, g, t)) return -1;   // stride-2 sub-lattice (py, px)
@@ -743,8 +741,6 @@ struct nope_unet {
         f.pre_wb = L.pre_wb;
       }
       f.out_lo = out.lo;
-      static const int dbg = std::getenv("NOPE_GN_DBG") ? std::atoi(std::getenv("NOPE_GN_DBG")) : 0;
-      f.dbg = dbg;
       f.emit = gs->emit;
       f.emit_parts = f.mt * p.n_tiles;
       NOPE_CHECK(f.ipt * f.gpt <= 64 && f.ipt <= 8, "fused GroupNorm: tile holds too many (image, group) pairs");
@@ -759,44 +755,10 @@ struct nope_unet {
     } else if (out.lo) {
       p.out_lo = out.lo;                // extras epilogue writes the remainder
     }
-    // development: NOPE_GN_TS=<k> records phase timestamps of the k-th fused launch into NOPE_GN_TS_FILE
-    unsigned long long* ts_dev = nullptr;
-    if (gs) {
-      static const int ts_k = std::getenv("NOPE_GN_TS") ? std::atoi(std::getenv("NOPE_GN_TS")) : -1;
-      static int ts_count = 0;
-      if (ts_k >= 0 && ts_count++ == ts_k) {
-        cudaMalloc(reinterpret_cast<void**>(&ts_dev), (size_t)num_sms * 64 * 16 * sizeof(unsigned long long));
-        cudaMemset(ts_dev, 0, (size_t)num_sms * 64 * 16 * sizeof(unsigned long long));
-        p.gn.ts = ts_dev;
-      }
-    }
     auto launch = [&]() {
       if (gs) return launch_conv_gn(p, L.bn, num_sms, st);
       return conv_impl == 2 ? launch_conv_tc2(p, L.bn, num_sms, st) : launch_conv_tc(p, L.bn, num_sms, st);
     };
-    if (ts_dev) {
-      const int rc = launch();
-      cudaDeviceSynchronize();
-      std::vector<unsigned long long> h((size_t)num_sms * 64 * 16);
-      cudaMemcpy(h.data(), ts_dev, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-      cudaFree(ts_dev);
-      if (FILE* f = std::fopen(std::getenv("NOPE_GN_TS_FILE") ? std::getenv("NOPE_GN_TS_FILE") : "gn_ts.csv", "w")) {
-        std::fprintf(f, "# So=%d n_img=%d cout=%d K=%d expected=%d m_tiles=%d n_tiles=%d\n", So, n_img, L.cout, L.K,
-                     p.gn.expected, p.m_tiles, p.n_tiles);
-        for (int c = 0; c < num_sms; ++c)
-          for (int it = 0; it < 64; ++it) {
-            const unsigned long long* r = &h[((size_t)c * 64 + it) * 16];
-            if (r[0] == 0) continue;
-            {
-              std::fprintf(f, "%d,%d", c, it);
-              for (int k = 0; k < 16; ++k) std::fprintf(f, ",%llu", r[k]);
-              std::fprintf(f, "\n");
-            }
-          }
-        std::fclose(f);
-      }
-      return rc;
-    }
     if (!profile) return launch();
     cudaEvent_t e0, e1;
     NOPE_CUDA(cudaEventCreate(&e0));
@@ -909,11 +871,8 @@ struct nope_unet {
       s2.silu = true;
       if (it != convs.end()) {
         Act r(TC.hi, co, split() ? TC.lo : nullptr);
-        // (routing this plain 1x1 through the EPI 4 role split measured 8 % slower than the plain epilogue:
-        // NOPE_PLAIN_EPI4=1 is the A/B switch)
-        static const bool plain_via_gn = std::getenv("NOPE_PLAIN_EPI4") && std::atoi(std::getenv("NOPE_PLAIN_EPI4"));
-        GnSpec s0;
-        if (conv(it->second, in0, in1, r, S, n, cap, st, nullptr, plain_via_gn ? &s0 : nullptr)) return -1;
+        // plain epilogue: routing this 1x1 through the GroupNorm-fused role split measured 8 % slower
+        if (conv(it->second, in0, in1, r, S, n, cap, st)) return -1;
         s2.res = r;
       } else {
         NOPE_CHECK(in1.hi == nullptr && in0.C == co, "resblock: identity residual needs Cin == Cout");
@@ -963,13 +922,11 @@ struct nope_unet {
       NOPE_CUDA(launch_pdl(linattn_kernel, dim3(4, n), dim3(kLinAttnThreads), 0, st, TD.hi, TC.hi, S * S, bf()));
     }
     ++launches;
-    // to_out (K = 128: two K-steps per tile) + GroupNorm(1) + residual in one kernel.  With the lock-step epilogue
-    // this measured slower than the plain convolution plus one normalisation pass (319 vs 244 us at 32x32); with the
-    // role-split epilogue the two forms take the same time (18.80 vs 18.71 ms over the step under ncu) and the fused
-    // one never rounds the un-normalised output to 16 bits (full-size configs[2] scores: 0.99e-3 vs 1.06e-3), so it is
-    // the default; NOPE_FUSE_TO_OUT=0 restores conv + gn_apply for A/B
-    static const bool fuse_to_out = !(std::getenv("NOPE_FUSE_TO_OUT") && !std::atoi(std::getenv("NOPE_FUSE_TO_OUT")));
-    if (fused() && (split() || fuse_to_out)) {
+    // to_out (K = 128: two K-steps per tile) + GroupNorm(1) + residual in one kernel.  With the role-split epilogue
+    // this takes the same time as the plain convolution plus one normalisation pass (18.80 vs 18.71 ms over the step
+    // under ncu; the lock-step epilogue measured slower: 319 vs 244 us at 32x32), and it never rounds the
+    // un-normalised output to 16 bits (full-size configs[2] scores: 0.99e-3 vs 1.06e-3)
+    if (fused()) {
       GnSpec s;
       s.norm = &norms.at(p + ".outnorm");
       s.res = x;

@@ -18,17 +18,13 @@ case "$step" in
   time)     rm -f gpurun_out/prof_dump.csv; NOPE_PROF_DUMP=gpurun_out/prof_dump.csv run "time_sweep" 900 python tools/time_sweep.py ${TIME_SPECS:-fp16 fp16:fuse_gn=0} --profile > gpurun_out/time_sweep.log 2>&1; cat gpurun_out/time_sweep.log ;;
   epi)      for d in ${EPI_LIST:-3 4 3 4}; do echo "NOPE_GN_EPI=$d"; NOPE_GN_EPI=$d timeout 600 python tools/time_sweep.py ${TIME_SPECS:-fp16} --steps 20 2>&1 | tail -1 | cut -c1-200; done > gpurun_out/epi_ab.log 2>&1; cat gpurun_out/epi_ab.log
             for d in 3 4; do NOPE_GN_EPI=$d NOPE_PROF_DUMP=gpurun_out/prof_dump_epi$d.csv timeout 600 python tools/time_sweep.py fp16 --profile > /dev/null 2>&1; done ;;
-  dbg)      for d in ${DBG_LIST:-0 8 16 24}; do echo "NOPE_GN_DBG=$d"; NOPE_GN_DBG=$d timeout 600 python tools/time_sweep.py fp16 --profile 2>&1 | tail -1; done > gpurun_out/dbg_sweep.log 2>&1; cat gpurun_out/dbg_sweep.log ;;
   pdl)      for d in ${PDL_LIST:-0 1 3 0 1 3 0 1 3}; do echo "NOPE_PDL=$d"; NOPE_PDL=$d timeout 600 python tools/time_sweep.py fp16 --steps 20 2>&1 | tail -1 | cut -c1-120; done > gpurun_out/pdl_ab.log 2>&1; cat gpurun_out/pdl_ab.log ;;
-  ts)       for k in ${TS_LAUNCHES:-2 8 20 24 30}; do NOPE_GN_TS=$k NOPE_GN_TS_FILE=gpurun_out/gn_ts_$k.csv timeout 600 python tools/time_sweep.py fp16 --steps 1 > /dev/null 2>&1; head -1 gpurun_out/gn_ts_$k.csv; done ;;
   ncu_gn)   run "ncu full: fused conv" 900 ncu --profile-from-start off --set full --clock-control none --import-source on --kernel-name-base demangled -k regex:"${NCU_KREGEX:-conv_tc2_kernel<\(int\)192, \(int\)6, \(int\)4>}" -s ${NCU_SKIP:-1} -c ${NCU_COUNT:-3} -o gpurun_out/prof_gn -f python tools/profile_step.py > gpurun_out/ncu_gn.log 2>&1
             ncu -i gpurun_out/prof_gn.ncu-rep --page raw --csv > gpurun_out/prof_gn_raw.csv 2>/dev/null ;;
   bench)    run "bench" 900 python bench.py --steps 10 --warmup 3 > gpurun_out/bench.log 2>&1; tail -1 gpurun_out/bench.log ;;
   benchall) for spec in "parity:--precision parity" "cfg2_fp16:--queries 8 --poses 2562" "cfg2_bf16:--queries 8 --poses 2562 --precision bf16" "ldm:--variant ldm" "ref:--impl reference"; do
               name=${spec%%:*}; fl=${spec#*:}; run "bench $name" 900 python bench.py --steps 10 --warmup 3 $fl > gpurun_out/bench_$name.log 2>&1; tail -1 gpurun_out/bench_$name.log | cut -c 1-900; done ;;
   smoke)    run "smoke" 900 python -c "import __graft_entry__ as g; g.smoke()" > gpurun_out/smoke.log 2>&1; tail -5 gpurun_out/smoke.log ;;
-  launches2) env ${ENV_B:-NOPE_FUSE_TO_OUT=1} timeout 900 ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches_b.csv python tools/profile_step.py > gpurun_out/ncu_list_b.log 2>&1
-            python tools/summarize_launches.py gpurun_out/launches_b.csv > gpurun_out/launch_summary_b.txt 2>&1; head -12 gpurun_out/launch_summary_b.txt ;;
   pipe)     run "ncu tensor-pipe list" 900 ncu --profile-from-start off --metrics gpu__time_duration.sum,sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_elapsed,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none --csv --log-file gpurun_out/pipe.csv python tools/profile_step.py > gpurun_out/ncu_pipe.log 2>&1
             python tools/summarize_pipe.py gpurun_out/pipe.csv gpurun_out/pipe_per_launch.csv > gpurun_out/pipe_summary.txt 2>&1; cat gpurun_out/pipe_summary.txt ;;
   pipe_cfg2) NOPE_POSES=2562 NOPE_QUERIES=8 run "ncu tensor-pipe list, configs[2] size (first 420 launches)" 900 ncu --profile-from-start off -c 420 --metrics gpu__time_duration.sum,sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_elapsed,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none --csv --log-file gpurun_out/pipe_cfg2.csv python tools/profile_step.py > gpurun_out/ncu_pipe_cfg2.log 2>&1
