@@ -242,19 +242,16 @@ void nope_ldm_destroy(nope_ldm_t* m);
 int nope_ldm_load_tensor(nope_ldm_t* m, const char* key, const float* data, const int64_t* shape,
                          int ndim);
 int nope_ldm_finalize(nope_ldm_t* m);
-int nope_ldm_set_chunk(nope_ldm_t* m, int hyps_per_chunk);       /* ~20.5 MB workspace / hypothesis */
-/* conv_impl: 2 = clustered wgmma kernel (default), 0 = single-CTA wgmma kernel;
+int nope_ldm_set_chunk(nope_ldm_t* m, int hyps_per_chunk);       /* ~15.6 MB workspace / hypothesis (model_channels 256) */
+/* conv_impl: 2 = clustered wgmma kernel (the only one; anything else is an error);
  * attn_impl: 0 = wgmma attention (default), 1 = CUDA-core twin (bring-up). */
 int nope_ldm_set_impl(nope_ldm_t* m, int conv_impl, int attn_impl);
-/* Named switches (bring-up / A-B measurements): "fuse_geglu" (default 1: GEGLU runs in the
- * epilogue of its projection GEMM; 0: separate elementwise kernel), "hoist" (default 1: the
- * pose-independent prefix -- input conv, first ResBlock, first transformer up to its
- * self-attention -- runs once per reference instead of once per hypothesis); before
- * nope_ldm_finalize only: "wide_tiles" (default 1: 256-channel GEMM tiles on the CTA-pair kernel),
- * "fold_residual" (default 1: residual adds ride in the GEMM as identity K-segments fed by TMA;
- * 0: added in the epilogue from global memory), "precision" (default 0: fp16 weights; 1: exact
- * weights -- packed rows hold [W_hi | W_lo] and every GEMM accumulates A W_hi + A W_lo, 2x the MMA
- * work; embeddings 1.1e-3 -> below the 1e-3 bar against the fp32 reference). */
+/* Named options: "hoist" (default 1: the pose-independent prefix -- input conv, first ResBlock,
+ * first transformer up to its self-attention -- runs once per reference instead of once per
+ * hypothesis); before nope_ldm_finalize only: "precision"
+ * (default 0: fp16 weights; 1: exact weights -- packed rows hold [W_hi | W_lo] and every GEMM
+ * accumulates A W_hi + A W_lo, 2x the MMA work; embeddings 1.1e-3 -> below the 1e-3 bar against
+ * the fp32 reference).  Any other name is an error. */
 int nope_ldm_set_option(nope_ldm_t* m, const char* name, int value);
 int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
                    const float* query_latent, float* out_emb, float* out_sim, int k,

@@ -95,8 +95,7 @@ struct GnFuse {
 struct ConvParams {
   CUtensorMap amap[kMaxAMaps];
   int n_amaps;
-  CUtensorMap bmap;
-  CUtensorMap bmap2;      // weight box of the clustered kernel's tile width (conv_tc2.cuh)
+  CUtensorMap bmap;     // weight box of the kernel's tile width (BN rows)
   CUtensorMap omap[4];  // one per output parity class when n_par == 4, else omap[0]
   CUtensorMap rmap;     // residual tensor (output geometry), EPI == 4 / 3 with gn.has_res
   GnFuse gn;            // EPI == 4 / 3
@@ -279,9 +278,10 @@ __device__ __forceinline__ int butterfly8(float (&v)[8], int lane) {
 // Epilogue of one 128 x BN accumulator tile, executed by the 8 epilogue warps of a CTA.
 // Warp e reads accumulator rows 32*(e&3).. (its pixel rows) and the 32-column half (e>>2) of every
 // 64-column sub-tile: +bias (from smem) -> GroupNorm partial sums -> fp16 -> swizzled staging.
-// EXTRAS (compile time) enables ReLU / residual add / (hi, lo) split / fp32 output: the template
-// encoder's epilogue.  The sweep instantiates EXTRAS = false so its epilogue stays minimal (the
-// extra predicates and registers cost ~10 % on the large convolutions when merely present).
+// EXTRAS (compile time) enables ReLU / residual add / (hi, lo) split / fp32 output: the epilogue of
+// the template encoder and of the LDM output convolution (clustered kernel only).  The sweep
+// instantiates EXTRAS = false so its epilogue stays minimal (the extra predicates and registers
+// cost ~10 % on the large convolutions when merely present).
 // Residual operands (high halves) of a tile, software-pipelined ONE TILE AHEAD by the epilogue
 // warps: while sub-tile cc of tile i is being combined, the loads of sub-tile cc of tile i+1 are
 // already in flight (into the registers that sub-tile just vacated).  With the loads issued next to
@@ -458,7 +458,7 @@ __device__ __forceinline__ void conv_epilogue_geglu(uint8_t* out_stage, const fl
   }
 }
 
-template <int BN, int STAGES, bool EXTRAS>
+template <int BN, int STAGES>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_tc_kernel(const __grid_constant__ ConvParams p) {
   using S = ConvSmem<BN, STAGES>;
@@ -544,7 +544,7 @@ conv_tc_kernel(const __grid_constant__ ConvParams p) {
       if (etid == 0) tma_store_wait_read0();
       asm volatile("bar.sync 1, 256;" ::: "memory");
       conv_mma_tile<BN, 2, STAGES, S::kStageBytes, S::kABytes>(p, smem, full_bar, empty_bar, stage, phase, s_acc);
-      conv_epilogue_tile<BN, EXTRAS>(p, out_stage, s_bias, s_acc, m_tile, n_chan0, e, lane);
+      conv_epilogue_tile<BN, false>(p, out_stage, s_bias, s_acc, m_tile, n_chan0, e, lane);
       acc_release(tempty_bar, lane);
       // make the generic-proxy smem writes visible to the TMA (async proxy), then store
       fence_proxy_async_smem();
@@ -659,7 +659,7 @@ inline bool conv_needs_extras(const ConvParams& p) {
   return p.relu || p.res_hi || p.out_lo || p.out_f32;
 }
 
-template <int BN, int STAGES, bool EXTRAS>
+template <int BN, int STAGES>
 inline int launch_conv_tc_t(const ConvParams& p, int num_sms, cudaStream_t stream) {
   using S = ConvSmem<BN, STAGES>;
   static bool attr_set[kMaxDevices];     // the opt-in is per device
@@ -667,26 +667,23 @@ inline int launch_conv_tc_t(const ConvParams& p, int num_sms, cudaStream_t strea
   NOPE_CUDA(cudaGetDevice(&dev));
   NOPE_CHECK(dev >= 0 && dev < kMaxDevices, "device index out of range");
   if (!attr_set[dev]) {
-    NOPE_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, EXTRAS>,
+    NOPE_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES>,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal));
     attr_set[dev] = true;
   }
   const int tiles = p.m_tiles * p.n_tiles;
   const int grid = tiles < num_sms ? tiles : num_sms;
-  conv_tc_kernel<BN, STAGES, EXTRAS><<<grid, kConvThreads, S::kTotal, stream>>>(p);
+  conv_tc_kernel<BN, STAGES><<<grid, kConvThreads, S::kTotal, stream>>>(p);
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }
 
 inline int launch_conv_tc(const ConvParams& p, int bn, int num_sms, cudaStream_t stream) {
-  const bool ex = conv_needs_extras(p);
+  if (conv_needs_extras(p)) return fail("launch_conv_tc: epilogue extras need the clustered kernel");
   switch (bn) {
-    case 192: return ex ? launch_conv_tc_t<192, 4, true>(p, num_sms, stream)
-                        : launch_conv_tc_t<192, 4, false>(p, num_sms, stream);
-    case 128: return ex ? launch_conv_tc_t<128, 5, true>(p, num_sms, stream)
-                        : launch_conv_tc_t<128, 5, false>(p, num_sms, stream);
-    case 64: return ex ? launch_conv_tc_t<64, 6, true>(p, num_sms, stream)
-                       : launch_conv_tc_t<64, 6, false>(p, num_sms, stream);
+    case 192: return launch_conv_tc_t<192, 4>(p, num_sms, stream);
+    case 128: return launch_conv_tc_t<128, 5>(p, num_sms, stream);
+    case 64: return launch_conv_tc_t<64, 6>(p, num_sms, stream);
   }
   return fail("launch_conv_tc: unsupported BN");
 }

@@ -1292,8 +1292,7 @@ __device__ __forceinline__ void conv_gn2_store_warp(const ConvParams& p, uint8_t
 // column split at 128 registers), spread over the statistics warp at 80 and the math warps at 144; at 512 threads
 // the four warpgroups average 128 registers, and moving registers between the roles moves the spills with them.
 // <128,4,4> 56 / 108 (statistics warp and epilogue), <128,4,3> 8 / 32, <192,4,3> 548 / 688 (the lock-step A/B
-// epilogue at 144), <256,3,1> 120 / 136 (the extras epilogue, not the K loop: the column split spills 232 / 232
-// there too, so the row split stays on for it).
+// epilogue at 144).
 __host__ __device__ constexpr int conv2_threads(int BN, int EPI) { return EPI >= 3 ? gn_threads(BN) : kConvThreads; }
 __host__ __device__ constexpr int conv2_ctl_regs(int EPI) { return EPI == 4 ? 80 : 56; }
 __host__ __device__ constexpr int conv2_launch_regs(int threads) { return 65536 / threads / 8 * 8; }
@@ -1336,7 +1335,7 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
 
   if (warp == 0 && lane == 0) {
     for (int i = 0; i < p.n_amaps; ++i) prefetch_tmap(&p.amap[i]);
-    prefetch_tmap(&p.bmap2);
+    prefetch_tmap(&p.bmap);
     for (int i = 0; i < p.n_par; ++i) prefetch_tmap(&p.omap[i]);
   }
   if (warp == 1 && lane == 0) {
@@ -1399,7 +1398,7 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
             uint8_t* sa = smem + stage * S::kStageBytes;
             mbar_expect_tx(&full_bar[stage], S::kStageBytes);
             tma_load_4d(sa, am, &full_bar[stage], ch * kBK, sg.dx + px, y0 + sg.dy + py, b0);
-            tma_load_2d(sa + S::kABytes, &p.bmap2, &full_bar[stage], kcol, n_tile * BN);
+            tma_load_2d(sa + S::kABytes, &p.bmap, &full_bar[stage], kcol, n_tile * BN);
           }
           kcol += kBK;
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -1584,8 +1583,9 @@ inline int launch_conv_tc2(const ConvParams& p, int bn, int num_sms, cudaStream_
   }
   switch (bn) {
     // 256-wide tiles (LDM variant: every width is a multiple of 256): twice the MMA work per byte of A
-    case 256: return ex ? launch_conv_tc2_t<256, 3, 1>(p, num_sms, stream)
-                        : launch_conv_tc2_t<256, 3, 0>(p, num_sms, stream);
+    case 256:
+      if (ex) return fail("launch_conv_tc2: epilogue extras need BN <= 192");
+      return launch_conv_tc2_t<256, 3, 0>(p, num_sms, stream);
     case 192: return ex ? launch_conv_tc2_t<192, 4, 1>(p, num_sms, stream)
                         : launch_conv_tc2_t<192, 4, 0>(p, num_sms, stream);
     case 128: return ex ? launch_conv_tc2_t<128, 5, 1>(p, num_sms, stream)

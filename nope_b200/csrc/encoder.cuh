@@ -302,7 +302,7 @@ struct nope_encoder {
         ksteps += 3 * nch;
       }
     NOPE_CHECK(nseg <= kMaxSeg && ksteps * 64 == L.K, "encoder conv: segment table");
-    p.bmap2 = L.wmap;
+    p.bmap = L.wmap;
     if (get_map(&m, out.hi, L.cout, g, -1)) return -1;
     for (int t = 0; t < 4; ++t) p.omap[t] = *m;
     p.bias = L.bias;

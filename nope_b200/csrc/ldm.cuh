@@ -9,15 +9,15 @@
 // Batched over all pose hypotheses of a chunk, NHWC fp16:
 //   ResBlock          GN32+SiLU (two-source: the skip concat is never materialised before the norm)
 //                     -> conv3x3 (+ emb bias) -> GN32+SiLU (statistics from the conv epilogue)
-//                     -> conv3x3 with the 1x1 skip_connection folded in as extra K segments
-//                        (or the identity skip added in the epilogue)
+//                     -> conv3x3 with the 1x1 skip_connection (or the identity skip) folded in
+//                        as extra K segments
 //   SpatialTransformer GN32 (statistics from the ResBlock's last epilogue) -> proj_in -> LN ->
 //                     q|k|v GEMM -> wgmma attention -> to_out (+x) -> [+cross term, LN] ->
 //                     GEGLU feed-forward (+x) -> proj_out (+x_in)
 //   Downsample        conv3x3 stride 2 through the four stride-2 TMA lattices of its input
 //   Upsample          nearest-x2 + conv3x3 folded into four 2x2 parity kernels
 //   out               GN32+SiLU -> conv3x3 (256 -> 4, padded to a 64-channel tile, fp32 store) -> l2 score
-// Every GEMM-shaped op runs on conv_tc2_kernel / conv_tc_kernel.
+// Every GEMM-shaped op runs on conv_tc2_kernel.
 #pragma once
 #include "conv_tc2.cuh"
 #include "kernels.cuh"
@@ -37,13 +37,12 @@ struct LdmConv {
   int mode = 0;   // 0: 3x3 pad 1, 1: 1x1 / linear, 3: nearest-x2 + 3x3 (folded), 4: 3x3 stride 2 pad 1
   int cin = 0, cout = 0, K = 0;
   int bn = 0;              // tile width of the clustered kernel (up to 256)
-  int bn1 = 0;             // tile width of the 1-CTA kernel (up to 192)
   int skip_c = 0;          // channels of a folded 1x1 skip_connection / identity residual (extra K columns)
   int k_alg = 0;           // K without identity-residual columns (algorithmic FLOP count)
   bool geglu = false;      // rows permuted to (64 x | 64 gate) tiles; the epilogue emits x * gelu(gate)
   __half* w = nullptr;     // [rows][K] fp16
   float* bias = nullptr;
-  CUtensorMap wmap, wmap2;      // weight boxes of bn1 / bn rows
+  CUtensorMap wmap;        // weight box of bn rows
 };
 struct LdmNorm {
   float* gamma = nullptr;
@@ -69,12 +68,8 @@ struct nope_ldm {
   int nres = 2;
   std::vector<int> mult{1, 2, 4};
   bool finalized = false;
-  int conv_impl = 2;   // 2: clustered wgmma kernel (default), 0: single-CTA wgmma kernel
   int attn_impl = 0;   // 0: wgmma attention, 1: CUDA-core twin
-  bool fold_residual = true;   // residual adds as identity K-segments of the GEMM (set before finalize)
-  bool wide_tiles = true;   // 256-channel tiles on the clustered kernel where Cout % 256 == 0 (set before finalize)
   bool hoist = true;        // pose-independent prefix once per reference (prestage)
-  bool fuse_geglu = true;   // GEGLU in the projection's epilogue (clustered kernel); false: separate kernel
   int precision = 0;        // 0: fp16 weights; 1: exact weights -- every packed row is [W_hi | W_lo] and the K loop
                             // walks its segment list twice (A W_hi + A W_lo), 2x the MMA work (set before finalize)
   int kp(int K) const { return precision ? 2 * K : K; }
@@ -99,7 +94,7 @@ struct nope_ldm {
   std::vector<__half*> HS;                     // skip stack, one buffer per input block
   __half *XA = nullptr, *XB = nullptr, *XC = nullptr, *R = nullptr, *T1 = nullptr, *T2 = nullptr,
          *T3 = nullptr, *XN = nullptr, *PI = nullptr, *PJ = nullptr, *QKV = nullptr,
-         *Vt = nullptr, *AO = nullptr, *FF = nullptr, *GG = nullptr, *x0ref = nullptr, *Rref = nullptr, *Pref = nullptr;
+         *Vt = nullptr, *AO = nullptr, *GG = nullptr, *x0ref = nullptr, *Rref = nullptr, *Pref = nullptr;
   float2 *S_in = nullptr, *S_mid = nullptr, *S_out = nullptr;
   float* cb = nullptr;
   float* OF = nullptr;                          // out[2] result, fp32 [cap * S0 * S0][64]
@@ -301,12 +296,10 @@ struct nope_ldm {
   int finish_conv(const std::string& name, nope::LdmConv& L, int rows, const std::vector<float>& bias) {
     using namespace nope;
     if (L.k_alg == 0) L.k_alg = L.K;
-    L.bn1 = pick_bn(L.cout);
-    L.bn = (!L.geglu && L.cout % 256 == 0 && wide_tiles) ? 256 : L.bn1;
+    L.bn = (!L.geglu && L.cout % 256 == 0) ? 256 : pick_bn(L.cout);
     NOPE_CHECK(L.bn != 0 && L.K % 64 == 0, name + ": channel counts must be multiples of 64");
     if (!bias.empty() && upload(bias, &L.bias)) return -1;
-    if (make_weight_map(&L.wmap, L.w, rows, kp(L.K), L.bn1)) return -1;
-    if (make_weight_map(&L.wmap2, L.w, rows, kp(L.K), L.bn)) return -1;
+    if (make_weight_map(&L.wmap, L.w, rows, kp(L.K), L.bn)) return -1;
     convs[name] = L;
     return 0;
   }
@@ -353,7 +346,6 @@ struct nope_ldm {
   }
   // linear layer (1x1) whose output gets a residual of `cout` channels added
   int make_lin_res(const std::string& name, const std::string& wkey, const std::string& bkey) {
-    if (!fold_residual) return make_conv(name, wkey, bkey, 1);
     const HostT& W = H(wkey);
     nope::LdmConv L;
     L.mode = 1;
@@ -395,7 +387,7 @@ struct nope_ldm {
       const auto& bs = H(p + ".skip_connection.bias").second;
       for (size_t i = 0; i < bias.size(); ++i) bias[i] += bs[i];
     }
-    const bool id_skip = !has_skip && fold_residual;      // identity skip as an identity K-segment
+    const bool id_skip = !has_skip;      // identity skip as an identity K-segment
     if (id_skip) L.skip_c = L.cout;
     L.K = 9 * L.cin + L.skip_c;
     if (id_skip) L.k_alg = 9 * L.cin;
@@ -413,8 +405,7 @@ struct nope_ldm {
     if (make_conv(p + ".proj_in", p + ".proj_in.weight", p + ".proj_in.bias", 1)) return -1;
     if (make_lin_res(p + ".proj_out", p + ".proj_out.weight", p + ".proj_out.bias")) return -1;
     if (make_lin_res(p + ".to_out", t + ".attn1.to_out.0.weight", t + ".attn1.to_out.0.bias")) return -1;
-    if (make_conv(p + ".ff1", t + ".ff.net.0.proj.weight", t + ".ff.net.0.proj.bias", 1)) return -1;
-    {  // the same projection with GEGLU fused into the epilogue (clustered kernel): tile t of 128 rows =
+    {  // the feed-forward projection with GEGLU fused into the epilogue: tile t of 128 rows =
        // x rows 64t..64t+63 followed by gate rows inner+64t..inner+64t+63
       const HostT& W = H(t + ".ff.net.0.proj.weight");
       const auto& b = H(t + ".ff.net.0.proj.bias").second;
@@ -574,10 +565,10 @@ struct nope_ldm {
       }
     }
     // widest tensors: block outputs <= 2u (512 ch at 32^2 after the last upsample), ResBlock
-    // inputs <= 3u (768 ch at 32^2), q|k|v 3u, V^T 1u, GEGLU input 8u, output 4u
+    // inputs <= 3u (768 ch at 32^2), q|k|v 3u, V^T 1u, GEGLU output 4u
     if (ws_half(&XA, c * 2 * u) || ws_half(&XB, c * 2 * u) || ws_half(&XC, c * 2 * u) || ws_half(&R, c * u) ||
         ws_half(&T1, c * 3 * u) || ws_half(&T2, c * u) || ws_half(&T3, c * u) || ws_half(&XN, c * u) ||
-        ws_half(&PI, c * u) || ws_half(&PJ, c * u) || ws_half(&QKV, c * 3 * u) || ws_half(&Vt, c * u) || ws_half(&AO, c * u) || ws_half(&FF, c * 8 * u) ||
+        ws_half(&PI, c * u) || ws_half(&PJ, c * u) || ws_half(&QKV, c * 3 * u) || ws_half(&Vt, c * u) || ws_half(&AO, c * u) ||
         ws_half(&GG, c * 4 * u) || ws_half(&x0ref, (size_t)cap_ref * u) || ws_half(&Rref, (size_t)cap_ref * u) ||
         ws_half(&Pref, (size_t)cap_ref * u))
       return -1;
@@ -604,9 +595,9 @@ struct nope_ldm {
   }
 
   // ------------------------------------------------------------------ op launchers
-  // out[n_img, So, So, cout] = conv(L, in) [+ 1x1 skip over cat(sk0, sk1)] + bias [+ res]
+  // out[n_img, So, So, cout] = conv(L, in) [+ 1x1 skip or identity residual over cat(sk0, sk1)] + bias
   int conv(const nope::LdmConv& L, const __half* in, __half* out, int So, int n_img, cudaStream_t st,
-           float2* stats = nullptr, const __half* res = nullptr, const __half* sk0 = nullptr, int skc0 = 0,
+           float2* stats = nullptr, const __half* sk0 = nullptr, int skc0 = 0,
            const __half* sk1 = nullptr, int skc1 = 0, float* out_f32 = nullptr) {
     using namespace nope;
     NOPE_CHECK(skc0 + skc1 == L.skip_c, "conv: skip channel mismatch");
@@ -670,7 +661,6 @@ struct nope_ldm {
     p.n_amaps = nmaps;
     for (int t = nmaps; t < kMaxAMaps; ++t) p.amap[t] = p.amap[0];
     p.bmap = L.wmap;
-    p.bmap2 = L.wmap2;
     if (L.mode == 3) {
       for (int t = 0; t < 4; ++t) {
         if (get_map(&m, out, L.cout, g, t)) return -1;
@@ -682,7 +672,6 @@ struct nope_ldm {
     }
     p.geglu = L.geglu ? 1 : 0;
     p.bias = L.bias;
-    p.res_hi = res;
     p.out_f32 = out_f32;
     p.stats = stats;
     p.stats_hw = So * So;
@@ -692,8 +681,7 @@ struct nope_ldm {
     p.nseg = nseg;
     p.ksteps = ksteps;
     p.m_tiles = geom_m_tiles(g, n_img);
-    const int bn = conv_impl == 2 ? L.bn : L.bn1;
-    p.n_tiles_par = L.cout / bn;
+    p.n_tiles_par = L.cout / L.bn;
     p.n_tiles = p.n_tiles_par * p.n_par;
     p.tiles_per_img = g.tiles_per_img;
     p.h_cnt = g.h_cnt;
@@ -709,20 +697,13 @@ struct nope_ldm {
     NOPE_CHECK(nseg <= kMaxSeg, "conv: segment table overflow");
     p.nseg = nseg;
     p.ksteps = ksteps;
-    NOPE_CHECK(!((stats || res) && L.mode == 3), "upsample conv has no fused statistics / residual");
+    NOPE_CHECK(!(stats && L.mode == 3), "upsample conv has no fused statistics");
     if (profile && prof_begin(st)) return -1;
-    const int rc = conv_impl == 2 ? launch_conv_tc2(p, bn, num_sms, st) : launch_conv_tc(p, bn, num_sms, st);
+    const int rc = launch_conv_tc2(p, L.bn, num_sms, st);
     // executed FLOPs (the folded upsample runs 4 parity GEMMs of K = 4 Cin over the source pixels)
     if (profile && prof_end(st, 2.0 * (double)n_img * g.H * g.W * (double)(L.mode == 3 ? 4 * L.cout : L.cout) * (double)L.k_alg, 0))
       return -1;
     return rc;
-  }
-
-  // out = L(in) + res: residual as an identity K-segment (fold_residual) or in the epilogue
-  int lin_res(const nope::LdmConv& L, const __half* in, __half* out, const __half* res, int C, int S, int n,
-              cudaStream_t st) {
-    if (L.skip_c) return conv(L, in, out, S, n, st, nullptr, nullptr, res, C);
-    return conv(L, in, out, S, n, st, nullptr, res);
   }
 
   static int parts_of(int S) { return S * S < 32 ? 1 : S * S / 32; }
@@ -832,9 +813,7 @@ struct nope_ldm {
     if (gn(norms.at(p + ".n1"), x0, C0, x1, C1, S_in, S, n, T1, true, 1e-5f, st)) return -1;
     if (conv(c1, T1, T2, S, n, st, S_mid)) return -1;
     if (gn(norms.at(p + ".n2"), T2, c1.cout, nullptr, 0, S_mid, S, n, T3, true, 1e-5f, st)) return -1;
-    if (c2.skip_c) return conv(c2, T3, out, S, n, st, S_out, nullptr, x0, C0, x1, C1);
-    NOPE_CHECK(x1 == nullptr && C0 == c2.cout, "resblock: identity skip needs Cin == Cout");
-    return conv(c2, T3, out, S, n, st, S_out, x0);    // epilogue add (fold_residual off)
+    return conv(c2, T3, out, S, n, st, S_out, x0, C0, x1, C1);
   }
 
   // SpatialTransformer.forward (ldm/attention.py:264-277) with one BasicTransformerBlock
@@ -846,7 +825,7 @@ struct nope_ldm {
     if (ln(norms.at(p + ".ln1"), PI, nullptr, nullptr, XN, C, S, n, st)) return -1;
     if (conv(convs.at(p + ".qkv"), XN, QKV, S, n, st)) return -1;
     if (attention(QKV, AO, C, S * S, n, st)) return -1;
-    return lin_res(convs.at(p + ".to_out"), AO, xs, PI, C, S, n, st);
+    return conv(convs.at(p + ".to_out"), AO, xs, S, n, st, nullptr, PI, C);
   }
   // st_post: x = attn2(norm2(x), context) + x -- the one-token cross-attention is the
   // per-hypothesis vector cb (see make_cross), added by the LayerNorm kernel, which also applies
@@ -855,18 +834,9 @@ struct nope_ldm {
   int st_post(const std::string& p, const __half* xs, const int* src_img, const __half* x_in, __half* out, int C,
               int S, int n, const float* cbp, cudaStream_t st) {
     if (ln(norms.at(p + ".ln3"), xs, PJ, cbp + cb_off.at(p), XN, C, S, n, st, src_img)) return -1;
-    // GEGLU: fused into the projection's epilogue on the clustered kernel
-    if (conv_impl == 2 && fuse_geglu) {
-      if (conv(convs.at(p + ".ff1g"), XN, GG, S, n, st)) return -1;
-    } else {
-      if (conv(convs.at(p + ".ff1"), XN, FF, S, n, st)) return -1;
-      nope::ldm_geglu_kernel<<<nope::ew_grid((long long)n * S * S * C / 2), 256, 0, st>>>(FF, GG, (long long)n * S * S,
-                                                                                        4 * C);
-      NOPE_CUDA(cudaGetLastError());
-      ++launches;
-    }
-    if (lin_res(convs.at(p + ".ff2"), GG, PI, PJ, C, S, n, st)) return -1;
-    return lin_res(convs.at(p + ".proj_out"), PI, out, x_in, C, S, n, st);
+    if (conv(convs.at(p + ".ff1g"), XN, GG, S, n, st)) return -1;   // GEGLU in the projection's epilogue
+    if (conv(convs.at(p + ".ff2"), GG, PI, S, n, st, nullptr, PJ, C)) return -1;
+    return conv(convs.at(p + ".proj_out"), PI, out, S, n, st, nullptr, x_in, C);
   }
   int transformer(const std::string& p, const __half* x_in, __half* out, int C, int S, int n, const float* cbp,
                   cudaStream_t st) {
@@ -971,7 +941,7 @@ struct nope_ldm {
     if (gn(norms.at("out.0"), curw, C, nullptr, 0, S_in, S, n, T1, true, 1e-5f, st)) return -1;
     const int hw = S * S;
     const int nslab = (hw + kFinalThreads - 1) / kFinalThreads;
-    if (conv(convs.at("out.2"), T1, T2, S, n, st, nullptr, nullptr, nullptr, 0, nullptr, 0, OF)) return -1;
+    if (conv(convs.at("out.2"), T1, T2, S, n, st, nullptr, nullptr, 0, nullptr, 0, OF)) return -1;
     ldm_score_kernel<<<dim3(nslab, n), kFinalThreads, 0, st>>>(
         OF, out_emb ? out_emb + (size_t)hyp0 * Cl * hw : nullptr, query, ref_of,
         score_part ? score_part + (size_t)hyp0 * nslab : nullptr, hw, Cl);

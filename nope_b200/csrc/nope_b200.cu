@@ -661,7 +661,6 @@ struct nope_unet {
       if (alo1) add_seg(map_index(0, 1, 1), t, c1 / 64, wbase + c0);
     }
     p.bmap = L.wmap;
-    p.bmap2 = L.wmap;
     p.bf16 = bf() ? 1 : 0;
     if (L.mode == 3) {
       for (int t = 0; t < 4; ++t) {
@@ -1806,30 +1805,18 @@ int nope_ldm_set_chunk(nope_ldm_t* m, int hyps) {
   return 0;
 }
 int nope_ldm_set_impl(nope_ldm_t* m, int conv_impl, int attn_impl) {
-  NOPE_CHECK(m && (conv_impl == 0 || conv_impl == 2), "conv_impl must be 0 (tensor cores) or 2 (tensor cores, clustered)");
+  NOPE_CHECK(m && conv_impl == 2, "conv_impl must be 2 (tensor cores, clustered)");
   NOPE_CHECK(attn_impl == 0 || attn_impl == 1, "attn_impl must be 0 (tensor cores) or 1 (CUDA cores)");
-  m->conv_impl = conv_impl;
   m->attn_impl = attn_impl;
   return 0;
 }
 int nope_ldm_set_option(nope_ldm_t* m, const char* name, int value) {
   NOPE_CHECK(m && name, "null argument");
-  if (std::strcmp(name, "fuse_geglu") == 0) { m->fuse_geglu = value != 0; return 0; }
   if (std::strcmp(name, "hoist") == 0) { m->hoist = value != 0; return 0; }
-  if (std::strcmp(name, "fold_residual") == 0) {
-    NOPE_CHECK(!m->finalized, "fold_residual must be set before finalize");
-    m->fold_residual = value != 0;
-    return 0;
-  }
   if (std::strcmp(name, "precision") == 0) {
     NOPE_CHECK(!m->finalized, "precision must be set before finalize");
     NOPE_CHECK(value == 0 || value == 1, "LDM precision: 0 (fp16 weights) or 1 (exact weights, W_hi + W_lo)");
     m->precision = value;
-    return 0;
-  }
-  if (std::strcmp(name, "wide_tiles") == 0) {
-    NOPE_CHECK(!m->finalized, "wide_tiles must be set before finalize");
-    m->wide_tiles = value != 0;
     return 0;
   }
   return fail(std::string("unknown option: ") + name);

@@ -97,7 +97,7 @@ class UNetModelPose:
             _lib.check(_lib.load().nope_ldm_set_chunk(self._h, hyps))
 
     def set_impl(self, conv="tcgen05_2cta", attn="tcgen05"):
-        _lib.check(_lib.load().nope_ldm_set_impl(self._handle(), {"tcgen05": 0, "tcgen05_2cta": 2}[conv],
+        _lib.check(_lib.load().nope_ldm_set_impl(self._handle(), {"tcgen05_2cta": 2}[conv],
                                                  {"tcgen05": 0, "simt": 1}[attn]))
 
     def set_option(self, name, value):
