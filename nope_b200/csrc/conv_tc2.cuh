@@ -69,8 +69,12 @@ struct Conv2Smem {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kOutBytes = (BN / 64) * kBM * 128;
   // narrow tiles double-buffer the output staging: the TMA store of tile i drains while the
-  // epilogue of tile i+1 fills the other buffer (the short-K 1x1 layers are epilogue bound)
-  static constexpr int kOutBufs = (BN <= 128 || (EPI == 4 && STAGES <= 4)) ? 2 : 1;
+  // epilogue of tile i+1 fills the other buffer (the short-K 1x1 layers are epilogue bound).  At BN = 192 the
+  // second buffer would cost a ring stage, and the fourth stage is worth more: with one wgmma group in flight
+  // the mainloop holds two stages, so three stages leave the producer one stage of lead (fused GroupNorm at
+  // BN = 192 on an H100 at 700 W: 3 stages + 2 buffers 45.0 ms per 642-pose step, 4 stages + 1 buffer 41.0-41.4,
+  // every layer class faster, the short-K to_qkv / to_out launches included; DESIGN.md section 6)
+  static constexpr int kOutBufs = BN <= 128 ? 2 : 1;
   static constexpr int kBarOffset = STAGES * kStageBytes + kOutBufs * kOutBytes;
   static constexpr int kBiasOffset = kBarOffset + 256;
   // EPI == 3 (GroupNorm fused): gamma | beta (fp32 [BN] each) | pose bias (fp16 [8][BN]) |
@@ -1288,8 +1292,8 @@ __device__ __forceinline__ void conv_gn2_store_warp(const ConvParams& p, uint8_t
 // producer, and with EPI == 4 the store and statistics warps) drops to conv2_ctl_regs, the math warpgroups share the
 // rest of the 64 K register file evenly: 224 per thread at 384 threads (208 with EPI == 4), 144 at 512 threads
 // (BN = 192, EPI 3 / 4).  Blocks of 256 threads already allow 255 registers per thread and keep that limit.
-// Not every instantiation is spill-free (ptxas -v, spill store / load bytes): <192,3,4> 126 / 212 (148 / 236 with the
-// column split at 128 registers), spread over the statistics warp at 80 and the math warps at 144; at 512 threads
+// Not every instantiation is spill-free (ptxas -v, spill store / load bytes): <192,4,4> 134 / 212,
+// spread over the statistics warp at 80 and the math warps at 144; at 512 threads
 // the four warpgroups average 128 registers, and moving registers between the roles moves the spills with them.
 // <128,4,4> 56 / 108 (statistics warp and epilogue), <128,4,3> 8 / 32, <192,4,3> 548 / 688 (the lock-step A/B
 // epilogue at 144).
@@ -1567,7 +1571,7 @@ inline int launch_conv_gn(const ConvParams& p, int bn, int num_sms, cudaStream_t
     }
   } else {
     switch (bn) {
-      case 192: return launch_conv_tc2_t<192, 3, 4>(p, num_sms, stream);
+      case 192: return launch_conv_tc2_t<192, 4, 4>(p, num_sms, stream);
       case 128: return launch_conv_tc2_t<128, 4, 4>(p, num_sms, stream);
       case 64: return launch_conv_tc2_t<64, 7, 4>(p, num_sms, stream);
     }
