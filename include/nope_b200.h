@@ -94,7 +94,7 @@ int nope_unet_get_option(const nope_unet_t* u, const char* name, int* value);
  * synchronises the device and calls cudaMalloc).  A host framework that wants every byte to come from
  * its own allocator asks for the size and hands a buffer over; the sweep then never allocates and
  * fails if the buffer is too small.  hyps = min(chunk, B*N) hypotheses per chunk, refs = B,
- * scores = B*N (0 when no query is scored).  The buffer must stay alive while the engine uses it. */
+ * scores = B*Q*N, the number of scored (reference, query, pose) triples (0 when no query is scored).  The buffer must stay alive while the engine uses it. */
 int64_t nope_unet_workspace_bytes(nope_unet_t* u, int hyps, int refs, int scores);
 int nope_unet_set_workspace(nope_unet_t* u, void* device_ptr, int64_t bytes, int hyps, int refs, int scores);
 
@@ -115,6 +115,18 @@ int nope_unet_set_workspace(nope_unet_t* u, void* device_ptr, int64_t bytes, int
 int nope_unet_sweep(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
                     const float* query_feat, float* out_emb, float* out_sim, int k,
                     float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream);
+
+/* One sweep per reference, Q queries per reference: the templates depend on the reference and the pose grid
+ * only, so several queries of one object (video frames, detections of several instances) share one sweep and
+ * are all scored in its last layer.  Arguments as nope_unet_sweep, plus Q >= 1, with
+ *   query_feat [B, Q, C, hw, hw] fp32
+ *   out_sim    [B, Q, N] fp32 or NULL
+ *   out_topv / out_topi  [B, Q, k]
+ * sim[b, q] is bit-identical to a Q = 1 sweep of query q alone; nope_unet_sweep is the Q = 1 case.  A
+ * caller-owned workspace must be sized for scores = B*Q*N. */
+int nope_unet_sweep_multi(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
+                          const float* query_feat, int Q, float* out_emb, float* out_sim, int k,
+                          float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream);
 
 /* Similarity metric of the scoring fused onto the sweep's last layer (NOPE_METRIC_*; default l2, the only
  * one the reference implements, model.py:254-266).  occlusion_threshold is used by NOPE_METRIC_COSINE_OCC. */
@@ -159,6 +171,14 @@ int64_t nope_encoder_last_launch_count(const nope_encoder_t* e);
 int nope_score_topk(const float* query_feat, const float* emb, int B, int N, int C, int HW,
                     int metric, float occlusion_threshold, int k, float* out_sim, float* out_topv,
                     int64_t* out_topi, int64_t idx_base, void* stream);
+/* The same with the reference's broadcasting of query_feat against template_feat (model.py:260-262):
+ *   query_feat [B, Q, C, HW] fp32, emb [Bt, N, C, HW] fp32 with Bt = 1 (one template set for every query)
+ *   or Bt = B (templates of row b for the Q queries of row b) -> sim [B, Q, N], topv/topi [B, Q, k].
+ * No [B*Q, N, C, HW] difference tensor is formed: each template is read once and scored against its queries.
+ * nope_score_topk is the Q = 1, Bt = B case. */
+int nope_score_topk_multi(const float* query_feat, const float* emb, int B, int Q, int Bt, int N, int C, int HW,
+                          int metric, float occlusion_threshold, int k, float* out_sim, float* out_topv,
+                          int64_t* out_topi, int64_t idx_base, void* stream);
 
 /* Rank an existing similarity matrix sim [B, N] (used to merge per-GPU shards). */
 int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_topi,
@@ -256,6 +276,11 @@ int nope_ldm_set_option(nope_ldm_t* m, const char* name, int value);
 int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
                    const float* query_latent, float* out_emb, float* out_sim, int k,
                    float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream);
+/* Q queries per reference, as nope_unet_sweep_multi: query_latent [B, Q, latent_ch, 32, 32], out_sim [B, Q, N],
+ * out_topv / out_topi [B, Q, k]; nope_ldm_sweep is the Q = 1 case. */
+int nope_ldm_sweep_multi(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
+                         const float* query_latent, int Q, float* out_emb, float* out_sim, int k,
+                         float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream);
 int64_t nope_ldm_last_launch_count(const nope_ldm_t* m);
 /* Profiling hook (bench.py roofline), as nope_unet_profile: CUDA events around every tensor-core
  * GEMM / convolution launch (index 0) and every attention launch (index 1) of later sweeps.

@@ -23,6 +23,8 @@ SIGNATURES = {
     "nope_unet_set_conv_impl": (C.c_int, [C.c_void_p, C.c_int]),
     "nope_unet_sweep": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, c_f32p,
                                   c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
+    "nope_unet_sweep_multi": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, c_f32p,
+                                        c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_unet_last_launch_count": (C.c_int64, [C.c_void_p]),
     "nope_unet_profile": (C.c_int, [C.c_void_p, C.c_int]),
     "nope_unet_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double),
@@ -42,6 +44,9 @@ SIGNATURES = {
     "nope_encoder_last_launch_count": (C.c_int64, [C.c_void_p]),
     "nope_score_topk": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                   C.c_int, c_f32p, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
+    "nope_score_topk_multi": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                        C.c_int, C.c_float, C.c_int, c_f32p, c_f32p, c_i64p, C.c_int64,
+                                        C.c_void_p]),
     "nope_unet_set_metric": (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
     "nope_topk": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_topk_pack_floats": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
@@ -66,6 +71,8 @@ SIGNATURES = {
     "nope_ldm_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "nope_ldm_sweep": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, c_f32p,
                                  c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
+    "nope_ldm_sweep_multi": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, c_f32p,
+                                       c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_ldm_last_launch_count": (C.c_int64, [C.c_void_p]),
     "nope_ldm_profile": (C.c_int, [C.c_void_p, C.c_int]),
     "nope_ldm_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double),

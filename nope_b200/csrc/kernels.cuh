@@ -746,8 +746,9 @@ __global__ void upsample2x_kernel(const __half* __restrict__ x, __half* __restri
 // final_conv[1] (1x1, C -> Cl <= 8, u_net.py:156) fused with the reference's "l2" score
 // (model.py:260-262):  score[h] = -sum_p sqrt( sum_c (q[c,p] - e[c,p])^4 ).
 // x: [n_hyp, hw, C] fp16; w fp32 [Cl, C]; emb (optional) fp32 [n_hyp, Cl, hw] (NCHW);
-// query (optional) fp32 [B, Cl, hw]; partial (optional) [n_hyp, nslab] positive sums.
-// One thread per pixel, 128 pixels per CTA.
+// query fp32 [B, Q, Cl, hw] (Q queries per reference; needed when partial is set);
+// partial (optional) [n_hyp, Q, nslab, kScoreParts] sums.
+// kFinalPPT pixels per thread, kFinalPix pixels per CTA.
 // ----------------------------------------------------------------------------
 constexpr int kFinalThreads = 128;
 constexpr int kFinalPPT = 4;                               // pixels per thread of final_conv_score_kernel
@@ -771,13 +772,13 @@ final_conv_score_kernel(const __half* __restrict__ x, const float* __restrict__ 
                         const float* __restrict__ query, const int* __restrict__ ref_of,
                         float* __restrict__ partial, int hw, int C, int Cl,
                         const __half* __restrict__ x_lo = nullptr, int metric = 0, float occ_thr = 0.f,
-                        bool bf = false) {
+                        bool bf = false, int Q = 1) {
   pdl_sync();
   // weights transposed to [C][kMaxLatent] (zero beyond Cl): the 8 outputs of one input channel are two aligned 16-byte
   // broadcast loads, and every loaded weight serves the kFinalPPT pixels of the thread.  (With a [Cl][C] table and one
   // pixel per thread every FMA had its own 4-byte shared-memory load: 1.5 TB/s, bound by the load-store unit.)
   extern __shared__ __align__(16) float s_w[];
-  __shared__ float s_part[kScoreParts][kFinalThreads / 32];
+  __shared__ float s_part[2][kScoreParts][kFinalThreads / 32];
   const int slab = blockIdx.x, h = blockIdx.y, nslab = gridDim.x;
   for (int i = threadIdx.x; i < kMaxLatent * C; i += kFinalThreads) {
     const int k = i / kMaxLatent, c = i - k * kMaxLatent;
@@ -830,18 +831,29 @@ final_conv_score_kernel(const __half* __restrict__ x, const float* __restrict__ 
       }
     }
   }
-  float dist = 0.f, d1 = 0.f, d2 = 0.f;      // metric-dependent partial sums over this thread's pixels
+  if (emb) {                                 // the template is stored once, whatever the number of queries
 #pragma unroll
-  for (int u = 0; u < kFinalPPT; ++u) {
-    const int p = pix[u];
-    if (p >= hw) continue;
-    if (emb) {
+    for (int u = 0; u < kFinalPPT; ++u) {
+      if (pix[u] >= hw) continue;
 #pragma unroll
       for (int c = 0; c < kMaxLatent; ++c)
-        if (c < Cl) emb[((long long)h * Cl + c) * hw + p] = acc[u][c];
+        if (c < Cl) emb[((long long)h * Cl + c) * hw + pix[u]] = acc[u][c];
     }
-    if (query) {
-      const float* qp = query + (long long)ref_of[h] * Cl * hw + p;
+  }
+  if (!partial) return;
+  // Every query of this hypothesis's reference is scored against the accumulators in registers.  The sums of
+  // one (hypothesis, query) pair run in the same order for any Q, so a Q-query sweep reproduces Q one-query
+  // sweeps bit for bit.  s_part is double-buffered: the writes of query q + 2 follow the barrier of q + 1,
+  // which the readers of query q have passed.
+  const long long qrow0 = (long long)ref_of[h] * Q;
+#pragma unroll 1
+  for (int qi = 0; qi < Q; ++qi) {
+    float dist = 0.f, d1 = 0.f, d2 = 0.f;      // metric-dependent partial sums over this thread's pixels
+#pragma unroll
+    for (int u = 0; u < kFinalPPT; ++u) {
+      const int p = pix[u];
+      if (p >= hw) continue;
+      const float* qp = query + (qrow0 + qi) * Cl * hw + p;     // coalesced: consecutive threads, consecutive pixels
       float s4 = 0.f, qe = 0.f, qq = 0.f, ee = 0.f;
 #pragma unroll
       for (int c = 0; c < kMaxLatent; ++c)
@@ -863,107 +875,114 @@ final_conv_score_kernel(const __half* __restrict__ x, const float* __restrict__ 
         dist += sc > occ_thr ? sc : 0.f;
       }
     }
-  }
-  if (partial) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       dist += __shfl_xor_sync(0xffffffffu, dist, o);
       d1 += __shfl_xor_sync(0xffffffffu, d1, o);
       d2 += __shfl_xor_sync(0xffffffffu, d2, o);
     }
+    float (*sp)[kFinalThreads / 32] = s_part[qi & 1];
     if ((threadIdx.x & 31) == 0) {
-      s_part[0][threadIdx.x >> 5] = dist;
-      s_part[1][threadIdx.x >> 5] = d1;
-      s_part[2][threadIdx.x >> 5] = d2;
+      sp[0][threadIdx.x >> 5] = dist;
+      sp[1][threadIdx.x >> 5] = d1;
+      sp[2][threadIdx.x >> 5] = d2;
     }
     __syncthreads();
     if (threadIdx.x < kScoreParts) {
       float t = 0.f;
-      for (int i = 0; i < kFinalThreads / 32; ++i) t += s_part[threadIdx.x][i];
-      partial[((long long)h * nslab + slab) * kScoreParts + threadIdx.x] = t;
+      for (int i = 0; i < kFinalThreads / 32; ++i) t += sp[threadIdx.x][i];
+      partial[(((long long)h * Q + qi) * nslab + slab) * kScoreParts + threadIdx.x] = t;
     }
   }
 }
 
 // Standalone score of materialised embeddings (PoseConditional.retrieval, model.py:254-266):
-// emb fp32 [B, N, Cl, hw], query fp32 [B, Cl, hw].  metric 0: reference "l2";
-// metric 1: cosine over the flattened descriptor (extension, eps 1e-8).
-// One CTA per (b, n).
+// emb fp32 [Bt, N, Cl, hw], query rows fp32 [Bt * rows, Cl, hw] -> sim [Bt * rows, N]: query row r is scored
+// against the templates of batch r / rows (the reference's broadcasting of query_feat against template_feat).
+// metric 0: reference "l2"; 1: cosine over the flattened descriptor; 2: occlusion-aware cosine (extensions).
+// One CTA per template (b, n) loops over its query rows: the template is read from DRAM once, and every row's
+// sum runs in the same order whatever the number of rows.
 __global__ void __launch_bounds__(256)
 score_kernel(const float* __restrict__ query, const float* __restrict__ emb,
-             float* __restrict__ sim, int N, int Cl, int hw, int metric, float occ_thr) {
-  __shared__ float s_a[8], s_b[8], s_c[8];
+             float* __restrict__ sim, int N, int Cl, int hw, int metric, float occ_thr, int rows = 1) {
+  __shared__ float s_a[2][8], s_b[2][8], s_c[2][8];     // double-buffered across rows
   const int n = blockIdx.x, b = blockIdx.y;
   const float* e = emb + ((long long)b * N + n) * Cl * hw;
-  const float* q = query + (long long)b * Cl * hw;
-  float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-  for (int p = threadIdx.x; p < hw; p += blockDim.x) {
-    if (metric == 0) {
-      float s4 = 0.f;
-      for (int c = 0; c < Cl; ++c) {
-        const float d = q[c * hw + p] - e[c * hw + p];
-        const float d2 = d * d;
-        s4 = fmaf(d2, d2, s4);
+  for (int j = 0; j < rows; ++j) {
+    const long long r = (long long)b * rows + j;
+    const float* q = query + r * Cl * hw;
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+    for (int p = threadIdx.x; p < hw; p += blockDim.x) {
+      if (metric == 0) {
+        float s4 = 0.f;
+        for (int c = 0; c < Cl; ++c) {
+          const float d = q[c * hw + p] - e[c * hw + p];
+          const float d2 = d * d;
+          s4 = fmaf(d2, d2, s4);
+        }
+        a0 += sqrtf(s4);
+      } else if (metric == 1) {
+        for (int c = 0; c < Cl; ++c) {
+          const float x = q[c * hw + p], y = e[c * hw + p];
+          a0 = fmaf(x, y, a0);
+          a1 = fmaf(x, x, a1);
+          a2 = fmaf(y, y, a2);
+        }
+      } else {
+        float qe = 0.f, qq = 0.f, ee = 0.f;
+        for (int c = 0; c < Cl; ++c) {
+          const float x = q[c * hw + p], y = e[c * hw + p];
+          qe = fmaf(x, y, qe);
+          qq = fmaf(x, x, qq);
+          ee = fmaf(y, y, ee);
+        }
+        const float sc = qe / (fmaxf(sqrtf(qq), 1e-8f) * fmaxf(sqrtf(ee), 1e-8f));
+        a0 += sc > occ_thr ? sc : 0.f;
       }
-      a0 += sqrtf(s4);
-    } else if (metric == 1) {
-      for (int c = 0; c < Cl; ++c) {
-        const float x = q[c * hw + p], y = e[c * hw + p];
-        a0 = fmaf(x, y, a0);
-        a1 = fmaf(x, x, a1);
-        a2 = fmaf(y, y, a2);
-      }
-    } else {
-      float qe = 0.f, qq = 0.f, ee = 0.f;
-      for (int c = 0; c < Cl; ++c) {
-        const float x = q[c * hw + p], y = e[c * hw + p];
-        qe = fmaf(x, y, qe);
-        qq = fmaf(x, x, qq);
-        ee = fmaf(y, y, ee);
-      }
-      const float sc = qe / (fmaxf(sqrtf(qq), 1e-8f) * fmaxf(sqrtf(ee), 1e-8f));
-      a0 += sc > occ_thr ? sc : 0.f;
     }
-  }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    a0 += __shfl_xor_sync(0xffffffffu, a0, o);
-    a1 += __shfl_xor_sync(0xffffffffu, a1, o);
-    a2 += __shfl_xor_sync(0xffffffffu, a2, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    s_a[threadIdx.x >> 5] = a0;
-    s_b[threadIdx.x >> 5] = a1;
-    s_c[threadIdx.x >> 5] = a2;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t0 = 0.f, t1 = 0.f, t2 = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { t0 += s_a[i]; t1 += s_b[i]; t2 += s_c[i]; }
-    sim[(long long)b * N + n] = finish_score(metric, t0, t1, t2, hw);
+    for (int o = 16; o > 0; o >>= 1) {
+      a0 += __shfl_xor_sync(0xffffffffu, a0, o);
+      a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+      a2 += __shfl_xor_sync(0xffffffffu, a2, o);
+    }
+    const int buf = j & 1;
+    if ((threadIdx.x & 31) == 0) {
+      s_a[buf][threadIdx.x >> 5] = a0;
+      s_b[buf][threadIdx.x >> 5] = a1;
+      s_c[buf][threadIdx.x >> 5] = a2;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float t0 = 0.f, t1 = 0.f, t2 = 0.f;
+      for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { t0 += s_a[buf][i]; t1 += s_b[buf][i]; t2 += s_c[buf][i]; }
+      sim[r * N + n] = finish_score(metric, t0, t1, t2, hw);
+    }
   }
 }
 
 // ----------------------------------------------------------------------------
 // sim = -(sum of slab partials) and top-k (model.py:265 topk(k=5)); descending score,
-// ties -> lowest index.  One CTA per batch row.  idx_base is added to the indices so a
-// shard reports global pose indices.
+// ties -> lowest index.  One CTA per row (b, q) of sim [B, Q, N]; partial is [B, N, Q, nslab, nparts].
+// idx_base is added to the indices so a shard reports global pose indices.
 // ----------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 sim_topk_kernel(const float* __restrict__ partial, int nslab, float* __restrict__ sim, int N,
                 int k, float* __restrict__ top_val, long long* __restrict__ top_idx,
-                long long idx_base, int nparts = 1, int metric = 0, int hw = 1) {
+                long long idx_base, int nparts = 1, int metric = 0, int hw = 1, int Q = 1) {
   pdl_sync();
   __shared__ float s_v[8];
   __shared__ int s_i[8];
   __shared__ int s_chosen[64];
-  const int b = blockIdx.x;
+  const int b = blockIdx.x;              // row b * Q + q
   float* srow = sim + (long long)b * N;
   if (partial) {
+    const int bb = b / Q, qi = b - bb * Q;
     for (int n = threadIdx.x; n < N; n += blockDim.x) {
       float t[3] = {0.f, 0.f, 0.f};
+      const float* pp = partial + (((long long)bb * N + n) * Q + qi) * nslab * nparts;
       for (int s = 0; s < nslab; ++s)
-        for (int q = 0; q < nparts; ++q) t[q] += partial[(((long long)b * N + n) * nslab + s) * nparts + q];
+        for (int q = 0; q < nparts; ++q) t[q] += pp[s * nparts + q];
       srow[n] = finish_score(metric, t[0], t[1], t[2], hw);
     }
     __syncthreads();

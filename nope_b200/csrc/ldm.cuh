@@ -871,8 +871,9 @@ struct nope_ldm {
   }
 
   // UNetModelPose.forward for hypotheses [hyp0, hyp0 + n) of the flattened (b, pose) list
+  // query [B, Q, Cl, hw]; score_part [B * N, Q, nslab]
   int forward_chunk(const float* poses, int hyp0, int n, int N, const float* query, float* out_emb,
-                    float* score_part, cudaStream_t st) {
+                    float* score_part, cudaStream_t st, int Q = 1) {
     using namespace nope;
     ldm_ref_of_kernel<<<(n + 255) / 256, 256, 0, st>>>(ref_of, hyp0, N, n);
     ++launches;
@@ -944,7 +945,7 @@ struct nope_ldm {
     if (conv(convs.at("out.2"), T1, T2, S, n, st, nullptr, nullptr, 0, nullptr, 0, OF)) return -1;
     ldm_score_kernel<<<dim3(nslab, n), kFinalThreads, 0, st>>>(
         OF, out_emb ? out_emb + (size_t)hyp0 * Cl * hw : nullptr, query, ref_of,
-        score_part ? score_part + (size_t)hyp0 * nslab : nullptr, hw, Cl);
+        score_part ? score_part + (size_t)hyp0 * Q * nslab : nullptr, hw, Cl, Q);
     NOPE_CUDA(cudaGetLastError());
     ++launches;
     return 0;

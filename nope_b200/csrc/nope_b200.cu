@@ -982,8 +982,9 @@ struct nope_unet {
   }
 
   // UNet.forward for hypotheses [hyp0, hyp0 + n) of the flattened (b, pose) list
+  // query_feat [B, Q, Cl, hw]; score_part [B * N, Q, nslab, kScoreParts]
   int forward_chunk(const float* poses, int hyp0, int n, int N, const float* query_feat,
-                    float* out_emb, float* score_part, cudaStream_t st) {
+                    float* out_emb, float* score_part, cudaStream_t st, int Q = 1) {
     const bool sp = split();
     auto A = [&](const Act& buf, int C) { return Act(buf.hi, C, sp ? buf.lo : nullptr); };
     // hypothesis -> reference image
@@ -1076,8 +1077,8 @@ struct nope_unet {
     const int nslab = (hw + kFinalPix - 1) / kFinalPix;
     NOPE_CUDA(launch_pdl(final_conv_score_kernel, dim3(nslab, n), dim3(kFinalThreads), (size_t)kMaxLatent * dim * sizeof(float),
                          st, curb.hi, final_w, final_b, out_emb ? out_emb + (size_t)hyp0 * Cl * hw : nullptr, query_feat,
-                         ref_of, score_part ? score_part + (size_t)hyp0 * nslab * kScoreParts : nullptr, hw, dim, Cl,
-                         sp ? curb.lo : nullptr, metric, occ_threshold, bf()));
+                         ref_of, score_part ? score_part + (size_t)hyp0 * Q * nslab * kScoreParts : nullptr, hw, dim,
+                         Cl, sp ? curb.lo : nullptr, metric, occ_threshold, bf(), Q));
     ++launches;
     return 0;
   }
@@ -1290,11 +1291,13 @@ int nope_unet_profile_read(nope_unet_t* u, double* conv_ms, double* conv_flops, 
   return 0;
 }
 
-int nope_unet_sweep(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
-                    const float* query_feat, float* out_emb, float* out_sim, int k, float* out_topv,
-                    int64_t* out_topi, int64_t idx_base, void* stream) {
+int nope_unet_sweep_multi(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
+                          const float* query_feat, int Q, float* out_emb, float* out_sim, int k, float* out_topv,
+                          int64_t* out_topi, int64_t idx_base, void* stream) {
   NOPE_CHECK(u && u->finalized, "engine not finalized");
   NOPE_CHECK(ref_feat && poses && B >= 1 && N >= 1, "bad arguments");
+  NOPE_CHECK(Q >= 1, "Q (queries per reference) must be >= 1");
+  NOPE_CHECK((int64_t)B * Q * N <= INT32_MAX, "B * Q * N exceeds the scored-triple limit (2^31 - 1)");
   NOPE_CHECK(!(out_sim || k > 0) || query_feat, "scores / top-k need query_feat");
   NOPE_CHECK(k >= 0 && k <= N && k <= 64, "k must be in [0, min(N, 64)]");
   NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
@@ -1305,7 +1308,7 @@ int nope_unet_sweep(nope_unet_t* u, const float* ref_feat, const float* poses, i
   const int cap = std::min(u->chunk, total);
   // no allocation here when the caller provided the workspace (nope_unet_set_workspace); otherwise the
   // engine grows its own slab (device synchronisation + cudaMalloc on growth only)
-  if (u->ensure_workspace(cap, B, query_feat ? total : 0)) return -1;
+  if (u->ensure_workspace(cap, B, query_feat ? total * Q : 0)) return -1;
   if (u->prepare_stream(st)) return -1;
   const int hw = u->S0 * u->S0;
   const int nslab = (hw + kFinalPix - 1) / kFinalPix;
@@ -1313,15 +1316,22 @@ int nope_unet_sweep(nope_unet_t* u, const float* ref_feat, const float* poses, i
   if (u->prestage(ref_feat, B, st)) return -1;
   for (int h0 = 0; h0 < total; h0 += cap) {
     const int n = std::min(cap, total - h0);
-    if (u->forward_chunk(poses, h0, n, N, query_feat, out_emb, part, st)) return -1;
+    if (u->forward_chunk(poses, h0, n, N, query_feat, out_emb, part, st, Q)) return -1;
   }
   if (query_feat && (out_sim || k > 0)) {
     float* sim = out_sim ? out_sim : u->sim_buf;
-    NOPE_CUDA(launch_pdl(sim_topk_kernel, dim3(B), dim3(256), 0, st, part, nslab, sim, N, k, out_topv,
-                         reinterpret_cast<long long*>(out_topi), (long long)idx_base, kScoreParts, u->metric, hw));
+    NOPE_CUDA(launch_pdl(sim_topk_kernel, dim3(B * Q), dim3(256), 0, st, part, nslab, sim, N, k, out_topv,
+                         reinterpret_cast<long long*>(out_topi), (long long)idx_base, kScoreParts, u->metric, hw, Q));
     ++u->launches;
   }
   return 0;
+}
+
+int nope_unet_sweep(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
+                    const float* query_feat, float* out_emb, float* out_sim, int k, float* out_topv,
+                    int64_t* out_topi, int64_t idx_base, void* stream) {
+  return nope_unet_sweep_multi(u, ref_feat, poses, B, N, query_feat, 1, out_emb, out_sim, k, out_topv, out_topi,
+                               idx_base, stream);
 }
 
 int nope_unet_set_metric(nope_unet_t* u, int metric, float occlusion_threshold) {
@@ -1333,23 +1343,36 @@ int nope_unet_set_metric(nope_unet_t* u, int metric, float occlusion_threshold) 
   return 0;
 }
 
-int nope_score_topk(const float* query_feat, const float* emb, int B, int N, int C, int HW, int metric,
-                    float occlusion_threshold, int k, float* out_sim, float* out_topv, int64_t* out_topi,
-                    int64_t idx_base, void* stream) {
+int nope_score_topk_multi(const float* query_feat, const float* emb, int B, int Q, int Bt, int N, int C, int HW,
+                          int metric, float occlusion_threshold, int k, float* out_sim, float* out_topv,
+                          int64_t* out_topi, int64_t idx_base, void* stream) {
   NOPE_CHECK(query_feat && emb && out_sim, "null argument");
+  NOPE_CHECK(B >= 1 && N >= 1 && C >= 1 && HW >= 1, "bad arguments");
+  NOPE_CHECK(Q >= 1, "Q (queries per batch row) must be >= 1");
+  NOPE_CHECK(Bt == 1 || Bt == B, "template batch Bt must be 1 or B");
+  NOPE_CHECK(Bt <= 65535 && (int64_t)B * Q * N <= INT32_MAX, "too many templates or (query, template) pairs");
   NOPE_CHECK(metric == NOPE_METRIC_L2 || metric == NOPE_METRIC_COSINE || metric == NOPE_METRIC_COSINE_OCC,
              "unknown similarity metric (l2, cosine and cosine_occlusion exist)");
   NOPE_CHECK(k >= 0 && k <= N && k <= 64, "k must be in [0, min(N, 64)]");
   NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  score_kernel<<<dim3(N, B), 256, 0, st>>>(query_feat, emb, out_sim, N, C, HW, metric, occlusion_threshold);
+  // query rows [B * Q] in order; template batch t serves rows [t * rows, (t + 1) * rows)
+  const int rows = B * Q / Bt;
+  score_kernel<<<dim3(N, Bt), 256, 0, st>>>(query_feat, emb, out_sim, N, C, HW, metric, occlusion_threshold, rows);
   NOPE_CUDA(cudaGetLastError());
   if (k > 0) {
-    sim_topk_kernel<<<B, 256, 0, st>>>(nullptr, 0, out_sim, N, k, out_topv,
-                                       reinterpret_cast<long long*>(out_topi), (long long)idx_base);
+    sim_topk_kernel<<<B * Q, 256, 0, st>>>(nullptr, 0, out_sim, N, k, out_topv,
+                                           reinterpret_cast<long long*>(out_topi), (long long)idx_base);
     NOPE_CUDA(cudaGetLastError());
   }
   return 0;
+}
+
+int nope_score_topk(const float* query_feat, const float* emb, int B, int N, int C, int HW, int metric,
+                    float occlusion_threshold, int k, float* out_sim, float* out_topv, int64_t* out_topi,
+                    int64_t idx_base, void* stream) {
+  return nope_score_topk_multi(query_feat, emb, B, 1, B, N, C, HW, metric, occlusion_threshold, k, out_sim, out_topv,
+                               out_topi, idx_base, stream);
 }
 
 int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_topi, int64_t idx_base,
@@ -1847,11 +1870,13 @@ int nope_ldm_profile_read(nope_ldm_t* m, double* ms, double* flops, int64_t* lau
   return 0;
 }
 
-int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
-                   const float* query_latent, float* out_emb, float* out_sim, int k, float* out_topv,
-                   int64_t* out_topi, int64_t idx_base, void* stream) {
+int nope_ldm_sweep_multi(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
+                         const float* query_latent, int Q, float* out_emb, float* out_sim, int k, float* out_topv,
+                         int64_t* out_topi, int64_t idx_base, void* stream) {
   NOPE_CHECK(m && m->finalized, "engine not finalized");
   NOPE_CHECK(ref_latent && poses && B >= 1 && N >= 1, "bad arguments");
+  NOPE_CHECK(Q >= 1, "Q (queries per reference) must be >= 1");
+  NOPE_CHECK((int64_t)B * Q * N <= INT32_MAX, "B * Q * N exceeds the scored-triple limit (2^31 - 1)");
   NOPE_CHECK(!(out_sim || k > 0) || query_latent, "scores / top-k need query_latent");
   NOPE_CHECK(k >= 0 && k <= N && k <= 64, "k must be in [0, min(N, 64)]");
   NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
@@ -1859,13 +1884,14 @@ int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, i
   NOPE_CUDA(cudaSetDevice(m->device));
   m->launches = 0;
   const int total = B * N;
+  const size_t scored = (size_t)total * Q;      // (b, q, pose) triples
   const int cap = std::min(m->chunk, total);
   if (m->ensure_workspace(cap, B)) return -1;
   const int hw = m->S0 * m->S0;
   const int nslab = (hw + kFinalThreads - 1) / kFinalThreads;
   float* part = nullptr;
   if (query_latent) {
-    const size_t need = (size_t)total * nslab;
+    const size_t need = scored * nslab;
     if (need > m->score_partial_cap) {
       NOPE_CUDA(cudaStreamSynchronize(st));
       if (m->score_partial) cudaFree(m->score_partial);
@@ -1877,25 +1903,32 @@ int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, i
   if (m->prestage(ref_latent, B, st)) return -1;
   for (int h0 = 0; h0 < total; h0 += cap) {
     const int n = std::min(cap, total - h0);
-    if (m->forward_chunk(poses, h0, n, N, query_latent, out_emb, part, st)) return -1;
+    if (m->forward_chunk(poses, h0, n, N, query_latent, out_emb, part, st, Q)) return -1;
   }
   if (query_latent && (out_sim || k > 0)) {
     float* sim = out_sim;
     if (!sim) {
-      if ((size_t)total > m->sim_buf_cap) {
+      if (scored > m->sim_buf_cap) {
         NOPE_CUDA(cudaStreamSynchronize(st));
         if (m->sim_buf) cudaFree(m->sim_buf);
-        NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&m->sim_buf), (size_t)total * sizeof(float)));
-        m->sim_buf_cap = total;
+        NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&m->sim_buf), scored * sizeof(float)));
+        m->sim_buf_cap = scored;
       }
       sim = m->sim_buf;
     }
-    sim_topk_kernel<<<B, 256, 0, st>>>(part, nslab, sim, N, k, out_topv, reinterpret_cast<long long*>(out_topi),
-                                       (long long)idx_base);
+    sim_topk_kernel<<<B * Q, 256, 0, st>>>(part, nslab, sim, N, k, out_topv, reinterpret_cast<long long*>(out_topi),
+                                           (long long)idx_base, 1, 0, 1, Q);
     NOPE_CUDA(cudaGetLastError());
     ++m->launches;
   }
   return 0;
+}
+
+int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
+                   const float* query_latent, float* out_emb, float* out_sim, int k, float* out_topv,
+                   int64_t* out_topi, int64_t idx_base, void* stream) {
+  return nope_ldm_sweep_multi(m, ref_latent, poses, B, N, query_latent, 1, out_emb, out_sim, k, out_topv, out_topi,
+                              idx_base, stream);
 }
 
 int nope_ldm_debug_tap(nope_ldm_t* m, const float* ref_latent, const float* poses, int N, const char* tap,

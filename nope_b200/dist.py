@@ -25,7 +25,8 @@ def shard_range(n_poses, rank, world):
 
 
 def record_layout(B, k, per, want_sim):
-    """Offsets (in floats) of the packed record: topv | pad | topi (int64) | sim slice | pad.
+    """Offsets (in floats) of the packed record: topv | pad | topi (int64) | sim slice | pad, for B rows (a
+    multi-query sweep has one row per (reference, query) pair: B = references * queries).
     The record length is a multiple of 4 floats: records sit back to back in the gathered buffer and the merge
     kernel reads the int64 indices of EVERY rank's record in place (an odd length -- e.g. the 10 248-pose grid on
     8 GPUs: 16 + 1281 floats -- put every second record's indices on a 4-byte boundary: misaligned address)."""
@@ -118,21 +119,26 @@ class ShardedSweep:
               want_emb=False, want_sim=True, threshold=0.2):
         """-> (sim [B,N] | None, topi [B,k], emb).  `emb` (want_emb) is this rank's LOCAL slice
         [B, n_local, C, 32, 32] of the templates together with its pose range, as (emb, lo, hi):
-        templates are never gathered (164 MB per query at N = 642)."""
+        templates are never gathered (164 MB per query at N = 642).  query_feat [B,Q,C,32,32] (Q queries per
+        reference) gives sim [B,Q,N] and topi [B,Q,k]: the B*Q (reference, query) pairs are the record's rows,
+        still with one all-gather per sweep."""
+        from .unet import query_rows
         N = all_relativeR.shape[1]
         lo, hi = shard_range(N, self.rank, self.world)
         B = reference_feat.shape[0]
+        Q, lead = query_rows(query_feat, reference_feat)
+        rows = B * Q
         dev = u_net.device
-        send, recv, topv_v, topi_v, off_s, pack, per = self.record(B, k, N, want_sim, dev)
+        send, recv, topv_v, topi_v, off_s, pack, per = self.record(rows, k, N, want_sim, dev)
         emb = None
         n_local = hi - lo
         u_net.set_metric(metric, threshold)
         in_place = n_local >= k
         if in_place:
             poses = all_relativeR[:, lo:hi].contiguous()
-            out = {"topv": topv_v, "topi": topi_v}
+            out = {"topv": topv_v.view(lead + (k,)), "topi": topi_v.view(lead + (k,))}
             if want_sim:
-                out["sim"] = send[off_s: off_s + B * n_local].view(B, n_local)
+                out["sim"] = send[off_s: off_s + rows * n_local].view(lead + (n_local,))
             r = u_net.sweep(reference_feat, poses, query_feat=query_feat, want_emb=want_emb,
                             want_sim=want_sim, k=k, idx_base=lo, out=out)
             emb = r["emb"]
@@ -140,9 +146,12 @@ class ShardedSweep:
             kl = min(k, n_local)
             poses = all_relativeR[:, lo:hi].contiguous()
             r = u_net.sweep(reference_feat, poses, query_feat=query_feat, want_emb=want_emb, k=kl, idx_base=lo)
-            sim_l, tv, ti, emb = r["sim"], r["topv"], r["topi"], r["emb"]
+            sim_l, tv, ti, emb = r["sim"], r["topv"].reshape(rows, kl), r["topi"].reshape(rows, kl), r["emb"]
             self.fill_record(send, topv_v, topi_v, off_s, sim_l if want_sim else None, tv, ti)
         else:
             self.fill_record(send, topv_v, topi_v, off_s, None, None, None)
-        sim, topi = self.gather_merge(send, recv, B, k, N, per, pack, want_sim)
+        sim, topi = self.gather_merge(send, recv, rows, k, N, per, pack, want_sim)
+        if len(lead) == 2:
+            sim = sim.view(lead + (N,)) if sim is not None else None
+            topi = topi.view(lead + (k,))
         return sim, topi, ((emb, lo, hi) if want_emb else None)

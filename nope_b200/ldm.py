@@ -14,6 +14,7 @@ import ctypes as C
 import torch
 
 from . import _lib
+from .unet import query_rows
 
 
 class UNetModelPose:
@@ -125,6 +126,8 @@ class UNetModelPose:
     def sweep(self, ref_latent, poses, query_latent=None, want_emb=True, want_sim=None, k=0, idx_base=0,
               query_feat=None, out=None):
         """ref_latent [B,C,32,32], poses [B,N,6] (+ query_latent) -> dict(emb, sim, topv, topi).
+        query_latent [B,C,32,32] gives sim [B,N] / topv, topi [B,k]; [B,Q,C,32,32] (Q queries per reference, one
+        sweep) gives [B,Q,N] / [B,Q,k].
         `query_feat` is an alias of `query_latent` and `out` may carry preallocated `sim` / `topv` / `topi`
         tensors (the keywords nope_b200.unet.UNet.sweep and nope_b200.dist.ShardedSweep use), so the pose grid
         shards across GPUs the same way."""
@@ -141,27 +144,29 @@ class UNetModelPose:
         assert poses.shape[2] == self.rot_representation_dim
         if want_sim is None:
             want_sim = query_latent is not None
+        Q, lead = 1, (B,)
         if query_latent is not None:
             query_latent = query_latent.to(dev, torch.float32).contiguous()
-            assert query_latent.shape == ref_latent.shape
+            Q, lead = query_rows(query_latent, ref_latent)
         emb = torch.empty((B, N, self.channels, 32, 32), device=dev, dtype=torch.float32) if want_emb else None
         out = out or {}
         sim = out.get("sim") if want_sim else None
         if want_sim and sim is None:
-            sim = torch.empty((B, N), device=dev, dtype=torch.float32)
+            sim = torch.empty(lead + (N,), device=dev, dtype=torch.float32)
         topv, topi = (out.get("topv"), out.get("topi")) if k > 0 else (None, None)
         if k > 0 and topv is None:
-            topv = torch.empty((B, k), device=dev, dtype=torch.float32)
-            topi = torch.empty((B, k), device=dev, dtype=torch.int64)
-        for t, shape, dt in ((sim, (B, N), torch.float32), (topv, (B, k), torch.float32), (topi, (B, k), torch.int64)):
+            topv = torch.empty(lead + (k,), device=dev, dtype=torch.float32)
+            topi = torch.empty(lead + (k,), device=dev, dtype=torch.int64)
+        for t, shape, dt in ((sim, lead + (N,), torch.float32), (topv, lead + (k,), torch.float32),
+                             (topi, lead + (k,), torch.int64)):
             if t is not None and (tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous()
                                   or t.device != dev):
                 raise ValueError("preallocated output has the wrong shape / dtype / device or is not contiguous")
         stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
-            _lib.check(lib.nope_ldm_sweep(self._handle(), _lib.ptr(ref_latent), _lib.ptr(poses), B, N,
-                                          _lib.ptr(query_latent), _lib.ptr(emb), _lib.ptr(sim), k,
-                                          _lib.ptr(topv), _lib.ptr(topi), idx_base, C.c_void_p(stream)))
+            _lib.check(lib.nope_ldm_sweep_multi(self._handle(), _lib.ptr(ref_latent), _lib.ptr(poses), B, N,
+                                                _lib.ptr(query_latent), Q, _lib.ptr(emb), _lib.ptr(sim), k,
+                                                _lib.ptr(topv), _lib.ptr(topi), idx_base, C.c_void_p(stream)))
         return {"emb": emb, "sim": sim, "topv": topv, "topi": topi}
 
     def __call__(self, x, pose):
@@ -172,12 +177,23 @@ class UNetModelPose:
 
     def predict_pose(self, query_latent, ref_latent, all_relativeR, template_poses, k=5):
         """Latent-space form of nope_b200.model.PoseConditional.predict_pose for this UNet:
-        -> (R [B,k,3,3], nearest_idx [B,k], similarity [B,N])."""
-        out = self.sweep(ref_latent, all_relativeR, query_latent, want_emb=False, want_sim=True, k=k)
-        idx = out["topi"]
+        -> (R [B,k,3,3], nearest_idx [B,k], similarity [B,N]).  As there, query_latent [B,Q,C,32,32] gives
+        [B,Q,...] outputs, and query_latent [Q,C,32,32] with one reference (ref_latent [1,...], all_relativeR
+        [1,N,6]) gives [Q,...]; both run one sweep."""
+        from .model import multi_query_form
+        q, squeeze = multi_query_form(query_latent, ref_latent)
+        out = self.sweep(ref_latent, all_relativeR, q, want_emb=False, want_sim=True, k=k)
+        idx, sim = out["topi"], out["sim"]
+        if squeeze:
+            idx, sim = idx[0], sim[0]
         tp = template_poses.to(idx.device)
-        R = tp[idx] if tp.dim() == 3 else torch.stack([tp[b][idx[b]] for b in range(idx.shape[0])])
-        return R, idx, out["sim"]
+        if squeeze and tp.dim() == 4:
+            tp = tp[0]                  # the one reference's grid
+        if tp.dim() == 3:
+            R = tp[idx]
+        else:
+            R = torch.stack([tp[b][idx[b]] for b in range(idx.shape[0])])
+        return R, idx, sim
 
     # ------------------------------------------------------------------ debug / parity hooks
     def debug_tap(self, ref_latent, poses, tap):

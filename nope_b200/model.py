@@ -93,6 +93,9 @@ class PoseConditional:
     # ------------------------------------------------------------------ model.py:254-266
     @torch.no_grad()
     def retrieval(self, query, template_feat, k=5):
+        """-> (similarity, nearest_idx).  Query and template batches follow the reference's broadcasting
+        (model.py:260-262): equal batches give [B,N]; templates [1,N,...] serve every query ([Bq,N]: templates
+        generated once, queries streamed); one query against [Bt,N,...] templates gives [Bt,N]."""
         metric = getattr(self.testing_config, "similarity_metric", "l2")
         if metric not in _METRICS:
             raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
@@ -110,15 +113,28 @@ class PoseConditional:
                      return_templates=False):
         """-> (R [B,k,3,3] | None, nearest_idx [B,k] int64, similarity [B,N]).  The scores and
         the ranking come out of the sweep's fused last layer; the [B,N,C,32,32] templates are
-        only materialised when asked for."""
+        only materialised when asked for.
+
+        Several queries of one object share the reference's sweep (the templates do not depend on the query):
+          query [B,Q,3,H,W] with reference [B,3,H,W] -> R [B,Q,k,3,3], nearest_idx [B,Q,k], similarity [B,Q,N];
+          query [Q,3,H,W] with reference [1,3,H,W] and all_relativeR [1,N,6] -> [Q,k,3,3], [Q,k], [Q,N]
+          (the reference's broadcasting of one template set against a query batch).
+        Query and reference images go through one encoder call, the templates through one sweep."""
         metric = getattr(self.testing_config, "similarity_metric", "l2")
         if metric not in _METRICS:
             raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+        query, squeeze = multi_query_form(query, reference)
         enc = self.u_net.encoder
         self.u_net.set_metric(metric, self._occlusion_threshold())     # scored in the sweep's last layer
-        B = query.shape[0]
-        feats = enc.encode_image(torch.cat([query.to(self.device), reference.to(self.device)]))
-        query_feat, reference_feat = feats[:B], feats[B:]
+        if query.dim() == reference.dim():
+            B = query.shape[0]
+            feats = enc.encode_image(torch.cat([query.to(self.device), reference.to(self.device)]))
+            query_feat, reference_feat = feats[:B], feats[B:]
+        else:
+            B, Q = query.shape[:2]
+            feats = enc.encode_image(torch.cat([query.reshape(B * Q, *query.shape[2:]).to(self.device),
+                                                reference.to(self.device)]))
+            query_feat, reference_feat = feats[:B * Q].view(B, Q, *feats.shape[1:]), feats[B * Q:]
         N = all_relativeR.shape[1]
         k = min(k, N)
         if self.dist is not None:
@@ -129,6 +145,8 @@ class PoseConditional:
             out = self.u_net.sweep(reference_feat, all_relativeR, query_feat=query_feat,
                                    want_emb=return_templates, k=k)
             sim, topi, emb = out["sim"], out["topi"], out["emb"]
+        if squeeze:
+            sim, topi = sim[0], topi[0]
         R = None
         if template_poses is not None:
             tp = template_poses[0] if template_poses.dim() == 4 else template_poses
@@ -185,28 +203,69 @@ class PoseConditional:
         return out
 
 
+def multi_query_form(query, reference):
+    """-> (query, squeeze).  query [B,...] with reference [B,...]: one query per reference, as given.
+    query [B,Q,...]: Q queries per reference, as given.  query [Q,...] with reference [1,...]: the broadcast form,
+    returned as [1,Q,...] with squeeze=True (outputs lose the leading 1).  Anything else raises ValueError."""
+    B, rest = reference.shape[0], tuple(reference.shape[1:])
+    if query.dim() == reference.dim() and tuple(query.shape[1:]) == rest:
+        if query.shape[0] == B:
+            return query, False
+        if B == 1 and query.shape[0] >= 1:
+            return query.unsqueeze(0), True
+    elif query.dim() == reference.dim() + 1 and tuple(query.shape[2:]) == rest and query.shape[0] == B \
+            and query.shape[1] >= 1:
+        return query, False
+    raise ValueError(f"query {tuple(query.shape)} does not fit reference {tuple(reference.shape)}: expected "
+                     f"[B, ...], [B, Q, ...] or (one reference) [Q, ...]")
+
+
+def broadcast_batches(bq, bt):
+    """Batch rule of the reference's retrieval (model.py:260-262), where [Bq,1,...] queries meet [Bt,N,...]
+    templates: -> (B, Q, Bt, rows of the result) in the terms of nope_score_topk_multi.  Equal batches pair
+    up, a template batch of 1 serves every query, a query batch of 1 is scored against every template batch;
+    anything else raises ValueError (torch would not broadcast it either)."""
+    if bq < 1 or bt < 1:
+        raise ValueError(f"empty batch (query {bq}, templates {bt})")
+    if bq == bt:
+        return bq, 1, bt, bq
+    if bt == 1:
+        return 1, bq, 1, bq
+    if bq == 1:
+        return bt, 1, bt, bt        # the one query is repeated per template batch
+    raise ValueError(f"query batch {bq} and template batch {bt} do not broadcast (equal, or one of them 1)")
+
+
 def score_topk(query_feat, template_feat, k=5, metric="l2", idx_base=0, threshold=0.2):
     """similarity [B,N] and nearest_idx [B,k] of materialised templates
-    (the arithmetic of model.py:260-265) on the GPU."""
+    (the arithmetic of model.py:260-265) on the GPU.  query_feat [Bq,C,h,w] and template_feat [Bt,N,C,h,w]
+    broadcast as in the reference (broadcast_batches): B = max(Bq, Bt)."""
     if metric not in _METRICS:
         raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+    if template_feat.dim() != 5 or query_feat.dim() != 4 or tuple(query_feat.shape[1:]) != tuple(template_feat.shape[2:]):
+        raise ValueError(f"query_feat [B,C,h,w] and template_feat [B,N,C,h,w] expected; got "
+                         f"{tuple(query_feat.shape)} and {tuple(template_feat.shape)}")
+    B, Q, Bt, rows = broadcast_batches(query_feat.shape[0], template_feat.shape[0])
     lib = _lib.load()
     dev = template_feat.device
     if dev.type != "cuda":
         raise _lib.NopeError("score_topk needs CUDA tensors (no CPU fallback)")
-    q = query_feat.to(dev, torch.float32).contiguous()
+    q = query_feat.to(dev, torch.float32)
+    if q.shape[0] != B * Q:
+        q = q.expand(B * Q, *q.shape[1:])
+    q = q.contiguous()
     t = template_feat.to(torch.float32).contiguous()
-    B, N, Cc = t.shape[0], t.shape[1], t.shape[2]
+    N, Cc = t.shape[1], t.shape[2]
     hw = t.shape[3] * t.shape[4]
     if k > N:
         raise RuntimeError(f"selected index k out of range (k={k}, N={N})")  # torch.topk's error
-    sim = torch.empty((B, N), device=dev, dtype=torch.float32)
-    topv = torch.empty((B, k), device=dev, dtype=torch.float32)
-    topi = torch.empty((B, k), device=dev, dtype=torch.int64)
+    sim = torch.empty((rows, N), device=dev, dtype=torch.float32)
+    topv = torch.empty((rows, k), device=dev, dtype=torch.float32)
+    topi = torch.empty((rows, k), device=dev, dtype=torch.int64)
     with torch.cuda.device(dev):
-        _lib.check(lib.nope_score_topk(_lib.ptr(q), _lib.ptr(t), B, N, Cc, hw, _METRICS[metric], float(threshold), k,
-                                       _lib.ptr(sim), _lib.ptr(topv), _lib.ptr(topi), idx_base,
-                                       C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        _lib.check(lib.nope_score_topk_multi(_lib.ptr(q), _lib.ptr(t), B, Q, Bt, N, Cc, hw, _METRICS[metric],
+                                             float(threshold), k, _lib.ptr(sim), _lib.ptr(topv), _lib.ptr(topi),
+                                             idx_base, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
     return sim, topi
 
 

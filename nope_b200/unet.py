@@ -222,6 +222,8 @@ class UNet:
               idx_base=0, out=None):
         """ref_feat [B,C,32,32], poses [B,N,6] (+ query_feat [B,C,32,32]) ->
         dict(emb [B,N,C,32,32] | None, sim [B,N] | None, topv/topi [B,k] | None).
+        query_feat may also be [B,Q,C,32,32]: Q queries per reference share the one sweep and
+        sim is [B,Q,N], topv/topi [B,Q,k].
         `out` may carry preallocated contiguous `sim` / `topv` / `topi` tensors to write into (the
         multi-GPU path points them into its all-gather record)."""
         if not self._finalized:
@@ -235,29 +237,31 @@ class UNet:
         assert poses.shape[2] == self.rot_representation_dim
         if want_sim is None:
             want_sim = query_feat is not None
+        Q, lead = 1, (B,)
         if query_feat is not None:
             query_feat = query_feat.to(dev, torch.float32).contiguous()
-            assert query_feat.shape == ref_feat.shape
+            Q, lead = query_rows(query_feat, ref_feat)
         emb = torch.empty((B, N, self.channels, 32, 32), device=dev, dtype=torch.float32) \
             if want_emb else None
         out = out or {}
         sim = out.get("sim") if want_sim else None
         if want_sim and sim is None:
-            sim = torch.empty((B, N), device=dev, dtype=torch.float32)
+            sim = torch.empty(lead + (N,), device=dev, dtype=torch.float32)
         topv, topi = (out.get("topv"), out.get("topi")) if k > 0 else (None, None)
         if k > 0 and topv is None:
-            topv = torch.empty((B, k), device=dev, dtype=torch.float32)
-            topi = torch.empty((B, k), device=dev, dtype=torch.int64)
-        for t, shape, dt in ((sim, (B, N), torch.float32), (topv, (B, k), torch.float32), (topi, (B, k), torch.int64)):
+            topv = torch.empty(lead + (k,), device=dev, dtype=torch.float32)
+            topi = torch.empty(lead + (k,), device=dev, dtype=torch.int64)
+        for t, shape, dt in ((sim, lead + (N,), torch.float32), (topv, lead + (k,), torch.float32),
+                             (topi, lead + (k,), torch.int64)):
             if t is not None:
                 assert t.is_contiguous() and tuple(t.shape) == shape and t.dtype == dt and t.device == dev
-        self.reserve(min(self._chunk, B * N), B, B * N if query_feat is not None else 0)
+        self.reserve(min(self._chunk, B * N), B, B * Q * N if query_feat is not None else 0)
         stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
-            _lib.check(lib.nope_unet_sweep(self._handle(), _lib.ptr(ref_feat), _lib.ptr(poses), B, N,
-                                           _lib.ptr(query_feat), _lib.ptr(emb), _lib.ptr(sim), k,
-                                           _lib.ptr(topv), _lib.ptr(topi), idx_base,
-                                           C.c_void_p(stream)))
+            _lib.check(lib.nope_unet_sweep_multi(self._handle(), _lib.ptr(ref_feat), _lib.ptr(poses), B, N,
+                                                 _lib.ptr(query_feat), Q, _lib.ptr(emb), _lib.ptr(sim), k,
+                                                 _lib.ptr(topv), _lib.ptr(topi), idx_base,
+                                                 C.c_void_p(stream)))
         return {"emb": emb, "sim": sim, "topv": topv, "topi": topi}
 
     def __call__(self, x, pose):
@@ -284,3 +288,16 @@ class UNet:
                                                tap.encode(), _lib.ptr(out), cap, C.byref(c),
                                                C.byref(s), C.c_void_p(stream)))
         return out[: N * c.value * s.value * s.value].view(N, c.value, s.value, s.value)
+
+
+def query_rows(query_feat, ref_feat):
+    """(Q, leading output shape) of a sweep's queries: [B,C,h,w] is one query per reference (outputs [B, ...]),
+    [B,Q,C,h,w] Q queries per reference (outputs [B,Q, ...])."""
+    B, rest = ref_feat.shape[0], tuple(ref_feat.shape[1:])
+    if query_feat.dim() == ref_feat.dim() and tuple(query_feat.shape) == (B,) + rest:
+        return 1, (B,)
+    if query_feat.dim() == ref_feat.dim() + 1 and query_feat.shape[0] == B and \
+            tuple(query_feat.shape[2:]) == rest and query_feat.shape[1] >= 1:
+        return int(query_feat.shape[1]), (B, int(query_feat.shape[1]))
+    raise ValueError(f"query_feat must be [B, ...] or [B, Q, ...] with the reference's per-image shape "
+                     f"{(B,) + rest}; got {tuple(query_feat.shape)}")
