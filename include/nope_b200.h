@@ -184,6 +184,23 @@ int nope_score_topk_multi(const float* query_feat, const float* emb, int B, int 
 int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_topi,
               int64_t idx_base, void* stream);
 
+/* Coarse-to-fine pose search (DESIGN.md section 9).  A cell table cells [n_coarse, F] int32 lists, for every
+ * pose of a coarse grid, the poses of the next finer grid whose nearest coarse pose it is (ascending, -1 padded,
+ * F = the largest cell); cells are disjoint.  Rows r = b * Q + q pair reference b with its query q.
+ * nope_pose_cells_expand: the row's keep coarse indices top_idx [R, keep] (int64; entries outside
+ * [0, n_coarse) and repeats are skipped) -> out_cand [R, M] int32, the union of their cells in top_idx order
+ * (ascending inside a cell, -1 after the last candidate), and out_poses [R, M, 6], those poses gathered from
+ * poses [B, n_fine, 6] of reference r / Q.  A padding slot gets the row's first candidate pose.
+ * Requires 1 <= keep <= 64, M >= keep * F and R == B * Q.
+ * nope_pose_cells_rank: sim [R, M] scored at cand [R, M] -> top-k over the scored candidates (descending, ties ->
+ * lowest fine index; ranks beyond the candidate count get -inf / -1) as fine indices, and optionally out_sim
+ * [R, n_fine]: -inf, with the scored entries scattered in.  Requires 1 <= k <= 64. */
+int nope_pose_cells_expand(const int64_t* top_idx, int R, int keep, const int32_t* cells, int n_coarse, int F,
+                           const float* poses, int B, int Q, int n_fine, int M,
+                           int32_t* out_cand, float* out_poses, void* stream);
+int nope_pose_cells_rank(const float* sim, const int32_t* cand, int R, int M, int n_fine, int k,
+                         float* out_sim, float* out_topv, int64_t* out_topi, void* stream);
+
 /* Multi-GPU merge (SURVEY.md 8e): each rank sweeps a contiguous slice of the pose grid and contributes
  * ONE packed record to a single all-gather:
  *   [ topv: B*k f32 | 1 pad float if B*k is odd | topi: B*k int64 (GLOBAL indices, -1 = padding) |

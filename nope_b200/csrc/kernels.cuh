@@ -962,6 +962,35 @@ score_kernel(const float* __restrict__ query, const float* __restrict__ emb,
 }
 
 // ----------------------------------------------------------------------------
+// CTA-wide arg-max of the per-thread candidates (bv, bi): descending value, ties -> lowest index,
+// bi == 0x7fffffff is "no candidate".  s_v / s_i hold one slot per warp.  The result is valid in
+// thread 0 only; the caller synchronises before it reuses s_v / s_i.
+// ----------------------------------------------------------------------------
+__device__ __forceinline__ void cta_argmax(float& bv, int& bi, float* s_v, int* s_i) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (oi != 0x7fffffff && (bi == 0x7fffffff || ov > bv || (ov == bv && oi < bi))) {
+      bv = ov;
+      bi = oi;
+    }
+  }
+  if ((threadIdx.x & 31) == 0) { s_v[threadIdx.x >> 5] = bv; s_i[threadIdx.x >> 5] = bi; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) {
+      const float ov = s_v[w];
+      const int oi = s_i[w];
+      if (oi != 0x7fffffff && (bi == 0x7fffffff || ov > bv || (ov == bv && oi < bi))) {
+        bv = ov;
+        bi = oi;
+      }
+    }
+  }
+}
+
+// ----------------------------------------------------------------------------
 // sim = -(sum of slab partials) and top-k (model.py:265 topk(k=5)); descending score,
 // ties -> lowest index.  One CTA per row (b, q) of sim [B, Q, N]; partial is [B, N, Q, nslab, nparts].
 // idx_base is added to the indices so a shard reports global pose indices.
@@ -998,29 +1027,116 @@ sim_topk_kernel(const float* __restrict__ partial, int nslab, float* __restrict_
       const float v = srow[n];
       if (v > bv || (v == bv && n < bi) || bi == 0x7fffffff) { bv = v; bi = n; }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (oi != 0x7fffffff && (bi == 0x7fffffff || ov > bv || (ov == bv && oi < bi))) {
-        bv = ov;
-        bi = oi;
-      }
-    }
-    if ((threadIdx.x & 31) == 0) { s_v[threadIdx.x >> 5] = bv; s_i[threadIdx.x >> 5] = bi; }
-    __syncthreads();
+    cta_argmax(bv, bi, s_v, s_i);
     if (threadIdx.x == 0) {
-      for (int w = 1; w < (int)(blockDim.x >> 5); ++w) {
-        const float ov = s_v[w];
-        const int oi = s_i[w];
-        if (oi != 0x7fffffff && (bi == 0x7fffffff || ov > bv || (ov == bv && oi < bi))) {
-          bv = ov;
-          bi = oi;
-        }
-      }
       s_chosen[r] = bi;
       top_val[(long long)b * k + r] = bv;
       top_idx[(long long)b * k + r] = (bi == 0x7fffffff) ? -1 : (long long)bi + idx_base;
+    }
+    __syncthreads();
+  }
+}
+
+// ----------------------------------------------------------------------------
+// Coarse-to-fine pose search (DESIGN.md section 9).  A cell table cells [n_coarse, F] lists, for every
+// coarse pose, the fine poses nearest to it (ascending, -1 padded); cells are disjoint.
+//
+// Expand: one CTA per row r = (reference r / Q, query r % Q).  The row's `keep` coarse indices top_idx [R, keep]
+// become the union of their cells, in top_idx order and ascending inside a cell: out_cand [R, M] (int32, -1 after
+// the last candidate) and the candidates' poses out_poses [R, M, 6] gathered from poses [B, n_fine, 6].  Entries
+// outside [0, n_coarse) and repeats of an earlier entry are skipped.  A padding slot carries the row's first
+// candidate pose (fine pose 0 if the row has none), so every hypothesis of the launch is a valid rotation.
+// ----------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+pose_cells_expand_kernel(const long long* __restrict__ top_idx, int keep, const int* __restrict__ cells,
+                         int n_coarse, int F, const float* __restrict__ poses, int Q, int n_fine, int M,
+                         int* __restrict__ out_cand, float* __restrict__ out_poses) {
+  __shared__ int s_cell[64];         // coarse index of slot j, -1 when skipped
+  __shared__ int s_off[65];          // first candidate slot of slot j; s_off[keep] = candidate count
+  const int r = blockIdx.x;
+  const int b = r / Q;
+  const long long* top = top_idx + (long long)r * keep;
+  if (threadIdx.x < keep) {
+    const int j = threadIdx.x;
+    const long long c = top[j];
+    bool ok = c >= 0 && c < n_coarse;
+    for (int i = 0; i < j && ok; ++i) ok = top[i] != c;
+    s_cell[j] = ok ? (int)c : -1;
+    int n = 0;
+    if (ok)
+      while (n < F && cells[c * F + n] >= 0) ++n;
+    s_off[j + 1] = n;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    s_off[0] = 0;
+    for (int j = 1; j <= keep; ++j) s_off[j] += s_off[j - 1];
+  }
+  __syncthreads();
+  const int total = s_off[keep];
+  int first = 0;
+  if (total > 0) {
+    int j = 0;
+    while (s_off[j + 1] == 0) ++j;
+    first = cells[s_cell[j] * F];
+  }
+  const float* pb = poses + (long long)b * n_fine * 6;
+  for (int m = threadIdx.x; m < M; m += blockDim.x) {
+    int fine = -1;
+    if (m < total) {
+      int j = 0;
+      while (s_off[j + 1] <= m) ++j;
+      fine = cells[s_cell[j] * F + (m - s_off[j])];
+    }
+    out_cand[(long long)r * M + m] = fine;
+    const float* src = pb + (long long)(fine >= 0 ? fine : first) * 6;
+    float* dst = out_poses + ((long long)r * M + m) * 6;
+#pragma unroll
+    for (int e = 0; e < 6; ++e) dst[e] = src[e];
+  }
+}
+
+// ----------------------------------------------------------------------------
+// Rank one stage of the coarse-to-fine search: one CTA per row of sim [R, M] scored at the fine indices
+// cand [R, M] (-1 = padding, not scored; valid entries distinct).  Top-k over the scored candidates only:
+// descending score, ties -> lowest FINE index; ranks beyond the candidate count get -inf / -1.  out_sim (optional)
+// receives the row over the whole fine grid [R, n_fine]: -inf, then the scored entries scattered in.
+// ----------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+pose_cells_rank_kernel(const float* __restrict__ sim, const int* __restrict__ cand, int M, int n_fine, int k,
+                       float* __restrict__ out_sim, float* __restrict__ top_val, long long* __restrict__ top_idx) {
+  __shared__ float s_v[8];
+  __shared__ int s_i[8];
+  __shared__ int s_chosen[64];
+  const int r = blockIdx.x;
+  const float* srow = sim + (long long)r * M;
+  const int* crow = cand + (long long)r * M;
+  if (out_sim) {
+    float* orow = out_sim + (long long)r * n_fine;
+    for (int n = threadIdx.x; n < n_fine; n += blockDim.x) orow[n] = -INFINITY;
+    __syncthreads();
+    for (int m = threadIdx.x; m < M; m += blockDim.x) {
+      const int c = crow[m];
+      if (c >= 0) orow[c] = srow[m];
+    }
+  }
+  for (int t = 0; t < k; ++t) {
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int m = threadIdx.x; m < M; m += blockDim.x) {
+      const int c = crow[m];
+      if (c < 0) continue;
+      bool used = false;
+      for (int i = 0; i < t; ++i) used |= (s_chosen[i] == c);
+      if (used) continue;
+      const float v = srow[m];
+      if (v > bv || (v == bv && c < bi) || bi == 0x7fffffff) { bv = v; bi = c; }
+    }
+    cta_argmax(bv, bi, s_v, s_i);
+    if (threadIdx.x == 0) {
+      s_chosen[t] = bi;
+      top_val[(long long)r * k + t] = bv;
+      top_idx[(long long)r * k + t] = (bi == 0x7fffffff) ? -1 : (long long)bi;
     }
     __syncthreads();
   }

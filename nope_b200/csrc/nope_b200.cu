@@ -1385,6 +1385,31 @@ int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_top
   return 0;
 }
 
+int nope_pose_cells_expand(const int64_t* top_idx, int R, int keep, const int32_t* cells, int n_coarse, int F,
+                           const float* poses, int B, int Q, int n_fine, int M, int32_t* out_cand, float* out_poses,
+                           void* stream) {
+  NOPE_CHECK(top_idx && cells && poses && out_cand && out_poses, "null argument");
+  NOPE_CHECK(keep >= 1 && keep <= 64, "keep must be in [1, 64]");
+  NOPE_CHECK(n_coarse >= 1 && F >= 1 && n_fine >= 1 && B >= 1 && Q >= 1, "bad arguments");
+  NOPE_CHECK(R >= 1 && (int64_t)B * Q == R, "R (rows) must equal B * Q");
+  NOPE_CHECK((int64_t)M >= (int64_t)keep * F, "M must be at least keep * F (the largest union of keep cells)");
+  pose_cells_expand_kernel<<<R, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const long long*>(top_idx), keep, cells, n_coarse, F, poses, Q, n_fine, M, out_cand, out_poses);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int nope_pose_cells_rank(const float* sim, const int32_t* cand, int R, int M, int n_fine, int k, float* out_sim,
+                         float* out_topv, int64_t* out_topi, void* stream) {
+  NOPE_CHECK(sim && cand && out_topv && out_topi, "null argument");
+  NOPE_CHECK(k >= 1 && k <= 64, "k must be in [1, 64]");
+  NOPE_CHECK(R >= 1 && M >= 1 && n_fine >= 1, "bad arguments");
+  pose_cells_rank_kernel<<<R, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      sim, cand, M, n_fine, k, out_sim, out_topv, reinterpret_cast<long long*>(out_topi));
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int64_t nope_topk_pack_floats(int B, int k, int n_local_max, int want_sim) {
   if (B < 1 || k < 1 || n_local_max < 0) return -1;
   const int64_t kk = ((int64_t)B * k + 1) & ~(int64_t)1;

@@ -195,6 +195,25 @@ class UNetModelPose:
             R = torch.stack([tp[b][idx[b]] for b in range(idx.shape[0])])
         return R, idx, sim
 
+    def predict_pose_coarse_to_fine(self, query_latent, ref_latent, all_relativeR_levels, hierarchy,
+                                    template_poses=None, k=5, keep=8):
+        """Latent-space form of nope_b200.model.PoseConditional.predict_pose_coarse_to_fine for this UNet:
+        -> (R | None, nearest_idx, similarity [..., N_L]) over the finest grid of `hierarchy`, -inf where the search
+        scored nothing; the query forms of predict_pose."""
+        from .hierarchy import check_search_args, search
+        from .model import multi_query_form
+        check_search_args(hierarchy, all_relativeR_levels, keep, k)
+        q, squeeze = multi_query_form(query_latent, ref_latent)
+        out = search(self, ref_latent, q, all_relativeR_levels, hierarchy, keep=keep, k=k)
+        idx, sim = out["topi"], out["sim"]
+        if squeeze:
+            idx, sim = idx[0], sim[0]
+        R = None
+        if template_poses is not None:
+            tp = template_poses[0] if template_poses.dim() == 4 else template_poses
+            R = tp.to(idx.device)[idx]
+        return R, idx, sim
+
     # ------------------------------------------------------------------ debug / parity hooks
     def debug_tap(self, ref_latent, poses, tap):
         lib = _lib.load()

@@ -156,6 +156,43 @@ class PoseConditional:
             return R, topi, sim, emb
         return R, topi, sim
 
+    @torch.no_grad()
+    def predict_pose_coarse_to_fine(self, query, reference, all_relativeR_levels, hierarchy, template_poses=None,
+                                    k=5, keep=8):
+        """predict_pose over the finest grid of a nested pose hierarchy (nope_b200.hierarchy, DESIGN.md section 9),
+        sweeping the coarsest grid and then only the finer poses around each row's best `keep`.
+        all_relativeR_levels[l] [B, N_l, 6] per level, coarsest first; hierarchy a PoseHierarchy over the same
+        levels; template_poses the finest grid's rotations, for the R lookup.
+        -> (R | None, nearest_idx, similarity [..., N_L]) in the shapes of predict_pose (the same three query
+        forms); similarity is -inf at poses the search did not score.  Every scored pose has exactly the score
+        predict_pose gives it.  One encoder call."""
+        from .hierarchy import check_search_args, search
+        if self.dist is not None:
+            raise NotImplementedError("predict_pose_coarse_to_fine does not shard across GPUs: the coarse-to-fine "
+                                      "search runs on one device (unset model.dist or use predict_pose)")
+        check_search_args(hierarchy, all_relativeR_levels, keep, k)
+        metric = getattr(self.testing_config, "similarity_metric", "l2")
+        if metric not in _METRICS:
+            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+        query, squeeze = multi_query_form(query, reference)
+        enc = self.u_net.encoder
+        self.u_net.set_metric(metric, self._occlusion_threshold())
+        B = reference.shape[0]
+        flat = query.reshape(-1, *query.shape[-3:])
+        feats = enc.encode_image(torch.cat([flat.to(self.device), reference.to(self.device)]))
+        query_feat, reference_feat = feats[:flat.shape[0]], feats[flat.shape[0]:]
+        if query.dim() != reference.dim():
+            query_feat = query_feat.view(B, query.shape[1], *feats.shape[1:])
+        out = search(self.u_net, reference_feat, query_feat, all_relativeR_levels, hierarchy, keep=keep, k=k)
+        sim, topi = out["sim"], out["topi"]
+        if squeeze:
+            sim, topi = sim[0], topi[0]
+        R = None
+        if template_poses is not None:
+            tp = template_poses[0] if template_poses.dim() == 4 else template_poses
+            R = tp.to(topi.device)[topi]
+        return R, topi, sim
+
 
     # ------------------------------------------------------------------ model.py:185-191, 268-376, 550-565
     def log(self, name, value, **kwargs):
