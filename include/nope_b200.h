@@ -201,6 +201,27 @@ int nope_pose_cells_expand(const int64_t* top_idx, int R, int keep, const int32_
 int nope_pose_cells_rank(const float* sim, const int32_t* cand, int R, int M, int n_fine, int k,
                          float* out_sim, float* out_topv, int64_t* out_topi, void* stream);
 
+/* Off-grid pose refinement (DESIGN.md section 10).  A candidate is (D, seed): D a 3x3 rotation (float32,
+ * row-major), seed an index of the grid all_relativeR [B, N, 6]; its relative rotation is D * S_seed (S_seed: rows
+ * 1-2 the grid's 6-D pose, row 3 their cross product).  Rows r = b * Q + q pair reference b with its query q.
+ * Products and sums are rounded one by one (no FMA) in a fixed order, so results are bit-reproducible.
+ * nope_pose_refine_propose: centres D [R, keep, 9] / seed [R, keep] int32 and stencil [27, 9] (rotation 0 the
+ * identity) -> M = keep * 27 candidates per row, slot c * 27 + j = (L_j * D_c, seed_c): out_D [R, M, 9],
+ * out_seed [R, M], out_rel [R, M, 9] (D * S_seed) and out_poses [R, M, 6] (its rows 1-2, the sweep's input).
+ * A centre whose seed lies outside [0, N) yields 27 padding slots: seed -1, otherwise a copy of the row's first
+ * valid candidate.  Requires 1 <= keep <= 64 and R == B * Q.
+ * nope_pose_refine_select: sim [R, M] scored at those candidates -> k entries per row, greedily: the highest
+ * score first (ties -> lowest slot), skipping padding and any candidate whose trace(rel_a rel_b^T) exceeds
+ * trace_threshold against an entry already chosen.  out_D / out_rel (optional) [R, k, 9], out_seed [R, k],
+ * out_score [R, k]; ranks with no candidate left get -inf, seed -1 and zero matrices.
+ * Requires 1 <= k <= 64, k <= M <= 64 * 27. */
+int nope_pose_refine_propose(const float* D, const int32_t* seed, int R, int keep, const float* all_relativeR,
+                             int B, int Q, int N, const float* stencil, float* out_D, int32_t* out_seed,
+                             float* out_rel, float* out_poses, void* stream);
+int nope_pose_refine_select(const float* sim, const float* cand_D, const int32_t* cand_seed, const float* cand_rel,
+                            int R, int M, int k, float trace_threshold, float* out_D, int32_t* out_seed,
+                            float* out_score, float* out_rel, void* stream);
+
 /* Multi-GPU merge (SURVEY.md 8e): each rank sweeps a contiguous slice of the pose grid and contributes
  * ONE packed record to a single all-gather:
  *   [ topv: B*k f32 | 1 pad float if B*k is odd | topi: B*k int64 (GLOBAL indices, -1 = padding) |

@@ -53,6 +53,10 @@ SIGNATURES = {
                                          C.c_int, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_void_p]),
     "nope_pose_cells_rank": (C.c_int, [c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p,
                                        c_i64p, C.c_void_p]),
+    "nope_pose_refine_propose": (C.c_int, [c_f32p, C.c_void_p, C.c_int, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int,
+                                           c_f32p, c_f32p, C.c_void_p, c_f32p, c_f32p, C.c_void_p]),
+    "nope_pose_refine_select": (C.c_int, [c_f32p, c_f32p, C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_float,
+                                          c_f32p, C.c_void_p, c_f32p, c_f32p, C.c_void_p]),
     "nope_topk_pack_floats": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "nope_topk_merge": (C.c_int, [c_f32p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                   c_f32p, c_f32p, c_i64p, C.c_void_p]),

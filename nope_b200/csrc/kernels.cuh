@@ -1143,6 +1143,143 @@ pose_cells_rank_kernel(const float* __restrict__ sim, const int* __restrict__ ca
 }
 
 // ----------------------------------------------------------------------------
+// Off-grid pose refinement (DESIGN.md section 10).  A candidate is (D, seed): D an accumulated 3x3 rotation
+// (row-major), seed a grid index; its relative rotation is D * S_seed, where S_seed has rows 1-2 from the grid's
+// 6-D pose and row 3 = row 1 x row 2.  Every product and sum is rounded on its own (__fmul_rn / __fadd_rn /
+// __fsub_rn, no FMA contraction) in the order written here, which oracle/refine_oracle.py restates op by op:
+// the kernels are bit-exact against it.  No sqrt or division: the stencil and the threshold come from the host.
+// ----------------------------------------------------------------------------
+constexpr int kRefineStencil = 27;                        // the 3x3x3 lattice, identity first
+constexpr int kRefineMaxM = 64 * kRefineStencil;          // keep <= 64 centres per row
+
+// c = a * b; c[i][j] = (a[i][0] b[0][j] + a[i][1] b[1][j]) + a[i][2] b[2][j]
+__device__ __forceinline__ void mat3_mul_rn(const float* a, const float* b, float* c) {
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+      c[i * 3 + j] = __fadd_rn(__fadd_rn(__fmul_rn(a[i * 3], b[j]), __fmul_rn(a[i * 3 + 1], b[3 + j])),
+                               __fmul_rn(a[i * 3 + 2], b[6 + j]));
+}
+
+// Propose: one CTA per row r = (reference r / Q, query r % Q).  Centre c (D [R, keep, 9], seed [R, keep]) and
+// stencil rotation j (stencil [27, 9], slot 0 the identity) give slot m = c * 27 + j: out_D = L_j * D_c,
+// out_seed, out_rel = out_D * S_seed [R, M, 9] and out_poses = its rows 1-2 [R, M, 6], M = keep * 27.  A centre
+// whose seed lies outside [0, N) yields 27 padding slots: seed -1 and a copy of the row's first valid candidate
+// (slot 0 of its first valid centre; D = I at seed 0 when the row has none), so every hypothesis of the sweep
+// is a valid rotation.
+__global__ void __launch_bounds__(256)
+pose_refine_propose_kernel(const float* __restrict__ D, const int* __restrict__ seed, int keep,
+                           const float* __restrict__ rel6, int Q, int N, const float* __restrict__ stencil,
+                           float* __restrict__ out_D, int* __restrict__ out_seed, float* __restrict__ out_rel,
+                           float* __restrict__ out_poses) {
+  const int r = blockIdx.x;
+  const int M = keep * kRefineStencil;
+  const float* Drow = D + (long long)r * keep * 9;
+  const int* srow = seed + (long long)r * keep;
+  const float* pb = rel6 + (long long)(r / Q) * N * 6;
+  int first = -1;
+  for (int c = 0; c < keep && first < 0; ++c)
+    if (srow[c] >= 0 && srow[c] < N) first = c;
+  for (int m = threadIdx.x; m < M; m += blockDim.x) {
+    int c = m / kRefineStencil, j = m - c * kRefineStencil;
+    int s = srow[c];
+    const bool valid = s >= 0 && s < N;
+    if (!valid) { c = first; j = 0; }
+    float dn[9];
+    if (c >= 0) {
+      float dc[9], l[9];
+      s = srow[c];
+#pragma unroll
+      for (int e = 0; e < 9; ++e) { dc[e] = Drow[c * 9 + e]; l[e] = stencil[j * 9 + e]; }
+      mat3_mul_rn(l, dc, dn);
+    } else {
+      s = 0;
+#pragma unroll
+      for (int e = 0; e < 9; ++e) dn[e] = (e % 4 == 0) ? 1.0f : 0.0f;
+    }
+    float S[9], rel[9];
+#pragma unroll
+    for (int e = 0; e < 6; ++e) S[e] = pb[(long long)s * 6 + e];
+    S[6] = __fsub_rn(__fmul_rn(S[1], S[5]), __fmul_rn(S[2], S[4]));
+    S[7] = __fsub_rn(__fmul_rn(S[2], S[3]), __fmul_rn(S[0], S[5]));
+    S[8] = __fsub_rn(__fmul_rn(S[0], S[4]), __fmul_rn(S[1], S[3]));
+    mat3_mul_rn(dn, S, rel);
+    const long long o = (long long)r * M + m;
+    out_seed[o] = valid ? s : -1;
+#pragma unroll
+    for (int e = 0; e < 9; ++e) { out_D[o * 9 + e] = dn[e]; out_rel[o * 9 + e] = rel[e]; }
+#pragma unroll
+    for (int e = 0; e < 6; ++e) out_poses[o * 6 + e] = rel[e];
+  }
+}
+
+// Select: one CTA per row of sim [R, M] scored at the candidates (cand_D / cand_rel [R, M, 9], cand_seed [R, M],
+// -1 = padding, never chosen).  Greedy: the highest score first, ties -> lowest slot; a candidate whose
+// trace(rel_a rel_b^T) (nine products summed in order) exceeds `thr` for an already chosen b is dropped.  Writes
+// k entries of D / rel (optional) [R, k, 9], seed [R, k] and score [R, k]; ranks with no candidate left get
+// -inf, seed -1 and zero matrices.
+__global__ void __launch_bounds__(256)
+pose_refine_select_kernel(const float* __restrict__ sim, const float* __restrict__ cand_D,
+                          const int* __restrict__ cand_seed, const float* __restrict__ cand_rel, int M, int k,
+                          float thr, float* __restrict__ out_D, int* __restrict__ out_seed,
+                          float* __restrict__ out_score, float* __restrict__ out_rel) {
+  __shared__ float s_v[8];
+  __shared__ int s_i[8];
+  __shared__ int s_pick;
+  __shared__ float s_rel[9];
+  __shared__ unsigned char s_dead[kRefineMaxM];
+  const int r = blockIdx.x;
+  const float* srow = sim + (long long)r * M;
+  const float* rrow = cand_rel + (long long)r * M * 9;
+  for (int m = threadIdx.x; m < M; m += blockDim.x) s_dead[m] = cand_seed[(long long)r * M + m] < 0;
+  __syncthreads();
+  for (int t = 0; t < k; ++t) {
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int m = threadIdx.x; m < M; m += blockDim.x) {
+      if (s_dead[m]) continue;
+      const float v = srow[m];
+      if (v > bv || (v == bv && m < bi) || bi == 0x7fffffff) { bv = v; bi = m; }
+    }
+    cta_argmax(bv, bi, s_v, s_i);
+    if (threadIdx.x == 0) s_pick = bi;
+    __syncthreads();
+    const int pick = s_pick;
+    const long long o = (long long)r * k + t;
+    if (pick == 0x7fffffff) {
+      if (threadIdx.x < 9) {
+        out_D[o * 9 + threadIdx.x] = 0.0f;
+        if (out_rel) out_rel[o * 9 + threadIdx.x] = 0.0f;
+      }
+      if (threadIdx.x == 0) { out_score[o] = -INFINITY; out_seed[o] = -1; }
+      continue;
+    }
+    const long long p = (long long)r * M + pick;
+    if (threadIdx.x < 9) {
+      s_rel[threadIdx.x] = cand_rel[p * 9 + threadIdx.x];
+      out_D[o * 9 + threadIdx.x] = cand_D[p * 9 + threadIdx.x];
+      if (out_rel) out_rel[o * 9 + threadIdx.x] = cand_rel[p * 9 + threadIdx.x];
+    }
+    if (threadIdx.x == 0) {
+      out_score[o] = bv;
+      out_seed[o] = cand_seed[p];
+      s_dead[pick] = 1;
+    }
+    __syncthreads();
+    for (int m = threadIdx.x; m < M; m += blockDim.x) {
+      if (s_dead[m]) continue;
+      const float* a = rrow + (long long)m * 9;
+      float tr = __fmul_rn(a[0], s_rel[0]);
+#pragma unroll
+      for (int e = 1; e < 9; ++e) tr = __fadd_rn(tr, __fmul_rn(a[e], s_rel[e]));
+      if (tr > thr) s_dead[m] = 1;
+    }
+    __syncthreads();
+  }
+}
+
+// ----------------------------------------------------------------------------
 // Multi-GPU merge (SURVEY.md 8e): every rank contributes ONE packed record to a single all-gather,
 //   [ topv: B*k f32 | pad to even | topi: B*k i64 | sim slice: B*n_local f32 (optional) ]      (`pack` floats)
 // with GLOBAL pose indices (idx -1 = padding).  This kernel turns the W gathered records into the

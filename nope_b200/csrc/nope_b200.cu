@@ -1410,6 +1410,33 @@ int nope_pose_cells_rank(const float* sim, const int32_t* cand, int R, int M, in
   return 0;
 }
 
+int nope_pose_refine_propose(const float* D, const int32_t* seed, int R, int keep, const float* all_relativeR, int B,
+                             int Q, int N, const float* stencil, float* out_D, int32_t* out_seed, float* out_rel,
+                             float* out_poses, void* stream) {
+  NOPE_CHECK(D && seed && all_relativeR && stencil && out_D && out_seed && out_rel && out_poses, "null argument");
+  NOPE_CHECK(keep >= 1 && keep <= 64, "keep must be in [1, 64]");
+  NOPE_CHECK(B >= 1 && Q >= 1 && N >= 1, "bad arguments");
+  NOPE_CHECK(R >= 1 && (int64_t)B * Q == R, "R (rows) must equal B * Q");
+  pose_refine_propose_kernel<<<R, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      D, seed, keep, all_relativeR, Q, N, stencil, out_D, out_seed, out_rel, out_poses);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int nope_pose_refine_select(const float* sim, const float* cand_D, const int32_t* cand_seed, const float* cand_rel,
+                            int R, int M, int k, float trace_threshold, float* out_D, int32_t* out_seed,
+                            float* out_score, float* out_rel, void* stream) {
+  NOPE_CHECK(sim && cand_D && cand_seed && cand_rel && out_D && out_seed && out_score, "null argument");
+  NOPE_CHECK(k >= 1 && k <= 64, "k must be in [1, 64]");
+  NOPE_CHECK(M >= 1 && M <= kRefineMaxM, "M (candidates per row) must be in [1, 64 * 27]");
+  NOPE_CHECK(k <= M, "k must not exceed M (candidates per row)");
+  NOPE_CHECK(R >= 1, "bad arguments");
+  pose_refine_select_kernel<<<R, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      sim, cand_D, cand_seed, cand_rel, M, k, trace_threshold, out_D, out_seed, out_score, out_rel);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int64_t nope_topk_pack_floats(int B, int k, int n_local_max, int want_sim) {
   if (B < 1 || k < 1 || n_local_max < 0) return -1;
   const int64_t kk = ((int64_t)B * k + 1) & ~(int64_t)1;

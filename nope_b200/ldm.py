@@ -214,6 +214,21 @@ class UNetModelPose:
             R = tp.to(idx.device)[idx]
         return R, idx, sim
 
+    def predict_pose_refined(self, query_latent, ref_latent, all_relativeR, refiner, k=5, keep=2):
+        """Latent-space form of nope_b200.model.PoseConditional.predict_pose_refined for this UNet:
+        -> (R [..., k, 3, 3] = D * template_poses[seed], seed_idx [..., k], score [..., k]); the query forms of
+        predict_pose."""
+        from .model import multi_query_form
+        from .refine import check_refine_args, refine, template_rotations
+        check_refine_args(refiner, all_relativeR, keep, k, ref_latent.shape[0])
+        q, squeeze = multi_query_form(query_latent, ref_latent)
+        seeds = self.sweep(ref_latent, all_relativeR, q, want_emb=False, want_sim=False, k=keep)["topi"]
+        out = refine(self, ref_latent, q, all_relativeR, seeds, refiner, k=k)
+        D, seed, score = out["D"], out["seed"], out["score"]
+        if squeeze:
+            D, seed, score = D[0], seed[0], score[0]
+        return template_rotations(D, seed, refiner), seed, score
+
     # ------------------------------------------------------------------ debug / parity hooks
     def debug_tap(self, ref_latent, poses, tap):
         lib = _lib.load()

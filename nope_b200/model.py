@@ -193,6 +193,40 @@ class PoseConditional:
             R = tp.to(topi.device)[topi]
         return R, topi, sim
 
+    @torch.no_grad()
+    def predict_pose_refined(self, query, reference, all_relativeR, refiner, k=5, keep=2):
+        """Poses between the grid poses (nope_b200.refine, DESIGN.md section 10): the exhaustive sweep of
+        all_relativeR [B, N, 6] seeds each (reference, query) row with its best `keep` grid poses, and the
+        refiner's steps search shrinking rotation lattices around them.  refiner: a PoseRefiner over the same grid.
+        -> (R [..., k, 3, 3] = D * template_poses[seed] (float64), seed_idx [..., k], score [..., k]) in the query
+        forms of predict_pose; descending score, each exactly the score a sweep of that pose gives.  One encoder
+        call.  keep = 2 by default: keep = 4 measured hardly more accurate for up to 1.8x the time (DESIGN.md
+        section 6)."""
+        from .refine import check_refine_args, refine, template_rotations
+        if self.dist is not None:
+            raise NotImplementedError("predict_pose_refined does not shard across GPUs: the refinement runs on one "
+                                      "device (unset model.dist or use predict_pose)")
+        check_refine_args(refiner, all_relativeR, keep, k, reference.shape[0])
+        metric = getattr(self.testing_config, "similarity_metric", "l2")
+        if metric not in _METRICS:
+            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+        query, squeeze = multi_query_form(query, reference)
+        enc = self.u_net.encoder
+        self.u_net.set_metric(metric, self._occlusion_threshold())
+        B = reference.shape[0]
+        flat = query.reshape(-1, *query.shape[-3:])
+        feats = enc.encode_image(torch.cat([flat.to(self.device), reference.to(self.device)]))
+        query_feat, reference_feat = feats[:flat.shape[0]], feats[flat.shape[0]:]
+        if query.dim() != reference.dim():
+            query_feat = query_feat.view(B, query.shape[1], *feats.shape[1:])
+        seeds = self.u_net.sweep(reference_feat, all_relativeR, query_feat=query_feat, want_emb=False,
+                                 want_sim=False, k=keep)["topi"]
+        out = refine(self.u_net, reference_feat, query_feat, all_relativeR, seeds, refiner, k=k)
+        D, seed, score = out["D"], out["seed"], out["score"]
+        if squeeze:
+            D, seed, score = D[0], seed[0], score[0]
+        return template_rotations(D, seed, refiner), seed, score
+
 
     # ------------------------------------------------------------------ model.py:185-191, 268-376, 550-565
     def log(self, name, value, **kwargs):

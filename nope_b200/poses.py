@@ -52,6 +52,12 @@ def icosphere_object_rotations(level, upper_only=False):
     pts = _icosphere(level)
     if upper_only:
         pts = pts[pts[:, 2] >= 0]
+    return viewpoint_rotations(pts)
+
+
+def viewpoint_rotations(pts):
+    """Object rotations whose camera sits at each point pts [N, 3] looking at the origin, built as the icosphere
+    grids are (the same up-vector rule).  [N,3,3] float64."""
     Rs = []
     for p in pts:
         z = p / np.linalg.norm(p)
