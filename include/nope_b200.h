@@ -165,6 +165,21 @@ int nope_encoder_finalize(nope_encoder_t* e);
 int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* out, void* stream);
 int64_t nope_encoder_last_launch_count(const nope_encoder_t* e);
 
+/* In-plane rotation search (DESIGN.md section 11).  cossin [A, 2] fp32 holds (cos, sin) of the angles
+ * alpha_a = a * 360 / A.  Rotated copy a of an image is I_a(x, y) = I(c + R2(alpha_a) ((x, y) - c)) in pixel-index
+ * coordinates (x right, y down), c = ((W - 1) / 2, (H - 1) / 2), R2 = [[cos, -sin], [sin, cos]], bilinear, taps
+ * outside the image read -1.  Products and sums are rounded one by one (no FMA) in a fixed order.  A match of copy a
+ * with a template of pose T means the query pose Rz(alpha_a) T.  Both calls require B >= 1 and 1 <= A <= 360 and
+ * refuse before any CUDA call.
+ * nope_inplane_rotate: images [B, 3, H, W] fp32 (device) -> out [B, A, 3, H, W] fp32 (device); H, W >= 1.
+ * nope_encoder_encode_inplane: images [B, 3, 256, 256] -> out [B, A, D, 32, 32], equal to nope_encoder_encode of
+ * the rotated batch [B * A, 3, 256, 256] without forming it: the (image, angle) pairs go 32 at a time through a
+ * staging buffer the engine allocates on its first call (25 MB). */
+int nope_inplane_rotate(const float* images, int B, int H, int W, const float* cossin, int A, float* out,
+                        void* stream);
+int nope_encoder_encode_inplane(nope_encoder_t* e, const float* images, int B, const float* cossin, int A,
+                                float* out, void* stream);
+
 /* Score materialised templates against a query and rank them: the arithmetic of
  * PoseConditional.retrieval (model.py:254-266) after encode_image.
  *   query_feat [B, C, HW] fp32, emb [B, N, C, HW] fp32 -> sim [B, N], topv/topi [B, k]. */

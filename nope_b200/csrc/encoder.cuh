@@ -57,6 +57,49 @@ enc_stem_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
   out_lo[pix * 64 + o] = __float2half_rn(acc - __half2float(hi));
 }
 
+// In-plane rotation of the query crops (DESIGN.md section 11): rotated copy a of image b is
+// I_a(x, y) = I(c + R2(alpha_a) ((x, y) - c)), c = ((W - 1) / 2, (H - 1) / 2), R2 = [[cos, -sin], [sin, cos]],
+// bilinear, taps outside the image read -1 (black in the model's [-1, 1] range).  One thread per output pixel
+// (all three channels); grid (ceil(H * W / 256), pairs): blockIdx.y is the pair p = pair0 + blockIdx.y = b * A + a,
+// and out is pair-major from pair0: [pairs, 3, H, W].  32-bit index arithmetic (H * W and B * A fit an int), so
+// no 64-bit division routine is called.  Every product and sum is rounded on its own, in the order
+// oracle/inplane_oracle.py restates: source coordinates, floor, fractions, the two row lerps, the column lerp.  At
+// quarter turns of a square image the fractions are 0 and the copy is an exact permutation.
+__global__ void __launch_bounds__(256)
+inplane_rotate_kernel(const float* __restrict__ img, const float* __restrict__ cossin, int A, int H, int W, int pair0,
+                      float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int hw_i = H * W;
+  if (i >= hw_i) return;
+  const long long hw = hw_i;
+  const int x = i % W, y = i / W;
+  const int p = pair0 + (int)blockIdx.y;
+  const int a = p % A, b = p / A;
+  const float c = cossin[2 * a], s = cossin[2 * a + 1];
+  const float cx = __fmul_rn((float)(W - 1), 0.5f), cy = __fmul_rn((float)(H - 1), 0.5f);
+  const float dx = __fsub_rn((float)x, cx), dy = __fsub_rn((float)y, cy);
+  const float sx = __fadd_rn(__fsub_rn(__fmul_rn(c, dx), __fmul_rn(s, dy)), cx);
+  const float sy = __fadd_rn(__fadd_rn(__fmul_rn(s, dx), __fmul_rn(c, dy)), cy);
+  const float x0 = floorf(sx), y0 = floorf(sy);
+  const float fx = __fsub_rn(sx, x0), fy = __fsub_rn(sy, y0);
+  const int ix = (int)x0, iy = (int)y0;
+  const bool in_x0 = ix >= 0 && ix < W, in_x1 = ix + 1 >= 0 && ix + 1 < W;
+  const bool in_y0 = iy >= 0 && iy < H, in_y1 = iy + 1 >= 0 && iy + 1 < H;
+  const float* src = img + (long long)b * 3 * hw;
+  float* dst = out + (long long)blockIdx.y * 3 * hw + i;
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) {
+    const float* plane = src + ch * hw;
+    const float v00 = in_y0 && in_x0 ? plane[(long long)iy * W + ix] : -1.f;
+    const float v01 = in_y0 && in_x1 ? plane[(long long)iy * W + ix + 1] : -1.f;
+    const float v10 = in_y1 && in_x0 ? plane[(long long)(iy + 1) * W + ix] : -1.f;
+    const float v11 = in_y1 && in_x1 ? plane[(long long)(iy + 1) * W + ix + 1] : -1.f;
+    const float top = __fadd_rn(v00, __fmul_rn(fx, __fsub_rn(v01, v00)));
+    const float bot = __fadd_rn(v10, __fmul_rn(fx, __fsub_rn(v11, v10)));
+    dst[ch * hw] = __fadd_rn(top, __fmul_rn(fy, __fsub_rn(bot, top)));
+  }
+}
+
 // [n_pix][ld] fp32 (first D columns valid) -> NCHW fp32 [B, D, hw]
 __global__ void enc_extract_kernel(const float* __restrict__ x, float* __restrict__ out, int B, int D,
                                    int hw, int ld) {
@@ -96,10 +139,13 @@ struct nope_encoder {
   std::vector<void*> ws_owned;
   std::map<std::tuple<const void*, int, int, int, int>, CUtensorMap> tmaps;
   int64_t launches = 0;
+  static constexpr int kChunk = 32;   // images per encode() call: the workspace holds this many
+  float* rot_stage = nullptr;         // kChunk rotated 256x256 crops (25 MB), allocated by the first encode_inplane
 
   ~nope_encoder() {
     for (void* p : owned) cudaFree(p);
     for (void* p : ws_owned) cudaFree(p);
+    if (rot_stage) cudaFree(rot_stage);
   }
 
   // ---------------------------------------------------------------- schema (resnet.py:93-133)
@@ -375,6 +421,29 @@ struct nope_encoder {
                                                                           convs.at("projector.3").cout);
     NOPE_CUDA(cudaGetLastError());
     ++launches;
+    return 0;
+  }
+
+  // images [B, 3, 256, 256] x angles cossin [A, 2] -> out [B, A, D, 32, 32]: the (image, angle) pairs in b-major
+  // order, kChunk at a time, each chunk rotated into rot_stage and encoded from there, so the [B, A, 3, 256, 256]
+  // rotated batch never exists.  The chunks are those nope_encoder_encode makes of that batch.
+  int encode_inplane(const float* images, int B, const float* cossin, int A, float* out, cudaStream_t st) {
+    using namespace nope;
+    constexpr long long kImg = 3LL * 256 * 256;
+    if (!rot_stage) {
+      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&rot_stage), kChunk * kImg * sizeof(float)));
+    }
+    NOPE_CHECK((int64_t)B * A <= INT32_MAX, "too many (image, angle) pairs");
+    const int pairs = B * A;
+    int64_t total = 0;
+    for (int lo = 0; lo < pairs; lo += kChunk) {
+      const int n = pairs - lo < kChunk ? pairs - lo : kChunk;
+      inplane_rotate_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, cossin, A, 256, 256, lo, rot_stage);
+      NOPE_CUDA(cudaGetLastError());
+      if (encode(rot_stage, n, out + (size_t)lo * D * 32 * 32, st)) return -1;
+      total += launches + 1;
+    }
+    launches = total;
     return 0;
   }
 };

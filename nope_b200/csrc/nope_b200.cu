@@ -1513,7 +1513,7 @@ int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* ou
   NOPE_CHECK(B >= 1, "B must be >= 1");
   NOPE_CUDA(cudaSetDevice(e->device));
   // The workspace is sized by the largest chunk (~80 MB per image): any B goes through, 32 images at a time.
-  constexpr int kChunk = 32;
+  constexpr int kChunk = nope_encoder::kChunk;
   int64_t launches = 0;
   for (int lo = 0; lo < B; lo += kChunk) {
     const int n = B - lo < kChunk ? B - lo : kChunk;
@@ -1523,6 +1523,34 @@ int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* ou
     launches += e->launches;
   }
   e->launches = launches;
+  return 0;
+}
+
+int nope_encoder_encode_inplane(nope_encoder_t* e, const float* images, int B, const float* cossin, int A, float* out,
+                                void* stream) {
+  NOPE_CHECK(images && cossin && out, "null images / cossin / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(A >= 1 && A <= 360, "A (in-plane angles) must be in [1, 360]");
+  NOPE_CHECK(e && e->finalized, "encoder not finalized");
+  NOPE_CUDA(cudaSetDevice(e->device));
+  return e->encode_inplane(images, B, cossin, A, out, static_cast<cudaStream_t>(stream));
+}
+
+int nope_inplane_rotate(const float* images, int B, int H, int W, const float* cossin, int A, float* out,
+                        void* stream) {
+  NOPE_CHECK(images && cossin && out, "null images / cossin / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(H >= 1 && W >= 1, "H and W must be >= 1");
+  NOPE_CHECK(A >= 1 && A <= 360, "A (in-plane angles) must be in [1, 360]");
+  NOPE_CHECK((int64_t)H * W <= INT32_MAX - 255 && (int64_t)B * A <= INT32_MAX, "images too large or too many");
+  const int pairs = B * A, hw = H * W;
+  constexpr int kMaxGridY = 65535;
+  for (int lo = 0; lo < pairs; lo += kMaxGridY) {
+    const int n = pairs - lo < kMaxGridY ? pairs - lo : kMaxGridY;
+    inplane_rotate_kernel<<<dim3((hw + 255) / 256, n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        images, cossin, A, H, W, lo, out + (size_t)lo * 3 * hw);
+    NOPE_CUDA(cudaGetLastError());
+  }
   return 0;
 }
 

@@ -162,3 +162,24 @@ class FeatureExtractor(nn.Module):
         if self.normalize:
             feat = F.normalize(feat, dim=1)
         return feat.float()
+
+    @torch.no_grad()
+    def encode_image_inplane(self, image, A):
+        """image [B,3,256,256] -> [B,A,D,32,32]: the latents of the A in-plane rotated copies of every image
+        (nope_b200.inplane, DESIGN.md section 11), equal to encode_image of inplane.rotate_images(image, A) flattened
+        to [B*A, ...], without forming that batch.  Native engine only: the torch backend raises NopeError."""
+        from .inplane import _on_device, check_angles, inplane_table
+        A = check_angles(A)
+        p = next(self.parameters())
+        if not self._use_native(p.device):
+            raise _lib.NopeError("encode_image_inplane needs the native engine on a CUDA device "
+                                 "(no torch-backend path)")
+        if image.dim() != 4 or tuple(image.shape[1:]) != (3, 256, 256):
+            raise _lib.NopeError("the native encoder is built for [B, 3, 256, 256] inputs")
+        x = image.to(device=p.device, dtype=torch.float32).contiguous()
+        out = torch.empty((x.shape[0], A, self.latent_dim, 32, 32), device=p.device, dtype=torch.float32)
+        with torch.cuda.device(p.device):
+            _lib.check(_lib.load().nope_encoder_encode_inplane(
+                self._engine(p.device), _lib.ptr(x), x.shape[0], _lib.ptr(_on_device(inplane_table, A, p.device)),
+                A, _lib.ptr(out), C.c_void_p(torch.cuda.current_stream(p.device).cuda_stream)))
+        return F.normalize(out, dim=2) if self.normalize else out

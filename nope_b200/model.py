@@ -227,6 +227,78 @@ class PoseConditional:
             D, seed, score = D[0], seed[0], score[0]
         return template_rotations(D, seed, refiner), seed, score
 
+    @torch.no_grad()
+    def predict_pose_inplane(self, query, reference, all_relativeR, template_poses=None, k=5, angles=36):
+        """predict_pose over pose x in-plane angle (nope_b200.inplane, DESIGN.md section 11): every query crop is
+        rotated by the A = `angles` angles a * 360 / A and each rotated copy is scored against the same templates.
+        -> (R [..., k, 3, 3] = Rz(alpha[angle_idx]) template_poses[nearest_idx] (float64) | None, nearest_idx [..., k],
+        angle_idx [..., k], similarity [..., A, N]) in the query forms of predict_pose; the top-k runs jointly over
+        (angle, pose), ties -> the lowest a * N + n.  One encoder call for the references, one encode_image_inplane
+        call for the queries, one sweep with Q * A query rows per reference.  angles = 1 is predict_pose."""
+        from .inplane import check_inplane_args, compose
+        if self.dist is not None:
+            raise NotImplementedError("predict_pose_inplane does not shard across GPUs: the in-plane search runs on "
+                                      "one device (unset model.dist or use predict_pose)")
+        if all_relativeR.dim() != 3 or all_relativeR.shape[0] != reference.shape[0] or all_relativeR.shape[2] != 6:
+            raise ValueError(f"all_relativeR [B, N, 6] with B = {reference.shape[0]} references expected, got "
+                             f"{tuple(all_relativeR.shape)}")
+        N = all_relativeR.shape[1]
+        A, k = check_inplane_args(angles, k, N)
+        metric = getattr(self.testing_config, "similarity_metric", "l2")
+        if metric not in _METRICS:
+            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+        query, squeeze = multi_query_form(query, reference)
+        B = reference.shape[0]
+        Q = 1 if query.dim() == reference.dim() else query.shape[1]
+        lead = (Q,) if squeeze else (B,) if query.dim() == reference.dim() else (B, Q)
+        enc = self.u_net.encoder
+        self.u_net.set_metric(metric, self._occlusion_threshold())
+        reference_feat = enc.encode_image(reference.to(self.device))
+        query_feat = enc.encode_image_inplane(query.reshape(B * Q, *query.shape[-3:]).to(self.device), A)
+        query_feat = query_feat.view(B, Q * A, *query_feat.shape[2:])
+        sim = self.u_net.sweep(reference_feat, all_relativeR, query_feat=query_feat, want_emb=False,
+                               want_sim=True, k=0)["sim"]                                  # [B, Q * A, N]
+        _, flat = topk(sim.view(B * Q, A * N), k)
+        nearest, angle = flat % N, flat // N
+        sim, nearest, angle = sim.view(lead + (A, N)), nearest.view(lead + (k,)), angle.view(lead + (k,))
+        R = compose(template_poses, nearest, angle, A) if template_poses is not None else None
+        return R, nearest, angle, sim
+
+    @torch.no_grad()
+    def retrieval_inplane(self, query, template_feat, k=5, angles=36):
+        """retrieval over pose x in-plane angle, for templates generated once and queries streamed: the A = `angles`
+        rotated copies of every query image [Bq, 3, 256, 256] against template_feat [Bt, N, C, h, w], batches
+        broadcast as in retrieval.  -> (similarity [rows, A, N], nearest_idx [rows, k], angle_idx [rows, k]); the
+        top-k runs jointly over (angle, pose), ties -> the lowest a * N + n."""
+        from .inplane import check_inplane_args
+        if query.dim() != 4 or template_feat.dim() != 5:
+            raise ValueError(f"query [B, 3, H, W] and template_feat [B, N, C, h, w] expected; got "
+                             f"{tuple(query.shape)} and {tuple(template_feat.shape)}")
+        enc = self.u_net.encoder
+        if template_feat.shape[2:] != (enc.latent_dim, 32, 32):
+            raise ValueError(f"template_feat [B, N, {enc.latent_dim}, 32, 32] expected, got "
+                             f"{tuple(template_feat.shape)}")
+        N = template_feat.shape[1]
+        A, k = check_inplane_args(angles, k, N)
+        metric = getattr(self.testing_config, "similarity_metric", "l2")
+        if metric not in _METRICS:
+            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+        B, Q, Bt, rows = broadcast_batches(query.shape[0], template_feat.shape[0])
+        dev = template_feat.device
+        if dev.type != "cuda":
+            raise _lib.NopeError("retrieval_inplane needs CUDA tensors (no CPU fallback)")
+        q = enc.encode_image_inplane(query.to(dev), A)                                     # [Bq, A, C, h, w]
+        q = q.reshape(-1, Q * A, *q.shape[2:]).expand(B, Q * A, *q.shape[2:]).contiguous()
+        t = template_feat.to(torch.float32).contiguous()
+        sim = torch.empty((rows, A, N), device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.load().nope_score_topk_multi(
+                _lib.ptr(q), _lib.ptr(t), B, Q * A, Bt, N, t.shape[2], t.shape[3] * t.shape[4], _METRICS[metric],
+                self._occlusion_threshold(), 0, _lib.ptr(sim), None, None, 0,
+                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        _, flat = topk(sim.view(rows, A * N), k)
+        return sim, flat % N, flat // N
+
 
     # ------------------------------------------------------------------ model.py:185-191, 268-376, 550-565
     def log(self, name, value, **kwargs):
