@@ -180,6 +180,27 @@ int nope_inplane_rotate(const float* images, int B, int H, int W, const float* c
 int nope_encoder_encode_inplane(nope_encoder_t* e, const float* images, int B, const float* cossin, int A,
                                 float* out, void* stream);
 
+/* T-LESS evaluation (DESIGN.md section 12): a depth rasterizer standing in for pyrender's DEPTH_ONLY render and the
+ * VSD error of src/poses/vsd.py:92-135 (visibility mode "bop19", src/poses/vsd_utils.py).  Both calls refuse bad
+ * arguments before any CUDA call and do not synchronise.
+ * nope_render_depth: vertices [V, 3] fp32 (model frame, mm), faces [F, 3] int32, poses [P, 4, 4] fp32 row-major (model
+ * -> OpenCV camera, mm) -> out [P, H, W] fp32 camera-Z depth, 0 where nothing is hit.  Pixel (r, c) samples the image
+ * point (c + 1/2, r + 1/2), u = fx X / Z + cx, v = fy Y / Z + cy.  Coverage is exact (8 sub-pixel bits, int64 edge
+ * functions, top-left rule, no culling); the output does not depend on face order or winding.  Faces with an index
+ * outside [0, V), a vertex at Z < znear or a projected coordinate beyond 2^20 px are skipped, as are degenerate ones.
+ * Requires V, F >= 1, 1 <= P <= 65535, 1 <= H, W <= 8192, znear > 0.
+ * nope_vsd_error: depth_test [F, H, W] fp64 (the sensor depth, mm), depth_gt [F, H, W] fp32 (the model rendered at the
+ * ground-truth pose), depth_est [F, P, H, W] fp32 (at P estimated poses), K [F, 4] fp64 (fx, fy, cx, cy) -> out [F, P]
+ * fp64, (cost + |union| - |inter|) / |union|, 1 where the union is empty.  delta (visibility tolerance, compared in
+ * fp32 as numpy compares a float32 array with a Python number) >= 0; tau (misalignment tolerance) > 0; cost_type
+ * NOPE_VSD_STEP or NOPE_VSD_TLINEAR.  Requires 1 <= F, P <= 65535, 1 <= H, W <= 8192. */
+#define NOPE_VSD_STEP 0      /* cost 1 where |dist_gt - dist_est| >= tau */
+#define NOPE_VSD_TLINEAR 1   /* cost min(|dist_gt - dist_est| / tau, 1) */
+int nope_render_depth(const float* vertices, int V, const int32_t* faces, int F, const float* poses, int P, float fx,
+                      float fy, float cx, float cy, float znear, int H, int W, float* out, void* stream);
+int nope_vsd_error(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H, int W,
+                   const double* K, double delta, double tau, int cost_type, double* out, void* stream);
+
 /* Score materialised templates against a query and rank them: the arithmetic of
  * PoseConditional.retrieval (model.py:254-266) after encode_image.
  *   query_feat [B, C, HW] fp32, emb [B, N, C, HW] fp32 -> sim [B, N], topv/topi [B, k]. */

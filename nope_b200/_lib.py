@@ -44,6 +44,10 @@ SIGNATURES = {
     "nope_encoder_last_launch_count": (C.c_int64, [C.c_void_p]),
     "nope_inplane_rotate": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, c_f32p, C.c_void_p]),
     "nope_encoder_encode_inplane": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, C.c_void_p]),
+    "nope_render_depth": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_int, C.c_float, C.c_float,
+                                    C.c_float, C.c_float, C.c_float, C.c_int, C.c_int, c_f32p, C.c_void_p]),
+    "nope_vsd_error": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                 C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p]),
     "nope_score_topk": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                   C.c_int, c_f32p, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_score_topk_multi": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,

@@ -23,6 +23,7 @@
 #include "linattn_tc.cuh"
 #include "encoder.cuh"
 #include "ldm.cuh"
+#include "render.cuh"
 
 using namespace nope;
 
@@ -1555,6 +1556,48 @@ int nope_inplane_rotate(const float* images, int B, int H, int W, const float* c
 }
 
 int64_t nope_encoder_last_launch_count(const nope_encoder_t* e) { return e ? e->launches : 0; }
+
+// ---------------------------------------------------------------------------------
+// T-LESS evaluation: depth rasterizer and VSD (render.cuh, DESIGN.md section 12)
+// ---------------------------------------------------------------------------------
+int nope_render_depth(const float* vertices, int V, const int32_t* faces, int F, const float* poses, int P, float fx,
+                      float fy, float cx, float cy, float znear, int H, int W, float* out, void* stream) {
+  NOPE_CHECK(vertices && faces && poses && out, "null argument");
+  NOPE_CHECK(V >= 1 && F >= 1 && P >= 1, "V, F and P must be >= 1");
+  NOPE_CHECK(P <= 65535, "P must be <= 65535");
+  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
+  NOPE_CHECK(znear > 0.f, "znear must be > 0");
+  NOPE_CHECK(std::isfinite(fx) && std::isfinite(fy) && std::isfinite(cx) && std::isfinite(cy) && std::isfinite(znear),
+             "intrinsics and znear must be finite");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  unsigned* z = reinterpret_cast<unsigned*>(out);
+  const long long n = (long long)P * H * W;
+  const int fill_blocks = (int)std::min<long long>((n + 255) / 256, 132LL * 16);
+  depth_fill_kernel<<<fill_blocks, 256, 0, st>>>(z, n);
+  NOPE_CUDA(cudaGetLastError());
+  depth_raster_kernel<<<dim3((F + 7) / 8, P), 256, 0, st>>>(vertices, V, faces, F, poses, fx, fy, cx, cy, znear, H, W,
+                                                            z);
+  NOPE_CUDA(cudaGetLastError());
+  depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, n);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int nope_vsd_error(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H, int W,
+                   const double* K, double delta, double tau, int cost_type, double* out, void* stream) {
+  NOPE_CHECK(depth_test && depth_gt && depth_est && K && out, "null argument");
+  NOPE_CHECK(F >= 1 && P >= 1, "F and P must be >= 1");
+  NOPE_CHECK(F <= 65535 && P <= 65535, "F and P must be <= 65535");
+  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
+  NOPE_CHECK(cost_type == NOPE_VSD_STEP || cost_type == NOPE_VSD_TLINEAR, "unknown cost_type (0 step, 1 tlinear)");
+  NOPE_CHECK(delta >= 0.0 && std::isfinite(delta), "delta must be finite and >= 0");
+  NOPE_CHECK(tau > 0.0 && std::isfinite(tau), "tau must be finite and > 0");
+  // the visibility test compares float32 differences with delta in float32, as numpy does with a Python number
+  vsd_kernel<<<dim3(kVsdCluster * P, F), kVsdThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      depth_test, depth_gt, depth_est, P, H, W, K, (float)delta, tau, cost_type, out);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
 
 // ---------------------------------------------------------------------------------
 // per-op entry points

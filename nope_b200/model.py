@@ -1,8 +1,9 @@
 """Host-side mirror of the reference task module `PoseConditional`
 (src/model/model.py:32-565), inference surface only: forward (loss), sample,
 generate_templates, retrieval, plus predict_pose (= eval_geodesic lines 313-357 without
-logging, SURVEY.md F2).  Training, VSD evaluation, wandb/video logging are out of scope
-(SURVEY.md section 8).
+logging, SURVEY.md F2) and the T-LESS VSD evaluation (eval_vsd, model.py:378-541, on the
+CUDA rasterizer and VSD kernels of nope_b200.vsd).  Training and wandb/video logging are out
+of scope (SURVEY.md section 8).
 
 Differences that are deliberate and documented:
   * generate_templates batches the whole pose grid through one engine sweep instead of a
@@ -12,6 +13,7 @@ Differences that are deliberate and documented:
   * ranking is deterministic: descending score, ties -> lowest index.
 """
 import ctypes as C
+import os
 import types
 
 import torch
@@ -41,6 +43,9 @@ class PoseConditional:
         self.metric = GeodesicError()              # model.py:56
         self.logged = {}                           # what Lightning's self.log would have received
         self.global_step, self.global_rank = 0, 0
+        # model.py:66: per-batch VSD errors go to <save_dir>/predictions (created on first save)
+        self.log_dir = None if save_dir is None else os.path.join(save_dir, "predictions")
+        self.tless_cad = {}                        # obj_id -> nope_b200.vsd.Mesh (load_mesh)
 
     @property
     def device(self):
@@ -332,14 +337,113 @@ class PoseConditional:
                      nearest_idx=nearest_idx.cpu().numpy())
         return error, nearest_idx, similarity
 
+    # ------------------------------------------------------------------ model.py:378-541 (T-LESS, DESIGN.md section 12)
+    def load_mesh(self, cad_dir, obj_ids=range(1, 31)):
+        """model.py:378-389: the T-LESS CAD models obj_{id:06d}.ply of `cad_dir` (ids 1 ... 30) as device meshes in
+        self.tless_cad."""
+        from .vsd import Mesh
+        for obj_id in obj_ids:
+            self.tless_cad[int(obj_id)] = Mesh.from_ply(os.path.join(cad_dir, f"obj_{int(obj_id):06d}.ply"),
+                                                        device=self.device)
+        return self
+
+    _VSD_KEYS = ("query", "reference", "gt_relativeR", "all_relativeR", "template_poses", "query_pose",
+                 "query_translation", "intrinsic", "depth_path", "obj_id")
+
+    def _check_vsd_batch(self, batch):
+        for key in self._VSD_KEYS:
+            if key not in batch:
+                raise KeyError(f"eval_vsd: the batch has no {key!r}")
+        B = batch["query"].shape[0]
+        tp, qp, qt, K = batch["template_poses"], batch["query_pose"], batch["query_translation"], batch["intrinsic"]
+        ar = batch["all_relativeR"]
+        if batch["query"].dim() != 4 or tuple(batch["reference"].shape) != tuple(batch["query"].shape) or B < 1:
+            raise ValueError(f"eval_vsd: query and reference [B, 3, H, W] expected, got "
+                             f"{tuple(batch['query'].shape)} and {tuple(batch['reference'].shape)}")
+        if tp.dim() != 4 or tp.shape[0] != B or tuple(tp.shape[2:]) != (3, 3) or ar.dim() != 3 or ar.shape[0] != B \
+                or ar.shape[1] != tp.shape[1]:
+            raise ValueError(f"eval_vsd: template_poses [B, N, 3, 3] and all_relativeR [B, N, 6] with B = {B} expected, "
+                             f"got {tuple(tp.shape)} and {tuple(ar.shape)}")
+        if tuple(qp.shape) != (B, 3, 3) or tuple(qt.shape) != (B, 3, 1):
+            raise ValueError(f"eval_vsd: query_pose [B, 3, 3] and query_translation [B, 3, 1] expected, got "
+                             f"{tuple(qp.shape)} and {tuple(qt.shape)}")
+        if K.numel() != B * 9:
+            raise ValueError(f"eval_vsd: intrinsic [B, 3, 3] expected, got {tuple(K.shape)}")
+        if len(batch["depth_path"]) != B or batch["obj_id"].numel() != B:
+            raise ValueError(f"eval_vsd: {B} depth_path entries and obj_id values expected, got "
+                             f"{len(batch['depth_path'])} and {batch['obj_id'].numel()}")
+        ids = [int(i) for i in batch["obj_id"].reshape(-1).tolist()]
+        missing = sorted(set(i for i in ids if i not in self.tless_cad))
+        if missing:
+            raise ValueError(f"eval_vsd: no mesh loaded for obj_id {missing} (load_mesh)")
+        return B, ids
+
+    @torch.no_grad()
+    def eval_vsd(self, batch, data_name, save_path=None):
+        """`eval_vsd` of the reference (model.py:391-541) without wandb and images: the validation loss under the
+        ground-truth pose, the top-5 template retrieval, and the VSD errors of the retrieved rotations at the
+        ground-truth translation (delta 15, tau 20, "step": vsd_obj's defaults), rendered and scored on the GPU.
+        Returns and logs the reference's final_scores; saves the top-1 errors to save_path (.npy) when given."""
+        import numpy as np
+        from . import vsd as _vsd
+        B, ids = self._check_vsd_batch(batch)
+        query, reference = batch["query"], batch["reference"]
+        loss = self.forward(query=query, relativeR=batch["gt_relativeR"], reference=reference)
+        self.log(f"loss/val_{data_name}", loss)
+        _, nearest_idx, _ = self.predict_pose(query, reference, batch["all_relativeR"], None, k=5)
+        dev = nearest_idx.device
+        # model.py:469-509: predicted rotations with the ground-truth translation, and the ground-truth pose
+        tp = batch["template_poses"].to(dev, torch.float32)
+        k = nearest_idx.shape[1]
+        R = tp[torch.arange(B, device=dev)[:, None].expand(B, k), nearest_idx]                 # [B, k, 3, 3]
+        t = batch["query_translation"].to(dev, torch.float32)                                  # [B, 3, 1]
+        poses = torch.zeros((B, 1 + k, 4, 4), device=dev, dtype=torch.float32)
+        poses[:, 0, :3, :3] = batch["query_pose"].to(dev, torch.float32)
+        poses[:, 1:, :3, :3] = R
+        poses[:, :, :3, 3] = t[:, None, :, 0]
+        poses[:, :, 3, 3] = 1.0
+        # vsd.py:72-74: the intrinsics and the sensor depth of every frame (PNG / 10.0), read on the host
+        import cv2
+        K = batch["intrinsic"].detach().cpu().to(torch.float64).reshape(B, 3, 3)
+        depth = []
+        for path in batch["depth_path"]:
+            d = cv2.imread(path, -1)
+            if d is None:
+                raise FileNotFoundError(f"eval_vsd: cannot read depth image {path!r}")
+            depth.append(d / 10.0)
+        if any(d.shape != depth[0].shape or d.ndim != 2 for d in depth):
+            raise ValueError("eval_vsd: the depth images of a batch must share one (H, W) size")
+        H, W = depth[0].shape
+        depth_test = torch.from_numpy(np.stack(depth)).pin_memory().to(dev, non_blocking=True)
+        K4 = torch.stack([K[:, 0, 0], K[:, 1, 1], K[:, 0, 2], K[:, 1, 2]], dim=1)
+        K4 = K4.pin_memory().to(dev, non_blocking=True)
+        rendered = torch.stack([_vsd.render_depth(self.tless_cad[ids[b]], poses[b], K[b], (H, W))
+                                for b in range(B)])                                            # [B, 1 + k, H, W]
+        vsd_error = _vsd.vsd_errors(depth_test, rendered[:, 0], rendered[:, 1:], K4)
+        vsd_error = vsd_error.cpu().numpy()                                                    # B x k
+        final_scores = {}
+        for kk in [1, 3, 5]:
+            best_vsd = np.min(vsd_error[:, :kk], 1)
+            final_scores[f"top {kk}, vsd_median"] = np.median(best_vsd)
+            for threshold in [0.3]:
+                final_scores[f"top {kk}, vsd_scores {threshold}"] = np.mean((best_vsd <= threshold) * 100.0)
+        self.log_score(final_scores, split_name=f"val_{data_name}")
+        if save_path is not None:
+            os.makedirs(os.path.dirname(os.path.abspath(save_path)), exist_ok=True)
+            np.save(save_path, vsd_error[:, 0])
+        return final_scores
+
     def test_step(self, batch, idx_batch):
-        """model.py:550-565: one entry per dataloader, keyed "<dataset>_<category>"."""
+        """model.py:550-565: one entry per dataloader, keyed "<dataset>_<category>"; tless_<category> goes to eval_vsd
+        (saving to log_dir when the model has one), anything else to eval_geodesic."""
         out = {}
         for dataloader_name in batch.keys():
             data_name, category = dataloader_name.split("_")
             if data_name in ["tless"]:
-                raise ValueError("the T-LESS / VSD evaluation (eval_vsd, pyrender) is outside this package's "
-                                 "scope (SURVEY.md section 2): only shapeNet_<category> dataloaders are handled")
+                save_path = None if self.log_dir is None else os.path.join(
+                    self.log_dir, f"vsd_{category}_batch{idx_batch}_rank_{self.global_rank}.npy")
+                out[dataloader_name] = self.eval_vsd(batch[dataloader_name], category, save_path=save_path)
+                continue
             out[dataloader_name] = self.eval_geodesic(batch[dataloader_name], category, visualize=True,
                                                       save_prediction=True)
         self.global_step += 1
