@@ -201,6 +201,18 @@ int nope_render_depth(const float* vertices, int V, const int32_t* faces, int F,
 int nope_vsd_error(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H, int W,
                    const double* K, double delta, double tau, int cost_type, double* out, void* stream);
 
+/* Full-frame crops (DESIGN.md section 13): the virtual-bounding-box crop of src/poses/utils.py:204-272 with the
+ * dataloaders' pipeline around it, bit for bit -- PIL's paste onto black through the mask, cv2.warpPerspective
+ * (bilinear, constant border 0), ToTensor and x*2-1.
+ * frames [F, H, W, C] uint8, C = 3 (RGB) or 4 (RGBA: channel 3 is the mask, and masks must be null); masks [B, H, W]
+ * uint8, one per crop, or null (255 everywhere); frame_idx [B] int32, or null when F == B; inv_maps [B, 9] fp64, the
+ * destination -> source map (cv2.invert of crop_frame's M, DECOMP_LU) -> out [B, 3, S, S] fp32 in [-1, 1].  A frame
+ * index outside [0, F) gives an all -1 crop and reads nothing.  All pointers are device pointers.  Requires F >= 1,
+ * 1 <= B <= 65535, 1 <= H, W <= 16384, 1 <= S <= 4096; refuses bad arguments before any CUDA call and does not
+ * synchronise. */
+int nope_crop_frames(const uint8_t* frames, int F, int H, int W, int C, const uint8_t* masks, const int32_t* frame_idx,
+                     const double* inv_maps, int B, int S, float* out, void* stream);
+
 /* Score materialised templates against a query and rank them: the arithmetic of
  * PoseConditional.retrieval (model.py:254-266) after encode_image.
  *   query_feat [B, C, HW] fp32, emb [B, N, C, HW] fp32 -> sim [B, N], topv/topi [B, k]. */

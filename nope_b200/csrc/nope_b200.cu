@@ -24,6 +24,7 @@
 #include "encoder.cuh"
 #include "ldm.cuh"
 #include "render.cuh"
+#include "crop.cuh"
 
 using namespace nope;
 
@@ -1595,6 +1596,29 @@ int nope_vsd_error(const double* depth_test, const float* depth_gt, const float*
   // the visibility test compares float32 differences with delta in float32, as numpy does with a Python number
   vsd_kernel<<<dim3(kVsdCluster * P, F), kVsdThreads, 0, static_cast<cudaStream_t>(stream)>>>(
       depth_test, depth_gt, depth_est, P, H, W, K, (float)delta, tau, cost_type, out);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// full-frame crops: the virtual-bounding-box perspective warp (crop.cuh, DESIGN.md section 13)
+// ---------------------------------------------------------------------------------
+int nope_crop_frames(const uint8_t* frames, int F, int H, int W, int C, const uint8_t* masks, const int32_t* frame_idx,
+                     const double* inv_maps, int B, int S, float* out, void* stream) {
+  NOPE_CHECK(frames && inv_maps && out, "null argument");
+  NOPE_CHECK(F >= 1 && B >= 1, "F and B must be >= 1");
+  NOPE_CHECK(B <= 65535, "B must be <= 65535");
+  NOPE_CHECK(H >= 1 && H <= kCropMaxSide && W >= 1 && W <= kCropMaxSide, "H and W must be in [1, 16384]");
+  NOPE_CHECK(S >= 1 && S <= kCropMaxS, "S must be in [1, 4096]");
+  NOPE_CHECK(C == 3 || C == 4, "C must be 3 (RGB) or 4 (RGBA)");
+  NOPE_CHECK(!(masks && C == 4), "a mask with C = 4: the alpha channel is the mask");
+  NOPE_CHECK(frame_idx || F == B, "without frame_idx F must equal B");
+  const dim3 grid((S * S + kCropThreads - 1) / kCropThreads, B);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (C == 3)
+    crop_warp_kernel<3><<<grid, kCropThreads, 0, st>>>(frames, F, H, W, masks, frame_idx, inv_maps, S, out);
+  else
+    crop_warp_kernel<4><<<grid, kCropThreads, 0, st>>>(frames, F, H, W, masks, frame_idx, inv_maps, S, out);
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }
