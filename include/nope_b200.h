@@ -180,6 +180,19 @@ int nope_inplane_rotate(const float* images, int B, int H, int W, const float* c
 int nope_encoder_encode_inplane(nope_encoder_t* e, const float* images, int B, const float* cossin, int A,
                                 float* out, void* stream);
 
+/* Rotated copies of arbitrary (image, roll) pairs (DESIGN.md section 14), with the arithmetic of
+ * nope_inplane_rotate: pair p rotates image image_idx[p] (int32) by (cossin[2p], cossin[2p + 1]), so a pair holding
+ * angle-table entry a equals copy a bit for bit.  An image index outside [0, B) gives a copy that is -1 everywhere.
+ * Both calls require B >= 1 and 1 <= P < 2^30 and refuse before any CUDA call.
+ * nope_inplane_rotate_pairs: images [B, 3, H, W] fp32 (device) -> out [P, 3, H, W]; H, W >= 1.
+ * nope_encoder_encode_rotated: images [B, 3, 256, 256] -> out [P, D, 32, 32], equal to nope_encoder_encode of the
+ * rotated pairs [P, 3, 256, 256]: they go 32 at a time, in pair order, through the staging buffer of
+ * nope_encoder_encode_inplane. */
+int nope_inplane_rotate_pairs(const float* images, int B, int H, int W, const int32_t* image_idx,
+                              const float* cossin, int P, float* out, void* stream);
+int nope_encoder_encode_rotated(nope_encoder_t* e, const float* images, int B, const int32_t* image_idx,
+                                const float* cossin, int P, float* out, void* stream);
+
 /* T-LESS evaluation (DESIGN.md section 12): a depth rasterizer standing in for pyrender's DEPTH_ONLY render and the
  * VSD error of src/poses/vsd.py:92-135 (visibility mode "bop19", src/poses/vsd_utils.py).  Both calls refuse bad
  * arguments before any CUDA call and do not synchronise.
@@ -269,6 +282,32 @@ int nope_pose_refine_propose(const float* D, const int32_t* seed, int R, int kee
 int nope_pose_refine_select(const float* sim, const float* cand_D, const int32_t* cand_seed, const float* cand_rel,
                             int R, int M, int k, float trace_threshold, float* out_D, int32_t* out_seed,
                             float* out_score, float* out_rel, void* stream);
+
+/* Joint roll and viewpoint refinement (DESIGN.md section 14).  A candidate is (D, seed, rho), rho = (cos, sin) an
+ * fp32 roll: the pose Rz(rho) * D * template_poses[seed], scored as the relative rotation D * S_seed against the
+ * query crop rotated by rho.  Same rounding discipline as above.
+ * nope_pose_refine_inplane_propose: centres D [R, keep, 9], seed [R, keep] int32, cossin [R, keep, 2]; stencil
+ * [9, 9] (rotation 0 the identity) and the roll step (roll_cos, roll_sin).  Pose slots c * 9 + j are those of
+ * nope_pose_refine_propose with this stencil (out_D, out_seed, out_rel [R, keep * 9, ...], out_poses [R, keep * 9,
+ * 6]); angle slots c * 3 + l (out_cossin [R, keep * 3, 2]) are rho_c for l = 0 (copied bit for bit), rho_c
+ * composed with (roll_cos, roll_sin) for l = 1 and with (roll_cos, -roll_sin) for l = 2.  A centre whose seed lies
+ * outside [0, N) gives padding pose slots (seed -1) and three copies of the first valid centre's rho.  Requires
+ * 1 <= keep <= 16 and R == B * Q.
+ * nope_pose_refine_inplane_select: sim [R, keep * 3, keep * 9] scored at the pairs (angle slot a, pose slot p) ->
+ * k entries per row, greedily: the highest score first (ties -> lowest a * keep * 9 + p), skipping pairs with a
+ * padding pose slot or angle slot, and any pair whose trace(E E_b^T), E = Rz(rho_a) * rel_p, exceeds
+ * trace_threshold against a pair already chosen.  out_D / out_rel (optional) [R, k, 9], out_seed [R, k],
+ * out_cossin [R, k, 2], out_aslot [R, k] (the angle slot), out_score [R, k]; ranks with no pair left get -inf,
+ * seed and aslot -1 and zeros.  Requires 1 <= keep <= 16, 1 <= k <= 64 and k <= 27 * keep^2.
+ * Neither call synchronises; both refuse bad arguments before any CUDA call. */
+int nope_pose_refine_inplane_propose(const float* D, const int32_t* seed, const float* cossin, int R, int keep,
+                                     const float* all_relativeR, int B, int Q, int N, const float* stencil,
+                                     float roll_cos, float roll_sin, float* out_D, int32_t* out_seed, float* out_rel,
+                                     float* out_poses, float* out_cossin, void* stream);
+int nope_pose_refine_inplane_select(const float* sim, const float* cand_D, const int32_t* cand_seed,
+                                    const float* cand_rel, const float* cand_cossin, int R, int keep, int k,
+                                    float trace_threshold, float* out_D, int32_t* out_seed, float* out_cossin,
+                                    int32_t* out_aslot, float* out_score, float* out_rel, void* stream);
 
 /* Multi-GPU merge (SURVEY.md 8e): each rank sweeps a contiguous slice of the pose grid and contributes
  * ONE packed record to a single all-gather:

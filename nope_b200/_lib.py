@@ -44,6 +44,10 @@ SIGNATURES = {
     "nope_encoder_last_launch_count": (C.c_int64, [C.c_void_p]),
     "nope_inplane_rotate": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, c_f32p, C.c_void_p]),
     "nope_encoder_encode_inplane": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, C.c_void_p]),
+    "nope_inplane_rotate_pairs": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_int, c_f32p,
+                                            C.c_void_p]),
+    "nope_encoder_encode_rotated": (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_void_p, c_f32p, C.c_int, c_f32p,
+                                              C.c_void_p]),
     "nope_render_depth": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_int, C.c_float, C.c_float,
                                     C.c_float, C.c_float, C.c_float, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     "nope_vsd_error": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
@@ -65,6 +69,12 @@ SIGNATURES = {
                                            c_f32p, c_f32p, C.c_void_p, c_f32p, c_f32p, C.c_void_p]),
     "nope_pose_refine_select": (C.c_int, [c_f32p, c_f32p, C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_float,
                                           c_f32p, C.c_void_p, c_f32p, c_f32p, C.c_void_p]),
+    "nope_pose_refine_inplane_propose": (C.c_int, [c_f32p, C.c_void_p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int,
+                                                   C.c_int, C.c_int, c_f32p, C.c_float, C.c_float, c_f32p, C.c_void_p,
+                                                   c_f32p, c_f32p, c_f32p, C.c_void_p]),
+    "nope_pose_refine_inplane_select": (C.c_int, [c_f32p, c_f32p, C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int,
+                                                  C.c_int, C.c_float, c_f32p, C.c_void_p, c_f32p, C.c_void_p, c_f32p,
+                                                  c_f32p, C.c_void_p]),
     "nope_topk_pack_floats": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "nope_topk_merge": (C.c_int, [c_f32p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                   c_f32p, c_f32p, c_i64p, C.c_void_p]),

@@ -65,17 +65,12 @@ enc_stem_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
 // no 64-bit division routine is called.  Every product and sum is rounded on its own, in the order
 // oracle/inplane_oracle.py restates: source coordinates, floor, fractions, the two row lerps, the column lerp.  At
 // quarter turns of a square image the fractions are 0 and the copy is an exact permutation.
-__global__ void __launch_bounds__(256)
-inplane_rotate_kernel(const float* __restrict__ img, const float* __restrict__ cossin, int A, int H, int W, int pair0,
-                      float* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int hw_i = H * W;
-  if (i >= hw_i) return;
-  const long long hw = hw_i;
+// The per-pixel body shared by both rotation kernels: pixel i = y * W + x of the copy of image src [3, H, W] rotated
+// by (c, s), written to dst[0], dst[hw], dst[2 hw].
+__device__ __forceinline__ void inplane_rotate_pixel(const float* __restrict__ src, float c, float s, int H, int W,
+                                                     int i, float* __restrict__ dst) {
+  const long long hw = (long long)H * W;
   const int x = i % W, y = i / W;
-  const int p = pair0 + (int)blockIdx.y;
-  const int a = p % A, b = p / A;
-  const float c = cossin[2 * a], s = cossin[2 * a + 1];
   const float cx = __fmul_rn((float)(W - 1), 0.5f), cy = __fmul_rn((float)(H - 1), 0.5f);
   const float dx = __fsub_rn((float)x, cx), dy = __fsub_rn((float)y, cy);
   const float sx = __fadd_rn(__fsub_rn(__fmul_rn(c, dx), __fmul_rn(s, dy)), cx);
@@ -85,8 +80,6 @@ inplane_rotate_kernel(const float* __restrict__ img, const float* __restrict__ c
   const int ix = (int)x0, iy = (int)y0;
   const bool in_x0 = ix >= 0 && ix < W, in_x1 = ix + 1 >= 0 && ix + 1 < W;
   const bool in_y0 = iy >= 0 && iy < H, in_y1 = iy + 1 >= 0 && iy + 1 < H;
-  const float* src = img + (long long)b * 3 * hw;
-  float* dst = out + (long long)blockIdx.y * 3 * hw + i;
 #pragma unroll
   for (int ch = 0; ch < 3; ++ch) {
     const float* plane = src + ch * hw;
@@ -98,6 +91,41 @@ inplane_rotate_kernel(const float* __restrict__ img, const float* __restrict__ c
     const float bot = __fadd_rn(v10, __fmul_rn(fx, __fsub_rn(v11, v10)));
     dst[ch * hw] = __fadd_rn(top, __fmul_rn(fy, __fsub_rn(bot, top)));
   }
+}
+
+__global__ void __launch_bounds__(256)
+inplane_rotate_kernel(const float* __restrict__ img, const float* __restrict__ cossin, int A, int H, int W, int pair0,
+                      float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int hw_i = H * W;
+  if (i >= hw_i) return;
+  const long long hw = hw_i;
+  const int p = pair0 + (int)blockIdx.y;
+  const int a = p % A, b = p / A;
+  inplane_rotate_pixel(img + (long long)b * 3 * hw, cossin[2 * a], cossin[2 * a + 1], H, W, i,
+                       out + (long long)blockIdx.y * 3 * hw + i);
+}
+
+// Rotated copies of arbitrary (image, roll) pairs (DESIGN.md section 14): pair p = pair0 + blockIdx.y rotates image
+// image_idx[p] of img [B, 3, H, W] by (cossin[2p], cossin[2p + 1]) into out [pairs, 3, H, W] (pair-major from pair0),
+// with the per-pixel body of inplane_rotate_kernel, so a pair holding table entry a equals copy a bit for bit.  An
+// image index outside [0, B) gives a copy that is -1 everywhere.
+__global__ void __launch_bounds__(256)
+inplane_rotate_pairs_kernel(const float* __restrict__ img, int B, const int* __restrict__ image_idx,
+                            const float* __restrict__ cossin, int H, int W, int pair0, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int hw_i = H * W;
+  if (i >= hw_i) return;
+  const long long hw = hw_i;
+  const int p = pair0 + (int)blockIdx.y;
+  const int b = image_idx[p];
+  float* dst = out + (long long)blockIdx.y * 3 * hw + i;
+  if (b < 0 || b >= B) {
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) dst[ch * hw] = -1.f;
+    return;
+  }
+  inplane_rotate_pixel(img + (long long)b * 3 * hw, cossin[2 * p], cossin[2 * p + 1], H, W, i, dst);
 }
 
 // [n_pix][ld] fp32 (first D columns valid) -> NCHW fp32 [B, D, hw]
@@ -439,6 +467,28 @@ struct nope_encoder {
     for (int lo = 0; lo < pairs; lo += kChunk) {
       const int n = pairs - lo < kChunk ? pairs - lo : kChunk;
       inplane_rotate_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, cossin, A, 256, 256, lo, rot_stage);
+      NOPE_CUDA(cudaGetLastError());
+      if (encode(rot_stage, n, out + (size_t)lo * D * 32 * 32, st)) return -1;
+      total += launches + 1;
+    }
+    launches = total;
+    return 0;
+  }
+
+  // images [B, 3, 256, 256] x pairs (image_idx [P], cossin [P, 2]) -> out [P, D, 32, 32]: the pairs in order, kChunk
+  // at a time through rot_stage, so the result equals nope_encoder_encode of the materialised [P, 3, 256, 256] batch.
+  int encode_rotated(const float* images, int B, const int* image_idx, const float* cossin, int P, float* out,
+                     cudaStream_t st) {
+    using namespace nope;
+    constexpr long long kImg = 3LL * 256 * 256;
+    if (!rot_stage) {
+      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&rot_stage), kChunk * kImg * sizeof(float)));
+    }
+    int64_t total = 0;
+    for (int lo = 0; lo < P; lo += kChunk) {
+      const int n = P - lo < kChunk ? P - lo : kChunk;
+      inplane_rotate_pairs_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, B, image_idx, cossin, 256, 256,
+                                                                             lo, rot_stage);
       NOPE_CUDA(cudaGetLastError());
       if (encode(rot_stage, n, out + (size_t)lo * D * 32 * 32, st)) return -1;
       total += launches + 1;

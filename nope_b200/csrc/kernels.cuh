@@ -1168,13 +1168,16 @@ __device__ __forceinline__ void mat3_mul_rn(const float* a, const float* b, floa
 // whose seed lies outside [0, N) yields 27 padding slots: seed -1 and a copy of the row's first valid candidate
 // (slot 0 of its first valid centre; D = I at seed 0 when the row has none), so every hypothesis of the sweep
 // is a valid rotation.
-__global__ void __launch_bounds__(256)
-pose_refine_propose_kernel(const float* __restrict__ D, const int* __restrict__ seed, int keep,
-                           const float* __restrict__ rel6, int Q, int N, const float* __restrict__ stencil,
-                           float* __restrict__ out_D, int* __restrict__ out_seed, float* __restrict__ out_rel,
-                           float* __restrict__ out_poses) {
+// The body of the propose kernels, for a stencil of kS rotations (27 here, 9 for the in-plane variant); returns the
+// row's first valid centre (-1 when it has none).
+template <int kS>
+__device__ __forceinline__ int refine_propose_row(const float* __restrict__ D, const int* __restrict__ seed, int keep,
+                                                  const float* __restrict__ rel6, int Q, int N,
+                                                  const float* __restrict__ stencil, float* __restrict__ out_D,
+                                                  int* __restrict__ out_seed, float* __restrict__ out_rel,
+                                                  float* __restrict__ out_poses) {
   const int r = blockIdx.x;
-  const int M = keep * kRefineStencil;
+  const int M = keep * kS;
   const float* Drow = D + (long long)r * keep * 9;
   const int* srow = seed + (long long)r * keep;
   const float* pb = rel6 + (long long)(r / Q) * N * 6;
@@ -1182,7 +1185,7 @@ pose_refine_propose_kernel(const float* __restrict__ D, const int* __restrict__ 
   for (int c = 0; c < keep && first < 0; ++c)
     if (srow[c] >= 0 && srow[c] < N) first = c;
   for (int m = threadIdx.x; m < M; m += blockDim.x) {
-    int c = m / kRefineStencil, j = m - c * kRefineStencil;
+    int c = m / kS, j = m - c * kS;
     int s = srow[c];
     const bool valid = s >= 0 && s < N;
     if (!valid) { c = first; j = 0; }
@@ -1212,6 +1215,15 @@ pose_refine_propose_kernel(const float* __restrict__ D, const int* __restrict__ 
 #pragma unroll
     for (int e = 0; e < 6; ++e) out_poses[o * 6 + e] = rel[e];
   }
+  return first;
+}
+
+__global__ void __launch_bounds__(256)
+pose_refine_propose_kernel(const float* __restrict__ D, const int* __restrict__ seed, int keep,
+                           const float* __restrict__ rel6, int Q, int N, const float* __restrict__ stencil,
+                           float* __restrict__ out_D, int* __restrict__ out_seed, float* __restrict__ out_rel,
+                           float* __restrict__ out_poses) {
+  refine_propose_row<kRefineStencil>(D, seed, keep, rel6, Q, N, stencil, out_D, out_seed, out_rel, out_poses);
 }
 
 // Select: one CTA per row of sim [R, M] scored at the candidates (cand_D / cand_rel [R, M, 9], cand_seed [R, M],
@@ -1273,6 +1285,153 @@ pose_refine_select_kernel(const float* __restrict__ sim, const float* __restrict
       float tr = __fmul_rn(a[0], s_rel[0]);
 #pragma unroll
       for (int e = 1; e < 9; ++e) tr = __fadd_rn(tr, __fmul_rn(a[e], s_rel[e]));
+      if (tr > thr) s_dead[m] = 1;
+    }
+    __syncthreads();
+  }
+}
+
+// ----------------------------------------------------------------------------
+// Joint roll and viewpoint refinement (DESIGN.md section 14).  A candidate is (D, seed, rho): D and seed as in the
+// off-grid refinement, rho = (cos, sin) a roll; it stands for the pose Rz(rho) * D * template_poses[seed] and is
+// scored as the relative rotation D * S_seed against the query crop rotated by rho.  Each centre proposes 9 pose
+// slots (an xy stencil about the camera's x and y axes, identity first) and 3 angle slots (rho, rho + phi,
+// rho - phi); every (angle slot, pose slot) pair is a hypothesis.  Same rounding discipline as above:
+// oracle/inplane_refine_oracle.py restates both kernels op by op.
+// ----------------------------------------------------------------------------
+constexpr int kInplaneXY = 9;                                           // pose slots per centre
+constexpr int kInplaneRoll = 3;                                         // angle slots per centre
+constexpr int kInplaneMaxKeep = 16;
+constexpr int kInplaneMaxPairs = kInplaneXY * kInplaneRoll * kInplaneMaxKeep * kInplaneMaxKeep;
+
+// e = Rz(c, s) * x: rows 1-2 mixed by the roll, row 3 copied
+__device__ __forceinline__ void rz_mul_rn(float c, float s, const float* x, float* e) {
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    e[j] = __fsub_rn(__fmul_rn(c, x[j]), __fmul_rn(s, x[3 + j]));
+    e[3 + j] = __fadd_rn(__fmul_rn(s, x[j]), __fmul_rn(c, x[3 + j]));
+    e[6 + j] = x[6 + j];
+  }
+}
+
+// Propose: one CTA per row.  Pose slots c * 9 + j exactly as pose_refine_propose_kernel with the 9-rotation
+// stencil.  Angle slots c * 3 + l (out_cossin [R, keep * 3, 2]): l = 0 copies rho_c, l = 1 / 2 compose it with
+// (roll_c, +roll_s) / (roll_c, -roll_s): (c c' - s s', s c' + c s').  A centre whose seed lies outside [0, N) gives
+// three copies of the first valid centre's rho ((1, 0) when the row has none).
+__global__ void __launch_bounds__(256)
+pose_refine_inplane_propose_kernel(const float* __restrict__ D, const int* __restrict__ seed,
+                                   const float* __restrict__ cossin, int keep, const float* __restrict__ rel6, int Q,
+                                   int N, const float* __restrict__ stencil, float roll_c, float roll_s,
+                                   float* __restrict__ out_D, int* __restrict__ out_seed, float* __restrict__ out_rel,
+                                   float* __restrict__ out_poses, float* __restrict__ out_cossin) {
+  const int first = refine_propose_row<kInplaneXY>(D, seed, keep, rel6, Q, N, stencil, out_D, out_seed, out_rel,
+                                                   out_poses);
+  const int r = blockIdx.x;
+  const int* srow = seed + (long long)r * keep;
+  const float* crow = cossin + (long long)r * keep * 2;
+  float* orow = out_cossin + (long long)r * keep * kInplaneRoll * 2;
+  for (int m = threadIdx.x; m < keep * kInplaneRoll; m += blockDim.x) {
+    int c = m / kInplaneRoll, l = m - c * kInplaneRoll;
+    const int s = srow[c];
+    if (s < 0 || s >= N) { c = first; l = 0; }
+    float oc = 1.0f, os = 0.0f;
+    if (c >= 0) {
+      const float ca = crow[2 * c], sa = crow[2 * c + 1];
+      if (l == 0) {
+        oc = ca;
+        os = sa;
+      } else {
+        const float sb = l == 1 ? roll_s : -roll_s;
+        oc = __fsub_rn(__fmul_rn(ca, roll_c), __fmul_rn(sa, sb));
+        os = __fadd_rn(__fmul_rn(sa, roll_c), __fmul_rn(ca, sb));
+      }
+    }
+    orow[2 * m] = oc;
+    orow[2 * m + 1] = os;
+  }
+}
+
+// Select: one CTA per row of sim [R, keep * 3, keep * 9], pair m = a * (keep * 9) + p of angle slot a and pose slot
+// p.  A pair is padding when its pose slot or its angle slot's centre has seed -1.  Greedy: the highest score first,
+// ties -> lowest m; a pair is dropped once trace(E_m E_b^T) > thr for a chosen b, E = Rz(rho_a) * rel_p (nine
+// products summed in order).  Writes k entries of D / rel (optional) [R, k, 9], seed [R, k], cossin [R, k, 2],
+// aslot [R, k] (the winner's angle slot) and score [R, k]; ranks with no pair left get -inf, seed and aslot -1 and
+// zeros.
+__global__ void __launch_bounds__(256)
+pose_refine_inplane_select_kernel(const float* __restrict__ sim, const float* __restrict__ cand_D,
+                                  const int* __restrict__ cand_seed, const float* __restrict__ cand_rel,
+                                  const float* __restrict__ cand_cossin, int keep, int k, float thr,
+                                  float* __restrict__ out_D, int* __restrict__ out_seed,
+                                  float* __restrict__ out_cossin, int* __restrict__ out_aslot,
+                                  float* __restrict__ out_score, float* __restrict__ out_rel) {
+  __shared__ float s_v[8];
+  __shared__ int s_i[8];
+  __shared__ int s_pick;
+  __shared__ float s_E[9];
+  __shared__ unsigned char s_dead[kInplaneMaxPairs];
+  const int r = blockIdx.x;
+  const int NP = keep * kInplaneXY, NA = keep * kInplaneRoll, M = NA * NP;
+  const float* srow = sim + (long long)r * M;
+  const float* rrow = cand_rel + (long long)r * NP * 9;
+  const float* crow = cand_cossin + (long long)r * NA * 2;
+  const int* seedrow = cand_seed + (long long)r * NP;
+  for (int m = threadIdx.x; m < M; m += blockDim.x) {
+    const int a = m / NP, p = m - a * NP;
+    s_dead[m] = seedrow[p] < 0 || seedrow[(a / kInplaneRoll) * kInplaneXY] < 0;
+  }
+  __syncthreads();
+  for (int t = 0; t < k; ++t) {
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int m = threadIdx.x; m < M; m += blockDim.x) {
+      if (s_dead[m]) continue;
+      const float v = srow[m];
+      if (v > bv || (v == bv && m < bi) || bi == 0x7fffffff) { bv = v; bi = m; }
+    }
+    cta_argmax(bv, bi, s_v, s_i);
+    if (threadIdx.x == 0) s_pick = bi;
+    __syncthreads();
+    const int pick = s_pick;
+    const long long o = (long long)r * k + t;
+    if (pick == 0x7fffffff) {
+      if (threadIdx.x < 9) {
+        out_D[o * 9 + threadIdx.x] = 0.0f;
+        if (out_rel) out_rel[o * 9 + threadIdx.x] = 0.0f;
+      }
+      if (threadIdx.x < 2) out_cossin[o * 2 + threadIdx.x] = 0.0f;
+      if (threadIdx.x == 0) { out_score[o] = -INFINITY; out_seed[o] = -1; out_aslot[o] = -1; }
+      continue;
+    }
+    const int pa = pick / NP, pp = pick - pa * NP;
+    const long long p = (long long)r * NP + pp;
+    if (threadIdx.x < 9) {
+      out_D[o * 9 + threadIdx.x] = cand_D[p * 9 + threadIdx.x];
+      if (out_rel) out_rel[o * 9 + threadIdx.x] = cand_rel[p * 9 + threadIdx.x];
+    }
+    if (threadIdx.x < 2) out_cossin[o * 2 + threadIdx.x] = crow[pa * 2 + threadIdx.x];
+    if (threadIdx.x == 0) {
+      float x[9], e[9];
+#pragma unroll
+      for (int i = 0; i < 9; ++i) x[i] = rrow[pp * 9 + i];
+      rz_mul_rn(crow[pa * 2], crow[pa * 2 + 1], x, e);
+#pragma unroll
+      for (int i = 0; i < 9; ++i) s_E[i] = e[i];
+      out_score[o] = bv;
+      out_seed[o] = cand_seed[p];
+      out_aslot[o] = pa;
+      s_dead[pick] = 1;
+    }
+    __syncthreads();
+    for (int m = threadIdx.x; m < M; m += blockDim.x) {
+      if (s_dead[m]) continue;
+      const int a = m / NP, pm = m - a * NP;
+      float x[9], e[9];
+#pragma unroll
+      for (int i = 0; i < 9; ++i) x[i] = rrow[pm * 9 + i];
+      rz_mul_rn(crow[a * 2], crow[a * 2 + 1], x, e);
+      float tr = __fmul_rn(e[0], s_E[0]);
+#pragma unroll
+      for (int i = 1; i < 9; ++i) tr = __fadd_rn(tr, __fmul_rn(e[i], s_E[i]));
       if (tr > thr) s_dead[m] = 1;
     }
     __syncthreads();

@@ -1439,6 +1439,39 @@ int nope_pose_refine_select(const float* sim, const float* cand_D, const int32_t
   return 0;
 }
 
+int nope_pose_refine_inplane_propose(const float* D, const int32_t* seed, const float* cossin, int R, int keep,
+                                     const float* all_relativeR, int B, int Q, int N, const float* stencil,
+                                     float roll_cos, float roll_sin, float* out_D, int32_t* out_seed, float* out_rel,
+                                     float* out_poses, float* out_cossin, void* stream) {
+  NOPE_CHECK(D && seed && cossin && all_relativeR && stencil && out_D && out_seed && out_rel && out_poses &&
+                 out_cossin, "null argument");
+  NOPE_CHECK(keep >= 1 && keep <= kInplaneMaxKeep, "keep must be in [1, 16]");
+  NOPE_CHECK(B >= 1 && Q >= 1 && N >= 1, "bad arguments");
+  NOPE_CHECK(R >= 1 && (int64_t)B * Q == R, "R (rows) must equal B * Q");
+  pose_refine_inplane_propose_kernel<<<R, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      D, seed, cossin, keep, all_relativeR, Q, N, stencil, roll_cos, roll_sin, out_D, out_seed, out_rel, out_poses,
+      out_cossin);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int nope_pose_refine_inplane_select(const float* sim, const float* cand_D, const int32_t* cand_seed,
+                                    const float* cand_rel, const float* cand_cossin, int R, int keep, int k,
+                                    float trace_threshold, float* out_D, int32_t* out_seed, float* out_cossin,
+                                    int32_t* out_aslot, float* out_score, float* out_rel, void* stream) {
+  NOPE_CHECK(sim && cand_D && cand_seed && cand_rel && cand_cossin && out_D && out_seed && out_cossin && out_aslot &&
+                 out_score, "null argument");
+  NOPE_CHECK(keep >= 1 && keep <= kInplaneMaxKeep, "keep must be in [1, 16]");
+  NOPE_CHECK(k >= 1 && k <= 64, "k must be in [1, 64]");
+  NOPE_CHECK(k <= kInplaneXY * kInplaneRoll * keep * keep, "k must not exceed the 27 * keep^2 pairs per row");
+  NOPE_CHECK(R >= 1, "bad arguments");
+  pose_refine_inplane_select_kernel<<<R, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      sim, cand_D, cand_seed, cand_rel, cand_cossin, keep, k, trace_threshold, out_D, out_seed, out_cossin, out_aslot,
+      out_score, out_rel);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int64_t nope_topk_pack_floats(int B, int k, int n_local_max, int want_sim) {
   if (B < 1 || k < 1 || n_local_max < 0) return -1;
   const int64_t kk = ((int64_t)B * k + 1) & ~(int64_t)1;
@@ -1554,6 +1587,34 @@ int nope_inplane_rotate(const float* images, int B, int H, int W, const float* c
     NOPE_CUDA(cudaGetLastError());
   }
   return 0;
+}
+
+int nope_inplane_rotate_pairs(const float* images, int B, int H, int W, const int32_t* image_idx, const float* cossin,
+                              int P, float* out, void* stream) {
+  NOPE_CHECK(images && image_idx && cossin && out, "null images / image_idx / cossin / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(H >= 1 && W >= 1, "H and W must be >= 1");
+  NOPE_CHECK(P >= 1 && P <= INT32_MAX / 2, "P (pairs) must be in [1, 2^30)");
+  NOPE_CHECK((int64_t)H * W <= INT32_MAX - 255, "images too large");
+  const int hw = H * W;
+  constexpr int kMaxGridY = 65535;
+  for (int lo = 0; lo < P; lo += kMaxGridY) {
+    const int n = P - lo < kMaxGridY ? P - lo : kMaxGridY;
+    inplane_rotate_pairs_kernel<<<dim3((hw + 255) / 256, n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        images, B, image_idx, cossin, H, W, lo, out + (size_t)lo * 3 * hw);
+    NOPE_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
+int nope_encoder_encode_rotated(nope_encoder_t* e, const float* images, int B, const int32_t* image_idx,
+                                const float* cossin, int P, float* out, void* stream) {
+  NOPE_CHECK(images && image_idx && cossin && out, "null images / image_idx / cossin / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(P >= 1 && P <= INT32_MAX / 2, "P (pairs) must be in [1, 2^30)");
+  NOPE_CHECK(e && e->finalized, "encoder not finalized");
+  NOPE_CUDA(cudaSetDevice(e->device));
+  return e->encode_rotated(images, B, image_idx, cossin, P, out, static_cast<cudaStream_t>(stream));
 }
 
 int64_t nope_encoder_last_launch_count(const nope_encoder_t* e) { return e ? e->launches : 0; }

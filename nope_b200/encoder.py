@@ -183,3 +183,29 @@ class FeatureExtractor(nn.Module):
                 self._engine(p.device), _lib.ptr(x), x.shape[0], _lib.ptr(_on_device(inplane_table, A, p.device)),
                 A, _lib.ptr(out), C.c_void_p(torch.cuda.current_stream(p.device).cuda_stream)))
         return F.normalize(out, dim=2) if self.normalize else out
+
+    @torch.no_grad()
+    def encode_image_rotated(self, image, image_idx, cossin):
+        """image [B,3,256,256], pairs image_idx [P] (int) and cossin [P, 2] (float32 (cos, sin)) -> [P,D,32,32]: the
+        latent of image image_idx[p] rotated by cossin[p] (the section 11 image convention, DESIGN.md section 14),
+        equal to encode_image of the materialised rotated pairs, without forming them.  An index outside [0, B)
+        encodes an all -1 crop.  Native engine only: the torch backend raises NopeError."""
+        p = next(self.parameters())
+        if not self._use_native(p.device):
+            raise _lib.NopeError("encode_image_rotated needs the native engine on a CUDA device "
+                                 "(no torch-backend path)")
+        if image.dim() != 4 or tuple(image.shape[1:]) != (3, 256, 256):
+            raise _lib.NopeError("the native encoder is built for [B, 3, 256, 256] inputs")
+        if image_idx.dim() != 1 or tuple(cossin.shape) != (image_idx.shape[0], 2) or image_idx.shape[0] < 1:
+            raise ValueError(f"image_idx [P] and cossin [P, 2] with P >= 1 expected, got {tuple(image_idx.shape)} and "
+                             f"{tuple(cossin.shape)}")
+        x = image.to(device=p.device, dtype=torch.float32).contiguous()
+        idx = image_idx.to(device=p.device, dtype=torch.int32).contiguous()
+        cs = cossin.to(device=p.device, dtype=torch.float32).contiguous()
+        P = idx.shape[0]
+        out = torch.empty((P, self.latent_dim, 32, 32), device=p.device, dtype=torch.float32)
+        with torch.cuda.device(p.device):
+            _lib.check(_lib.load().nope_encoder_encode_rotated(
+                self._engine(p.device), _lib.ptr(x), x.shape[0], _lib.ptr(idx), _lib.ptr(cs), P, _lib.ptr(out),
+                C.c_void_p(torch.cuda.current_stream(p.device).cuda_stream)))
+        return F.normalize(out, dim=1) if self.normalize else out

@@ -270,6 +270,48 @@ class PoseConditional:
         return R, nearest, angle, sim
 
     @torch.no_grad()
+    def predict_pose_inplane_refined(self, query, reference, all_relativeR, refiner, k=5, keep=2):
+        """Roll and viewpoint between the bins and the grid poses (nope_b200.inplane_refine, DESIGN.md section 14):
+        the in-plane search over the refiner's A angles seeds each (reference, query) row with its joint top-`keep`
+        (angle, pose) pairs, and the refiner's steps refine the viewpoint on the template side and the roll on the
+        query side.  refiner: an InplaneRefiner over the grid of all_relativeR [B, N, 6].
+        -> (R [..., k, 3, 3] = Rz(rho) D template_poses[seed] (float64), seed [..., k], alpha_deg [..., k] =
+        atan2(sin, cos) of the roll rho, score [..., k]) in the query forms of predict_pose; descending score, each
+        exactly the score a sweep of that pose against that rolled latent gives."""
+        from .inplane_refine import check_inplane_refine_args, pose_rotations, refine_inplane, roll_degrees
+        if self.dist is not None:
+            raise NotImplementedError("predict_pose_inplane_refined does not shard across GPUs: the refinement runs "
+                                      "on one device (unset model.dist or use predict_pose)")
+        check_inplane_refine_args(refiner, all_relativeR, keep, k, reference.shape[0])
+        metric = getattr(self.testing_config, "similarity_metric", "l2")
+        if metric not in _METRICS:
+            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+        query, squeeze = multi_query_form(query, reference)
+        B, A, N = reference.shape[0], refiner.angles, refiner.num_poses
+        Q = 1 if query.dim() == reference.dim() else query.shape[1]
+        enc = self.u_net.encoder
+        self.u_net.set_metric(metric, self._occlusion_threshold())
+        reference_feat = enc.encode_image(reference.to(self.device))
+        flat_q = query.reshape(B * Q, *query.shape[-3:]).to(self.device)
+        query_feat = enc.encode_image_inplane(flat_q, A)                                   # [B * Q, A, C, h, w]
+        sim = self.u_net.sweep(reference_feat, all_relativeR, want_emb=False, want_sim=True, k=0,
+                               query_feat=query_feat.view(B, Q * A, *query_feat.shape[2:]))["sim"]   # [B, Q * A, N]
+        _, flat = topk(sim.view(B * Q, A * N), keep)
+        pose_idx, angle_idx = flat % N, flat // N
+        rows = torch.arange(B * Q, device=flat.device)[:, None]
+        lat = query_feat[rows, angle_idx]                                                  # [B * Q, keep, C, h, w]
+        lead = (B,) if query.dim() == reference.dim() else (B, Q)
+        images = flat_q.view(*lead, *query.shape[-3:])
+        out = refine_inplane(self.u_net, enc, reference_feat, images, all_relativeR,
+                             (pose_idx.view(*lead, keep), angle_idx.view(*lead, keep)),
+                             lat.view(*lead, keep, *lat.shape[2:]), refiner, k=k)
+        R = pose_rotations(out["D"], out["seed"], out["cossin"], refiner)
+        seed, alpha, score = out["seed"], roll_degrees(out["cossin"]), out["score"]
+        if squeeze:
+            R, seed, alpha, score = R[0], seed[0], alpha[0], score[0]
+        return R, seed, alpha, score
+
+    @torch.no_grad()
     def retrieval_inplane(self, query, template_feat, k=5, angles=36):
         """retrieval over pose x in-plane angle, for templates generated once and queries streamed: the A = `angles`
         rotated copies of every query image [Bq, 3, 256, 256] against template_feat [Bt, N, C, h, w], batches
