@@ -214,6 +214,23 @@ int nope_render_depth(const float* vertices, int V, const int32_t* faces, int F,
 int nope_vsd_error(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H, int W,
                    const double* K, double delta, double tau, int cost_type, double* out, void* stream);
 
+/* BOP 2019 errors (DESIGN.md section 15).
+ * nope_vsd_error_taus: nope_vsd_error at T misalignment tolerances in one pass (the distance images, visibility
+ * masks and counts are shared): taus HOST [T] fp64, each finite and > 0, 1 <= T <= 16; K HOST [F, 4] fp64, finite,
+ * fx and fy non-zero -> out [F, P, T] fp64; out[f, p, j] equals nope_vsd_error at tau = taus[j] bit for bit.
+ * nope_pose_errors: MSSD (mm) and MSPD (px) of P estimated poses per row, minimised over S symmetry transforms:
+ * points [V, 3] fp32 (model frame, mm), sym [S, 12], gt [F, 12] and est [F, P, 12] fp64 row-major 3x4 (R | t),
+ * K HOST [F, 4] fp64 (fx, fy, cx, cy; finite, fx and fy non-zero) -> out_mssd, out_mspd [F, P] fp64.
+ * MSSD = min_s max_x |(R_e x + t_e) - (R_g (R_s x + t_s) + t_g)|, MSPD the same between the projections
+ * u = fx X / Z + cx, v = fy Y / Z + cy; a symmetry under which a point has Z <= 0 for either pose counts +inf.
+ * Requires V, S >= 1, S <= 2^24, 1 <= F, P <= 65535.  The result does not depend on the launch shape.
+ * Both calls refuse bad arguments before any CUDA call, stage K in stream order and do not synchronise. */
+int nope_vsd_error_taus(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H,
+                        int W, const double* K, double delta, int cost_type, const double* taus, int T, double* out,
+                        void* stream);
+int nope_pose_errors(const float* points, int V, const double* sym, int S, const double* gt, const double* est,
+                     const double* K, int F, int P, double* out_mssd, double* out_mspd, void* stream);
+
 /* Full-frame crops (DESIGN.md section 13): the virtual-bounding-box crop of src/poses/utils.py:204-272 with the
  * dataloaders' pipeline around it, bit for bit -- PIL's paste onto black through the mask, cv2.warpPerspective
  * (bilinear, constant border 0), ToTensor and x*2-1.

@@ -24,6 +24,7 @@
 #include "encoder.cuh"
 #include "ldm.cuh"
 #include "render.cuh"
+#include "pose_error.cuh"
 #include "crop.cuh"
 
 using namespace nope;
@@ -1654,9 +1655,93 @@ int nope_vsd_error(const double* depth_test, const float* depth_gt, const float*
   NOPE_CHECK(cost_type == NOPE_VSD_STEP || cost_type == NOPE_VSD_TLINEAR, "unknown cost_type (0 step, 1 tlinear)");
   NOPE_CHECK(delta >= 0.0 && std::isfinite(delta), "delta must be finite and >= 0");
   NOPE_CHECK(tau > 0.0 && std::isfinite(tau), "tau must be finite and > 0");
+  VsdTaus taus{};
+  taus.v[0] = tau;
   // the visibility test compares float32 differences with delta in float32, as numpy does with a Python number
-  vsd_kernel<<<dim3(kVsdCluster * P, F), kVsdThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-      depth_test, depth_gt, depth_est, P, H, W, K, (float)delta, tau, cost_type, out);
+  vsd_kernel<1><<<dim3(kVsdCluster * P, F), kVsdThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      depth_test, depth_gt, depth_est, P, H, W, K, (float)delta, taus, 1, cost_type, out);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// HOST K [F, 4]: finite, fx and fy non-zero
+static int check_host_intrinsics(const double* K, int F) {
+  for (int f = 0; f < F; ++f) {
+    const double* k = K + 4 * (size_t)f;
+    NOPE_CHECK(std::isfinite(k[0]) && std::isfinite(k[1]) && std::isfinite(k[2]) && std::isfinite(k[3]),
+               "intrinsics must be finite");
+    NOPE_CHECK(k[0] != 0.0 && k[1] != 0.0, "fx and fy must be non-zero");
+  }
+  return 0;
+}
+
+// A stream-ordered device copy of a small HOST array: the pageable source is staged at once (no host
+// synchronisation) and the copy is freed in stream order after the kernels that read it.
+struct StagedHost {
+  void* dev = nullptr;
+  cudaStream_t st = nullptr;
+  int upload(const void* host, size_t bytes, cudaStream_t stream) {
+    st = stream;
+    NOPE_CUDA(cudaMallocAsync(&dev, bytes, st));
+    NOPE_CUDA(cudaMemcpyAsync(dev, host, bytes, cudaMemcpyHostToDevice, st));
+    return 0;
+  }
+  ~StagedHost() {
+    if (dev) cudaFreeAsync(dev, st);
+  }
+};
+
+int nope_vsd_error_taus(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H,
+                        int W, const double* K, double delta, int cost_type, const double* taus, int T, double* out,
+                        void* stream) {
+  NOPE_CHECK(depth_test && depth_gt && depth_est && K && taus && out, "null argument");
+  NOPE_CHECK(F >= 1 && P >= 1, "F and P must be >= 1");
+  NOPE_CHECK(F <= 65535 && P <= 65535, "F and P must be <= 65535");
+  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
+  NOPE_CHECK(T >= 1 && T <= kVsdMaxTaus, "T (tolerances) must be in [1, 16]");
+  NOPE_CHECK(cost_type == NOPE_VSD_STEP || cost_type == NOPE_VSD_TLINEAR, "unknown cost_type (0 step, 1 tlinear)");
+  NOPE_CHECK(delta >= 0.0 && std::isfinite(delta), "delta must be finite and >= 0");
+  VsdTaus tv{};
+  for (int j = 0; j < T; ++j) {
+    NOPE_CHECK(taus[j] > 0.0 && std::isfinite(taus[j]), "every tau must be finite and > 0");
+    tv.v[j] = taus[j];
+  }
+  if (check_host_intrinsics(K, F)) return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  StagedHost k;
+  if (k.upload(K, sizeof(double) * 4 * (size_t)F, st)) return -1;
+  const double* kd = static_cast<const double*>(k.dev);
+  const dim3 grid(kVsdCluster * P, F);
+  if (T == 1)
+    vsd_kernel<1><<<grid, kVsdThreads, 0, st>>>(depth_test, depth_gt, depth_est, P, H, W, kd, (float)delta, tv, T,
+                                                 cost_type, out);
+  else
+    vsd_kernel<kVsdMaxTaus><<<grid, kVsdThreads, 0, st>>>(depth_test, depth_gt, depth_est, P, H, W, kd, (float)delta,
+                                                           tv, T, cost_type, out);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// BOP pose errors: symmetry-aware MSSD / MSPD (pose_error.cuh, DESIGN.md section 15)
+// ---------------------------------------------------------------------------------
+int nope_pose_errors(const float* points, int V, const double* sym, int S, const double* gt, const double* est,
+                     const double* K, int F, int P, double* out_mssd, double* out_mspd, void* stream) {
+  NOPE_CHECK(points && sym && gt && est && K && out_mssd && out_mspd, "null argument");
+  NOPE_CHECK(V >= 1 && S >= 1 && F >= 1 && P >= 1, "V, S, F and P must be >= 1");
+  NOPE_CHECK(F <= 65535 && P <= 65535, "F and P must be <= 65535");
+  NOPE_CHECK(S <= (1 << 24), "S must be <= 2^24");
+  if (check_host_intrinsics(K, F)) return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  StagedHost k;
+  if (k.upload(K, sizeof(double) * 4 * (size_t)F, st)) return -1;
+  const int n = F * P;
+  auto* om = reinterpret_cast<unsigned long long*>(out_mssd);
+  auto* op = reinterpret_cast<unsigned long long*>(out_mspd);
+  pose_error_fill_kernel<<<std::min((n + 255) / 256, 1024), 256, 0, st>>>(om, op, n);
+  NOPE_CUDA(cudaGetLastError());
+  pose_error_kernel<<<dim3((S + kPoseErrSyms - 1) / kPoseErrSyms, P, F), kPoseErrThreads, 0, st>>>(
+      points, V, sym, S, gt, est, static_cast<const double*>(k.dev), P, om, op);
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }

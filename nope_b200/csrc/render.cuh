@@ -10,7 +10,8 @@
 // restates every step in torch.
 //
 // VSD: vsd_obj's per-pose body (reference src/poses/vsd.py:92-135 with src/poses/vsd_utils.py, visibility "bop19"),
-// one 8-CTA cluster per (frame, pose), reduced over the image in a fixed order.
+// one 8-CTA cluster per (frame, pose), reduced over the image in a fixed order; one pass serves up to 16 tolerances tau
+// (DESIGN.md section 15).
 #pragma once
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
@@ -130,15 +131,25 @@ __device__ __forceinline__ double vsd_dist(double prex, double prey, double d) {
   return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(a, a), __dmul_rn(b, b)), __dmul_rn(d, d)));
 }
 
+constexpr int kVsdMaxTaus = 16;              // misalignment tolerances served by one pass
+
+struct VsdTaus {
+  double v[kVsdMaxTaus];                       // v[0 .. T) are used
+};
+
 // One cluster of kVsdCluster CTAs per (pose p, frame f): grid (kVsdCluster * P, F).  CTA rank r of the cluster
 // takes pixels r * kVsdThreads + t, r * kVsdThreads + t + kVsdCluster * kVsdThreads, ...; each CTA reduces its
 // partial counts in a fixed tree order and rank 0 adds the kVsdCluster partials in rank order through distributed
 // shared memory: no workspace, no atomics, and a result that does not depend on scheduling.  K [F, 4] =
-// (fx, fy, cx, cy) float64.  cost_type 0 = "step", 1 = "tlinear".  out [F, P] float64.
+// (fx, fy, cx, cy) float64.  cost_type 0 = "step", 1 = "tlinear".  One pass scores T <= kMaxT tolerances taus.v[j]:
+// the distance images, the visibility masks and the intersection / union counts are shared, each tolerance keeps
+// its own cost and is reduced through the same tree, one after the other.  out [F, P, T] float64.
+template <int kMaxT>
 __global__ void __cluster_dims__(kVsdCluster, 1, 1) __launch_bounds__(kVsdThreads)
 vsd_kernel(const double* __restrict__ depth_test, const float* __restrict__ depth_gt, const float* __restrict__ depth_est,
-           int P, int H, int W, const double* __restrict__ K, float delta, double tau, int cost_type,
+           int P, int H, int W, const double* __restrict__ K, float delta, const VsdTaus taus, int T, int cost_type,
            double* __restrict__ out) {
+  static_assert(kMaxT >= 1 && kMaxT <= kVsdMaxTaus, "1 <= kMaxT <= kVsdMaxTaus");
   namespace cg = cooperative_groups;
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
@@ -148,8 +159,10 @@ vsd_kernel(const double* __restrict__ depth_test, const float* __restrict__ dept
   const double* dt_f = depth_test + (size_t)f * hw;
   const float* dg_f = depth_gt + (size_t)f * hw;
   const float* de_f = depth_est + ((size_t)f * P + p) * hw;
-  int n_inter = 0, n_union = 0, n_cost = 0;
-  double s_cost = 0.0;
+  int n_inter = 0, n_union = 0, n_cost[kMaxT];
+  double s_cost[kMaxT];
+#pragma unroll
+  for (int j = 0; j < kMaxT; ++j) { n_cost[j] = 0; s_cost[j] = 0.0; }
   for (int i = rank * kVsdThreads + threadIdx.x; i < hw; i += kVsdCluster * kVsdThreads) {
     const int y = i / W, x = i % W;
     const double prex = __ddiv_rn(__dsub_rn((double)x, cx), fx), prey = __ddiv_rn(__dsub_rn((double)y, cy), fy);
@@ -166,38 +179,57 @@ vsd_kernel(const double* __restrict__ depth_test, const float* __restrict__ dept
     if (vis_gt && vis_est) {
       ++n_inter;
       const double dd = fabs(__dsub_rn(d_gt, d_est));
-      if (cost_type == 0) n_cost += dd >= tau ? 1 : 0;
-      else s_cost = __dadd_rn(s_cost, fmin(__ddiv_rn(dd, tau), 1.0));
+#pragma unroll
+      for (int j = 0; j < kMaxT; ++j) {
+        if (kMaxT == 1 || j < T) {                 // the T = 1 instantiation needs no test
+          if (cost_type == 0) n_cost[j] += dd >= taus.v[j] ? 1 : 0;
+          else s_cost[j] = __dadd_rn(s_cost[j], fmin(__ddiv_rn(dd, taus.v[j]), 1.0));
+        }
+      }
     }
   }
   __shared__ int si[3][kVsdThreads];
   __shared__ double sd[kVsdThreads];
+  __shared__ int part_i[2 + kMaxT];                // this CTA's inter, union and per-tolerance costs
+  __shared__ double part_d[kMaxT];
   const int t = threadIdx.x;
-  si[0][t] = n_inter; si[1][t] = n_union; si[2][t] = n_cost; sd[t] = s_cost;
-  __syncthreads();
-  for (int s = kVsdThreads / 2; s > 0; s >>= 1) {  // fixed tree order
-    if (t < s) {
-      si[0][t] += si[0][t + s]; si[1][t] += si[1][t + s]; si[2][t] += si[2][t + s];
-      sd[t] = __dadd_rn(sd[t], sd[t + s]);
+  si[0][t] = n_inter; si[1][t] = n_union;
+#pragma unroll
+  for (int j = 0; j < kMaxT; ++j) {
+    if (kMaxT == 1 || j < T) {
+      si[2][t] = n_cost[j]; sd[t] = s_cost[j];
+      __syncthreads();
+      for (int s = kVsdThreads / 2; s > 0; s >>= 1) {  // fixed tree order, the same for every tolerance
+        if (t < s) {
+          if (j == 0) { si[0][t] += si[0][t + s]; si[1][t] += si[1][t + s]; }
+          si[2][t] += si[2][t + s];
+          sd[t] = __dadd_rn(sd[t], sd[t + s]);
+        }
+        __syncthreads();
+      }
+      if (t == 0) {
+        if (j == 0) { part_i[0] = si[0][0]; part_i[1] = si[1][0]; }
+        part_i[2 + j] = si[2][0]; part_d[j] = sd[0];
+      }
+      __syncthreads();                             // si[2] / sd are rewritten for the next tolerance
     }
-    __syncthreads();
   }
   cluster.sync();                                  // every CTA's partials are in its shared memory
-  if (rank == 0 && t == 0) {
+  if (rank == 0 && t < T) {                        // one thread per tolerance
     int inter = 0, uni = 0, cost = 0;
     double sum = 0.0;
     for (int r = 0; r < kVsdCluster; ++r) {        // rank order
-      const int* ri = cluster.map_shared_rank(&si[0][0], r);
-      const double* rd = cluster.map_shared_rank(&sd[0], r);
-      inter += ri[0]; uni += ri[kVsdThreads]; cost += ri[2 * kVsdThreads];
-      sum = __dadd_rn(sum, rd[0]);
+      const int* ri = cluster.map_shared_rank(&part_i[0], r);
+      const double* rd = cluster.map_shared_rank(&part_d[0], r);
+      inter += ri[0]; uni += ri[1]; cost += ri[2 + t];
+      sum = __dadd_rn(sum, rd[t]);
     }
     double e = 1.0;
     // (sum(costs) + (union - inter)) / union: an integer sum for "step", a float64 sum for "tlinear"
     if (uni > 0)
       e = cost_type == 0 ? __ddiv_rn((double)(cost + uni - inter), (double)uni)
                          : __ddiv_rn(__dadd_rn(sum, (double)(uni - inter)), (double)uni);
-    out[(size_t)f * P + p] = e;
+    out[((size_t)f * P + p) * T + t] = e;
   }
   cluster.sync();                                  // no CTA leaves while rank 0 reads its shared memory
 }

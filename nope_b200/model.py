@@ -46,6 +46,7 @@ class PoseConditional:
         # model.py:66: per-batch VSD errors go to <save_dir>/predictions (created on first save)
         self.log_dir = None if save_dir is None else os.path.join(save_dir, "predictions")
         self.tless_cad = {}                        # obj_id -> nope_b200.vsd.Mesh (load_mesh)
+        self.bop_models = {}                       # obj_id -> {"diameter", "symmetries"} (load_models_info)
 
     @property
     def device(self):
@@ -432,12 +433,38 @@ class PoseConditional:
         query, reference = batch["query"], batch["reference"]
         loss = self.forward(query=query, relativeR=batch["gt_relativeR"], reference=reference)
         self.log(f"loss/val_{data_name}", loss)
-        _, nearest_idx, _ = self.predict_pose(query, reference, batch["all_relativeR"], None, k=5)
+        R = self._grid_rotations(batch, B)
+        depth_test, rendered, _, K4 = self._render_frames(batch, B, ids, R)
+        vsd_error = _vsd.vsd_errors(depth_test, rendered[:, 0], rendered[:, 1:], K4)
+        vsd_error = vsd_error.cpu().numpy()                                                    # B x k
+        final_scores = {}
+        for kk in [1, 3, 5]:
+            best_vsd = np.min(vsd_error[:, :kk], 1)
+            final_scores[f"top {kk}, vsd_median"] = np.median(best_vsd)
+            for threshold in [0.3]:
+                final_scores[f"top {kk}, vsd_scores {threshold}"] = np.mean((best_vsd <= threshold) * 100.0)
+        self.log_score(final_scores, split_name=f"val_{data_name}")
+        if save_path is not None:
+            os.makedirs(os.path.dirname(os.path.abspath(save_path)), exist_ok=True)
+            np.save(save_path, vsd_error[:, 0])
+        return final_scores
+
+    def _grid_rotations(self, batch, B):
+        """the grid retrieval's top-5 rotations template_poses[nearest_idx] [B, 5, 3, 3] float32 (model.py:469-509)"""
+        _, nearest_idx, _ = self.predict_pose(batch["query"], batch["reference"], batch["all_relativeR"], None, k=5)
         dev = nearest_idx.device
-        # model.py:469-509: predicted rotations with the ground-truth translation, and the ground-truth pose
         tp = batch["template_poses"].to(dev, torch.float32)
         k = nearest_idx.shape[1]
-        R = tp[torch.arange(B, device=dev)[:, None].expand(B, k), nearest_idx]                 # [B, k, 3, 3]
+        return tp[torch.arange(B, device=dev)[:, None].expand(B, k), nearest_idx]
+
+    def _render_frames(self, batch, B, ids, R):
+        """The sensor depth of every frame and the model rendered at the ground-truth pose and at the rotations R
+        [B, k, 3, 3] with the ground-truth translation: -> (depth_test [B, H, W] float64, rendered [B, 1 + k, H, W],
+        K [B, 3, 3] float64 on the host, K4 [B, 4] on the device)."""
+        import numpy as np
+        from . import vsd as _vsd
+        dev = self.device
+        k = R.shape[1]
         t = batch["query_translation"].to(dev, torch.float32)                                  # [B, 3, 1]
         poses = torch.zeros((B, 1 + k, 4, 4), device=dev, dtype=torch.float32)
         poses[:, 0, :3, :3] = batch["query_pose"].to(dev, torch.float32)
@@ -461,18 +488,73 @@ class PoseConditional:
         K4 = K4.pin_memory().to(dev, non_blocking=True)
         rendered = torch.stack([_vsd.render_depth(self.tless_cad[ids[b]], poses[b], K[b], (H, W))
                                 for b in range(B)])                                            # [B, 1 + k, H, W]
-        vsd_error = _vsd.vsd_errors(depth_test, rendered[:, 0], rendered[:, 1:], K4)
-        vsd_error = vsd_error.cpu().numpy()                                                    # B x k
+        return depth_test, rendered, K, K4
+
+    # ------------------------------------------------------------------ BOP 2019 average recall (DESIGN.md section 15)
+    def load_models_info(self, path):
+        """A BOP models_info.json: the diameter (mm) and the symmetry transforms [S, 3, 4] of every object, in
+        self.bop_models[obj_id] = {"diameter", "symmetries"}."""
+        from . import bop
+        for obj_id, info in bop.load_models_info(path).items():
+            self.bop_models[obj_id] = {"diameter": info["diameter"], "symmetries": bop.symmetry_transformations(info)}
+        return self
+
+    @torch.no_grad()
+    def eval_bop(self, batch, data_name, R_est=None, save_path=None):
+        """BOP 2019 average recall of a T-LESS batch (the `eval_vsd` schema): the grid retrieval's top-5 rotations, or
+        R_est [B, k, 3, 3] from any search, at the ground-truth translation.  Each frame is rendered once (ground
+        truth and k estimates); one multi-tau VSD call (tau = 0.05 ... 0.5 x diameter) and one pose_errors call per
+        distinct object.  Logs and returns {"top kk, ar_vsd" / "ar_mssd" / "ar_mspd" / "ar"} for kk in {1, 3, 5}
+        (up to k): the per-metric minimum over the first kk estimates; kk = 1 is the BOP figure.  Saves the errors
+        (vsd [B, k, 10], mssd [B, k], mspd [B, k], obj_id [B]) to save_path (.npz) when given."""
+        import numpy as np
+        from . import bop
+        from . import vsd as _vsd
+        B, ids = self._check_vsd_batch(batch)
+        missing = sorted(set(i for i in ids if i not in self.bop_models))
+        if missing:
+            raise ValueError(f"eval_bop: no models_info entry for obj_id {missing} (load_models_info)")
+        if R_est is None:
+            R = self._grid_rotations(batch, B)
+        else:
+            R = torch.as_tensor(np.asarray(R_est) if not torch.is_tensor(R_est) else R_est)
+            if R.dim() != 4 or R.shape[0] != B or R.shape[2:] != (3, 3) or R.shape[1] < 1:
+                raise ValueError(f"eval_bop: R_est [B, k, 3, 3] with B = {B} expected, got {tuple(R.shape)}")
+            R = R.to(self.device)
+        k = R.shape[1]
+        depth_test, rendered, K, K4 = self._render_frames(batch, B, ids, R)
+        W = depth_test.shape[2]
+        dev = rendered.device
+        vsd = torch.empty((B, k, len(bop.VSD_TAUS)), device=dev, dtype=torch.float64)
+        mssd = torch.empty((B, k), device=dev, dtype=torch.float64)
+        mspd = torch.empty((B, k), device=dev, dtype=torch.float64)
+        gt = torch.cat([batch["query_pose"].detach().to(torch.float64).reshape(B, 3, 3),
+                        batch["query_translation"].detach().to(torch.float64).reshape(B, 3, 1)], dim=2)
+        gt = gt.pin_memory().to(dev, non_blocking=True) if gt.device.type == "cpu" else gt.to(dev)
+        R_gt, t_gt = gt[:, :, :3], gt[:, :, 3]
+        diameter = np.array([self.bop_models[i]["diameter"] for i in ids])
+        for obj in sorted(set(ids)):
+            rows = [b for b in range(B) if ids[b] == obj]
+            ri = torch.tensor(rows, dtype=torch.int64)
+            rd = ri.pin_memory().to(dev, non_blocking=True)
+            info = self.bop_models[obj]
+            vsd[rd] = _vsd.vsd_errors(depth_test[rd], rendered[rd, 0], rendered[rd, 1:], K[ri],
+                                      tau=bop.VSD_TAUS * info["diameter"])
+            e_mssd, e_mspd = bop.pose_errors(self.tless_cad[obj].vertices, R[rd], t_gt[rd], R_gt[rd], t_gt[rd], K[ri],
+                                             info["symmetries"])
+            mssd[rd], mspd[rd] = e_mssd, e_mspd
+        vsd, mssd, mspd = vsd.cpu().numpy(), mssd.cpu().numpy(), mspd.cpu().numpy()
         final_scores = {}
         for kk in [1, 3, 5]:
-            best_vsd = np.min(vsd_error[:, :kk], 1)
-            final_scores[f"top {kk}, vsd_median"] = np.median(best_vsd)
-            for threshold in [0.3]:
-                final_scores[f"top {kk}, vsd_scores {threshold}"] = np.mean((best_vsd <= threshold) * 100.0)
+            if kk > k:
+                continue
+            ar = bop.average_recall(vsd[:, :kk], mssd[:, :kk], mspd[:, :kk], diameter, W)
+            for name, value in ar.items():
+                final_scores[f"top {kk}, {name}"] = value
         self.log_score(final_scores, split_name=f"val_{data_name}")
         if save_path is not None:
             os.makedirs(os.path.dirname(os.path.abspath(save_path)), exist_ok=True)
-            np.save(save_path, vsd_error[:, 0])
+            np.savez(save_path, vsd=vsd, mssd=mssd, mspd=mspd, obj_id=np.array(ids))
         return final_scores
 
     def test_step(self, batch, idx_batch):

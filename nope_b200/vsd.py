@@ -11,6 +11,7 @@ from . import _lib
 
 COST_TYPES = {"step": 0, "tlinear": 1}          # NOPE_VSD_* of include/nope_b200.h
 MAX_SIDE = 8192
+MAX_TAUS = 16                                   # tolerances of one multi-tau VSD pass
 
 _PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2",
               "ushort": "u2", "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4",
@@ -226,11 +227,15 @@ def vsd_errors(depth_test, depth_gt, depth_est, K, delta=15, tau=20, cost_type="
       depth_gt   [F, H, W] float32 (the model rendered at the ground-truth pose),
       depth_est  [F, P, H, W] float32 (the model rendered at the estimated poses),
       K          [F, 3, 3] or [F, 4] (fx, fy, cx, cy), float64.
-    delta, tau and cost_type default to vsd_obj's.  The three depth tensors must be on one CUDA device."""
+    delta, tau and cost_type default to vsd_obj's.  The three depth tensors must be on one CUDA device.
+    A 1-D `tau` of T <= 16 tolerances scores all of them in one pass and returns [F, P, T]; entry [..., j] equals the
+    scalar call at tau[j] bit for bit.  K is then read on the host (DESIGN.md section 15)."""
     if cost_type not in COST_TYPES:
         raise ValueError(f"unknown cost_type {cost_type!r} (supported: {sorted(COST_TYPES)})")
     if not float(delta) >= 0:
         raise ValueError(f"delta must be >= 0, got {delta}")
+    if np.ndim(tau) == 1:
+        return _vsd_errors_taus(depth_test, depth_gt, depth_est, K, delta, tau, cost_type)
     if not float(tau) > 0:
         raise ValueError(f"tau must be > 0, got {tau}")
     if depth_test.dim() != 3 or depth_gt.shape != depth_test.shape or depth_est.dim() != 4 or \
@@ -258,4 +263,41 @@ def vsd_errors(depth_test, depth_gt, depth_est, K, delta=15, tau=20, cost_type="
         _lib.check(_lib.load().nope_vsd_error(
             _lib.ptr(dt), _lib.ptr(dg), _lib.ptr(de), F_, P, H, W, _lib.ptr(k), float(delta), float(tau),
             COST_TYPES[cost_type], _lib.ptr(out), _stream(dev)))
+    return out
+
+
+def _vsd_errors_taus(depth_test, depth_gt, depth_est, K, delta, tau, cost_type):
+    taus = np.asarray(tau.detach().cpu() if torch.is_tensor(tau) else tau, dtype=np.float64)
+    if not 1 <= len(taus) <= MAX_TAUS:
+        raise ValueError(f"1 to {MAX_TAUS} tolerances expected, got {len(taus)}")
+    if not (np.isfinite(taus).all() and (taus > 0).all()):
+        raise ValueError(f"every tau must be finite and > 0, got {taus.tolist()}")
+    if depth_test.dim() != 3 or depth_gt.shape != depth_test.shape or depth_est.dim() != 4 or \
+            depth_est.shape[0] != depth_test.shape[0] or depth_est.shape[2:] != depth_test.shape[1:]:
+        raise ValueError(f"depth_test [F, H, W], depth_gt [F, H, W] and depth_est [F, P, H, W] expected, got "
+                         f"{tuple(depth_test.shape)}, {tuple(depth_gt.shape)}, {tuple(depth_est.shape)}")
+    F_, P, H, W = depth_est.shape
+    if F_ < 1 or P < 1:
+        raise ValueError("empty batch")
+    _image_size((H, W))
+    dev = depth_est.device
+    if dev.type != "cuda" or depth_gt.device != dev or depth_test.device != dev:
+        raise _lib.NopeError("vsd_errors needs the three depth tensors on one CUDA device (no CPU fallback)")
+    K = torch.as_tensor(np.asarray(K) if not torch.is_tensor(K) else K).detach().cpu().to(torch.float64)
+    if K.dim() == 3 and K.shape[1:] == (3, 3):
+        K = torch.stack([K[:, 0, 0], K[:, 1, 1], K[:, 0, 2], K[:, 1, 2]], dim=1)
+    if K.shape != (F_, 4):
+        raise ValueError(f"K [F, 3, 3] or [F, 4] with F = {F_} expected, got {tuple(K.shape)}")
+    k = K.contiguous()
+    if not torch.isfinite(k).all() or (k[:, :2] == 0).any():
+        raise ValueError("intrinsics must be finite with fx and fy non-zero")
+    taus = np.ascontiguousarray(taus)
+    dt = depth_test.to(torch.float64).contiguous()
+    dg = depth_gt.to(torch.float32).contiguous()
+    de = depth_est.to(torch.float32).contiguous()
+    out = torch.empty((F_, P, len(taus)), device=dev, dtype=torch.float64)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().nope_vsd_error_taus(
+            _lib.ptr(dt), _lib.ptr(dg), _lib.ptr(de), F_, P, H, W, k.data_ptr(), float(delta), COST_TYPES[cost_type],
+            taus.ctypes.data, len(taus), _lib.ptr(out), _stream(dev)))
     return out
