@@ -193,6 +193,31 @@ int nope_inplane_rotate_pairs(const float* images, int B, int H, int W, const in
 int nope_encoder_encode_rotated(nope_encoder_t* e, const float* images, int B, const int32_t* image_idx,
                                 const float* cossin, int P, float* out, void* stream);
 
+/* Stable Diffusion VAE encoder (DESIGN.md section 16): AutoencoderKL.encode(x).latent_dist.mode() * 0.18215 of the
+ * SD v1 configuration (block_out_channels 128, 256, 512, 512; two resnets per block; GroupNorm(32, eps 1e-6); one
+ * 512-channel attention head; latent_channels 4), the encoder of the LDM variant and of vae_base.yaml.
+ * Convolutions run on the wgmma kernel with split-precision (fp16 hi + lo) operands; the attention core in fp32.
+ * nope_vae_load_tensor takes the diffusers state_dict names with the 0.14-era attention projections
+ * (`encoder.mid_block.attentions.0.{query,key,value,proj_attn}`), HOST fp32 pointers, shape-checked; every key of
+ * the schema is required by nope_vae_finalize, which also allocates the workspace (16 images, ~3.2 GB).
+ * Encode calls: images [B, 3, 256, 256] fp32 NCHW (device) in [-1, 1]; any B >= 1, 16 images at a time, and a latent
+ * does not depend on the batch it was encoded in.  nope_vae_encode -> out [B, 4, 32, 32];
+ * nope_vae_encode_inplane (1 <= A <= 360, cossin [A, 2]) -> out [B, A, 4, 32, 32] and nope_vae_encode_rotated
+ * (1 <= P < 2^30, image_idx [P] int32, cossin [P, 2]) -> out [P, 4, 32, 32] rotate exactly as
+ * nope_encoder_encode_inplane / nope_encoder_encode_rotated and equal nope_vae_encode of the rotated batch.  Bad
+ * arguments are refused before any CUDA call; no call synchronises the host. */
+typedef struct nope_vae nope_vae_t;
+int nope_vae_create(nope_vae_t** out, int device);
+void nope_vae_destroy(nope_vae_t* v);
+int nope_vae_load_tensor(nope_vae_t* v, const char* key, const float* data, const int64_t* shape, int ndim);
+int nope_vae_finalize(nope_vae_t* v);
+int nope_vae_encode(nope_vae_t* v, const float* images, int B, float* out, void* stream);
+int nope_vae_encode_inplane(nope_vae_t* v, const float* images, int B, const float* cossin, int A, float* out,
+                            void* stream);
+int nope_vae_encode_rotated(nope_vae_t* v, const float* images, int B, const int32_t* image_idx, const float* cossin,
+                            int P, float* out, void* stream);
+int64_t nope_vae_last_launch_count(const nope_vae_t* v);
+
 /* T-LESS evaluation (DESIGN.md section 12): a depth rasterizer standing in for pyrender's DEPTH_ONLY render and the
  * VSD error of src/poses/vsd.py:92-135 (visibility mode "bop19", src/poses/vsd_utils.py).  Both calls refuse bad
  * arguments before any CUDA call and do not synchronise.

@@ -48,7 +48,16 @@ SIGNATURES = {
                                             C.c_void_p]),
     "nope_encoder_encode_rotated": (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_void_p, c_f32p, C.c_int, c_f32p,
                                               C.c_void_p]),
-    "nope_render_depth": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_int, C.c_float, C.c_float,
+    "nope_vae_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int]),
+    "nope_vae_destroy": (None, [C.c_void_p]),
+    "nope_vae_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.POINTER(C.c_int64), C.c_int]),
+    "nope_vae_finalize": (C.c_int, [C.c_void_p]),
+    "nope_vae_encode": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_void_p]),
+    "nope_vae_encode_inplane": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, C.c_void_p]),
+    "nope_vae_encode_rotated": (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_void_p, c_f32p, C.c_int, c_f32p,
+                                          C.c_void_p]),
+    "nope_vae_last_launch_count": (C.c_int64, [C.c_void_p]),
+    "nope_render_depth":(C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_int, C.c_float, C.c_float,
                                     C.c_float, C.c_float, C.c_float, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     "nope_vsd_error": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                  C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p]),

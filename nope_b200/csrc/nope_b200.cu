@@ -22,6 +22,7 @@
 #include "kernels.cuh"
 #include "linattn_tc.cuh"
 #include "encoder.cuh"
+#include "vae.cuh"
 #include "ldm.cuh"
 #include "render.cuh"
 #include "pose_error.cuh"
@@ -1619,6 +1620,89 @@ int nope_encoder_encode_rotated(nope_encoder_t* e, const float* images, int B, c
 }
 
 int64_t nope_encoder_last_launch_count(const nope_encoder_t* e) { return e ? e->launches : 0; }
+
+// ---------------------------------------------------------------------------------
+// Stable Diffusion VAE encoder (vae.cuh, DESIGN.md section 16)
+// ---------------------------------------------------------------------------------
+int nope_vae_create(nope_vae_t** out, int device) {
+  NOPE_CHECK(out != nullptr, "null out pointer");
+  int ndev = 0;
+  NOPE_CUDA(cudaGetDeviceCount(&ndev));
+  NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
+  cudaDeviceProp prop;
+  NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
+  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
+  auto v = std::make_unique<nope_vae>();
+  v->device = device;
+  v->num_sms = prop.multiProcessorCount;
+  v->build_schema();
+  *out = v.release();
+  return 0;
+}
+
+void nope_vae_destroy(nope_vae_t* v) { delete v; }
+
+int nope_vae_load_tensor(nope_vae_t* v, const char* key, const float* data, const int64_t* shape, int ndim) {
+  NOPE_CHECK(v && key && data && shape, "null argument");
+  NOPE_CHECK(!v->finalized, "VAE already finalized");
+  auto it = v->expected.find(key);
+  NOPE_CHECK(it != v->expected.end(), std::string("unexpected VAE state_dict key: ") + key);
+  NOPE_CHECK((int)it->second.size() == ndim, std::string("rank mismatch for ") + key);
+  size_t n = 1;
+  for (int i = 0; i < ndim; ++i) {
+    NOPE_CHECK(it->second[i] == shape[i], std::string("shape mismatch for ") + key);
+    n *= (size_t)shape[i];
+  }
+  auto& slot = v->host[key];
+  slot.first.assign(shape, shape + ndim);
+  slot.second.assign(data, data + n);
+  return 0;
+}
+
+int nope_vae_finalize(nope_vae_t* v) {
+  NOPE_CHECK(v, "null VAE");
+  return v->finalize();
+}
+
+int nope_vae_encode(nope_vae_t* v, const float* images, int B, float* out, void* stream) {
+  NOPE_CHECK(images && out, "null images / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(v && v->finalized, "VAE not finalized");
+  NOPE_CUDA(cudaSetDevice(v->device));
+  constexpr int kChunk = nope_vae::kChunk;
+  int64_t launches = 0;
+  for (int lo = 0; lo < B; lo += kChunk) {
+    const int n = B - lo < kChunk ? B - lo : kChunk;
+    const int rc = v->encode(images + (size_t)lo * 3 * 256 * 256, n, out + (size_t)lo * 4 * 32 * 32,
+                             static_cast<cudaStream_t>(stream));
+    if (rc != 0) return rc;
+    launches += v->launches;
+  }
+  v->launches = launches;
+  return 0;
+}
+
+int nope_vae_encode_inplane(nope_vae_t* v, const float* images, int B, const float* cossin, int A, float* out,
+                            void* stream) {
+  NOPE_CHECK(images && cossin && out, "null images / cossin / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(A >= 1 && A <= 360, "A (in-plane angles) must be in [1, 360]");
+  NOPE_CHECK(v && v->finalized, "VAE not finalized");
+  NOPE_CUDA(cudaSetDevice(v->device));
+  return v->encode_inplane(images, B, cossin, A, out, static_cast<cudaStream_t>(stream));
+}
+
+int nope_vae_encode_rotated(nope_vae_t* v, const float* images, int B, const int32_t* image_idx, const float* cossin,
+                            int P, float* out, void* stream) {
+  NOPE_CHECK(images && image_idx && cossin && out, "null images / image_idx / cossin / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(P >= 1 && P <= INT32_MAX / 2, "P (pairs) must be in [1, 2^30)");
+  NOPE_CHECK(v && v->finalized, "VAE not finalized");
+  NOPE_CUDA(cudaSetDevice(v->device));
+  return v->encode_rotated(images, B, image_idx, cossin, P, out, static_cast<cudaStream_t>(stream));
+}
+
+int64_t nope_vae_last_launch_count(const nope_vae_t* v) { return v ? v->launches : 0; }
 
 // ---------------------------------------------------------------------------------
 // T-LESS evaluation: depth rasterizer and VSD (render.cuh, DESIGN.md section 12)

@@ -1,0 +1,738 @@
+// nope_b200 -- Stable Diffusion VAE encoder (diffusers AutoencoderKL, SD v1 configuration), fp32-accurate.
+//
+// latent = AutoencoderKL.encode(x).latent_dist.mode() * 0.18215 for x [B, 3, 256, 256] in [-1, 1]
+// (DESIGN.md section 16): conv_in 3x3 (3 -> 128); four down blocks of two ResnetBlock2D each
+// (128, 256, 512, 512 channels; blocks 0-2 end in pad (0, 1, 0, 1) + 3x3 stride-2 conv); the mid block
+// (ResnetBlock2D, one-head self-attention over 32x32 tokens, ResnetBlock2D); GroupNorm(32) + SiLU, conv_out
+// 3x3 (512 -> 8) and quant_conv 1x1, of which the four mean channels are kept.
+//
+// Precision follows encoder.cuh: every convolution runs on the wgmma kernel (conv_tc2.cuh, the EXTRAS epilogue
+// the template encoder already instantiates) with split-precision fp16 (hi, lo) operands -- three K-segments per
+// filter tap.  GroupNorm statistics come from the fp32 outputs in a separate pass that sums in float64, per image
+// in a fixed order, so they do not depend on the batch or the chunk.  The residual stream is kept as fp32 (for
+// the statistics) and as (hi, lo) (for the identity shortcut, added in the conv2 epilogue, and for the 1x1
+// shortcut, extra K-segments of conv2).  The attention core (q k^T, softmax, p v) runs on CUDA cores in fp32.
+//
+// The 256 x 256 level is wider than one 128-pixel tile row, which the convolution's tile geometry requires.
+// Its activations are therefore stored parity-planar: plane (py, px) = 2 py + px holds the pixels (2 Y + py,
+// 2 X + px) of every image of the chunk as a [cap, 128, 128, C] NHWC tensor.  A 3x3 convolution at that level is
+// four launches, one per output plane, each reading the four input planes with the tap offsets of its parity;
+// the stride-2 downsample reads the planes as the four sub-lattices of its input.
+#pragma once
+#include "conv_tc2.cuh"
+#include "encoder.cuh"
+
+#include <cmath>
+#include <map>
+#include <string>
+#include <tuple>
+#include <vector>
+
+namespace nope {
+
+constexpr int kVaeSlab = 1024;   // pixels per GroupNorm partial sum (divides every level's H*W per plane)
+
+// conv_in: 3x3 pad 1 (3 -> 128), fp32 direct, -> parity-planar fp32 + (hi, lo).  w: [128][3][3][3] fp32.
+// Block = 128 output channels x 2 pixels.
+__global__ void __launch_bounds__(256)
+vae_conv_in_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
+                   float* __restrict__ out32, __half* __restrict__ out_hi, __half* __restrict__ out_lo, int n,
+                   int cap) {
+  __shared__ float s_w[128 * 27];
+  for (int i = threadIdx.x; i < 128 * 27; i += 256) s_w[i] = w[i];
+  __syncthreads();
+  const int o = threadIdx.x & 127;
+  const int pix = blockIdx.x * 2 + (threadIdx.x >> 7);
+  if (pix >= n * 65536) return;
+  const int b = pix >> 16, y = (pix >> 8) & 255, xx = pix & 255;
+  float acc = bias[o];
+  for (int c = 0; c < 3; ++c)
+    for (int ky = 0; ky < 3; ++ky) {
+      const int yy = y + ky - 1;
+      if (yy < 0 || yy > 255) continue;
+      const float* xr = x + (((size_t)b * 3 + c) * 256 + yy) * 256;
+      const float* wr = s_w + o * 27 + (c * 3 + ky) * 3;
+#pragma unroll
+      for (int kx = 0; kx < 3; ++kx) {
+        const int xc = xx + kx - 1;
+        if (xc >= 0 && xc < 256) acc = fmaf(xr[xc], wr[kx], acc);
+      }
+    }
+  const size_t plane = (size_t)((y & 1) * 2 + (xx & 1));
+  const size_t dst = (((plane * cap + b) * 128 + (y >> 1)) * 128 + (xx >> 1)) * 128 + o;
+  out32[dst] = acc;
+  const __half hi = __float2half_rn(acc);
+  out_hi[dst] = hi;
+  out_lo[dst] = __float2half_rn(acc - __half2float(hi));
+}
+
+// GroupNorm(32) partial sums of fp32 NHWC activations: image b's pixels lie in `planes` planes of [cap, hw, C]
+// (plane q of image b at x + (q * cap + b) * hw * C).  grid (planes * hw / kVaeSlab, n): block s sums slab s of
+// image b in float64 in a fixed order -> part[(b * gridDim.x + s) * 32 + g] = (sum, sum of squares) of group g.
+// C in {128, 256, 512}: a thread owns one 4-channel quad (groups have 4, 8 or 16 channels).
+__global__ void __launch_bounds__(256)
+vae_gn_partial_kernel(const float* __restrict__ x, int C, int hw, int cap, double2* __restrict__ part) {
+  __shared__ double s1[256], s2[256];
+  const int b = blockIdx.y, spp = hw / kVaeSlab;
+  const int q = blockIdx.x / spp, s0 = (blockIdx.x - q * spp) * kVaeSlab;
+  const float* base = x + (((size_t)q * cap + b) * hw + s0) * C;
+  const int quads = C >> 2, rows = 256 / quads;
+  const int qd = threadIdx.x % quads, r = threadIdx.x / quads;
+  double a = 0.0, a2 = 0.0;
+  for (int p = r; p < kVaeSlab; p += rows) {
+    const float4 v = *reinterpret_cast<const float4*>(base + (size_t)p * C + qd * 4);
+    const double v0 = v.x, v1 = v.y, v2 = v.z, v3 = v.w;
+    a += (v0 + v1) + (v2 + v3);
+    a2 += (v0 * v0 + v1 * v1) + (v2 * v2 + v3 * v3);
+  }
+  s1[threadIdx.x] = a;
+  s2[threadIdx.x] = a2;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    const int g = threadIdx.x, qpg = quads / 32;
+    double t = 0.0, t2 = 0.0;
+    for (int rr = 0; rr < rows; ++rr)
+      for (int k = 0; k < qpg; ++k) {
+        const int i = rr * quads + g * qpg + k;
+        t += s1[i];
+        t2 += s2[i];
+      }
+    part[((size_t)b * gridDim.x + blockIdx.x) * 32 + g] = make_double2(t, t2);
+  }
+}
+
+// (mean, rstd) of every (image, group) from the partial sums, in slab order.  grid n, 32 threads.
+__global__ void __launch_bounds__(32)
+vae_gn_finalize_kernel(const double2* __restrict__ part, int nparts, double inv_cnt, double eps,
+                       float2* __restrict__ stats) {
+  const int b = blockIdx.x, g = threadIdx.x;
+  double t = 0.0, t2 = 0.0;
+  for (int k = 0; k < nparts; ++k) {
+    const double2 v = part[((size_t)b * nparts + k) * 32 + g];
+    t += v.x;
+    t2 += v.y;
+  }
+  const double mean = t * inv_cnt;
+  double var = t2 * inv_cnt - mean * mean;
+  if (var < 0.0) var = 0.0;
+  // 1 / sqrt(var + eps): rsqrtf refined by one Newton step in float64 (no call to the IEEE slow paths)
+  const double v = var + eps, r0 = (double)rsqrtf((float)v);
+  stats[b * 32 + g] = make_float2((float)mean, (float)(r0 * (1.5 - 0.5 * v * r0 * r0)));
+}
+
+// y = [SiLU]((x - mean) * rstd * gamma + beta) -> (hi, lo), same layout as x; 4 channels per thread.
+// grid (ceil(hw * C / 1024), planes * n): blockIdx.y = q * n + b is image b of plane q (its cap slots hold the n
+// images of the chunk first).
+__global__ void __launch_bounds__(256)
+vae_gn_apply_kernel(const float* __restrict__ x, const float2* __restrict__ stats, const float* __restrict__ gamma,
+                    const float* __restrict__ beta, int C, int hw, int n, int cap, int silu,
+                    __half* __restrict__ out_hi, __half* __restrict__ out_lo) {
+  const int quads = C >> 2;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= hw * quads) return;
+  const int q = (int)blockIdx.y / n, b = (int)blockIdx.y - q * n;
+  const int c4 = i % quads;
+  const size_t off = ((size_t)q * cap + b) * hw * quads + i;
+  const float4 v = reinterpret_cast<const float4*>(x)[off];
+  const float2 ms = stats[b * 32 + c4 * 4 / (C >> 5)];
+  const float4 ga = reinterpret_cast<const float4*>(gamma)[c4];
+  const float4 be = reinterpret_cast<const float4*>(beta)[c4];
+  float y[4] = {(v.x - ms.x) * ms.y * ga.x + be.x, (v.y - ms.x) * ms.y * ga.y + be.y,
+                (v.z - ms.x) * ms.y * ga.z + be.z, (v.w - ms.x) * ms.y * ga.w + be.w};
+  if (silu) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) y[k] = __fdividef(y[k], 1.f + expf(-y[k]));
+  }
+  float l[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) l[k] = y[k] - __half2float(__float2half_rn(y[k]));
+  reinterpret_cast<uint2*>(out_hi)[off] = make_uint2(pack_half2(y[0], y[1]), pack_half2(y[2], y[3]));
+  reinterpret_cast<uint2*>(out_lo)[off] = make_uint2(pack_half2(l[0], l[1]), pack_half2(l[2], l[3]));
+}
+
+// Batched fp32 GEMM of the attention core, one image per blockIdx.z, 64 x 64 tile per block, 4 x 4 per thread,
+// every output summed over k in ascending order:
+//   C[m, j] = alpha * sum_k A[m, k] B(k, j),  B(k, j) = Bm[j * ldb + k] (KT) or Bm[k * ldb + j].
+// SPLIT stores (hi, lo) halves, else fp32.  M, N multiples of 64, K a multiple of 16.
+template <bool KT, bool SPLIT>
+__global__ void __launch_bounds__(256)
+vae_attn_gemm_kernel(const float* __restrict__ A, int lda, long long sa, const float* __restrict__ Bm, int ldb,
+                     long long sb, int K, float alpha, float* __restrict__ C32, __half* __restrict__ Chi,
+                     __half* __restrict__ Clo, int ldc, long long sc) {
+  __shared__ float As[16][64 + 4], Bs[16][64 + 4];
+  const int t = threadIdx.x, tx = t & 15, ty = t >> 4;
+  const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
+  A += blockIdx.z * sa;
+  Bm += blockIdx.z * sb;
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+  for (int k0 = 0; k0 < K; k0 += 16) {
+#pragma unroll
+    for (int l = t; l < 1024; l += 256) {
+      const int m = l >> 4, k = l & 15;
+      As[k][m] = A[(size_t)(m0 + m) * lda + k0 + k];
+      if (KT) {
+        Bs[k][m] = Bm[(size_t)(n0 + m) * ldb + k0 + k];
+      } else {
+        const int kk = l >> 6, j = l & 63;
+        Bs[kk][j] = Bm[(size_t)(k0 + kk) * ldb + n0 + j];
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+      float a[4], bv[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[i] = As[k][ty + 16 * i];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) bv[j] = Bs[k][tx + 16 * j];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], bv[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const size_t o = blockIdx.z * sc + (size_t)(m0 + ty + 16 * i) * ldc + n0 + tx + 16 * j;
+      const float v = acc[i][j] * alpha;
+      if (SPLIT) {
+        const __half hi = __float2half_rn(v);
+        Chi[o] = hi;
+        Clo[o] = __float2half_rn(v - __half2float(hi));
+      } else {
+        C32[o] = v;
+      }
+    }
+}
+
+// Row softmax in place over rows of 1024 fp32 scores: exp(s - max) / sum, both reductions in a fixed tree order.
+__global__ void __launch_bounds__(256) vae_softmax_kernel(float* __restrict__ s) {
+  __shared__ float red[8];
+  float* row = s + (size_t)blockIdx.x * 1024;
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  float v[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) v[k] = row[t + 256 * k];
+  float m = fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (lane == 0) red[w] = m;
+  __syncthreads();
+  m = red[0];
+#pragma unroll
+  for (int k = 1; k < 8; ++k) m = fmaxf(m, red[k]);
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) v[k] = expf(v[k] - m);
+  float sum = (v[0] + v[1]) + (v[2] + v[3]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  if (lane == 0) red[w] = sum;
+  __syncthreads();
+  sum = ((red[0] + red[1]) + (red[2] + red[3])) + ((red[4] + red[5]) + (red[6] + red[7]));
+#pragma unroll
+  for (int k = 0; k < 4; ++k) row[t + 256 * k] = __fdividef(v[k], sum);
+}
+
+// A convolution of the VAE: packed split-precision weights [cout][K] fp16, K = taps x (W_hi | W_lo | W_hi) x cin,
+// then, for a ResnetBlock2D conv2 with a 1x1 shortcut, (S_hi | S_lo | S_hi) x cin_sc; bias = b2 (+ b_shortcut).
+struct VaeConv {
+  int cin = 0, cin_sc = 0, cout = 0, k = 1, K = 0, bn = 0;
+  __half* w = nullptr;
+  float* bias = nullptr;
+  CUtensorMap wmap;
+};
+
+struct VaeNorm {
+  float* gamma = nullptr;
+  float* beta = nullptr;
+};
+
+// One tap of a convolution: input pair (hi map 2 * pair, lo map 2 * pair + 1) at offset (dy, dx).
+struct VaeTap {
+  int pair, dy, dx;
+};
+
+}  // namespace nope
+
+struct nope_vae {
+  static constexpr int kChunk = 16;           // images per pass: the workspace holds this many (~200 MB each)
+  static constexpr int kCh[4] = {128, 256, 512, 512};
+  int device = 0, num_sms = 132;
+  bool finalized = false;
+  std::map<std::string, std::pair<std::vector<int64_t>, std::vector<float>>> host;
+  std::map<std::string, std::vector<int64_t>> expected;
+  std::map<std::string, nope::VaeConv> convs;
+  std::map<std::string, nope::VaeNorm> norms;
+  float *in_w = nullptr, *in_b = nullptr;
+  std::vector<void*> owned;
+  // workspace, each buffer sized for kChunk images of the 256 x 256 x 128 level
+  float* x32[2] = {nullptr, nullptr};         // residual stream, fp32
+  nope::ActPair xs[2];                        // residual stream, (hi, lo)
+  nope::ActPair nrm;                          // normalised activations / attention output, (hi, lo)
+  float* t32 = nullptr;                       // conv1 / qkv / conv_out output, fp32
+  double2* gn_part = nullptr;                 // GroupNorm partial sums
+  float2* gn_stats = nullptr;                 // GroupNorm (mean, rstd)
+  float* rot_stage = nullptr;                 // kChunk rotated crops
+  std::map<std::tuple<const void*, int, int, int>, CUtensorMap> tmaps;
+  int64_t launches = 0;
+
+  ~nope_vae() {
+    for (void* p : owned) cudaFree(p);
+  }
+
+  // ---------------------------------------------------------------- schema (diffusers AutoencoderKL, SD v1)
+  void expect_norm(const std::string& p, int c) {
+    expected[p + ".weight"] = {c};
+    expected[p + ".bias"] = {c};
+  }
+  void expect_conv(const std::string& p, int cout, int cin, int k) {
+    expected[p + ".weight"] = {cout, cin, k, k};
+    expected[p + ".bias"] = {cout};
+  }
+  void expect_resnet(const std::string& p, int cin, int cout) {
+    expect_norm(p + ".norm1", cin);
+    expect_conv(p + ".conv1", cout, cin, 3);
+    expect_norm(p + ".norm2", cout);
+    expect_conv(p + ".conv2", cout, cout, 3);
+    if (cin != cout) expect_conv(p + ".conv_shortcut", cout, cin, 1);
+  }
+  void build_schema() {
+    expect_conv("encoder.conv_in", 128, 3, 3);
+    int cin = 128;
+    for (int i = 0; i < 4; ++i) {
+      for (int j = 0; j < 2; ++j) {
+        expect_resnet("encoder.down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), cin, kCh[i]);
+        cin = kCh[i];
+      }
+      if (i < 3) expect_conv("encoder.down_blocks." + std::to_string(i) + ".downsamplers.0.conv", kCh[i], kCh[i], 3);
+    }
+    for (int j = 0; j < 2; ++j) expect_resnet("encoder.mid_block.resnets." + std::to_string(j), 512, 512);
+    const std::string a = "encoder.mid_block.attentions.0.";
+    expect_norm(a + "group_norm", 512);
+    for (const char* s : {"query", "key", "value", "proj_attn"}) {
+      expected[a + s + ".weight"] = {512, 512};
+      expected[a + s + ".bias"] = {512};
+    }
+    expect_norm("encoder.conv_norm_out", 512);
+    expect_conv("encoder.conv_out", 8, 512, 3);
+    expect_conv("quant_conv", 8, 8, 1);
+  }
+
+  // ---------------------------------------------------------------- weights
+  template <typename T>
+  int upload(T** dst, const std::vector<T>& v) {
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(dst), v.size() * sizeof(T)));
+    owned.push_back(*dst);
+    NOPE_CUDA(cudaMemcpy(*dst, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    return 0;
+  }
+  const std::vector<float>& h(const std::string& k) { return host.at(k).second; }
+
+  // W [cout_real][cin][k*k], bias [cout_real] (float64), optional 1x1 shortcut Ws [cout_real][cin_sc] + its bias
+  int pack_conv(const std::string& name, int cout_real, int cin, int k, const std::vector<double>& W,
+                const std::vector<double>& bias, int cin_sc = 0, const std::vector<double>* Ws = nullptr) {
+    using namespace nope;
+    VaeConv L;
+    L.cin = cin;
+    L.cin_sc = cin_sc;
+    L.k = k;
+    L.cout = (cout_real + 63) / 64 * 64;
+    const int taps = k * k;
+    L.K = taps * 3 * cin + 3 * cin_sc;
+    NOPE_CHECK(cin % 64 == 0 && cin_sc % 64 == 0, name + ": input channels must be a multiple of 64");
+    L.bn = pick_bn(L.cout);
+    std::vector<__half> packed((size_t)L.cout * L.K, __float2half_rn(0.f));
+    auto put = [&](__half* dst, int c, int stride, double v) {
+      const float wf = (float)v;
+      const __half hi = __float2half_rn(wf);
+      dst[c] = hi;
+      dst[stride + c] = __float2half_rn(wf - __half2float(hi));
+      dst[2 * stride + c] = hi;
+    };
+    for (int o = 0; o < cout_real; ++o) {
+      for (int c = 0; c < cin; ++c)
+        for (int t = 0; t < taps; ++t)
+          put(&packed[(size_t)o * L.K + (size_t)t * 3 * cin], c, cin, W[((size_t)o * cin + c) * taps + t]);
+      for (int c = 0; c < cin_sc; ++c)
+        put(&packed[(size_t)o * L.K + (size_t)taps * 3 * cin], c, cin_sc, (*Ws)[(size_t)o * cin_sc + c]);
+    }
+    std::vector<float> b(L.cout, 0.f);
+    for (int o = 0; o < cout_real; ++o) b[o] = (float)bias[o];
+    if (upload(&L.w, packed) || upload(&L.bias, b)) return -1;
+    if (make_weight_map(&L.wmap, L.w, L.cout, L.K, L.bn)) return -1;
+    convs[name] = L;
+    return 0;
+  }
+  std::vector<double> dvec(const std::string& k) {
+    const auto& v = h(k);
+    return std::vector<double>(v.begin(), v.end());
+  }
+  int make_plain(const std::string& name, int k) {
+    const auto& s = host.at(name + ".weight").first;
+    return pack_conv(name, (int)s[0], (int)s[1], k, dvec(name + ".weight"), dvec(name + ".bias"));
+  }
+  int make_norm(const std::string& name) {
+    nope::VaeNorm N;
+    if (upload(&N.gamma, h(name + ".weight")) || upload(&N.beta, h(name + ".bias"))) return -1;
+    norms[name] = N;
+    return 0;
+  }
+  int make_resnet(const std::string& p, int cin, int cout) {
+    if (make_norm(p + ".norm1") || make_norm(p + ".norm2") || make_plain(p + ".conv1", 3)) return -1;
+    std::vector<double> b = dvec(p + ".conv2.bias");
+    if (cin == cout) return pack_conv(p + ".conv2", cout, cout, 3, dvec(p + ".conv2.weight"), b);
+    const std::vector<double> ws = dvec(p + ".conv_shortcut.weight"), bs = dvec(p + ".conv_shortcut.bias");
+    for (int o = 0; o < cout; ++o) b[o] += bs[o];
+    return pack_conv(p + ".conv2", cout, cout, 3, dvec(p + ".conv2.weight"), b, cin, &ws);
+  }
+
+  int finalize() {
+    using namespace nope;
+    NOPE_CHECK(!finalized, "already finalized");
+    for (const auto& kv : expected) NOPE_CHECK(host.count(kv.first), "state_dict is missing " + kv.first);
+    NOPE_CUDA(cudaSetDevice(device));
+    if (upload(&in_w, h("encoder.conv_in.weight")) || upload(&in_b, h("encoder.conv_in.bias"))) return -1;
+    int cin = 128;
+    for (int i = 0; i < 4; ++i) {
+      const std::string blk = "encoder.down_blocks." + std::to_string(i);
+      for (int j = 0; j < 2; ++j) {
+        if (make_resnet(blk + ".resnets." + std::to_string(j), cin, kCh[i])) return -1;
+        cin = kCh[i];
+      }
+      if (i < 3 && make_plain(blk + ".downsamplers.0.conv", 3)) return -1;
+    }
+    for (int j = 0; j < 2; ++j)
+      if (make_resnet("encoder.mid_block.resnets." + std::to_string(j), 512, 512)) return -1;
+    const std::string a = "encoder.mid_block.attentions.0.";
+    if (make_norm(a + "group_norm")) return -1;
+    {  // q, k, v as one 1x1 convolution 512 -> 1536
+      std::vector<double> W, b;
+      for (const char* s : {"query", "key", "value"}) {
+        const auto w = dvec(a + s + ".weight"), bb = dvec(a + s + ".bias");
+        W.insert(W.end(), w.begin(), w.end());
+        b.insert(b.end(), bb.begin(), bb.end());
+      }
+      if (pack_conv(a + "qkv", 1536, 512, 1, W, b)) return -1;
+    }
+    if (pack_conv(a + "proj_attn", 512, 512, 1, dvec(a + "proj_attn.weight"), dvec(a + "proj_attn.bias"))) return -1;
+    if (make_norm("encoder.conv_norm_out")) return -1;
+    {  // conv_out followed by quant_conv rows 0-3 (the mean) and the 0.18215 scale, folded in float64
+      const auto W = dvec("encoder.conv_out.weight"), b = dvec("encoder.conv_out.bias");
+      const auto Q = dvec("quant_conv.weight"), qb = dvec("quant_conv.bias");
+      constexpr double kScale = 0.18215;
+      std::vector<double> Wf((size_t)4 * 512 * 9, 0.0), bf(4, 0.0);
+      for (int o = 0; o < 4; ++o) {
+        double bo = qb[o];
+        for (int j = 0; j < 8; ++j) {
+          bo += Q[o * 8 + j] * b[j];
+          for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] += Q[o * 8 + j] * W[(size_t)j * 512 * 9 + i];
+        }
+        bf[o] = kScale * bo;
+        for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] *= kScale;
+      }
+      if (pack_conv("conv_out", 4, 512, 3, Wf, bf)) return -1;
+    }
+    host.clear();
+    // workspace for kChunk images, allocated once so that no encode call allocates (or synchronises)
+    const size_t E = (size_t)kChunk * 256 * 256 * 128;
+    for (int s = 0; s < 2; ++s) {
+      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&x32[s]), E * sizeof(float)));
+      owned.push_back(x32[s]);
+      for (__half** p : {&xs[s].hi, &xs[s].lo}) {
+        NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(p), E * sizeof(__half)));
+        owned.push_back(*p);
+      }
+    }
+    for (__half** p : {&nrm.hi, &nrm.lo}) {
+      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(p), E * sizeof(__half)));
+      owned.push_back(*p);
+    }
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&t32), E * sizeof(float)));
+    owned.push_back(t32);
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&gn_part), (size_t)kChunk * 64 * 32 * sizeof(double2)));
+    owned.push_back(gn_part);
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&gn_stats), (size_t)kChunk * 32 * sizeof(float2)));
+    owned.push_back(gn_stats);
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&rot_stage), (size_t)kChunk * 3 * 256 * 256 * sizeof(float)));
+    owned.push_back(rot_stage);
+    finalized = true;
+    return 0;
+  }
+
+  // ---------------------------------------------------------------- launches
+  // NHWC map of `cap` images of side H x H and C channels at base; lattice >= 0: the stride-2 sub-lattice
+  // (lattice >> 1, lattice & 1) of a 2H x 2H tensor
+  int get_map(const CUtensorMap** out, const void* base, int C, int H, int lattice) {
+    using namespace nope;
+    const auto key = std::make_tuple(base, lattice, C, H);
+    auto it = tmaps.find(key);
+    if (it == tmaps.end()) {
+      TileGeom g;
+      if (make_geom(H, H, &g)) return -1;
+      CUtensorMap m;
+      const int rc = lattice < 0 ? make_act_map(&m, base, kChunk, C, g)
+                                 : make_unshuffle_map(&m, base, kChunk, C, g, lattice >> 1, lattice & 1);
+      if (rc) return -1;
+      it = tmaps.emplace(key, m).first;
+    }
+    *out = &it->second;
+    return 0;
+  }
+  // offset of plane q of a parity-planar level-0 tensor with C channels
+  static size_t plane_off(int q, int C) { return (size_t)q * kChunk * 128 * 128 * C; }
+
+  // out = conv(taps over the input pairs `in`) [+ shortcut taps over pair sc] + bias [+ res]; output H x H.
+  // in: (hi, lo) base pointers of each input pair with their lattice (-1: plain NHWC of side H).
+  int conv(const nope::VaeConv& L, const std::vector<std::pair<nope::ActPair, int>>& in, int Hin_map,
+           const std::vector<nope::VaeTap>& taps, int sc_pair, int H, int n, __half* out_hi, __half* out_lo,
+           float* out_f32, const nope::ActPair* res, cudaStream_t st) {
+    using namespace nope;
+    TileGeom g;
+    if (make_geom(H, H, &g)) return -1;
+    ConvParams p;
+    memset(&p, 0, sizeof p);
+    const CUtensorMap* m = nullptr;
+    NOPE_CHECK(in.size() <= (size_t)kMaxAMaps / 2, "vae conv: too many input maps");
+    for (size_t i = 0; i < in.size(); ++i) {
+      const int C = (int)i == sc_pair ? L.cin_sc : L.cin;
+      if (get_map(&m, in[i].first.hi, C, Hin_map, in[i].second)) return -1;
+      p.amap[2 * i] = *m;
+      if (get_map(&m, in[i].first.lo, C, Hin_map, in[i].second)) return -1;
+      p.amap[2 * i + 1] = *m;
+    }
+    p.n_amaps = 2 * (int)in.size();
+    int nseg = 0, ksteps = 0;
+    auto add = [&](const VaeTap& t, int nch) {
+      p.seg[nseg++] = ConvSeg{(int16_t)(2 * t.pair), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};       // A_hi W_hi
+      p.seg[nseg++] = ConvSeg{(int16_t)(2 * t.pair), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};       // A_hi W_lo
+      p.seg[nseg++] = ConvSeg{(int16_t)(2 * t.pair + 1), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};   // A_lo W_hi
+      ksteps += 3 * nch;
+    };
+    for (const VaeTap& t : taps) add(t, L.cin / 64);
+    if (sc_pair >= 0) add(VaeTap{sc_pair, 0, 0}, L.cin_sc / 64);
+    NOPE_CHECK(nseg <= kMaxSeg && ksteps * 64 == L.K, "vae conv: segment table");
+    p.bmap = L.wmap;
+    if (get_map(&m, out_hi, L.cout, H, -1)) return -1;
+    p.omap[0] = *m;
+    p.bias = L.bias;
+    p.stats_hw = H * H;
+    p.stats_noct = L.cout / 8;
+    p.n_total = L.cout;
+    p.m_valid = n * H * H;
+    p.nseg = nseg;
+    p.ksteps = ksteps;
+    p.m_tiles = geom_m_tiles(g, n);
+    p.n_par = 1;
+    p.n_tiles_par = L.cout / L.bn;
+    p.n_tiles = p.n_tiles_par;
+    p.tiles_per_img = g.tiles_per_img;
+    p.h_cnt = g.h_cnt;
+    p.b_cnt = g.b_cnt;
+    p.res_hi = res ? res->hi : nullptr;
+    p.res_lo = res ? res->lo : nullptr;
+    p.out_lo = out_lo;
+    p.out_f32 = out_f32;
+    ++launches;
+    return launch_conv_tc2(p, L.bn, num_sms, st);
+  }
+
+  // 3x3 pad-1 convolution at the current level.  Level 0 (parity-planar): one launch per output plane (py, px);
+  // tap (oy, ox) of that plane reads input plane ((py + oy) & 1, (px + ox) & 1) at offset ((py + oy) >> 1, ...).
+  // Output: out_f32 (+ (hi, lo) when out_lo), residual res (same layout) or the conv's 1x1 shortcut over sc.
+  int conv3(const nope::VaeConv& L, const nope::ActPair& in, int H, int n, const nope::ActPair& out, bool want_lo,
+            float* out_f32, const nope::ActPair* res, const nope::ActPair* sc, cudaStream_t st) {
+    using namespace nope;
+    std::vector<VaeTap> taps;
+    if (H < 256) {
+      for (int oy = -1; oy <= 1; ++oy)
+        for (int ox = -1; ox <= 1; ++ox) taps.push_back(VaeTap{0, oy, ox});
+      std::vector<std::pair<ActPair, int>> src{{in, -1}};
+      if (sc) src.push_back({*sc, -1});
+      return conv(L, src, H, taps, sc ? 1 : -1, H, n, out.hi, want_lo ? out.lo : nullptr, out_f32, res, st);
+    }
+    NOPE_CHECK(!sc, "vae conv: no shortcut at the 256 x 256 level");
+    std::vector<std::pair<ActPair, int>> src;
+    for (int q = 0; q < 4; ++q) {
+      const size_t o = plane_off(q, L.cin);
+      src.push_back({ActPair{in.hi + o, in.lo + o}, -1});
+    }
+    for (int q = 0; q < 4; ++q) {
+      const int py = q >> 1, px = q & 1;
+      taps.clear();
+      for (int oy = -1; oy <= 1; ++oy)
+        for (int ox = -1; ox <= 1; ++ox) {
+          const int sy = py + oy, sx = px + ox;
+          taps.push_back(VaeTap{(sy & 1) * 2 + (sx & 1), sy >> 1, sx >> 1});
+        }
+      const size_t o = plane_off(q, L.cout);
+      ActPair r;
+      if (res) r = ActPair{res->hi + o, res->lo + o};
+      if (conv(L, src, 128, taps, -1, 128, n, out.hi + o, want_lo ? out.lo + o : nullptr, out_f32 + o,
+               res ? &r : nullptr, st))
+        return -1;
+    }
+    return 0;
+  }
+
+  // Downsample2D: pad (0, 1, 0, 1) + 3x3 stride 2 from side 2H to H.  Tap (ky, kx) reads input (2y + ky, 2x + kx):
+  // sub-lattice (ky & 1, kx & 1) at offset (ky >> 1, kx >> 1); the bottom / right zero padding is the TMA's
+  // out-of-bounds fill of offset 1.  The 256 x 256 input's sub-lattices are its planes.
+  int downsample(const nope::VaeConv& L, const nope::ActPair& in, int Hin, int n, const nope::ActPair& out,
+                 float* out_f32, cudaStream_t st) {
+    using namespace nope;
+    const int H = Hin / 2;
+    std::vector<std::pair<ActPair, int>> src;
+    for (int q = 0; q < 4; ++q) {
+      if (Hin == 256) {
+        const size_t o = plane_off(q, L.cin);
+        src.push_back({ActPair{in.hi + o, in.lo + o}, -1});
+      } else {
+        src.push_back({in, q});
+      }
+    }
+    std::vector<VaeTap> taps;
+    for (int ky = 0; ky < 3; ++ky)
+      for (int kx = 0; kx < 3; ++kx) taps.push_back(VaeTap{(ky & 1) * 2 + (kx & 1), ky >> 1, kx >> 1});
+    return conv(L, src, H, taps, -1, H, n, out.hi, out.lo, out_f32, nullptr, st);
+  }
+
+  // GroupNorm(32, eps 1e-6) [+ SiLU] of the fp32 tensor x (C channels, side H; parity-planar at 256) -> nrm
+  int group_norm(const std::string& name, const float* x, int C, int H, int n, bool silu, cudaStream_t st) {
+    using namespace nope;
+    const VaeNorm& N = norms.at(name);
+    const int planes = H == 256 ? 4 : 1, hw = H == 256 ? 128 * 128 : H * H;
+    const int nparts = planes * hw / kVaeSlab;
+    vae_gn_partial_kernel<<<dim3(nparts, n), 256, 0, st>>>(x, C, hw, kChunk, gn_part);
+    NOPE_CUDA(cudaGetLastError());
+    vae_gn_finalize_kernel<<<n, 32, 0, st>>>(gn_part, nparts, 1.0 / ((double)planes * hw * (C / 32)), 1e-6,
+                                             gn_stats);
+    NOPE_CUDA(cudaGetLastError());
+    vae_gn_apply_kernel<<<dim3((hw * C / 4 + 255) / 256, planes * n), 256, 0, st>>>(
+        x, gn_stats, N.gamma, N.beta, C, hw, n, kChunk, silu ? 1 : 0, nrm.hi, nrm.lo);
+    NOPE_CUDA(cudaGetLastError());
+    launches += 3;
+    return 0;
+  }
+
+  // ResnetBlock2D on the residual stream `cur` -> 1 - cur
+  int resnet(const std::string& p, int cin, int cout, int H, int n, int& cur, cudaStream_t st) {
+    const int nxt = 1 - cur;
+    if (group_norm(p + ".norm1", x32[cur], cin, H, n, true, st)) return -1;
+    // conv1 -> t32; its fp16 high halves land in xs[nxt].hi, which conv2 overwrites
+    if (conv3(convs.at(p + ".conv1"), nrm, H, n, xs[nxt], false, t32, nullptr, nullptr, st)) return -1;
+    if (group_norm(p + ".norm2", t32, cout, H, n, true, st)) return -1;
+    const bool sc = cin != cout;
+    if (conv3(convs.at(p + ".conv2"), nrm, H, n, xs[nxt], true, x32[nxt], sc ? nullptr : &xs[cur],
+              sc ? &xs[cur] : nullptr, st))
+      return -1;
+    cur = nxt;
+    return 0;
+  }
+
+  // mid-block attention on the 32 x 32 residual stream `cur` -> 1 - cur
+  int attention(int n, int& cur, cudaStream_t st) {
+    using namespace nope;
+    const int nxt = 1 - cur;
+    const std::string a = "encoder.mid_block.attentions.0.";
+    if (group_norm(a + "group_norm", x32[cur], 512, 32, n, false, st)) return -1;
+    // qkv [n * 1024, 1536] fp32 -> t32 (high halves into xs[nxt].hi, overwritten by proj_attn)
+    const VaeConv& qkv = convs.at(a + "qkv");
+    if (conv(qkv, {{nrm, -1}}, 32, {VaeTap{0, 0, 0}}, -1, 32, n, xs[nxt].hi, nullptr, t32, nullptr, st)) return -1;
+    // S = q k^T / sqrt(512) -> x32[nxt] (overwritten by proj_attn), softmax over keys in place
+    float* S = x32[nxt];
+    vae_attn_gemm_kernel<true, false><<<dim3(16, 16, n), 256, 0, st>>>(
+        t32, 1536, 1024LL * 1536, t32 + 512, 1536, 1024LL * 1536, 512, (float)(1.0 / std::sqrt(512.0)), S, nullptr,
+        nullptr, 1024, 1024LL * 1024);
+    NOPE_CUDA(cudaGetLastError());
+    vae_softmax_kernel<<<n * 1024, 256, 0, st>>>(S);
+    NOPE_CUDA(cudaGetLastError());
+    // O = P v -> nrm (hi, lo) [n * 1024, 512]
+    vae_attn_gemm_kernel<false, true><<<dim3(8, 16, n), 256, 0, st>>>(
+        S, 1024, 1024LL * 1024, t32 + 1024, 1536, 1024LL * 1536, 1024, 1.f, nullptr, nrm.hi, nrm.lo, 512,
+        1024LL * 512);
+    NOPE_CUDA(cudaGetLastError());
+    launches += 3;
+    // x + proj_attn(O)
+    if (conv(convs.at(a + "proj_attn"), {{nrm, -1}}, 32, {VaeTap{0, 0, 0}}, -1, 32, n, xs[nxt].hi, xs[nxt].lo,
+             x32[nxt], &xs[cur], st))
+      return -1;
+    cur = nxt;
+    return 0;
+  }
+
+  // n <= kChunk images [n, 3, 256, 256] -> out [n, 4, 32, 32]
+  int encode(const float* images, int n, float* out, cudaStream_t st) {
+    using namespace nope;
+    launches = 0;
+    vae_conv_in_kernel<<<n * 65536 / 2, 256, 0, st>>>(images, in_w, in_b, x32[0], xs[0].hi, xs[0].lo, n, kChunk);
+    NOPE_CUDA(cudaGetLastError());
+    ++launches;
+    int cur = 0, H = 256, cin = 128;
+    for (int i = 0; i < 4; ++i) {
+      const std::string blk = "encoder.down_blocks." + std::to_string(i);
+      for (int j = 0; j < 2; ++j) {
+        if (resnet(blk + ".resnets." + std::to_string(j), cin, kCh[i], H, n, cur, st)) return -1;
+        cin = kCh[i];
+      }
+      if (i < 3) {
+        if (downsample(convs.at(blk + ".downsamplers.0.conv"), xs[cur], H, n, xs[1 - cur], x32[1 - cur], st))
+          return -1;
+        cur = 1 - cur;
+        H /= 2;
+      }
+    }
+    if (resnet("encoder.mid_block.resnets.0", 512, 512, 32, n, cur, st)) return -1;
+    if (attention(n, cur, st)) return -1;
+    if (resnet("encoder.mid_block.resnets.1", 512, 512, 32, n, cur, st)) return -1;
+    if (group_norm("encoder.conv_norm_out", x32[cur], 512, 32, n, true, st)) return -1;
+    const VaeConv& co = convs.at("conv_out");
+    if (conv3(co, nrm, 32, n, xs[1 - cur], false, t32, nullptr, nullptr, st)) return -1;
+    enc_extract_kernel<<<ew_grid((long long)n * 4 * 1024), 256, 0, st>>>(t32, out, n, 4, 1024, co.cout);
+    NOPE_CUDA(cudaGetLastError());
+    ++launches;
+    return 0;
+  }
+
+  // images [B, 3, 256, 256] x angles cossin [A, 2] -> out [B, A, 4, 32, 32]: the (image, angle) pairs in b-major
+  // order, kChunk at a time rotated into rot_stage and encoded from there (the chunks encode() makes of that batch)
+  int encode_inplane(const float* images, int B, const float* cossin, int A, float* out, cudaStream_t st) {
+    using namespace nope;
+    NOPE_CHECK((int64_t)B * A <= INT32_MAX, "too many (image, angle) pairs");
+    const int pairs = B * A;
+    int64_t total = 0;
+    for (int lo = 0; lo < pairs; lo += kChunk) {
+      const int n = pairs - lo < kChunk ? pairs - lo : kChunk;
+      inplane_rotate_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, cossin, A, 256, 256, lo, rot_stage);
+      NOPE_CUDA(cudaGetLastError());
+      if (encode(rot_stage, n, out + (size_t)lo * 4 * 32 * 32, st)) return -1;
+      total += launches + 1;
+    }
+    launches = total;
+    return 0;
+  }
+
+  // images [B, 3, 256, 256] x pairs (image_idx [P], cossin [P, 2]) -> out [P, 4, 32, 32], kChunk pairs at a time
+  int encode_rotated(const float* images, int B, const int* image_idx, const float* cossin, int P, float* out,
+                     cudaStream_t st) {
+    using namespace nope;
+    int64_t total = 0;
+    for (int lo = 0; lo < P; lo += kChunk) {
+      const int n = P - lo < kChunk ? P - lo : kChunk;
+      inplane_rotate_pairs_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, B, image_idx, cossin, 256, 256,
+                                                                             lo, rot_stage);
+      NOPE_CUDA(cudaGetLastError());
+      if (encode(rot_stage, n, out + (size_t)lo * 4 * 32 * 32, st)) return -1;
+      total += launches + 1;
+    }
+    launches = total;
+    return 0;
+  }
+};

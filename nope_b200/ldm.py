@@ -6,8 +6,8 @@ Same constructor keywords as the reference class; `load_state_dict` takes its 62
 `__call__(x, pose)` is `UNetModelPose.forward`; `sweep` batches all pose hypotheses of a
 reference latent and fuses the l2 score + top-k like `nope_b200.unet.UNet.sweep`.  All arithmetic
 runs in libnope_b200.so.  The VAE encoder of this variant (diffusers AutoencoderKL,
-src/model/encoder/AutoencoderKL.py:16-47) is not part of the reference tree; pass any object
-with `latent_dim` / `name` (and `encode_image` if images are to be encoded) as `encoder`.
+src/model/encoder/AutoencoderKL.py:16-47) is nope_b200.vae.VAE_StableDiffusion (DESIGN.md section 16);
+any object with `latent_dim` / `name` (and `encode_image` if images are to be encoded) may stand in.
 """
 import ctypes as C
 
@@ -79,7 +79,10 @@ class UNetModelPose:
         return self
 
     def load_state_dict(self, state_dict, strict=True):
-        """Reference UNetModelPose.state_dict() keys; `encoder.*` entries are skipped."""
+        """Reference UNetModelPose.state_dict() keys; `encoder.*` entries are skipped, except that a
+        VAE_StableDiffusion encoder receives the `encoder.encoder.*` entries (AutoencoderKL keys)."""
+        from .unet import encoder_entries
+        from .vae import VAE_StableDiffusion
         lib = _lib.load()
         h = self._handle()
         for k, v in state_dict.items():
@@ -90,6 +93,10 @@ class UNetModelPose:
             _lib.check(lib.nope_ldm_load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
         _lib.check(lib.nope_ldm_finalize(h))
         self._finalized = True
+        if isinstance(self.encoder, VAE_StableDiffusion):
+            vae_sd = encoder_entries(state_dict, self.encoder)
+            if vae_sd:
+                self.encoder.load_state_dict(vae_sd, strict=strict)
         return self
 
     def set_chunk(self, hyps):

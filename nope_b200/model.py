@@ -76,8 +76,8 @@ class PoseConditional:
 
     @torch.no_grad()
     def forward(self, query, reference, relativeR):
-        query_feat = self.u_net.encoder.encode_image(query)
-        reference_feat = self.u_net.encoder.encode_image(reference, mode="mode")
+        query_feat = self.u_net.encoder.encode_image(query.to(self.device))
+        reference_feat = self.u_net.encoder.encode_image(reference.to(self.device), mode="mode")
         pred = self.u_net(reference_feat, relativeR)
         return self.compute_loss(pred, query_feat)
 
@@ -86,13 +86,13 @@ class PoseConditional:
     # ------------------------------------------------------------------ model.py:113-124
     @torch.no_grad()
     def sample(self, reference, relativeR):
-        reference_feat = self.u_net.encoder.encode_image(reference, mode="mode")
+        reference_feat = self.u_net.encoder.encode_image(reference.to(self.device), mode="mode")
         return self.u_net(reference_feat, relativeR), None   # template encoder: no decoder
 
     # ------------------------------------------------------------------ model.py:193-252
     @torch.no_grad()
     def generate_templates(self, reference, all_relativeR, gt_templates=None, visualize=False):
-        reference_feat = self.u_net.encoder.encode_image(reference, mode="mode")
+        reference_feat = self.u_net.encoder.encode_image(reference.to(self.device), mode="mode")
         emb = self.u_net.sweep(reference_feat, all_relativeR, want_emb=True)["emb"]
         return emb, None, None
 
@@ -105,7 +105,7 @@ class PoseConditional:
         metric = getattr(self.testing_config, "similarity_metric", "l2")
         if metric not in _METRICS:
             raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
-        query_feat = self.u_net.encoder.encode_image(query, mode="mode")
+        query_feat = self.u_net.encoder.encode_image(query.to(self.device), mode="mode")
         return score_topk(query_feat, template_feat, k=k, metric=metric, threshold=self._occlusion_threshold())
 
     def _occlusion_threshold(self):

@@ -25,6 +25,25 @@ class _Incompatible:
         return f"<missing_keys={self.missing_keys}, unexpected_keys={self.unexpected_keys}>"
 
 
+def encoder_entries(state_dict, encoder):
+    """The `encoder.*` entries of a UNet state_dict that `encoder` loads, prefix stripped.  The SD VAE
+    (nope_b200.vae.VAE_StableDiffusion) takes `encoder.encoder.*`: the AutoencoderKL it wraps
+    (AutoencoderKL.py:16).  The template encoder takes `encoder.backbone.*` / `encoder.projector.*`; its
+    `encoder.encoder.*` aliases (template.py:40) repeat the same tensors and are skipped."""
+    from .vae import VAE_StableDiffusion
+    out = {}
+    for k, v in state_dict.items():
+        if not k.startswith("encoder."):
+            continue
+        kk = k[len("encoder."):]
+        if isinstance(encoder, VAE_StableDiffusion):
+            if kk.startswith("encoder."):
+                out[kk[len("encoder."):]] = v
+        elif kk.startswith("backbone.") or kk.startswith("projector."):
+            out[kk] = v
+    return out
+
+
 class UNet:
     def __init__(self, u_net_dim, rot_representation_dim, encoder, pose_mlp_name="single_layer",
                  init_dim=None, out_dim=None, use_hard_up_down=True, dim_mults=(1, 2, 4, 8),
@@ -113,13 +132,11 @@ class UNet:
         (src/utils/weight.py:6-37) is nope_b200.weight.load_checkpoint."""
         lib = _lib.load()
         want = self.expected_shapes()
-        enc_sd, unet_sd, unexpected = {}, {}, []
+        unet_sd, unexpected = {}, []
+        enc_sd = encoder_entries(state_dict, self.encoder)
         for k, v in state_dict.items():
             if k.startswith("encoder."):
-                kk = k[len("encoder."):]
-                if kk.startswith("backbone.") or kk.startswith("projector."):
-                    enc_sd[kk] = v
-                continue      # the `encoder.encoder.*` aliases (template.py:40) repeat the same tensors
+                continue
             if k not in want:
                 unexpected.append(k)
                 continue
