@@ -218,6 +218,24 @@ int nope_vae_encode_rotated(nope_vae_t* v, const float* images, int B, const int
                             int P, float* out, void* stream);
 int64_t nope_vae_last_launch_count(const nope_vae_t* v);
 
+/* Stable Diffusion VAE decoder (DESIGN.md section 17): AutoencoderKL.decode(z / 0.18215).sample of the SD v1
+ * configuration (post_quant_conv 1x1; conv_in 3x3 4 -> 512; mid block as the encoder's; four UpDecoderBlock2D of three
+ * resnets with 512, 512, 256, 128 channels, blocks 0-2 ending in nearest x2 + 3x3 conv; GroupNorm(32, eps 1e-6),
+ * SiLU, conv_out 3x3 128 -> 3), with the encoder's split-precision scheme.  A handle of its own: it takes the 140
+ * `decoder.*` / `post_quant_conv.*` tensors (0.14-era attention names under `decoder.mid_block.attentions.0.`), HOST
+ * fp32 pointers, shape-checked; every key is required by nope_vae_decoder_finalize, which also allocates the workspace
+ * (8 images, ~3.2 GB).  nope_vae_decoder_decode: latents [B, 4, 32, 32] fp32 (device) -> out [B, 3, 256, 256] fp32
+ * NCHW, unclamped; any B >= 1, 8 latents at a time, and an image does not depend on the batch it was decoded in.
+ * Bad arguments are refused before any CUDA call; no call synchronises the host. */
+typedef struct nope_vae_decoder nope_vae_decoder_t;
+int nope_vae_decoder_create(nope_vae_decoder_t** out, int device);
+void nope_vae_decoder_destroy(nope_vae_decoder_t* d);
+int nope_vae_decoder_load_tensor(nope_vae_decoder_t* d, const char* key, const float* data, const int64_t* shape,
+                                 int ndim);
+int nope_vae_decoder_finalize(nope_vae_decoder_t* d);
+int nope_vae_decoder_decode(nope_vae_decoder_t* d, const float* latents, int B, float* out, void* stream);
+int64_t nope_vae_decoder_last_launch_count(const nope_vae_decoder_t* d);
+
 /* T-LESS evaluation (DESIGN.md section 12): a depth rasterizer standing in for pyrender's DEPTH_ONLY render and the
  * VSD error of src/poses/vsd.py:92-135 (visibility mode "bop19", src/poses/vsd_utils.py).  Both calls refuse bad
  * arguments before any CUDA call and do not synchronise.

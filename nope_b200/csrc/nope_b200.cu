@@ -1705,6 +1705,70 @@ int nope_vae_encode_rotated(nope_vae_t* v, const float* images, int B, const int
 int64_t nope_vae_last_launch_count(const nope_vae_t* v) { return v ? v->launches : 0; }
 
 // ---------------------------------------------------------------------------------
+// Stable Diffusion VAE decoder (vae.cuh, DESIGN.md section 17)
+// ---------------------------------------------------------------------------------
+int nope_vae_decoder_create(nope_vae_decoder_t** out, int device) {
+  NOPE_CHECK(out != nullptr, "null out pointer");
+  int ndev = 0;
+  NOPE_CUDA(cudaGetDeviceCount(&ndev));
+  NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
+  cudaDeviceProp prop;
+  NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
+  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
+  auto d = std::make_unique<nope_vae_decoder>();
+  d->device = device;
+  d->num_sms = prop.multiProcessorCount;
+  d->build_schema();
+  *out = d.release();
+  return 0;
+}
+
+void nope_vae_decoder_destroy(nope_vae_decoder_t* d) { delete d; }
+
+int nope_vae_decoder_load_tensor(nope_vae_decoder_t* d, const char* key, const float* data, const int64_t* shape,
+                                 int ndim) {
+  NOPE_CHECK(d && key && data && shape, "null argument");
+  NOPE_CHECK(!d->finalized, "VAE decoder already finalized");
+  auto it = d->expected.find(key);
+  NOPE_CHECK(it != d->expected.end(), std::string("unexpected VAE decoder state_dict key: ") + key);
+  NOPE_CHECK((int)it->second.size() == ndim, std::string("rank mismatch for ") + key);
+  size_t n = 1;
+  for (int i = 0; i < ndim; ++i) {
+    NOPE_CHECK(it->second[i] == shape[i], std::string("shape mismatch for ") + key);
+    n *= (size_t)shape[i];
+  }
+  auto& slot = d->host[key];
+  slot.first.assign(shape, shape + ndim);
+  slot.second.assign(data, data + n);
+  return 0;
+}
+
+int nope_vae_decoder_finalize(nope_vae_decoder_t* d) {
+  NOPE_CHECK(d, "null VAE decoder");
+  return d->finalize();
+}
+
+int nope_vae_decoder_decode(nope_vae_decoder_t* d, const float* latents, int B, float* out, void* stream) {
+  NOPE_CHECK(latents && out, "null latents / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(d && d->finalized, "VAE decoder not finalized");
+  NOPE_CUDA(cudaSetDevice(d->device));
+  constexpr int kChunk = nope_vae_decoder::kChunk;
+  int64_t launches = 0;
+  for (int lo = 0; lo < B; lo += kChunk) {
+    const int n = B - lo < kChunk ? B - lo : kChunk;
+    const int rc = d->decode(latents + (size_t)lo * 4 * 32 * 32, n, out + (size_t)lo * 3 * 256 * 256,
+                             static_cast<cudaStream_t>(stream));
+    if (rc != 0) return rc;
+    launches += d->launches;
+  }
+  d->launches = launches;
+  return 0;
+}
+
+int64_t nope_vae_decoder_last_launch_count(const nope_vae_decoder_t* d) { return d ? d->launches : 0; }
+
+// ---------------------------------------------------------------------------------
 // T-LESS evaluation: depth rasterizer and VSD (render.cuh, DESIGN.md section 12)
 // ---------------------------------------------------------------------------------
 int nope_render_depth(const float* vertices, int V, const int32_t* faces, int F, const float* poses, int P, float fx,

@@ -1,4 +1,6 @@
-// nope_b200 -- Stable Diffusion VAE encoder (diffusers AutoencoderKL, SD v1 configuration), fp32-accurate.
+// nope_b200 -- Stable Diffusion VAE encoder and decoder (diffusers AutoencoderKL, SD v1 configuration), fp32-accurate.
+// The decoder (nope_vae_decoder at the end of this file, DESIGN.md section 17) shares the host side below
+// (nope::VaeEngine) and every kernel but its conv_in, its upsample repack and its output extraction.
 //
 // latent = AutoencoderKL.encode(x).latent_dist.mode() * 0.18215 for x [B, 3, 256, 256] in [-1, 1]
 // (DESIGN.md section 16): conv_in 3x3 (3 -> 128); four down blocks of two ResnetBlock2D each
@@ -260,31 +262,119 @@ struct VaeTap {
   int pair, dy, dx;
 };
 
-}  // namespace nope
+// ---------------------------------------------------------------- decoder kernels (DESIGN.md section 17)
 
-struct nope_vae {
-  static constexpr int kChunk = 16;           // images per pass: the workspace holds this many (~200 MB each)
-  static constexpr int kCh[4] = {128, 256, 512, 512};
+// post_quant_conv (1x1, 4 -> 4, the 1 / 0.18215 scale folded into pq_w) then decoder.conv_in (3x3 pad 1, 4 -> 512),
+// fp32 direct, -> NHWC [n, 32, 32, 512] fp32 + (hi, lo).  z: [n, 4, 32, 32] NCHW; w: [512][4][3][3].  conv_in's zero
+// padding applies to post_quant_conv's output, so a border pixel sees fewer of post_quant_conv's bias taps.
+// grid (32 rows, n, 2 channel halves); one output channel per thread, the 32 pixels of the row in turn.
+__global__ void __launch_bounds__(256)
+vae_dec_conv_in_kernel(const float* __restrict__ z, const float* __restrict__ pq_w, const float* __restrict__ pq_b,
+                       const float* __restrict__ w, const float* __restrict__ bias, float* __restrict__ out32,
+                       __half* __restrict__ out_hi, __half* __restrict__ out_lo) {
+  __shared__ float s_w[36 * 256];   // [tap][channel]
+  __shared__ float s_p[3][34][4];   // post_quant_conv output of rows y - 1 .. y + 1, zero outside the image
+  const int y = blockIdx.x, b = blockIdx.y, o0 = blockIdx.z * 256, t = threadIdx.x;
+  for (int i = t; i < 36 * 256; i += 256) {
+    const int o = i / 36, j = i - o * 36;
+    s_w[j * 256 + o] = w[(size_t)o0 * 36 + i];
+  }
+  if (t < 3 * 34) {
+    const int r = t / 34, xx = t - r * 34 - 1, yy = y + r - 1;
+    float p[4] = {0.f, 0.f, 0.f, 0.f};
+    if (yy >= 0 && yy < 32 && xx >= 0 && xx < 32) {
+      float zc[4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) zc[c] = z[(((size_t)b * 4 + c) * 32 + yy) * 32 + xx];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        float a = pq_b[k];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) a = fmaf(pq_w[k * 4 + c], zc[c], a);
+        p[k] = a;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) s_p[r][xx + 1][k] = p[k];
+  }
+  __syncthreads();
+  float wr[36];
+#pragma unroll
+  for (int j = 0; j < 36; ++j) wr[j] = s_w[j * 256 + t];
+  const int o = o0 + t;
+  const float bo = bias[o];
+  for (int x = 0; x < 32; ++x) {
+    float acc = bo;
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+#pragma unroll
+      for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx) acc = fmaf(s_p[ky][x + kx][c], wr[(c * 3 + ky) * 3 + kx], acc);
+    const size_t dst = (((size_t)b * 32 + y) * 32 + x) * 512 + o;
+    out32[dst] = acc;
+    const __half hi = __float2half_rn(acc);
+    out_hi[dst] = hi;
+    out_lo[dst] = __float2half_rn(acc - __half2float(hi));
+  }
+}
+
+// The four parity planes of an upsample's output ([4][cap][H][H][C]; plane (py, px) = 2 py + px holds the pixels
+// (2 Y + py, 2 X + px)) -> plain NHWC [n, 2H, 2H, C], fp32 and (hi, lo); 4 channels per thread.
+__global__ void __launch_bounds__(256)
+vae_dec_repack_kernel(const float* __restrict__ p32, const __half* __restrict__ phi, const __half* __restrict__ plo,
+                      int C, int H, int n, int cap, float* __restrict__ o32, __half* __restrict__ ohi,
+                      __half* __restrict__ olo) {
+  const int quads = C >> 2, W2 = 2 * H;
+  const int total = n * W2 * W2 * quads;
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < total; i += gridDim.x * 256) {
+    const int c4 = i % quads, pix = i / quads;
+    const int xx = pix % W2, yy = (pix / W2) % W2, b = pix / (W2 * W2);
+    const int q = (yy & 1) * 2 + (xx & 1);
+    const size_t src = ((((size_t)q * cap + b) * H + (yy >> 1)) * H + (xx >> 1)) * quads + c4;
+    reinterpret_cast<float4*>(o32)[i] = reinterpret_cast<const float4*>(p32)[src];
+    reinterpret_cast<uint2*>(ohi)[i] = reinterpret_cast<const uint2*>(phi)[src];
+    reinterpret_cast<uint2*>(olo)[i] = reinterpret_cast<const uint2*>(plo)[src];
+  }
+}
+
+// conv_out's parity-planar fp32 output ([4][cap][128][128][ld], channels 0-2 real) -> NCHW [n, 3, 256, 256]
+__global__ void __launch_bounds__(256)
+vae_dec_extract_kernel(const float* __restrict__ t, int ld, int cap, int n, float* __restrict__ out) {
+  const int total = n * 3 * 65536;
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < total; i += gridDim.x * 256) {
+    const int xx = i & 255, yy = (i >> 8) & 255, bc = i >> 16, c = bc % 3, b = bc / 3;
+    const int q = (yy & 1) * 2 + (xx & 1);
+    out[i] = t[((((size_t)q * cap + b) * 128 + (yy >> 1)) * 128 + (xx >> 1)) * ld + c];
+  }
+}
+
+// ---------------------------------------------------------------- host side shared by the encoder and the decoder
+// The state_dict schema helpers, the split-precision weight packing, the workspace, and the launches of a
+// convolution, GroupNorm, ResnetBlock2D and the mid-block attention.  Every buffer holds `cap` images.
+struct VaeEngine {
+  const int cap;                              // images per pass
   int device = 0, num_sms = 132;
   bool finalized = false;
   std::map<std::string, std::pair<std::vector<int64_t>, std::vector<float>>> host;
   std::map<std::string, std::vector<int64_t>> expected;
-  std::map<std::string, nope::VaeConv> convs;
-  std::map<std::string, nope::VaeNorm> norms;
-  float *in_w = nullptr, *in_b = nullptr;
+  std::map<std::string, VaeConv> convs;
+  std::map<std::string, VaeNorm> norms;
   std::vector<void*> owned;
-  // workspace, each buffer sized for kChunk images of the 256 x 256 x 128 level
+  // workspace (alloc_workspace), each activation buffer sized for cap images of the widest level
   float* x32[2] = {nullptr, nullptr};         // residual stream, fp32
-  nope::ActPair xs[2];                        // residual stream, (hi, lo)
-  nope::ActPair nrm;                          // normalised activations / attention output, (hi, lo)
+  ActPair xs[2];                              // residual stream, (hi, lo)
+  ActPair nrm;                                // normalised activations / attention output, (hi, lo)
   float* t32 = nullptr;                       // conv1 / qkv / conv_out output, fp32
   double2* gn_part = nullptr;                 // GroupNorm partial sums
   float2* gn_stats = nullptr;                 // GroupNorm (mean, rstd)
-  float* rot_stage = nullptr;                 // kChunk rotated crops
   std::map<std::tuple<const void*, int, int, int>, CUtensorMap> tmaps;
   int64_t launches = 0;
 
-  ~nope_vae() {
+  explicit VaeEngine(int cap_) : cap(cap_) {}
+  VaeEngine(const VaeEngine&) = delete;
+  VaeEngine& operator=(const VaeEngine&) = delete;
+  ~VaeEngine() {
     for (void* p : owned) cudaFree(p);
   }
 
@@ -304,26 +394,12 @@ struct nope_vae {
     expect_conv(p + ".conv2", cout, cout, 3);
     if (cin != cout) expect_conv(p + ".conv_shortcut", cout, cin, 1);
   }
-  void build_schema() {
-    expect_conv("encoder.conv_in", 128, 3, 3);
-    int cin = 128;
-    for (int i = 0; i < 4; ++i) {
-      for (int j = 0; j < 2; ++j) {
-        expect_resnet("encoder.down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), cin, kCh[i]);
-        cin = kCh[i];
-      }
-      if (i < 3) expect_conv("encoder.down_blocks." + std::to_string(i) + ".downsamplers.0.conv", kCh[i], kCh[i], 3);
-    }
-    for (int j = 0; j < 2; ++j) expect_resnet("encoder.mid_block.resnets." + std::to_string(j), 512, 512);
-    const std::string a = "encoder.mid_block.attentions.0.";
+  void expect_attention(const std::string& a) {
     expect_norm(a + "group_norm", 512);
     for (const char* s : {"query", "key", "value", "proj_attn"}) {
       expected[a + s + ".weight"] = {512, 512};
       expected[a + s + ".bias"] = {512};
     }
-    expect_norm("encoder.conv_norm_out", 512);
-    expect_conv("encoder.conv_out", 8, 512, 3);
-    expect_conv("quant_conv", 8, 8, 1);
   }
 
   // ---------------------------------------------------------------- weights
@@ -339,7 +415,6 @@ struct nope_vae {
   // W [cout_real][cin][k*k], bias [cout_real] (float64), optional 1x1 shortcut Ws [cout_real][cin_sc] + its bias
   int pack_conv(const std::string& name, int cout_real, int cin, int k, const std::vector<double>& W,
                 const std::vector<double>& bias, int cin_sc = 0, const std::vector<double>* Ws = nullptr) {
-    using namespace nope;
     VaeConv L;
     L.cin = cin;
     L.cin_sc = cin_sc;
@@ -380,38 +455,25 @@ struct nope_vae {
     return pack_conv(name, (int)s[0], (int)s[1], k, dvec(name + ".weight"), dvec(name + ".bias"));
   }
   int make_norm(const std::string& name) {
-    nope::VaeNorm N;
+    VaeNorm N;
     if (upload(&N.gamma, h(name + ".weight")) || upload(&N.beta, h(name + ".bias"))) return -1;
     norms[name] = N;
     return 0;
   }
-  int make_resnet(const std::string& p, int cin, int cout) {
+  // planar: the block runs at the parity-planar 256 x 256 level, where a 1x1 shortcut is its own convolution (no
+  // bias) whose (hi, lo) output is conv2's residual; elsewhere it rides in conv2 as extra K-segments.  Either way
+  // the shortcut's bias is added to conv2's in float64.
+  int make_resnet(const std::string& p, int cin, int cout, bool planar = false) {
     if (make_norm(p + ".norm1") || make_norm(p + ".norm2") || make_plain(p + ".conv1", 3)) return -1;
     std::vector<double> b = dvec(p + ".conv2.bias");
     if (cin == cout) return pack_conv(p + ".conv2", cout, cout, 3, dvec(p + ".conv2.weight"), b);
     const std::vector<double> ws = dvec(p + ".conv_shortcut.weight"), bs = dvec(p + ".conv_shortcut.bias");
     for (int o = 0; o < cout; ++o) b[o] += bs[o];
-    return pack_conv(p + ".conv2", cout, cout, 3, dvec(p + ".conv2.weight"), b, cin, &ws);
+    if (!planar) return pack_conv(p + ".conv2", cout, cout, 3, dvec(p + ".conv2.weight"), b, cin, &ws);
+    if (pack_conv(p + ".conv_shortcut", cout, cin, 1, ws, std::vector<double>(cout, 0.0))) return -1;
+    return pack_conv(p + ".conv2", cout, cout, 3, dvec(p + ".conv2.weight"), b);
   }
-
-  int finalize() {
-    using namespace nope;
-    NOPE_CHECK(!finalized, "already finalized");
-    for (const auto& kv : expected) NOPE_CHECK(host.count(kv.first), "state_dict is missing " + kv.first);
-    NOPE_CUDA(cudaSetDevice(device));
-    if (upload(&in_w, h("encoder.conv_in.weight")) || upload(&in_b, h("encoder.conv_in.bias"))) return -1;
-    int cin = 128;
-    for (int i = 0; i < 4; ++i) {
-      const std::string blk = "encoder.down_blocks." + std::to_string(i);
-      for (int j = 0; j < 2; ++j) {
-        if (make_resnet(blk + ".resnets." + std::to_string(j), cin, kCh[i])) return -1;
-        cin = kCh[i];
-      }
-      if (i < 3 && make_plain(blk + ".downsamplers.0.conv", 3)) return -1;
-    }
-    for (int j = 0; j < 2; ++j)
-      if (make_resnet("encoder.mid_block.resnets." + std::to_string(j), 512, 512)) return -1;
-    const std::string a = "encoder.mid_block.attentions.0.";
+  int make_attention(const std::string& a) {
     if (make_norm(a + "group_norm")) return -1;
     {  // q, k, v as one 1x1 convolution 512 -> 1536
       std::vector<double> W, b;
@@ -422,27 +484,11 @@ struct nope_vae {
       }
       if (pack_conv(a + "qkv", 1536, 512, 1, W, b)) return -1;
     }
-    if (pack_conv(a + "proj_attn", 512, 512, 1, dvec(a + "proj_attn.weight"), dvec(a + "proj_attn.bias"))) return -1;
-    if (make_norm("encoder.conv_norm_out")) return -1;
-    {  // conv_out followed by quant_conv rows 0-3 (the mean) and the 0.18215 scale, folded in float64
-      const auto W = dvec("encoder.conv_out.weight"), b = dvec("encoder.conv_out.bias");
-      const auto Q = dvec("quant_conv.weight"), qb = dvec("quant_conv.bias");
-      constexpr double kScale = 0.18215;
-      std::vector<double> Wf((size_t)4 * 512 * 9, 0.0), bf(4, 0.0);
-      for (int o = 0; o < 4; ++o) {
-        double bo = qb[o];
-        for (int j = 0; j < 8; ++j) {
-          bo += Q[o * 8 + j] * b[j];
-          for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] += Q[o * 8 + j] * W[(size_t)j * 512 * 9 + i];
-        }
-        bf[o] = kScale * bo;
-        for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] *= kScale;
-      }
-      if (pack_conv("conv_out", 4, 512, 3, Wf, bf)) return -1;
-    }
-    host.clear();
-    // workspace for kChunk images, allocated once so that no encode call allocates (or synchronises)
-    const size_t E = (size_t)kChunk * 256 * 256 * 128;
+    return pack_conv(a + "proj_attn", 512, 512, 1, dvec(a + "proj_attn.weight"), dvec(a + "proj_attn.bias"));
+  }
+
+  // workspace of E elements per activation buffer, allocated once so that no call allocates (or synchronises)
+  int alloc_workspace(size_t E) {
     for (int s = 0; s < 2; ++s) {
       NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&x32[s]), E * sizeof(float)));
       owned.push_back(x32[s]);
@@ -457,13 +503,10 @@ struct nope_vae {
     }
     NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&t32), E * sizeof(float)));
     owned.push_back(t32);
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&gn_part), (size_t)kChunk * 64 * 32 * sizeof(double2)));
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&gn_part), (size_t)cap * 64 * 32 * sizeof(double2)));
     owned.push_back(gn_part);
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&gn_stats), (size_t)kChunk * 32 * sizeof(float2)));
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&gn_stats), (size_t)cap * 32 * sizeof(float2)));
     owned.push_back(gn_stats);
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&rot_stage), (size_t)kChunk * 3 * 256 * 256 * sizeof(float)));
-    owned.push_back(rot_stage);
-    finalized = true;
     return 0;
   }
 
@@ -471,15 +514,14 @@ struct nope_vae {
   // NHWC map of `cap` images of side H x H and C channels at base; lattice >= 0: the stride-2 sub-lattice
   // (lattice >> 1, lattice & 1) of a 2H x 2H tensor
   int get_map(const CUtensorMap** out, const void* base, int C, int H, int lattice) {
-    using namespace nope;
     const auto key = std::make_tuple(base, lattice, C, H);
     auto it = tmaps.find(key);
     if (it == tmaps.end()) {
       TileGeom g;
       if (make_geom(H, H, &g)) return -1;
       CUtensorMap m;
-      const int rc = lattice < 0 ? make_act_map(&m, base, kChunk, C, g)
-                                 : make_unshuffle_map(&m, base, kChunk, C, g, lattice >> 1, lattice & 1);
+      const int rc = lattice < 0 ? make_act_map(&m, base, cap, C, g)
+                                 : make_unshuffle_map(&m, base, cap, C, g, lattice >> 1, lattice & 1);
       if (rc) return -1;
       it = tmaps.emplace(key, m).first;
     }
@@ -487,14 +529,13 @@ struct nope_vae {
     return 0;
   }
   // offset of plane q of a parity-planar level-0 tensor with C channels
-  static size_t plane_off(int q, int C) { return (size_t)q * kChunk * 128 * 128 * C; }
+  size_t plane_off(int q, int C) const { return (size_t)q * cap * 128 * 128 * C; }
 
   // out = conv(taps over the input pairs `in`) [+ shortcut taps over pair sc] + bias [+ res]; output H x H.
   // in: (hi, lo) base pointers of each input pair with their lattice (-1: plain NHWC of side H).
-  int conv(const nope::VaeConv& L, const std::vector<std::pair<nope::ActPair, int>>& in, int Hin_map,
-           const std::vector<nope::VaeTap>& taps, int sc_pair, int H, int n, __half* out_hi, __half* out_lo,
-           float* out_f32, const nope::ActPair* res, cudaStream_t st) {
-    using namespace nope;
+  int conv(const VaeConv& L, const std::vector<std::pair<ActPair, int>>& in, int Hin_map,
+           const std::vector<VaeTap>& taps, int sc_pair, int H, int n, __half* out_hi, __half* out_lo,
+           float* out_f32, const ActPair* res, cudaStream_t st) {
     TileGeom g;
     if (make_geom(H, H, &g)) return -1;
     ConvParams p;
@@ -547,9 +588,8 @@ struct nope_vae {
   // 3x3 pad-1 convolution at the current level.  Level 0 (parity-planar): one launch per output plane (py, px);
   // tap (oy, ox) of that plane reads input plane ((py + oy) & 1, (px + ox) & 1) at offset ((py + oy) >> 1, ...).
   // Output: out_f32 (+ (hi, lo) when out_lo), residual res (same layout) or the conv's 1x1 shortcut over sc.
-  int conv3(const nope::VaeConv& L, const nope::ActPair& in, int H, int n, const nope::ActPair& out, bool want_lo,
-            float* out_f32, const nope::ActPair* res, const nope::ActPair* sc, cudaStream_t st) {
-    using namespace nope;
+  int conv3(const VaeConv& L, const ActPair& in, int H, int n, const ActPair& out, bool want_lo, float* out_f32,
+            const ActPair* res, const ActPair* sc, cudaStream_t st) {
     std::vector<VaeTap> taps;
     if (H < 256) {
       for (int oy = -1; oy <= 1; ++oy)
@@ -558,7 +598,7 @@ struct nope_vae {
       if (sc) src.push_back({*sc, -1});
       return conv(L, src, H, taps, sc ? 1 : -1, H, n, out.hi, want_lo ? out.lo : nullptr, out_f32, res, st);
     }
-    NOPE_CHECK(!sc, "vae conv: no shortcut at the 256 x 256 level");
+    NOPE_CHECK(!sc, "vae conv: no shortcut segments at the 256 x 256 level");
     std::vector<std::pair<ActPair, int>> src;
     for (int q = 0; q < 4; ++q) {
       const size_t o = plane_off(q, L.cin);
@@ -582,41 +622,18 @@ struct nope_vae {
     return 0;
   }
 
-  // Downsample2D: pad (0, 1, 0, 1) + 3x3 stride 2 from side 2H to H.  Tap (ky, kx) reads input (2y + ky, 2x + kx):
-  // sub-lattice (ky & 1, kx & 1) at offset (ky >> 1, kx >> 1); the bottom / right zero padding is the TMA's
-  // out-of-bounds fill of offset 1.  The 256 x 256 input's sub-lattices are its planes.
-  int downsample(const nope::VaeConv& L, const nope::ActPair& in, int Hin, int n, const nope::ActPair& out,
-                 float* out_f32, cudaStream_t st) {
-    using namespace nope;
-    const int H = Hin / 2;
-    std::vector<std::pair<ActPair, int>> src;
-    for (int q = 0; q < 4; ++q) {
-      if (Hin == 256) {
-        const size_t o = plane_off(q, L.cin);
-        src.push_back({ActPair{in.hi + o, in.lo + o}, -1});
-      } else {
-        src.push_back({in, q});
-      }
-    }
-    std::vector<VaeTap> taps;
-    for (int ky = 0; ky < 3; ++ky)
-      for (int kx = 0; kx < 3; ++kx) taps.push_back(VaeTap{(ky & 1) * 2 + (kx & 1), ky >> 1, kx >> 1});
-    return conv(L, src, H, taps, -1, H, n, out.hi, out.lo, out_f32, nullptr, st);
-  }
-
   // GroupNorm(32, eps 1e-6) [+ SiLU] of the fp32 tensor x (C channels, side H; parity-planar at 256) -> nrm
   int group_norm(const std::string& name, const float* x, int C, int H, int n, bool silu, cudaStream_t st) {
-    using namespace nope;
     const VaeNorm& N = norms.at(name);
     const int planes = H == 256 ? 4 : 1, hw = H == 256 ? 128 * 128 : H * H;
     const int nparts = planes * hw / kVaeSlab;
-    vae_gn_partial_kernel<<<dim3(nparts, n), 256, 0, st>>>(x, C, hw, kChunk, gn_part);
+    vae_gn_partial_kernel<<<dim3(nparts, n), 256, 0, st>>>(x, C, hw, cap, gn_part);
     NOPE_CUDA(cudaGetLastError());
     vae_gn_finalize_kernel<<<n, 32, 0, st>>>(gn_part, nparts, 1.0 / ((double)planes * hw * (C / 32)), 1e-6,
                                              gn_stats);
     NOPE_CUDA(cudaGetLastError());
     vae_gn_apply_kernel<<<dim3((hw * C / 4 + 255) / 256, planes * n), 256, 0, st>>>(
-        x, gn_stats, N.gamma, N.beta, C, hw, n, kChunk, silu ? 1 : 0, nrm.hi, nrm.lo);
+        x, gn_stats, N.gamma, N.beta, C, hw, n, cap, silu ? 1 : 0, nrm.hi, nrm.lo);
     NOPE_CUDA(cudaGetLastError());
     launches += 3;
     return 0;
@@ -626,22 +643,34 @@ struct nope_vae {
   int resnet(const std::string& p, int cin, int cout, int H, int n, int& cur, cudaStream_t st) {
     const int nxt = 1 - cur;
     if (group_norm(p + ".norm1", x32[cur], cin, H, n, true, st)) return -1;
+    const bool sc = cin != cout, planar_sc = sc && H == 256;
+    ActPair sres;
+    if (planar_sc) {
+      // the 1x1 shortcut, one launch per plane, into x32[cur]'s memory (norm1 was its last reader)
+      __half* s = reinterpret_cast<__half*>(x32[cur]);
+      sres = ActPair{s, s + 4 * plane_off(1, cout)};
+      const VaeConv& S = convs.at(p + ".conv_shortcut");
+      for (int q = 0; q < 4; ++q) {
+        const size_t i = plane_off(q, cin), o = plane_off(q, cout);
+        if (conv(S, {{ActPair{xs[cur].hi + i, xs[cur].lo + i}, -1}}, 128, {VaeTap{0, 0, 0}}, -1, 128, n,
+                 sres.hi + o, sres.lo + o, nullptr, nullptr, st))
+          return -1;
+      }
+    }
     // conv1 -> t32; its fp16 high halves land in xs[nxt].hi, which conv2 overwrites
     if (conv3(convs.at(p + ".conv1"), nrm, H, n, xs[nxt], false, t32, nullptr, nullptr, st)) return -1;
     if (group_norm(p + ".norm2", t32, cout, H, n, true, st)) return -1;
-    const bool sc = cin != cout;
-    if (conv3(convs.at(p + ".conv2"), nrm, H, n, xs[nxt], true, x32[nxt], sc ? nullptr : &xs[cur],
-              sc ? &xs[cur] : nullptr, st))
+    const ActPair* res = !sc ? &xs[cur] : planar_sc ? &sres : nullptr;
+    if (conv3(convs.at(p + ".conv2"), nrm, H, n, xs[nxt], true, x32[nxt], res, sc && !planar_sc ? &xs[cur] : nullptr,
+              st))
       return -1;
     cur = nxt;
     return 0;
   }
 
-  // mid-block attention on the 32 x 32 residual stream `cur` -> 1 - cur
-  int attention(int n, int& cur, cudaStream_t st) {
-    using namespace nope;
+  // mid-block attention (parameters under prefix a) on the 32 x 32 residual stream `cur` -> 1 - cur
+  int attention(const std::string& a, int n, int& cur, cudaStream_t st) {
     const int nxt = 1 - cur;
-    const std::string a = "encoder.mid_block.attentions.0.";
     if (group_norm(a + "group_norm", x32[cur], 512, 32, n, false, st)) return -1;
     // qkv [n * 1024, 1536] fp32 -> t32 (high halves into xs[nxt].hi, overwritten by proj_attn)
     const VaeConv& qkv = convs.at(a + "qkv");
@@ -667,6 +696,101 @@ struct nope_vae {
     cur = nxt;
     return 0;
   }
+};
+
+}  // namespace nope
+
+// ---------------------------------------------------------------- encoder (DESIGN.md section 16)
+struct nope_vae : nope::VaeEngine {
+  static constexpr int kChunk = 16;           // images per pass: the workspace holds this many (~200 MB each)
+  static constexpr int kCh[4] = {128, 256, 512, 512};
+  float *in_w = nullptr, *in_b = nullptr;
+  float* rot_stage = nullptr;                 // kChunk rotated crops
+
+  nope_vae() : VaeEngine(kChunk) {}
+
+  void build_schema() {
+    expect_conv("encoder.conv_in", 128, 3, 3);
+    int cin = 128;
+    for (int i = 0; i < 4; ++i) {
+      for (int j = 0; j < 2; ++j) {
+        expect_resnet("encoder.down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), cin, kCh[i]);
+        cin = kCh[i];
+      }
+      if (i < 3) expect_conv("encoder.down_blocks." + std::to_string(i) + ".downsamplers.0.conv", kCh[i], kCh[i], 3);
+    }
+    for (int j = 0; j < 2; ++j) expect_resnet("encoder.mid_block.resnets." + std::to_string(j), 512, 512);
+    expect_attention("encoder.mid_block.attentions.0.");
+    expect_norm("encoder.conv_norm_out", 512);
+    expect_conv("encoder.conv_out", 8, 512, 3);
+    expect_conv("quant_conv", 8, 8, 1);
+  }
+
+  int finalize() {
+    using namespace nope;
+    NOPE_CHECK(!finalized, "already finalized");
+    for (const auto& kv : expected) NOPE_CHECK(host.count(kv.first), "state_dict is missing " + kv.first);
+    NOPE_CUDA(cudaSetDevice(device));
+    if (upload(&in_w, h("encoder.conv_in.weight")) || upload(&in_b, h("encoder.conv_in.bias"))) return -1;
+    int cin = 128;
+    for (int i = 0; i < 4; ++i) {
+      const std::string blk = "encoder.down_blocks." + std::to_string(i);
+      for (int j = 0; j < 2; ++j) {
+        if (make_resnet(blk + ".resnets." + std::to_string(j), cin, kCh[i])) return -1;
+        cin = kCh[i];
+      }
+      if (i < 3 && make_plain(blk + ".downsamplers.0.conv", 3)) return -1;
+    }
+    for (int j = 0; j < 2; ++j)
+      if (make_resnet("encoder.mid_block.resnets." + std::to_string(j), 512, 512)) return -1;
+    if (make_attention("encoder.mid_block.attentions.0.")) return -1;
+    if (make_norm("encoder.conv_norm_out")) return -1;
+    {  // conv_out followed by quant_conv rows 0-3 (the mean) and the 0.18215 scale, folded in float64
+      const auto W = dvec("encoder.conv_out.weight"), b = dvec("encoder.conv_out.bias");
+      const auto Q = dvec("quant_conv.weight"), qb = dvec("quant_conv.bias");
+      constexpr double kScale = 0.18215;
+      std::vector<double> Wf((size_t)4 * 512 * 9, 0.0), bf(4, 0.0);
+      for (int o = 0; o < 4; ++o) {
+        double bo = qb[o];
+        for (int j = 0; j < 8; ++j) {
+          bo += Q[o * 8 + j] * b[j];
+          for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] += Q[o * 8 + j] * W[(size_t)j * 512 * 9 + i];
+        }
+        bf[o] = kScale * bo;
+        for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] *= kScale;
+      }
+      if (pack_conv("conv_out", 4, 512, 3, Wf, bf)) return -1;
+    }
+    host.clear();
+    // workspace for kChunk images of the 256 x 256 x 128 level
+    if (alloc_workspace((size_t)kChunk * 256 * 256 * 128)) return -1;
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&rot_stage), (size_t)kChunk * 3 * 256 * 256 * sizeof(float)));
+    owned.push_back(rot_stage);
+    finalized = true;
+    return 0;
+  }
+
+  // Downsample2D: pad (0, 1, 0, 1) + 3x3 stride 2 from side 2H to H.  Tap (ky, kx) reads input (2y + ky, 2x + kx):
+  // sub-lattice (ky & 1, kx & 1) at offset (ky >> 1, kx >> 1); the bottom / right zero padding is the TMA's
+  // out-of-bounds fill of offset 1.  The 256 x 256 input's sub-lattices are its planes.
+  int downsample(const nope::VaeConv& L, const nope::ActPair& in, int Hin, int n, const nope::ActPair& out,
+                 float* out_f32, cudaStream_t st) {
+    using namespace nope;
+    const int H = Hin / 2;
+    std::vector<std::pair<ActPair, int>> src;
+    for (int q = 0; q < 4; ++q) {
+      if (Hin == 256) {
+        const size_t o = plane_off(q, L.cin);
+        src.push_back({ActPair{in.hi + o, in.lo + o}, -1});
+      } else {
+        src.push_back({in, q});
+      }
+    }
+    std::vector<VaeTap> taps;
+    for (int ky = 0; ky < 3; ++ky)
+      for (int kx = 0; kx < 3; ++kx) taps.push_back(VaeTap{(ky & 1) * 2 + (kx & 1), ky >> 1, kx >> 1});
+    return conv(L, src, H, taps, -1, H, n, out.hi, out.lo, out_f32, nullptr, st);
+  }
 
   // n <= kChunk images [n, 3, 256, 256] -> out [n, 4, 32, 32]
   int encode(const float* images, int n, float* out, cudaStream_t st) {
@@ -690,7 +814,7 @@ struct nope_vae {
       }
     }
     if (resnet("encoder.mid_block.resnets.0", 512, 512, 32, n, cur, st)) return -1;
-    if (attention(n, cur, st)) return -1;
+    if (attention("encoder.mid_block.attentions.0.", n, cur, st)) return -1;
     if (resnet("encoder.mid_block.resnets.1", 512, 512, 32, n, cur, st)) return -1;
     if (group_norm("encoder.conv_norm_out", x32[cur], 512, 32, n, true, st)) return -1;
     const VaeConv& co = convs.at("conv_out");
@@ -733,6 +857,151 @@ struct nope_vae {
       total += launches + 1;
     }
     launches = total;
+    return 0;
+  }
+};
+
+// ---------------------------------------------------------------- decoder (DESIGN.md section 17)
+// image = AutoencoderKL.decode(z / 0.18215).sample for z [B, 4, 32, 32]: post_quant_conv 1x1 (4 -> 4); conv_in 3x3
+// (4 -> 512); the mid block at 32 x 32; four up blocks of three ResnetBlock2D (512, 512, 256, 128 channels; blocks 0-2
+// end in Upsample2D, nearest x2 + 3x3 conv); GroupNorm(32) + SiLU and conv_out 3x3 (128 -> 3).  Up block 3 runs at
+// the parity-planar 256 x 256 level; the 64 x 64 and 128 x 128 levels are plain NHWC, as in the encoder.
+struct nope_vae_decoder : nope::VaeEngine {
+  static constexpr int kChunk = 8;            // images per pass: 256 x 256 x 256 is 67 MB of fp32 per image
+  static constexpr int kCh[4] = {512, 512, 256, 128};
+  static constexpr const char* kAttn = "decoder.mid_block.attentions.0.";
+  float *in_w = nullptr, *in_b = nullptr, *pq_w = nullptr, *pq_b = nullptr;
+
+  nope_vae_decoder() : VaeEngine(kChunk) {}
+
+  static std::string up(int i) { return "decoder.up_blocks." + std::to_string(i); }
+
+  void build_schema() {
+    expect_conv("post_quant_conv", 4, 4, 1);
+    expect_conv("decoder.conv_in", 512, 4, 3);
+    expect_resnet("decoder.mid_block.resnets.0", 512, 512);
+    expect_attention(kAttn);
+    expect_resnet("decoder.mid_block.resnets.1", 512, 512);
+    int cin = 512;
+    for (int i = 0; i < 4; ++i) {
+      for (int j = 0; j < 3; ++j) {
+        expect_resnet(up(i) + ".resnets." + std::to_string(j), cin, kCh[i]);
+        cin = kCh[i];
+      }
+      if (i < 3) expect_conv(up(i) + ".upsamplers.0.conv", kCh[i], kCh[i], 3);
+    }
+    expect_norm("decoder.conv_norm_out", 128);
+    expect_conv("decoder.conv_out", 3, 128, 3);
+  }
+
+  // Upsample2D's 3x3 kernel folded into one 2x2 kernel per output parity (py, px), in float64.  Output row 2 Y + py
+  // with tap ky reads upsampled row 2 Y + py + ky - 1, i.e. source row Y + floor((py + ky - 1) / 2): offsets
+  // py - 1 + a, a = 0, 1, and the fold adds the taps that land on the same source row (the same for columns).
+  static int fold_dy(int p, int k) { return (p + k + 1) / 2 - 1; }
+  int make_upsample(const std::string& name, int C) {
+    const std::vector<double> W = dvec(name + ".weight"), b = dvec(name + ".bias");
+    for (int q = 0; q < 4; ++q) {
+      const int py = q >> 1, px = q & 1;
+      std::vector<double> Wf((size_t)C * C * 4, 0.0);
+      for (size_t oc = 0; oc < (size_t)C * C; ++oc)
+        for (int ky = 0; ky < 3; ++ky)
+          for (int kx = 0; kx < 3; ++kx) {
+            const int a = fold_dy(py, ky) - py + 1, bb = fold_dy(px, kx) - px + 1;
+            Wf[oc * 4 + a * 2 + bb] += W[oc * 9 + ky * 3 + kx];
+          }
+      if (pack_conv(name + ".p" + std::to_string(q), C, C, 2, Wf, b)) return -1;
+    }
+    return 0;
+  }
+
+  int finalize() {
+    using namespace nope;
+    NOPE_CHECK(!finalized, "already finalized");
+    for (const auto& kv : expected) NOPE_CHECK(host.count(kv.first), "state_dict is missing " + kv.first);
+    NOPE_CUDA(cudaSetDevice(device));
+    {  // post_quant_conv with the 1 / 0.18215 scale folded into its weight in float64; its bias stays separate
+      const auto W = dvec("post_quant_conv.weight");
+      std::vector<float> w(16);
+      for (int i = 0; i < 16; ++i) w[i] = (float)(W[i] / 0.18215);
+      if (upload(&pq_w, w) || upload(&pq_b, h("post_quant_conv.bias"))) return -1;
+    }
+    if (upload(&in_w, h("decoder.conv_in.weight")) || upload(&in_b, h("decoder.conv_in.bias"))) return -1;
+    if (make_resnet("decoder.mid_block.resnets.0", 512, 512) || make_attention(kAttn) ||
+        make_resnet("decoder.mid_block.resnets.1", 512, 512))
+      return -1;
+    int cin = 512;
+    for (int i = 0; i < 4; ++i) {
+      for (int j = 0; j < 3; ++j) {
+        if (make_resnet(up(i) + ".resnets." + std::to_string(j), cin, kCh[i], i == 3)) return -1;
+        cin = kCh[i];
+      }
+      if (i < 3 && make_upsample(up(i) + ".upsamplers.0.conv", kCh[i])) return -1;
+    }
+    if (make_norm("decoder.conv_norm_out") || make_plain("decoder.conv_out", 3)) return -1;
+    host.clear();
+    // workspace for kChunk images of the 256 x 256 x 256 level (the same 3.2 GB as the encoder's)
+    if (alloc_workspace((size_t)kChunk * 256 * 256 * 256)) return -1;
+    finalized = true;
+    return 0;
+  }
+
+  // Upsample2D from side H (residual stream `cur`, plain NHWC) to 2H -> 1 - cur.  One launch per output parity
+  // (py, px), four taps over the source; the zero padding one row / column past the source's edge is the TMA's
+  // out-of-bounds fill.  Into the 256 x 256 level the parity planes are that level's layout; below it they go to
+  // (t32, nrm) and are interleaved into plain NHWC.
+  int upsample(const std::string& name, int C, int H, int n, int& cur, cudaStream_t st) {
+    using namespace nope;
+    const int nxt = 1 - cur;
+    const bool planar = 2 * H == 256;
+    for (int q = 0; q < 4; ++q) {
+      const int py = q >> 1, px = q & 1;
+      std::vector<VaeTap> taps;
+      for (int a = 0; a < 2; ++a)
+        for (int b = 0; b < 2; ++b) taps.push_back(VaeTap{0, py - 1 + a, px - 1 + b});
+      const size_t o = (size_t)q * cap * H * H * C;
+      float* f = (planar ? x32[nxt] : t32) + o;
+      const ActPair d = planar ? ActPair{xs[nxt].hi + o, xs[nxt].lo + o} : ActPair{nrm.hi + o, nrm.lo + o};
+      if (conv(convs.at(name + ".p" + std::to_string(q)), {{xs[cur], -1}}, H, taps, -1, H, n, d.hi, d.lo, f, nullptr,
+               st))
+        return -1;
+    }
+    if (!planar) {
+      vae_dec_repack_kernel<<<ew_grid((long long)n * 4 * H * H * (C / 4)), 256, 0, st>>>(
+          t32, nrm.hi, nrm.lo, C, H, n, cap, x32[nxt], xs[nxt].hi, xs[nxt].lo);
+      NOPE_CUDA(cudaGetLastError());
+      ++launches;
+    }
+    cur = nxt;
+    return 0;
+  }
+
+  // n <= kChunk latents [n, 4, 32, 32] -> images out [n, 3, 256, 256] (unclamped)
+  int decode(const float* z, int n, float* out, cudaStream_t st) {
+    using namespace nope;
+    launches = 0;
+    vae_dec_conv_in_kernel<<<dim3(32, n, 2), 256, 0, st>>>(z, pq_w, pq_b, in_w, in_b, x32[0], xs[0].hi, xs[0].lo);
+    NOPE_CUDA(cudaGetLastError());
+    ++launches;
+    int cur = 0, H = 32, cin = 512;
+    if (resnet("decoder.mid_block.resnets.0", 512, 512, 32, n, cur, st) || attention(kAttn, n, cur, st) ||
+        resnet("decoder.mid_block.resnets.1", 512, 512, 32, n, cur, st))
+      return -1;
+    for (int i = 0; i < 4; ++i) {
+      for (int j = 0; j < 3; ++j) {
+        if (resnet(up(i) + ".resnets." + std::to_string(j), cin, kCh[i], H, n, cur, st)) return -1;
+        cin = kCh[i];
+      }
+      if (i < 3) {
+        if (upsample(up(i) + ".upsamplers.0.conv", kCh[i], H, n, cur, st)) return -1;
+        H *= 2;
+      }
+    }
+    if (group_norm("decoder.conv_norm_out", x32[cur], 128, 256, n, true, st)) return -1;
+    const VaeConv& co = convs.at("decoder.conv_out");
+    if (conv3(co, nrm, 256, n, xs[1 - cur], false, t32, nullptr, nullptr, st)) return -1;
+    vae_dec_extract_kernel<<<ew_grid((long long)n * 3 * 65536), 256, 0, st>>>(t32, co.cout, cap, n, out);
+    NOPE_CUDA(cudaGetLastError());
+    ++launches;
     return 0;
   }
 };

@@ -87,14 +87,26 @@ class PoseConditional:
     @torch.no_grad()
     def sample(self, reference, relativeR):
         reference_feat = self.u_net.encoder.encode_image(reference.to(self.device), mode="mode")
-        return self.u_net(reference_feat, relativeR), None   # template encoder: no decoder
+        pred = self.u_net(reference_feat, relativeR)
+        return pred, self._decode(pred)
 
     # ------------------------------------------------------------------ model.py:193-252
     @torch.no_grad()
     def generate_templates(self, reference, all_relativeR, gt_templates=None, visualize=False):
         reference_feat = self.u_net.encoder.encode_image(reference.to(self.device), mode="mode")
         emb = self.u_net.sweep(reference_feat, all_relativeR, want_emb=True)["emb"]
-        return emb, None, None
+        images = self._decode(emb.flatten(0, 1))
+        if images is not None:
+            images = images.view(*emb.shape[:2], *images.shape[1:])
+        return emb, images, None
+
+    def _decode(self, latents):
+        """unnormalize_to_zero_to_one(decode_latent(latents)) (model.py:119-120, utils.py:12-15) when the encoder is
+        a VAE with its decoder weights; None for the template encoder or a VAE loaded without a decoder."""
+        enc = self.u_net.encoder
+        if not getattr(enc, "has_decoder", False):
+            return None
+        return ((enc.decode_latent(latents) + 1) * 0.5).clamp(0, 1)
 
     # ------------------------------------------------------------------ model.py:254-266
     @torch.no_grad()

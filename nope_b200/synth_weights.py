@@ -396,32 +396,37 @@ def ldm_flops_per_hyp(model_channels=256, channel_mult=(1, 2, 4), num_res_blocks
     return {"gemm": gemm, "attention": attn, "total": gemm + attn}
 
 
-def make_vae_state_dict(seed=0, attention="legacy"):
+def make_vae_state_dict(seed=0, attention="legacy", decoder=False):
     """Seeded AutoencoderKL encoder state_dict (nope_b200.vae.vae_param_shapes, 108 tensors, 34.16 M parameters):
     conv / linear weights and biases U(-1, 1) / sqrt(fan_in) (torch's default init), GroupNorm weights
     1 + 0.2 U(-1, 1) and biases 0.2 U(-1, 1), so activations stay O(1) through the 22 GroupNorms.
     attention="legacy" names the mid-block projections query / key / value / proj_attn (diffusers 0.14),
-    "new" to_q / to_k / to_v / to_out.0; both hold the same tensors."""
-    from .vae import vae_param_shapes
+    "new" to_q / to_k / to_v / to_out.0; both hold the same tensors.  decoder=True appends the 140 decoder tensors
+    (nope_b200.vae.vae_decoder_param_shapes, 49.49 M parameters) with the same rules from a generator of their own,
+    so the encoder tensors are those of decoder=False."""
+    from .vae import vae_decoder_param_shapes, vae_param_shapes
     if attention not in ("legacy", "new"):
         raise ValueError("attention must be 'legacy' or 'new'")
-    g = torch.Generator(device="cpu").manual_seed(5000 + seed)
     rename = {"query.": "to_q.", "key.": "to_k.", "value.": "to_v.", "proj_attn.": "to_out.0."}
-    attn = "encoder.mid_block.attentions.0."
     sd = OrderedDict()
-    fan = {}
-    for k, shape in vae_param_shapes().items():
-        u = torch.rand(shape, generator=g, dtype=torch.float32) * 2 - 1
-        p, leaf = k.rsplit(".", 1)
-        if "norm" in p:
-            t = 1.0 + 0.2 * u if leaf == "weight" else 0.2 * u
-        else:
-            if leaf == "weight":
-                fan[p] = math.prod(shape[1:])
-            t = u / math.sqrt(fan[p])
-        if attention == "new" and k.startswith(attn):
-            for a, b in rename.items():
-                if k[len(attn):].startswith(a):
-                    k = attn + b + k[len(attn) + len(a):]
-        sd[k] = t
+    parts = [(vae_param_shapes(), 5000 + seed, "encoder.mid_block.attentions.0.")]
+    if decoder:
+        parts.append((vae_decoder_param_shapes(), 6000 + seed, "decoder.mid_block.attentions.0."))
+    for shapes, gseed, attn in parts:
+        g = torch.Generator(device="cpu").manual_seed(gseed)
+        fan = {}
+        for k, shape in shapes.items():
+            u = torch.rand(shape, generator=g, dtype=torch.float32) * 2 - 1
+            p, leaf = k.rsplit(".", 1)
+            if "norm" in p:
+                t = 1.0 + 0.2 * u if leaf == "weight" else 0.2 * u
+            else:
+                if leaf == "weight":
+                    fan[p] = math.prod(shape[1:])
+                t = u / math.sqrt(fan[p])
+            if attention == "new" and k.startswith(attn):
+                for a, b in rename.items():
+                    if k[len(attn):].startswith(a):
+                        k = attn + b + k[len(attn) + len(a):]
+            sd[k] = t
     return sd

@@ -1,16 +1,20 @@
-"""Stable Diffusion VAE encoder: image [B,3,256,256] in [-1, 1] -> latent [B,4,32,32].
+"""Stable Diffusion VAE: encoder image [B,3,256,256] in [-1, 1] -> latent [B,4,32,32], decoder back.
 
 Mirrors reference `VAE_StableDiffusion` (src/model/encoder/AutoencoderKL.py:6-47), the encoder of the LDM
 variant (configs/model/vae_cin_ldm.yaml) and of configs/model/vae_base.yaml: `encode_image` is
 diffusers `AutoencoderKL.encode(x).latent_dist.mode() * 0.18215` for the Stable Diffusion v1 VAE
 configuration (SD_V1_CONFIG), computed by the native engine in libnope_b200.so (`nope_vae_*`,
 csrc/vae.cuh, DESIGN.md section 16): every convolution on the wgmma kernel with split-precision fp16
-(hi, lo) operands, fp32-accurate.  There is no CPU path and no decoder (`decode_latent`, the KL
-distribution of `using_KL=True` and the training loss are out of scope).
+(hi, lo) operands, fp32-accurate.  `decode_latent` is diffusers `AutoencoderKL.decode(z / 0.18215).sample`
+(AutoencoderKL.py:44-47), computed by a second engine (`nope_vae_decoder_*`, DESIGN.md section 17) that is
+built on the first decode.  There is no CPU path; the KL distribution of `using_KL=True` and the training
+loss are out of scope.
 
 Weights use the diffusers AutoencoderKL state_dict layout.  The mid-block attention projections are
 accepted under both of diffusers' namings (`query` / `key` / `value` / `proj_attn` and `to_q` / `to_k` /
-`to_v` / `to_out.0`); `decoder.*` and `post_quant_conv.*` entries are ignored.
+`to_v` / `to_out.0`), in the decoder's mid block as in the encoder's.  The decoder's 140 `decoder.*` /
+`post_quant_conv.*` tensors are optional: each one present is checked, and `decode_latent` is available once
+all of them are.
 """
 from collections import OrderedDict
 import ctypes as C
@@ -118,6 +122,89 @@ def map_state_dict(sd):
     return out
 
 
+_DEC_ATTN = "decoder.mid_block.attentions.0."
+# the decoder-side fields of the SD v1 config.json the decoder engine is built for, and diffusers' defaults
+SD_V1_DECODER_CONFIG = {"out_channels": 3, "up_block_types": ["UpDecoderBlock2D"] * 4}
+_DECODER_CONFIG_DEFAULTS = {"out_channels": 3, "up_block_types": ["UpDecoderBlock2D"]}
+
+
+def check_decoder_config(cfg):
+    """Raises ValueError unless `cfg` has the SD v1 decoder fields (out_channels 3, up_block_types
+    4 x UpDecoderBlock2D); the other decoder dimensions are the encoder's fields, which check_config checks."""
+    for k, want in SD_V1_DECODER_CONFIG.items():
+        got = cfg.get(k, _DECODER_CONFIG_DEFAULTS[k])
+        if isinstance(got, tuple):
+            got = list(got)
+        if got != want or type(got) is not type(want):
+            raise ValueError(f"unsupported AutoencoderKL config: {k} = {got!r} (the decoder is built for {want!r})")
+
+
+def vae_decoder_param_shapes():
+    """key -> shape of the 140 AutoencoderKL decoder tensors (post_quant_conv and decoder.*, 0.14-era attention
+    names) the decoder engine loads."""
+    s = OrderedDict()
+
+    def conv(p, cout, cin, k):
+        s[p + ".weight"] = (cout, cin, k, k)
+        s[p + ".bias"] = (cout,)
+
+    def norm(p, c):
+        s[p + ".weight"] = (c,)
+        s[p + ".bias"] = (c,)
+
+    def resnet(p, cin, cout):
+        norm(p + ".norm1", cin)
+        conv(p + ".conv1", cout, cin, 3)
+        norm(p + ".norm2", cout)
+        conv(p + ".conv2", cout, cout, 3)
+        if cin != cout:
+            conv(p + ".conv_shortcut", cout, cin, 1)
+
+    conv("post_quant_conv", 4, 4, 1)
+    conv("decoder.conv_in", 512, 4, 3)
+    resnet("decoder.mid_block.resnets.0", 512, 512)
+    norm(_DEC_ATTN + "group_norm", 512)
+    for n in ("query", "key", "value", "proj_attn"):
+        s[_DEC_ATTN + n + ".weight"] = (512, 512)
+        s[_DEC_ATTN + n + ".bias"] = (512,)
+    resnet("decoder.mid_block.resnets.1", 512, 512)
+    cin = 512
+    for i, c in enumerate(reversed(SD_V1_CONFIG["block_out_channels"])):
+        for j in range(3):
+            resnet(f"decoder.up_blocks.{i}.resnets.{j}", cin, c)
+            cin = c
+        if i < 3:
+            conv(f"decoder.up_blocks.{i}.upsamplers.0.conv", c, c, 3)
+    norm("decoder.conv_norm_out", 128)
+    conv("decoder.conv_out", 3, 128, 3)
+    return s
+
+
+def map_decoder_state_dict(sd):
+    """The `decoder.*` / `post_quant_conv.*` entries of an AutoencoderKL state_dict (either attention naming) ->
+    {schema key: CPU fp32 tensor}; other entries are left to map_state_dict.  Raises KeyError for an unknown key and
+    ValueError for a wrong shape; missing keys are allowed (a checkpoint without a decoder)."""
+    want = vae_decoder_param_shapes()
+    out = {}
+    for k, v in sd.items():
+        if not (k.startswith("decoder.") or k.startswith("post_quant_conv.")):
+            continue
+        kk = k
+        if k.startswith(_DEC_ATTN):
+            rest = k[len(_DEC_ATTN):]
+            for a, b in _ATTN_RENAME.items():
+                if rest.startswith(a):
+                    kk = _DEC_ATTN + b + rest[len(a):]
+        if kk not in want:
+            raise KeyError(f"unexpected AutoencoderKL state_dict key: {k}")
+        if kk in out:
+            raise KeyError(f"AutoencoderKL state_dict has {kk} under both attention namings")
+        if tuple(v.shape) != tuple(want[kk]):
+            raise ValueError(f"size mismatch for {k}: checkpoint {tuple(v.shape)} vs model {tuple(want[kk])}")
+        out[kk] = v.detach().to("cpu", torch.float32).contiguous()
+    return OrderedDict((k, out[k]) for k in want if k in out)
+
+
 def load_pretrained(path):
     """<path>/config.json (checked) and <path>/diffusion_pytorch_model.bin (or .safetensors) -> state_dict."""
     with open(os.path.join(path, "config.json")) as f:
@@ -137,6 +224,7 @@ class VAE_StableDiffusion:
 
     def __init__(self, pretrained_path=None, latent_dim=4, name="vae", using_KL=False, device="cuda:0", **kwargs):
         self._h = None
+        self._dec_h = None
         if using_KL:
             raise ValueError("using_KL=True (the latent distribution of the training-only KL loss) is not supported")
         if latent_dim != 4:
@@ -147,21 +235,43 @@ class VAE_StableDiffusion:
         self.encode_mode = "mode"
         self.device = torch.device(device)
         self._sd = None
+        self._dec_sd = {}
+        self._dec_config_error = None     # why the config.json's decoder fields cannot be decoded, if they cannot
         if pretrained_path is not None:
             self.load_state_dict(load_pretrained(pretrained_path))
+            with open(os.path.join(pretrained_path, "config.json")) as f:
+                try:
+                    check_decoder_config(json.load(f))
+                except ValueError as e:
+                    self._dec_config_error = str(e)
 
     # ------------------------------------------------------------------ weights
     def load_state_dict(self, state_dict, strict=True):
-        """AutoencoderKL keys (see map_state_dict); the engine is rebuilt on the next encode."""
-        self._sd = map_state_dict(state_dict)
+        """AutoencoderKL keys (see map_state_dict and map_decoder_state_dict); the engines are rebuilt on the next
+        encode / decode."""
+        sd = map_state_dict(state_dict)
+        dec = map_decoder_state_dict(state_dict)
+        self._sd, self._dec_sd = sd, dec
         self._drop_engine()
         return self
 
     def state_dict(self):
-        """The module's keys as in the reference (`encoder.` + AutoencoderKL key), encoder tensors only."""
+        """The module's keys as in the reference (`encoder.` + AutoencoderKL key): the encoder tensors, and the
+        decoder's when all of them are loaded."""
         if self._sd is None:
             return {}
-        return {"encoder." + k: v for k, v in self._sd.items()}
+        out = {"encoder." + k: v for k, v in self._sd.items()}
+        if len(self._dec_sd) == len(vae_decoder_param_shapes()):
+            out.update({"encoder." + k: v for k, v in self._dec_sd.items()})
+        return out
+
+    def _missing_decoder_keys(self):
+        return [k for k in vae_decoder_param_shapes() if k not in self._dec_sd]
+
+    @property
+    def has_decoder(self):
+        """True when all 140 decoder tensors are loaded and the config (if any) is the SD v1 decoder's."""
+        return self._dec_config_error is None and not self._missing_decoder_keys()
 
     def to(self, device):
         device = torch.device(device)
@@ -173,14 +283,17 @@ class VAE_StableDiffusion:
     def eval(self):
         return self
 
-    # ------------------------------------------------------------------ native engine
+    # ------------------------------------------------------------------ native engines
     def _drop_engine(self):
-        if self._h is not None:
-            try:
-                _lib.load().nope_vae_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
+        """Destroys both engines (encoder and decoder)."""
+        for attr, fn in (("_h", "nope_vae_destroy"), ("_dec_h", "nope_vae_decoder_destroy")):
+            h = getattr(self, attr, None)
+            if h is not None:
+                try:
+                    getattr(_lib.load(), fn)(h)
+                except Exception:
+                    pass
+                setattr(self, attr, None)
 
     def __del__(self):
         self._drop_engine()
@@ -264,6 +377,52 @@ class VAE_StableDiffusion:
             _lib.check(_lib.load().nope_vae_encode_rotated(
                 self._engine(), _lib.ptr(x), x.shape[0], _lib.ptr(idx), _lib.ptr(cs), P, _lib.ptr(out),
                 self._stream()))
+        return out
+
+    # ------------------------------------------------------------------ decoder
+    def _decoder(self):
+        if self._dec_h is not None:
+            return self._dec_h
+        if self._dec_config_error is not None:
+            raise ValueError(f"decode_latent: {self._dec_config_error}")
+        missing = self._missing_decoder_keys()
+        if missing:
+            raise _lib.NopeError(f"decode_latent needs the AutoencoderKL decoder weights: {len(missing)} of the "
+                                 f"{len(vae_decoder_param_shapes())} decoder tensors are missing, e.g. {missing[:5]}")
+        lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(lib.nope_vae_decoder_create(C.byref(h), self.device.index or 0))
+        try:
+            for k, t in self._dec_sd.items():
+                shape = (C.c_int64 * t.dim())(*t.shape)
+                _lib.check(lib.nope_vae_decoder_load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
+            _lib.check(lib.nope_vae_decoder_finalize(h))
+        except Exception:
+            lib.nope_vae_decoder_destroy(h)
+            raise
+        self._dec_h = h
+        return h
+
+    @property
+    def last_decode_launch_count(self):
+        return int(_lib.load().nope_vae_decoder_last_launch_count(self._dec_h)) if self._dec_h is not None else 0
+
+    @torch.no_grad()
+    def decode_latent(self, latent):
+        """AutoencoderKL.py:44-47: latent [B,4,32,32] (CUDA) -> AutoencoderKL.decode(latent / 0.18215).sample,
+        fp32 [B,3,256,256], not clamped.  The decoder engine is built on the first call."""
+        if self.device.type != "cuda":
+            raise _lib.NopeError("VAE_StableDiffusion needs a CUDA device (no CPU path)")
+        if not isinstance(latent, torch.Tensor) or latent.device.type != "cuda":
+            raise _lib.NopeError("VAE_StableDiffusion decodes CUDA tensors only (no CPU path)")
+        if latent.dim() != 4 or tuple(latent.shape[1:]) != (self.latent_dim, 32, 32) or latent.shape[0] < 1:
+            raise _lib.NopeError(f"the VAE decoder is built for [B, 4, 32, 32] latents, got {tuple(latent.shape)}")
+        h = self._decoder()
+        z = latent.to(device=self.device, dtype=torch.float32).contiguous()
+        out = torch.empty((z.shape[0], 3, 256, 256), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().nope_vae_decoder_decode(h, _lib.ptr(z), z.shape[0], _lib.ptr(out),
+                                                           self._stream()))
         return out
 
 
