@@ -301,7 +301,9 @@ int nope_score_topk_multi(const float* query_feat, const float* emb, int B, int 
                           int metric, float occlusion_threshold, int k, float* out_sim, float* out_topv,
                           int64_t* out_topi, int64_t idx_base, void* stream);
 
-/* Rank an existing similarity matrix sim [B, N] (used to merge per-GPU shards). */
+/* Rank an existing similarity matrix sim [B, N] (used to merge per-GPU shards): top-k per row, descending score,
+ * ties (+0 == -0, inf == inf) -> lowest index, NaN after every number and NaNs by index.  Every ranking call below
+ * uses this order. */
 int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_topi,
               int64_t idx_base, void* stream);
 
@@ -314,8 +316,8 @@ int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_top
  * poses [B, n_fine, 6] of reference r / Q.  A padding slot gets the row's first candidate pose.
  * Requires 1 <= keep <= 64, M >= keep * F and R == B * Q.
  * nope_pose_cells_rank: sim [R, M] scored at cand [R, M] -> top-k over the scored candidates (descending, ties ->
- * lowest fine index; ranks beyond the candidate count get -inf / -1) as fine indices, and optionally out_sim
- * [R, n_fine]: -inf, with the scored entries scattered in.  Requires 1 <= k <= 64. */
+ * lowest fine index, NaN last; ranks beyond the candidate count get -inf / -1) as fine indices, and optionally
+ * out_sim [R, n_fine]: -inf, with the scored entries scattered in.  Requires 1 <= k <= 64. */
 int nope_pose_cells_expand(const int64_t* top_idx, int R, int keep, const int32_t* cells, int n_coarse, int F,
                            const float* poses, int B, int Q, int n_fine, int M,
                            int32_t* out_cand, float* out_poses, void* stream);
@@ -332,8 +334,8 @@ int nope_pose_cells_rank(const float* sim, const int32_t* cand, int R, int M, in
  * A centre whose seed lies outside [0, N) yields 27 padding slots: seed -1, otherwise a copy of the row's first
  * valid candidate.  Requires 1 <= keep <= 64 and R == B * Q.
  * nope_pose_refine_select: sim [R, M] scored at those candidates -> k entries per row, greedily: the highest
- * score first (ties -> lowest slot), skipping padding and any candidate whose trace(rel_a rel_b^T) exceeds
- * trace_threshold against an entry already chosen.  out_D / out_rel (optional) [R, k, 9], out_seed [R, k],
+ * score first (ties -> lowest slot, NaN after every number), skipping padding and any candidate whose
+ * trace(rel_a rel_b^T) exceeds trace_threshold against an entry already chosen.  out_D / out_rel (optional) [R, k, 9], out_seed [R, k],
  * out_score [R, k]; ranks with no candidate left get -inf, seed -1 and zero matrices.
  * Requires 1 <= k <= 64, k <= M <= 64 * 27. */
 int nope_pose_refine_propose(const float* D, const int32_t* seed, int R, int keep, const float* all_relativeR,
@@ -354,9 +356,9 @@ int nope_pose_refine_select(const float* sim, const float* cand_D, const int32_t
  * outside [0, N) gives padding pose slots (seed -1) and three copies of the first valid centre's rho.  Requires
  * 1 <= keep <= 16 and R == B * Q.
  * nope_pose_refine_inplane_select: sim [R, keep * 3, keep * 9] scored at the pairs (angle slot a, pose slot p) ->
- * k entries per row, greedily: the highest score first (ties -> lowest a * keep * 9 + p), skipping pairs with a
- * padding pose slot or angle slot, and any pair whose trace(E E_b^T), E = Rz(rho_a) * rel_p, exceeds
- * trace_threshold against a pair already chosen.  out_D / out_rel (optional) [R, k, 9], out_seed [R, k],
+ * k entries per row, greedily: the highest score first (ties -> lowest a * keep * 9 + p, NaN after every number),
+ * skipping pairs with a padding pose slot or angle slot, and any pair whose trace(E E_b^T), E = Rz(rho_a) * rel_p,
+ * exceeds trace_threshold against a pair already chosen.  out_D / out_rel (optional) [R, k, 9], out_seed [R, k],
  * out_cossin [R, k, 2], out_aslot [R, k] (the angle slot), out_score [R, k]; ranks with no pair left get -inf,
  * seed and aslot -1 and zeros.  Requires 1 <= keep <= 16, 1 <= k <= 64 and k <= 27 * keep^2.
  * Neither call synchronises; both refuse bad arguments before any CUDA call. */
@@ -376,7 +378,7 @@ int nope_pose_refine_inplane_select(const float* sim, const float* cand_D, const
  * nope_topk_pack_floats gives the record length in floats (n_local_max = ceil(N / world)); records sit back to back
  * in the gathered buffer, so the length keeps every record's int64 block 8-byte aligned.
  * nope_topk_merge turns the `world` gathered records (each pack_floats long) into the global top-k
- * per batch row (descending, ties -> lowest index; identical on every rank) and, when has_sim, the
+ * per batch row (descending, ties -> lowest index, NaN last; identical on every rank) and, when has_sim, the
  * full similarity rows [B, N].  Rank r owns poses [r*per, min(N, (r+1)*per)). */
 int64_t nope_topk_pack_floats(int B, int k, int n_local_max, int want_sim);
 int nope_topk_merge(const float* gathered, int world, int64_t pack_floats, int B, int k, int N, int per,

@@ -962,7 +962,20 @@ score_kernel(const float* __restrict__ query, const float* __restrict__ emb,
 }
 
 // ----------------------------------------------------------------------------
-// CTA-wide arg-max of the per-thread candidates (bv, bi): descending value, ties -> lowest index,
+// The order of every ranking kernel: candidate (v, i) ranks before (bv, bi) when v is a number and bv is NaN, or
+// both are numbers and v > bv, or v == bv (+0 == -0, inf == inf) and i < bi, or both are NaN and i < bi.  It is
+// the order of a stable sort of -score, which the oracles use: descending score, ties -> lowest index, NaN last.
+// A total order over distinct indices, so no NaN can stick as a running best or share a rank.
+// ----------------------------------------------------------------------------
+template <typename I>
+__device__ __forceinline__ bool ranks_before(float v, I i, float bv, I bi) {
+  const bool vn = isnan(v), bn = isnan(bv);
+  if (vn || bn) return !vn || (bn && i < bi);
+  return v > bv || (v == bv && i < bi);
+}
+
+// ----------------------------------------------------------------------------
+// CTA-wide arg-max of the per-thread candidates (bv, bi) in the order of ranks_before;
 // bi == 0x7fffffff is "no candidate".  s_v / s_i hold one slot per warp.  The result is valid in
 // thread 0 only; the caller synchronises before it reuses s_v / s_i.
 // ----------------------------------------------------------------------------
@@ -971,7 +984,7 @@ __device__ __forceinline__ void cta_argmax(float& bv, int& bi, float* s_v, int* 
   for (int o = 16; o > 0; o >>= 1) {
     const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
     const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (oi != 0x7fffffff && (bi == 0x7fffffff || ov > bv || (ov == bv && oi < bi))) {
+    if (oi != 0x7fffffff && (bi == 0x7fffffff || ranks_before(ov, oi, bv, bi))) {
       bv = ov;
       bi = oi;
     }
@@ -982,7 +995,7 @@ __device__ __forceinline__ void cta_argmax(float& bv, int& bi, float* s_v, int* 
     for (int w = 1; w < (int)(blockDim.x >> 5); ++w) {
       const float ov = s_v[w];
       const int oi = s_i[w];
-      if (oi != 0x7fffffff && (bi == 0x7fffffff || ov > bv || (ov == bv && oi < bi))) {
+      if (oi != 0x7fffffff && (bi == 0x7fffffff || ranks_before(ov, oi, bv, bi))) {
         bv = ov;
         bi = oi;
       }
@@ -992,7 +1005,8 @@ __device__ __forceinline__ void cta_argmax(float& bv, int& bi, float* s_v, int* 
 
 // ----------------------------------------------------------------------------
 // sim = -(sum of slab partials) and top-k (model.py:265 topk(k=5)); descending score,
-// ties -> lowest index.  One CTA per row (b, q) of sim [B, Q, N]; partial is [B, N, Q, nslab, nparts].
+// ties -> lowest index, NaN last (ranks_before).  One CTA per row (b, q) of sim [B, Q, N]; partial is
+// [B, N, Q, nslab, nparts].
 // idx_base is added to the indices so a shard reports global pose indices.
 // ----------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
@@ -1025,7 +1039,7 @@ sim_topk_kernel(const float* __restrict__ partial, int nslab, float* __restrict_
       for (int c = 0; c < r; ++c) used |= (s_chosen[c] == n);
       if (used) continue;
       const float v = srow[n];
-      if (v > bv || (v == bv && n < bi) || bi == 0x7fffffff) { bv = v; bi = n; }
+      if (bi == 0x7fffffff || ranks_before(v, n, bv, bi)) { bv = v; bi = n; }
     }
     cta_argmax(bv, bi, s_v, s_i);
     if (threadIdx.x == 0) {
@@ -1099,8 +1113,8 @@ pose_cells_expand_kernel(const long long* __restrict__ top_idx, int keep, const 
 // ----------------------------------------------------------------------------
 // Rank one stage of the coarse-to-fine search: one CTA per row of sim [R, M] scored at the fine indices
 // cand [R, M] (-1 = padding, not scored; valid entries distinct).  Top-k over the scored candidates only:
-// descending score, ties -> lowest FINE index; ranks beyond the candidate count get -inf / -1.  out_sim (optional)
-// receives the row over the whole fine grid [R, n_fine]: -inf, then the scored entries scattered in.
+// descending score, ties -> lowest FINE index, NaN last; ranks beyond the candidate count get -inf / -1.  out_sim
+// (optional) receives the row over the whole fine grid [R, n_fine]: -inf, then the scored entries scattered in.
 // ----------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 pose_cells_rank_kernel(const float* __restrict__ sim, const int* __restrict__ cand, int M, int n_fine, int k,
@@ -1130,7 +1144,7 @@ pose_cells_rank_kernel(const float* __restrict__ sim, const int* __restrict__ ca
       for (int i = 0; i < t; ++i) used |= (s_chosen[i] == c);
       if (used) continue;
       const float v = srow[m];
-      if (v > bv || (v == bv && c < bi) || bi == 0x7fffffff) { bv = v; bi = c; }
+      if (bi == 0x7fffffff || ranks_before(v, c, bv, bi)) { bv = v; bi = c; }
     }
     cta_argmax(bv, bi, s_v, s_i);
     if (threadIdx.x == 0) {
@@ -1252,7 +1266,7 @@ pose_refine_select_kernel(const float* __restrict__ sim, const float* __restrict
     for (int m = threadIdx.x; m < M; m += blockDim.x) {
       if (s_dead[m]) continue;
       const float v = srow[m];
-      if (v > bv || (v == bv && m < bi) || bi == 0x7fffffff) { bv = v; bi = m; }
+      if (bi == 0x7fffffff || ranks_before(v, m, bv, bi)) { bv = v; bi = m; }
     }
     cta_argmax(bv, bi, s_v, s_i);
     if (threadIdx.x == 0) s_pick = bi;
@@ -1386,7 +1400,7 @@ pose_refine_inplane_select_kernel(const float* __restrict__ sim, const float* __
     for (int m = threadIdx.x; m < M; m += blockDim.x) {
       if (s_dead[m]) continue;
       const float v = srow[m];
-      if (v > bv || (v == bv && m < bi) || bi == 0x7fffffff) { bv = v; bi = m; }
+      if (bi == 0x7fffffff || ranks_before(v, m, bv, bi)) { bv = v; bi = m; }
     }
     cta_argmax(bv, bi, s_v, s_i);
     if (threadIdx.x == 0) s_pick = bi;
@@ -1442,9 +1456,9 @@ pose_refine_inplane_select_kernel(const float* __restrict__ sim, const float* __
 // Multi-GPU merge (SURVEY.md 8e): every rank contributes ONE packed record to a single all-gather,
 //   [ topv: B*k f32 | pad to even | topi: B*k i64 | sim slice: B*n_local f32 (optional) ]      (`pack` floats)
 // with GLOBAL pose indices (idx -1 = padding).  This kernel turns the W gathered records into the
-// global top-k per batch row (descending score, ties -> lowest index: deterministic, identical on
-// every rank) and the full similarity rows.  One CTA per batch row; candidates W*k <= 1024.
-// rank r owns poses [r*per, min(N, (r+1)*per)).
+// global top-k per batch row (the order of ranks_before: descending score, ties -> lowest index, NaN last;
+// deterministic, identical on every rank) and the full similarity rows.  One CTA per batch row; candidates
+// W*k <= 1024.  rank r owns poses [r*per, min(N, (r+1)*per)).
 // ----------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 topk_merge_kernel(const float* __restrict__ gathered, int world, long long pack, int B, int k, int N, int per,
@@ -1467,12 +1481,11 @@ topk_merge_kernel(const float* __restrict__ gathered, int world, long long pack,
     const float v = s_v[c];
     const long long i = s_i[c];
     if (i < 0) continue;
-    int rank = 0;                                     // candidates that beat this one
+    int rank = 0;                                     // candidates that beat this one: a permutation of the valid ones
     for (int o = 0; o < ncand; ++o) {
       const long long io = s_i[o];
       if (io < 0 || o == c) continue;
-      const float vo = s_v[o];
-      rank += (vo > v || (vo == v && io < i)) ? 1 : 0;
+      rank += ranks_before(s_v[o], io, v, i) ? 1 : 0;
     }
     if (rank < k) {
       top_val[(long long)b * k + rank] = v;

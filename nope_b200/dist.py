@@ -38,14 +38,16 @@ def record_layout(B, k, per, want_sim):
 def merge_topk(vals, idx, k):
     """Torch restatement of the merge rule (CPU tests; oracle of the CUDA kernel): vals/idx
     [W*k', B] candidates (any order, idx -1 = padding) -> top-k per batch row, descending score,
-    ties -> lowest global index."""
+    ties -> lowest global index, NaN after every number; padding (-inf, -1) after every candidate."""
     vals = vals.clone()
     vals[idx < 0] = float("-inf")
     order = torch.sort(idx, dim=0, stable=True).indices           # ascending index first ...
     v1, i1 = torch.gather(vals, 0, order), torch.gather(idx, 0, order)
-    order2 = torch.sort(-v1, dim=0, stable=True).indices          # ... then stable by score
+    order2 = torch.sort(-v1, dim=0, stable=True).indices          # ... then stable by score (NaN last) ...
     v2, i2 = torch.gather(v1, 0, order2), torch.gather(i1, 0, order2)
-    return v2[:k].t().contiguous(), i2[:k].t().contiguous()
+    order3 = torch.sort((i2 < 0).to(torch.uint8), dim=0, stable=True).indices     # ... then padding last
+    v3, i3 = torch.gather(v2, 0, order3), torch.gather(i2, 0, order3)
+    return v3[:k].t().contiguous(), i3[:k].t().contiguous()
 
 
 class ShardedSweep:
