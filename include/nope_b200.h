@@ -257,6 +257,25 @@ int nope_render_depth(const float* vertices, int V, const int32_t* faces, int F,
 int nope_vsd_error(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H, int W,
                    const double* K, double delta, double tau, int cost_type, double* out, void* stream);
 
+/* Translation from the object mask (DESIGN.md section 18).
+ * nope_fit_translation: for F frames and P rotation hypotheses per frame, fit the translation so that the silhouette
+ * of the mesh (vertices [V, 3] fp32, faces [NF, 3] int32, as nope_render_depth) lines up with the frame's mask:
+ * R [F, P, 9] fp64 row-major and t_init [F, P, 3] fp64 (model -> OpenCV camera, mm), masks [F, H, W] uint8 (nonzero =
+ * object), all on the device; K HOST [F, 4] fp64 (fx, fy, cx, cy; finite, fx and fy non-zero), staged in stream order.
+ * Each of the `iters` updates renders [R | t] rounded to fp32 with nope_render_depth's rasterizer, scales t's distance
+ * by sqrt of the ratio of the silhouette's to the mask's box area and moves the origin so that the box centres meet;
+ * an empty silhouette leaves t unchanged.  -> t_out [F, P, 3] fp64, iou [F, P] fp64 = |S n M| / |S u M| of the
+ * silhouette S at t_out (0 when S is empty); both NaN for every hypothesis of a frame whose mask is empty.
+ * stats_out [F, P, 6] int32 (n_S, |S n M|, row0, row1, col0, col1 of S at t_out; an empty box is (INT_MAX, -1)) may be
+ * null.  depth [F P, H, W] fp32 is the caller's workspace; on return it holds nope_render_depth's image at the last
+ * rendered translation of each hypothesis.  Requires V, NF >= 1, 1 <= F, P <= 65535, 1 <= H, W <= 8192, iters >= 0,
+ * znear finite and > 0.  Refuses bad arguments before any CUDA call; all iterations are enqueued without
+ * synchronising the host.  The result does not depend on the batch or on scheduling. */
+int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
+                         const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
+                         float znear, int iters, float* depth, double* t_out, double* iou, int32_t* stats_out,
+                         void* stream);
+
 /* BOP 2019 errors (DESIGN.md section 15).
  * nope_vsd_error_taus: nope_vsd_error at T misalignment tolerances in one pass (the distance images, visibility
  * masks and counts are shared): taus HOST [T] fp64, each finite and > 0, 1 <= T <= 16; K HOST [F, 4] fp64, finite,

@@ -69,6 +69,9 @@ SIGNATURES = {
                                  C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p]),
     "nope_vsd_error_taus": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                       C.c_double, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "nope_fit_translation": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, c_f32p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "nope_pose_errors": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "nope_crop_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

@@ -27,6 +27,7 @@
 #include "render.cuh"
 #include "pose_error.cuh"
 #include "crop.cuh"
+#include "translation.cuh"
 
 using namespace nope;
 
@@ -1890,6 +1891,70 @@ int nope_pose_errors(const float* points, int V, const double* sym, int S, const
   NOPE_CUDA(cudaGetLastError());
   pose_error_kernel<<<dim3((S + kPoseErrSyms - 1) / kPoseErrSyms, P, F), kPoseErrThreads, 0, st>>>(
       points, V, sym, S, gt, est, static_cast<const double*>(k.dev), P, om, op);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// translation from the object mask (translation.cuh, DESIGN.md section 18)
+// ---------------------------------------------------------------------------------
+int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
+                         const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
+                         float znear, int iters, float* depth, double* t_out, double* iou, int32_t* stats_out,
+                         void* stream) {
+  NOPE_CHECK(vertices && faces && R && t_init && masks && K && depth && t_out && iou, "null argument");
+  NOPE_CHECK(V >= 1 && NF >= 1, "V and NF must be >= 1");
+  NOPE_CHECK(F >= 1 && F <= 65535 && P >= 1 && P <= 65535, "F and P must be in [1, 65535]");
+  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
+  NOPE_CHECK(iters >= 0, "iters must be >= 0");
+  NOPE_CHECK(znear > 0.f && std::isfinite(znear), "znear must be finite and > 0");
+  if (check_host_intrinsics(K, F)) return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  StagedHost k;
+  if (k.upload(K, sizeof(double) * 4 * (size_t)F, st)) return -1;
+  const double* kd = static_cast<const double*>(k.dev);
+  // stream-ordered scratch: the current translations, the float32 poses and the integer statistics
+  const size_t n = (size_t)F * P;
+  StagedHost scratch;
+  const size_t t_bytes = sizeof(double) * 3 * n, pose_bytes = sizeof(float) * 16 * n;
+  const size_t stat_bytes = sizeof(int) * kFitStats * (n + F);
+  scratch.st = st;
+  NOPE_CUDA(cudaMallocAsync(&scratch.dev, t_bytes + pose_bytes + stat_bytes, st));
+  double* t = static_cast<double*>(scratch.dev);
+  float* poses = reinterpret_cast<float*>(static_cast<char*>(scratch.dev) + t_bytes);
+  int* sil_stats = reinterpret_cast<int*>(static_cast<char*>(scratch.dev) + t_bytes + pose_bytes);
+  int* mask_stats = sil_stats + kFitStats * n;
+  const int ew_blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 16);
+  fit_init_kernel<<<ew_blocks, 256, 0, st>>>(R, t_init, F, P, t, poses, sil_stats, mask_stats);
+  NOPE_CUDA(cudaGetLastError());
+  const long long hw = (long long)H * W;
+  const int stat_blocks = (int)((hw + kFitPixelsPerCta - 1) / kFitPixelsPerCta);
+  fit_stats_kernel<false><<<dim3(stat_blocks, 1, F), kFitThreads, 0, st>>>(nullptr, masks, P, H, W, mask_stats);
+  NOPE_CUDA(cudaGetLastError());
+  unsigned* z = reinterpret_cast<unsigned*>(depth);
+  const long long nz = (long long)n * hw;
+  const int fill_blocks = (int)std::min<long long>((nz + 255) / 256, 132LL * 16);
+  for (int it = 0; it <= iters; ++it) {
+    // the rasterizer of nope_render_depth, one launch per frame over its P poses (K differs per frame)
+    depth_fill_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);
+    NOPE_CUDA(cudaGetLastError());
+    for (int f = 0; f < F; ++f) {
+      const double* kf = K + 4 * (size_t)f;
+      depth_raster_kernel<<<dim3((NF + 7) / 8, P), 256, 0, st>>>(
+          vertices, V, faces, NF, poses + 16 * (size_t)f * P, (float)kf[0], (float)kf[1], (float)kf[2], (float)kf[3],
+          znear, H, W, z + (size_t)f * P * hw);
+      NOPE_CUDA(cudaGetLastError());
+    }
+    fit_stats_kernel<true><<<dim3(stat_blocks, P, F), kFitThreads, 0, st>>>(z, masks, P, H, W, sil_stats);
+    NOPE_CUDA(cudaGetLastError());
+    if (it < iters) {
+      fit_update_kernel<<<ew_blocks, 256, 0, st>>>(R, kd, mask_stats, F, P, t, poses, sil_stats);
+      NOPE_CUDA(cudaGetLastError());
+    }
+  }
+  fit_final_kernel<<<ew_blocks, 256, 0, st>>>(t, mask_stats, sil_stats, F, P, t_out, iou, stats_out);
+  NOPE_CUDA(cudaGetLastError());
+  depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);      // depth holds render_depth at the returned t
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }

@@ -469,10 +469,10 @@ class PoseConditional:
         k = nearest_idx.shape[1]
         return tp[torch.arange(B, device=dev)[:, None].expand(B, k), nearest_idx]
 
-    def _render_frames(self, batch, B, ids, R):
+    def _render_frames(self, batch, B, ids, R, t_est=None):
         """The sensor depth of every frame and the model rendered at the ground-truth pose and at the rotations R
-        [B, k, 3, 3] with the ground-truth translation: -> (depth_test [B, H, W] float64, rendered [B, 1 + k, H, W],
-        K [B, 3, 3] float64 on the host, K4 [B, 4] on the device)."""
+        [B, k, 3, 3] with the ground-truth translation, or with t_est [B, k, 3] when given: -> (depth_test [B, H, W]
+        float64, rendered [B, 1 + k, H, W], K [B, 3, 3] float64 on the host, K4 [B, 4] on the device)."""
         import numpy as np
         from . import vsd as _vsd
         dev = self.device
@@ -482,6 +482,8 @@ class PoseConditional:
         poses[:, 0, :3, :3] = batch["query_pose"].to(dev, torch.float32)
         poses[:, 1:, :3, :3] = R
         poses[:, :, :3, 3] = t[:, None, :, 0]
+        if t_est is not None:
+            poses[:, 1:, :3, 3] = t_est
         poses[:, :, 3, 3] = 1.0
         # vsd.py:72-74: the intrinsics and the sensor depth of every frame (PNG / 10.0), read on the host
         import cv2
@@ -512,13 +514,52 @@ class PoseConditional:
         return self
 
     @torch.no_grad()
-    def eval_bop(self, batch, data_name, R_est=None, save_path=None):
+    def estimate_translation(self, batch, R, masks, iters=4):
+        """The translation of every rotation hypothesis R [B, k, 3, 3] of a T-LESS batch (the `eval_vsd` schema; its
+        "intrinsic" and "obj_id" are used) fitted to the object's mask of each frame, masks [B, H, W] (uint8 or bool,
+        nonzero = object), starting from `translation.initial_translation` with the object's diameter
+        (load_models_info) and the mesh of load_mesh; DESIGN.md section 18.  One call per distinct object.
+        -> (t float64 [B, k, 3] mm, iou float64 [B, k]) on the model's device, without synchronising."""
+        import numpy as np
+        from . import translation
+        for key in ("intrinsic", "obj_id"):
+            if key not in batch:
+                raise KeyError(f"estimate_translation: the batch has no {key!r}")
+        ids = [int(i) for i in batch["obj_id"].reshape(-1).tolist()]
+        B = len(ids)
+        R = torch.as_tensor(np.asarray(R) if not torch.is_tensor(R) else R)
+        if R.dim() != 4 or R.shape[0] != B or R.shape[2:] != (3, 3) or R.shape[1] < 1:
+            raise ValueError(f"estimate_translation: R [B, k, 3, 3] with B = {B} expected, got {tuple(R.shape)}")
+        masks = torch.as_tensor(np.asarray(masks) if not torch.is_tensor(masks) else masks)
+        if masks.dim() != 3 or masks.shape[0] != B:
+            raise ValueError(f"estimate_translation: masks [B, H, W] with B = {B} expected, got {tuple(masks.shape)}")
+        missing = sorted(set(i for i in ids if i not in self.tless_cad or i not in self.bop_models))
+        if missing:
+            raise ValueError(f"estimate_translation: no mesh or models_info entry for obj_id {missing} "
+                             "(load_mesh, load_models_info)")
+        K = batch["intrinsic"].detach().cpu().to(torch.float64).reshape(B, 3, 3)
+        dev = self.device
+        t = torch.empty((B, R.shape[1], 3), device=dev, dtype=torch.float64)
+        iou = torch.empty((B, R.shape[1]), device=dev, dtype=torch.float64)
+        for obj in sorted(set(ids)):
+            ri = torch.tensor([b for b in range(B) if ids[b] == obj], dtype=torch.int64)
+            rd = ri.pin_memory().to(dev, non_blocking=True)
+            rm = rd if masks.device.type == "cuda" else ri
+            rr = rd if R.device.type == "cuda" else ri
+            t[rd], iou[rd] = translation.estimate_translation(
+                self.tless_cad[obj], R[rr], K[ri], masks[rm], diameter=self.bop_models[obj]["diameter"], iters=iters)
+        return t, iou
+
+    @torch.no_grad()
+    def eval_bop(self, batch, data_name, R_est=None, save_path=None, t_est=None):
         """BOP 2019 average recall of a T-LESS batch (the `eval_vsd` schema): the grid retrieval's top-5 rotations, or
-        R_est [B, k, 3, 3] from any search, at the ground-truth translation.  Each frame is rendered once (ground
-        truth and k estimates); one multi-tau VSD call (tau = 0.05 ... 0.5 x diameter) and one pose_errors call per
-        distinct object.  Logs and returns {"top kk, ar_vsd" / "ar_mssd" / "ar_mspd" / "ar"} for kk in {1, 3, 5}
-        (up to k): the per-metric minimum over the first kk estimates; kk = 1 is the BOP figure.  Saves the errors
-        (vsd [B, k, 10], mssd [B, k], mspd [B, k], obj_id [B]) to save_path (.npz) when given."""
+        R_est [B, k, 3, 3] from any search, at the ground-truth translation, or at t_est [B, k, 3] (mm, e.g. from
+        `estimate_translation`) when given: the estimates are then rendered, and MSSD / MSPD computed, at t_est; the
+        ground truth keeps its pose.  Each frame is rendered once (ground truth and k estimates); one multi-tau VSD
+        call (tau = 0.05 ... 0.5 x diameter) and one pose_errors call per distinct object.  Logs and returns
+        {"top kk, ar_vsd" / "ar_mssd" / "ar_mspd" / "ar"} for kk in {1, 3, 5} (up to k): the per-metric minimum over
+        the first kk estimates; kk = 1 is the BOP figure.  Saves the errors (vsd [B, k, 10], mssd [B, k], mspd [B, k],
+        obj_id [B]) to save_path (.npz) when given."""
         import numpy as np
         from . import bop
         from . import vsd as _vsd
@@ -534,7 +575,12 @@ class PoseConditional:
                 raise ValueError(f"eval_bop: R_est [B, k, 3, 3] with B = {B} expected, got {tuple(R.shape)}")
             R = R.to(self.device)
         k = R.shape[1]
-        depth_test, rendered, K, K4 = self._render_frames(batch, B, ids, R)
+        if t_est is not None:
+            t_est = torch.as_tensor(np.asarray(t_est) if not torch.is_tensor(t_est) else t_est)
+            if tuple(t_est.shape) != (B, k, 3):
+                raise ValueError(f"eval_bop: t_est [{B}, {k}, 3] expected, got {tuple(t_est.shape)}")
+            t_est = bop._to_dev(t_est, self.device, torch.float64)
+        depth_test, rendered, K, K4 = self._render_frames(batch, B, ids, R, t_est)
         W = depth_test.shape[2]
         dev = rendered.device
         vsd = torch.empty((B, k, len(bop.VSD_TAUS)), device=dev, dtype=torch.float64)
@@ -552,8 +598,8 @@ class PoseConditional:
             info = self.bop_models[obj]
             vsd[rd] = _vsd.vsd_errors(depth_test[rd], rendered[rd, 0], rendered[rd, 1:], K[ri],
                                       tau=bop.VSD_TAUS * info["diameter"])
-            e_mssd, e_mspd = bop.pose_errors(self.tless_cad[obj].vertices, R[rd], t_gt[rd], R_gt[rd], t_gt[rd], K[ri],
-                                             info["symmetries"])
+            e_mssd, e_mspd = bop.pose_errors(self.tless_cad[obj].vertices, R[rd], t_gt[rd] if t_est is None else
+                                             t_est[rd], R_gt[rd], t_gt[rd], K[ri], info["symmetries"])
             mssd[rd], mspd[rd] = e_mssd, e_mspd
         vsd, mssd, mspd = vsd.cpu().numpy(), mssd.cpu().numpy(), mspd.cpu().numpy()
         final_scores = {}
