@@ -15,10 +15,6 @@ SIGNATURES = {
     "nope_last_error": (C.c_char_p, []),
     "nope_abi_version": (C.c_int, []),
     "nope_build_arch": (C.c_char_p, []),
-    "nope_unet_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]),
-    "nope_unet_destroy": (None, [C.c_void_p]),
-    "nope_unet_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.POINTER(C.c_int64), C.c_int]),
-    "nope_unet_finalize": (C.c_int, [C.c_void_p]),
     "nope_unet_set_chunk": (C.c_int, [C.c_void_p, C.c_int]),
     "nope_unet_set_conv_impl": (C.c_int, [C.c_void_p, C.c_int]),
     "nope_unet_sweep": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, c_f32p,
@@ -36,10 +32,6 @@ SIGNATURES = {
     "nope_op_conv_gn_fused": (C.c_int, [C.c_int, C.c_int, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, c_f32p,
                                         c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, c_f32p, C.c_int, c_f32p,
                                         c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    "nope_encoder_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int]),
-    "nope_encoder_destroy": (None, [C.c_void_p]),
-    "nope_encoder_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.POINTER(C.c_int64), C.c_int]),
-    "nope_encoder_finalize": (C.c_int, [C.c_void_p]),
     "nope_encoder_encode": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_void_p]),
     "nope_encoder_last_launch_count": (C.c_int64, [C.c_void_p]),
     "nope_inplane_rotate": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, c_f32p, C.c_void_p]),
@@ -48,19 +40,11 @@ SIGNATURES = {
                                             C.c_void_p]),
     "nope_encoder_encode_rotated": (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_void_p, c_f32p, C.c_int, c_f32p,
                                               C.c_void_p]),
-    "nope_vae_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int]),
-    "nope_vae_destroy": (None, [C.c_void_p]),
-    "nope_vae_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.POINTER(C.c_int64), C.c_int]),
-    "nope_vae_finalize": (C.c_int, [C.c_void_p]),
     "nope_vae_encode": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_void_p]),
     "nope_vae_encode_inplane": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, C.c_void_p]),
     "nope_vae_encode_rotated": (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_void_p, c_f32p, C.c_int, c_f32p,
                                           C.c_void_p]),
     "nope_vae_last_launch_count": (C.c_int64, [C.c_void_p]),
-    "nope_vae_decoder_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int]),
-    "nope_vae_decoder_destroy": (None, [C.c_void_p]),
-    "nope_vae_decoder_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.POINTER(C.c_int64), C.c_int]),
-    "nope_vae_decoder_finalize": (C.c_int, [C.c_void_p]),
     "nope_vae_decoder_decode": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_void_p]),
     "nope_vae_decoder_last_launch_count": (C.c_int64, [C.c_void_p]),
     "nope_render_depth":(C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_int, C.c_float, C.c_float,
@@ -110,10 +94,6 @@ SIGNATURES = {
     "nope_op_linear_attention": (C.c_int, [C.c_int, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_op_attention": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_op_upsample2x": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    "nope_ldm_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
-    "nope_ldm_destroy": (None, [C.c_void_p]),
-    "nope_ldm_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.POINTER(C.c_int64), C.c_int]),
-    "nope_ldm_finalize": (C.c_int, [C.c_void_p]),
     "nope_ldm_set_chunk": (C.c_int, [C.c_void_p, C.c_int]),
     "nope_ldm_set_impl": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
     "nope_ldm_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
@@ -133,6 +113,16 @@ SIGNATURES = {
     "nope_unet_debug_tap": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_char_p, c_f32p,
                                       C.c_int64, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
 }
+
+# the lifecycle entries of the five weight-holding engines: kind -> nope_<kind>_create's arguments after the out handle
+ENGINE_CREATE_ARGS = {"unet": 4, "encoder": 2, "vae": 1, "vae_decoder": 1, "ldm": 5}
+for _kind, _n in ENGINE_CREATE_ARGS.items():
+    SIGNATURES.update({
+        f"nope_{_kind}_create": (C.c_int, [C.POINTER(C.c_void_p)] + [C.c_int] * _n),
+        f"nope_{_kind}_destroy": (None, [C.c_void_p]),
+        f"nope_{_kind}_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.POINTER(C.c_int64), C.c_int]),
+        f"nope_{_kind}_finalize": (C.c_int, [C.c_void_p]),
+    })
 
 EXPECTED_ABI = 2     # include/nope_b200.h "ABI version"; a stale build with other signatures must not bind
 
@@ -186,3 +176,27 @@ def check(rc):
 def ptr(t):
     """Device/host pointer of a torch tensor (None -> NULL)."""
     return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def build_engine(kind, create_args, tensors, configure=None):
+    """Builds a `kind` engine ("unet", "encoder", "vae", "vae_decoder" or "ldm"): nope_<kind>_create(&h,
+    *create_args), then configure(lib, h) (options that must precede the weights), then every (key, tensor) of
+    `tensors` staged as contiguous CPU fp32, then nope_<kind>_finalize.  Returns the handle; if any step raises, the
+    engine is destroyed first."""
+    import torch
+    lib = load()
+    h = C.c_void_p()
+    check(getattr(lib, f"nope_{kind}_create")(C.byref(h), *create_args))
+    try:
+        if configure is not None:
+            configure(lib, h)
+        load_tensor = getattr(lib, f"nope_{kind}_load_tensor")
+        for k, v in tensors:
+            t = v.detach().to("cpu", torch.float32).contiguous()
+            shape = (C.c_int64 * t.dim())(*t.shape)
+            check(load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
+        check(getattr(lib, f"nope_{kind}_finalize")(h))
+    except BaseException:
+        getattr(lib, f"nope_{kind}_destroy")(h)
+        raise
+    return h

@@ -16,6 +16,7 @@
 // TMA maps (same trick as HardDownsample).  65 GFLOP per image in fp32 terms, 195 executed.
 #pragma once
 #include "conv_tc2.cuh"
+#include "engine.cuh"
 #include "kernels.cuh"
 
 #include <cmath>
@@ -154,65 +155,59 @@ struct ActPair {
 }  // namespace nope
 
 struct nope_encoder {
+  static constexpr const char* kName = "encoder";
   int D = 8, device = 0, num_sms = 132;
   bool finalized = false;
-  std::map<std::string, std::pair<std::vector<int64_t>, std::vector<float>>> host;
-  std::map<std::string, std::vector<int64_t>> expected;
+  nope::StagedWeights staged;
   std::map<std::string, nope::EncConv> convs;
   float *stem_w = nullptr, *stem_b = nullptr;
-  std::vector<void*> owned;
+  nope::DeviceAllocs mem;             // weights, rot_stage
   int cap = 0;
   nope::ActPair buf[5];
   float* proj_out = nullptr;
-  std::vector<void*> ws_owned;
+  nope::DeviceAllocs ws_mem;          // workspace for cap images (ensure_workspace)
   std::map<std::tuple<const void*, int, int, int, int>, CUtensorMap> tmaps;
   int64_t launches = 0;
   static constexpr int kChunk = 32;   // images per encode() call: the workspace holds this many
   float* rot_stage = nullptr;         // kChunk rotated 256x256 crops (25 MB), allocated by the first encode_inplane
 
-  ~nope_encoder() {
-    for (void* p : owned) cudaFree(p);
-    for (void* p : ws_owned) cudaFree(p);
-    if (rot_stage) cudaFree(rot_stage);
-  }
-
   // ---------------------------------------------------------------- schema (resnet.py:93-133)
   void expect_bn(const std::string& p, int c) {
-    for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) expected[p + s] = {c};
+    for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) staged.expect(p + s, {c});
   }
   void build_schema() {
-    expected["backbone.conv1.weight"] = {64, 3, 7, 7};
+    staged.expect("backbone.conv1.weight", {64, 3, 7, 7});
     expect_bn("backbone.bn1", 64);
     int inplanes = 64;
     const int planes[4] = {64, 128, 256, 512}, blocks[4] = {3, 4, 6, 3}, strides[4] = {1, 2, 2, 1};
     for (int li = 0; li < 4; ++li)
       for (int b = 0; b < blocks[li]; ++b) {
         const std::string p = "backbone.layer" + std::to_string(li + 1) + "." + std::to_string(b);
-        expected[p + ".conv1.weight"] = {planes[li], inplanes, 1, 1};
+        staged.expect(p + ".conv1.weight", {planes[li], inplanes, 1, 1});
         expect_bn(p + ".bn1", planes[li]);
-        expected[p + ".conv2.weight"] = {planes[li], planes[li], 3, 3};
+        staged.expect(p + ".conv2.weight", {planes[li], planes[li], 3, 3});
         expect_bn(p + ".bn2", planes[li]);
-        expected[p + ".conv3.weight"] = {planes[li] * 4, planes[li], 1, 1};
+        staged.expect(p + ".conv3.weight", {planes[li] * 4, planes[li], 1, 1});
         expect_bn(p + ".bn3", planes[li] * 4);
         if (b == 0 && (strides[li] != 1 || inplanes != planes[li] * 4)) {
-          expected[p + ".downsample.0.weight"] = {planes[li] * 4, inplanes, 1, 1};
+          staged.expect(p + ".downsample.0.weight", {planes[li] * 4, inplanes, 1, 1});
           expect_bn(p + ".downsample.1", planes[li] * 4);
         }
         inplanes = planes[li] * 4;
       }
-    expected["projector.1.weight"] = {256, 2048, 1, 1};
-    expected["projector.3.weight"] = {D, 256, 1, 1};
+    staged.expect("projector.1.weight", {256, 2048, 1, 1});
+    staged.expect("projector.3.weight", {D, 256, 1, 1});
   }
 
   // ---------------------------------------------------------------- weights
   // fold eval-mode BN (eps 1e-5) into the conv in double, split into fp16 (hi, lo), pack
   int make_conv(const std::string& name, const std::string& wkey, const std::string& bnkey, int stride) {
     using namespace nope;
-    const auto& W = host.at(wkey);
+    const HostTensor& W = staged.at(wkey);
     EncConv L;
-    L.cout_real = (int)W.first[0];
-    L.cin = (int)W.first[1];
-    L.k = (int)W.first[2];
+    L.cout_real = (int)W.shape[0];
+    L.cin = (int)W.shape[1];
+    L.k = (int)W.shape[2];
     L.stride = stride;
     L.cout = (L.cout_real + 63) / 64 * 64;
     const int taps = L.k * L.k;
@@ -221,8 +216,8 @@ struct nope_encoder {
     L.bn = pick_bn(L.cout);
     std::vector<double> scale(L.cout_real, 1.0), shift(L.cout_real, 0.0);
     if (!bnkey.empty()) {
-      const auto &g = host.at(bnkey + ".weight").second, &b = host.at(bnkey + ".bias").second,
-                 &m = host.at(bnkey + ".running_mean").second, &v = host.at(bnkey + ".running_var").second;
+      const auto &g = staged.at(bnkey + ".weight").data, &b = staged.at(bnkey + ".bias").data,
+                 &m = staged.at(bnkey + ".running_mean").data, &v = staged.at(bnkey + ".running_var").data;
       for (int o = 0; o < L.cout_real; ++o) {
         scale[o] = (double)g[o] / std::sqrt((double)v[o] + 1e-5);
         shift[o] = (double)b[o] - (double)m[o] * scale[o];
@@ -232,7 +227,7 @@ struct nope_encoder {
     for (int o = 0; o < L.cout_real; ++o)
       for (int c = 0; c < L.cin; ++c)
         for (int t = 0; t < taps; ++t) {
-          const float wf = (float)((double)W.second[((size_t)o * L.cin + c) * taps + t] * scale[o]);
+          const float wf = (float)((double)W.data[((size_t)o * L.cin + c) * taps + t] * scale[o]);
           const __half hi = __float2half_rn(wf);
           const __half lo = __float2half_rn(wf - __half2float(hi));
           __half* dst = &packed[(size_t)o * L.K + (size_t)t * 3 * L.cin];
@@ -240,40 +235,27 @@ struct nope_encoder {
           dst[L.cin + c] = lo;
           dst[2 * L.cin + c] = hi;
         }
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&L.w), packed.size() * sizeof(__half)));
-    owned.push_back(L.w);
-    NOPE_CUDA(cudaMemcpy(L.w, packed.data(), packed.size() * sizeof(__half), cudaMemcpyHostToDevice));
     std::vector<float> bias(L.cout, 0.f);
     for (int o = 0; o < L.cout_real; ++o) bias[o] = (float)shift[o];
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&L.bias), bias.size() * sizeof(float)));
-    owned.push_back(L.bias);
-    NOPE_CUDA(cudaMemcpy(L.bias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice));
+    if (mem.upload(&L.w, packed) || mem.upload(&L.bias, bias)) return -1;
     if (make_weight_map(&L.wmap, L.w, L.cout, L.K, L.bn)) return -1;
     convs[name] = L;
     return 0;
   }
 
+  // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
   int finalize() {
-    using namespace nope;
-    NOPE_CHECK(!finalized, "already finalized");
-    for (const auto& kv : expected) NOPE_CHECK(host.count(kv.first), "state_dict is missing " + kv.first);
-    NOPE_CUDA(cudaSetDevice(device));
     {  // stem: fold bn1 into conv1, keep fp32
-      const auto& W = host.at("backbone.conv1.weight").second;
-      const auto &g = host.at("backbone.bn1.weight").second, &b = host.at("backbone.bn1.bias").second,
-                 &m = host.at("backbone.bn1.running_mean").second, &v = host.at("backbone.bn1.running_var").second;
+      const auto& W = staged.at("backbone.conv1.weight").data;
+      const auto &g = staged.at("backbone.bn1.weight").data, &b = staged.at("backbone.bn1.bias").data,
+                 &m = staged.at("backbone.bn1.running_mean").data, &v = staged.at("backbone.bn1.running_var").data;
       std::vector<float> w(64 * 147), bias(64);
       for (int o = 0; o < 64; ++o) {
         const double s = (double)g[o] / std::sqrt((double)v[o] + 1e-5);
         for (int i = 0; i < 147; ++i) w[o * 147 + i] = (float)((double)W[o * 147 + i] * s);
         bias[o] = (float)((double)b[o] - (double)m[o] * s);
       }
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&stem_w), w.size() * 4));
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&stem_b), bias.size() * 4));
-      owned.push_back(stem_w);
-      owned.push_back(stem_b);
-      NOPE_CUDA(cudaMemcpy(stem_w, w.data(), w.size() * 4, cudaMemcpyHostToDevice));
-      NOPE_CUDA(cudaMemcpy(stem_b, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice));
+      if (mem.upload(&stem_w, w) || mem.upload(&stem_b, bias)) return -1;
     }
     const int blocks[4] = {3, 4, 6, 3}, strides[4] = {1, 2, 2, 1};
     for (int li = 0; li < 4; ++li)
@@ -283,34 +265,24 @@ struct nope_encoder {
         if (make_conv(p + ".conv1", p + ".conv1.weight", p + ".bn1", 1)) return -1;
         if (make_conv(p + ".conv2", p + ".conv2.weight", p + ".bn2", st)) return -1;   // resnet.py:62
         if (make_conv(p + ".conv3", p + ".conv3.weight", p + ".bn3", 1)) return -1;
-        if (host.count(p + ".downsample.0.weight"))
+        if (staged.has(p + ".downsample.0.weight"))
           if (make_conv(p + ".down", p + ".downsample.0.weight", p + ".downsample.1", st)) return -1;
       }
     if (make_conv("projector.1", "projector.1.weight", "", 1)) return -1;
-    if (make_conv("projector.3", "projector.3.weight", "", 1)) return -1;
-    host.clear();
-    finalized = true;
-    return 0;
+    return make_conv("projector.3", "projector.3.weight", "", 1);
   }
 
   // ---------------------------------------------------------------- workspace / maps
   int ensure_workspace(int B) {
     if (B <= cap) return 0;
     NOPE_CUDA(cudaDeviceSynchronize());
-    for (void* p : ws_owned) cudaFree(p);
-    ws_owned.clear();
+    ws_mem.release();
     tmaps.clear();
     cap = B;
     const size_t n = (size_t)cap * 128 * 128 * 256;     // largest activation: layer1 output
-    for (auto& b : buf) {
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&b.hi), n * sizeof(__half)));
-      ws_owned.push_back(b.hi);
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&b.lo), n * sizeof(__half)));
-      ws_owned.push_back(b.lo);
-    }
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&proj_out), (size_t)cap * 1024 * 64 * sizeof(float)));
-    ws_owned.push_back(proj_out);
-    return 0;
+    for (auto& b : buf)
+      if (ws_mem.alloc(&b.hi, n) || ws_mem.alloc(&b.lo, n)) return -1;
+    return ws_mem.alloc(&proj_out, (size_t)cap * 1024 * 64);
   }
   int get_map(const CUtensorMap** out, const void* base, int C, const nope::TileGeom& g, int kind) {
     using namespace nope;
@@ -458,9 +430,7 @@ struct nope_encoder {
   int encode_inplane(const float* images, int B, const float* cossin, int A, float* out, cudaStream_t st) {
     using namespace nope;
     constexpr long long kImg = 3LL * 256 * 256;
-    if (!rot_stage) {
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&rot_stage), kChunk * kImg * sizeof(float)));
-    }
+    if (!rot_stage && mem.alloc(&rot_stage, kChunk * kImg)) return -1;
     NOPE_CHECK((int64_t)B * A <= INT32_MAX, "too many (image, angle) pairs");
     const int pairs = B * A;
     int64_t total = 0;
@@ -481,9 +451,7 @@ struct nope_encoder {
                      cudaStream_t st) {
     using namespace nope;
     constexpr long long kImg = 3LL * 256 * 256;
-    if (!rot_stage) {
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&rot_stage), kChunk * kImg * sizeof(float)));
-    }
+    if (!rot_stage && mem.alloc(&rot_stage, kChunk * kImg)) return -1;
     int64_t total = 0;
     for (int lo = 0; lo < P; lo += kChunk) {
       const int n = P - lo < kChunk ? P - lo : kChunk;

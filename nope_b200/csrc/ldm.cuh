@@ -20,11 +20,13 @@
 // Every GEMM-shaped op runs on conv_tc2_kernel.
 #pragma once
 #include "conv_tc2.cuh"
+#include "engine.cuh"
 #include "kernels.cuh"
 #include "ldm_kernels.cuh"
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <map>
 #include <memory>
 #include <string>
@@ -63,7 +65,8 @@ __global__ void ldm_ref_of_kernel(int* r, int h0, int N, int n) {
 }  // namespace nope
 
 struct nope_ldm {
-  using HostT = std::pair<std::vector<int64_t>, std::vector<float>>;
+  using HostTensor = nope::HostTensor;
+  static constexpr const char* kName = "LDM";
   int mc = 256, ctx = 512, Cl = 4, S0 = 32, rot_dim = 6, device = 0, num_sms = 132;
   int nres = 2;
   std::vector<int> mult{1, 2, 4};
@@ -79,15 +82,14 @@ struct nope_ldm {
   std::vector<nope::LdmBlock> inp, outp;
   int mid_ch = 0;
 
-  std::map<std::string, HostT> host;
-  std::map<std::string, std::vector<int64_t>> expected;
+  nope::StagedWeights staged;
   std::map<std::string, nope::LdmConv> convs;
   std::map<std::string, nope::LdmNorm> norms;
   std::map<std::string, int> cb_off;   // transformer prefix -> offset in the cross-term vector
   int cb_width = 0;
   float *cross_w = nullptr, *cross_b = nullptr;      // [cb_width][6], [cb_width]
   float *in_w = nullptr, *in_b = nullptr;
-  std::vector<void*> owned;
+  nope::DeviceAllocs mem;                      // weights
 
   // workspace (per chunk of `cap` hypotheses; `cap_ref` reference latents)
   int cap = 0, cap_ref = 0;
@@ -103,7 +105,7 @@ struct nope_ldm {
   size_t score_partial_cap = 0;
   float* sim_buf = nullptr;
   size_t sim_buf_cap = 0;
-  std::vector<void*> ws_owned;
+  nope::DeviceAllocs ws_mem;                   // workspace for cap hypotheses, cap_ref references (ensure_workspace)
   std::map<std::tuple<const void*, int, int, int, int>, CUtensorMap> tmaps;
   std::map<std::tuple<const void*, int, int, int>, CUtensorMap> tmaps3;
 
@@ -137,8 +139,6 @@ struct nope_ldm {
   bool tap_hit = false;
 
   ~nope_ldm() {
-    for (void* p : owned) cudaFree(p);
-    for (void* p : ws_owned) cudaFree(p);
     if (score_partial) cudaFree(score_partial);
     if (sim_buf) cudaFree(sim_buf);
     for (cudaEvent_t e : prof_ev) cudaEventDestroy(e);
@@ -173,7 +173,7 @@ struct nope_ldm {
         ch = mc * mult[level];
       }
   }
-  void expect(const std::string& k, std::vector<int64_t> s) { expected[k] = std::move(s); }
+  void expect(const std::string& k, std::vector<int64_t> s) { staged.expect(k, std::move(s)); }
   void expect_res(const std::string& p, int cin, int cout) {
     const int temb = 4 * mc;
     expect(p + ".in_layers.0.weight", {cin});
@@ -259,23 +259,24 @@ struct nope_ldm {
     expect("pose_mlp.0.bias", {ctx});
   }
 
-  // ------------------------------------------------------------------ weights
-  int upload(const std::vector<float>& v, float** out) {
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(out), std::max<size_t>(v.size(), 1) * sizeof(float)));
-    owned.push_back(*out);
-    NOPE_CUDA(cudaMemcpy(*out, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
-    return 0;
+  // accepted for schema compatibility, never read (nope_ldm_load_tensor keeps their shapes only): emb = 0
+  // (adapt_openaimodel.py:143-146) and the one-token cross-attention does not depend on its queries / keys
+  static bool never_read(const char* key) {
+    return std::strncmp(key, "time_embed.", 11) == 0 || std::strstr(key, ".emb_layers.1.weight") ||
+           std::strstr(key, ".attn2.to_q.") || std::strstr(key, ".attn2.to_k.") || std::strstr(key, ".norm2.");
   }
-  const HostT& H(const std::string& k) const { return host.at(k); }
+
+  // ------------------------------------------------------------------ weights
+  const HostTensor& H(const std::string& k) const { return staged.at(k); }
   // dst[(row_off + o) * K + col_off + t * cin + c] = fp16(src[o][c][t])
-  int pack_into(__half* dst, int K, int row_off, int col_off, const HostT& t, int cout, int cin, int taps,
+  int pack_into(__half* dst, int K, int row_off, int col_off, const HostTensor& t, int cout, int cin, int taps,
                 bool fold_up = false) {
     using namespace nope;
     float *tmp = nullptr, *folded = nullptr;
-    const size_t n = t.second.size();
+    const size_t n = t.data.size();
     NOPE_CHECK(n == (size_t)cout * cin * (fold_up ? 9 : taps), "pack_into: size mismatch");
     NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&tmp), n * sizeof(float)));
-    NOPE_CUDA(cudaMemcpy(tmp, t.second.data(), n * sizeof(float), cudaMemcpyHostToDevice));
+    NOPE_CUDA(cudaMemcpy(tmp, t.data.data(), n * sizeof(float), cudaMemcpyHostToDevice));
     const float* src = tmp;
     int rows = cout;
     if (fold_up) {
@@ -298,24 +299,20 @@ struct nope_ldm {
     if (L.k_alg == 0) L.k_alg = L.K;
     L.bn = (!L.geglu && L.cout % 256 == 0) ? 256 : pick_bn(L.cout);
     NOPE_CHECK(L.bn != 0 && L.K % 64 == 0, name + ": channel counts must be multiples of 64");
-    if (!bias.empty() && upload(bias, &L.bias)) return -1;
+    if (!bias.empty() && mem.upload(&L.bias, bias)) return -1;
     if (make_weight_map(&L.wmap, L.w, rows, kp(L.K), L.bn)) return -1;
     convs[name] = L;
     return 0;
   }
-  int alloc_w(nope::LdmConv& L, int rows) {
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&L.w), (size_t)rows * kp(L.K) * sizeof(__half)));
-    owned.push_back(L.w);
-    return 0;
-  }
+  int alloc_w(nope::LdmConv& L, int rows) { return mem.alloc(&L.w, (size_t)rows * kp(L.K)); }
   // plain convolution / linear layer.  extra_bias (optional) is added to the bias.
   int make_conv(const std::string& name, const std::string& wkey, const std::string& bkey, int mode,
                 const std::string& extra_bias = "") {
-    const HostT& W = H(wkey);
+    const HostTensor& W = H(wkey);
     nope::LdmConv L;
     L.mode = mode;
-    L.cout = (int)W.first[0];
-    L.cin = (int)W.first[1];
+    L.cout = (int)W.shape[0];
+    L.cin = (int)W.shape[1];
     const int taps = mode == 1 ? 1 : (mode == 3 ? 4 : 9);
     L.K = L.cin * taps;
     const int rows = mode == 3 ? 4 * L.cout : L.cout;
@@ -323,9 +320,9 @@ struct nope_ldm {
     if (pack_into(L.w, L.K, 0, 0, W, L.cout, L.cin, taps, mode == 3)) return -1;
     std::vector<float> bias;
     if (!bkey.empty()) {
-      bias = H(bkey).second;
+      bias = H(bkey).data;
       if (!extra_bias.empty()) {
-        const auto& e = H(extra_bias).second;
+        const auto& e = H(extra_bias).data;
         for (size_t i = 0; i < bias.size(); ++i) bias[i] += e[i];
       }
     }
@@ -337,33 +334,33 @@ struct nope_ldm {
   // other operand instead of through per-row global loads in the epilogue (which stalled the short
   // 1x1 layers on long-scoreboard waits), the plain epilogue and the 256-wide tiles apply, and the
   // extra MMAs land on a tensor pipe that idles in these layers anyway.
-  static HostT identity(int c) {
-    HostT t;
-    t.first = {c, c};
-    t.second.assign((size_t)c * c, 0.f);
-    for (int i = 0; i < c; ++i) t.second[(size_t)i * c + i] = 1.f;
+  static HostTensor identity(int c) {
+    HostTensor t;
+    t.shape = {c, c};
+    t.data.assign((size_t)c * c, 0.f);
+    for (int i = 0; i < c; ++i) t.data[(size_t)i * c + i] = 1.f;
     return t;
   }
   // linear layer (1x1) whose output gets a residual of `cout` channels added
   int make_lin_res(const std::string& name, const std::string& wkey, const std::string& bkey) {
-    const HostT& W = H(wkey);
+    const HostTensor& W = H(wkey);
     nope::LdmConv L;
     L.mode = 1;
-    L.cout = (int)W.first[0];
-    L.cin = (int)W.first[1];
+    L.cout = (int)W.shape[0];
+    L.cin = (int)W.shape[1];
     L.skip_c = L.cout;
     L.K = L.cin + L.skip_c;
     L.k_alg = L.cin;
     if (alloc_w(L, L.cout)) return -1;
     if (pack_into(L.w, L.K, 0, 0, W, L.cout, L.cin, 1) || pack_into(L.w, L.K, 0, L.cin, identity(L.cout), L.cout, L.cout, 1))
       return -1;
-    return finish_conv(name, L, L.cout, H(bkey).second);
+    return finish_conv(name, L, L.cout, H(bkey).data);
   }
   int make_norm(const std::string& name, const std::string& prefix) {
     nope::LdmNorm n;
-    n.C = (int)H(prefix + ".weight").first[0];
+    n.C = (int)H(prefix + ".weight").shape[0];
     NOPE_CHECK(n.C % 256 == 0 && n.C <= nope::kLdmMaxC, prefix + ": GroupNorm(32) needs C % 256 == 0, C <= 2048");
-    if (upload(H(prefix + ".weight").second, &n.gamma) || upload(H(prefix + ".bias").second, &n.beta)) return -1;
+    if (mem.upload(&n.gamma, H(prefix + ".weight").data) || mem.upload(&n.beta, H(prefix + ".bias").data)) return -1;
     norms[name] = n;
     return 0;
   }
@@ -373,18 +370,18 @@ struct nope_ldm {
     if (make_norm(p + ".n1", p + ".in_layers.0") || make_norm(p + ".n2", p + ".out_layers.0")) return -1;
     if (make_conv(p + ".c1", p + ".in_layers.2.weight", p + ".in_layers.2.bias", 0, p + ".emb_layers.1.bias"))
       return -1;
-    const HostT& W2 = H(p + ".out_layers.3.weight");
+    const HostTensor& W2 = H(p + ".out_layers.3.weight");
     nope::LdmConv L;
     L.mode = 0;
-    L.cout = (int)W2.first[0];
-    L.cin = (int)W2.first[1];
-    std::vector<float> bias = H(p + ".out_layers.3.bias").second;
-    const bool has_skip = host.count(p + ".skip_connection.weight") != 0;
+    L.cout = (int)W2.shape[0];
+    L.cin = (int)W2.shape[1];
+    std::vector<float> bias = H(p + ".out_layers.3.bias").data;
+    const bool has_skip = staged.has(p + ".skip_connection.weight");
     if (has_skip) {
       // skip_connection (1x1 on the block input) rides in the same GEMM: extra K columns
-      const HostT& Ws = H(p + ".skip_connection.weight");
-      L.skip_c = (int)Ws.first[1];
-      const auto& bs = H(p + ".skip_connection.bias").second;
+      const HostTensor& Ws = H(p + ".skip_connection.weight");
+      L.skip_c = (int)Ws.shape[1];
+      const auto& bs = H(p + ".skip_connection.bias").data;
       for (size_t i = 0; i < bias.size(); ++i) bias[i] += bs[i];
     }
     const bool id_skip = !has_skip;      // identity skip as an identity K-segment
@@ -400,26 +397,26 @@ struct nope_ldm {
   }
   int make_st(const std::string& p) {
     const std::string t = p + ".transformer_blocks.0";
-    const int c = (int)H(p + ".norm.weight").first[0];
+    const int c = (int)H(p + ".norm.weight").shape[0];
     if (make_norm(p + ".norm", p + ".norm")) return -1;
     if (make_conv(p + ".proj_in", p + ".proj_in.weight", p + ".proj_in.bias", 1)) return -1;
     if (make_lin_res(p + ".proj_out", p + ".proj_out.weight", p + ".proj_out.bias")) return -1;
     if (make_lin_res(p + ".to_out", t + ".attn1.to_out.0.weight", t + ".attn1.to_out.0.bias")) return -1;
     {  // the feed-forward projection with GEGLU fused into the epilogue: tile t of 128 rows =
        // x rows 64t..64t+63 followed by gate rows inner+64t..inner+64t+63
-      const HostT& W = H(t + ".ff.net.0.proj.weight");
-      const auto& b = H(t + ".ff.net.0.proj.bias").second;
+      const HostTensor& W = H(t + ".ff.net.0.proj.weight");
+      const auto& b = H(t + ".ff.net.0.proj.bias").data;
       const int inner = 4 * c;
-      HostT Wp;
-      Wp.first = W.first;
-      Wp.second.resize(W.second.size());
+      HostTensor Wp;
+      Wp.shape = W.shape;
+      Wp.data.resize(W.data.size());
       std::vector<float> bp(2 * inner);
       for (int tl = 0; tl < inner / 64; ++tl)
         for (int half = 0; half < 2; ++half)
           for (int j = 0; j < 64; ++j) {
             const int src = half * inner + tl * 64 + j, dst = tl * 128 + half * 64 + j;
-            std::copy(W.second.begin() + (size_t)src * c, W.second.begin() + (size_t)(src + 1) * c,
-                      Wp.second.begin() + (size_t)dst * c);
+            std::copy(W.data.begin() + (size_t)src * c, W.data.begin() + (size_t)(src + 1) * c,
+                      Wp.data.begin() + (size_t)dst * c);
             bp[dst] = b[src];
           }
       nope::LdmConv L;
@@ -450,8 +447,8 @@ struct nope_ldm {
     for (int n = 1; n <= 3; n += 2) {   // norm2 only feeds attn2's queries, which cancel (see below)
       nope::LdmNorm ln;
       ln.C = c;
-      if (upload(H(t + ".norm" + std::to_string(n) + ".weight").second, &ln.gamma) ||
-          upload(H(t + ".norm" + std::to_string(n) + ".bias").second, &ln.beta))
+      if (mem.upload(&ln.gamma, H(t + ".norm" + std::to_string(n) + ".weight").data) ||
+          mem.upload(&ln.beta, H(t + ".norm" + std::to_string(n) + ".bias").data))
         return -1;
       norms[p + ".ln" + std::to_string(n)] = ln;
     }
@@ -464,13 +461,13 @@ struct nope_ldm {
   // Wc = Wo Wv Wp and bc = Wo Wv bp + bo in double, for all transformer blocks at once.
   int make_cross() {
     std::vector<float> Wc((size_t)cb_width * rot_dim), bc(cb_width);
-    const auto& Wp = H("pose_mlp.0.weight").second;   // [ctx][6]
-    const auto& bp = H("pose_mlp.0.bias").second;
+    const auto& Wp = H("pose_mlp.0.weight").data;   // [ctx][6]
+    const auto& bp = H("pose_mlp.0.bias").data;
     for (const auto& kv : cb_off) {
       const std::string t = kv.first + ".transformer_blocks.0.attn2";
-      const auto& Wv = H(t + ".to_v.weight").second;       // [c][ctx]
-      const auto& Wo = H(t + ".to_out.0.weight").second;   // [c][c]
-      const auto& bo = H(t + ".to_out.0.bias").second;
+      const auto& Wv = H(t + ".to_v.weight").data;       // [c][ctx]
+      const auto& Wo = H(t + ".to_out.0.weight").data;   // [c][c]
+      const auto& bo = H(t + ".to_out.0.bias").data;
       const int c = (int)bo.size();
       std::vector<double> A((size_t)c * (rot_dim + 1), 0.0);   // Wv [Wp | bp]
       for (int i = 0; i < c; ++i)
@@ -489,23 +486,21 @@ struct nope_ldm {
         bc[kv.second + o] = (float)(acc[rot_dim] + bo[o]);
       }
     }
-    return upload(Wc, &cross_w) || upload(bc, &cross_b) ? -1 : 0;
+    return mem.upload(&cross_w, Wc) || mem.upload(&cross_b, bc) ? -1 : 0;
   }
 
+  // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
   int finalize() {
-    NOPE_CHECK(!finalized, "already finalized");
-    for (const auto& kv : expected) NOPE_CHECK(host.count(kv.first), "state_dict is missing " + kv.first);
-    NOPE_CUDA(cudaSetDevice(device));
-    if (upload(H("input_blocks.0.0.weight").second, &in_w) || upload(H("input_blocks.0.0.bias").second, &in_b))
+    if (mem.upload(&in_w, H("input_blocks.0.0.weight").data) || mem.upload(&in_b, H("input_blocks.0.0.bias").data))
       return -1;
     {  // out[2]: Cl output channels padded to one 64-wide tile of the tensor-core kernel
-      HostT W;
-      W.first = {64, mc, 3, 3};
-      W.second.assign((size_t)64 * mc * 9, 0.f);
-      const auto& w = H("out.2.weight").second;
-      std::copy(w.begin(), w.end(), W.second.begin());
+      HostTensor W;
+      W.shape = {64, mc, 3, 3};
+      W.data.assign((size_t)64 * mc * 9, 0.f);
+      const auto& w = H("out.2.weight").data;
+      std::copy(w.begin(), w.end(), W.data.begin());
       std::vector<float> bias(64, 0.f);
-      std::copy(H("out.2.bias").second.begin(), H("out.2.bias").second.end(), bias.begin());
+      std::copy(H("out.2.bias").data.begin(), H("out.2.bias").data.end(), bias.begin());
       nope::LdmConv L;
       L.mode = 0;
       L.cout = 64;
@@ -528,28 +523,14 @@ struct nope_ldm {
       if (outp[i].up && make_conv(p + ".2.conv", p + ".2.conv.weight", p + ".2.conv.bias", 3)) return -1;
     }
     if (make_norm("out.0", "out.0")) return -1;
-    if (make_cross()) return -1;
-    host.clear();
-    finalized = true;
-    return 0;
+    return make_cross();
   }
 
   // ------------------------------------------------------------------ workspace
-  int ws_half(__half** p, size_t n) {
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(__half)));
-    ws_owned.push_back(*p);
-    return 0;
-  }
-  template <typename T> int ws_any(T** p, size_t n) {
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
-    ws_owned.push_back(*p);
-    return 0;
-  }
   int ensure_workspace(int need_cap, int need_ref) {
     if (need_cap <= cap && need_ref <= cap_ref) return 0;
     NOPE_CUDA(cudaDeviceSynchronize());
-    for (void* p : ws_owned) cudaFree(p);
-    ws_owned.clear();
+    ws_mem.release();
     tmaps.clear();
     tmaps3.clear();
     cap = std::max(cap, need_cap);
@@ -561,20 +542,22 @@ struct nope_ldm {
       int S = S0;
       for (size_t i = 0; i < inp.size(); ++i) {
         if (inp[i].kind == 2) S /= 2;
-        if (ws_half(&HS[i], c * S * S * inp[i].cout)) return -1;
+        if (ws_mem.alloc(&HS[i], c * S * S * inp[i].cout)) return -1;
       }
     }
     // widest tensors: block outputs <= 2u (512 ch at 32^2 after the last upsample), ResBlock
     // inputs <= 3u (768 ch at 32^2), q|k|v 3u, V^T 1u, GEGLU output 4u
-    if (ws_half(&XA, c * 2 * u) || ws_half(&XB, c * 2 * u) || ws_half(&XC, c * 2 * u) || ws_half(&R, c * u) ||
-        ws_half(&T1, c * 3 * u) || ws_half(&T2, c * u) || ws_half(&T3, c * u) || ws_half(&XN, c * u) ||
-        ws_half(&PI, c * u) || ws_half(&PJ, c * u) || ws_half(&QKV, c * 3 * u) || ws_half(&Vt, c * u) || ws_half(&AO, c * u) ||
-        ws_half(&GG, c * 4 * u) || ws_half(&x0ref, (size_t)cap_ref * u) || ws_half(&Rref, (size_t)cap_ref * u) ||
-        ws_half(&Pref, (size_t)cap_ref * u))
+    if (ws_mem.alloc(&XA, c * 2 * u) || ws_mem.alloc(&XB, c * 2 * u) || ws_mem.alloc(&XC, c * 2 * u) ||
+        ws_mem.alloc(&R, c * u) || ws_mem.alloc(&T1, c * 3 * u) || ws_mem.alloc(&T2, c * u) ||
+        ws_mem.alloc(&T3, c * u) || ws_mem.alloc(&XN, c * u) || ws_mem.alloc(&PI, c * u) || ws_mem.alloc(&PJ, c * u) ||
+        ws_mem.alloc(&QKV, c * 3 * u) || ws_mem.alloc(&Vt, c * u) || ws_mem.alloc(&AO, c * u) ||
+        ws_mem.alloc(&GG, c * 4 * u) || ws_mem.alloc(&x0ref, (size_t)cap_ref * u) ||
+        ws_mem.alloc(&Rref, (size_t)cap_ref * u) || ws_mem.alloc(&Pref, (size_t)cap_ref * u))
       return -1;
     const size_t st = (size_t)32 * 256;   // parts (<= 32) x octets (<= 256) per image
-    if (ws_any(&S_in, c * st) || ws_any(&S_mid, c * st) || ws_any(&S_out, c * st)) return -1;
-    if (ws_any(&cb, c * (size_t)cb_width) || ws_any(&ref_of, c) || ws_any(&OF, c * S0 * S0 * 64)) return -1;
+    if (ws_mem.alloc(&S_in, c * st) || ws_mem.alloc(&S_mid, c * st) || ws_mem.alloc(&S_out, c * st)) return -1;
+    if (ws_mem.alloc(&cb, c * (size_t)cb_width) || ws_mem.alloc(&ref_of, c) || ws_mem.alloc(&OF, c * S0 * S0 * 64))
+      return -1;
     return 0;
   }
 

@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "engine.cuh"
 #include "conv_tc.cuh"
 #include "conv_tc2.cuh"
 #include "kernels.cuh"
@@ -35,11 +36,6 @@ namespace {
 
 constexpr int kAbiVersion = 2;
 constexpr int kHeadsHidden = 128;  // 4 heads x 32 (model_utils.py:368,394)
-
-struct HostTensor {
-  std::vector<int64_t> shape;
-  std::vector<float> data;
-};
 
 struct ConvLayer {
   int mode = 0;  // 0: 3x3 pad1, 1: 1x1, 2: unshuffle+1x1, 3: nearest-x2 upsample + 3x3 (folded)
@@ -96,6 +92,7 @@ struct Bump {
 }  // namespace
 
 struct nope_unet {
+  static constexpr const char* kName = "UNet";
   int dim = 0, Cl = 0, S0 = 0, rot_dim = 6, cemb = 0, device = 0, num_sms = 132;
   int dims[5] = {0, 0, 0, 0, 0};
   bool finalized = false;
@@ -111,8 +108,7 @@ struct nope_unet {
   int chunk = 642;
   int64_t launches = 0;
 
-  std::map<std::string, HostTensor> host;
-  std::map<std::string, std::vector<int64_t>> expected;  // key -> shape
+  StagedWeights staged;
 
   std::map<std::string, ConvLayer> convs;
   std::map<std::string, NormLayer> norms;
@@ -121,7 +117,7 @@ struct nope_unet {
   ConvLayer poseproj;
   float *pose_w = nullptr, *pose_b = nullptr, *init_w = nullptr, *init_b = nullptr,
         *final_w = nullptr, *final_b = nullptr;
-  std::vector<void*> owned;  // every cudaMalloc'd weight pointer
+  DeviceAllocs mem;  // every weight buffer
 
   // workspace: one slab, either caller-provided (nope_unet_set_workspace) or owned
   int cap = 0, cap_ref = 0;
@@ -158,7 +154,6 @@ struct nope_unet {
   bool tap_hit = false;
 
   ~nope_unet() {
-    for (void* p : owned) cudaFree(p);
     if (ws_base && !ws_external) cudaFree(ws_base);
     for (cudaEvent_t e : prof_ev) cudaEventDestroy(e);
   }
@@ -171,7 +166,7 @@ struct nope_unet {
   bool bf() const { return precision == 3; }     // bf16 storage (BASELINE configs[2]); fp16 otherwise
 
   // ------------------------------------------------------------------ schema
-  void expect(const std::string& k, std::vector<int64_t> s) { expected[k] = std::move(s); }
+  void expect(const std::string& k, std::vector<int64_t> s) { staged.expect(k, std::move(s)); }
   void expect_resblock(const std::string& p, int cin, int cout, bool mlp = true) {
     if (mlp) {
       expect(p + ".mlp.1.weight", {cout, cemb});
@@ -248,22 +243,13 @@ struct nope_unet {
   }
 
   // ------------------------------------------------------------------ weights
-  int upload_f32(const std::string& key, float** out) {
-    auto it = host.find(key);
-    NOPE_CHECK(it != host.end(), "missing tensor " + key);
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(out), it->second.data.size() * sizeof(float)));
-    owned.push_back(*out);
-    NOPE_CUDA(cudaMemcpy(*out, it->second.data.data(), it->second.data.size() * sizeof(float),
-                         cudaMemcpyHostToDevice));
-    return 0;
-  }
+  int upload_f32(const std::string& key, float** out) { return mem.upload(out, staged.at(key).data); }
   // pack one conv weight (+ bias) into a ConvLayer.  mode 3 (nearest-x2 upsample + conv3x3,
   // HardUpsample) first folds the 3x3 kernel into four 2x2 parity kernels (fold_upconv_kernel).
   // precision >= 1 appends the fp16 remainders as a second K-block: rows are [W_hi (K) | W_lo (K)].
   int make_conv(const std::string& name, const std::string& wkey, const std::string& bkey, int mode) {
-    auto it = host.find(wkey);
-    NOPE_CHECK(it != host.end(), "missing tensor " + wkey);
-    const auto& sh = it->second.shape;
+    const HostTensor& W = staged.at(wkey);
+    const auto& sh = W.shape;
     ConvLayer L;
     L.mode = mode;
     L.cout = (int)sh[0];
@@ -277,9 +263,9 @@ struct nope_unet {
     L.bn = pick_bn(L.cout);
     NOPE_CHECK(L.bn != 0, wkey + ": output channels must be a multiple of 64");
     float *tmp = nullptr, *folded = nullptr;
-    const size_t n = it->second.data.size();
+    const size_t n = W.data.size();
     NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&tmp), n * sizeof(float)));
-    NOPE_CUDA(cudaMemcpy(tmp, it->second.data.data(), n * sizeof(float), cudaMemcpyHostToDevice));
+    NOPE_CUDA(cudaMemcpy(tmp, W.data.data(), n * sizeof(float), cudaMemcpyHostToDevice));
     const size_t npack = (size_t)rows * L.Kp;
     const float* src = tmp;
     if (mode == 3) {
@@ -289,8 +275,7 @@ struct nope_unet {
       NOPE_CUDA(cudaGetLastError());
       src = folded;
     }
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&L.w), npack * sizeof(__half)));
-    owned.push_back(L.w);
+    if (mem.alloc(&L.w, npack)) return -1;
     pack_weight_kernel<<<ew_grid((long long)rows * L.K), 256>>>(src, L.w, rows, L.cin, taps, L.Kp, 0,
                                                                 wlo ? L.K : 0, bf() ? 1 : 0);
     NOPE_CUDA(cudaGetLastError());
@@ -307,9 +292,7 @@ struct nope_unet {
   }
   int make_norm(const std::string& name, const std::string& prefix, int G) {
     NormLayer n;
-    auto it = host.find(prefix + ".weight");
-    NOPE_CHECK(it != host.end(), "missing tensor " + prefix + ".weight");
-    n.C = (int)it->second.shape[0];
+    n.C = (int)staged.at(prefix + ".weight").shape[0];
     n.G = G;
     NOPE_CHECK(n.C % (8 * G) == 0, prefix + ": channels per group must be a multiple of 8");
     if (upload_f32(prefix + ".weight", &n.gamma)) return -1;
@@ -322,7 +305,7 @@ struct nope_unet {
     if (make_conv(p + ".block2", p + ".block2.proj.weight", p + ".block2.proj.bias", 0)) return -1;
     if (make_norm(p + ".norm1", p + ".block1.norm", 8)) return -1;
     if (make_norm(p + ".norm2", p + ".block2.norm", 8)) return -1;
-    if (host.count(p + ".res_conv.weight"))
+    if (staged.has(p + ".res_conv.weight"))
       if (make_conv(p + ".res", p + ".res_conv.weight", p + ".res_conv.bias", 1)) return -1;
     return 0;
   }
@@ -330,9 +313,9 @@ struct nope_unet {
   // W' = W diag(gamma); w1[c] = sum_k W'[c,k] over the values the tensor core actually multiplies
   // (fp16 hi, + lo in the exact-weight modes); wb[c] = sum_k W[c,k] beta[k].
   int make_qkv_folded(const std::string& name, const std::string& wkey, const std::string& nprefix) {
-    const HostTensor& W = host.at(wkey);
-    const std::vector<float>& gm = host.at(nprefix + ".weight").data;
-    const std::vector<float>& bt = host.at(nprefix + ".bias").data;
+    const HostTensor& W = staged.at(wkey);
+    const std::vector<float>& gm = staged.at(nprefix + ".weight").data;
+    const std::vector<float>& bt = staged.at(nprefix + ".bias").data;
     const int rows = (int)W.shape[0], cin = (int)W.shape[1];
     HostTensor Wf;
     Wf.shape = W.shape;
@@ -362,16 +345,10 @@ struct nope_unet {
       wb[o] = (float)sb;
     }
     const std::string tmpkey = "__folded." + name;
-    host[tmpkey] = std::move(Wf);
+    staged.put(tmpkey, std::move(Wf));
     if (make_conv(name, tmpkey, "", 1)) return -1;
-    host.erase(tmpkey);
     ConvLayer& L = convs[name];
-    for (auto pr : {std::make_pair(&L.pre_w1, &w1), std::make_pair(&L.pre_wb, &wb)}) {
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(pr.first), rows * sizeof(float)));
-      owned.push_back(*pr.first);
-      NOPE_CUDA(cudaMemcpy(*pr.first, pr.second->data(), rows * sizeof(float), cudaMemcpyHostToDevice));
-    }
-    return 0;
+    return mem.upload(&L.pre_w1, w1) || mem.upload(&L.pre_wb, wb) ? -1 : 0;
   }
   int make_linattn(const std::string& p) {
     if (make_norm(p + ".prenorm", p + ".fn.norm", 1)) return -1;
@@ -394,8 +371,8 @@ struct nope_unet {
     std::vector<float> w, bias;
     P = 0;
     for (const auto& b : blocks) {
-      const HostTensor& hw = host.at(b + ".mlp.1.weight");
-      const HostTensor& hb = host.at(b + ".mlp.1.bias");
+      const HostTensor& hw = staged.at(b + ".mlp.1.weight");
+      const HostTensor& hb = staged.at(b + ".mlp.1.bias");
       pb_off[b] = P;
       P += (int)hw.shape[0];
       w.insert(w.end(), hw.data.begin(), hw.data.end());
@@ -407,20 +384,17 @@ struct nope_unet {
     HostTensor tb;
     tb.shape = {P};
     tb.data = std::move(bias);
-    host["__poseproj.weight"] = std::move(tw);
-    host["__poseproj.bias"] = std::move(tb);
+    staged.put("__poseproj.weight", std::move(tw));
+    staged.put("__poseproj.bias", std::move(tb));
     if (make_conv("__poseproj", "__poseproj.weight", "__poseproj.bias", 1)) return -1;
     poseproj = convs["__poseproj"];
     return 0;
   }
 
+  // packs the staged weights (engine_finalize: every schema key is present, device selected)
   int finalize() {
-    NOPE_CHECK(!finalized, "already finalized");
-    for (const auto& kv : expected)
-      NOPE_CHECK(host.count(kv.first), "state_dict is missing " + kv.first);
     NOPE_CHECK(precision == 0 || conv_impl != 1, "the SIMT debug convolution only runs fp16 weights");
     NOPE_CHECK(precision < 2 || fused(), "split precision / bf16 need the fused schedule on the CTA-pair kernel");
-    NOPE_CUDA(cudaSetDevice(device));
     if (upload_f32("pose_mlp.0.weight", &pose_w) || upload_f32("pose_mlp.0.bias", &pose_b) ||
         upload_f32("init_conv.weight", &init_w) || upload_f32("init_conv.bias", &init_b) ||
         upload_f32("final_conv.1.weight", &final_w) || upload_f32("final_conv.1.bias", &final_b))
@@ -450,10 +424,7 @@ struct nope_unet {
       }
     }
     if (make_resblock("final_res_block") || make_resblock("final_conv.0")) return -1;
-    if (make_poseproj()) return -1;
-    host.clear();
-    finalized = true;
-    return 0;
+    return make_poseproj();
   }
 
   // ------------------------------------------------------------------ workspace
@@ -1148,19 +1119,13 @@ int nope_unet_create(nope_unet_t** out, int u_net_dim, int latent_ch, int latent
   NOPE_CHECK(u_net_dim > 0 && u_net_dim % 64 == 0, "u_net_dim must be a positive multiple of 64");
   NOPE_CHECK(latent_ch >= 1 && latent_ch <= kMaxLatent, "latent_ch must be in [1, 8]");
   NOPE_CHECK(latent_hw == 32, "latent_hw must be 32 (256x256 images) in this build");
-  int ndev = 0;
-  NOPE_CUDA(cudaGetDeviceCount(&ndev));
-  NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
-  cudaDeviceProp prop;
-  NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
-  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
   auto u = std::make_unique<nope_unet>();
+  if (open_device(device, &u->num_sms)) return -1;
   u->dim = u_net_dim;
   u->Cl = latent_ch;
   u->S0 = latent_hw;
   u->cemb = 4 * u_net_dim;
   u->device = device;
-  u->num_sms = prop.multiProcessorCount;
   const int mults[4] = {1, 2, 4, 8};
   u->dims[0] = u_net_dim;
   for (int i = 0; i < 4; ++i) u->dims[i + 1] = u_net_dim * mults[i];
@@ -1173,27 +1138,10 @@ void nope_unet_destroy(nope_unet_t* u) { delete u; }
 
 int nope_unet_load_tensor(nope_unet_t* u, const char* key, const float* data, const int64_t* shape,
                           int ndim) {
-  NOPE_CHECK(u && key && data && shape, "null argument");
-  NOPE_CHECK(!u->finalized, "engine already finalized");
-  auto it = u->expected.find(key);
-  NOPE_CHECK(it != u->expected.end(), std::string("unexpected state_dict key: ") + key);
-  NOPE_CHECK((int)it->second.size() == ndim, std::string("rank mismatch for ") + key);
-  size_t n = 1;
-  for (int i = 0; i < ndim; ++i) {
-    NOPE_CHECK(it->second[i] == shape[i], std::string("shape mismatch for ") + key);
-    n *= (size_t)shape[i];
-  }
-  HostTensor t;
-  t.shape.assign(shape, shape + ndim);
-  t.data.assign(data, data + n);
-  u->host[key] = std::move(t);
-  return 0;
+  return engine_load_tensor(u, key, data, shape, ndim);
 }
 
-int nope_unet_finalize(nope_unet_t* u) {
-  NOPE_CHECK(u, "null engine");
-  return u->finalize();
-}
+int nope_unet_finalize(nope_unet_t* u) { return engine_finalize(u); }
 
 int nope_unet_set_chunk(nope_unet_t* u, int hyps) {
   NOPE_CHECK(u && hyps >= 1 && hyps <= 4096, "chunk must be in [1, 4096]");
@@ -1299,13 +1247,7 @@ int nope_unet_profile_read(nope_unet_t* u, double* conv_ms, double* conv_flops, 
 int nope_unet_sweep_multi(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
                           const float* query_feat, int Q, float* out_emb, float* out_sim, int k, float* out_topv,
                           int64_t* out_topi, int64_t idx_base, void* stream) {
-  NOPE_CHECK(u && u->finalized, "engine not finalized");
-  NOPE_CHECK(ref_feat && poses && B >= 1 && N >= 1, "bad arguments");
-  NOPE_CHECK(Q >= 1, "Q (queries per reference) must be >= 1");
-  NOPE_CHECK((int64_t)B * Q * N <= INT32_MAX, "B * Q * N exceeds the scored-triple limit (2^31 - 1)");
-  NOPE_CHECK(!(out_sim || k > 0) || query_feat, "scores / top-k need query_feat");
-  NOPE_CHECK(k >= 0 && k <= N && k <= 64, "k must be in [0, min(N, 64)]");
-  NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
+  if (check_sweep(u, ref_feat, poses, B, N, query_feat, Q, out_sim, k, out_topv, out_topi)) return -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   NOPE_CUDA(cudaSetDevice(u->device));
   u->launches = 0;
@@ -1505,16 +1447,10 @@ int nope_topk_merge(const float* gathered, int world, int64_t pack_floats, int B
 int nope_encoder_create(nope_encoder_t** out, int descriptor_size, int device) {
   NOPE_CHECK(out != nullptr, "null out pointer");
   NOPE_CHECK(descriptor_size >= 1 && descriptor_size <= 64, "descriptor_size must be in [1, 64]");
-  int ndev = 0;
-  NOPE_CUDA(cudaGetDeviceCount(&ndev));
-  NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
-  cudaDeviceProp prop;
-  NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
-  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
   auto e = std::make_unique<nope_encoder>();
+  if (open_device(device, &e->num_sms)) return -1;
   e->D = descriptor_size;
   e->device = device;
-  e->num_sms = prop.multiProcessorCount;
   e->build_schema();
   *out = e.release();
   return 0;
@@ -1524,26 +1460,10 @@ void nope_encoder_destroy(nope_encoder_t* e) { delete e; }
 
 int nope_encoder_load_tensor(nope_encoder_t* e, const char* key, const float* data, const int64_t* shape,
                              int ndim) {
-  NOPE_CHECK(e && key && data && shape, "null argument");
-  NOPE_CHECK(!e->finalized, "encoder already finalized");
-  auto it = e->expected.find(key);
-  NOPE_CHECK(it != e->expected.end(), std::string("unexpected encoder state_dict key: ") + key);
-  NOPE_CHECK((int)it->second.size() == ndim, std::string("rank mismatch for ") + key);
-  size_t n = 1;
-  for (int i = 0; i < ndim; ++i) {
-    NOPE_CHECK(it->second[i] == shape[i], std::string("shape mismatch for ") + key);
-    n *= (size_t)shape[i];
-  }
-  auto& slot = e->host[key];
-  slot.first.assign(shape, shape + ndim);
-  slot.second.assign(data, data + n);
-  return 0;
+  return engine_load_tensor(e, key, data, shape, ndim);
 }
 
-int nope_encoder_finalize(nope_encoder_t* e) {
-  NOPE_CHECK(e, "null encoder");
-  return e->finalize();
-}
+int nope_encoder_finalize(nope_encoder_t* e) { return engine_finalize(e); }
 
 int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* out, void* stream) {
   NOPE_CHECK(e && e->finalized, "encoder not finalized");
@@ -1551,17 +1471,7 @@ int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* ou
   NOPE_CHECK(B >= 1, "B must be >= 1");
   NOPE_CUDA(cudaSetDevice(e->device));
   // The workspace is sized by the largest chunk (~80 MB per image): any B goes through, 32 images at a time.
-  constexpr int kChunk = nope_encoder::kChunk;
-  int64_t launches = 0;
-  for (int lo = 0; lo < B; lo += kChunk) {
-    const int n = B - lo < kChunk ? B - lo : kChunk;
-    const int rc = e->encode(images + (size_t)lo * 3 * 256 * 256, n, out + (size_t)lo * e->D * 32 * 32,
-                             static_cast<cudaStream_t>(stream));
-    if (rc != 0) return rc;
-    launches += e->launches;
-  }
-  e->launches = launches;
-  return 0;
+  return per_chunk(e, &nope_encoder::encode, images, 3 * 256 * 256, B, out, (size_t)e->D * 32 * 32, stream);
 }
 
 int nope_encoder_encode_inplane(nope_encoder_t* e, const float* images, int B, const float* cossin, int A, float* out,
@@ -1627,15 +1537,9 @@ int64_t nope_encoder_last_launch_count(const nope_encoder_t* e) { return e ? e->
 // ---------------------------------------------------------------------------------
 int nope_vae_create(nope_vae_t** out, int device) {
   NOPE_CHECK(out != nullptr, "null out pointer");
-  int ndev = 0;
-  NOPE_CUDA(cudaGetDeviceCount(&ndev));
-  NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
-  cudaDeviceProp prop;
-  NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
-  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
   auto v = std::make_unique<nope_vae>();
+  if (open_device(device, &v->num_sms)) return -1;
   v->device = device;
-  v->num_sms = prop.multiProcessorCount;
   v->build_schema();
   *out = v.release();
   return 0;
@@ -1644,43 +1548,17 @@ int nope_vae_create(nope_vae_t** out, int device) {
 void nope_vae_destroy(nope_vae_t* v) { delete v; }
 
 int nope_vae_load_tensor(nope_vae_t* v, const char* key, const float* data, const int64_t* shape, int ndim) {
-  NOPE_CHECK(v && key && data && shape, "null argument");
-  NOPE_CHECK(!v->finalized, "VAE already finalized");
-  auto it = v->expected.find(key);
-  NOPE_CHECK(it != v->expected.end(), std::string("unexpected VAE state_dict key: ") + key);
-  NOPE_CHECK((int)it->second.size() == ndim, std::string("rank mismatch for ") + key);
-  size_t n = 1;
-  for (int i = 0; i < ndim; ++i) {
-    NOPE_CHECK(it->second[i] == shape[i], std::string("shape mismatch for ") + key);
-    n *= (size_t)shape[i];
-  }
-  auto& slot = v->host[key];
-  slot.first.assign(shape, shape + ndim);
-  slot.second.assign(data, data + n);
-  return 0;
+  return engine_load_tensor(v, key, data, shape, ndim);
 }
 
-int nope_vae_finalize(nope_vae_t* v) {
-  NOPE_CHECK(v, "null VAE");
-  return v->finalize();
-}
+int nope_vae_finalize(nope_vae_t* v) { return engine_finalize(v); }
 
 int nope_vae_encode(nope_vae_t* v, const float* images, int B, float* out, void* stream) {
   NOPE_CHECK(images && out, "null images / out pointer");
   NOPE_CHECK(B >= 1, "B must be >= 1");
   NOPE_CHECK(v && v->finalized, "VAE not finalized");
   NOPE_CUDA(cudaSetDevice(v->device));
-  constexpr int kChunk = nope_vae::kChunk;
-  int64_t launches = 0;
-  for (int lo = 0; lo < B; lo += kChunk) {
-    const int n = B - lo < kChunk ? B - lo : kChunk;
-    const int rc = v->encode(images + (size_t)lo * 3 * 256 * 256, n, out + (size_t)lo * 4 * 32 * 32,
-                             static_cast<cudaStream_t>(stream));
-    if (rc != 0) return rc;
-    launches += v->launches;
-  }
-  v->launches = launches;
-  return 0;
+  return per_chunk(v, &nope_vae::encode, images, 3 * 256 * 256, B, out, 4 * 32 * 32, stream);
 }
 
 int nope_vae_encode_inplane(nope_vae_t* v, const float* images, int B, const float* cossin, int A, float* out,
@@ -1710,15 +1588,9 @@ int64_t nope_vae_last_launch_count(const nope_vae_t* v) { return v ? v->launches
 // ---------------------------------------------------------------------------------
 int nope_vae_decoder_create(nope_vae_decoder_t** out, int device) {
   NOPE_CHECK(out != nullptr, "null out pointer");
-  int ndev = 0;
-  NOPE_CUDA(cudaGetDeviceCount(&ndev));
-  NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
-  cudaDeviceProp prop;
-  NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
-  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
   auto d = std::make_unique<nope_vae_decoder>();
+  if (open_device(device, &d->num_sms)) return -1;
   d->device = device;
-  d->num_sms = prop.multiProcessorCount;
   d->build_schema();
   *out = d.release();
   return 0;
@@ -1728,43 +1600,17 @@ void nope_vae_decoder_destroy(nope_vae_decoder_t* d) { delete d; }
 
 int nope_vae_decoder_load_tensor(nope_vae_decoder_t* d, const char* key, const float* data, const int64_t* shape,
                                  int ndim) {
-  NOPE_CHECK(d && key && data && shape, "null argument");
-  NOPE_CHECK(!d->finalized, "VAE decoder already finalized");
-  auto it = d->expected.find(key);
-  NOPE_CHECK(it != d->expected.end(), std::string("unexpected VAE decoder state_dict key: ") + key);
-  NOPE_CHECK((int)it->second.size() == ndim, std::string("rank mismatch for ") + key);
-  size_t n = 1;
-  for (int i = 0; i < ndim; ++i) {
-    NOPE_CHECK(it->second[i] == shape[i], std::string("shape mismatch for ") + key);
-    n *= (size_t)shape[i];
-  }
-  auto& slot = d->host[key];
-  slot.first.assign(shape, shape + ndim);
-  slot.second.assign(data, data + n);
-  return 0;
+  return engine_load_tensor(d, key, data, shape, ndim);
 }
 
-int nope_vae_decoder_finalize(nope_vae_decoder_t* d) {
-  NOPE_CHECK(d, "null VAE decoder");
-  return d->finalize();
-}
+int nope_vae_decoder_finalize(nope_vae_decoder_t* d) { return engine_finalize(d); }
 
 int nope_vae_decoder_decode(nope_vae_decoder_t* d, const float* latents, int B, float* out, void* stream) {
   NOPE_CHECK(latents && out, "null latents / out pointer");
   NOPE_CHECK(B >= 1, "B must be >= 1");
   NOPE_CHECK(d && d->finalized, "VAE decoder not finalized");
   NOPE_CUDA(cudaSetDevice(d->device));
-  constexpr int kChunk = nope_vae_decoder::kChunk;
-  int64_t launches = 0;
-  for (int lo = 0; lo < B; lo += kChunk) {
-    const int n = B - lo < kChunk ? B - lo : kChunk;
-    const int rc = d->decode(latents + (size_t)lo * 4 * 32 * 32, n, out + (size_t)lo * 3 * 256 * 256,
-                             static_cast<cudaStream_t>(stream));
-    if (rc != 0) return rc;
-    launches += d->launches;
-  }
-  d->launches = launches;
-  return 0;
+  return per_chunk(d, &nope_vae_decoder::decode, latents, 4 * 32 * 32, B, out, 3 * 256 * 256, stream);
 }
 
 int64_t nope_vae_decoder_last_launch_count(const nope_vae_decoder_t* d) { return d ? d->launches : 0; }
@@ -2279,19 +2125,13 @@ int nope_ldm_create(nope_ldm_t** out, int model_channels, int context_dim, int l
   NOPE_CHECK(context_dim >= 1, "context_dim must be positive");
   NOPE_CHECK(latent_ch >= 1 && latent_ch <= kMaxLatent, "latent_ch must be in [1, 8]");
   NOPE_CHECK(latent_hw == 32, "latent_hw must be 32 in this build");
-  int ndev = 0;
-  NOPE_CUDA(cudaGetDeviceCount(&ndev));
-  NOPE_CHECK(device >= 0 && device < ndev, "no such CUDA device");
-  cudaDeviceProp prop;
-  NOPE_CUDA(cudaGetDeviceProperties(&prop, device));
-  NOPE_CHECK(prop.major == 9 && prop.minor == 0, "nope_b200 kernels are built for sm_90a (H100) only");
   auto m = std::make_unique<nope_ldm>();
+  if (open_device(device, &m->num_sms)) return -1;
   m->mc = model_channels;
   m->ctx = context_dim;
   m->Cl = latent_ch;
   m->S0 = latent_hw;
   m->device = device;
-  m->num_sms = prop.multiProcessorCount;
   m->build_plan();
   m->build_schema();
   *out = m.release();
@@ -2301,33 +2141,10 @@ int nope_ldm_create(nope_ldm_t** out, int model_channels, int context_dim, int l
 void nope_ldm_destroy(nope_ldm_t* m) { delete m; }
 
 int nope_ldm_load_tensor(nope_ldm_t* m, const char* key, const float* data, const int64_t* shape, int ndim) {
-  NOPE_CHECK(m && key && data && shape, "null argument");
-  NOPE_CHECK(!m->finalized, "engine already finalized");
-  auto it = m->expected.find(key);
-  NOPE_CHECK(it != m->expected.end(), std::string("unexpected state_dict key: ") + key);
-  NOPE_CHECK((int)it->second.size() == ndim, std::string("rank mismatch for ") + key);
-  size_t n = 1;
-  for (int i = 0; i < ndim; ++i) {
-    NOPE_CHECK(it->second[i] == shape[i], std::string("shape mismatch for ") + key);
-    n *= (size_t)shape[i];
-  }
-  if (std::strncmp(key, "time_embed.", 11) == 0 || std::strstr(key, ".emb_layers.1.weight") ||
-      std::strstr(key, ".attn2.to_q.") || std::strstr(key, ".attn2.to_k.") || std::strstr(key, ".norm2.")) {
-    // accepted for schema compatibility, never read: emb = 0 (adapt_openaimodel.py:143-146) and
-    // the one-token cross-attention does not depend on its queries / keys
-    m->host[key] = nope_ldm::HostT{std::vector<int64_t>(shape, shape + ndim), {}};
-    return 0;
-  }
-  auto& slot = m->host[key];
-  slot.first.assign(shape, shape + ndim);
-  slot.second.assign(data, data + n);
-  return 0;
+  return engine_load_tensor(m, key, data, shape, ndim, !(key && nope_ldm::never_read(key)));
 }
 
-int nope_ldm_finalize(nope_ldm_t* m) {
-  NOPE_CHECK(m, "null engine");
-  return m->finalize();
-}
+int nope_ldm_finalize(nope_ldm_t* m) { return engine_finalize(m); }
 int nope_ldm_set_chunk(nope_ldm_t* m, int hyps) {
   NOPE_CHECK(m && hyps >= 1 && hyps <= 2048, "chunk must be in [1, 2048]");
   m->chunk = hyps;
@@ -2379,13 +2196,7 @@ int nope_ldm_profile_read(nope_ldm_t* m, double* ms, double* flops, int64_t* lau
 int nope_ldm_sweep_multi(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
                          const float* query_latent, int Q, float* out_emb, float* out_sim, int k, float* out_topv,
                          int64_t* out_topi, int64_t idx_base, void* stream) {
-  NOPE_CHECK(m && m->finalized, "engine not finalized");
-  NOPE_CHECK(ref_latent && poses && B >= 1 && N >= 1, "bad arguments");
-  NOPE_CHECK(Q >= 1, "Q (queries per reference) must be >= 1");
-  NOPE_CHECK((int64_t)B * Q * N <= INT32_MAX, "B * Q * N exceeds the scored-triple limit (2^31 - 1)");
-  NOPE_CHECK(!(out_sim || k > 0) || query_latent, "scores / top-k need query_latent");
-  NOPE_CHECK(k >= 0 && k <= N && k <= 64, "k must be in [0, min(N, 64)]");
-  NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
+  if (check_sweep(m, ref_latent, poses, B, N, query_latent, Q, out_sim, k, out_topv, out_topi)) return -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   NOPE_CUDA(cudaSetDevice(m->device));
   m->launches = 0;
@@ -2505,7 +2316,7 @@ int nope_op_mh_attention(int impl, const float* qkv, float* out, int n_img, int 
   e.attn_impl = impl;
   const size_t tok = (size_t)n_img * n_tok;
   __half *q16 = nullptr, *o16 = nullptr;
-  if (e.ws_half(&q16, tok * 3 * C) || e.ws_half(&o16, tok * C) || e.ws_half(&e.Vt, tok * C)) return -1;
+  if (e.ws_mem.alloc(&q16, tok * 3 * C) || e.ws_mem.alloc(&o16, tok * C) || e.ws_mem.alloc(&e.Vt, tok * C)) return -1;
   // [n_img, n_tok, 3C] fp32 is already token-major: a plain fp32 -> fp16 cast ("NCHW" with hw = 1)
   nchw_f32_to_nhwc_f16_kernel<<<ew_grid((long long)tok * 3 * C), 256, 0, st>>>(qkv, q16, (int)tok, 3 * C, 1);
   NOPE_CUDA(cudaGetLastError());

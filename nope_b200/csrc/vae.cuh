@@ -356,11 +356,10 @@ struct VaeEngine {
   const int cap;                              // images per pass
   int device = 0, num_sms = 132;
   bool finalized = false;
-  std::map<std::string, std::pair<std::vector<int64_t>, std::vector<float>>> host;
-  std::map<std::string, std::vector<int64_t>> expected;
+  StagedWeights staged;
   std::map<std::string, VaeConv> convs;
   std::map<std::string, VaeNorm> norms;
-  std::vector<void*> owned;
+  DeviceAllocs mem;                           // weights and workspace
   // workspace (alloc_workspace), each activation buffer sized for cap images of the widest level
   float* x32[2] = {nullptr, nullptr};         // residual stream, fp32
   ActPair xs[2];                              // residual stream, (hi, lo)
@@ -372,20 +371,15 @@ struct VaeEngine {
   int64_t launches = 0;
 
   explicit VaeEngine(int cap_) : cap(cap_) {}
-  VaeEngine(const VaeEngine&) = delete;
-  VaeEngine& operator=(const VaeEngine&) = delete;
-  ~VaeEngine() {
-    for (void* p : owned) cudaFree(p);
-  }
 
   // ---------------------------------------------------------------- schema (diffusers AutoencoderKL, SD v1)
   void expect_norm(const std::string& p, int c) {
-    expected[p + ".weight"] = {c};
-    expected[p + ".bias"] = {c};
+    staged.expect(p + ".weight", {c});
+    staged.expect(p + ".bias", {c});
   }
   void expect_conv(const std::string& p, int cout, int cin, int k) {
-    expected[p + ".weight"] = {cout, cin, k, k};
-    expected[p + ".bias"] = {cout};
+    staged.expect(p + ".weight", {cout, cin, k, k});
+    staged.expect(p + ".bias", {cout});
   }
   void expect_resnet(const std::string& p, int cin, int cout) {
     expect_norm(p + ".norm1", cin);
@@ -397,20 +391,13 @@ struct VaeEngine {
   void expect_attention(const std::string& a) {
     expect_norm(a + "group_norm", 512);
     for (const char* s : {"query", "key", "value", "proj_attn"}) {
-      expected[a + s + ".weight"] = {512, 512};
-      expected[a + s + ".bias"] = {512};
+      staged.expect(a + s + ".weight", {512, 512});
+      staged.expect(a + s + ".bias", {512});
     }
   }
 
   // ---------------------------------------------------------------- weights
-  template <typename T>
-  int upload(T** dst, const std::vector<T>& v) {
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(dst), v.size() * sizeof(T)));
-    owned.push_back(*dst);
-    NOPE_CUDA(cudaMemcpy(*dst, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return 0;
-  }
-  const std::vector<float>& h(const std::string& k) { return host.at(k).second; }
+  const std::vector<float>& h(const std::string& k) const { return staged.at(k).data; }
 
   // W [cout_real][cin][k*k], bias [cout_real] (float64), optional 1x1 shortcut Ws [cout_real][cin_sc] + its bias
   int pack_conv(const std::string& name, int cout_real, int cin, int k, const std::vector<double>& W,
@@ -441,7 +428,7 @@ struct VaeEngine {
     }
     std::vector<float> b(L.cout, 0.f);
     for (int o = 0; o < cout_real; ++o) b[o] = (float)bias[o];
-    if (upload(&L.w, packed) || upload(&L.bias, b)) return -1;
+    if (mem.upload(&L.w, packed) || mem.upload(&L.bias, b)) return -1;
     if (make_weight_map(&L.wmap, L.w, L.cout, L.K, L.bn)) return -1;
     convs[name] = L;
     return 0;
@@ -451,12 +438,12 @@ struct VaeEngine {
     return std::vector<double>(v.begin(), v.end());
   }
   int make_plain(const std::string& name, int k) {
-    const auto& s = host.at(name + ".weight").first;
+    const auto& s = staged.at(name + ".weight").shape;
     return pack_conv(name, (int)s[0], (int)s[1], k, dvec(name + ".weight"), dvec(name + ".bias"));
   }
   int make_norm(const std::string& name) {
     VaeNorm N;
-    if (upload(&N.gamma, h(name + ".weight")) || upload(&N.beta, h(name + ".bias"))) return -1;
+    if (mem.upload(&N.gamma, h(name + ".weight")) || mem.upload(&N.beta, h(name + ".bias"))) return -1;
     norms[name] = N;
     return 0;
   }
@@ -489,25 +476,10 @@ struct VaeEngine {
 
   // workspace of E elements per activation buffer, allocated once so that no call allocates (or synchronises)
   int alloc_workspace(size_t E) {
-    for (int s = 0; s < 2; ++s) {
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&x32[s]), E * sizeof(float)));
-      owned.push_back(x32[s]);
-      for (__half** p : {&xs[s].hi, &xs[s].lo}) {
-        NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(p), E * sizeof(__half)));
-        owned.push_back(*p);
-      }
-    }
-    for (__half** p : {&nrm.hi, &nrm.lo}) {
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(p), E * sizeof(__half)));
-      owned.push_back(*p);
-    }
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&t32), E * sizeof(float)));
-    owned.push_back(t32);
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&gn_part), (size_t)cap * 64 * 32 * sizeof(double2)));
-    owned.push_back(gn_part);
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&gn_stats), (size_t)cap * 32 * sizeof(float2)));
-    owned.push_back(gn_stats);
-    return 0;
+    for (int s = 0; s < 2; ++s)
+      if (mem.alloc(&x32[s], E) || mem.alloc(&xs[s].hi, E) || mem.alloc(&xs[s].lo, E)) return -1;
+    if (mem.alloc(&nrm.hi, E) || mem.alloc(&nrm.lo, E) || mem.alloc(&t32, E)) return -1;
+    return mem.alloc(&gn_part, (size_t)cap * 64 * 32) || mem.alloc(&gn_stats, (size_t)cap * 32) ? -1 : 0;
   }
 
   // ---------------------------------------------------------------- launches
@@ -702,6 +674,7 @@ struct VaeEngine {
 
 // ---------------------------------------------------------------- encoder (DESIGN.md section 16)
 struct nope_vae : nope::VaeEngine {
+  static constexpr const char* kName = "VAE";
   static constexpr int kChunk = 16;           // images per pass: the workspace holds this many (~200 MB each)
   static constexpr int kCh[4] = {128, 256, 512, 512};
   float *in_w = nullptr, *in_b = nullptr;
@@ -726,12 +699,10 @@ struct nope_vae : nope::VaeEngine {
     expect_conv("quant_conv", 8, 8, 1);
   }
 
+  // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
   int finalize() {
     using namespace nope;
-    NOPE_CHECK(!finalized, "already finalized");
-    for (const auto& kv : expected) NOPE_CHECK(host.count(kv.first), "state_dict is missing " + kv.first);
-    NOPE_CUDA(cudaSetDevice(device));
-    if (upload(&in_w, h("encoder.conv_in.weight")) || upload(&in_b, h("encoder.conv_in.bias"))) return -1;
+    if (mem.upload(&in_w, h("encoder.conv_in.weight")) || mem.upload(&in_b, h("encoder.conv_in.bias"))) return -1;
     int cin = 128;
     for (int i = 0; i < 4; ++i) {
       const std::string blk = "encoder.down_blocks." + std::to_string(i);
@@ -761,13 +732,9 @@ struct nope_vae : nope::VaeEngine {
       }
       if (pack_conv("conv_out", 4, 512, 3, Wf, bf)) return -1;
     }
-    host.clear();
     // workspace for kChunk images of the 256 x 256 x 128 level
     if (alloc_workspace((size_t)kChunk * 256 * 256 * 128)) return -1;
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&rot_stage), (size_t)kChunk * 3 * 256 * 256 * sizeof(float)));
-    owned.push_back(rot_stage);
-    finalized = true;
-    return 0;
+    return mem.alloc(&rot_stage, (size_t)kChunk * 3 * 256 * 256);
   }
 
   // Downsample2D: pad (0, 1, 0, 1) + 3x3 stride 2 from side 2H to H.  Tap (ky, kx) reads input (2y + ky, 2x + kx):
@@ -867,6 +834,7 @@ struct nope_vae : nope::VaeEngine {
 // end in Upsample2D, nearest x2 + 3x3 conv); GroupNorm(32) + SiLU and conv_out 3x3 (128 -> 3).  Up block 3 runs at
 // the parity-planar 256 x 256 level; the 64 x 64 and 128 x 128 levels are plain NHWC, as in the encoder.
 struct nope_vae_decoder : nope::VaeEngine {
+  static constexpr const char* kName = "VAE decoder";
   static constexpr int kChunk = 8;            // images per pass: 256 x 256 x 256 is 67 MB of fp32 per image
   static constexpr int kCh[4] = {512, 512, 256, 128};
   static constexpr const char* kAttn = "decoder.mid_block.attentions.0.";
@@ -914,18 +882,16 @@ struct nope_vae_decoder : nope::VaeEngine {
     return 0;
   }
 
+  // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
   int finalize() {
     using namespace nope;
-    NOPE_CHECK(!finalized, "already finalized");
-    for (const auto& kv : expected) NOPE_CHECK(host.count(kv.first), "state_dict is missing " + kv.first);
-    NOPE_CUDA(cudaSetDevice(device));
     {  // post_quant_conv with the 1 / 0.18215 scale folded into its weight in float64; its bias stays separate
       const auto W = dvec("post_quant_conv.weight");
       std::vector<float> w(16);
       for (int i = 0; i < 16; ++i) w[i] = (float)(W[i] / 0.18215);
-      if (upload(&pq_w, w) || upload(&pq_b, h("post_quant_conv.bias"))) return -1;
+      if (mem.upload(&pq_w, w) || mem.upload(&pq_b, h("post_quant_conv.bias"))) return -1;
     }
-    if (upload(&in_w, h("decoder.conv_in.weight")) || upload(&in_b, h("decoder.conv_in.bias"))) return -1;
+    if (mem.upload(&in_w, h("decoder.conv_in.weight")) || mem.upload(&in_b, h("decoder.conv_in.bias"))) return -1;
     if (make_resnet("decoder.mid_block.resnets.0", 512, 512) || make_attention(kAttn) ||
         make_resnet("decoder.mid_block.resnets.1", 512, 512))
       return -1;
@@ -938,11 +904,8 @@ struct nope_vae_decoder : nope::VaeEngine {
       if (i < 3 && make_upsample(up(i) + ".upsamplers.0.conv", kCh[i])) return -1;
     }
     if (make_norm("decoder.conv_norm_out") || make_plain("decoder.conv_out", 3)) return -1;
-    host.clear();
     // workspace for kChunk images of the 256 x 256 x 256 level (the same 3.2 GB as the encoder's)
-    if (alloc_workspace((size_t)kChunk * 256 * 256 * 256)) return -1;
-    finalized = true;
-    return 0;
+    return alloc_workspace((size_t)kChunk * 256 * 256 * 256);
   }
 
   // Upsample2D from side H (residual stream `cur`, plain NHWC) to 2H -> 1 - cur.  One launch per output parity

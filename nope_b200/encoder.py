@@ -115,18 +115,11 @@ class FeatureExtractor(nn.Module):
         if self._h is not None and self._h_device == device:
             return self._h
         self._drop_engine()
-        lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(lib.nope_encoder_create(C.byref(h), self.latent_dim, device.index or 0))
-        for k, v in self.state_dict().items():
-            if k.endswith("num_batches_tracked") or k.startswith("backbone.fc."):
-                continue
-            t = v.detach().to("cpu", torch.float32).contiguous()
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            _lib.check(lib.nope_encoder_load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
-        _lib.check(lib.nope_encoder_finalize(h))
-        self._h, self._h_device = h, device
-        return h
+        tensors = [(k, v) for k, v in self.state_dict().items()
+                   if not (k.endswith("num_batches_tracked") or k.startswith("backbone.fc."))]
+        self._h = _lib.build_engine("encoder", (self.latent_dim, device.index or 0), tensors)
+        self._h_device = device
+        return self._h
 
     def _use_native(self, device):
         if self.backend == "torch":

@@ -50,28 +50,43 @@ class UNetModelPose:
         if precision not in ("fp16", "fp16_w2"):
             raise ValueError("UNetModelPose precision: 'fp16' or 'fp16_w2'")
         self.precision = precision
+        self._impl = (2, 0)         # nope_ldm_set_impl (conv, attn)
+        self._options = {}          # nope_ldm_set_option name -> value, re-applied to every engine
         self._h = None
         self._finalized = False
 
+    def _create_args(self):
+        if self.device.type != "cuda":
+            raise _lib.NopeError("nope_b200.UNetModelPose needs a CUDA device (no CPU fallback)")
+        return self.model_channels, self.context_dim, self.channels, 32, self.device.index or 0
+
+    def _configure(self, lib, h):
+        """chunk, precision, implementation and options: applied to every engine before its weights"""
+        _lib.check(lib.nope_ldm_set_chunk(h, self._chunk))
+        if self.precision == "fp16_w2":
+            _lib.check(lib.nope_ldm_set_option(h, b"precision", 1))
+        _lib.check(lib.nope_ldm_set_impl(h, *self._impl))
+        for k, v in self._options.items():
+            _lib.check(lib.nope_ldm_set_option(h, k.encode(), v))
+
     def _handle(self):
-        if self._h is None:
+        if self._h is None:         # an engine without weights yet
             lib = _lib.load()
-            if self.device.type != "cuda":
-                raise _lib.NopeError("nope_b200.UNetModelPose needs a CUDA device (no CPU fallback)")
             h = C.c_void_p()
-            _lib.check(lib.nope_ldm_create(C.byref(h), self.model_channels, self.context_dim,
-                                           self.channels, 32, self.device.index or 0))
+            _lib.check(lib.nope_ldm_create(C.byref(h), *self._create_args()))
             self._h = h
-            _lib.check(lib.nope_ldm_set_chunk(h, self._chunk))
-            if self.precision == "fp16_w2":
-                _lib.check(lib.nope_ldm_set_option(h, b"precision", 1))
+            self._configure(lib, h)
         return self._h
+
+    def _destroy(self):
+        if self._h is not None:
+            _lib.load().nope_ldm_destroy(self._h)
+            self._h = None
+        self._finalized = False
 
     def __del__(self):
         try:
-            if self._h is not None:
-                _lib.load().nope_ldm_destroy(self._h)
-                self._h = None
+            self._destroy()
         except Exception:
             pass
 
@@ -80,18 +95,15 @@ class UNetModelPose:
 
     def load_state_dict(self, state_dict, strict=True):
         """Reference UNetModelPose.state_dict() keys; `encoder.*` entries are skipped, except that a
-        VAE_StableDiffusion encoder receives the `encoder.encoder.*` entries (AutoencoderKL keys)."""
+        VAE_StableDiffusion encoder receives the `encoder.encoder.*` entries (AutoencoderKL keys).  May be called
+        again: every call builds a fresh engine (the weights are packed at finalize)."""
         from .unet import encoder_entries
         from .vae import VAE_StableDiffusion
-        lib = _lib.load()
-        h = self._handle()
-        for k, v in state_dict.items():
-            if k.startswith("encoder."):
-                continue
-            t = v.detach().to("cpu", torch.float32).contiguous()
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            _lib.check(lib.nope_ldm_load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
-        _lib.check(lib.nope_ldm_finalize(h))
+        create_args = self._create_args()
+        self._destroy()
+        self._h = _lib.build_engine("ldm", create_args,
+                                    ((k, v) for k, v in state_dict.items() if not k.startswith("encoder.")),
+                                    self._configure)
         self._finalized = True
         if isinstance(self.encoder, VAE_StableDiffusion):
             vae_sd = encoder_entries(state_dict, self.encoder)
@@ -105,11 +117,13 @@ class UNetModelPose:
             _lib.check(_lib.load().nope_ldm_set_chunk(self._h, hyps))
 
     def set_impl(self, conv="tcgen05_2cta", attn="tcgen05"):
-        _lib.check(_lib.load().nope_ldm_set_impl(self._handle(), {"tcgen05_2cta": 2}[conv],
-                                                 {"tcgen05": 0, "simt": 1}[attn]))
+        impl = ({"tcgen05_2cta": 2}[conv], {"tcgen05": 0, "simt": 1}[attn])
+        _lib.check(_lib.load().nope_ldm_set_impl(self._handle(), *impl))
+        self._impl = impl
 
     def set_option(self, name, value):
         _lib.check(_lib.load().nope_ldm_set_option(self._handle(), name.encode(), int(value)))
+        self._options[name] = int(value)
 
     @property
     def last_launch_count(self):

@@ -75,19 +75,25 @@ class UNet:
         self._state = None         # last loaded UNet tensors (CPU fp32), kept for reload / partial load
 
     # ------------------------------------------------------------------ lifetime
+    def _create_args(self):
+        if self.device.type != "cuda":
+            raise _lib.NopeError("nope_b200.UNet needs a CUDA device (no CPU fallback)")
+        return self.u_net_dim, self.channels, 32, self.device.index or 0
+
+    def _configure(self, lib, h):
+        """chunk, precision and options: applied to every engine before its weights"""
+        _lib.check(lib.nope_unet_set_chunk(h, self._chunk))
+        _lib.check(lib.nope_unet_set_option(h, b"precision", PRECISIONS[self.precision]))
+        for k, v in self._options.items():
+            _lib.check(lib.nope_unet_set_option(h, k.encode(), int(v)))
+
     def _handle(self):
-        if self._h is None:
+        if self._h is None:         # an engine without weights yet
             lib = _lib.load()
-            if self.device.type != "cuda":
-                raise _lib.NopeError("nope_b200.UNet needs a CUDA device (no CPU fallback)")
             h = C.c_void_p()
-            _lib.check(lib.nope_unet_create(C.byref(h), self.u_net_dim, self.channels, 32,
-                                            self.device.index or 0))
+            _lib.check(lib.nope_unet_create(C.byref(h), *self._create_args()))
             self._h = h
-            _lib.check(lib.nope_unet_set_chunk(h, self._chunk))
-            _lib.check(lib.nope_unet_set_option(h, b"precision", PRECISIONS[self.precision]))
-            for k, v in self._options.items():
-                _lib.check(lib.nope_unet_set_option(h, k.encode(), int(v)))
+            self._configure(lib, h)
         return self._h
 
     def _destroy(self):
@@ -130,7 +136,6 @@ class UNet:
         and the (missing, unexpected) lists are returned.  A shape mismatch always raises, as
         nn.Module.load_state_dict does; the shape-FILTERED load of the reference
         (src/utils/weight.py:6-37) is nope_b200.weight.load_checkpoint."""
-        lib = _lib.load()
         want = self.expected_shapes()
         unet_sd, unexpected = {}, []
         enc_sd = encoder_entries(state_dict, self.encoder)
@@ -152,15 +157,11 @@ class UNet:
         still = [k for k in want if k not in merged]
         if still:
             raise RuntimeError(f"UNet tensors never provided: {still[:5]}{'...' if len(still) > 5 else ''}")
-        if self._h is not None and self._finalized:
-            self._destroy()       # weights are repacked at finalize: a reload builds a fresh engine
-        h = self._handle()
-        for k, t in merged.items():
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            _lib.check(lib.nope_unet_load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
+        create_args = self._create_args()
         if enc_sd:
             self.encoder.load_state_dict(enc_sd, strict=strict)
-        _lib.check(lib.nope_unet_finalize(h))
+        self._destroy()           # weights are repacked at finalize: every load builds a fresh engine
+        self._h = _lib.build_engine("unet", create_args, merged.items(), self._configure)
         self._state = merged
         self._finalized = True
         self.encoder.to(self.device)

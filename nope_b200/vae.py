@@ -303,19 +303,8 @@ class VAE_StableDiffusion:
             return self._h
         if self._sd is None:
             raise _lib.NopeError("VAE_StableDiffusion has no weights: pass pretrained_path or call load_state_dict")
-        lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(lib.nope_vae_create(C.byref(h), self.device.index or 0))
-        try:
-            for k, t in self._sd.items():
-                shape = (C.c_int64 * t.dim())(*t.shape)
-                _lib.check(lib.nope_vae_load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
-            _lib.check(lib.nope_vae_finalize(h))
-        except Exception:
-            lib.nope_vae_destroy(h)
-            raise
-        self._h = h
-        return h
+        self._h = _lib.build_engine("vae", (self.device.index or 0,), self._sd.items())
+        return self._h
 
     def _images(self, image):
         if self.device.type != "cuda":
@@ -389,19 +378,8 @@ class VAE_StableDiffusion:
         if missing:
             raise _lib.NopeError(f"decode_latent needs the AutoencoderKL decoder weights: {len(missing)} of the "
                                  f"{len(vae_decoder_param_shapes())} decoder tensors are missing, e.g. {missing[:5]}")
-        lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(lib.nope_vae_decoder_create(C.byref(h), self.device.index or 0))
-        try:
-            for k, t in self._dec_sd.items():
-                shape = (C.c_int64 * t.dim())(*t.shape)
-                _lib.check(lib.nope_vae_decoder_load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
-            _lib.check(lib.nope_vae_decoder_finalize(h))
-        except Exception:
-            lib.nope_vae_decoder_destroy(h)
-            raise
-        self._dec_h = h
-        return h
+        self._dec_h = _lib.build_engine("vae_decoder", (self.device.index or 0,), self._dec_sd.items())
+        return self._dec_h
 
     @property
     def last_decode_launch_count(self):
