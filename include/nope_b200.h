@@ -67,9 +67,9 @@ int nope_unet_load_tensor(nope_unet_t* u, const char* key, const float* data,
  * pose projections concatenated into one GEMM) and uploads them. */
 int nope_unet_finalize(nope_unet_t* u);
 
-/* Tunables: hypotheses per chunk (workspace = ~5.5 MB per hypothesis), and the
- * convolution implementation: 0 = wgmma tensor cores, single-CTA kernel, 1 = SIMT debug
- * twin, 2 = wgmma, clustered kernel with the fused epilogues (default). */
+/* Tunables: hypotheses per chunk (workspace = ~4.7 MB per hypothesis at u_net_dim 192), and the
+ * convolution implementation: 2 = wgmma, clustered kernel with the fused epilogues (the only one;
+ * anything else is an error). */
 int nope_unet_set_chunk(nope_unet_t* u, int hyps_per_chunk);
 int nope_unet_set_conv_impl(nope_unet_t* u, int impl);
 /* Named options:
@@ -81,9 +81,6 @@ int nope_unet_set_conv_impl(nope_unet_t* u, int impl);
  *       activations (BASELINE configs[2]; 8-bit mantissa: embeddings ~1e-2 of the fp32 reference),
  *       4 = split precision with single-fp16 tensors inside the ResnetBlocks (block2 convolutions run two
  *       products instead of three; embeddings ~5e-4: the fastest mode inside the 1e-3 tolerance);
- *   "fuse_gn" (default 1): GroupNorm + SiLU + pose bias + residual run in the epilogue of the producing
- *       convolution (Block.forward / ResnetBlock.forward, model_utils.py:237-279); 0 = separate
- *       gn_apply pass (round-1 schedule; also what conv_impl 0 / 1 use);
  *   "conv_impl": as nope_unet_set_conv_impl;
  *   "attn_impl": LinearAttention core, 0 = wgmma kernel at 32x32 / 16x16 (CUDA cores below 128 tokens),
  *       1 = CUDA-core kernel everywhere. */
@@ -411,16 +408,17 @@ int nope_topk_merge(const float* gathered, int world, int64_t pack_floats, int B
  *       [n, C0, 2H, 2W], weight [Cout, 4*C0]), 3 = nearest-x2 upsample + 3x3 (HardUpsample,
  *       model_utils.py:161-165; input is [n, C0, H/2, W/2], weight [Cout, C0, 3, 3], folded
  *       inside into four 2x2 parity kernels).  x1 (optional) is concatenated after x0 along
- *       channels (u_net.py:186).  impl as in nope_unet_set_conv_impl. */
+ *       channels (u_net.py:186).  impl must be 2, as in nope_unet_set_conv_impl. */
 int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, int C1,
                  const float* weight, const float* bias, float* out, int n_img, int H, int W,
                  int Cout, void* stream);
-/* Block.forward (model_utils.py:248-252): [SiLU](GroupNorm_G(conv(x) + bias)) with the
- * GroupNorm statistics taken from the convolution epilogue -- the fused path the sweep uses. */
+/* Block.forward (model_utils.py:248-252): [SiLU](GroupNorm_G(conv(x) + bias)), normalised on the host
+ * from nothing but the per-(32 pixels, 8 channels) partial sums the plain convolution epilogue writes
+ * (the statistics the LDM engine's GroupNorms use).  mode 0..2 as nope_op_conv, impl must be 2. */
 int nope_op_conv_gn(int impl, int mode, const float* x0, int C0, const float* x1, int C1,
                     const float* weight, const float* bias, const float* gamma, const float* beta,
                     int G, int silu, float* out, int n_img, int H, int W, int Cout, void* stream);
-/* The sweep's fused layer (conv_impl 2): out = [SiLU](GroupNorm_G(conv(x) + bias)) + chan_bias[n, c] +
+/* The sweep's fused layer: out = [SiLU](GroupNorm_G(conv(x) + bias)) + chan_bias[n, c] +
  * residual[n / res_div] with everything after the convolution applied in its epilogue
  * (ResnetBlock.forward, model_utils.py:271-279; G = 0: no normalisation).  mode 0..2 as nope_op_conv.
  * precision as nope_unet_set_option.  chan_bias [n, Cout], residual [ceil(n / res_div), Cout, H, W]
@@ -430,10 +428,6 @@ int nope_op_conv_gn_fused(int mode, int precision, const float* x0, int C0, cons
                           const float* weight, const float* bias, const float* gamma, const float* beta,
                           int G, int silu, const float* chan_bias, const float* residual, int res_div,
                           float* out, float* emit_out, int n_img, int H, int W, int Cout, void* stream);
-/* y = [SiLU](GroupNorm_G(x)) + chan_bias[n, c] + residual   (model_utils.py:237-253,271-279) */
-int nope_op_groupnorm(const float* x, const float* gamma, const float* beta, int G, int silu,
-                      const float* chan_bias, const float* residual, float* out, int n_img,
-                      int C, int H, int W, void* stream);
 /* LinearAttention core on qkv [n, 384, H, W] -> [n, 128, H, W] (model_utils.py:403-417).
  * impl 0: wgmma kernel (both contractions on tensor cores, H*W a multiple of 128), 1: CUDA cores. */
 int nope_op_linear_attention(int impl, const float* qkv, float* out, int n_img, int H, int W, void* stream);

@@ -89,8 +89,6 @@ SIGNATURES = {
     "nope_op_conv_gn": (C.c_int, [C.c_int, C.c_int, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, c_f32p,
                                   c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int,
                                   C.c_int, C.c_void_p]),
-    "nope_op_groupnorm": (C.c_int, [c_f32p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, c_f32p, c_f32p,
-                                    C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_op_linear_attention": (C.c_int, [C.c_int, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_op_attention": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_op_upsample2x": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),

@@ -1,6 +1,8 @@
-// nope_b200 -- implicit-GEMM convolution on wgmma tensor cores (sm_90a).
+// nope_b200 -- implicit-GEMM convolution on wgmma tensor cores (sm_90a): the pieces the clustered
+// kernel (conv_tc2_kernel, conv_tc2.cuh) is built from -- launch parameters (ConvParams, GnFuse), the
+// wgmma mainloop of one tile (conv_mma_tile), the plain and GEGLU epilogues, and the tensor-map helpers.
 //
-// One kernel serves every GEMM-shaped op of the pose-conditioned UNet
+// The convolution serves every GEMM-shaped op of the pose-conditioned UNet
 // (reference: src/model/u_net/denoising_diffusion_pytorch/model_utils.py:240
 //  conv3x3, :171 1x1-after-unshuffle, :269 res_conv, :373-374/:399-401 qkv and
 //  to_out 1x1, :261-263 the pose projection Linear):
@@ -17,12 +19,6 @@
 // the canonical wgmma operand layout.  Channel concatenation (skip
 // connections, u_net.py:186-194) is two source tensor maps walked by the same K
 // loop; pixel-unshuffle + 1x1 (HardDownsample) is four stride-2 tensor maps.
-//
-// CTA = 12 warps, persistent over (m_tile, n_tile) work items:
-//   warp 0        : TMA producer      (smem ring, full/empty mbarriers; one elected lane issues)
-//   warps 4..11   : two warpgroups: wgmma mainloop (warpgroup w owns rows 64 w .. 64 w + 63 and all of the
-//                   tile's columns, accumulator in registers), then the fp32 tile through shared memory
-//                   (conv_mma_tile) -> +bias -> GroupNorm partial sums -> fp16 -> swizzled smem -> TMA store
 #pragma once
 #include "common.cuh"
 #include <cudaTypedefs.h>
@@ -134,19 +130,6 @@ struct ConvParams {
   int tiles_per_img;  // H*W/128 when H*W >= 128, else 0
   int h_cnt, b_cnt;   // box rows per tile / images per tile
   ConvSeg seg[kMaxSeg];
-};
-
-template <int BN, int STAGES>
-struct ConvSmem {
-  static constexpr int kABytes = kBM * kBK * 2;
-  static constexpr int kBBytes = BN * kBK * 2;
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kOutBytes = (BN / 64) * kBM * 128;
-  static constexpr int kBarOffset = STAGES * kStageBytes + kOutBytes;
-  static constexpr int kBiasOffset = kBarOffset + 256;
-  static constexpr int kTotal = kBiasOffset + BN * 4 + 1024;  // + alignment slack
-  static_assert(STAGES * kStageBytes >= kBM * (BN + 4) * 4, "the fp32 accumulator tile must fit in the operand ring");
-  static_assert(kTotal <= 227 * 1024, "shared memory per block");
 };
 
 __device__ __forceinline__ void conv_tile_coords(const ConvParams& p, int m_tile, int& b0,
@@ -458,108 +441,6 @@ __device__ __forceinline__ void conv_epilogue_geglu(uint8_t* out_stage, const fl
   }
 }
 
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(kConvThreads, 1)
-conv_tc_kernel(const __grid_constant__ ConvParams p) {
-  using S = ConvSmem<BN, STAGES>;
-  static_assert(BN % 64 == 0 && BN <= 256, "BN must be a multiple of 64");
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* out_stage = smem + STAGES * S::kStageBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tempty_bar = empty_bar + STAGES;
-  float* s_bias = reinterpret_cast<float*>(smem + S::kBiasOffset);
-  float* s_acc = reinterpret_cast<float*>(smem);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int num_tiles = p.m_tiles * p.n_tiles;
-
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < p.n_amaps; ++i) prefetch_tmap(&p.amap[i]);
-    prefetch_tmap(&p.bmap);
-    for (int i = 0; i < p.n_par; ++i) prefetch_tmap(&p.omap[i]);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], conv_mma_warps(2));
-    }
-    mbar_init(tempty_bar, kEpiWarps);
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  // The producer runs its loop warp-converged and elects one lane only around the instruction issue:
-  // control flow and address arithmetic stay on the uniform datapath.
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    int stage = 0;
-    uint32_t phase = 0;
-    int iter = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++iter) {
-      const int m_tile = tile / p.n_tiles;
-      const int n_tile = tile - m_tile * p.n_tiles;
-      const int par = n_tile / p.n_tiles_par;          // 0 unless n_par == 4
-      const int py = par >> 1, px = par & 1;
-      int b0, y0;
-      conv_tile_coords(p, m_tile, b0, y0);
-      if (iter > 0) mbar_wait(tempty_bar, (iter - 1) & 1);     // the previous accumulator tile left the ring
-      int kcol = 0;
-      for (int s = 0; s < p.nseg; ++s) {
-        const ConvSeg sg = p.seg[s];
-        const CUtensorMap* am = &p.amap[sg.map];
-        if (sg.wcol1) kcol = sg.wcol1 - 1;
-        for (int ch = 0; ch < sg.nchunks; ++ch) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (elect_one()) {
-            uint8_t* sa = smem + stage * S::kStageBytes;
-            mbar_expect_tx(&full_bar[stage], S::kStageBytes);
-            tma_load_4d(sa, am, &full_bar[stage], ch * kBK, sg.dx + px, y0 + sg.dy + py, b0);
-            tma_load_2d(sa + S::kABytes, &p.bmap, &full_bar[stage], kcol, n_tile * BN);
-          }
-          kcol += kBK;
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== mainloop + epilogue (8 warps) =====================
-    const int e = warp - 4;
-    const int etid = threadIdx.x - 128;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_tile = tile / p.n_tiles;
-      const int n_tile = tile - m_tile * p.n_tiles;
-      const int par = n_tile / p.n_tiles_par;
-      const int n_chan0 = (n_tile - par * p.n_tiles_par) * BN;   // first output channel of the tile
-      int b0, y0;
-      conv_tile_coords(p, m_tile, b0, y0);
-      if (etid < BN) s_bias[etid] = p.bias ? __ldg(p.bias + n_chan0 + etid) : 0.f;
-      // staging buffer must have been fully read by the previous TMA store; bias visible
-      if (etid == 0) tma_store_wait_read0();
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      conv_mma_tile<BN, 2, STAGES, S::kStageBytes, S::kABytes>(p, smem, full_bar, empty_bar, stage, phase, s_acc);
-      conv_epilogue_tile<BN, false>(p, out_stage, s_bias, s_acc, m_tile, n_chan0, e, lane);
-      acc_release(tempty_bar, lane);
-      // make the generic-proxy smem writes visible to the TMA (async proxy), then store
-      fence_proxy_async_smem();
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (etid == 0) {
-#pragma unroll 1
-        for (int cc = 0; cc < BN / 64; ++cc)
-          tma_store_4d(&p.omap[par], out_stage + cc * (kBM * 128), n_chan0 + cc * 64, 0, y0, b0);
-        tma_store_commit();
-      }
-    }
-    if (etid == 0) tma_store_wait_all();
-  }
-}
-
 // ----------------------------------------------------------------------------
 // host side: tensor maps + launch
 // ----------------------------------------------------------------------------
@@ -657,35 +538,6 @@ inline int pick_bn(int n_total) {
 
 inline bool conv_needs_extras(const ConvParams& p) {
   return p.relu || p.res_hi || p.out_lo || p.out_f32;
-}
-
-template <int BN, int STAGES>
-inline int launch_conv_tc_t(const ConvParams& p, int num_sms, cudaStream_t stream) {
-  using S = ConvSmem<BN, STAGES>;
-  static bool attr_set[kMaxDevices];     // the opt-in is per device
-  int dev = 0;
-  NOPE_CUDA(cudaGetDevice(&dev));
-  NOPE_CHECK(dev >= 0 && dev < kMaxDevices, "device index out of range");
-  if (!attr_set[dev]) {
-    NOPE_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES>,
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal));
-    attr_set[dev] = true;
-  }
-  const int tiles = p.m_tiles * p.n_tiles;
-  const int grid = tiles < num_sms ? tiles : num_sms;
-  conv_tc_kernel<BN, STAGES><<<grid, kConvThreads, S::kTotal, stream>>>(p);
-  NOPE_CUDA(cudaGetLastError());
-  return 0;
-}
-
-inline int launch_conv_tc(const ConvParams& p, int bn, int num_sms, cudaStream_t stream) {
-  if (conv_needs_extras(p)) return fail("launch_conv_tc: epilogue extras need the clustered kernel");
-  switch (bn) {
-    case 192: return launch_conv_tc_t<192, 4>(p, num_sms, stream);
-    case 128: return launch_conv_tc_t<128, 5>(p, num_sms, stream);
-    case 64: return launch_conv_tc_t<64, 6>(p, num_sms, stream);
-  }
-  return fail("launch_conv_tc: unsupported BN");
 }
 
 }  // namespace nope

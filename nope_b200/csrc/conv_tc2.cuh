@@ -1,6 +1,6 @@
-// nope_b200 -- clustered variant of the implicit-GEMM convolution, with the fused epilogues.
+// nope_b200 -- the implicit-GEMM convolution kernel, with the fused epilogues.
 //
-// Same math, parameters and epilogue as conv_tc_kernel (conv_tc.cuh); CTAs are launched in
+// Math, parameters, mainloop and plain epilogue come from conv_tc.cuh; CTAs are launched in
 // thread-block clusters of 2 that walk the tile list in PAIRS of 128-pixel M-tiles (tile
 // (m_pair, n_tile) -> M-tiles 2 m_pair and 2 m_pair + 1, one per CTA), so the two CTAs of a pair
 // read the same weight tile at the same time and the second read is served by L2.  Each CTA

@@ -1,7 +1,6 @@
 // nope_b200 -- the HBM-bound kernels around the tensor-core convolutions:
-// weight packing, pose embedding, GroupNorm(+SiLU,+pose bias,+residual), linear
-// attention, bottleneck attention, nearest upsample, the fused final 1x1 conv +
-// l2 score, top-k.  All activations are NHWC fp16; statistics, softmax and
+// weight packing, pose embedding, linear attention, bottleneck attention, nearest
+// upsample, the fused final 1x1 conv + l2 score, top-k.  All activations are NHWC fp16; statistics, softmax and
 // scores are fp32.  Each kernel cites the reference code it reproduces (paths
 // relative to the reference root).
 #pragma once
@@ -199,288 +198,13 @@ __global__ void bcast_add_kernel(const __half* __restrict__ src, const int* __re
   }
 }
 
-// ----------------------------------------------------------------------------
-// GroupNorm (model_utils.py:241-252 Block.norm, :230 PreNorm, :401 to_out[1]), eps 1e-5,
-// biased variance, fp32 statistics.  Two kernels: deterministic partial sums per
-// (hypothesis, pixel slab, group), then a fused apply:
-//   y = [SiLU](x * scale + shift) + pose_bias[h, c] + residual[res_of[h], p, c]
-// Thread mapping: blockDim = octets * rows, thread -> (8-channel octet, pixel row);
-// consecutive threads read consecutive 16-byte vectors of one pixel (coalesced).
-// ----------------------------------------------------------------------------
-__host__ __device__ inline int gn_rows(int C) {
-  const int octs = C / 8;
-  const int r = 384 / octs;
-  return r < 1 ? 1 : r;
-}
-
-__global__ void gn_stats_kernel(const __half* __restrict__ x, float2* __restrict__ partial,
-                                int hw, int C, int G, int nslab) {
-  extern __shared__ float2 s_red[];
-  const int octs = C / 8;
-  const int rows = blockDim.x / octs;
-  const int o = threadIdx.x % octs;
-  const int r = threadIdx.x / octs;
-  const int slab = blockIdx.x, h = blockIdx.y;
-  const int pps = hw / nslab;
-  const __half* base = x + ((long long)h * hw + (long long)slab * pps) * C + o * 8;
-  float s = 0.f, ss = 0.f;
-  for (int p = r; p < pps; p += rows) {
-    const uint4 v = *reinterpret_cast<const uint4*>(base + (long long)p * C);
-    const __half2* hv = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float2 f = __half22float2(hv[q]);
-      s += f.x + f.y;
-      ss = fmaf(f.x, f.x, ss);
-      ss = fmaf(f.y, f.y, ss);
-    }
-  }
-  s_red[threadIdx.x] = make_float2(s, ss);
-  __syncthreads();
-  if (threadIdx.x < G) {
-    const int opg = octs / G;
-    float a = 0.f, b = 0.f;
-    for (int rr = 0; rr < rows; ++rr)
-      for (int oo = 0; oo < opg; ++oo) {
-        const float2 t = s_red[rr * octs + threadIdx.x * opg + oo];
-        a += t.x;
-        b += t.y;
-      }
-    partial[((long long)h * nslab + slab) * G + threadIdx.x] = make_float2(a, b);
-  }
-}
-
-// Statistics of an NHWC fp16 tensor in the conv-epilogue format (parts of 32 pixels x
-// 8-channel octets); used only behind the SIMT debug convolution.  grid (parts, img).
-__global__ void stats_ref_kernel(const __half* __restrict__ x, float2* __restrict__ stats, int hw,
-                                 int C) {
-  const int part = blockIdx.x, img = blockIdx.y, parts = gridDim.x;
-  const int noct = C / 8;
-  const int npx = hw < 32 ? hw : 32;
-  for (int o = threadIdx.x; o < noct; o += blockDim.x) {
-    float s = 0.f, ss = 0.f;
-    for (int p = 0; p < npx; ++p) {
-      const __half* px = x + ((size_t)img * hw + part * 32 + p) * C + o * 8;
-      for (int i = 0; i < 8; ++i) {
-        const float f = __half2float(px[i]);
-        s += f;
-        ss = fmaf(f, f, ss);
-      }
-    }
-    stats[((size_t)img * parts + part) * noct + o] = make_float2(s, ss);
-  }
-}
-
-struct GnApplyArgs {
-  const __half* x;
-  __half* y;
-  // Partial statistics [img][parts][noct] of (sum, sum of squares); the channels of group g
-  // are covered by entries g*opg .. g*opg+opg-1 of each part (opg = noct / G).  Producers:
-  // the conv epilogue (parts = max(1, hw/32), noct = C/8), gn_stats_kernel (parts = nslab,
-  // noct = G) or a previous gn_apply with `emit` (parts = nslab, noct = 1, G = 1).
-  // nullptr => no normalisation (y = x + ...).
-  const float2* stats;
-  int st_parts, st_noct;
-  const float* gamma;
-  const float* beta;
-  const __half* pb;       // per-hypothesis channel bias (added after the activation) or nullptr
-  const __half* res;      // residual or nullptr
-  const int* res_of;      // hypothesis -> residual image index, nullptr => identity
-  float2* emit;           // optional: per (img, fixed sub-slab) sum / sum of squares of y
-  int emit_parts;         // fixed sub-slabs per image (independent of nslab)
-  int pb_stride, pb_off;
-  int hw, C, G, nslab;
-  int silu;
-  float eps;
-  int bf16;               // 16-bit storage format of x / y / pb / res
-};
-
+// 16-byte load that does not allocate in L1: for tensors each thread reads exactly once
 __device__ __forceinline__ uint4 ld_stream16(const __half* p) {
   uint4 r;
   asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
                : "l"(p));
   return r;
-}
-
-constexpr int kGnUnroll = 4;   // independent 16-byte loads in flight per thread
-
-template <bool SILU, bool PB, bool RES>
-__global__ void __launch_bounds__(384, 2) gn_apply_kernel(const GnApplyArgs a) {
-  pdl_sync();
-  __shared__ float2 s_red[256];
-  __shared__ float2 s_grp[8];
-  const int octs = a.C / 8;
-  const int rows = blockDim.x / octs;
-  const int o = threadIdx.x % octs;
-  const int r = threadIdx.x / octs;
-  const int slab = blockIdx.x, h = blockIdx.y;
-  float scale[8], shift[8], pbv[8];
-  const bool bf = a.bf16 != 0;
-  if (a.stats) {
-    // independent loads first (affine parameters), then the partial statistics
-    float4 g0 = *reinterpret_cast<const float4*>(a.gamma + o * 8);
-    float4 g1 = *reinterpret_cast<const float4*>(a.gamma + o * 8 + 4);
-    float4 be0 = *reinterpret_cast<const float4*>(a.beta + o * 8);
-    float4 be1 = *reinterpret_cast<const float4*>(a.beta + o * 8 + 4);
-    // cooperative, fixed-order reduction of this image's partials: tpg threads per group
-    const int opg = a.st_noct / a.G;
-    const int E = a.st_parts * opg;
-    int tpg = 256 / a.G;
-    if (tpg > E) tpg = E;
-    if ((int)threadIdx.x < a.G * tpg) {
-      const int g = threadIdx.x / tpg, li = threadIdx.x - g * tpg;
-      float s = 0.f, ss = 0.f;
-      for (int e = li; e < E; e += tpg) {
-        const int part = e / opg, oo = e - part * opg;
-        const float2 t = a.stats[((size_t)h * a.st_parts + part) * a.st_noct + g * opg + oo];
-        s += t.x;
-        ss += t.y;
-      }
-      s_red[threadIdx.x] = make_float2(s, ss);
-    }
-    __syncthreads();
-    if ((int)threadIdx.x < a.G) {
-      float s = 0.f, ss = 0.f;
-      for (int i = 0; i < tpg; ++i) {
-        const float2 t = s_red[threadIdx.x * tpg + i];
-        s += t.x;
-        ss += t.y;
-      }
-      s_grp[threadIdx.x] = make_float2(s, ss);
-    }
-    __syncthreads();
-    const float2 tot = s_grp[o / (octs / a.G)];
-    const float cnt = (float)a.hw * (float)(a.C / a.G);
-    const float mean = tot.x / cnt;
-    const float var = fmaxf(tot.y / cnt - mean * mean, 0.f);
-    const float rstd = rsqrtf(var + a.eps);
-    const float gm[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-    const float bt[8] = {be0.x, be0.y, be0.z, be0.w, be1.x, be1.y, be1.z, be1.w};
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      scale[i] = rstd * gm[i];
-      shift[i] = bt[i] - mean * scale[i];
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { scale[i] = 1.f; shift[i] = 0.f; }
-  }
-  if (PB) {
-    const uint4 pv = *reinterpret_cast<const uint4*>(a.pb + (long long)h * a.pb_stride + a.pb_off + o * 8);
-    const uint32_t* hp = reinterpret_cast<const uint32_t*>(&pv);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float2 t = unpack2(hp[q], bf);
-      pbv[2 * q] = t.x;
-      pbv[2 * q + 1] = t.y;
-    }
-  }
-  // The CTA covers pixel slab `slab` of nslab; statistics are emitted per FIXED sub-slab
-  // (a.emit_parts per image, independent of nslab) and every sub-slab is reduced with the same
-  // thread->pixel assignment and the same tree, so the emitted sums -- and everything
-  // downstream -- do not depend on how many images share the launch.
-  const int pps = a.hw / a.nslab;
-  const int nsub = a.emit ? a.emit_parts / a.nslab : 1;   // fixed sub-slabs handled by this CTA
-  const int spp = pps / nsub;                             // pixels per sub-slab
-  const __half* xp = a.x + ((long long)h * a.hw + (long long)slab * pps) * a.C + o * 8;
-  __half* yp = a.y + ((long long)h * a.hw + (long long)slab * pps) * a.C + o * 8;
-  const __half* rp = nullptr;
-  if (RES)
-    rp = a.res + ((long long)(a.res_of ? a.res_of[h] : h) * a.hw + (long long)slab * pps) * a.C + o * 8;
-  for (int sub = 0; sub < nsub; ++sub) {
-    float es = 0.f, ess = 0.f;
-    const int pbeg = sub * spp, pend = pbeg + spp;
-    for (int p0 = pbeg + r; p0 < pend; p0 += rows * kGnUnroll) {
-      uint4 xv[kGnUnroll], rv[kGnUnroll];
-#pragma unroll
-      for (int u = 0; u < kGnUnroll; ++u) {
-        const int p = p0 + u * rows;
-        if (p < pend) {
-          xv[u] = ld_stream16(xp + (long long)p * a.C);
-          if (RES) rv[u] = ld_stream16(rp + (long long)p * a.C);
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < kGnUnroll; ++u) {
-        const int p = p0 + u * rows;
-        if (p >= pend) break;
-        const uint32_t* hv = reinterpret_cast<const uint32_t*>(&xv[u]);
-        float f[8];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float2 t = unpack2(hv[q], bf);
-          f[2 * q] = t.x;
-          f[2 * q + 1] = t.y;
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float t = fmaf(f[i], scale[i], shift[i]);
-          if (SILU) t = silu_f(t);
-          if (PB) t += pbv[i];
-          f[i] = t;
-        }
-        if (RES) {
-          const uint32_t* hr = reinterpret_cast<const uint32_t*>(&rv[u]);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float2 t = unpack2(hr[q], bf);
-            f[2 * q] += t.x;
-            f[2 * q + 1] += t.y;
-          }
-        }
-        uint4 w;
-        w.x = pack2(f[0], f[1], bf);
-        w.y = pack2(f[2], f[3], bf);
-        w.z = pack2(f[4], f[5], bf);
-        w.w = pack2(f[6], f[7], bf);
-        *reinterpret_cast<uint4*>(yp + (long long)p * a.C) = w;
-        if (a.emit) {
-          // statistics of the values as stored (fp16-rounded), what the consumer will read
-          const uint32_t* hw2 = reinterpret_cast<const uint32_t*>(&w);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float2 t = unpack2(hw2[q], bf);
-            es += t.x + t.y;
-            ess = fmaf(t.x, t.x, ess);
-            ess = fmaf(t.y, t.y, ess);
-          }
-        }
-      }
-    }
-    if (a.emit) {
-      __syncthreads();   // s_red reuse
-#pragma unroll
-      for (int off2 = 16; off2 > 0; off2 >>= 1) {
-        es += __shfl_xor_sync(0xffffffffu, es, off2);
-        ess += __shfl_xor_sync(0xffffffffu, ess, off2);
-      }
-      if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = make_float2(es, ess);
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        float s = 0.f, ss = 0.f;
-        for (int i = 0; i < (int)((blockDim.x + 31) >> 5); ++i) {
-          s += s_red[i].x;
-          ss += s_red[i].y;
-        }
-        a.emit[(size_t)h * a.emit_parts + slab * nsub + sub] = make_float2(s, ss);
-      }
-    }
-  }
-}
-
-inline cudaError_t launch_gn_apply(const GnApplyArgs& a, dim3 grid, int threads, cudaStream_t st) {
-  const int key = (a.silu ? 4 : 0) | (a.pb ? 2 : 0) | (a.res ? 1 : 0);
-  switch (key) {
-    case 0: return launch_pdl(gn_apply_kernel<false, false, false>, grid, dim3(threads), 0, st, a);
-    case 1: return launch_pdl(gn_apply_kernel<false, false, true>, grid, dim3(threads), 0, st, a);
-    case 2: return launch_pdl(gn_apply_kernel<false, true, false>, grid, dim3(threads), 0, st, a);
-    case 3: return launch_pdl(gn_apply_kernel<false, true, true>, grid, dim3(threads), 0, st, a);
-    case 4: return launch_pdl(gn_apply_kernel<true, false, false>, grid, dim3(threads), 0, st, a);
-    case 5: return launch_pdl(gn_apply_kernel<true, false, true>, grid, dim3(threads), 0, st, a);
-    case 6: return launch_pdl(gn_apply_kernel<true, true, false>, grid, dim3(threads), 0, st, a);
-    default: return launch_pdl(gn_apply_kernel<true, true, true>, grid, dim3(threads), 0, st, a);
-  }
 }
 
 // ----------------------------------------------------------------------------
@@ -1500,66 +1224,6 @@ topk_merge_kernel(const float* __restrict__ gathered, int world, long long pack,
       const float* rec = gathered + (long long)r * pack + kk + 2 * B * k;
       out_sim[(long long)b * N + n] = rec[(long long)b * (hi - lo) + j];
     }
-  }
-}
-
-// ----------------------------------------------------------------------------
-// SIMT implicit-GEMM convolution: a slow, obviously-correct CUDA-core twin of the
-// wgmma kernel (same packed weights, same segment semantics).  Debug / bring-up
-// only (NOPE_CONV_IMPL=simt); never the default path.
-// mode 0: 3x3 pad 1; mode 1: 1x1; mode 2: pixel-unshuffle(2) + 1x1 (input is 2H x 2W);
-// mode 3: parity-folded nearest-x2 upsample + 3x3 (input is H/2 x W/2, weights [4*Cout][4*Cin]).
-// ----------------------------------------------------------------------------
-struct SimtConvArgs {
-  const __half* src0;
-  const __half* src1;
-  int C0, C1;
-  const __half* w;   // [Cout][K]
-  const float* bias;
-  __half* out;
-  int n_img, H, W, Cout, K, mode;
-};
-
-__global__ void conv_simt_kernel(const SimtConvArgs a) {
-  const long long total = (long long)a.n_img * a.H * a.W * a.Cout;
-  const int Ccat = a.C0 + a.C1;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int o = (int)(i % a.Cout);
-    const int px = (int)((i / a.Cout) % a.W);
-    const int py = (int)((i / ((long long)a.Cout * a.W)) % a.H);
-    const int b = (int)(i / ((long long)a.Cout * a.W * a.H));
-    const int par = a.mode == 3 ? ((py & 1) * 2 + (px & 1)) : 0;
-    const __half* wr = a.w + ((long long)par * a.Cout + o) * a.K;
-    float acc = a.bias ? a.bias[o] : 0.f;
-    const int taps = a.mode == 0 ? 9 : (a.mode == 1 ? 1 : 4);
-    for (int t = 0; t < taps; ++t) {
-      int yy, xx, Hs = a.H, Ws = a.W;
-      if (a.mode == 0) { yy = py + t / 3 - 1; xx = px + t % 3 - 1; }
-      else if (a.mode == 1) { yy = py; xx = px; }
-      else if (a.mode == 2) { Hs = 2 * a.H; Ws = 2 * a.W; yy = 2 * py + t / 2; xx = 2 * px + t % 2; }
-      else { Hs = a.H / 2; Ws = a.W / 2; yy = (py >> 1) + t / 2 - 1 + (py & 1); xx = (px >> 1) + t % 2 - 1 + (px & 1); }
-      if (yy < 0 || yy >= Hs || xx < 0 || xx >= Ws) continue;
-      const long long pix = ((long long)b * Hs + yy) * Ws + xx;
-      const __half* s0 = a.src0 + pix * a.C0;
-      const __half* wk = wr + t * Ccat;
-      for (int c = 0; c < a.C0; c += 2) {
-        const float2 x = __half22float2(*reinterpret_cast<const __half2*>(s0 + c));
-        const float2 y = __half22float2(*reinterpret_cast<const __half2*>(wk + c));
-        acc = fmaf(x.x, y.x, acc);
-        acc = fmaf(x.y, y.y, acc);
-      }
-      if (a.src1) {
-        const __half* s1 = a.src1 + pix * a.C1;
-        for (int c = 0; c < a.C1; c += 2) {
-          const float2 x = __half22float2(*reinterpret_cast<const __half2*>(s1 + c));
-          const float2 y = __half22float2(*reinterpret_cast<const __half2*>(wk + a.C0 + c));
-          acc = fmaf(x.x, y.x, acc);
-          acc = fmaf(x.y, y.y, acc);
-        }
-      }
-    }
-    a.out[i] = __float2half_rn(acc);
   }
 }
 

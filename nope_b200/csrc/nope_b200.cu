@@ -3,10 +3,12 @@
 // The engine owns the repacked UNet weights, a per-chunk activation workspace and the
 // layer schedule of UNet.forward (reference:
 // src/model/u_net/denoising_diffusion_pytorch/u_net.py:160-198), batched over all pose
-// hypotheses of a chunk.  Host code is plain C++; kernels live in conv_tc.cuh / kernels.cuh.
+// hypotheses of a chunk.  Host code is plain C++; kernels live in conv_tc2.cuh (convolution, with
+// conv_tc.cuh) / kernels.cuh.
 #include "../../include/nope_b200.h"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -96,8 +98,6 @@ struct nope_unet {
   int dim = 0, Cl = 0, S0 = 0, rot_dim = 6, cemb = 0, device = 0, num_sms = 132;
   int dims[5] = {0, 0, 0, 0, 0};
   bool finalized = false;
-  int conv_impl = 2;   // 0: wgmma single-CTA kernel, 1: SIMT debug twin, 2: clustered wgmma kernel (default)
-  bool fuse_gn = true; // GroupNorm / SiLU / pose bias / residual in the conv epilogue (conv_impl 2 only)
   // 0: fp16 operands; 1: exact weights (W_hi + W_lo K-segments, 2x the MMA work); 2: split precision
   // (exact weights + activations carried as hi + lo: A_hi W_hi + A_hi W_lo + A_lo W_hi, 3x);
   // 3: bf16 operands and activations (8-bit mantissa: its own, looser tolerance)
@@ -126,12 +126,10 @@ struct nope_unet {
   bool ws_external = false;
   bool ws_fresh = false;            // counters not zeroed yet
   Act sk[4][2];
-  Act TA, TB, TC, TD, XA, XB, RB;
+  Act TB, TC, TD, XA, XB, RB;
   __half *cs = nullptr, *pb = nullptr;
   Act x0, g1;                       // per-reference pre-stage
-  __half* pt = nullptr;
-  float2* gn_partial = nullptr;   // gn_stats_kernel output (per-op test path only)
-  float2 *SA = nullptr, *SB = nullptr;   // unfused statistics: conv epilogue / gn_apply emit; SB also fused emit
+  float2* SB = nullptr;           // GroupNorm(1) partial sums a fused epilogue emits for the next pre-norm
   uint2* xpart = nullptr;         // fused GroupNorm: cross-tile partial sums, {value, epoch} words
   size_t xpart_words = 0;
   unsigned gn_epoch = 0;          // tag of the last fused launch that exchanged partial sums
@@ -157,12 +155,11 @@ struct nope_unet {
     if (ws_base && !ws_external) cudaFree(ws_base);
     for (cudaEvent_t e : prof_ev) cudaEventDestroy(e);
   }
-  bool fused() const { return fuse_gn && conv_impl == 2; }
-  bool split() const { return (precision == 2 || precision == 4) && fused(); }
+  bool split() const { return precision == 2 || precision == 4; }
   // precision 4: the residual stream, skip tensors and resampled maps keep their (hi, lo) pair, the tensor INSIDE a
   // ResnetBlock (block1's output h, consumed only by block2's convolution) is a single fp16 value -- block2 runs two
   // products per tap instead of three.  CPU budget (tools/precision_sim.py): h alone costs 4.3e-4 on the embeddings.
-  bool h_lo() const { return precision == 2 && fused(); }
+  bool h_lo() const { return precision == 2; }
   bool bf() const { return precision == 3; }     // bf16 storage (BASELINE configs[2]); fp16 otherwise
 
   // ------------------------------------------------------------------ schema
@@ -351,8 +348,6 @@ struct nope_unet {
     return mem.upload(&L.pre_w1, w1) || mem.upload(&L.pre_wb, wb) ? -1 : 0;
   }
   int make_linattn(const std::string& p) {
-    if (make_norm(p + ".prenorm", p + ".fn.norm", 1)) return -1;
-    if (make_conv(p + ".qkv", p + ".fn.fn.to_qkv.weight", "", 1)) return -1;
     if (make_qkv_folded(p + ".qkvf", p + ".fn.fn.to_qkv.weight", p + ".fn.norm")) return -1;
     if (make_conv(p + ".out", p + ".fn.fn.to_out.0.weight", p + ".fn.fn.to_out.0.bias", 1)) return -1;
     if (make_norm(p + ".outnorm", p + ".fn.fn.to_out.1", 1)) return -1;
@@ -393,8 +388,6 @@ struct nope_unet {
 
   // packs the staged weights (engine_finalize: every schema key is present, device selected)
   int finalize() {
-    NOPE_CHECK(precision == 0 || conv_impl != 1, "the SIMT debug convolution only runs fp16 weights");
-    NOPE_CHECK(precision < 2 || fused(), "split precision / bf16 need the fused schedule on the CTA-pair kernel");
     if (upload_f32("pose_mlp.0.weight", &pose_w) || upload_f32("pose_mlp.0.bias", &pose_b) ||
         upload_f32("init_conv.weight", &init_w) || upload_f32("init_conv.bias", &init_b) ||
         upload_f32("final_conv.1.weight", &final_w) || upload_f32("final_conv.1.bias", &final_b))
@@ -409,8 +402,6 @@ struct nope_unet {
       }
     }
     if (make_resblock("mid_block1") || make_resblock("mid_block2")) return -1;
-    if (make_norm("mid_attn.prenorm", "mid_attn.fn.norm", 1)) return -1;
-    if (make_conv("mid_attn.qkv", "mid_attn.fn.fn.to_qkv.weight", "", 1)) return -1;
     if (make_qkv_folded("mid_attn.qkvf", "mid_attn.fn.fn.to_qkv.weight", "mid_attn.fn.norm")) return -1;
     if (make_conv("mid_attn.out", "mid_attn.fn.fn.to_out.weight", "mid_attn.fn.fn.to_out.bias", 1))
       return -1;
@@ -428,7 +419,8 @@ struct nope_unet {
   }
 
   // ------------------------------------------------------------------ workspace
-  // One slab carved by a bump allocator: ~6 MB per hypothesis (12 MB in the split-precision mode).
+  // One slab carved by a bump allocator: ~4.7 MB per hypothesis at u_net_dim 192 (8.6 MB in the split-precision
+  // modes), nearly all of it the 8 skip tensors, 3 temporaries of 786 KB and 3 feature maps of 393 KB.
   // layout(b) assigns every buffer for capacities (c hypotheses, r references).
   void take_act(Bump& b, Act* a, size_t n, int C, bool with_lo) {
     if (b.base) {
@@ -449,7 +441,6 @@ struct nope_unet {
       const int s = S0 >> i;
       for (int k = 0; k < 2; ++k) take_act(b, &sk[i][k], c * s * s * dims[i], dims[i], lo);
     }
-    take_act(b, &TA, c * big, 0, false);
     take_act(b, &TB, c * big, 0, lo);
     take_act(b, &TC, c * big, 0, lo);
     take_act(b, &TD, c * big, 0, false);
@@ -460,11 +451,8 @@ struct nope_unet {
     b.take(&pb, c * (size_t)P);
     take_act(b, &x0, r * xsz, dim, lo);
     take_act(b, &g1, r * xsz, dim, lo);
-    b.take(&pt, r * xsz);
     const size_t m = std::max(c, r);
-    b.take(&gn_partial, m * 8 * 8);
     b.take(&ref_of, m);
-    b.take(&SA, m * ((size_t)S0 * S0 * dim / 256));   // (hw/32) x (C/8) at the top level
     b.take(&SB, m * 8);
     // <= 64 (slot, image, group) entries of two {value, epoch} words per image
     if (b.base) xpart_words = (m + 8) * 64 * 2;
@@ -541,28 +529,13 @@ struct nope_unet {
   // ------------------------------------------------------------------ op launchers
   // out[n_img, So, So, cout] = conv(L, in0 (++ in1)).  The K loop walks, per filter tap and source
   // tensor, up to three products: A_hi W_hi, A_hi W_lo (precision >= 1), A_lo W_hi (sources that
-  // carry a remainder).  `gs` selects the fused GroupNorm epilogue; `stats` the unfused partial sums.
+  // carry a remainder).  `gs` selects the fused GroupNorm epilogue; `stats` (plain epilogue only) receives the
+  // GroupNorm partial sums of the output in the ConvParams::stats layout (nope_op_conv_gn checks them).
   int conv(const ConvLayer& L, const Act& in0, const Act& in1, const Act& out, int So, int n_img, int cap_img,
-           cudaStream_t st, float2* stats = nullptr, const GnSpec* gs = nullptr) {
+           cudaStream_t st, const GnSpec* gs = nullptr, float2* stats = nullptr) {
     const int c0 = in0.C, c1 = in1.hi ? in1.C : 0;
     NOPE_CHECK(c0 + c1 == L.cin, "conv: channel mismatch");
     ++launches;
-    if (conv_impl == 1) {
-      NOPE_CHECK(!gs && L.Kp == L.K, "the SIMT debug convolution has no fused epilogue / split weights");
-      SimtConvArgs a;
-      a.src0 = in0.hi; a.src1 = in1.hi; a.C0 = c0; a.C1 = c1; a.w = L.w; a.bias = L.bias; a.out = out.hi;
-      a.n_img = n_img; a.H = So; a.W = So; a.Cout = L.cout; a.K = L.K; a.mode = L.mode;
-      conv_simt_kernel<<<ew_grid((long long)n_img * So * So * L.cout, 256, 132 * 32), 256, 0, st>>>(a);
-      NOPE_CUDA(cudaGetLastError());
-      if (stats) {
-        // the SIMT twin has no fused statistics: produce them in the conv-epilogue format
-        // (parts = max(1, hw/32), noct = C/8) with a plain reduction kernel
-        const int hw = So * So;
-        stats_ref_kernel<<<dim3(hw < 32 ? 1 : hw / 32, n_img), 256, 0, st>>>(out.hi, stats, hw, L.cout);
-        NOPE_CUDA(cudaGetLastError());
-      }
-      return 0;
-    }
     TileGeom g;
     if (make_geom(So, So, &g)) return -1;
     ConvParams p;
@@ -665,7 +638,7 @@ struct nope_unet {
     p.b_cnt = g.b_cnt;
     NOPE_CHECK(!(stats && L.mode == 3), "fused statistics are not available on the upsample conv");
     if (gs) {
-      NOPE_CHECK(conv_impl == 2 && L.mode != 3 && !stats, "fused GroupNorm epilogue: CTA-pair kernel, no upsample");
+      NOPE_CHECK(L.mode != 3 && !stats, "fused GroupNorm epilogue: no upsample, no plain statistics");
       GnFuse& f = p.gn;
       const int hw = So * So;
       f.G = gs->norm ? gs->norm->G : 0;
@@ -731,8 +704,7 @@ struct nope_unet {
       p.out_lo = out.lo;                // extras epilogue writes the remainder
     }
     auto launch = [&]() {
-      if (gs) return launch_conv_gn(p, L.bn, num_sms, st);
-      return conv_impl == 2 ? launch_conv_tc2(p, L.bn, num_sms, st) : launch_conv_tc(p, L.bn, num_sms, st);
+      return gs ? launch_conv_gn(p, L.bn, num_sms, st) : launch_conv_tc2(p, L.bn, num_sms, st);
     };
     if (!profile) return launch();
     cudaEvent_t e0, e1;
@@ -753,54 +725,6 @@ struct nope_unet {
   std::vector<double> prof_alg;     // algorithmic (fp16-mode) FLOPs of the same launches
   std::vector<int4> prof_shape;     // (GEMM resolution, mode 0 3x3 / 1 1x1 / 2 unshuffle / 3 folded upsample, Cout, K)
 
-  // pixel slabs per image for the GroupNorm kernels: as few as keep >= ~4 CTAs per SM in
-  // flight (every CTA pays a fixed statistics prologue), at most 8, and >= 32 pixels each
-  static int gn_nslab(int hw, int n_img) {
-    int ns = 1;
-    while (ns < 8 && hw / (ns * 2) >= 32 && (long long)n_img * ns < 600) ns *= 2;
-    return ns;
-  }
-
-  // y = [silu](GN(x)) + pb[:, off:off+C] + res.  Statistics come from `stats`
-  // ([img][st_parts][st_noct], see GnApplyArgs); stats == nullptr with N != nullptr runs the
-  // stand-alone gn_stats_kernel first (per-op test path).  `emit` (optional) receives the
-  // per-(img, slab) sums of y for a following GroupNorm(1, C).
-  int gn(const NormLayer* N, const __half* x, __half* y, int S, int C, int n_img, bool silu,
-         int pb_offset, const __half* res, const int* res_map, cudaStream_t st,
-         const float2* stats = nullptr, int st_parts = 0, int st_noct = 0, float2* emit = nullptr) {
-    const int hw = S * S;
-    const int nslab = gn_nslab(hw, n_img);
-    const int threads = (C / 8) * gn_rows(C);
-    NOPE_CHECK(threads <= 1024 && threads % 32 == 0 && threads >= 256 && C % 8 == 0,
-               "gn: unsupported channel count");
-    if (N) {
-      NOPE_CHECK(N->C == C, "gn: channel mismatch");
-      if (!stats) {
-        gn_stats_kernel<<<dim3(nslab, n_img), threads, threads * sizeof(float2), st>>>(
-            x, gn_partial, hw, C, N->G, nslab);
-        NOPE_CUDA(cudaGetLastError());
-        ++launches;
-        stats = gn_partial;
-        st_parts = nslab;
-        st_noct = N->G;
-      }
-      NOPE_CHECK(st_noct % N->G == 0, "gn: statistics granularity does not match the groups");
-    }
-    GnApplyArgs a;
-    a.x = x; a.y = y; a.stats = N ? stats : nullptr; a.st_parts = st_parts; a.st_noct = st_noct;
-    a.gamma = N ? N->gamma : nullptr; a.beta = N ? N->beta : nullptr;
-    a.pb = pb_offset >= 0 ? pb : nullptr; a.pb_stride = P; a.pb_off = pb_offset >= 0 ? pb_offset : 0;
-    a.res = res; a.res_of = res_map; a.emit = emit; a.emit_parts = emit_parts_of(hw);
-    a.hw = hw; a.C = C; a.G = N ? N->G : 1; a.nslab = nslab;
-    a.silu = silu ? 1 : 0; a.eps = 1e-5f; a.bf16 = bf() ? 1 : 0;
-    NOPE_CUDA(launch_gn_apply(a, dim3(nslab, n_img), threads, st));
-    ++launches;
-    return 0;
-  }
-  static int st_parts_of(int S) { return S * S < 32 ? 1 : S * S / 32; }
-  // fixed number of sub-slabs per image for statistics emitted by gn_apply (<= 8, >= 32 pixels
-  // each): independent of the number of images, so results do not depend on chunk / shard size
-  static int emit_parts_of(int hw) { return hw >= 256 ? 8 : (hw >= 32 ? hw / 32 : 1); }
   // partial sums per image emitted by the fused epilogue: one per (M-tile of the image, N-tile)
   static int fused_emit_parts(int S, int C) {
     return std::max(1, S * S / kBM) * (C / pick_bn(C));
@@ -816,81 +740,54 @@ struct nope_unet {
     return 0;
   }
 
-  // ResnetBlock.forward (model_utils.py:271-279) on NHWC fp16.
-  // Fused schedule: conv1 [GN8 + SiLU + pose bias] -> h ; (res_conv) ; conv2 [GN8 + SiLU + residual] -> out:
+  // ResnetBlock.forward (model_utils.py:271-279) on NHWC fp16:
+  // conv1 [GN8 + SiLU + pose bias] -> h ; (res_conv) ; conv2 [GN8 + SiLU + residual] -> out:
   // two or three launches, no tensor is written un-normalised.  `emit_g1` makes conv2's epilogue also
   // emit the GroupNorm(1, C) statistics of the block output into SB for a following attention pre-norm.
-  // Unfused schedule (conv_impl 0 / 1 or fuse_gn off): GroupNorm statistics ride on the conv epilogues
-  // (SA) and gn_apply_kernel normalises in a separate pass.
   int resblock(const std::string& p, const Act& in0, const Act& in1, const Act& out, int S, int n, bool pose,
                cudaStream_t st, bool emit_g1 = false, int res_div = 0, int res_base = 0, const Act* hoisted_h = nullptr) {
     const ConvLayer& b1 = convs.at(p + ".block1");
     const ConvLayer& b2 = convs.at(p + ".block2");
     const int co = b1.cout;
-    const int parts = st_parts_of(S);
     auto it = convs.find(p + ".res");
-    if (fused()) {
-      Act h(TB.hi, co, h_lo() ? TB.lo : nullptr);
-      if (hoisted_h) {
-        h = *hoisted_h;
-        if (!h_lo()) h.lo = nullptr;
-      } else {
-        GnSpec s1;
-        s1.norm = &norms.at(p + ".norm1");
-        s1.silu = true;
-        s1.pb_offset = pose ? pb_off.at(p) : -1;
-        if (conv(b1, in0, in1, h, S, n, cap, st, nullptr, &s1)) return -1;
-      }
-      GnSpec s2;
-      s2.norm = &norms.at(p + ".norm2");
-      s2.silu = true;
-      if (it != convs.end()) {
-        Act r(TC.hi, co, split() ? TC.lo : nullptr);
-        // plain epilogue: routing this 1x1 through the GroupNorm-fused role split measured 8 % slower
-        if (conv(it->second, in0, in1, r, S, n, cap, st)) return -1;
-        s2.res = r;
-      } else {
-        NOPE_CHECK(in1.hi == nullptr && in0.C == co, "resblock: identity residual needs Cin == Cout");
-        s2.res = in0;
-        s2.res_div = res_div;
-        s2.res_base = res_base;
-      }
-      s2.emit = emit_g1 ? SB : nullptr;
-      return conv(b2, h, Act(), out, S, n, cap, st, nullptr, &s2);
+    Act h(TB.hi, co, h_lo() ? TB.lo : nullptr);
+    if (hoisted_h) {
+      h = *hoisted_h;
+      if (!h_lo()) h.lo = nullptr;
+    } else {
+      GnSpec s1;
+      s1.norm = &norms.at(p + ".norm1");
+      s1.silu = true;
+      s1.pb_offset = pose ? pb_off.at(p) : -1;
+      if (conv(b1, in0, in1, h, S, n, cap, st, &s1)) return -1;
     }
-    NOPE_CHECK(!hoisted_h && res_div == 0, "resblock: hoisting arguments belong to the fused schedule");
-    if (conv(b1, in0, in1, Act(TA.hi, co), S, n, cap, st, SA)) return -1;
-    if (gn(&norms.at(p + ".norm1"), TA.hi, TB.hi, S, co, n, true, pose ? pb_off.at(p) : -1, nullptr, nullptr, st,
-           SA, parts, co / 8))
-      return -1;
-    if (conv(b2, Act(TB.hi, co), Act(), Act(TA.hi, co), S, n, cap, st, SA)) return -1;
-    const __half* res = in0.hi;
+    GnSpec s2;
+    s2.norm = &norms.at(p + ".norm2");
+    s2.silu = true;
     if (it != convs.end()) {
-      if (conv(it->second, in0, in1, Act(TC.hi, co), S, n, cap, st)) return -1;
-      res = TC.hi;
+      Act r(TC.hi, co, split() ? TC.lo : nullptr);
+      // plain epilogue: routing this 1x1 through the GroupNorm-fused role split measured 8 % slower
+      if (conv(it->second, in0, in1, r, S, n, cap, st)) return -1;
+      s2.res = r;
     } else {
       NOPE_CHECK(in1.hi == nullptr && in0.C == co, "resblock: identity residual needs Cin == Cout");
+      s2.res = in0;
+      s2.res_div = res_div;
+      s2.res_base = res_base;
     }
-    return gn(&norms.at(p + ".norm2"), TA.hi, out.hi, S, co, n, true, -1, res, nullptr, st, SA, parts, co / 8,
-              emit_g1 ? SB : nullptr);
+    s2.emit = emit_g1 ? SB : nullptr;
+    return conv(b2, h, Act(), out, S, n, cap, st, &s2);
   }
 
   // Residual(PreNorm(LinearAttention)) (model_utils.py:393-418).  x's GroupNorm(1) statistics
   // were emitted into SB by the producer of x; to_out[1] (GroupNorm(1)) + the residual add run in the
-  // to_out convolution's epilogue (fused) or come from its epilogue statistics (unfused).
+  // to_out convolution's epilogue.
   int linattn(const std::string& p, const Act& x, const Act& out, int C, int S, int n, cudaStream_t st) {
-    const int eparts = fused() ? fused_emit_parts(S, C) : emit_parts_of(S * S);
-    if (fused()) {
-      // pre-norm folded into to_qkv: x is read once, un-normalised, by the 1x1 itself
-      GnSpec s;
-      s.pre_stats = SB;
-      s.pre_parts = eparts;
-      if (conv(convs.at(p + ".qkvf"), x, Act(), Act(TD.hi, 3 * kHeadsHidden), S, n, cap, st, nullptr, &s)) return -1;
-    } else {
-      if (gn(&norms.at(p + ".prenorm"), x.hi, TB.hi, S, C, n, false, -1, nullptr, nullptr, st, SB, eparts, 1))
-        return -1;
-      if (conv(convs.at(p + ".qkv"), Act(TB.hi, C), Act(), Act(TD.hi, 3 * kHeadsHidden), S, n, cap, st)) return -1;
-    }
+    // pre-norm folded into to_qkv: x is read once, un-normalised, by the 1x1 itself
+    GnSpec sq;
+    sq.pre_stats = SB;
+    sq.pre_parts = fused_emit_parts(S, C);
+    if (conv(convs.at(p + ".qkvf"), x, Act(), Act(TD.hi, 3 * kHeadsHidden), S, n, cap, st, &sq)) return -1;
     if (attn_impl == 0 && S * S >= kBM) {
       if (launch_linattn_tc(TD.hi, TC.hi, n, S * S, num_sms, st, bf())) return -1;
     } else {
@@ -901,40 +798,24 @@ struct nope_unet {
     // this takes the same time as the plain convolution plus one normalisation pass (18.80 vs 18.71 ms over the step
     // under ncu; the lock-step epilogue measured slower: 319 vs 244 us at 32x32), and it never rounds the
     // un-normalised output to 16 bits (full-size configs[2] scores: 0.99e-3 vs 1.06e-3)
-    if (fused()) {
-      GnSpec s;
-      s.norm = &norms.at(p + ".outnorm");
-      s.res = x;
-      return conv(convs.at(p + ".out"), Act(TC.hi, kHeadsHidden), Act(), out, S, n, cap, st, nullptr, &s);
-    }
-    if (conv(convs.at(p + ".out"), Act(TC.hi, kHeadsHidden), Act(), Act(TA.hi, C), S, n, cap, st, SA)) return -1;
-    return gn(&norms.at(p + ".outnorm"), TA.hi, out.hi, S, C, n, false, -1, x.hi, nullptr, st, SA, st_parts_of(S),
-              C / 8);
+    GnSpec so;
+    so.norm = &norms.at(p + ".outnorm");
+    so.res = x;
+    return conv(convs.at(p + ".out"), Act(TC.hi, kHeadsHidden), Act(), out, S, n, cap, st, &so);
   }
 
   // Residual(PreNorm(Attention)) (model_utils.py:367-390)
   int midattn(const Act& x, const Act& out, int C, int S, int n, cudaStream_t st) {
     NOPE_CHECK(S * S <= 32, "bottleneck attention supports at most 32 tokens");
-    const int eparts = fused() ? fused_emit_parts(S, C) : emit_parts_of(S * S);
-    if (fused()) {
-      GnSpec s;
-      s.pre_stats = SB;
-      s.pre_parts = eparts;
-      if (conv(convs.at("mid_attn.qkvf"), x, Act(), Act(TD.hi, 3 * kHeadsHidden), S, n, cap, st, nullptr, &s)) return -1;
-    } else {
-      if (gn(&norms.at("mid_attn.prenorm"), x.hi, TB.hi, S, C, n, false, -1, nullptr, nullptr, st, SB, eparts, 1))
-        return -1;
-      if (conv(convs.at("mid_attn.qkv"), Act(TB.hi, C), Act(), Act(TD.hi, 3 * kHeadsHidden), S, n, cap, st)) return -1;
-    }
+    GnSpec sq;
+    sq.pre_stats = SB;
+    sq.pre_parts = fused_emit_parts(S, C);
+    if (conv(convs.at("mid_attn.qkvf"), x, Act(), Act(TD.hi, 3 * kHeadsHidden), S, n, cap, st, &sq)) return -1;
     NOPE_CUDA(launch_pdl(midattn_kernel, dim3(n), dim3(128), 0, st, TD.hi, TC.hi, S * S, bf()));
     ++launches;
-    if (fused()) {
-      GnSpec s;                // no normalisation: out = to_out(attn) + x
-      s.res = x;
-      return conv(convs.at("mid_attn.out"), Act(TC.hi, kHeadsHidden), Act(), out, S, n, cap, st, nullptr, &s);
-    }
-    if (conv(convs.at("mid_attn.out"), Act(TC.hi, kHeadsHidden), Act(), Act(TA.hi, C), S, n, cap, st)) return -1;
-    return gn(nullptr, TA.hi, out.hi, S, C, n, false, -1, x.hi, nullptr, st);
+    GnSpec so;                 // no normalisation: out = to_out(attn) + x
+    so.res = x;
+    return conv(convs.at("mid_attn.out"), Act(TC.hi, kHeadsHidden), Act(), out, S, n, cap, st, &so);
   }
 
   // pose-independent prefix, once per reference image: x0 = init_conv(ref),
@@ -945,16 +826,11 @@ struct nope_unet {
     NOPE_CUDA(cudaGetLastError());
     ++launches;
     const Act xin(x0.hi, dim, split() ? x0.lo : nullptr);
-    if (fused()) {
-      GnSpec s;
-      s.norm = &norms.at("downs.0.0.norm1");
-      s.silu = true;
-      return conv(convs.at("downs.0.0.block1"), xin, Act(), Act(g1.hi, dim, h_lo() ? g1.lo : nullptr), S0, B,
-                  cap_ref, st, nullptr, &s);
-    }
-    if (conv(convs.at("downs.0.0.block1"), xin, Act(), Act(pt, dim), S0, B, cap_ref, st, SA)) return -1;
-    return gn(&norms.at("downs.0.0.norm1"), pt, g1.hi, S0, dim, B, true, -1, nullptr, nullptr, st, SA,
-              st_parts_of(S0), dim / 8);
+    GnSpec s;
+    s.norm = &norms.at("downs.0.0.norm1");
+    s.silu = true;
+    return conv(convs.at("downs.0.0.block1"), xin, Act(), Act(g1.hi, dim, h_lo() ? g1.lo : nullptr), S0, B,
+                cap_ref, st, &s);
   }
 
   // UNet.forward for hypotheses [hyp0, hyp0 + n) of the flattened (b, pose) list
@@ -990,15 +866,8 @@ struct nope_unet {
       const Act s0 = A(sk[i][0], C), s1 = A(sk[i][1], C);
       if (i == 0) {
         // block 0 with its block1 half hoisted: TB already holds SiLU(GN(conv(x0))) + pose bias
-        if (fused()) {
-          const Act h = A(TB, C);
-          if (resblock(p + ".0", A(x0, C), Act(), s0, S, n, true, st, false, N, hyp0, &h)) return -1;
-        } else {
-          if (conv(convs.at(p + ".0.block2"), Act(TB.hi, C), Act(), Act(TA.hi, C), S, n, cap, st, SA)) return -1;
-          if (gn(&norms.at(p + ".0.norm2"), TA.hi, s0.hi, S, C, n, true, -1, x0.hi, ref_of, st, SA,
-                 st_parts_of(S), C / 8))
-            return -1;
-        }
+        const Act h = A(TB, C);
+        if (resblock(p + ".0", A(x0, C), Act(), s0, S, n, true, st, false, N, hyp0, &h)) return -1;
       } else {
         if (resblock(p + ".0", cur, Act(), s0, S, n, true, st)) return -1;
       }
@@ -1149,21 +1018,13 @@ int nope_unet_set_chunk(nope_unet_t* u, int hyps) {
   return 0;
 }
 int nope_unet_set_conv_impl(nope_unet_t* u, int impl) {
-  NOPE_CHECK(u && impl >= 0 && impl <= 2, "impl must be 0 (tensor cores), 1 (simt) or 2 (tensor cores, clustered)");
-  NOPE_CHECK(impl != 1 || u->precision == 0, "the SIMT debug convolution only runs fp16 weights");
-  u->conv_impl = impl;
+  NOPE_CHECK(u && impl == 2, "conv_impl must be 2 (tensor cores, clustered: conv_tc2_kernel)");
   return 0;
 }
 int nope_unet_set_option(nope_unet_t* u, const char* name, int value) {
   NOPE_CHECK(u && name, "null argument");
-  if (std::strcmp(name, "fuse_gn") == 0) {
-    NOPE_CHECK(value != 0 || u->precision < 2, "split precision / bf16 need the fused GroupNorm epilogue");
-    u->fuse_gn = value != 0;
-    return 0;
-  }
   if (std::strcmp(name, "precision") == 0) {
     NOPE_CHECK(!u->finalized, "precision must be set before nope_unet_finalize");
-    NOPE_CHECK(value == 0 || u->conv_impl != 1, "the SIMT debug convolution only runs fp16 weights");
     NOPE_CHECK(value >= 0 && value <= 4, "precision must be 0 (fp16), 1 (exact weights), 2 (split), 3 (bf16) or 4 (split, fp16 inside ResnetBlocks)");
     u->precision = value;
     return 0;
@@ -1178,9 +1039,8 @@ int nope_unet_set_option(nope_unet_t* u, const char* name, int value) {
 }
 int nope_unet_get_option(const nope_unet_t* u, const char* name, int* value) {
   NOPE_CHECK(u && name && value, "null argument");
-  if (std::strcmp(name, "fuse_gn") == 0) { *value = u->fuse_gn ? 1 : 0; return 0; }
   if (std::strcmp(name, "precision") == 0) { *value = u->precision; return 0; }
-  if (std::strcmp(name, "conv_impl") == 0) { *value = u->conv_impl; return 0; }
+  if (std::strcmp(name, "conv_impl") == 0) { *value = 2; return 0; }
   if (std::strcmp(name, "attn_impl") == 0) { *value = u->attn_impl; return 0; }
   return fail(std::string("unknown option: ") + name);
 }
@@ -1836,6 +1696,7 @@ int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, i
                  const float* weight, const float* bias, float* out, int n_img, int H, int W,
                  int Cout, void* stream) {
   NOPE_CHECK(x0 && weight && out, "null argument");
+  NOPE_CHECK(impl == 2, "impl must be 2 (tensor cores, clustered: conv_tc2_kernel)");
   NOPE_CHECK(mode >= 0 && mode <= 3, "mode must be 0..3");
   NOPE_CHECK(H == W, "square images only");
   NOPE_CHECK(C0 % 64 == 0 && C1 % 64 == 0 && Cout % 64 == 0, "channels must be multiples of 64");
@@ -1861,7 +1722,6 @@ int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, i
                                                                            cin * taps, 0);
   NOPE_CUDA(cudaGetLastError());
   nope_unet eng;  // only used for its conv launcher / map cache
-  eng.conv_impl = impl;
   cudaDeviceProp prop;
   int dev = 0;
   NOPE_CUDA(cudaGetDevice(&dev));
@@ -1875,8 +1735,7 @@ int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, i
     NOPE_CUDA(cudaMemcpyAsync(dbias, bias, Cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
   L.bias = dbias;
-  if (impl != 1 && (make_weight_map(&L.wmap, wp, rows, L.K, L.bn)))
-    return -1;
+  if (make_weight_map(&L.wmap, wp, rows, L.K, L.bn)) return -1;
   if (eng.conv(L, Act(a0, C0), x1 ? Act(a1, C1) : Act(), Act(o, Cout), H, n_img, n_img, st)) return -1;
   if (to_nchw(o, out, n_img, Cout, H * W, st)) return -1;
   NOPE_CUDA(cudaStreamSynchronize(st));
@@ -1887,24 +1746,27 @@ int nope_op_conv_gn(int impl, int mode, const float* x0, int C0, const float* x1
                     const float* weight, const float* bias, const float* gamma, const float* beta,
                     int G, int silu, float* out, int n_img, int H, int W, int Cout, void* stream) {
   NOPE_CHECK(x0 && weight && gamma && beta && out, "null argument");
+  NOPE_CHECK(impl == 2, "impl must be 2 (tensor cores, clustered: conv_tc2_kernel)");
   NOPE_CHECK(mode >= 0 && mode <= 2 && H == W, "bad mode / non-square image");
   NOPE_CHECK(C0 % 64 == 0 && C1 % 64 == 0 && Cout % 64 == 0, "channels must be multiples of 64");
+  NOPE_CHECK(G >= 1 && (Cout / 8) % G == 0, "groups must divide the 8-channel octets");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   Scratch s;
   const int taps = mode == 0 ? 9 : (mode == 1 ? 1 : 4);
   const int cin = C0 + (x1 ? C1 : 0);
   const int Hin = mode == 2 ? 2 * H : H;
-  __half *a0 = nullptr, *a1 = nullptr, *wp = nullptr, *o = nullptr, *y = nullptr;
+  const int hw = H * W, parts = hw < 32 ? 1 : hw / 32, noct = Cout / 8;
+  __half *a0 = nullptr, *a1 = nullptr, *wp = nullptr, *o = nullptr;
+  float2* stats = nullptr;
   if (to_nhwc(x0, &a0, s, n_img, C0, Hin * Hin, st)) return -1;
   if (x1 && to_nhwc(x1, &a1, s, n_img, C1, Hin * Hin, st)) return -1;
-  if (s.get(&wp, (size_t)Cout * cin * taps) || s.get(&o, (size_t)n_img * H * W * Cout) ||
-      s.get(&y, (size_t)n_img * H * W * Cout))
+  if (s.get(&wp, (size_t)Cout * cin * taps) || s.get(&o, (size_t)n_img * hw * Cout) ||
+      s.get(&stats, (size_t)n_img * parts * noct))
     return -1;
   pack_weight_kernel<<<ew_grid((long long)Cout * cin * taps), 256, 0, st>>>(weight, wp, Cout, cin, taps,
                                                                             cin * taps, 0);
   NOPE_CUDA(cudaGetLastError());
   nope_unet eng;
-  eng.conv_impl = impl;
   cudaDeviceProp prop;
   int dev = 0;
   NOPE_CUDA(cudaGetDevice(&dev));
@@ -1913,20 +1775,40 @@ int nope_op_conv_gn(int impl, int mode, const float* x0, int C0, const float* x1
   ConvLayer L;
   L.mode = mode; L.cin = cin; L.cout = Cout; L.K = cin * taps; L.Kp = L.K; L.bn = pick_bn(Cout); L.w = wp;
   L.bias = const_cast<float*>(bias);
-  if (impl != 1 && (make_weight_map(&L.wmap, wp, Cout, L.K, L.bn)))
+  if (make_weight_map(&L.wmap, wp, Cout, L.K, L.bn)) return -1;
+  if (eng.conv(L, Act(a0, C0), x1 ? Act(a1, C1) : Act(), Act(o, Cout), H, n_img, n_img, st, nullptr, stats))
     return -1;
-  const int parts = nope_unet::st_parts_of(H);
-  float2* stats = nullptr;
-  if (s.get(&stats, (size_t)n_img * parts * (Cout / 8))) return -1;
-  if (eng.conv(L, Act(a0, C0), x1 ? Act(a1, C1) : Act(), Act(o, Cout), H, n_img, n_img, st, stats)) return -1;
-  NormLayer N;
-  N.C = Cout; N.G = G;
-  N.gamma = const_cast<float*>(gamma);
-  N.beta = const_cast<float*>(beta);
-  if (eng.gn(&N, o, y, H, Cout, n_img, silu != 0, -1, nullptr, nullptr, st, stats, parts, Cout / 8))
-    return -1;
-  if (to_nchw(y, out, n_img, Cout, H * W, st)) return -1;
+  // GroupNorm on the host, in double, from the epilogue's [img][parts][octet] partial sums alone: a group's sum and
+  // sum of squares are the totals of its octets over all parts (the layout the LDM engine normalises from)
+  std::vector<__half> ho((size_t)n_img * hw * Cout);
+  std::vector<float2> hs((size_t)n_img * parts * noct);
+  std::vector<float> hg(Cout), hb(Cout), y((size_t)n_img * Cout * hw);
   NOPE_CUDA(cudaStreamSynchronize(st));
+  NOPE_CUDA(cudaMemcpy(ho.data(), o, ho.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+  NOPE_CUDA(cudaMemcpy(hs.data(), stats, hs.size() * sizeof(float2), cudaMemcpyDeviceToHost));
+  NOPE_CUDA(cudaMemcpy(hg.data(), gamma, Cout * sizeof(float), cudaMemcpyDeviceToHost));
+  NOPE_CUDA(cudaMemcpy(hb.data(), beta, Cout * sizeof(float), cudaMemcpyDeviceToHost));
+  const int opg = noct / G, cpg = Cout / G;
+  const double cnt = (double)hw * cpg;
+  for (int i = 0; i < n_img; ++i)
+    for (int g = 0; g < G; ++g) {
+      double sum = 0.0, sq = 0.0;
+      for (int part = 0; part < parts; ++part)
+        for (int oc = g * opg; oc < (g + 1) * opg; ++oc) {
+          const float2 t = hs[((size_t)i * parts + part) * noct + oc];
+          sum += t.x;
+          sq += t.y;
+        }
+      const double mean = sum / cnt;
+      const double rstd = 1.0 / std::sqrt(std::max(sq / cnt - mean * mean, 0.0) + 1e-5);
+      for (int c = g * cpg; c < (g + 1) * cpg; ++c)
+        for (int px = 0; px < hw; ++px) {
+          double v = ((double)__half2float(ho[((size_t)i * hw + px) * Cout + c]) - mean) * rstd * hg[c] + hb[c];
+          if (silu) v /= 1.0 + std::exp(-v);
+          y[((size_t)i * Cout + c) * hw + px] = (float)v;
+        }
+    }
+  NOPE_CUDA(cudaMemcpy(out, y.data(), y.size() * sizeof(float), cudaMemcpyHostToDevice));
   return 0;
 }
 
@@ -1963,7 +1845,6 @@ int nope_op_conv_gn_fused(int mode, int precision, const float* x0, int C0, cons
                                                                     precision >= 1 ? K : 0);
   NOPE_CUDA(cudaGetLastError());
   nope_unet eng;
-  eng.conv_impl = 2;
   eng.precision = precision;
   cudaDeviceProp prop;
   int dev = 0;
@@ -1997,7 +1878,7 @@ int nope_op_conv_gn_fused(int mode, int precision, const float* x0, int C0, cons
     gs.emit = em;
   }
   if (eng.conv(L, Act(a0, C0, a0l), x1 ? Act(a1, C1, a1l) : Act(), Act(o, Cout, ol), H, n_img,
-               n_img, st, nullptr, &gs))
+               n_img, st, &gs))
     return -1;
   if (to_nchw(o, out, n_img, Cout, hw, st, ol)) return -1;
   if (emit_out) {
@@ -2013,32 +1894,6 @@ int nope_op_conv_gn_fused(int mode, int precision, const float* x0, int C0, cons
       }
     NOPE_CUDA(cudaMemcpy(emit_out, sums.data(), sums.size() * sizeof(float), cudaMemcpyHostToDevice));
   }
-  NOPE_CUDA(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int nope_op_groupnorm(const float* x, const float* gamma, const float* beta, int G, int silu,
-                      const float* chan_bias, const float* residual, float* out, int n_img, int C,
-                      int H, int W, void* stream) {
-  NOPE_CHECK(x && gamma && beta && out && H == W, "bad argument");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  Scratch s;
-  const int hw = H * W;
-  __half *a = nullptr, *r = nullptr, *o = nullptr, *pbh = nullptr;
-  if (to_nhwc(x, &a, s, n_img, C, hw, st)) return -1;
-  if (residual && to_nhwc(residual, &r, s, n_img, C, hw, st)) return -1;
-  if (chan_bias && to_nhwc(chan_bias, &pbh, s, n_img, C, 1, st)) return -1;
-  if (s.get(&o, (size_t)n_img * C * hw)) return -1;
-  nope_unet eng;
-  if (s.get(&eng.gn_partial, (size_t)n_img * 64)) return -1;
-  NormLayer N;
-  N.C = C; N.G = G;
-  N.gamma = const_cast<float*>(gamma);
-  N.beta = const_cast<float*>(beta);
-  eng.pb = pbh;
-  eng.P = C;
-  if (eng.gn(&N, a, o, H, C, n_img, silu != 0, chan_bias ? 0 : -1, r, nullptr, st)) return -1;
-  if (to_nchw(o, out, n_img, C, hw, st)) return -1;
   NOPE_CUDA(cudaStreamSynchronize(st));
   return 0;
 }

@@ -7,7 +7,7 @@ import torch
 
 from . import _lib
 
-_IMPL = {"tcgen05": 0, "simt": 1, "tcgen05_2cta": 2}
+_IMPL = {"tcgen05_2cta": 2}
 
 
 def _stream(dev):
@@ -18,7 +18,7 @@ def _f32(t):
     return None if t is None else t.to(torch.float32).contiguous()
 
 
-def conv(x0, weight, bias=None, x1=None, mode="3x3", impl="tcgen05"):
+def conv(x0, weight, bias=None, x1=None, mode="3x3", impl="tcgen05_2cta"):
     """mode '3x3' (pad 1), '1x1', 'unshuffle' (pixel-unshuffle(2) + 1x1; weight
     [Cout, 4*Cin, 1, 1]) or 'upsample3x3' (nearest x2 + conv3x3, folded into four 2x2 parity
     kernels; x0 is the low-resolution input).  x1 is concatenated after x0 along channels."""
@@ -36,8 +36,8 @@ def conv(x0, weight, bias=None, x1=None, mode="3x3", impl="tcgen05"):
     return out
 
 
-def conv_gn(x0, weight, bias, gamma, beta, groups, silu=True, x1=None, mode="3x3", impl="tcgen05"):
-    """[SiLU](GroupNorm(conv(x))) with statistics from the conv epilogue (the sweep's path)."""
+def conv_gn(x0, weight, bias, gamma, beta, groups, silu=True, x1=None, mode="3x3", impl="tcgen05_2cta"):
+    """[SiLU](GroupNorm(conv(x))), normalised on the host from the partial sums of the plain conv epilogue."""
     lib = _lib.load()
     m = {"3x3": 0, "1x1": 1, "unshuffle": 2}[mode]
     x0, x1, weight, bias, gamma, beta = map(_f32, (x0, x1, weight, bias, gamma, beta))
@@ -75,19 +75,6 @@ def conv_gn_fused(x0, weight, bias, gamma=None, beta=None, groups=8, silu=True, 
             _lib.ptr(chan_bias), _lib.ptr(residual), res_div, _lib.ptr(out), _lib.ptr(emit), n, h, w, cout,
             _stream(x0.device)))
     return (out, emit) if want_emit else out
-
-
-def groupnorm(x, gamma, beta, groups, silu=False, chan_bias=None, residual=None):
-    lib = _lib.load()
-    x, gamma, beta = _f32(x), _f32(gamma), _f32(beta)
-    chan_bias, residual = _f32(chan_bias), _f32(residual)
-    n, c, h, w = x.shape
-    out = torch.empty_like(x)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.nope_op_groupnorm(_lib.ptr(x), _lib.ptr(gamma), _lib.ptr(beta), groups,
-                                         1 if silu else 0, _lib.ptr(chan_bias), _lib.ptr(residual),
-                                         _lib.ptr(out), n, c, h, w, _stream(x.device)))
-    return out
 
 
 def linear_attention(qkv, impl="simt"):

@@ -185,7 +185,8 @@ class UNet:
             _lib.check(_lib.load().nope_unet_set_chunk(self._h, hyps))
 
     def set_option(self, name, value):
-        """'fuse_gn' (1: GroupNorm/SiLU/pose bias/residual in the conv epilogue, default)."""
+        """Named engine option (include/nope_b200.h, nope_unet_set_option): 'attn_impl' (0: LinearAttention
+        on tensor cores, 1: CUDA cores) or 'conv_impl' (2, the only one).  Unknown names raise NopeError."""
         self._options[name] = int(value)
         if self._h is not None:
             _lib.check(_lib.load().nope_unet_set_option(self._h, name.encode(), int(value)))
@@ -197,10 +198,10 @@ class UNet:
         _lib.check(_lib.load().nope_unet_set_metric(self._handle(), _METRICS[metric], float(threshold)))
 
     def set_conv_impl(self, impl):
-        """'tcgen05_2cta' (clustered kernel with the fused epilogues, default), 'tcgen05' (single-CTA
-        wgmma kernel) or 'simt' (debug twin); the names are kept from the first version of the engine."""
-        _lib.check(_lib.load().nope_unet_set_conv_impl(
-            self._handle(), {"tcgen05": 0, "simt": 1, "tcgen05_2cta": 2}[impl]))
+        """'tcgen05_2cta': the clustered kernel with the fused epilogues, the engine's only convolution."""
+        if impl != "tcgen05_2cta":
+            raise _lib.NopeError(f"unknown conv impl {impl!r}: the only convolution is 'tcgen05_2cta' (conv_tc2_kernel)")
+        _lib.check(_lib.load().nope_unet_set_conv_impl(self._handle(), 2))
 
     @property
     def last_launch_count(self):

@@ -293,6 +293,26 @@ def test_bad_arguments_raise(gpu_model):
     rf = torch.zeros(1, 8, 32, 32)
     with pytest.raises(NopeError):
         gpu_model.u_net.sweep(rf, torch.zeros(1, 3, 6), query_feat=rf, k=5)   # k > N
+    # on an engine before finalize, where every option it has is accepted: convolutions other than the
+    # clustered kernel and the fuse_gn option do not exist
+    import ctypes as C
+    from nope_b200 import _lib
+    from nope_b200.encoder import FeatureExtractor
+    from nope_b200.unet import UNet
+    fresh = UNet(u_net_dim=192, rot_representation_dim=6, encoder=FeatureExtractor(descriptor_size=8),
+                 device="cuda:0")
+    h = fresh._handle()
+    for impl in ("tcgen05", "simt"):
+        with pytest.raises(NopeError):
+            fresh.set_conv_impl(impl)
+    with pytest.raises(NopeError):
+        _lib.check(_lib.load().nope_unet_set_conv_impl(h, 0))
+    with pytest.raises(NopeError):
+        fresh.set_option("fuse_gn", 0)
+    fresh.set_conv_impl("tcgen05_2cta")
+    v = C.c_int()
+    _lib.check(_lib.load().nope_unet_get_option(h, b"conv_impl", C.byref(v)))
+    assert v.value == 2
 
 
 def test_full_size_grid_properties(gpu_model):

@@ -1,7 +1,7 @@
 #!/bin/bash
 # One parameterised GPU script (replaces the round-1 gpu_*.sh collection).  Run under gpurun:
 #   gpurun --timeout 900 -- 'bash tools/gpu.sh <step> [<step> ...]'
-# steps: fused | unet | tests | ldmtests | time | bench | benchall | launches | ncu_conv | ncu_mem | smoke | sanitize
+# steps: fused | unet | tests | ldmtests | bench | benchall | launches | ncu_conv | ncu_mem | smoke | sanitize
 # Logs land in gpurun_out/ (merged back by gpurun, < 64 MiB).
 cd "${GRAFT_REPO_ROOT:-/root/repo}"
 mkdir -p gpurun_out
@@ -15,7 +15,6 @@ case "$step" in
   tests)    rm -f gpurun_out/parity_log.jsonl; run "pytest -m gpu" 2400 python -m pytest tests -m gpu -q -rA --tb=short > gpurun_out/pytest_gpu.log 2>&1; tail -8 gpurun_out/pytest_gpu.log ;;
   dflt)     rm -f gpurun_out/parity_log.jsonl; run "pytest -m gpu (default path)" 2400 python -m pytest tests -m gpu -q --tb=short --ignore=tests/test_ldm_gpu.py > gpurun_out/pytest_dflt.log 2>&1; tail -25 gpurun_out/pytest_dflt.log ;;
   ldmtests) run "ldm tests" 1500 python -m pytest tests/test_ldm_gpu.py -m gpu -q --tb=short > gpurun_out/t_ldm.log 2>&1; tail -5 gpurun_out/t_ldm.log ;;
-  time)     rm -f gpurun_out/prof_dump.csv; NOPE_PROF_DUMP=gpurun_out/prof_dump.csv run "time_sweep" 900 python tools/time_sweep.py ${TIME_SPECS:-fp16 fp16:fuse_gn=0} --profile > gpurun_out/time_sweep.log 2>&1; cat gpurun_out/time_sweep.log ;;
   epi)      for d in ${EPI_LIST:-3 4 3 4}; do echo "NOPE_GN_EPI=$d"; NOPE_GN_EPI=$d timeout 600 python tools/time_sweep.py ${TIME_SPECS:-fp16} --steps 20 2>&1 | tail -1 | cut -c1-200; done > gpurun_out/epi_ab.log 2>&1; cat gpurun_out/epi_ab.log
             for d in 3 4; do NOPE_GN_EPI=$d NOPE_PROF_DUMP=gpurun_out/prof_dump_epi$d.csv timeout 600 python tools/time_sweep.py fp16 --profile > /dev/null 2>&1; done ;;
   pdl)      for d in ${PDL_LIST:-0 1 3 0 1 3 0 1 3}; do echo "NOPE_PDL=$d"; NOPE_PDL=$d timeout 600 python tools/time_sweep.py fp16 --steps 20 2>&1 | tail -1 | cut -c1-120; done > gpurun_out/pdl_ab.log 2>&1; cat gpurun_out/pdl_ab.log ;;

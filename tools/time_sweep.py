@@ -1,6 +1,6 @@
 """Time the resident sweep (latents + poses in HBM, CUDA events on the current stream) for one or
 several engine configurations in ONE process, e.g.
-    python tools/time_sweep.py fp16 fp16:fuse_gn=0 parity fp16_w2 --poses 642 --queries 1
+    python tools/time_sweep.py fp16 fp16:attn_impl=1 parity fp16_w2 --poses 642 --queries 1
 Each spec is precision[:option=value,...].  Prints one JSON line per spec (hyp/s, ms, parity vs the
 first spec's scores) -- a development aid, not the bench."""
 import argparse
