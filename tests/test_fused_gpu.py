@@ -4,12 +4,18 @@ PreNorm / to_out of LinearAttention, model_utils.py:230, 393-418) -- one layer a
 C ABI against torch fp32.  Covers every tile geometry of the UNet: images spanning 8 / 2 M-tiles
 (statistics exchanged between CTAs), 2 / 8 images per tile, groups spanning several N-tiles
 (GroupNorm(1) at 384..1536 channels), odd image counts (phantom peer tiles), the hoisted-prefix
-residual mapping, and the three precision modes."""
+residual mapping, and the three precision modes.
+
+The kernel is persistent (tile pairs cluster, cluster + clusters, ...).  The first CASES run one tile
+per CTA; MANY_TILES run at least three per CTA (asserted from the shape: n = 53 / 41 / 197 / 401 at
+sides 32 / 16 / 8 / 4), which reaches what only runs from a CTA's second tile on: the channel-parameter
+cache, the double-buffered staging, the next tile's residual / pose-bias prefetch and several GroupNorm
+sync groups per launch.  Errors are the worst rel-L2 over (image, N-tile) blocks, against float64."""
 import pytest
 import torch
 import torch.nn.functional as F
 
-from _util import h, log, max_rel, rel_l2
+from _util import h, log, max_rel, min_many_tile_pairs, pair_tiles, pick_bn, rounds, worst_block_rel_l2
 
 pytestmark = pytest.mark.gpu
 
@@ -43,6 +49,24 @@ CASES = [
     ("1x1", 3, 128, 0, 512, 4, 1, False, False, True, 0),     # 128-wide tiles, group over 4 N-tiles
     ("unshuffle", 3, 64, 0, 128, 16, 8, True, False, False, 0),
 ]
+MANY_TILES = [
+    # >= 3 tiles per CTA on 132 SMs (asserted from the shape).  Each pass-2 variant of the role-split epilogue
+    # (conv_gn2_math_warps) runs with and without emit, which selects a different variant: the first launch of
+    # the test emits, the second does not and must reproduce it bit for bit.  Shapes with several N-tiles have
+    # 4, 5 or 8 of them, counts that do not divide the 66 clusters: CTAs change N-tile between their tiles.
+    ("3x3", 53, 64, 0, 192, 32, 8, True, True, False, 0),      # Block 1, table path: pose bias
+    ("3x3", 53, 64, 0, 192, 32, 8, True, False, True, 0),      # Block 2, table path: residual
+    ("3x3", 197, 128, 0, 768, 8, 8, True, True, False, 0),     # Block 1, 2 images per tile, phantom peer
+    ("3x3", 197, 128, 0, 768, 8, 8, True, False, True, 0),     # Block 2, 2 images per tile, phantom peer
+    ("3x3", 41, 64, 64, 640, 16, 10, True, True, True, 0),     # generic: two sources, pose bias + residual, 5 N-tiles
+    ("3x3", 54, 64, 0, 192, 32, 8, True, False, True, 3),      # residual of the hoisted prefix
+    ("1x1", 41, 128, 0, 640, 16, 1, False, False, True, 0),    # GroupNorm(1) over 5 N-tiles x 2 M-tiles
+    ("1x1", 401, 128, 0, 1536, 4, 1, False, False, True, 0),   # GroupNorm(1) over 8 N-tiles, ragged
+    ("3x3", 53, 64, 0, 128, 32, 8, True, True, True, 0),       # 128-wide tiles
+    ("3x3", 53, 64, 0, 64, 32, 8, True, True, True, 0),        # 64-wide tiles
+    ("unshuffle", 41, 64, 0, 640, 16, 10, True, False, False, 0),
+]
+CASES = CASES + MANY_TILES
 
 
 def _reference(mode, x0, x1, w, b, gamma, beta, G, silu, cb, rs, res_div):
@@ -60,7 +84,8 @@ def _reference(mode, x0, x1, w, b, gamma, beta, G, silu, cb, rs, res_div):
     if cb is not None:
         y = y + cb[:, :, None, None]
     if rs is not None:
-        idx = torch.arange(y.shape[0]) // res_div if res_div > 0 else torch.arange(y.shape[0])
+        idx = torch.arange(y.shape[0], device=y.device)
+        idx = idx // res_div if res_div > 0 else idx
         y = y + rs[idx]
     return y
 
@@ -70,8 +95,11 @@ def _reference(mode, x0, x1, w, b, gamma, beta, G, silu, cb, rs, res_div):
 def test_conv_gn_fused(dev, case, precision):
     from nope_b200 import ops
     mode, n, C0, C1, Cout, S, G, silu, pb, res, res_div = case
-    if precision == 1 and n > 3 and S == 32:
+    if precision == 1 and 3 < n < 50 and S == 32:
         pytest.skip("exact-weights mode covered by the smaller cases")
+    pairs = pair_tiles(n, S, S, Cout, pick_bn(Cout))
+    if case in MANY_TILES:
+        assert pairs >= min_many_tile_pairs(dev), (case, pairs, "fewer than three tiles per CTA")
     g = torch.Generator().manual_seed(CASES.index(case) * 7 + 1)
     Sin = 2 * S if mode == "unshuffle" else S
     k = 3 if mode == "3x3" else 1
@@ -88,20 +116,21 @@ def test_conv_gn_fused(dev, case, precision):
     cb = h(torch.randn(n, Cout, generator=g)) if pb else None
     n_res = (n + res_div - 1) // res_div if res_div > 0 else n
     rs = r16(torch.randn(n_res, Cout, S, S, generator=g)) if res else None
-    ref = _reference(mode, x0.double(), None if x1 is None else x1.double(), w.double(), b.double(), gamma.double(),
-                     beta.double(), G, silu, None if cb is None else cb.double(), None if rs is None else rs.double(),
-                     res_div)
+    d64 = lambda t: None if t is None else t.to(dev, torch.float64)
+    ref = _reference(mode, d64(x0), d64(x1), d64(w), d64(b), d64(gamma), d64(beta), G, silu, d64(cb), d64(rs), res_div)
     D = lambda t: None if t is None else t.to(dev)
     out, emit = ops.conv_gn_fused(D(x0), D(w), D(b), D(gamma), D(beta), groups=G, silu=silu, x1=D(x1), mode=mode,
                                   precision=precision, chan_bias=D(cb), residual=D(rs), res_div=res_div,
                                   want_emit=True)
-    e, m = rel_l2(out, ref), max_rel(out, ref)
+    (e, blk), m = worst_block_rel_l2(out, ref, pick_bn(Cout)), max_rel(out, ref)
     # emitted GroupNorm(1) statistics = sums over the stored (fp16 hi) output
     o16 = out.cpu() if precision != 2 else out.cpu().half().float()
     es = torch.stack([o16.flatten(1).sum(1), (o16 ** 2).flatten(1).sum(1)], 1)
     e_emit = max_rel(emit, es)
-    log("conv_gn_fused", case=list(case), precision=precision, rel_l2=e, max_rel=m, emit_rel=e_emit)
-    assert e < TOL[precision], (case, precision, e)
+    log("conv_gn_fused", case=list(case), precision=precision, pair_tiles=pairs, rounds=rounds(pairs, dev),
+        n_tiles=Cout // pick_bn(Cout), worst_block_rel_l2=e,
+        worst_block=blk, max_rel=m, emit_rel=e_emit)
+    assert e < TOL[precision], (case, precision, "worst (image, N-tile)", blk, e)
     assert e_emit < 2e-3
     # bitwise reproducible, whatever the arrival order of the tiles
     out2 = ops.conv_gn_fused(D(x0), D(w), D(b), D(gamma), D(beta), groups=G, silu=silu, x1=D(x1), mode=mode,
@@ -114,16 +143,27 @@ def test_fused_result_independent_of_batch_composition(dev):
     CTA assignment, arrival order): slices of a batch reproduce the full batch bit for bit."""
     from nope_b200 import ops
     g = torch.Generator().manual_seed(5)
-    for S, C in [(32, 192), (16, 384), (8, 768), (4, 1536)]:
-        n = 13
+    # n = 13: one tile per CTA; the larger n: >= 3 tiles per CTA, so slices start in the first, a middle and the
+    # last round of the full launch
+    for S, C, n, G in [(32, 192, 13, 8), (16, 384, 13, 8), (8, 768, 13, 8), (4, 1536, 13, 8),
+                       (32, 192, 53, 8), (16, 640, 41, 10), (8, 768, 197, 8), (4, 1536, 401, 8)]:
+        if n > 13:
+            assert pair_tiles(n, S, S, C, pick_bn(C)) >= min_many_tile_pairs(dev), (S, C, n)
         x = h(torch.randn(n, C, S, S, generator=g))
         w = h(torch.randn(C, C, 3, 3, generator=g) / (9 * C) ** 0.5)
         b = 0.1 * torch.randn(C, generator=g)
         gamma, beta = 1 + 0.2 * torch.randn(C, generator=g), 0.2 * torch.randn(C, generator=g)
         cb = h(torch.randn(n, C, generator=g))
         D = lambda t: t.to(dev)
-        full = ops.conv_gn_fused(D(x), D(w), D(b), D(gamma), D(beta), groups=8, silu=True, chan_bias=D(cb), residual=D(x))
-        for lo, hi in [(0, 1), (3, 8), (12, 13), (5, 13)]:
-            part = ops.conv_gn_fused(D(x[lo:hi]), D(w), D(b), D(gamma), D(beta), groups=8, silu=True,
-                                     chan_bias=D(cb[lo:hi]), residual=D(x[lo:hi]))
-            assert torch.equal(part, full[lo:hi]), (S, C, lo, hi)
+        run = lambda lo, hi: ops.conv_gn_fused(D(x[lo:hi]), D(w), D(b), D(gamma), D(beta), groups=G, silu=True,
+                                               chan_bias=D(cb[lo:hi]), residual=D(x[lo:hi]))
+        full = run(0, n)
+        assert torch.equal(run(0, n), full), (S, C, n, "second launch")
+        slices = [(0, 1), (3, 8), (12, 13), (5, 13)] if n == 13 else \
+            [(0, 1), (n // 3, 2 * n // 3), (n - 1, n), ((n // 2) | 1, n)]
+        for lo, hi in slices:
+            part = run(lo, hi)
+            if not torch.equal(part, full[lo:hi]):
+                diff = (part != full[lo:hi]).flatten(1).any(1).nonzero().flatten() + lo
+                raise AssertionError(f"S={S} C={C} n={n}: slice [{lo}, {hi}) differs from the full batch in "
+                                     f"images {diff.tolist()[:8]}")

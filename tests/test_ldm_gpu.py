@@ -244,3 +244,149 @@ def test_rejects_bad_input(ldm_model):
             fresh.set_option(name, 1)
     with pytest.raises(_lib.NopeError):
         _lib.check(_lib.load().nope_ldm_set_impl(fresh._handle(), 0, 0))
+
+
+# ---------------------------------------------------------------- production batch sizes
+# One module per (kind, resolution, one- or two-source) group that the network has, at a batch that gives the
+# module's narrowest convolution (256-wide tiles) at least three tiles per CTA: the persistent kernel's
+# second-and-later-tile paths.  At 8x8 two images share a tile and n = 197 leaves the last pair with a phantom peer.
+# (module, kind, n, side of the GEMM, narrowest Cout, parities)
+MANY_TILE_MODULES = [
+    ("input_blocks.1.0", "res", 50, 32, 256, 1),            # identity skip
+    ("input_blocks.5.0", "res", 100, 16, 512, 1),
+    ("input_blocks.8.0", "res", 197, 8, 1024, 1),
+    ("input_blocks.4.0", "res", 100, 16, 512, 1),           # 1x1 skip (the 32x32 one has two sources)
+    ("input_blocks.7.0", "res", 197, 8, 1024, 1),
+    ("output_blocks.8.0", "res", 50, 32, 256, 1),           # two sources, 1x1 skip
+    ("output_blocks.3.0", "res", 100, 16, 512, 1),
+    ("output_blocks.0.0", "res", 197, 8, 1024, 1),
+    ("input_blocks.1.1", "st", 50, 32, 256, 1),
+    ("input_blocks.4.1", "st", 100, 16, 512, 1),
+    ("input_blocks.7.1", "st", 197, 8, 1024, 1),
+    ("input_blocks.3.0.op", "resample", 200, 16, 256, 1),   # stride-2 3x3, 32 -> 16
+    ("input_blocks.6.0.op", "resample", 397, 8, 512, 1),    # stride-2 3x3, 16 -> 8: odd m-tile count
+    ("output_blocks.2.2.conv", "resample", 49, 8, 1024, 4), # folded nearest-x2 + 3x3, 8 -> 16: odd m-tile count
+    ("output_blocks.5.2.conv", "resample", 25, 16, 512, 4), # folded nearest-x2 + 3x3, 16 -> 32
+]
+W2_MODULES = ("input_blocks.1.0", "input_blocks.4.0", "input_blocks.7.1")   # also run in precision="fp16_w2"
+REF_SLICE = 8       # images per float64 oracle evaluation: its attention materialises [b, heads, tok, tok]
+
+
+@pytest.fixture(scope="module")
+def grid642(golden_dir):
+    return torch.from_numpy(np.load(f"{golden_dir}/level2_642_b1.npz")["all_relativeR"])
+
+
+def _oracle_module(sd, name, kind, x0, x1, poses):
+    """the oracle's own module functions, on whatever dtype / device sd and the inputs have"""
+    import torch.nn.functional as F
+    from oracle import ldm_oracle
+    if kind == "res":
+        return ldm_oracle.res_block(x0 if x1 is None else torch.cat([x0, x1], 1), sd, name)
+    if kind == "st":
+        ctx = (poses @ sd["pose_mlp.0.weight"].t() + sd["pose_mlp.0.bias"])[:, None, :]
+        return ldm_oracle.spatial_transformer(x0, ctx, sd, name)
+    w, b = sd[name + ".weight"], sd[name + ".bias"]
+    if name.endswith(".op"):
+        return F.conv2d(x0, w, b, stride=2, padding=1)
+    return F.conv2d(F.interpolate(x0, scale_factor=2, mode="nearest"), w, b, padding=1)
+
+
+def _like_tap(tap, n, gen):
+    """seeded input with the per-channel mean and spread of an oracle tap"""
+    m, s = tap.mean((0, 2, 3)), tap.std((0, 2, 3))
+    return torch.randn((n,) + tuple(tap.shape[1:]), generator=gen) * s[:, None, None] + m[:, None, None]
+
+
+@pytest.mark.parametrize("mod", MANY_TILE_MODULES, ids=lambda m: m[0])
+def test_module_many_tiles(ldm_model, ldm_model_w2, ldm_sd, oracle_taps, grid642, mod):
+    """run_block at production batch sizes against the oracle in float64 on the GPU: the worst per-image rel-L2,
+    and slices of the batch (first, middle, last, odd start) equal the full run bit for bit"""
+    from _util import min_many_tile_pairs, pair_tiles, rounds, worst_block_rel_l2
+    name, kind, n, side, cout, n_par = mod
+    pairs = pair_tiles(n, side, side, cout, 256, n_par)
+    assert pairs >= min_many_tile_pairs(0), (name, n, pairs)
+    spec = next(m for m in _modules() if m[0] == name)
+    (in0, in1), out_tap = spec[2], spec[3]
+    want = oracle_taps[out_tap]
+    gen = torch.Generator().manual_seed(n + len(name))
+    x0 = _like_tap(oracle_taps[in0], n, gen)
+    x1 = _like_tap(oracle_taps[in1], n, gen) if in1 else None
+    poses = grid642[0, :n] if kind == "st" else None
+    dev = torch.device("cuda:0")
+    d64 = lambda t: None if t is None else t.to(dev, torch.float64)
+    sd = {k: d64(v) for k, v in ldm_sd.items() if k.startswith(name + ".") or k.startswith("pose_mlp.")}
+    with torch.no_grad():
+        ref = torch.cat([_oracle_module(sd, name, kind, d64(x0[i:i + REF_SLICE]),
+                                        None if x1 is None else d64(x1[i:i + REF_SLICE]),
+                                        None if poses is None else d64(poses[i:i + REF_SLICE]))
+                         for i in range(0, n, REF_SLICE)])
+    models = [("fp16", ldm_model)] + ([("fp16_w2", ldm_model_w2)] if name in W2_MODULES else [])
+    for prec, m in models:
+        run = lambda lo, hi: m.run_block(name, x0[lo:hi], None if x1 is None else x1[lo:hi],
+                                         poses=None if poses is None else poses[lo:hi],
+                                         out_channels=want.shape[1], out_side=ref.shape[2])
+        got = run(0, n)
+        e, img = worst_block_rel_l2(got, ref)
+        log("ldm_module_many_tiles", module=name, precision=prec, n=n, pair_tiles=pairs, rounds=rounds(pairs, 0),
+            worst_image_rel_l2=e,
+            worst_image=img)
+        assert e < BLOCK_TOL, (name, prec, "worst image", img, e)
+        for lo, hi in [(0, REF_SLICE), (n // 3, 2 * n // 3), (n - 1, n), ((n // 2) | 1, n)]:
+            part = run(lo, hi)
+            assert torch.equal(part, got[lo:hi]), (name, prec, lo, hi)
+
+
+SWEEP_HYPS = (0, 255, 256, 511, 512, 641)     # first / last of each 256-chunk of the 642 poses
+
+
+@pytest.fixture(scope="module")
+def ldm_model_256(ldm_sd):
+    if not torch.cuda.is_available():
+        pytest.skip("no CUDA device")
+    from nope_b200.ldm import UNetModelPose
+    return UNetModelPose(device="cuda:0", chunk=256).load_state_dict(ldm_sd)
+
+
+def test_sweep_chunk256_bitwise_and_vs_oracle(ldm_model_256, ldm_sd, grid642):
+    """The 642 poses of level2_642 at chunk 256 (chunks of 256 + 256 + 130), Q = 4 queries: (a) the same call twice,
+    (b) chunks of 7 and 642 and (d) chosen hypotheses swept alone all give the same bits; those hypotheses are within
+    EMB_TOL_FP16 / SIM_TOL of the oracle's forward in float64.  (c), four one-query sweeps equal to the Q = 4 sweep,
+    is test_multi_query_gpu.test_ldm_multi_query_fused_scores_match_standalone on the same inputs."""
+    from oracle import ldm_oracle
+    from oracle import unet_oracle as orc
+    m = ldm_model_256
+    gen = torch.Generator().manual_seed(4)
+    ref = torch.randn(1, 4, 32, 32, generator=gen)
+    qry = torch.randn(1, 4, 4, 32, 32, generator=gen)
+    poses = grid642
+    base = m.sweep(ref, poses, qry, want_emb=True, k=5)
+    keys = ("emb", "sim", "topv", "topi")
+
+    def same(a, b, what):
+        for k in keys:
+            assert torch.equal(a[k], b[k]), (what, k)
+
+    same(m.sweep(ref, poses, qry, want_emb=True, k=5), base, "second call")                  # (a)
+    try:
+        for chunk in (7, 642):                                                                 # (b)
+            m.set_chunk(chunk)
+            same(m.sweep(ref, poses, qry, want_emb=True, k=5), base, f"chunk {chunk}")
+    finally:
+        m.set_chunk(256)
+    hyps = list(SWEEP_HYPS)
+    for i in hyps:                                                                             # (d)
+        alone = m.sweep(ref, poses[:, i:i + 1], qry, want_emb=True, k=1)
+        assert torch.equal(alone["emb"][0, 0], base["emb"][0, i]), i
+        assert torch.equal(alone["sim"][0, :, 0], base["sim"][0, :, i]), i
+    dev = torch.device("cuda:0")
+    sd = {k: v.to(dev, torch.float64) for k, v in ldm_sd.items()}
+    with torch.no_grad():
+        emb_o = ldm_oracle.ldm_forward(sd, ref.to(dev, torch.float64).expand(len(hyps), -1, -1, -1),
+                                       poses[0, hyps].to(dev, torch.float64))
+        sim_o = torch.stack([orc.l2_similarity(qry[:, q].to(dev, torch.float64), emb_o[None])[0]
+                             for q in range(qry.shape[1])])                                  # [Q, hyps]
+    e_emb = [rel_l2(base["emb"][0, i], emb_o[j]) for j, i in enumerate(hyps)]
+    e_sim = max_rel(base["sim"][0][:, hyps], sim_o)
+    log("ldm_sweep_chunk256", hyps=hyps, emb_rel_l2=e_emb, sim_max_rel=e_sim)
+    assert max(e_emb) < EMB_TOL_FP16 and e_sim < SIM_TOL, (e_emb, e_sim)

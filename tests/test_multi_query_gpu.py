@@ -180,8 +180,8 @@ def test_predict_pose_multi_query_forms(gpu_model, golden_dir):
 
 
 def test_ldm_multi_query_fused_scores_match_standalone(golden_dir):
-    """LDM variant, 642 poses, Q = 4: the fused l2 scores equal a standalone scoring of the templates the
-    same call wrote (two LDM sweeps are not bit-identical, so the comparison stays inside one call)."""
+    """LDM variant, 642 poses at chunk 256, Q = 4: the fused l2 scores equal a standalone scoring of the templates
+    the same call wrote, and each query's scores and top-k equal a one-query sweep of that query bit for bit."""
     from nope_b200.ldm import UNetModelPose
     from nope_b200.model import score_topk
     from nope_b200.synth_weights import make_ldm_state_dict
@@ -199,6 +199,12 @@ def test_ldm_multi_query_fused_scores_match_standalone(golden_dir):
     log("ldm_multi_query", vs_standalone=e)
     assert e < 1e-5
     assert torch.equal(out["topi"][0].cpu(), orc.topk_lowest_index(out["sim"][0].cpu(), 5))
+    for q in range(qry.shape[1]):
+        one = m.sweep(ref, poses, qry[:, q], want_emb=True, k=5)
+        assert torch.equal(one["emb"], out["emb"]), q
+        assert torch.equal(one["sim"], out["sim"][:, q]), q
+        assert torch.equal(one["topv"], out["topv"][:, q]), q
+        assert torch.equal(one["topi"], out["topi"][:, q]), q
     # the latent-space predict_pose takes the same forms
     tp = torch.eye(3).expand(642, 3, 3).contiguous()
     R, idx, sim = m.predict_pose(qry[0], ref, poses, tp, k=5)
