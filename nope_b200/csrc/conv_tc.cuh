@@ -40,7 +40,7 @@ struct ConvSeg {
                     // (split precision re-reads the W_hi columns for the A_lo product)
 };
 
-// GroupNorm applied in the epilogue of the producing convolution (clustered kernel, EPI == 4 / 3):
+// GroupNorm applied in the epilogue of the producing convolution (clustered kernel, EPI == 4):
 //   y = [SiLU]((acc - mean) * rstd * gamma + beta) + pose_bias[img, c] + residual[pixel, c]
 // (Block.forward / ResnetBlock.forward, model_utils.py:237-253, 271-279; PreNorm / to_out[1] of
 // LinearAttention, model_utils.py:230, 401).  The statistics of an image are spread over the CTA
@@ -93,8 +93,8 @@ struct ConvParams {
   int n_amaps;
   CUtensorMap bmap;     // weight box of the kernel's tile width (BN rows)
   CUtensorMap omap[4];  // one per output parity class when n_par == 4, else omap[0]
-  CUtensorMap rmap;     // residual tensor (output geometry), EPI == 4 / 3 with gn.has_res
-  GnFuse gn;            // EPI == 4 / 3
+  CUtensorMap rmap;     // residual tensor (output geometry), EPI == 4 with gn.has_res
+  GnFuse gn;            // EPI == 4
   const float* bias;  // [n_total] or nullptr
   // Sub-pixel ("parity") decomposition of nearest-x2-upsample + conv3x3 (HardUpsample,
   // model_utils.py:161-165): n_par == 4 makes n_tile enumerate (parity, channel tile); parity

@@ -15,10 +15,8 @@
 // the output staging.  EPI selects the epilogue at compile time: 0 plain (+ GroupNorm partial
 // sums), 1 extras (ReLU, residual add, (hi, lo) split, fp32 store: template encoder, LDM out conv),
 // 2 GEGLU (conv_tc.cuh), 4 GroupNorm fused (GnFuse, conv_tc.cuh) with the CTA split into math /
-// statistics / store roles (conv_gn2_* below): the default UNet's Block / ResnetBlock / to_qkv /
-// to_out epilogues -- the normalised, activated tensor is the only thing that reaches HBM.  3 is the
-// same epilogue in lock step (all epilogue warps walk through the tile together; kept behind
-// NOPE_GN_EPI=3 as the A/B baseline the role split was measured against).
+// statistics / store roles (conv_gn_* below): the default UNet's Block / ResnetBlock / to_qkv /
+// to_out epilogues -- the normalised, activated tensor is the only thing that reaches HBM.
 //
 // Protocol (per CTA):
 //   full[s]   count 1: the producer's arrive.expect_tx; the stage's TMA loads complete_tx on it
@@ -49,9 +47,9 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// shared-memory map of the EPI == 4 epilogue (conv_gn2_* below), relative to Conv2Smem::kGnOffset
+// shared-memory map of the EPI == 4 epilogue (conv_gn_* below), relative to Conv2Smem::kGnOffset
 template <int BN>
-struct Gn2Smem {
+struct GnSmem {
   static constexpr int kOct = BN / 8;
   static constexpr int kPart = 0;                          // fp32 [8 row segments][kOct][2]
   static constexpr int kMr = kPart + 8 * kOct * 8;         // float2 [2][64]: (mean, rstd) per (image, group) / image
@@ -77,12 +75,8 @@ struct Conv2Smem {
   static constexpr int kOutBufs = BN <= 128 ? 2 : 1;
   static constexpr int kBarOffset = STAGES * kStageBytes + kOutBufs * kOutBytes;
   static constexpr int kBiasOffset = kBarOffset + 256;
-  // EPI == 3 (GroupNorm fused): gamma | beta (fp32 [BN] each) | pose bias (fp16 [8][BN]) |
-  // segment partial sums (fp32 [8][BN/8][2]) | (mean, rstd) [64] | octet -> group table [BN/8] | emit scratch |
-  // gathered cross-CTA partials (fp32 [256])
   static constexpr int kGnOffset = kBiasOffset + BN * 4;
-  static constexpr int kGnBytes = EPI == 3 ? (2 * BN * 4 + 8 * BN * 2 + 8 * (BN / 8) * 8 + 64 * 8 + (BN / 8) * 4 + 32 * 8 + 256 * 4)
-                                            : (EPI == 4 ? Gn2Smem<BN>::kBytes : 0);
+  static constexpr int kGnBytes = EPI == 4 ? GnSmem<BN>::kBytes : 0;
   static constexpr int kTotal = kGnOffset + kGnBytes + 1024;
   static_assert(STAGES * kStageBytes >= kBM * (BN + 4) * 4, "the fp32 accumulator tile must fit in the operand ring");
   static_assert(kTotal <= 227 * 1024, "shared memory per block");
@@ -99,21 +93,27 @@ __device__ __forceinline__ void st_volatile_u2(uint2* p, uint2 v) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// EPI == 3: the whole epilogue loop of a CTA with GroupNorm fused (GnFuse, conv_tc.cuh).
-// Per tile, the 8 epilogue warps
-//   1. start the residual tile's TMA load into the output staging buffer (if any), stage
-//      bias / gamma / beta / pose-bias rows in shared memory;
-//   2. run the mainloop, pull the accumulator tile into registers (+bias) and hand the ring straight
-//      back to the MMA warp -- the mainloop of the next-but-one tile never waits for this epilogue;
-//   3. reduce per-(image, group) sums over the tile (butterfly over pixel rows, fixed order over
-//      row segments and channel octets), publish them and wait for the other tiles of the sync group
-//      (skipped when the tile holds whole images and whole groups);
-//   4. normalise, activate, add pose bias / residual in place in the swizzled staging buffer, TMA-store.
+// EPI == 4: the GroupNorm-fused epilogue (GnFuse, conv_tc.cuh), with the CTA split into roles.  Warps 2 and 3 take
+// the bookkeeping -- the statistics exchange, the table build and the drain of the TMA store -- and talk to the math
+// warps through mbarriers only, so none of it sits on the critical path of the warps that do the arithmetic:
+//
+//   warps 4..   math: wgmma mainloop, accumulator -> registers (+bias), release the ring, per-octet partial sums -> s_part,
+//               arrive part_bar | wait stats_bar[b], res_bar | normalise / SiLU / pose bias / residual in place
+//               in the staging tile | arrive out_bar, tabfree_bar[b].   No block-wide barrier anywhere.
+//   warp 3      statistics: wait part_bar | per-(image, group) sums, publish {value, epoch} words, poll the peer
+//               tiles, fixed-order totals | per-channel scale / shift table (or (mean, rstd) pairs) into buffer
+//               b = tile parity | arrive stats_bar[b].  The pre-norm fold's per-image scalars are independent of
+//               the accumulator, so for those launches this warp runs a tile ahead of the math warps.
+//   warp 2      store: wait out_bar | GroupNorm(1) sums of the stored tile (emit) | TMA store | once the store has
+//               read the staging buffer: TMA load of the NEXT tile's residual into it (or a plain arrive), res_bar.
+//
+// Per-channel parameters (bias, gamma, beta, pose-bias rows) are read through the read-only L1 path rather than
+// staged in shared memory per tile, so no barrier has to publish them.
 // ---------------------------------------------------------------------------------------------
 // read-only shared-memory tables of pass 2: plain (non-volatile, no memory clobber) asm loads, so the
 // compiler may hoist them above the in-place stores to the staging tile (same shared array: it must
 // otherwise assume they alias and serialises every 8-channel octet).  `tok` is produced by a volatile asm
-// after the barrier that publishes the tables, which keeps the loads below that barrier.
+// after the mbarrier waits that publish the tables, which keeps the loads below those waits.
 __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
   float4 r;
   asm("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(addr));
@@ -147,438 +147,7 @@ __device__ __forceinline__ float silu_ftz(float x) {
 __host__ __device__ constexpr int gn_epi_warps(int BN) { return 4 * (BN / 64); }           // one (lane quarter, 64-column sub-tile) each
 __host__ __device__ constexpr int gn_threads(int BN) { return 128 + 32 * gn_epi_warps(BN); }
 
-template <int BN, int STAGES, bool MMA>
-__device__ __forceinline__ void conv_gn_epilogue_loop(const ConvParams& p, uint8_t* smem, uint64_t* full_bar,
-                                                      uint64_t* empty_bar, uint64_t* tempty_bar, uint64_t* res_bar,
-                                                      int tile0, int tile_step, int num_tiles, uint32_t rank) {
-  using S = Conv2Smem<BN, STAGES, 3>;
-  constexpr int kOct = BN / 8;
-  constexpr int kNS = BN / 64;                       // 64-column sub-tiles
-  constexpr int kEpiThreads = 32 * gn_epi_warps(BN);
-  uint8_t* out_stage = smem + STAGES * S::kStageBytes;
-  float* s_bias = reinterpret_cast<float*>(smem + S::kBiasOffset);
-  float* s_gamma = reinterpret_cast<float*>(smem + S::kGnOffset);
-  float* s_beta = s_gamma + BN;
-  __half* s_pb = reinterpret_cast<__half*>(s_beta + BN);                 // [8][BN]
-  float* s_part = reinterpret_cast<float*>(s_pb + 8 * BN);               // [8 segs][kOct][2]
-  float2* s_mr = reinterpret_cast<float2*>(s_part + 8 * kOct * 2);       // [ipt * gpt] (mean, rstd)
-  int* s_og = reinterpret_cast<int*>(s_mr + 64);                         // [kOct] octet -> group in tile
-  float2* s_em = reinterpret_cast<float2*>(s_og + kOct);                 // [4][8] emit scratch
-  float* s_x = reinterpret_cast<float*>(s_em + 32);                      // [expected][npairs][2] gathered partials
-
-  const GnFuse& g = p.gn;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int e = warp - 4, etid = threadIdx.x - 128;
-  const int q = e & 3, cc = e >> 2;                  // row quarter, 64-column sub-tile of this warp
-  const int row = q * 32 + lane;
-  const int hw = p.stats_hw;
-  const bool small = hw < 32;                       // 4x4 images: 16-row segments, two per warp
-  const int it = hw < kBM ? (row >> g.hw_shift) : 0;    // image of this thread's row inside the tile
-  const int npairs = g.ipt * g.gpt;
-  // one image per tile (>= 128-pixel images, always synchronised across tiles): normalisation through
-  // per-channel scale / shift tables, which live behind the single pose-bias row in the s_pb region
-  const bool use_tab = g.G > 0 && g.ipt == 1 && g.expected > 1;
-  float* s_sc = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(s_pb) + 512);
-  float* s_sh = s_sc + BN;
-  static_assert(512 + 2 * BN * 4 <= 8 * BN * 2, "scale / shift tables must fit behind the first pose-bias row");
-  if (etid < kOct) s_og[etid] = (g.G > 0 && g.cpg < BN) ? (etid * 8) / g.cpg : 0;
-#define NOPE_EPI_BAR() asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory")
-
-  int obuf = 0;
-  uint32_t res_phase = 0;
-  int kstage = 0;
-  uint32_t kphase = 0;
-  float* s_acc = reinterpret_cast<float*>(smem);
-  // The residual tile of tile t is TMA-loaded into the staging buffer tile t will be written to (same box /
-  // swizzle as the store).  It is issued by the thread that issues the stores, as soon as the store that
-  // last used the buffer has read it: right after tile t-1's store (or before the loop for the first
-  // tile), so the load latency hides behind tile t's accumulator read-out and tile sync.
-  auto stage_residual = [&](int t, int buf) {
-    if (t >= num_tiles) return;
-    const int mp = t / p.n_tiles;
-    const int nt = t - mp * p.n_tiles;
-    const int mt2 = 2 * mp + (int)rank;
-    if constexpr (S::kOutBufs == 2) tma_store_wait_read1();
-    else tma_store_wait_read0();
-    if (g.has_res && mt2 < p.m_tiles) {
-      int bb, yy;
-      conv_tile_coords(p, mt2, bb, yy);
-      const int rb = g.res_div > 0 ? (g.res_base + bb) / g.res_div : bb;
-      uint8_t* dst = out_stage + buf * S::kOutBytes;
-      mbar_expect_tx(res_bar, S::kOutBytes);
-#pragma unroll 1
-      for (int c2 = 0; c2 < kNS; ++c2)
-        tma_load_4d(dst + c2 * (kBM * 128), &p.rmap, res_bar, nt * BN + c2 * 64, 0, yy, rb);
-    }
-  };
-  if (etid == 0) stage_residual(tile0, 0);
-  // pose-bias rows of the NEXT tile are fetched into a register while the current tile is normalised
-  uint4 pb_next = make_uint4(0, 0, 0, 0);
-  auto fetch_pb = [&](int t) {
-    if (!g.pb || t >= num_tiles || etid >= g.ipt * kOct) return;
-    const int mp = t / p.n_tiles;
-    const int nt = t - mp * p.n_tiles;
-    const int mt2 = 2 * mp + (int)rank;
-    const int i0 = p.tiles_per_img > 0 ? mt2 / g.mt : mt2 * g.ipt;
-    const int ii = etid / kOct, o8 = etid - ii * kOct;
-    pb_next = make_uint4(0, 0, 0, 0);
-    if (i0 + ii < g.n_img)
-      pb_next = *reinterpret_cast<const uint4*>(g.pb + (size_t)(i0 + ii) * g.pb_stride + g.pb_off + nt * BN + o8 * 8);
-  };
-  static_assert(8 * kOct <= kEpiThreads, "one thread per (image, octet) of the pose-bias rows");
-  fetch_pb(tile0);
-  for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-    const int m_pair = tile / p.n_tiles;
-    const int n_tile = tile - m_pair * p.n_tiles;
-    const int m_tile = 2 * m_pair + (int)rank;
-    const int n_chan0 = n_tile * BN;
-    const bool live = m_tile < p.m_tiles;          // the peer of an odd last pair owns a phantom tile
-    int b0, y0;
-    conv_tile_coords(p, m_tile, b0, y0);
-    const int img0 = p.tiles_per_img > 0 ? m_tile / g.mt : m_tile * g.ipt;   // first image of the tile
-    uint8_t* ost = out_stage + obuf * S::kOutBytes;
-    if (etid < BN && (tile == tile0 || p.n_tiles > 1)) {     // channel parameters of this N-tile
-      s_bias[etid] = p.bias ? __ldg(p.bias + n_chan0 + etid) : 0.f;
-      if (g.G > 0) {
-        s_gamma[etid] = __ldg(g.gamma + n_chan0 + etid);
-        s_beta[etid] = __ldg(g.beta + n_chan0 + etid);
-      } else if (g.pre_stats) {
-        s_gamma[etid] = __ldg(g.pre_w1 + n_chan0 + etid);
-        s_beta[etid] = __ldg(g.pre_wb + n_chan0 + etid);
-      }
-    }
-    if (g.pb && etid < g.ipt * kOct)
-      *reinterpret_cast<uint4*>(s_pb + (etid / kOct) * BN + (etid % kOct) * 8) = pb_next;
-    NOPE_EPI_BAR();
-    fetch_pb(tile + tile_step);
-    conv_mma_tile<BN, BN / 64, STAGES, S::kStageBytes, S::kABytes, MMA>(p, smem, full_bar, empty_bar, kstage, kphase, s_acc);
-
-    // ---- pass 1: accumulator -> registers, free the ring, per-octet partial sums
-    uint32_t a[64];
-    {
-      const float* a_row = s_acc + row * acc_ld(BN) + cc * 64;
-      acc_ld_32(a_row, *reinterpret_cast<uint32_t(*)[32]>(&a[0]));
-      acc_ld_32(a_row + 32, *reinterpret_cast<uint32_t(*)[32]>(&a[32]));
-      acc_release(tempty_bar, lane);
-    }
-    if (live) {
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const float* bs = s_bias + cc * 64 + hh * 32;
-        float st[8];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 c0 = *reinterpret_cast<const float4*>(bs + j * 8);
-          const float4 c1 = *reinterpret_cast<const float4*>(bs + j * 8 + 4);
-          const float bb[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-          float f[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            f[i] = __uint_as_float(a[hh * 32 + j * 8 + i]) + bb[i];
-            a[hh * 32 + j * 8 + i] = __float_as_uint(f[i]);
-          }
-          float sm = (f[0] + f[1]) + (f[2] + f[3]) + ((f[4] + f[5]) + (f[6] + f[7]));
-          float q2 = f[0] * f[0];
-#pragma unroll
-          for (int i = 1; i < 8; ++i) q2 = fmaf(f[i], f[i], q2);
-          st[2 * j] = sm;
-          st[2 * j + 1] = q2;
-        }
-        if (g.G > 0) {
-          const int idx = small ? butterfly8<16>(st, lane) : butterfly8<32>(st, lane);
-          const bool writer = small ? ((lane & 1) == 0) : ((lane & 3) == 0);
-          const int segi = small ? (q * 2 + (lane >> 4)) : q;
-          if (writer) s_part[(segi * kOct + cc * 8 + hh * 4) * 2 + idx] = st[0];   // idx = octet * 2 + {sum, sumsq}
-        }
-      }
-      if (g.G > 0) {
-        NOPE_EPI_BAR();
-        float Sx = 0.f, Qx = 0.f;
-        if (etid < npairs) {
-          const int ii = etid / g.gpt, gl = etid - ii * g.gpt;
-          const int spi = hw >= kBM ? 4 : (small ? 1 : (hw >> 5));   // row segments of this image in the tile
-          const int s0 = hw >= kBM ? 0 : ii * spi;
-          const int opg = (g.cpg < BN ? g.cpg : BN) >> 3;
-          const int o0 = gl * opg;
-          for (int sgm = s0; sgm < s0 + spi; ++sgm)
-            for (int o = o0; o < o0 + opg; ++o) {
-              Sx += s_part[(sgm * kOct + o) * 2];
-              Qx += s_part[(sgm * kOct + o) * 2 + 1];
-            }
-        }
-        if (g.expected > 1) {
-          // publish {value, epoch}; then one thread per word of the sync group's [slot][pair][2] block polls
-          // until its word carries this launch's epoch (every poll of the CTA in flight at once)
-          const int sg = (m_tile / g.mt) * (p.n_tiles / g.tpg) + n_tile / g.tpg;
-          const int slot = (m_tile % g.mt) * g.tpg + (n_tile % g.tpg);
-          uint2* xp = g.xpart + (size_t)sg * g.expected * npairs * 2;
-          if (etid < npairs) {
-            st_volatile_u2(xp + ((size_t)slot * npairs + etid) * 2, make_uint2(__float_as_uint(Sx), g.epoch));
-            st_volatile_u2(xp + ((size_t)slot * npairs + etid) * 2 + 1, make_uint2(__float_as_uint(Qx), g.epoch));
-          }
-          if (etid < g.expected * npairs * 2) {
-            uint2 u = ld_volatile_u2(xp + etid);
-            if (u.y != g.epoch) {
-              const long long t0 = clock64();
-              do {
-                u = ld_volatile_u2(xp + etid);
-                if (clock64() - t0 > 4000000000LL) __trap();   // no printf: see mbar_wait
-              } while (u.y != g.epoch);
-            }
-            s_x[etid] = __uint_as_float(u.x);
-          }
-          NOPE_EPI_BAR();
-          if (use_tab) {
-            // one image per tile: per-channel scale / shift tables, y = x * sc[c] + sh[c]; every channel's
-            // thread sums its group's partials itself (fixed slot order), no (mean, rstd) hand-over
-            if (etid < BN) {
-              const int gl = s_og[etid >> 3];
-              float s1 = 0.f, s2 = 0.f;
-              for (int sl = 0; sl < g.expected; ++sl) {
-                s1 += s_x[(sl * npairs + gl) * 2];
-                s2 += s_x[(sl * npairs + gl) * 2 + 1];
-              }
-              const float mean = s1 * g.inv_cnt;
-              const float var = fmaxf(s2 * g.inv_cnt - mean * mean, 0.f);
-              const float sc = rsqrtf(var + g.eps) * s_gamma[etid];
-              s_sc[etid] = sc;
-              s_sh[etid] = s_beta[etid] - mean * sc;
-            }
-          } else if (etid < npairs) {           // fixed slot order
-            Sx = 0.f; Qx = 0.f;
-            for (int sl = 0; sl < g.expected; ++sl) {
-              Sx += s_x[(sl * npairs + etid) * 2];
-              Qx += s_x[(sl * npairs + etid) * 2 + 1];
-            }
-          }
-        }
-        if (!use_tab && etid < npairs) {
-          const float mean = Sx * g.inv_cnt;
-          const float var = fmaxf(Qx * g.inv_cnt - mean * mean, 0.f);
-          s_mr[etid] = make_float2(mean, rsqrtf(var + g.eps));
-        }
-        NOPE_EPI_BAR();
-      }
-
-      if (g.pre_stats) {
-        // folded pre-norm: (mean, rstd) of each input image of the tile from its producer's partial sums
-        if (g.ipt == 1) {
-          if (etid < BN) {
-            float s1 = 0.f, s2 = 0.f;
-            for (int k = 0; k < g.pre_parts; ++k) {
-              const float2 t = g.pre_stats[(size_t)img0 * g.pre_parts + k];
-              s1 += t.x;
-              s2 += t.y;
-            }
-            const float mean = s1 * g.pre_inv_cnt;
-            const float rstd = rsqrtf(fmaxf(s2 * g.pre_inv_cnt - mean * mean, 0.f) + g.eps);
-            s_sc[etid] = rstd;
-            s_sh[etid] = s_beta[etid] - rstd * mean * s_gamma[etid];
-          }
-        } else if (etid < g.ipt) {
-          float s1 = 0.f, s2 = 0.f;
-          if (img0 + etid < g.n_img)
-            for (int k = 0; k < g.pre_parts; ++k) {
-              const float2 t = g.pre_stats[(size_t)(img0 + etid) * g.pre_parts + k];
-              s1 += t.x;
-              s2 += t.y;
-            }
-          const float mean = s1 * g.pre_inv_cnt;
-          s_mr[etid] = make_float2(mean, rsqrtf(fmaxf(s2 * g.pre_inv_cnt - mean * mean, 0.f) + g.eps));
-        }
-        NOPE_EPI_BAR();
-      }
-
-      // ---- pass 2: normalise / activate / add, in place in the swizzled staging tile
-      if (g.has_res) mbar_wait(res_bar, res_phase);
-      float e1 = 0.f, e2 = 0.f;
-      const uint32_t tok = order_token(smem_u32(smem));          // tables below are read after the barrier above
-      const uint32_t a_gamma = tok + (uint32_t)(reinterpret_cast<uint8_t*>(s_gamma) - smem) + cc * 256;
-      const uint32_t a_beta = tok + (uint32_t)(reinterpret_cast<uint8_t*>(s_beta) - smem) + cc * 256;
-      const uint32_t a_pb = tok + (uint32_t)(reinterpret_cast<uint8_t*>(s_pb) - smem) + (it * BN + cc * 64) * 2;
-      const uint32_t a_mr = tok + (uint32_t)(reinterpret_cast<uint8_t*>(s_mr) - smem) + it * g.gpt * 8;
-      const uint32_t a_sc = tok + (uint32_t)(reinterpret_cast<uint8_t*>(s_sc) - smem) + cc * 256;
-      const uint32_t a_sh = tok + (uint32_t)(reinterpret_cast<uint8_t*>(s_sh) - smem) + cc * 256;
-      const int grow = m_tile * kBM + row;            // linear output pixel
-      const bool row_ok = grow < p.m_valid;
-      // residual pixel under the hoisted-prefix image mapping (32x32 images: one image per tile)
-      const long long rpix = g.res_div > 0
-          ? (long long)((g.res_base + b0) / g.res_div) * hw + (m_tile % g.mt) * kBM + row
-          : (long long)grow;
-      uint8_t* srow = ost + cc * (kBM * 128) + row * 128;
-      const bool do_norm = g.G > 0;
-      const bool do_silu = g.silu;
-      const bool pre = g.pre_stats != nullptr;
-      // Every step below runs over all 64 values of the thread with its (launch-uniform) condition tested
-      // OUTSIDE the unrolled loop: one long basic block per step, so the scheduler can keep tens of
-      // independent shared-memory loads / MUFU chains in flight (with the tests inside a per-octet loop
-      // every octet fell apart into five short blocks and the pass ran at a quarter of the issue rate).
-      float* f = reinterpret_cast<float*>(a);
-      const bool bf = p.bf16 != 0;
-      if (pre && g.ipt > 1) {
-        const float2 mr = lds_f2(tok + (uint32_t)(reinterpret_cast<uint8_t*>(s_mr) - smem) + it * 8);
-        const float nm = -mr.x * mr.y;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float4 w1 = lds_f4(a_gamma + j * 16), wb = lds_f4(a_beta + j * 16);
-          f[4 * j + 0] = fmaf(f[4 * j + 0], mr.y, fmaf(nm, w1.x, wb.x));
-          f[4 * j + 1] = fmaf(f[4 * j + 1], mr.y, fmaf(nm, w1.y, wb.y));
-          f[4 * j + 2] = fmaf(f[4 * j + 2], mr.y, fmaf(nm, w1.z, wb.z));
-          f[4 * j + 3] = fmaf(f[4 * j + 3], mr.y, fmaf(nm, w1.w, wb.w));
-        }
-      } else if ((do_norm && use_tab) || pre) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float4 sc = lds_f4(a_sc + j * 16), sh = lds_f4(a_sh + j * 16);
-          f[4 * j + 0] = fmaf(f[4 * j + 0], sc.x, sh.x);
-          f[4 * j + 1] = fmaf(f[4 * j + 1], sc.y, sh.y);
-          f[4 * j + 2] = fmaf(f[4 * j + 2], sc.z, sh.z);
-          f[4 * j + 3] = fmaf(f[4 * j + 3], sc.w, sh.w);
-        }
-      } else if (do_norm) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float2 mr = lds_f2(a_mr + s_og[(cc * 64 + j * 8) >> 3] * 8);
-#pragma unroll
-          for (int h2 = 0; h2 < 2; ++h2) {
-            const float4 gm = lds_f4(a_gamma + j * 32 + h2 * 16), bt = lds_f4(a_beta + j * 32 + h2 * 16);
-            float* ff = f + j * 8 + h2 * 4;
-            ff[0] = fmaf(ff[0] - mr.x, mr.y * gm.x, bt.x);
-            ff[1] = fmaf(ff[1] - mr.x, mr.y * gm.y, bt.y);
-            ff[2] = fmaf(ff[2] - mr.x, mr.y * gm.z, bt.z);
-            ff[3] = fmaf(ff[3] - mr.x, mr.y * gm.w, bt.w);
-          }
-        }
-      }
-      if (do_silu) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) f[i] = silu_ftz(f[i]);
-      }
-      if (g.pb) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint4 pv = lds_u4(a_pb + j * 16);
-          const uint32_t* hp = reinterpret_cast<const uint32_t*>(&pv);
-#pragma unroll
-          for (int k2 = 0; k2 < 4; ++k2) {
-            const float2 t = unpack2(hp[k2], bf);
-            f[j * 8 + 2 * k2] += t.x;
-            f[j * 8 + 2 * k2 + 1] += t.y;
-          }
-        }
-      }
-      if (g.has_res) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint4 rv = *reinterpret_cast<const uint4*>(srow + ((j ^ (row & 7)) << 4));
-          const uint32_t* hr = reinterpret_cast<const uint32_t*>(&rv);
-#pragma unroll
-          for (int k2 = 0; k2 < 4; ++k2) {
-            const float2 t = unpack2(hr[k2], bf);
-            f[j * 8 + 2 * k2] += t.x;
-            f[j * 8 + 2 * k2 + 1] += t.y;
-          }
-        }
-        if (g.res_lo && row_ok) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint4 rl = *reinterpret_cast<const uint4*>(g.res_lo + rpix * p.n_total + n_chan0 + cc * 64 + j * 8);
-            const __half2* hl = reinterpret_cast<const __half2*>(&rl);
-#pragma unroll
-            for (int k2 = 0; k2 < 4; ++k2) {
-              const float2 t = __half22float2(hl[k2]);
-              f[j * 8 + 2 * k2] += t.x;
-              f[j * 8 + 2 * k2 + 1] += t.y;
-            }
-          }
-        }
-      }
-      const bool want_lo = g.out_lo && row_ok;
-      const bool want_emit = g.emit != nullptr;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        uint4 w;
-        w.x = pack2(f[j * 8 + 0], f[j * 8 + 1], bf);
-        w.y = pack2(f[j * 8 + 2], f[j * 8 + 3], bf);
-        w.z = pack2(f[j * 8 + 4], f[j * 8 + 5], bf);
-        w.w = pack2(f[j * 8 + 6], f[j * 8 + 7], bf);
-        *reinterpret_cast<uint4*>(srow + ((j ^ (row & 7)) << 4)) = w;
-        if (want_lo || want_emit) {
-          const uint32_t* hw2 = reinterpret_cast<const uint32_t*>(&w);
-          uint4 wl;
-          uint32_t* pl = reinterpret_cast<uint32_t*>(&wl);
-#pragma unroll
-          for (int k2 = 0; k2 < 4; ++k2) {
-            const float2 t = unpack2(hw2[k2], bf);
-            pl[k2] = pack_half2(f[j * 8 + 2 * k2] - t.x, f[j * 8 + 2 * k2 + 1] - t.y);
-            e1 += t.x + t.y;                 // statistics of the values as stored (what the consumer reads)
-            e2 = fmaf(t.x, t.x, e2);
-            e2 = fmaf(t.y, t.y, e2);
-          }
-          if (want_lo)
-            *reinterpret_cast<uint4*>(g.out_lo + (size_t)grow * p.n_total + n_chan0 + cc * 64 + j * 8) = wl;
-        }
-      }
-      if (g.has_res) res_phase ^= 1;
-      if (g.emit) {
-        // 16-row segments: every image is a whole number of them at every resolution
-#pragma unroll
-        for (int off = 8; off > 0; off >>= 1) {
-          e1 += __shfl_xor_sync(0xffffffffu, e1, off);
-          e2 += __shfl_xor_sync(0xffffffffu, e2, off);
-        }
-        if ((lane & 15) == 0) s_em[cc * 8 + (row >> 4)] = make_float2(e1, e2);
-        NOPE_EPI_BAR();
-        if (etid < g.ipt && img0 + etid < g.n_img) {
-          const int r16 = hw >= kBM ? 8 : (hw >> 4);
-          float s1 = 0.f, s2 = 0.f;
-          for (int h2 = 0; h2 < kNS; ++h2)
-            for (int r = etid * r16; r < (etid + 1) * r16; ++r) {
-              s1 += s_em[h2 * 8 + r].x;
-              s2 += s_em[h2 * 8 + r].y;
-            }
-          g.emit[(size_t)(img0 + etid) * g.emit_parts + (m_tile % g.mt) * p.n_tiles + n_tile] = make_float2(s1, s2);
-        }
-      }
-      fence_proxy_async_smem();
-      NOPE_EPI_BAR();
-      if (etid == 0) {
-#pragma unroll 1
-        for (int c2 = 0; c2 < kNS; ++c2)
-          tma_store_4d(&p.omap[0], ost + c2 * (kBM * 128), n_chan0 + c2 * 64, 0, y0, b0);
-        tma_store_commit();
-      }
-    }
-    if (etid == 0) stage_residual(tile + tile_step, obuf ^ (S::kOutBufs - 1));
-    obuf ^= S::kOutBufs - 1;
-  }
-  if (etid == 0) tma_store_wait_all();
-#undef NOPE_EPI_BAR
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// EPI == 4: the GroupNorm-fused epilogue with the bookkeeping moved off the math warps.
-//
-// EPI == 3 walks all epilogue warps through the tile in lock step: five to six block-wide barriers per tile,
-// the statistics exchange, the table build and the drain of the TMA store all sit on the critical path of the
-// warps that do the arithmetic.  Here warps 2 and 3 take that work and talk to the math warps through mbarriers only:
-//
-//   warps 4..   math: wgmma mainloop, accumulator -> registers (+bias), release the ring, per-octet partial sums -> s_part,
-//               arrive part_bar | wait stats_bar[b], res_bar | normalise / SiLU / pose bias / residual in place
-//               in the staging tile | arrive out_bar, tabfree_bar[b].   No block-wide barrier anywhere.
-//   warp 3      statistics: wait part_bar | per-(image, group) sums, publish {value, epoch} words, poll the peer
-//               tiles, fixed-order totals | per-channel scale / shift table (or (mean, rstd) pairs) into buffer
-//               b = tile parity | arrive stats_bar[b].  The pre-norm fold's per-image scalars are independent of
-//               the accumulator, so for those launches this warp runs a tile ahead of the math warps.
-//   warp 2      store: wait out_bar | GroupNorm(1) sums of the stored tile (emit) | TMA store | once the store has
-//               read the staging buffer: TMA load of the NEXT tile's residual into it (or a plain arrive), res_bar.
-//
-// Per-channel parameters (bias, gamma, beta, pose-bias rows) are read through the read-only L1 path instead of
-// being staged in shared memory per tile, which removes the staging barrier.  Results agree with EPI == 3 up to
-// the summation order of the statistics; the two are not bit-identical.
-// ---------------------------------------------------------------------------------------------
-struct Gn2Bars {
+struct GnBars {
   uint64_t* full;       // [STAGES] operand stage landed (producer -> math warps)
   uint64_t* empty;      // [STAGES] operand stage consumed (math warps -> producer)
   uint64_t* tempty;     // accumulator tile read out of the ring (math warps -> producer)
@@ -599,10 +168,10 @@ struct Gn2Bars {
 // Shared-memory operands are read with non-volatile asm loads whose address derives from the order token taken after
 // the barrier waits: the compiler may hoist them above the in-place stores (other octets, other addresses).
 template <int NORM, bool SILU, bool PB, bool RES, bool EMIT>
-__device__ __forceinline__ void gn2_pass2_octets(float* f, uint32_t a_sc, uint32_t a_sh, uint32_t a_mr, const int* og,
-                                                 int it_gpt, const float4* gm4, const float4* bt4, const uint4* pb4,
-                                                 bool img_ok, uint8_t* srow, uint32_t a_srow, int row, bool bf,
-                                                 float& e1, float& e2) {
+__device__ __forceinline__ void gn_pass2_octets(float* f, uint32_t a_sc, uint32_t a_sh, uint32_t a_mr, const int* og,
+                                                int it_gpt, const float4* gm4, const float4* bt4, const uint4* pb4,
+                                                bool img_ok, uint8_t* srow, uint32_t a_srow, int row, bool bf,
+                                                float& e1, float& e2) {
   float2 mr3 = make_float2(0.f, 0.f);
   if (NORM == 3) mr3 = lds_f2(a_mr);
 #pragma unroll
@@ -679,17 +248,17 @@ __device__ __forceinline__ void gn2_pass2_octets(float* f, uint32_t a_sc, uint32
 
 
 template <int BN, int STAGES, bool MMA>
-__device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t* smem, uint8_t* gsm,
-                                                    const Gn2Bars& B, int tile0, int tile_step, int num_tiles,
-                                                    uint32_t rank) {
+__device__ __forceinline__ void conv_gn_math_warps(const ConvParams& p, uint8_t* smem, uint8_t* gsm,
+                                                   const GnBars& B, int tile0, int tile_step, int num_tiles,
+                                                   uint32_t rank) {
   using S = Conv2Smem<BN, STAGES, 4>;
-  using G2 = Gn2Smem<BN>;
+  using GS = GnSmem<BN>;
   constexpr int kOct = BN / 8;
   constexpr int kNB = S::kOutBufs;                   // staging buffers: tile i uses buffer i % kNB
   uint8_t* ost0 = smem + STAGES * S::kStageBytes;
-  float* s_part = reinterpret_cast<float*>(gsm + G2::kPart);
-  const int* s_og = reinterpret_cast<const int*>(gsm + G2::kOg);
-  float2* s_em0 = reinterpret_cast<float2*>(gsm + G2::kEm);
+  float* s_part = reinterpret_cast<float*>(gsm + GS::kPart);
+  const int* s_og = reinterpret_cast<const int*>(gsm + GS::kOg);
+  float2* s_em0 = reinterpret_cast<float2*>(gsm + GS::kEm);
 
   const GnFuse& g = p.gn;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -704,7 +273,7 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
   const bool wait_stats = g.G > 0 || pre;
   const bool bf = p.bf16 != 0;
   const uint32_t gsm_off = (uint32_t)(gsm - smem);
-  // pass-2 variant: the hot epilogue shapes run gn2_pass2_octets, everything else the phase-per-step code
+  // pass-2 variant: the hot epilogue shapes run gn_pass2_octets, everything else the phase-per-step code
   int variant = -1;
   if (!(g.out_lo || g.res_lo)) {
     if (g.G > 0 && g.silu) {
@@ -788,8 +357,8 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
     // ---- pass 2: normalise / activate / add, in place in the swizzled staging tile
     float e1 = 0.f, e2 = 0.f;
     const uint32_t tok = order_token(smem_u32(smem));          // tables below are read after the waits above
-    const uint32_t a_mr = tok + gsm_off + G2::kMr + b * 64 * 8;
-    const uint32_t a_sc = tok + gsm_off + G2::kTab + b * 2 * BN * 4 + cc * 256;
+    const uint32_t a_mr = tok + gsm_off + GS::kMr + b * 64 * 8;
+    const uint32_t a_sc = tok + gsm_off + GS::kTab + b * 2 * BN * 4 + cc * 256;
     const uint32_t a_sh = a_sc + BN * 4;
     const int grow = m_tile * kBM + row;            // linear output pixel
     const bool row_ok = grow < p.m_valid;
@@ -808,14 +377,14 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
       const int* og = s_og + cc * 8;
       const int it_gpt = it * g.gpt;
       switch (variant) {
-        case 0: gn2_pass2_octets<1, true, true, false, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
-        case 1: gn2_pass2_octets<2, true, true, false, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
-        case 2: gn2_pass2_octets<1, true, false, true, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
-        case 3: gn2_pass2_octets<1, true, false, true, true>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
-        case 4: gn2_pass2_octets<2, true, false, true, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
-        case 5: gn2_pass2_octets<2, true, false, true, true>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
-        case 6: gn2_pass2_octets<1, false, false, false, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
-        default: gn2_pass2_octets<3, false, false, false, false>(f, a_sc, a_sh, a_mr + it * 8, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
+        case 0: gn_pass2_octets<1, true, true, false, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
+        case 1: gn_pass2_octets<2, true, true, false, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
+        case 2: gn_pass2_octets<1, true, false, true, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
+        case 3: gn_pass2_octets<1, true, false, true, true>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
+        case 4: gn_pass2_octets<2, true, false, true, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
+        case 5: gn_pass2_octets<2, true, false, true, true>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
+        case 6: gn_pass2_octets<1, false, false, false, false>(f, a_sc, a_sh, a_mr, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
+        default: gn_pass2_octets<3, false, false, false, false>(f, a_sc, a_sh, a_mr + it * 8, og, it_gpt, gm4, bt4, pb4, img_ok, srow, a_srow, row, bf, e1, e2); break;
       }
     } else {
     // every step runs over all 64 values of the thread with its (launch-uniform) condition tested outside the
@@ -949,15 +518,15 @@ __device__ __forceinline__ void conv_gn2_math_warps(const ConvParams& p, uint8_t
 
 // statistics warp (warp 3) of the EPI == 4 epilogue
 template <int BN, int STAGES>
-__device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t* gsm, const Gn2Bars& B, int tile0,
-                                                    int tile_step, int num_tiles, uint32_t rank) {
-  using G2 = Gn2Smem<BN>;
+__device__ __forceinline__ void conv_gn_stats_warp(const ConvParams& p, uint8_t* gsm, const GnBars& B, int tile0,
+                                                   int tile_step, int num_tiles, uint32_t rank) {
+  using GS = GnSmem<BN>;
   constexpr int kOct = BN / 8;
-  const float* s_part = reinterpret_cast<const float*>(gsm + G2::kPart);
-  float2* s_mr = reinterpret_cast<float2*>(gsm + G2::kMr);
-  float* s_tab = reinterpret_cast<float*>(gsm + G2::kTab);
-  int* s_og = reinterpret_cast<int*>(gsm + G2::kOg);
-  float* s_x = reinterpret_cast<float*>(gsm + G2::kX);
+  const float* s_part = reinterpret_cast<const float*>(gsm + GS::kPart);
+  float2* s_mr = reinterpret_cast<float2*>(gsm + GS::kMr);
+  float* s_tab = reinterpret_cast<float*>(gsm + GS::kTab);
+  int* s_og = reinterpret_cast<int*>(gsm + GS::kOg);
+  float* s_x = reinterpret_cast<float*>(gsm + GS::kX);
   const GnFuse& g = p.gn;
   const int lane = threadIdx.x & 31;
   const int hw = p.stats_hw;
@@ -1210,14 +779,14 @@ __device__ __forceinline__ void conv_gn2_stats_warp(const ConvParams& p, uint8_t
 
 // store warp (warp 2) of the EPI == 4 epilogue
 template <int BN, int STAGES>
-__device__ __forceinline__ void conv_gn2_store_warp(const ConvParams& p, uint8_t* smem, uint8_t* gsm, const Gn2Bars& B,
-                                                    int tile0, int tile_step, int num_tiles, uint32_t rank) {
+__device__ __forceinline__ void conv_gn_store_warp(const ConvParams& p, uint8_t* smem, uint8_t* gsm, const GnBars& B,
+                                                   int tile0, int tile_step, int num_tiles, uint32_t rank) {
   using S = Conv2Smem<BN, STAGES, 4>;
-  using G2 = Gn2Smem<BN>;
+  using GS = GnSmem<BN>;
   constexpr int kNS = BN / 64;
   constexpr int kNB = S::kOutBufs;
   uint8_t* ost0 = smem + STAGES * S::kStageBytes;
-  const float2* s_em0 = reinterpret_cast<const float2*>(gsm + G2::kEm);
+  const float2* s_em0 = reinterpret_cast<const float2*>(gsm + GS::kEm);
   const GnFuse& g = p.gn;
   const int lane = threadIdx.x & 31;
   const int hw = p.stats_hw;
@@ -1287,17 +856,16 @@ __device__ __forceinline__ void conv_gn2_store_warp(const ConvParams& p, uint8_t
   if (lane == 0) tma_store_wait_all();
 }
 
-// EPI: 0 = plain epilogue (the sweep), 1 = extras (ReLU / residual / hi-lo / fp32), 2 = GEGLU
+// EPI: 0 = plain epilogue (the sweep), 1 = extras (ReLU / residual / hi-lo / fp32), 2 = GEGLU, 4 = GroupNorm fused
 // Register split (setmaxnreg) of the clustered kernel at 384 and 512 threads: the control warpgroup (warps 0-3: the
 // producer, and with EPI == 4 the store and statistics warps) drops to conv2_ctl_regs, the math warpgroups share the
 // rest of the 64 K register file evenly: 224 per thread at 384 threads (208 with EPI == 4), 144 at 512 threads
-// (BN = 192, EPI 3 / 4).  Blocks of 256 threads already allow 255 registers per thread and keep that limit.
+// (BN = 192, EPI == 4).  Blocks of 256 threads already allow 255 registers per thread and keep that limit.
 // Not every instantiation is spill-free (ptxas -v, spill store / load bytes): <192,4,4> 134 / 212,
 // spread over the statistics warp at 80 and the math warps at 144; at 512 threads
 // the four warpgroups average 128 registers, and moving registers between the roles moves the spills with them.
-// <128,4,4> 56 / 108 (statistics warp and epilogue), <128,4,3> 8 / 32, <192,4,3> 548 / 688 (the lock-step A/B
-// epilogue at 144).
-__host__ __device__ constexpr int conv2_threads(int BN, int EPI) { return EPI >= 3 ? gn_threads(BN) : kConvThreads; }
+// <128,4,4> 60 / 112 (statistics warp and epilogue).
+__host__ __device__ constexpr int conv2_threads(int BN, int EPI) { return EPI == 4 ? gn_threads(BN) : kConvThreads; }
 __host__ __device__ constexpr int conv2_ctl_regs(int EPI) { return EPI == 4 ? 80 : 56; }
 __host__ __device__ constexpr int conv2_launch_regs(int threads) { return 65536 / threads / 8 * 8; }
 __host__ __device__ constexpr int conv2_math_regs(int threads, int EPI) {
@@ -1324,8 +892,8 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* tempty_bar = empty_bar + STAGES;
-  uint64_t* res_bar = tempty_bar + 1;                                 // EPI >= 3: residual tile landed
-  uint64_t* gn2_bar = res_bar + 1;                                    // EPI == 4: part, stats[2], tabfree[2], out[2], res of buffer 1
+  uint64_t* res_bar = tempty_bar + 1;                                 // EPI == 4: residual tile landed
+  uint64_t* gn_bar = res_bar + 1;                                     // EPI == 4: part, stats[2], tabfree[2], out[2], res of buffer 1
   static_assert((2 * STAGES + 2 + 8) * 8 <= 256, "barrier block overflow");
   float* s_bias = reinterpret_cast<float*>(smem + S::kBiasOffset);
   float* s_acc = reinterpret_cast<float*>(smem);
@@ -1350,14 +918,14 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
     mbar_init(tempty_bar, kMathWarps);
     mbar_init(res_bar, 1);
     if constexpr (EPI == 4) {
-      mbar_init(&gn2_bar[0], gn_epi_warps(BN));                         // part
-      mbar_init(&gn2_bar[1], 1);                                        // stats[0]
-      mbar_init(&gn2_bar[2], 1);                                        // stats[1]
-      mbar_init(&gn2_bar[3], gn_epi_warps(BN));                         // tabfree[0]
-      mbar_init(&gn2_bar[4], gn_epi_warps(BN));                         // tabfree[1]
-      mbar_init(&gn2_bar[5], gn_epi_warps(BN));                         // out[0]
-      mbar_init(&gn2_bar[6], gn_epi_warps(BN));                         // out[1]
-      mbar_init(&gn2_bar[7], 1);                                        // res of staging buffer 1
+      mbar_init(&gn_bar[0], gn_epi_warps(BN));                          // part
+      mbar_init(&gn_bar[1], 1);                                         // stats[0]
+      mbar_init(&gn_bar[2], 1);                                         // stats[1]
+      mbar_init(&gn_bar[3], gn_epi_warps(BN));                          // tabfree[0]
+      mbar_init(&gn_bar[4], gn_epi_warps(BN));                          // tabfree[1]
+      mbar_init(&gn_bar[5], gn_epi_warps(BN));                          // out[0]
+      mbar_init(&gn_bar[6], gn_epi_warps(BN));                          // out[1]
+      mbar_init(&gn_bar[7], 1);                                         // res of staging buffer 1
     }
     fence_mbar_init();
   }
@@ -1366,10 +934,10 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
   // and may overlap the tail of the previous kernel in the stream; from here on the kernel reads what that kernel
   // wrote.  The next kernel's CTAs may be scheduled as soon as this grid's CTAs retire.
   pdl_sync();
-  auto gn2_bars = [&] {                                               // EPI == 4
-    Gn2Bars B;
-    B.full = full_bar; B.empty = empty_bar; B.tempty = tempty_bar; B.res[0] = res_bar; B.res[1] = &gn2_bar[7];
-    B.part = &gn2_bar[0]; B.stats = &gn2_bar[1]; B.tabfree = &gn2_bar[3]; B.out = &gn2_bar[5];
+  auto gn_bars = [&] {                                                // EPI == 4
+    GnBars B;
+    B.full = full_bar; B.empty = empty_bar; B.tempty = tempty_bar; B.res[0] = res_bar; B.res[1] = &gn_bar[7];
+    B.part = &gn_bar[0]; B.stats = &gn_bar[1]; B.tabfree = &gn_bar[3]; B.out = &gn_bar[5];
     return B;
   };
   uint8_t* gsm = smem + S::kGnOffset;
@@ -1411,28 +979,17 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
     }
     } else if constexpr (EPI == 4) {
       // ===================== GroupNorm-fused epilogue: store warp 2, statistics warp 3 =====================
-      const Gn2Bars B = gn2_bars();
-      if (warp == 2) conv_gn2_store_warp<BN, STAGES>(p, smem, gsm, B, tile0, tile_step, num_tiles, rank);
-      else if (warp == 3) conv_gn2_stats_warp<BN, STAGES>(p, gsm, B, tile0, tile_step, num_tiles, rank);
+      const GnBars B = gn_bars();
+      if (warp == 2) conv_gn_store_warp<BN, STAGES>(p, smem, gsm, B, tile0, tile_step, num_tiles, rank);
+      else if (warp == 3) conv_gn_stats_warp<BN, STAGES>(p, gsm, B, tile0, tile_step, num_tiles, rank);
     }
   } else if constexpr (EPI == 4) {
     // ===================== mainloop + epilogue with GroupNorm fused, bookkeeping on warps 2 / 3 =====================
     if constexpr (kRegSplit) setmaxnreg_inc<kMathRegs>();
     if (warp >= 12) {                       // BN = 192: the third math warpgroup runs the epilogue only
-      if constexpr (kMathWarps == 12) conv_gn2_math_warps<BN, STAGES, false>(p, smem, gsm, gn2_bars(), tile0, tile_step, num_tiles, rank);
+      if constexpr (kMathWarps == 12) conv_gn_math_warps<BN, STAGES, false>(p, smem, gsm, gn_bars(), tile0, tile_step, num_tiles, rank);
     } else {
-      conv_gn2_math_warps<BN, STAGES, true>(p, smem, gsm, gn2_bars(), tile0, tile_step, num_tiles, rank);
-    }
-  } else if constexpr (EPI == 3) {
-    // ===================== mainloop + epilogue with GroupNorm fused =====================
-    if constexpr (kRegSplit) setmaxnreg_inc<kMathRegs>();
-    if (warp >= 12) {                       // BN = 192: the third math warpgroup runs the epilogue only
-      if constexpr (kMathWarps == 12)
-        conv_gn_epilogue_loop<BN, STAGES, false>(p, smem, full_bar, empty_bar, tempty_bar, res_bar, tile0, tile_step,
-                                                 num_tiles, rank);
-    } else {
-      conv_gn_epilogue_loop<BN, STAGES, true>(p, smem, full_bar, empty_bar, tempty_bar, res_bar, tile0, tile_step,
-                                              num_tiles, rank);
+      conv_gn_math_warps<BN, STAGES, true>(p, smem, gsm, gn_bars(), tile0, tile_step, num_tiles, rank);
     }
   } else {
     // ===================== mainloop + epilogue (own 128 rows, 8 warps) =====================
@@ -1516,7 +1073,7 @@ inline int launch_conv_tc2_t(const ConvParams& p, int num_sms, cudaStream_t stre
     NOPE_CUDA(cudaFuncSetAttribute(conv_tc2_kernel<BN, STAGES, EPI>,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal));
     int mc = num_sms / 2;
-    if (EPI >= 3) {
+    if (EPI == 4) {
       // tiles of one image wait for each other: every cluster of the grid must be resident
       cudaLaunchConfig_t cfg;
       memset(&cfg, 0, sizeof cfg);
@@ -1557,24 +1114,11 @@ inline int launch_conv_tc2_t(const ConvParams& p, int num_sms, cudaStream_t stre
 inline int launch_conv_gn(const ConvParams& p, int bn, int num_sms, cudaStream_t stream) {
   if (p.n_par != 1 || p.geglu || conv_needs_extras(p) || p.stats)
     return fail("launch_conv_gn: the fused GroupNorm epilogue takes a plain convolution");
-  // NOPE_GN_EPI=3 selects the lock-step epilogue (EPI == 3) for A/B measurements; default: EPI == 4
-  static const int epi = [] {
-    const char* e = getenv("NOPE_GN_EPI");
-    return e && atoi(e) == 3 ? 3 : 4;
-  }();
   // ring depths: the deepest ring that fits 227 KB of shared memory beside the staging buffers
-  if (epi == 3) {
-    switch (bn) {
-      case 192: return launch_conv_tc2_t<192, 4, 3>(p, num_sms, stream);
-      case 128: return launch_conv_tc2_t<128, 4, 3>(p, num_sms, stream);
-      case 64: return launch_conv_tc2_t<64, 6, 3>(p, num_sms, stream);
-    }
-  } else {
-    switch (bn) {
-      case 192: return launch_conv_tc2_t<192, 4, 4>(p, num_sms, stream);
-      case 128: return launch_conv_tc2_t<128, 4, 4>(p, num_sms, stream);
-      case 64: return launch_conv_tc2_t<64, 7, 4>(p, num_sms, stream);
-    }
+  switch (bn) {
+    case 192: return launch_conv_tc2_t<192, 4, 4>(p, num_sms, stream);
+    case 128: return launch_conv_tc2_t<128, 4, 4>(p, num_sms, stream);
+    case 64: return launch_conv_tc2_t<64, 7, 4>(p, num_sms, stream);
   }
   return fail("launch_conv_gn: unsupported BN");
 }

@@ -794,10 +794,9 @@ struct nope_unet {
       NOPE_CUDA(launch_pdl(linattn_kernel, dim3(4, n), dim3(kLinAttnThreads), 0, st, TD.hi, TC.hi, S * S, bf()));
     }
     ++launches;
-    // to_out (K = 128: two K-steps per tile) + GroupNorm(1) + residual in one kernel.  With the role-split epilogue
-    // this takes the same time as the plain convolution plus one normalisation pass (18.80 vs 18.71 ms over the step
-    // under ncu; the lock-step epilogue measured slower: 319 vs 244 us at 32x32), and it never rounds the
-    // un-normalised output to 16 bits (full-size configs[2] scores: 0.99e-3 vs 1.06e-3)
+    // to_out (K = 128: two K-steps per tile) + GroupNorm(1) + residual in one kernel.  This takes the same time as
+    // the plain convolution plus one normalisation pass (18.80 vs 18.71 ms over the step under ncu), and it never
+    // rounds the un-normalised output to 16 bits (full-size configs[2] scores: 0.99e-3 vs 1.06e-3)
     GnSpec so;
     so.norm = &norms.at(p + ".outnorm");
     so.res = x;

@@ -15,8 +15,6 @@ case "$step" in
   tests)    rm -f gpurun_out/parity_log.jsonl; run "pytest -m gpu" 2400 python -m pytest tests -m gpu -q -rA --tb=short > gpurun_out/pytest_gpu.log 2>&1; tail -8 gpurun_out/pytest_gpu.log ;;
   dflt)     rm -f gpurun_out/parity_log.jsonl; run "pytest -m gpu (default path)" 2400 python -m pytest tests -m gpu -q --tb=short --ignore=tests/test_ldm_gpu.py > gpurun_out/pytest_dflt.log 2>&1; tail -25 gpurun_out/pytest_dflt.log ;;
   ldmtests) run "ldm tests" 1500 python -m pytest tests/test_ldm_gpu.py -m gpu -q --tb=short > gpurun_out/t_ldm.log 2>&1; tail -5 gpurun_out/t_ldm.log ;;
-  epi)      for d in ${EPI_LIST:-3 4 3 4}; do echo "NOPE_GN_EPI=$d"; NOPE_GN_EPI=$d timeout 600 python tools/time_sweep.py ${TIME_SPECS:-fp16} --steps 20 2>&1 | tail -1 | cut -c1-200; done > gpurun_out/epi_ab.log 2>&1; cat gpurun_out/epi_ab.log
-            for d in 3 4; do NOPE_GN_EPI=$d NOPE_PROF_DUMP=gpurun_out/prof_dump_epi$d.csv timeout 600 python tools/time_sweep.py fp16 --profile > /dev/null 2>&1; done ;;
   pdl)      for d in ${PDL_LIST:-0 1 3 0 1 3 0 1 3}; do echo "NOPE_PDL=$d"; NOPE_PDL=$d timeout 600 python tools/time_sweep.py fp16 --steps 20 2>&1 | tail -1 | cut -c1-120; done > gpurun_out/pdl_ab.log 2>&1; cat gpurun_out/pdl_ab.log ;;
   ncu_gn)   run "ncu full: fused conv" 900 ncu --profile-from-start off --set full --clock-control none --import-source on --kernel-name-base demangled -k regex:"${NCU_KREGEX:-conv_tc2_kernel<\(int\)192, \(int\)6, \(int\)4>}" -s ${NCU_SKIP:-1} -c ${NCU_COUNT:-3} -o gpurun_out/prof_gn -f python tools/profile_step.py > gpurun_out/ncu_gn.log 2>&1
             ncu -i gpurun_out/prof_gn.ncu-rep --page raw --csv > gpurun_out/prof_gn_raw.csv 2>/dev/null ;;
