@@ -273,6 +273,28 @@ int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int
                          float znear, int iters, float* depth, double* t_out, double* iou, int32_t* stats_out,
                          void* stream);
 
+/* Pose refinement from the sensor depth (DESIGN.md section 19).
+ * nope_refine_depth: projective point-to-plane ICP of P pose hypotheses per frame for F frames against the frame's
+ * sensor depth.  Mesh as nope_render_depth; R [F, P, 9] fp64 row-major and t_init [F, P, 3] fp64 (model -> OpenCV
+ * camera, mm), depth_sensor [F, H, W] fp64 (mm, 0 = no reading), masks [F, H, W] uint8 (nonzero = object; null: every
+ * pixel counts), all on the device; K HOST [F, 4] fp64 (fx, fy, cx, cy; finite, fx and fy non-zero), staged in stream
+ * order; rho the largest vertex norm of the mesh (finite, > 0); tau HOST [iters + 1] fp64 the pairing tolerances (mm,
+ * each finite and > 0).  Iteration i renders [R | t] rounded to fp32 with nope_render_depth's rasterizer, pairs every
+ * interior pixel whose render and its four neighbours are hit, inside the mask, with a sensor reading S and
+ * |S - D| <= tau[i], and applies one damped Gauss-Newton step of the point-to-plane distances (rotation about t).
+ * -> R_out [F, P, 9], t_out [F, P, 3] fp64 after `iters` steps; fit_out [F, P, 4] fp64 = (n_in, n_valid, rms, score)
+ * at the returned pose and tau[iters]: the pairs, the mask pixels with a reading, tau sqrt(sum e^2 / n_in) in mm (NaN
+ * when n_in = 0) and n_in / n_valid (NaN when n_valid = 0).  sums_out [F, P, 29] int64 (the fixed-point sums of the
+ * last render, units of 2^-32: J J^T upper triangle, J e, e^2, n_in) may be null.  depth [F P, H, W] fp32 is the
+ * caller's workspace; on return it holds nope_render_depth's image at the returned pose.  Requires V, NF >= 1,
+ * 1 <= F, P <= 65535, 1 <= H, W <= 8192, 0 <= iters <= 1024, znear finite and > 0.  Refuses bad arguments before any
+ * CUDA call; all iterations are enqueued without synchronising the host.  The result does not depend on the batch or
+ * on scheduling. */
+int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF, const double* R, const double* t_init,
+                      const double* depth_sensor, const uint8_t* masks, const double* K, int F, int P, int H, int W,
+                      double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
+                      double* t_out, double* fit_out, int64_t* sums_out, void* stream);
+
 /* BOP 2019 errors (DESIGN.md section 15).
  * nope_vsd_error_taus: nope_vsd_error at T misalignment tolerances in one pass (the distance images, visibility
  * masks and counts are shared): taus HOST [T] fp64, each finite and > 0, 1 <= T <= 16; K HOST [F, 4] fp64, finite,

@@ -31,6 +31,7 @@
 #include "pose_error.cuh"
 #include "crop.cuh"
 #include "translation.cuh"
+#include "depth_refine.cuh"
 
 using namespace nope;
 
@@ -1660,6 +1661,76 @@ int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int
   fit_final_kernel<<<ew_blocks, 256, 0, st>>>(t, mask_stats, sil_stats, F, P, t_out, iou, stats_out);
   NOPE_CUDA(cudaGetLastError());
   depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);      // depth holds render_depth at the returned t
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// pose refinement from the sensor depth (depth_refine.cuh, DESIGN.md section 19)
+// ---------------------------------------------------------------------------------
+int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF, const double* R, const double* t_init,
+                      const double* depth_sensor, const uint8_t* masks, const double* K, int F, int P, int H, int W,
+                      double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
+                      double* t_out, double* fit_out, int64_t* sums_out, void* stream) {
+  NOPE_CHECK(vertices && faces && R && t_init && depth_sensor && K && tau && depth && R_out && t_out && fit_out,
+             "null argument");
+  NOPE_CHECK(V >= 1 && NF >= 1, "V and NF must be >= 1");
+  NOPE_CHECK(F >= 1 && F <= 65535 && P >= 1 && P <= 65535, "F and P must be in [1, 65535]");
+  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
+  NOPE_CHECK(iters >= 0 && iters <= 1024, "iters must be in [0, 1024]");
+  NOPE_CHECK(std::isfinite(rho) && rho > 0.0, "rho must be finite and > 0");
+  NOPE_CHECK(znear > 0.f && std::isfinite(znear), "znear must be finite and > 0");
+  for (int i = 0; i <= iters; ++i) NOPE_CHECK(std::isfinite(tau[i]) && tau[i] > 0.0, "tau must be finite and > 0");
+  if (check_host_intrinsics(K, F)) return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // one stream-ordered block: K, the current R and t, the integer sums, the float32 poses and n_valid
+  const size_t n = (size_t)F * P;
+  const size_t k_bytes = sizeof(double) * 4 * F, R_bytes = sizeof(double) * 9 * n, t_bytes = sizeof(double) * 3 * n;
+  const size_t sum_bytes = sizeof(unsigned long long) * kIcpSums * n, pose_bytes = sizeof(float) * 16 * n;
+  StagedHost scratch;
+  scratch.st = st;
+  NOPE_CUDA(cudaMallocAsync(&scratch.dev, k_bytes + R_bytes + t_bytes + sum_bytes + pose_bytes + sizeof(int) * F, st));
+  char* base = static_cast<char*>(scratch.dev);
+  double* kd = reinterpret_cast<double*>(base);
+  double* Rc = reinterpret_cast<double*>(base + k_bytes);
+  double* tc = reinterpret_cast<double*>(base + k_bytes + R_bytes);
+  auto* sums = reinterpret_cast<unsigned long long*>(base + k_bytes + R_bytes + t_bytes);
+  float* poses = reinterpret_cast<float*>(base + k_bytes + R_bytes + t_bytes + sum_bytes);
+  int* n_valid = reinterpret_cast<int*>(base + k_bytes + R_bytes + t_bytes + sum_bytes + pose_bytes);
+  NOPE_CUDA(cudaMemcpyAsync(kd, K, k_bytes, cudaMemcpyHostToDevice, st));
+  const int ew_blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 16);
+  icp_init_kernel<<<ew_blocks, 256, 0, st>>>(R, t_init, F, P, Rc, tc, poses, sums, n_valid);
+  NOPE_CUDA(cudaGetLastError());
+  const long long hw = (long long)H * W;
+  const int px_blocks = (int)((hw + kIcpPixelsPerCta - 1) / kIcpPixelsPerCta);
+  icp_valid_kernel<<<dim3(px_blocks, 1, F), kIcpThreads, 0, st>>>(depth_sensor, masks, H, W, n_valid);
+  NOPE_CUDA(cudaGetLastError());
+  unsigned* z = reinterpret_cast<unsigned*>(depth);
+  const long long nz = (long long)n * hw;
+  const int fill_blocks = (int)std::min<long long>((nz + 255) / 256, 132LL * 16);
+  for (int it = 0; it <= iters; ++it) {
+    // the rasterizer of nope_render_depth, one launch per frame over its P poses (K differs per frame)
+    depth_fill_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);
+    NOPE_CUDA(cudaGetLastError());
+    for (int f = 0; f < F; ++f) {
+      const double* kf = K + 4 * (size_t)f;
+      depth_raster_kernel<<<dim3((NF + 7) / 8, P), 256, 0, st>>>(
+          vertices, V, faces, NF, poses + 16 * (size_t)f * P, (float)kf[0], (float)kf[1], (float)kf[2], (float)kf[3],
+          znear, H, W, z + (size_t)f * P * hw);
+      NOPE_CUDA(cudaGetLastError());
+    }
+    icp_accumulate_kernel<<<dim3(px_blocks, P, F), kIcpThreads, 0, st>>>(z, depth_sensor, masks, kd, tc, P, H, W,
+                                                                         tau[it], rho, sums);
+    NOPE_CUDA(cudaGetLastError());
+    if (it < iters) {
+      icp_solve_kernel<<<ew_blocks, 256, 0, st>>>(F, P, tau[it], rho, Rc, tc, poses, sums);
+      NOPE_CUDA(cudaGetLastError());
+    }
+  }
+  icp_final_kernel<<<ew_blocks, 256, 0, st>>>(Rc, tc, sums, n_valid, F, P, tau[iters], R_out, t_out, fit_out,
+                                              reinterpret_cast<long long*>(sums_out));
+  NOPE_CUDA(cudaGetLastError());
+  depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);      // depth holds render_depth at the returned pose
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }

@@ -469,11 +469,26 @@ class PoseConditional:
         k = nearest_idx.shape[1]
         return tp[torch.arange(B, device=dev)[:, None].expand(B, k), nearest_idx]
 
+    @staticmethod
+    def _read_sensor_depth(batch):
+        """The sensor depth of every frame of a T-LESS batch, its "depth_path" PNG / 10.0 (mm, 0 = no reading), as the
+        reference's vsd.py:72-74 reads it: -> float64 [B, H, W] on the host."""
+        import cv2
+        import numpy as np
+        depth = []
+        for path in batch["depth_path"]:
+            d = cv2.imread(path, -1)
+            if d is None:
+                raise FileNotFoundError(f"eval_vsd: cannot read depth image {path!r}")
+            depth.append(d / 10.0)
+        if any(d.shape != depth[0].shape or d.ndim != 2 for d in depth):
+            raise ValueError("eval_vsd: the depth images of a batch must share one (H, W) size")
+        return torch.from_numpy(np.stack(depth))
+
     def _render_frames(self, batch, B, ids, R, t_est=None):
         """The sensor depth of every frame and the model rendered at the ground-truth pose and at the rotations R
         [B, k, 3, 3] with the ground-truth translation, or with t_est [B, k, 3] when given: -> (depth_test [B, H, W]
         float64, rendered [B, 1 + k, H, W], K [B, 3, 3] float64 on the host, K4 [B, 4] on the device)."""
-        import numpy as np
         from . import vsd as _vsd
         dev = self.device
         k = R.shape[1]
@@ -486,18 +501,10 @@ class PoseConditional:
             poses[:, 1:, :3, 3] = t_est
         poses[:, :, 3, 3] = 1.0
         # vsd.py:72-74: the intrinsics and the sensor depth of every frame (PNG / 10.0), read on the host
-        import cv2
         K = batch["intrinsic"].detach().cpu().to(torch.float64).reshape(B, 3, 3)
-        depth = []
-        for path in batch["depth_path"]:
-            d = cv2.imread(path, -1)
-            if d is None:
-                raise FileNotFoundError(f"eval_vsd: cannot read depth image {path!r}")
-            depth.append(d / 10.0)
-        if any(d.shape != depth[0].shape or d.ndim != 2 for d in depth):
-            raise ValueError("eval_vsd: the depth images of a batch must share one (H, W) size")
-        H, W = depth[0].shape
-        depth_test = torch.from_numpy(np.stack(depth)).pin_memory().to(dev, non_blocking=True)
+        depth_test = self._read_sensor_depth(batch)
+        H, W = depth_test.shape[1:]
+        depth_test = depth_test.pin_memory().to(dev, non_blocking=True)
         K4 = torch.stack([K[:, 0, 0], K[:, 1, 1], K[:, 0, 2], K[:, 1, 2]], dim=1)
         K4 = K4.pin_memory().to(dev, non_blocking=True)
         rendered = torch.stack([_vsd.render_depth(self.tless_cad[ids[b]], poses[b], K[b], (H, W))
@@ -549,6 +556,62 @@ class PoseConditional:
             t[rd], iou[rd] = translation.estimate_translation(
                 self.tless_cad[obj], R[rr], K[ri], masks[rm], diameter=self.bop_models[obj]["diameter"], iters=iters)
         return t, iou
+
+    @torch.no_grad()
+    def refine_depth(self, batch, R, t, masks=None, iters=None, rerank=False):
+        """Refine every pose hypothesis (R [B, k, 3, 3], t [B, k, 3] mm, e.g. a search's rotations with
+        `estimate_translation`) of a T-LESS batch (the `eval_vsd` schema; its "intrinsic", "depth_path" and "obj_id"
+        are used) against each frame's sensor depth, read as `eval_vsd` reads it, by point-to-plane ICP
+        (`depth_refine.refine_pose_depth`, DESIGN.md section 19) with the mesh of load_mesh and the default tolerance
+        schedule of the object's diameter (load_models_info); masks [B, H, W] (uint8 or bool, nonzero = object) limit
+        the pairs to the object, None uses every pixel.  One call per distinct object.  -> (R float64 [B, k, 3, 3],
+        t float64 [B, k, 3], score float64 [B, k]) on the model's device, score = the share of the mask's sensor
+        pixels explained by the refined pose (NaN for a frame without readings); with rerank, each row's hypotheses
+        sorted by descending score (stable, NaN last).  The output feeds eval_bop(R_est=R, t_est=t)."""
+        import numpy as np
+        from . import depth_refine
+        iters = depth_refine.DEFAULT_ITERS if iters is None else iters
+        for key in ("intrinsic", "obj_id", "depth_path"):
+            if key not in batch:
+                raise KeyError(f"refine_depth: the batch has no {key!r}")
+        ids = [int(i) for i in batch["obj_id"].reshape(-1).tolist()]
+        B = len(ids)
+        R = torch.as_tensor(np.asarray(R) if not torch.is_tensor(R) else R)
+        if R.dim() != 4 or R.shape[0] != B or R.shape[2:] != (3, 3) or R.shape[1] < 1:
+            raise ValueError(f"refine_depth: R [B, k, 3, 3] with B = {B} expected, got {tuple(R.shape)}")
+        k = R.shape[1]
+        t = torch.as_tensor(np.asarray(t) if not torch.is_tensor(t) else t)
+        if tuple(t.shape) != (B, k, 3):
+            raise ValueError(f"refine_depth: t [{B}, {k}, 3] expected, got {tuple(t.shape)}")
+        if masks is not None:
+            masks = torch.as_tensor(np.asarray(masks) if not torch.is_tensor(masks) else masks)
+            if masks.dim() != 3 or masks.shape[0] != B:
+                raise ValueError(f"refine_depth: masks [B, H, W] with B = {B} expected, got {tuple(masks.shape)}")
+        if len(batch["depth_path"]) != B:
+            raise ValueError(f"refine_depth: {B} depth_path entries expected, got {len(batch['depth_path'])}")
+        missing = sorted(set(i for i in ids if i not in self.tless_cad or i not in self.bop_models))
+        if missing:
+            raise ValueError(f"refine_depth: no mesh or models_info entry for obj_id {missing} "
+                             "(load_mesh, load_models_info)")
+        K = batch["intrinsic"].detach().cpu().to(torch.float64).reshape(B, 3, 3)
+        depth = self._read_sensor_depth(batch)
+        dev = self.device
+        R_out = torch.empty((B, k, 3, 3), device=dev, dtype=torch.float64)
+        t_out = torch.empty((B, k, 3), device=dev, dtype=torch.float64)
+        score = torch.empty((B, k), device=dev, dtype=torch.float64)
+        for obj in sorted(set(ids)):
+            ri = torch.tensor([b for b in range(B) if ids[b] == obj], dtype=torch.int64)
+            rd = ri.pin_memory().to(dev, non_blocking=True)
+            pick = lambda x: None if x is None else x[rd if x.device.type == "cuda" else ri]   # noqa: E731
+            tau = depth_refine.default_tau(self.bop_models[obj]["diameter"], iters)
+            R_out[rd], t_out[rd], fit = depth_refine.refine_pose_depth(
+                self.tless_cad[obj], pick(R), pick(t), K[ri], depth[ri], masks=pick(masks), iters=iters, tau=tau)
+            score[rd] = fit["score"]
+        if rerank:
+            order = torch.sort(-score, dim=1, stable=True).indices                     # NaN sorts last
+            rows = torch.arange(B, device=dev)[:, None]
+            R_out, t_out, score = R_out[rows, order], t_out[rows, order], score[rows, order]
+        return R_out, t_out, score
 
     @torch.no_grad()
     def eval_bop(self, batch, data_name, R_est=None, save_path=None, t_est=None):

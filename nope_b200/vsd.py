@@ -157,6 +157,8 @@ class Mesh:
             raise ValueError(f"face index outside [0, {v.shape[0]})")
         self.vertices = v.to(device=device, dtype=torch.float32).contiguous()
         self.faces = fc64.to(torch.int32).to(device).contiguous()
+        v64 = v.detach().cpu().to(torch.float32).to(torch.float64)
+        self.radius = float(torch.sqrt((v64 * v64).sum(1)).max())    # the largest vertex norm (mm)
 
     @classmethod
     def from_ply(cls, path, device="cuda"):
