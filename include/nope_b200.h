@@ -295,6 +295,29 @@ int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF
                       double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
                       double* t_out, double* fit_out, int64_t* sums_out, void* stream);
 
+/* Pose refinement from the object mask's contour (DESIGN.md section 20).
+ * nope_mask_sdf: the signed distance field sdf_out [F, H, W] fp64 of masks [F, H, W] uint8 (nonzero = object), both
+ * on the device: sqrt(d2_out) - 1/2 off the object and 1/2 - sqrt(d2_in) on it, with d2_out (d2_in) the exact squared
+ * distance in px to the nearest object (background) pixel of the frame; NaN everywhere for a mask that is empty or
+ * covers the whole frame.  Requires 1 <= F <= 65535, 1 <= H, W <= 8192.
+ * nope_refine_contour: damped Gauss-Newton alignment of the rendered silhouette's contour with the mask, for P pose
+ * hypotheses per frame and F frames.  Mesh, R, t_init, K, rho, znear, iters, the workspace depth and sums_out as
+ * nope_refine_depth; masks [F, H, W] uint8 on the device; tau HOST [iters + 1] fp64 the pairing tolerances as
+ * fractions of the mask's box size sqrt(w h) (each finite and > 0).  Iteration i renders [R | t] rounded to fp32,
+ * pairs every interior contour pixel of the render (hit, a 4-neighbour not hit) whose residual phi + 1/2 lies within
+ * tau[i] sqrt(w h) px with the mask through its signed distance field phi, and applies one step of the six pose
+ * parameters (rotation about t).  A frame whose mask is empty or full keeps every pose.
+ * -> R_out [F, P, 9], t_out [F, P, 3] fp64 after `iters` steps; fit_out [F, P, 4] fp64 = (n_in, n_contour, rms, iou)
+ * at the returned pose: the pairs at tau[iters], the contour pixels of the render, the RMS residual in px (NaN when
+ * n_in = 0) and the silhouette IoU with the mask; rms and iou are NaN for a frame whose mask is empty or full.
+ * Refuses bad arguments before any CUDA call; all iterations are enqueued without synchronising the host.  The result
+ * does not depend on the batch or on scheduling. */
+int nope_mask_sdf(const uint8_t* masks, int F, int H, int W, double* sdf_out, void* stream);
+int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
+                        const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
+                        double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
+                        double* t_out, double* fit_out, int64_t* sums_out, void* stream);
+
 /* BOP 2019 errors (DESIGN.md section 15).
  * nope_vsd_error_taus: nope_vsd_error at T misalignment tolerances in one pass (the distance images, visibility
  * masks and counts are shared): taus HOST [T] fp64, each finite and > 0, 1 <= T <= 16; K HOST [F, 4] fp64, finite,

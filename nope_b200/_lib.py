@@ -60,6 +60,10 @@ SIGNATURES = {
                                     C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_void_p,
                                     C.c_int, C.c_float, c_f32p, C.c_void_p, C.c_void_p, C.c_void_p, c_i64p,
                                     C.c_void_p]),
+    "nope_mask_sdf": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "nope_refine_contour": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_int,
+                                      C.c_float, c_f32p, C.c_void_p, C.c_void_p, C.c_void_p, c_i64p, C.c_void_p]),
     "nope_pose_errors": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "nope_crop_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

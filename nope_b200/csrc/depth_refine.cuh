@@ -176,102 +176,128 @@ __device__ __forceinline__ double icp_unfix(unsigned long long s) {
   return __dmul_rn(__ll2double_rn((long long)s), 1.0 / kIcpFixedScale);
 }
 
+// hypothesis i: R, t = the inputs, the first pose, its sums reset
+__device__ __forceinline__ void icp_init_one(long long i, const double* __restrict__ R_in,
+                                             const double* __restrict__ t_in, double* __restrict__ R,
+                                             double* __restrict__ t, float* __restrict__ poses,
+                                             unsigned long long* __restrict__ sums) {
+#pragma unroll
+  for (int k = 0; k < 9; ++k) R[9 * i + k] = R_in[9 * i + k];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) t[3 * i + k] = t_in[3 * i + k];
+  icp_write_pose(R_in + 9 * i, t_in + 3 * i, poses + 16 * i);
+  for (int k = 0; k < kIcpSums; ++k) sums[kIcpSums * i + k] = 0ull;
+}
+
 // One thread per (f, p), n = F P: R, t = the inputs, the first pose, every sum and n_valid reset.
 __global__ void icp_init_kernel(const double* __restrict__ R_in, const double* __restrict__ t_in, int F, int P,
                                 double* __restrict__ R, double* __restrict__ t, float* __restrict__ poses,
                                 unsigned long long* __restrict__ sums, int* __restrict__ n_valid) {
   const long long n = (long long)F * P;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-#pragma unroll
-    for (int k = 0; k < 9; ++k) R[9 * i + k] = R_in[9 * i + k];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) t[3 * i + k] = t_in[3 * i + k];
-    icp_write_pose(R_in + 9 * i, t_in + 3 * i, poses + 16 * i);
-    for (int k = 0; k < kIcpSums; ++k) sums[kIcpSums * i + k] = 0ull;
+    icp_init_one(i, R_in, t_in, R, t, poses, sums);
     if (i < F) n_valid[i] = 0;
   }
 }
 
-// One update per (f, p), DESIGN.md section 19, every float64 operation rounded on its own.  With n_in >= 6: A = the
-// 21 J J^T sums, g = the 6 J e sums, M = A + mu I with mu = kIcpDamping max diag(A), M = L L^T by Cholesky (column by
-// column, every inner sum in ascending k), L y = -g forward and L^T delta = y backward (inner sums in ascending k);
-// omega = (delta_w tau) / rho, v = delta_v tau; R <- R_delta R with R_delta the rotation of the unit quaternion
-// (1, omega / 2) / sqrt(1 + |omega|^2 / 4), t <- t + v.  A non-positive pivot leaves the pose unchanged.  Writes the
-// next float32 pose and resets the sums for the next render.
+// One update of one hypothesis from its sums s [29], DESIGN.md section 19, every float64 operation rounded on its own.
+// With n_in >= 6: A = the 21 J J^T sums, g = the 6 J e sums, M = A + mu I with mu = kIcpDamping max diag(A), M = L L^T
+// by Cholesky (column by column, every inner sum in ascending k), L y = -g forward and L^T delta = y backward (inner
+// sums in ascending k); omega = (delta_w tau) / rho, v = delta_v tau; R <- R_delta R with R_delta the rotation of the
+// unit quaternion (1, omega / 2) / sqrt(1 + |omega|^2 / 4), t <- t + v.  Fewer pairs or a non-positive pivot leave the
+// pose unchanged.  tau is the hypothesis's metric tolerance (mm): the pairing tolerance of the depth fit, or the
+// contour fit's pixel tolerance scaled to the object's distance (contour_refine.cuh).
+__device__ __forceinline__ void icp_step(const unsigned long long* s, double tau, double rho, double* Ri, double* ti) {
+  if ((long long)s[kIcpSums - 1] >= 6) {
+    double M[6][6], g[6];
+    int q = 0;
+    for (int a = 0; a < 6; ++a)
+      for (int b = a; b < 6; ++b) { M[a][b] = icp_unfix(s[q++]); M[b][a] = M[a][b]; }
+    for (int a = 0; a < 6; ++a) g[a] = icp_unfix(s[kIcpJJ + a]);
+    double dmax = M[0][0];
+    for (int a = 1; a < 6; ++a) dmax = fmax(dmax, M[a][a]);
+    const double mu = __dmul_rn(kIcpDamping, dmax);
+    for (int a = 0; a < 6; ++a) M[a][a] = __dadd_rn(M[a][a], mu);
+    double L[6][6];
+    bool ok = true;
+    for (int j = 0; j < 6 && ok; ++j) {
+      double d = M[j][j];
+      for (int k = 0; k < j; ++k) d = __dsub_rn(d, __dmul_rn(L[j][k], L[j][k]));
+      if (!(d > 0.0)) { ok = false; break; }
+      L[j][j] = __dsqrt_rn(d);
+      for (int r = j + 1; r < 6; ++r) {
+        double x = M[r][j];
+        for (int k = 0; k < j; ++k) x = __dsub_rn(x, __dmul_rn(L[r][k], L[j][k]));
+        L[r][j] = __ddiv_rn(x, L[j][j]);
+      }
+    }
+    if (ok) {
+      double y[6], dl[6];
+      for (int r = 0; r < 6; ++r) {
+        double x = -g[r];
+        for (int k = 0; k < r; ++k) x = __dsub_rn(x, __dmul_rn(L[r][k], y[k]));
+        y[r] = __ddiv_rn(x, L[r][r]);
+      }
+      for (int r = 5; r >= 0; --r) {
+        double x = y[r];
+        for (int k = r + 1; k < 6; ++k) x = __dsub_rn(x, __dmul_rn(L[k][r], dl[k]));
+        dl[r] = __ddiv_rn(x, L[r][r]);
+      }
+      double h[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) h[k] = __dmul_rn(__ddiv_rn(__dmul_rn(dl[k], tau), rho), 0.5);   // omega / 2
+      const double sn = __dsqrt_rn(__dadd_rn(1.0, icp_dot(h, h)));
+      const double qw = __ddiv_rn(1.0, sn), qx = __ddiv_rn(h[0], sn), qy = __ddiv_rn(h[1], sn),
+                   qz = __ddiv_rn(h[2], sn);
+      const double xx = __dmul_rn(qx, qx), yy = __dmul_rn(qy, qy), zz = __dmul_rn(qz, qz);
+      const double xy = __dmul_rn(qx, qy), xz = __dmul_rn(qx, qz), yz = __dmul_rn(qy, qz);
+      const double wx = __dmul_rn(qw, qx), wy = __dmul_rn(qw, qy), wz = __dmul_rn(qw, qz);
+      const double Rd[9] = {
+          __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(yy, zz))), __dmul_rn(2.0, __dsub_rn(xy, wz)),
+          __dmul_rn(2.0, __dadd_rn(xz, wy)),
+          __dmul_rn(2.0, __dadd_rn(xy, wz)), __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(xx, zz))),
+          __dmul_rn(2.0, __dsub_rn(yz, wx)),
+          __dmul_rn(2.0, __dsub_rn(xz, wy)), __dmul_rn(2.0, __dadd_rn(yz, wx)),
+          __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(xx, yy)))};
+      double Rn[9];
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+          Rn[3 * r + c] = __dadd_rn(__dadd_rn(__dmul_rn(Rd[3 * r], Ri[c]), __dmul_rn(Rd[3 * r + 1], Ri[3 + c])),
+                                    __dmul_rn(Rd[3 * r + 2], Ri[6 + c]));
+      }
+#pragma unroll
+      for (int k = 0; k < 9; ++k) Ri[k] = Rn[k];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) ti[k] = __dadd_rn(ti[k], __dmul_rn(dl[3 + k], tau));
+    }
+  }
+}
+
+// One update per (f, p) at the pairing tolerance tau (icp_step); writes the next float32 pose and resets the sums for
+// the next render.
 __global__ void icp_solve_kernel(int F, int P, double tau, double rho, double* __restrict__ R, double* __restrict__ t,
                                  float* __restrict__ poses, unsigned long long* __restrict__ sums) {
   const long long n = (long long)F * P;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     unsigned long long* s = sums + kIcpSums * i;
-    double* Ri = R + 9 * i;
-    double* ti = t + 3 * i;
-    if ((long long)s[kIcpSums - 1] >= 6) {
-      double M[6][6], g[6];
-      int q = 0;
-      for (int a = 0; a < 6; ++a)
-        for (int b = a; b < 6; ++b) { M[a][b] = icp_unfix(s[q++]); M[b][a] = M[a][b]; }
-      for (int a = 0; a < 6; ++a) g[a] = icp_unfix(s[kIcpJJ + a]);
-      double dmax = M[0][0];
-      for (int a = 1; a < 6; ++a) dmax = fmax(dmax, M[a][a]);
-      const double mu = __dmul_rn(kIcpDamping, dmax);
-      for (int a = 0; a < 6; ++a) M[a][a] = __dadd_rn(M[a][a], mu);
-      double L[6][6];
-      bool ok = true;
-      for (int j = 0; j < 6 && ok; ++j) {
-        double d = M[j][j];
-        for (int k = 0; k < j; ++k) d = __dsub_rn(d, __dmul_rn(L[j][k], L[j][k]));
-        if (!(d > 0.0)) { ok = false; break; }
-        L[j][j] = __dsqrt_rn(d);
-        for (int r = j + 1; r < 6; ++r) {
-          double x = M[r][j];
-          for (int k = 0; k < j; ++k) x = __dsub_rn(x, __dmul_rn(L[r][k], L[j][k]));
-          L[r][j] = __ddiv_rn(x, L[j][j]);
-        }
-      }
-      if (ok) {
-        double y[6], dl[6];
-        for (int r = 0; r < 6; ++r) {
-          double x = -g[r];
-          for (int k = 0; k < r; ++k) x = __dsub_rn(x, __dmul_rn(L[r][k], y[k]));
-          y[r] = __ddiv_rn(x, L[r][r]);
-        }
-        for (int r = 5; r >= 0; --r) {
-          double x = y[r];
-          for (int k = r + 1; k < 6; ++k) x = __dsub_rn(x, __dmul_rn(L[k][r], dl[k]));
-          dl[r] = __ddiv_rn(x, L[r][r]);
-        }
-        double h[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) h[k] = __dmul_rn(__ddiv_rn(__dmul_rn(dl[k], tau), rho), 0.5);   // omega / 2
-        const double sn = __dsqrt_rn(__dadd_rn(1.0, icp_dot(h, h)));
-        const double qw = __ddiv_rn(1.0, sn), qx = __ddiv_rn(h[0], sn), qy = __ddiv_rn(h[1], sn),
-                     qz = __ddiv_rn(h[2], sn);
-        const double xx = __dmul_rn(qx, qx), yy = __dmul_rn(qy, qy), zz = __dmul_rn(qz, qz);
-        const double xy = __dmul_rn(qx, qy), xz = __dmul_rn(qx, qz), yz = __dmul_rn(qy, qz);
-        const double wx = __dmul_rn(qw, qx), wy = __dmul_rn(qw, qy), wz = __dmul_rn(qw, qz);
-        const double Rd[9] = {
-            __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(yy, zz))), __dmul_rn(2.0, __dsub_rn(xy, wz)),
-            __dmul_rn(2.0, __dadd_rn(xz, wy)),
-            __dmul_rn(2.0, __dadd_rn(xy, wz)), __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(xx, zz))),
-            __dmul_rn(2.0, __dsub_rn(yz, wx)),
-            __dmul_rn(2.0, __dsub_rn(xz, wy)), __dmul_rn(2.0, __dadd_rn(yz, wx)),
-            __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(xx, yy)))};
-        double Rn[9];
-#pragma unroll
-        for (int r = 0; r < 3; ++r) {
-#pragma unroll
-          for (int c = 0; c < 3; ++c)
-            Rn[3 * r + c] = __dadd_rn(__dadd_rn(__dmul_rn(Rd[3 * r], Ri[c]), __dmul_rn(Rd[3 * r + 1], Ri[3 + c])),
-                                      __dmul_rn(Rd[3 * r + 2], Ri[6 + c]));
-        }
-#pragma unroll
-        for (int k = 0; k < 9; ++k) Ri[k] = Rn[k];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) ti[k] = __dadd_rn(ti[k], __dmul_rn(dl[3 + k], tau));
-      }
-    }
-    icp_write_pose(Ri, ti, poses + 16 * i);
+    icp_step(s, tau, rho, R + 9 * i, t + 3 * i);
+    icp_write_pose(R + 9 * i, t + 3 * i, poses + 16 * i);
     for (int k = 0; k < kIcpSums; ++k) s[k] = 0ull;
+  }
+}
+
+// hypothesis i's pose into R_out [F, P, 9], t_out [F, P, 3] and its sums into sums_out [F, P, 29] (when not null)
+__device__ __forceinline__ void icp_out_one(long long i, const double* __restrict__ R, const double* __restrict__ t,
+                                            const unsigned long long* __restrict__ sums, double* __restrict__ R_out,
+                                            double* __restrict__ t_out, long long* __restrict__ sums_out) {
+#pragma unroll
+  for (int k = 0; k < 9; ++k) R_out[9 * i + k] = R[9 * i + k];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) t_out[3 * i + k] = t[3 * i + k];
+  if (sums_out) {
+    for (int k = 0; k < kIcpSums; ++k) sums_out[kIcpSums * i + k] = (long long)sums[kIcpSums * i + k];
   }
 }
 
@@ -285,18 +311,12 @@ __global__ void icp_final_kernel(const double* __restrict__ R, const double* __r
   const long long n = (long long)F * P;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const unsigned long long* s = sums + kIcpSums * i;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) R_out[9 * i + k] = R[9 * i + k];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) t_out[3 * i + k] = t[3 * i + k];
+    icp_out_one(i, R, t, sums, R_out, t_out, sums_out);
     const double nin = (double)(long long)s[kIcpSums - 1], nv = (double)n_valid[i / P];
     fit[4 * i] = nin;
     fit[4 * i + 1] = nv;
     fit[4 * i + 2] = __dmul_rn(tau, __dsqrt_rn(__ddiv_rn(icp_unfix(s[kIcpSums - 2]), nin)));
     fit[4 * i + 3] = __ddiv_rn(nin, nv);
-    if (sums_out) {
-      for (int k = 0; k < kIcpSums; ++k) sums_out[kIcpSums * i + k] = (long long)s[k];
-    }
   }
 }
 

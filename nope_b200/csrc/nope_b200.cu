@@ -32,6 +32,7 @@
 #include "crop.cuh"
 #include "translation.cuh"
 #include "depth_refine.cuh"
+#include "contour_refine.cuh"
 
 using namespace nope;
 
@@ -1729,6 +1730,112 @@ int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF
   }
   icp_final_kernel<<<ew_blocks, 256, 0, st>>>(Rc, tc, sums, n_valid, F, P, tau[iters], R_out, t_out, fit_out,
                                               reinterpret_cast<long long*>(sums_out));
+  NOPE_CUDA(cudaGetLastError());
+  depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);      // depth holds render_depth at the returned pose
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// pose refinement from the object mask's contour (contour_refine.cuh, DESIGN.md section 20)
+// ---------------------------------------------------------------------------------
+// phi [F, H, W] of masks [F, H, W] through the column pass into g [F, H, W] and the row pass
+static int launch_mask_sdf(const uint8_t* masks, int F, int H, int W, unsigned* g, double* phi, cudaStream_t st) {
+  mask_sdf_cols_kernel<<<dim3((W + kSdfColThreads - 1) / kSdfColThreads, F), kSdfColThreads, 0, st>>>(masks, H, W, g);
+  NOPE_CUDA(cudaGetLastError());
+  const int rows = mask_sdf_rows_per_cta(W);
+  mask_sdf_rows_kernel<<<dim3((H + rows - 1) / rows, F), rows, sizeof(unsigned) * rows * W, st>>>(g, H, W, phi);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int nope_mask_sdf(const uint8_t* masks, int F, int H, int W, double* sdf_out, void* stream) {
+  NOPE_CHECK(masks && sdf_out, "null argument");
+  NOPE_CHECK(F >= 1 && F <= 65535, "F must be in [1, 65535]");
+  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  StagedHost scratch;                                           // the column pass's distances, freed in stream order
+  scratch.st = st;
+  NOPE_CUDA(cudaMallocAsync(&scratch.dev, sizeof(unsigned) * (size_t)F * H * W, st));
+  return launch_mask_sdf(masks, F, H, W, static_cast<unsigned*>(scratch.dev), sdf_out, st);
+}
+
+int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
+                        const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
+                        double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
+                        double* t_out, double* fit_out, int64_t* sums_out, void* stream) {
+  NOPE_CHECK(vertices && faces && R && t_init && masks && K && tau && depth && R_out && t_out && fit_out,
+             "null argument");
+  NOPE_CHECK(V >= 1 && NF >= 1, "V and NF must be >= 1");
+  NOPE_CHECK(F >= 1 && F <= 65535 && P >= 1 && P <= 65535, "F and P must be in [1, 65535]");
+  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
+  NOPE_CHECK(iters >= 0 && iters <= 1024, "iters must be in [0, 1024]");
+  NOPE_CHECK(std::isfinite(rho) && rho > 0.0, "rho must be finite and > 0");
+  NOPE_CHECK(znear > 0.f && std::isfinite(znear), "znear must be finite and > 0");
+  for (int i = 0; i <= iters; ++i) NOPE_CHECK(std::isfinite(tau[i]) && tau[i] > 0.0, "tau must be finite and > 0");
+  if (check_host_intrinsics(K, F)) return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // one stream-ordered block: K, the current R and t, the integer sums, phi (8-byte fields first), then the float32
+  // poses, the column pass's distances, the mask and silhouette statistics and n_contour
+  const size_t n = (size_t)F * P, fhw = (size_t)F * H * W;
+  const size_t k_bytes = sizeof(double) * 4 * F, R_bytes = sizeof(double) * 9 * n, t_bytes = sizeof(double) * 3 * n;
+  const size_t sum_bytes = sizeof(unsigned long long) * kIcpSums * n, phi_bytes = sizeof(double) * fhw;
+  const size_t pose_bytes = sizeof(float) * 16 * n, g_bytes = sizeof(unsigned) * fhw;
+  const size_t stat_bytes = sizeof(int) * kFitStats * (n + F), nc_bytes = sizeof(int) * n;
+  StagedHost scratch;
+  scratch.st = st;
+  NOPE_CUDA(cudaMallocAsync(&scratch.dev, k_bytes + R_bytes + t_bytes + sum_bytes + phi_bytes + pose_bytes + g_bytes +
+                                              stat_bytes + nc_bytes, st));
+  char* p = static_cast<char*>(scratch.dev);
+  double* kd = reinterpret_cast<double*>(p);                      p += k_bytes;
+  double* Rc = reinterpret_cast<double*>(p);                      p += R_bytes;
+  double* tc = reinterpret_cast<double*>(p);                      p += t_bytes;
+  auto* sums = reinterpret_cast<unsigned long long*>(p);          p += sum_bytes;
+  double* phi = reinterpret_cast<double*>(p);                     p += phi_bytes;
+  float* poses = reinterpret_cast<float*>(p);                     p += pose_bytes;
+  unsigned* g = reinterpret_cast<unsigned*>(p);                   p += g_bytes;
+  int* sil_stats = reinterpret_cast<int*>(p);
+  int* mask_stats = sil_stats + kFitStats * n;
+  int* n_contour = mask_stats + kFitStats * F;
+  NOPE_CUDA(cudaMemcpyAsync(kd, K, k_bytes, cudaMemcpyHostToDevice, st));
+  const int ew_blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 16);
+  contour_init_kernel<<<ew_blocks, 256, 0, st>>>(R, t_init, F, P, Rc, tc, poses, sums, n_contour, sil_stats,
+                                                 mask_stats);
+  NOPE_CUDA(cudaGetLastError());
+  const long long hw = (long long)H * W;
+  const int px_blocks = (int)((hw + kIcpPixelsPerCta - 1) / kIcpPixelsPerCta);
+  const int stat_blocks = (int)((hw + kFitPixelsPerCta - 1) / kFitPixelsPerCta);
+  fit_stats_kernel<false><<<dim3(stat_blocks, 1, F), kFitThreads, 0, st>>>(nullptr, masks, P, H, W, mask_stats);
+  NOPE_CUDA(cudaGetLastError());
+  if (launch_mask_sdf(masks, F, H, W, g, phi, st)) return -1;
+  unsigned* z = reinterpret_cast<unsigned*>(depth);
+  const long long nz = (long long)n * hw;
+  const int fill_blocks = (int)std::min<long long>((nz + 255) / 256, 132LL * 16);
+  for (int it = 0; it <= iters; ++it) {
+    // the rasterizer of nope_render_depth, one launch per frame over its P poses (K differs per frame)
+    depth_fill_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);
+    NOPE_CUDA(cudaGetLastError());
+    for (int f = 0; f < F; ++f) {
+      const double* kf = K + 4 * (size_t)f;
+      depth_raster_kernel<<<dim3((NF + 7) / 8, P), 256, 0, st>>>(
+          vertices, V, faces, NF, poses + 16 * (size_t)f * P, (float)kf[0], (float)kf[1], (float)kf[2], (float)kf[3],
+          znear, H, W, z + (size_t)f * P * hw);
+      NOPE_CUDA(cudaGetLastError());
+    }
+    contour_accumulate_kernel<<<dim3(px_blocks, P, F), kIcpThreads, 0, st>>>(z, phi, kd, tc, mask_stats, P, H, W,
+                                                                             tau[it], rho, sums, n_contour);
+    NOPE_CUDA(cudaGetLastError());
+    if (it < iters) {
+      contour_solve_kernel<<<ew_blocks, 256, 0, st>>>(F, P, hw, tau[it], rho, mask_stats, kd, Rc, tc, poses, sums,
+                                                      n_contour);
+      NOPE_CUDA(cudaGetLastError());
+    }
+  }
+  fit_stats_kernel<true><<<dim3(stat_blocks, P, F), kFitThreads, 0, st>>>(z, masks, P, H, W, sil_stats);
+  NOPE_CUDA(cudaGetLastError());
+  contour_final_kernel<<<ew_blocks, 256, 0, st>>>(Rc, tc, sums, n_contour, mask_stats, sil_stats, F, P, hw,
+                                                  tau[iters], R_out, t_out, fit_out,
+                                                  reinterpret_cast<long long*>(sums_out));
   NOPE_CUDA(cudaGetLastError());
   depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);      // depth holds render_depth at the returned pose
   NOPE_CUDA(cudaGetLastError());

@@ -614,6 +614,56 @@ class PoseConditional:
         return R_out, t_out, score
 
     @torch.no_grad()
+    def refine_contour(self, batch, R, t, masks, iters=None, rerank=False):
+        """Refine every pose hypothesis (R [B, k, 3, 3], t [B, k, 3] mm, e.g. a search's rotations with
+        `estimate_translation`) of a T-LESS batch (the `eval_vsd` schema; its "intrinsic" and "obj_id" are used)
+        against each frame's object mask masks [B, H, W] (uint8 or bool, nonzero = object; (H, W) the frame size) by
+        aligning the rendered silhouette's contour with the mask's (`contour_refine.refine_pose_contour`, DESIGN.md
+        section 20), with the mesh of load_mesh and the default tolerance schedule.  No depth image is read.  One call
+        per distinct object.  -> (R float64 [B, k, 3, 3], t float64 [B, k, 3], iou float64 [B, k]) on the model's
+        device, iou = the refined pose's silhouette IoU with the mask (NaN for a frame whose mask is empty or full);
+        with rerank, each row's hypotheses sorted by descending IoU (stable, NaN last).  The output feeds
+        eval_bop(R_est=R, t_est=t); refine_depth can follow when the frame has depth."""
+        import numpy as np
+        from . import contour_refine
+        iters = contour_refine.DEFAULT_ITERS if iters is None else iters
+        for key in ("intrinsic", "obj_id"):
+            if key not in batch:
+                raise KeyError(f"refine_contour: the batch has no {key!r}")
+        ids = [int(i) for i in batch["obj_id"].reshape(-1).tolist()]
+        B = len(ids)
+        R = torch.as_tensor(np.asarray(R) if not torch.is_tensor(R) else R)
+        if R.dim() != 4 or R.shape[0] != B or R.shape[2:] != (3, 3) or R.shape[1] < 1:
+            raise ValueError(f"refine_contour: R [B, k, 3, 3] with B = {B} expected, got {tuple(R.shape)}")
+        k = R.shape[1]
+        t = torch.as_tensor(np.asarray(t) if not torch.is_tensor(t) else t)
+        if tuple(t.shape) != (B, k, 3):
+            raise ValueError(f"refine_contour: t [{B}, {k}, 3] expected, got {tuple(t.shape)}")
+        masks = torch.as_tensor(np.asarray(masks) if not torch.is_tensor(masks) else masks)
+        if masks.dim() != 3 or masks.shape[0] != B:
+            raise ValueError(f"refine_contour: masks [B, H, W] with B = {B} expected, got {tuple(masks.shape)}")
+        missing = sorted(set(i for i in ids if i not in self.tless_cad))
+        if missing:
+            raise ValueError(f"refine_contour: no mesh for obj_id {missing} (load_mesh)")
+        K = batch["intrinsic"].detach().cpu().to(torch.float64).reshape(B, 3, 3)
+        dev = self.device
+        R_out = torch.empty((B, k, 3, 3), device=dev, dtype=torch.float64)
+        t_out = torch.empty((B, k, 3), device=dev, dtype=torch.float64)
+        iou = torch.empty((B, k), device=dev, dtype=torch.float64)
+        for obj in sorted(set(ids)):
+            ri = torch.tensor([b for b in range(B) if ids[b] == obj], dtype=torch.int64)
+            rd = ri.pin_memory().to(dev, non_blocking=True)
+            pick = lambda x: x[rd if x.device.type == "cuda" else ri]   # noqa: E731
+            R_out[rd], t_out[rd], fit = contour_refine.refine_pose_contour(
+                self.tless_cad[obj], pick(R), pick(t), K[ri], pick(masks), iters=iters)
+            iou[rd] = fit["iou"]
+        if rerank:
+            order = torch.sort(-iou, dim=1, stable=True).indices                     # NaN sorts last
+            rows = torch.arange(B, device=dev)[:, None]
+            R_out, t_out, iou = R_out[rows, order], t_out[rows, order], iou[rows, order]
+        return R_out, t_out, iou
+
+    @torch.no_grad()
     def eval_bop(self, batch, data_name, R_est=None, save_path=None, t_est=None):
         """BOP 2019 average recall of a T-LESS batch (the `eval_vsd` schema): the grid retrieval's top-5 rotations, or
         R_est [B, k, 3, 3] from any search, at the ground-truth translation, or at t_est [B, k, 3] (mm, e.g. from
