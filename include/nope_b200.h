@@ -161,6 +161,14 @@ int nope_encoder_finalize(nope_encoder_t* e);
  * Any B >= 1: the engine walks the batch 32 images at a time (workspace ~80 MB per image of a chunk). */
 int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* out, void* stream);
 int64_t nope_encoder_last_launch_count(const nope_encoder_t* e);
+/* Debug / parity: run ONE module of the encoder in isolation, the launches encode makes for it.
+ *   name "stem" (x = images [n, 3, 256, 256]), "backbone.layer<l>.<b>" (a bottleneck) or "projector";
+ *   x [n, C, H, H] fp32 NCHW (device), C and H the module's input shape, 1 <= n <= 32 -> out fp32 NCHW (device):
+ *   hi + lo of the module's (hi, lo) output, the projector's fp32 output [n, D, 32, 32].  An unknown name, a C or H
+ *   that does not fit it, n out of range or an out_capacity_floats below the output's size fail.
+ * Synchronises the stream. */
+int nope_encoder_run_block(nope_encoder_t* e, const char* name, const float* x, int C, int H, int n, float* out,
+                           int64_t out_capacity_floats, void* stream);
 
 /* In-plane rotation search (DESIGN.md section 11).  cossin [A, 2] fp32 holds (cos, sin) of the angles
  * alpha_a = a * 360 / A.  Rotated copy a of an image is I_a(x, y) = I(c + R2(alpha_a) ((x, y) - c)) in pixel-index
@@ -214,6 +222,15 @@ int nope_vae_encode_inplane(nope_vae_t* v, const float* images, int B, const flo
 int nope_vae_encode_rotated(nope_vae_t* v, const float* images, int B, const int32_t* image_idx, const float* cossin,
                             int P, float* out, void* stream);
 int64_t nope_vae_last_launch_count(const nope_vae_t* v);
+/* Debug / parity: run ONE module of the encoder in isolation, through the member functions encode calls.
+ *   name "encoder.conv_in" (x = images [n, 3, 256, 256]), "encoder.down_blocks.<i>.resnets.<j>",
+ *   "encoder.down_blocks.<i>.downsamplers.0", "encoder.mid_block.resnets.<j>", "encoder.mid_block.attentions.0" or
+ *   "encoder.conv_out" (conv_norm_out + SiLU + conv_out + quant_conv mean x 0.18215 -> [n, 4, 32, 32]);
+ *   x [n, C, H, H] fp32 NCHW (device), the module's input shape, 1 <= n <= 16 -> out: the fp32 residual stream after
+ *   the module, out_pair (nullable; not for conv_out): hi + lo of its (hi, lo) copy, both fp32 NCHW (device).
+ * Synchronises the stream. */
+int nope_vae_run_block(nope_vae_t* v, const char* name, const float* x, int C, int H, int n, float* out,
+                       float* out_pair, int64_t out_capacity_floats, void* stream);
 
 /* Stable Diffusion VAE decoder (DESIGN.md section 17): AutoencoderKL.decode(z / 0.18215).sample of the SD v1
  * configuration (post_quant_conv 1x1; conv_in 3x3 4 -> 512; mid block as the encoder's; four UpDecoderBlock2D of three
@@ -232,6 +249,12 @@ int nope_vae_decoder_load_tensor(nope_vae_decoder_t* d, const char* key, const f
 int nope_vae_decoder_finalize(nope_vae_decoder_t* d);
 int nope_vae_decoder_decode(nope_vae_decoder_t* d, const float* latents, int B, float* out, void* stream);
 int64_t nope_vae_decoder_last_launch_count(const nope_vae_decoder_t* d);
+/* Debug / parity: as nope_vae_run_block, for the modules of decode: "decoder.conv_in" (post_quant_conv with
+ * 1 / 0.18215, then conv_in; x = latents [n, 4, 32, 32]), "decoder.mid_block.resnets.<j>",
+ * "decoder.mid_block.attentions.0", "decoder.up_blocks.<i>.resnets.<j>", "decoder.up_blocks.<i>.upsamplers.0" and
+ * "decoder.conv_out" (conv_norm_out + SiLU + conv_out -> [n, 3, 256, 256]); 1 <= n <= 8. */
+int nope_vae_decoder_run_block(nope_vae_decoder_t* d, const char* name, const float* x, int C, int H, int n,
+                               float* out, float* out_pair, int64_t out_capacity_floats, void* stream);
 
 /* T-LESS evaluation (DESIGN.md section 12): a depth rasterizer standing in for pyrender's DEPTH_ONLY render and the
  * VSD error of src/poses/vsd.py:92-135 (visibility mode "bop19", src/poses/vsd_utils.py).  Both calls refuse bad

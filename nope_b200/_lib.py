@@ -47,6 +47,12 @@ SIGNATURES = {
     "nope_vae_last_launch_count": (C.c_int64, [C.c_void_p]),
     "nope_vae_decoder_decode": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_void_p]),
     "nope_vae_decoder_last_launch_count": (C.c_int64, [C.c_void_p]),
+    "nope_encoder_run_block": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p,
+                                         C.c_int64, C.c_void_p]),
+    "nope_vae_run_block": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p,
+                                     C.c_int64, C.c_void_p]),
+    "nope_vae_decoder_run_block": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p,
+                                             c_f32p, C.c_int64, C.c_void_p]),
     "nope_render_depth":(C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_int, C.c_float, C.c_float,
                                     C.c_float, C.c_float, C.c_float, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     "nope_vsd_error": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,

@@ -375,44 +375,42 @@ struct nope_encoder {
     return launch_conv_tc2(p, L.bn, num_sms, st);
   }
 
-  int encode(const float* images, int B, float* out, cudaStream_t st) {
+  // stem: images [B, 3, 256, 256] -> buf[0] (128 x 128 x 64)
+  int stem(const float* images, int B, cudaStream_t st) {
+    const long long npix = (long long)B * 128 * 128;
+    nope::enc_stem_kernel<<<(unsigned)((npix + 3) / 4), 256, 0, st>>>(images, stem_w, stem_b, buf[0].hi, buf[0].lo,
+                                                                      B, 256, 256);
+    NOPE_CUDA(cudaGetLastError());
+    ++launches;
+    return 0;
+  }
+
+  // bottleneck p (conv2 / downsample stride stv) on buf[cur] of side H -> buf[cur] (the new cur), side H / stv
+  int bottleneck(const std::string& p, int stv, int H, int B, int& cur, cudaStream_t st) {
     using namespace nope;
-    if (ensure_workspace(B)) return -1;
-    launches = 0;
-    int H = 128;
-    {
-      const long long npix = (long long)B * H * H;
-      enc_stem_kernel<<<(unsigned)((npix + 3) / 4), 256, 0, st>>>(images, stem_w, stem_b, buf[0].hi, buf[0].lo,
-                                                                  B, 256, 256);
-      NOPE_CUDA(cudaGetLastError());
-      ++launches;
+    // free buffers: the four that are not `cur`
+    int f[4], nf = 0;
+    for (int i = 0; i < 5; ++i)
+      if (i != cur) f[nf++] = i;
+    const ActPair &x = buf[cur], &a = buf[f[0]], &bb = buf[f[1]], &r = buf[f[2]], &o = buf[f[3]];
+    if (conv(convs.at(p + ".conv1"), x, H, a, B, true, nullptr, nullptr, st)) return -1;
+    if (conv(convs.at(p + ".conv2"), a, H, bb, B, true, nullptr, nullptr, st)) return -1;
+    const int Ho = H / stv;
+    const ActPair* res = &x;
+    auto it = convs.find(p + ".down");
+    if (it != convs.end()) {
+      if (conv(it->second, x, H, r, B, false, nullptr, nullptr, st)) return -1;
+      res = &r;
     }
-    int cur = 0;   // buf[cur] holds the block input
-    const int blocks[4] = {3, 4, 6, 3}, strides[4] = {1, 2, 2, 1};
-    for (int li = 0; li < 4; ++li)
-      for (int b = 0; b < blocks[li]; ++b) {
-        const std::string p = "backbone.layer" + std::to_string(li + 1) + "." + std::to_string(b);
-        const int stv = b == 0 ? strides[li] : 1;
-        // free buffers: the four that are not `cur`
-        int f[4], nf = 0;
-        for (int i = 0; i < 5; ++i)
-          if (i != cur) f[nf++] = i;
-        const ActPair &x = buf[cur], &a = buf[f[0]], &bb = buf[f[1]], &r = buf[f[2]], &o = buf[f[3]];
-        if (conv(convs.at(p + ".conv1"), x, H, a, B, true, nullptr, nullptr, st)) return -1;
-        if (conv(convs.at(p + ".conv2"), a, H, bb, B, true, nullptr, nullptr, st)) return -1;
-        const int Ho = H / stv;
-        const ActPair* res = &x;
-        auto it = convs.find(p + ".down");
-        if (it != convs.end()) {
-          if (conv(it->second, x, H, r, B, false, nullptr, nullptr, st)) return -1;
-          res = &r;
-        }
-        if (conv(convs.at(p + ".conv3"), bb, Ho, o, B, true, res, nullptr, st)) return -1;
-        cur = f[3];
-        H = Ho;
-      }
-    // projector (template.py:34-39): ReLU (idempotent on the post-ReLU backbone output) ->
-    // 1x1 2048->256 -> ReLU -> 1x1 256->D (no bias, no BN)
+    if (conv(convs.at(p + ".conv3"), bb, Ho, o, B, true, res, nullptr, st)) return -1;
+    cur = f[3];
+    return 0;
+  }
+
+  // projector (template.py:34-39) on buf[cur] of side H: ReLU (idempotent on the post-ReLU backbone output) ->
+  // 1x1 2048->256 -> ReLU -> 1x1 256->D (no bias, no BN) -> out [B, D, H, H] fp32 NCHW
+  int projector(int cur, int H, int B, float* out, cudaStream_t st) {
+    using namespace nope;
     const int nxt = (cur + 1) % 5;
     if (conv(convs.at("projector.1"), buf[cur], H, buf[nxt], B, true, nullptr, nullptr, st)) return -1;
     const int nx2 = (cur + 2) % 5;
@@ -422,6 +420,80 @@ struct nope_encoder {
     NOPE_CUDA(cudaGetLastError());
     ++launches;
     return 0;
+  }
+
+  static constexpr int kBlocks[4] = {3, 4, 6, 3}, kStrides[4] = {1, 2, 2, 1};
+  static std::string block_name(int li, int b) {
+    return "backbone.layer" + std::to_string(li + 1) + "." + std::to_string(b);
+  }
+
+  int encode(const float* images, int B, float* out, cudaStream_t st) {
+    if (ensure_workspace(B)) return -1;
+    launches = 0;
+    if (stem(images, B, st)) return -1;
+    int H = 128, cur = 0;   // buf[cur] holds the block input
+    for (int li = 0; li < 4; ++li)
+      for (int b = 0; b < kBlocks[li]; ++b) {
+        const int stv = b == 0 ? kStrides[li] : 1;
+        if (bottleneck(block_name(li, b), stv, H, B, cur, st)) return -1;
+        H /= stv;
+      }
+    return projector(cur, H, B, out, st);
+  }
+
+  // Runs one module on its own (nope_encoder_run_block): "stem" on images [n, 3, 256, 256], a bottleneck
+  // "backbone.layer<l>.<b>" or "projector" on x [n, C, H, H] fp32 NCHW, staged as (hi, lo) into the block's input
+  // buffer -> out fp32 NCHW: hi + lo of the block's output pair, the projector's fp32 output.  *Co, *Ho: its shape.
+  int run_block(const std::string& name, const float* x, int C, int H, int n, float* out, int64_t cap_floats,
+                cudaStream_t st) {
+    using namespace nope;
+    NOPE_CHECK(n >= 1 && n <= kChunk, "run_block: n must be in [1, " + std::to_string(kChunk) + "]");
+    int Ci = 0, Hi = 0, Co = 0, Ho = 0, stv = 1;
+    if (name == "stem") {
+      Ci = 3, Hi = 256, Co = 64, Ho = 128;
+    } else if (name == "projector") {
+      Ci = 2048, Hi = 32, Co = D, Ho = 32;
+    } else {
+      int h = 128;
+      for (int li = 0; li < 4 && !Ci; ++li)
+        for (int b = 0; b < kBlocks[li]; ++b) {
+          const int s = b == 0 ? kStrides[li] : 1;
+          if (name == block_name(li, b)) {
+            Ci = convs.at(name + ".conv1").cin, Hi = h, Co = convs.at(name + ".conv3").cout, Ho = h / s, stv = s;
+            break;
+          }
+          h /= s;
+        }
+      NOPE_CHECK(Ci, "run_block: unknown encoder module " + name);
+    }
+    NOPE_CHECK(C == Ci && H == Hi, "run_block: " + name + " takes [n, " + std::to_string(Ci) + ", " +
+                                       std::to_string(Hi) + ", " + std::to_string(Hi) + "] inputs, got C = " +
+                                       std::to_string(C) + ", H = " + std::to_string(H));
+    NOPE_CHECK(cap_floats >= (int64_t)n * Co * Ho * Ho, "run_block: output buffer too small");
+    if (ensure_workspace(n)) return -1;
+    launches = 0;
+    if (name == "stem") {
+      if (stem(x, n, st)) return -1;
+      to_nchw_pair(buf[0], out, n, Co, Ho, st);
+    } else {
+      nchw_f32_to_nhwc_f16_kernel<<<ew_grid((long long)n * C * H * H), 256, 0, st>>>(x, buf[0].hi, n, C, H * H,
+                                                                                     buf[0].lo);
+      NOPE_CUDA(cudaGetLastError());
+      int cur = 0;
+      if (name == "projector") {
+        if (projector(cur, H, n, out, st)) return -1;
+      } else {
+        if (bottleneck(name, stv, H, n, cur, st)) return -1;
+        to_nchw_pair(buf[cur], out, n, Co, Ho, st);
+      }
+    }
+    NOPE_CUDA(cudaGetLastError());
+    NOPE_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  }
+  static void to_nchw_pair(const nope::ActPair& a, float* out, int n, int C, int H, cudaStream_t st) {
+    nope::nhwc_f16_to_nchw_f32_kernel<<<nope::ew_grid((long long)n * C * H * H), 256, 0, st>>>(a.hi, out, n, C, H * H,
+                                                                                               a.lo);
   }
 
   // images [B, 3, 256, 256] x angles cossin [A, 2] -> out [B, A, D, 32, 32]: the (image, angle) pairs in b-major

@@ -1227,10 +1227,18 @@ topk_merge_kernel(const float* __restrict__ gathered, int world, long long pack,
   }
 }
 
-// fp32 NCHW <-> fp16 NHWC helpers for the per-op test entry points
+// fp32 NCHW <-> fp16 NHWC helpers for the per-op test entry points.  NHWC element (b, p, c) of image b's pixel p:
+// plain [n_img, hw, C], or, with plane_cap > 0, the parity-planar layout of a 256 x 256 level (vae.cuh): plane
+// (py, px) of a [4][plane_cap][128][128][C] tensor holds the pixels (2 Y + py, 2 X + px).
+__device__ __forceinline__ long long nhwc_index(int b, int p, int c, int C, int hw, int plane_cap) {
+  if (!plane_cap) return ((long long)b * hw + p) * C + c;
+  const int y = p >> 8, x = p & 255, q = (y & 1) * 2 + (x & 1);
+  return ((((long long)q * plane_cap + b) * 128 + (y >> 1)) * 128 + (x >> 1)) * C + c;
+}
+// y32 (optional) receives the fp32 values in the same NHWC layout
 __global__ void nchw_f32_to_nhwc_f16_kernel(const float* __restrict__ x, __half* __restrict__ y,
                                             int n_img, int C, int hw, __half* __restrict__ y_lo = nullptr,
-                                            bool bf = false) {
+                                            bool bf = false, float* __restrict__ y32 = nullptr, int plane_cap = 0) {
   const long long total = (long long)n_img * C * hw;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
@@ -1238,23 +1246,27 @@ __global__ void nchw_f32_to_nhwc_f16_kernel(const float* __restrict__ x, __half*
     const int p = (int)((i / C) % hw);
     const int b = (int)(i / ((long long)C * hw));
     const float v = x[((long long)b * C + c) * hw + p];
-    if (bf) { st16(y + i, v, true); continue; }
+    const long long j = plane_cap ? nhwc_index(b, p, c, C, hw, plane_cap) : i;
+    if (bf) { st16(y + j, v, true); continue; }
     const __half hi = __float2half_rn(v);
-    y[i] = hi;
-    if (y_lo) y_lo[i] = __float2half_rn(v - __half2float(hi));
+    y[j] = hi;
+    if (y_lo) y_lo[j] = __float2half_rn(v - __half2float(hi));
+    if (y32) y32[j] = v;
   }
 }
+// x32 (optional) is read instead of the fp16 pair
 __global__ void nhwc_f16_to_nchw_f32_kernel(const __half* __restrict__ x, float* __restrict__ y,
                                             int n_img, int C, int hw,
-                                            const __half* __restrict__ x_lo = nullptr, bool bf = false) {
+                                            const __half* __restrict__ x_lo = nullptr, bool bf = false,
+                                            const float* __restrict__ x32 = nullptr, int plane_cap = 0) {
   const long long total = (long long)n_img * C * hw;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const int p = (int)(i % hw);
     const int c = (int)((i / hw) % C);
     const int b = (int)(i / ((long long)C * hw));
-    const long long j = ((long long)b * hw + p) * C + c;
-    y[i] = ld16(x + j, bf) + (x_lo ? __half2float(x_lo[j]) : 0.f);
+    const long long j = nhwc_index(b, p, c, C, hw, plane_cap);
+    y[i] = x32 ? x32[j] : ld16(x + j, bf) + (x_lo ? __half2float(x_lo[j]) : 0.f);
   }
 }
 

@@ -1393,6 +1393,14 @@ int nope_encoder_encode_rotated(nope_encoder_t* e, const float* images, int B, c
 
 int64_t nope_encoder_last_launch_count(const nope_encoder_t* e) { return e ? e->launches : 0; }
 
+int nope_encoder_run_block(nope_encoder_t* e, const char* name, const float* x, int C, int H, int n, float* out,
+                           int64_t out_capacity_floats, void* stream) {
+  NOPE_CHECK(e && e->finalized, "encoder not finalized");
+  NOPE_CHECK(name && x && out, "null name / x / out pointer");
+  NOPE_CUDA(cudaSetDevice(e->device));
+  return e->run_block(name, x, C, H, n, out, out_capacity_floats, static_cast<cudaStream_t>(stream));
+}
+
 // ---------------------------------------------------------------------------------
 // Stable Diffusion VAE encoder (vae.cuh, DESIGN.md section 16)
 // ---------------------------------------------------------------------------------
@@ -1444,6 +1452,14 @@ int nope_vae_encode_rotated(nope_vae_t* v, const float* images, int B, const int
 
 int64_t nope_vae_last_launch_count(const nope_vae_t* v) { return v ? v->launches : 0; }
 
+int nope_vae_run_block(nope_vae_t* v, const char* name, const float* x, int C, int H, int n, float* out,
+                       float* out_pair, int64_t out_capacity_floats, void* stream) {
+  NOPE_CHECK(v && v->finalized, "VAE not finalized");
+  NOPE_CHECK(name && x && out, "null name / x / out pointer");
+  NOPE_CUDA(cudaSetDevice(v->device));
+  return v->run_block(name, x, C, H, n, out, out_pair, out_capacity_floats, static_cast<cudaStream_t>(stream));
+}
+
 // ---------------------------------------------------------------------------------
 // Stable Diffusion VAE decoder (vae.cuh, DESIGN.md section 17)
 // ---------------------------------------------------------------------------------
@@ -1475,6 +1491,14 @@ int nope_vae_decoder_decode(nope_vae_decoder_t* d, const float* latents, int B, 
 }
 
 int64_t nope_vae_decoder_last_launch_count(const nope_vae_decoder_t* d) { return d ? d->launches : 0; }
+
+int nope_vae_decoder_run_block(nope_vae_decoder_t* d, const char* name, const float* x, int C, int H, int n,
+                               float* out, float* out_pair, int64_t out_capacity_floats, void* stream) {
+  NOPE_CHECK(d && d->finalized, "VAE decoder not finalized");
+  NOPE_CHECK(name && x && out, "null name / x / out pointer");
+  NOPE_CUDA(cudaSetDevice(d->device));
+  return d->run_block(name, x, C, H, n, out, out_pair, out_capacity_floats, static_cast<cudaStream_t>(stream));
+}
 
 // ---------------------------------------------------------------------------------
 // T-LESS evaluation: depth rasterizer and VSD (render.cuh, DESIGN.md section 12)

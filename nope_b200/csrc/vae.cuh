@@ -668,6 +668,37 @@ struct VaeEngine {
     cur = nxt;
     return 0;
   }
+
+  // ---------------------------------------------------------------- one module on its own (run_block)
+  // x [n, C, H, H] fp32 NCHW -> residual stream 0: x32[0] and xs[0] (parity-planar at 256)
+  int stage_stream(const float* x, int C, int H, int n, cudaStream_t st) {
+    nchw_f32_to_nhwc_f16_kernel<<<ew_grid((long long)n * C * H * H), 256, 0, st>>>(
+        x, xs[0].hi, n, C, H * H, xs[0].lo, false, x32[0], H == 256 ? cap : 0);
+    NOPE_CUDA(cudaGetLastError());
+    return 0;
+  }
+  // residual stream `cur` -> out (fp32 stream) and out_pair (hi + lo, if given), [n, C, H, H] fp32 NCHW
+  int extract_stream(int cur, int C, int H, int n, float* out, float* out_pair, cudaStream_t st) {
+    const int pc = H == 256 ? cap : 0;
+    const int g = ew_grid((long long)n * C * H * H);
+    nhwc_f16_to_nchw_f32_kernel<<<g, 256, 0, st>>>(nullptr, out, n, C, H * H, nullptr, false, x32[cur], pc);
+    if (out_pair)
+      nhwc_f16_to_nchw_f32_kernel<<<g, 256, 0, st>>>(xs[cur].hi, out_pair, n, C, H * H, xs[cur].lo, false, nullptr,
+                                                     pc);
+    NOPE_CUDA(cudaGetLastError());
+    return 0;
+  }
+  // the checks every run_block makes once the module's input shape (Ci, Hi) and output shape (Co, Ho) are known
+  int check_block(const std::string& name, int chunk, int C, int H, int n, int Ci, int Hi, int Co, int Ho,
+                  int64_t cap_floats) {
+    NOPE_CHECK(Ci, "run_block: unknown module " + name);
+    NOPE_CHECK(n >= 1 && n <= chunk, "run_block: n must be in [1, " + std::to_string(chunk) + "]");
+    NOPE_CHECK(C == Ci && H == Hi, "run_block: " + name + " takes [n, " + std::to_string(Ci) + ", " +
+                                       std::to_string(Hi) + ", " + std::to_string(Hi) + "] inputs, got C = " +
+                                       std::to_string(C) + ", H = " + std::to_string(H));
+    NOPE_CHECK(cap_floats >= (int64_t)n * Co * Ho * Ho, "run_block: output buffer too small");
+    return 0;
+  }
 };
 
 }  // namespace nope
@@ -789,6 +820,62 @@ struct nope_vae : nope::VaeEngine {
     enc_extract_kernel<<<ew_grid((long long)n * 4 * 1024), 256, 0, st>>>(t32, out, n, 4, 1024, co.cout);
     NOPE_CUDA(cudaGetLastError());
     ++launches;
+    return 0;
+  }
+
+  // Runs one module of encode() on its own (nope_vae_run_block): x [n, C, H, H] fp32 NCHW (images for conv_in)
+  // staged as the residual stream -> out: the fp32 stream after the module, out_pair (nullable): its (hi, lo) pair
+  // as hi + lo.  "encoder.conv_out" is conv_norm_out + SiLU + conv_out + quant_conv's mean x 0.18215 and has no pair.
+  int run_block(const std::string& name, const float* x, int C, int H, int n, float* out, float* out_pair,
+                int64_t cap_floats, cudaStream_t st) {
+    using namespace nope;
+    enum { kResnet, kDown, kAttention, kIn, kOut } kind = kResnet;
+    int Ci = 0, Hi = 0, Co = 0, Ho = 0;
+    if (name == "encoder.conv_in") {
+      kind = kIn, Ci = 3, Hi = 256, Co = 128, Ho = 256;
+    } else if (name == "encoder.conv_out") {
+      kind = kOut, Ci = 512, Hi = 32, Co = 4, Ho = 32;
+    } else if (name == "encoder.mid_block.attentions.0") {
+      kind = kAttention, Ci = Co = 512, Hi = Ho = 32;
+    } else if (name == "encoder.mid_block.resnets.0" || name == "encoder.mid_block.resnets.1") {
+      Ci = Co = 512, Hi = Ho = 32;
+    } else {
+      int cin = 128;
+      for (int i = 0; i < 4; ++i) {
+        const std::string blk = "encoder.down_blocks." + std::to_string(i);
+        for (int j = 0; j < 2; ++j) {
+          if (name == blk + ".resnets." + std::to_string(j)) Ci = cin, Co = kCh[i], Hi = Ho = 256 >> i;
+          cin = kCh[i];
+        }
+        if (i < 3 && name == blk + ".downsamplers.0") kind = kDown, Ci = Co = kCh[i], Hi = 256 >> i, Ho = Hi / 2;
+      }
+    }
+    if (check_block(name, kChunk, C, H, n, Ci, Hi, Co, Ho, cap_floats)) return -1;
+    NOPE_CHECK(!out_pair || kind != kOut, "run_block: encoder.conv_out has no (hi, lo) output");
+    launches = 0;
+    int cur = 0;
+    if (kind == kIn) {
+      vae_conv_in_kernel<<<n * 65536 / 2, 256, 0, st>>>(x, in_w, in_b, x32[0], xs[0].hi, xs[0].lo, n, kChunk);
+      NOPE_CUDA(cudaGetLastError());
+    } else if (stage_stream(x, C, H, n, st)) {
+      return -1;
+    }
+    if (kind == kResnet) {
+      if (resnet(name, Ci, Co, H, n, cur, st)) return -1;
+    } else if (kind == kAttention) {
+      if (attention(name + ".", n, cur, st)) return -1;
+    } else if (kind == kDown) {
+      if (downsample(convs.at(name + ".conv"), xs[cur], H, n, xs[1 - cur], x32[1 - cur], st)) return -1;
+      cur = 1 - cur;
+    } else if (kind == kOut) {
+      if (group_norm("encoder.conv_norm_out", x32[cur], 512, 32, n, true, st)) return -1;
+      const VaeConv& co = convs.at("conv_out");
+      if (conv3(co, nrm, 32, n, xs[1 - cur], false, t32, nullptr, nullptr, st)) return -1;
+      enc_extract_kernel<<<ew_grid((long long)n * 4 * 1024), 256, 0, st>>>(t32, out, n, 4, 1024, co.cout);
+      NOPE_CUDA(cudaGetLastError());
+    }
+    if (kind != kOut && extract_stream(cur, Co, Ho, n, out, out_pair, st)) return -1;
+    NOPE_CUDA(cudaStreamSynchronize(st));
     return 0;
   }
 
@@ -965,6 +1052,60 @@ struct nope_vae_decoder : nope::VaeEngine {
     vae_dec_extract_kernel<<<ew_grid((long long)n * 3 * 65536), 256, 0, st>>>(t32, co.cout, cap, n, out);
     NOPE_CUDA(cudaGetLastError());
     ++launches;
+    return 0;
+  }
+
+  // Runs one module of decode() on its own (nope_vae_decoder_run_block), as nope_vae::run_block: "decoder.conv_in"
+  // (post_quant_conv with 1 / 0.18215, then conv_in) takes latents [n, 4, 32, 32]; "decoder.conv_out"
+  // (conv_norm_out + SiLU + conv_out) gives images [n, 3, 256, 256] and has no pair.
+  int run_block(const std::string& name, const float* x, int C, int H, int n, float* out, float* out_pair,
+                int64_t cap_floats, cudaStream_t st) {
+    using namespace nope;
+    enum { kResnet, kUp, kAttention, kIn, kOut } kind = kResnet;
+    int Ci = 0, Hi = 0, Co = 0, Ho = 0;
+    if (name == "decoder.conv_in") {
+      kind = kIn, Ci = 4, Hi = 32, Co = 512, Ho = 32;
+    } else if (name == "decoder.conv_out") {
+      kind = kOut, Ci = 128, Hi = 256, Co = 3, Ho = 256;
+    } else if (name + "." == kAttn) {
+      kind = kAttention, Ci = Co = 512, Hi = Ho = 32;
+    } else if (name == "decoder.mid_block.resnets.0" || name == "decoder.mid_block.resnets.1") {
+      Ci = Co = 512, Hi = Ho = 32;
+    } else {
+      int cin = 512;
+      for (int i = 0; i < 4; ++i) {
+        for (int j = 0; j < 3; ++j) {
+          if (name == up(i) + ".resnets." + std::to_string(j)) Ci = cin, Co = kCh[i], Hi = Ho = 32 << i;
+          cin = kCh[i];
+        }
+        if (i < 3 && name == up(i) + ".upsamplers.0") kind = kUp, Ci = Co = kCh[i], Hi = 32 << i, Ho = 2 * Hi;
+      }
+    }
+    if (check_block(name, kChunk, C, H, n, Ci, Hi, Co, Ho, cap_floats)) return -1;
+    NOPE_CHECK(!out_pair || kind != kOut, "run_block: decoder.conv_out has no (hi, lo) output");
+    launches = 0;
+    int cur = 0;
+    if (kind == kIn) {
+      vae_dec_conv_in_kernel<<<dim3(32, n, 2), 256, 0, st>>>(x, pq_w, pq_b, in_w, in_b, x32[0], xs[0].hi, xs[0].lo);
+      NOPE_CUDA(cudaGetLastError());
+    } else if (stage_stream(x, C, H, n, st)) {
+      return -1;
+    }
+    if (kind == kResnet) {
+      if (resnet(name, Ci, Co, H, n, cur, st)) return -1;
+    } else if (kind == kAttention) {
+      if (attention(kAttn, n, cur, st)) return -1;
+    } else if (kind == kUp) {
+      if (upsample(name + ".conv", Co, H, n, cur, st)) return -1;
+    } else if (kind == kOut) {
+      if (group_norm("decoder.conv_norm_out", x32[cur], 128, 256, n, true, st)) return -1;
+      const VaeConv& co = convs.at("decoder.conv_out");
+      if (conv3(co, nrm, 256, n, xs[1 - cur], false, t32, nullptr, nullptr, st)) return -1;
+      vae_dec_extract_kernel<<<ew_grid((long long)n * 3 * 65536), 256, 0, st>>>(t32, co.cout, cap, n, out);
+      NOPE_CUDA(cudaGetLastError());
+    }
+    if (kind != kOut && extract_stream(cur, Co, Ho, n, out, out_pair, st)) return -1;
+    NOPE_CUDA(cudaStreamSynchronize(st));
     return 0;
   }
 };

@@ -73,6 +73,19 @@ class _Backbone(nn.Module):
         return self.layer4(self.layer3(self.layer2(self.layer1(x))))
 
 
+def _encoder_block_out(name, D):
+    """(C, H, W) of a native-engine module's output (FeatureExtractor.run_block); (1, 1, 1) for an unknown name,
+    which the engine refuses."""
+    if name == "stem":
+        return (64, 128, 128)
+    if name == "projector":
+        return (D, 32, 32)
+    for li, (planes, blocks, side) in enumerate([(64, 3, 128), (128, 4, 64), (256, 6, 32), (512, 3, 32)], start=1):
+        if name in [f"backbone.layer{li}.{b}" for b in range(blocks)]:
+            return (planes * 4, side, side)
+    return (1, 1, 1)
+
+
 class FeatureExtractor(nn.Module):
     """Same constructor/attributes as the reference (template.py:25-45)."""
 
@@ -155,6 +168,24 @@ class FeatureExtractor(nn.Module):
         if self.normalize:
             feat = F.normalize(feat, dim=1)
         return feat.float()
+
+    @torch.no_grad()
+    def run_block(self, name, x):
+        """Debug / parity: one module of the native engine on its own (nope_encoder_run_block).  name "stem"
+        (x = images [n, 3, 256, 256]), "backbone.layer<l>.<b>" or "projector"; x [n, C, H, H] (CUDA) -> the module's
+        output, fp32 NCHW: hi + lo of its (hi, lo) pair, the projector's fp32 output.  n <= 32."""
+        p = next(self.parameters())
+        if not self._use_native(p.device):
+            raise _lib.NopeError("run_block needs the native engine on a CUDA device")
+        x = x.to(device=p.device, dtype=torch.float32).contiguous()
+        if x.dim() != 4:
+            raise _lib.NopeError(f"run_block takes [n, C, H, H] inputs, got {tuple(x.shape)}")
+        out = torch.empty((x.shape[0],) + _encoder_block_out(name, self.latent_dim), device=p.device)
+        with torch.cuda.device(p.device):
+            _lib.check(_lib.load().nope_encoder_run_block(
+                self._engine(p.device), name.encode(), _lib.ptr(x), x.shape[1], x.shape[2], x.shape[0], _lib.ptr(out),
+                out.numel(), C.c_void_p(torch.cuda.current_stream(p.device).cuda_stream)))
+        return out
 
     @torch.no_grad()
     def encode_image_inplane(self, image, A):

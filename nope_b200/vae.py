@@ -219,6 +219,25 @@ def load_pretrained(path):
     return load_file(st, device="cpu")
 
 
+def _vae_block_out(name):
+    """(C, H, W) of the output of an encoder or decoder engine module (VAE_StableDiffusion.run_block); (1, 1, 1) for
+    an unknown name, which the engine refuses."""
+    fixed = {"encoder.conv_in": (128, 256), "encoder.conv_out": (4, 32), "decoder.conv_in": (512, 32),
+             "decoder.conv_out": (3, 256)}
+    for p in ("encoder.mid_block.", "decoder.mid_block."):
+        fixed.update({p + "resnets.0": (512, 32), p + "resnets.1": (512, 32), p + "attentions.0": (512, 32)})
+    for i, c in enumerate((128, 256, 512, 512)):
+        fixed.update({f"encoder.down_blocks.{i}.resnets.{j}": (c, 256 >> i) for j in range(2)})
+        if i < 3:
+            fixed[f"encoder.down_blocks.{i}.downsamplers.0"] = (c, 128 >> i)
+    for i, c in enumerate((512, 512, 256, 128)):
+        fixed.update({f"decoder.up_blocks.{i}.resnets.{j}": (c, 32 << i) for j in range(3)})
+        if i < 3:
+            fixed[f"decoder.up_blocks.{i}.upsamplers.0"] = (c, 64 << i)
+    c, s = fixed.get(name, (1, 1))
+    return (c, s, s)
+
+
 class VAE_StableDiffusion:
     """Same constructor and attributes as the reference (AutoencoderKL.py:6-27)."""
 
@@ -367,6 +386,25 @@ class VAE_StableDiffusion:
                 self._engine(), _lib.ptr(x), x.shape[0], _lib.ptr(idx), _lib.ptr(cs), P, _lib.ptr(out),
                 self._stream()))
         return out
+
+    @torch.no_grad()
+    def run_block(self, name, x, want_pair=True):
+        """Debug / parity: one module of the encoder engine, or of the decoder engine for a "decoder." name, on its
+        own (nope_vae_run_block / nope_vae_decoder_run_block).  x [n, C, H, H] (CUDA) -> (out, pair): the fp32
+        residual stream after the module and, when want_pair, hi + lo of its (hi, lo) copy, both fp32 NCHW.
+        "encoder.conv_out" / "decoder.conv_out" give the latent / the image and no pair."""
+        if not isinstance(x, torch.Tensor) or x.device.type != "cuda" or x.dim() != 4:
+            raise _lib.NopeError("run_block takes [n, C, H, H] CUDA tensors")
+        dec = name.startswith("decoder.")
+        h = self._decoder() if dec else self._engine()
+        x = x.to(device=self.device, dtype=torch.float32).contiguous()
+        out = torch.empty((x.shape[0],) + _vae_block_out(name), device=self.device)
+        pair = torch.empty_like(out) if want_pair else None
+        fn = _lib.load().nope_vae_decoder_run_block if dec else _lib.load().nope_vae_run_block
+        with torch.cuda.device(self.device):
+            _lib.check(fn(h, name.encode(), _lib.ptr(x), x.shape[1], x.shape[2], x.shape[0], _lib.ptr(out),
+                          _lib.ptr(pair), out.numel(), self._stream()))
+        return out, pair
 
     # ------------------------------------------------------------------ decoder
     def _decoder(self):

@@ -166,20 +166,28 @@ def _bottleneck(sd, p, x, stride):
     return F.relu(out + x)
 
 
-def encode_image(sd, image, prefix=""):
+def encode_image(sd, image, prefix="", taps=None):
     """ResNet-50 without max-pool, layer4 stride 1 (=> /8), eval-mode BN, then
     ReLU -> 1x1(2048->256) -> ReLU -> 1x1(256->D); normalize=False
-    (configs/model/template_base.yaml:12)."""
-    g = lambda k: prefix + k
+    (configs/model/template_base.yaml:12).  taps, if a dict, receives (input, output) of every module the native
+    engine runs on its own (nope_encoder_run_block) under its name: "stem" (conv1 + bn1 + ReLU),
+    "backbone.layer<l>.<b>" and "projector"."""
     sdp = {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)} if prefix else sd
-    x = F.conv2d(image, sdp["backbone.conv1.weight"], stride=2, padding=3)
-    x = F.relu(_bn(sdp, "backbone.bn1", x))
+
+    def module(name, fn, h):
+        out = fn(h)
+        if taps is not None:
+            taps[name] = (h, out)
+        return out
+
+    x = module("stem", lambda t: F.relu(_bn(sdp, "backbone.bn1", F.conv2d(t, sdp["backbone.conv1.weight"], stride=2,
+                                                                           padding=3))), image)
     for li, (blocks, stride) in enumerate([(3, 1), (4, 2), (6, 2), (3, 1)], start=1):
         for b in range(blocks):
-            x = _bottleneck(sdp, f"backbone.layer{li}.{b}", x, stride if b == 0 else 1)
-    x = F.conv2d(F.relu(x), sdp["projector.1.weight"])
-    x = F.conv2d(F.relu(x), sdp["projector.3.weight"])
-    return x
+            p = f"backbone.layer{li}.{b}"
+            x = module(p, lambda t: _bottleneck(sdp, p, t, stride if b == 0 else 1), x)
+    return module("projector", lambda t: F.conv2d(F.relu(F.conv2d(F.relu(t), sdp["projector.1.weight"])),
+                                                  sdp["projector.3.weight"]), x)
 
 
 # ----------------------------------------------------------------------------

@@ -66,22 +66,41 @@ def attention(x, sd, p=ATTN):
 @torch.no_grad()
 def encode(sd, x, taps=None, dtype=torch.float64):
     """x [B, 3, 256, 256] -> latent [B, 4, 32, 32] (dtype).  taps, if a dict, receives the activations after
-    each down block ("down0" .. "down3") and after the mid block ("mid")."""
+    each down block ("down0" .. "down3") and after the mid block ("mid"), and (input, output) of every module the
+    engine runs on its own (nope_vae_run_block) under its name: "encoder.conv_in",
+    "encoder.down_blocks.<i>.resnets.<j>", "encoder.down_blocks.<i>.downsamplers.0", "encoder.mid_block.resnets.<j>",
+    "encoder.mid_block.attentions.0" and "encoder.conv_out" (conv_norm_out + SiLU + conv_out + quant_conv mean x
+    0.18215, whose output is the latent)."""
     sd = canonical(sd, x.device, dtype)
-    h = F.conv2d(x.to(dtype), sd["encoder.conv_in.weight"], sd["encoder.conv_in.bias"], padding=1)
+    x = x.to(dtype)
+
+    def module(name, fn, h):
+        out = fn(h)
+        if taps is not None:
+            taps[name] = (h, out)
+        return out
+
+    h = module("encoder.conv_in", lambda t: F.conv2d(t, sd["encoder.conv_in.weight"], sd["encoder.conv_in.bias"],
+                                                     padding=1), x)
     for i in range(4):
         for j in range(2):
-            h = resnet(h, sd, f"encoder.down_blocks.{i}.resnets.{j}")
+            p = f"encoder.down_blocks.{i}.resnets.{j}"
+            h = module(p, lambda t: resnet(t, sd, p), h)
         if i < 3:
-            p = f"encoder.down_blocks.{i}.downsamplers.0.conv"
-            h = downsample(h, sd[p + ".weight"], sd[p + ".bias"])
+            p = f"encoder.down_blocks.{i}.downsamplers.0"
+            h = module(p, lambda t: downsample(t, sd[p + ".conv.weight"], sd[p + ".conv.bias"]), h)
         if taps is not None:
             taps[f"down{i}"] = h
-    h = resnet(h, sd, "encoder.mid_block.resnets.0")
-    h = attention(h, sd)
-    h = resnet(h, sd, "encoder.mid_block.resnets.1")
+    h = module("encoder.mid_block.resnets.0", lambda t: resnet(t, sd, "encoder.mid_block.resnets.0"), h)
+    h = module("encoder.mid_block.attentions.0", lambda t: attention(t, sd), h)
+    h = module("encoder.mid_block.resnets.1", lambda t: resnet(t, sd, "encoder.mid_block.resnets.1"), h)
     if taps is not None:
         taps["mid"] = h
+    return module("encoder.conv_out", lambda t: conv_out(t, sd), h)
+
+
+def conv_out(h, sd):
+    """conv_norm_out + SiLU, conv_out, quant_conv, the mean's four channels x 0.18215"""
     h = F.silu(group_norm(h, sd, "encoder.conv_norm_out"))
     h = F.conv2d(h, sd["encoder.conv_out.weight"], sd["encoder.conv_out.bias"], padding=1)
     h = F.conv2d(h, sd["quant_conv.weight"], sd["quant_conv.bias"])

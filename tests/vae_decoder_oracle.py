@@ -67,25 +67,43 @@ def upsample_folded(x, w, b):
 @torch.no_grad()
 def decode(sd, z, taps=None, dtype=torch.float64):
     """z [B, 4, 32, 32] -> image [B, 3, 256, 256] (dtype), not clamped.  taps, if a dict, receives the activations
-    after the mid block ("mid") and after each up block ("up0" .. "up3")."""
+    after the mid block ("mid") and after each up block ("up0" .. "up3"), and (input, output) of every module the
+    engine runs on its own (nope_vae_decoder_run_block) under its name: "decoder.conv_in" (post_quant_conv with
+    1 / 0.18215, then conv_in), "decoder.mid_block.resnets.<j>", "decoder.mid_block.attentions.0",
+    "decoder.up_blocks.<i>.resnets.<j>", "decoder.up_blocks.<i>.upsamplers.0" and "decoder.conv_out"
+    (conv_norm_out + SiLU + conv_out, whose output is the image)."""
     sd = canonical(sd, z.device, dtype)
-    h = F.conv2d(z.to(dtype) / E.SCALE, sd["post_quant_conv.weight"], sd["post_quant_conv.bias"])
-    h = F.conv2d(h, sd["decoder.conv_in.weight"], sd["decoder.conv_in.bias"], padding=1)
-    h = E.resnet(h, sd, "decoder.mid_block.resnets.0")
-    h = E.attention(h, sd, ATTN)
-    h = E.resnet(h, sd, "decoder.mid_block.resnets.1")
+
+    def module(name, fn, h):
+        out = fn(h)
+        if taps is not None:
+            taps[name] = (h, out)
+        return out
+
+    def conv_in(t):
+        t = F.conv2d(t / E.SCALE, sd["post_quant_conv.weight"], sd["post_quant_conv.bias"])
+        return F.conv2d(t, sd["decoder.conv_in.weight"], sd["decoder.conv_in.bias"], padding=1)
+
+    def conv_out(t):
+        t = F.silu(E.group_norm(t, sd, "decoder.conv_norm_out"))
+        return F.conv2d(t, sd["decoder.conv_out.weight"], sd["decoder.conv_out.bias"], padding=1)
+
+    h = module("decoder.conv_in", conv_in, z.to(dtype))
+    h = module("decoder.mid_block.resnets.0", lambda t: E.resnet(t, sd, "decoder.mid_block.resnets.0"), h)
+    h = module("decoder.mid_block.attentions.0", lambda t: E.attention(t, sd, ATTN), h)
+    h = module("decoder.mid_block.resnets.1", lambda t: E.resnet(t, sd, "decoder.mid_block.resnets.1"), h)
     if taps is not None:
         taps["mid"] = h
     for i in range(4):
         for j in range(3):
-            h = E.resnet(h, sd, f"decoder.up_blocks.{i}.resnets.{j}")
+            p = f"decoder.up_blocks.{i}.resnets.{j}"
+            h = module(p, lambda t: E.resnet(t, sd, p), h)
         if i < 3:
-            p = f"decoder.up_blocks.{i}.upsamplers.0.conv"
-            h = upsample(h, sd[p + ".weight"], sd[p + ".bias"])
+            p = f"decoder.up_blocks.{i}.upsamplers.0"
+            h = module(p, lambda t: upsample(t, sd[p + ".conv.weight"], sd[p + ".conv.bias"]), h)
         if taps is not None:
             taps[f"up{i}"] = h
-    h = F.silu(E.group_norm(h, sd, "decoder.conv_norm_out"))
-    return F.conv2d(h, sd["decoder.conv_out.weight"], sd["decoder.conv_out.bias"], padding=1)
+    return module("decoder.conv_out", conv_out, h)
 
 
 def flops_per_image():
