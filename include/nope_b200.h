@@ -391,6 +391,20 @@ int nope_score_topk_multi(const float* query_feat, const float* emb, int B, int 
 int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_topi,
               int64_t idx_base, void* stream);
 
+/* Distinct pose hypotheses (DESIGN.md section 21): greedy non-maximum suppression of every row of sim [R, N] in the
+ * order of nope_topk, modulo each row's symmetry group.  Row r's rotations are rot [G_r, N, 3, 3] fp64 at r / Q (at 0
+ * when G_r = 1), object -> camera.  Entries i, j are within theta when c(i, j) >= c_thr = 1 + 2 cos(theta), where c
+ * is the largest trace over the group: M_d = D_d Rot_j^T Rot_i, c = max_d tr M_d, or with an axis a,
+ * max_d a^T M_d a + sqrt((tr M_d - a^T M_d a)^2 + s^2), s = a . (M32 - M23, M13 - M31, M21 - M12).  The best entry
+ * left is taken (ties -> lowest index; -inf and NaN never), everything within theta of it is dropped, k times ->
+ * idx_out [R, k] int64, score_out [R, k] fp32, (-1, -inf) where no entry is left.
+ * HOST arrays: sym_disc [sum n_disc, 3, 3] fp64 (group g's n_disc[g] rotations in turn, the identity first),
+ * n_disc [G] int32 (1..32), axis [G, 3] fp64 (a unit vector, or zeros for none), group [R] int32 (0..G-1).
+ * Requires 1 <= k <= 64, -1 <= c_thr <= 3, G_r == 1 or G_r * Q == R.  No host synchronisation. */
+int nope_distinct_topk(const float* sim, int R, int N, const double* rot, int G_r, int Q, const double* sym_disc,
+                       const int32_t* n_disc, const double* axis, int G, const int32_t* group, int k, double c_thr,
+                       int64_t* idx_out, float* score_out, void* stream);
+
 /* Coarse-to-fine pose search (DESIGN.md section 9).  A cell table cells [n_coarse, F] int32 lists, for every
  * pose of a coarse grid, the poses of the next finer grid whose nearest coarse pose it is (ascending, -1 padded,
  * F = the largest cell); cells are disjoint.  Rows r = b * Q + q pair reference b with its query q.

@@ -81,6 +81,9 @@ SIGNATURES = {
                                         C.c_void_p]),
     "nope_unet_set_metric": (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
     "nope_topk": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
+    "nope_distinct_topk": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_double, c_i64p, c_f32p,
+                                     C.c_void_p]),
     "nope_pose_cells_expand": (C.c_int, [c_i64p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, c_f32p, C.c_int,
                                          C.c_int, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_void_p]),
     "nope_pose_cells_rank": (C.c_int, [c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p,

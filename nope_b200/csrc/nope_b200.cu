@@ -33,6 +33,7 @@
 #include "translation.cuh"
 #include "depth_refine.cuh"
 #include "contour_refine.cuh"
+#include "distinct.cuh"
 
 using namespace nope;
 
@@ -1570,6 +1571,57 @@ struct StagedHost {
     if (dev) cudaFreeAsync(dev, st);
   }
 };
+
+int nope_distinct_topk(const float* sim, int R, int N, const double* rot, int G_r, int Q, const double* sym_disc,
+                       const int32_t* n_disc, const double* axis, int G, const int32_t* group, int k, double c_thr,
+                       int64_t* idx_out, float* score_out, void* stream) {
+  NOPE_CHECK(sim && rot && sym_disc && n_disc && axis && group && idx_out && score_out, "null argument");
+  NOPE_CHECK(R >= 1 && N >= 1 && N <= (1 << 30), "R (rows) must be >= 1 and N (entries per row) in [1, 2^30]");
+  NOPE_CHECK(G_r >= 1 && Q >= 1 && (G_r == 1 || (int64_t)G_r * Q == R),
+             "G_r (rotation sets) must be 1 or R / Q, with Q >= 1");
+  NOPE_CHECK(k >= 1 && k <= kDistinctMaxK, "k must be in [1, 64]");
+  NOPE_CHECK(c_thr >= -1.0 && c_thr <= 3.0, "c_thr = 1 + 2 cos(theta) must be in [-1, 3]");
+  NOPE_CHECK(G >= 1 && G <= 65536, "G (symmetry groups) must be in [1, 65536]");
+  // HOST symmetry groups, checked and packed for one stream-ordered upload together with the row -> group table
+  std::vector<DistinctGroup> packed((size_t)G);
+  std::memset(packed.data(), 0, sizeof(DistinctGroup) * (size_t)G);
+  int64_t off = 0;
+  for (int g = 0; g < G; ++g) {
+    const int n = n_disc[g];
+    NOPE_CHECK(n >= 1 && n <= kDistinctMaxSym, "every group needs 1 to 32 discrete rotations");
+    const double* d = sym_disc + 9 * off;
+    for (int e = 0; e < 9 * n; ++e) NOPE_CHECK(std::isfinite(d[e]), "discrete symmetries must be finite");
+    for (int e = 0; e < 9; ++e)
+      NOPE_CHECK(d[e] == (e % 4 == 0 ? 1.0 : 0.0), "the first discrete rotation of every group must be the identity");
+    std::memcpy(packed[g].d, d, sizeof(double) * 9 * n);
+    packed[g].n = n;
+    off += n;
+    const double* a = axis + 3 * (size_t)g;
+    NOPE_CHECK(std::isfinite(a[0]) && std::isfinite(a[1]) && std::isfinite(a[2]), "axes must be finite");
+    const double a2 = a[0] * a[0] + a[1] * a[1] + a[2] * a[2];
+    NOPE_CHECK(a2 == 0.0 || std::fabs(a2 - 1.0) <= 1e-12, "an axis must be a unit vector, or zero for none");
+    std::memcpy(packed[g].axis, a, sizeof(double) * 3);
+    packed[g].has_axis = a2 != 0.0;
+  }
+  for (int r = 0; r < R; ++r) NOPE_CHECK(group[r] >= 0 && group[r] < G, "group indices must be in [0, G)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t nwords = ((int64_t)N + 31) / 32;
+  const size_t g_bytes = sizeof(DistinctGroup) * (size_t)G, r_bytes = sizeof(int32_t) * (size_t)R;
+  const size_t m_off = (g_bytes + r_bytes + 255) & ~(size_t)255;
+  const size_t m_bytes = nwords > kDistinctSmemWords ? sizeof(unsigned) * (size_t)nwords * R : 0;
+  StagedHost scratch;                                   // groups, row -> group, and (large N) the removal masks
+  scratch.st = st;
+  NOPE_CUDA(cudaMallocAsync(&scratch.dev, m_off + m_bytes, st));
+  char* base = static_cast<char*>(scratch.dev);
+  NOPE_CUDA(cudaMemcpyAsync(base, packed.data(), g_bytes, cudaMemcpyHostToDevice, st));
+  NOPE_CUDA(cudaMemcpyAsync(base + g_bytes, group, r_bytes, cudaMemcpyHostToDevice, st));
+  distinct_topk_kernel<<<R, kDistinctThreads, 0, st>>>(
+      sim, N, rot, G_r, Q, reinterpret_cast<const DistinctGroup*>(base), reinterpret_cast<const int*>(base + g_bytes),
+      k, c_thr, m_bytes ? reinterpret_cast<unsigned*>(base + m_off) : nullptr, reinterpret_cast<long long*>(idx_out),
+      score_out);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
 
 int nope_vsd_error_taus(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H,
                         int W, const double* K, double delta, int cost_type, const double* taus, int T, double* out,

@@ -514,11 +514,52 @@ class PoseConditional:
     # ------------------------------------------------------------------ BOP 2019 average recall (DESIGN.md section 15)
     def load_models_info(self, path):
         """A BOP models_info.json: the diameter (mm) and the symmetry transforms [S, 3, 4] of every object, in
-        self.bop_models[obj_id] = {"diameter", "symmetries"}."""
+        self.bop_models[obj_id] = {"diameter", "symmetries", "info"}; "info" is the `bop.load_models_info` entry, whose
+        discrete and continuous symmetries `select_distinct` uses."""
         from . import bop
         for obj_id, info in bop.load_models_info(path).items():
-            self.bop_models[obj_id] = {"diameter": info["diameter"], "symmetries": bop.symmetry_transformations(info)}
+            self.bop_models[obj_id] = {"diameter": info["diameter"], "symmetries": bop.symmetry_transformations(info),
+                                       "info": info}
         return self
+
+    @torch.no_grad()
+    def select_distinct(self, sim, rotations, obj_ids=None, k=5, *, min_angle_deg):
+        """k distinct pose hypotheses per row of a search's similarity (`distinct.distinct_topk`, DESIGN.md section
+        21): the best-scoring entries such that no two rotations lie within min_angle_deg of each other, modulo the
+        object's symmetries, in place of the search's top-k, which are mostly grid neighbours of one mode.
+          sim        [B, N], [B, Q, N] or [Q, N] from predict_pose (or predict_pose_coarse_to_fine: its -inf entries
+                     were not scored and are never taken);
+          rotations  [B | 1, N, 3, 3] the entries' rotations, e.g. template_poses;
+          obj_ids    None (no symmetry) or one object id per index of sim's first dimension, looked up in
+                     self.bop_models (load_models_info first);
+          min_angle_deg  theta in [0, 180] degrees.  It has no default: no value has been chosen from measured
+                     accuracy.
+        In-plane search: pass sim.flatten(-2) ([..., A * N]) and, for every (angle a, pose n) at a * N + n,
+        inplane.compose(template_poses, n, a, A); then angle_idx, nearest_idx = divmod(idx, N) for idx >= 0.
+        -> (R float64 [..., k, 3, 3] (zeros at padding), idx int64 [..., k] (-1 at padding), score float32 [..., k]
+        (-inf at padding)) on sim's device, without synchronising.  R goes unchanged into estimate_translation,
+        refine_depth, refine_contour and eval_bop(R_est=)."""
+        import numpy as np
+        from .distinct import distinct_topk
+        syms = None
+        if obj_ids is not None:
+            ids = [int(i) for i in np.asarray(obj_ids.detach().cpu() if torch.is_tensor(obj_ids) else obj_ids)
+                   .reshape(-1).tolist()]
+            missing = sorted(set(i for i in ids if i not in self.bop_models))
+            if missing:
+                raise ValueError(f"select_distinct: no models_info entry for obj_id {missing} (load_models_info)")
+            syms = [self.bop_models[i]["info"] for i in ids]
+        score, idx = distinct_topk(sim, rotations, k, min_angle_deg, syms)
+        rot = torch.as_tensor(np.asarray(rotations) if not torch.is_tensor(rotations) else rotations)
+        rot = rot.to(idx.device, torch.float64)
+        lead = idx.shape[:-1]
+        rows = idx.reshape(lead[0] if lead else 1, -1)
+        if rot.shape[0] == 1:
+            R = rot[0][rows.clamp_min(0)]
+        else:
+            R = rot[torch.arange(rot.shape[0], device=idx.device)[:, None], rows.clamp_min(0)]
+        R = torch.where((rows >= 0)[..., None, None], R, torch.zeros((), dtype=R.dtype, device=R.device))
+        return R.reshape(idx.shape + (3, 3)), idx, score
 
     @torch.no_grad()
     def estimate_translation(self, batch, R, masks, iters=4):
