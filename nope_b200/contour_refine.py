@@ -9,10 +9,10 @@ import numpy as np
 import torch
 
 from . import _lib
-from .bop import _host_k, _to_dev
-from .depth_refine import MAX_ITERS, _tensor
-from .translation import MAX_BATCH, _masks
-from .vsd import Mesh, _stream
+from ._posefit import MAX_BATCH, MAX_ITERS, _masks, broadcast_t, check_iters, cuda_device, fit_args, geometric, \
+    pack_refined, refine_outputs, taus, workspace
+from .bop import _to_dev
+from .vsd import _stream
 
 DEFAULT_ITERS = 10           # from the convergence table of DESIGN.md section 20
 TAU_START = 0.15             # the default schedule: tau_0 = TAU_START s ... tau_iters = TAU_END s, geometric, with
@@ -23,13 +23,10 @@ FIT_FIELDS = ("n_in", "n_contour", "rms", "iou")
 def default_tau(iters=DEFAULT_ITERS, start=TAU_START, end=TAU_END):
     """The pairing tolerances float64 [iters + 1], as fractions of the mask's box size: geometric from `start` down to
     `end` (by default TAU_START and TAU_END), so the fit at the returned pose is always scored at `end`."""
-    if isinstance(iters, bool) or int(iters) != iters or not 0 <= iters <= MAX_ITERS:
-        raise ValueError(f"iters must be an integer in [0, {MAX_ITERS}], got {iters!r}")
+    iters = check_iters(iters, MAX_ITERS)
     if not (np.isfinite(start) and np.isfinite(end) and start > 0 and end > 0):
         raise ValueError(f"start and end must be finite and > 0, got {(start, end)}")
-    iters = int(iters)
-    i = np.arange(iters + 1, dtype=np.float64)
-    return end * (start / end) ** ((iters - i) / max(iters, 1))
+    return geometric(end, start / end, iters)
 
 
 def mask_sdf(masks):
@@ -70,55 +67,22 @@ def refine_pose_contour(mesh, R, t, K, masks, iters=DEFAULT_ITERS, tau=None, zne
     with the mask.  A hypothesis with fewer than 6 pairs keeps its pose; a frame whose mask is empty or full keeps
     every pose, with NaN "rms" and "iou".  With return_sums, also the int64 [F, P, 29] fixed-point sums of the last
     render.  Runs on the mesh's device and current stream without synchronising."""
-    if not isinstance(mesh, Mesh):
-        raise ValueError("mesh must be a nope_b200.vsd.Mesh")
-    R = _tensor(R)
-    if R.dim() == 3:
-        R = R[:, None]
-    if R.dim() != 4 or R.shape[2:] != (3, 3) or R.shape[0] < 1 or R.shape[1] < 1:
-        raise ValueError(f"R [F, P, 3, 3] or [F, 3, 3] expected, got {tuple(R.shape)}")
-    if R.dtype not in (torch.float32, torch.float64):
-        raise ValueError(f"R must be float32 or float64, got {R.dtype}")
-    F_, P = R.shape[:2]
-    if F_ > MAX_BATCH or P > MAX_BATCH:
-        raise ValueError(f"F and P must be <= {MAX_BATCH}, got {(F_, P)}")
-    t = _tensor(t)
-    if t.shape not in ((F_, 3), (F_, P, 3)):
-        raise ValueError(f"t [{F_}, 3] or [{F_}, {P}, 3] expected, got {tuple(t.shape)}")
+    R, t, k, F_, P, iters = fit_args(mesh, R, t, K, iters, znear, MAX_ITERS)
     masks = _masks(masks)
     if masks.shape[0] != F_:
         raise ValueError(f"masks [{F_}, H, W] expected, got {tuple(masks.shape)}")
     H, W = masks.shape[1:]
-    if isinstance(iters, bool) or int(iters) != iters or not 0 <= iters <= MAX_ITERS:
-        raise ValueError(f"iters must be an integer in [0, {MAX_ITERS}], got {iters!r}")
-    iters = int(iters)
-    if not (np.isfinite(znear) and znear > 0):
-        raise ValueError(f"znear must be finite and > 0, got {znear}")
-    k = _host_k(K, F_)
-    taus = default_tau(iters) if tau is None else np.asarray(
-        tau.detach().cpu() if torch.is_tensor(tau) else tau, dtype=np.float64).reshape(-1)
-    if taus.size == 1:
-        taus = np.repeat(taus, iters + 1)
-    if taus.size != iters + 1 or not (np.isfinite(taus).all() and (taus > 0).all()):
-        raise ValueError(f"tau: one or iters + 1 = {iters + 1} finite numbers > 0 expected, got {taus}")
-    taus = np.ascontiguousarray(taus)
-    dev = mesh.device
-    if dev.type != "cuda":
-        raise _lib.NopeError("refine_pose_contour needs a CUDA mesh (no CPU fallback)")
+    tv = taus(default_tau(iters) if tau is None else tau, iters)
+    dev = cuda_device(mesh, "refine_pose_contour")
     with torch.cuda.device(dev):
         md = _to_dev(masks, dev, torch.uint8)
-        t0 = _to_dev(t, dev, torch.float64)
-        t0 = t0[:, None].expand(F_, P, 3).contiguous() if t0.dim() == 2 else t0
+        t0 = broadcast_t(t, F_, P, dev)
         Rd = _to_dev(R, dev, torch.float64)
-        ws = torch.empty((F_ * P, H, W), device=dev, dtype=torch.float32)
-        R_out = torch.empty((F_, P, 3, 3), device=dev, dtype=torch.float64)
-        t_out = torch.empty((F_, P, 3), device=dev, dtype=torch.float64)
-        fit = torch.empty((F_, P, 4), device=dev, dtype=torch.float64)
-        sums = torch.empty((F_, P, 29), device=dev, dtype=torch.int64) if return_sums else None
+        ws = workspace(dev, F_, P, H, W)
+        R_out, t_out, fit, sums = refine_outputs(dev, F_, P, return_sums)
         _lib.check(_lib.load().nope_refine_contour(
             _lib.ptr(mesh.vertices), mesh.vertices.shape[0], _lib.ptr(mesh.faces), mesh.num_faces, _lib.ptr(Rd),
-            _lib.ptr(t0), _lib.ptr(md), k.data_ptr(), F_, P, H, W, mesh.radius, taus.ctypes.data, iters,
+            _lib.ptr(t0), _lib.ptr(md), k.data_ptr(), F_, P, H, W, mesh.radius, tv.ctypes.data, iters,
             float(znear), _lib.ptr(ws), _lib.ptr(R_out), _lib.ptr(t_out), _lib.ptr(fit), _lib.ptr(sums),
             _stream(dev)))
-    out = {name: fit[..., i] for i, name in enumerate(FIT_FIELDS)}
-    return (R_out, t_out, out, sums) if return_sums else (R_out, t_out, out)
+    return pack_refined(R_out, t_out, fit, sums, FIT_FIELDS)

@@ -180,37 +180,10 @@ contour_accumulate_kernel(const unsigned* __restrict__ z, const double* __restri
     icp_cross(A, J + 3, J);
 #pragma unroll
     for (int k = 0; k < 3; ++k) J[k] = __ddiv_rn(J[k], rho);
-    const double et = __ddiv_rn(e, tau);
-    int q = 0;
-#pragma unroll
-    for (int a = 0; a < 6; ++a) {
-#pragma unroll
-      for (int b = a; b < 6; ++b) acc[q++] += icp_fixed(__dmul_rn(J[a], J[b]));
-    }
-#pragma unroll
-    for (int a = 0; a < 6; ++a) acc[kIcpJJ + a] += icp_fixed(__dmul_rn(J[a], et));
-    acc[kIcpJJ + 6] += icp_fixed(__dmul_rn(et, et));
+    icp_add_pair(acc, J, __ddiv_rn(e, tau));
     ++n;
   }
-  __shared__ long long part[kIcpThreads / 32][kIcpSums + 1];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#pragma unroll
-  for (int k = 0; k < kIcpSums - 1; ++k) {
-    long long v = acc[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) part[warp][k] = v;
-  }
-  n = __reduce_add_sync(0xffffffffu, n);
-  nc = __reduce_add_sync(0xffffffffu, nc);
-  if (lane == 0) { part[warp][kIcpSums - 1] = n; part[warp][kIcpSums] = nc; }
-  __syncthreads();
-  if (threadIdx.x > kIcpSums) return;
-  long long v = 0;
-  for (int w = 0; w < kIcpThreads / 32; ++w) v += part[w][threadIdx.x];
-  if (v == 0) return;
-  if (threadIdx.x < kIcpSums) atomicAdd(sums + h * kIcpSums + threadIdx.x, (unsigned long long)v);   // wraps
-  else atomicAdd(n_contour + h, (int)v);
+  icp_flush_sums<true>(acc, n, nc, sums + h * kIcpSums, n_contour + h);
 }
 
 // One thread per (f, p), n = F P: R, t = the inputs, the first pose, the sums, n_contour and the silhouette and mask
@@ -244,7 +217,7 @@ __global__ void contour_solve_kernel(int F, int P, long long hw, double tau_frac
       const double tau = contour_tau(tau_frac, mask_stats + kFitStats * f, hw);
       icp_step(s, __dmul_rn(tau, contour_kappa(ti[2], K[4 * f], K[4 * f + 1])), rho, R + 9 * i, ti);
     }
-    icp_write_pose(R + 9 * i, ti, poses + 16 * i);
+    render_write_pose(R + 9 * i, ti, poses + 16 * i);
     for (int k = 0; k < kIcpSums; ++k) s[k] = 0ull;
     n_contour[i] = 0;
   }

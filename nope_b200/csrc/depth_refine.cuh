@@ -50,6 +50,51 @@ __device__ __forceinline__ double icp_dot(const double* a, const double* b) {
 
 __device__ __forceinline__ bool icp_hit(unsigned bits) { return bits != kDepthInfBits; }
 
+// One pair's fixed-point products added to a thread's 28 int64 registers: acc[0, 21) the upper triangle of J J^T row
+// by row, acc[21, 27) J e, acc[27] e^2.
+__device__ __forceinline__ void icp_add_pair(long long* acc, const double* J, double e) {
+  int q = 0;
+#pragma unroll
+  for (int a = 0; a < 6; ++a) {
+#pragma unroll
+    for (int b = a; b < 6; ++b) acc[q++] += icp_fixed(__dmul_rn(J[a], J[b]));
+  }
+#pragma unroll
+  for (int a = 0; a < 6; ++a) acc[kIcpJJ + a] += icp_fixed(__dmul_rn(J[a], e));
+  acc[kIcpJJ + 6] += icp_fixed(__dmul_rn(e, e));
+}
+
+// The CTA's flush of an accumulate kernel: every thread's 28 registers acc and pair count n are reduced through warp
+// shuffles and shared memory, and the CTA adds its partials to the hypothesis's sums [29] with one integer atomic per
+// field.  kContour also reduces the contour pixel counts nc into *n_contour.  Called by every thread of the CTA.
+template <bool kContour>
+__device__ __forceinline__ void icp_flush_sums(const long long* acc, int n, int nc, unsigned long long* __restrict__ sums,
+                                               int* __restrict__ n_contour) {
+  constexpr int kFields = kIcpSums + (kContour ? 1 : 0);
+  __shared__ long long part[kIcpThreads / 32][kFields];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int k = 0; k < kIcpSums - 1; ++k) {
+    long long v = acc[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) part[warp][k] = v;
+  }
+  n = __reduce_add_sync(0xffffffffu, n);
+  if (kContour) nc = __reduce_add_sync(0xffffffffu, nc);
+  if (lane == 0) {
+    part[warp][kIcpSums - 1] = n;
+    if (kContour) part[warp][kIcpSums] = nc;
+  }
+  __syncthreads();
+  if (threadIdx.x >= kFields) return;
+  long long v = 0;
+  for (int w = 0; w < kIcpThreads / 32; ++w) v += part[w][threadIdx.x];
+  if (v == 0) return;
+  if (!kContour || threadIdx.x < kIcpSums) atomicAdd(sums + threadIdx.x, (unsigned long long)v);   // wraps
+  else atomicAdd(n_contour, (int)v);
+}
+
 // The pairs of one iteration: grid (ceil(H W / kIcpPixelsPerCta), P, F).  z [F, P, H, W] the render of hypothesis
 // (f, p) (float bits, +inf where nothing is hit), S [F, H, W] the sensor depth (mm, 0 = no reading), masks [F, H, W]
 // or null, K [F, 4], t [F, P, 3] the hypotheses' current origins.  Each pixel that takes part adds its fixed-point
@@ -109,34 +154,10 @@ icp_accumulate_kernel(const unsigned* __restrict__ z, const double* __restrict__
     icp_cross(A, J + 3, J);
 #pragma unroll
     for (int k = 0; k < 3; ++k) J[k] = __ddiv_rn(J[k], rho);
-    const double e = __ddiv_rn(icp_dot(J + 3, B), tau);
-    int q = 0;
-#pragma unroll
-    for (int a = 0; a < 6; ++a) {
-#pragma unroll
-      for (int b = a; b < 6; ++b) acc[q++] += icp_fixed(__dmul_rn(J[a], J[b]));
-    }
-#pragma unroll
-    for (int a = 0; a < 6; ++a) acc[kIcpJJ + a] += icp_fixed(__dmul_rn(J[a], e));
-    acc[kIcpJJ + 6] += icp_fixed(__dmul_rn(e, e));
+    icp_add_pair(acc, J, __ddiv_rn(icp_dot(J + 3, B), tau));
     ++n;
   }
-  __shared__ long long part[kIcpThreads / 32][kIcpSums];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#pragma unroll
-  for (int k = 0; k < kIcpSums - 1; ++k) {
-    long long v = acc[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) part[warp][k] = v;
-  }
-  n = __reduce_add_sync(0xffffffffu, n);
-  if (lane == 0) part[warp][kIcpSums - 1] = n;
-  __syncthreads();
-  if (threadIdx.x >= kIcpSums) return;
-  long long v = 0;
-  for (int w = 0; w < kIcpThreads / 32; ++w) v += part[w][threadIdx.x];
-  if (v != 0) atomicAdd(sums + h * kIcpSums + threadIdx.x, (unsigned long long)v);   // two's complement wraps
+  icp_flush_sums<false>(acc, n, 0, sums + h * kIcpSums, nullptr);
 }
 
 // n_valid [F] += the pixels of each frame with a sensor reading inside its mask: grid (ceil(H W / kIcpPixelsPerCta),
@@ -160,17 +181,6 @@ icp_valid_kernel(const double* __restrict__ S, const uint8_t* __restrict__ masks
   if (n) atomicAdd(n_valid + f, n);
 }
 
-// the rasterizer's pose: [R | t] rounded to float32, row-major 4x4
-__device__ __forceinline__ void icp_write_pose(const double* R, const double* t, float* __restrict__ pose) {
-#pragma unroll
-  for (int r = 0; r < 3; ++r) {
-#pragma unroll
-    for (int c = 0; c < 3; ++c) pose[4 * r + c] = __double2float_rn(R[3 * r + c]);
-    pose[4 * r + 3] = __double2float_rn(t[r]);
-  }
-  pose[12] = 0.f; pose[13] = 0.f; pose[14] = 0.f; pose[15] = 1.f;
-}
-
 // a fixed-point sum as float64: rounded to nearest, times 2^-32 (exact)
 __device__ __forceinline__ double icp_unfix(unsigned long long s) {
   return __dmul_rn(__ll2double_rn((long long)s), 1.0 / kIcpFixedScale);
@@ -185,7 +195,7 @@ __device__ __forceinline__ void icp_init_one(long long i, const double* __restri
   for (int k = 0; k < 9; ++k) R[9 * i + k] = R_in[9 * i + k];
 #pragma unroll
   for (int k = 0; k < 3; ++k) t[3 * i + k] = t_in[3 * i + k];
-  icp_write_pose(R_in + 9 * i, t_in + 3 * i, poses + 16 * i);
+  render_write_pose(R_in + 9 * i, t_in + 3 * i, poses + 16 * i);
   for (int k = 0; k < kIcpSums; ++k) sums[kIcpSums * i + k] = 0ull;
 }
 
@@ -283,7 +293,7 @@ __global__ void icp_solve_kernel(int F, int P, double tau, double rho, double* _
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     unsigned long long* s = sums + kIcpSums * i;
     icp_step(s, tau, rho, R + 9 * i, t + 3 * i);
-    icp_write_pose(R + 9 * i, t + 3 * i, poses + 16 * i);
+    render_write_pose(R + 9 * i, t + 3 * i, poses + 16 * i);
     for (int k = 0; k < kIcpSums; ++k) s[k] = 0ull;
   }
 }

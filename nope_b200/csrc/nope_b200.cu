@@ -8,14 +8,17 @@
 #include "../../include/nope_b200.h"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
 #include <tuple>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -974,6 +977,59 @@ int to_nchw(const __half* x, float* out, int n, int C, int hw, cudaStream_t st, 
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }
+
+// A launcher's stream-ordered scratch: every field is declared with add(), each aligned to 256 bytes, then alloc()
+// makes one cudaMallocAsync, points the fields into it and copies in those declared with a HOST source (pageable,
+// staged at once: no host synchronisation).  The block is freed in stream order, after the kernels that use it, when
+// the arena goes out of scope.
+class ScratchArena {
+ public:
+  explicit ScratchArena(cudaStream_t st) : st_(st) {}
+  ScratchArena(const ScratchArena&) = delete;
+  ScratchArena& operator=(const ScratchArena&) = delete;
+  ~ScratchArena() {
+    if (base_) cudaFreeAsync(base_, st_);
+  }
+  template <typename T> void add(T** field, size_t count, const std::remove_const_t<T>* host = nullptr) {
+    bytes_ = (bytes_ + kAlign - 1) & ~(kAlign - 1);
+    fields_.push_back({[field](char* p) { *field = reinterpret_cast<T*>(p); }, bytes_, host, sizeof(T) * count});
+    bytes_ += sizeof(T) * count;
+  }
+  int alloc() {
+    NOPE_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&base_), std::max<size_t>(bytes_, 1), st_));
+    for (const Field& f : fields_) {
+      f.point(base_ + f.offset);
+      if (f.host) NOPE_CUDA(cudaMemcpyAsync(base_ + f.offset, f.host, f.bytes, cudaMemcpyHostToDevice, st_));
+    }
+    return 0;
+  }
+
+ private:
+  struct Field {
+    std::function<void(char*)> point;
+    size_t offset;
+    const void* host;
+    size_t bytes;
+  };
+  static constexpr size_t kAlign = 256;
+  cudaStream_t st_;
+  char* base_ = nullptr;
+  size_t bytes_ = 0;
+  std::vector<Field> fields_;
+};
+
+// HOST intrinsics K [F, 4] (fx, fy, cx, cy): checked (finite, fx and fy non-zero) and declared as an arena field that
+// alloc() copies in
+int stage_host_intrinsics(ScratchArena& arena, const double** dev, const double* K, int F) {
+  for (int f = 0; f < F; ++f) {
+    const double* k = K + 4 * (size_t)f;
+    NOPE_CHECK(std::isfinite(k[0]) && std::isfinite(k[1]) && std::isfinite(k[2]) && std::isfinite(k[3]),
+               "intrinsics must be finite");
+    NOPE_CHECK(k[0] != 0.0 && k[1] != 0.0, "fx and fy must be non-zero");
+  }
+  arena.add(dev, 4 * (size_t)F, K);
+  return 0;
+}
 }  // namespace
 
 // =============================================================================
@@ -1504,6 +1560,29 @@ int nope_vae_decoder_run_block(nope_vae_decoder_t* d, const char* name, const fl
 // ---------------------------------------------------------------------------------
 // T-LESS evaluation: depth rasterizer and VSD (render.cuh, DESIGN.md section 12)
 // ---------------------------------------------------------------------------------
+// The depth bits z [F, P, H, W] of a mesh under F frames x P poses [F, P, 4, 4]: filled with +inf, then one raster
+// launch per frame with that frame's HOST intrinsics K [F, 4].  launch_depth_finish turns +inf into 0 afterwards.
+static int render_frames(const float* vertices, int V, const int32_t* faces, int NF, const float* poses,
+                         const double* K, int F, int P, float znear, int H, int W, unsigned* z, cudaStream_t st) {
+  const long long hw = (long long)H * W, n = (long long)F * P * hw;
+  depth_fill_kernel<<<ew_grid(n), 256, 0, st>>>(z, n);
+  NOPE_CUDA(cudaGetLastError());
+  for (int f = 0; f < F; ++f) {
+    const double* kf = K + 4 * (size_t)f;
+    depth_raster_kernel<<<dim3((NF + 7) / 8, P), 256, 0, st>>>(
+        vertices, V, faces, NF, poses + 16 * (size_t)f * P, (float)kf[0], (float)kf[1], (float)kf[2], (float)kf[3],
+        znear, H, W, z + (size_t)f * P * hw);
+    NOPE_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
+static int launch_depth_finish(unsigned* z, long long n, cudaStream_t st) {
+  depth_finish_kernel<<<ew_grid(n), 256, 0, st>>>(z, n);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int nope_render_depth(const float* vertices, int V, const int32_t* faces, int F, const float* poses, int P, float fx,
                       float fy, float cx, float cy, float znear, int H, int W, float* out, void* stream) {
   NOPE_CHECK(vertices && faces && poses && out, "null argument");
@@ -1515,16 +1594,9 @@ int nope_render_depth(const float* vertices, int V, const int32_t* faces, int F,
              "intrinsics and znear must be finite");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   unsigned* z = reinterpret_cast<unsigned*>(out);
-  const long long n = (long long)P * H * W;
-  const int fill_blocks = (int)std::min<long long>((n + 255) / 256, 132LL * 16);
-  depth_fill_kernel<<<fill_blocks, 256, 0, st>>>(z, n);
-  NOPE_CUDA(cudaGetLastError());
-  depth_raster_kernel<<<dim3((F + 7) / 8, P), 256, 0, st>>>(vertices, V, faces, F, poses, fx, fy, cx, cy, znear, H, W,
-                                                            z);
-  NOPE_CUDA(cudaGetLastError());
-  depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, n);
-  NOPE_CUDA(cudaGetLastError());
-  return 0;
+  const double K[4] = {fx, fy, cx, cy};             // one frame; float -> double -> float is exact
+  if (render_frames(vertices, V, faces, F, poses, K, 1, P, znear, H, W, z, st)) return -1;
+  return launch_depth_finish(z, (long long)P * H * W, st);
 }
 
 int nope_vsd_error(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H, int W,
@@ -1544,33 +1616,6 @@ int nope_vsd_error(const double* depth_test, const float* depth_gt, const float*
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }
-
-// HOST K [F, 4]: finite, fx and fy non-zero
-static int check_host_intrinsics(const double* K, int F) {
-  for (int f = 0; f < F; ++f) {
-    const double* k = K + 4 * (size_t)f;
-    NOPE_CHECK(std::isfinite(k[0]) && std::isfinite(k[1]) && std::isfinite(k[2]) && std::isfinite(k[3]),
-               "intrinsics must be finite");
-    NOPE_CHECK(k[0] != 0.0 && k[1] != 0.0, "fx and fy must be non-zero");
-  }
-  return 0;
-}
-
-// A stream-ordered device copy of a small HOST array: the pageable source is staged at once (no host
-// synchronisation) and the copy is freed in stream order after the kernels that read it.
-struct StagedHost {
-  void* dev = nullptr;
-  cudaStream_t st = nullptr;
-  int upload(const void* host, size_t bytes, cudaStream_t stream) {
-    st = stream;
-    NOPE_CUDA(cudaMallocAsync(&dev, bytes, st));
-    NOPE_CUDA(cudaMemcpyAsync(dev, host, bytes, cudaMemcpyHostToDevice, st));
-    return 0;
-  }
-  ~StagedHost() {
-    if (dev) cudaFreeAsync(dev, st);
-  }
-};
 
 int nope_distinct_topk(const float* sim, int R, int N, const double* rot, int G_r, int Q, const double* sym_disc,
                        const int32_t* n_disc, const double* axis, int G, const int32_t* group, int k, double c_thr,
@@ -1606,19 +1651,16 @@ int nope_distinct_topk(const float* sim, int R, int N, const double* rot, int G_
   for (int r = 0; r < R; ++r) NOPE_CHECK(group[r] >= 0 && group[r] < G, "group indices must be in [0, G)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t nwords = ((int64_t)N + 31) / 32;
-  const size_t g_bytes = sizeof(DistinctGroup) * (size_t)G, r_bytes = sizeof(int32_t) * (size_t)R;
-  const size_t m_off = (g_bytes + r_bytes + 255) & ~(size_t)255;
-  const size_t m_bytes = nwords > kDistinctSmemWords ? sizeof(unsigned) * (size_t)nwords * R : 0;
-  StagedHost scratch;                                   // groups, row -> group, and (large N) the removal masks
-  scratch.st = st;
-  NOPE_CUDA(cudaMallocAsync(&scratch.dev, m_off + m_bytes, st));
-  char* base = static_cast<char*>(scratch.dev);
-  NOPE_CUDA(cudaMemcpyAsync(base, packed.data(), g_bytes, cudaMemcpyHostToDevice, st));
-  NOPE_CUDA(cudaMemcpyAsync(base + g_bytes, group, r_bytes, cudaMemcpyHostToDevice, st));
-  distinct_topk_kernel<<<R, kDistinctThreads, 0, st>>>(
-      sim, N, rot, G_r, Q, reinterpret_cast<const DistinctGroup*>(base), reinterpret_cast<const int*>(base + g_bytes),
-      k, c_thr, m_bytes ? reinterpret_cast<unsigned*>(base + m_off) : nullptr, reinterpret_cast<long long*>(idx_out),
-      score_out);
+  ScratchArena arena(st);                               // groups, row -> group, and (large N) the removal masks
+  const DistinctGroup* groups_d;
+  const int* group_d;
+  unsigned* masks = nullptr;
+  arena.add(&groups_d, (size_t)G, packed.data());
+  arena.add(&group_d, (size_t)R, group);
+  if (nwords > kDistinctSmemWords) arena.add(&masks, (size_t)nwords * R);
+  if (arena.alloc()) return -1;
+  distinct_topk_kernel<<<R, kDistinctThreads, 0, st>>>(sim, N, rot, G_r, Q, groups_d, group_d, k, c_thr, masks,
+                                                      reinterpret_cast<long long*>(idx_out), score_out);
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1638,11 +1680,10 @@ int nope_vsd_error_taus(const double* depth_test, const float* depth_gt, const f
     NOPE_CHECK(taus[j] > 0.0 && std::isfinite(taus[j]), "every tau must be finite and > 0");
     tv.v[j] = taus[j];
   }
-  if (check_host_intrinsics(K, F)) return -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  StagedHost k;
-  if (k.upload(K, sizeof(double) * 4 * (size_t)F, st)) return -1;
-  const double* kd = static_cast<const double*>(k.dev);
+  ScratchArena arena(st);
+  const double* kd;
+  if (stage_host_intrinsics(arena, &kd, K, F) || arena.alloc()) return -1;
   const dim3 grid(kVsdCluster * P, F);
   if (T == 1)
     vsd_kernel<1><<<grid, kVsdThreads, 0, st>>>(depth_test, depth_gt, depth_est, P, H, W, kd, (float)delta, tv, T,
@@ -1663,51 +1704,64 @@ int nope_pose_errors(const float* points, int V, const double* sym, int S, const
   NOPE_CHECK(V >= 1 && S >= 1 && F >= 1 && P >= 1, "V, S, F and P must be >= 1");
   NOPE_CHECK(F <= 65535 && P <= 65535, "F and P must be <= 65535");
   NOPE_CHECK(S <= (1 << 24), "S must be <= 2^24");
-  if (check_host_intrinsics(K, F)) return -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  StagedHost k;
-  if (k.upload(K, sizeof(double) * 4 * (size_t)F, st)) return -1;
+  ScratchArena arena(st);
+  const double* kd;
+  if (stage_host_intrinsics(arena, &kd, K, F) || arena.alloc()) return -1;
   const int n = F * P;
   auto* om = reinterpret_cast<unsigned long long*>(out_mssd);
   auto* op = reinterpret_cast<unsigned long long*>(out_mspd);
   pose_error_fill_kernel<<<std::min((n + 255) / 256, 1024), 256, 0, st>>>(om, op, n);
   NOPE_CUDA(cudaGetLastError());
   pose_error_kernel<<<dim3((S + kPoseErrSyms - 1) / kPoseErrSyms, P, F), kPoseErrThreads, 0, st>>>(
-      points, V, sym, S, gt, est, static_cast<const double*>(k.dev), P, om, op);
+      points, V, sym, S, gt, est, kd, P, om, op);
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }
 
 // ---------------------------------------------------------------------------------
-// translation from the object mask (translation.cuh, DESIGN.md section 18)
+// pose fits from the frame: translation (translation.cuh, DESIGN.md section 18), depth ICP (depth_refine.cuh,
+// section 19) and contour alignment (contour_refine.cuh, section 20)
 // ---------------------------------------------------------------------------------
+// The arguments the three fits share.  iters_max bounds iters (INT_MAX: no bound).  Null pointers, rho and tau differ
+// between the fits and each launcher checks its own; the host K is checked where it is staged.
+static int check_fit_args(int V, int NF, int F, int P, int H, int W, float znear, int iters, int iters_max) {
+  NOPE_CHECK(V >= 1 && NF >= 1, "V and NF must be >= 1");
+  NOPE_CHECK(F >= 1 && F <= 65535 && P >= 1 && P <= 65535, "F and P must be in [1, 65535]");
+  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
+  NOPE_CHECK(iters >= 0 && iters <= iters_max, "iters must be in [0, iters_max]");
+  NOPE_CHECK(znear > 0.f && std::isfinite(znear), "znear must be finite and > 0");
+  return 0;
+}
+
+// the refinements' rho > 0 and tau [iters + 1] > 0, all finite
+static int check_rho_tau(double rho, const double* tau, int iters) {
+  NOPE_CHECK(std::isfinite(rho) && rho > 0.0, "rho must be finite and > 0");
+  for (int i = 0; i <= iters; ++i) NOPE_CHECK(std::isfinite(tau[i]) && tau[i] > 0.0, "tau must be finite and > 0");
+  return 0;
+}
+
 int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
                          const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
                          float znear, int iters, float* depth, double* t_out, double* iou, int32_t* stats_out,
                          void* stream) {
   NOPE_CHECK(vertices && faces && R && t_init && masks && K && depth && t_out && iou, "null argument");
-  NOPE_CHECK(V >= 1 && NF >= 1, "V and NF must be >= 1");
-  NOPE_CHECK(F >= 1 && F <= 65535 && P >= 1 && P <= 65535, "F and P must be in [1, 65535]");
-  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
-  NOPE_CHECK(iters >= 0, "iters must be >= 0");
-  NOPE_CHECK(znear > 0.f && std::isfinite(znear), "znear must be finite and > 0");
-  if (check_host_intrinsics(K, F)) return -1;
+  if (check_fit_args(V, NF, F, P, H, W, znear, iters, INT_MAX)) return -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  StagedHost k;
-  if (k.upload(K, sizeof(double) * 4 * (size_t)F, st)) return -1;
-  const double* kd = static_cast<const double*>(k.dev);
-  // stream-ordered scratch: the current translations, the float32 poses and the integer statistics
+  // stream-ordered scratch: K, the current translations, the float32 poses and the integer statistics
   const size_t n = (size_t)F * P;
-  StagedHost scratch;
-  const size_t t_bytes = sizeof(double) * 3 * n, pose_bytes = sizeof(float) * 16 * n;
-  const size_t stat_bytes = sizeof(int) * kFitStats * (n + F);
-  scratch.st = st;
-  NOPE_CUDA(cudaMallocAsync(&scratch.dev, t_bytes + pose_bytes + stat_bytes, st));
-  double* t = static_cast<double*>(scratch.dev);
-  float* poses = reinterpret_cast<float*>(static_cast<char*>(scratch.dev) + t_bytes);
-  int* sil_stats = reinterpret_cast<int*>(static_cast<char*>(scratch.dev) + t_bytes + pose_bytes);
-  int* mask_stats = sil_stats + kFitStats * n;
-  const int ew_blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 16);
+  ScratchArena arena(st);
+  const double* kd;
+  double* t;
+  float* poses;
+  int *sil_stats, *mask_stats;
+  if (stage_host_intrinsics(arena, &kd, K, F)) return -1;
+  arena.add(&t, 3 * n);
+  arena.add(&poses, 16 * n);
+  arena.add(&sil_stats, kFitStats * n);
+  arena.add(&mask_stats, kFitStats * (size_t)F);
+  if (arena.alloc()) return -1;
+  const int ew_blocks = ew_grid((long long)n);
   fit_init_kernel<<<ew_blocks, 256, 0, st>>>(R, t_init, F, P, t, poses, sil_stats, mask_stats);
   NOPE_CUDA(cudaGetLastError());
   const long long hw = (long long)H * W;
@@ -1715,19 +1769,8 @@ int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int
   fit_stats_kernel<false><<<dim3(stat_blocks, 1, F), kFitThreads, 0, st>>>(nullptr, masks, P, H, W, mask_stats);
   NOPE_CUDA(cudaGetLastError());
   unsigned* z = reinterpret_cast<unsigned*>(depth);
-  const long long nz = (long long)n * hw;
-  const int fill_blocks = (int)std::min<long long>((nz + 255) / 256, 132LL * 16);
   for (int it = 0; it <= iters; ++it) {
-    // the rasterizer of nope_render_depth, one launch per frame over its P poses (K differs per frame)
-    depth_fill_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);
-    NOPE_CUDA(cudaGetLastError());
-    for (int f = 0; f < F; ++f) {
-      const double* kf = K + 4 * (size_t)f;
-      depth_raster_kernel<<<dim3((NF + 7) / 8, P), 256, 0, st>>>(
-          vertices, V, faces, NF, poses + 16 * (size_t)f * P, (float)kf[0], (float)kf[1], (float)kf[2], (float)kf[3],
-          znear, H, W, z + (size_t)f * P * hw);
-      NOPE_CUDA(cudaGetLastError());
-    }
+    if (render_frames(vertices, V, faces, NF, poses, K, F, P, znear, H, W, z, st)) return -1;
     fit_stats_kernel<true><<<dim3(stat_blocks, P, F), kFitThreads, 0, st>>>(z, masks, P, H, W, sil_stats);
     NOPE_CUDA(cudaGetLastError());
     if (it < iters) {
@@ -1737,45 +1780,33 @@ int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int
   }
   fit_final_kernel<<<ew_blocks, 256, 0, st>>>(t, mask_stats, sil_stats, F, P, t_out, iou, stats_out);
   NOPE_CUDA(cudaGetLastError());
-  depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);      // depth holds render_depth at the returned t
-  NOPE_CUDA(cudaGetLastError());
-  return 0;
+  return launch_depth_finish(z, (long long)n * hw, st);      // depth holds render_depth at the returned t
 }
 
-// ---------------------------------------------------------------------------------
-// pose refinement from the sensor depth (depth_refine.cuh, DESIGN.md section 19)
-// ---------------------------------------------------------------------------------
 int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF, const double* R, const double* t_init,
                       const double* depth_sensor, const uint8_t* masks, const double* K, int F, int P, int H, int W,
                       double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
                       double* t_out, double* fit_out, int64_t* sums_out, void* stream) {
   NOPE_CHECK(vertices && faces && R && t_init && depth_sensor && K && tau && depth && R_out && t_out && fit_out,
              "null argument");
-  NOPE_CHECK(V >= 1 && NF >= 1, "V and NF must be >= 1");
-  NOPE_CHECK(F >= 1 && F <= 65535 && P >= 1 && P <= 65535, "F and P must be in [1, 65535]");
-  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
-  NOPE_CHECK(iters >= 0 && iters <= 1024, "iters must be in [0, 1024]");
-  NOPE_CHECK(std::isfinite(rho) && rho > 0.0, "rho must be finite and > 0");
-  NOPE_CHECK(znear > 0.f && std::isfinite(znear), "znear must be finite and > 0");
-  for (int i = 0; i <= iters; ++i) NOPE_CHECK(std::isfinite(tau[i]) && tau[i] > 0.0, "tau must be finite and > 0");
-  if (check_host_intrinsics(K, F)) return -1;
+  if (check_fit_args(V, NF, F, P, H, W, znear, iters, 1024) || check_rho_tau(rho, tau, iters)) return -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // one stream-ordered block: K, the current R and t, the integer sums, the float32 poses and n_valid
+  // stream-ordered scratch: K, the current R and t, the integer sums, the float32 poses and n_valid
   const size_t n = (size_t)F * P;
-  const size_t k_bytes = sizeof(double) * 4 * F, R_bytes = sizeof(double) * 9 * n, t_bytes = sizeof(double) * 3 * n;
-  const size_t sum_bytes = sizeof(unsigned long long) * kIcpSums * n, pose_bytes = sizeof(float) * 16 * n;
-  StagedHost scratch;
-  scratch.st = st;
-  NOPE_CUDA(cudaMallocAsync(&scratch.dev, k_bytes + R_bytes + t_bytes + sum_bytes + pose_bytes + sizeof(int) * F, st));
-  char* base = static_cast<char*>(scratch.dev);
-  double* kd = reinterpret_cast<double*>(base);
-  double* Rc = reinterpret_cast<double*>(base + k_bytes);
-  double* tc = reinterpret_cast<double*>(base + k_bytes + R_bytes);
-  auto* sums = reinterpret_cast<unsigned long long*>(base + k_bytes + R_bytes + t_bytes);
-  float* poses = reinterpret_cast<float*>(base + k_bytes + R_bytes + t_bytes + sum_bytes);
-  int* n_valid = reinterpret_cast<int*>(base + k_bytes + R_bytes + t_bytes + sum_bytes + pose_bytes);
-  NOPE_CUDA(cudaMemcpyAsync(kd, K, k_bytes, cudaMemcpyHostToDevice, st));
-  const int ew_blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 16);
+  ScratchArena arena(st);
+  const double* kd;
+  double *Rc, *tc;
+  unsigned long long* sums;
+  float* poses;
+  int* n_valid;
+  if (stage_host_intrinsics(arena, &kd, K, F)) return -1;
+  arena.add(&Rc, 9 * n);
+  arena.add(&tc, 3 * n);
+  arena.add(&sums, kIcpSums * n);
+  arena.add(&poses, 16 * n);
+  arena.add(&n_valid, (size_t)F);
+  if (arena.alloc()) return -1;
+  const int ew_blocks = ew_grid((long long)n);
   icp_init_kernel<<<ew_blocks, 256, 0, st>>>(R, t_init, F, P, Rc, tc, poses, sums, n_valid);
   NOPE_CUDA(cudaGetLastError());
   const long long hw = (long long)H * W;
@@ -1783,19 +1814,8 @@ int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF
   icp_valid_kernel<<<dim3(px_blocks, 1, F), kIcpThreads, 0, st>>>(depth_sensor, masks, H, W, n_valid);
   NOPE_CUDA(cudaGetLastError());
   unsigned* z = reinterpret_cast<unsigned*>(depth);
-  const long long nz = (long long)n * hw;
-  const int fill_blocks = (int)std::min<long long>((nz + 255) / 256, 132LL * 16);
   for (int it = 0; it <= iters; ++it) {
-    // the rasterizer of nope_render_depth, one launch per frame over its P poses (K differs per frame)
-    depth_fill_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);
-    NOPE_CUDA(cudaGetLastError());
-    for (int f = 0; f < F; ++f) {
-      const double* kf = K + 4 * (size_t)f;
-      depth_raster_kernel<<<dim3((NF + 7) / 8, P), 256, 0, st>>>(
-          vertices, V, faces, NF, poses + 16 * (size_t)f * P, (float)kf[0], (float)kf[1], (float)kf[2], (float)kf[3],
-          znear, H, W, z + (size_t)f * P * hw);
-      NOPE_CUDA(cudaGetLastError());
-    }
+    if (render_frames(vertices, V, faces, NF, poses, K, F, P, znear, H, W, z, st)) return -1;
     icp_accumulate_kernel<<<dim3(px_blocks, P, F), kIcpThreads, 0, st>>>(z, depth_sensor, masks, kd, tc, P, H, W,
                                                                          tau[it], rho, sums);
     NOPE_CUDA(cudaGetLastError());
@@ -1807,14 +1827,9 @@ int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF
   icp_final_kernel<<<ew_blocks, 256, 0, st>>>(Rc, tc, sums, n_valid, F, P, tau[iters], R_out, t_out, fit_out,
                                               reinterpret_cast<long long*>(sums_out));
   NOPE_CUDA(cudaGetLastError());
-  depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);      // depth holds render_depth at the returned pose
-  NOPE_CUDA(cudaGetLastError());
-  return 0;
+  return launch_depth_finish(z, (long long)n * hw, st);      // depth holds render_depth at the returned pose
 }
 
-// ---------------------------------------------------------------------------------
-// pose refinement from the object mask's contour (contour_refine.cuh, DESIGN.md section 20)
-// ---------------------------------------------------------------------------------
 // phi [F, H, W] of masks [F, H, W] through the column pass into g [F, H, W] and the row pass
 static int launch_mask_sdf(const uint8_t* masks, int F, int H, int W, unsigned* g, double* phi, cudaStream_t st) {
   mask_sdf_cols_kernel<<<dim3((W + kSdfColThreads - 1) / kSdfColThreads, F), kSdfColThreads, 0, st>>>(masks, H, W, g);
@@ -1830,10 +1845,11 @@ int nope_mask_sdf(const uint8_t* masks, int F, int H, int W, double* sdf_out, vo
   NOPE_CHECK(F >= 1 && F <= 65535, "F must be in [1, 65535]");
   NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  StagedHost scratch;                                           // the column pass's distances, freed in stream order
-  scratch.st = st;
-  NOPE_CUDA(cudaMallocAsync(&scratch.dev, sizeof(unsigned) * (size_t)F * H * W, st));
-  return launch_mask_sdf(masks, F, H, W, static_cast<unsigned*>(scratch.dev), sdf_out, st);
+  ScratchArena arena(st);                                       // the column pass's distances
+  unsigned* g;
+  arena.add(&g, (size_t)F * H * W);
+  if (arena.alloc()) return -1;
+  return launch_mask_sdf(masks, F, H, W, g, sdf_out, st);
 }
 
 int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
@@ -1842,39 +1858,30 @@ int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int 
                         double* t_out, double* fit_out, int64_t* sums_out, void* stream) {
   NOPE_CHECK(vertices && faces && R && t_init && masks && K && tau && depth && R_out && t_out && fit_out,
              "null argument");
-  NOPE_CHECK(V >= 1 && NF >= 1, "V and NF must be >= 1");
-  NOPE_CHECK(F >= 1 && F <= 65535 && P >= 1 && P <= 65535, "F and P must be in [1, 65535]");
-  NOPE_CHECK(H >= 1 && H <= kRenderMaxSide && W >= 1 && W <= kRenderMaxSide, "H and W must be in [1, 8192]");
-  NOPE_CHECK(iters >= 0 && iters <= 1024, "iters must be in [0, 1024]");
-  NOPE_CHECK(std::isfinite(rho) && rho > 0.0, "rho must be finite and > 0");
-  NOPE_CHECK(znear > 0.f && std::isfinite(znear), "znear must be finite and > 0");
-  for (int i = 0; i <= iters; ++i) NOPE_CHECK(std::isfinite(tau[i]) && tau[i] > 0.0, "tau must be finite and > 0");
-  if (check_host_intrinsics(K, F)) return -1;
+  if (check_fit_args(V, NF, F, P, H, W, znear, iters, 1024) || check_rho_tau(rho, tau, iters)) return -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // one stream-ordered block: K, the current R and t, the integer sums, phi (8-byte fields first), then the float32
-  // poses, the column pass's distances, the mask and silhouette statistics and n_contour
+  // stream-ordered scratch: K, the current R and t, the integer sums, phi, the float32 poses, the column pass's
+  // distances, the silhouette and mask statistics and n_contour
   const size_t n = (size_t)F * P, fhw = (size_t)F * H * W;
-  const size_t k_bytes = sizeof(double) * 4 * F, R_bytes = sizeof(double) * 9 * n, t_bytes = sizeof(double) * 3 * n;
-  const size_t sum_bytes = sizeof(unsigned long long) * kIcpSums * n, phi_bytes = sizeof(double) * fhw;
-  const size_t pose_bytes = sizeof(float) * 16 * n, g_bytes = sizeof(unsigned) * fhw;
-  const size_t stat_bytes = sizeof(int) * kFitStats * (n + F), nc_bytes = sizeof(int) * n;
-  StagedHost scratch;
-  scratch.st = st;
-  NOPE_CUDA(cudaMallocAsync(&scratch.dev, k_bytes + R_bytes + t_bytes + sum_bytes + phi_bytes + pose_bytes + g_bytes +
-                                              stat_bytes + nc_bytes, st));
-  char* p = static_cast<char*>(scratch.dev);
-  double* kd = reinterpret_cast<double*>(p);                      p += k_bytes;
-  double* Rc = reinterpret_cast<double*>(p);                      p += R_bytes;
-  double* tc = reinterpret_cast<double*>(p);                      p += t_bytes;
-  auto* sums = reinterpret_cast<unsigned long long*>(p);          p += sum_bytes;
-  double* phi = reinterpret_cast<double*>(p);                     p += phi_bytes;
-  float* poses = reinterpret_cast<float*>(p);                     p += pose_bytes;
-  unsigned* g = reinterpret_cast<unsigned*>(p);                   p += g_bytes;
-  int* sil_stats = reinterpret_cast<int*>(p);
-  int* mask_stats = sil_stats + kFitStats * n;
-  int* n_contour = mask_stats + kFitStats * F;
-  NOPE_CUDA(cudaMemcpyAsync(kd, K, k_bytes, cudaMemcpyHostToDevice, st));
-  const int ew_blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 16);
+  ScratchArena arena(st);
+  const double* kd;
+  double *Rc, *tc, *phi;
+  unsigned long long* sums;
+  float* poses;
+  unsigned* g;
+  int *sil_stats, *mask_stats, *n_contour;
+  if (stage_host_intrinsics(arena, &kd, K, F)) return -1;
+  arena.add(&Rc, 9 * n);
+  arena.add(&tc, 3 * n);
+  arena.add(&sums, kIcpSums * n);
+  arena.add(&phi, fhw);
+  arena.add(&poses, 16 * n);
+  arena.add(&g, fhw);
+  arena.add(&sil_stats, kFitStats * n);
+  arena.add(&mask_stats, kFitStats * (size_t)F);
+  arena.add(&n_contour, n);
+  if (arena.alloc()) return -1;
+  const int ew_blocks = ew_grid((long long)n);
   contour_init_kernel<<<ew_blocks, 256, 0, st>>>(R, t_init, F, P, Rc, tc, poses, sums, n_contour, sil_stats,
                                                  mask_stats);
   NOPE_CUDA(cudaGetLastError());
@@ -1885,19 +1892,8 @@ int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int 
   NOPE_CUDA(cudaGetLastError());
   if (launch_mask_sdf(masks, F, H, W, g, phi, st)) return -1;
   unsigned* z = reinterpret_cast<unsigned*>(depth);
-  const long long nz = (long long)n * hw;
-  const int fill_blocks = (int)std::min<long long>((nz + 255) / 256, 132LL * 16);
   for (int it = 0; it <= iters; ++it) {
-    // the rasterizer of nope_render_depth, one launch per frame over its P poses (K differs per frame)
-    depth_fill_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);
-    NOPE_CUDA(cudaGetLastError());
-    for (int f = 0; f < F; ++f) {
-      const double* kf = K + 4 * (size_t)f;
-      depth_raster_kernel<<<dim3((NF + 7) / 8, P), 256, 0, st>>>(
-          vertices, V, faces, NF, poses + 16 * (size_t)f * P, (float)kf[0], (float)kf[1], (float)kf[2], (float)kf[3],
-          znear, H, W, z + (size_t)f * P * hw);
-      NOPE_CUDA(cudaGetLastError());
-    }
+    if (render_frames(vertices, V, faces, NF, poses, K, F, P, znear, H, W, z, st)) return -1;
     contour_accumulate_kernel<<<dim3(px_blocks, P, F), kIcpThreads, 0, st>>>(z, phi, kd, tc, mask_stats, P, H, W,
                                                                              tau[it], rho, sums, n_contour);
     NOPE_CUDA(cudaGetLastError());
@@ -1913,9 +1909,7 @@ int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int 
                                                   tau[iters], R_out, t_out, fit_out,
                                                   reinterpret_cast<long long*>(sums_out));
   NOPE_CUDA(cudaGetLastError());
-  depth_finish_kernel<<<fill_blocks, 256, 0, st>>>(z, nz);      // depth holds render_depth at the returned pose
-  NOPE_CUDA(cudaGetLastError());
-  return 0;
+  return launch_depth_finish(z, (long long)n * hw, st);      // depth holds render_depth at the returned pose
 }
 
 // ---------------------------------------------------------------------------------

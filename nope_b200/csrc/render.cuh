@@ -37,6 +37,17 @@ __global__ void depth_finish_kernel(unsigned* __restrict__ z, long long n) {
     if (z[i] == kDepthInfBits) z[i] = 0u;
 }
 
+// the rasterizer's pose: [R | t] (float64, R row-major 3x3) rounded to float32, row-major 4x4
+__device__ __forceinline__ void render_write_pose(const double* R, const double* t, float* __restrict__ pose) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) pose[4 * r + c] = __double2float_rn(R[3 * r + c]);
+    pose[4 * r + 3] = __double2float_rn(t[r]);
+  }
+  pose[12] = 0.f; pose[13] = 0.f; pose[14] = 0.f; pose[15] = 1.f;
+}
+
 struct RVert {
   float z;      // camera Z
   int x, y;     // fixed-point image position, 8 sub-pixel bits

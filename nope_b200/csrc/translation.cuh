@@ -72,17 +72,6 @@ fit_stats_kernel(const unsigned* __restrict__ z, const uint8_t* __restrict__ mas
   atomicMin(s + 2, r0); atomicMax(s + 3, r1); atomicMin(s + 4, c0); atomicMax(s + 5, c1);
 }
 
-// the rasterizer's pose: [R | t] rounded to float32, row-major 4x4
-__device__ __forceinline__ void fit_write_pose(const double* __restrict__ R, const double* t, float* __restrict__ pose) {
-#pragma unroll
-  for (int r = 0; r < 3; ++r) {
-#pragma unroll
-    for (int c = 0; c < 3; ++c) pose[4 * r + c] = __double2float_rn(R[3 * r + c]);
-    pose[4 * r + 3] = __double2float_rn(t[r]);
-  }
-  pose[12] = 0.f; pose[13] = 0.f; pose[14] = 0.f; pose[15] = 1.f;
-}
-
 // box centre (lo + hi + 1) / 2 and size hi - lo + 1 of an integer pixel range, exact in float64
 __device__ __forceinline__ double fit_centre(int lo, int hi) { return __dmul_rn((double)(lo + hi + 1), 0.5); }
 __device__ __forceinline__ double fit_size(int lo, int hi) { return (double)(hi - lo + 1); }
@@ -96,7 +85,7 @@ __global__ void fit_init_kernel(const double* __restrict__ R, const double* __re
     double ti[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) { ti[k] = t_init[3 * i + k]; t[3 * i + k] = ti[k]; }
-    fit_write_pose(R + 9 * i, ti, poses + 16 * i);
+    render_write_pose(R + 9 * i, ti, poses + 16 * i);
     fit_stats_reset(sil_stats + kFitStats * i);
     if (i < F) fit_stats_reset(mask_stats + kFitStats * i);
   }
@@ -133,7 +122,7 @@ __global__ void fit_update_kernel(const double* __restrict__ R, const double* __
 #pragma unroll
       for (int c = 0; c < 3; ++c) t[3 * i + c] = ti[c];
     }
-    fit_write_pose(R + 9 * i, ti, poses + 16 * i);
+    render_write_pose(R + 9 * i, ti, poses + 16 * i);
     fit_stats_reset(ss);
   }
 }

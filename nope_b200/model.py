@@ -561,6 +561,52 @@ class PoseConditional:
         R = torch.where((rows >= 0)[..., None, None], R, torch.zeros((), dtype=R.dtype, device=R.device))
         return R.reshape(idx.shape + (3, 3)), idx, score
 
+    def _pose_fit_batch(self, name, batch, keys, R, t=None, masks=None, models_info=True):
+        """The arguments of a pose fit on a T-LESS batch, checked: the batch's `keys`, R [B, k, 3, 3], t [B, k, 3] and
+        masks [B, H, W] when given, and a mesh (with models_info, also a models_info entry) for every object.
+        -> (ids, R, t, masks, K float64 [B, 3, 3] on the host); errors name the fit."""
+        from ._posefit import _tensor
+        for key in keys:
+            if key not in batch:
+                raise KeyError(f"{name}: the batch has no {key!r}")
+        ids = [int(i) for i in batch["obj_id"].reshape(-1).tolist()]
+        B = len(ids)
+        R = _tensor(R)
+        if R.dim() != 4 or R.shape[0] != B or R.shape[2:] != (3, 3) or R.shape[1] < 1:
+            raise ValueError(f"{name}: R [B, k, 3, 3] with B = {B} expected, got {tuple(R.shape)}")
+        k = R.shape[1]
+        if t is not None:
+            t = _tensor(t)
+            if tuple(t.shape) != (B, k, 3):
+                raise ValueError(f"{name}: t [{B}, {k}, 3] expected, got {tuple(t.shape)}")
+        if masks is not None:
+            masks = _tensor(masks)
+            if masks.dim() != 3 or masks.shape[0] != B:
+                raise ValueError(f"{name}: masks [B, H, W] with B = {B} expected, got {tuple(masks.shape)}")
+        missing = sorted(set(i for i in ids if i not in self.tless_cad or (models_info and i not in self.bop_models)))
+        if missing:
+            raise ValueError(f"{name}: no mesh or models_info entry for obj_id {missing} (load_mesh, load_models_info)"
+                             if models_info else f"{name}: no mesh for obj_id {missing} (load_mesh)")
+        K = batch["intrinsic"].detach().cpu().to(torch.float64).reshape(B, 3, 3)
+        return ids, R, t, masks, K
+
+    def _object_rows(self, ids):
+        """The rows of a batch split by object: yields (obj, ri, rd, pick) for every distinct obj_id in ascending
+        order, with the object's row indices ri on the host and rd on the model's device, and pick(x) x's rows (by rd
+        for a CUDA tensor, by ri otherwise; None stays None)."""
+        for obj in sorted(set(ids)):
+            ri = torch.tensor([b for b, i in enumerate(ids) if i == obj], dtype=torch.int64)
+            rd = ri.pin_memory().to(self.device, non_blocking=True)
+            yield obj, ri, rd, lambda x, ri=ri, rd=rd: None if x is None else x[rd if x.device.type == "cuda" else ri]
+
+    @staticmethod
+    def _rerank(score, *xs):
+        """each row of score [B, k] and of every x [B, k, ...] sorted by descending score (stable, NaN last):
+        -> (*xs, score)"""
+        order = torch.sort(-score, dim=1, stable=True).indices                     # NaN sorts last
+        rows = torch.arange(score.shape[0], device=score.device)[:, None]
+        return tuple(x[rows, order] for x in xs) + (score[rows, order],)
+
     @torch.no_grad()
     def estimate_translation(self, batch, R, masks, iters=4):
         """The translation of every rotation hypothesis R [B, k, 3, 3] of a T-LESS batch (the `eval_vsd` schema; its
@@ -568,34 +614,16 @@ class PoseConditional:
         nonzero = object), starting from `translation.initial_translation` with the object's diameter
         (load_models_info) and the mesh of load_mesh; DESIGN.md section 18.  One call per distinct object.
         -> (t float64 [B, k, 3] mm, iou float64 [B, k]) on the model's device, without synchronising."""
-        import numpy as np
         from . import translation
-        for key in ("intrinsic", "obj_id"):
-            if key not in batch:
-                raise KeyError(f"estimate_translation: the batch has no {key!r}")
-        ids = [int(i) for i in batch["obj_id"].reshape(-1).tolist()]
-        B = len(ids)
-        R = torch.as_tensor(np.asarray(R) if not torch.is_tensor(R) else R)
-        if R.dim() != 4 or R.shape[0] != B or R.shape[2:] != (3, 3) or R.shape[1] < 1:
-            raise ValueError(f"estimate_translation: R [B, k, 3, 3] with B = {B} expected, got {tuple(R.shape)}")
-        masks = torch.as_tensor(np.asarray(masks) if not torch.is_tensor(masks) else masks)
-        if masks.dim() != 3 or masks.shape[0] != B:
-            raise ValueError(f"estimate_translation: masks [B, H, W] with B = {B} expected, got {tuple(masks.shape)}")
-        missing = sorted(set(i for i in ids if i not in self.tless_cad or i not in self.bop_models))
-        if missing:
-            raise ValueError(f"estimate_translation: no mesh or models_info entry for obj_id {missing} "
-                             "(load_mesh, load_models_info)")
-        K = batch["intrinsic"].detach().cpu().to(torch.float64).reshape(B, 3, 3)
-        dev = self.device
-        t = torch.empty((B, R.shape[1], 3), device=dev, dtype=torch.float64)
-        iou = torch.empty((B, R.shape[1]), device=dev, dtype=torch.float64)
-        for obj in sorted(set(ids)):
-            ri = torch.tensor([b for b in range(B) if ids[b] == obj], dtype=torch.int64)
-            rd = ri.pin_memory().to(dev, non_blocking=True)
-            rm = rd if masks.device.type == "cuda" else ri
-            rr = rd if R.device.type == "cuda" else ri
+        ids, R, _, masks, K = self._pose_fit_batch("estimate_translation", batch, ("intrinsic", "obj_id"), R,
+                                                   masks=masks)
+        B, k = R.shape[:2]
+        t = torch.empty((B, k, 3), device=self.device, dtype=torch.float64)
+        iou = torch.empty((B, k), device=self.device, dtype=torch.float64)
+        for obj, ri, rd, pick in self._object_rows(ids):
             t[rd], iou[rd] = translation.estimate_translation(
-                self.tless_cad[obj], R[rr], K[ri], masks[rm], diameter=self.bop_models[obj]["diameter"], iters=iters)
+                self.tless_cad[obj], pick(R), K[ri], pick(masks), diameter=self.bop_models[obj]["diameter"],
+                iters=iters)
         return t, iou
 
     @torch.no_grad()
@@ -609,50 +637,23 @@ class PoseConditional:
         t float64 [B, k, 3], score float64 [B, k]) on the model's device, score = the share of the mask's sensor
         pixels explained by the refined pose (NaN for a frame without readings); with rerank, each row's hypotheses
         sorted by descending score (stable, NaN last).  The output feeds eval_bop(R_est=R, t_est=t)."""
-        import numpy as np
         from . import depth_refine
         iters = depth_refine.DEFAULT_ITERS if iters is None else iters
-        for key in ("intrinsic", "obj_id", "depth_path"):
-            if key not in batch:
-                raise KeyError(f"refine_depth: the batch has no {key!r}")
-        ids = [int(i) for i in batch["obj_id"].reshape(-1).tolist()]
-        B = len(ids)
-        R = torch.as_tensor(np.asarray(R) if not torch.is_tensor(R) else R)
-        if R.dim() != 4 or R.shape[0] != B or R.shape[2:] != (3, 3) or R.shape[1] < 1:
-            raise ValueError(f"refine_depth: R [B, k, 3, 3] with B = {B} expected, got {tuple(R.shape)}")
-        k = R.shape[1]
-        t = torch.as_tensor(np.asarray(t) if not torch.is_tensor(t) else t)
-        if tuple(t.shape) != (B, k, 3):
-            raise ValueError(f"refine_depth: t [{B}, {k}, 3] expected, got {tuple(t.shape)}")
-        if masks is not None:
-            masks = torch.as_tensor(np.asarray(masks) if not torch.is_tensor(masks) else masks)
-            if masks.dim() != 3 or masks.shape[0] != B:
-                raise ValueError(f"refine_depth: masks [B, H, W] with B = {B} expected, got {tuple(masks.shape)}")
+        ids, R, t, masks, K = self._pose_fit_batch("refine_depth", batch, ("intrinsic", "obj_id", "depth_path"), R, t,
+                                                   masks)
+        B, k = R.shape[:2]
         if len(batch["depth_path"]) != B:
             raise ValueError(f"refine_depth: {B} depth_path entries expected, got {len(batch['depth_path'])}")
-        missing = sorted(set(i for i in ids if i not in self.tless_cad or i not in self.bop_models))
-        if missing:
-            raise ValueError(f"refine_depth: no mesh or models_info entry for obj_id {missing} "
-                             "(load_mesh, load_models_info)")
-        K = batch["intrinsic"].detach().cpu().to(torch.float64).reshape(B, 3, 3)
         depth = self._read_sensor_depth(batch)
-        dev = self.device
-        R_out = torch.empty((B, k, 3, 3), device=dev, dtype=torch.float64)
-        t_out = torch.empty((B, k, 3), device=dev, dtype=torch.float64)
-        score = torch.empty((B, k), device=dev, dtype=torch.float64)
-        for obj in sorted(set(ids)):
-            ri = torch.tensor([b for b in range(B) if ids[b] == obj], dtype=torch.int64)
-            rd = ri.pin_memory().to(dev, non_blocking=True)
-            pick = lambda x: None if x is None else x[rd if x.device.type == "cuda" else ri]   # noqa: E731
+        R_out = torch.empty((B, k, 3, 3), device=self.device, dtype=torch.float64)
+        t_out = torch.empty((B, k, 3), device=self.device, dtype=torch.float64)
+        score = torch.empty((B, k), device=self.device, dtype=torch.float64)
+        for obj, ri, rd, pick in self._object_rows(ids):
             tau = depth_refine.default_tau(self.bop_models[obj]["diameter"], iters)
             R_out[rd], t_out[rd], fit = depth_refine.refine_pose_depth(
                 self.tless_cad[obj], pick(R), pick(t), K[ri], depth[ri], masks=pick(masks), iters=iters, tau=tau)
             score[rd] = fit["score"]
-        if rerank:
-            order = torch.sort(-score, dim=1, stable=True).indices                     # NaN sorts last
-            rows = torch.arange(B, device=dev)[:, None]
-            R_out, t_out, score = R_out[rows, order], t_out[rows, order], score[rows, order]
-        return R_out, t_out, score
+        return self._rerank(score, R_out, t_out) if rerank else (R_out, t_out, score)
 
     @torch.no_grad()
     def refine_contour(self, batch, R, t, masks, iters=None, rerank=False):
@@ -665,44 +666,19 @@ class PoseConditional:
         device, iou = the refined pose's silhouette IoU with the mask (NaN for a frame whose mask is empty or full);
         with rerank, each row's hypotheses sorted by descending IoU (stable, NaN last).  The output feeds
         eval_bop(R_est=R, t_est=t); refine_depth can follow when the frame has depth."""
-        import numpy as np
         from . import contour_refine
         iters = contour_refine.DEFAULT_ITERS if iters is None else iters
-        for key in ("intrinsic", "obj_id"):
-            if key not in batch:
-                raise KeyError(f"refine_contour: the batch has no {key!r}")
-        ids = [int(i) for i in batch["obj_id"].reshape(-1).tolist()]
-        B = len(ids)
-        R = torch.as_tensor(np.asarray(R) if not torch.is_tensor(R) else R)
-        if R.dim() != 4 or R.shape[0] != B or R.shape[2:] != (3, 3) or R.shape[1] < 1:
-            raise ValueError(f"refine_contour: R [B, k, 3, 3] with B = {B} expected, got {tuple(R.shape)}")
-        k = R.shape[1]
-        t = torch.as_tensor(np.asarray(t) if not torch.is_tensor(t) else t)
-        if tuple(t.shape) != (B, k, 3):
-            raise ValueError(f"refine_contour: t [{B}, {k}, 3] expected, got {tuple(t.shape)}")
-        masks = torch.as_tensor(np.asarray(masks) if not torch.is_tensor(masks) else masks)
-        if masks.dim() != 3 or masks.shape[0] != B:
-            raise ValueError(f"refine_contour: masks [B, H, W] with B = {B} expected, got {tuple(masks.shape)}")
-        missing = sorted(set(i for i in ids if i not in self.tless_cad))
-        if missing:
-            raise ValueError(f"refine_contour: no mesh for obj_id {missing} (load_mesh)")
-        K = batch["intrinsic"].detach().cpu().to(torch.float64).reshape(B, 3, 3)
-        dev = self.device
-        R_out = torch.empty((B, k, 3, 3), device=dev, dtype=torch.float64)
-        t_out = torch.empty((B, k, 3), device=dev, dtype=torch.float64)
-        iou = torch.empty((B, k), device=dev, dtype=torch.float64)
-        for obj in sorted(set(ids)):
-            ri = torch.tensor([b for b in range(B) if ids[b] == obj], dtype=torch.int64)
-            rd = ri.pin_memory().to(dev, non_blocking=True)
-            pick = lambda x: x[rd if x.device.type == "cuda" else ri]   # noqa: E731
+        ids, R, t, masks, K = self._pose_fit_batch("refine_contour", batch, ("intrinsic", "obj_id"), R, t, masks,
+                                                   models_info=False)
+        B, k = R.shape[:2]
+        R_out = torch.empty((B, k, 3, 3), device=self.device, dtype=torch.float64)
+        t_out = torch.empty((B, k, 3), device=self.device, dtype=torch.float64)
+        iou = torch.empty((B, k), device=self.device, dtype=torch.float64)
+        for obj, ri, rd, pick in self._object_rows(ids):
             R_out[rd], t_out[rd], fit = contour_refine.refine_pose_contour(
                 self.tless_cad[obj], pick(R), pick(t), K[ri], pick(masks), iters=iters)
             iou[rd] = fit["iou"]
-        if rerank:
-            order = torch.sort(-iou, dim=1, stable=True).indices                     # NaN sorts last
-            rows = torch.arange(B, device=dev)[:, None]
-            R_out, t_out, iou = R_out[rows, order], t_out[rows, order], iou[rows, order]
-        return R_out, t_out, iou
+        return self._rerank(iou, R_out, t_out) if rerank else (R_out, t_out, iou)
 
     @torch.no_grad()
     def eval_bop(self, batch, data_name, R_est=None, save_path=None, t_est=None):
@@ -745,10 +721,7 @@ class PoseConditional:
         gt = gt.pin_memory().to(dev, non_blocking=True) if gt.device.type == "cpu" else gt.to(dev)
         R_gt, t_gt = gt[:, :, :3], gt[:, :, 3]
         diameter = np.array([self.bop_models[i]["diameter"] for i in ids])
-        for obj in sorted(set(ids)):
-            rows = [b for b in range(B) if ids[b] == obj]
-            ri = torch.tensor(rows, dtype=torch.int64)
-            rd = ri.pin_memory().to(dev, non_blocking=True)
+        for obj, ri, rd, _ in self._object_rows(ids):
             info = self.bop_models[obj]
             vsd[rd] = _vsd.vsd_errors(depth_test[rd], rendered[rd, 0], rendered[rd, 1:], K[ri],
                                       tau=bop.VSD_TAUS * info["diameter"])

@@ -11,30 +11,16 @@ import numpy as np
 import torch
 
 from . import _lib
-from .bop import _host_k, _to_dev
-from .vsd import MAX_SIDE, Mesh, _stream
+from ._posefit import _masks, _tensor, broadcast_t, cuda_device, fit_args, workspace
+from .bop import _to_dev
+from .vsd import _stream
 
 DEFAULT_ITERS = 4            # from the convergence table of DESIGN.md section 18
-MAX_BATCH = 65535            # F and P
-
-
-def _masks(masks):
-    m = torch.as_tensor(np.asarray(masks) if not torch.is_tensor(masks) else masks)
-    if m.dim() == 2:
-        m = m[None]
-    if m.dim() != 3 or m.shape[0] < 1:
-        raise ValueError(f"masks [F, H, W] expected, got {tuple(m.shape)}")
-    if m.dtype not in (torch.uint8, torch.bool):
-        raise ValueError(f"masks must be uint8 or bool, got {m.dtype}")
-    H, W = m.shape[1:]
-    if not (1 <= H <= MAX_SIDE and 1 <= W <= MAX_SIDE):
-        raise ValueError(f"H and W must be in [1, {MAX_SIDE}], got {(H, W)}")
-    return m
 
 
 def _k4(K, F, device):
     """K [F, 3, 3], [F, 4], [3, 3] or [4] -> float64 [F, 4] (fx, fy, cx, cy) on `device`, without synchronising"""
-    k = torch.as_tensor(np.asarray(K) if not torch.is_tensor(K) else K)
+    k = _tensor(K)
     if k.shape in ((3, 3), (4,)):
         k = k[None]
     if k.dim() == 3 and k.shape[1:] == (3, 3):
@@ -78,7 +64,7 @@ def initial_translation(masks, K, diameter):
     dev = n.device
     F = n.shape[0]
     k = _k4(K, F, dev)
-    d = torch.as_tensor(np.asarray(diameter) if not torch.is_tensor(diameter) else diameter).to(torch.float64)
+    d = _tensor(diameter).to(torch.float64)
     if d.dim() > 1 or (d.dim() == 1 and d.shape[0] not in (1, F)):
         raise ValueError(f"diameter: a number or [F] with F = {F} expected, got {tuple(d.shape)}")
     d = _to_dev(d, dev, torch.float64).expand(F)                  # a host number: pinned, no synchronisation
@@ -105,47 +91,24 @@ def estimate_translation(mesh, R, K, masks, t_init=None, diameter=None, iters=DE
     (0 for an empty silhouette); NaN for both where the frame's mask is empty.  With return_stats, also int32
     [F, P, 6]: n_S, |S n M| and the silhouette's box (row0, row1, col0, col1) at the returned t.  Runs on the mesh's
     device and current stream without synchronising."""
-    if not isinstance(mesh, Mesh):
-        raise ValueError("mesh must be a nope_b200.vsd.Mesh")
-    dev = mesh.device
-    if dev.type != "cuda":
-        raise _lib.NopeError("estimate_translation needs a CUDA mesh (no CPU fallback)")
-    R = torch.as_tensor(np.asarray(R) if not torch.is_tensor(R) else R)
-    if R.dim() == 3:
-        R = R[:, None]
-    if R.dim() != 4 or R.shape[2:] != (3, 3) or R.shape[0] < 1 or R.shape[1] < 1:
-        raise ValueError(f"R [F, P, 3, 3] or [F, 3, 3] expected, got {tuple(R.shape)}")
-    if R.dtype not in (torch.float32, torch.float64):
-        raise ValueError(f"R must be float32 or float64, got {R.dtype}")
-    F_, P = R.shape[:2]
-    if F_ > MAX_BATCH or P > MAX_BATCH:
-        raise ValueError(f"F and P must be <= {MAX_BATCH}, got {(F_, P)}")
+    dev = cuda_device(mesh, "estimate_translation")
+    R, t_init, k, F_, P, iters = fit_args(mesh, R, t_init, K, iters, znear, t_name="t_init")
     m = _masks(masks)
     if m.shape[0] != F_:
         raise ValueError(f"masks for {F_} frames expected, got {tuple(m.shape)}")
     H, W = m.shape[1:]
-    if isinstance(iters, bool) or int(iters) != iters or iters < 0:
-        raise ValueError(f"iters must be an integer >= 0, got {iters!r}")
-    if not (np.isfinite(znear) and znear > 0):
-        raise ValueError(f"znear must be finite and > 0, got {znear}")
-    k = _host_k(K, F_)
     if t_init is None and diameter is None:
         raise ValueError("estimate_translation needs t_init or the object diameter")
-    if t_init is not None:
-        t0 = torch.as_tensor(np.asarray(t_init) if not torch.is_tensor(t_init) else t_init)
-        if t0.shape not in ((F_, 3), (F_, P, 3)):
-            raise ValueError(f"t_init [{F_}, 3] or [{F_}, {P}, 3] expected, got {tuple(t0.shape)}")
     with torch.cuda.device(dev):
         m = _to_dev(m, dev, torch.uint8)
-        t0 = initial_translation(m, k, diameter) if t_init is None else _to_dev(t0, dev, torch.float64)
-        t0 = t0[:, None].expand(F_, P, 3).contiguous() if t0.dim() == 2 else t0.contiguous()
+        t0 = broadcast_t(initial_translation(m, k, diameter) if t_init is None else t_init, F_, P, dev)
         Rd = _to_dev(R, dev, torch.float64)
-        depth = torch.empty((F_ * P, H, W), device=dev, dtype=torch.float32)
+        depth = workspace(dev, F_, P, H, W)
         t = torch.empty((F_, P, 3), device=dev, dtype=torch.float64)
         iou = torch.empty((F_, P), device=dev, dtype=torch.float64)
         stats = torch.empty((F_, P, 6), device=dev, dtype=torch.int32) if return_stats else None
         _lib.check(_lib.load().nope_fit_translation(
             _lib.ptr(mesh.vertices), mesh.vertices.shape[0], _lib.ptr(mesh.faces), mesh.num_faces, _lib.ptr(Rd),
-            _lib.ptr(t0), _lib.ptr(m), k.data_ptr(), F_, P, H, W, float(znear), int(iters), _lib.ptr(depth),
+            _lib.ptr(t0), _lib.ptr(m), k.data_ptr(), F_, P, H, W, float(znear), iters, _lib.ptr(depth),
             _lib.ptr(t), _lib.ptr(iou), _lib.ptr(stats), _stream(dev)))
     return (t, iou, stats) if return_stats else (t, iou)

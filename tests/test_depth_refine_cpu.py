@@ -148,6 +148,19 @@ def test_default_tau_schedule():
         default_tau(0.0)
 
 
+def test_default_tau_schedules_are_bit_exact():
+    """both fits' default schedules equal their closed forms to the last bit: the depth fit's d TAU_END (TAU_START /
+    TAU_END)^x and the contour fit's end (start / end)^x, x = (iters - i) / max(iters, 1)"""
+    from nope_b200 import contour_refine as cr, depth_refine as dr
+    for iters in range(13):
+        x = (iters - np.arange(iters + 1, dtype=np.float64)) / max(iters, 1)
+        for d in (1e-3, 0.7, 80.0, 123.456, 2.0 * 97.3, 1e5):
+            assert np.array_equal(dr.default_tau(d, iters), d * dr.TAU_END * (dr.TAU_START / dr.TAU_END) ** x)
+        for start, end in ((cr.TAU_START, cr.TAU_END), (0.3, 0.05), (0.5, 0.5), (0.01, 0.2)):
+            assert np.array_equal(cr.default_tau(iters, start, end), end * (start / end) ** x)
+        assert np.array_equal(cr.default_tau(iters), cr.TAU_END * (cr.TAU_START / cr.TAU_END) ** x)
+
+
 # ------------------------------------------------------------------ argument errors
 def test_argument_errors():
     from nope_b200 import _lib
