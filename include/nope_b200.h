@@ -17,6 +17,7 @@
  * ABI version 2 (round 2): nope_unet_set_option / get_option, caller-owned workspace
  * (nope_unet_workspace_bytes / nope_unet_set_workspace), nope_unet_profile_read reports executed and
  * algorithmic FLOPs, nope_op_conv_gn_fused, nope_topk_merge, nope_score_topk metric 2.
+ * Later additions under version 2 include nope_encoder_set_option and nope_vae_set_option.
  */
 #ifndef NOPE_B200_H
 #define NOPE_B200_H
@@ -157,6 +158,12 @@ void nope_encoder_destroy(nope_encoder_t* e);
 int nope_encoder_load_tensor(nope_encoder_t* e, const char* key, const float* data,
                              const int64_t* shape, int ndim);
 int nope_encoder_finalize(nope_encoder_t* e);
+/* Named options, before nope_encoder_finalize only (the weight packing depends on them):
+ *   "precision": 0 = split precision (default; the fp32-accurate latents above), 1 = fp16: one fp16 weight per tap
+ *       (BatchNorm folded in float64, then rounded once), one fp16 copy of every stored activation, fp32 accumulation,
+ *       one K-segment per tap instead of three (DESIGN.md section 22).  Every encode and run_block call honours it.
+ * An unknown name or value, or a call after finalize, is refused before any CUDA call. */
+int nope_encoder_set_option(nope_encoder_t* e, const char* name, int value);
 /* images [B, 3, 256, 256] fp32 NCHW (device) -> out [B, D, 32, 32] fp32 NCHW (device).
  * Any B >= 1: the engine walks the batch 32 images at a time (workspace ~80 MB per image of a chunk). */
 int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* out, void* stream);
@@ -216,6 +223,10 @@ int nope_vae_create(nope_vae_t** out, int device);
 void nope_vae_destroy(nope_vae_t* v);
 int nope_vae_load_tensor(nope_vae_t* v, const char* key, const float* data, const int64_t* shape, int ndim);
 int nope_vae_finalize(nope_vae_t* v);
+/* "precision" as nope_encoder_set_option (0 = split, the default; 1 = fp16 operands and stored activations, with the
+ * fp32 residual stream, float64 GroupNorm statistics, fp32 attention core and fp32 conv_out kept), before
+ * nope_vae_finalize only; refusals as there. */
+int nope_vae_set_option(nope_vae_t* v, const char* name, int value);
 int nope_vae_encode(nope_vae_t* v, const float* images, int B, float* out, void* stream);
 int nope_vae_encode_inplane(nope_vae_t* v, const float* images, int B, const float* cossin, int A, float* out,
                             void* stream);

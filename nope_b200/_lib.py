@@ -33,6 +33,8 @@ SIGNATURES = {
                                         c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, c_f32p, C.c_int, c_f32p,
                                         c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_encoder_encode": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_void_p]),
+    "nope_encoder_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
+    "nope_vae_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "nope_encoder_last_launch_count": (C.c_int64, [C.c_void_p]),
     "nope_inplane_rotate": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, c_f32p, C.c_void_p]),
     "nope_encoder_encode_inplane": (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, C.c_void_p]),

@@ -14,6 +14,10 @@
 // ReLU, the bottleneck's residual add and the (hi, lo) split of the output run in the conv
 // epilogue.  Stride-2 convolutions read the four stride-2 sub-lattices of their input through
 // TMA maps (same trick as HardDownsample).  65 GFLOP per image in fp32 terms, 195 executed.
+//
+// precision 1 (nope_encoder_set_option, DESIGN.md section 22) is the opt-in single-fp16 mode: every weight is one
+// fp16 value (BatchNorm still folded in double first), every stored activation one fp16 tensor (lo = nullptr, never
+// allocated, written or read), one K-segment per tap; the stem's arithmetic and the accumulation stay fp32.
 #pragma once
 #include "conv_tc2.cuh"
 #include "engine.cuh"
@@ -26,7 +30,7 @@
 
 namespace nope {
 
-// stem: conv 7x7 stride 2 pad 3 (3 -> 64) + folded BN + ReLU, fp32 direct, -> (hi, lo) NHWC.
+// stem: conv 7x7 stride 2 pad 3 (3 -> 64) + folded BN + ReLU, fp32 direct, -> (hi, lo) NHWC (out_lo nullptr: hi only).
 // Block = 64 output channels x 4 pixels.  w: [64][3][7][7] folded, fp32.
 __global__ void __launch_bounds__(256)
 enc_stem_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
@@ -36,15 +40,16 @@ enc_stem_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
   __syncthreads();
   const int Ho = Hin / 2, Wo = Win / 2;
   const int o = threadIdx.x & 63;
-  const long long pix = (long long)blockIdx.x * 4 + (threadIdx.x >> 6);
-  if (pix >= (long long)B * Ho * Wo) return;
-  const int px = (int)(pix % Wo), py = (int)((pix / Wo) % Ho), b = (int)(pix / ((long long)Wo * Ho));
+  // 32-bit pixel arithmetic (B <= 32 images of a chunk), so no 64-bit division routine is called
+  const int pix = blockIdx.x * 4 + (threadIdx.x >> 6);
+  if (pix >= B * Ho * Wo) return;
+  const int px = pix % Wo, py = (pix / Wo) % Ho, b = pix / (Wo * Ho);
   float acc = bias[o];
   for (int c = 0; c < 3; ++c)
     for (int ky = 0; ky < 7; ++ky) {
       const int yy = 2 * py + ky - 3;
       if (yy < 0 || yy >= Hin) continue;
-      const float* xr = x + (((long long)b * 3 + c) * Hin + yy) * Win;
+      const float* xr = x + (size_t)((b * 3 + c) * Hin + yy) * Win;
       const float* wr = s_w + o * 147 + (c * 7 + ky) * 7;
 #pragma unroll
       for (int kx = 0; kx < 7; ++kx) {
@@ -54,8 +59,8 @@ enc_stem_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
     }
   acc = fmaxf(acc, 0.f);
   const __half hi = __float2half_rn(acc);
-  out_hi[pix * 64 + o] = hi;
-  out_lo[pix * 64 + o] = __float2half_rn(acc - __half2float(hi));
+  out_hi[(size_t)pix * 64 + o] = hi;
+  if (out_lo) out_lo[(size_t)pix * 64 + o] = __float2half_rn(acc - __half2float(hi));
 }
 
 // In-plane rotation of the query crops (DESIGN.md section 11): rotated copy a of image b is
@@ -142,21 +147,28 @@ __global__ void enc_extract_kernel(const float* __restrict__ x, float* __restric
 
 struct EncConv {
   int cin = 0, cout = 0, cout_real = 0, k = 1, stride = 1, K = 0, bn = 0;
-  __half* w = nullptr;   // [cout][taps][3][cin] fp16: (W_hi | W_lo | W_hi) per tap
+  __half* w = nullptr;   // [cout][taps][3][cin] fp16: (W_hi | W_lo | W_hi) per tap; fp16 mode [cout][taps][cin]
   float* bias = nullptr;
   CUtensorMap wmap;
 };
 
 struct ActPair {
   __half* hi = nullptr;
-  __half* lo = nullptr;
+  __half* lo = nullptr;   // nullptr: a single fp16 tensor
 };
+// the pair at element offset o of a (hi, lo) pair, keeping a null lo null
+inline ActPair act_at(const ActPair& a, size_t o) { return ActPair{a.hi + o, a.lo ? a.lo + o : nullptr}; }
+
+// the number of fp16 products per filter tap of a convolution: 3 in split precision (A_hi W_hi, A_hi W_lo,
+// A_lo W_hi), 1 in the single-fp16 mode
+inline int tap_products(int precision) { return precision == 0 ? 3 : 1; }
 
 }  // namespace nope
 
 struct nope_encoder {
   static constexpr const char* kName = "encoder";
   int D = 8, device = 0, num_sms = 132;
+  int precision = 0;                  // 0: split (hi, lo) operands; 1: single fp16 (set before finalize)
   bool finalized = false;
   nope::StagedWeights staged;
   std::map<std::string, nope::EncConv> convs;
@@ -200,7 +212,7 @@ struct nope_encoder {
   }
 
   // ---------------------------------------------------------------- weights
-  // fold eval-mode BN (eps 1e-5) into the conv in double, split into fp16 (hi, lo), pack
+  // fold eval-mode BN (eps 1e-5) into the conv in double, split into fp16 (hi, lo), pack; fp16 mode: hi only
   int make_conv(const std::string& name, const std::string& wkey, const std::string& bnkey, int stride) {
     using namespace nope;
     const HostTensor& W = staged.at(wkey);
@@ -211,7 +223,8 @@ struct nope_encoder {
     L.stride = stride;
     L.cout = (L.cout_real + 63) / 64 * 64;
     const int taps = L.k * L.k;
-    L.K = taps * 3 * L.cin;
+    const int prods = tap_products(precision);
+    L.K = taps * prods * L.cin;
     NOPE_CHECK(L.cin % 64 == 0, wkey + ": input channels must be a multiple of 64");
     L.bn = pick_bn(L.cout);
     std::vector<double> scale(L.cout_real, 1.0), shift(L.cout_real, 0.0);
@@ -230,8 +243,9 @@ struct nope_encoder {
           const float wf = (float)((double)W.data[((size_t)o * L.cin + c) * taps + t] * scale[o]);
           const __half hi = __float2half_rn(wf);
           const __half lo = __float2half_rn(wf - __half2float(hi));
-          __half* dst = &packed[(size_t)o * L.K + (size_t)t * 3 * L.cin];
+          __half* dst = &packed[(size_t)o * L.K + (size_t)t * prods * L.cin];
           dst[c] = hi;
+          if (prods == 1) continue;
           dst[L.cin + c] = lo;
           dst[2 * L.cin + c] = hi;
         }
@@ -281,7 +295,7 @@ struct nope_encoder {
     cap = B;
     const size_t n = (size_t)cap * 128 * 128 * 256;     // largest activation: layer1 output
     for (auto& b : buf)
-      if (ws_mem.alloc(&b.hi, n) || ws_mem.alloc(&b.lo, n)) return -1;
+      if (ws_mem.alloc(&b.hi, n) || (precision == 0 && ws_mem.alloc(&b.lo, n))) return -1;
     return ws_mem.alloc(&proj_out, (size_t)cap * 1024 * 64);
   }
   int get_map(const CUtensorMap** out, const void* base, int C, const nope::TileGeom& g, int kind) {
@@ -311,20 +325,24 @@ struct nope_encoder {
     const CUtensorMap* m = nullptr;
     int nseg = 0, ksteps = 0;
     const int nch = L.cin / 64;
+    const bool split = precision == 0;   // fp16 mode: the hi maps only, one segment per tap
     if (L.stride == 1) {
       if (get_map(&m, in.hi, L.cin, g, -1)) return -1;
       p.amap[0] = *m;
-      if (get_map(&m, in.lo, L.cin, g, -1)) return -1;
-      p.amap[1] = *m;
-      p.n_amaps = 2;
+      if (split) {
+        if (get_map(&m, in.lo, L.cin, g, -1)) return -1;
+        p.amap[1] = *m;
+      }
+      p.n_amaps = split ? 2 : 1;
     } else {
       for (int t = 0; t < 4; ++t) {
         if (get_map(&m, in.hi, L.cin, g, t)) return -1;
         p.amap[t] = *m;
+        if (!split) continue;
         if (get_map(&m, in.lo, L.cin, g, t)) return -1;
         p.amap[4 + t] = *m;
       }
-      p.n_amaps = 8;
+      p.n_amaps = split ? 8 : 4;
     }
     for (int ky = 0; ky < L.k; ++ky)
       for (int kx = 0; kx < L.k; ++kx) {
@@ -343,9 +361,11 @@ struct nope_encoder {
           ml = 4 + mh;
         }
         p.seg[nseg++] = ConvSeg{(int16_t)mh, (int16_t)dy, (int16_t)dx, (int16_t)nch};   // A_hi W_hi
+        ksteps += nch;
+        if (!split) continue;
         p.seg[nseg++] = ConvSeg{(int16_t)mh, (int16_t)dy, (int16_t)dx, (int16_t)nch};   // A_hi W_lo
         p.seg[nseg++] = ConvSeg{(int16_t)ml, (int16_t)dy, (int16_t)dx, (int16_t)nch};   // A_lo W_hi
-        ksteps += 3 * nch;
+        ksteps += 2 * nch;
       }
     NOPE_CHECK(nseg <= kMaxSeg && ksteps * 64 == L.K, "encoder conv: segment table");
     p.bmap = L.wmap;

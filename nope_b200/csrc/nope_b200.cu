@@ -1383,6 +1383,22 @@ int nope_encoder_load_tensor(nope_encoder_t* e, const char* key, const float* da
 
 int nope_encoder_finalize(nope_encoder_t* e) { return engine_finalize(e); }
 
+// "precision" of the template encoder and the VAE encoder: the name and the value are checked before the handle, so
+// every refusal happens before any CUDA call
+extern "C++" template <class Engine>
+int encoder_set_option(Engine* e, const char* name, int value) {
+  NOPE_CHECK(name, "null option name");
+  if (std::strcmp(name, "precision") != 0) return fail(std::string("unknown option: ") + name);
+  NOPE_CHECK(value == 0 || value == 1, "precision must be 0 (split) or 1 (fp16)");
+  NOPE_CHECK(e, "null engine");
+  NOPE_CHECK(!e->finalized, "precision must be set before finalize");
+  e->precision = value;
+  return 0;
+}
+int nope_encoder_set_option(nope_encoder_t* e, const char* name, int value) {
+  return encoder_set_option(e, name, value);
+}
+
 int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* out, void* stream) {
   NOPE_CHECK(e && e->finalized, "encoder not finalized");
   NOPE_CHECK(images && out, "null images / out pointer");
@@ -1478,6 +1494,7 @@ int nope_vae_load_tensor(nope_vae_t* v, const char* key, const float* data, cons
 }
 
 int nope_vae_finalize(nope_vae_t* v) { return engine_finalize(v); }
+int nope_vae_set_option(nope_vae_t* v, const char* name, int value) { return encoder_set_option(v, name, value); }
 
 int nope_vae_encode(nope_vae_t* v, const float* images, int B, float* out, void* stream) {
   NOPE_CHECK(images && out, "null images / out pointer");

@@ -14,6 +14,9 @@
 // in a fixed order, so they do not depend on the batch or the chunk.  The residual stream is kept as fp32 (for
 // the statistics) and as (hi, lo) (for the identity shortcut, added in the conv2 epilogue, and for the 1x1
 // shortcut, extra K-segments of conv2).  The attention core (q k^T, softmax, p v) runs on CUDA cores in fp32.
+// The encoder's opt-in single-fp16 mode (precision 1, DESIGN.md section 22) packs one fp16 weight per tap, keeps one
+// fp16 copy of every stored activation (the lo halves are not allocated; the kernels below skip a null lo) and runs
+// one K-segment per tap and source; the fp32 stream, the float64 statistics and the attention core are unchanged.
 //
 // The 256 x 256 level is wider than one 128-pixel tile row, which the convolution's tile geometry requires.
 // Its activations are therefore stored parity-planar: plane (py, px) = 2 py + px holds the pixels (2 Y + py,
@@ -34,7 +37,8 @@ namespace nope {
 
 constexpr int kVaeSlab = 1024;   // pixels per GroupNorm partial sum (divides every level's H*W per plane)
 
-// conv_in: 3x3 pad 1 (3 -> 128), fp32 direct, -> parity-planar fp32 + (hi, lo).  w: [128][3][3][3] fp32.
+// conv_in: 3x3 pad 1 (3 -> 128), fp32 direct, -> parity-planar fp32 + (hi, lo) (out_lo nullptr: hi only).
+// w: [128][3][3][3] fp32.
 // Block = 128 output channels x 2 pixels.
 __global__ void __launch_bounds__(256)
 vae_conv_in_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
@@ -65,7 +69,7 @@ vae_conv_in_kernel(const float* __restrict__ x, const float* __restrict__ w, con
   out32[dst] = acc;
   const __half hi = __float2half_rn(acc);
   out_hi[dst] = hi;
-  out_lo[dst] = __float2half_rn(acc - __half2float(hi));
+  if (out_lo) out_lo[dst] = __float2half_rn(acc - __half2float(hi));
 }
 
 // GroupNorm(32) partial sums of fp32 NHWC activations: image b's pixels lie in `planes` planes of [cap, hw, C]
@@ -122,7 +126,8 @@ vae_gn_finalize_kernel(const double2* __restrict__ part, int nparts, double inv_
   stats[b * 32 + g] = make_float2((float)mean, (float)(r0 * (1.5 - 0.5 * v * r0 * r0)));
 }
 
-// y = [SiLU]((x - mean) * rstd * gamma + beta) -> (hi, lo), same layout as x; 4 channels per thread.
+// y = [SiLU]((x - mean) * rstd * gamma + beta) -> (hi, lo) (out_lo nullptr: hi only), same layout as x; 4 channels
+// per thread.
 // grid (ceil(hw * C / 1024), planes * n): blockIdx.y = q * n + b is image b of plane q (its cap slots hold the n
 // images of the chunk first).
 __global__ void __launch_bounds__(256)
@@ -145,17 +150,18 @@ vae_gn_apply_kernel(const float* __restrict__ x, const float2* __restrict__ stat
 #pragma unroll
     for (int k = 0; k < 4; ++k) y[k] = __fdividef(y[k], 1.f + expf(-y[k]));
   }
+  reinterpret_cast<uint2*>(out_hi)[off] = make_uint2(pack_half2(y[0], y[1]), pack_half2(y[2], y[3]));
+  if (!out_lo) return;
   float l[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) l[k] = y[k] - __half2float(__float2half_rn(y[k]));
-  reinterpret_cast<uint2*>(out_hi)[off] = make_uint2(pack_half2(y[0], y[1]), pack_half2(y[2], y[3]));
   reinterpret_cast<uint2*>(out_lo)[off] = make_uint2(pack_half2(l[0], l[1]), pack_half2(l[2], l[3]));
 }
 
 // Batched fp32 GEMM of the attention core, one image per blockIdx.z, 64 x 64 tile per block, 4 x 4 per thread,
 // every output summed over k in ascending order:
 //   C[m, j] = alpha * sum_k A[m, k] B(k, j),  B(k, j) = Bm[j * ldb + k] (KT) or Bm[k * ldb + j].
-// SPLIT stores (hi, lo) halves, else fp32.  M, N multiples of 64, K a multiple of 16.
+// SPLIT stores (hi, lo) halves (Clo nullptr: hi only), else fp32.  M, N multiples of 64, K a multiple of 16.
 template <bool KT, bool SPLIT>
 __global__ void __launch_bounds__(256)
 vae_attn_gemm_kernel(const float* __restrict__ A, int lda, long long sa, const float* __restrict__ Bm, int ldb,
@@ -207,7 +213,7 @@ vae_attn_gemm_kernel(const float* __restrict__ A, int lda, long long sa, const f
       if (SPLIT) {
         const __half hi = __float2half_rn(v);
         Chi[o] = hi;
-        Clo[o] = __float2half_rn(v - __half2float(hi));
+        if (Clo) Clo[o] = __float2half_rn(v - __half2float(hi));
       } else {
         C32[o] = v;
       }
@@ -245,6 +251,7 @@ __global__ void __launch_bounds__(256) vae_softmax_kernel(float* __restrict__ s)
 
 // A convolution of the VAE: packed split-precision weights [cout][K] fp16, K = taps x (W_hi | W_lo | W_hi) x cin,
 // then, for a ResnetBlock2D conv2 with a 1x1 shortcut, (S_hi | S_lo | S_hi) x cin_sc; bias = b2 (+ b_shortcut).
+// In the single-fp16 mode each tap holds W_hi alone: K = taps x cin (+ cin_sc).
 struct VaeConv {
   int cin = 0, cin_sc = 0, cout = 0, k = 1, K = 0, bn = 0;
   __half* w = nullptr;
@@ -257,7 +264,7 @@ struct VaeNorm {
   float* beta = nullptr;
 };
 
-// One tap of a convolution: input pair (hi map 2 * pair, lo map 2 * pair + 1) at offset (dy, dx).
+// One tap of a convolution: input pair (hi map 2 * pair, lo map 2 * pair + 1; fp16 mode: map pair) at (dy, dx).
 struct VaeTap {
   int pair, dy, dx;
 };
@@ -355,6 +362,7 @@ vae_dec_extract_kernel(const float* __restrict__ t, int ld, int cap, int n, floa
 struct VaeEngine {
   const int cap;                              // images per pass
   int device = 0, num_sms = 132;
+  int precision = 0;                          // 0: split (hi, lo) operands; 1: single fp16 (encoder, before finalize)
   bool finalized = false;
   StagedWeights staged;
   std::map<std::string, VaeConv> convs;
@@ -407,8 +415,8 @@ struct VaeEngine {
     L.cin_sc = cin_sc;
     L.k = k;
     L.cout = (cout_real + 63) / 64 * 64;
-    const int taps = k * k;
-    L.K = taps * 3 * cin + 3 * cin_sc;
+    const int taps = k * k, prods = tap_products(precision);
+    L.K = (taps * cin + cin_sc) * prods;
     NOPE_CHECK(cin % 64 == 0 && cin_sc % 64 == 0, name + ": input channels must be a multiple of 64");
     L.bn = pick_bn(L.cout);
     std::vector<__half> packed((size_t)L.cout * L.K, __float2half_rn(0.f));
@@ -416,15 +424,16 @@ struct VaeEngine {
       const float wf = (float)v;
       const __half hi = __float2half_rn(wf);
       dst[c] = hi;
+      if (prods == 1) return;
       dst[stride + c] = __float2half_rn(wf - __half2float(hi));
       dst[2 * stride + c] = hi;
     };
     for (int o = 0; o < cout_real; ++o) {
       for (int c = 0; c < cin; ++c)
         for (int t = 0; t < taps; ++t)
-          put(&packed[(size_t)o * L.K + (size_t)t * 3 * cin], c, cin, W[((size_t)o * cin + c) * taps + t]);
+          put(&packed[(size_t)o * L.K + (size_t)t * prods * cin], c, cin, W[((size_t)o * cin + c) * taps + t]);
       for (int c = 0; c < cin_sc; ++c)
-        put(&packed[(size_t)o * L.K + (size_t)taps * 3 * cin], c, cin_sc, (*Ws)[(size_t)o * cin_sc + c]);
+        put(&packed[(size_t)o * L.K + (size_t)taps * prods * cin], c, cin_sc, (*Ws)[(size_t)o * cin_sc + c]);
     }
     std::vector<float> b(L.cout, 0.f);
     for (int o = 0; o < cout_real; ++o) b[o] = (float)bias[o];
@@ -474,11 +483,13 @@ struct VaeEngine {
     return pack_conv(a + "proj_attn", 512, 512, 1, dvec(a + "proj_attn.weight"), dvec(a + "proj_attn.bias"));
   }
 
-  // workspace of E elements per activation buffer, allocated once so that no call allocates (or synchronises)
+  // workspace of E elements per activation buffer, allocated once so that no call allocates (or synchronises); the
+  // lo halves only in split precision
   int alloc_workspace(size_t E) {
+    const bool split = precision == 0;
     for (int s = 0; s < 2; ++s)
-      if (mem.alloc(&x32[s], E) || mem.alloc(&xs[s].hi, E) || mem.alloc(&xs[s].lo, E)) return -1;
-    if (mem.alloc(&nrm.hi, E) || mem.alloc(&nrm.lo, E) || mem.alloc(&t32, E)) return -1;
+      if (mem.alloc(&x32[s], E) || mem.alloc(&xs[s].hi, E) || (split && mem.alloc(&xs[s].lo, E))) return -1;
+    if (mem.alloc(&nrm.hi, E) || (split && mem.alloc(&nrm.lo, E)) || mem.alloc(&t32, E)) return -1;
     return mem.alloc(&gn_part, (size_t)cap * 64 * 32) || mem.alloc(&gn_stats, (size_t)cap * 32) ? -1 : 0;
   }
 
@@ -504,7 +515,7 @@ struct VaeEngine {
   size_t plane_off(int q, int C) const { return (size_t)q * cap * 128 * 128 * C; }
 
   // out = conv(taps over the input pairs `in`) [+ shortcut taps over pair sc] + bias [+ res]; output H x H.
-  // in: (hi, lo) base pointers of each input pair with their lattice (-1: plain NHWC of side H).
+  // in: (hi, lo) base pointers of each input pair with their lattice (-1: plain NHWC of side H); fp16 mode: hi only.
   int conv(const VaeConv& L, const std::vector<std::pair<ActPair, int>>& in, int Hin_map,
            const std::vector<VaeTap>& taps, int sc_pair, int H, int n, __half* out_hi, __half* out_lo,
            float* out_f32, const ActPair* res, cudaStream_t st) {
@@ -514,20 +525,25 @@ struct VaeEngine {
     memset(&p, 0, sizeof p);
     const CUtensorMap* m = nullptr;
     NOPE_CHECK(in.size() <= (size_t)kMaxAMaps / 2, "vae conv: too many input maps");
+    const bool split = precision == 0;   // fp16 mode: one map per input (its hi), one segment per tap
+    const int mps = split ? 2 : 1;       // maps per input
     for (size_t i = 0; i < in.size(); ++i) {
       const int C = (int)i == sc_pair ? L.cin_sc : L.cin;
       if (get_map(&m, in[i].first.hi, C, Hin_map, in[i].second)) return -1;
-      p.amap[2 * i] = *m;
+      p.amap[mps * i] = *m;
+      if (!split) continue;
       if (get_map(&m, in[i].first.lo, C, Hin_map, in[i].second)) return -1;
       p.amap[2 * i + 1] = *m;
     }
-    p.n_amaps = 2 * (int)in.size();
+    p.n_amaps = mps * (int)in.size();
     int nseg = 0, ksteps = 0;
     auto add = [&](const VaeTap& t, int nch) {
-      p.seg[nseg++] = ConvSeg{(int16_t)(2 * t.pair), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};       // A_hi W_hi
+      p.seg[nseg++] = ConvSeg{(int16_t)(mps * t.pair), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};     // A_hi W_hi
+      ksteps += nch;
+      if (!split) return;
       p.seg[nseg++] = ConvSeg{(int16_t)(2 * t.pair), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};       // A_hi W_lo
       p.seg[nseg++] = ConvSeg{(int16_t)(2 * t.pair + 1), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};   // A_lo W_hi
-      ksteps += 3 * nch;
+      ksteps += 2 * nch;
     };
     for (const VaeTap& t : taps) add(t, L.cin / 64);
     if (sc_pair >= 0) add(VaeTap{sc_pair, 0, 0}, L.cin_sc / 64);
@@ -572,10 +588,7 @@ struct VaeEngine {
     }
     NOPE_CHECK(!sc, "vae conv: no shortcut segments at the 256 x 256 level");
     std::vector<std::pair<ActPair, int>> src;
-    for (int q = 0; q < 4; ++q) {
-      const size_t o = plane_off(q, L.cin);
-      src.push_back({ActPair{in.hi + o, in.lo + o}, -1});
-    }
+    for (int q = 0; q < 4; ++q) src.push_back({act_at(in, plane_off(q, L.cin)), -1});
     for (int q = 0; q < 4; ++q) {
       const int py = q >> 1, px = q & 1;
       taps.clear();
@@ -586,8 +599,8 @@ struct VaeEngine {
         }
       const size_t o = plane_off(q, L.cout);
       ActPair r;
-      if (res) r = ActPair{res->hi + o, res->lo + o};
-      if (conv(L, src, 128, taps, -1, 128, n, out.hi + o, want_lo ? out.lo + o : nullptr, out_f32 + o,
+      if (res) r = act_at(*res, o);
+      if (conv(L, src, 128, taps, -1, 128, n, out.hi + o, want_lo ? act_at(out, o).lo : nullptr, out_f32 + o,
                res ? &r : nullptr, st))
         return -1;
     }
@@ -620,12 +633,12 @@ struct VaeEngine {
     if (planar_sc) {
       // the 1x1 shortcut, one launch per plane, into x32[cur]'s memory (norm1 was its last reader)
       __half* s = reinterpret_cast<__half*>(x32[cur]);
-      sres = ActPair{s, s + 4 * plane_off(1, cout)};
+      sres = ActPair{s, precision == 0 ? s + 4 * plane_off(1, cout) : nullptr};
       const VaeConv& S = convs.at(p + ".conv_shortcut");
       for (int q = 0; q < 4; ++q) {
         const size_t i = plane_off(q, cin), o = plane_off(q, cout);
-        if (conv(S, {{ActPair{xs[cur].hi + i, xs[cur].lo + i}, -1}}, 128, {VaeTap{0, 0, 0}}, -1, 128, n,
-                 sres.hi + o, sres.lo + o, nullptr, nullptr, st))
+        if (conv(S, {{act_at(xs[cur], i), -1}}, 128, {VaeTap{0, 0, 0}}, -1, 128, n, sres.hi + o, act_at(sres, o).lo,
+                 nullptr, nullptr, st))
           return -1;
       }
     }
@@ -778,8 +791,7 @@ struct nope_vae : nope::VaeEngine {
     std::vector<std::pair<ActPair, int>> src;
     for (int q = 0; q < 4; ++q) {
       if (Hin == 256) {
-        const size_t o = plane_off(q, L.cin);
-        src.push_back({ActPair{in.hi + o, in.lo + o}, -1});
+        src.push_back({act_at(in, plane_off(q, L.cin)), -1});
       } else {
         src.push_back({in, q});
       }

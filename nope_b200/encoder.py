@@ -14,6 +14,10 @@ total stride is 8), eval-mode BatchNorm, then ReLU -> 1x1(2048->256) -> ReLU -> 
 Parameter names equal the reference's `backbone.*` / `projector.*` keys so its
 state_dict loads unchanged; the duplicate `encoder.{0,1}.*` aliases the reference
 registers (template.py:40) are accepted and ignored.
+
+`precision` picks the native engine's arithmetic (DESIGN.md section 22): "split" (default) is the fp32-accurate
+split precision above; "fp16" is the opt-in fast mode with single fp16 weights and stored activations and fp32
+accumulation, one tensor-core product per tap instead of three.  "fp16" has no torch-backend or CPU path.
 """
 import ctypes as C
 
@@ -22,6 +26,25 @@ from torch import nn
 import torch.nn.functional as F
 
 from . import _lib
+
+# FeatureExtractor / VAE_StableDiffusion `precision` -> the engines' "precision" option
+ENCODER_PRECISIONS = {"split": 0, "fp16": 1}
+
+
+def check_precision(precision):
+    """Returns the engine option value of an encoder `precision`; ValueError for anything else."""
+    if not isinstance(precision, str) or precision not in ENCODER_PRECISIONS:
+        raise ValueError(f"encoder precision must be one of {sorted(ENCODER_PRECISIONS)}, got {precision!r}")
+    return ENCODER_PRECISIONS[precision]
+
+
+def precision_option(kind, precision):
+    """The build_engine `configure` step that sets the "precision" option of a `kind` engine ("encoder" or "vae"),
+    or None for the default split precision (the engine's own default, so that mode makes no extra call)."""
+    value = check_precision(precision)
+    if value == 0:
+        return None
+    return lambda lib, h: _lib.check(getattr(lib, f"nope_{kind}_set_option")(h, b"precision", value))
 
 
 class _Bottleneck(nn.Module):
@@ -89,13 +112,19 @@ def _encoder_block_out(name, D):
 class FeatureExtractor(nn.Module):
     """Same constructor/attributes as the reference (template.py:25-45)."""
 
-    def __init__(self, descriptor_size=8, threshold=0.2, normalize=False, backend="auto", **kwargs):
+    def __init__(self, descriptor_size=8, threshold=0.2, normalize=False, backend="auto", precision="split",
+                 **kwargs):
         super().__init__()
         if backend not in ("auto", "b200", "torch"):
             raise ValueError("backend must be 'auto', 'b200' or 'torch'")
         self.backend = backend
         self._h = None
         self._h_device = None
+        check_precision(precision)
+        if precision != "split" and backend == "torch":
+            raise _lib.NopeError(f"precision={precision!r} is a mode of the native engine; the torch backend has "
+                                 "none (no fallback)")
+        self.precision = precision
         self.latent_dim = descriptor_size
         self.normalize = normalize
         self.threshold = threshold
@@ -130,7 +159,8 @@ class FeatureExtractor(nn.Module):
         self._drop_engine()
         tensors = [(k, v) for k, v in self.state_dict().items()
                    if not (k.endswith("num_batches_tracked") or k.startswith("backbone.fc."))]
-        self._h = _lib.build_engine("encoder", (self.latent_dim, device.index or 0), tensors)
+        self._h = _lib.build_engine("encoder", (self.latent_dim, device.index or 0), tensors,
+                                    configure=precision_option("encoder", self.precision))
         self._h_device = device
         return self._h
 
@@ -140,6 +170,9 @@ class FeatureExtractor(nn.Module):
         if device.type != "cuda":
             if self.backend == "b200":
                 raise _lib.NopeError("backend='b200' needs a CUDA device (no CPU fallback)")
+            if self.precision != "split":
+                raise _lib.NopeError(f"precision={self.precision!r} needs the native engine on a CUDA device "
+                                     "(no CPU fallback)")
             return False          # 'auto' on CPU tensors: the torch module (CPU tests only)
         return True
 

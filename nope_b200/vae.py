@@ -5,7 +5,8 @@ variant (configs/model/vae_cin_ldm.yaml) and of configs/model/vae_base.yaml: `en
 diffusers `AutoencoderKL.encode(x).latent_dist.mode() * 0.18215` for the Stable Diffusion v1 VAE
 configuration (SD_V1_CONFIG), computed by the native engine in libnope_b200.so (`nope_vae_*`,
 csrc/vae.cuh, DESIGN.md section 16): every convolution on the wgmma kernel with split-precision fp16
-(hi, lo) operands, fp32-accurate.  `decode_latent` is diffusers `AutoencoderKL.decode(z / 0.18215).sample`
+(hi, lo) operands, fp32-accurate (`precision="split"`, the default) or, opt-in, single fp16 operands
+(`precision="fp16"`, DESIGN.md section 22).  `decode_latent` is diffusers `AutoencoderKL.decode(z / 0.18215).sample`
 (AutoencoderKL.py:44-47), computed by a second engine (`nope_vae_decoder_*`, DESIGN.md section 17) that is
 built on the first decode.  There is no CPU path; the KL distribution of `using_KL=True` and the training
 loss are out of scope.
@@ -241,9 +242,15 @@ def _vae_block_out(name):
 class VAE_StableDiffusion:
     """Same constructor and attributes as the reference (AutoencoderKL.py:6-27)."""
 
-    def __init__(self, pretrained_path=None, latent_dim=4, name="vae", using_KL=False, device="cuda:0", **kwargs):
+    def __init__(self, pretrained_path=None, latent_dim=4, name="vae", using_KL=False, device="cuda:0",
+                 precision="split", **kwargs):
+        """precision: the encoder engine's arithmetic, "split" (default, fp32-accurate) or "fp16" (the fast mode,
+        DESIGN.md section 22); the decoder is always split precision."""
+        from .encoder import check_precision
         self._h = None
         self._dec_h = None
+        check_precision(precision)
+        self.precision = precision
         if using_KL:
             raise ValueError("using_KL=True (the latent distribution of the training-only KL loss) is not supported")
         if latent_dim != 4:
@@ -253,6 +260,8 @@ class VAE_StableDiffusion:
         self.using_KL = using_KL
         self.encode_mode = "mode"
         self.device = torch.device(device)
+        if precision != "split" and self.device.type != "cuda":
+            raise _lib.NopeError(f"precision={precision!r} needs a CUDA device (no CPU path)")
         self._sd = None
         self._dec_sd = {}
         self._dec_config_error = None     # why the config.json's decoder fields cannot be decoded, if they cannot
@@ -322,7 +331,9 @@ class VAE_StableDiffusion:
             return self._h
         if self._sd is None:
             raise _lib.NopeError("VAE_StableDiffusion has no weights: pass pretrained_path or call load_state_dict")
-        self._h = _lib.build_engine("vae", (self.device.index or 0,), self._sd.items())
+        from .encoder import precision_option
+        self._h = _lib.build_engine("vae", (self.device.index or 0,), self._sd.items(),
+                                    configure=precision_option("vae", self.precision))
         return self._h
 
     def _images(self, image):
@@ -443,13 +454,15 @@ class VAE_StableDiffusion:
 
 
 def build_vae_model(unet="ldm", vae_path=None, device="cuda:0", chunk=None, precision=None, vae_state_dict=None,
-                    similarity_metric="l2"):
+                    similarity_metric="l2", vae_precision="split"):
     """PoseConditional with the SD VAE encoder: unet="ldm" is configs/model/vae_cin_ldm.yaml (UNetModelPose),
     "base" is configs/model/vae_base.yaml (the default UNet at u_net_dim 192 on 4 latent channels).  The VAE
     weights come from `vae_path` (a diffusers directory) or `vae_state_dict`, or later through the
-    PoseConditional's load_state_dict (a reference checkpoint's `u_net.encoder.encoder.*` entries)."""
+    PoseConditional's load_state_dict (a reference checkpoint's `u_net.encoder.encoder.*` entries).  `precision` is
+    the UNet's; `vae_precision` the VAE encoder's ("split" or "fp16", VAE_StableDiffusion)."""
     from .model import PoseConditional
-    enc = VAE_StableDiffusion(pretrained_path=vae_path, latent_dim=4, name="VAE", device=device)
+    enc = VAE_StableDiffusion(pretrained_path=vae_path, latent_dim=4, name="VAE", device=device,
+                              precision=vae_precision)
     if vae_state_dict is not None:
         enc.load_state_dict(vae_state_dict)
     if unet == "ldm":
