@@ -381,6 +381,20 @@ int nope_pose_errors(const float* points, int V, const double* sym, int S, const
 int nope_crop_frames(const uint8_t* frames, int F, int H, int W, int C, const uint8_t* masks, const int32_t* frame_idx,
                      const double* inv_maps, int B, int S, float* out, void* stream);
 
+/* The crop camera (DESIGN.md section 23): a crop_frame crop is the view of a pinhole camera that shares the real
+ * camera's centre, with rotation R_v (rows x_v = right / |right|, y_v = -upper / |upper|, z_v = o / |o|, o the object
+ * centre) and intrinsics [[S |o| / s, 0, S/2], [0, S |o| / s, S/2], [0, 0, 1]].  A rotation in the crop's camera is
+ * R_crop = R_v R_cam.  float64, every operation rounded on its own, in the order DESIGN.md section 23 fixes.
+ * nope_crop_camera: pose HOST [F, 16] fp64 row-major (object -> camera; keep_inplane = 1 reads only the translation,
+ * keep_inplane = 0 the top three rows, as crop_frame's flag) -> Rv [F, 9] fp64 row-major (device).  crop_frame's
+ * image-axes fallback (upper = right = 0) gives R_v = I.  Refuses a null pointer, F outside [1, 65535], a non-finite
+ * entry it reads and, with keep_inplane = 1, Z <= 0, all before any CUDA call; the pose is staged in stream order.
+ * nope_crop_rotate: Rv [F, 9], R [F, P, 9] fp64 (device) -> out [F, P, 9] = Rv^T R (to_camera = 1) or Rv R
+ * (to_camera = 0); out may alias R; a non-finite R gives NaN, not an error.  Refuses a null pointer and F or P
+ * outside [1, 65535] before any CUDA call.  Neither call synchronises. */
+int nope_crop_camera(const double* pose, int F, int keep_inplane, double* Rv, void* stream);
+int nope_crop_rotate(const double* Rv, int F, const double* R, int P, int to_camera, double* out, void* stream);
+
 /* Score materialised templates against a query and rank them: the arithmetic of
  * PoseConditional.retrieval (model.py:254-266) after encode_image.
  *   query_feat [B, C, HW] fp32, emb [B, N, C, HW] fp32 -> sim [B, N], topv/topi [B, k]. */

@@ -192,3 +192,155 @@ def crop_frames(frames, inv_maps, image_size=256, masks=None, frame_idx=None):
             _lib.ptr(fr), F_, H, W, Cn, _lib.ptr(mk), _lib.ptr(fi), _lib.ptr(mp), B, S, _lib.ptr(out),
             C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
     return out
+
+
+# ------------------------------------------------------------------ the crop camera (DESIGN.md section 23)
+MAX_CAMERAS = 65535      # F (poses, detections) and P (rotations per pose) of nope_crop_camera / nope_crop_rotate
+
+
+def _stream(dev):
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def _camera(pose, keep_inplane, dev):
+    """R_v float64 [F, 3, 3] on `dev` of host poses float64 [F, 4, 4]; the pose is checked here and staged by the
+    library in stream order: no synchronisation"""
+    F_ = pose.shape[0]
+    if F_ > MAX_CAMERAS:
+        raise ValueError(f"at most {MAX_CAMERAS} poses, got {F_}")
+    read = pose[:, :3, 3] if keep_inplane else pose[:, :3]
+    if not np.isfinite(read).all():
+        raise ValueError("pose must be finite")
+    if keep_inplane and not (pose[:, 2, 3] > 0).all():
+        raise ValueError("keep_inplane needs every object centre in front of the camera (Z > 0)")
+    host = np.ascontiguousarray(pose, dtype=np.float64)
+    with torch.cuda.device(dev):
+        out = torch.empty((F_, 3, 3), device=dev, dtype=torch.float64)
+        _lib.check(_lib.load().nope_crop_camera(C.c_void_p(host.ctypes.data), F_, int(bool(keep_inplane)),
+                                                _lib.ptr(out), _stream(dev)))
+    return out
+
+
+def crop_camera(pose, keep_inplane=True):
+    """The crop camera's rotation R_v float64 [F, 3, 3] (or [3, 3] for one pose) of the crops `crop_transforms` cuts
+    around pose [F, 4, 4] or [4, 4] (object -> OpenCV camera): a crop is the view of a pinhole camera at the real
+    camera's centre, with rotation R_v and intrinsics `crop_intrinsics`, so a rotation R in the real camera is
+    R_v R in the crop's (`to_crop`, `to_camera`).  keep_inplane as crop_transforms: True reads the translation only
+    (Z > 0), False the top three rows.  The pose must be a CUDA tensor (there is no CPU fallback); it is read on the
+    host, one device -> host copy, because the library checks every pose before it launches.  ValueError for a
+    malformed or non-finite pose, NopeError for a host one."""
+    if not torch.is_tensor(pose) or pose.device.type != "cuda":
+        raise _lib.NopeError("crop_camera needs a CUDA pose tensor (no CPU fallback)")
+    one = pose.dim() == 2
+    P = _batched(pose.detach().to("cpu", torch.float64).numpy(), (4, 4), "pose")
+    out = _camera(P, keep_inplane, pose.device)
+    return out[0] if one else out
+
+
+def crop_intrinsics(pose, virtual_bbox_size, image_size=256):
+    """The crop camera's intrinsics K_v float64 [F, 3, 3] (or [3, 3] for one pose) of the crops `crop_transforms`
+    cuts around pose [F, 4, 4] or [4, 4] with side virtual_bbox_size (a number or [F], the pose's units) and crop
+    side S = image_size: f_v = S |o| / s and the principal point (S/2, S/2), o = pose[:3, 3].  Plain torch on the
+    pose's device.  Exact up to the int32 truncation of crop_frame's corners, and not in crop_frame's image-axes
+    fallback (crop_camera's R_v = I), whose square is not perpendicular to o."""
+    from .translation import _sqrt
+    p = _tensor(pose).to(torch.float64)
+    one = p.dim() == 2
+    p = p[None] if one else p
+    if p.dim() != 3 or p.shape[1:] != (4, 4):
+        raise ValueError(f"pose [4, 4] or [F, 4, 4] expected, got {list(p.shape)}")
+    S = int(image_size)
+    if S != image_size or not 1 <= S <= MAX_CROP:
+        raise ValueError(f"image_size must be an integer in [1, {MAX_CROP}], got {image_size!r}")
+    s = _tensor(virtual_bbox_size).to(device=p.device, dtype=torch.float64).reshape(-1)
+    if s.shape[0] not in (1, p.shape[0]):
+        raise ValueError(f"virtual_bbox_size: a number or [F] with F = {p.shape[0]} expected, got {list(s.shape)}")
+    o = p[:, :3, 3]
+    norm = _sqrt((o[:, 0] * o[:, 0] + o[:, 1] * o[:, 1]) + o[:, 2] * o[:, 2])
+    K = torch.zeros((p.shape[0], 3, 3), dtype=torch.float64, device=p.device)
+    K[:, 0, 0] = K[:, 1, 1] = S * norm / s
+    K[:, 0, 2] = K[:, 1, 2] = S / 2
+    K[:, 2, 2] = 1.0
+    return K[0] if one else K
+
+
+def _rotate(R, Rv, to_camera, name):
+    if not (torch.is_tensor(R) and torch.is_tensor(Rv)) or R.device.type != "cuda" or Rv.device != R.device:
+        raise _lib.NopeError(f"{name} needs R and Rv as CUDA tensors on one device (no CPU fallback)")
+    if R.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"R must be float32 or float64, got {R.dtype}")
+    if R.dim() not in (3, 4) or R.shape[-2:] != (3, 3) or Rv.shape != (R.shape[0], 3, 3) or R.shape[0] < 1 or \
+            (R.dim() == 4 and R.shape[1] < 1):
+        raise ValueError(f"R [F, P, 3, 3] or [F, 3, 3] and Rv [F, 3, 3] expected, got {list(R.shape)} and "
+                         f"{list(Rv.shape)}")
+    F_, P = R.shape[0], (R.shape[1] if R.dim() == 4 else 1)
+    if F_ > MAX_CAMERAS or P > MAX_CAMERAS:
+        raise ValueError(f"F and P must be at most {MAX_CAMERAS}, got {F_} and {P}")
+    if Rv.dtype != torch.float64:
+        raise ValueError(f"Rv must be float64 (crop_camera's), got {Rv.dtype}")
+    dev = R.device
+    with torch.cuda.device(dev):
+        src = R.detach().to(torch.float64).contiguous()
+        out = torch.empty_like(src)
+        _lib.check(_lib.load().nope_crop_rotate(_lib.ptr(Rv.contiguous()), F_, _lib.ptr(src), P, int(to_camera),
+                                                _lib.ptr(out), _stream(dev)))
+    return out
+
+
+def to_camera(R_crop, Rv):
+    """A rotation in the crop's camera re-expressed in the real camera: R_v^T R_crop, float64 in R_crop's shape
+    ([F, P, 3, 3] or [F, 3, 3], float32 or float64) on its CUDA device; Rv [F, 3, 3] from crop_camera.  Runs on the
+    current stream without synchronising."""
+    return _rotate(R_crop, Rv, True, "to_camera")
+
+
+def to_crop(R_cam, Rv):
+    """A rotation in the real camera expressed in the crop's camera: R_v R_cam; shapes and devices as to_camera.
+    For a reference cut from a real frame, its pose's rotation in its crop's camera, e.g. for
+    poses.relative_rotation_6d."""
+    return _rotate(R_cam, Rv, False, "to_crop")
+
+
+def frame_crops(frames, masks, K, diameter, image_size=256, frame_idx=None, bbox_scale=1.2):
+    """Crops of B detections in camera frames for the pose searches, and the crop cameras that map the searches'
+    rotations back to the frames (DESIGN.md section 23):
+      frames     uint8 [F, H, W, 3] RGB (host or CUDA; the crops go to the frames' CUDA device, or the current one)
+      masks      uint8 or bool [B, H, W], one per detection, nonzero = object (host or on the frames' device); a
+                 uint8 mask is pasted as crop_frames pastes it (a BOP mask_visib is 0 / 255), a bool one as 0 / 255
+      K          [3, 3] or [B, 3, 3] intrinsics, read on the host (host data saves a copy)
+      diameter   the object diameter, a number or [B] (mm)
+      frame_idx  integer [B], or None when F == B: the frame of each detection
+      bbox_scale the crop's square is bbox_scale * diameter wide (1.2, as src/dataloader/bop.py:193-194)
+    It runs `translation.initial_translation` on the masks' device (t0 [B, 3], mm), `crop_transforms(K, t0,
+    bbox_scale * diameter, keep_inplane=True)` on the host, `crop_frames` and `crop_camera`.
+    -> (crops float32 [B, 3, S, S], t0 float64 [B, 3] on the masks' device, R_v float64 [B, 3, 3] on the crops'
+    device, inv_maps float64 [B, 3, 3] on the host).  The one host synchronisation is the copy of t0 that the host
+    geometry needs (none for host masks).  ValueError for an empty mask or a malformed argument."""
+    from .translation import initial_translation
+    m = _tensor(masks)
+    if m.dim() != 3 or m.shape[0] < 1 or m.dtype not in (torch.uint8, torch.bool):
+        raise ValueError(f"masks must be uint8 or bool [B, H, W], got {m.dtype} {list(m.shape)}")
+    B = m.shape[0]
+    Kh = _batched(_as_numpy(K, "K"), (3, 3), "K")
+    if len(Kh) not in (1, B):
+        raise ValueError(f"K [3, 3] or [B, 3, 3] with B = {B} expected, got {list(Kh.shape)}")
+    Kh = np.ascontiguousarray(np.broadcast_to(Kh, (B, 3, 3)))
+    d = _as_numpy(diameter, "diameter").reshape(-1)
+    if len(d) not in (1, B) or not (np.isfinite(d).all() and (d > 0).all()):
+        raise ValueError(f"diameter: a finite number > 0 or [B] with B = {B} expected, got {d.tolist()}")
+    t0 = initial_translation(m, torch.from_numpy(Kh), torch.from_numpy(np.broadcast_to(d, (B,)).copy()))
+    th = t0.cpu().numpy()                                   # the host geometry's one copy
+    bad = np.flatnonzero(~np.isfinite(th).all(1))
+    if len(bad):
+        raise ValueError(f"detections {bad.tolist()} have an empty mask")
+    pose = np.tile(np.eye(4), (B, 1, 1))
+    pose[:, :3, 3] = th
+    inv_maps = crop_transforms(Kh, pose, bbox_scale * d, image_size, keep_inplane=True)
+    fr = _tensor(frames)
+    if fr.dim() != 4 or fr.shape[3] != 3:
+        raise ValueError(f"frames must be uint8 [F, H, W, 3], got {fr.dtype} {list(fr.shape)}")
+    dev = fr.device if fr.device.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
+    paste = m.to(torch.uint8) * 255 if m.dtype == torch.bool else m
+    crops = crop_frames(fr, torch.from_numpy(inv_maps), image_size, masks=paste, frame_idx=frame_idx)
+    Rv = _camera(pose, True, dev)
+    return crops, t0, Rv, torch.from_numpy(inv_maps)

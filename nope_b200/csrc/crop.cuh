@@ -108,4 +108,82 @@ __global__ void __launch_bounds__(kCropThreads) crop_warp_kernel(
   }
 }
 
+// ---------------------------------------------------------------------------------
+// The crop camera (DESIGN.md section 23).  crop_frame maps the square of side s around the object centre o, spanned
+// by `upper` and `right`, onto the crop: the warp is the view of a pinhole camera at the real camera's centre with
+// rotation R_v (rows right / |right|, -upper / |upper|, o / |o|) and K_v = [[S |o| / s, 0, S/2], [0, S |o| / s, S/2],
+// [0, 0, 1]].  float64, every operation rounded on its own; norms sqrt((a a + b b) + c c), divisions per component,
+// products (p0 + p1) + p2.  tests/crop_camera_oracle.py restates it op by op.
+constexpr int kCropCamMax = 65535;     // F, P
+
+__device__ __forceinline__ double crop_cam_norm(double a, double b, double c) {
+  return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(a, a), __dmul_rn(b, b)), __dmul_rn(c, c)));
+}
+
+// a b - c d, each product rounded
+__device__ __forceinline__ double crop_cam_cross(double a, double b, double c, double d) {
+  return __dsub_rn(__dmul_rn(a, b), __dmul_rn(c, d));
+}
+
+// pose [F, 16] row-major (object -> camera) -> Rv [F, 9] row-major; one thread per pose
+__global__ void __launch_bounds__(256) crop_camera_kernel(const double* __restrict__ pose, int F, int keep_inplane,
+                                                          double* __restrict__ Rv) {
+  for (int f = blockIdx.x * blockDim.x + threadIdx.x; f < F; f += gridDim.x * blockDim.x) {
+    const double* p = pose + 16 * (size_t)f;
+    const double ox = p[3], oy = p[7], oz = p[11];
+    double ux, uy, uz, rx, ry, rz;                                  // upper, right
+    if (keep_inplane) {
+      ux = 0.0, uy = -oz, uz = oy;
+      rx = __dadd_rn(__dmul_rn(oy, oy), __dmul_rn(oz, oz));
+      ry = -__dmul_rn(ox, oy);
+      rz = -__dmul_rn(ox, oz);
+    } else {
+      // up = pose . ([0, 0, 6] - o, 1); right = o x up; upper = right x o
+      const double ax = __dsub_rn(0.0, ox), ay = __dsub_rn(0.0, oy), az = __dsub_rn(6.0, oz);
+      double up[3];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        const double* r = p + 4 * i;
+        up[i] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[0], ax), __dmul_rn(r[1], ay)), __dmul_rn(r[2], az)), r[3]);
+      }
+      rx = crop_cam_cross(oy, up[2], oz, up[1]);
+      ry = crop_cam_cross(oz, up[0], ox, up[2]);
+      rz = crop_cam_cross(ox, up[1], oy, up[0]);
+      ux = crop_cam_cross(ry, oz, rz, oy);
+      uy = crop_cam_cross(rz, ox, rx, oz);
+      uz = crop_cam_cross(rx, oy, ry, ox);
+    }
+    const double nu = crop_cam_norm(ux, uy, uz), nr = crop_cam_norm(rx, ry, rz), no = crop_cam_norm(ox, oy, oz);
+    double* o = Rv + 9 * (size_t)f;
+    if (nu == 0.0 && nr == 0.0) {
+      // crop_frame's image-axes fallback: the square lies parallel to the image plane, R_v = I
+#pragma unroll
+      for (int i = 0; i < 9; ++i) o[i] = i % 4 == 0 ? 1.0 : 0.0;
+      continue;
+    }
+    o[0] = __ddiv_rn(rx, nr), o[1] = __ddiv_rn(ry, nr), o[2] = __ddiv_rn(rz, nr);
+    o[3] = -__ddiv_rn(ux, nu), o[4] = -__ddiv_rn(uy, nu), o[5] = -__ddiv_rn(uz, nu);
+    o[6] = __ddiv_rn(ox, no), o[7] = __ddiv_rn(oy, no), o[8] = __ddiv_rn(oz, no);
+  }
+}
+
+// out[f, p] = A R[f, p] with A = Rv[f]^T (to_camera) or Rv[f]; one thread per 3 x 3, which is read whole before it
+// is written, so out may alias R
+__global__ void __launch_bounds__(256) crop_rotate_kernel(const double* __restrict__ Rv, const double* R, int P,
+                                                          long long n, int to_camera, double* out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const double* v = Rv + 9 * (size_t)((unsigned)i / (unsigned)P);     // i < F P < 2^32: a 32-bit division
+    double a[9], r[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) a[k] = __ldg(v + (to_camera ? (k % 3) * 3 + k / 3 : k)), r[k] = R[9 * i + k];
+#pragma unroll
+    for (int row = 0; row < 3; ++row)
+#pragma unroll
+      for (int col = 0; col < 3; ++col)
+        out[9 * i + 3 * row + col] = __dadd_rn(__dadd_rn(__dmul_rn(a[3 * row], r[col]),
+                                                         __dmul_rn(a[3 * row + 1], r[3 + col])),
+                                               __dmul_rn(a[3 * row + 2], r[6 + col]));
+  }
+}
+
 }  // namespace nope

@@ -1952,6 +1952,39 @@ int nope_crop_frames(const uint8_t* frames, int F, int H, int W, int C, const ui
   return 0;
 }
 
+// the crop camera (crop.cuh, DESIGN.md section 23)
+int nope_crop_camera(const double* pose, int F, int keep_inplane, double* Rv, void* stream) {
+  NOPE_CHECK(pose && Rv, "null argument");
+  NOPE_CHECK(F >= 1 && F <= kCropCamMax, "F must be in [1, 65535]");
+  NOPE_CHECK(keep_inplane == 0 || keep_inplane == 1, "keep_inplane must be 0 or 1");
+  for (int f = 0; f < F; ++f) {
+    const double* p = pose + 16 * (size_t)f;
+    // keep_inplane reads the translation only, the other mode the top three rows
+    for (int i = 0; i < 12; ++i)
+      NOPE_CHECK(std::isfinite(p[i]) || (keep_inplane && i % 4 != 3), "poses must be finite");
+    NOPE_CHECK(!keep_inplane || p[11] > 0.0, "keep_inplane needs the object centre in front of the camera (Z > 0)");
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ScratchArena arena(st);
+  const double* pd;
+  arena.add(&pd, 16 * (size_t)F, pose);
+  if (arena.alloc()) return -1;
+  crop_camera_kernel<<<ew_grid(F), 256, 0, st>>>(pd, F, keep_inplane, Rv);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int nope_crop_rotate(const double* Rv, int F, const double* R, int P, int to_camera, double* out, void* stream) {
+  NOPE_CHECK(Rv && R && out, "null argument");
+  NOPE_CHECK(F >= 1 && F <= kCropCamMax && P >= 1 && P <= kCropCamMax, "F and P must be in [1, 65535]");
+  NOPE_CHECK(to_camera == 0 || to_camera == 1, "to_camera must be 0 or 1");
+  const long long n = (long long)F * P;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  crop_rotate_kernel<<<ew_grid(n), 256, 0, st>>>(Rv, R, P, n, to_camera, out);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // ---------------------------------------------------------------------------------
 // per-op entry points
 // ---------------------------------------------------------------------------------

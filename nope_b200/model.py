@@ -681,6 +681,67 @@ class PoseConditional:
         return self._rerank(iou, R_out, t_out) if rerank else (R_out, t_out, iou)
 
     @torch.no_grad()
+    def predict_pose_frames(self, frames, masks, K, obj_ids, reference, all_relativeR, template_poses, angles=36, k=5,
+                            refiner=None, refine=None, frame_idx=None):
+        """6D poses of B detections in camera frames (DESIGN.md section 23): `crop.frame_crops` cuts a keep_inplane
+        crop around each mask's `initial_translation` t0, the in-plane search (`predict_pose_inplane`, or
+        `predict_pose_inplane_refined` with a refiner) finds the rotation in the crop's camera, `crop.to_camera`
+        re-expresses it in the real camera, and `translation.estimate_translation` fits t from t0, with
+        `contour_refine.refine_pose_contour` after it for refine="contour".
+          frames     uint8 [F, H, W, 3] RGB; masks uint8 or bool [B, H, W] (one per detection, nonzero = object)
+          K          [3, 3] or [B, 3, 3] intrinsics, read on the host; obj_ids B ids on the host, each with a mesh
+                     (load_mesh) and a models_info entry (load_models_info: the diameter)
+          reference  [1 | B, 3, 256, 256], all_relativeR [1 | B, N, 6] and template_poses [N, 3, 3] as
+                     predict_pose_inplane takes them: the templates' rotations in the query crop's camera
+          frame_idx  integer [B], or None when F == B
+          angles     the search's in-plane bins; a refiner brings its own (refiner.angles)
+        -> {"R": float64 [B, k, 3, 3] in the real camera, "t": float64 [B, k, 3] mm, "score": the search's [B, k],
+        "iou": the silhouette IoU [B, k], "R_crop": the search's rotations [B, k, 3, 3], "t0": [B, 3],
+        "crops": [B, 3, 256, 256]}.  R and t go unchanged into eval_bop(R_est=, t_est=), refine_depth and
+        select_distinct.  The only host synchronisation beyond the search's is frame_crops' copy of t0."""
+        from . import contour_refine, translation
+        from .crop import _as_numpy, _tensor, frame_crops, to_camera
+        import numpy as np
+        if refine not in (None, "contour"):
+            raise ValueError(f"refine must be None or 'contour', got {refine!r}")
+        ids = [int(i) for i in np.asarray(obj_ids.detach().cpu() if torch.is_tensor(obj_ids) else obj_ids)
+               .reshape(-1).tolist()]
+        B = len(ids)
+        if masks.shape[0] != B:
+            raise ValueError(f"predict_pose_frames: {B} obj_ids for {masks.shape[0]} masks")
+        missing = sorted(set(i for i in ids if i not in self.tless_cad or i not in self.bop_models))
+        if missing:
+            raise ValueError(f"predict_pose_frames: no mesh or models_info entry for obj_id {missing} (load_mesh, "
+                             "load_models_info)")
+        if reference.shape[0] not in (1, B):
+            raise ValueError(f"predict_pose_frames: reference [1 | B, 3, 256, 256] with B = {B} expected, got "
+                             f"{tuple(reference.shape)}")
+        diameter = np.array([self.bop_models[i]["diameter"] for i in ids], dtype=np.float64)
+        crops, t0, Rv, _ = frame_crops(frames, masks, K, diameter, image_size=256, frame_idx=frame_idx)
+        if refiner is None:
+            R_crop, nearest, angle, sim = self.predict_pose_inplane(crops, reference, all_relativeR, template_poses,
+                                                                    k=k, angles=angles)
+            N = sim.shape[-1]
+            score = sim.reshape(B, -1).gather(1, angle * N + nearest)
+        else:
+            R_crop, _, _, score = self.predict_pose_inplane_refined(crops, reference, all_relativeR, refiner, k=k)
+        R = to_camera(R_crop.to(self.device), Rv.to(self.device))
+        masks = _tensor(masks)
+        Kh = torch.from_numpy(np.ascontiguousarray(np.broadcast_to(_as_numpy(K, "K").reshape(-1, 3, 3), (B, 3, 3))))
+        kk = R.shape[1]
+        t = torch.empty((B, kk, 3), device=self.device, dtype=torch.float64)
+        iou = torch.empty((B, kk), device=self.device, dtype=torch.float64)
+        R_out = torch.empty_like(R) if refine == "contour" else R
+        for obj, ri, rd, pick in self._object_rows(ids):
+            mesh = self.tless_cad[obj]
+            t_o, iou_o = translation.estimate_translation(mesh, pick(R), Kh[ri], pick(masks), t_init=pick(t0))
+            if refine == "contour":
+                R_o, t_o, fit = contour_refine.refine_pose_contour(mesh, pick(R), t_o, Kh[ri], pick(masks))
+                R_out[rd], iou_o = R_o, fit["iou"]
+            t[rd], iou[rd] = t_o, iou_o
+        return {"R": R_out, "t": t, "score": score, "iou": iou, "R_crop": R_crop, "t0": t0, "crops": crops}
+
+    @torch.no_grad()
     def eval_bop(self, batch, data_name, R_est=None, save_path=None, t_est=None):
         """BOP 2019 average recall of a T-LESS batch (the `eval_vsd` schema): the grid retrieval's top-5 rotations, or
         R_est [B, k, 3, 3] from any search, at the ground-truth translation, or at t_est [B, k, 3] (mm, e.g. from
