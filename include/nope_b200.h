@@ -307,6 +307,24 @@ int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int
                          float znear, int iters, float* depth, double* t_out, double* iou, int32_t* stats_out,
                          void* stream);
 
+/* Pose fits under occlusion (DESIGN.md section 24).  occluders [F, H, W] uint8 on the device (nonzero = something may
+ * be in front of the object there; U = the other pixels) or NULL.  The mask becomes M' = M n U: O wins over M.
+ * nope_fit_translation_occluded: nope_fit_translation with the silhouette statistics (n_S, |S n M|, box) those of
+ * S' = S n U and the mask statistics those of M'; iou = |S' n M'| / |S' u M'|, stats_out those of S'.
+ * nope_refine_contour_occluded: nope_refine_contour with phi the signed distance field of M', the box size that scales
+ * tau that of M', and a contour pixel counted and paired only when it and its four neighbours lie in U; iou uses S'
+ * and M', and "empty or full" is judged on M'.  With occluders NULL (or all zero) both equal the plain entry points
+ * bit for bit, which forward to them.  Arguments, refusals and guarantees otherwise as the plain entry points. */
+int nope_fit_translation_occluded(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
+                                  const double* t_init, const uint8_t* masks, const uint8_t* occluders,
+                                  const double* K, int F, int P, int H, int W, float znear, int iters, float* depth,
+                                  double* t_out, double* iou, int32_t* stats_out, void* stream);
+int nope_refine_contour_occluded(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
+                                 const double* t_init, const uint8_t* masks, const uint8_t* occluders,
+                                 const double* K, int F, int P, int H, int W, double rho, const double* tau, int iters,
+                                 float znear, float* depth, double* R_out, double* t_out, double* fit_out,
+                                 int64_t* sums_out, void* stream);
+
 /* Pose refinement from the sensor depth (DESIGN.md section 19).
  * nope_refine_depth: projective point-to-plane ICP of P pose hypotheses per frame for F frames against the frame's
  * sensor depth.  Mesh as nope_render_depth; R [F, P, 9] fp64 row-major and t_init [F, P, 3] fp64 (model -> OpenCV

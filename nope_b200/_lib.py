@@ -64,6 +64,10 @@ SIGNATURES = {
     "nope_fit_translation": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, c_f32p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "nope_fit_translation_occluded": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                C.c_int, C.c_float, C.c_int, c_f32p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p]),
     "nope_refine_depth": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_void_p,
                                     C.c_int, C.c_float, c_f32p, C.c_void_p, C.c_void_p, C.c_void_p, c_i64p,
@@ -72,6 +76,10 @@ SIGNATURES = {
     "nope_refine_contour": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_int,
                                       C.c_float, c_f32p, C.c_void_p, C.c_void_p, C.c_void_p, c_i64p, C.c_void_p]),
+    "nope_refine_contour_occluded": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                               C.c_double, C.c_void_p, C.c_int, C.c_float, c_f32p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, c_i64p, C.c_void_p]),
     "nope_pose_errors": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "nope_crop_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

@@ -11,6 +11,7 @@ import torch
 from . import _lib
 from ._posefit import MAX_BATCH, MAX_ITERS, _masks, broadcast_t, check_iters, cuda_device, fit_args, geometric, \
     pack_refined, refine_outputs, taus, workspace
+from .translation import occluder_masks
 from .bop import _to_dev
 from .vsd import _stream
 
@@ -51,7 +52,8 @@ def mask_sdf(masks):
     return out
 
 
-def refine_pose_contour(mesh, R, t, K, masks, iters=DEFAULT_ITERS, tau=None, znear=0.05, return_sums=False):
+def refine_pose_contour(mesh, R, t, K, masks, iters=DEFAULT_ITERS, tau=None, znear=0.05, return_sums=False,
+                        occluders=None):
     """Refine every pose hypothesis against its frame's object mask (DESIGN.md section 20):
       mesh   a CUDA `nope_b200.vsd.Mesh` (mm, model frame),
       R      [F, P, 3, 3] (or [F, 3, 3] for P = 1), float32 or float64, model -> OpenCV camera,
@@ -60,7 +62,12 @@ def refine_pose_contour(mesh, R, t, K, masks, iters=DEFAULT_ITERS, tau=None, zne
       masks  [F, H, W] (or [H, W] for F = 1) uint8 or bool, nonzero = object; (H, W) is the frame size,
       iters  updates (default 10); tau: the pairing tolerances as fractions of the mask's box size sqrt(w h), a number
              or iters + 1 numbers (iteration i pairs at tau[i], the returned fit is scored at tau[iters]); None:
-             `default_tau(iters)`; znear as `render_depth`.
+             `default_tau(iters)`; znear as `render_depth`,
+      occluders  None, or [F, H, W] uint8 or bool with the masks' shape: nonzero where something may be in front of
+             the object (DESIGN.md section 24).  The fit then aligns with the mask minus the occluders (its signed
+             distance field and box size), and pairs only the contour pixels that, with their four neighbours, lie
+             outside them; "n_contour" counts those and "iou" is taken outside them.  None (or all zero) is the plain
+             refinement, bit for bit.  `mask_sdf` takes no occluders: pass it the mask minus them.
     -> (R float64 [F, P, 3, 3], t float64 [F, P, 3], fit): the pose after `iters` updates and a dict of float64 [F, P]
     tensors at it: "n_in" the contour pixels paired with the mask, "n_contour" every contour pixel of the render,
     "rms" the RMS distance of the pairs to the mask's outline (px, NaN without pairs) and "iou" the silhouette IoU
@@ -71,18 +78,20 @@ def refine_pose_contour(mesh, R, t, K, masks, iters=DEFAULT_ITERS, tau=None, zne
     masks = _masks(masks)
     if masks.shape[0] != F_:
         raise ValueError(f"masks [{F_}, H, W] expected, got {tuple(masks.shape)}")
+    occ = occluder_masks(occluders, masks)
     H, W = masks.shape[1:]
     tv = taus(default_tau(iters) if tau is None else tau, iters)
     dev = cuda_device(mesh, "refine_pose_contour")
     with torch.cuda.device(dev):
         md = _to_dev(masks, dev, torch.uint8)
+        od = None if occ is None else _to_dev(occ, dev, torch.uint8)
         t0 = broadcast_t(t, F_, P, dev)
         Rd = _to_dev(R, dev, torch.float64)
         ws = workspace(dev, F_, P, H, W)
         R_out, t_out, fit, sums = refine_outputs(dev, F_, P, return_sums)
-        _lib.check(_lib.load().nope_refine_contour(
+        _lib.check(_lib.load().nope_refine_contour_occluded(
             _lib.ptr(mesh.vertices), mesh.vertices.shape[0], _lib.ptr(mesh.faces), mesh.num_faces, _lib.ptr(Rd),
-            _lib.ptr(t0), _lib.ptr(md), k.data_ptr(), F_, P, H, W, mesh.radius, tv.ctypes.data, iters,
+            _lib.ptr(t0), _lib.ptr(md), _lib.ptr(od), k.data_ptr(), F_, P, H, W, mesh.radius, tv.ctypes.data, iters,
             float(znear), _lib.ptr(ws), _lib.ptr(R_out), _lib.ptr(t_out), _lib.ptr(fit), _lib.ptr(sums),
             _stream(dev)))
     return pack_refined(R_out, t_out, fit, sums, FIT_FIELDS)

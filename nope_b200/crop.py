@@ -344,3 +344,33 @@ def frame_crops(frames, masks, K, diameter, image_size=256, frame_idx=None, bbox
     crops = crop_frames(fr, torch.from_numpy(inv_maps), image_size, masks=paste, frame_idx=frame_idx)
     Rv = _camera(pose, True, dev)
     return crops, t0, Rv, torch.from_numpy(inv_maps)
+
+
+def detection_occluders(masks, frame_idx=None, num_frames=None):
+    """The occluders of B detections that share frames (DESIGN.md section 24): O_b = (the union of the masks of the
+    other detections of frame frame_idx[b]) minus b's own mask, uint8 [B, H, W] (1 = another detection may hide the
+    object there) on the masks' device.
+      masks      uint8 or bool [B, H, W], one per detection, nonzero = object (host or CUDA)
+      frame_idx  integer [B] (host or on the masks' device), or None for one frame per detection (every O_b empty)
+      num_frames F, the number of frames; indices outside [0, F) share one group below 0 and one at F or above (they
+                 are crop_frames' all-black crops).  None: max(frame_idx) + 1, read on the host.
+    A per-frame count of the masks (`index_add_`) minus the detection's own: plain torch, no host synchronisation for
+    host frame indices or a given num_frames."""
+    m = _tensor(masks)
+    if m.dim() != 3 or m.shape[0] < 1 or m.dtype not in (torch.uint8, torch.bool):
+        raise ValueError(f"masks must be uint8 or bool [B, H, W], got {m.dtype} {list(m.shape)}")
+    B = m.shape[0]
+    if frame_idx is None:
+        fi, F_ = torch.arange(B), B
+    else:
+        fi = _tensor(frame_idx)
+        if fi.is_floating_point() or fi.is_complex() or fi.dtype == torch.bool or tuple(fi.shape) != (B,):
+            raise ValueError(f"frame_idx must be integer [B] = [{B}], got {fi.dtype} {list(fi.shape)}")
+        F_ = int(fi.max()) + 1 if num_frames is None else int(num_frames)
+    if F_ < 1:
+        raise ValueError(f"num_frames must be >= 1, got {F_}")
+    from .bop import _to_dev
+    fi = _to_dev(fi, m.device, torch.int64).clamp(-1, F_) + 1              # groups 0 ... F + 1
+    own = (m != 0).to(torch.int32)
+    count = torch.zeros((F_ + 2,) + tuple(m.shape[1:]), dtype=torch.int32, device=m.device).index_add_(0, fi, own)
+    return ((count[fi] > own) & (own == 0)).to(torch.uint8)

@@ -32,24 +32,27 @@ constexpr int kSdfSmemBytes = 48 * 1024;         // the row pass's envelopes: 4 
 
 // Column pass: grid (ceil(W / kSdfColThreads), F), one thread per column.  g [F, H, W] packs, for each pixel, the row
 // distance to the nearest object pixel of its column (low 16 bits) and to the nearest background pixel (high 16
-// bits); "none in the column" is INF = H + W, which is larger than any distance in the frame.  Adjacent threads read
-// and write adjacent columns, so every row access is coalesced.
+// bits); "none in the column" is INF = H + W, which is larger than any distance in the frame.  occ [F, H, W] may be
+// null; where it is nonzero the pixel is background, so the field is that of M n U (DESIGN.md section 24).  Adjacent
+// threads read and write adjacent columns, so every row access is coalesced.
 __global__ void __launch_bounds__(kSdfColThreads)
-mask_sdf_cols_kernel(const uint8_t* __restrict__ masks, int H, int W, unsigned* __restrict__ g) {
+mask_sdf_cols_kernel(const uint8_t* __restrict__ masks, const uint8_t* __restrict__ occ, int H, int W,
+                     unsigned* __restrict__ g) {
   const int f = blockIdx.y, c = blockIdx.x * kSdfColThreads + threadIdx.x;
   if (c >= W) return;
   const size_t base = (size_t)f * H * W + c;
   const uint8_t* m = masks + base;
+  const uint8_t* o = occ ? occ + base : nullptr;
   unsigned* gc = g + base;
   const int inf = H + W;
   int lo = -inf, lb = -inf;                      // the last object / background row above
   for (int r = 0; r < H; ++r) {
-    if (m[(size_t)r * W]) lo = r; else lb = r;
+    if (m[(size_t)r * W] && !(o && o[(size_t)r * W])) lo = r; else lb = r;
     gc[(size_t)r * W] = (unsigned)min(r - lo, inf) | ((unsigned)min(r - lb, inf) << 16);
   }
   lo = H - 1 + inf; lb = H - 1 + inf;            // the next object / background row below
   for (int r = H - 1; r >= 0; --r) {
-    if (m[(size_t)r * W]) lo = r; else lb = r;
+    if (m[(size_t)r * W] && !(o && o[(size_t)r * W])) lo = r; else lb = r;
     const unsigned v = gc[(size_t)r * W];
     gc[(size_t)r * W] = (unsigned)min((int)(v & 0xffffu), lo - r) | ((unsigned)min((int)(v >> 16), lb - r) << 16);
   }
@@ -133,19 +136,21 @@ __device__ __forceinline__ double contour_kappa(double t2, double fx, double fy)
 // The pairs of one iteration: grid (ceil(H W / kIcpPixelsPerCta), P, F).  z [F, P, H, W] the render of hypothesis
 // (f, p) (float bits, +inf where nothing is hit), phi [F, H, W], K [F, 4], t [F, P, 3] the hypotheses' current
 // origins.  A contour pixel (interior, hit, a neighbour not hit) is counted into n_contour [F, P]; with e = phi + 1/2
-// in [-tau, tau] and a non-zero gradient of phi it adds its fixed-point products to 28 int64 registers.  The CTA
-// reduces them through warp shuffles and shared memory and adds its partials to sums [F, P, 29] with one integer
-// atomic per field.
+// in [-tau, tau] and a non-zero gradient of phi it adds its fixed-point products to 28 int64 registers.  occ [F, H, W]
+// may be null; otherwise a contour pixel counts only when neither it nor a 4-neighbour is in occ (DESIGN.md section
+// 24): next to an occluder the object's outline is unknown.  The CTA reduces the registers through warp shuffles and
+// shared memory and adds its partials to sums [F, P, 29] with one integer atomic per field.
 __global__ void __launch_bounds__(kIcpThreads)
-contour_accumulate_kernel(const unsigned* __restrict__ z, const double* __restrict__ phi, const double* __restrict__ K,
-                          const double* __restrict__ t, const int* __restrict__ mask_stats, int P, int H, int W,
-                          double tau_frac, double rho, unsigned long long* __restrict__ sums,
-                          int* __restrict__ n_contour) {
+contour_accumulate_kernel(const unsigned* __restrict__ z, const double* __restrict__ phi,
+                          const uint8_t* __restrict__ occ, const double* __restrict__ K, const double* __restrict__ t,
+                          const int* __restrict__ mask_stats, int P, int H, int W, double tau_frac, double rho,
+                          unsigned long long* __restrict__ sums, int* __restrict__ n_contour) {
   const int p = blockIdx.y, f = blockIdx.z;
   const int hw = H * W;
   const size_t h = (size_t)f * P + p;
   const unsigned* zi = z + h * hw;
   const double* ph = phi + (size_t)f * hw;
+  const uint8_t* o = occ ? occ + (size_t)f * hw : nullptr;
   const double fx = K[4 * f], fy = K[4 * f + 1], cx = K[4 * f + 2], cy = K[4 * f + 3];
   const double to[3] = {t[3 * h], t[3 * h + 1], t[3 * h + 2]};
   const double tau = contour_tau(tau_frac, mask_stats + kFitStats * f, hw);
@@ -161,6 +166,7 @@ contour_accumulate_kernel(const unsigned* __restrict__ z, const double* __restri
     const unsigned d0 = zi[i];
     if (!icp_hit(d0)) continue;
     if (icp_hit(zi[i - 1]) && icp_hit(zi[i + 1]) && icp_hit(zi[i - W]) && icp_hit(zi[i + W])) continue;
+    if (o && (o[i] | o[i - 1] | o[i + 1] | o[i - W] | o[i + W])) continue;
     ++nc;
     const double e = __dadd_rn(ph[i], 0.5);
     if (!(fabs(e) <= tau)) continue;
@@ -224,8 +230,9 @@ __global__ void contour_solve_kernel(int F, int P, long long hw, double tau_frac
 }
 
 // The outputs after the last render: R_out [F, P, 9], t_out [F, P, 3], fit [F, P, 4] = (n_in, n_contour,
-// rms = tau sqrt(sum e^2 / n_in) px, iou = |S n M| / |S u M|) -- rms is NaN when n_in = 0, rms and iou are NaN for a
-// frame without a contour -- and sums_out [F, P, 29] (optional) the integer sums of the last render.
+// rms = tau sqrt(sum e^2 / n_in) px, iou = |S n M| / |S u M| over the known pixels) -- rms is NaN when n_in = 0,
+// rms and iou are NaN for a frame without a contour -- and sums_out [F, P, 29] (optional) the integer sums of the last
+// render.
 __global__ void contour_final_kernel(const double* __restrict__ R, const double* __restrict__ t,
                                      const unsigned long long* __restrict__ sums, const int* __restrict__ n_contour,
                                      const int* __restrict__ mask_stats, const int* __restrict__ sil_stats, int F,

@@ -1762,6 +1762,16 @@ int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int
                          const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
                          float znear, int iters, float* depth, double* t_out, double* iou, int32_t* stats_out,
                          void* stream) {
+  return nope_fit_translation_occluded(vertices, V, faces, NF, R, t_init, masks, nullptr, K, F, P, H, W, znear, iters,
+                                       depth, t_out, iou, stats_out, stream);
+}
+
+// occluders [F, H, W] (nullable): the pixels where the object may be hidden count for neither the silhouette nor the
+// mask (DESIGN.md section 24); null is the plain fit, bit for bit
+int nope_fit_translation_occluded(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
+                                  const double* t_init, const uint8_t* masks, const uint8_t* occluders,
+                                  const double* K, int F, int P, int H, int W, float znear, int iters, float* depth,
+                                  double* t_out, double* iou, int32_t* stats_out, void* stream) {
   NOPE_CHECK(vertices && faces && R && t_init && masks && K && depth && t_out && iou, "null argument");
   if (check_fit_args(V, NF, F, P, H, W, znear, iters, INT_MAX)) return -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1783,12 +1793,14 @@ int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int
   NOPE_CUDA(cudaGetLastError());
   const long long hw = (long long)H * W;
   const int stat_blocks = (int)((hw + kFitPixelsPerCta - 1) / kFitPixelsPerCta);
-  fit_stats_kernel<false><<<dim3(stat_blocks, 1, F), kFitThreads, 0, st>>>(nullptr, masks, P, H, W, mask_stats);
+  fit_stats_kernel<false><<<dim3(stat_blocks, 1, F), kFitThreads, 0, st>>>(nullptr, masks, occluders, P, H, W,
+                                                                          mask_stats);
   NOPE_CUDA(cudaGetLastError());
   unsigned* z = reinterpret_cast<unsigned*>(depth);
   for (int it = 0; it <= iters; ++it) {
     if (render_frames(vertices, V, faces, NF, poses, K, F, P, znear, H, W, z, st)) return -1;
-    fit_stats_kernel<true><<<dim3(stat_blocks, P, F), kFitThreads, 0, st>>>(z, masks, P, H, W, sil_stats);
+    fit_stats_kernel<true><<<dim3(stat_blocks, P, F), kFitThreads, 0, st>>>(z, masks, occluders, P, H, W,
+                                                                           sil_stats);
     NOPE_CUDA(cudaGetLastError());
     if (it < iters) {
       fit_update_kernel<<<ew_blocks, 256, 0, st>>>(R, kd, mask_stats, F, P, t, poses, sil_stats);
@@ -1847,9 +1859,12 @@ int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF
   return launch_depth_finish(z, (long long)n * hw, st);      // depth holds render_depth at the returned pose
 }
 
-// phi [F, H, W] of masks [F, H, W] through the column pass into g [F, H, W] and the row pass
-static int launch_mask_sdf(const uint8_t* masks, int F, int H, int W, unsigned* g, double* phi, cudaStream_t st) {
-  mask_sdf_cols_kernel<<<dim3((W + kSdfColThreads - 1) / kSdfColThreads, F), kSdfColThreads, 0, st>>>(masks, H, W, g);
+// phi [F, H, W] of masks [F, H, W] minus the nullable occluders [F, H, W] through the column pass into g [F, H, W] and
+// the row pass
+static int launch_mask_sdf(const uint8_t* masks, const uint8_t* occ, int F, int H, int W, unsigned* g, double* phi,
+                           cudaStream_t st) {
+  mask_sdf_cols_kernel<<<dim3((W + kSdfColThreads - 1) / kSdfColThreads, F), kSdfColThreads, 0, st>>>(masks, occ, H,
+                                                                                                     W, g);
   NOPE_CUDA(cudaGetLastError());
   const int rows = mask_sdf_rows_per_cta(W);
   mask_sdf_rows_kernel<<<dim3((H + rows - 1) / rows, F), rows, sizeof(unsigned) * rows * W, st>>>(g, H, W, phi);
@@ -1866,13 +1881,24 @@ int nope_mask_sdf(const uint8_t* masks, int F, int H, int W, double* sdf_out, vo
   unsigned* g;
   arena.add(&g, (size_t)F * H * W);
   if (arena.alloc()) return -1;
-  return launch_mask_sdf(masks, F, H, W, g, sdf_out, st);
+  return launch_mask_sdf(masks, nullptr, F, H, W, g, sdf_out, st);
 }
 
 int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
                         const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
                         double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
                         double* t_out, double* fit_out, int64_t* sums_out, void* stream) {
+  return nope_refine_contour_occluded(vertices, V, faces, NF, R, t_init, masks, nullptr, K, F, P, H, W, rho, tau,
+                                      iters, znear, depth, R_out, t_out, fit_out, sums_out, stream);
+}
+
+// occluders [F, H, W] (nullable): phi and the mask statistics are those of the mask minus the occluders, and a contour
+// pixel next to an occluder is not paired (DESIGN.md section 24); null is the plain refinement, bit for bit
+int nope_refine_contour_occluded(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
+                                 const double* t_init, const uint8_t* masks, const uint8_t* occluders,
+                                 const double* K, int F, int P, int H, int W, double rho, const double* tau, int iters,
+                                 float znear, float* depth, double* R_out, double* t_out, double* fit_out,
+                                 int64_t* sums_out, void* stream) {
   NOPE_CHECK(vertices && faces && R && t_init && masks && K && tau && depth && R_out && t_out && fit_out,
              "null argument");
   if (check_fit_args(V, NF, F, P, H, W, znear, iters, 1024) || check_rho_tau(rho, tau, iters)) return -1;
@@ -1905,14 +1931,15 @@ int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int 
   const long long hw = (long long)H * W;
   const int px_blocks = (int)((hw + kIcpPixelsPerCta - 1) / kIcpPixelsPerCta);
   const int stat_blocks = (int)((hw + kFitPixelsPerCta - 1) / kFitPixelsPerCta);
-  fit_stats_kernel<false><<<dim3(stat_blocks, 1, F), kFitThreads, 0, st>>>(nullptr, masks, P, H, W, mask_stats);
+  fit_stats_kernel<false><<<dim3(stat_blocks, 1, F), kFitThreads, 0, st>>>(nullptr, masks, occluders, P, H, W,
+                                                                          mask_stats);
   NOPE_CUDA(cudaGetLastError());
-  if (launch_mask_sdf(masks, F, H, W, g, phi, st)) return -1;
+  if (launch_mask_sdf(masks, occluders, F, H, W, g, phi, st)) return -1;
   unsigned* z = reinterpret_cast<unsigned*>(depth);
   for (int it = 0; it <= iters; ++it) {
     if (render_frames(vertices, V, faces, NF, poses, K, F, P, znear, H, W, z, st)) return -1;
-    contour_accumulate_kernel<<<dim3(px_blocks, P, F), kIcpThreads, 0, st>>>(z, phi, kd, tc, mask_stats, P, H, W,
-                                                                             tau[it], rho, sums, n_contour);
+    contour_accumulate_kernel<<<dim3(px_blocks, P, F), kIcpThreads, 0, st>>>(z, phi, occluders, kd, tc, mask_stats, P,
+                                                                             H, W, tau[it], rho, sums, n_contour);
     NOPE_CUDA(cudaGetLastError());
     if (it < iters) {
       contour_solve_kernel<<<ew_blocks, 256, 0, st>>>(F, P, hw, tau[it], rho, mask_stats, kd, Rc, tc, poses, sums,
@@ -1920,7 +1947,7 @@ int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int 
       NOPE_CUDA(cudaGetLastError());
     }
   }
-  fit_stats_kernel<true><<<dim3(stat_blocks, P, F), kFitThreads, 0, st>>>(z, masks, P, H, W, sil_stats);
+  fit_stats_kernel<true><<<dim3(stat_blocks, P, F), kFitThreads, 0, st>>>(z, masks, occluders, P, H, W, sil_stats);
   NOPE_CUDA(cudaGetLastError());
   contour_final_kernel<<<ew_blocks, 256, 0, st>>>(Rc, tc, sums, n_contour, mask_stats, sil_stats, F, P, hw,
                                                   tau[iters], R_out, t_out, fit_out,

@@ -25,20 +25,24 @@ __device__ __forceinline__ void fit_stats_reset(int* s) {
 
 // Integer statistics of one image: grid (ceil(H W / kFitPixelsPerCta), P, F).  kSil: the silhouette of hypothesis
 // (f, p), z [F, P, H, W] depth bits (+inf where nothing is hit), with its intersection with the mask of frame f, into
-// stats [F, P, 6]; otherwise the mask of frame f (nonzero = object) into stats [F, 6] (n_inter unused).  Each CTA
+// stats [F, P, 6]; otherwise the mask of frame f (nonzero = object) into stats [F, 6] (n_inter unused).  occ
+// [F, H, W] (nonzero = something may hide the object; DESIGN.md section 24) may be null: its pixels count for neither
+// the silhouette nor the mask, so the statistics are those of S n U and M n U with U the pixels outside occ.  Each CTA
 // reduces its pixels through warp reductions and shared memory and adds its partials with one integer atomic per
 // field: integer sums, minima and maxima do not depend on the order, so neither does the result.
 template <bool kSil>
 __global__ void __launch_bounds__(kFitThreads)
-fit_stats_kernel(const unsigned* __restrict__ z, const uint8_t* __restrict__ masks, int P, int H, int W,
-                 int* __restrict__ stats) {
+fit_stats_kernel(const unsigned* __restrict__ z, const uint8_t* __restrict__ masks, const uint8_t* __restrict__ occ,
+                 int P, int H, int W, int* __restrict__ stats) {
   const int p = blockIdx.y, f = blockIdx.z;
   const int hw = H * W;
   const uint8_t* m = masks + (size_t)f * hw;
+  const uint8_t* o = occ ? occ + (size_t)f * hw : nullptr;
   const unsigned* zi = kSil ? z + ((size_t)f * P + p) * hw : nullptr;
   const int lo = blockIdx.x * kFitPixelsPerCta, hi = min(lo + kFitPixelsPerCta, hw);
   int n = 0, ni = 0, r0 = 0x7fffffff, r1 = -1, c0 = 0x7fffffff, c1 = -1;
   for (int i = lo + (int)threadIdx.x; i < hi; i += kFitThreads) {
+    if (o && o[i] != 0) continue;                // unknown: neither silhouette nor mask
     const bool in_m = m[i] != 0;
     const bool in = kSil ? zi[i] != kDepthInfBits : in_m;
     if (!in) continue;
@@ -127,8 +131,8 @@ __global__ void fit_update_kernel(const double* __restrict__ R, const double* __
   }
 }
 
-// The outputs after the last render: t_out [F, P, 3], iou [F, P] = |S n M| / |S u M| (0 for an empty silhouette),
-// both NaN for a frame whose mask is empty; stats_out [F, P, 6] (optional) the silhouette's statistics.
+// The outputs after the last render: t_out [F, P, 3], iou [F, P] = |S n M| / |S u M| (0 for an empty silhouette; S
+// and M are restricted to the known pixels when there are occluders), both NaN for a frame whose mask is empty; stats_out [F, P, 6] (optional) the silhouette's statistics.
 __global__ void fit_final_kernel(const double* __restrict__ t, const int* __restrict__ mask_stats,
                                  const int* __restrict__ sil_stats, int F, int P, double* __restrict__ t_out,
                                  double* __restrict__ iou, int* __restrict__ stats_out) {

@@ -608,23 +608,38 @@ class PoseConditional:
         return tuple(x[rows, order] for x in xs) + (score[rows, order],)
 
     @torch.no_grad()
-    def estimate_translation(self, batch, R, masks, iters=4):
+    def estimate_translation(self, batch, R, masks, iters=4, occluders=None):
         """The translation of every rotation hypothesis R [B, k, 3, 3] of a T-LESS batch (the `eval_vsd` schema; its
         "intrinsic" and "obj_id" are used) fitted to the object's mask of each frame, masks [B, H, W] (uint8 or bool,
         nonzero = object), starting from `translation.initial_translation` with the object's diameter
-        (load_models_info) and the mesh of load_mesh; DESIGN.md section 18.  One call per distinct object.
-        -> (t float64 [B, k, 3] mm, iou float64 [B, k]) on the model's device, without synchronising."""
+        (load_models_info) and the mesh of load_mesh; DESIGN.md section 18.  occluders [B, H, W] (uint8 or bool,
+        nonzero = something may hide the object there) make the fit ignore those pixels (DESIGN.md section 24); None
+        is the plain fit.  One call per distinct object.  -> (t float64 [B, k, 3] mm, iou float64 [B, k]) on the
+        model's device, without synchronising."""
         from . import translation
         ids, R, _, masks, K = self._pose_fit_batch("estimate_translation", batch, ("intrinsic", "obj_id"), R,
                                                    masks=masks)
+        occluders = self._occluders("estimate_translation", occluders, masks)
         B, k = R.shape[:2]
         t = torch.empty((B, k, 3), device=self.device, dtype=torch.float64)
         iou = torch.empty((B, k), device=self.device, dtype=torch.float64)
         for obj, ri, rd, pick in self._object_rows(ids):
             t[rd], iou[rd] = translation.estimate_translation(
                 self.tless_cad[obj], pick(R), K[ri], pick(masks), diameter=self.bop_models[obj]["diameter"],
-                iters=iters)
+                iters=iters, occluders=pick(occluders))
         return t, iou
+
+    @staticmethod
+    def _occluders(name, occluders, masks):
+        """occluders [B, H, W] with the masks' shape, or None; errors name the fit"""
+        if occluders is None:
+            return None
+        from ._posefit import _tensor
+        occluders = _tensor(occluders)
+        if tuple(occluders.shape) != tuple(masks.shape):
+            raise ValueError(f"{name}: occluders {tuple(masks.shape)} (the masks' shape) expected, got "
+                             f"{tuple(occluders.shape)}")
+        return occluders
 
     @torch.no_grad()
     def refine_depth(self, batch, R, t, masks=None, iters=None, rerank=False):
@@ -656,13 +671,14 @@ class PoseConditional:
         return self._rerank(score, R_out, t_out) if rerank else (R_out, t_out, score)
 
     @torch.no_grad()
-    def refine_contour(self, batch, R, t, masks, iters=None, rerank=False):
+    def refine_contour(self, batch, R, t, masks, iters=None, rerank=False, occluders=None):
         """Refine every pose hypothesis (R [B, k, 3, 3], t [B, k, 3] mm, e.g. a search's rotations with
         `estimate_translation`) of a T-LESS batch (the `eval_vsd` schema; its "intrinsic" and "obj_id" are used)
         against each frame's object mask masks [B, H, W] (uint8 or bool, nonzero = object; (H, W) the frame size) by
         aligning the rendered silhouette's contour with the mask's (`contour_refine.refine_pose_contour`, DESIGN.md
-        section 20), with the mesh of load_mesh and the default tolerance schedule.  No depth image is read.  One call
-        per distinct object.  -> (R float64 [B, k, 3, 3], t float64 [B, k, 3], iou float64 [B, k]) on the model's
+        section 20), with the mesh of load_mesh and the default tolerance schedule.  No depth image is read.
+        occluders [B, H, W] (uint8 or bool, nonzero = something may hide the object there) keep the fit off those
+        pixels (DESIGN.md section 24); None is the plain refinement.  One call per distinct object.  -> (R float64 [B, k, 3, 3], t float64 [B, k, 3], iou float64 [B, k]) on the model's
         device, iou = the refined pose's silhouette IoU with the mask (NaN for a frame whose mask is empty or full);
         with rerank, each row's hypotheses sorted by descending IoU (stable, NaN last).  The output feeds
         eval_bop(R_est=R, t_est=t); refine_depth can follow when the frame has depth."""
@@ -670,19 +686,20 @@ class PoseConditional:
         iters = contour_refine.DEFAULT_ITERS if iters is None else iters
         ids, R, t, masks, K = self._pose_fit_batch("refine_contour", batch, ("intrinsic", "obj_id"), R, t, masks,
                                                    models_info=False)
+        occluders = self._occluders("refine_contour", occluders, masks)
         B, k = R.shape[:2]
         R_out = torch.empty((B, k, 3, 3), device=self.device, dtype=torch.float64)
         t_out = torch.empty((B, k, 3), device=self.device, dtype=torch.float64)
         iou = torch.empty((B, k), device=self.device, dtype=torch.float64)
         for obj, ri, rd, pick in self._object_rows(ids):
             R_out[rd], t_out[rd], fit = contour_refine.refine_pose_contour(
-                self.tless_cad[obj], pick(R), pick(t), K[ri], pick(masks), iters=iters)
+                self.tless_cad[obj], pick(R), pick(t), K[ri], pick(masks), iters=iters, occluders=pick(occluders))
             iou[rd] = fit["iou"]
         return self._rerank(iou, R_out, t_out) if rerank else (R_out, t_out, iou)
 
     @torch.no_grad()
     def predict_pose_frames(self, frames, masks, K, obj_ids, reference, all_relativeR, template_poses, angles=36, k=5,
-                            refiner=None, refine=None, frame_idx=None):
+                            refiner=None, refine=None, frame_idx=None, occluders=None):
         """6D poses of B detections in camera frames (DESIGN.md section 23): `crop.frame_crops` cuts a keep_inplane
         crop around each mask's `initial_translation` t0, the in-plane search (`predict_pose_inplane`, or
         `predict_pose_inplane_refined` with a refiner) finds the rotation in the crop's camera, `crop.to_camera`
@@ -695,15 +712,21 @@ class PoseConditional:
                      predict_pose_inplane takes them: the templates' rotations in the query crop's camera
           frame_idx  integer [B], or None when F == B
           angles     the search's in-plane bins; a refiner brings its own (refiner.angles)
+          occluders  None; [B, H, W] uint8 or bool (nonzero = something may hide the detection's object there); or
+                     "detections": each detection's occluders are the other detections of its frame
+                     (`crop.detection_occluders`).  The translation fit and the contour refinement then ignore those
+                     pixels (DESIGN.md section 24); None is the plain fits, bit for bit.
         -> {"R": float64 [B, k, 3, 3] in the real camera, "t": float64 [B, k, 3] mm, "score": the search's [B, k],
         "iou": the silhouette IoU [B, k], "R_crop": the search's rotations [B, k, 3, 3], "t0": [B, 3],
         "crops": [B, 3, 256, 256]}.  R and t go unchanged into eval_bop(R_est=, t_est=), refine_depth and
         select_distinct.  The only host synchronisation beyond the search's is frame_crops' copy of t0."""
         from . import contour_refine, translation
-        from .crop import _as_numpy, _tensor, frame_crops, to_camera
+        from .crop import _as_numpy, _tensor, detection_occluders, frame_crops, to_camera
         import numpy as np
         if refine not in (None, "contour"):
             raise ValueError(f"refine must be None or 'contour', got {refine!r}")
+        if isinstance(occluders, str) and occluders != "detections":
+            raise ValueError(f"occluders must be None, a tensor or 'detections', got {occluders!r}")
         ids = [int(i) for i in np.asarray(obj_ids.detach().cpu() if torch.is_tensor(obj_ids) else obj_ids)
                .reshape(-1).tolist()]
         B = len(ids)
@@ -727,6 +750,11 @@ class PoseConditional:
             R_crop, _, _, score = self.predict_pose_inplane_refined(crops, reference, all_relativeR, refiner, k=k)
         R = to_camera(R_crop.to(self.device), Rv.to(self.device))
         masks = _tensor(masks)
+        if isinstance(occluders, str):
+            from .bop import _to_dev
+            md = masks if masks.device.type == "cuda" else _to_dev(masks, self.device, masks.dtype)
+            occluders = detection_occluders(md, frame_idx, num_frames=_tensor(frames).shape[0])
+        occluders = self._occluders("predict_pose_frames", occluders, masks)
         Kh = torch.from_numpy(np.ascontiguousarray(np.broadcast_to(_as_numpy(K, "K").reshape(-1, 3, 3), (B, 3, 3))))
         kk = R.shape[1]
         t = torch.empty((B, kk, 3), device=self.device, dtype=torch.float64)
@@ -734,9 +762,11 @@ class PoseConditional:
         R_out = torch.empty_like(R) if refine == "contour" else R
         for obj, ri, rd, pick in self._object_rows(ids):
             mesh = self.tless_cad[obj]
-            t_o, iou_o = translation.estimate_translation(mesh, pick(R), Kh[ri], pick(masks), t_init=pick(t0))
+            t_o, iou_o = translation.estimate_translation(mesh, pick(R), Kh[ri], pick(masks), t_init=pick(t0),
+                                                          occluders=pick(occluders))
             if refine == "contour":
-                R_o, t_o, fit = contour_refine.refine_pose_contour(mesh, pick(R), t_o, Kh[ri], pick(masks))
+                R_o, t_o, fit = contour_refine.refine_pose_contour(mesh, pick(R), t_o, Kh[ri], pick(masks),
+                                                                   occluders=pick(occluders))
                 R_out[rd], iou_o = R_o, fit["iou"]
             t[rd], iou[rd] = t_o, iou_o
         return {"R": R_out, "t": t, "score": score, "iou": iou, "R_crop": R_crop, "t0": t0, "crops": crops}
