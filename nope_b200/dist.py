@@ -124,7 +124,7 @@ class ShardedSweep:
         templates are never gathered (164 MB per query at N = 642).  query_feat [B,Q,C,32,32] (Q queries per
         reference) gives sim [B,Q,N] and topi [B,Q,k]: the B*Q (reference, query) pairs are the record's rows,
         still with one all-gather per sweep."""
-        from .unet import query_rows
+        from .search import query_rows
         N = all_relativeR.shape[1]
         lo, hi = shard_range(N, self.rank, self.world)
         B = reference_feat.shape[0]

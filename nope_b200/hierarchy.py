@@ -15,7 +15,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .unet import query_rows
+from .search import row_pairs
 
 MAX_KEEP = 64        # keep and k: the CTA-wide ranking kernels hold at most 64 chosen entries
 
@@ -152,21 +152,15 @@ def search(engine, ref_feat, query_feat, all_relativeR_levels, hierarchy, keep=8
     cells at level l (keep * F_l slots per row, one reference per row with its query) and ranks it.  Everything
     runs on the current stream; all sizes are known on the host, so nothing waits for the device."""
     check_search_args(hierarchy, all_relativeR_levels, keep, k)
-    dev = engine.device
-    ref_feat = ref_feat.to(dev, torch.float32).contiguous()
-    query_feat = query_feat.to(dev, torch.float32).contiguous()
-    Q, lead = query_rows(query_feat, ref_feat)
     B = ref_feat.shape[0]
     for l, p in enumerate(all_relativeR_levels):
         if p.shape[0] != B:
             raise ValueError(f"all_relativeR_levels[{l}] has {p.shape[0]} references, ref_feat {B}")
-    rows = B * Q
+    dev = engine.device
+    ref_feat, query_feat, Q, lead, ref_rows, query_rows_ = row_pairs(dev, ref_feat, query_feat)
     levels = [p.to(dev, torch.float32).contiguous() for p in all_relativeR_levels]
     top = engine.sweep(ref_feat, levels[0], query_feat=query_feat, want_emb=False, want_sim=False,
-                       k=keep)["topi"].reshape(rows, keep)
-    # every fine stage sweeps one row per (reference, query): the reference repeated for its queries, Q = 1
-    ref_rows = ref_feat[:, None].expand(B, Q, *ref_feat.shape[1:]).reshape(rows, *ref_feat.shape[1:])
-    query_rows_ = query_feat.reshape(rows, *ref_feat.shape[1:])
+                       k=keep)["topi"].reshape(B * Q, keep)
     last = hierarchy.num_levels - 1
     sim = topv = None
     for l in range(1, last + 1):

@@ -23,8 +23,8 @@ import torch
 
 from . import _lib
 from .inplane import check_angles, inplane_table
-from .refine import axis_angle_matrix, nearest_neighbour_angles
-from .unet import query_rows
+from .refine import axis_angle_matrix, grid_constants, identity_centres
+from .search import row_pairs
 
 XY = 9              # pose slots per centre: the 3x3 xy lattice, identity first, then lexicographic (i, j)
 ROLL = 3            # angle slots per centre: rho, rho + phi, rho - phi
@@ -48,18 +48,12 @@ class InplaneRefiner:
     made on first use."""
 
     def __init__(self, template_poses, angles=36, steps=4):
-        R = np.asarray(template_poses.cpu().numpy() if torch.is_tensor(template_poses) else template_poses,
-                       dtype=np.float64)
-        if R.ndim != 3 or R.shape[1:] != (3, 3) or R.shape[0] < 2:
-            raise ValueError(f"template_poses must be [N >= 2, 3, 3], got {tuple(R.shape)}")
         self.angles = check_angles(angles)
         if isinstance(steps, bool) or not isinstance(steps, numbers.Integral) or steps < 1:
             raise ValueError(f"steps must be a positive integer, got {steps!r}")
         self.steps = int(steps)
-        self.num_poses = int(R.shape[0])
-        self.template_poses = torch.from_numpy(R.copy())
-        self.theta0 = 0.5 * float(np.median(nearest_neighbour_angles(R)))
-        self.thetas = tuple(self.theta0 * 2.0 ** -s for s in range(self.steps))
+        self.template_poses, self.theta0, self.thetas = grid_constants(template_poses, self.steps)
+        self.num_poses = int(self.template_poses.shape[0])
         self.phi0 = math.pi / self.angles
         self.phis = tuple(self.phi0 * 2.0 ** -s for s in range(self.steps))
         self.stencils = torch.from_numpy(np.stack([xy_stencil(t).reshape(XY, 9) for t in self.thetas])
@@ -192,28 +186,17 @@ def refine_inplane(engine, encoder, ref_feat, query_images, all_relativeR, seeds
     keep = int(pose_idx.shape[-1])
     check_inplane_refine_args(refiner, all_relativeR, keep, k, ref_feat.shape[0])
     dev = engine.device
-    ref_feat = ref_feat.to(dev, torch.float32).contiguous()
-    B = ref_feat.shape[0]
-    img_rest = (3, 256, 256)
-    if query_images.dim() == 4 and tuple(query_images.shape) == (B,) + img_rest:
-        Q, lead = 1, (B,)
-    elif query_images.dim() == 5 and query_images.shape[0] == B and tuple(query_images.shape[2:]) == img_rest:
-        Q, lead = int(query_images.shape[1]), (B, int(query_images.shape[1]))
-    else:
-        raise ValueError(f"query_images must be [{B}, 3, 256, 256] or [{B}, Q, 3, 256, 256], got "
-                         f"{tuple(query_images.shape)}")
+    _, _, Q, lead, ref_rows, images = row_pairs(dev, ref_feat, query_images, (3, 256, 256))
     if tuple(pose_idx.shape) != lead + (keep,) or tuple(angle_idx.shape) != lead + (keep,):
         raise ValueError(f"seeds must be two {lead + (keep,)} tensors, got {tuple(pose_idx.shape)} and "
                          f"{tuple(angle_idx.shape)}")
     rest = tuple(ref_feat.shape[1:])
     if tuple(seed_latents.shape) != lead + (keep,) + rest:
         raise ValueError(f"seed_latents must be {lead + (keep,) + rest}, got {tuple(seed_latents.shape)}")
-    rows = B * Q
+    rows = ref_rows.shape[0]
     stencils, _, table = refiner._on(dev)
     rel = all_relativeR.to(dev, torch.float32).contiguous()
-    images = query_images.to(dev, torch.float32).reshape(rows, *img_rest).contiguous()
-    ref_rows = ref_feat[:, None].expand(B, Q, *rest).reshape(rows, *rest)
-    cur = {"D": torch.eye(3, device=dev, dtype=torch.float32).reshape(1, 1, 9).expand(rows, keep, 9).contiguous(),
+    cur = {"D": identity_centres(rows, keep, dev),
            "seed": pose_idx.to(dev).reshape(rows, keep).to(torch.int32),
            "cossin": table[angle_idx.to(dev).reshape(rows, keep)].contiguous()}
     lat = seed_latents.to(dev, torch.float32).reshape(rows, keep, *rest)

@@ -14,7 +14,8 @@ import ctypes as C
 import torch
 
 from . import _lib
-from .unet import query_rows
+from .search import coarse_to_fine_search, grid_search, refined_search
+from .unet import stage_sweep
 
 
 class UNetModelPose:
@@ -158,31 +159,9 @@ class UNetModelPose:
             raise _lib.NopeError("load_state_dict() must be called before the sweep")
         lib = _lib.load()
         dev = self.device
-        ref_latent = ref_latent.to(dev, torch.float32).contiguous()
-        poses = poses.to(dev, torch.float32).contiguous()
+        ref_latent, poses, query_latent, Q, emb, sim, topv, topi = stage_sweep(self, ref_latent, poses, query_latent,
+                                                                               want_emb, want_sim, k, out)
         B, N = poses.shape[0], poses.shape[1]
-        assert ref_latent.shape == (B, self.channels, 32, 32), ref_latent.shape
-        assert poses.shape[2] == self.rot_representation_dim
-        if want_sim is None:
-            want_sim = query_latent is not None
-        Q, lead = 1, (B,)
-        if query_latent is not None:
-            query_latent = query_latent.to(dev, torch.float32).contiguous()
-            Q, lead = query_rows(query_latent, ref_latent)
-        emb = torch.empty((B, N, self.channels, 32, 32), device=dev, dtype=torch.float32) if want_emb else None
-        out = out or {}
-        sim = out.get("sim") if want_sim else None
-        if want_sim and sim is None:
-            sim = torch.empty(lead + (N,), device=dev, dtype=torch.float32)
-        topv, topi = (out.get("topv"), out.get("topi")) if k > 0 else (None, None)
-        if k > 0 and topv is None:
-            topv = torch.empty(lead + (k,), device=dev, dtype=torch.float32)
-            topi = torch.empty(lead + (k,), device=dev, dtype=torch.int64)
-        for t, shape, dt in ((sim, lead + (N,), torch.float32), (topv, lead + (k,), torch.float32),
-                             (topi, lead + (k,), torch.int64)):
-            if t is not None and (tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous()
-                                  or t.device != dev):
-                raise ValueError("preallocated output has the wrong shape / dtype / device or is not contiguous")
         stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
             _lib.check(lib.nope_ldm_sweep_multi(self._handle(), _lib.ptr(ref_latent), _lib.ptr(poses), B, N,
@@ -200,55 +179,22 @@ class UNetModelPose:
         """Latent-space form of nope_b200.model.PoseConditional.predict_pose for this UNet:
         -> (R [B,k,3,3], nearest_idx [B,k], similarity [B,N]).  As there, query_latent [B,Q,C,32,32] gives
         [B,Q,...] outputs, and query_latent [Q,C,32,32] with one reference (ref_latent [1,...], all_relativeR
-        [1,N,6]) gives [Q,...]; both run one sweep."""
-        from .model import multi_query_form
-        q, squeeze = multi_query_form(query_latent, ref_latent)
-        out = self.sweep(ref_latent, all_relativeR, q, want_emb=False, want_sim=True, k=k)
-        idx, sim = out["topi"], out["sim"]
-        if squeeze:
-            idx, sim = idx[0], sim[0]
-        tp = template_poses.to(idx.device)
-        if squeeze and tp.dim() == 4:
-            tp = tp[0]                  # the one reference's grid
-        if tp.dim() == 3:
-            R = tp[idx]
-        else:
-            R = torch.stack([tp[b][idx[b]] for b in range(idx.shape[0])])
-        return R, idx, sim
+        [1,N,6]) gives [Q,...]; both run one sweep.  k is clamped to N; template_poses [B,N,3,3] is read at row 0."""
+        return grid_search(self, ref_latent, query_latent, all_relativeR, template_poses, k=k)
 
     def predict_pose_coarse_to_fine(self, query_latent, ref_latent, all_relativeR_levels, hierarchy,
                                     template_poses=None, k=5, keep=8):
         """Latent-space form of nope_b200.model.PoseConditional.predict_pose_coarse_to_fine for this UNet:
         -> (R | None, nearest_idx, similarity [..., N_L]) over the finest grid of `hierarchy`, -inf where the search
         scored nothing; the query forms of predict_pose."""
-        from .hierarchy import check_search_args, search
-        from .model import multi_query_form
-        check_search_args(hierarchy, all_relativeR_levels, keep, k)
-        q, squeeze = multi_query_form(query_latent, ref_latent)
-        out = search(self, ref_latent, q, all_relativeR_levels, hierarchy, keep=keep, k=k)
-        idx, sim = out["topi"], out["sim"]
-        if squeeze:
-            idx, sim = idx[0], sim[0]
-        R = None
-        if template_poses is not None:
-            tp = template_poses[0] if template_poses.dim() == 4 else template_poses
-            R = tp.to(idx.device)[idx]
-        return R, idx, sim
+        return coarse_to_fine_search(self, ref_latent, query_latent, all_relativeR_levels, hierarchy, template_poses,
+                                     k=k, keep=keep)
 
     def predict_pose_refined(self, query_latent, ref_latent, all_relativeR, refiner, k=5, keep=2):
         """Latent-space form of nope_b200.model.PoseConditional.predict_pose_refined for this UNet:
         -> (R [..., k, 3, 3] = D * template_poses[seed], seed_idx [..., k], score [..., k]); the query forms of
         predict_pose."""
-        from .model import multi_query_form
-        from .refine import check_refine_args, refine, template_rotations
-        check_refine_args(refiner, all_relativeR, keep, k, ref_latent.shape[0])
-        q, squeeze = multi_query_form(query_latent, ref_latent)
-        seeds = self.sweep(ref_latent, all_relativeR, q, want_emb=False, want_sim=False, k=keep)["topi"]
-        out = refine(self, ref_latent, q, all_relativeR, seeds, refiner, k=k)
-        D, seed, score = out["D"], out["seed"], out["score"]
-        if squeeze:
-            D, seed, score = D[0], seed[0], score[0]
-        return template_rotations(D, seed, refiner), seed, score
+        return refined_search(self, ref_latent, query_latent, all_relativeR, refiner, k=k, keep=keep)
 
     # ------------------------------------------------------------------ debug / parity hooks
     def debug_tap(self, ref_latent, poses, tap):

@@ -20,8 +20,8 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-
-_METRICS = {"l2": 0, "cosine": 1, "cosine_occlusion": 2}     # NOPE_METRIC_* of include/nope_b200.h
+from .search import (_METRICS, check_metric, coarse_to_fine_search, grid_search, multi_query_form,
+                     refined_search)
 
 
 def _ns(d):
@@ -114,9 +114,7 @@ class PoseConditional:
         """-> (similarity, nearest_idx).  Query and template batches follow the reference's broadcasting
         (model.py:260-262): equal batches give [B,N]; templates [1,N,...] serve every query ([Bq,N]: templates
         generated once, queries streamed); one query against [Bt,N,...] templates gives [Bt,N]."""
-        metric = getattr(self.testing_config, "similarity_metric", "l2")
-        if metric not in _METRICS:
-            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+        metric = self._metric()
         query_feat = self.u_net.encoder.encode_image(query.to(self.device), mode="mode")
         return score_topk(query_feat, template_feat, k=k, metric=metric, threshold=self._occlusion_threshold())
 
@@ -124,6 +122,30 @@ class PoseConditional:
         """`threshold` of the template encoder (OcclusionAwareSimilarity, base_template.py:67-75;
         configs/model/template_base.yaml: 0.2)."""
         return float(getattr(self.u_net.encoder, "threshold", 0.2))
+
+    def _metric(self):
+        return check_metric(getattr(self.testing_config, "similarity_metric", "l2"))
+
+    def _checked(self, query, reference, unsharded=None, check=None):
+        """The refusals of a search, all before anything is encoded: model.dist for a search that runs on one device
+        (`unsharded`, its name), the search's own argument check check(), the similarity metric and the query form.
+        -> (metric, what check returned)"""
+        if unsharded is not None and self.dist is not None:
+            raise NotImplementedError(f"{unsharded} does not shard across GPUs: it runs on one device (unset "
+                                      "model.dist or use predict_pose)")
+        checked = None if check is None else check()
+        metric = self._metric()
+        multi_query_form(query, reference)
+        return metric, checked
+
+    def _encode(self, query, reference, metric):
+        """The metric set for the sweep's last layer, then queries and references through one encoder call over
+        cat([flattened queries, references]).  -> (query latents in the query's form, reference latents)"""
+        self.u_net.set_metric(metric, self._occlusion_threshold())
+        flat = query.reshape(-1, *query.shape[-3:])
+        feats = self.u_net.encoder.encode_image(torch.cat([flat.to(self.device), reference.to(self.device)]))
+        n = flat.shape[0]
+        return feats[:n].view(*query.shape[:-3], *feats.shape[1:]), feats[n:]
 
     # ------------------------------------------------------------------ model.py:313-357
     @torch.no_grad()
@@ -138,41 +160,12 @@ class PoseConditional:
           query [Q,3,H,W] with reference [1,3,H,W] and all_relativeR [1,N,6] -> [Q,k,3,3], [Q,k], [Q,N]
           (the reference's broadcasting of one template set against a query batch).
         Query and reference images go through one encoder call, the templates through one sweep."""
-        metric = getattr(self.testing_config, "similarity_metric", "l2")
-        if metric not in _METRICS:
-            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
-        query, squeeze = multi_query_form(query, reference)
-        enc = self.u_net.encoder
-        self.u_net.set_metric(metric, self._occlusion_threshold())     # scored in the sweep's last layer
-        if query.dim() == reference.dim():
-            B = query.shape[0]
-            feats = enc.encode_image(torch.cat([query.to(self.device), reference.to(self.device)]))
-            query_feat, reference_feat = feats[:B], feats[B:]
-        else:
-            B, Q = query.shape[:2]
-            feats = enc.encode_image(torch.cat([query.reshape(B * Q, *query.shape[2:]).to(self.device),
-                                                reference.to(self.device)]))
-            query_feat, reference_feat = feats[:B * Q].view(B, Q, *feats.shape[1:]), feats[B * Q:]
-        N = all_relativeR.shape[1]
-        k = min(k, N)
-        if self.dist is not None:
-            sim, topi, emb = self.dist.sweep(self.u_net, reference_feat, all_relativeR, query_feat,
-                                             k=k, metric=metric, want_emb=return_templates,
-                                             threshold=self._occlusion_threshold())
-        else:
-            out = self.u_net.sweep(reference_feat, all_relativeR, query_feat=query_feat,
-                                   want_emb=return_templates, k=k)
-            sim, topi, emb = out["sim"], out["topi"], out["emb"]
-        if squeeze:
-            sim, topi = sim[0], topi[0]
-        R = None
-        if template_poses is not None:
-            tp = template_poses[0] if template_poses.dim() == 4 else template_poses
-            R = tp.to(topi.device)[topi]          # model.py:352-354
-        if return_templates:
-            # under sharding `emb` is (local templates, lo, hi): each rank keeps only its slice
-            return R, topi, sim, emb
-        return R, topi, sim
+        metric, _ = self._checked(query, reference)
+        query_feat, reference_feat = self._encode(query, reference, metric)
+        # under sharding the templates are (local templates, lo, hi): each rank keeps only its slice
+        return grid_search(self.u_net, reference_feat, query_feat, all_relativeR, template_poses, k=k,
+                           return_templates=return_templates, dist=self.dist, metric=metric,
+                           threshold=self._occlusion_threshold())
 
     @torch.no_grad()
     def predict_pose_coarse_to_fine(self, query, reference, all_relativeR_levels, hierarchy, template_poses=None,
@@ -184,32 +177,12 @@ class PoseConditional:
         -> (R | None, nearest_idx, similarity [..., N_L]) in the shapes of predict_pose (the same three query
         forms); similarity is -inf at poses the search did not score.  Every scored pose has exactly the score
         predict_pose gives it.  One encoder call."""
-        from .hierarchy import check_search_args, search
-        if self.dist is not None:
-            raise NotImplementedError("predict_pose_coarse_to_fine does not shard across GPUs: the coarse-to-fine "
-                                      "search runs on one device (unset model.dist or use predict_pose)")
-        check_search_args(hierarchy, all_relativeR_levels, keep, k)
-        metric = getattr(self.testing_config, "similarity_metric", "l2")
-        if metric not in _METRICS:
-            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
-        query, squeeze = multi_query_form(query, reference)
-        enc = self.u_net.encoder
-        self.u_net.set_metric(metric, self._occlusion_threshold())
-        B = reference.shape[0]
-        flat = query.reshape(-1, *query.shape[-3:])
-        feats = enc.encode_image(torch.cat([flat.to(self.device), reference.to(self.device)]))
-        query_feat, reference_feat = feats[:flat.shape[0]], feats[flat.shape[0]:]
-        if query.dim() != reference.dim():
-            query_feat = query_feat.view(B, query.shape[1], *feats.shape[1:])
-        out = search(self.u_net, reference_feat, query_feat, all_relativeR_levels, hierarchy, keep=keep, k=k)
-        sim, topi = out["sim"], out["topi"]
-        if squeeze:
-            sim, topi = sim[0], topi[0]
-        R = None
-        if template_poses is not None:
-            tp = template_poses[0] if template_poses.dim() == 4 else template_poses
-            R = tp.to(topi.device)[topi]
-        return R, topi, sim
+        from .hierarchy import check_search_args
+        metric, _ = self._checked(query, reference, "predict_pose_coarse_to_fine",
+                                  lambda: check_search_args(hierarchy, all_relativeR_levels, keep, k))
+        query_feat, reference_feat = self._encode(query, reference, metric)
+        return coarse_to_fine_search(self.u_net, reference_feat, query_feat, all_relativeR_levels, hierarchy,
+                                     template_poses, k=k, keep=keep)
 
     @torch.no_grad()
     def predict_pose_refined(self, query, reference, all_relativeR, refiner, k=5, keep=2):
@@ -220,30 +193,28 @@ class PoseConditional:
         forms of predict_pose; descending score, each exactly the score a sweep of that pose gives.  One encoder
         call.  keep = 2 by default: keep = 4 measured hardly more accurate for up to 1.8x the time (DESIGN.md
         section 6)."""
-        from .refine import check_refine_args, refine, template_rotations
-        if self.dist is not None:
-            raise NotImplementedError("predict_pose_refined does not shard across GPUs: the refinement runs on one "
-                                      "device (unset model.dist or use predict_pose)")
-        check_refine_args(refiner, all_relativeR, keep, k, reference.shape[0])
-        metric = getattr(self.testing_config, "similarity_metric", "l2")
-        if metric not in _METRICS:
-            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
-        query, squeeze = multi_query_form(query, reference)
+        from .refine import check_refine_args
+        metric, _ = self._checked(query, reference, "predict_pose_refined",
+                                  lambda: check_refine_args(refiner, all_relativeR, keep, k, reference.shape[0]))
+        query_feat, reference_feat = self._encode(query, reference, metric)
+        return refined_search(self.u_net, reference_feat, query_feat, all_relativeR, refiner, k=k, keep=keep)
+
+    def _inplane_sweep(self, query, reference, all_relativeR, metric, A, k):
+        """The in-plane search's sweep (DESIGN.md section 11): the references encoded on their own, the A rotated
+        copies of each of the B * Q queries by one encode_image_inplane call, one sweep with Q * A query rows per
+        reference, and the top-k of each (reference, query) row jointly over (angle, pose).
+        -> (sim [B, Q * A, N], top [B * Q, k] at a * N + n, query latents [B * Q, A, C, h, w], the flattened query
+        images [B * Q, 3, H, W] and the reference latents, on the device)"""
         enc = self.u_net.encoder
         self.u_net.set_metric(metric, self._occlusion_threshold())
-        B = reference.shape[0]
-        flat = query.reshape(-1, *query.shape[-3:])
-        feats = enc.encode_image(torch.cat([flat.to(self.device), reference.to(self.device)]))
-        query_feat, reference_feat = feats[:flat.shape[0]], feats[flat.shape[0]:]
-        if query.dim() != reference.dim():
-            query_feat = query_feat.view(B, query.shape[1], *feats.shape[1:])
-        seeds = self.u_net.sweep(reference_feat, all_relativeR, query_feat=query_feat, want_emb=False,
-                                 want_sim=False, k=keep)["topi"]
-        out = refine(self.u_net, reference_feat, query_feat, all_relativeR, seeds, refiner, k=k)
-        D, seed, score = out["D"], out["seed"], out["score"]
-        if squeeze:
-            D, seed, score = D[0], seed[0], score[0]
-        return template_rotations(D, seed, refiner), seed, score
+        B, N = reference.shape[0], all_relativeR.shape[1]
+        reference_feat = enc.encode_image(reference.to(self.device))
+        images = query.reshape(-1, *query.shape[-3:]).to(self.device)
+        query_feat = enc.encode_image_inplane(images, A)
+        sim = self.u_net.sweep(reference_feat, all_relativeR, query_feat=query_feat.view(B, -1, *query_feat.shape[2:]),
+                               want_emb=False, want_sim=True, k=0)["sim"]
+        _, top = topk(sim.view(-1, A * N), k)
+        return sim, top, query_feat, images, reference_feat
 
     @torch.no_grad()
     def predict_pose_inplane(self, query, reference, all_relativeR, template_poses=None, k=5, angles=36):
@@ -254,33 +225,19 @@ class PoseConditional:
         (angle, pose), ties -> the lowest a * N + n.  One encoder call for the references, one encode_image_inplane
         call for the queries, one sweep with Q * A query rows per reference.  angles = 1 is predict_pose."""
         from .inplane import check_inplane_args, compose
-        if self.dist is not None:
-            raise NotImplementedError("predict_pose_inplane does not shard across GPUs: the in-plane search runs on "
-                                      "one device (unset model.dist or use predict_pose)")
-        if all_relativeR.dim() != 3 or all_relativeR.shape[0] != reference.shape[0] or all_relativeR.shape[2] != 6:
-            raise ValueError(f"all_relativeR [B, N, 6] with B = {reference.shape[0]} references expected, got "
-                             f"{tuple(all_relativeR.shape)}")
-        N = all_relativeR.shape[1]
-        A, k = check_inplane_args(angles, k, N)
-        metric = getattr(self.testing_config, "similarity_metric", "l2")
-        if metric not in _METRICS:
-            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
-        query, squeeze = multi_query_form(query, reference)
-        B = reference.shape[0]
-        Q = 1 if query.dim() == reference.dim() else query.shape[1]
-        lead = (Q,) if squeeze else (B,) if query.dim() == reference.dim() else (B, Q)
-        enc = self.u_net.encoder
-        self.u_net.set_metric(metric, self._occlusion_threshold())
-        reference_feat = enc.encode_image(reference.to(self.device))
-        query_feat = enc.encode_image_inplane(query.reshape(B * Q, *query.shape[-3:]).to(self.device), A)
-        query_feat = query_feat.view(B, Q * A, *query_feat.shape[2:])
-        sim = self.u_net.sweep(reference_feat, all_relativeR, query_feat=query_feat, want_emb=False,
-                               want_sim=True, k=0)["sim"]                                  # [B, Q * A, N]
-        _, flat = topk(sim.view(B * Q, A * N), k)
-        nearest, angle = flat % N, flat // N
-        sim, nearest, angle = sim.view(lead + (A, N)), nearest.view(lead + (k,)), angle.view(lead + (k,))
+
+        def check():
+            if all_relativeR.dim() != 3 or all_relativeR.shape[0] != reference.shape[0] or all_relativeR.shape[2] != 6:
+                raise ValueError(f"all_relativeR [B, N, 6] with B = {reference.shape[0]} references expected, got "
+                                 f"{tuple(all_relativeR.shape)}")
+            return check_inplane_args(angles, k, all_relativeR.shape[1])
+
+        metric, (A, k) = self._checked(query, reference, "predict_pose_inplane", check)
+        sim, top, _, _, _ = self._inplane_sweep(query, reference, all_relativeR, metric, A, k)
+        N, lead = all_relativeR.shape[1], tuple(query.shape[:-3])
+        nearest, angle = (top % N).view(lead + (k,)), (top // N).view(lead + (k,))
         R = compose(template_poses, nearest, angle, A) if template_poses is not None else None
-        return R, nearest, angle, sim
+        return R, nearest, angle, sim.view(lead + (A, N))
 
     @torch.no_grad()
     def predict_pose_inplane_refined(self, query, reference, all_relativeR, refiner, k=5, keep=2):
@@ -292,31 +249,18 @@ class PoseConditional:
         atan2(sin, cos) of the roll rho, score [..., k]) in the query forms of predict_pose; descending score, each
         exactly the score a sweep of that pose against that rolled latent gives."""
         from .inplane_refine import check_inplane_refine_args, pose_rotations, refine_inplane, roll_degrees
-        if self.dist is not None:
-            raise NotImplementedError("predict_pose_inplane_refined does not shard across GPUs: the refinement runs "
-                                      "on one device (unset model.dist or use predict_pose)")
-        check_inplane_refine_args(refiner, all_relativeR, keep, k, reference.shape[0])
-        metric = getattr(self.testing_config, "similarity_metric", "l2")
-        if metric not in _METRICS:
-            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+        metric, _ = self._checked(
+            query, reference, "predict_pose_inplane_refined",
+            lambda: check_inplane_refine_args(refiner, all_relativeR, keep, k, reference.shape[0]))
+        _, top, query_feat, images, reference_feat = self._inplane_sweep(query, reference, all_relativeR, metric,
+                                                                         refiner.angles, keep)
+        N = refiner.num_poses
+        pose_idx, angle_idx = top % N, top // N
+        lat = query_feat[torch.arange(top.shape[0], device=top.device)[:, None], angle_idx]   # [B * Q, keep, C, h, w]
         query, squeeze = multi_query_form(query, reference)
-        B, A, N = reference.shape[0], refiner.angles, refiner.num_poses
-        Q = 1 if query.dim() == reference.dim() else query.shape[1]
-        enc = self.u_net.encoder
-        self.u_net.set_metric(metric, self._occlusion_threshold())
-        reference_feat = enc.encode_image(reference.to(self.device))
-        flat_q = query.reshape(B * Q, *query.shape[-3:]).to(self.device)
-        query_feat = enc.encode_image_inplane(flat_q, A)                                   # [B * Q, A, C, h, w]
-        sim = self.u_net.sweep(reference_feat, all_relativeR, want_emb=False, want_sim=True, k=0,
-                               query_feat=query_feat.view(B, Q * A, *query_feat.shape[2:]))["sim"]   # [B, Q * A, N]
-        _, flat = topk(sim.view(B * Q, A * N), keep)
-        pose_idx, angle_idx = flat % N, flat // N
-        rows = torch.arange(B * Q, device=flat.device)[:, None]
-        lat = query_feat[rows, angle_idx]                                                  # [B * Q, keep, C, h, w]
-        lead = (B,) if query.dim() == reference.dim() else (B, Q)
-        images = flat_q.view(*lead, *query.shape[-3:])
-        out = refine_inplane(self.u_net, enc, reference_feat, images, all_relativeR,
-                             (pose_idx.view(*lead, keep), angle_idx.view(*lead, keep)),
+        lead = tuple(query.shape[:-3])
+        out = refine_inplane(self.u_net, self.u_net.encoder, reference_feat, images.view(*lead, *query.shape[-3:]),
+                             all_relativeR, (pose_idx.view(*lead, keep), angle_idx.view(*lead, keep)),
                              lat.view(*lead, keep, *lat.shape[2:]), refiner, k=k)
         R = pose_rotations(out["D"], out["seed"], out["cossin"], refiner)
         seed, alpha, score = out["seed"], roll_degrees(out["cossin"]), out["score"]
@@ -340,25 +284,17 @@ class PoseConditional:
                              f"{tuple(template_feat.shape)}")
         N = template_feat.shape[1]
         A, k = check_inplane_args(angles, k, N)
-        metric = getattr(self.testing_config, "similarity_metric", "l2")
-        if metric not in _METRICS:
-            raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
-        B, Q, Bt, rows = broadcast_batches(query.shape[0], template_feat.shape[0])
+        metric = self._metric()
+        B, Q, _, rows = broadcast_batches(query.shape[0], template_feat.shape[0])
         dev = template_feat.device
         if dev.type != "cuda":
             raise _lib.NopeError("retrieval_inplane needs CUDA tensors (no CPU fallback)")
         q = enc.encode_image_inplane(query.to(dev), A)                                     # [Bq, A, C, h, w]
         q = q.reshape(-1, Q * A, *q.shape[2:]).expand(B, Q * A, *q.shape[2:]).contiguous()
-        t = template_feat.to(torch.float32).contiguous()
-        sim = torch.empty((rows, A, N), device=dev, dtype=torch.float32)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().nope_score_topk_multi(
-                _lib.ptr(q), _lib.ptr(t), B, Q * A, Bt, N, t.shape[2], t.shape[3] * t.shape[4], _METRICS[metric],
-                self._occlusion_threshold(), 0, _lib.ptr(sim), None, None, 0,
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        sim, _, _ = _score_multi(q, template_feat.to(torch.float32).contiguous(), B, Q * A, metric,
+                                 self._occlusion_threshold())
         _, flat = topk(sim.view(rows, A * N), k)
-        return sim, flat % N, flat // N
-
+        return sim.view(rows, A, N), flat % N, flat // N
 
     # ------------------------------------------------------------------ model.py:185-191, 268-376, 550-565
     def log(self, name, value, **kwargs):
@@ -850,23 +786,6 @@ class PoseConditional:
         return out
 
 
-def multi_query_form(query, reference):
-    """-> (query, squeeze).  query [B,...] with reference [B,...]: one query per reference, as given.
-    query [B,Q,...]: Q queries per reference, as given.  query [Q,...] with reference [1,...]: the broadcast form,
-    returned as [1,Q,...] with squeeze=True (outputs lose the leading 1).  Anything else raises ValueError."""
-    B, rest = reference.shape[0], tuple(reference.shape[1:])
-    if query.dim() == reference.dim() and tuple(query.shape[1:]) == rest:
-        if query.shape[0] == B:
-            return query, False
-        if B == 1 and query.shape[0] >= 1:
-            return query.unsqueeze(0), True
-    elif query.dim() == reference.dim() + 1 and tuple(query.shape[2:]) == rest and query.shape[0] == B \
-            and query.shape[1] >= 1:
-        return query, False
-    raise ValueError(f"query {tuple(query.shape)} does not fit reference {tuple(reference.shape)}: expected "
-                     f"[B, ...], [B, Q, ...] or (one reference) [Q, ...]")
-
-
 def broadcast_batches(bq, bt):
     """Batch rule of the reference's retrieval (model.py:260-262), where [Bq,1,...] queries meet [Bt,N,...]
     templates: -> (B, Q, Bt, rows of the result) in the terms of nope_score_topk_multi.  Equal batches pair
@@ -887,33 +806,38 @@ def score_topk(query_feat, template_feat, k=5, metric="l2", idx_base=0, threshol
     """similarity [B,N] and nearest_idx [B,k] of materialised templates
     (the arithmetic of model.py:260-265) on the GPU.  query_feat [Bq,C,h,w] and template_feat [Bt,N,C,h,w]
     broadcast as in the reference (broadcast_batches): B = max(Bq, Bt)."""
-    if metric not in _METRICS:
-        raise ValueError(f"unknown similarity_metric {metric!r} (supported: {sorted(_METRICS)})")
+    check_metric(metric)
     if template_feat.dim() != 5 or query_feat.dim() != 4 or tuple(query_feat.shape[1:]) != tuple(template_feat.shape[2:]):
         raise ValueError(f"query_feat [B,C,h,w] and template_feat [B,N,C,h,w] expected; got "
                          f"{tuple(query_feat.shape)} and {tuple(template_feat.shape)}")
-    B, Q, Bt, rows = broadcast_batches(query_feat.shape[0], template_feat.shape[0])
-    lib = _lib.load()
+    B, Q, _, _ = broadcast_batches(query_feat.shape[0], template_feat.shape[0])
     dev = template_feat.device
     if dev.type != "cuda":
         raise _lib.NopeError("score_topk needs CUDA tensors (no CPU fallback)")
+    N = template_feat.shape[1]
+    if k > N:
+        raise RuntimeError(f"selected index k out of range (k={k}, N={N})")  # torch.topk's error
     q = query_feat.to(dev, torch.float32)
     if q.shape[0] != B * Q:
         q = q.expand(B * Q, *q.shape[1:])
-    q = q.contiguous()
-    t = template_feat.to(torch.float32).contiguous()
-    N, Cc = t.shape[1], t.shape[2]
-    hw = t.shape[3] * t.shape[4]
-    if k > N:
-        raise RuntimeError(f"selected index k out of range (k={k}, N={N})")  # torch.topk's error
-    sim = torch.empty((rows, N), device=dev, dtype=torch.float32)
-    topv = torch.empty((rows, k), device=dev, dtype=torch.float32)
-    topi = torch.empty((rows, k), device=dev, dtype=torch.int64)
-    with torch.cuda.device(dev):
-        _lib.check(lib.nope_score_topk_multi(_lib.ptr(q), _lib.ptr(t), B, Q, Bt, N, Cc, hw, _METRICS[metric],
-                                             float(threshold), k, _lib.ptr(sim), _lib.ptr(topv), _lib.ptr(topi),
-                                             idx_base, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    sim, _, topi = _score_multi(q.contiguous(), template_feat.to(torch.float32).contiguous(), B, Q, metric,
+                                threshold, k, idx_base)
     return sim, topi
+
+
+def _score_multi(q, t, B, Q, metric, threshold, k=0, idx_base=0):
+    """nope_score_topk_multi on the current stream: q [B * Q, C, h, w] scored against t [Bt, N, C, h, w] (float32,
+    contiguous, on one CUDA device) -> (sim [B * Q, N], topv [B * Q, k], topi [B * Q, k])"""
+    dev = t.device
+    sim = torch.empty((B * Q, t.shape[1]), device=dev, dtype=torch.float32)
+    topv = torch.empty((B * Q, k), device=dev, dtype=torch.float32)
+    topi = torch.empty((B * Q, k), device=dev, dtype=torch.int64)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().nope_score_topk_multi(
+            _lib.ptr(q), _lib.ptr(t), B, Q, t.shape[0], t.shape[1], t.shape[2], t.shape[3] * t.shape[4],
+            _METRICS[metric], float(threshold), k, _lib.ptr(sim), _lib.ptr(topv), _lib.ptr(topi), idx_base,
+            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    return sim, topv, topi
 
 
 def topk(sim, k, idx_base=0):

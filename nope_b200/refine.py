@@ -19,7 +19,7 @@ import torch
 
 from . import _lib
 from .hierarchy import MAX_KEEP, rotation_trace
-from .unet import query_rows
+from .search import row_pairs
 
 STENCIL = 27        # the 3x3x3 lattice: slot 0 the identity, then the other 26 in lexicographic (i, j, l) order
 _OFFSETS = [(0, 0, 0)] + [v for v in itertools.product((-1, 0, 1), repeat=3) if v != (0, 0, 0)]
@@ -52,6 +52,23 @@ def stencil(theta):
     return np.stack([axis_angle_matrix(theta * np.asarray(v, dtype=np.float64)) for v in _OFFSETS])
 
 
+def grid_constants(template_poses, steps):
+    """The grid constants of a refiner over template_poses [N >= 2, 3, 3] with `steps` (checked) steps: ->
+    (template_poses float64 on the host, theta0 = half the grid's median nearest-neighbour geodesic angle, thetas =
+    theta0 * 2^-s for each step s)."""
+    R = np.asarray(template_poses.cpu().numpy() if torch.is_tensor(template_poses) else template_poses,
+                   dtype=np.float64)
+    if R.ndim != 3 or R.shape[1:] != (3, 3) or R.shape[0] < 2:
+        raise ValueError(f"template_poses must be [N >= 2, 3, 3], got {tuple(R.shape)}")
+    theta0 = 0.5 * float(np.median(nearest_neighbour_angles(R)))
+    return torch.from_numpy(R.copy()), theta0, tuple(theta0 * 2.0 ** -s for s in range(steps))
+
+
+def identity_centres(rows, keep, device):
+    """The first step's centres D: the identity for each of a row's `keep` seeds, float32 [rows, keep, 9]"""
+    return torch.eye(3, device=device, dtype=torch.float32).reshape(1, 1, 9).expand(rows, keep, 9).contiguous()
+
+
 class PoseRefiner:
     """The per-step constants of a refinement over one pose grid.
 
@@ -61,17 +78,11 @@ class PoseRefiner:
     All computed once on the host in float64; device copies are made on first use."""
 
     def __init__(self, template_poses, steps=4):
-        R = np.asarray(template_poses.cpu().numpy() if torch.is_tensor(template_poses) else template_poses,
-                       dtype=np.float64)
-        if R.ndim != 3 or R.shape[1:] != (3, 3) or R.shape[0] < 2:
-            raise ValueError(f"template_poses must be [N >= 2, 3, 3], got {tuple(R.shape)}")
         if int(steps) != steps or steps < 1:
             raise ValueError(f"steps must be a positive integer, got {steps}")
         self.steps = int(steps)
-        self.num_poses = int(R.shape[0])
-        self.template_poses = torch.from_numpy(R.copy())
-        self.theta0 = 0.5 * float(np.median(nearest_neighbour_angles(R)))
-        self.thetas = tuple(self.theta0 * 2.0 ** -s for s in range(self.steps))
+        self.template_poses, self.theta0, self.thetas = grid_constants(template_poses, self.steps)
+        self.num_poses = int(self.template_poses.shape[0])
         self.stencils = torch.from_numpy(np.stack([stencil(t).reshape(STENCIL, 9) for t in self.thetas])
                                          .astype(np.float32))
         self.thresholds = tuple(float(np.float32(1.0 + 2.0 * np.cos(t / 2.0))) for t in self.thetas)
@@ -158,19 +169,13 @@ def refine(engine, ref_feat, query_feat, all_relativeR, seed_idx, refiner, k=5):
     keep = int(seed_idx.shape[-1])
     check_refine_args(refiner, all_relativeR, keep, k, ref_feat.shape[0])
     dev = engine.device
-    ref_feat = ref_feat.to(dev, torch.float32).contiguous()
-    query_feat = query_feat.to(dev, torch.float32).contiguous()
-    Q, lead = query_rows(query_feat, ref_feat)
+    _, _, Q, lead, ref_rows, query_rows_ = row_pairs(dev, ref_feat, query_feat)
     if tuple(seed_idx.shape[:-1]) != lead:
         raise ValueError(f"seed_idx must be {lead + (keep,)} for these queries, got {tuple(seed_idx.shape)}")
-    B = ref_feat.shape[0]
-    rows = B * Q
+    rows = ref_rows.shape[0]
     rel = all_relativeR.to(dev, torch.float32).contiguous()
     stencils, _ = refiner._on(dev)
-    ref_rows = ref_feat[:, None].expand(B, Q, *ref_feat.shape[1:]).reshape(rows, *ref_feat.shape[1:])
-    query_rows_ = query_feat.reshape(rows, *ref_feat.shape[1:])
-    cur = {"D": torch.eye(3, device=dev, dtype=torch.float32).reshape(1, 1, 9).expand(rows, keep, 9).contiguous(),
-           "seed": seed_idx.to(dev).reshape(rows, keep).to(torch.int32)}
+    cur = {"D": identity_centres(rows, keep, dev), "seed": seed_idx.to(dev).reshape(rows, keep).to(torch.int32)}
     for s in range(refiner.steps):
         cand = propose(cur["D"], cur["seed"], rel, stencils[s], Q)
         sim = engine.sweep(ref_rows, cand["poses"], query_feat=query_rows_, want_emb=False, want_sim=True,

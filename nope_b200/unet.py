@@ -10,6 +10,7 @@ import ctypes as C
 import torch
 
 from . import _lib
+from .search import _METRICS, query_rows
 
 # precision option of the engine (include/nope_b200.h, nope_unet_set_option)
 PRECISIONS = {"fp16": 0, "fp16_w2": 1, "parity": 2, "bf16": 3, "parity_fast": 4}
@@ -194,7 +195,6 @@ class UNet:
     def set_metric(self, metric, threshold=0.2):
         """Similarity metric of the scoring fused onto the sweep: 'l2' (the reference's, model.py:254-266),
         'cosine' or 'cosine_occlusion' (extensions; include/nope_b200.h NOPE_METRIC_*)."""
-        from .model import _METRICS
         _lib.check(_lib.load().nope_unet_set_metric(self._handle(), _METRICS[metric], float(threshold)))
 
     def set_conv_impl(self, impl):
@@ -249,31 +249,9 @@ class UNet:
             raise _lib.NopeError("load_state_dict() must be called before the sweep")
         lib = _lib.load()
         dev = self.device
-        ref_feat = ref_feat.to(dev, torch.float32).contiguous()
-        poses = poses.to(dev, torch.float32).contiguous()
+        ref_feat, poses, query_feat, Q, emb, sim, topv, topi = stage_sweep(self, ref_feat, poses, query_feat,
+                                                                           want_emb, want_sim, k, out)
         B, N = poses.shape[0], poses.shape[1]
-        assert ref_feat.shape == (B, self.channels, 32, 32), ref_feat.shape
-        assert poses.shape[2] == self.rot_representation_dim
-        if want_sim is None:
-            want_sim = query_feat is not None
-        Q, lead = 1, (B,)
-        if query_feat is not None:
-            query_feat = query_feat.to(dev, torch.float32).contiguous()
-            Q, lead = query_rows(query_feat, ref_feat)
-        emb = torch.empty((B, N, self.channels, 32, 32), device=dev, dtype=torch.float32) \
-            if want_emb else None
-        out = out or {}
-        sim = out.get("sim") if want_sim else None
-        if want_sim and sim is None:
-            sim = torch.empty(lead + (N,), device=dev, dtype=torch.float32)
-        topv, topi = (out.get("topv"), out.get("topi")) if k > 0 else (None, None)
-        if k > 0 and topv is None:
-            topv = torch.empty(lead + (k,), device=dev, dtype=torch.float32)
-            topi = torch.empty(lead + (k,), device=dev, dtype=torch.int64)
-        for t, shape, dt in ((sim, lead + (N,), torch.float32), (topv, lead + (k,), torch.float32),
-                             (topi, lead + (k,), torch.int64)):
-            if t is not None:
-                assert t.is_contiguous() and tuple(t.shape) == shape and t.dtype == dt and t.device == dev
         self.reserve(min(self._chunk, B * N), B, B * Q * N if query_feat is not None else 0)
         stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
@@ -309,14 +287,34 @@ class UNet:
         return out[: N * c.value * s.value * s.value].view(N, c.value, s.value, s.value)
 
 
-def query_rows(query_feat, ref_feat):
-    """(Q, leading output shape) of a sweep's queries: [B,C,h,w] is one query per reference (outputs [B, ...]),
-    [B,Q,C,h,w] Q queries per reference (outputs [B,Q, ...])."""
-    B, rest = ref_feat.shape[0], tuple(ref_feat.shape[1:])
-    if query_feat.dim() == ref_feat.dim() and tuple(query_feat.shape) == (B,) + rest:
-        return 1, (B,)
-    if query_feat.dim() == ref_feat.dim() + 1 and query_feat.shape[0] == B and \
-            tuple(query_feat.shape[2:]) == rest and query_feat.shape[1] >= 1:
-        return int(query_feat.shape[1]), (B, int(query_feat.shape[1]))
-    raise ValueError(f"query_feat must be [B, ...] or [B, Q, ...] with the reference's per-image shape "
-                     f"{(B,) + rest}; got {tuple(query_feat.shape)}")
+def stage_sweep(engine, ref_feat, poses, query_feat, want_emb, want_sim, k, out):
+    """The tensors of one sweep by `engine` (UNet or UNetModelPose): the inputs as contiguous float32 on its device,
+    and the outputs, allocated or taken from `out` (preallocated `sim` / `topv` / `topi`, ValueError unless each has
+    the output's shape and dtype, on the device, contiguous).  want_sim None means: when there are queries.
+    -> (ref_feat, poses, query_feat | None, Q, emb | None, sim | None, topv | None, topi | None)"""
+    dev = engine.device
+    ref_feat = ref_feat.to(dev, torch.float32).contiguous()
+    poses = poses.to(dev, torch.float32).contiguous()
+    B, N = poses.shape[0], poses.shape[1]
+    assert ref_feat.shape == (B, engine.channels, 32, 32), ref_feat.shape
+    assert poses.shape[2] == engine.rot_representation_dim
+    if want_sim is None:
+        want_sim = query_feat is not None
+    Q, lead = 1, (B,)
+    if query_feat is not None:
+        query_feat = query_feat.to(dev, torch.float32).contiguous()
+        Q, lead = query_rows(query_feat, ref_feat)
+    emb = torch.empty((B, N, engine.channels, 32, 32), device=dev, dtype=torch.float32) if want_emb else None
+    out = out or {}
+    sim = out.get("sim") if want_sim else None
+    if want_sim and sim is None:
+        sim = torch.empty(lead + (N,), device=dev, dtype=torch.float32)
+    topv, topi = (out.get("topv"), out.get("topi")) if k > 0 else (None, None)
+    if k > 0 and topv is None:
+        topv = torch.empty(lead + (k,), device=dev, dtype=torch.float32)
+        topi = torch.empty(lead + (k,), device=dev, dtype=torch.int64)
+    for t, shape, dt in ((sim, lead + (N,), torch.float32), (topv, lead + (k,), torch.float32),
+                         (topi, lead + (k,), torch.int64)):
+        if t is not None and (tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous() or t.device != dev):
+            raise ValueError("preallocated output has the wrong shape / dtype / device or is not contiguous")
+    return ref_feat, poses, query_feat, Q, emb, sim, topv, topi

@@ -98,8 +98,10 @@ def test_score_topk_batch_mismatch_raises_before_touching_a_device():
 
 
 def test_query_forms():
-    from nope_b200.model import multi_query_form
-    from nope_b200.unet import query_rows
+    import types
+    from nope_b200.ldm import UNetModelPose
+    from nope_b200.model import PoseConditional
+    from nope_b200.search import multi_query_form, query_rows
     ref = torch.zeros(2, 3, 8, 8)
     q, sq = multi_query_form(torch.zeros(2, 3, 8, 8), ref)          # one query per reference
     assert q.shape == (2, 3, 8, 8) and not sq
@@ -107,10 +109,16 @@ def test_query_forms():
     assert q.shape == (2, 5, 3, 8, 8) and not sq
     q, sq = multi_query_form(torch.zeros(7, 3, 8, 8), ref[:1])      # broadcast form: one reference
     assert q.shape == (1, 7, 3, 8, 8) and sq
+    # the grid search of both front ends refuses these forms before any encoder call or sweep
+    model = PoseConditional(types.SimpleNamespace(device=torch.device("cpu")))
+    ldm = UNetModelPose(device="cpu")
+    rel, tp = torch.zeros(2, 6, 6), torch.zeros(6, 3, 3)
     for bad, r in ((torch.zeros(3, 3, 8, 8), ref), (torch.zeros(2, 0, 3, 8, 8), ref),
                    (torch.zeros(1, 5, 3, 8, 8), ref), (torch.zeros(2, 5, 4, 8, 8), ref)):
-        with pytest.raises(ValueError):
-            multi_query_form(bad, r)
+        for search in (multi_query_form, lambda q, r: model.predict_pose(q, r, rel, tp),
+                       lambda q, r: ldm.predict_pose(q, r, rel, tp)):
+            with pytest.raises(ValueError):
+                search(bad, r)
     f = torch.zeros(2, 8, 32, 32)
     assert query_rows(torch.zeros(2, 8, 32, 32), f) == (1, (2,))
     assert query_rows(torch.zeros(2, 4, 8, 32, 32), f) == (4, (2, 4))

@@ -209,6 +209,17 @@ def test_ldm_multi_query_fused_scores_match_standalone(golden_dir):
     tp = torch.eye(3).expand(642, 3, 3).contiguous()
     R, idx, sim = m.predict_pose(qry[0], ref, poses, tp, k=5)
     assert R.shape == (4, 5, 3, 3) and idx.shape == (4, 5) and sim.shape == (4, 642)
+    # as in PoseConditional.predict_pose: k > N is clamped to N, and template_poses [B, N, 3, 3] are read at row 0
+    R4, idx4, sim4 = m.predict_pose(qry[0], ref, poses[:, :4], tp[:4], k=4)
+    R5, idx5, sim5 = m.predict_pose(qry[0], ref, poses[:, :4], tp[:4], k=5)
+    assert idx5.shape == (4, 4) and torch.equal(idx5, idx4) and torch.equal(sim5, sim4) and torch.equal(R5, R4)
+    refs = torch.cat([ref, torch.randn(1, 4, 32, 32, generator=gen)])
+    tp2 = torch.randn(2, 40, 3, 3, generator=gen)                           # a different grid per reference
+    R2, idx2, _ = m.predict_pose(qry[0, :2], refs, poses[:, :40].expand(2, 40, 6), tp2, k=5)
+    assert torch.equal(R2, tp2[0].cuda()[idx2]) and not torch.equal(R2[1], tp2[1].cuda()[idx2[1]])
+    # a preallocated output that does not fit is refused, as by UNet.sweep
+    with pytest.raises(ValueError):
+        m.sweep(ref, poses, qry, want_emb=False, k=5, out={"sim": torch.empty((1, 4, 641), device="cuda:0")})
     del m
 
 
@@ -243,4 +254,9 @@ def test_caller_workspace_sized_for_one_query(seeded_state_dict, golden_dir):
     _lib.check(run())
     ref = u.sweep(rf, poses, query_feat=qs, want_emb=False, k=5)
     assert torch.equal(ref["sim"], sim) and torch.equal(ref["topi"], topi)
+    # preallocated outputs that do not fit are refused with ValueError, as by UNetModelPose.sweep
+    for out in ({"sim": sim[:, :1]}, {"sim": sim.transpose(1, 2).contiguous().transpose(1, 2)},
+                {"topv": topv, "topi": topi.to(torch.int32)}):
+        with pytest.raises(ValueError):
+            u.sweep(rf, poses, query_feat=qs, want_emb=False, k=5, out=out)
     del m
