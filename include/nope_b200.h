@@ -427,6 +427,19 @@ int nope_score_topk(const float* query_feat, const float* emb, int B, int N, int
 int nope_score_topk_multi(const float* query_feat, const float* emb, int B, int Q, int Bt, int N, int C, int HW,
                           int metric, float occlusion_threshold, int k, float* out_sim, float* out_topv,
                           int64_t* out_topi, int64_t idx_base, void* stream);
+/* The same scoring against a template bank (DESIGN.md section 25), rows grouped by template set:
+ *   query_feat [R, C, HW] fp32, emb [O, N, C, HW] fp32, slots [G] and row_off [G + 1] int32 (device): group g's rows
+ *   [row_off[g], row_off[g + 1]) are scored against template set slots[g] -> sim [R, N].  Per pair, the arithmetic
+ *   and summation order of nope_score_topk_multi, so every row's scores are bit-identical to that call's.
+ *   With k > 0, also the joint top-k over (a, n) of every A consecutive rows -> topv/topi [R / A, k], indices a * N + n,
+ *   in the order of nope_topk.
+ * Refuses null pointers, G outside [1, 65535], R not a multiple of A, k outside [0, min(64, A * N)], O > 65535,
+ * R * N > INT32_MAX and an unknown metric, all before any CUDA call.  The contents of slots and row_off are not
+ * checked (they are device data): 0 <= slots[g] < O and 0 <= row_off[0] <= ... <= row_off[G] <= R are the caller's. */
+int nope_score_topk_grouped(const float* query_feat, const float* emb, int R, int O, int N, int C, int HW,
+                            const int32_t* slots, const int32_t* row_off, int G, int A, int metric,
+                            float occlusion_threshold, int k, float* out_sim, float* out_topv, int64_t* out_topi,
+                            void* stream);
 
 /* Rank an existing similarity matrix sim [B, N] (used to merge per-GPU shards): top-k per row, descending score,
  * ties (+0 == -0, inf == inf) -> lowest index, NaN after every number and NaNs by index.  Every ranking call below

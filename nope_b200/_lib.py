@@ -91,6 +91,9 @@ SIGNATURES = {
     "nope_score_topk_multi": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                         C.c_int, C.c_float, C.c_int, c_f32p, c_f32p, c_i64p, C.c_int64,
                                         C.c_void_p]),
+    "nope_score_topk_grouped": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                          C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, c_f32p, c_f32p,
+                                          c_i64p, C.c_void_p]),
     "nope_unet_set_metric": (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
     "nope_topk": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_distinct_topk": (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

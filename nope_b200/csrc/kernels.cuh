@@ -626,14 +626,21 @@ final_conv_score_kernel(const __half* __restrict__ x, const float* __restrict__ 
 // metric 0: reference "l2"; 1: cosine over the flattened descriptor; 2: occlusion-aware cosine (extensions).
 // One CTA per template (b, n) loops over its query rows: the template is read from DRAM once, and every row's
 // sum runs in the same order whatever the number of rows.
+// Grouped form (a template bank, DESIGN.md section 25): with slots [G] and row_off [G + 1] (device, both non-null),
+// blockIdx.y is a group g that reads template batch slots[g] and scores query rows [row_off[g], row_off[g + 1]);
+// `rows` is then unused.  With null pointers group b is template batch b and rows [b * rows, (b + 1) * rows).
 __global__ void __launch_bounds__(256)
 score_kernel(const float* __restrict__ query, const float* __restrict__ emb,
-             float* __restrict__ sim, int N, int Cl, int hw, int metric, float occ_thr, int rows = 1) {
+             float* __restrict__ sim, int N, int Cl, int hw, int metric, float occ_thr, int rows = 1,
+             const int* __restrict__ slots = nullptr, const int* __restrict__ row_off = nullptr) {
   __shared__ float s_a[2][8], s_b[2][8], s_c[2][8];     // double-buffered across rows
   const int n = blockIdx.x, b = blockIdx.y;
-  const float* e = emb + ((long long)b * N + n) * Cl * hw;
-  for (int j = 0; j < rows; ++j) {
-    const long long r = (long long)b * rows + j;
+  const long long tb = slots ? slots[b] : b;
+  const long long r0 = row_off ? row_off[b] : (long long)b * rows;
+  const int nrows = row_off ? row_off[b + 1] - row_off[b] : rows;
+  const float* e = emb + (tb * N + n) * Cl * hw;
+  for (int j = 0; j < nrows; ++j) {
+    const long long r = r0 + j;
     const float* q = query + r * Cl * hw;
     float a0 = 0.f, a1 = 0.f, a2 = 0.f;
     for (int p = threadIdx.x; p < hw; p += blockDim.x) {

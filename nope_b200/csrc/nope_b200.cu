@@ -1233,6 +1233,33 @@ int nope_score_topk_multi(const float* query_feat, const float* emb, int B, int 
   return 0;
 }
 
+int nope_score_topk_grouped(const float* query_feat, const float* emb, int R, int O, int N, int C, int HW,
+                            const int32_t* slots, const int32_t* row_off, int G, int A, int metric,
+                            float occlusion_threshold, int k, float* out_sim, float* out_topv, int64_t* out_topi,
+                            void* stream) {
+  NOPE_CHECK(query_feat && emb && slots && row_off && out_sim, "null argument");
+  NOPE_CHECK(R >= 1 && O >= 1 && N >= 1 && C >= 1 && HW >= 1, "bad arguments");
+  NOPE_CHECK(G >= 1 && G <= 65535, "G (row groups) must be in [1, 65535]");
+  NOPE_CHECK(A >= 1 && R % A == 0, "R (query rows) must be a multiple of A (rows per search row) >= 1");
+  NOPE_CHECK(O <= 65535 && (int64_t)R * N <= INT32_MAX, "too many templates or (query, template) pairs");
+  NOPE_CHECK(metric == NOPE_METRIC_L2 || metric == NOPE_METRIC_COSINE || metric == NOPE_METRIC_COSINE_OCC,
+             "unknown similarity metric (l2, cosine and cosine_occlusion exist)");
+  NOPE_CHECK(k >= 0 && k <= 64 && (int64_t)k <= (int64_t)A * N, "k must be in [0, min(64, A * N)]");
+  NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // one CTA per (template n, group g): slot slots[g]'s template n against the group's rows
+  score_kernel<<<dim3(N, G), 256, 0, st>>>(query_feat, emb, out_sim, N, C, HW, metric, occlusion_threshold, 0,
+                                           slots, row_off);
+  NOPE_CUDA(cudaGetLastError());
+  if (k > 0) {
+    // the joint top-k over (row a, template n) of every A consecutive rows: sim viewed as [R / A, A * N]
+    sim_topk_kernel<<<R / A, 256, 0, st>>>(nullptr, 0, out_sim, A * N, k, out_topv,
+                                           reinterpret_cast<long long*>(out_topi), 0LL);
+    NOPE_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
 int nope_score_topk(const float* query_feat, const float* emb, int B, int N, int C, int HW, int metric,
                     float occlusion_threshold, int k, float* out_sim, float* out_topv, int64_t* out_topi,
                     int64_t idx_base, void* stream) {

@@ -128,14 +128,16 @@ class PoseConditional:
 
     def _checked(self, query, reference, unsharded=None, check=None):
         """The refusals of a search, all before anything is encoded: model.dist for a search that runs on one device
-        (`unsharded`, its name), the search's own argument check check(), the similarity metric and the query form.
+        (`unsharded`, its name), the search's own argument check check(), the similarity metric and, given a reference
+        (a bank search has none), the query form.
         -> (metric, what check returned)"""
         if unsharded is not None and self.dist is not None:
             raise NotImplementedError(f"{unsharded} does not shard across GPUs: it runs on one device (unset "
                                       "model.dist or use predict_pose)")
         checked = None if check is None else check()
         metric = self._metric()
-        multi_query_form(query, reference)
+        if reference is not None:
+            multi_query_form(query, reference)
         return metric, checked
 
     def _encode(self, query, reference, metric):
@@ -295,6 +297,92 @@ class PoseConditional:
                                  self._occlusion_threshold())
         _, flat = topk(sim.view(rows, A * N), k)
         return sim.view(rows, A, N), flat % N, flat // N
+
+    # ------------------------------------------------------------------ template banks (DESIGN.md section 25)
+    @torch.no_grad()
+    def build_template_bank(self, obj_ids, reference, all_relativeR, template_poses):
+        """Sweep every object's reference once and keep its templates: obj_ids [O] (unique), reference [O, 3, 256,
+        256], all_relativeR [O, N, 6], template_poses [N, 3, 3] (one grid for every object).  One encoder call, then
+        one sweep (bank.TemplateBank.build).  -> TemplateBank on the model's device; bank.save / TemplateBank.load
+        keep it across processes.  The bank holds the templates generate_templates gives, bit for bit."""
+        from .bank import TemplateBank
+        if reference.dim() != 4 or reference.shape[0] != len(obj_ids):
+            raise ValueError(f"reference [O, 3, H, W] with O = {len(obj_ids)} obj_ids expected, got "
+                             f"{tuple(reference.shape)}")
+        if all_relativeR.dim() != 3 or all_relativeR.shape[0] != reference.shape[0]:
+            raise ValueError(f"all_relativeR [O, N, 6] with O = {reference.shape[0]} expected, got "
+                             f"{tuple(all_relativeR.shape)}")
+        if len(set(int(i) for i in obj_ids)) != len(obj_ids):
+            raise ValueError(f"duplicate obj_ids in {list(obj_ids)}")
+        if tuple(torch.as_tensor(template_poses).shape) != (all_relativeR.shape[1], 3, 3):
+            raise ValueError(f"template_poses [{all_relativeR.shape[1]}, 3, 3] expected (the grid of all_relativeR), "
+                             f"got {tuple(torch.as_tensor(template_poses).shape)}")
+        reference_feat = self.u_net.encoder.encode_image(reference.to(self.device), mode="mode")
+        return TemplateBank.build(self.u_net, reference_feat, obj_ids, all_relativeR, template_poses)
+
+    def _bank_query(self, name, query, obj_ids, bank, angles, k):
+        """the refusals of a bank search, before any device work (model.dist, the bank, the engine descriptor, the
+        ids, the in-plane arguments, the metric) -> (metric, A, k, the bank slot of every detection)"""
+        from .bank import check_bank_search
+        if query.dim() != 4 or query.shape[1] != 3:
+            raise ValueError(f"{name}: query [D, 3, H, W] (one crop per detection) expected, got {tuple(query.shape)}")
+        metric, (A, k, slots) = self._checked(
+            query, None, name, lambda: check_bank_search(bank, self.u_net, query.shape[0], obj_ids, angles, k))
+        return metric, A, k, slots
+
+    def _bank_scores(self, query, bank, slots, metric, A, k):
+        """the detections' crops grouped by slot, their A rotated copies encoded by one encode_image_inplane call and
+        scored against the bank by one nope_score_topk_grouped call.  -> (plan, query latents, sim [D, A, N], top
+        [D, k]), all in the plan's group order"""
+        from .bank import RowPlan, score_rows
+        plan = RowPlan(slots, A, bank.device)
+        images = plan.grouped(query.to(self.device))
+        lat = self.u_net.encoder.encode_image_inplane(images, A)
+        sim, top = score_rows(bank, lat, plan, metric, self._occlusion_threshold(), k)
+        return plan, lat, sim, top
+
+    @torch.no_grad()
+    def predict_pose_bank(self, query, obj_ids, bank, k=5, angles=36):
+        """predict_pose_inplane against a template bank: query [D, 3, 256, 256], one crop per detection, obj_ids [D]
+        (host) its objects, each held by `bank` (build_template_bank).  -> (R [D, k, 3, 3] = Rz(alpha[angle_idx])
+        template_poses[nearest_idx] (float64), nearest_idx [D, k], angle_idx [D, k], similarity [D, A, N]) in the
+        detections' order: what predict_pose_inplane returns for reference[slot], with each detection scored against
+        its object's stored templates (the arithmetic of retrieval_inplane) instead of a sweep.  Detections of one
+        object share each template read.  One encode_image_inplane call over all D crops, one scoring call, no host
+        synchronisation.  angles = 1 is the plain grid search.  Scores use the model's current metric."""
+        from .inplane import compose
+        metric, A, k, slots = self._bank_query("predict_pose_bank", query, obj_ids, bank, angles, k)
+        plan, _, sim, top = self._bank_scores(query, bank, slots, metric, A, k)
+        sim, top = plan.restore(sim), plan.restore(top)
+        N = bank.num_poses
+        nearest, angle = top % N, top // N
+        return compose(bank.template_poses, nearest, angle, A), nearest, angle, sim
+
+    @torch.no_grad()
+    def predict_pose_bank_refined(self, query, obj_ids, bank, refiner, k=5, keep=2):
+        """predict_pose_inplane_refined against a template bank: the bank search over the refiner's angles seeds each
+        detection with its joint top-`keep` (angle, pose) pairs, and refine_inplane continues from them with the
+        detection's reference_latents[slot] and all_relativeR[slot].  refiner: an InplaneRefiner over the bank's grid.
+        -> (R [D, k, 3, 3], seed [D, k], alpha_deg [D, k], score [D, k]) as predict_pose_inplane_refined returns."""
+        from .inplane_refine import (InplaneRefiner, check_inplane_refine_args, pose_rotations, refine_inplane,
+                                     roll_degrees)
+        if not isinstance(refiner, InplaneRefiner):
+            raise ValueError("refiner must be a nope_b200.inplane_refine.InplaneRefiner")
+        metric, A, _, slots = self._bank_query("predict_pose_bank_refined", query, obj_ids, bank, refiner.angles,
+                                               keep)
+        check_inplane_refine_args(refiner, bank.all_relativeR, keep, k)
+        bank.check_grid(refiner.template_poses)
+        plan, lat, _, top = self._bank_scores(query, bank, slots, metric, A, keep)
+        N = bank.num_poses
+        pose_idx, angle_idx = top % N, top // N
+        seed_lat = lat[torch.arange(plan.D, device=top.device)[:, None], angle_idx]     # [D, keep, C, h, w]
+        pose_idx, angle_idx, seed_lat = plan.restore(pose_idx), plan.restore(angle_idx), plan.restore(seed_lat)
+        ref_feat = bank.reference_latents.index_select(0, plan.det_slots)
+        rel = bank.all_relativeR.index_select(0, plan.det_slots)
+        out = refine_inplane(self.u_net, self.u_net.encoder, ref_feat, query.to(self.device), rel,
+                             (pose_idx, angle_idx), seed_lat, refiner, k=k)
+        R = pose_rotations(out["D"], out["seed"], out["cossin"], refiner)
+        return R, out["seed"], roll_degrees(out["cossin"]), out["score"]
 
     # ------------------------------------------------------------------ model.py:185-191, 268-376, 550-565
     def log(self, name, value, **kwargs):
@@ -634,8 +722,8 @@ class PoseConditional:
         return self._rerank(iou, R_out, t_out) if rerank else (R_out, t_out, iou)
 
     @torch.no_grad()
-    def predict_pose_frames(self, frames, masks, K, obj_ids, reference, all_relativeR, template_poses, angles=36, k=5,
-                            refiner=None, refine=None, frame_idx=None, occluders=None):
+    def predict_pose_frames(self, frames, masks, K, obj_ids, reference=None, all_relativeR=None, template_poses=None,
+                            angles=36, k=5, refiner=None, refine=None, frame_idx=None, occluders=None, bank=None):
         """6D poses of B detections in camera frames (DESIGN.md section 23): `crop.frame_crops` cuts a keep_inplane
         crop around each mask's `initial_translation` t0, the in-plane search (`predict_pose_inplane`, or
         `predict_pose_inplane_refined` with a refiner) finds the rotation in the crop's camera, `crop.to_camera`
@@ -652,6 +740,10 @@ class PoseConditional:
                      "detections": each detection's occluders are the other detections of its frame
                      (`crop.detection_occluders`).  The translation fit and the contour refinement then ignore those
                      pixels (DESIGN.md section 24); None is the plain fits, bit for bit.
+          bank       a TemplateBank (build_template_bank) holding every obj_id, in place of reference, all_relativeR
+                     and template_poses: the search is then predict_pose_bank (predict_pose_bank_refined with a
+                     refiner), which scores each crop against its object's stored templates instead of sweeping the
+                     reference (DESIGN.md section 25).  Give either the bank or reference and all_relativeR.
         -> {"R": float64 [B, k, 3, 3] in the real camera, "t": float64 [B, k, 3] mm, "score": the search's [B, k],
         "iou": the silhouette IoU [B, k], "R_crop": the search's rotations [B, k, 3, 3], "t0": [B, 3],
         "crops": [B, 3, 256, 256]}.  R and t go unchanged into eval_bop(R_est=, t_est=), refine_depth and
@@ -672,12 +764,28 @@ class PoseConditional:
         if missing:
             raise ValueError(f"predict_pose_frames: no mesh or models_info entry for obj_id {missing} (load_mesh, "
                              "load_models_info)")
-        if reference.shape[0] not in (1, B):
+        if bank is not None:
+            if reference is not None or all_relativeR is not None or template_poses is not None:
+                raise ValueError("predict_pose_frames: give either a bank or reference, all_relativeR and "
+                                 "template_poses, not both")
+            from .bank import check_bank_search
+            # the bank, the engine and the ids before the crops; the search checks its own k / keep again
+            check_bank_search(bank, self.u_net, B, ids, getattr(refiner, "angles", angles), 1)
+        elif reference is None or all_relativeR is None:
+            raise ValueError("predict_pose_frames: reference and all_relativeR (with template_poses), or a bank, "
+                             "expected")
+        elif reference.shape[0] not in (1, B):
             raise ValueError(f"predict_pose_frames: reference [1 | B, 3, 256, 256] with B = {B} expected, got "
                              f"{tuple(reference.shape)}")
         diameter = np.array([self.bop_models[i]["diameter"] for i in ids], dtype=np.float64)
         crops, t0, Rv, _ = frame_crops(frames, masks, K, diameter, image_size=256, frame_idx=frame_idx)
-        if refiner is None:
+        if bank is not None and refiner is None:
+            R_crop, nearest, angle, sim = self.predict_pose_bank(crops, ids, bank, k=k, angles=angles)
+            N = sim.shape[-1]
+            score = sim.reshape(B, -1).gather(1, angle * N + nearest)
+        elif bank is not None:
+            R_crop, _, _, score = self.predict_pose_bank_refined(crops, ids, bank, refiner, k=k)
+        elif refiner is None:
             R_crop, nearest, angle, sim = self.predict_pose_inplane(crops, reference, all_relativeR, template_poses,
                                                                     k=k, angles=angles)
             N = sim.shape[-1]
