@@ -23,6 +23,10 @@
 #include "common.cuh"
 #include <cudaTypedefs.h>
 
+#include <cstring>
+#include <map>
+#include <tuple>
+
 namespace nope {
 
 constexpr int kBM = 128;         // pixels per tile (UMMA M)
@@ -539,5 +543,111 @@ inline int pick_bn(int n_total) {
 inline bool conv_needs_extras(const ConvParams& p) {
   return p.relu || p.res_hi || p.out_lo || p.out_f32;
 }
+
+// Tensor maps of activation buffers, encoded once per (base, image capacity, lattice, C, H, W).  lattice < 0: the
+// plain NHWC map of geometry g (make_act_map); 0..3: the stride-2 sub-lattice (lattice >> 1, lattice & 1) of a
+// 2H x 2W tensor seen from g (make_unshuffle_map).  Call clear() whenever the buffers are reallocated.
+class TmapCache {
+ public:
+  int get(const CUtensorMap** out, const void* base, int cap_img, int C, const TileGeom& g, int lattice) {
+    const auto key = std::make_tuple(base, cap_img, lattice, C, g.H, g.W);
+    auto it = maps_.find(key);
+    if (it == maps_.end()) {
+      CUtensorMap m;
+      const int rc = lattice < 0 ? make_act_map(&m, base, cap_img, C, g)
+                                 : make_unshuffle_map(&m, base, cap_img, C, g, lattice >> 1, lattice & 1);
+      if (rc) return -1;
+      it = maps_.emplace(key, m).first;
+    }
+    *out = &it->second;
+    return 0;
+  }
+  void clear() { maps_.clear(); }
+
+ private:
+  std::map<std::tuple<const void*, int, int, int, int, int>, CUtensorMap> maps_;
+};
+
+// What a convolution layer of every engine holds.  K is the engine's GEMM depth (its weight layout decides whether
+// the W_lo columns are counted); each engine's layer adds its own extras.
+struct ConvLayerBase {
+  int cin = 0, cout = 0, K = 0, bn = 0;
+  __half* w = nullptr;     // packed fp16 weights, K-major
+  float* bias = nullptr;   // [cout] or nullptr
+  CUtensorMap wmap;        // weight box of bn rows
+};
+
+// One filter tap: activation lattice (0 for a plain map) and pixel offset.
+struct ConvTap {
+  int lat, dy, dx;
+};
+// Tap (oy, ox) of a stride-2 convolution seen from its output geometry: input pixel (2y + oy, 2x + ox) lies on the
+// stride-2 sub-lattice (oy & 1, ox & 1) at offset ((oy - (oy & 1)) / 2, (ox - (ox & 1)) / 2).  Pixel-unshuffle +
+// 1x1 is the case oy, ox in {0, 1}.
+inline ConvTap stride2_tap(int oy, int ox) {
+  const int p1 = oy & 1, p2 = ox & 1;
+  return ConvTap{p1 * 2 + p2, (oy - p1) / 2, (ox - p2) / 2};
+}
+
+// Builds the ConvParams of one launch.  The engine adds its activation maps and, in its accumulation order, the
+// K segments, then sets its epilogue fields around finish(), which fills everything that follows from the geometry,
+// the layer and the output.  A map that cannot be encoded or a segment past kMaxSeg is remembered and returned by
+// finish(), so no launch is made from a half-built block.
+struct ConvBuilder {
+  ConvParams p;
+  TmapCache& maps;
+  const TileGeom g;      // tile geometry: the output's, the source's for the folded upsample
+  const int cap_img;     // images the activation buffers hold
+  int err = 0;
+
+  ConvBuilder(TmapCache& m, const TileGeom& geom, int cap) : maps(m), g(geom), cap_img(cap) {
+    memset(&p, 0, sizeof p);
+  }
+  // appends the map of `base` (lattice as TmapCache::get) and returns its index
+  int map(const void* base, int C, int lattice = -1) {
+    const CUtensorMap* m = nullptr;
+    if (p.n_amaps >= kMaxAMaps) err = fail("conv: activation map table overflow");
+    else if (maps.get(&m, base, cap_img, C, g, lattice)) err = -1;
+    if (err) return 0;
+    p.amap[p.n_amaps] = *m;
+    return p.n_amaps++;
+  }
+  // appends a segment of nch 64-channel chunks (wcol1 as ConvSeg::wcol1)
+  void seg(int map, int dy, int dx, int nch, int wcol1 = 0) {
+    if (p.nseg >= kMaxSeg) {
+      err = fail("conv: segment table overflow");
+      return;
+    }
+    p.seg[p.nseg++] = ConvSeg{(int16_t)map, (int16_t)dy, (int16_t)dx, (int16_t)nch, wcol1};
+    p.ksteps += nch;
+  }
+  // n_par == 4: the folded upsample, whose output `out` (out_C channels) has 2H x 2W pixels and is stored through
+  // its four parity sub-lattices
+  int finish(const ConvLayerBase& L, const void* out, int out_C, int n_img, int n_par) {
+    if (err) return err;
+    for (int i = p.n_amaps; i < kMaxAMaps; ++i) p.amap[i] = p.amap[0];   // never read: any valid descriptor
+    p.bmap = L.wmap;
+    const CUtensorMap* m = nullptr;
+    for (int t = 0; t < 4; ++t) {   // n_par == 1: omap[0] is the store map, the others copies of it
+      if ((t == 0 || n_par == 4) && maps.get(&m, out, cap_img, out_C, g, n_par == 4 ? t : -1)) return -1;
+      p.omap[t] = *m;
+    }
+    p.bias = L.bias;
+    p.n_par = n_par;
+    p.src_w = g.W;
+    p.src_hw = g.H * g.W;
+    p.stats_hw = n_par * g.H * g.W;
+    p.stats_noct = L.cout / 8;
+    p.n_total = L.cout;
+    p.m_valid = n_img * g.H * g.W;     // rows of the GEMM (source pixels for the folded upsample)
+    p.m_tiles = geom_m_tiles(g, n_img);
+    p.n_tiles_par = L.cout / L.bn;
+    p.n_tiles = p.n_tiles_par * n_par;
+    p.tiles_per_img = g.tiles_per_img;
+    p.h_cnt = g.h_cnt;
+    p.b_cnt = g.b_cnt;
+    return 0;
+  }
+};
 
 }  // namespace nope

@@ -145,11 +145,9 @@ __global__ void enc_extract_kernel(const float* __restrict__ x, float* __restric
   }
 }
 
-struct EncConv {
-  int cin = 0, cout = 0, cout_real = 0, k = 1, stride = 1, K = 0, bn = 0;
-  __half* w = nullptr;   // [cout][taps][3][cin] fp16: (W_hi | W_lo | W_hi) per tap; fp16 mode [cout][taps][cin]
-  float* bias = nullptr;
-  CUtensorMap wmap;
+// w: [cout][taps][3][cin] fp16: (W_hi | W_lo | W_hi) per tap; fp16 mode [cout][taps][cin].  K: the packed row length.
+struct EncConv : ConvLayerBase {
+  int cout_real = 0, k = 1, stride = 1;
 };
 
 struct ActPair {
@@ -162,6 +160,25 @@ inline ActPair act_at(const ActPair& a, size_t o) { return ActPair{a.hi + o, a.l
 // the number of fp16 products per filter tap of a convolution: 3 in split precision (A_hi W_hi, A_hi W_lo,
 // A_lo W_hi), 1 in the single-fp16 mode
 inline int tap_products(int precision) { return precision == 0 ? 3 : 1; }
+
+// Weight w of one filter tap in the layout split_tap reads: dst[0] = W_hi = fp16(w); with 3 products also
+// dst[stride] = W_lo = fp16(w - W_hi) and dst[2 stride] = W_hi.
+inline void put_split_weight(__half* dst, int stride, int prods, float w) {
+  const __half hi = __float2half_rn(w);
+  dst[0] = hi;
+  if (prods == 1) return;
+  dst[stride] = __float2half_rn(w - __half2float(hi));
+  dst[2 * stride] = hi;
+}
+
+// The K segments of one filter tap over (W_hi | W_lo | W_hi) weight columns: A_hi W_hi, A_hi W_lo, A_lo W_hi from
+// the maps hi and lo; lo < 0 (single-fp16 mode): A_hi W_hi alone.
+inline void split_tap(ConvBuilder& b, int hi, int lo, int dy, int dx, int nch) {
+  b.seg(hi, dy, dx, nch);
+  if (lo < 0) return;
+  b.seg(hi, dy, dx, nch);
+  b.seg(lo, dy, dx, nch);
+}
 
 }  // namespace nope
 
@@ -178,7 +195,7 @@ struct nope_encoder {
   nope::ActPair buf[5];
   float* proj_out = nullptr;
   nope::DeviceAllocs ws_mem;          // workspace for cap images (ensure_workspace)
-  std::map<std::tuple<const void*, int, int, int, int>, CUtensorMap> tmaps;
+  nope::TmapCache tmaps;
   int64_t launches = 0;
   static constexpr int kChunk = 32;   // images per encode() call: the workspace holds this many
   float* rot_stage = nullptr;         // kChunk rotated 256x256 crops (25 MB), allocated by the first encode_inplane
@@ -239,16 +256,9 @@ struct nope_encoder {
     std::vector<__half> packed((size_t)L.cout * L.K, __float2half_rn(0.f));
     for (int o = 0; o < L.cout_real; ++o)
       for (int c = 0; c < L.cin; ++c)
-        for (int t = 0; t < taps; ++t) {
-          const float wf = (float)((double)W.data[((size_t)o * L.cin + c) * taps + t] * scale[o]);
-          const __half hi = __float2half_rn(wf);
-          const __half lo = __float2half_rn(wf - __half2float(hi));
-          __half* dst = &packed[(size_t)o * L.K + (size_t)t * prods * L.cin];
-          dst[c] = hi;
-          if (prods == 1) continue;
-          dst[L.cin + c] = lo;
-          dst[2 * L.cin + c] = hi;
-        }
+        for (int t = 0; t < taps; ++t)
+          put_split_weight(&packed[(size_t)o * L.K + (size_t)t * prods * L.cin + c], L.cin, prods,
+                           (float)((double)W.data[((size_t)o * L.cin + c) * taps + t] * scale[o]));
     std::vector<float> bias(L.cout, 0.f);
     for (int o = 0; o < L.cout_real; ++o) bias[o] = (float)shift[o];
     if (mem.upload(&L.w, packed) || mem.upload(&L.bias, bias)) return -1;
@@ -286,7 +296,7 @@ struct nope_encoder {
     return make_conv("projector.3", "projector.3.weight", "", 1);
   }
 
-  // ---------------------------------------------------------------- workspace / maps
+  // ---------------------------------------------------------------- workspace
   int ensure_workspace(int B) {
     if (B <= cap) return 0;
     NOPE_CUDA(cudaDeviceSynchronize());
@@ -298,20 +308,6 @@ struct nope_encoder {
       if (ws_mem.alloc(&b.hi, n) || (precision == 0 && ws_mem.alloc(&b.lo, n))) return -1;
     return ws_mem.alloc(&proj_out, (size_t)cap * 1024 * 64);
   }
-  int get_map(const CUtensorMap** out, const void* base, int C, const nope::TileGeom& g, int kind) {
-    using namespace nope;
-    auto key = std::make_tuple(base, kind + 1, C, g.H, g.W);
-    auto it = tmaps.find(key);
-    if (it == tmaps.end()) {
-      CUtensorMap m;
-      const int rc = kind < 0 ? make_act_map(&m, base, cap, C, g)
-                              : make_unshuffle_map(&m, base, cap, C, g, kind >> 1, kind & 1);
-      if (rc) return -1;
-      it = tmaps.emplace(key, m).first;
-    }
-    *out = &it->second;
-    return 0;
-  }
 
   // out = [relu](conv(in) + bias [+ res]); Hin = input side; returns output side in *Hout
   int conv(const nope::EncConv& L, const nope::ActPair& in, int Hin, const nope::ActPair& out, int n_img,
@@ -320,72 +316,22 @@ struct nope_encoder {
     const int Ho = Hin / L.stride;
     TileGeom g;
     if (make_geom(Ho, Ho, &g)) return -1;
-    ConvParams p;
-    memset(&p, 0, sizeof p);
-    const CUtensorMap* m = nullptr;
-    int nseg = 0, ksteps = 0;
-    const int nch = L.cin / 64;
-    const bool split = precision == 0;   // fp16 mode: the hi maps only, one segment per tap
-    if (L.stride == 1) {
-      if (get_map(&m, in.hi, L.cin, g, -1)) return -1;
-      p.amap[0] = *m;
-      if (split) {
-        if (get_map(&m, in.lo, L.cin, g, -1)) return -1;
-        p.amap[1] = *m;
-      }
-      p.n_amaps = split ? 2 : 1;
-    } else {
-      for (int t = 0; t < 4; ++t) {
-        if (get_map(&m, in.hi, L.cin, g, t)) return -1;
-        p.amap[t] = *m;
-        if (!split) continue;
-        if (get_map(&m, in.lo, L.cin, g, t)) return -1;
-        p.amap[4 + t] = *m;
-      }
-      p.n_amaps = split ? 8 : 4;
-    }
+    ConvBuilder b(tmaps, g, cap);
+    ConvParams& p = b.p;
+    // maps: hi then lo (fp16 mode: hi only), each as the four stride-2 lattices for a stride-2 convolution
+    const int n_lat = L.stride == 1 ? 1 : 4;
+    int mh[4] = {}, ml[4] = {-1, -1, -1, -1};
+    for (int t = 0; t < n_lat; ++t) mh[t] = b.map(in.hi, L.cin, L.stride == 1 ? -1 : t);
+    if (precision == 0)
+      for (int t = 0; t < n_lat; ++t) ml[t] = b.map(in.lo, L.cin, L.stride == 1 ? -1 : t);
     for (int ky = 0; ky < L.k; ++ky)
       for (int kx = 0; kx < L.k; ++kx) {
-        int mh, ml, dy, dx;
-        if (L.stride == 1) {
-          mh = 0; ml = 1;
-          dy = L.k == 3 ? ky - 1 : 0;
-          dx = L.k == 3 ? kx - 1 : 0;
-        } else {
-          // in(2y + ky - pad, 2x + kx - pad) on the stride-2 lattices: odd offsets live on lattice 1
-          const int oy = L.k == 3 ? ky - 1 : 0, ox = L.k == 3 ? kx - 1 : 0;
-          const int p1 = oy & 1, p2 = ox & 1;
-          dy = (oy - p1) / 2;
-          dx = (ox - p2) / 2;
-          mh = p1 * 2 + p2;
-          ml = 4 + mh;
-        }
-        p.seg[nseg++] = ConvSeg{(int16_t)mh, (int16_t)dy, (int16_t)dx, (int16_t)nch};   // A_hi W_hi
-        ksteps += nch;
-        if (!split) continue;
-        p.seg[nseg++] = ConvSeg{(int16_t)mh, (int16_t)dy, (int16_t)dx, (int16_t)nch};   // A_hi W_lo
-        p.seg[nseg++] = ConvSeg{(int16_t)ml, (int16_t)dy, (int16_t)dx, (int16_t)nch};   // A_lo W_hi
-        ksteps += 2 * nch;
+        const int oy = L.k == 3 ? ky - 1 : 0, ox = L.k == 3 ? kx - 1 : 0;
+        const ConvTap t = L.stride == 1 ? ConvTap{0, oy, ox} : stride2_tap(oy, ox);
+        split_tap(b, mh[t.lat], ml[t.lat], t.dy, t.dx, L.cin / 64);
       }
-    NOPE_CHECK(nseg <= kMaxSeg && ksteps * 64 == L.K, "encoder conv: segment table");
-    p.bmap = L.wmap;
-    if (get_map(&m, out.hi, L.cout, g, -1)) return -1;
-    for (int t = 0; t < 4; ++t) p.omap[t] = *m;
-    p.bias = L.bias;
-    p.stats = nullptr;
-    p.stats_hw = Ho * Ho;
-    p.stats_noct = L.cout / 8;
-    p.n_total = L.cout;
-    p.m_valid = n_img * Ho * Ho;
-    p.nseg = nseg;
-    p.ksteps = ksteps;
-    p.m_tiles = geom_m_tiles(g, n_img);
-    p.n_par = 1;
-    p.n_tiles_par = L.cout / L.bn;
-    p.n_tiles = p.n_tiles_par;
-    p.tiles_per_img = g.tiles_per_img;
-    p.h_cnt = g.h_cnt;
-    p.b_cnt = g.b_cnt;
+    if (b.finish(L, out.hi, L.cout, n_img, 1)) return -1;
+    NOPE_CHECK(p.ksteps * 64 == L.K, "encoder conv: segment table");
     p.relu = relu ? 1 : 0;
     p.res_hi = res ? res->hi : nullptr;
     p.res_lo = res ? res->lo : nullptr;

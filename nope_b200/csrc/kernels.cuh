@@ -1284,4 +1284,31 @@ inline int ew_grid(long long total, int threads = 256, int cap = 132 * 16) {
   return (int)g;
 }
 
+// Packs one convolution weight with pack_weight_kernel (row_stride, col_off, lo_off and bf16 as there).  src is fp32
+// [cout][cin][taps] in host or device memory; with fold_up it is a [cout][cin][3][3] kernel that fold_upconv_kernel
+// first folds into 4 cout rows of four taps.  src is staged in temporary device memory, freed once `st` has run the
+// packing.
+inline int pack_conv_weight(const float* src, __half* dst, int cout, int cin, int taps, bool fold_up, int row_stride,
+                            int col_off, int lo_off, int bf16, cudaStream_t st) {
+  const size_t n = (size_t)cout * cin * (fold_up ? 9 : taps);
+  const int rows = fold_up ? 4 * cout : cout;
+  float *tmp = nullptr, *folded = nullptr;
+  NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&tmp), n * sizeof(float)));
+  NOPE_CUDA(cudaMemcpyAsync(tmp, src, n * sizeof(float), cudaMemcpyDefault, st));
+  const float* w = tmp;
+  if (fold_up) {
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&folded), (size_t)rows * cin * taps * sizeof(float)));
+    fold_upconv_kernel<<<ew_grid((long long)4 * cout * cin), 256, 0, st>>>(tmp, folded, cout, cin);
+    NOPE_CUDA(cudaGetLastError());
+    w = folded;
+  }
+  pack_weight_kernel<<<ew_grid((long long)rows * cin * taps), 256, 0, st>>>(w, dst, rows, cin, taps, row_stride,
+                                                                            col_off, lo_off, bf16);
+  NOPE_CUDA(cudaGetLastError());
+  NOPE_CUDA(cudaStreamSynchronize(st));
+  NOPE_CUDA(cudaFree(tmp));
+  if (folded) NOPE_CUDA(cudaFree(folded));
+  return 0;
+}
+
 }  // namespace nope

@@ -35,16 +35,12 @@
 
 namespace nope {
 
-struct LdmConv {
+// w: [rows][kp(K)] fp16; bn: the tile width of the clustered kernel (up to 256)
+struct LdmConv : ConvLayerBase {
   int mode = 0;   // 0: 3x3 pad 1, 1: 1x1 / linear, 3: nearest-x2 + 3x3 (folded), 4: 3x3 stride 2 pad 1
-  int cin = 0, cout = 0, K = 0;
-  int bn = 0;              // tile width of the clustered kernel (up to 256)
   int skip_c = 0;          // channels of a folded 1x1 skip_connection / identity residual (extra K columns)
   int k_alg = 0;           // K without identity-residual columns (algorithmic FLOP count)
   bool geglu = false;      // rows permuted to (64 x | 64 gate) tiles; the epilogue emits x * gelu(gate)
-  __half* w = nullptr;     // [rows][K] fp16
-  float* bias = nullptr;
-  CUtensorMap wmap;        // weight box of bn rows
 };
 struct LdmNorm {
   float* gamma = nullptr;
@@ -106,7 +102,7 @@ struct nope_ldm {
   float* sim_buf = nullptr;
   size_t sim_buf_cap = 0;
   nope::DeviceAllocs ws_mem;                   // workspace for cap hypotheses, cap_ref references (ensure_workspace)
-  std::map<std::tuple<const void*, int, int, int, int>, CUtensorMap> tmaps;
+  nope::TmapCache tmaps;
   std::map<std::tuple<const void*, int, int, int>, CUtensorMap> tmaps3;
 
   // per-launch CUDA-event profile (bench.py roofline): kind 0 = convolution / GEMM, 1 = attention
@@ -271,28 +267,9 @@ struct nope_ldm {
   // dst[(row_off + o) * K + col_off + t * cin + c] = fp16(src[o][c][t])
   int pack_into(__half* dst, int K, int row_off, int col_off, const HostTensor& t, int cout, int cin, int taps,
                 bool fold_up = false) {
-    using namespace nope;
-    float *tmp = nullptr, *folded = nullptr;
-    const size_t n = t.data.size();
-    NOPE_CHECK(n == (size_t)cout * cin * (fold_up ? 9 : taps), "pack_into: size mismatch");
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&tmp), n * sizeof(float)));
-    NOPE_CUDA(cudaMemcpy(tmp, t.data.data(), n * sizeof(float), cudaMemcpyHostToDevice));
-    const float* src = tmp;
-    int rows = cout;
-    if (fold_up) {
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&folded), (size_t)4 * cout * cin * 4 * sizeof(float)));
-      fold_upconv_kernel<<<ew_grid((long long)4 * cout * cin), 256>>>(tmp, folded, cout, cin);
-      NOPE_CUDA(cudaGetLastError());
-      src = folded;
-      rows = 4 * cout;
-    }
-    pack_weight_kernel<<<ew_grid((long long)rows * cin * taps), 256>>>(
-        src, dst + (size_t)row_off * kp(K), rows, cin, taps, kp(K), col_off, precision ? K : 0);
-    NOPE_CUDA(cudaGetLastError());
-    NOPE_CUDA(cudaDeviceSynchronize());
-    NOPE_CUDA(cudaFree(tmp));
-    if (folded) NOPE_CUDA(cudaFree(folded));
-    return 0;
+    NOPE_CHECK(t.data.size() == (size_t)cout * cin * (fold_up ? 9 : taps), "pack_into: size mismatch");
+    return nope::pack_conv_weight(t.data.data(), dst + (size_t)row_off * kp(K), cout, cin, taps, fold_up, kp(K),
+                                  col_off, precision ? K : 0, 0, 0);
   }
   int finish_conv(const std::string& name, nope::LdmConv& L, int rows, const std::vector<float>& bias) {
     using namespace nope;
@@ -561,22 +538,6 @@ struct nope_ldm {
     return 0;
   }
 
-  // ------------------------------------------------------------------ tensor maps
-  int get_map(const CUtensorMap** out, const void* base, int C, const nope::TileGeom& g, int kind) {
-    using namespace nope;
-    auto key = std::make_tuple(base, kind + 1, C, g.H, g.W);
-    auto it = tmaps.find(key);
-    if (it == tmaps.end()) {
-      CUtensorMap m;
-      const int rc = kind < 0 ? make_act_map(&m, base, cap, C, g)
-                              : make_unshuffle_map(&m, base, cap, C, g, kind >> 1, kind & 1);
-      if (rc) return -1;
-      it = tmaps.emplace(key, m).first;
-    }
-    *out = &it->second;
-    return 0;
-  }
-
   // ------------------------------------------------------------------ op launchers
   // out[n_img, So, So, cout] = conv(L, in) [+ 1x1 skip or identity residual over cat(sk0, sk1)] + bias
   int conv(const nope::LdmConv& L, const __half* in, __half* out, int So, int n_img, cudaStream_t st,
@@ -584,103 +545,48 @@ struct nope_ldm {
            const __half* sk1 = nullptr, int skc1 = 0, float* out_f32 = nullptr) {
     using namespace nope;
     NOPE_CHECK(skc0 + skc1 == L.skip_c, "conv: skip channel mismatch");
+    NOPE_CHECK(!L.skip_c || ((L.mode == 0 || L.mode == 1) && sk0 && skc0 % 64 == 0 && skc1 % 64 == 0),
+               "conv: bad skip sources");
+    NOPE_CHECK(!(stats && L.mode == 3), "upsample conv has no fused statistics");
     ++launches;
     TileGeom g;
     if (make_geom(L.mode == 3 ? So / 2 : So, L.mode == 3 ? So / 2 : So, &g)) return -1;
-    ConvParams p;
-    memset(&p, 0, sizeof p);
-    const CUtensorMap* m = nullptr;
-    int nseg = 0, ksteps = 0, nmaps = 0;
+    ConvBuilder b(tmaps, g, cap);
+    ConvParams& p = b.p;
     const int nch = L.cin / 64;
-    p.n_par = 1;
-    if (L.mode == 3) {
-      if (get_map(&m, in, L.cin, g, -1)) return -1;
-      p.amap[nmaps++] = *m;
-      for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b) {
-          p.seg[nseg++] = ConvSeg{0, (int16_t)(a - 1), (int16_t)(b - 1), (int16_t)nch};
-          ksteps += nch;
-        }
-      p.n_par = 4;
-    } else if (L.mode == 4) {
+    if (L.mode == 4) {
       // in(2y + ky - 1, 2x + kx - 1) on the four stride-2 lattices of the 2So x 2So input
-      for (int t = 0; t < 4; ++t) {
-        if (get_map(&m, in, L.cin, g, t)) return -1;
-        p.amap[nmaps++] = *m;
-      }
+      int m[4];
+      for (int t = 0; t < 4; ++t) m[t] = b.map(in, L.cin, t);
       for (int ky = 0; ky < 3; ++ky)
         for (int kx = 0; kx < 3; ++kx) {
-          const int oy = ky - 1, ox = kx - 1;
-          const int p1 = oy & 1, p2 = ox & 1;
-          p.seg[nseg++] = ConvSeg{(int16_t)(p1 * 2 + p2), (int16_t)((oy - p1) / 2), (int16_t)((ox - p2) / 2),
-                                  (int16_t)nch};
-          ksteps += nch;
+          const ConvTap t = stride2_tap(ky - 1, kx - 1);
+          b.seg(m[t.lat], t.dy, t.dx, nch);
         }
     } else {
-      if (get_map(&m, in, L.cin, g, -1)) return -1;
-      p.amap[nmaps++] = *m;
-      const int taps = L.mode == 0 ? 9 : 1;
-      for (int t = 0; t < taps; ++t) {
-        p.seg[nseg++] = ConvSeg{0, (int16_t)(L.mode == 0 ? t / 3 - 1 : 0), (int16_t)(L.mode == 0 ? t % 3 - 1 : 0),
-                                (int16_t)nch};
-        ksteps += nch;
+      const int m = b.map(in, L.cin);
+      if (L.mode == 3) {
+        for (int a = 0; a < 2; ++a)
+          for (int c = 0; c < 2; ++c) b.seg(m, a - 1, c - 1, nch);
+      } else {
+        const int taps = L.mode == 0 ? 9 : 1;
+        for (int t = 0; t < taps; ++t) b.seg(m, L.mode == 0 ? t / 3 - 1 : 0, L.mode == 0 ? t % 3 - 1 : 0, nch);
       }
     }
     if (L.skip_c) {
-      NOPE_CHECK((L.mode == 0 || L.mode == 1) && sk0 && skc0 % 64 == 0 && skc1 % 64 == 0, "conv: bad skip sources");
-      if (get_map(&m, sk0, skc0, g, -1)) return -1;
-      p.amap[nmaps] = *m;
-      p.seg[nseg++] = ConvSeg{(int16_t)nmaps, 0, 0, (int16_t)(skc0 / 64)};
-      ksteps += skc0 / 64;
-      ++nmaps;
-      if (sk1) {
-        if (get_map(&m, sk1, skc1, g, -1)) return -1;
-        p.amap[nmaps] = *m;
-        p.seg[nseg++] = ConvSeg{(int16_t)nmaps, 0, 0, (int16_t)(skc1 / 64)};
-        ksteps += skc1 / 64;
-        ++nmaps;
-      }
+      b.seg(b.map(sk0, skc0), 0, 0, skc0 / 64);
+      if (sk1) b.seg(b.map(sk1, skc1), 0, 0, skc1 / 64);
     }
-    p.n_amaps = nmaps;
-    for (int t = nmaps; t < kMaxAMaps; ++t) p.amap[t] = p.amap[0];
-    p.bmap = L.wmap;
-    if (L.mode == 3) {
-      for (int t = 0; t < 4; ++t) {
-        if (get_map(&m, out, L.cout, g, t)) return -1;
-        p.omap[t] = *m;
-      }
-    } else {
-      if (get_map(&m, out, L.geglu ? L.cout / 2 : L.cout, g, -1)) return -1;
-      for (int t = 0; t < 4; ++t) p.omap[t] = *m;
+    NOPE_CHECK(p.ksteps * 64 == L.K, "conv: K mismatch");
+    // exact weights: the same segments again over the W_lo columns (weight columns simply continue past K)
+    for (int i = 0, n = precision ? p.nseg : 0; i < n; ++i) {
+      const ConvSeg s = p.seg[i];
+      b.seg(s.map, s.dy, s.dx, s.nchunks, s.wcol1);
     }
+    if (b.finish(L, out, L.geglu ? L.cout / 2 : L.cout, n_img, L.mode == 3 ? 4 : 1)) return -1;
     p.geglu = L.geglu ? 1 : 0;
-    p.bias = L.bias;
     p.out_f32 = out_f32;
     p.stats = stats;
-    p.stats_hw = So * So;
-    p.stats_noct = L.cout / 8;
-    p.n_total = L.cout;
-    p.m_valid = n_img * g.H * g.W;
-    p.nseg = nseg;
-    p.ksteps = ksteps;
-    p.m_tiles = geom_m_tiles(g, n_img);
-    p.n_tiles_par = L.cout / L.bn;
-    p.n_tiles = p.n_tiles_par * p.n_par;
-    p.tiles_per_img = g.tiles_per_img;
-    p.h_cnt = g.h_cnt;
-    p.b_cnt = g.b_cnt;
-    NOPE_CHECK(ksteps * 64 == L.K, "conv: K mismatch");
-    if (precision) {
-      // exact weights: the same segments again over the W_lo columns (weight columns simply continue past K)
-      NOPE_CHECK(2 * nseg <= kMaxSeg, "conv: segment table overflow");
-      for (int i = 0; i < nseg; ++i) p.seg[nseg + i] = p.seg[i];
-      nseg *= 2;
-      ksteps *= 2;
-    }
-    NOPE_CHECK(nseg <= kMaxSeg, "conv: segment table overflow");
-    p.nseg = nseg;
-    p.ksteps = ksteps;
-    NOPE_CHECK(!(stats && L.mode == 3), "upsample conv has no fused statistics");
     if (profile && prof_begin(st)) return -1;
     const int rc = launch_conv_tc2(p, L.bn, num_sms, st);
     // executed FLOPs (the folded upsample runs 4 parity GEMMs of K = 4 Cin over the source pixels)

@@ -45,14 +45,10 @@ namespace {
 constexpr int kAbiVersion = 2;
 constexpr int kHeadsHidden = 128;  // 4 heads x 32 (model_utils.py:368,394)
 
-struct ConvLayer {
+// w: [rows][Kp] fp16, K = cin x taps
+struct ConvLayer : ConvLayerBase {
   int mode = 0;  // 0: 3x3 pad1, 1: 1x1, 2: unshuffle+1x1, 3: nearest-x2 upsample + 3x3 (folded)
-  int cin = 0, cout = 0, K = 0, bn = 0;
   int Kp = 0;             // packed row length: K (fp16 weights) or 2K (W_hi | W_lo, precision >= 1)
-  __half* w = nullptr;    // [rows][Kp] fp16
-  float* bias = nullptr;  // [cout] fp32 or nullptr
-  CUtensorMap wmap;
-  bool has_map = false;
   // pre-norm folded into this (bias-free 1x1) layer: weights hold W diag(gamma); see GnFuse::pre_*
   float* pre_w1 = nullptr;
   float* pre_wb = nullptr;
@@ -143,7 +139,7 @@ struct nope_unet {
   float* score_partial = nullptr;
   float* sim_buf = nullptr;
 
-  std::map<std::tuple<const void*, int, int, int, int>, CUtensorMap> tmaps;
+  TmapCache tmaps;
 
   // per-launch CUDA-event profile of the convolution kernel (bench.py roofline)
   bool profile = false;
@@ -265,31 +261,14 @@ struct nope_unet {
     NOPE_CHECK(L.cin % 64 == 0, wkey + ": input channels must be a multiple of 64");
     L.bn = pick_bn(L.cout);
     NOPE_CHECK(L.bn != 0, wkey + ": output channels must be a multiple of 64");
-    float *tmp = nullptr, *folded = nullptr;
-    const size_t n = W.data.size();
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&tmp), n * sizeof(float)));
-    NOPE_CUDA(cudaMemcpy(tmp, W.data.data(), n * sizeof(float), cudaMemcpyHostToDevice));
-    const size_t npack = (size_t)rows * L.Kp;
-    const float* src = tmp;
-    if (mode == 3) {
-      NOPE_CHECK(sh.size() == 4 && sh[2] == 3 && sh[3] == 3, wkey + ": expected a 3x3 kernel");
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&folded), (size_t)rows * L.K * sizeof(float)));
-      fold_upconv_kernel<<<ew_grid((long long)4 * L.cout * L.cin), 256>>>(tmp, folded, L.cout, L.cin);
-      NOPE_CUDA(cudaGetLastError());
-      src = folded;
-    }
-    if (mem.alloc(&L.w, npack)) return -1;
-    pack_weight_kernel<<<ew_grid((long long)rows * L.K), 256>>>(src, L.w, rows, L.cin, taps, L.Kp, 0,
-                                                                wlo ? L.K : 0, bf() ? 1 : 0);
-    NOPE_CUDA(cudaGetLastError());
-    NOPE_CUDA(cudaDeviceSynchronize());
-    NOPE_CUDA(cudaFree(tmp));
-    if (folded) NOPE_CUDA(cudaFree(folded));
+    NOPE_CHECK(mode != 3 || (sh.size() == 4 && sh[2] == 3 && sh[3] == 3), wkey + ": expected a 3x3 kernel");
+    if (mem.alloc(&L.w, (size_t)rows * L.Kp)) return -1;
+    if (pack_conv_weight(W.data.data(), L.w, L.cout, L.cin, taps, mode == 3, L.Kp, 0, wlo ? L.K : 0, bf() ? 1 : 0, 0))
+      return -1;
     if (!bkey.empty()) {
       if (upload_f32(bkey, &L.bias)) return -1;
     }
     if (make_weight_map(&L.wmap, L.w, rows, L.Kp, L.bn)) return -1;
-    L.has_map = true;
     convs[name] = L;
     return 0;
   }
@@ -516,22 +495,6 @@ struct nope_unet {
     return 0;
   }
 
-  // ------------------------------------------------------------------ tensor maps
-  int get_map(const CUtensorMap** out, const void* base, int cap_img, int C, const TileGeom& g,
-              int kind /* -1: plain, 0..3: unshuffle (p1*2+p2) */) {
-    auto key = std::make_tuple(base, cap_img * 8 + (kind + 1), C, g.H, g.W);
-    auto it = tmaps.find(key);
-    if (it == tmaps.end()) {
-      CUtensorMap m;
-      int rc = kind < 0 ? make_act_map(&m, base, cap_img, C, g)
-                        : make_unshuffle_map(&m, base, cap_img, C, g, kind >> 1, kind & 1);
-      if (rc) return -1;
-      it = tmaps.emplace(key, m).first;
-    }
-    *out = &it->second;
-    return 0;
-  }
-
   // ------------------------------------------------------------------ op launchers
   // out[n_img, So, So, cout] = conv(L, in0 (++ in1)).  The K loop walks, per filter tap and source
   // tensor, up to three products: A_hi W_hi, A_hi W_lo (precision >= 1), A_lo W_hi (sources that
@@ -541,107 +504,53 @@ struct nope_unet {
            cudaStream_t st, const GnSpec* gs = nullptr, float2* stats = nullptr) {
     const int c0 = in0.C, c1 = in1.hi ? in1.C : 0;
     NOPE_CHECK(c0 + c1 == L.cin, "conv: channel mismatch");
+    NOPE_CHECK(L.mode != 3 || (in1.hi == nullptr && So % 2 == 0), "upsample conv takes one source");
+    NOPE_CHECK(L.mode != 2 || in1.hi == nullptr, "unshuffle conv takes one source");
     ++launches;
+    // the folded upsample's So is the OUTPUT side (2x the source side); tiles and input maps use the source geometry
+    const int Sg = L.mode == 3 ? So / 2 : So;
     TileGeom g;
-    if (make_geom(So, So, &g)) return -1;
-    ConvParams p;
-    memset(&p, 0, sizeof p);
-    const CUtensorMap* m = nullptr;
-    p.n_par = 1;
-    const bool wlo = L.Kp > L.K;                       // packed rows carry W_lo at column K + ...
-    const bool alo0 = in0.lo != nullptr, alo1 = in1.hi && in1.lo != nullptr;
-    // taps: (dy, dx, lattice) ; sources: (hi map, lo map, channels, weight column offset inside a tap)
-    struct Tap { int dy, dx, lat; };
-    std::vector<Tap> taps;
-    int n_lat = 1;
+    if (make_geom(Sg, Sg, &g)) return -1;
+    ConvBuilder b(tmaps, g, cap_img);
+    ConvParams& p = b.p;
+    ConvTap taps[9];
+    int n_taps = 0;
     if (L.mode == 3) {
-      // So is the OUTPUT side (2x the source side); tiles and input maps use the source geometry
-      NOPE_CHECK(in1.hi == nullptr && So % 2 == 0, "upsample conv takes one source");
-      if (make_geom(So / 2, So / 2, &g)) return -1;
       for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b) taps.push_back(Tap{a - 1, b - 1, 0});
-      p.n_par = 4;
+        for (int c = 0; c < 2; ++c) taps[n_taps++] = ConvTap{0, a - 1, c - 1};
     } else if (L.mode == 2) {
-      NOPE_CHECK(in1.hi == nullptr, "unshuffle conv takes one source");
-      for (int t = 0; t < 4; ++t) taps.push_back(Tap{0, 0, t});
-      n_lat = 4;
+      for (int t = 0; t < 4; ++t) taps[n_taps++] = stride2_tap(t >> 1, t & 1);
     } else if (L.mode == 0) {
-      for (int t = 0; t < 9; ++t) taps.push_back(Tap{t / 3 - 1, t % 3 - 1, 0});
+      for (int t = 0; t < 9; ++t) taps[n_taps++] = ConvTap{0, t / 3 - 1, t % 3 - 1};
     } else {
-      taps.push_back(Tap{0, 0, 0});
+      taps[n_taps++] = ConvTap{0, 0, 0};
     }
-    // activation maps: index = lattice + n_lat * (source + 2 * is_lo)
-    auto map_index = [&](int lat, int src, int lo) { return lat + n_lat * (src + 2 * lo); };
-    int max_map = 0;
-    bool map_set[kMaxAMaps] = {false};
-    for (int lat = 0; lat < n_lat; ++lat)
-      for (int src = 0; src < (in1.hi ? 2 : 1); ++src)
-        for (int lo = 0; lo < 2; ++lo) {
-          const Act& a = src ? in1 : in0;
-          const __half* base = lo ? a.lo : a.hi;
-          if (!base) continue;
-          // unshuffle with a remainder: 4 lattices x (hi, lo) of ONE source = maps 0..3, 4..7
-          const int idx = (n_lat == 4) ? lat + 4 * lo : map_index(lat, src, lo);
-          NOPE_CHECK(idx < kMaxAMaps, "conv: activation map table overflow");
-          if (get_map(&m, base, cap_img, a.C, g, L.mode == 2 ? lat : -1)) return -1;
-          p.amap[idx] = *m;
-          map_set[idx] = true;
-          max_map = std::max(max_map, idx);
-        }
-    p.n_amaps = max_map + 1;
-    for (int i = 1; i < p.n_amaps; ++i)      // unused slots: any valid descriptor (they are only prefetched)
-      if (!map_set[i]) p.amap[i] = p.amap[0];
-    int nseg = 0, ksteps = 0;
-    auto add_seg = [&](int map, const Tap& t, int nch, int wcol) {
-      p.seg[nseg++] = ConvSeg{(int16_t)map, (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch, wcol + 1};
-      ksteps += nch;
-    };
-    const int n_products = 1 + (wlo ? 1 : 0) + ((alo0 || alo1) ? 1 : 0);
-    NOPE_CHECK((int)taps.size() * (in1.hi ? 2 : 1) * n_products <= kMaxSeg, "conv: segment table overflow");
-    for (size_t ti = 0; ti < taps.size(); ++ti) {
-      const Tap& t = taps[ti];
-      const int wbase = (int)ti * L.cin;
-      const int mh0 = (n_lat == 4) ? t.lat : map_index(0, 0, 0);
-      const int ml0 = (n_lat == 4) ? t.lat + 4 : map_index(0, 0, 1);
-      // A_hi W_hi
-      add_seg(mh0, t, c0 / 64, wbase);
-      if (in1.hi) add_seg(map_index(0, 1, 0), t, c1 / 64, wbase + c0);
-      // A_hi W_lo
+    // activation maps: in0 (hi, lo) per lattice, in1 (hi, lo)
+    const int n_lat = L.mode == 2 ? 4 : 1;
+    int h0[4] = {}, l0[4] = {}, h1 = 0, l1 = 0;
+    for (int lat = 0; lat < n_lat; ++lat) h0[lat] = b.map(in0.hi, c0, L.mode == 2 ? lat : -1);
+    if (in1.hi) h1 = b.map(in1.hi, c1);
+    if (in0.lo)
+      for (int lat = 0; lat < n_lat; ++lat) l0[lat] = b.map(in0.lo, c0, L.mode == 2 ? lat : -1);
+    const bool alo1 = in1.hi && in1.lo;
+    if (alo1) l1 = b.map(in1.lo, c1);
+    // per filter tap and source: A_hi W_hi, A_hi W_lo (packed rows carry W_lo at column K + ...), A_lo W_hi
+    const bool wlo = L.Kp > L.K;
+    for (int ti = 0; ti < n_taps; ++ti) {
+      const ConvTap& t = taps[ti];
+      const int wcol = ti * L.cin + 1;      // ConvSeg::wcol1 of the tap's first source
+      b.seg(h0[t.lat], t.dy, t.dx, c0 / 64, wcol);
+      if (in1.hi) b.seg(h1, t.dy, t.dx, c1 / 64, wcol + c0);
       if (wlo) {
-        add_seg(mh0, t, c0 / 64, L.K + wbase);
-        if (in1.hi) add_seg(map_index(0, 1, 0), t, c1 / 64, L.K + wbase + c0);
+        b.seg(h0[t.lat], t.dy, t.dx, c0 / 64, L.K + wcol);
+        if (in1.hi) b.seg(h1, t.dy, t.dx, c1 / 64, L.K + wcol + c0);
       }
-      // A_lo W_hi
-      if (alo0) add_seg(ml0, t, c0 / 64, wbase);
-      if (alo1) add_seg(map_index(0, 1, 1), t, c1 / 64, wbase + c0);
+      if (in0.lo) b.seg(l0[t.lat], t.dy, t.dx, c0 / 64, wcol);
+      if (alo1) b.seg(l1, t.dy, t.dx, c1 / 64, wcol + c0);
     }
-    p.bmap = L.wmap;
+    if (b.finish(L, out.hi, L.cout, n_img, L.mode == 3 ? 4 : 1)) return -1;
     p.bf16 = bf() ? 1 : 0;
-    if (L.mode == 3) {
-      for (int t = 0; t < 4; ++t) {
-        if (get_map(&m, out.hi, cap_img, L.cout, g, t)) return -1;   // stride-2 sub-lattice (py, px)
-        p.omap[t] = *m;
-      }
-      p.src_w = g.W;
-      p.src_hw = g.H * g.W;
-    } else {
-      if (get_map(&m, out.hi, cap_img, L.cout, g, -1)) return -1;
-      for (int t = 0; t < 4; ++t) p.omap[t] = *m;
-    }
-    p.bias = L.bias;
     p.stats = stats;
-    p.stats_hw = So * So;
-    p.stats_noct = L.cout / 8;
-    p.n_total = L.cout;
-    p.m_valid = n_img * g.H * g.W;     // rows of the GEMM (source pixels for the folded upsample conv)
-    p.nseg = nseg;
-    p.ksteps = ksteps;
-    p.m_tiles = geom_m_tiles(g, n_img);
-    p.n_tiles_par = L.cout / L.bn;
-    p.n_tiles = p.n_tiles_par * p.n_par;
-    p.tiles_per_img = g.tiles_per_img;
-    p.h_cnt = g.h_cnt;
-    p.b_cnt = g.b_cnt;
     NOPE_CHECK(!(stats && L.mode == 3), "fused statistics are not available on the upsample conv");
     if (gs) {
       NOPE_CHECK(L.mode != 3 && !stats, "fused GroupNorm epilogue: no upsample, no plain statistics");
@@ -677,7 +586,8 @@ struct nope_unet {
       if (gs->res.hi) {
         NOPE_CHECK(gs->res.C == L.cout, "fused residual: channel mismatch");
         NOPE_CHECK(gs->res_div == 0 || g.tiles_per_img > 0, "residual image mapping needs >= 128-pixel images");
-        if (get_map(&m, gs->res.hi, gs->res_div > 0 ? cap_ref : cap_img, L.cout, g, -1)) return -1;
+        const CUtensorMap* m = nullptr;
+        if (tmaps.get(&m, gs->res.hi, gs->res_div > 0 ? cap_ref : cap_img, L.cout, g, -1)) return -1;
         p.rmap = *m;
         f.has_res = 1;
         f.res_lo = gs->res.lo;
@@ -723,7 +633,7 @@ struct nope_unet {
     prof_ev.push_back(e1);
     // executed FLOPs: mode 3 runs 4 parity GEMMs of K = 4 Cin over the source-resolution pixels;
     // the split-precision modes execute 2x / 3x the K-steps of the fp16 mode
-    prof_flops.push_back(2.0 * (double)n_img * So * So * (double)L.cout * (double)ksteps * 64.0);
+    prof_flops.push_back(2.0 * (double)n_img * So * So * (double)L.cout * (double)p.ksteps * 64.0);
     prof_alg.push_back(2.0 * (double)n_img * So * So * (double)L.cout * (double)L.K);
     prof_shape.push_back(make_int4(So, L.mode, L.cout, L.K));
     return rc;
@@ -2043,52 +1953,62 @@ int nope_crop_rotate(const double* Rv, int F, const double* R, int P, int to_cam
 // per-op entry points
 // ---------------------------------------------------------------------------------
 
+namespace {
+// What the per-op convolution entry points share: the argument checks, the inputs staged as NHWC fp16 (with their
+// fp16 remainders at precision 2), the output buffer, the packed layer, and a UNet engine on the current device to
+// launch through.
+struct OpConv {
+  Scratch s;
+  nope_unet eng;
+  ConvLayer L;
+  Act in0, in1, out;
+
+  int setup(int mode, int max_mode, int precision, const float* x0, int C0, const float* x1, int C1,
+            const float* weight, const float* bias, int n_img, int H, int W, int Cout, cudaStream_t st) {
+    NOPE_CHECK(x0 && weight, "null argument");
+    NOPE_CHECK(mode >= 0 && mode <= max_mode, "mode must be 0.." + std::to_string(max_mode));
+    NOPE_CHECK(H == W, "square images only");
+    NOPE_CHECK(C0 % 64 == 0 && C1 % 64 == 0 && Cout % 64 == 0, "channels must be multiples of 64");
+    const bool sp = precision == 2;
+    const int taps = mode == 0 ? 9 : (mode == 1 ? 1 : 4);
+    const int Hin = mode == 2 ? 2 * H : (mode == 3 ? H / 2 : H);
+    __half *a0 = nullptr, *a0l = nullptr, *a1 = nullptr, *a1l = nullptr, *o = nullptr, *ol = nullptr;
+    if (to_nhwc(x0, &a0, s, n_img, C0, Hin * Hin, st, sp ? &a0l : nullptr)) return -1;
+    if (x1 && to_nhwc(x1, &a1, s, n_img, C1, Hin * Hin, st, sp ? &a1l : nullptr)) return -1;
+    in0 = Act(a0, C0, a0l);
+    if (x1) in1 = Act(a1, C1, a1l);
+    if (s.get(&o, (size_t)n_img * H * W * Cout) || (sp && s.get(&ol, (size_t)n_img * H * W * Cout))) return -1;
+    out = Act(o, Cout, ol);
+    L.mode = mode;
+    L.cin = C0 + (x1 ? C1 : 0);
+    L.cout = Cout;
+    L.K = L.cin * taps;
+    L.Kp = precision >= 1 ? 2 * L.K : L.K;
+    L.bn = pick_bn(Cout);
+    L.bias = const_cast<float*>(bias);
+    const int rows = mode == 3 ? 4 * Cout : Cout;
+    if (s.get(&L.w, (size_t)rows * L.Kp)) return -1;
+    if (pack_conv_weight(weight, L.w, Cout, L.cin, taps, mode == 3, L.Kp, 0, precision >= 1 ? L.K : 0, 0, st))
+      return -1;
+    if (make_weight_map(&L.wmap, L.w, rows, L.Kp, L.bn)) return -1;
+    eng.precision = precision;
+    NOPE_CUDA(cudaGetDevice(&eng.device));
+    NOPE_CUDA(cudaDeviceGetAttribute(&eng.num_sms, cudaDevAttrMultiProcessorCount, eng.device));
+    return 0;
+  }
+};
+}  // namespace
+
 int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, int C1,
                  const float* weight, const float* bias, float* out, int n_img, int H, int W,
                  int Cout, void* stream) {
-  NOPE_CHECK(x0 && weight && out, "null argument");
+  NOPE_CHECK(out, "null argument");
   NOPE_CHECK(impl == 2, "impl must be 2 (tensor cores, clustered: conv_tc2_kernel)");
-  NOPE_CHECK(mode >= 0 && mode <= 3, "mode must be 0..3");
-  NOPE_CHECK(H == W, "square images only");
-  NOPE_CHECK(C0 % 64 == 0 && C1 % 64 == 0 && Cout % 64 == 0, "channels must be multiples of 64");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  Scratch s;
-  const int taps = mode == 0 ? 9 : (mode == 1 ? 1 : 4);
-  const int cin = C0 + (x1 ? C1 : 0);
-  const int Hin = mode == 2 ? 2 * H : (mode == 3 ? H / 2 : H);
-  const int rows = mode == 3 ? 4 * Cout : Cout;
-  __half *a0 = nullptr, *a1 = nullptr, *wp = nullptr, *o = nullptr;
-  if (to_nhwc(x0, &a0, s, n_img, C0, Hin * Hin, st)) return -1;
-  if (x1 && to_nhwc(x1, &a1, s, n_img, C1, Hin * Hin, st)) return -1;
-  if (s.get(&wp, (size_t)rows * cin * taps) || s.get(&o, (size_t)n_img * H * W * Cout)) return -1;
-  const float* wsrc = weight;
-  if (mode == 3) {
-    float* folded = nullptr;
-    if (s.get(&folded, (size_t)rows * cin * taps)) return -1;
-    fold_upconv_kernel<<<ew_grid((long long)4 * Cout * cin), 256, 0, st>>>(weight, folded, Cout, cin);
-    NOPE_CUDA(cudaGetLastError());
-    wsrc = folded;
-  }
-  pack_weight_kernel<<<ew_grid((long long)rows * cin * taps), 256, 0, st>>>(wsrc, wp, rows, cin, taps,
-                                                                           cin * taps, 0);
-  NOPE_CUDA(cudaGetLastError());
-  nope_unet eng;  // only used for its conv launcher / map cache
-  cudaDeviceProp prop;
-  int dev = 0;
-  NOPE_CUDA(cudaGetDevice(&dev));
-  NOPE_CUDA(cudaGetDeviceProperties(&prop, dev));
-  eng.num_sms = prop.multiProcessorCount;
-  ConvLayer L;
-  L.mode = mode; L.cin = cin; L.cout = Cout; L.K = cin * taps; L.Kp = L.K; L.bn = pick_bn(Cout); L.w = wp;
-  float* dbias = nullptr;
-  if (bias) {
-    if (s.get(&dbias, Cout)) return -1;
-    NOPE_CUDA(cudaMemcpyAsync(dbias, bias, Cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  }
-  L.bias = dbias;
-  if (make_weight_map(&L.wmap, wp, rows, L.K, L.bn)) return -1;
-  if (eng.conv(L, Act(a0, C0), x1 ? Act(a1, C1) : Act(), Act(o, Cout), H, n_img, n_img, st)) return -1;
-  if (to_nchw(o, out, n_img, Cout, H * W, st)) return -1;
+  OpConv op;
+  if (op.setup(mode, 3, 0, x0, C0, x1, C1, weight, bias, n_img, H, W, Cout, st)) return -1;
+  if (op.eng.conv(op.L, op.in0, op.in1, op.out, H, n_img, n_img, st)) return -1;
+  if (to_nchw(op.out.hi, out, n_img, Cout, H * W, st)) return -1;
   NOPE_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
@@ -2096,46 +2016,23 @@ int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, i
 int nope_op_conv_gn(int impl, int mode, const float* x0, int C0, const float* x1, int C1,
                     const float* weight, const float* bias, const float* gamma, const float* beta,
                     int G, int silu, float* out, int n_img, int H, int W, int Cout, void* stream) {
-  NOPE_CHECK(x0 && weight && gamma && beta && out, "null argument");
+  NOPE_CHECK(gamma && beta && out, "null argument");
   NOPE_CHECK(impl == 2, "impl must be 2 (tensor cores, clustered: conv_tc2_kernel)");
-  NOPE_CHECK(mode >= 0 && mode <= 2 && H == W, "bad mode / non-square image");
-  NOPE_CHECK(C0 % 64 == 0 && C1 % 64 == 0 && Cout % 64 == 0, "channels must be multiples of 64");
   NOPE_CHECK(G >= 1 && (Cout / 8) % G == 0, "groups must divide the 8-channel octets");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  Scratch s;
-  const int taps = mode == 0 ? 9 : (mode == 1 ? 1 : 4);
-  const int cin = C0 + (x1 ? C1 : 0);
-  const int Hin = mode == 2 ? 2 * H : H;
   const int hw = H * W, parts = hw < 32 ? 1 : hw / 32, noct = Cout / 8;
-  __half *a0 = nullptr, *a1 = nullptr, *wp = nullptr, *o = nullptr;
+  OpConv op;
+  if (op.setup(mode, 2, 0, x0, C0, x1, C1, weight, bias, n_img, H, W, Cout, st)) return -1;
   float2* stats = nullptr;
-  if (to_nhwc(x0, &a0, s, n_img, C0, Hin * Hin, st)) return -1;
-  if (x1 && to_nhwc(x1, &a1, s, n_img, C1, Hin * Hin, st)) return -1;
-  if (s.get(&wp, (size_t)Cout * cin * taps) || s.get(&o, (size_t)n_img * hw * Cout) ||
-      s.get(&stats, (size_t)n_img * parts * noct))
-    return -1;
-  pack_weight_kernel<<<ew_grid((long long)Cout * cin * taps), 256, 0, st>>>(weight, wp, Cout, cin, taps,
-                                                                            cin * taps, 0);
-  NOPE_CUDA(cudaGetLastError());
-  nope_unet eng;
-  cudaDeviceProp prop;
-  int dev = 0;
-  NOPE_CUDA(cudaGetDevice(&dev));
-  NOPE_CUDA(cudaGetDeviceProperties(&prop, dev));
-  eng.num_sms = prop.multiProcessorCount;
-  ConvLayer L;
-  L.mode = mode; L.cin = cin; L.cout = Cout; L.K = cin * taps; L.Kp = L.K; L.bn = pick_bn(Cout); L.w = wp;
-  L.bias = const_cast<float*>(bias);
-  if (make_weight_map(&L.wmap, wp, Cout, L.K, L.bn)) return -1;
-  if (eng.conv(L, Act(a0, C0), x1 ? Act(a1, C1) : Act(), Act(o, Cout), H, n_img, n_img, st, nullptr, stats))
-    return -1;
+  if (op.s.get(&stats, (size_t)n_img * parts * noct)) return -1;
+  if (op.eng.conv(op.L, op.in0, op.in1, op.out, H, n_img, n_img, st, nullptr, stats)) return -1;
   // GroupNorm on the host, in double, from the epilogue's [img][parts][octet] partial sums alone: a group's sum and
   // sum of squares are the totals of its octets over all parts (the layout the LDM engine normalises from)
   std::vector<__half> ho((size_t)n_img * hw * Cout);
   std::vector<float2> hs((size_t)n_img * parts * noct);
   std::vector<float> hg(Cout), hb(Cout), y((size_t)n_img * Cout * hw);
   NOPE_CUDA(cudaStreamSynchronize(st));
-  NOPE_CUDA(cudaMemcpy(ho.data(), o, ho.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+  NOPE_CUDA(cudaMemcpy(ho.data(), op.out.hi, ho.size() * sizeof(__half), cudaMemcpyDeviceToHost));
   NOPE_CUDA(cudaMemcpy(hs.data(), stats, hs.size() * sizeof(float2), cudaMemcpyDeviceToHost));
   NOPE_CUDA(cudaMemcpy(hg.data(), gamma, Cout * sizeof(float), cudaMemcpyDeviceToHost));
   NOPE_CUDA(cudaMemcpy(hb.data(), beta, Cout * sizeof(float), cudaMemcpyDeviceToHost));
@@ -2170,48 +2067,21 @@ int nope_op_conv_gn_fused(int mode, int precision, const float* x0, int C0, cons
                           const float* weight, const float* bias, const float* gamma, const float* beta, int G,
                           int silu, const float* chan_bias, const float* residual, int res_div, float* out,
                           float* emit_out, int n_img, int H, int W, int Cout, void* stream) {
-  NOPE_CHECK(x0 && weight && out, "null argument");
-  NOPE_CHECK(mode >= 0 && mode <= 2 && H == W, "bad mode / non-square image");
+  NOPE_CHECK(out, "null argument");
   NOPE_CHECK(precision >= 0 && precision <= 2, "precision must be 0..2");
-  NOPE_CHECK(C0 % 64 == 0 && C1 % 64 == 0 && Cout % 64 == 0, "channels must be multiples of 64");
   NOPE_CHECK(G == 0 || (gamma && beta), "GroupNorm needs gamma / beta");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  Scratch s;
-  const bool sp = precision == 2;
-  const int taps = mode == 0 ? 9 : (mode == 1 ? 1 : 4);
-  const int cin = C0 + (x1 ? C1 : 0);
-  const int Hin = mode == 2 ? 2 * H : H;
   const int hw = H * W;
-  __half *a0 = nullptr, *a0l = nullptr, *a1 = nullptr, *a1l = nullptr, *wp = nullptr, *o = nullptr, *ol = nullptr,
-         *r = nullptr, *rl = nullptr, *pbh = nullptr;
-  if (to_nhwc(x0, &a0, s, n_img, C0, Hin * Hin, st, sp ? &a0l : nullptr)) return -1;
-  if (x1 && to_nhwc(x1, &a1, s, n_img, C1, Hin * Hin, st, sp ? &a1l : nullptr)) return -1;
+  OpConv op;
+  if (op.setup(mode, 2, precision, x0, C0, x1, C1, weight, bias, n_img, H, W, Cout, st)) return -1;
+  __half *r = nullptr, *rl = nullptr, *pbh = nullptr;
   const int n_res = residual ? (res_div > 0 ? (n_img + res_div - 1) / res_div : n_img) : 0;
-  if (residual && to_nhwc(residual, &r, s, n_res, Cout, hw, st, sp ? &rl : nullptr)) return -1;
-  if (chan_bias && to_nhwc(chan_bias, &pbh, s, n_img, Cout, 1, st)) return -1;
-  const int K = cin * taps, Kp = precision >= 1 ? 2 * K : K;
-  if (s.get(&wp, (size_t)Cout * Kp) || s.get(&o, (size_t)n_img * hw * Cout)) return -1;
-  if (sp && s.get(&ol, (size_t)n_img * hw * Cout)) return -1;
-  pack_weight_kernel<<<ew_grid((long long)Cout * K), 256, 0, st>>>(weight, wp, Cout, cin, taps, Kp, 0,
-                                                                    precision >= 1 ? K : 0);
-  NOPE_CUDA(cudaGetLastError());
-  nope_unet eng;
-  eng.precision = precision;
-  cudaDeviceProp prop;
-  int dev = 0;
-  NOPE_CUDA(cudaGetDevice(&dev));
-  NOPE_CUDA(cudaGetDeviceProperties(&prop, dev));
-  eng.num_sms = prop.multiProcessorCount;
-  eng.device = dev;
-  if (eng.ensure_workspace(n_img, std::max(n_res, 1))) return -1;
-  if (eng.prepare_stream(st)) return -1;
-  eng.pb = pbh;
-  eng.P = Cout;
-  ConvLayer L;
-  L.mode = mode; L.cin = cin; L.cout = Cout; L.K = K; L.Kp = Kp; L.bn = pick_bn(Cout); L.w = wp;
-  L.bias = const_cast<float*>(bias);
-  if (make_weight_map(&L.wmap, wp, Cout, Kp, L.bn))
-    return -1;
+  if (residual && to_nhwc(residual, &r, op.s, n_res, Cout, hw, st, precision == 2 ? &rl : nullptr)) return -1;
+  if (chan_bias && to_nhwc(chan_bias, &pbh, op.s, n_img, Cout, 1, st)) return -1;
+  if (op.eng.ensure_workspace(n_img, std::max(n_res, 1))) return -1;
+  if (op.eng.prepare_stream(st)) return -1;
+  op.eng.pb = pbh;
+  op.eng.P = Cout;
   NormLayer N;
   N.C = Cout; N.G = std::max(G, 1);
   N.gamma = const_cast<float*>(gamma);
@@ -2225,13 +2095,11 @@ int nope_op_conv_gn_fused(int mode, int precision, const float* x0, int C0, cons
   float2* em = nullptr;
   const int eparts = nope_unet::fused_emit_parts(H, Cout);
   if (emit_out) {
-    if (s.get(&em, (size_t)n_img * eparts)) return -1;
+    if (op.s.get(&em, (size_t)n_img * eparts)) return -1;
     gs.emit = em;
   }
-  if (eng.conv(L, Act(a0, C0, a0l), x1 ? Act(a1, C1, a1l) : Act(), Act(o, Cout, ol), H, n_img,
-               n_img, st, &gs))
-    return -1;
-  if (to_nchw(o, out, n_img, Cout, hw, st, ol)) return -1;
+  if (op.eng.conv(op.L, op.in0, op.in1, op.out, H, n_img, n_img, st, &gs)) return -1;
+  if (to_nchw(op.out.hi, out, n_img, Cout, hw, st, op.out.lo)) return -1;
   if (emit_out) {
     // fold the per-tile partials on the host side of the test: [n_img][eparts] -> [n_img][2]
     std::vector<float2> h((size_t)n_img * eparts);

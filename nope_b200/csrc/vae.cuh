@@ -252,21 +252,13 @@ __global__ void __launch_bounds__(256) vae_softmax_kernel(float* __restrict__ s)
 // A convolution of the VAE: packed split-precision weights [cout][K] fp16, K = taps x (W_hi | W_lo | W_hi) x cin,
 // then, for a ResnetBlock2D conv2 with a 1x1 shortcut, (S_hi | S_lo | S_hi) x cin_sc; bias = b2 (+ b_shortcut).
 // In the single-fp16 mode each tap holds W_hi alone: K = taps x cin (+ cin_sc).
-struct VaeConv {
-  int cin = 0, cin_sc = 0, cout = 0, k = 1, K = 0, bn = 0;
-  __half* w = nullptr;
-  float* bias = nullptr;
-  CUtensorMap wmap;
+struct VaeConv : ConvLayerBase {
+  int cin_sc = 0, k = 1;
 };
 
 struct VaeNorm {
   float* gamma = nullptr;
   float* beta = nullptr;
-};
-
-// One tap of a convolution: input pair (hi map 2 * pair, lo map 2 * pair + 1; fp16 mode: map pair) at (dy, dx).
-struct VaeTap {
-  int pair, dy, dx;
 };
 
 // ---------------------------------------------------------------- decoder kernels (DESIGN.md section 17)
@@ -375,7 +367,7 @@ struct VaeEngine {
   float* t32 = nullptr;                       // conv1 / qkv / conv_out output, fp32
   double2* gn_part = nullptr;                 // GroupNorm partial sums
   float2* gn_stats = nullptr;                 // GroupNorm (mean, rstd)
-  std::map<std::tuple<const void*, int, int, int>, CUtensorMap> tmaps;
+  TmapCache tmaps;
   int64_t launches = 0;
 
   explicit VaeEngine(int cap_) : cap(cap_) {}
@@ -420,20 +412,14 @@ struct VaeEngine {
     NOPE_CHECK(cin % 64 == 0 && cin_sc % 64 == 0, name + ": input channels must be a multiple of 64");
     L.bn = pick_bn(L.cout);
     std::vector<__half> packed((size_t)L.cout * L.K, __float2half_rn(0.f));
-    auto put = [&](__half* dst, int c, int stride, double v) {
-      const float wf = (float)v;
-      const __half hi = __float2half_rn(wf);
-      dst[c] = hi;
-      if (prods == 1) return;
-      dst[stride + c] = __float2half_rn(wf - __half2float(hi));
-      dst[2 * stride + c] = hi;
-    };
     for (int o = 0; o < cout_real; ++o) {
       for (int c = 0; c < cin; ++c)
         for (int t = 0; t < taps; ++t)
-          put(&packed[(size_t)o * L.K + (size_t)t * prods * cin], c, cin, W[((size_t)o * cin + c) * taps + t]);
+          put_split_weight(&packed[(size_t)o * L.K + (size_t)t * prods * cin + c], cin, prods,
+                           (float)W[((size_t)o * cin + c) * taps + t]);
       for (int c = 0; c < cin_sc; ++c)
-        put(&packed[(size_t)o * L.K + (size_t)taps * prods * cin], c, cin_sc, (*Ws)[(size_t)o * cin_sc + c]);
+        put_split_weight(&packed[(size_t)o * L.K + (size_t)taps * prods * cin + c], cin_sc, prods,
+                         (float)(*Ws)[(size_t)o * cin_sc + c]);
     }
     std::vector<float> b(L.cout, 0.f);
     for (int o = 0; o < cout_real; ++o) b[o] = (float)bias[o];
@@ -494,77 +480,30 @@ struct VaeEngine {
   }
 
   // ---------------------------------------------------------------- launches
-  // NHWC map of `cap` images of side H x H and C channels at base; lattice >= 0: the stride-2 sub-lattice
-  // (lattice >> 1, lattice & 1) of a 2H x 2H tensor
-  int get_map(const CUtensorMap** out, const void* base, int C, int H, int lattice) {
-    const auto key = std::make_tuple(base, lattice, C, H);
-    auto it = tmaps.find(key);
-    if (it == tmaps.end()) {
-      TileGeom g;
-      if (make_geom(H, H, &g)) return -1;
-      CUtensorMap m;
-      const int rc = lattice < 0 ? make_act_map(&m, base, cap, C, g)
-                                 : make_unshuffle_map(&m, base, cap, C, g, lattice >> 1, lattice & 1);
-      if (rc) return -1;
-      it = tmaps.emplace(key, m).first;
-    }
-    *out = &it->second;
-    return 0;
-  }
   // offset of plane q of a parity-planar level-0 tensor with C channels
   size_t plane_off(int q, int C) const { return (size_t)q * cap * 128 * 128 * C; }
 
   // out = conv(taps over the input pairs `in`) [+ shortcut taps over pair sc] + bias [+ res]; output H x H.
   // in: (hi, lo) base pointers of each input pair with their lattice (-1: plain NHWC of side H); fp16 mode: hi only.
-  int conv(const VaeConv& L, const std::vector<std::pair<ActPair, int>>& in, int Hin_map,
-           const std::vector<VaeTap>& taps, int sc_pair, int H, int n, __half* out_hi, __half* out_lo,
-           float* out_f32, const ActPair* res, cudaStream_t st) {
+  // A tap's lat is the index of its input pair.
+  int conv(const VaeConv& L, const std::vector<std::pair<ActPair, int>>& in, const std::vector<ConvTap>& taps,
+           int sc_pair, int H, int n, __half* out_hi, __half* out_lo, float* out_f32, const ActPair* res,
+           cudaStream_t st) {
     TileGeom g;
     if (make_geom(H, H, &g)) return -1;
-    ConvParams p;
-    memset(&p, 0, sizeof p);
-    const CUtensorMap* m = nullptr;
     NOPE_CHECK(in.size() <= (size_t)kMaxAMaps / 2, "vae conv: too many input maps");
-    const bool split = precision == 0;   // fp16 mode: one map per input (its hi), one segment per tap
-    const int mps = split ? 2 : 1;       // maps per input
+    ConvBuilder b(tmaps, g, cap);
+    ConvParams& p = b.p;
+    int mh[kMaxAMaps / 2], ml[kMaxAMaps / 2];
     for (size_t i = 0; i < in.size(); ++i) {
       const int C = (int)i == sc_pair ? L.cin_sc : L.cin;
-      if (get_map(&m, in[i].first.hi, C, Hin_map, in[i].second)) return -1;
-      p.amap[mps * i] = *m;
-      if (!split) continue;
-      if (get_map(&m, in[i].first.lo, C, Hin_map, in[i].second)) return -1;
-      p.amap[2 * i + 1] = *m;
+      mh[i] = b.map(in[i].first.hi, C, in[i].second);
+      ml[i] = precision == 0 ? b.map(in[i].first.lo, C, in[i].second) : -1;   // fp16 mode: the hi maps only
     }
-    p.n_amaps = mps * (int)in.size();
-    int nseg = 0, ksteps = 0;
-    auto add = [&](const VaeTap& t, int nch) {
-      p.seg[nseg++] = ConvSeg{(int16_t)(mps * t.pair), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};     // A_hi W_hi
-      ksteps += nch;
-      if (!split) return;
-      p.seg[nseg++] = ConvSeg{(int16_t)(2 * t.pair), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};       // A_hi W_lo
-      p.seg[nseg++] = ConvSeg{(int16_t)(2 * t.pair + 1), (int16_t)t.dy, (int16_t)t.dx, (int16_t)nch};   // A_lo W_hi
-      ksteps += 2 * nch;
-    };
-    for (const VaeTap& t : taps) add(t, L.cin / 64);
-    if (sc_pair >= 0) add(VaeTap{sc_pair, 0, 0}, L.cin_sc / 64);
-    NOPE_CHECK(nseg <= kMaxSeg && ksteps * 64 == L.K, "vae conv: segment table");
-    p.bmap = L.wmap;
-    if (get_map(&m, out_hi, L.cout, H, -1)) return -1;
-    p.omap[0] = *m;
-    p.bias = L.bias;
-    p.stats_hw = H * H;
-    p.stats_noct = L.cout / 8;
-    p.n_total = L.cout;
-    p.m_valid = n * H * H;
-    p.nseg = nseg;
-    p.ksteps = ksteps;
-    p.m_tiles = geom_m_tiles(g, n);
-    p.n_par = 1;
-    p.n_tiles_par = L.cout / L.bn;
-    p.n_tiles = p.n_tiles_par;
-    p.tiles_per_img = g.tiles_per_img;
-    p.h_cnt = g.h_cnt;
-    p.b_cnt = g.b_cnt;
+    for (const ConvTap& t : taps) split_tap(b, mh[t.lat], ml[t.lat], t.dy, t.dx, L.cin / 64);
+    if (sc_pair >= 0) split_tap(b, mh[sc_pair], ml[sc_pair], 0, 0, L.cin_sc / 64);
+    if (b.finish(L, out_hi, L.cout, n, 1)) return -1;
+    NOPE_CHECK(p.ksteps * 64 == L.K, "vae conv: segment table");
     p.res_hi = res ? res->hi : nullptr;
     p.res_lo = res ? res->lo : nullptr;
     p.out_lo = out_lo;
@@ -578,13 +517,13 @@ struct VaeEngine {
   // Output: out_f32 (+ (hi, lo) when out_lo), residual res (same layout) or the conv's 1x1 shortcut over sc.
   int conv3(const VaeConv& L, const ActPair& in, int H, int n, const ActPair& out, bool want_lo, float* out_f32,
             const ActPair* res, const ActPair* sc, cudaStream_t st) {
-    std::vector<VaeTap> taps;
+    std::vector<ConvTap> taps;
     if (H < 256) {
       for (int oy = -1; oy <= 1; ++oy)
-        for (int ox = -1; ox <= 1; ++ox) taps.push_back(VaeTap{0, oy, ox});
+        for (int ox = -1; ox <= 1; ++ox) taps.push_back(ConvTap{0, oy, ox});
       std::vector<std::pair<ActPair, int>> src{{in, -1}};
       if (sc) src.push_back({*sc, -1});
-      return conv(L, src, H, taps, sc ? 1 : -1, H, n, out.hi, want_lo ? out.lo : nullptr, out_f32, res, st);
+      return conv(L, src, taps, sc ? 1 : -1, H, n, out.hi, want_lo ? out.lo : nullptr, out_f32, res, st);
     }
     NOPE_CHECK(!sc, "vae conv: no shortcut segments at the 256 x 256 level");
     std::vector<std::pair<ActPair, int>> src;
@@ -593,14 +532,11 @@ struct VaeEngine {
       const int py = q >> 1, px = q & 1;
       taps.clear();
       for (int oy = -1; oy <= 1; ++oy)
-        for (int ox = -1; ox <= 1; ++ox) {
-          const int sy = py + oy, sx = px + ox;
-          taps.push_back(VaeTap{(sy & 1) * 2 + (sx & 1), sy >> 1, sx >> 1});
-        }
+        for (int ox = -1; ox <= 1; ++ox) taps.push_back(stride2_tap(py + oy, px + ox));
       const size_t o = plane_off(q, L.cout);
       ActPair r;
       if (res) r = act_at(*res, o);
-      if (conv(L, src, 128, taps, -1, 128, n, out.hi + o, want_lo ? act_at(out, o).lo : nullptr, out_f32 + o,
+      if (conv(L, src, taps, -1, 128, n, out.hi + o, want_lo ? act_at(out, o).lo : nullptr, out_f32 + o,
                res ? &r : nullptr, st))
         return -1;
     }
@@ -637,7 +573,7 @@ struct VaeEngine {
       const VaeConv& S = convs.at(p + ".conv_shortcut");
       for (int q = 0; q < 4; ++q) {
         const size_t i = plane_off(q, cin), o = plane_off(q, cout);
-        if (conv(S, {{act_at(xs[cur], i), -1}}, 128, {VaeTap{0, 0, 0}}, -1, 128, n, sres.hi + o, act_at(sres, o).lo,
+        if (conv(S, {{act_at(xs[cur], i), -1}}, {ConvTap{0, 0, 0}}, -1, 128, n, sres.hi + o, act_at(sres, o).lo,
                  nullptr, nullptr, st))
           return -1;
       }
@@ -659,7 +595,7 @@ struct VaeEngine {
     if (group_norm(a + "group_norm", x32[cur], 512, 32, n, false, st)) return -1;
     // qkv [n * 1024, 1536] fp32 -> t32 (high halves into xs[nxt].hi, overwritten by proj_attn)
     const VaeConv& qkv = convs.at(a + "qkv");
-    if (conv(qkv, {{nrm, -1}}, 32, {VaeTap{0, 0, 0}}, -1, 32, n, xs[nxt].hi, nullptr, t32, nullptr, st)) return -1;
+    if (conv(qkv, {{nrm, -1}}, {ConvTap{0, 0, 0}}, -1, 32, n, xs[nxt].hi, nullptr, t32, nullptr, st)) return -1;
     // S = q k^T / sqrt(512) -> x32[nxt] (overwritten by proj_attn), softmax over keys in place
     float* S = x32[nxt];
     vae_attn_gemm_kernel<true, false><<<dim3(16, 16, n), 256, 0, st>>>(
@@ -675,7 +611,7 @@ struct VaeEngine {
     NOPE_CUDA(cudaGetLastError());
     launches += 3;
     // x + proj_attn(O)
-    if (conv(convs.at(a + "proj_attn"), {{nrm, -1}}, 32, {VaeTap{0, 0, 0}}, -1, 32, n, xs[nxt].hi, xs[nxt].lo,
+    if (conv(convs.at(a + "proj_attn"), {{nrm, -1}}, {ConvTap{0, 0, 0}}, -1, 32, n, xs[nxt].hi, xs[nxt].lo,
              x32[nxt], &xs[cur], st))
       return -1;
     cur = nxt;
@@ -796,10 +732,10 @@ struct nope_vae : nope::VaeEngine {
         src.push_back({in, q});
       }
     }
-    std::vector<VaeTap> taps;
+    std::vector<ConvTap> taps;
     for (int ky = 0; ky < 3; ++ky)
-      for (int kx = 0; kx < 3; ++kx) taps.push_back(VaeTap{(ky & 1) * 2 + (kx & 1), ky >> 1, kx >> 1});
-    return conv(L, src, H, taps, -1, H, n, out.hi, out.lo, out_f32, nullptr, st);
+      for (int kx = 0; kx < 3; ++kx) taps.push_back(stride2_tap(ky, kx));
+    return conv(L, src, taps, -1, H, n, out.hi, out.lo, out_f32, nullptr, st);
   }
 
   // n <= kChunk images [n, 3, 256, 256] -> out [n, 4, 32, 32]
@@ -1017,13 +953,13 @@ struct nope_vae_decoder : nope::VaeEngine {
     const bool planar = 2 * H == 256;
     for (int q = 0; q < 4; ++q) {
       const int py = q >> 1, px = q & 1;
-      std::vector<VaeTap> taps;
+      std::vector<ConvTap> taps;
       for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b) taps.push_back(VaeTap{0, py - 1 + a, px - 1 + b});
+        for (int b = 0; b < 2; ++b) taps.push_back(ConvTap{0, py - 1 + a, px - 1 + b});
       const size_t o = (size_t)q * cap * H * H * C;
       float* f = (planar ? x32[nxt] : t32) + o;
       const ActPair d = planar ? ActPair{xs[nxt].hi + o, xs[nxt].lo + o} : ActPair{nrm.hi + o, nrm.lo + o};
-      if (conv(convs.at(name + ".p" + std::to_string(q)), {{xs[cur], -1}}, H, taps, -1, H, n, d.hi, d.lo, f, nullptr,
+      if (conv(convs.at(name + ".p" + std::to_string(q)), {{xs[cur], -1}}, taps, -1, H, n, d.hi, d.lo, f, nullptr,
                st))
         return -1;
     }
