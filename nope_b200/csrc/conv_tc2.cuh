@@ -1033,7 +1033,7 @@ conv_tc2_kernel(const __grid_constant__ ConvParams p) {
       if constexpr (EPI == 2)
         conv_epilogue_geglu(ost, s_bias, s_acc, e, lane);
       else if constexpr (kPrefetchRes)
-        conv_epilogue_tile<BN, true>(p, ost, s_bias, s_acc, m_tile, n_chan0, e, lane, &pre);
+        conv_epilogue_tile<BN, true>(p, ost, s_bias, s_acc, m_tile, n_chan0, e, lane, &pre, par);
       else if constexpr (EPI == 1)
         conv_epilogue_tile<BN, true>(p, ost, s_bias, s_acc, m_tile, n_chan0, e, lane, nullptr, par);
       else

@@ -198,7 +198,8 @@ struct nope_encoder {
   nope::TmapCache tmaps;
   int64_t launches = 0;
   static constexpr int kChunk = 32;   // images per encode() call: the workspace holds this many
-  float* rot_stage = nullptr;         // kChunk rotated 256x256 crops (25 MB), allocated by the first encode_inplane
+  float* rot_stage = nullptr;         // kChunk rotated 256x256 crops (25 MB), allocated by the first rotated encode
+  size_t out_floats() const { return (size_t)D * 32 * 32; }   // per encoded image
 
   // ---------------------------------------------------------------- schema (resnet.py:93-133)
   void expect_bn(const std::string& p, int c) {
@@ -413,7 +414,6 @@ struct nope_encoder {
   int run_block(const std::string& name, const float* x, int C, int H, int n, float* out, int64_t cap_floats,
                 cudaStream_t st) {
     using namespace nope;
-    NOPE_CHECK(n >= 1 && n <= kChunk, "run_block: n must be in [1, " + std::to_string(kChunk) + "]");
     int Ci = 0, Hi = 0, Co = 0, Ho = 0, stv = 1;
     if (name == "stem") {
       Ci = 3, Hi = 256, Co = 64, Ho = 128;
@@ -432,10 +432,7 @@ struct nope_encoder {
         }
       NOPE_CHECK(Ci, "run_block: unknown encoder module " + name);
     }
-    NOPE_CHECK(C == Ci && H == Hi, "run_block: " + name + " takes [n, " + std::to_string(Ci) + ", " +
-                                       std::to_string(Hi) + ", " + std::to_string(Hi) + "] inputs, got C = " +
-                                       std::to_string(C) + ", H = " + std::to_string(H));
-    NOPE_CHECK(cap_floats >= (int64_t)n * Co * Ho * Ho, "run_block: output buffer too small");
+    if (check_block(name, kChunk, C, H, n, Ci, Hi, Co, Ho, cap_floats)) return -1;
     if (ensure_workspace(n)) return -1;
     launches = 0;
     if (name == "stem") {
@@ -460,46 +457,5 @@ struct nope_encoder {
   static void to_nchw_pair(const nope::ActPair& a, float* out, int n, int C, int H, cudaStream_t st) {
     nope::nhwc_f16_to_nchw_f32_kernel<<<nope::ew_grid((long long)n * C * H * H), 256, 0, st>>>(a.hi, out, n, C, H * H,
                                                                                                a.lo);
-  }
-
-  // images [B, 3, 256, 256] x angles cossin [A, 2] -> out [B, A, D, 32, 32]: the (image, angle) pairs in b-major
-  // order, kChunk at a time, each chunk rotated into rot_stage and encoded from there, so the [B, A, 3, 256, 256]
-  // rotated batch never exists.  The chunks are those nope_encoder_encode makes of that batch.
-  int encode_inplane(const float* images, int B, const float* cossin, int A, float* out, cudaStream_t st) {
-    using namespace nope;
-    constexpr long long kImg = 3LL * 256 * 256;
-    if (!rot_stage && mem.alloc(&rot_stage, kChunk * kImg)) return -1;
-    NOPE_CHECK((int64_t)B * A <= INT32_MAX, "too many (image, angle) pairs");
-    const int pairs = B * A;
-    int64_t total = 0;
-    for (int lo = 0; lo < pairs; lo += kChunk) {
-      const int n = pairs - lo < kChunk ? pairs - lo : kChunk;
-      inplane_rotate_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, cossin, A, 256, 256, lo, rot_stage);
-      NOPE_CUDA(cudaGetLastError());
-      if (encode(rot_stage, n, out + (size_t)lo * D * 32 * 32, st)) return -1;
-      total += launches + 1;
-    }
-    launches = total;
-    return 0;
-  }
-
-  // images [B, 3, 256, 256] x pairs (image_idx [P], cossin [P, 2]) -> out [P, D, 32, 32]: the pairs in order, kChunk
-  // at a time through rot_stage, so the result equals nope_encoder_encode of the materialised [P, 3, 256, 256] batch.
-  int encode_rotated(const float* images, int B, const int* image_idx, const float* cossin, int P, float* out,
-                     cudaStream_t st) {
-    using namespace nope;
-    constexpr long long kImg = 3LL * 256 * 256;
-    if (!rot_stage && mem.alloc(&rot_stage, kChunk * kImg)) return -1;
-    int64_t total = 0;
-    for (int lo = 0; lo < P; lo += kChunk) {
-      const int n = P - lo < kChunk ? P - lo : kChunk;
-      inplane_rotate_pairs_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, B, image_idx, cossin, 256, 256,
-                                                                             lo, rot_stage);
-      NOPE_CUDA(cudaGetLastError());
-      if (encode(rot_stage, n, out + (size_t)lo * D * 32 * 32, st)) return -1;
-      total += launches + 1;
-    }
-    launches = total;
-    return 0;
   }
 };

@@ -1,11 +1,22 @@
-// nope_b200 -- the host-side lifecycle every weight-holding engine (UNet, template encoder, VAE encoder, VAE decoder,
+// nope_b200 -- the host-side code every weight-holding engine (UNet, template encoder, VAE encoder, VAE decoder,
 // LDM) shares: the state_dict schema and the host copies staged against it until finalize, the device allocations
 // freed with the engine, the device check of every *_create, and the bodies of the *_load_tensor / *_finalize /
-// per-chunk C-ABI entry points.
+// per-chunk C-ABI entry points.  The two sweep engines (UNet, LDM) also share the sweep driver, the debug tap and the
+// per-launch profile; the two image encoders share the rotated-encode loop and the run_block shape checks.
 //
 // An engine E provides: `static constexpr const char* kName` (the name its errors carry), `bool finalized`,
 // `int device`, `StagedWeights staged`, and `int finalize()` (packs the staged tensors; runs once every schema key
 // is present, on E's device).
+//
+// A sweep engine (engine_sweep, engine_debug_tap) also provides `int chunk`, `int64_t launches`, `DebugTap dtap`,
+// `float* score_partial` and `float* sim_buf`, and
+//   int ensure_workspace(int hyps, int refs, int scores, cudaStream_t)  sizes the workspace (and the score partials
+//       and similarity scratch of `scores` (reference, query, pose) triples) before a launch on the stream;
+//   int prestage(const float* ref, int B, cudaStream_t)                  the pose-independent prefix per reference;
+//   int forward_chunk(poses, hyp0, n, N, query, out_emb, score_part, cudaStream_t, int Q);
+//   int rank(part, sim, B, N, Q, k, topv, topi, idx_base, cudaStream_t) the similarities and top-k from the partials.
+// An image encoder (per_rotated_chunk) provides `kChunk`, `int64_t launches`, `DeviceAllocs mem`, `float* rot_stage`
+// and `int encode(const float*, int, float*, cudaStream_t)`.
 #pragma once
 #include <algorithm>
 #include <map>
@@ -13,6 +24,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "kernels.cuh"
 
 namespace nope {
 
@@ -153,6 +165,158 @@ int check_sweep(const E* e, const float* ref, const float* poses, int B, int N, 
   NOPE_CHECK(!(out_sim || k > 0) || query, "scores / top-k need the query");
   NOPE_CHECK(k >= 0 && k <= N && k <= 64, "k must be in [0, min(N, 64)]");
   NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
+  return 0;
+}
+
+// The debug tap of a sweep engine (nope_*_debug_tap): the first time forward_chunk passes the activation called
+// `name`, capture() writes it to `out` as [n, C, S, S] fp32 and records its shape.
+struct DebugTap {
+  std::string name;
+  float* out = nullptr;      // nullptr: no tap armed
+  int64_t cap = 0;           // floats at out
+  int C = 0, S = 0;
+  bool hit = false;
+  int capture(const char* at, const __half* hi, const __half* lo, bool bf16, int C_, int S_, int n, cudaStream_t st) {
+    if (out == nullptr || name != at || hit) return 0;
+    NOPE_CHECK((int64_t)n * C_ * S_ * S_ <= cap, "debug tap: output buffer too small");
+    nhwc_f16_to_nchw_f32_kernel<<<ew_grid((long long)n * C_ * S_ * S_), 256, 0, st>>>(hi, out, n, C_, S_ * S_, lo,
+                                                                                       bf16);
+    NOPE_CUDA(cudaGetLastError());
+    C = C_;
+    S = S_;
+    hit = true;
+    return 0;
+  }
+};
+
+// What one profiled launch computed: executed FLOPs, algorithmic FLOPs (those of the fp16 mode), and the engine's
+// own launch kind and shape.
+struct LaunchRecord {
+  double flops = 0.0, alg_flops = 0.0;
+  int kind = 0;
+  int4 shape = {0, 0, 0, 0};
+};
+
+// CUDA-event times of an engine's heavy launches (bench.py's roofline): begin() and end() bracket one launch and do
+// nothing while profiling is off.
+struct LaunchProfile {
+  bool on = false;
+  std::vector<cudaEvent_t> ev;       // one (begin, end) pair per record
+  std::vector<LaunchRecord> rec;
+
+  LaunchProfile() = default;
+  LaunchProfile(const LaunchProfile&) = delete;
+  LaunchProfile& operator=(const LaunchProfile&) = delete;
+  ~LaunchProfile() { reset(false); }
+  void reset(bool enable) {
+    for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    ev.clear();
+    rec.clear();
+    on = enable;
+  }
+  int begin(cudaStream_t st) { return on ? record(st) : 0; }
+  int end(cudaStream_t st, const LaunchRecord& r) {
+    if (!on) return 0;
+    if (record(st)) return -1;
+    rec.push_back(r);
+    return 0;
+  }
+  // milliseconds of launch i (its events must have completed)
+  int ms(size_t i, float* t) const {
+    NOPE_CUDA(cudaEventElapsedTime(t, ev[2 * i], ev[2 * i + 1]));
+    return 0;
+  }
+
+ private:
+  int record(cudaStream_t st) {
+    cudaEvent_t e;
+    NOPE_CUDA(cudaEventCreate(&e));
+    ev.push_back(e);
+    NOPE_CUDA(cudaEventRecord(e, st));
+    return 0;
+  }
+};
+
+// nope_unet_sweep_multi / nope_ldm_sweep_multi: the B references' N poses in chunks of the engine's `chunk`
+// hypotheses, each scored against its reference's Q queries, then ranked.  A sweep of a shape the engine has served
+// before makes no allocation and no host synchronisation.
+template <typename E>
+int engine_sweep(E* e, const float* ref, const float* poses, int B, int N, const float* query, int Q, float* out_emb,
+                 float* out_sim, int k, float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream) {
+  if (check_sweep(e, ref, poses, B, N, query, Q, out_sim, k, out_topv, out_topi)) return -1;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  NOPE_CUDA(cudaSetDevice(e->device));
+  e->launches = 0;
+  const int total = B * N;
+  const int cap = std::min(e->chunk, total);
+  if (e->ensure_workspace(cap, B, query ? total * Q : 0, st)) return -1;
+  float* part = query ? e->score_partial : nullptr;
+  if (e->prestage(ref, B, st)) return -1;
+  for (int h0 = 0; h0 < total; h0 += cap) {
+    const int n = std::min(cap, total - h0);
+    if (e->forward_chunk(poses, h0, n, N, query, out_emb, part, st, Q)) return -1;
+  }
+  if (query && (out_sim || k > 0)) {
+    if (e->rank(part, out_sim ? out_sim : e->sim_buf, B, N, Q, k, out_topv, out_topi, idx_base, st)) return -1;
+    ++e->launches;
+  }
+  return 0;
+}
+
+// nope_unet_debug_tap / nope_ldm_debug_tap: one reference's N <= chunk poses up to the activation called `name`,
+// copied to out as [N, C, H, H] fp32.
+template <typename E>
+int engine_debug_tap(E* e, const float* ref, const float* poses, int N, const char* name, float* out,
+                     int64_t out_capacity_floats, int* out_C, int* out_H, void* stream) {
+  NOPE_CHECK(e && e->finalized && ref && poses && name && out, "bad argument");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  NOPE_CHECK(N <= e->chunk, "debug tap: N must fit one chunk");
+  NOPE_CUDA(cudaSetDevice(e->device));
+  if (e->ensure_workspace(N, 1, 0, st)) return -1;
+  DebugTap& t = e->dtap;
+  t.name = name;
+  t.out = out;
+  t.cap = out_capacity_floats;
+  t.hit = false;
+  int rc = e->prestage(ref, 1, st);
+  if (!rc) rc = e->forward_chunk(poses, 0, N, N, nullptr, nullptr, nullptr, st, 1);
+  t.out = nullptr;
+  if (rc) return rc;
+  NOPE_CUDA(cudaStreamSynchronize(st));
+  NOPE_CHECK(t.hit, std::string("unknown tap name: ") + name);
+  if (out_C) *out_C = t.C;
+  if (out_H) *out_H = t.S;
+  return 0;
+}
+
+// P rotated 256 x 256 images through E::encode, E::kChunk at a time: rotate(lo, n) launches the rotation of pairs
+// [lo, lo + n) into rot_stage (allocated on first use), whose encodings go to out rows [lo, lo + n) of out_per floats.
+// The launch count is each chunk's plus its rotation.
+template <typename E, typename Rotate>
+int per_rotated_chunk(E* e, int P, float* out, size_t out_per, cudaStream_t st, Rotate rotate) {
+  if (!e->rot_stage && e->mem.alloc(&e->rot_stage, (size_t)E::kChunk * 3 * 256 * 256)) return -1;
+  int64_t launches = 0;
+  for (int lo = 0; lo < P; lo += E::kChunk) {
+    const int n = std::min(E::kChunk, P - lo);
+    rotate(lo, n);
+    NOPE_CUDA(cudaGetLastError());
+    if (e->encode(e->rot_stage, n, out + (size_t)lo * out_per, st)) return -1;
+    launches += e->launches + 1;
+  }
+  e->launches = launches;
+  return 0;
+}
+
+// The checks every *_run_block of an image engine makes once the module's input shape (Ci, Hi) and output shape
+// (Co, Ho) are known; Ci == 0: no such module.
+inline int check_block(const std::string& name, int chunk, int C, int H, int n, int Ci, int Hi, int Co, int Ho,
+                       int64_t cap_floats) {
+  NOPE_CHECK(Ci, "run_block: unknown module " + name);
+  NOPE_CHECK(n >= 1 && n <= chunk, "run_block: n must be in [1, " + std::to_string(chunk) + "]");
+  NOPE_CHECK(C == Ci && H == Hi, "run_block: " + name + " takes [n, " + std::to_string(Ci) + ", " +
+                                     std::to_string(Hi) + ", " + std::to_string(Hi) + "] inputs, got C = " +
+                                     std::to_string(C) + ", H = " + std::to_string(H));
+  NOPE_CHECK(cap_floats >= (int64_t)n * Co * Ho * Ho, "run_block: output buffer too small");
   return 0;
 }
 

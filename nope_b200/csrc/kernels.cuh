@@ -117,6 +117,12 @@ __global__ void init_conv_kernel(const float* __restrict__ x, const float* __res
   }
 }
 
+// hypotheses [h0, h0 + n) of the flattened (reference, pose) list -> their reference image: r[i] = (h0 + i) / N
+__global__ void ref_of_kernel(int* r, int h0, int N, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) r[i] = (h0 + i) / N;
+}
+
 // ----------------------------------------------------------------------------
 // broadcast a per-reference tensor to every hypothesis of that reference, optionally
 // adding the per-hypothesis pose projection (ResnetBlock.forward, model_utils.py:274-276,

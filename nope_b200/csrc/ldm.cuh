@@ -53,11 +53,6 @@ struct LdmBlock {      // one entry of input_blocks / output_blocks
   bool up = false;
 };
 
-__global__ void ldm_ref_of_kernel(int* r, int h0, int N, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) r[i] = (h0 + i) / N;
-}
-
 }  // namespace nope
 
 struct nope_ldm {
@@ -105,39 +100,13 @@ struct nope_ldm {
   nope::TmapCache tmaps;
   std::map<std::tuple<const void*, int, int, int>, CUtensorMap> tmaps3;
 
-  // per-launch CUDA-event profile (bench.py roofline): kind 0 = convolution / GEMM, 1 = attention
-  bool profile = false;
-  std::vector<cudaEvent_t> prof_ev;
-  std::vector<double> prof_flops;
-  std::vector<int> prof_kind;
-  int prof_begin(cudaStream_t st) {
-    cudaEvent_t e0;
-    NOPE_CUDA(cudaEventCreate(&e0));
-    NOPE_CUDA(cudaEventRecord(e0, st));
-    prof_ev.push_back(e0);
-    return 0;
-  }
-  int prof_end(cudaStream_t st, double flops, int kind) {
-    cudaEvent_t e1;
-    NOPE_CUDA(cudaEventCreate(&e1));
-    NOPE_CUDA(cudaEventRecord(e1, st));
-    prof_ev.push_back(e1);
-    prof_flops.push_back(flops);
-    prof_kind.push_back(kind);
-    return 0;
-  }
-
-  // debug tap
-  std::string tap_name;
-  float* tap_out = nullptr;
-  int64_t tap_cap = 0;
-  int tap_C = 0, tap_S = 0;
-  bool tap_hit = false;
+  // per-launch profile: record kind 0 = convolution / GEMM, 1 = attention
+  nope::LaunchProfile prof;
+  nope::DebugTap dtap;
 
   ~nope_ldm() {
     if (score_partial) cudaFree(score_partial);
     if (sim_buf) cudaFree(sim_buf);
-    for (cudaEvent_t e : prof_ev) cudaEventDestroy(e);
   }
 
   // ------------------------------------------------------------------ plan + schema
@@ -504,7 +473,25 @@ struct nope_ldm {
   }
 
   // ------------------------------------------------------------------ workspace
-  int ensure_workspace(int need_cap, int need_ref) {
+  // Sizes the workspace for `need_cap` hypotheses and `need_ref` references, and the score partials and similarity
+  // scratch for `need_scores` (reference, query, pose) triples.  Each grows on demand only (a host synchronisation and
+  // cudaMalloc then).
+  int ensure_workspace(int need_cap, int need_ref, int need_scores, cudaStream_t st) {
+    const size_t scored = (size_t)need_scores, part = scored * nslab();
+    if (part > score_partial_cap) {
+      NOPE_CUDA(cudaStreamSynchronize(st));
+      if (score_partial) cudaFree(score_partial);
+      score_partial = nullptr;
+      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&score_partial), part * sizeof(float)));
+      score_partial_cap = part;
+    }
+    if (scored > sim_buf_cap) {
+      NOPE_CUDA(cudaStreamSynchronize(st));
+      if (sim_buf) cudaFree(sim_buf);
+      sim_buf = nullptr;
+      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&sim_buf), scored * sizeof(float)));
+      sim_buf_cap = scored;
+    }
     if (need_cap <= cap && need_ref <= cap_ref) return 0;
     NOPE_CUDA(cudaDeviceSynchronize());
     ws_mem.release();
@@ -531,8 +518,8 @@ struct nope_ldm {
         ws_mem.alloc(&GG, c * 4 * u) || ws_mem.alloc(&x0ref, (size_t)cap_ref * u) ||
         ws_mem.alloc(&Rref, (size_t)cap_ref * u) || ws_mem.alloc(&Pref, (size_t)cap_ref * u))
       return -1;
-    const size_t st = (size_t)32 * 256;   // parts (<= 32) x octets (<= 256) per image
-    if (ws_mem.alloc(&S_in, c * st) || ws_mem.alloc(&S_mid, c * st) || ws_mem.alloc(&S_out, c * st)) return -1;
+    const size_t sts = (size_t)32 * 256;   // parts (<= 32) x octets (<= 256) per image
+    if (ws_mem.alloc(&S_in, c * sts) || ws_mem.alloc(&S_mid, c * sts) || ws_mem.alloc(&S_out, c * sts)) return -1;
     if (ws_mem.alloc(&cb, c * (size_t)cb_width) || ws_mem.alloc(&ref_of, c) || ws_mem.alloc(&OF, c * S0 * S0 * 64))
       return -1;
     return 0;
@@ -587,11 +574,11 @@ struct nope_ldm {
     p.geglu = L.geglu ? 1 : 0;
     p.out_f32 = out_f32;
     p.stats = stats;
-    if (profile && prof_begin(st)) return -1;
+    if (prof.begin(st)) return -1;
     const int rc = launch_conv_tc2(p, L.bn, num_sms, st);
     // executed FLOPs (the folded upsample runs 4 parity GEMMs of K = 4 Cin over the source pixels)
-    if (profile && prof_end(st, 2.0 * (double)n_img * g.H * g.W * (double)(L.mode == 3 ? 4 * L.cout : L.cout) * (double)L.k_alg, 0))
-      return -1;
+    const double fl = 2.0 * (double)n_img * g.H * g.W * (double)(L.mode == 3 ? 4 * L.cout : L.cout) * (double)L.k_alg;
+    if (prof.end(st, {fl, fl, 0})) return -1;
     return rc;
   }
 
@@ -655,7 +642,7 @@ struct nope_ldm {
     NOPE_CUDA(cudaGetLastError());
     const float sl2e = 0.17677669529663687f * 1.4426950408889634f;   // 32^-1/2 * log2(e)
     const dim3 grid((unsigned)(n * Hh) * (unsigned)((ntok + 127) / 128));
-    if (profile && prof_begin(st)) return -1;
+    if (prof.begin(st)) return -1;
     if (attn_impl == 1) {
       ldm_attn_simt_kernel<<<grid, 128, 0, st>>>(qkv, Vt, out, ntok, Hh, C, sl2e);
     } else {
@@ -677,18 +664,14 @@ struct nope_ldm {
       ldm_attn_tc_kernel<<<grid, 128, kAttnSmem, st>>>(p);
     }
     NOPE_CUDA(cudaGetLastError());
-    if (profile && prof_end(st, 4.0 * (double)n * ntok * (double)ntok * C, 1)) return -1;
+    const double fl = 4.0 * (double)n * ntok * (double)ntok * C;
+    if (prof.end(st, {fl, fl, 1})) return -1;
     launches += 2;
     return 0;
   }
 
   int tap(const std::string& name, const __half* buf, int C, int S, int n, cudaStream_t st) {
-    if (tap_out == nullptr || tap_name != name || tap_hit) return 0;
-    NOPE_CHECK((int64_t)n * C * S * S <= tap_cap, "debug tap: output buffer too small");
-    nope::nhwc_f16_to_nchw_f32_kernel<<<nope::ew_grid((long long)n * C * S * S), 256, 0, st>>>(buf, tap_out, n, C, S * S);
-    NOPE_CUDA(cudaGetLastError());
-    tap_C = C; tap_S = S; tap_hit = true;
-    return 0;
+    return dtap.capture(name.c_str(), buf, nullptr, false, C, S, n, st);
   }
 
   // ResBlock._forward (ldm/openaimodel.py:265-286) on cat(x0, x1).  Leaves the GroupNorm
@@ -764,7 +747,7 @@ struct nope_ldm {
   int forward_chunk(const float* poses, int hyp0, int n, int N, const float* query, float* out_emb,
                     float* score_part, cudaStream_t st, int Q = 1) {
     using namespace nope;
-    ldm_ref_of_kernel<<<(n + 255) / 256, 256, 0, st>>>(ref_of, hyp0, N, n);
+    ref_of_kernel<<<(n + 255) / 256, 256, 0, st>>>(ref_of, hyp0, N, n);
     ++launches;
     if (cross_terms(poses + (size_t)hyp0 * rot_dim, n, st)) return -1;
     int S = S0;
@@ -837,6 +820,17 @@ struct nope_ldm {
         score_part ? score_part + (size_t)hyp0 * Q * nslab : nullptr, hw, Cl, Q);
     NOPE_CUDA(cudaGetLastError());
     ++launches;
+    return 0;
+  }
+
+  // score slabs per (hypothesis, query) of ldm_score_kernel
+  int nslab() const { return (S0 * S0 + nope::kFinalThreads - 1) / nope::kFinalThreads; }
+  // similarities (sim [B * Q, N]) and top-k of every (reference, query) row from the score partials
+  int rank(const float* part, float* sim, int B, int N, int Q, int k, float* topv, int64_t* topi, int64_t idx_base,
+           cudaStream_t st) {
+    nope::sim_topk_kernel<<<B * Q, 256, 0, st>>>(part, nslab(), sim, N, k, topv, reinterpret_cast<long long*>(topi),
+                                                 (long long)idx_base, 1, 0, 1, Q);
+    NOPE_CUDA(cudaGetLastError());
     return 0;
   }
 };

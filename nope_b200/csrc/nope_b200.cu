@@ -1,10 +1,5 @@
-// nope_b200 -- engine + C ABI (include/nope_b200.h).
-//
-// The engine owns the repacked UNet weights, a per-chunk activation workspace and the
-// layer schedule of UNet.forward (reference:
-// src/model/u_net/denoising_diffusion_pytorch/u_net.py:160-198), batched over all pose
-// hypotheses of a chunk.  Host code is plain C++; kernels live in conv_tc2.cuh (convolution, with
-// conv_tc.cuh) / kernels.cuh.
+// nope_b200 -- the C ABI (include/nope_b200.h) over the engines (unet.cuh, encoder.cuh, vae.cuh, ldm.cuh) and the
+// stand-alone kernels, with the launch-scoped helpers its entry points use.  Host code is plain C++.
 #include "../../include/nope_b200.h"
 
 #include <algorithm>
@@ -27,6 +22,7 @@
 #include "conv_tc2.cuh"
 #include "kernels.cuh"
 #include "linattn_tc.cuh"
+#include "unet.cuh"
 #include "encoder.cuh"
 #include "vae.cuh"
 #include "ldm.cuh"
@@ -43,827 +39,7 @@ using namespace nope;
 namespace {
 
 constexpr int kAbiVersion = 2;
-constexpr int kHeadsHidden = 128;  // 4 heads x 32 (model_utils.py:368,394)
 
-// w: [rows][Kp] fp16, K = cin x taps
-struct ConvLayer : ConvLayerBase {
-  int mode = 0;  // 0: 3x3 pad1, 1: 1x1, 2: unshuffle+1x1, 3: nearest-x2 upsample + 3x3 (folded)
-  int Kp = 0;             // packed row length: K (fp16 weights) or 2K (W_hi | W_lo, precision >= 1)
-  // pre-norm folded into this (bias-free 1x1) layer: weights hold W diag(gamma); see GnFuse::pre_*
-  float* pre_w1 = nullptr;
-  float* pre_wb = nullptr;
-};
-
-struct NormLayer {
-  float* gamma = nullptr;
-  float* beta = nullptr;
-  int C = 0, G = 1;
-};
-
-// NHWC fp16 activation [n_img, S, S, C]; `lo` carries the fp16 remainder x - fp16(x) in the
-// split-precision mode (nullptr otherwise)
-struct Act {
-  __half* hi = nullptr;
-  __half* lo = nullptr;
-  int C = 0;
-  Act() {}
-  Act(__half* h, int c, __half* l = nullptr) : hi(h), lo(l), C(c) {}
-};
-
-// what the fused epilogue applies after the convolution (ResnetBlock / Block / to_out)
-struct GnSpec {
-  const NormLayer* norm = nullptr;   // nullptr: no normalisation
-  bool silu = false;
-  int pb_offset = -1;                // pose-projection columns of this block, -1: none
-  Act res;                           // residual (hi == nullptr: none)
-  int res_div = 0, res_base = 0;     // residual image = (res_base + img) / res_div (hoisted prefix)
-  float2* emit = nullptr;            // GroupNorm(1) partial sums of the output for a following pre-norm
-  const float2* pre_stats = nullptr; // folded pre-norm: partial sums of the INPUT images ([img][pre_parts])
-  int pre_parts = 0;
-};
-
-// bump allocator over one device slab (base == nullptr: size computation only)
-struct Bump {
-  uint8_t* base = nullptr;
-  size_t off = 0;
-  template <typename T> void take(T** out, size_t n) {
-    off = (off + 255) & ~static_cast<size_t>(255);
-    if (base) *out = reinterpret_cast<T*>(base + off);     // size-only passes leave the engine untouched
-    off += n * sizeof(T);
-  }
-};
-
-}  // namespace
-
-struct nope_unet {
-  static constexpr const char* kName = "UNet";
-  int dim = 0, Cl = 0, S0 = 0, rot_dim = 6, cemb = 0, device = 0, num_sms = 132;
-  int dims[5] = {0, 0, 0, 0, 0};
-  bool finalized = false;
-  // 0: fp16 operands; 1: exact weights (W_hi + W_lo K-segments, 2x the MMA work); 2: split precision
-  // (exact weights + activations carried as hi + lo: A_hi W_hi + A_hi W_lo + A_lo W_hi, 3x);
-  // 3: bf16 operands and activations (8-bit mantissa: its own, looser tolerance)
-  int precision = 0;
-  int attn_impl = 0;         // LinearAttention core: 0 wgmma (token counts >= 128), 1 CUDA cores
-  int metric = 0;            // NOPE_METRIC_* of the fused scoring
-  float occ_threshold = 0.2f;
-  int chunk = 642;
-  int64_t launches = 0;
-
-  StagedWeights staged;
-
-  std::map<std::string, ConvLayer> convs;
-  std::map<std::string, NormLayer> norms;
-  std::map<std::string, int> pb_off;
-  int P = 0;  // total pose-projection width
-  ConvLayer poseproj;
-  float *pose_w = nullptr, *pose_b = nullptr, *init_w = nullptr, *init_b = nullptr,
-        *final_w = nullptr, *final_b = nullptr;
-  DeviceAllocs mem;  // every weight buffer
-
-  // workspace: one slab, either caller-provided (nope_unet_set_workspace) or owned
-  int cap = 0, cap_ref = 0;
-  uint8_t* ws_base = nullptr;
-  size_t ws_bytes = 0;
-  bool ws_external = false;
-  bool ws_fresh = false;            // counters not zeroed yet
-  Act sk[4][2];
-  Act TB, TC, TD, XA, XB, RB;
-  __half *cs = nullptr, *pb = nullptr;
-  Act x0, g1;                       // per-reference pre-stage
-  float2* SB = nullptr;           // GroupNorm(1) partial sums a fused epilogue emits for the next pre-norm
-  uint2* xpart = nullptr;         // fused GroupNorm: cross-tile partial sums, {value, epoch} words
-  size_t xpart_words = 0;
-  unsigned gn_epoch = 0;          // tag of the last fused launch that exchanged partial sums
-  int* ref_of = nullptr;
-  float* score_partial = nullptr;
-  float* sim_buf = nullptr;
-
-  TmapCache tmaps;
-
-  // per-launch CUDA-event profile of the convolution kernel (bench.py roofline)
-  bool profile = false;
-  std::vector<cudaEvent_t> prof_ev;      // pairs
-  std::vector<double> prof_flops;
-
-  // debug tap
-  std::string tap_name;
-  float* tap_out = nullptr;
-  int64_t tap_cap = 0;
-  int tap_C = 0, tap_S = 0;
-  bool tap_hit = false;
-
-  ~nope_unet() {
-    if (ws_base && !ws_external) cudaFree(ws_base);
-    for (cudaEvent_t e : prof_ev) cudaEventDestroy(e);
-  }
-  bool split() const { return precision == 2 || precision == 4; }
-  // precision 4: the residual stream, skip tensors and resampled maps keep their (hi, lo) pair, the tensor INSIDE a
-  // ResnetBlock (block1's output h, consumed only by block2's convolution) is a single fp16 value -- block2 runs two
-  // products per tap instead of three.  CPU budget (tools/precision_sim.py): h alone costs 4.3e-4 on the embeddings.
-  bool h_lo() const { return precision == 2; }
-  bool bf() const { return precision == 3; }     // bf16 storage (BASELINE configs[2]); fp16 otherwise
-
-  // ------------------------------------------------------------------ schema
-  void expect(const std::string& k, std::vector<int64_t> s) { staged.expect(k, std::move(s)); }
-  void expect_resblock(const std::string& p, int cin, int cout, bool mlp = true) {
-    if (mlp) {
-      expect(p + ".mlp.1.weight", {cout, cemb});
-      expect(p + ".mlp.1.bias", {cout});
-    }
-    expect(p + ".block1.proj.weight", {cout, cin, 3, 3});
-    expect(p + ".block1.proj.bias", {cout});
-    expect(p + ".block1.norm.weight", {cout});
-    expect(p + ".block1.norm.bias", {cout});
-    expect(p + ".block2.proj.weight", {cout, cout, 3, 3});
-    expect(p + ".block2.proj.bias", {cout});
-    expect(p + ".block2.norm.weight", {cout});
-    expect(p + ".block2.norm.bias", {cout});
-    if (cin != cout) {
-      expect(p + ".res_conv.weight", {cout, cin, 1, 1});
-      expect(p + ".res_conv.bias", {cout});
-    }
-  }
-  void expect_linattn(const std::string& p, int d) {
-    expect(p + ".fn.fn.to_qkv.weight", {3 * kHeadsHidden, d, 1, 1});
-    expect(p + ".fn.fn.to_out.0.weight", {d, kHeadsHidden, 1, 1});
-    expect(p + ".fn.fn.to_out.0.bias", {d});
-    expect(p + ".fn.fn.to_out.1.weight", {d});
-    expect(p + ".fn.fn.to_out.1.bias", {d});
-    expect(p + ".fn.norm.weight", {d});
-    expect(p + ".fn.norm.bias", {d});
-  }
-  // state_dict schema of the reference UNet (u_net.py:27-158), encoder excluded.
-  void build_schema() {
-    expect("pose_mlp.0.weight", {cemb, rot_dim});
-    expect("pose_mlp.0.bias", {cemb});
-    expect("init_conv.weight", {dim, Cl, 3, 3});
-    expect("init_conv.bias", {dim});
-    for (int i = 0; i < 4; ++i) {
-      const int din = dims[i], dout = dims[i + 1];
-      const std::string p = "downs." + std::to_string(i);
-      expect_resblock(p + ".0", din, din);
-      expect_resblock(p + ".1", din, din);
-      expect_linattn(p + ".2", din);
-      if (i < 3) {
-        expect(p + ".3.1.weight", {dout, din * 4, 1, 1});
-        expect(p + ".3.1.bias", {dout});
-      } else {
-        expect(p + ".3.weight", {dout, din, 3, 3});
-        expect(p + ".3.bias", {dout});
-      }
-    }
-    const int mid = dims[4];
-    expect("mid_attn.fn.fn.to_qkv.weight", {3 * kHeadsHidden, mid, 1, 1});
-    expect("mid_attn.fn.fn.to_out.weight", {mid, kHeadsHidden, 1, 1});
-    expect("mid_attn.fn.fn.to_out.bias", {mid});
-    expect("mid_attn.fn.norm.weight", {mid});
-    expect("mid_attn.fn.norm.bias", {mid});
-    expect_resblock("mid_block1", mid, mid);
-    expect_resblock("mid_block2", mid, mid);
-    for (int j = 0; j < 4; ++j) {
-      const int din = dims[3 - j], dout = dims[4 - j];
-      const std::string p = "ups." + std::to_string(j);
-      expect_resblock(p + ".0", dout + din, dout);
-      expect_resblock(p + ".1", dout + din, dout);
-      expect_linattn(p + ".2", dout);
-      if (j < 3) {
-        expect(p + ".3.1.weight", {din, dout, 3, 3});
-        expect(p + ".3.1.bias", {din});
-      } else {
-        expect(p + ".3.weight", {din, dout, 3, 3});
-        expect(p + ".3.bias", {din});
-      }
-    }
-    expect_resblock("final_res_block", 2 * dim, dim);
-    expect_resblock("final_conv.0", dim, dim);  // owns an unused mlp.1 (u_net.py:154-157)
-    expect("final_conv.1.weight", {Cl, dim, 1, 1});
-    expect("final_conv.1.bias", {Cl});
-  }
-
-  // ------------------------------------------------------------------ weights
-  int upload_f32(const std::string& key, float** out) { return mem.upload(out, staged.at(key).data); }
-  // pack one conv weight (+ bias) into a ConvLayer.  mode 3 (nearest-x2 upsample + conv3x3,
-  // HardUpsample) first folds the 3x3 kernel into four 2x2 parity kernels (fold_upconv_kernel).
-  // precision >= 1 appends the fp16 remainders as a second K-block: rows are [W_hi (K) | W_lo (K)].
-  int make_conv(const std::string& name, const std::string& wkey, const std::string& bkey, int mode) {
-    const HostTensor& W = staged.at(wkey);
-    const auto& sh = W.shape;
-    ConvLayer L;
-    L.mode = mode;
-    L.cout = (int)sh[0];
-    const int rows = mode == 3 ? 4 * L.cout : L.cout;   // weight-matrix rows
-    const int taps = mode == 0 ? 9 : (mode == 1 ? 1 : 4);
-    L.cin = mode == 2 ? (int)sh[1] / 4 : (int)sh[1];
-    L.K = L.cin * taps;
-    const bool wlo = precision == 1 || precision == 2 || precision == 4;
-    L.Kp = wlo ? 2 * L.K : L.K;
-    NOPE_CHECK(L.cin % 64 == 0, wkey + ": input channels must be a multiple of 64");
-    L.bn = pick_bn(L.cout);
-    NOPE_CHECK(L.bn != 0, wkey + ": output channels must be a multiple of 64");
-    NOPE_CHECK(mode != 3 || (sh.size() == 4 && sh[2] == 3 && sh[3] == 3), wkey + ": expected a 3x3 kernel");
-    if (mem.alloc(&L.w, (size_t)rows * L.Kp)) return -1;
-    if (pack_conv_weight(W.data.data(), L.w, L.cout, L.cin, taps, mode == 3, L.Kp, 0, wlo ? L.K : 0, bf() ? 1 : 0, 0))
-      return -1;
-    if (!bkey.empty()) {
-      if (upload_f32(bkey, &L.bias)) return -1;
-    }
-    if (make_weight_map(&L.wmap, L.w, rows, L.Kp, L.bn)) return -1;
-    convs[name] = L;
-    return 0;
-  }
-  int make_norm(const std::string& name, const std::string& prefix, int G) {
-    NormLayer n;
-    n.C = (int)staged.at(prefix + ".weight").shape[0];
-    n.G = G;
-    NOPE_CHECK(n.C % (8 * G) == 0, prefix + ": channels per group must be a multiple of 8");
-    if (upload_f32(prefix + ".weight", &n.gamma)) return -1;
-    if (upload_f32(prefix + ".bias", &n.beta)) return -1;
-    norms[name] = n;
-    return 0;
-  }
-  int make_resblock(const std::string& p) {
-    if (make_conv(p + ".block1", p + ".block1.proj.weight", p + ".block1.proj.bias", 0)) return -1;
-    if (make_conv(p + ".block2", p + ".block2.proj.weight", p + ".block2.proj.bias", 0)) return -1;
-    if (make_norm(p + ".norm1", p + ".block1.norm", 8)) return -1;
-    if (make_norm(p + ".norm2", p + ".block2.norm", 8)) return -1;
-    if (staged.has(p + ".res_conv.weight"))
-      if (make_conv(p + ".res", p + ".res_conv.weight", p + ".res_conv.bias", 1)) return -1;
-    return 0;
-  }
-  // to_qkv with the PreNorm GroupNorm(1) folded in (model_utils.py:226-234, 399): packed weights
-  // W' = W diag(gamma); w1[c] = sum_k W'[c,k] over the values the tensor core actually multiplies
-  // (fp16 hi, + lo in the exact-weight modes); wb[c] = sum_k W[c,k] beta[k].
-  int make_qkv_folded(const std::string& name, const std::string& wkey, const std::string& nprefix) {
-    const HostTensor& W = staged.at(wkey);
-    const std::vector<float>& gm = staged.at(nprefix + ".weight").data;
-    const std::vector<float>& bt = staged.at(nprefix + ".bias").data;
-    const int rows = (int)W.shape[0], cin = (int)W.shape[1];
-    HostTensor Wf;
-    Wf.shape = W.shape;
-    Wf.data.resize(W.data.size());
-    std::vector<float> w1(rows), wb(rows);
-    for (int o = 0; o < rows; ++o) {
-      double s1 = 0.0, sb = 0.0;
-      for (int k = 0; k < cin; ++k) {
-        const float w = W.data[(size_t)o * cin + k];
-        const float wf = w * gm[k];
-        Wf.data[(size_t)o * cin + k] = wf;
-        if (precision == 3) {
-          uint32_t u;
-          std::memcpy(&u, &wf, 4);
-          u = (u + 0x7fffu + ((u >> 16) & 1u)) & 0xffff0000u;        // round to nearest even bf16
-          float r;
-          std::memcpy(&r, &u, 4);
-          s1 += (double)r;
-        } else {
-          const __half hi = __float2half_rn(wf);
-          s1 += (double)__half2float(hi);
-          if (precision >= 1) s1 += (double)__half2float(__float2half_rn(wf - __half2float(hi)));
-        }
-        sb += (double)w * (double)bt[k];
-      }
-      w1[o] = (float)s1;
-      wb[o] = (float)sb;
-    }
-    const std::string tmpkey = "__folded." + name;
-    staged.put(tmpkey, std::move(Wf));
-    if (make_conv(name, tmpkey, "", 1)) return -1;
-    ConvLayer& L = convs[name];
-    return mem.upload(&L.pre_w1, w1) || mem.upload(&L.pre_wb, wb) ? -1 : 0;
-  }
-  int make_linattn(const std::string& p) {
-    if (make_qkv_folded(p + ".qkvf", p + ".fn.fn.to_qkv.weight", p + ".fn.norm")) return -1;
-    if (make_conv(p + ".out", p + ".fn.fn.to_out.0.weight", p + ".fn.fn.to_out.0.bias", 1)) return -1;
-    if (make_norm(p + ".outnorm", p + ".fn.fn.to_out.1", 1)) return -1;
-    return 0;
-  }
-  // concatenate the 19 pose projections (model_utils.py:261-263) into one [P, cemb] GEMM
-  int make_poseproj() {
-    std::vector<std::string> blocks;
-    for (int i = 0; i < 4; ++i)
-      for (int b = 0; b < 2; ++b) blocks.push_back("downs." + std::to_string(i) + "." + std::to_string(b));
-    blocks.push_back("mid_block1");
-    blocks.push_back("mid_block2");
-    for (int j = 0; j < 4; ++j)
-      for (int b = 0; b < 2; ++b) blocks.push_back("ups." + std::to_string(j) + "." + std::to_string(b));
-    blocks.push_back("final_res_block");
-    std::vector<float> w, bias;
-    P = 0;
-    for (const auto& b : blocks) {
-      const HostTensor& hw = staged.at(b + ".mlp.1.weight");
-      const HostTensor& hb = staged.at(b + ".mlp.1.bias");
-      pb_off[b] = P;
-      P += (int)hw.shape[0];
-      w.insert(w.end(), hw.data.begin(), hw.data.end());
-      bias.insert(bias.end(), hb.data.begin(), hb.data.end());
-    }
-    HostTensor tw;
-    tw.shape = {P, cemb, 1, 1};
-    tw.data = std::move(w);
-    HostTensor tb;
-    tb.shape = {P};
-    tb.data = std::move(bias);
-    staged.put("__poseproj.weight", std::move(tw));
-    staged.put("__poseproj.bias", std::move(tb));
-    if (make_conv("__poseproj", "__poseproj.weight", "__poseproj.bias", 1)) return -1;
-    poseproj = convs["__poseproj"];
-    return 0;
-  }
-
-  // packs the staged weights (engine_finalize: every schema key is present, device selected)
-  int finalize() {
-    if (upload_f32("pose_mlp.0.weight", &pose_w) || upload_f32("pose_mlp.0.bias", &pose_b) ||
-        upload_f32("init_conv.weight", &init_w) || upload_f32("init_conv.bias", &init_b) ||
-        upload_f32("final_conv.1.weight", &final_w) || upload_f32("final_conv.1.bias", &final_b))
-      return -1;
-    for (int i = 0; i < 4; ++i) {
-      const std::string p = "downs." + std::to_string(i);
-      if (make_resblock(p + ".0") || make_resblock(p + ".1") || make_linattn(p + ".2")) return -1;
-      if (i < 3) {
-        if (make_conv(p + ".3", p + ".3.1.weight", p + ".3.1.bias", 2)) return -1;
-      } else {
-        if (make_conv(p + ".3", p + ".3.weight", p + ".3.bias", 0)) return -1;
-      }
-    }
-    if (make_resblock("mid_block1") || make_resblock("mid_block2")) return -1;
-    if (make_qkv_folded("mid_attn.qkvf", "mid_attn.fn.fn.to_qkv.weight", "mid_attn.fn.norm")) return -1;
-    if (make_conv("mid_attn.out", "mid_attn.fn.fn.to_out.weight", "mid_attn.fn.fn.to_out.bias", 1))
-      return -1;
-    for (int j = 0; j < 4; ++j) {
-      const std::string p = "ups." + std::to_string(j);
-      if (make_resblock(p + ".0") || make_resblock(p + ".1") || make_linattn(p + ".2")) return -1;
-      if (j < 3) {
-        if (make_conv(p + ".3", p + ".3.1.weight", p + ".3.1.bias", 3)) return -1;
-      } else {
-        if (make_conv(p + ".3", p + ".3.weight", p + ".3.bias", 0)) return -1;
-      }
-    }
-    if (make_resblock("final_res_block") || make_resblock("final_conv.0")) return -1;
-    return make_poseproj();
-  }
-
-  // ------------------------------------------------------------------ workspace
-  // One slab carved by a bump allocator: ~4.7 MB per hypothesis at u_net_dim 192 (8.6 MB in the split-precision
-  // modes), nearly all of it the 8 skip tensors, 3 temporaries of 786 KB and 3 feature maps of 393 KB.
-  // layout(b) assigns every buffer for capacities (c hypotheses, r references).
-  void take_act(Bump& b, Act* a, size_t n, int C, bool with_lo) {
-    if (b.base) {
-      a->C = C;
-      a->lo = nullptr;
-    }
-    b.take(&a->hi, n);
-    if (with_lo) b.take(&a->lo, n);
-  }
-  size_t layout(Bump& b, int c_hyp, int c_ref, int n_total_scores) {
-    const size_t c = (size_t)c_hyp, r = (size_t)c_ref;
-    const bool lo = precision == 2 || precision == 4;
-    // temporaries hold the widest full-resolution tensor: a concat-conv output (<= 2*dim
-    // channels) or the attention qkv tensor (3 x 128 channels, independent of dim)
-    const size_t big = (size_t)S0 * S0 * std::max(dim * 2, 3 * kHeadsHidden);
-    const size_t xsz = (size_t)S0 * S0 * dim;      // one full-resolution feature map
-    for (int i = 0; i < 4; ++i) {
-      const int s = S0 >> i;
-      for (int k = 0; k < 2; ++k) take_act(b, &sk[i][k], c * s * s * dims[i], dims[i], lo);
-    }
-    take_act(b, &TB, c * big, 0, lo);
-    take_act(b, &TC, c * big, 0, lo);
-    take_act(b, &TD, c * big, 0, false);
-    take_act(b, &XA, c * xsz, 0, lo);
-    take_act(b, &XB, c * xsz, 0, lo);
-    take_act(b, &RB, c * xsz, dim, lo);
-    b.take(&cs, c * cemb);
-    b.take(&pb, c * (size_t)P);
-    take_act(b, &x0, r * xsz, dim, lo);
-    take_act(b, &g1, r * xsz, dim, lo);
-    const size_t m = std::max(c, r);
-    b.take(&ref_of, m);
-    b.take(&SB, m * 8);
-    // <= 64 (slot, image, group) entries of two {value, epoch} words per image
-    if (b.base) xpart_words = (m + 8) * 64 * 2;
-    b.take(&xpart, (m + 8) * 64 * 2);
-    const int nslab = (S0 * S0 + kFinalPix - 1) / kFinalPix;
-    b.take(&score_partial, (size_t)n_total_scores * nslab * kScoreParts);
-    b.take(&sim_buf, (size_t)n_total_scores);
-    return b.off;
-  }
-  size_t workspace_bytes(int c_hyp, int c_ref, int n_scores) {
-    Bump b;
-    return layout(b, c_hyp, c_ref, n_scores) + 256;
-  }
-  int scores_cap = 0;
-  int ensure_workspace(int need_cap, int need_ref, int need_scores = 0) {
-    if (need_cap <= cap && need_ref <= cap_ref && need_scores <= scores_cap) return 0;
-    NOPE_CHECK(!ws_external, "the caller-provided workspace is too small for this sweep "
-                             "(nope_unet_workspace_bytes / nope_unet_set_workspace)");
-    NOPE_CUDA(cudaDeviceSynchronize());
-    if (ws_base) cudaFree(ws_base);
-    ws_base = nullptr;
-    const int c = std::max(cap, need_cap), r = std::max(cap_ref, need_ref), sc = std::max(scores_cap, need_scores);
-    const size_t bytes = workspace_bytes(c, r, sc);
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&ws_base), bytes));
-    ws_bytes = bytes;
-    return adopt(c, r, sc);
-  }
-  int adopt(int c, int r, int sc) {
-    tmaps.clear();
-    cap = c; cap_ref = r; scores_cap = sc;
-    Bump b;
-    b.base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws_base) + 255) & ~static_cast<uintptr_t>(255));
-    layout(b, c, r, sc);
-    ws_fresh = true;
-    return 0;
-  }
-  int set_workspace(void* ptr, size_t bytes, int c, int r, int sc) {
-    NOPE_CHECK(ptr && c >= 1 && r >= 1, "bad workspace arguments");
-    NOPE_CHECK(bytes >= workspace_bytes(c, r, sc), "workspace buffer smaller than nope_unet_workspace_bytes");
-    if (ws_base && !ws_external) {
-      NOPE_CUDA(cudaDeviceSynchronize());
-      cudaFree(ws_base);
-    }
-    ws_base = static_cast<uint8_t*>(ptr);
-    ws_bytes = bytes;
-    ws_external = true;
-    return adopt(c, r, sc);
-  }
-  // the tile-sync words of a fresh slab carry epoch 0, which no launch uses
-  int prepare_stream(cudaStream_t st) {
-    if (ws_fresh) {
-      NOPE_CUDA(cudaMemsetAsync(xpart, 0, xpart_words * sizeof(uint2), st));
-      ws_fresh = false;
-    }
-    return 0;
-  }
-
-  // ------------------------------------------------------------------ op launchers
-  // out[n_img, So, So, cout] = conv(L, in0 (++ in1)).  The K loop walks, per filter tap and source
-  // tensor, up to three products: A_hi W_hi, A_hi W_lo (precision >= 1), A_lo W_hi (sources that
-  // carry a remainder).  `gs` selects the fused GroupNorm epilogue; `stats` (plain epilogue only) receives the
-  // GroupNorm partial sums of the output in the ConvParams::stats layout (nope_op_conv_gn checks them).
-  int conv(const ConvLayer& L, const Act& in0, const Act& in1, const Act& out, int So, int n_img, int cap_img,
-           cudaStream_t st, const GnSpec* gs = nullptr, float2* stats = nullptr) {
-    const int c0 = in0.C, c1 = in1.hi ? in1.C : 0;
-    NOPE_CHECK(c0 + c1 == L.cin, "conv: channel mismatch");
-    NOPE_CHECK(L.mode != 3 || (in1.hi == nullptr && So % 2 == 0), "upsample conv takes one source");
-    NOPE_CHECK(L.mode != 2 || in1.hi == nullptr, "unshuffle conv takes one source");
-    ++launches;
-    // the folded upsample's So is the OUTPUT side (2x the source side); tiles and input maps use the source geometry
-    const int Sg = L.mode == 3 ? So / 2 : So;
-    TileGeom g;
-    if (make_geom(Sg, Sg, &g)) return -1;
-    ConvBuilder b(tmaps, g, cap_img);
-    ConvParams& p = b.p;
-    ConvTap taps[9];
-    int n_taps = 0;
-    if (L.mode == 3) {
-      for (int a = 0; a < 2; ++a)
-        for (int c = 0; c < 2; ++c) taps[n_taps++] = ConvTap{0, a - 1, c - 1};
-    } else if (L.mode == 2) {
-      for (int t = 0; t < 4; ++t) taps[n_taps++] = stride2_tap(t >> 1, t & 1);
-    } else if (L.mode == 0) {
-      for (int t = 0; t < 9; ++t) taps[n_taps++] = ConvTap{0, t / 3 - 1, t % 3 - 1};
-    } else {
-      taps[n_taps++] = ConvTap{0, 0, 0};
-    }
-    // activation maps: in0 (hi, lo) per lattice, in1 (hi, lo)
-    const int n_lat = L.mode == 2 ? 4 : 1;
-    int h0[4] = {}, l0[4] = {}, h1 = 0, l1 = 0;
-    for (int lat = 0; lat < n_lat; ++lat) h0[lat] = b.map(in0.hi, c0, L.mode == 2 ? lat : -1);
-    if (in1.hi) h1 = b.map(in1.hi, c1);
-    if (in0.lo)
-      for (int lat = 0; lat < n_lat; ++lat) l0[lat] = b.map(in0.lo, c0, L.mode == 2 ? lat : -1);
-    const bool alo1 = in1.hi && in1.lo;
-    if (alo1) l1 = b.map(in1.lo, c1);
-    // per filter tap and source: A_hi W_hi, A_hi W_lo (packed rows carry W_lo at column K + ...), A_lo W_hi
-    const bool wlo = L.Kp > L.K;
-    for (int ti = 0; ti < n_taps; ++ti) {
-      const ConvTap& t = taps[ti];
-      const int wcol = ti * L.cin + 1;      // ConvSeg::wcol1 of the tap's first source
-      b.seg(h0[t.lat], t.dy, t.dx, c0 / 64, wcol);
-      if (in1.hi) b.seg(h1, t.dy, t.dx, c1 / 64, wcol + c0);
-      if (wlo) {
-        b.seg(h0[t.lat], t.dy, t.dx, c0 / 64, L.K + wcol);
-        if (in1.hi) b.seg(h1, t.dy, t.dx, c1 / 64, L.K + wcol + c0);
-      }
-      if (in0.lo) b.seg(l0[t.lat], t.dy, t.dx, c0 / 64, wcol);
-      if (alo1) b.seg(l1, t.dy, t.dx, c1 / 64, wcol + c0);
-    }
-    if (b.finish(L, out.hi, L.cout, n_img, L.mode == 3 ? 4 : 1)) return -1;
-    p.bf16 = bf() ? 1 : 0;
-    p.stats = stats;
-    NOPE_CHECK(!(stats && L.mode == 3), "fused statistics are not available on the upsample conv");
-    if (gs) {
-      NOPE_CHECK(L.mode != 3 && !stats, "fused GroupNorm epilogue: no upsample, no plain statistics");
-      GnFuse& f = p.gn;
-      const int hw = So * So;
-      f.G = gs->norm ? gs->norm->G : 0;
-      if (gs->norm) {
-        NOPE_CHECK(gs->norm->C == L.cout, "fused GroupNorm: channel mismatch");
-        f.gamma = gs->norm->gamma;
-        f.beta = gs->norm->beta;
-        f.cpg = L.cout / f.G;
-        NOPE_CHECK(f.cpg % 8 == 0 && (f.cpg >= L.bn ? f.cpg % L.bn == 0 : L.bn % f.cpg == 0),
-                   "fused GroupNorm: groups must tile the channel tiles");
-      } else {
-        f.cpg = L.cout;
-      }
-      f.gpt = std::max(1, L.bn / f.cpg);
-      f.tpg = std::max(1, f.cpg / L.bn);
-      f.mt = std::max(1, g.tiles_per_img);
-      f.ipt = g.tiles_per_img > 0 ? 1 : g.b_cnt;
-      f.expected = f.G > 0 ? f.mt * f.tpg : 1;
-      int sh = 0;
-      while ((1 << sh) < hw) ++sh;
-      NOPE_CHECK((1 << sh) == hw, "fused GroupNorm: H*W must be a power of two");
-      f.hw_shift = sh;
-      f.inv_cnt = 1.0f / ((float)hw * (float)f.cpg);
-      f.eps = 1e-5f;
-      f.silu = gs->silu ? 1 : 0;
-      f.pb = gs->pb_offset >= 0 ? pb : nullptr;
-      f.pb_stride = P;
-      f.pb_off = std::max(gs->pb_offset, 0);
-      f.n_img = n_img;
-      if (gs->res.hi) {
-        NOPE_CHECK(gs->res.C == L.cout, "fused residual: channel mismatch");
-        NOPE_CHECK(gs->res_div == 0 || g.tiles_per_img > 0, "residual image mapping needs >= 128-pixel images");
-        const CUtensorMap* m = nullptr;
-        if (tmaps.get(&m, gs->res.hi, gs->res_div > 0 ? cap_ref : cap_img, L.cout, g, -1)) return -1;
-        p.rmap = *m;
-        f.has_res = 1;
-        f.res_lo = gs->res.lo;
-      } else {
-        p.rmap = p.omap[0];
-      }
-      f.res_div = gs->res_div;
-      f.res_base = gs->res_base;
-      if (gs->pre_stats) {
-        NOPE_CHECK(!gs->norm && L.pre_w1 && L.pre_wb && L.mode == 1 && !L.bias, "pre-norm fold: bias-free 1x1 layer with folded weights");
-        f.pre_stats = gs->pre_stats;
-        f.pre_parts = gs->pre_parts;
-        f.pre_inv_cnt = 1.0f / ((float)hw * (float)L.cin);
-        f.pre_w1 = L.pre_w1;
-        f.pre_wb = L.pre_wb;
-      }
-      f.out_lo = out.lo;
-      f.emit = gs->emit;
-      f.emit_parts = f.mt * p.n_tiles;
-      NOPE_CHECK(f.ipt * f.gpt <= 64 && f.ipt <= 8, "fused GroupNorm: tile holds too many (image, group) pairs");
-      if (f.expected > 1) {
-        const size_t n_sg = (size_t)(p.m_tiles / f.mt + 1) * (p.n_tiles / f.tpg);
-        NOPE_CHECK(xpart && f.expected * f.ipt * f.gpt * 2 <= 256, "fused GroupNorm: sync group too large");
-        NOPE_CHECK(n_sg * f.expected * f.ipt * f.gpt * 2 <= xpart_words, "fused GroupNorm: partial-sum buffer too small");
-        f.xpart = xpart;
-        if (++gn_epoch == 0) ++gn_epoch;     // 0 is the tag of a fresh buffer
-        f.epoch = gn_epoch;
-      }
-    } else if (out.lo) {
-      p.out_lo = out.lo;                // extras epilogue writes the remainder
-    }
-    auto launch = [&]() {
-      return gs ? launch_conv_gn(p, L.bn, num_sms, st) : launch_conv_tc2(p, L.bn, num_sms, st);
-    };
-    if (!profile) return launch();
-    cudaEvent_t e0, e1;
-    NOPE_CUDA(cudaEventCreate(&e0));
-    NOPE_CUDA(cudaEventCreate(&e1));
-    NOPE_CUDA(cudaEventRecord(e0, st));
-    const int rc = launch();
-    NOPE_CUDA(cudaEventRecord(e1, st));
-    prof_ev.push_back(e0);
-    prof_ev.push_back(e1);
-    // executed FLOPs: mode 3 runs 4 parity GEMMs of K = 4 Cin over the source-resolution pixels;
-    // the split-precision modes execute 2x / 3x the K-steps of the fp16 mode
-    prof_flops.push_back(2.0 * (double)n_img * So * So * (double)L.cout * (double)p.ksteps * 64.0);
-    prof_alg.push_back(2.0 * (double)n_img * So * So * (double)L.cout * (double)L.K);
-    prof_shape.push_back(make_int4(So, L.mode, L.cout, L.K));
-    return rc;
-  }
-  std::vector<double> prof_alg;     // algorithmic (fp16-mode) FLOPs of the same launches
-  std::vector<int4> prof_shape;     // (GEMM resolution, mode 0 3x3 / 1 1x1 / 2 unshuffle / 3 folded upsample, Cout, K)
-
-  // partial sums per image emitted by the fused epilogue: one per (M-tile of the image, N-tile)
-  static int fused_emit_parts(int S, int C) {
-    return std::max(1, S * S / kBM) * (C / pick_bn(C));
-  }
-
-  int tap(const char* name, const Act& buf, int C, int S, int n, cudaStream_t st) {
-    if (tap_out == nullptr || tap_name != name || tap_hit) return 0;
-    NOPE_CHECK((int64_t)n * C * S * S <= tap_cap, "debug tap: output buffer too small");
-    nhwc_f16_to_nchw_f32_kernel<<<ew_grid((long long)n * C * S * S), 256, 0, st>>>(buf.hi, tap_out, n, C, S * S,
-                                                                                   buf.lo, bf());
-    NOPE_CUDA(cudaGetLastError());
-    tap_C = C; tap_S = S; tap_hit = true;
-    return 0;
-  }
-
-  // ResnetBlock.forward (model_utils.py:271-279) on NHWC fp16:
-  // conv1 [GN8 + SiLU + pose bias] -> h ; (res_conv) ; conv2 [GN8 + SiLU + residual] -> out:
-  // two or three launches, no tensor is written un-normalised.  `emit_g1` makes conv2's epilogue also
-  // emit the GroupNorm(1, C) statistics of the block output into SB for a following attention pre-norm.
-  int resblock(const std::string& p, const Act& in0, const Act& in1, const Act& out, int S, int n, bool pose,
-               cudaStream_t st, bool emit_g1 = false, int res_div = 0, int res_base = 0, const Act* hoisted_h = nullptr) {
-    const ConvLayer& b1 = convs.at(p + ".block1");
-    const ConvLayer& b2 = convs.at(p + ".block2");
-    const int co = b1.cout;
-    auto it = convs.find(p + ".res");
-    Act h(TB.hi, co, h_lo() ? TB.lo : nullptr);
-    if (hoisted_h) {
-      h = *hoisted_h;
-      if (!h_lo()) h.lo = nullptr;
-    } else {
-      GnSpec s1;
-      s1.norm = &norms.at(p + ".norm1");
-      s1.silu = true;
-      s1.pb_offset = pose ? pb_off.at(p) : -1;
-      if (conv(b1, in0, in1, h, S, n, cap, st, &s1)) return -1;
-    }
-    GnSpec s2;
-    s2.norm = &norms.at(p + ".norm2");
-    s2.silu = true;
-    if (it != convs.end()) {
-      Act r(TC.hi, co, split() ? TC.lo : nullptr);
-      // plain epilogue: routing this 1x1 through the GroupNorm-fused role split measured 8 % slower
-      if (conv(it->second, in0, in1, r, S, n, cap, st)) return -1;
-      s2.res = r;
-    } else {
-      NOPE_CHECK(in1.hi == nullptr && in0.C == co, "resblock: identity residual needs Cin == Cout");
-      s2.res = in0;
-      s2.res_div = res_div;
-      s2.res_base = res_base;
-    }
-    s2.emit = emit_g1 ? SB : nullptr;
-    return conv(b2, h, Act(), out, S, n, cap, st, &s2);
-  }
-
-  // Residual(PreNorm(LinearAttention)) (model_utils.py:393-418).  x's GroupNorm(1) statistics
-  // were emitted into SB by the producer of x; to_out[1] (GroupNorm(1)) + the residual add run in the
-  // to_out convolution's epilogue.
-  int linattn(const std::string& p, const Act& x, const Act& out, int C, int S, int n, cudaStream_t st) {
-    // pre-norm folded into to_qkv: x is read once, un-normalised, by the 1x1 itself
-    GnSpec sq;
-    sq.pre_stats = SB;
-    sq.pre_parts = fused_emit_parts(S, C);
-    if (conv(convs.at(p + ".qkvf"), x, Act(), Act(TD.hi, 3 * kHeadsHidden), S, n, cap, st, &sq)) return -1;
-    if (attn_impl == 0 && S * S >= kBM) {
-      if (launch_linattn_tc(TD.hi, TC.hi, n, S * S, num_sms, st, bf())) return -1;
-    } else {
-      NOPE_CUDA(launch_pdl(linattn_kernel, dim3(4, n), dim3(kLinAttnThreads), 0, st, TD.hi, TC.hi, S * S, bf()));
-    }
-    ++launches;
-    // to_out (K = 128: two K-steps per tile) + GroupNorm(1) + residual in one kernel.  This takes the same time as
-    // the plain convolution plus one normalisation pass (18.80 vs 18.71 ms over the step under ncu), and it never
-    // rounds the un-normalised output to 16 bits (full-size configs[2] scores: 0.99e-3 vs 1.06e-3)
-    GnSpec so;
-    so.norm = &norms.at(p + ".outnorm");
-    so.res = x;
-    return conv(convs.at(p + ".out"), Act(TC.hi, kHeadsHidden), Act(), out, S, n, cap, st, &so);
-  }
-
-  // Residual(PreNorm(Attention)) (model_utils.py:367-390)
-  int midattn(const Act& x, const Act& out, int C, int S, int n, cudaStream_t st) {
-    NOPE_CHECK(S * S <= 32, "bottleneck attention supports at most 32 tokens");
-    GnSpec sq;
-    sq.pre_stats = SB;
-    sq.pre_parts = fused_emit_parts(S, C);
-    if (conv(convs.at("mid_attn.qkvf"), x, Act(), Act(TD.hi, 3 * kHeadsHidden), S, n, cap, st, &sq)) return -1;
-    NOPE_CUDA(launch_pdl(midattn_kernel, dim3(n), dim3(128), 0, st, TD.hi, TC.hi, S * S, bf()));
-    ++launches;
-    GnSpec so;                 // no normalisation: out = to_out(attn) + x
-    so.res = x;
-    return conv(convs.at("mid_attn.out"), Act(TC.hi, kHeadsHidden), Act(), out, S, n, cap, st, &so);
-  }
-
-  // pose-independent prefix, once per reference image: x0 = init_conv(ref),
-  // g1 = SiLU(GN(downs.0.0.block1.proj(x0)))   (u_net.py:161; model_utils.py:272)
-  int prestage(const float* ref_feat, int B, cudaStream_t st) {
-    init_conv_kernel<<<ew_grid((long long)B * S0 * S0 * dim), 256, 0, st>>>(ref_feat, init_w, init_b, x0.hi,
-                                                                            B, Cl, S0, S0, dim, split() ? x0.lo : nullptr, bf());
-    NOPE_CUDA(cudaGetLastError());
-    ++launches;
-    const Act xin(x0.hi, dim, split() ? x0.lo : nullptr);
-    GnSpec s;
-    s.norm = &norms.at("downs.0.0.norm1");
-    s.silu = true;
-    return conv(convs.at("downs.0.0.block1"), xin, Act(), Act(g1.hi, dim, h_lo() ? g1.lo : nullptr), S0, B,
-                cap_ref, st, &s);
-  }
-
-  // UNet.forward for hypotheses [hyp0, hyp0 + n) of the flattened (b, pose) list
-  // query_feat [B, Q, Cl, hw]; score_part [B * N, Q, nslab, kScoreParts]
-  int forward_chunk(const float* poses, int hyp0, int n, int N, const float* query_feat,
-                    float* out_emb, float* score_part, cudaStream_t st, int Q = 1) {
-    const bool sp = split();
-    auto A = [&](const Act& buf, int C) { return Act(buf.hi, C, sp ? buf.lo : nullptr); };
-    // hypothesis -> reference image
-    iota_div(ref_of, hyp0, N, n, st);
-    // pose embedding + all 19 pose projections in one GEMM
-    NOPE_CUDA(launch_pdl(pose_embed_kernel, dim3(n), dim3(256), 0, st, poses + (size_t)hyp0 * rot_dim, pose_w, pose_b,
-                         cs, n, rot_dim, cemb, bf()));
-    ++launches;
-    if (conv_pose(n, st)) return -1;
-
-    // r (= init_conv output) and the hoisted block1 output, broadcast per hypothesis
-    const int hw0 = S0 * S0;
-    NOPE_CUDA(launch_pdl(bcast_add_kernel, dim3(ew_grid((long long)hw0 * dim / 8 / 4), n), dim3(256), 0, st, x0.hi, ref_of,
-                         nullptr, 0, 0, RB.hi, n, hw0, dim, sp ? x0.lo : nullptr, sp ? RB.lo : nullptr, bf()));
-    NOPE_CUDA(launch_pdl(bcast_add_kernel, dim3(ew_grid((long long)hw0 * dim / 8 / 4), n), dim3(256), 0, st, g1.hi, ref_of,
-                         pb, P, pb_off.at("downs.0.0"), TB.hi, n, hw0, dim, h_lo() ? g1.lo : nullptr,
-                         h_lo() ? TB.lo : nullptr, bf()));
-    launches += 2;
-    if (tap("init_conv", A(RB, dim), dim, S0, n, st)) return -1;
-
-    // ---- downs
-    Act cur;
-    int S = S0;
-    for (int i = 0; i < 4; ++i) {
-      const int C = dims[i];
-      const std::string p = "downs." + std::to_string(i);
-      const Act s0 = A(sk[i][0], C), s1 = A(sk[i][1], C);
-      if (i == 0) {
-        // block 0 with its block1 half hoisted: TB already holds SiLU(GN(conv(x0))) + pose bias
-        const Act h = A(TB, C);
-        if (resblock(p + ".0", A(x0, C), Act(), s0, S, n, true, st, false, N, hyp0, &h)) return -1;
-      } else {
-        if (resblock(p + ".0", cur, Act(), s0, S, n, true, st)) return -1;
-      }
-      if (tap((p + ".0").c_str(), s0, C, S, n, st)) return -1;
-      if (resblock(p + ".1", s0, Act(), A(XA, C), S, n, true, st, true)) return -1;
-      if (tap((p + ".1").c_str(), A(XA, C), C, S, n, st)) return -1;
-      if (linattn(p + ".2", A(XA, C), s1, C, S, n, st)) return -1;
-      if (tap((p + ".2").c_str(), s1, C, S, n, st)) return -1;
-      if (i < 3) S >>= 1;
-      if (conv(convs.at(p + ".3"), s1, Act(), A(XB, dims[i + 1]), S, n, cap, st)) return -1;
-      if (tap((p + ".3").c_str(), A(XB, dims[i + 1]), dims[i + 1], S, n, st)) return -1;
-      cur = A(XB, dims[i + 1]);
-    }
-    // ---- mid, twice with shared weights (u_net.py:177-183)
-    const int Cm = dims[4];
-    Act xa = XA, xb = XB;
-    for (int rep = 0; rep < 2; ++rep) {
-      if (resblock("mid_block1", A(xb, Cm), Act(), A(xa, Cm), S, n, true, st, true)) return -1;
-      if (midattn(A(xa, Cm), A(xb, Cm), Cm, S, n, st)) return -1;
-      if (resblock("mid_block2", A(xb, Cm), Act(), A(xa, Cm), S, n, true, st)) return -1;
-      if (tap(rep == 0 ? "mid.0" : "mid.1", A(xa, Cm), Cm, S, n, st)) return -1;
-      std::swap(xa, xb);
-    }
-    Act curb = xb, othb = xa;     // buffers (channel counts vary per level)
-    // ---- ups
-    int ccur = Cm;
-    for (int j = 0; j < 4; ++j) {
-      const int din = dims[3 - j], dout = dims[4 - j];
-      const std::string p = "ups." + std::to_string(j);
-      if (resblock(p + ".0", A(curb, dout), A(sk[3 - j][1], din), A(othb, dout), S, n, true, st)) return -1;
-      std::swap(curb, othb);
-      if (tap((p + ".0").c_str(), A(curb, dout), dout, S, n, st)) return -1;
-      if (resblock(p + ".1", A(curb, dout), A(sk[3 - j][0], din), A(othb, dout), S, n, true, st, true)) return -1;
-      std::swap(curb, othb);
-      if (linattn(p + ".2", A(curb, dout), A(othb, dout), dout, S, n, st)) return -1;
-      std::swap(curb, othb);
-      if (tap((p + ".2").c_str(), A(curb, dout), dout, S, n, st)) return -1;
-      if (j < 3) S <<= 1;   // folded nearest-x2 + conv3x3: reads `cur` at S/2, writes `oth` at S
-      if (conv(convs.at(p + ".3"), A(curb, dout), Act(), A(othb, din), S, n, cap, st)) return -1;
-      std::swap(curb, othb);
-      ccur = din;
-      if (tap((p + ".3").c_str(), A(curb, din), din, S, n, st)) return -1;
-    }
-    // ---- head
-    if (resblock("final_res_block", A(curb, ccur), A(RB, dim), A(othb, dim), S, n, true, st)) return -1;
-    std::swap(curb, othb);
-    if (tap("final_res_block", A(curb, dim), dim, S, n, st)) return -1;
-    if (resblock("final_conv.0", A(curb, dim), Act(), A(othb, dim), S, n, false, st)) return -1;
-    std::swap(curb, othb);
-    if (tap("final_conv.0", A(curb, dim), dim, S, n, st)) return -1;
-    const int hw = S * S;
-    const int nslab = (hw + kFinalPix - 1) / kFinalPix;
-    NOPE_CUDA(launch_pdl(final_conv_score_kernel, dim3(nslab, n), dim3(kFinalThreads), (size_t)kMaxLatent * dim * sizeof(float),
-                         st, curb.hi, final_w, final_b, out_emb ? out_emb + (size_t)hyp0 * Cl * hw : nullptr, query_feat,
-                         ref_of, score_part ? score_part + (size_t)hyp0 * Q * nslab * kScoreParts : nullptr, hw, dim,
-                         Cl, sp ? curb.lo : nullptr, metric, occ_threshold, bf(), Q));
-    ++launches;
-    return 0;
-  }
-
-  int iota_div(int* r, int h0, int N, int n, cudaStream_t st);
-  int conv_pose(int n, cudaStream_t st) {
-    // pb[n, P] = cs[n, cemb] @ Wp^T + bp : the 1x1 "image" geometry of the conv kernel
-    return conv(poseproj, Act(cs, cemb), Act(), Act(pb, P), 1, n, cap, st);
-  }
-};
-
-namespace {
-__global__ void iota_div_kernel(int* r, int h0, int N, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) r[i] = (h0 + i) / N;
-}
-}  // namespace
-
-int nope_unet::iota_div(int* r, int h0, int N, int n, cudaStream_t st) {
-  iota_div_kernel<<<(n + 255) / 256, 256, 0, st>>>(r, h0, N, n);
-  ++launches;
-  return 0;
-}
-
-namespace {
 struct Scratch {
   std::vector<void*> p;
   ~Scratch() { for (void* q : p) cudaFree(q); }
@@ -1029,12 +205,7 @@ int nope_unet_set_workspace(nope_unet_t* u, void* ptr, int64_t bytes, int hyps, 
 
 int nope_unet_profile(nope_unet_t* u, int enable) {
   NOPE_CHECK(u, "null engine");
-  for (cudaEvent_t e : u->prof_ev) cudaEventDestroy(e);
-  u->prof_ev.clear();
-  u->prof_flops.clear();
-  u->prof_alg.clear();
-  u->prof_shape.clear();
-  u->profile = enable != 0;
+  u->prof.reset(enable != 0);
   return 0;
 }
 
@@ -1042,24 +213,25 @@ int nope_unet_profile_read(nope_unet_t* u, double* conv_ms, double* conv_flops, 
                            int64_t* conv_launches, double* max_launch_tflops) {
   NOPE_CHECK(u && conv_ms && conv_flops && conv_launches, "null argument");
   NOPE_CUDA(cudaDeviceSynchronize());
+  const LaunchProfile& pr = u->prof;
   double ms = 0.0, fl = 0.0, alg = 0.0, best = 0.0;
-  for (size_t i = 0; i < u->prof_flops.size(); ++i) {
+  for (size_t i = 0; i < pr.rec.size(); ++i) {
     float t = 0.f;
-    NOPE_CUDA(cudaEventElapsedTime(&t, u->prof_ev[2 * i], u->prof_ev[2 * i + 1]));
+    if (pr.ms(i, &t)) return -1;
     ms += t;
-    fl += u->prof_flops[i];
-    alg += u->prof_alg[i];
-    if (t > 0.f) best = std::max(best, u->prof_flops[i] / (t * 1e-3) / 1e12);
+    fl += pr.rec[i].flops;
+    alg += pr.rec[i].alg_flops;
+    if (t > 0.f) best = std::max(best, pr.rec[i].flops / (t * 1e-3) / 1e12);
   }
   if (const char* path = std::getenv("NOPE_PROF_DUMP")) {     // development aid: per-launch table
     if (FILE* f = std::fopen(path, "a")) {
       std::fprintf(f, "# launch,ms,executed_gflop,algorithmic_gflop,res,mode,cout,k\n");
-      for (size_t i = 0; i < u->prof_flops.size(); ++i) {
+      for (size_t i = 0; i < pr.rec.size(); ++i) {
         float t = 0.f;
-        cudaEventElapsedTime(&t, u->prof_ev[2 * i], u->prof_ev[2 * i + 1]);
-        const int4 sh = u->prof_shape[i];
-        std::fprintf(f, "%zu,%.4f,%.3f,%.3f,%d,%d,%d,%d\n", i, t, u->prof_flops[i] / 1e9, u->prof_alg[i] / 1e9, sh.x,
-                     sh.y, sh.z, sh.w);
+        pr.ms(i, &t);
+        const int4 sh = pr.rec[i].shape;
+        std::fprintf(f, "%zu,%.4f,%.3f,%.3f,%d,%d,%d,%d\n", i, t, pr.rec[i].flops / 1e9, pr.rec[i].alg_flops / 1e9,
+                     sh.x, sh.y, sh.z, sh.w);
       }
       std::fclose(f);
     }
@@ -1067,7 +239,7 @@ int nope_unet_profile_read(nope_unet_t* u, double* conv_ms, double* conv_flops, 
   *conv_ms = ms;
   *conv_flops = fl;
   if (conv_alg_flops) *conv_alg_flops = alg;
-  *conv_launches = (int64_t)u->prof_flops.size();
+  *conv_launches = (int64_t)pr.rec.size();
   if (max_launch_tflops) *max_launch_tflops = best;
   return 0;
 }
@@ -1075,31 +247,8 @@ int nope_unet_profile_read(nope_unet_t* u, double* conv_ms, double* conv_flops, 
 int nope_unet_sweep_multi(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
                           const float* query_feat, int Q, float* out_emb, float* out_sim, int k, float* out_topv,
                           int64_t* out_topi, int64_t idx_base, void* stream) {
-  if (check_sweep(u, ref_feat, poses, B, N, query_feat, Q, out_sim, k, out_topv, out_topi)) return -1;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  NOPE_CUDA(cudaSetDevice(u->device));
-  u->launches = 0;
-  const int total = B * N;
-  const int cap = std::min(u->chunk, total);
-  // no allocation here when the caller provided the workspace (nope_unet_set_workspace); otherwise the
-  // engine grows its own slab (device synchronisation + cudaMalloc on growth only)
-  if (u->ensure_workspace(cap, B, query_feat ? total * Q : 0)) return -1;
-  if (u->prepare_stream(st)) return -1;
-  const int hw = u->S0 * u->S0;
-  const int nslab = (hw + kFinalPix - 1) / kFinalPix;
-  float* part = query_feat ? u->score_partial : nullptr;
-  if (u->prestage(ref_feat, B, st)) return -1;
-  for (int h0 = 0; h0 < total; h0 += cap) {
-    const int n = std::min(cap, total - h0);
-    if (u->forward_chunk(poses, h0, n, N, query_feat, out_emb, part, st, Q)) return -1;
-  }
-  if (query_feat && (out_sim || k > 0)) {
-    float* sim = out_sim ? out_sim : u->sim_buf;
-    NOPE_CUDA(launch_pdl(sim_topk_kernel, dim3(B * Q), dim3(256), 0, st, part, nslab, sim, N, k, out_topv,
-                         reinterpret_cast<long long*>(out_topi), (long long)idx_base, kScoreParts, u->metric, hw, Q));
-    ++u->launches;
-  }
-  return 0;
+  return engine_sweep(u, ref_feat, poses, B, N, query_feat, Q, out_emb, out_sim, k, out_topv, out_topi, idx_base,
+                      stream);
 }
 
 int nope_unet_sweep(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
@@ -1336,23 +485,74 @@ int nope_encoder_set_option(nope_encoder_t* e, const char* name, int value) {
   return encoder_set_option(e, name, value);
 }
 
-int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* out, void* stream) {
-  NOPE_CHECK(e && e->finalized, "encoder not finalized");
-  NOPE_CHECK(images && out, "null images / out pointer");
-  NOPE_CHECK(B >= 1, "B must be >= 1");
+// The entry points of the image engines (template encoder, VAE encoder, VAE decoder) check their arguments, then the
+// handle (image_engine_ready), so every refusal comes before any CUDA call.
+extern "C++" template <class Engine>
+int image_engine_ready(Engine* e) {
+  NOPE_CHECK(e && e->finalized, std::string(Engine::kName) + " not finalized");
   NOPE_CUDA(cudaSetDevice(e->device));
-  // The workspace is sized by the largest chunk (~80 MB per image): any B goes through, 32 images at a time.
-  return per_chunk(e, &nope_encoder::encode, images, 3 * 256 * 256, B, out, (size_t)e->D * 32 * 32, stream);
+  return 0;
+}
+
+// *_encode / *_decode: B inputs of in_per floats, any B, Engine::kChunk at a time through step
+extern "C++" template <class Engine>
+int engine_encode(Engine* e, int (Engine::*step)(const float*, int, float*, cudaStream_t), const char* what,
+                  const float* in, size_t in_per, int B, float* out, void* stream) {
+  NOPE_CHECK(in && out, std::string("null ") + what + " / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  if (image_engine_ready(e)) return -1;
+  return per_chunk(e, step, in, in_per, B, out, e->out_floats(), stream);
+}
+
+// *_encode_inplane: images [B, 3, 256, 256] x angles cossin [A, 2] -> out [B, A, ...]: the (image, angle) pairs in
+// b-major order, rotated a chunk at a time, so the [B, A, 3, 256, 256] rotated batch never exists.  The chunks are
+// those *_encode makes of that batch.
+extern "C++" template <class Engine>
+int engine_encode_inplane(Engine* e, const float* images, int B, const float* cossin, int A, float* out,
+                          void* stream) {
+  NOPE_CHECK(images && cossin && out, "null images / cossin / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(A >= 1 && A <= 360, "A (in-plane angles) must be in [1, 360]");
+  NOPE_CHECK((int64_t)B * A <= INT32_MAX, "too many (image, angle) pairs");
+  if (image_engine_ready(e)) return -1;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return per_rotated_chunk(e, B * A, out, e->out_floats(), st, [&](int lo, int n) {
+    inplane_rotate_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, cossin, A, 256, 256, lo, e->rot_stage);
+  });
+}
+
+// *_encode_rotated: images [B, 3, 256, 256] x pairs (image_idx [P], cossin [P, 2]) -> out [P, ...]: the pairs in
+// order, rotated a chunk at a time, so the result equals *_encode of the materialised [P, 3, 256, 256] batch.
+extern "C++" template <class Engine>
+int engine_encode_rotated(Engine* e, const float* images, int B, const int32_t* image_idx, const float* cossin, int P,
+                          float* out, void* stream) {
+  NOPE_CHECK(images && image_idx && cossin && out, "null images / image_idx / cossin / out pointer");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(P >= 1 && P <= INT32_MAX / 2, "P (pairs) must be in [1, 2^30)");
+  if (image_engine_ready(e)) return -1;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return per_rotated_chunk(e, P, out, e->out_floats(), st, [&](int lo, int n) {
+    inplane_rotate_pairs_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, B, image_idx, cossin, 256, 256, lo,
+                                                                           e->rot_stage);
+  });
+}
+
+// *_run_block of the VAE encoder and decoder
+extern "C++" template <class Engine>
+int vae_run_block(Engine* e, const char* name, const float* x, int C, int H, int n, float* out, float* out_pair,
+                  int64_t out_capacity_floats, void* stream) {
+  NOPE_CHECK(name && x && out, "null name / x / out pointer");
+  if (image_engine_ready(e)) return -1;
+  return e->run_block(name, x, C, H, n, out, out_pair, out_capacity_floats, static_cast<cudaStream_t>(stream));
+}
+
+int nope_encoder_encode(nope_encoder_t* e, const float* images, int B, float* out, void* stream) {
+  return engine_encode(e, &nope_encoder::encode, "images", images, 3 * 256 * 256, B, out, stream);
 }
 
 int nope_encoder_encode_inplane(nope_encoder_t* e, const float* images, int B, const float* cossin, int A, float* out,
                                 void* stream) {
-  NOPE_CHECK(images && cossin && out, "null images / cossin / out pointer");
-  NOPE_CHECK(B >= 1, "B must be >= 1");
-  NOPE_CHECK(A >= 1 && A <= 360, "A (in-plane angles) must be in [1, 360]");
-  NOPE_CHECK(e && e->finalized, "encoder not finalized");
-  NOPE_CUDA(cudaSetDevice(e->device));
-  return e->encode_inplane(images, B, cossin, A, out, static_cast<cudaStream_t>(stream));
+  return engine_encode_inplane(e, images, B, cossin, A, out, stream);
 }
 
 int nope_inplane_rotate(const float* images, int B, int H, int W, const float* cossin, int A, float* out,
@@ -1393,21 +593,15 @@ int nope_inplane_rotate_pairs(const float* images, int B, int H, int W, const in
 
 int nope_encoder_encode_rotated(nope_encoder_t* e, const float* images, int B, const int32_t* image_idx,
                                 const float* cossin, int P, float* out, void* stream) {
-  NOPE_CHECK(images && image_idx && cossin && out, "null images / image_idx / cossin / out pointer");
-  NOPE_CHECK(B >= 1, "B must be >= 1");
-  NOPE_CHECK(P >= 1 && P <= INT32_MAX / 2, "P (pairs) must be in [1, 2^30)");
-  NOPE_CHECK(e && e->finalized, "encoder not finalized");
-  NOPE_CUDA(cudaSetDevice(e->device));
-  return e->encode_rotated(images, B, image_idx, cossin, P, out, static_cast<cudaStream_t>(stream));
+  return engine_encode_rotated(e, images, B, image_idx, cossin, P, out, stream);
 }
 
 int64_t nope_encoder_last_launch_count(const nope_encoder_t* e) { return e ? e->launches : 0; }
 
 int nope_encoder_run_block(nope_encoder_t* e, const char* name, const float* x, int C, int H, int n, float* out,
                            int64_t out_capacity_floats, void* stream) {
-  NOPE_CHECK(e && e->finalized, "encoder not finalized");
   NOPE_CHECK(name && x && out, "null name / x / out pointer");
-  NOPE_CUDA(cudaSetDevice(e->device));
+  if (image_engine_ready(e)) return -1;
   return e->run_block(name, x, C, H, n, out, out_capacity_floats, static_cast<cudaStream_t>(stream));
 }
 
@@ -1434,41 +628,24 @@ int nope_vae_finalize(nope_vae_t* v) { return engine_finalize(v); }
 int nope_vae_set_option(nope_vae_t* v, const char* name, int value) { return encoder_set_option(v, name, value); }
 
 int nope_vae_encode(nope_vae_t* v, const float* images, int B, float* out, void* stream) {
-  NOPE_CHECK(images && out, "null images / out pointer");
-  NOPE_CHECK(B >= 1, "B must be >= 1");
-  NOPE_CHECK(v && v->finalized, "VAE not finalized");
-  NOPE_CUDA(cudaSetDevice(v->device));
-  return per_chunk(v, &nope_vae::encode, images, 3 * 256 * 256, B, out, 4 * 32 * 32, stream);
+  return engine_encode(v, &nope_vae::encode, "images", images, 3 * 256 * 256, B, out, stream);
 }
 
 int nope_vae_encode_inplane(nope_vae_t* v, const float* images, int B, const float* cossin, int A, float* out,
                             void* stream) {
-  NOPE_CHECK(images && cossin && out, "null images / cossin / out pointer");
-  NOPE_CHECK(B >= 1, "B must be >= 1");
-  NOPE_CHECK(A >= 1 && A <= 360, "A (in-plane angles) must be in [1, 360]");
-  NOPE_CHECK(v && v->finalized, "VAE not finalized");
-  NOPE_CUDA(cudaSetDevice(v->device));
-  return v->encode_inplane(images, B, cossin, A, out, static_cast<cudaStream_t>(stream));
+  return engine_encode_inplane(v, images, B, cossin, A, out, stream);
 }
 
 int nope_vae_encode_rotated(nope_vae_t* v, const float* images, int B, const int32_t* image_idx, const float* cossin,
                             int P, float* out, void* stream) {
-  NOPE_CHECK(images && image_idx && cossin && out, "null images / image_idx / cossin / out pointer");
-  NOPE_CHECK(B >= 1, "B must be >= 1");
-  NOPE_CHECK(P >= 1 && P <= INT32_MAX / 2, "P (pairs) must be in [1, 2^30)");
-  NOPE_CHECK(v && v->finalized, "VAE not finalized");
-  NOPE_CUDA(cudaSetDevice(v->device));
-  return v->encode_rotated(images, B, image_idx, cossin, P, out, static_cast<cudaStream_t>(stream));
+  return engine_encode_rotated(v, images, B, image_idx, cossin, P, out, stream);
 }
 
 int64_t nope_vae_last_launch_count(const nope_vae_t* v) { return v ? v->launches : 0; }
 
 int nope_vae_run_block(nope_vae_t* v, const char* name, const float* x, int C, int H, int n, float* out,
                        float* out_pair, int64_t out_capacity_floats, void* stream) {
-  NOPE_CHECK(v && v->finalized, "VAE not finalized");
-  NOPE_CHECK(name && x && out, "null name / x / out pointer");
-  NOPE_CUDA(cudaSetDevice(v->device));
-  return v->run_block(name, x, C, H, n, out, out_pair, out_capacity_floats, static_cast<cudaStream_t>(stream));
+  return vae_run_block(v, name, x, C, H, n, out, out_pair, out_capacity_floats, stream);
 }
 
 // ---------------------------------------------------------------------------------
@@ -1494,21 +671,14 @@ int nope_vae_decoder_load_tensor(nope_vae_decoder_t* d, const char* key, const f
 int nope_vae_decoder_finalize(nope_vae_decoder_t* d) { return engine_finalize(d); }
 
 int nope_vae_decoder_decode(nope_vae_decoder_t* d, const float* latents, int B, float* out, void* stream) {
-  NOPE_CHECK(latents && out, "null latents / out pointer");
-  NOPE_CHECK(B >= 1, "B must be >= 1");
-  NOPE_CHECK(d && d->finalized, "VAE decoder not finalized");
-  NOPE_CUDA(cudaSetDevice(d->device));
-  return per_chunk(d, &nope_vae_decoder::decode, latents, 4 * 32 * 32, B, out, 3 * 256 * 256, stream);
+  return engine_encode(d, &nope_vae_decoder::decode, "latents", latents, 4 * 32 * 32, B, out, stream);
 }
 
 int64_t nope_vae_decoder_last_launch_count(const nope_vae_decoder_t* d) { return d ? d->launches : 0; }
 
 int nope_vae_decoder_run_block(nope_vae_decoder_t* d, const char* name, const float* x, int C, int H, int n,
                                float* out, float* out_pair, int64_t out_capacity_floats, void* stream) {
-  NOPE_CHECK(d && d->finalized, "VAE decoder not finalized");
-  NOPE_CHECK(name && x && out, "null name / x / out pointer");
-  NOPE_CUDA(cudaSetDevice(d->device));
-  return d->run_block(name, x, C, H, n, out, out_pair, out_capacity_floats, static_cast<cudaStream_t>(stream));
+  return vae_run_block(d, name, x, C, H, n, out, out_pair, out_capacity_floats, stream);
 }
 
 // ---------------------------------------------------------------------------------
@@ -2078,8 +1248,7 @@ int nope_op_conv_gn_fused(int mode, int precision, const float* x0, int C0, cons
   const int n_res = residual ? (res_div > 0 ? (n_img + res_div - 1) / res_div : n_img) : 0;
   if (residual && to_nhwc(residual, &r, op.s, n_res, Cout, hw, st, precision == 2 ? &rl : nullptr)) return -1;
   if (chan_bias && to_nhwc(chan_bias, &pbh, op.s, n_img, Cout, 1, st)) return -1;
-  if (op.eng.ensure_workspace(n_img, std::max(n_res, 1))) return -1;
-  if (op.eng.prepare_stream(st)) return -1;
+  if (op.eng.ensure_workspace(n_img, std::max(n_res, 1), 0, st)) return -1;
   op.eng.pb = pbh;
   op.eng.P = Cout;
   NormLayer N;
@@ -2167,25 +1336,7 @@ int nope_op_upsample2x(const float* x, float* out, int n_img, int C, int H, int 
 
 int nope_unet_debug_tap(nope_unet_t* u, const float* ref_feat, const float* poses, int N, const char* tap,
                         float* out, int64_t out_capacity_floats, int* out_C, int* out_H, void* stream) {
-  NOPE_CHECK(u && u->finalized && ref_feat && poses && tap && out, "bad argument");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  NOPE_CHECK(N <= u->chunk, "debug tap: N must fit one chunk");
-  NOPE_CUDA(cudaSetDevice(u->device));
-  if (u->ensure_workspace(N, 1)) return -1;
-  if (u->prepare_stream(st)) return -1;
-  u->tap_name = tap;
-  u->tap_out = out;
-  u->tap_cap = out_capacity_floats;
-  u->tap_hit = false;
-  int rc = u->prestage(ref_feat, 1, st);
-  if (!rc) rc = u->forward_chunk(poses, 0, N, N, nullptr, nullptr, nullptr, st);
-  u->tap_out = nullptr;
-  if (rc) return rc;
-  NOPE_CUDA(cudaStreamSynchronize(st));
-  NOPE_CHECK(u->tap_hit, std::string("unknown tap name: ") + tap);
-  if (out_C) *out_C = u->tap_C;
-  if (out_H) *out_H = u->tap_S;
-  return 0;
+  return engine_debug_tap(u, ref_feat, poses, N, tap, out, out_capacity_floats, out_C, out_H, stream);
 }
 
 // ---------------------------------------------------------------------------------
@@ -2245,23 +1396,19 @@ int64_t nope_ldm_last_launch_count(const nope_ldm_t* m) { return m ? m->launches
 
 int nope_ldm_profile(nope_ldm_t* m, int enable) {
   NOPE_CHECK(m, "null engine");
-  for (cudaEvent_t e : m->prof_ev) cudaEventDestroy(e);
-  m->prof_ev.clear();
-  m->prof_flops.clear();
-  m->prof_kind.clear();
-  m->profile = enable != 0;
+  m->prof.reset(enable != 0);
   return 0;
 }
 int nope_ldm_profile_read(nope_ldm_t* m, double* ms, double* flops, int64_t* launches) {
   NOPE_CHECK(m && ms && flops && launches, "null argument");
   NOPE_CUDA(cudaDeviceSynchronize());
   for (int k = 0; k < 2; ++k) { ms[k] = 0.0; flops[k] = 0.0; launches[k] = 0; }
-  for (size_t i = 0; i < m->prof_flops.size(); ++i) {
+  for (size_t i = 0; i < m->prof.rec.size(); ++i) {
     float t = 0.f;
-    NOPE_CUDA(cudaEventElapsedTime(&t, m->prof_ev[2 * i], m->prof_ev[2 * i + 1]));
-    const int k = m->prof_kind[i];
+    if (m->prof.ms(i, &t)) return -1;
+    const int k = m->prof.rec[i].kind;
     ms[k] += t;
-    flops[k] += m->prof_flops[i];
+    flops[k] += m->prof.rec[i].flops;
     launches[k] += 1;
   }
   return 0;
@@ -2270,49 +1417,8 @@ int nope_ldm_profile_read(nope_ldm_t* m, double* ms, double* flops, int64_t* lau
 int nope_ldm_sweep_multi(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
                          const float* query_latent, int Q, float* out_emb, float* out_sim, int k, float* out_topv,
                          int64_t* out_topi, int64_t idx_base, void* stream) {
-  if (check_sweep(m, ref_latent, poses, B, N, query_latent, Q, out_sim, k, out_topv, out_topi)) return -1;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  NOPE_CUDA(cudaSetDevice(m->device));
-  m->launches = 0;
-  const int total = B * N;
-  const size_t scored = (size_t)total * Q;      // (b, q, pose) triples
-  const int cap = std::min(m->chunk, total);
-  if (m->ensure_workspace(cap, B)) return -1;
-  const int hw = m->S0 * m->S0;
-  const int nslab = (hw + kFinalThreads - 1) / kFinalThreads;
-  float* part = nullptr;
-  if (query_latent) {
-    const size_t need = scored * nslab;
-    if (need > m->score_partial_cap) {
-      NOPE_CUDA(cudaStreamSynchronize(st));
-      if (m->score_partial) cudaFree(m->score_partial);
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&m->score_partial), need * sizeof(float)));
-      m->score_partial_cap = need;
-    }
-    part = m->score_partial;
-  }
-  if (m->prestage(ref_latent, B, st)) return -1;
-  for (int h0 = 0; h0 < total; h0 += cap) {
-    const int n = std::min(cap, total - h0);
-    if (m->forward_chunk(poses, h0, n, N, query_latent, out_emb, part, st, Q)) return -1;
-  }
-  if (query_latent && (out_sim || k > 0)) {
-    float* sim = out_sim;
-    if (!sim) {
-      if (scored > m->sim_buf_cap) {
-        NOPE_CUDA(cudaStreamSynchronize(st));
-        if (m->sim_buf) cudaFree(m->sim_buf);
-        NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&m->sim_buf), scored * sizeof(float)));
-        m->sim_buf_cap = scored;
-      }
-      sim = m->sim_buf;
-    }
-    sim_topk_kernel<<<B * Q, 256, 0, st>>>(part, nslab, sim, N, k, out_topv, reinterpret_cast<long long*>(out_topi),
-                                           (long long)idx_base, 1, 0, 1, Q);
-    NOPE_CUDA(cudaGetLastError());
-    ++m->launches;
-  }
-  return 0;
+  return engine_sweep(m, ref_latent, poses, B, N, query_latent, Q, out_emb, out_sim, k, out_topv, out_topi, idx_base,
+                      stream);
 }
 
 int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
@@ -2324,23 +1430,7 @@ int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, i
 
 int nope_ldm_debug_tap(nope_ldm_t* m, const float* ref_latent, const float* poses, int N, const char* tap,
                        float* out, int64_t out_capacity_floats, int* out_C, int* out_H, void* stream) {
-  NOPE_CHECK(m && m->finalized && ref_latent && poses && tap && out, "bad argument");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  NOPE_CHECK(N <= m->chunk, "debug tap: N must fit one chunk");
-  if (m->ensure_workspace(N, 1)) return -1;
-  m->tap_name = tap;
-  m->tap_out = out;
-  m->tap_cap = out_capacity_floats;
-  m->tap_hit = false;
-  int rc = m->prestage(ref_latent, 1, st);
-  if (!rc) rc = m->forward_chunk(poses, 0, N, N, nullptr, nullptr, nullptr, st);
-  m->tap_out = nullptr;
-  if (rc) return rc;
-  NOPE_CUDA(cudaStreamSynchronize(st));
-  NOPE_CHECK(m->tap_hit, std::string("unknown tap name: ") + tap);
-  if (out_C) *out_C = m->tap_C;
-  if (out_H) *out_H = m->tap_S;
-  return 0;
+  return engine_debug_tap(m, ref_latent, poses, N, tap, out, out_capacity_floats, out_C, out_H, stream);
 }
 
 int nope_ldm_run_block(nope_ldm_t* m, const char* name, const float* x0, int C0, const float* x1, int C1, int S,
@@ -2349,7 +1439,7 @@ int nope_ldm_run_block(nope_ldm_t* m, const char* name, const float* x0, int C0,
   NOPE_CHECK(S == 8 || S == 16 || S == 32, "side must be 8, 16 or 32");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   NOPE_CUDA(cudaSetDevice(m->device));
-  if (m->ensure_workspace(std::max(n, 1), 1)) return -1;
+  if (m->ensure_workspace(std::max(n, 1), 1, 0, st)) return -1;
   NOPE_CHECK(n <= m->cap, "run_block: n exceeds the workspace");
   const std::string nm = name;
   // stage the inputs in XA / XB (NHWC fp16); results land in XC

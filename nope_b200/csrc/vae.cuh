@@ -359,7 +359,7 @@ struct VaeEngine {
   StagedWeights staged;
   std::map<std::string, VaeConv> convs;
   std::map<std::string, VaeNorm> norms;
-  DeviceAllocs mem;                           // weights and workspace
+  DeviceAllocs mem;                           // weights, workspace and rot_stage
   // workspace (alloc_workspace), each activation buffer sized for cap images of the widest level
   float* x32[2] = {nullptr, nullptr};         // residual stream, fp32
   ActPair xs[2];                              // residual stream, (hi, lo)
@@ -637,17 +637,6 @@ struct VaeEngine {
     NOPE_CUDA(cudaGetLastError());
     return 0;
   }
-  // the checks every run_block makes once the module's input shape (Ci, Hi) and output shape (Co, Ho) are known
-  int check_block(const std::string& name, int chunk, int C, int H, int n, int Ci, int Hi, int Co, int Ho,
-                  int64_t cap_floats) {
-    NOPE_CHECK(Ci, "run_block: unknown module " + name);
-    NOPE_CHECK(n >= 1 && n <= chunk, "run_block: n must be in [1, " + std::to_string(chunk) + "]");
-    NOPE_CHECK(C == Ci && H == Hi, "run_block: " + name + " takes [n, " + std::to_string(Ci) + ", " +
-                                       std::to_string(Hi) + ", " + std::to_string(Hi) + "] inputs, got C = " +
-                                       std::to_string(C) + ", H = " + std::to_string(H));
-    NOPE_CHECK(cap_floats >= (int64_t)n * Co * Ho * Ho, "run_block: output buffer too small");
-    return 0;
-  }
 };
 
 }  // namespace nope
@@ -658,7 +647,8 @@ struct nope_vae : nope::VaeEngine {
   static constexpr int kChunk = 16;           // images per pass: the workspace holds this many (~200 MB each)
   static constexpr int kCh[4] = {128, 256, 512, 512};
   float *in_w = nullptr, *in_b = nullptr;
-  float* rot_stage = nullptr;                 // kChunk rotated crops
+  float* rot_stage = nullptr;                 // kChunk rotated crops, allocated by the first rotated encode
+  size_t out_floats() const { return 4 * 32 * 32; }   // per encoded image
 
   nope_vae() : VaeEngine(kChunk) {}
 
@@ -713,8 +703,7 @@ struct nope_vae : nope::VaeEngine {
       if (pack_conv("conv_out", 4, 512, 3, Wf, bf)) return -1;
     }
     // workspace for kChunk images of the 256 x 256 x 128 level
-    if (alloc_workspace((size_t)kChunk * 256 * 256 * 128)) return -1;
-    return mem.alloc(&rot_stage, (size_t)kChunk * 3 * 256 * 256);
+    return alloc_workspace((size_t)kChunk * 256 * 256 * 128);
   }
 
   // Downsample2D: pad (0, 1, 0, 1) + 3x3 stride 2 from side 2H to H.  Tap (ky, kx) reads input (2y + ky, 2x + kx):
@@ -826,41 +815,6 @@ struct nope_vae : nope::VaeEngine {
     NOPE_CUDA(cudaStreamSynchronize(st));
     return 0;
   }
-
-  // images [B, 3, 256, 256] x angles cossin [A, 2] -> out [B, A, 4, 32, 32]: the (image, angle) pairs in b-major
-  // order, kChunk at a time rotated into rot_stage and encoded from there (the chunks encode() makes of that batch)
-  int encode_inplane(const float* images, int B, const float* cossin, int A, float* out, cudaStream_t st) {
-    using namespace nope;
-    NOPE_CHECK((int64_t)B * A <= INT32_MAX, "too many (image, angle) pairs");
-    const int pairs = B * A;
-    int64_t total = 0;
-    for (int lo = 0; lo < pairs; lo += kChunk) {
-      const int n = pairs - lo < kChunk ? pairs - lo : kChunk;
-      inplane_rotate_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, cossin, A, 256, 256, lo, rot_stage);
-      NOPE_CUDA(cudaGetLastError());
-      if (encode(rot_stage, n, out + (size_t)lo * 4 * 32 * 32, st)) return -1;
-      total += launches + 1;
-    }
-    launches = total;
-    return 0;
-  }
-
-  // images [B, 3, 256, 256] x pairs (image_idx [P], cossin [P, 2]) -> out [P, 4, 32, 32], kChunk pairs at a time
-  int encode_rotated(const float* images, int B, const int* image_idx, const float* cossin, int P, float* out,
-                     cudaStream_t st) {
-    using namespace nope;
-    int64_t total = 0;
-    for (int lo = 0; lo < P; lo += kChunk) {
-      const int n = P - lo < kChunk ? P - lo : kChunk;
-      inplane_rotate_pairs_kernel<<<dim3(256 * 256 / 256, n), 256, 0, st>>>(images, B, image_idx, cossin, 256, 256,
-                                                                             lo, rot_stage);
-      NOPE_CUDA(cudaGetLastError());
-      if (encode(rot_stage, n, out + (size_t)lo * 4 * 32 * 32, st)) return -1;
-      total += launches + 1;
-    }
-    launches = total;
-    return 0;
-  }
 };
 
 // ---------------------------------------------------------------- decoder (DESIGN.md section 17)
@@ -874,6 +828,7 @@ struct nope_vae_decoder : nope::VaeEngine {
   static constexpr int kCh[4] = {512, 512, 256, 128};
   static constexpr const char* kAttn = "decoder.mid_block.attentions.0.";
   float *in_w = nullptr, *in_b = nullptr, *pq_w = nullptr, *pq_b = nullptr;
+  size_t out_floats() const { return 3 * 256 * 256; }   // per decoded image
 
   nope_vae_decoder() : VaeEngine(kChunk) {}
 
