@@ -155,6 +155,7 @@ for _kind, _n in ENGINE_CREATE_ARGS.items():
     })
 
 EXPECTED_ABI = 2     # include/nope_b200.h "ABI version"; a stale build with other signatures must not bind
+MAX_TOPK = 64        # the most entries a ranking call selects per row (k, keep): mirrors kMaxTopK in csrc/rank.cuh
 
 _lib = None
 

@@ -5,12 +5,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "kernels.cuh"
+#include "rank.cuh"
 
 namespace nope {
 
 constexpr int kDistinctMaxSym = 32;                       // discrete rotations per group, the identity first
-constexpr int kDistinctMaxK = 64;
 constexpr int kDistinctThreads = 512;
 constexpr int kDistinctSmemWords = 4096;                  // 131 072 entries: 36 x 2562 in-plane rows fit
 
@@ -99,27 +98,57 @@ __device__ __forceinline__ bool distinct_within(const double* ri, const double* 
   return false;
 }
 
+// The scan of distinct_topk_kernel: a warp per 32-entry word of the mask, which marks the removed entries (taken,
+// suppressed, or scored -inf / NaN).  Each round removes what lies within theta of the last pick.
+struct DistinctSel : TopkOut {
+  const float* row;                    // sim [N]
+  int N, nwords;
+  const double* rot;                   // [N, 9]
+  const DistinctGroup* g;              // in shared memory
+  double c_thr;
+  unsigned* mask;                      // [nwords]
+
+  __device__ __forceinline__ void scan(int t, const int* picks, float& bv, int& bi) const {
+    const int lane = threadIdx.x & 31;
+    const int pick = t > 0 ? picks[t - 1] : -1;
+    double ri[9];
+    if (t > 0)
+#pragma unroll
+      for (int e = 0; e < 9; ++e) ri[e] = rot[(long long)pick * 9 + e];
+    for (int w = threadIdx.x >> 5; w < nwords; w += kDistinctThreads / 32) {
+      const unsigned word = mask[w];
+      if (word == 0xffffffffu) continue;
+      const int j = (w << 5) + lane;
+      bool dead = ((word >> lane) & 1u) || j >= N;
+      if (!dead) {
+        const float v = row[j];
+        if (!(v > -INFINITY) || j == pick) {
+          dead = true;
+        } else if (t > 0 && distinct_within(ri, rot + (long long)j * 9, *g, c_thr)) {
+          dead = true;
+        } else {
+          offer(v, j, bv, bi);
+        }
+      }
+      const unsigned now = __ballot_sync(0xffffffffu, dead);
+      if (lane == 0 && now != word) mask[w] = now;
+    }
+  }
+};
+
 // One CTA per row r of sim [R, N].  The row's rotations are rot [G_r, N, 9] at r / Q (0 when G_r = 1), its group
-// groups[group[r]].  A bit mask marks the removed entries (taken, suppressed, or scored -inf / NaN); it lives in
-// shared memory up to kDistinctSmemWords words, else at gmask + r * ceil(N / 32).  Each pass over the row removes
-// what lies within theta of the last pick and finds the best entry left (ranks_before, cta_argmax), so k picks cost
-// k passes.  Ranks with nothing left get -inf / -1.
+// groups[group[r]].  The removal mask lives in shared memory up to kDistinctSmemWords words, else at
+// gmask + r * ceil(N / 32).  k picks cost k passes over the row (select_rounds); ranks with nothing left get -inf / -1.
 __global__ void __launch_bounds__(kDistinctThreads)
 distinct_topk_kernel(const float* __restrict__ sim, int N, const double* __restrict__ rot, int G_r, int Q,
                      const DistinctGroup* __restrict__ groups, const int* __restrict__ group, int k, double c_thr,
                      unsigned* __restrict__ gmask, long long* __restrict__ idx_out, float* __restrict__ score_out) {
   __shared__ DistinctGroup s_g;
   __shared__ unsigned s_mask[kDistinctSmemWords];
-  __shared__ double s_ri[9];
-  __shared__ float s_v[kDistinctThreads / 32];
-  __shared__ int s_i[kDistinctThreads / 32];
-  __shared__ int s_pick;
+  __shared__ SelectSmem<kDistinctThreads> sm;
   const int r = blockIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int nwords = (N + 31) >> 5;
   unsigned* mask = gmask ? gmask + (long long)r * nwords : s_mask;
-  const float* srow = sim + (long long)r * N;
-  const double* rrow = rot + (long long)(G_r == 1 ? 0 : r / Q) * N * 9;
   {
     const long long* src = reinterpret_cast<const long long*>(groups + group[r]);
     long long* dst = reinterpret_cast<long long*>(&s_g);
@@ -127,53 +156,10 @@ distinct_topk_kernel(const float* __restrict__ sim, int N, const double* __restr
   }
   for (int w = threadIdx.x; w < nwords; w += blockDim.x) mask[w] = 0u;
   __syncthreads();
-  for (int t = 0;; ++t) {
-    float bv = -INFINITY;
-    int bi = 0x7fffffff;
-    double ri[9];
-    if (t > 0)
-#pragma unroll
-      for (int e = 0; e < 9; ++e) ri[e] = s_ri[e];
-    const int pick = t > 0 ? s_pick : -1;
-    for (int w = warp; w < nwords; w += kDistinctThreads / 32) {
-      const unsigned word = mask[w];
-      if (word == 0xffffffffu) continue;
-      const int j = (w << 5) + lane;
-      bool dead = ((word >> lane) & 1u) || j >= N;
-      if (!dead) {
-        const float v = srow[j];
-        if (!(v > -INFINITY) || j == pick) {
-          dead = true;
-        } else if (t > 0 && distinct_within(ri, rrow + (long long)j * 9, s_g, c_thr)) {
-          dead = true;
-        } else if (bi == 0x7fffffff || ranks_before(v, j, bv, bi)) {
-          bv = v;
-          bi = j;
-        }
-      }
-      const unsigned now = __ballot_sync(0xffffffffu, dead);
-      if (lane == 0 && now != word) mask[w] = now;
-    }
-    cta_argmax(bv, bi, s_v, s_i);
-    const long long o = (long long)r * k + t;
-    if (threadIdx.x == 0) {
-      s_pick = bi;
-      score_out[o] = bi == 0x7fffffff ? -INFINITY : bv;
-      idx_out[o] = bi == 0x7fffffff ? -1 : (long long)bi;
-    }
-    __syncthreads();
-    const int next = s_pick;
-    if (next == 0x7fffffff) {
-      for (int u = t + 1 + threadIdx.x; u < k; u += blockDim.x) {
-        score_out[(long long)r * k + u] = -INFINITY;
-        idx_out[(long long)r * k + u] = -1;
-      }
-      return;
-    }
-    if (t + 1 == k) return;
-    if (threadIdx.x < 9) s_ri[threadIdx.x] = rrow[(long long)next * 9 + threadIdx.x];
-    __syncthreads();
-  }
+  const long long o = (long long)r * k;
+  select_rounds(DistinctSel{{score_out + o, idx_out + o, 0}, sim + (long long)r * N, N, nwords,
+                            rot + (long long)(G_r == 1 ? 0 : r / Q) * N * 9, &s_g, c_thr, mask},
+                k, sm);
 }
 
 }  // namespace nope

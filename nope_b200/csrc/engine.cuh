@@ -25,6 +25,7 @@
 
 #include "common.cuh"
 #include "kernels.cuh"
+#include "rank.cuh"
 
 namespace nope {
 
@@ -163,7 +164,7 @@ int check_sweep(const E* e, const float* ref, const float* poses, int B, int N, 
   NOPE_CHECK(Q >= 1, "Q (queries per reference) must be >= 1");
   NOPE_CHECK((int64_t)B * Q * N <= INT32_MAX, "B * Q * N exceeds the scored-triple limit (2^31 - 1)");
   NOPE_CHECK(!(out_sim || k > 0) || query, "scores / top-k need the query");
-  NOPE_CHECK(k >= 0 && k <= N && k <= 64, "k must be in [0, min(N, 64)]");
+  NOPE_CHECK(k >= 0 && k <= N && k <= kMaxTopK, "k must be in [0, min(N, 64)]");
   NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
   return 0;
 }

@@ -23,6 +23,7 @@
 #include "engine.cuh"
 #include "kernels.cuh"
 #include "ldm_kernels.cuh"
+#include "rank.cuh"
 
 #include <algorithm>
 #include <cmath>

@@ -21,6 +21,7 @@
 #include "conv_tc.cuh"
 #include "conv_tc2.cuh"
 #include "kernels.cuh"
+#include "rank.cuh"
 #include "linattn_tc.cuh"
 #include "unet.cuh"
 #include "encoder.cuh"
@@ -277,7 +278,7 @@ int nope_score_topk_multi(const float* query_feat, const float* emb, int B, int 
   NOPE_CHECK(Bt <= 65535 && (int64_t)B * Q * N <= INT32_MAX, "too many templates or (query, template) pairs");
   NOPE_CHECK(metric == NOPE_METRIC_L2 || metric == NOPE_METRIC_COSINE || metric == NOPE_METRIC_COSINE_OCC,
              "unknown similarity metric (l2, cosine and cosine_occlusion exist)");
-  NOPE_CHECK(k >= 0 && k <= N && k <= 64, "k must be in [0, min(N, 64)]");
+  NOPE_CHECK(k >= 0 && k <= N && k <= kMaxTopK, "k must be in [0, min(N, 64)]");
   NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // query rows [B * Q] in order; template batch t serves rows [t * rows, (t + 1) * rows)
@@ -303,7 +304,7 @@ int nope_score_topk_grouped(const float* query_feat, const float* emb, int R, in
   NOPE_CHECK(O <= 65535 && (int64_t)R * N <= INT32_MAX, "too many templates or (query, template) pairs");
   NOPE_CHECK(metric == NOPE_METRIC_L2 || metric == NOPE_METRIC_COSINE || metric == NOPE_METRIC_COSINE_OCC,
              "unknown similarity metric (l2, cosine and cosine_occlusion exist)");
-  NOPE_CHECK(k >= 0 && k <= 64 && (int64_t)k <= (int64_t)A * N, "k must be in [0, min(64, A * N)]");
+  NOPE_CHECK(k >= 0 && k <= kMaxTopK && (int64_t)k <= (int64_t)A * N, "k must be in [0, min(64, A * N)]");
   NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // one CTA per (template n, group g): slot slots[g]'s template n against the group's rows
@@ -329,7 +330,7 @@ int nope_score_topk(const float* query_feat, const float* emb, int B, int N, int
 int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_topi, int64_t idx_base,
               void* stream) {
   NOPE_CHECK(sim && out_topv && out_topi, "null argument");
-  NOPE_CHECK(k >= 1 && k <= N && k <= 64, "k must be in [1, min(N, 64)]");
+  NOPE_CHECK(k >= 1 && k <= N && k <= kMaxTopK, "k must be in [1, min(N, 64)]");
   sim_topk_kernel<<<B, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       nullptr, 0, sim, N, k, out_topv, reinterpret_cast<long long*>(out_topi), (long long)idx_base);
   NOPE_CUDA(cudaGetLastError());
@@ -340,7 +341,7 @@ int nope_pose_cells_expand(const int64_t* top_idx, int R, int keep, const int32_
                            const float* poses, int B, int Q, int n_fine, int M, int32_t* out_cand, float* out_poses,
                            void* stream) {
   NOPE_CHECK(top_idx && cells && poses && out_cand && out_poses, "null argument");
-  NOPE_CHECK(keep >= 1 && keep <= 64, "keep must be in [1, 64]");
+  NOPE_CHECK(keep >= 1 && keep <= kMaxTopK, "keep must be in [1, 64]");
   NOPE_CHECK(n_coarse >= 1 && F >= 1 && n_fine >= 1 && B >= 1 && Q >= 1, "bad arguments");
   NOPE_CHECK(R >= 1 && (int64_t)B * Q == R, "R (rows) must equal B * Q");
   NOPE_CHECK((int64_t)M >= (int64_t)keep * F, "M must be at least keep * F (the largest union of keep cells)");
@@ -353,7 +354,7 @@ int nope_pose_cells_expand(const int64_t* top_idx, int R, int keep, const int32_
 int nope_pose_cells_rank(const float* sim, const int32_t* cand, int R, int M, int n_fine, int k, float* out_sim,
                          float* out_topv, int64_t* out_topi, void* stream) {
   NOPE_CHECK(sim && cand && out_topv && out_topi, "null argument");
-  NOPE_CHECK(k >= 1 && k <= 64, "k must be in [1, 64]");
+  NOPE_CHECK(k >= 1 && k <= kMaxTopK, "k must be in [1, 64]");
   NOPE_CHECK(R >= 1 && M >= 1 && n_fine >= 1, "bad arguments");
   pose_cells_rank_kernel<<<R, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       sim, cand, M, n_fine, k, out_sim, out_topv, reinterpret_cast<long long*>(out_topi));
@@ -365,7 +366,7 @@ int nope_pose_refine_propose(const float* D, const int32_t* seed, int R, int kee
                              int Q, int N, const float* stencil, float* out_D, int32_t* out_seed, float* out_rel,
                              float* out_poses, void* stream) {
   NOPE_CHECK(D && seed && all_relativeR && stencil && out_D && out_seed && out_rel && out_poses, "null argument");
-  NOPE_CHECK(keep >= 1 && keep <= 64, "keep must be in [1, 64]");
+  NOPE_CHECK(keep >= 1 && keep <= kMaxTopK, "keep must be in [1, 64]");
   NOPE_CHECK(B >= 1 && Q >= 1 && N >= 1, "bad arguments");
   NOPE_CHECK(R >= 1 && (int64_t)B * Q == R, "R (rows) must equal B * Q");
   pose_refine_propose_kernel<<<R, 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -378,7 +379,7 @@ int nope_pose_refine_select(const float* sim, const float* cand_D, const int32_t
                             int R, int M, int k, float trace_threshold, float* out_D, int32_t* out_seed,
                             float* out_score, float* out_rel, void* stream) {
   NOPE_CHECK(sim && cand_D && cand_seed && cand_rel && out_D && out_seed && out_score, "null argument");
-  NOPE_CHECK(k >= 1 && k <= 64, "k must be in [1, 64]");
+  NOPE_CHECK(k >= 1 && k <= kMaxTopK, "k must be in [1, 64]");
   NOPE_CHECK(M >= 1 && M <= kRefineMaxM, "M (candidates per row) must be in [1, 64 * 27]");
   NOPE_CHECK(k <= M, "k must not exceed M (candidates per row)");
   NOPE_CHECK(R >= 1, "bad arguments");
@@ -411,7 +412,7 @@ int nope_pose_refine_inplane_select(const float* sim, const float* cand_D, const
   NOPE_CHECK(sim && cand_D && cand_seed && cand_rel && cand_cossin && out_D && out_seed && out_cossin && out_aslot &&
                  out_score, "null argument");
   NOPE_CHECK(keep >= 1 && keep <= kInplaneMaxKeep, "keep must be in [1, 16]");
-  NOPE_CHECK(k >= 1 && k <= 64, "k must be in [1, 64]");
+  NOPE_CHECK(k >= 1 && k <= kMaxTopK, "k must be in [1, 64]");
   NOPE_CHECK(k <= kInplaneXY * kInplaneRoll * keep * keep, "k must not exceed the 27 * keep^2 pairs per row");
   NOPE_CHECK(R >= 1, "bad arguments");
   pose_refine_inplane_select_kernel<<<R, 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -748,7 +749,7 @@ int nope_distinct_topk(const float* sim, int R, int N, const double* rot, int G_
   NOPE_CHECK(R >= 1 && N >= 1 && N <= (1 << 30), "R (rows) must be >= 1 and N (entries per row) in [1, 2^30]");
   NOPE_CHECK(G_r >= 1 && Q >= 1 && (G_r == 1 || (int64_t)G_r * Q == R),
              "G_r (rotation sets) must be 1 or R / Q, with Q >= 1");
-  NOPE_CHECK(k >= 1 && k <= kDistinctMaxK, "k must be in [1, 64]");
+  NOPE_CHECK(k >= 1 && k <= kMaxTopK, "k must be in [1, 64]");
   NOPE_CHECK(c_thr >= -1.0 && c_thr <= 3.0, "c_thr = 1 + 2 cos(theta) must be in [-1, 3]");
   NOPE_CHECK(G >= 1 && G <= 65536, "G (symmetry groups) must be in [1, 65536]");
   // HOST symmetry groups, checked and packed for one stream-ordered upload together with the row -> group table

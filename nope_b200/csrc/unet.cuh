@@ -10,6 +10,7 @@
 #include "engine.cuh"
 #include "kernels.cuh"
 #include "linattn_tc.cuh"
+#include "rank.cuh"
 
 #include <algorithm>
 #include <cstring>

@@ -15,10 +15,10 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._lib import MAX_TOPK
 from .bop import _to_dev
 from .vsd import _stream
 
-MAX_K = 64
 MAX_SYM = 32          # discrete rotations per group, the identity included
 
 
@@ -71,8 +71,8 @@ def distinct_topk(sim, rotations, k, min_angle_deg, symmetries=None):
                          f"{tuple(sim.shape) if torch.is_tensor(sim) else type(sim).__name__}")
     if sim.dtype != torch.float32:
         raise ValueError(f"sim must be float32, got {sim.dtype}")
-    if isinstance(k, bool) or not isinstance(k, numbers.Integral) or not 1 <= k <= MAX_K:
-        raise ValueError(f"k must be an integer in [1, {MAX_K}], got {k!r}")
+    if isinstance(k, bool) or not isinstance(k, numbers.Integral) or not 1 <= k <= MAX_TOPK:
+        raise ValueError(f"k must be an integer in [1, {MAX_TOPK}], got {k!r}")
     c_thr = threshold(min_angle_deg)
     lead, N = tuple(sim.shape[:-1]), sim.shape[-1]
     R = math.prod(lead)

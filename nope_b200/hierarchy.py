@@ -15,9 +15,8 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._lib import MAX_TOPK
 from .search import row_pairs
-
-MAX_KEEP = 64        # keep and k: the CTA-wide ranking kernels hold at most 64 chosen entries
 
 
 def rotation_trace(fine_R, coarse_R):
@@ -103,12 +102,12 @@ def check_search_args(hierarchy, all_relativeR_levels, keep, k):
     for l, (p, n) in enumerate(zip(all_relativeR_levels, hierarchy.sizes)):
         if p.dim() != 3 or p.shape[1] != n or p.shape[2] != 6:
             raise ValueError(f"all_relativeR_levels[{l}] must be [B, {n}, 6], got {tuple(p.shape)}")
-    if not 1 <= keep <= MAX_KEEP:
-        raise ValueError(f"keep must be in [1, {MAX_KEEP}], got {keep}")
+    if not 1 <= keep <= MAX_TOPK:
+        raise ValueError(f"keep must be in [1, {MAX_TOPK}], got {keep}")
     if keep > hierarchy.sizes[0]:
         raise ValueError(f"keep ({keep}) exceeds the coarsest grid ({hierarchy.sizes[0]} poses)")
-    if not 1 <= k <= MAX_KEEP:
-        raise ValueError(f"k must be in [1, {MAX_KEEP}], got {k}")
+    if not 1 <= k <= MAX_TOPK:
+        raise ValueError(f"k must be in [1, {MAX_TOPK}], got {k}")
 
 
 def expand(top_idx, cells, poses, Q, M):

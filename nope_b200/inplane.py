@@ -20,9 +20,9 @@ import numbers
 import torch
 
 from . import _lib
+from ._lib import MAX_TOPK
 
 MAX_ANGLES = 360
-MAX_K = 64        # nope_topk
 
 
 def check_angles(A):
@@ -34,8 +34,8 @@ def check_angles(A):
 def check_inplane_args(A, k, N):
     """A angles, top-k over A * N (angle, pose) pairs: ValueError unless 1 <= A <= 360, 1 <= k <= 64, k <= A * N."""
     A = check_angles(A)
-    if isinstance(k, bool) or not isinstance(k, numbers.Integral) or not 1 <= k <= MAX_K:
-        raise ValueError(f"k must be an integer in [1, {MAX_K}], got {k!r}")
+    if isinstance(k, bool) or not isinstance(k, numbers.Integral) or not 1 <= k <= MAX_TOPK:
+        raise ValueError(f"k must be an integer in [1, {MAX_TOPK}], got {k!r}")
     if N < 1 or k > A * N:
         raise ValueError(f"k = {k} exceeds the {A} x {N} (angle, pose) pairs")
     return A, int(k)

@@ -22,6 +22,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._lib import MAX_TOPK
 from .inplane import check_angles, inplane_table
 from .refine import axis_angle_matrix, grid_constants, identity_centres
 from .search import row_pairs
@@ -29,7 +30,6 @@ from .search import row_pairs
 XY = 9              # pose slots per centre: the 3x3 xy lattice, identity first, then lexicographic (i, j)
 ROLL = 3            # angle slots per centre: rho, rho + phi, rho - phi
 MAX_KEEP = 16
-MAX_K = 64
 _XY_OFFSETS = [(0, 0)] + [v for v in itertools.product((-1, 0, 1), repeat=2) if v != (0, 0)]
 
 
@@ -88,7 +88,7 @@ def check_inplane_refine_args(refiner, all_relativeR, keep, k, B=None):
         raise ValueError(f"all_relativeR must be [B, {n}, 6] (the refiner's grid), got {tuple(all_relativeR.shape)}")
     if B is not None and all_relativeR.shape[0] != B:
         raise ValueError(f"all_relativeR has {all_relativeR.shape[0]} references, the reference batch {B}")
-    for name, v, hi in (("keep", keep, MAX_KEEP), ("k", k, MAX_K)):
+    for name, v, hi in (("keep", keep, MAX_KEEP), ("k", k, MAX_TOPK)):
         if isinstance(v, bool) or not isinstance(v, numbers.Integral) or not 1 <= v <= hi:
             raise ValueError(f"{name} must be an integer in [1, {hi}], got {v!r}")
     if keep > refiner.angles * n:

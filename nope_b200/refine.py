@@ -18,7 +18,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .hierarchy import MAX_KEEP, rotation_trace
+from ._lib import MAX_TOPK
+from .hierarchy import rotation_trace
 from .search import row_pairs
 
 STENCIL = 27        # the 3x3x3 lattice: slot 0 the identity, then the other 26 in lexicographic (i, j, l) order
@@ -108,12 +109,12 @@ def check_refine_args(refiner, all_relativeR, keep, k, B=None):
         raise ValueError(f"all_relativeR must be [B, {n}, 6] (the refiner's grid), got {tuple(all_relativeR.shape)}")
     if B is not None and all_relativeR.shape[0] != B:
         raise ValueError(f"all_relativeR has {all_relativeR.shape[0]} references, the reference batch {B}")
-    if not 1 <= keep <= MAX_KEEP:
-        raise ValueError(f"keep must be in [1, {MAX_KEEP}], got {keep}")
+    if not 1 <= keep <= MAX_TOPK:
+        raise ValueError(f"keep must be in [1, {MAX_TOPK}], got {keep}")
     if keep > n:
         raise ValueError(f"keep ({keep}) exceeds the grid ({n} poses)")
-    if not 1 <= k <= MAX_KEEP:
-        raise ValueError(f"k must be in [1, {MAX_KEEP}], got {k}")
+    if not 1 <= k <= MAX_TOPK:
+        raise ValueError(f"k must be in [1, {MAX_TOPK}], got {k}")
     if k > keep * STENCIL:
         raise ValueError(f"k ({k}) exceeds the {keep * STENCIL} candidates of keep = {keep}")
 
