@@ -209,11 +209,17 @@ def ptr(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def stream(device):
+    """The current CUDA stream of `device`, as the last argument of every launching entry point takes it."""
+    import torch
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
 def build_engine(kind, create_args, tensors, configure=None):
     """Builds a `kind` engine ("unet", "encoder", "vae", "vae_decoder" or "ldm"): nope_<kind>_create(&h,
     *create_args), then configure(lib, h) (options that must precede the weights), then every (key, tensor) of
-    `tensors` staged as contiguous CPU fp32, then nope_<kind>_finalize.  Returns the handle; if any step raises, the
-    engine is destroyed first."""
+    `tensors` staged as contiguous CPU fp32, then nope_<kind>_finalize.  tensors None stops before the weights: the
+    engine is weightless and not finalized.  Returns the handle; if any step raises, the engine is destroyed first."""
     import torch
     lib = load()
     h = C.c_void_p()
@@ -221,13 +227,54 @@ def build_engine(kind, create_args, tensors, configure=None):
     try:
         if configure is not None:
             configure(lib, h)
-        load_tensor = getattr(lib, f"nope_{kind}_load_tensor")
-        for k, v in tensors:
-            t = v.detach().to("cpu", torch.float32).contiguous()
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            check(load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
-        check(getattr(lib, f"nope_{kind}_finalize")(h))
+        if tensors is not None:
+            load_tensor = getattr(lib, f"nope_{kind}_load_tensor")
+            for k, v in tensors:
+                t = v.detach().to("cpu", torch.float32).contiguous()
+                shape = (C.c_int64 * t.dim())(*t.shape)
+                check(load_tensor(h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
+            check(getattr(lib, f"nope_{kind}_finalize")(h))
     except BaseException:
         getattr(lib, f"nope_{kind}_destroy")(h)
         raise
     return h
+
+
+class Engine:
+    """Owns one nope_<kind>_* handle `h` (None while there is none).  `handle` creates it weightless and configured,
+    `build` builds it with weights (destroying the previous one first), `destroy` releases it; a handle a build
+    leaves half made is destroyed by build_engine, so `h` is either None or a whole engine."""
+
+    def __init__(self, kind):
+        self.kind, self.h, self.finalized = kind, None, False
+
+    def handle(self, create_args, configure=None):
+        """The handle; a weightless one, configured, if there is none yet."""
+        if self.h is None:
+            self.h = build_engine(self.kind, create_args, None, configure)
+        return self.h
+
+    def build(self, create_args, tensors, configure=None):
+        self.destroy()
+        self.h = build_engine(self.kind, create_args, tensors, configure)
+        self.finalized = True
+        return self.h
+
+    def destroy(self):
+        h, self.h, self.finalized = self.h, None, False
+        if h is not None:
+            getattr(load(), f"nope_{self.kind}_destroy")(h)
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
+
+    def call(self, name, *args):
+        """nope_<kind>_<name>(h, *args), raising NopeError if it fails."""
+        check(getattr(load(), f"nope_{self.kind}_{name}")(self.h, *args))
+
+    def launch_count(self):
+        """Kernels the handle's last call launched; 0 without a handle."""
+        return 0 if self.h is None else int(getattr(load(), f"nope_{self.kind}_last_launch_count")(self.h))

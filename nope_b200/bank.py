@@ -13,7 +13,6 @@ precision and the encoder's.  A search refuses a model whose descriptor differs.
 under the same architecture and precision: a bank built before `load_state_dict` of other weights is stale, and it is
 the caller's to rebuild it.  The bank is independent of the similarity metric: a search scores with the model's
 current metric and threshold.  Written against any engine with `sweep()` (`UNet`, `UNetModelPose`)."""
-import ctypes as C
 
 import torch
 
@@ -259,7 +258,7 @@ def score_rows(bank, query, plan, metric, threshold, k):
             _lib.ptr(q), _lib.ptr(t), D * A, t.shape[0], N, t.shape[2], t.shape[3] * t.shape[4],
             _lib.ptr(plan.gslots), _lib.ptr(plan.row_off), plan.G, A, _METRICS[metric], float(threshold), k,
             _lib.ptr(sim), _lib.ptr(topv) if k else None, _lib.ptr(topi) if k else None,
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            _lib.stream(dev)))
     return sim, (topi if k else None)
 
 

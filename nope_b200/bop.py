@@ -9,7 +9,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .vsd import _stream
 
 # the recall thresholds: float64 values of numpy.arange, so ties at exactly a threshold depend on their last bits
 VSD_TAUS = np.arange(0.05, 0.51, 0.05)          # x diameter: the misalignment tolerances of AR_VSD
@@ -168,7 +167,7 @@ def pose_errors(points, R_est, t_est, R_gt, t_gt, K, syms):
         mspd = torch.empty((F_, P), device=dev, dtype=torch.float64)
         _lib.check(_lib.load().nope_pose_errors(
             _lib.ptr(p), p.shape[0], _lib.ptr(s), s.shape[0], _lib.ptr(gt), _lib.ptr(est), k.data_ptr(), F_, P,
-            _lib.ptr(mssd), _lib.ptr(mspd), _stream(dev)))
+            _lib.ptr(mssd), _lib.ptr(mspd), _lib.stream(dev)))
     return mssd, mspd
 
 

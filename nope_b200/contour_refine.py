@@ -13,7 +13,6 @@ from ._posefit import MAX_BATCH, MAX_ITERS, _masks, broadcast_t, check_iters, cu
     pack_refined, refine_outputs, taus, workspace
 from .translation import occluder_masks
 from .bop import _to_dev
-from .vsd import _stream
 
 DEFAULT_ITERS = 10           # from the convergence table of DESIGN.md section 20
 TAU_START = 0.15             # the default schedule: tau_0 = TAU_START s ... tau_iters = TAU_END s, geometric, with
@@ -48,7 +47,7 @@ def mask_sdf(masks):
     with torch.cuda.device(dev):
         md = _to_dev(m, dev, torch.uint8)
         out = torch.empty((F_, H, W), device=dev, dtype=torch.float64)
-        _lib.check(_lib.load().nope_mask_sdf(_lib.ptr(md), F_, H, W, _lib.ptr(out), _stream(dev)))
+        _lib.check(_lib.load().nope_mask_sdf(_lib.ptr(md), F_, H, W, _lib.ptr(out), _lib.stream(dev)))
     return out
 
 
@@ -93,5 +92,5 @@ def refine_pose_contour(mesh, R, t, K, masks, iters=DEFAULT_ITERS, tau=None, zne
             _lib.ptr(mesh.vertices), mesh.vertices.shape[0], _lib.ptr(mesh.faces), mesh.num_faces, _lib.ptr(Rd),
             _lib.ptr(t0), _lib.ptr(md), _lib.ptr(od), k.data_ptr(), F_, P, H, W, mesh.radius, tv.ctypes.data, iters,
             float(znear), _lib.ptr(ws), _lib.ptr(R_out), _lib.ptr(t_out), _lib.ptr(fit), _lib.ptr(sums),
-            _stream(dev)))
+            _lib.stream(dev)))
     return pack_refined(R_out, t_out, fit, sums, FIT_FIELDS)

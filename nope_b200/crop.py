@@ -190,16 +190,13 @@ def crop_frames(frames, inv_maps, image_size=256, masks=None, frame_idx=None):
         out = torch.empty((B, 3, S, S), device=dev, dtype=torch.float32)
         _lib.check(_lib.load().nope_crop_frames(
             _lib.ptr(fr), F_, H, W, Cn, _lib.ptr(mk), _lib.ptr(fi), _lib.ptr(mp), B, S, _lib.ptr(out),
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            _lib.stream(dev)))
     return out
 
 
 # ------------------------------------------------------------------ the crop camera (DESIGN.md section 23)
 MAX_CAMERAS = 65535      # F (poses, detections) and P (rotations per pose) of nope_crop_camera / nope_crop_rotate
 
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _camera(pose, keep_inplane, dev):
@@ -217,7 +214,7 @@ def _camera(pose, keep_inplane, dev):
     with torch.cuda.device(dev):
         out = torch.empty((F_, 3, 3), device=dev, dtype=torch.float64)
         _lib.check(_lib.load().nope_crop_camera(C.c_void_p(host.ctypes.data), F_, int(bool(keep_inplane)),
-                                                _lib.ptr(out), _stream(dev)))
+                                                _lib.ptr(out), _lib.stream(dev)))
     return out
 
 
@@ -283,7 +280,7 @@ def _rotate(R, Rv, to_camera, name):
         src = R.detach().to(torch.float64).contiguous()
         out = torch.empty_like(src)
         _lib.check(_lib.load().nope_crop_rotate(_lib.ptr(Rv.contiguous()), F_, _lib.ptr(src), P, int(to_camera),
-                                                _lib.ptr(out), _stream(dev)))
+                                                _lib.ptr(out), _lib.stream(dev)))
     return out
 
 

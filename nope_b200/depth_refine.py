@@ -11,7 +11,7 @@ from . import _lib
 from ._posefit import MAX_ITERS, _masks, _tensor, broadcast_t, cuda_device, fit_args, geometric, pack_refined, \
     refine_outputs, taus, workspace
 from .bop import _to_dev
-from .vsd import MAX_SIDE, _stream
+from .vsd import MAX_SIDE
 
 DEFAULT_ITERS = 6            # from the convergence table of DESIGN.md section 19
 TAU_START = 0.5              # the default schedule: tau_0 = TAU_START d ... tau_iters = TAU_END d, geometric
@@ -72,5 +72,5 @@ def refine_pose_depth(mesh, R, t, K, depth, masks=None, iters=DEFAULT_ITERS, tau
             _lib.ptr(mesh.vertices), mesh.vertices.shape[0], _lib.ptr(mesh.faces), mesh.num_faces, _lib.ptr(Rd),
             _lib.ptr(t0), _lib.ptr(Sd), _lib.ptr(md), k.data_ptr(), F_, P, H, W, rho, tv.ctypes.data, iters,
             float(znear), _lib.ptr(ws), _lib.ptr(R_out), _lib.ptr(t_out), _lib.ptr(fit), _lib.ptr(sums),
-            _stream(dev)))
+            _lib.stream(dev)))
     return pack_refined(R_out, t_out, fit, sums, FIT_FIELDS)

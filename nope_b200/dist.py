@@ -8,7 +8,6 @@ merges the gathered records, and the buffers are preallocated: no torch sort / g
 the path.  One process per GPU, torch.distributed (NCCL on GPUs; gloo in the CPU tests of the
 collective plumbing, where the merge runs as the torch restatement `merge_topk`).  The reference
 has no inference-time sharding; Lightning DDP there only shards the dataloader."""
-import ctypes as C
 
 import torch
 import torch.distributed as dist
@@ -85,7 +84,7 @@ class ShardedSweep:
                 _lib.check(_lib.load().nope_topk_merge(
                     _lib.ptr(recv), self.world, pack, B, k, n_poses, per, 1 if want_sim else 0,
                     _lib.ptr(sim), _lib.ptr(topv), _lib.ptr(topi),
-                    C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                    _lib.stream(dev)))
             return sim, topi
         # CPU (gloo) restatement: the collective plumbing tests
         off_i, off_s, _ = record_layout(B, k, per, want_sim)

@@ -17,7 +17,6 @@ import torch
 from . import _lib
 from ._lib import MAX_TOPK
 from .bop import _to_dev
-from .vsd import _stream
 
 MAX_SYM = 32          # discrete rotations per group, the identity included
 
@@ -105,5 +104,5 @@ def distinct_topk(sim, rotations, k, min_angle_deg, symmetries=None):
         idx = torch.empty(lead + (k,), device=dev, dtype=torch.int64)
         _lib.check(_lib.load().nope_distinct_topk(
             _lib.ptr(s), R, N, _lib.ptr(rd), G_r, R // G_r, disc.ctypes.data, n_disc.ctypes.data, axis.ctypes.data,
-            len(groups), group.ctypes.data, k, c_thr, _lib.ptr(idx), _lib.ptr(score), _stream(dev)))
+            len(groups), group.ctypes.data, k, c_thr, _lib.ptr(idx), _lib.ptr(score), _lib.stream(dev)))
     return score, idx

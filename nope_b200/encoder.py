@@ -19,8 +19,6 @@ registers (template.py:40) are accepted and ignored.
 split precision above; "fp16" is the opt-in fast mode with single fp16 weights and stored activations and fp32
 accumulation, one tensor-core product per tap instead of three.  "fp16" has no torch-backend or CPU path.
 """
-import ctypes as C
-
 import torch
 from torch import nn
 import torch.nn.functional as F
@@ -45,6 +43,50 @@ def precision_option(kind, precision):
     if value == 0:
         return None
     return lambda lib, h: _lib.check(getattr(lib, f"nope_{kind}_set_option")(h, b"precision", value))
+
+
+def native_encode(kind, engine, device, image, D, name, A=None, pairs=None):
+    """One encode by the native `kind` engine ("encoder" or "vae"), which `engine()` returns built, on `device`:
+    images [B,3,256,256] -> D-channel latents [B,D,32,32] (nope_<kind>_encode); with A (checked), the latents of the
+    A in-plane rotated copies of every image, [B,A,D,32,32] (_encode_inplane); with pairs = (image_idx [P], cossin
+    [P, 2]), the latent of image image_idx[p] rotated by cossin[p], [P,D,32,32] (_encode_rotated).  Images of another
+    shape raise NopeError naming the `name` encoder; malformed pairs raise ValueError."""
+    if image.dim() != 4 or tuple(image.shape[1:]) != (3, 256, 256) or image.shape[0] < 1:
+        raise _lib.NopeError(f"the {name} encoder is built for [B, 3, 256, 256] inputs, got {tuple(image.shape)}")
+    x = image.to(device=device, dtype=torch.float32).contiguous()
+    B = x.shape[0]
+    fn, args, lead = "encode", (), (B,)
+    if A is not None:
+        from .inplane import _on_device, inplane_table
+        fn, args, lead = "encode_inplane", (_lib.ptr(_on_device(inplane_table, A, device)), A), (B, A)
+    elif pairs is not None:
+        image_idx, cossin = pairs
+        if image_idx.dim() != 1 or tuple(cossin.shape) != (image_idx.shape[0], 2) or image_idx.shape[0] < 1:
+            raise ValueError(f"image_idx [P] and cossin [P, 2] with P >= 1 expected, got {tuple(image_idx.shape)} and "
+                             f"{tuple(cossin.shape)}")
+        idx = image_idx.to(device=device, dtype=torch.int32).contiguous()
+        cs = cossin.to(device=device, dtype=torch.float32).contiguous()
+        fn, args, lead = "encode_rotated", (_lib.ptr(idx), _lib.ptr(cs), idx.shape[0]), (idx.shape[0],)
+    out = torch.empty(lead + (D, 32, 32), device=device, dtype=torch.float32)
+    with torch.cuda.device(device):
+        _lib.check(getattr(_lib.load(), f"nope_{kind}_{fn}")(engine(), _lib.ptr(x), B, *args, _lib.ptr(out),
+                                                            _lib.stream(device)))
+    return out
+
+
+def native_run_block(kind, h, device, name, x, out_chw, want_pair=None):
+    """One module `name` of the built native `kind` engine `h` on its own (nope_<kind>_run_block): x [n, C, H, H] ->
+    out [n, *out_chw], fp32 NCHW.  want_pair None is the template encoder, whose call has no (hi, lo) output; else
+    -> (out, pair), pair the hi + lo copy when want_pair, else None."""
+    x = x.to(device=device, dtype=torch.float32).contiguous()
+    out = torch.empty((x.shape[0],) + out_chw, device=device)
+    pair = torch.empty_like(out) if want_pair else None
+    outs = (_lib.ptr(out),) if want_pair is None else (_lib.ptr(out), _lib.ptr(pair))
+    with torch.cuda.device(device):
+        _lib.check(getattr(_lib.load(), f"nope_{kind}_run_block")(h, name.encode(), _lib.ptr(x), x.shape[1],
+                                                                 x.shape[2], x.shape[0], *outs, out.numel(),
+                                                                 _lib.stream(device)))
+    return out if want_pair is None else (out, pair)
 
 
 class _Bottleneck(nn.Module):
@@ -118,8 +160,8 @@ class FeatureExtractor(nn.Module):
         if backend not in ("auto", "b200", "torch"):
             raise ValueError("backend must be 'auto', 'b200' or 'torch'")
         self.backend = backend
-        self._h = None
-        self._h_device = None
+        self._native = _lib.Engine("encoder")
+        self._native_device = None
         check_precision(precision)
         if precision != "split" and backend == "torch":
             raise _lib.NopeError(f"precision={precision!r} is a mode of the native engine; the torch backend has "
@@ -141,28 +183,23 @@ class FeatureExtractor(nn.Module):
         return super().load_state_dict(own, strict=strict)
 
     # ------------------------------------------------------------------ native engine
-    def _drop_engine(self):
-        if self._h is not None:
-            try:
-                _lib.load().nope_encoder_destroy(self._h)
-            except Exception:
-                pass
-            self._h = None
+    @property
+    def _h(self):
+        """the native engine's handle, None while there is none"""
+        return self._native.h
 
-    def __del__(self):
-        self._drop_engine()
+    def _drop_engine(self):
+        self._native.destroy()
 
     def _engine(self, device):
         """Builds the native engine from this module's current parameters (once per device)."""
-        if self._h is not None and self._h_device == device:
-            return self._h
-        self._drop_engine()
-        tensors = [(k, v) for k, v in self.state_dict().items()
-                   if not (k.endswith("num_batches_tracked") or k.startswith("backbone.fc."))]
-        self._h = _lib.build_engine("encoder", (self.latent_dim, device.index or 0), tensors,
-                                    configure=precision_option("encoder", self.precision))
-        self._h_device = device
-        return self._h
+        if self._native.h is None or self._native_device != device:
+            tensors = [(k, v) for k, v in self.state_dict().items()
+                       if not (k.endswith("num_batches_tracked") or k.startswith("backbone.fc."))]
+            self._native.build((self.latent_dim, device.index or 0), tensors,
+                               precision_option("encoder", self.precision))
+            self._native_device = device
+        return self._native.h
 
     def _use_native(self, device):
         if self.backend == "torch":
@@ -182,14 +219,7 @@ class FeatureExtractor(nn.Module):
         reference's fp32 path; `mode` is accepted and ignored as in the reference."""
         p = next(self.parameters())
         if self._use_native(p.device):
-            if image.shape[-2:] != (256, 256):
-                raise _lib.NopeError("the native encoder is built for 256x256 inputs")
-            x = image.to(device=p.device, dtype=torch.float32).contiguous()
-            out = torch.empty((x.shape[0], self.latent_dim, 32, 32), device=p.device, dtype=torch.float32)
-            with torch.cuda.device(p.device):
-                _lib.check(_lib.load().nope_encoder_encode(
-                    self._engine(p.device), _lib.ptr(x), x.shape[0], _lib.ptr(out),
-                    C.c_void_p(torch.cuda.current_stream(p.device).cuda_stream)))
+            out = native_encode("encoder", lambda: self._engine(p.device), p.device, image, self.latent_dim, "native")
             return F.normalize(out, dim=1) if self.normalize else out
         image = image.to(device=p.device, dtype=p.dtype)
         prev = torch.backends.cudnn.allow_tf32
@@ -210,35 +240,23 @@ class FeatureExtractor(nn.Module):
         p = next(self.parameters())
         if not self._use_native(p.device):
             raise _lib.NopeError("run_block needs the native engine on a CUDA device")
-        x = x.to(device=p.device, dtype=torch.float32).contiguous()
         if x.dim() != 4:
             raise _lib.NopeError(f"run_block takes [n, C, H, H] inputs, got {tuple(x.shape)}")
-        out = torch.empty((x.shape[0],) + _encoder_block_out(name, self.latent_dim), device=p.device)
-        with torch.cuda.device(p.device):
-            _lib.check(_lib.load().nope_encoder_run_block(
-                self._engine(p.device), name.encode(), _lib.ptr(x), x.shape[1], x.shape[2], x.shape[0], _lib.ptr(out),
-                out.numel(), C.c_void_p(torch.cuda.current_stream(p.device).cuda_stream)))
-        return out
+        return native_run_block("encoder", self._engine(p.device), p.device, name, x,
+                                _encoder_block_out(name, self.latent_dim))
 
     @torch.no_grad()
     def encode_image_inplane(self, image, A):
         """image [B,3,256,256] -> [B,A,D,32,32]: the latents of the A in-plane rotated copies of every image
         (nope_b200.inplane, DESIGN.md section 11), equal to encode_image of inplane.rotate_images(image, A) flattened
         to [B*A, ...], without forming that batch.  Native engine only: the torch backend raises NopeError."""
-        from .inplane import _on_device, check_angles, inplane_table
+        from .inplane import check_angles
         A = check_angles(A)
         p = next(self.parameters())
         if not self._use_native(p.device):
             raise _lib.NopeError("encode_image_inplane needs the native engine on a CUDA device "
                                  "(no torch-backend path)")
-        if image.dim() != 4 or tuple(image.shape[1:]) != (3, 256, 256):
-            raise _lib.NopeError("the native encoder is built for [B, 3, 256, 256] inputs")
-        x = image.to(device=p.device, dtype=torch.float32).contiguous()
-        out = torch.empty((x.shape[0], A, self.latent_dim, 32, 32), device=p.device, dtype=torch.float32)
-        with torch.cuda.device(p.device):
-            _lib.check(_lib.load().nope_encoder_encode_inplane(
-                self._engine(p.device), _lib.ptr(x), x.shape[0], _lib.ptr(_on_device(inplane_table, A, p.device)),
-                A, _lib.ptr(out), C.c_void_p(torch.cuda.current_stream(p.device).cuda_stream)))
+        out = native_encode("encoder", lambda: self._engine(p.device), p.device, image, self.latent_dim, "native", A=A)
         return F.normalize(out, dim=2) if self.normalize else out
 
     @torch.no_grad()
@@ -251,18 +269,6 @@ class FeatureExtractor(nn.Module):
         if not self._use_native(p.device):
             raise _lib.NopeError("encode_image_rotated needs the native engine on a CUDA device "
                                  "(no torch-backend path)")
-        if image.dim() != 4 or tuple(image.shape[1:]) != (3, 256, 256):
-            raise _lib.NopeError("the native encoder is built for [B, 3, 256, 256] inputs")
-        if image_idx.dim() != 1 or tuple(cossin.shape) != (image_idx.shape[0], 2) or image_idx.shape[0] < 1:
-            raise ValueError(f"image_idx [P] and cossin [P, 2] with P >= 1 expected, got {tuple(image_idx.shape)} and "
-                             f"{tuple(cossin.shape)}")
-        x = image.to(device=p.device, dtype=torch.float32).contiguous()
-        idx = image_idx.to(device=p.device, dtype=torch.int32).contiguous()
-        cs = cossin.to(device=p.device, dtype=torch.float32).contiguous()
-        P = idx.shape[0]
-        out = torch.empty((P, self.latent_dim, 32, 32), device=p.device, dtype=torch.float32)
-        with torch.cuda.device(p.device):
-            _lib.check(_lib.load().nope_encoder_encode_rotated(
-                self._engine(p.device), _lib.ptr(x), x.shape[0], _lib.ptr(idx), _lib.ptr(cs), P, _lib.ptr(out),
-                C.c_void_p(torch.cuda.current_stream(p.device).cuda_stream)))
+        out = native_encode("encoder", lambda: self._engine(p.device), p.device, image, self.latent_dim, "native",
+                            pairs=(image_idx, cossin))
         return F.normalize(out, dim=1) if self.normalize else out

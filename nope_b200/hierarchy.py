@@ -9,7 +9,6 @@ Every fine pose is assigned to its nearest coarse pose (its *cell*); cells are d
 pose the search scores gets exactly the score the exhaustive sweep gives it: the search differs from the exhaustive
 one only in which poses it scores.
 """
-import ctypes as C
 
 import numpy as np
 import torch
@@ -121,7 +120,7 @@ def expand(top_idx, cells, poses, Q, M):
     with torch.cuda.device(dev):
         _lib.check(_lib.load().nope_pose_cells_expand(
             _lib.ptr(top_idx), R, keep, _lib.ptr(cells), cells.shape[0], cells.shape[1], _lib.ptr(poses), B, Q,
-            n_fine, M, _lib.ptr(cand), _lib.ptr(out), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            n_fine, M, _lib.ptr(cand), _lib.ptr(out), _lib.stream(dev)))
     return cand, out
 
 
@@ -136,7 +135,7 @@ def rank(sim, cand, n_fine, k, want_sim=True):
     with torch.cuda.device(dev):
         _lib.check(_lib.load().nope_pose_cells_rank(
             _lib.ptr(sim), _lib.ptr(cand), R, M, n_fine, k, _lib.ptr(out_sim), _lib.ptr(topv), _lib.ptr(topi),
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            _lib.stream(dev)))
     return out_sim, topv, topi
 
 

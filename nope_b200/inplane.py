@@ -13,7 +13,6 @@ The search rotates each query crop by A angles and scores every rotated copy aga
 cos / sin are computed on the host in float64 and rounded once to float32; quarter turns (4a a multiple of A) are
 exactly 0 and +-1, so bin 0 copies the image bit for bit and the 90-degree bin of a square image equals
 torch.rot90(I, 1, dims=(-2, -1))."""
-import ctypes as C
 import math
 import numbers
 
@@ -99,7 +98,7 @@ def rotate_images(images, A):
     with torch.cuda.device(x.device):
         _lib.check(_lib.load().nope_inplane_rotate(
             _lib.ptr(x), B, H, W, _lib.ptr(_on_device(inplane_table, A, x.device)), A, _lib.ptr(out),
-            C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
+            _lib.stream(x.device)))
     return out
 
 

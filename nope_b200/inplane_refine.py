@@ -13,7 +13,6 @@ image convention), and the pose it stands for R = Rz(rho) * D * template_poses[s
 pose slot, unchanged roll) is swept with the same pose bits and the same latent bits as before, so a row's best score
 never decreases and never falls below its best in-plane search score.
 """
-import ctypes as C
 import itertools
 import math
 import numbers
@@ -97,9 +96,6 @@ def check_inplane_refine_args(refiner, all_relativeR, keep, k, B=None):
         raise ValueError(f"k ({k}) exceeds the {XY * ROLL * keep * keep} pairs of keep = {keep}")
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
 
 def rotate_pairs(images, image_idx, cossin):
     """images [B, 3, H, W] (CUDA), image_idx [P] (int), cossin [P, 2] (float32) -> [P, 3, H, W] float32: image
@@ -120,7 +116,7 @@ def rotate_pairs(images, image_idx, cossin):
     out = torch.empty((idx.shape[0], 3, H, W), device=dev, dtype=torch.float32)
     with torch.cuda.device(dev):
         _lib.check(_lib.load().nope_inplane_rotate_pairs(_lib.ptr(x), B, H, W, _lib.ptr(idx), _lib.ptr(cs),
-                                                         idx.shape[0], _lib.ptr(out), _stream(dev)))
+                                                         idx.shape[0], _lib.ptr(out), _lib.stream(dev)))
     return out
 
 
@@ -141,7 +137,7 @@ def propose(D, seed, cossin, all_relativeR, stencil_, roll, Q):
         _lib.check(_lib.load().nope_pose_refine_inplane_propose(
             _lib.ptr(D), _lib.ptr(seed), _lib.ptr(cossin), R, keep, _lib.ptr(all_relativeR), B, Q, N,
             _lib.ptr(stencil_), float(roll[0]), float(roll[1]), _lib.ptr(out["D"]), _lib.ptr(out["seed"]),
-            _lib.ptr(out["rel"]), _lib.ptr(out["poses"]), _lib.ptr(out["cossin"]), _stream(dev)))
+            _lib.ptr(out["rel"]), _lib.ptr(out["poses"]), _lib.ptr(out["cossin"]), _lib.stream(dev)))
     return out
 
 
@@ -163,7 +159,7 @@ def select(sim, cand, threshold, k):
             _lib.ptr(sim), _lib.ptr(cand["D"]), _lib.ptr(cand["seed"]), _lib.ptr(cand["rel"]),
             _lib.ptr(cand["cossin"]), R, keep, k, float(threshold), _lib.ptr(out["D"]), _lib.ptr(out["seed"]),
             _lib.ptr(out["cossin"]), _lib.ptr(out["aslot"]), _lib.ptr(out["score"]), _lib.ptr(out["rel"]),
-            _stream(dev)))
+            _lib.stream(dev)))
     return out
 
 

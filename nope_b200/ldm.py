@@ -15,10 +15,10 @@ import torch
 
 from . import _lib
 from .search import coarse_to_fine_search, grid_search, refined_search
-from .unet import stage_sweep
+from .unet import SweepEngine
 
 
-class UNetModelPose:
+class UNetModelPose(SweepEngine):
     def __init__(self, injecting_condition_twice=False, pose_mlp_name="single_layer",
                  rot_representation_dim=6, encoder=None, image_size=32, in_channels=4,
                  model_channels=256, out_channels=4, num_res_blocks=2,
@@ -45,16 +45,13 @@ class UNetModelPose:
         self.context_dim = context_dim
         self.rot_representation_dim = rot_representation_dim
         self.device = torch.device(device)
-        self._chunk = chunk
         # "fp16": fp16 weights (fast); "fp16_w2": exact weights as fp16 (hi, lo) K-segments, 2x the MMA work --
         # the mode that meets the 1e-3 embedding bar (the weight rounding alone is 0.6e-3 of the fp16 mode's 1.1e-3)
         if precision not in ("fp16", "fp16_w2"):
             raise ValueError("UNetModelPose precision: 'fp16' or 'fp16_w2'")
         self.precision = precision
         self._impl = (2, 0)         # nope_ldm_set_impl (conv, attn)
-        self._options = {}          # nope_ldm_set_option name -> value, re-applied to every engine
-        self._h = None
-        self._finalized = False
+        super().__init__("ldm", chunk, 2 * model_channels)
 
     def _create_args(self):
         if self.device.type != "cuda":
@@ -70,27 +67,6 @@ class UNetModelPose:
         for k, v in self._options.items():
             _lib.check(lib.nope_ldm_set_option(h, k.encode(), v))
 
-    def _handle(self):
-        if self._h is None:         # an engine without weights yet
-            lib = _lib.load()
-            h = C.c_void_p()
-            _lib.check(lib.nope_ldm_create(C.byref(h), *self._create_args()))
-            self._h = h
-            self._configure(lib, h)
-        return self._h
-
-    def _destroy(self):
-        if self._h is not None:
-            _lib.load().nope_ldm_destroy(self._h)
-            self._h = None
-        self._finalized = False
-
-    def __del__(self):
-        try:
-            self._destroy()
-        except Exception:
-            pass
-
     def eval(self):
         return self
 
@@ -100,38 +76,18 @@ class UNetModelPose:
         again: every call builds a fresh engine (the weights are packed at finalize)."""
         from .unet import encoder_entries
         from .vae import VAE_StableDiffusion
-        create_args = self._create_args()
-        self._destroy()
-        self._h = _lib.build_engine("ldm", create_args,
-                                    ((k, v) for k, v in state_dict.items() if not k.startswith("encoder.")),
-                                    self._configure)
-        self._finalized = True
+        self._native.build(self._create_args(),
+                           ((k, v) for k, v in state_dict.items() if not k.startswith("encoder.")), self._configure)
         if isinstance(self.encoder, VAE_StableDiffusion):
             vae_sd = encoder_entries(state_dict, self.encoder)
             if vae_sd:
                 self.encoder.load_state_dict(vae_sd, strict=strict)
         return self
 
-    def set_chunk(self, hyps):
-        self._chunk = hyps
-        if self._h is not None:
-            _lib.check(_lib.load().nope_ldm_set_chunk(self._h, hyps))
-
     def set_impl(self, conv="tcgen05_2cta", attn="tcgen05"):
         impl = ({"tcgen05_2cta": 2}[conv], {"tcgen05": 0, "simt": 1}[attn])
         _lib.check(_lib.load().nope_ldm_set_impl(self._handle(), *impl))
         self._impl = impl
-
-    def set_option(self, name, value):
-        _lib.check(_lib.load().nope_ldm_set_option(self._handle(), name.encode(), int(value)))
-        self._options[name] = int(value)
-
-    @property
-    def last_launch_count(self):
-        return int(_lib.load().nope_ldm_last_launch_count(self._handle()))
-
-    def profile(self, enable):
-        _lib.check(_lib.load().nope_ldm_profile(self._handle(), 1 if enable else 0))
 
     def profile_read(self):
         """-> {'gemm': {...}, 'attention': {...}} with ms / flops / launches since profile(True)."""
@@ -155,25 +111,7 @@ class UNetModelPose:
         shards across GPUs the same way."""
         if query_feat is not None:
             query_latent = query_feat
-        if not self._finalized:
-            raise _lib.NopeError("load_state_dict() must be called before the sweep")
-        lib = _lib.load()
-        dev = self.device
-        ref_latent, poses, query_latent, Q, emb, sim, topv, topi = stage_sweep(self, ref_latent, poses, query_latent,
-                                                                               want_emb, want_sim, k, out)
-        B, N = poses.shape[0], poses.shape[1]
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            _lib.check(lib.nope_ldm_sweep_multi(self._handle(), _lib.ptr(ref_latent), _lib.ptr(poses), B, N,
-                                                _lib.ptr(query_latent), Q, _lib.ptr(emb), _lib.ptr(sim), k,
-                                                _lib.ptr(topv), _lib.ptr(topi), idx_base, C.c_void_p(stream)))
-        return {"emb": emb, "sim": sim, "topv": topv, "topi": topi}
-
-    def __call__(self, x, pose):
-        """UNetModelPose.forward(x [B,C,32,32], pose [B,6]) -> [B,C,32,32]."""
-        return self.sweep(x, pose[:, None, :], want_emb=True)["emb"][:, 0]
-
-    forward = __call__
+        return super().sweep(ref_latent, poses, query_latent, want_emb, want_sim, k, idx_base, out)
 
     def predict_pose(self, query_latent, ref_latent, all_relativeR, template_poses, k=5):
         """Latent-space form of nope_b200.model.PoseConditional.predict_pose for this UNet:
@@ -197,22 +135,6 @@ class UNetModelPose:
         return refined_search(self, ref_latent, query_latent, all_relativeR, refiner, k=k, keep=keep)
 
     # ------------------------------------------------------------------ debug / parity hooks
-    def debug_tap(self, ref_latent, poses, tap):
-        lib = _lib.load()
-        dev = self.device
-        ref_latent = ref_latent.to(dev, torch.float32).contiguous()
-        poses = poses.to(dev, torch.float32).contiguous()
-        N = poses.shape[0]
-        cap = N * 32 * 32 * 2 * self.model_channels
-        out = torch.empty(cap, device=dev, dtype=torch.float32)
-        c, s = C.c_int(), C.c_int()
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            _lib.check(lib.nope_ldm_debug_tap(self._handle(), _lib.ptr(ref_latent), _lib.ptr(poses), N,
-                                              tap.encode(), _lib.ptr(out), cap, C.byref(c), C.byref(s),
-                                              C.c_void_p(stream)))
-        return out[: N * c.value * s.value * s.value].view(N, c.value, s.value, s.value)
-
     def run_block(self, name, x0, x1=None, poses=None, out_channels=None, out_side=None):
         """One module in isolation (fp32 NCHW in / out); see nope_ldm_run_block."""
         lib = _lib.load()
@@ -226,10 +148,9 @@ class UNetModelPose:
         if poses is not None:
             poses = poses.to(dev, torch.float32).contiguous()
         out = torch.empty((n, out_channels, out_side, out_side), device=dev, dtype=torch.float32)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
             _lib.check(lib.nope_ldm_run_block(self._handle(), name.encode(), _lib.ptr(x0), C0, _lib.ptr(x1), C1,
-                                              S, n, _lib.ptr(poses), _lib.ptr(out), C.c_void_p(stream)))
+                                              S, n, _lib.ptr(poses), _lib.ptr(out), _lib.stream(dev)))
         return out
 
 
@@ -239,8 +160,7 @@ def mh_attention(qkv, impl="tcgen05"):
     qkv = qkv.to(torch.float32).contiguous()
     n_img, n_tok, c3 = qkv.shape
     out = torch.empty((n_img, n_tok, c3 // 3), device=qkv.device, dtype=torch.float32)
-    stream = torch.cuda.current_stream(qkv.device).cuda_stream
     with torch.cuda.device(qkv.device):
         _lib.check(lib.nope_op_mh_attention({"tcgen05": 0, "simt": 1}[impl], _lib.ptr(qkv), _lib.ptr(out),
-                                            n_img, n_tok, c3 // 3, C.c_void_p(stream)))
+                                            n_img, n_tok, c3 // 3, _lib.stream(qkv.device)))
     return out

@@ -12,7 +12,6 @@ Differences that are deliberate and documented:
     (model.py:256 falls through); "cosine" is an extension (SURVEY.md F3).
   * ranking is deterministic: descending score, ties -> lowest index.
 """
-import ctypes as C
 import os
 import types
 
@@ -944,7 +943,7 @@ def _score_multi(q, t, B, Q, metric, threshold, k=0, idx_base=0):
         _lib.check(_lib.load().nope_score_topk_multi(
             _lib.ptr(q), _lib.ptr(t), B, Q, t.shape[0], t.shape[1], t.shape[2], t.shape[3] * t.shape[4],
             _METRICS[metric], float(threshold), k, _lib.ptr(sim), _lib.ptr(topv), _lib.ptr(topi), idx_base,
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            _lib.stream(dev)))
     return sim, topv, topi
 
 
@@ -957,7 +956,7 @@ def topk(sim, k, idx_base=0):
     topi = torch.empty((B, k), device=sim.device, dtype=torch.int64)
     with torch.cuda.device(sim.device):
         _lib.check(lib.nope_topk(_lib.ptr(sim), B, N, k, _lib.ptr(topv), _lib.ptr(topi), idx_base,
-                                 C.c_void_p(torch.cuda.current_stream(sim.device).cuda_stream)))
+                                 _lib.stream(sim.device)))
     return topv, topi
 
 

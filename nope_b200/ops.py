@@ -1,7 +1,6 @@
 """Per-op entry points of the C ABI (include/nope_b200.h, "per-op entry points"), bound
 for the parity tests: each runs ONE layer type of the reference UNet on fp32 NCHW CUDA
 tensors through the same kernels the sweep uses."""
-import ctypes as C
 
 import torch
 
@@ -9,9 +8,6 @@ from . import _lib
 
 _IMPL = {"tcgen05_2cta": 2}
 
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _f32(t):
@@ -32,7 +28,7 @@ def conv(x0, weight, bias=None, x1=None, mode="3x3", impl="tcgen05_2cta"):
     with torch.cuda.device(x0.device):
         _lib.check(lib.nope_op_conv(_IMPL[impl], m, _lib.ptr(x0), c0, _lib.ptr(x1),
                                     0 if x1 is None else x1.shape[1], _lib.ptr(weight),
-                                    _lib.ptr(bias), _lib.ptr(out), n, h, w, cout, _stream(x0.device)))
+                                    _lib.ptr(bias), _lib.ptr(out), n, h, w, cout, _lib.stream(x0.device)))
     return out
 
 
@@ -50,7 +46,7 @@ def conv_gn(x0, weight, bias, gamma, beta, groups, silu=True, x1=None, mode="3x3
                                        0 if x1 is None else x1.shape[1], _lib.ptr(weight),
                                        _lib.ptr(bias), _lib.ptr(gamma), _lib.ptr(beta), groups,
                                        1 if silu else 0, _lib.ptr(out), n, h, w, cout,
-                                       _stream(x0.device)))
+                                       _lib.stream(x0.device)))
     return out
 
 
@@ -73,7 +69,7 @@ def conv_gn_fused(x0, weight, bias, gamma=None, beta=None, groups=8, silu=True, 
             m, precision, _lib.ptr(x0), c0, _lib.ptr(x1), 0 if x1 is None else x1.shape[1],
             _lib.ptr(weight), _lib.ptr(bias), _lib.ptr(gamma), _lib.ptr(beta), groups, 1 if silu else 0,
             _lib.ptr(chan_bias), _lib.ptr(residual), res_div, _lib.ptr(out), _lib.ptr(emit), n, h, w, cout,
-            _stream(x0.device)))
+            _lib.stream(x0.device)))
     return (out, emit) if want_emit else out
 
 
@@ -86,7 +82,7 @@ def linear_attention(qkv, impl="simt"):
     out = torch.empty((n, 128, h, w), device=qkv.device, dtype=torch.float32)
     with torch.cuda.device(qkv.device):
         _lib.check(lib.nope_op_linear_attention({"tcgen05": 0, "simt": 1}[impl], _lib.ptr(qkv), _lib.ptr(out),
-                                                n, h, w, _stream(qkv.device)))
+                                                n, h, w, _lib.stream(qkv.device)))
     return out
 
 
@@ -97,7 +93,7 @@ def attention(qkv):
     assert c == 384
     out = torch.empty((n, 128, h, w), device=qkv.device, dtype=torch.float32)
     with torch.cuda.device(qkv.device):
-        _lib.check(lib.nope_op_attention(_lib.ptr(qkv), _lib.ptr(out), n, h, w, _stream(qkv.device)))
+        _lib.check(lib.nope_op_attention(_lib.ptr(qkv), _lib.ptr(out), n, h, w, _lib.stream(qkv.device)))
     return out
 
 
@@ -107,5 +103,5 @@ def upsample2x(x):
     n, c, h, w = x.shape
     out = torch.empty((n, c, 2 * h, 2 * w), device=x.device, dtype=torch.float32)
     with torch.cuda.device(x.device):
-        _lib.check(lib.nope_op_upsample2x(_lib.ptr(x), _lib.ptr(out), n, c, h, w, _stream(x.device)))
+        _lib.check(lib.nope_op_upsample2x(_lib.ptr(x), _lib.ptr(out), n, c, h, w, _lib.stream(x.device)))
     return out

@@ -11,7 +11,6 @@ is re-proposed with the identity and re-scored to the same bits, so a row's best
 step to the next.  A hypothesis's score does not depend on the other hypotheses of its launch, so every refined pose
 has exactly the score a separate sweep of it gives.
 """
-import ctypes as C
 import itertools
 
 import numpy as np
@@ -134,7 +133,7 @@ def propose(D, seed, all_relativeR, stencil_, Q):
         _lib.check(_lib.load().nope_pose_refine_propose(
             _lib.ptr(D), _lib.ptr(seed), R, keep, _lib.ptr(all_relativeR), B, Q, N, _lib.ptr(stencil_),
             _lib.ptr(out["D"]), _lib.ptr(out["seed"]), _lib.ptr(out["rel"]), _lib.ptr(out["poses"]),
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            _lib.stream(dev)))
     return out
 
 
@@ -151,7 +150,7 @@ def select(sim, cand, threshold, k):
         _lib.check(_lib.load().nope_pose_refine_select(
             _lib.ptr(sim), _lib.ptr(cand["D"]), _lib.ptr(cand["seed"]), _lib.ptr(cand["rel"]), R, M, k,
             float(threshold), _lib.ptr(out["D"]), _lib.ptr(out["seed"]), _lib.ptr(out["score"]), _lib.ptr(out["rel"]),
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            _lib.stream(dev)))
     return out
 
 

@@ -13,7 +13,6 @@ import torch
 from . import _lib
 from ._posefit import _masks, _tensor, broadcast_t, cuda_device, fit_args, workspace
 from .bop import _to_dev
-from .vsd import _stream
 
 DEFAULT_ITERS = 4            # from the convergence table of DESIGN.md section 18
 
@@ -129,5 +128,5 @@ def estimate_translation(mesh, R, K, masks, t_init=None, diameter=None, iters=DE
         _lib.check(_lib.load().nope_fit_translation_occluded(
             _lib.ptr(mesh.vertices), mesh.vertices.shape[0], _lib.ptr(mesh.faces), mesh.num_faces, _lib.ptr(Rd),
             _lib.ptr(t0), _lib.ptr(m), _lib.ptr(o), k.data_ptr(), F_, P, H, W, float(znear), iters, _lib.ptr(depth),
-            _lib.ptr(t), _lib.ptr(iou), _lib.ptr(stats), _stream(dev)))
+            _lib.ptr(t), _lib.ptr(iou), _lib.ptr(stats), _lib.stream(dev)))
     return (t, iou, stats) if return_stats else (t, iou)

@@ -45,7 +45,90 @@ def encoder_entries(state_dict, encoder):
     return out
 
 
-class UNet:
+class SweepEngine:
+    """What UNet and UNetModelPose share on top of their nope_<kind>_* engine: the handle, chunk and options, the
+    launch profile and count, the sweep, forward and the debug tap.  A subclass provides `_create_args()` and
+    `_configure(lib, h)`, which every handle gets before its weights."""
+
+    def __init__(self, kind, chunk, tap_channels):
+        self._native = _lib.Engine(kind)
+        self._chunk = chunk
+        self._options = {}                  # nope_<kind>_set_option name -> value, applied to every engine
+        self._tap_channels = tap_channels   # debug_tap's output capacity: channels at 32 x 32 per pose
+
+    def _handle(self):
+        return self._native.handle(self._create_args(), self._configure)
+
+    def _reserve(self, hyps, refs, scores):
+        """Sizes the caller-owned workspace before a launch (UNet.reserve); the LDM engine has none."""
+
+    def set_chunk(self, hyps):
+        self._chunk = hyps
+        if self._native.h is not None:
+            self._native.call("set_chunk", hyps)
+
+    def set_option(self, name, value):
+        """Named engine option (include/nope_b200.h, nope_<kind>_set_option), e.g. the UNet's 'attn_impl' (0:
+        LinearAttention on tensor cores, 1: CUDA cores) or 'conv_impl' (2, the only one).  It is applied at once,
+        to a weightless engine if none is built yet, and kept for every later build; unknown names raise NopeError
+        and are not kept."""
+        self._handle()
+        self._native.call("set_option", name.encode(), int(value))
+        self._options[name] = int(value)
+
+    @property
+    def last_launch_count(self):
+        self._handle()
+        return self._native.launch_count()
+
+    def profile(self, enable):
+        self._handle()
+        self._native.call("profile", 1 if enable else 0)
+
+    def sweep(self, ref_feat, poses, query_feat=None, want_emb=True, want_sim=None, k=0, idx_base=0, out=None):
+        """ref_feat [B,C,32,32], poses [B,N,6] (+ query_feat [B,C,32,32]) ->
+        dict(emb [B,N,C,32,32] | None, sim [B,N] | None, topv/topi [B,k] | None).
+        query_feat may also be [B,Q,C,32,32]: Q queries per reference share the one sweep and
+        sim is [B,Q,N], topv/topi [B,Q,k].
+        `out` may carry preallocated contiguous `sim` / `topv` / `topi` tensors to write into (the
+        multi-GPU path points them into its all-gather record)."""
+        if not self._native.finalized:
+            raise _lib.NopeError("load_state_dict() must be called before the sweep")
+        dev = self.device
+        ref_feat, poses, query_feat, Q, emb, sim, topv, topi = stage_sweep(self, ref_feat, poses, query_feat,
+                                                                           want_emb, want_sim, k, out)
+        B, N = poses.shape[0], poses.shape[1]
+        self._reserve(min(self._chunk, B * N), B, B * Q * N if query_feat is not None else 0)
+        with torch.cuda.device(dev):
+            self._native.call("sweep_multi", _lib.ptr(ref_feat), _lib.ptr(poses), B, N, _lib.ptr(query_feat), Q,
+                              _lib.ptr(emb), _lib.ptr(sim), k, _lib.ptr(topv), _lib.ptr(topi), idx_base,
+                              _lib.stream(dev))
+        return {"emb": emb, "sim": sim, "topv": topv, "topi": topi}
+
+    def __call__(self, x, pose):
+        """forward(x [B,C,32,32], pose [B,6]) -> [B,C,32,32] (u_net.py:160-198, adapt_openaimodel.py)."""
+        return self.sweep(x, pose[:, None, :], want_emb=True)["emb"][:, 0]
+
+    forward = __call__
+
+    def debug_tap(self, ref_feat, poses, tap):
+        """Activation named `tap` (oracle tap names) for poses [N,6] of ONE reference."""
+        dev = self.device
+        ref_feat = ref_feat.to(dev, torch.float32).contiguous()
+        poses = poses.to(dev, torch.float32).contiguous()
+        N = poses.shape[0]
+        cap = N * 32 * 32 * self._tap_channels
+        out = torch.empty(cap, device=dev, dtype=torch.float32)
+        c, s = C.c_int(), C.c_int()
+        self._reserve(N, 1, 0)
+        self._handle()
+        with torch.cuda.device(dev):
+            self._native.call("debug_tap", _lib.ptr(ref_feat), _lib.ptr(poses), N, tap.encode(), _lib.ptr(out), cap,
+                              C.byref(c), C.byref(s), _lib.stream(dev))
+        return out[: N * c.value * s.value * s.value].view(N, c.value, s.value, s.value)
+
+
+class UNet(SweepEngine):
     def __init__(self, u_net_dim, rot_representation_dim, encoder, pose_mlp_name="single_layer",
                  init_dim=None, out_dim=None, use_hard_up_down=True, dim_mults=(1, 2, 4, 8),
                  resnet_block_groups=8, device="cuda:0", chunk=642, precision="fp16", **kwargs):
@@ -67,10 +150,7 @@ class UNet:
         self.rot_representation_dim = rot_representation_dim
         self.device = torch.device(device)
         self.precision = precision
-        self._chunk = chunk
-        self._h = None
-        self._finalized = False
-        self._options = {}
+        super().__init__("unet", chunk, 8 * u_net_dim)
         self._ws = None            # torch-owned workspace (uint8), handed to the engine
         self._ws_shape = (0, 0, 0)
         self._state = None         # last loaded UNet tensors (CPU fp32), kept for reload / partial load
@@ -86,32 +166,10 @@ class UNet:
         _lib.check(lib.nope_unet_set_chunk(h, self._chunk))
         _lib.check(lib.nope_unet_set_option(h, b"precision", PRECISIONS[self.precision]))
         for k, v in self._options.items():
-            _lib.check(lib.nope_unet_set_option(h, k.encode(), int(v)))
-
-    def _handle(self):
-        if self._h is None:         # an engine without weights yet
-            lib = _lib.load()
-            h = C.c_void_p()
-            _lib.check(lib.nope_unet_create(C.byref(h), *self._create_args()))
-            self._h = h
-            self._configure(lib, h)
-        return self._h
-
-    def _destroy(self):
-        if self._h is not None:
-            _lib.load().nope_unet_destroy(self._h)
-            self._h = None
-        self._finalized = False
-        self._ws, self._ws_shape = None, (0, 0, 0)
-
-    def __del__(self):
-        try:
-            self._destroy()
-        except Exception:
-            pass
+            _lib.check(lib.nope_unet_set_option(h, k.encode(), v))
 
     def to(self, device):
-        if self._h is not None and torch.device(device) != self.device:
+        if self._native.h is not None and torch.device(device) != self.device:
             raise _lib.NopeError("cannot move a finalized engine; construct it on the target device")
         self.device = torch.device(device)
         self.encoder.to(self.device)
@@ -161,10 +219,10 @@ class UNet:
         create_args = self._create_args()
         if enc_sd:
             self.encoder.load_state_dict(enc_sd, strict=strict)
-        self._destroy()           # weights are repacked at finalize: every load builds a fresh engine
-        self._h = _lib.build_engine("unet", create_args, merged.items(), self._configure)
+        self._native.destroy()    # weights are repacked at finalize: every load builds a fresh engine
+        self._ws, self._ws_shape = None, (0, 0, 0)
+        self._native.build(create_args, merged.items(), self._configure)
         self._state = merged
-        self._finalized = True
         self.encoder.to(self.device)
         return _Incompatible(missing, unexpected) if not strict else self
 
@@ -180,18 +238,6 @@ class UNet:
                 sd["encoder." + k] = v.detach().to("cpu")
         return sd
 
-    def set_chunk(self, hyps):
-        self._chunk = hyps
-        if self._h is not None:
-            _lib.check(_lib.load().nope_unet_set_chunk(self._h, hyps))
-
-    def set_option(self, name, value):
-        """Named engine option (include/nope_b200.h, nope_unet_set_option): 'attn_impl' (0: LinearAttention
-        on tensor cores, 1: CUDA cores) or 'conv_impl' (2, the only one).  Unknown names raise NopeError."""
-        self._options[name] = int(value)
-        if self._h is not None:
-            _lib.check(_lib.load().nope_unet_set_option(self._h, name.encode(), int(value)))
-
     def set_metric(self, metric, threshold=0.2):
         """Similarity metric of the scoring fused onto the sweep: 'l2' (the reference's, model.py:254-266),
         'cosine' or 'cosine_occlusion' (extensions; include/nope_b200.h NOPE_METRIC_*)."""
@@ -202,13 +248,6 @@ class UNet:
         if impl != "tcgen05_2cta":
             raise _lib.NopeError(f"unknown conv impl {impl!r}: the only convolution is 'tcgen05_2cta' (conv_tc2_kernel)")
         _lib.check(_lib.load().nope_unet_set_conv_impl(self._handle(), 2))
-
-    @property
-    def last_launch_count(self):
-        return int(_lib.load().nope_unet_last_launch_count(self._handle()))
-
-    def profile(self, enable):
-        _lib.check(_lib.load().nope_unet_profile(self._handle(), 1 if enable else 0))
 
     def profile_read(self):
         """-> dict(conv_ms, conv_flops (executed), conv_alg_flops, conv_launches, max_launch_tflops)."""
@@ -236,55 +275,7 @@ class UNet:
                                                    hyps, refs, scores))
         self._ws, self._ws_shape = ws, (hyps, refs, scores)
 
-    # ------------------------------------------------------------------ hot path
-    def sweep(self, ref_feat, poses, query_feat=None, want_emb=True, want_sim=None, k=0,
-              idx_base=0, out=None):
-        """ref_feat [B,C,32,32], poses [B,N,6] (+ query_feat [B,C,32,32]) ->
-        dict(emb [B,N,C,32,32] | None, sim [B,N] | None, topv/topi [B,k] | None).
-        query_feat may also be [B,Q,C,32,32]: Q queries per reference share the one sweep and
-        sim is [B,Q,N], topv/topi [B,Q,k].
-        `out` may carry preallocated contiguous `sim` / `topv` / `topi` tensors to write into (the
-        multi-GPU path points them into its all-gather record)."""
-        if not self._finalized:
-            raise _lib.NopeError("load_state_dict() must be called before the sweep")
-        lib = _lib.load()
-        dev = self.device
-        ref_feat, poses, query_feat, Q, emb, sim, topv, topi = stage_sweep(self, ref_feat, poses, query_feat,
-                                                                           want_emb, want_sim, k, out)
-        B, N = poses.shape[0], poses.shape[1]
-        self.reserve(min(self._chunk, B * N), B, B * Q * N if query_feat is not None else 0)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            _lib.check(lib.nope_unet_sweep_multi(self._handle(), _lib.ptr(ref_feat), _lib.ptr(poses), B, N,
-                                                 _lib.ptr(query_feat), Q, _lib.ptr(emb), _lib.ptr(sim), k,
-                                                 _lib.ptr(topv), _lib.ptr(topi), idx_base,
-                                                 C.c_void_p(stream)))
-        return {"emb": emb, "sim": sim, "topv": topv, "topi": topi}
-
-    def __call__(self, x, pose):
-        """UNet.forward(x [B,C,32,32], pose [B,6]) -> [B,C,32,32] (u_net.py:160-198)."""
-        out = self.sweep(x, pose[:, None, :], want_emb=True)["emb"]
-        return out[:, 0]
-
-    forward = __call__
-
-    def debug_tap(self, ref_feat, poses, tap):
-        """Activation named `tap` (oracle tap names) for poses [N,6] of ONE reference."""
-        lib = _lib.load()
-        dev = self.device
-        ref_feat = ref_feat.to(dev, torch.float32).contiguous()
-        poses = poses.to(dev, torch.float32).contiguous()
-        N = poses.shape[0]
-        cap = N * 32 * 32 * 8 * self.u_net_dim
-        out = torch.empty(cap, device=dev, dtype=torch.float32)
-        c, s = C.c_int(), C.c_int()
-        self.reserve(N, 1, 0)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            _lib.check(lib.nope_unet_debug_tap(self._handle(), _lib.ptr(ref_feat), _lib.ptr(poses), N,
-                                               tap.encode(), _lib.ptr(out), cap, C.byref(c),
-                                               C.byref(s), C.c_void_p(stream)))
-        return out[: N * c.value * s.value * s.value].view(N, c.value, s.value, s.value)
+    _reserve = reserve
 
 
 def stage_sweep(engine, ref_feat, poses, query_feat, want_emb, want_sim, k, out):

@@ -18,7 +18,6 @@ accepted under both of diffusers' namings (`query` / `key` / `value` / `proj_att
 all of them are.
 """
 from collections import OrderedDict
-import ctypes as C
 import json
 import os
 
@@ -45,71 +44,88 @@ _ATTN = "encoder.mid_block.attentions.0."
 _ATTN_RENAME = {"to_q.": "query.", "to_k.": "key.", "to_v.": "value.", "to_out.0.": "proj_attn."}
 
 
-def check_config(cfg):
-    """Raises ValueError unless `cfg` (a parsed config.json) has the SD v1 encoder configuration.  Decoder-only
-    fields (out_channels, up_block_types) and sample_size do not change the encoder and are not checked."""
-    for k, want in SD_V1_CONFIG.items():
-        got = cfg.get(k, _CONFIG_DEFAULTS[k])
+def _check_fields(cfg, fields, defaults, what):
+    """Raises ValueError unless `cfg` (a parsed config.json) has every value of `fields`; `defaults` are diffusers'
+    values for a field the file leaves out."""
+    for k, want in fields.items():
+        got = cfg.get(k, defaults[k])
         if isinstance(got, tuple):
             got = list(got)
         if got != want or type(got) is not type(want):
-            raise ValueError(f"unsupported AutoencoderKL config: {k} = {got!r} (the engine is built for {want!r})")
+            raise ValueError(f"unsupported AutoencoderKL config: {k} = {got!r} (the {what} is built for {want!r})")
+
+
+def check_config(cfg):
+    """Raises ValueError unless `cfg` (a parsed config.json) has the SD v1 encoder configuration.  Decoder-only
+    fields (out_channels, up_block_types) and sample_size do not change the encoder and are not checked."""
+    _check_fields(cfg, SD_V1_CONFIG, _CONFIG_DEFAULTS, "engine")
+
+
+class _Shapes(OrderedDict):
+    """AutoencoderKL key -> shape, in the order the layers are added"""
+
+    def conv(self, p, cout, cin, k):
+        self[p + ".weight"] = (cout, cin, k, k)
+        self[p + ".bias"] = (cout,)
+
+    def norm(self, p, c):
+        self[p + ".weight"] = (c,)
+        self[p + ".bias"] = (c,)
+
+    def resnet(self, p, cin, cout):
+        self.norm(p + ".norm1", cin)
+        self.conv(p + ".conv1", cout, cin, 3)
+        self.norm(p + ".norm2", cout)
+        self.conv(p + ".conv2", cout, cout, 3)
+        if cin != cout:
+            self.conv(p + ".conv_shortcut", cout, cin, 1)
+
+    def attention(self, p, c):
+        """a mid block's attention, 0.14-era names"""
+        self.norm(p + "group_norm", c)
+        for n in ("query", "key", "value", "proj_attn"):
+            self[p + n + ".weight"] = (c, c)
+            self[p + n + ".bias"] = (c,)
 
 
 def vae_param_shapes():
     """key -> shape of the 108 AutoencoderKL encoder tensors (0.14-era attention names) the engine loads."""
-    s = OrderedDict()
-
-    def conv(p, cout, cin, k):
-        s[p + ".weight"] = (cout, cin, k, k)
-        s[p + ".bias"] = (cout,)
-
-    def norm(p, c):
-        s[p + ".weight"] = (c,)
-        s[p + ".bias"] = (c,)
-
-    def resnet(p, cin, cout):
-        norm(p + ".norm1", cin)
-        conv(p + ".conv1", cout, cin, 3)
-        norm(p + ".norm2", cout)
-        conv(p + ".conv2", cout, cout, 3)
-        if cin != cout:
-            conv(p + ".conv_shortcut", cout, cin, 1)
-
-    conv("encoder.conv_in", 128, 3, 3)
+    s = _Shapes()
+    s.conv("encoder.conv_in", 128, 3, 3)
     cin = 128
     for i, c in enumerate(SD_V1_CONFIG["block_out_channels"]):
         for j in range(2):
-            resnet(f"encoder.down_blocks.{i}.resnets.{j}", cin, c)
+            s.resnet(f"encoder.down_blocks.{i}.resnets.{j}", cin, c)
             cin = c
         if i < 3:
-            conv(f"encoder.down_blocks.{i}.downsamplers.0.conv", c, c, 3)
-    resnet("encoder.mid_block.resnets.0", 512, 512)
-    norm(_ATTN + "group_norm", 512)
-    for n in ("query", "key", "value", "proj_attn"):
-        s[_ATTN + n + ".weight"] = (512, 512)
-        s[_ATTN + n + ".bias"] = (512,)
-    resnet("encoder.mid_block.resnets.1", 512, 512)
-    norm("encoder.conv_norm_out", 512)
-    conv("encoder.conv_out", 8, 512, 3)
-    conv("quant_conv", 8, 8, 1)
+            s.conv(f"encoder.down_blocks.{i}.downsamplers.0.conv", c, c, 3)
+    s.resnet("encoder.mid_block.resnets.0", 512, 512)
+    s.attention(_ATTN, 512)
+    s.resnet("encoder.mid_block.resnets.1", 512, 512)
+    s.norm("encoder.conv_norm_out", 512)
+    s.conv("encoder.conv_out", 8, 512, 3)
+    s.conv("quant_conv", 8, 8, 1)
     return s
 
 
-def map_state_dict(sd):
-    """AutoencoderKL state_dict (either attention naming) -> {schema key: CPU fp32 tensor}.  Ignores `decoder.*`
-    and `post_quant_conv.*`; raises KeyError for a missing or unknown key and ValueError for a wrong shape."""
-    want = vae_param_shapes()
+_DECODER_PREFIXES = ("decoder.", "post_quant_conv.")
+
+
+def _map_keys(sd, want, attn, decoder):
+    """The entries of an AutoencoderKL state_dict (either attention naming, under the attention prefix `attn`) on one
+    side, the decoder's (`decoder.*` / `post_quant_conv.*`) when `decoder`, else all others -> {schema key: CPU fp32
+    tensor}, in the order of `sd`.  Raises KeyError for a key not in `want` and ValueError for a wrong shape; a
+    missing key is a KeyError on the encoder side only."""
     out = {}
     for k, v in sd.items():
-        if k.startswith("decoder.") or k.startswith("post_quant_conv."):
+        if k.startswith(_DECODER_PREFIXES) != decoder:
             continue
         kk = k
-        if k.startswith(_ATTN):
-            rest = k[len(_ATTN):]
+        if k.startswith(attn):
+            rest = k[len(attn):]
             for a, b in _ATTN_RENAME.items():
                 if rest.startswith(a):
-                    kk = _ATTN + b + rest[len(a):]
+                    kk = attn + b + rest[len(a):]
         if kk not in want:
             raise KeyError(f"unexpected AutoencoderKL state_dict key: {k}")
         if kk in out:
@@ -118,9 +134,15 @@ def map_state_dict(sd):
             raise ValueError(f"size mismatch for {k}: checkpoint {tuple(v.shape)} vs model {tuple(want[kk])}")
         out[kk] = v.detach().to("cpu", torch.float32).contiguous()
     missing = [k for k in want if k not in out]
-    if missing:
+    if missing and not decoder:
         raise KeyError(f"AutoencoderKL state_dict is missing {len(missing)} encoder keys: {missing[:5]}")
     return out
+
+
+def map_state_dict(sd):
+    """AutoencoderKL state_dict (either attention naming) -> {schema key: CPU fp32 tensor}.  Ignores `decoder.*`
+    and `post_quant_conv.*`; raises KeyError for a missing or unknown key and ValueError for a wrong shape."""
+    return _map_keys(sd, vae_param_shapes(), _ATTN, decoder=False)
 
 
 _DEC_ATTN = "decoder.mid_block.attentions.0."
@@ -132,52 +154,27 @@ _DECODER_CONFIG_DEFAULTS = {"out_channels": 3, "up_block_types": ["UpDecoderBloc
 def check_decoder_config(cfg):
     """Raises ValueError unless `cfg` has the SD v1 decoder fields (out_channels 3, up_block_types
     4 x UpDecoderBlock2D); the other decoder dimensions are the encoder's fields, which check_config checks."""
-    for k, want in SD_V1_DECODER_CONFIG.items():
-        got = cfg.get(k, _DECODER_CONFIG_DEFAULTS[k])
-        if isinstance(got, tuple):
-            got = list(got)
-        if got != want or type(got) is not type(want):
-            raise ValueError(f"unsupported AutoencoderKL config: {k} = {got!r} (the decoder is built for {want!r})")
+    _check_fields(cfg, SD_V1_DECODER_CONFIG, _DECODER_CONFIG_DEFAULTS, "decoder")
 
 
 def vae_decoder_param_shapes():
     """key -> shape of the 140 AutoencoderKL decoder tensors (post_quant_conv and decoder.*, 0.14-era attention
     names) the decoder engine loads."""
-    s = OrderedDict()
-
-    def conv(p, cout, cin, k):
-        s[p + ".weight"] = (cout, cin, k, k)
-        s[p + ".bias"] = (cout,)
-
-    def norm(p, c):
-        s[p + ".weight"] = (c,)
-        s[p + ".bias"] = (c,)
-
-    def resnet(p, cin, cout):
-        norm(p + ".norm1", cin)
-        conv(p + ".conv1", cout, cin, 3)
-        norm(p + ".norm2", cout)
-        conv(p + ".conv2", cout, cout, 3)
-        if cin != cout:
-            conv(p + ".conv_shortcut", cout, cin, 1)
-
-    conv("post_quant_conv", 4, 4, 1)
-    conv("decoder.conv_in", 512, 4, 3)
-    resnet("decoder.mid_block.resnets.0", 512, 512)
-    norm(_DEC_ATTN + "group_norm", 512)
-    for n in ("query", "key", "value", "proj_attn"):
-        s[_DEC_ATTN + n + ".weight"] = (512, 512)
-        s[_DEC_ATTN + n + ".bias"] = (512,)
-    resnet("decoder.mid_block.resnets.1", 512, 512)
+    s = _Shapes()
+    s.conv("post_quant_conv", 4, 4, 1)
+    s.conv("decoder.conv_in", 512, 4, 3)
+    s.resnet("decoder.mid_block.resnets.0", 512, 512)
+    s.attention(_DEC_ATTN, 512)
+    s.resnet("decoder.mid_block.resnets.1", 512, 512)
     cin = 512
     for i, c in enumerate(reversed(SD_V1_CONFIG["block_out_channels"])):
         for j in range(3):
-            resnet(f"decoder.up_blocks.{i}.resnets.{j}", cin, c)
+            s.resnet(f"decoder.up_blocks.{i}.resnets.{j}", cin, c)
             cin = c
         if i < 3:
-            conv(f"decoder.up_blocks.{i}.upsamplers.0.conv", c, c, 3)
-    norm("decoder.conv_norm_out", 128)
-    conv("decoder.conv_out", 3, 128, 3)
+            s.conv(f"decoder.up_blocks.{i}.upsamplers.0.conv", c, c, 3)
+    s.norm("decoder.conv_norm_out", 128)
+    s.conv("decoder.conv_out", 3, 128, 3)
     return s
 
 
@@ -186,23 +183,7 @@ def map_decoder_state_dict(sd):
     {schema key: CPU fp32 tensor}; other entries are left to map_state_dict.  Raises KeyError for an unknown key and
     ValueError for a wrong shape; missing keys are allowed (a checkpoint without a decoder)."""
     want = vae_decoder_param_shapes()
-    out = {}
-    for k, v in sd.items():
-        if not (k.startswith("decoder.") or k.startswith("post_quant_conv.")):
-            continue
-        kk = k
-        if k.startswith(_DEC_ATTN):
-            rest = k[len(_DEC_ATTN):]
-            for a, b in _ATTN_RENAME.items():
-                if rest.startswith(a):
-                    kk = _DEC_ATTN + b + rest[len(a):]
-        if kk not in want:
-            raise KeyError(f"unexpected AutoencoderKL state_dict key: {k}")
-        if kk in out:
-            raise KeyError(f"AutoencoderKL state_dict has {kk} under both attention namings")
-        if tuple(v.shape) != tuple(want[kk]):
-            raise ValueError(f"size mismatch for {k}: checkpoint {tuple(v.shape)} vs model {tuple(want[kk])}")
-        out[kk] = v.detach().to("cpu", torch.float32).contiguous()
+    out = _map_keys(sd, want, _DEC_ATTN, decoder=True)
     return OrderedDict((k, out[k]) for k in want if k in out)
 
 
@@ -247,8 +228,8 @@ class VAE_StableDiffusion:
         """precision: the encoder engine's arithmetic, "split" (default, fp32-accurate) or "fp16" (the fast mode,
         DESIGN.md section 22); the decoder is always split precision."""
         from .encoder import check_precision
-        self._h = None
-        self._dec_h = None
+        self._native = _lib.Engine("vae")
+        self._native_decoder = _lib.Engine("vae_decoder")
         check_precision(precision)
         self.precision = precision
         if using_KL:
@@ -314,89 +295,51 @@ class VAE_StableDiffusion:
     # ------------------------------------------------------------------ native engines
     def _drop_engine(self):
         """Destroys both engines (encoder and decoder)."""
-        for attr, fn in (("_h", "nope_vae_destroy"), ("_dec_h", "nope_vae_decoder_destroy")):
-            h = getattr(self, attr, None)
-            if h is not None:
-                try:
-                    getattr(_lib.load(), fn)(h)
-                except Exception:
-                    pass
-                setattr(self, attr, None)
-
-    def __del__(self):
-        self._drop_engine()
+        self._native.destroy()
+        self._native_decoder.destroy()
 
     def _engine(self):
-        if self._h is not None:
-            return self._h
-        if self._sd is None:
-            raise _lib.NopeError("VAE_StableDiffusion has no weights: pass pretrained_path or call load_state_dict")
-        from .encoder import precision_option
-        self._h = _lib.build_engine("vae", (self.device.index or 0,), self._sd.items(),
-                                    configure=precision_option("vae", self.precision))
-        return self._h
+        if self._native.h is None:
+            if self._sd is None:
+                raise _lib.NopeError("VAE_StableDiffusion has no weights: pass pretrained_path or call load_state_dict")
+            from .encoder import precision_option
+            self._native.build((self.device.index or 0,), self._sd.items(), precision_option("vae", self.precision))
+        return self._native.h
 
-    def _images(self, image):
+    def _encode(self, image, **kwargs):
+        """the CUDA-only refusals, then encoder.native_encode (A= or pairs= in `kwargs`) on the encoder engine"""
+        from .encoder import native_encode
         if self.device.type != "cuda":
             raise _lib.NopeError("VAE_StableDiffusion needs a CUDA device (no CPU path)")
         if not isinstance(image, torch.Tensor) or image.device.type != "cuda":
             raise _lib.NopeError("VAE_StableDiffusion encodes CUDA tensors only (no CPU path)")
-        if image.dim() != 4 or tuple(image.shape[1:]) != (3, 256, 256) or image.shape[0] < 1:
-            raise _lib.NopeError(f"the VAE encoder is built for [B, 3, 256, 256] inputs, got {tuple(image.shape)}")
-        return image.to(device=self.device, dtype=torch.float32).contiguous()
-
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return native_encode("vae", self._engine, self.device, image, self.latent_dim, "VAE", **kwargs)
 
     @property
     def last_launch_count(self):
-        return int(_lib.load().nope_vae_last_launch_count(self._h)) if self._h is not None else 0
+        return self._native.launch_count()
 
     @torch.no_grad()
     def encode_image(self, image, mode=None):
         """AutoencoderKL.py:29-42 with mode "mode" (None means "mode"): the latent mean times 0.18215."""
         if mode not in (None, "mode"):
             raise NotImplementedError(f"encode_image mode {mode!r} (only 'mode' is supported)")
-        x = self._images(image)
-        out = torch.empty((x.shape[0], self.latent_dim, 32, 32), device=self.device, dtype=torch.float32)
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nope_vae_encode(self._engine(), _lib.ptr(x), x.shape[0], _lib.ptr(out),
-                                                   self._stream()))
-        return out
+        return self._encode(image)
 
     @torch.no_grad()
     def encode_image_inplane(self, image, A):
         """image [B,3,256,256] -> [B,A,4,32,32]: the latents of the A in-plane rotated copies of every image
         (the FeatureExtractor.encode_image_inplane contract, DESIGN.md section 11), equal bit for bit to
         encode_image of inplane.rotate_images(image, A) flattened to [B*A, ...]."""
-        from .inplane import _on_device, check_angles, inplane_table
-        A = check_angles(A)
-        x = self._images(image)
-        out = torch.empty((x.shape[0], A, self.latent_dim, 32, 32), device=self.device, dtype=torch.float32)
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nope_vae_encode_inplane(
-                self._engine(), _lib.ptr(x), x.shape[0], _lib.ptr(_on_device(inplane_table, A, self.device)), A,
-                _lib.ptr(out), self._stream()))
-        return out
+        from .inplane import check_angles
+        return self._encode(image, A=check_angles(A))
 
     @torch.no_grad()
     def encode_image_rotated(self, image, image_idx, cossin):
         """image [B,3,256,256], pairs image_idx [P] and cossin [P, 2] -> [P,4,32,32] (the
         FeatureExtractor.encode_image_rotated contract, DESIGN.md section 14): the latent of image image_idx[p]
         rotated by cossin[p]; an index outside [0, B) encodes an all -1 crop."""
-        if image_idx.dim() != 1 or tuple(cossin.shape) != (image_idx.shape[0], 2) or image_idx.shape[0] < 1:
-            raise ValueError(f"image_idx [P] and cossin [P, 2] with P >= 1 expected, got {tuple(image_idx.shape)} and "
-                             f"{tuple(cossin.shape)}")
-        x = self._images(image)
-        idx = image_idx.to(device=self.device, dtype=torch.int32).contiguous()
-        cs = cossin.to(device=self.device, dtype=torch.float32).contiguous()
-        P = idx.shape[0]
-        out = torch.empty((P, self.latent_dim, 32, 32), device=self.device, dtype=torch.float32)
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().nope_vae_encode_rotated(
-                self._engine(), _lib.ptr(x), x.shape[0], _lib.ptr(idx), _lib.ptr(cs), P, _lib.ptr(out),
-                self._stream()))
-        return out
+        return self._encode(image, pairs=(image_idx, cossin))
 
     @torch.no_grad()
     def run_block(self, name, x, want_pair=True):
@@ -406,33 +349,28 @@ class VAE_StableDiffusion:
         "encoder.conv_out" / "decoder.conv_out" give the latent / the image and no pair."""
         if not isinstance(x, torch.Tensor) or x.device.type != "cuda" or x.dim() != 4:
             raise _lib.NopeError("run_block takes [n, C, H, H] CUDA tensors")
+        from .encoder import native_run_block
         dec = name.startswith("decoder.")
         h = self._decoder() if dec else self._engine()
-        x = x.to(device=self.device, dtype=torch.float32).contiguous()
-        out = torch.empty((x.shape[0],) + _vae_block_out(name), device=self.device)
-        pair = torch.empty_like(out) if want_pair else None
-        fn = _lib.load().nope_vae_decoder_run_block if dec else _lib.load().nope_vae_run_block
-        with torch.cuda.device(self.device):
-            _lib.check(fn(h, name.encode(), _lib.ptr(x), x.shape[1], x.shape[2], x.shape[0], _lib.ptr(out),
-                          _lib.ptr(pair), out.numel(), self._stream()))
-        return out, pair
+        return native_run_block("vae_decoder" if dec else "vae", h, self.device, name, x, _vae_block_out(name),
+                                bool(want_pair))
 
     # ------------------------------------------------------------------ decoder
     def _decoder(self):
-        if self._dec_h is not None:
-            return self._dec_h
-        if self._dec_config_error is not None:
-            raise ValueError(f"decode_latent: {self._dec_config_error}")
-        missing = self._missing_decoder_keys()
-        if missing:
-            raise _lib.NopeError(f"decode_latent needs the AutoencoderKL decoder weights: {len(missing)} of the "
-                                 f"{len(vae_decoder_param_shapes())} decoder tensors are missing, e.g. {missing[:5]}")
-        self._dec_h = _lib.build_engine("vae_decoder", (self.device.index or 0,), self._dec_sd.items())
-        return self._dec_h
+        if self._native_decoder.h is None:
+            if self._dec_config_error is not None:
+                raise ValueError(f"decode_latent: {self._dec_config_error}")
+            missing = self._missing_decoder_keys()
+            if missing:
+                raise _lib.NopeError(f"decode_latent needs the AutoencoderKL decoder weights: {len(missing)} of the "
+                                     f"{len(vae_decoder_param_shapes())} decoder tensors are missing, e.g. "
+                                     f"{missing[:5]}")
+            self._native_decoder.build((self.device.index or 0,), self._dec_sd.items())
+        return self._native_decoder.h
 
     @property
     def last_decode_launch_count(self):
-        return int(_lib.load().nope_vae_decoder_last_launch_count(self._dec_h)) if self._dec_h is not None else 0
+        return self._native_decoder.launch_count()
 
     @torch.no_grad()
     def decode_latent(self, latent):
@@ -449,7 +387,7 @@ class VAE_StableDiffusion:
         out = torch.empty((z.shape[0], 3, 256, 256), device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
             _lib.check(_lib.load().nope_vae_decoder_decode(h, _lib.ptr(z), z.shape[0], _lib.ptr(out),
-                                                           self._stream()))
+                                                           _lib.stream(self.device)))
         return out
 
 

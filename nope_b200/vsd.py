@@ -2,7 +2,6 @@
 DEPTH_ONLY render (reference src/poses/vsd.py:25-55) and the VSD error of `vsd_obj` (src/poses/vsd.py:92-135,
 src/poses/vsd_utils.py, visibility mode "bop19").  Both hot paths are CUDA kernels (render.cuh); there is no CPU
 fallback."""
-import ctypes as C
 
 import numpy as np
 import torch
@@ -12,6 +11,7 @@ from . import _lib
 COST_TYPES = {"step": 0, "tlinear": 1}          # NOPE_VSD_* of include/nope_b200.h
 MAX_SIDE = 8192
 MAX_TAUS = 16                                   # tolerances of one multi-tau VSD pass
+_stream = _lib.stream                           # the name the render and pose-fit tests import
 
 _PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2",
               "ushort": "u2", "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4",
@@ -191,9 +191,6 @@ def _image_size(image_size):
     return H, W
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
 
 def render_depth(mesh, poses, K, image_size, znear=0.05):
     """Camera-Z depth (float32 [P, H, W], 0 where nothing is hit) of `mesh` under poses [P, 4, 4] or [4, 4]
@@ -219,7 +216,7 @@ def render_depth(mesh, poses, K, image_size, znear=0.05):
     with torch.cuda.device(dev):
         _lib.check(_lib.load().nope_render_depth(
             _lib.ptr(mesh.vertices), mesh.vertices.shape[0], _lib.ptr(mesh.faces), mesh.num_faces, _lib.ptr(p),
-            p.shape[0], fx, fy, cx, cy, float(znear), H, W, _lib.ptr(out), _stream(dev)))
+            p.shape[0], fx, fy, cx, cy, float(znear), H, W, _lib.ptr(out), _lib.stream(dev)))
     return out
 
 
@@ -264,7 +261,7 @@ def vsd_errors(depth_test, depth_gt, depth_est, K, delta=15, tau=20, cost_type="
     with torch.cuda.device(dev):
         _lib.check(_lib.load().nope_vsd_error(
             _lib.ptr(dt), _lib.ptr(dg), _lib.ptr(de), F_, P, H, W, _lib.ptr(k), float(delta), float(tau),
-            COST_TYPES[cost_type], _lib.ptr(out), _stream(dev)))
+            COST_TYPES[cost_type], _lib.ptr(out), _lib.stream(dev)))
     return out
 
 
@@ -301,5 +298,5 @@ def _vsd_errors_taus(depth_test, depth_gt, depth_est, K, delta, tau, cost_type):
     with torch.cuda.device(dev):
         _lib.check(_lib.load().nope_vsd_error_taus(
             _lib.ptr(dt), _lib.ptr(dg), _lib.ptr(de), F_, P, H, W, k.data_ptr(), float(delta), COST_TYPES[cost_type],
-            taus.ctypes.data, len(taus), _lib.ptr(out), _stream(dev)))
+            taus.ctypes.data, len(taus), _lib.ptr(out), _lib.stream(dev)))
     return out

@@ -1,5 +1,6 @@
 """CPU: the lifecycle the five weight-holding engines share, without a device -- every *_create fails with an error
-message (no fallback), and _lib.build_engine destroys an engine whose build fails part way."""
+message (no fallback), _lib.build_engine destroys an engine whose build fails part way, and _lib.Engine, the handle
+owner of the Python classes, makes, rebuilds and destroys its one handle in order."""
 import ctypes as C
 
 import pytest
@@ -58,3 +59,72 @@ def test_build_engine_destroys_the_engine_when_a_step_fails(monkeypatch, bad):
             _lib.build_engine("vae", (0,), tensors, lambda lib, h: configured.append(h.value))
         assert fake.calls == ["nope_vae_create"] + ["nope_vae_load_tensor"] * 2 + ["nope_vae_destroy"]
     assert configured == [1234]
+
+
+# ------------------------------------------------------------------ _lib.Engine, the handle owner of the Python classes
+@pytest.fixture
+def fake(monkeypatch):
+    lib = _FakeLib(None)
+    monkeypatch.setattr(_lib, "load", lambda: lib)
+    return lib
+
+
+def _configure(lib, h):
+    lib.calls.append(f"configure {h.value}")
+
+
+TENSORS = [("a", torch.zeros(2)), ("b", torch.ones(3))]
+BUILD = ["nope_ldm_create", "configure 1234"] + ["nope_ldm_load_tensor"] * 2 + ["nope_ldm_finalize"]
+
+
+def test_engine_makes_one_weightless_configured_handle(fake):
+    e = _lib.Engine("ldm")
+    h = e.handle((256, 0), _configure)
+    assert e.handle((256, 0), _configure) is h and h.value == 1234 and not e.finalized
+    assert fake.calls == ["nope_ldm_create", "configure 1234"]            # configured, nothing loaded
+    e.destroy()
+
+
+def test_engine_rebuild_destroys_the_old_handle_first(fake):
+    e = _lib.Engine("ldm")
+    e.handle((0,), _configure)
+    e.build((0,), TENSORS, _configure)
+    assert e.finalized
+    e.build((0,), TENSORS, _configure)
+    assert fake.calls == ["nope_ldm_create", "configure 1234"] + ["nope_ldm_destroy"] + BUILD + \
+        ["nope_ldm_destroy"] + BUILD
+    e.destroy()
+
+
+def test_engine_failed_build_leaves_no_handle(fake):
+    e = _lib.Engine("ldm")
+    fake.bad = b"b"
+    with pytest.raises(_lib.NopeError, match="refused"):
+        e.build((0,), TENSORS, _configure)
+    assert e.h is None and not e.finalized
+    assert fake.calls == BUILD[:-1] + ["nope_ldm_destroy"]        # the load of `b` fails
+    fake.bad, fake.calls = None, []
+    assert e.build((0,), TENSORS, _configure).value == 1234 and e.finalized
+    assert fake.calls == BUILD
+    e.destroy()
+
+
+def test_engine_second_destroy_is_a_no_op(fake):
+    e = _lib.Engine("vae")
+    e.build((0,), TENSORS)
+    e.destroy()
+    e.destroy()
+    assert e.h is None and not e.finalized
+    assert fake.calls.count("nope_vae_destroy") == 1 and fake.calls[-1] == "nope_vae_destroy"
+
+
+def test_engine_del_does_not_raise_when_load_fails(fake, monkeypatch):
+    e = _lib.Engine("vae")
+    e.build((0,), TENSORS)
+
+    def fail():
+        raise _lib.NopeError("no library")
+    monkeypatch.setattr(_lib, "load", fail)
+    e.__del__()
+    assert e.h is None
+    del e
