@@ -413,6 +413,17 @@ int nope_crop_frames(const uint8_t* frames, int F, int H, int W, int C, const ui
 int nope_crop_camera(const double* pose, int F, int keep_inplane, double* Rv, void* stream);
 int nope_crop_rotate(const double* Rv, int F, const double* R, int P, int to_camera, double* out, void* stream);
 
+/* Pose tracking (DESIGN.md section 26): prior rotations to centres of the joint roll and viewpoint refinement.
+ * Rc [H, 9] fp64 row-major (priors in the crop camera), T [N, 9] fp64 row-major (the refiner's grid), device ->
+ * out_D [H, 9] fp32, out_seed [H] int32, out_cossin [H, 2] fp32 with Rz(rho) D T[seed] = Rc, Rz(rho) = [[c, -s, 0],
+ * [s, c, 0], [0, 0, 1]]: seed maximises score_n = |(M00 + M11, M10 - M01)| + M22 over M = Rc T[n]^T (ties -> the
+ * lowest n, a NaN never chosen), (c, s) = (M00 + M11, M10 - M01) / |.| ((1, 0) at 0) and D = Rz(-rho) M.  float64,
+ * every operation rounded on its own, D and (c, s) rounded to fp32 once.  A prior with a non-finite entry, or no
+ * score that is a number, gives seed 0, D = I and (1, 0).  Requires H, N >= 1; refuses bad arguments before any CUDA
+ * call and does not synchronise. */
+int nope_track_seeds(const double* Rc, int H, const double* T, int N, float* out_D, int32_t* out_seed,
+                     float* out_cossin, void* stream);
+
 /* Score materialised templates against a query and rank them: the arithmetic of
  * PoseConditional.retrieval (model.py:254-266) after encode_image.
  *   query_feat [B, C, HW] fp32, emb [B, N, C, HW] fp32 -> sim [B, N], topv/topi [B, k]. */

@@ -86,6 +86,8 @@ SIGNATURES = {
                                    C.c_void_p, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     "nope_crop_camera": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "nope_crop_rotate": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "nope_track_seeds": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_void_p, c_f32p,
+                                   C.c_void_p]),
     "nope_score_topk": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                   C.c_int, c_f32p, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_score_topk_multi": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,

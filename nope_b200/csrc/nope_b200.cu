@@ -34,6 +34,7 @@
 #include "depth_refine.cuh"
 #include "contour_refine.cuh"
 #include "distinct.cuh"
+#include "track.cuh"
 
 using namespace nope;
 
@@ -1116,6 +1117,17 @@ int nope_crop_rotate(const double* Rv, int F, const double* R, int P, int to_cam
   const long long n = (long long)F * P;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   crop_rotate_kernel<<<ew_grid(n), 256, 0, st>>>(Rv, R, P, n, to_camera, out);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// pose tracking: prior rotations to refinement centres (track.cuh, DESIGN.md section 26)
+int nope_track_seeds(const double* Rc, int H, const double* T, int N, float* out_D, int32_t* out_seed,
+                     float* out_cossin, void* stream) {
+  NOPE_CHECK(Rc && T && out_D && out_seed && out_cossin, "null argument");
+  NOPE_CHECK(H >= 1 && N >= 1, "H and N must be >= 1");
+  track_seed_kernel<<<H, kTrackThreads, 0, static_cast<cudaStream_t>(stream)>>>(Rc, T, N, out_D, out_seed,
+                                                                               out_cossin);
   NOPE_CUDA(cudaGetLastError());
   return 0;
 }

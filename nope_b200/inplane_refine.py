@@ -24,7 +24,7 @@ from . import _lib
 from ._lib import MAX_TOPK
 from .inplane import check_angles, inplane_table
 from .refine import axis_angle_matrix, grid_constants, identity_centres
-from .search import row_pairs
+from .search import query_rows, row_pairs
 
 XY = 9              # pose slots per centre: the 3x3 xy lattice, identity first, then lexicographic (i, j)
 ROLL = 3            # angle slots per centre: rho, rho + phi, rho - phi
@@ -163,13 +163,40 @@ def select(sim, cand, threshold, k):
     return out
 
 
+def check_centres(seeds, lead):
+    """ValueError unless seeds is refine_inplane's dict of explicit centres for rows of shape `lead` (checked on the
+    host): D float32 [*lead, keep, 3, 3], seed integer [*lead, keep], cossin float32 [*lead, keep, 2].  -> keep"""
+    if set(seeds) != {"D", "seed", "cossin"} or not all(torch.is_tensor(v) for v in seeds.values()):
+        raise ValueError(f"centre seeds must be a dict of tensors D, seed and cossin, got keys {sorted(seeds)}")
+    D, seed, cs = seeds["D"], seeds["seed"], seeds["cossin"]
+    if seed.is_floating_point() or seed.is_complex() or seed.dtype == torch.bool:
+        raise ValueError(f"seeds['seed'] must be an integer tensor, got {seed.dtype}")
+    if D.dtype != torch.float32 or cs.dtype != torch.float32:
+        raise ValueError(f"seeds['D'] and seeds['cossin'] must be float32, got {D.dtype} and {cs.dtype}")
+    keep = int(seed.shape[-1]) if seed.dim() == len(lead) + 1 else 0
+    if keep < 1 or tuple(seed.shape) != lead + (keep,) or tuple(D.shape) != lead + (keep, 3, 3) or \
+            tuple(cs.shape) != lead + (keep, 2):
+        raise ValueError(f"centre seeds D {lead + ('keep', 3, 3)}, seed {lead + ('keep',)} and cossin "
+                         f"{lead + ('keep', 2)} expected, got {tuple(D.shape)}, {tuple(seed.shape)} and "
+                         f"{tuple(cs.shape)}")
+    return keep
+
+
+def _check_seed_latents(seed_latents, shape):
+    if tuple(seed_latents.shape) != shape:
+        raise ValueError(f"seed_latents must be {shape}, got {tuple(seed_latents.shape)}")
+
+
 def refine_inplane(engine, encoder, ref_feat, query_images, all_relativeR, seeds, seed_latents, refiner, k=5):
     """Refine each (reference, query) row from its best (angle, pose) pairs, with any engine that has `sweep()`.
 
     ref_feat [B, C, 32, 32]; query_images [B, 3, 256, 256] or [B, Q, 3, 256, 256]; all_relativeR [B, N, 6], the grid
     of `refiner`; seeds = (pose_idx, angle_idx), each [B(, Q), keep] (keep = their last dimension, e.g. the joint
-    top-keep of the in-plane search); seed_latents [B(, Q), keep, C, 32, 32], the search's latents of those angle
-    copies (gathered, not re-encoded); encoder: a FeatureExtractor on the native engine.
+    top-keep of the in-plane search), or explicit centres dict(D [B(, Q), keep, 3, 3] float32, seed [B(, Q), keep]
+    integer, cossin [B(, Q), keep, 2] float32), e.g. track.seed_centres of prior rotations ((pose_idx, angle_idx) is
+    the centre (I, pose_idx, inplane_table(A)[angle_idx])); seed_latents [B(, Q), keep, C, 32, 32], the latents of
+    the crops rotated by the seeds' rolls (for the tuple, the search's latents of those angle copies, gathered, not
+    re-encoded); encoder: a FeatureExtractor on the native engine.
     -> dict(D [B(, Q), k, 3, 3], seed [B(, Q), k] int64, cossin [B(, Q), k, 2], score [B(, Q), k], rel6d [B(, Q), k,
     6] and latent [B(, Q), k, C, 32, 32] (the pose and query latent each score was swept at), hypotheses and crops
     (per row, by the steps)).  Descending score; ranks past the last distinct pair have score -inf and seed -1.
@@ -178,23 +205,33 @@ def refine_inplane(engine, encoder, ref_feat, query_images, all_relativeR, seeds
     pairs with one reference row per (reference, query) and selects the next `keep` centres (the last step: k).
     Everything runs on the current stream with no host synchronisation (device copies of the refiner's constants
     are made by the first call on a device)."""
-    pose_idx, angle_idx = seeds
-    keep = int(pose_idx.shape[-1])
+    centres = isinstance(seeds, dict)
+    rest = tuple(ref_feat.shape[1:])
+    if centres:
+        lead = query_rows(query_images, ref_feat, (3, 256, 256))[1]
+        keep = check_centres(seeds, lead)
+        _check_seed_latents(seed_latents, lead + (keep,) + rest)
+    else:
+        pose_idx, angle_idx = seeds
+        keep = int(pose_idx.shape[-1])
     check_inplane_refine_args(refiner, all_relativeR, keep, k, ref_feat.shape[0])
     dev = engine.device
     _, _, Q, lead, ref_rows, images = row_pairs(dev, ref_feat, query_images, (3, 256, 256))
-    if tuple(pose_idx.shape) != lead + (keep,) or tuple(angle_idx.shape) != lead + (keep,):
+    if not centres and (tuple(pose_idx.shape) != lead + (keep,) or tuple(angle_idx.shape) != lead + (keep,)):
         raise ValueError(f"seeds must be two {lead + (keep,)} tensors, got {tuple(pose_idx.shape)} and "
                          f"{tuple(angle_idx.shape)}")
-    rest = tuple(ref_feat.shape[1:])
-    if tuple(seed_latents.shape) != lead + (keep,) + rest:
-        raise ValueError(f"seed_latents must be {lead + (keep,) + rest}, got {tuple(seed_latents.shape)}")
+    _check_seed_latents(seed_latents, lead + (keep,) + rest)
     rows = ref_rows.shape[0]
     stencils, _, table = refiner._on(dev)
     rel = all_relativeR.to(dev, torch.float32).contiguous()
-    cur = {"D": identity_centres(rows, keep, dev),
-           "seed": pose_idx.to(dev).reshape(rows, keep).to(torch.int32),
-           "cossin": table[angle_idx.to(dev).reshape(rows, keep)].contiguous()}
+    if centres:
+        cur = {"D": seeds["D"].to(dev).reshape(rows, keep, 9).contiguous(),
+               "seed": seeds["seed"].to(dev).reshape(rows, keep).to(torch.int32),
+               "cossin": seeds["cossin"].to(dev).reshape(rows, keep, 2).contiguous()}
+    else:
+        cur = {"D": identity_centres(rows, keep, dev),
+               "seed": pose_idx.to(dev).reshape(rows, keep).to(torch.int32),
+               "cossin": table[angle_idx.to(dev).reshape(rows, keep)].contiguous()}
     lat = seed_latents.to(dev, torch.float32).reshape(rows, keep, *rest)
     row_ix = torch.arange(rows, device=dev)
     for s in range(refiner.steps):

@@ -747,37 +747,12 @@ class PoseConditional:
         "iou": the silhouette IoU [B, k], "R_crop": the search's rotations [B, k, 3, 3], "t0": [B, 3],
         "crops": [B, 3, 256, 256]}.  R and t go unchanged into eval_bop(R_est=, t_est=), refine_depth and
         select_distinct.  The only host synchronisation beyond the search's is frame_crops' copy of t0."""
-        from . import contour_refine, translation
-        from .crop import _as_numpy, _tensor, detection_occluders, frame_crops, to_camera
-        import numpy as np
-        if refine not in (None, "contour"):
-            raise ValueError(f"refine must be None or 'contour', got {refine!r}")
-        if isinstance(occluders, str) and occluders != "detections":
-            raise ValueError(f"occluders must be None, a tensor or 'detections', got {occluders!r}")
-        ids = [int(i) for i in np.asarray(obj_ids.detach().cpu() if torch.is_tensor(obj_ids) else obj_ids)
-               .reshape(-1).tolist()]
+        from .crop import frame_crops
+        ids = self._frame_ids("predict_pose_frames", masks, obj_ids, refine, occluders)
         B = len(ids)
-        if masks.shape[0] != B:
-            raise ValueError(f"predict_pose_frames: {B} obj_ids for {masks.shape[0]} masks")
-        missing = sorted(set(i for i in ids if i not in self.tless_cad or i not in self.bop_models))
-        if missing:
-            raise ValueError(f"predict_pose_frames: no mesh or models_info entry for obj_id {missing} (load_mesh, "
-                             "load_models_info)")
-        if bank is not None:
-            if reference is not None or all_relativeR is not None or template_poses is not None:
-                raise ValueError("predict_pose_frames: give either a bank or reference, all_relativeR and "
-                                 "template_poses, not both")
-            from .bank import check_bank_search
-            # the bank, the engine and the ids before the crops; the search checks its own k / keep again
-            check_bank_search(bank, self.u_net, B, ids, getattr(refiner, "angles", angles), 1)
-        elif reference is None or all_relativeR is None:
-            raise ValueError("predict_pose_frames: reference and all_relativeR (with template_poses), or a bank, "
-                             "expected")
-        elif reference.shape[0] not in (1, B):
-            raise ValueError(f"predict_pose_frames: reference [1 | B, 3, 256, 256] with B = {B} expected, got "
-                             f"{tuple(reference.shape)}")
-        diameter = np.array([self.bop_models[i]["diameter"] for i in ids], dtype=np.float64)
-        crops, t0, Rv, _ = frame_crops(frames, masks, K, diameter, image_size=256, frame_idx=frame_idx)
+        self._frame_templates("predict_pose_frames", B, ids, bank, reference, all_relativeR, template_poses,
+                              getattr(refiner, "angles", angles))
+        crops, t0, Rv, _ = frame_crops(frames, masks, K, self._diameters(ids), image_size=256, frame_idx=frame_idx)
         if bank is not None and refiner is None:
             R_crop, nearest, angle, sim = self.predict_pose_bank(crops, ids, bank, k=k, angles=angles)
             N = sim.shape[-1]
@@ -791,13 +766,63 @@ class PoseConditional:
             score = sim.reshape(B, -1).gather(1, angle * N + nearest)
         else:
             R_crop, _, _, score = self.predict_pose_inplane_refined(crops, reference, all_relativeR, refiner, k=k)
+        return self._frame_fits("predict_pose_frames", frames, masks, K, ids, frame_idx, occluders, refine, R_crop,
+                                score, crops, t0, Rv)
+
+    def _frame_ids(self, name, masks, obj_ids, refine, occluders):
+        """The refusals of a pose from camera frames that do not depend on the search: refine, occluders, one obj_id
+        per mask and a mesh and models_info entry for each.  -> the ids (host ints)"""
+        import numpy as np
+        if refine not in (None, "contour"):
+            raise ValueError(f"refine must be None or 'contour', got {refine!r}")
+        if isinstance(occluders, str) and occluders != "detections":
+            raise ValueError(f"occluders must be None, a tensor or 'detections', got {occluders!r}")
+        ids = [int(i) for i in np.asarray(obj_ids.detach().cpu() if torch.is_tensor(obj_ids) else obj_ids)
+               .reshape(-1).tolist()]
+        B = len(ids)
+        if masks.shape[0] != B:
+            raise ValueError(f"{name}: {B} obj_ids for {masks.shape[0]} masks")
+        missing = sorted(set(i for i in ids if i not in self.tless_cad or i not in self.bop_models))
+        if missing:
+            raise ValueError(f"{name}: no mesh or models_info entry for obj_id {missing} (load_mesh, "
+                             "load_models_info)")
+        return ids
+
+    def _frame_templates(self, name, B, ids, bank, reference, all_relativeR, template_poses, angles):
+        """The refusals of where a frame search's templates come from: either a bank holding every id (checked
+        with `angles` bins) or reference [1 | B] and all_relativeR"""
+        if bank is not None:
+            if reference is not None or all_relativeR is not None or template_poses is not None:
+                raise ValueError(f"{name}: give either a bank or reference, all_relativeR and template_poses, not "
+                                 "both")
+            from .bank import check_bank_search
+            # the bank, the engine and the ids before the crops; the search checks its own k / keep again
+            check_bank_search(bank, self.u_net, B, ids, angles, 1)
+        elif reference is None or all_relativeR is None:
+            raise ValueError(f"{name}: reference and all_relativeR (with template_poses), or a bank, expected")
+        elif reference.shape[0] not in (1, B):
+            raise ValueError(f"{name}: reference [1 | B, 3, 256, 256] with B = {B} expected, got "
+                             f"{tuple(reference.shape)}")
+
+    def _diameters(self, ids):
+        import numpy as np
+        return np.array([self.bop_models[i]["diameter"] for i in ids], dtype=np.float64)
+
+    def _frame_fits(self, name, frames, masks, K, ids, frame_idx, occluders, refine, R_crop, score, crops, t0, Rv):
+        """The stages of a pose from camera frames after the search: crop-camera rotations R_crop [B, k, 3, 3] to the
+        real camera, the occluders, the translation fit from t0 and, for refine="contour", the contour refinement.
+        -> the dict of predict_pose_frames"""
+        from . import contour_refine, translation
+        from .crop import _as_numpy, _tensor, detection_occluders, to_camera
+        import numpy as np
+        B = len(ids)
         R = to_camera(R_crop.to(self.device), Rv.to(self.device))
         masks = _tensor(masks)
         if isinstance(occluders, str):
             from .bop import _to_dev
             md = masks if masks.device.type == "cuda" else _to_dev(masks, self.device, masks.dtype)
             occluders = detection_occluders(md, frame_idx, num_frames=_tensor(frames).shape[0])
-        occluders = self._occluders("predict_pose_frames", occluders, masks)
+        occluders = self._occluders(name, occluders, masks)
         Kh = torch.from_numpy(np.ascontiguousarray(np.broadcast_to(_as_numpy(K, "K").reshape(-1, 3, 3), (B, 3, 3))))
         kk = R.shape[1]
         t = torch.empty((B, kk, 3), device=self.device, dtype=torch.float64)
@@ -813,6 +838,58 @@ class PoseConditional:
                 R_out[rd], iou_o = R_o, fit["iou"]
             t[rd], iou[rd] = t_o, iou_o
         return {"R": R_out, "t": t, "score": score, "iou": iou, "R_crop": R_crop, "t0": t0, "crops": crops}
+
+    @torch.no_grad()
+    def track_pose_frames(self, frames, masks, K, obj_ids, R_prior, refiner, bank=None, reference=None,
+                          all_relativeR=None, template_poses=None, k=5, refine=None, frame_idx=None, occluders=None):
+        """predict_pose_frames with the search replaced by a refinement from prior rotations (DESIGN.md section 26):
+        R_prior [B, P, 3, 3] (1 <= P <= 16) in the real camera, e.g. the previous frame's R[:, :keep], is taken into
+        each new crop's camera (crop.to_crop), mapped to refinement centres and refined by the refiner's steps
+        (track.track_inplane), without the A rotated copies of a search.  refiner: an InplaneRefiner over the grid of
+        the bank or of all_relativeR (template_poses, when given, must be that grid).  frames, masks, K, obj_ids, bank
+        or reference / all_relativeR, refine, frame_idx and occluders as predict_pose_frames takes them.
+        -> predict_pose_frames' dict, "score" the refined score of each of the k poses.  Per detection it encodes P *
+        (1 + 2 * steps) rotated crops and sweeps 9 * P * steps hypotheses; the host synchronises as often as in
+        predict_pose_frames."""
+        from .crop import frame_crops, to_crop
+        from .inplane_refine import InplaneRefiner, pose_rotations
+        from .track import check_track_args, track_inplane
+        if self.dist is not None:
+            raise NotImplementedError("track_pose_frames does not shard across GPUs: it runs on one device (unset "
+                                      "model.dist)")
+        if not isinstance(refiner, InplaneRefiner):
+            raise ValueError("refiner must be a nope_b200.inplane_refine.InplaneRefiner")
+        ids = self._frame_ids("track_pose_frames", masks, obj_ids, refine, occluders)
+        B = len(ids)
+        self._frame_templates("track_pose_frames", B, ids, bank, reference, all_relativeR, template_poses,
+                              refiner.angles)
+        R_prior = R_prior if torch.is_tensor(R_prior) else torch.as_tensor(R_prior)
+        if bank is not None:
+            bank.check_grid(refiner.template_poses)
+            check_track_args(refiner, bank.all_relativeR, R_prior, k, B)
+        else:
+            check_track_args(refiner, all_relativeR, R_prior, k, B, reference.shape[0])
+            if template_poses is not None and not torch.equal(
+                    torch.as_tensor(template_poses).detach().cpu().to(torch.float64), refiner.template_poses):
+                raise ValueError("track_pose_frames: template_poses is not the refiner's grid")
+        metric = self._metric()
+        crops, t0, Rv, _ = frame_crops(frames, masks, K, self._diameters(ids), image_size=256, frame_idx=frame_idx)
+        dev = self.device
+        R_prior_crop = to_crop(R_prior.to(dev), Rv.to(dev))
+        self.u_net.set_metric(metric, self._occlusion_threshold())
+        if bank is not None:
+            from .track import _index
+            slots = _index(bank.slots(ids), bank.device)
+            ref_feat = bank.reference_latents.index_select(0, slots)
+            rel = bank.all_relativeR.index_select(0, slots)
+        else:
+            ref_feat = self.u_net.encoder.encode_image(reference.to(dev))
+            ref_feat = ref_feat.expand(B, *ref_feat.shape[1:])
+            rel = all_relativeR.to(dev).expand(B, *all_relativeR.shape[1:])
+        out = track_inplane(self.u_net, self.u_net.encoder, ref_feat, crops, rel, R_prior_crop, refiner, k=k)
+        R_crop = pose_rotations(out["D"], out["seed"], out["cossin"], refiner)
+        return self._frame_fits("track_pose_frames", frames, masks, K, ids, frame_idx, occluders, refine, R_crop,
+                                out["score"], crops, t0, Rv)
 
     @torch.no_grad()
     def eval_bop(self, batch, data_name, R_est=None, save_path=None, t_est=None):
