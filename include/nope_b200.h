@@ -14,10 +14,14 @@
  *   similarity        fp32 [B, N]; nearest_idx int64 [B, k]
  * Inside the library activations are NHWC fp16 and weights are repacked K-major fp16.
  *
- * ABI version 2 (round 2): nope_unet_set_option / get_option, caller-owned workspace
+ * ABI version 2 (round 2): nope_unet_set_option, caller-owned workspace
  * (nope_unet_workspace_bytes / nope_unet_set_workspace), nope_unet_profile_read reports executed and
- * algorithmic FLOPs, nope_op_conv_gn_fused, nope_topk_merge, nope_score_topk metric 2.
+ * algorithmic FLOPs, nope_op_conv_gn_fused, nope_topk_merge, NOPE_METRIC_COSINE_OCC in the score calls.
  * Later additions under version 2 include nope_encoder_set_option and nope_vae_set_option.
+ * ABI version 3: one entry point per operation.  The entry points that only forwarded to another one with a constant
+ * (Q = 1, Bt = B, no occluders) are removed, as are the convolution-implementation setters, the option getter and the
+ * attention switches; nope_op_conv, nope_op_conv_gn and nope_op_mh_attention lost their leading implementation
+ * argument.  A ctypes caller checks nope_abi_version() before binding.
  */
 #ifndef NOPE_B200_H
 #define NOPE_B200_H
@@ -68,12 +72,9 @@ int nope_unet_load_tensor(nope_unet_t* u, const char* key, const float* data,
  * pose projections concatenated into one GEMM) and uploads them. */
 int nope_unet_finalize(nope_unet_t* u);
 
-/* Tunables: hypotheses per chunk (workspace = ~4.7 MB per hypothesis at u_net_dim 192), and the
- * convolution implementation: 2 = wgmma, clustered kernel with the fused epilogues (the only one;
- * anything else is an error). */
+/* Hypotheses per chunk (workspace = ~4.7 MB per hypothesis at u_net_dim 192). */
 int nope_unet_set_chunk(nope_unet_t* u, int hyps_per_chunk);
-int nope_unet_set_conv_impl(nope_unet_t* u, int impl);
-/* Named options:
+/* Named options (any other name is an error):
  *   "precision" (before nope_unet_finalize): 0 = fp16 operands (default; embeddings ~1.3e-3 rel-L2 of the
  *       fp32 reference, u_net.py:160-198), 1 = exact weights: every weight is an fp16 pair W_hi + W_lo and
  *       each convolution accumulates A W_hi + A W_lo (2x the tensor-core work), 2 = split precision:
@@ -81,12 +82,8 @@ int nope_unet_set_conv_impl(nope_unet_t* u, int impl);
  *       the "parity" mode that meets the 1e-3 embedding tolerance with margin), 3 = bf16 operands and
  *       activations (BASELINE configs[2]; 8-bit mantissa: embeddings ~1e-2 of the fp32 reference),
  *       4 = split precision with single-fp16 tensors inside the ResnetBlocks (block2 convolutions run two
- *       products instead of three; embeddings ~5e-4: the fastest mode inside the 1e-3 tolerance);
- *   "conv_impl": as nope_unet_set_conv_impl;
- *   "attn_impl": LinearAttention core, 0 = wgmma kernel at 32x32 / 16x16 (CUDA cores below 128 tokens),
- *       1 = CUDA-core kernel everywhere. */
+ *       products instead of three; embeddings ~5e-4: the fastest mode inside the 1e-3 tolerance). */
 int nope_unet_set_option(nope_unet_t* u, const char* name, int value);
-int nope_unet_get_option(const nope_unet_t* u, const char* name, int* value);
 
 /* Workspace ownership.  By default the engine owns one device slab and grows it on demand (a growth
  * synchronises the device and calls cudaMalloc).  A host framework that wants every byte to come from
@@ -100,28 +97,19 @@ int nope_unet_set_workspace(nope_unet_t* u, void* device_ptr, int64_t bytes, int
  * Sweep over the pose grid.  Replaces the Python loop of
  * PoseConditional.generate_templates (src/model/model.py:193-252) around
  * UNet.forward (u_net.py:160-198) and, when query_feat != NULL, the scoring and top-k of
- * PoseConditional.retrieval (model.py:254-266) fused onto the last layer.
+ * PoseConditional.retrieval (model.py:254-266) fused onto the last layer.  One sweep per reference, Q >= 1
+ * queries per reference: the templates depend on the reference and the pose grid only, so several queries of one
+ * object (video frames, detections of several instances) share one sweep and are all scored in its last layer.
  *   ref_feat   [B, C, hw, hw] fp32   encode_image(reference)
  *   poses      [B, N, 6] fp32        all_relativeR
- *   query_feat [B, C, hw, hw] fp32 or NULL
+ *   query_feat [B, Q, C, hw, hw] fp32 or NULL
  *   out_emb    [B, N, C, hw, hw] fp32 or NULL (skip materialising the templates)
- *   out_sim    [B, N] fp32 or NULL   (requires query_feat)
- *   out_topv / out_topi  [B, k] fp32 / int64 or NULL; descending score, ties broken by
+ *   out_sim    [B, Q, N] fp32 or NULL   (requires query_feat)
+ *   out_topv / out_topi  [B, Q, k] fp32 / int64 or NULL; descending score, ties broken by
  *              the lowest index; indices are offset by idx_base (global index of this
  *              shard's first pose).  k = 0 skips the ranking.
- * Kernels are enqueued on `stream`; the call does not synchronise. */
-int nope_unet_sweep(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
-                    const float* query_feat, float* out_emb, float* out_sim, int k,
-                    float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream);
-
-/* One sweep per reference, Q queries per reference: the templates depend on the reference and the pose grid
- * only, so several queries of one object (video frames, detections of several instances) share one sweep and
- * are all scored in its last layer.  Arguments as nope_unet_sweep, plus Q >= 1, with
- *   query_feat [B, Q, C, hw, hw] fp32
- *   out_sim    [B, Q, N] fp32 or NULL
- *   out_topv / out_topi  [B, Q, k]
- * sim[b, q] is bit-identical to a Q = 1 sweep of query q alone; nope_unet_sweep is the Q = 1 case.  A
- * caller-owned workspace must be sized for scores = B*Q*N. */
+ * sim[b, q] is bit-identical to a Q = 1 sweep of query q alone.  A caller-owned workspace must be sized for
+ * scores = B*Q*N.  Kernels are enqueued on `stream`; the call does not synchronise. */
 int nope_unet_sweep_multi(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
                           const float* query_feat, int Q, float* out_emb, float* out_sim, int k,
                           float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream);
@@ -130,7 +118,7 @@ int nope_unet_sweep_multi(nope_unet_t* u, const float* ref_feat, const float* po
  * one the reference implements, model.py:254-266).  occlusion_threshold is used by NOPE_METRIC_COSINE_OCC. */
 int nope_unet_set_metric(nope_unet_t* u, int metric, float occlusion_threshold);
 
-/* Number of kernels the last nope_unet_sweep call enqueued (for bench.py's gpu_launches). */
+/* Number of kernels the last nope_unet_sweep_multi call enqueued (for bench.py's gpu_launches). */
 int64_t nope_unet_last_launch_count(const nope_unet_t* u);
 
 /* Profiling hook for bench.py's roofline: when enabled, every tensor-core convolution
@@ -288,42 +276,28 @@ int nope_render_depth(const float* vertices, int V, const int32_t* faces, int F,
 int nope_vsd_error(const double* depth_test, const float* depth_gt, const float* depth_est, int F, int P, int H, int W,
                    const double* K, double delta, double tau, int cost_type, double* out, void* stream);
 
-/* Translation from the object mask (DESIGN.md section 18).
- * nope_fit_translation: for F frames and P rotation hypotheses per frame, fit the translation so that the silhouette
- * of the mesh (vertices [V, 3] fp32, faces [NF, 3] int32, as nope_render_depth) lines up with the frame's mask:
- * R [F, P, 9] fp64 row-major and t_init [F, P, 3] fp64 (model -> OpenCV camera, mm), masks [F, H, W] uint8 (nonzero =
- * object), all on the device; K HOST [F, 4] fp64 (fx, fy, cx, cy; finite, fx and fy non-zero), staged in stream order.
- * Each of the `iters` updates renders [R | t] rounded to fp32 with nope_render_depth's rasterizer, scales t's distance
- * by sqrt of the ratio of the silhouette's to the mask's box area and moves the origin so that the box centres meet;
- * an empty silhouette leaves t unchanged.  -> t_out [F, P, 3] fp64, iou [F, P] fp64 = |S n M| / |S u M| of the
- * silhouette S at t_out (0 when S is empty); both NaN for every hypothesis of a frame whose mask is empty.
+/* Translation from the object mask (DESIGN.md section 18), under occlusion (DESIGN.md section 24).
+ * nope_fit_translation_occluded: for F frames and P rotation hypotheses per frame, fit the translation so that the
+ * silhouette of the mesh (vertices [V, 3] fp32, faces [NF, 3] int32, as nope_render_depth) lines up with the frame's
+ * mask: R [F, P, 9] fp64 row-major and t_init [F, P, 3] fp64 (model -> OpenCV camera, mm), masks [F, H, W] uint8
+ * (nonzero = object), all on the device; K HOST [F, 4] fp64 (fx, fy, cx, cy; finite, fx and fy non-zero), staged in
+ * stream order.  Each of the `iters` updates renders [R | t] rounded to fp32 with nope_render_depth's rasterizer, scales
+ * t's distance by sqrt of the ratio of the silhouette's to the mask's box area and moves the origin so that the box
+ * centres meet; an empty silhouette leaves t unchanged.  -> t_out [F, P, 3] fp64, iou [F, P] fp64 = |S n M| / |S u M|
+ * of the silhouette S at t_out (0 when S is empty); both NaN for every hypothesis of a frame whose mask is empty.
  * stats_out [F, P, 6] int32 (n_S, |S n M|, row0, row1, col0, col1 of S at t_out; an empty box is (INT_MAX, -1)) may be
  * null.  depth [F P, H, W] fp32 is the caller's workspace; on return it holds nope_render_depth's image at the last
  * rendered translation of each hypothesis.  Requires V, NF >= 1, 1 <= F, P <= 65535, 1 <= H, W <= 8192, iters >= 0,
- * znear finite and > 0.  Refuses bad arguments before any CUDA call; all iterations are enqueued without
- * synchronising the host.  The result does not depend on the batch or on scheduling. */
-int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
-                         const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
-                         float znear, int iters, float* depth, double* t_out, double* iou, int32_t* stats_out,
-                         void* stream);
-
-/* Pose fits under occlusion (DESIGN.md section 24).  occluders [F, H, W] uint8 on the device (nonzero = something may
- * be in front of the object there; U = the other pixels) or NULL.  The mask becomes M' = M n U: O wins over M.
- * nope_fit_translation_occluded: nope_fit_translation with the silhouette statistics (n_S, |S n M|, box) those of
- * S' = S n U and the mask statistics those of M'; iou = |S' n M'| / |S' u M'|, stats_out those of S'.
- * nope_refine_contour_occluded: nope_refine_contour with phi the signed distance field of M', the box size that scales
- * tau that of M', and a contour pixel counted and paired only when it and its four neighbours lie in U; iou uses S'
- * and M', and "empty or full" is judged on M'.  With occluders NULL (or all zero) both equal the plain entry points
- * bit for bit, which forward to them.  Arguments, refusals and guarantees otherwise as the plain entry points. */
+ * znear finite and > 0.  Refuses bad arguments before any CUDA call; all iterations are enqueued without synchronising
+ * the host.  The result does not depend on the batch or on scheduling.
+ * occluders [F, H, W] uint8 on the device (nonzero = something may be in front of the object there; U = the other
+ * pixels) or NULL (every pixel is in U).  The mask becomes M' = M n U: O wins over M.  The silhouette statistics
+ * (n_S, |S n M|, box) are those of S' = S n U and the mask statistics those of M'; iou = |S' n M'| / |S' u M'|,
+ * stats_out those of S'.  With occluders NULL or all zero, S' = S and M' = M. */
 int nope_fit_translation_occluded(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
                                   const double* t_init, const uint8_t* masks, const uint8_t* occluders,
                                   const double* K, int F, int P, int H, int W, float znear, int iters, float* depth,
                                   double* t_out, double* iou, int32_t* stats_out, void* stream);
-int nope_refine_contour_occluded(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
-                                 const double* t_init, const uint8_t* masks, const uint8_t* occluders,
-                                 const double* K, int F, int P, int H, int W, double rho, const double* tau, int iters,
-                                 float znear, float* depth, double* R_out, double* t_out, double* fit_out,
-                                 int64_t* sums_out, void* stream);
 
 /* Pose refinement from the sensor depth (DESIGN.md section 19).
  * nope_refine_depth: projective point-to-plane ICP of P pose hypotheses per frame for F frames against the frame's
@@ -347,13 +321,13 @@ int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF
                       double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
                       double* t_out, double* fit_out, int64_t* sums_out, void* stream);
 
-/* Pose refinement from the object mask's contour (DESIGN.md section 20).
+/* Pose refinement from the object mask's contour (DESIGN.md section 20), under occlusion (DESIGN.md section 24).
  * nope_mask_sdf: the signed distance field sdf_out [F, H, W] fp64 of masks [F, H, W] uint8 (nonzero = object), both
  * on the device: sqrt(d2_out) - 1/2 off the object and 1/2 - sqrt(d2_in) on it, with d2_out (d2_in) the exact squared
  * distance in px to the nearest object (background) pixel of the frame; NaN everywhere for a mask that is empty or
  * covers the whole frame.  Requires 1 <= F <= 65535, 1 <= H, W <= 8192.
- * nope_refine_contour: damped Gauss-Newton alignment of the rendered silhouette's contour with the mask, for P pose
- * hypotheses per frame and F frames.  Mesh, R, t_init, K, rho, znear, iters, the workspace depth and sums_out as
+ * nope_refine_contour_occluded: damped Gauss-Newton alignment of the rendered silhouette's contour with the mask, for
+ * P pose hypotheses per frame and F frames.  Mesh, R, t_init, K, rho, znear, iters, the workspace depth and sums_out as
  * nope_refine_depth; masks [F, H, W] uint8 on the device; tau HOST [iters + 1] fp64 the pairing tolerances as
  * fractions of the mask's box size sqrt(w h) (each finite and > 0).  Iteration i renders [R | t] rounded to fp32,
  * pairs every interior contour pixel of the render (hit, a 4-neighbour not hit) whose residual phi + 1/2 lies within
@@ -363,12 +337,16 @@ int nope_refine_depth(const float* vertices, int V, const int32_t* faces, int NF
  * at the returned pose: the pairs at tau[iters], the contour pixels of the render, the RMS residual in px (NaN when
  * n_in = 0) and the silhouette IoU with the mask; rms and iou are NaN for a frame whose mask is empty or full.
  * Refuses bad arguments before any CUDA call; all iterations are enqueued without synchronising the host.  The result
- * does not depend on the batch or on scheduling. */
+ * does not depend on the batch or on scheduling.
+ * occluders [F, H, W] uint8 (device) or NULL, U and M' as nope_fit_translation_occluded: phi is the signed distance
+ * field of M', the box size that scales tau is that of M', and a contour pixel is counted and paired only when it and
+ * its four neighbours lie in U; iou uses S' and M', and "empty or full" is judged on M'. */
 int nope_mask_sdf(const uint8_t* masks, int F, int H, int W, double* sdf_out, void* stream);
-int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
-                        const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
-                        double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
-                        double* t_out, double* fit_out, int64_t* sums_out, void* stream);
+int nope_refine_contour_occluded(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
+                                 const double* t_init, const uint8_t* masks, const uint8_t* occluders,
+                                 const double* K, int F, int P, int H, int W, double rho, const double* tau, int iters,
+                                 float znear, float* depth, double* R_out, double* t_out, double* fit_out,
+                                 int64_t* sums_out, void* stream);
 
 /* BOP 2019 errors (DESIGN.md section 15).
  * nope_vsd_error_taus: nope_vsd_error at T misalignment tolerances in one pass (the distance images, visibility
@@ -424,17 +402,12 @@ int nope_crop_rotate(const double* Rv, int F, const double* R, int P, int to_cam
 int nope_track_seeds(const double* Rc, int H, const double* T, int N, float* out_D, int32_t* out_seed,
                      float* out_cossin, void* stream);
 
-/* Score materialised templates against a query and rank them: the arithmetic of
- * PoseConditional.retrieval (model.py:254-266) after encode_image.
- *   query_feat [B, C, HW] fp32, emb [B, N, C, HW] fp32 -> sim [B, N], topv/topi [B, k]. */
-int nope_score_topk(const float* query_feat, const float* emb, int B, int N, int C, int HW,
-                    int metric, float occlusion_threshold, int k, float* out_sim, float* out_topv,
-                    int64_t* out_topi, int64_t idx_base, void* stream);
-/* The same with the reference's broadcasting of query_feat against template_feat (model.py:260-262):
+/* Score materialised templates against queries and rank them: the arithmetic of PoseConditional.retrieval
+ * (model.py:254-266) after encode_image, with the reference's broadcasting of query_feat against template_feat
+ * (model.py:260-262):
  *   query_feat [B, Q, C, HW] fp32, emb [Bt, N, C, HW] fp32 with Bt = 1 (one template set for every query)
  *   or Bt = B (templates of row b for the Q queries of row b) -> sim [B, Q, N], topv/topi [B, Q, k].
- * No [B*Q, N, C, HW] difference tensor is formed: each template is read once and scored against its queries.
- * nope_score_topk is the Q = 1, Bt = B case. */
+ * No [B*Q, N, C, HW] difference tensor is formed: each template is read once and scored against its queries. */
 int nope_score_topk_multi(const float* query_feat, const float* emb, int B, int Q, int Bt, int N, int C, int HW,
                           int metric, float occlusion_threshold, int k, float* out_sim, float* out_topv,
                           int64_t* out_topi, int64_t idx_base, void* stream);
@@ -557,16 +530,15 @@ int nope_topk_merge(const float* gathered, int world, int64_t pack_floats, int B
  *       [n, C0, 2H, 2W], weight [Cout, 4*C0]), 3 = nearest-x2 upsample + 3x3 (HardUpsample,
  *       model_utils.py:161-165; input is [n, C0, H/2, W/2], weight [Cout, C0, 3, 3], folded
  *       inside into four 2x2 parity kernels).  x1 (optional) is concatenated after x0 along
- *       channels (u_net.py:186).  impl must be 2, as in nope_unet_set_conv_impl. */
-int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, int C1,
-                 const float* weight, const float* bias, float* out, int n_img, int H, int W,
-                 int Cout, void* stream);
+ *       channels (u_net.py:186). */
+int nope_op_conv(int mode, const float* x0, int C0, const float* x1, int C1, const float* weight, const float* bias,
+                 float* out, int n_img, int H, int W, int Cout, void* stream);
 /* Block.forward (model_utils.py:248-252): [SiLU](GroupNorm_G(conv(x) + bias)), normalised on the host
  * from nothing but the per-(32 pixels, 8 channels) partial sums the plain convolution epilogue writes
- * (the statistics the LDM engine's GroupNorms use).  mode 0..2 as nope_op_conv, impl must be 2. */
-int nope_op_conv_gn(int impl, int mode, const float* x0, int C0, const float* x1, int C1,
-                    const float* weight, const float* bias, const float* gamma, const float* beta,
-                    int G, int silu, float* out, int n_img, int H, int W, int Cout, void* stream);
+ * (the statistics the LDM engine's GroupNorms use).  mode 0..2 as nope_op_conv. */
+int nope_op_conv_gn(int mode, const float* x0, int C0, const float* x1, int C1, const float* weight,
+                    const float* bias, const float* gamma, const float* beta, int G, int silu, float* out, int n_img,
+                    int H, int W, int Cout, void* stream);
 /* The sweep's fused layer: out = [SiLU](GroupNorm_G(conv(x) + bias)) + chan_bias[n, c] +
  * residual[n / res_div] with everything after the convolution applied in its epilogue
  * (ResnetBlock.forward, model_utils.py:271-279; G = 0: no normalisation).  mode 0..2 as nope_op_conv.
@@ -602,8 +574,8 @@ int nope_unet_debug_tap(nope_unet_t* u, const float* ref_feat, const float* pose
  * Keys are the reference's state_dict names (628 tensors for model_channels 256; the unused
  * time_embed.* entries are accepted); HOST fp32 pointers, shape-checked.  The VAE encoder
  * (diffusers AutoencoderKL, not part of the reference tree) is out of scope: the sweep takes
- * latents.  Arguments of nope_ldm_sweep are those of nope_unet_sweep with
- * ref_feat / query_feat = [B, latent_ch, 32, 32] latents. */
+ * latents.  Arguments of nope_ldm_sweep_multi are those of nope_unet_sweep_multi with
+ * ref_feat = [B, latent_ch, 32, 32] and query_feat = [B, Q, latent_ch, 32, 32] latents. */
 typedef struct nope_ldm nope_ldm_t;
 int nope_ldm_create(nope_ldm_t** out, int model_channels, int context_dim, int latent_ch,
                     int latent_hw, int device);
@@ -612,9 +584,6 @@ int nope_ldm_load_tensor(nope_ldm_t* m, const char* key, const float* data, cons
                          int ndim);
 int nope_ldm_finalize(nope_ldm_t* m);
 int nope_ldm_set_chunk(nope_ldm_t* m, int hyps_per_chunk);       /* ~15.6 MB workspace / hypothesis (model_channels 256) */
-/* conv_impl: 2 = clustered wgmma kernel (the only one; anything else is an error);
- * attn_impl: 0 = wgmma attention (default), 1 = CUDA-core twin (bring-up). */
-int nope_ldm_set_impl(nope_ldm_t* m, int conv_impl, int attn_impl);
 /* Named options: "hoist" (default 1: the pose-independent prefix -- input conv, first ResBlock,
  * first transformer up to its self-attention -- runs once per reference instead of once per
  * hypothesis); before nope_ldm_finalize only: "precision"
@@ -622,11 +591,6 @@ int nope_ldm_set_impl(nope_ldm_t* m, int conv_impl, int attn_impl);
  * accumulates A W_hi + A W_lo, 2x the MMA work; embeddings 1.1e-3 -> below the 1e-3 bar against
  * the fp32 reference).  Any other name is an error. */
 int nope_ldm_set_option(nope_ldm_t* m, const char* name, int value);
-int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
-                   const float* query_latent, float* out_emb, float* out_sim, int k,
-                   float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream);
-/* Q queries per reference, as nope_unet_sweep_multi: query_latent [B, Q, latent_ch, 32, 32], out_sim [B, Q, N],
- * out_topv / out_topi [B, Q, k]; nope_ldm_sweep is the Q = 1 case. */
 int nope_ldm_sweep_multi(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
                          const float* query_latent, int Q, float* out_emb, float* out_sim, int k,
                          float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream);
@@ -651,9 +615,8 @@ int nope_ldm_debug_tap(nope_ldm_t* m, const float* ref_latent, const float* pose
 int nope_ldm_run_block(nope_ldm_t* m, const char* name, const float* x0, int C0, const float* x1,
                        int C1, int S, int n, const float* poses, float* out, void* stream);
 /* Multi-head self-attention core (ldm/attention.py:177-194, heads of 32 channels):
- * qkv [n_img, n_tok, 3C] fp32 (q | k | v) -> out [n_img, n_tok, C] fp32.  impl as attn_impl. */
-int nope_op_mh_attention(int impl, const float* qkv, float* out, int n_img, int n_tok, int C,
-                         void* stream);
+ * qkv [n_img, n_tok, 3C] fp32 (q | k | v) -> out [n_img, n_tok, C] fp32, on the wgmma attention kernel. */
+int nope_op_mh_attention(const float* qkv, float* out, int n_img, int n_tok, int C, void* stream);
 
 #ifdef __cplusplus
 }

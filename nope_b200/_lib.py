@@ -16,9 +16,6 @@ SIGNATURES = {
     "nope_abi_version": (C.c_int, []),
     "nope_build_arch": (C.c_char_p, []),
     "nope_unet_set_chunk": (C.c_int, [C.c_void_p, C.c_int]),
-    "nope_unet_set_conv_impl": (C.c_int, [C.c_void_p, C.c_int]),
-    "nope_unet_sweep": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, c_f32p,
-                                  c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_unet_sweep_multi": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, c_f32p,
                                         c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_unet_last_launch_count": (C.c_int64, [C.c_void_p]),
@@ -26,7 +23,6 @@ SIGNATURES = {
     "nope_unet_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double),
                                          C.POINTER(C.c_double), C.POINTER(C.c_int64), C.POINTER(C.c_double)]),
     "nope_unet_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
-    "nope_unet_get_option": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_int)]),
     "nope_unet_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "nope_unet_set_workspace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int]),
     "nope_op_conv_gn_fused": (C.c_int, [C.c_int, C.c_int, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, c_f32p,
@@ -61,9 +57,6 @@ SIGNATURES = {
                                  C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p]),
     "nope_vsd_error_taus": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                       C.c_double, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
-    "nope_fit_translation": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
-                                       C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, c_f32p,
-                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "nope_fit_translation_occluded": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                                 C.c_int, C.c_float, C.c_int, c_f32p, C.c_void_p, C.c_void_p,
@@ -73,9 +66,6 @@ SIGNATURES = {
                                     C.c_int, C.c_float, c_f32p, C.c_void_p, C.c_void_p, C.c_void_p, c_i64p,
                                     C.c_void_p]),
     "nope_mask_sdf": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
-    "nope_refine_contour": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
-                                      C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_int,
-                                      C.c_float, c_f32p, C.c_void_p, C.c_void_p, C.c_void_p, c_i64p, C.c_void_p]),
     "nope_refine_contour_occluded": (C.c_int, [c_f32p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                                C.c_double, C.c_void_p, C.c_int, C.c_float, c_f32p, C.c_void_p,
@@ -88,8 +78,6 @@ SIGNATURES = {
     "nope_crop_rotate": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "nope_track_seeds": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_void_p, c_f32p,
                                    C.c_void_p]),
-    "nope_score_topk": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                  C.c_int, c_f32p, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_score_topk_multi": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                         C.c_int, C.c_float, C.c_int, c_f32p, c_f32p, c_i64p, C.c_int64,
                                         C.c_void_p]),
@@ -118,19 +106,16 @@ SIGNATURES = {
     "nope_topk_pack_floats": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "nope_topk_merge": (C.c_int, [c_f32p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                   c_f32p, c_f32p, c_i64p, C.c_void_p]),
-    "nope_op_conv": (C.c_int, [C.c_int, C.c_int, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, c_f32p,
+    "nope_op_conv": (C.c_int, [C.c_int, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, c_f32p,
                                c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    "nope_op_conv_gn": (C.c_int, [C.c_int, C.c_int, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, c_f32p,
+    "nope_op_conv_gn": (C.c_int, [C.c_int, c_f32p, C.c_int, c_f32p, C.c_int, c_f32p, c_f32p,
                                   c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int,
                                   C.c_int, C.c_void_p]),
     "nope_op_linear_attention": (C.c_int, [C.c_int, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_op_attention": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_op_upsample2x": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_ldm_set_chunk": (C.c_int, [C.c_void_p, C.c_int]),
-    "nope_ldm_set_impl": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
     "nope_ldm_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
-    "nope_ldm_sweep": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, c_f32p,
-                                 c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_ldm_sweep_multi": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, c_f32p,
                                        c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
     "nope_ldm_last_launch_count": (C.c_int64, [C.c_void_p]),
@@ -141,7 +126,7 @@ SIGNATURES = {
                                      C.c_int64, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
     "nope_ldm_run_block": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int, c_f32p, C.c_int, C.c_int,
                                      C.c_int, c_f32p, c_f32p, C.c_void_p]),
-    "nope_op_mh_attention": (C.c_int, [C.c_int, c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "nope_op_mh_attention": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_unet_debug_tap": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_char_p, c_f32p,
                                       C.c_int64, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
 }
@@ -156,7 +141,7 @@ for _kind, _n in ENGINE_CREATE_ARGS.items():
         f"nope_{_kind}_finalize": (C.c_int, [C.c_void_p]),
     })
 
-EXPECTED_ABI = 2     # include/nope_b200.h "ABI version"; a stale build with other signatures must not bind
+EXPECTED_ABI = 3     # include/nope_b200.h "ABI version"; a stale build with other signatures must not bind
 MAX_TOPK = 64        # the most entries a ranking call selects per row (k, keep): mirrors kMaxTopK in csrc/rank.cuh
 
 _lib = None

@@ -3,8 +3,8 @@ iteration renders every pose hypothesis with the depth rasterizer of `nope_b200.
 rendered silhouette with the frame's object mask through the mask's signed distance field (`mask_sdf`), and takes one
 damped Gauss-Newton step of the rotation (about the object's origin) and the translation that moves the contour onto
 the mask's.  The pairing tolerance is a fraction of the mask's box size that shrinks from one iteration to the next.
-The fit runs on the GPU (`nope_mask_sdf`, `nope_refine_contour`, csrc/contour_refine.cuh); there is no CPU
-fallback."""
+The fit runs on the GPU (`nope_mask_sdf`, `nope_refine_contour_occluded`, csrc/contour_refine.cuh); there is no
+CPU fallback."""
 import numpy as np
 import torch
 

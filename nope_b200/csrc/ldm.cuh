@@ -63,7 +63,6 @@ struct nope_ldm {
   int nres = 2;
   std::vector<int> mult{1, 2, 4};
   bool finalized = false;
-  int attn_impl = 0;   // 0: wgmma attention, 1: CUDA-core twin
   bool hoist = true;        // pose-independent prefix once per reference (prestage)
   int precision = 0;        // 0: fp16 weights; 1: exact weights -- every packed row is [W_hi | W_lo] and the K loop
                             // walks its segment list twice (A W_hi + A W_lo), 2x the MMA work (set before finalize)
@@ -644,26 +643,22 @@ struct nope_ldm {
     const float sl2e = 0.17677669529663687f * 1.4426950408889634f;   // 32^-1/2 * log2(e)
     const dim3 grid((unsigned)(n * Hh) * (unsigned)((ntok + 127) / 128));
     if (prof.begin(st)) return -1;
-    if (attn_impl == 1) {
-      ldm_attn_simt_kernel<<<grid, 128, 0, st>>>(qkv, Vt, out, ntok, Hh, C, sl2e);
-    } else {
-      static bool attr_set[kMaxDevices];     // the shared-memory opt-in is per device
-      int dev = 0;
-      NOPE_CUDA(cudaGetDevice(&dev));
-      NOPE_CHECK(dev >= 0 && dev < kMaxDevices, "device index out of range");
-      if (!attr_set[dev]) {
-        NOPE_CUDA(cudaFuncSetAttribute(ldm_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
-        attr_set[dev] = true;
-      }
-      AttnParams p;
-      const CUtensorMap* m = nullptr;
-      if (get_map3(&m, qkv, 3 * C, ntok, n, 64, 128)) return -1;
-      p.qkmap = *m;
-      if (get_map3(&m, Vt, ntok, 32, n * Hh, 64, 32)) return -1;
-      p.vmap = *m;
-      p.out = out; p.n = ntok; p.H = Hh; p.C = C; p.scale_log2e = sl2e;
-      ldm_attn_tc_kernel<<<grid, 128, kAttnSmem, st>>>(p);
+    static bool attr_set[kMaxDevices];     // the shared-memory opt-in is per device
+    int dev = 0;
+    NOPE_CUDA(cudaGetDevice(&dev));
+    NOPE_CHECK(dev >= 0 && dev < kMaxDevices, "device index out of range");
+    if (!attr_set[dev]) {
+      NOPE_CUDA(cudaFuncSetAttribute(ldm_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
+      attr_set[dev] = true;
     }
+    AttnParams p;
+    const CUtensorMap* m = nullptr;
+    if (get_map3(&m, qkv, 3 * C, ntok, n, 64, 128)) return -1;
+    p.qkmap = *m;
+    if (get_map3(&m, Vt, ntok, 32, n * Hh, 64, 32)) return -1;
+    p.vmap = *m;
+    p.out = out; p.n = ntok; p.H = Hh; p.C = C; p.scale_log2e = sl2e;
+    ldm_attn_tc_kernel<<<grid, 128, kAttnSmem, st>>>(p);
     NOPE_CUDA(cudaGetLastError());
     const double fl = 4.0 * (double)n * ntok * (double)ntok * C;
     if (prof.end(st, {fl, fl, 1})) return -1;

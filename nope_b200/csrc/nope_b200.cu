@@ -40,7 +40,7 @@ using namespace nope;
 
 namespace {
 
-constexpr int kAbiVersion = 2;
+constexpr int kAbiVersion = 3;
 
 struct Scratch {
   std::vector<void*> p;
@@ -163,10 +163,6 @@ int nope_unet_set_chunk(nope_unet_t* u, int hyps) {
   u->chunk = hyps;
   return 0;
 }
-int nope_unet_set_conv_impl(nope_unet_t* u, int impl) {
-  NOPE_CHECK(u && impl == 2, "conv_impl must be 2 (tensor cores, clustered: conv_tc2_kernel)");
-  return 0;
-}
 int nope_unet_set_option(nope_unet_t* u, const char* name, int value) {
   NOPE_CHECK(u && name, "null argument");
   if (std::strcmp(name, "precision") == 0) {
@@ -175,19 +171,6 @@ int nope_unet_set_option(nope_unet_t* u, const char* name, int value) {
     u->precision = value;
     return 0;
   }
-  if (std::strcmp(name, "conv_impl") == 0) return nope_unet_set_conv_impl(u, value);
-  if (std::strcmp(name, "attn_impl") == 0) {
-    NOPE_CHECK(value == 0 || value == 1, "attn_impl must be 0 (tensor cores) or 1 (CUDA cores)");
-    u->attn_impl = value;
-    return 0;
-  }
-  return fail(std::string("unknown option: ") + name);
-}
-int nope_unet_get_option(const nope_unet_t* u, const char* name, int* value) {
-  NOPE_CHECK(u && name && value, "null argument");
-  if (std::strcmp(name, "precision") == 0) { *value = u->precision; return 0; }
-  if (std::strcmp(name, "conv_impl") == 0) { *value = 2; return 0; }
-  if (std::strcmp(name, "attn_impl") == 0) { *value = u->attn_impl; return 0; }
   return fail(std::string("unknown option: ") + name);
 }
 int64_t nope_unet_last_launch_count(const nope_unet_t* u) { return u ? u->launches : 0; }
@@ -253,13 +236,6 @@ int nope_unet_sweep_multi(nope_unet_t* u, const float* ref_feat, const float* po
                       stream);
 }
 
-int nope_unet_sweep(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
-                    const float* query_feat, float* out_emb, float* out_sim, int k, float* out_topv,
-                    int64_t* out_topi, int64_t idx_base, void* stream) {
-  return nope_unet_sweep_multi(u, ref_feat, poses, B, N, query_feat, 1, out_emb, out_sim, k, out_topv, out_topi,
-                               idx_base, stream);
-}
-
 int nope_unet_set_metric(nope_unet_t* u, int metric, float occlusion_threshold) {
   NOPE_CHECK(u, "null engine");
   NOPE_CHECK(metric == NOPE_METRIC_L2 || metric == NOPE_METRIC_COSINE || metric == NOPE_METRIC_COSINE_OCC,
@@ -319,13 +295,6 @@ int nope_score_topk_grouped(const float* query_feat, const float* emb, int R, in
     NOPE_CUDA(cudaGetLastError());
   }
   return 0;
-}
-
-int nope_score_topk(const float* query_feat, const float* emb, int B, int N, int C, int HW, int metric,
-                    float occlusion_threshold, int k, float* out_sim, float* out_topv, int64_t* out_topi,
-                    int64_t idx_base, void* stream) {
-  return nope_score_topk_multi(query_feat, emb, B, 1, B, N, C, HW, metric, occlusion_threshold, k, out_sim, out_topv,
-                               out_topi, idx_base, stream);
 }
 
 int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_topi, int64_t idx_base,
@@ -867,16 +836,8 @@ static int check_rho_tau(double rho, const double* tau, int iters) {
   return 0;
 }
 
-int nope_fit_translation(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
-                         const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
-                         float znear, int iters, float* depth, double* t_out, double* iou, int32_t* stats_out,
-                         void* stream) {
-  return nope_fit_translation_occluded(vertices, V, faces, NF, R, t_init, masks, nullptr, K, F, P, H, W, znear, iters,
-                                       depth, t_out, iou, stats_out, stream);
-}
-
 // occluders [F, H, W] (nullable): the pixels where the object may be hidden count for neither the silhouette nor the
-// mask (DESIGN.md section 24); null is the plain fit, bit for bit
+// mask (DESIGN.md section 24); null: every pixel counts
 int nope_fit_translation_occluded(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
                                   const double* t_init, const uint8_t* masks, const uint8_t* occluders,
                                   const double* K, int F, int P, int H, int W, float znear, int iters, float* depth,
@@ -993,16 +954,8 @@ int nope_mask_sdf(const uint8_t* masks, int F, int H, int W, double* sdf_out, vo
   return launch_mask_sdf(masks, nullptr, F, H, W, g, sdf_out, st);
 }
 
-int nope_refine_contour(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
-                        const double* t_init, const uint8_t* masks, const double* K, int F, int P, int H, int W,
-                        double rho, const double* tau, int iters, float znear, float* depth, double* R_out,
-                        double* t_out, double* fit_out, int64_t* sums_out, void* stream) {
-  return nope_refine_contour_occluded(vertices, V, faces, NF, R, t_init, masks, nullptr, K, F, P, H, W, rho, tau,
-                                      iters, znear, depth, R_out, t_out, fit_out, sums_out, stream);
-}
-
 // occluders [F, H, W] (nullable): phi and the mask statistics are those of the mask minus the occluders, and a contour
-// pixel next to an occluder is not paired (DESIGN.md section 24); null is the plain refinement, bit for bit
+// pixel next to an occluder is not paired (DESIGN.md section 24); null: every pixel counts
 int nope_refine_contour_occluded(const float* vertices, int V, const int32_t* faces, int NF, const double* R,
                                  const double* t_init, const uint8_t* masks, const uint8_t* occluders,
                                  const double* K, int F, int P, int H, int W, double rho, const double* tau, int iters,
@@ -1182,11 +1135,9 @@ struct OpConv {
 };
 }  // namespace
 
-int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, int C1,
-                 const float* weight, const float* bias, float* out, int n_img, int H, int W,
-                 int Cout, void* stream) {
+int nope_op_conv(int mode, const float* x0, int C0, const float* x1, int C1, const float* weight, const float* bias,
+                 float* out, int n_img, int H, int W, int Cout, void* stream) {
   NOPE_CHECK(out, "null argument");
-  NOPE_CHECK(impl == 2, "impl must be 2 (tensor cores, clustered: conv_tc2_kernel)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   OpConv op;
   if (op.setup(mode, 3, 0, x0, C0, x1, C1, weight, bias, n_img, H, W, Cout, st)) return -1;
@@ -1196,11 +1147,10 @@ int nope_op_conv(int impl, int mode, const float* x0, int C0, const float* x1, i
   return 0;
 }
 
-int nope_op_conv_gn(int impl, int mode, const float* x0, int C0, const float* x1, int C1,
-                    const float* weight, const float* bias, const float* gamma, const float* beta,
-                    int G, int silu, float* out, int n_img, int H, int W, int Cout, void* stream) {
+int nope_op_conv_gn(int mode, const float* x0, int C0, const float* x1, int C1, const float* weight,
+                    const float* bias, const float* gamma, const float* beta, int G, int silu, float* out, int n_img,
+                    int H, int W, int Cout, void* stream) {
   NOPE_CHECK(gamma && beta && out, "null argument");
-  NOPE_CHECK(impl == 2, "impl must be 2 (tensor cores, clustered: conv_tc2_kernel)");
   NOPE_CHECK(G >= 1 && (Cout / 8) % G == 0, "groups must divide the 8-channel octets");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int hw = H * W, parts = hw < 32 ? 1 : hw / 32, noct = Cout / 8;
@@ -1388,12 +1338,6 @@ int nope_ldm_set_chunk(nope_ldm_t* m, int hyps) {
   m->chunk = hyps;
   return 0;
 }
-int nope_ldm_set_impl(nope_ldm_t* m, int conv_impl, int attn_impl) {
-  NOPE_CHECK(m && conv_impl == 2, "conv_impl must be 2 (tensor cores, clustered)");
-  NOPE_CHECK(attn_impl == 0 || attn_impl == 1, "attn_impl must be 0 (tensor cores) or 1 (CUDA cores)");
-  m->attn_impl = attn_impl;
-  return 0;
-}
 int nope_ldm_set_option(nope_ldm_t* m, const char* name, int value) {
   NOPE_CHECK(m && name, "null argument");
   if (std::strcmp(name, "hoist") == 0) { m->hoist = value != 0; return 0; }
@@ -1432,13 +1376,6 @@ int nope_ldm_sweep_multi(nope_ldm_t* m, const float* ref_latent, const float* po
                          int64_t* out_topi, int64_t idx_base, void* stream) {
   return engine_sweep(m, ref_latent, poses, B, N, query_latent, Q, out_emb, out_sim, k, out_topv, out_topi, idx_base,
                       stream);
-}
-
-int nope_ldm_sweep(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
-                   const float* query_latent, float* out_emb, float* out_sim, int k, float* out_topv,
-                   int64_t* out_topi, int64_t idx_base, void* stream) {
-  return nope_ldm_sweep_multi(m, ref_latent, poses, B, N, query_latent, 1, out_emb, out_sim, k, out_topv, out_topi,
-                              idx_base, stream);
 }
 
 int nope_ldm_debug_tap(nope_ldm_t* m, const float* ref_latent, const float* poses, int N, const char* tap,
@@ -1484,13 +1421,11 @@ int nope_ldm_run_block(nope_ldm_t* m, const char* name, const float* x0, int C0,
   return 0;
 }
 
-int nope_op_mh_attention(int impl, const float* qkv, float* out, int n_img, int n_tok, int C, void* stream) {
+int nope_op_mh_attention(const float* qkv, float* out, int n_img, int n_tok, int C, void* stream) {
   NOPE_CHECK(qkv && out && n_img >= 1 && n_tok >= 64 && n_tok % 64 == 0 && C % 64 == 0 && C >= 64,
              "bad arguments (n_tok and C must be multiples of 64)");
-  NOPE_CHECK(impl == 0 || impl == 1, "impl must be 0 (tensor cores) or 1 (CUDA cores)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   nope_ldm e;    // only the attention staging buffers are used; freed by the destructor
-  e.attn_impl = impl;
   const size_t tok = (size_t)n_img * n_tok;
   __half *q16 = nullptr, *o16 = nullptr;
   if (e.ws_mem.alloc(&q16, tok * 3 * C) || e.ws_mem.alloc(&o16, tok * C) || e.ws_mem.alloc(&e.Vt, tok * C)) return -1;

@@ -79,7 +79,6 @@ struct UNetEngine {
   // (exact weights + activations carried as hi + lo: A_hi W_hi + A_hi W_lo + A_lo W_hi, 3x);
   // 3: bf16 operands and activations (8-bit mantissa: its own, looser tolerance)
   int precision = 0;
-  int attn_impl = 0;         // LinearAttention core: 0 wgmma (token counts >= 128), 1 CUDA cores
   int metric = 0;            // NOPE_METRIC_* of the fused scoring
   float occ_threshold = 0.2f;
   int chunk = 642;
@@ -656,7 +655,7 @@ struct UNetEngine {
     sq.pre_stats = SB;
     sq.pre_parts = fused_emit_parts(S, C);
     if (conv(convs.at(p + ".qkvf"), x, Act(), Act(TD.hi, 3 * kHeadsHidden), S, n, cap, st, &sq)) return -1;
-    if (attn_impl == 0 && S * S >= kBM) {
+    if (S * S >= kBM) {
       if (launch_linattn_tc(TD.hi, TC.hi, n, S * S, num_sms, st, bf())) return -1;
     } else {
       NOPE_CUDA(launch_pdl(linattn_kernel, dim3(4, n), dim3(kLinAttnThreads), 0, st, TD.hi, TC.hi, S * S, bf()));

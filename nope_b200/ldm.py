@@ -50,7 +50,6 @@ class UNetModelPose(SweepEngine):
         if precision not in ("fp16", "fp16_w2"):
             raise ValueError("UNetModelPose precision: 'fp16' or 'fp16_w2'")
         self.precision = precision
-        self._impl = (2, 0)         # nope_ldm_set_impl (conv, attn)
         super().__init__("ldm", chunk, 2 * model_channels)
 
     def _create_args(self):
@@ -59,11 +58,10 @@ class UNetModelPose(SweepEngine):
         return self.model_channels, self.context_dim, self.channels, 32, self.device.index or 0
 
     def _configure(self, lib, h):
-        """chunk, precision, implementation and options: applied to every engine before its weights"""
+        """chunk, precision and options: applied to every engine before its weights"""
         _lib.check(lib.nope_ldm_set_chunk(h, self._chunk))
         if self.precision == "fp16_w2":
             _lib.check(lib.nope_ldm_set_option(h, b"precision", 1))
-        _lib.check(lib.nope_ldm_set_impl(h, *self._impl))
         for k, v in self._options.items():
             _lib.check(lib.nope_ldm_set_option(h, k.encode(), v))
 
@@ -83,11 +81,6 @@ class UNetModelPose(SweepEngine):
             if vae_sd:
                 self.encoder.load_state_dict(vae_sd, strict=strict)
         return self
-
-    def set_impl(self, conv="tcgen05_2cta", attn="tcgen05"):
-        impl = ({"tcgen05_2cta": 2}[conv], {"tcgen05": 0, "simt": 1}[attn])
-        _lib.check(_lib.load().nope_ldm_set_impl(self._handle(), *impl))
-        self._impl = impl
 
     def profile_read(self):
         """-> {'gemm': {...}, 'attention': {...}} with ms / flops / launches since profile(True)."""
@@ -154,13 +147,13 @@ class UNetModelPose(SweepEngine):
         return out
 
 
-def mh_attention(qkv, impl="tcgen05"):
+def mh_attention(qkv):
     """Multi-head self-attention core on qkv [n_img, n_tok, 3C] (CUDA fp32) -> [n_img, n_tok, C]."""
     lib = _lib.load()
     qkv = qkv.to(torch.float32).contiguous()
     n_img, n_tok, c3 = qkv.shape
     out = torch.empty((n_img, n_tok, c3 // 3), device=qkv.device, dtype=torch.float32)
     with torch.cuda.device(qkv.device):
-        _lib.check(lib.nope_op_mh_attention({"tcgen05": 0, "simt": 1}[impl], _lib.ptr(qkv), _lib.ptr(out),
-                                            n_img, n_tok, c3 // 3, _lib.stream(qkv.device)))
+        _lib.check(lib.nope_op_mh_attention(_lib.ptr(qkv), _lib.ptr(out), n_img, n_tok, c3 // 3,
+                                            _lib.stream(qkv.device)))
     return out

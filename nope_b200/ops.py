@@ -6,15 +6,12 @@ import torch
 
 from . import _lib
 
-_IMPL = {"tcgen05_2cta": 2}
-
-
 
 def _f32(t):
     return None if t is None else t.to(torch.float32).contiguous()
 
 
-def conv(x0, weight, bias=None, x1=None, mode="3x3", impl="tcgen05_2cta"):
+def conv(x0, weight, bias=None, x1=None, mode="3x3"):
     """mode '3x3' (pad 1), '1x1', 'unshuffle' (pixel-unshuffle(2) + 1x1; weight
     [Cout, 4*Cin, 1, 1]) or 'upsample3x3' (nearest x2 + conv3x3, folded into four 2x2 parity
     kernels; x0 is the low-resolution input).  x1 is concatenated after x0 along channels."""
@@ -26,13 +23,13 @@ def conv(x0, weight, bias=None, x1=None, mode="3x3", impl="tcgen05_2cta"):
     cout = weight.shape[0]
     out = torch.empty((n, cout, h, w), device=x0.device, dtype=torch.float32)
     with torch.cuda.device(x0.device):
-        _lib.check(lib.nope_op_conv(_IMPL[impl], m, _lib.ptr(x0), c0, _lib.ptr(x1),
+        _lib.check(lib.nope_op_conv(m, _lib.ptr(x0), c0, _lib.ptr(x1),
                                     0 if x1 is None else x1.shape[1], _lib.ptr(weight),
                                     _lib.ptr(bias), _lib.ptr(out), n, h, w, cout, _lib.stream(x0.device)))
     return out
 
 
-def conv_gn(x0, weight, bias, gamma, beta, groups, silu=True, x1=None, mode="3x3", impl="tcgen05_2cta"):
+def conv_gn(x0, weight, bias, gamma, beta, groups, silu=True, x1=None, mode="3x3"):
     """[SiLU](GroupNorm(conv(x))), normalised on the host from the partial sums of the plain conv epilogue."""
     lib = _lib.load()
     m = {"3x3": 0, "1x1": 1, "unshuffle": 2}[mode]
@@ -42,7 +39,7 @@ def conv_gn(x0, weight, bias, gamma, beta, groups, silu=True, x1=None, mode="3x3
     cout = weight.shape[0]
     out = torch.empty((n, cout, h, w), device=x0.device, dtype=torch.float32)
     with torch.cuda.device(x0.device):
-        _lib.check(lib.nope_op_conv_gn(_IMPL[impl], m, _lib.ptr(x0), c0, _lib.ptr(x1),
+        _lib.check(lib.nope_op_conv_gn(m, _lib.ptr(x0), c0, _lib.ptr(x1),
                                        0 if x1 is None else x1.shape[1], _lib.ptr(weight),
                                        _lib.ptr(bias), _lib.ptr(gamma), _lib.ptr(beta), groups,
                                        1 if silu else 0, _lib.ptr(out), n, h, w, cout,

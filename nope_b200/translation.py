@@ -3,9 +3,10 @@ module fits, for each frame and rotation hypothesis, the translation whose rende
 object's mask in the frame, and reports the silhouette IoU there.
 
 `initial_translation` is a rotation-agnostic start from the mask's bounding box and the object diameter (plain torch,
-CPU or GPU).  `estimate_translation` runs the fit on the GPU (`nope_fit_translation`, csrc/translation.cuh): each
-update renders the silhouette with the depth rasterizer of `nope_b200.vsd`, scales the distance by the ratio of the
-bounding-box sizes and moves the origin so the silhouette's box centre lands on the mask's.  There is no CPU fallback.
+CPU or GPU).  `estimate_translation` runs the fit on the GPU (`nope_fit_translation_occluded`,
+csrc/translation.cuh): each update renders the silhouette with the depth rasterizer of `nope_b200.vsd`, scales the
+distance by the ratio of the bounding-box sizes and moves the origin so the silhouette's box centre lands on the
+mask's.  There is no CPU fallback.
 A mask cut by the frame border has a cut bounding box, and the fit follows it: no special handling."""
 import numpy as np
 import torch

@@ -68,10 +68,9 @@ class SweepEngine:
             self._native.call("set_chunk", hyps)
 
     def set_option(self, name, value):
-        """Named engine option (include/nope_b200.h, nope_<kind>_set_option), e.g. the UNet's 'attn_impl' (0:
-        LinearAttention on tensor cores, 1: CUDA cores) or 'conv_impl' (2, the only one).  It is applied at once,
-        to a weightless engine if none is built yet, and kept for every later build; unknown names raise NopeError
-        and are not kept."""
+        """Named engine option (include/nope_b200.h, nope_<kind>_set_option), e.g. the LDM engine's 'hoist'.  It is
+        applied at once, to a weightless engine if none is built yet, and kept for every later build; unknown names
+        raise NopeError and are not kept."""
         self._handle()
         self._native.call("set_option", name.encode(), int(value))
         self._options[name] = int(value)
@@ -244,10 +243,10 @@ class UNet(SweepEngine):
         _lib.check(_lib.load().nope_unet_set_metric(self._handle(), _METRICS[metric], float(threshold)))
 
     def set_conv_impl(self, impl):
-        """'tcgen05_2cta': the clustered kernel with the fused epilogues, the engine's only convolution."""
+        """'tcgen05_2cta': the clustered kernel with the fused epilogues, the engine's only convolution.  Anything else
+        raises NopeError; the call changes nothing in the engine."""
         if impl != "tcgen05_2cta":
             raise _lib.NopeError(f"unknown conv impl {impl!r}: the only convolution is 'tcgen05_2cta' (conv_tc2_kernel)")
-        _lib.check(_lib.load().nope_unet_set_conv_impl(self._handle(), 2))
 
     def profile_read(self):
         """-> dict(conv_ms, conv_flops (executed), conv_alg_flops, conv_launches, max_launch_tflops)."""

@@ -18,7 +18,7 @@ def test_library_builds_and_loads():
     build.build()
     from nope_b200 import _lib
     lib = _lib.load()
-    assert lib.nope_abi_version() == _lib.EXPECTED_ABI == 2
+    assert lib.nope_abi_version() == _lib.EXPECTED_ABI == 3
     assert lib.nope_build_arch() == b"sm_90a"
 
 

@@ -114,7 +114,7 @@ def test_header_declares_and_lib_binds_the_new_calls():
     from nope_b200 import _lib
     for n in ("nope_pose_cells_expand", "nope_pose_cells_rank"):
         assert n in _declared() and n in _lib.SIGNATURES
-    assert _lib.EXPECTED_ABI == 2
+    assert _lib.EXPECTED_ABI == 3
 
 
 @pytest.mark.parametrize("args,needle", [

@@ -234,7 +234,7 @@ def test_c_abi_refuses_bad_arguments():
                 None]
         if null is not None:
             args[null] = None
-        return lib.nope_refine_contour(*args)
+        return lib.nope_refine_contour_occluded(*args[:7], None, *args[7:])     # occluders NULL
     for kw in (dict(F=0), dict(F=65536), dict(P=0), dict(P=65536), dict(H=0), dict(W=8193), dict(iters=-1),
                dict(iters=1025), dict(znear=0.0), dict(znear=math.inf), dict(rho=0.0), dict(rho=-1.0),
                dict(rho=math.nan), dict(tv=tau * [1, 1, 0]), dict(tv=tau * [1, -1, 1]), dict(tv=tau * [np.nan, 1, 1]),

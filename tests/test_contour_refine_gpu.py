@@ -1,8 +1,8 @@
 """GPU: the contour refinement (DESIGN.md section 20).  nope_mask_sdf against the numpy oracle bit for bit, at 720 x 540
-and on edge cases; nope_refine_contour against the oracle bit for bit, integer sums included, on the same render_depth
-images after 0 ... 6 updates; the true pose kept to the bit; accuracy from perturbed starts; batch independence;
-masks without a contour; no host synchronisation; `PoseConditional.refine_contour` with rerank, and eval_bop at
-refined poses."""
+and on edge cases; nope_refine_contour_occluded without occluders against the oracle bit for bit, integer sums included,
+on the same render_depth images after 0 ... 6 updates; the true pose kept to the bit; accuracy from perturbed starts;
+batch independence; masks without a contour; no host synchronisation; `PoseConditional.refine_contour` with rerank, and
+eval_bop at refined poses."""
 import os
 
 import numpy as np
@@ -102,9 +102,9 @@ def test_workspace_holds_the_final_render():
     t = torch.empty((2, 3, 3), device="cuda", dtype=torch.float64)
     fit = torch.empty((2, 3, 4), device="cuda", dtype=torch.float64)
     tau = TAUS[:4].copy()
-    _lib.check(_lib.load().nope_refine_contour(
+    _lib.check(_lib.load().nope_refine_contour_occluded(
         _lib.ptr(mesh.vertices), mesh.vertices.shape[0], _lib.ptr(mesh.faces), mesh.num_faces, _lib.ptr(Rd),
-        _lib.ptr(td), _lib.ptr(M), K.ctypes.data, 2, 3, H, W, mesh.radius, tau.ctypes.data, 3, 0.05,
+        _lib.ptr(td), _lib.ptr(M), None, K.ctypes.data, 2, 3, H, W, mesh.radius, tau.ctypes.data, 3, 0.05,
         _lib.ptr(depth), _lib.ptr(R), _lib.ptr(t), _lib.ptr(fit), None, _stream(torch.device("cuda"))))
     Rh, th = R.cpu().numpy(), t.cpu().numpy()
     for f in range(2):

@@ -66,8 +66,7 @@ def test_conv_2cta(dev, n, C0, C1, Cout, S, mode):
         check_rounds(dev, case, pairs)
     x0, x1, w, b = make_conv_case(n, C0, C1, Cout, S, mode)
     ref = conv_reference(*_d64(dev, x0, x1, w, b), mode)
-    out = ops.conv(x0.to(dev), w.to(dev), b.to(dev), None if x1 is None else x1.to(dev),
-                   mode=mode, impl="tcgen05_2cta")
+    out = ops.conv(x0.to(dev), w.to(dev), b.to(dev), None if x1 is None else x1.to(dev), mode=mode)
     e, blk = worst_block_rel_l2(out, ref, pick_bn(Cout))
     log("conv_2cta", n=n, C0=C0, C1=C1, Cout=Cout, S=S, mode=mode, pair_tiles=pairs, rounds=rounds(pairs, dev),
         n_tiles=Cout // pick_bn(Cout), worst_block_rel_l2=e,
@@ -79,7 +78,7 @@ def _no_bias_case(dev, n, C0, C1, Cout=384):
     from nope_b200 import ops
     x0, x1, w, _ = make_conv_case(n, C0, C1, Cout, 16, "3x3", seed=9)
     ref = conv_reference(*_d64(dev, x0, x1, w), None, "3x3")
-    out = ops.conv(x0.to(dev), w.to(dev), None, x1.to(dev), mode="3x3", impl="tcgen05_2cta")
+    out = ops.conv(x0.to(dev), w.to(dev), None, x1.to(dev), mode="3x3")
     e, blk = worst_block_rel_l2(out, ref, pick_bn(Cout))
     pairs = conv_pairs(n, Cout, 16, "3x3")
     log("conv_2cta_no_bias", n=n, Cout=Cout, pair_tiles=pairs, rounds=rounds(pairs, dev), worst_block_rel_l2=e,
@@ -120,7 +119,7 @@ def test_conv_gn(dev, n, C0, C1, Cout, S, mode, G):
     x0d, x1d, wd, bd, gd, btd = _d64(dev, x0, x1, w, b, gamma, beta)
     ref = F.silu(F.group_norm(conv_reference(x0d, x1d, wd, bd, mode), G, gd, btd, eps=1e-5))
     out = ops.conv_gn(x0.to(dev), w.to(dev), b.to(dev), gamma.to(dev), beta.to(dev), G, silu=True,
-                      x1=None if x1 is None else x1.to(dev), mode=mode, impl="tcgen05_2cta")
+                      x1=None if x1 is None else x1.to(dev), mode=mode)
     e, blk = worst_block_rel_l2(out, ref, pick_bn(Cout))
     log("conv_gn", n=n, Cout=Cout, S=S, G=G, pair_tiles=pairs, rounds=rounds(pairs, dev), worst_block_rel_l2=e,
         worst_block=blk)

@@ -187,7 +187,7 @@ def test_header_declares_and_lib_binds_crop():
     from nope_b200 import _lib
     lib = _lib.load()
     assert "nope_crop_frames" in _declared() and "nope_crop_frames" in _lib.SIGNATURES
-    assert hasattr(lib, "nope_crop_frames") and lib.nope_abi_version() == 2
+    assert hasattr(lib, "nope_crop_frames") and lib.nope_abi_version() == 3
 
 
 P = C.c_void_p(256)

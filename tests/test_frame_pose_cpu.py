@@ -146,7 +146,7 @@ def test_header_declares_and_lib_binds_crop_camera():
     lib = _lib.load()
     for name in ("nope_crop_camera", "nope_crop_rotate"):
         assert name in _declared() and name in _lib.SIGNATURES and hasattr(lib, name)
-    assert lib.nope_abi_version() == 2
+    assert lib.nope_abi_version() == 3
 
 
 def _pose_buf(F=2, **set_):

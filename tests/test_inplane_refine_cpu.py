@@ -194,7 +194,7 @@ def test_header_declares_and_lib_binds_the_new_calls():
     lib = _lib.load()
     for n in NEW_CALLS:
         assert n in _declared() and n in _lib.SIGNATURES and hasattr(lib, n)
-    assert _lib.EXPECTED_ABI == 2 and lib.nope_abi_version() == 2
+    assert _lib.EXPECTED_ABI == 3 and lib.nope_abi_version() == 3
 
 
 P = C.c_void_p(256)     # never dereferenced: every case below is refused before any CUDA call

@@ -91,20 +91,19 @@ def ldm_model(ldm_sd):
 
 
 @pytest.mark.parametrize("n_tok,C", [(64, 1024), (256, 512), (1024, 256), (320, 64)])
-@pytest.mark.parametrize("impl", ["simt", "tcgen05"])
-def test_mh_attention(impl, n_tok, C):
+def test_mh_attention(n_tok, C):
     """softmax(q k^T / sqrt(32)) v per head against torch fp32 on the fp16-rounded operands."""
     from nope_b200.ldm import mh_attention
     g = torch.Generator().manual_seed(n_tok + C)
     qkv = torch.randn(2, n_tok, 3 * C, generator=g) * 1.5
     qkv = qkv.half().float()
-    out = mh_attention(qkv.cuda(), impl=impl).cpu()
+    out = mh_attention(qkv.cuda()).cpu()
     H = C // 32
     q, k, v = [t.reshape(2, n_tok, H, 32).permute(0, 2, 1, 3) for t in qkv.chunk(3, dim=-1)]
     att = (torch.einsum("bhid,bhjd->bhij", q, k) * 32 ** -0.5).softmax(dim=-1)
     ref = torch.einsum("bhij,bhjd->bhid", att, v).permute(0, 2, 1, 3).reshape(2, n_tok, C)
     e = rel_l2(out, ref)
-    log("ldm_mh_attention", impl=impl, n_tok=n_tok, C=C, rel_l2=e, max_rel=max_rel(out, ref))
+    log("ldm_mh_attention", n_tok=n_tok, C=C, rel_l2=e, max_rel=max_rel(out, ref))
     assert e < 1.5e-3
 
 
@@ -121,16 +120,11 @@ def test_module_in_isolation(ldm_model, oracle_taps, mod):
     assert e < BLOCK_TOL
 
 
-@pytest.mark.parametrize("attn", ["tcgen05", "simt"])
-def test_forward_vs_oracle(ldm_model, oracle_taps, golden, attn):
-    ldm_model.set_impl(attn=attn)
-    try:
-        ref = torch.from_numpy(golden["ref_latent"])
-        emb = ldm_model(ref.expand(N_HYP, -1, -1, -1), oracle_taps["poses"])
-    finally:
-        ldm_model.set_impl()
+def test_forward_vs_oracle(ldm_model, oracle_taps, golden):
+    ref = torch.from_numpy(golden["ref_latent"])
+    emb = ldm_model(ref.expand(N_HYP, -1, -1, -1), oracle_taps["poses"])
     e = rel_l2(emb, oracle_taps["emb"])
-    log("ldm_forward_vs_oracle", attn=attn, emb_rel_l2=e, launches=ldm_model.last_launch_count)
+    log("ldm_forward_vs_oracle", emb_rel_l2=e, launches=ldm_model.last_launch_count)
     assert e < EMB_TOL_FP16
 
 
@@ -236,14 +230,16 @@ def test_rejects_bad_input(ldm_model):
     from nope_b200.ldm import UNetModelPose
     with pytest.raises(ValueError):
         UNetModelPose(channel_mult=(1, 2, 4, 8))
-    # on an engine before finalize, where every option it has is accepted: names it does not have and
-    # conv_impl 0 are errors
+    # on an engine before finalize, where every option it has is accepted: names it does not have are errors,
+    # the implementation switches included
     fresh = UNetModelPose(device="cuda:0", chunk=1)
-    for name in ("fuse_geglu", "fold_residual", "wide_tiles"):
+    for name, value in (("fuse_geglu", 1), ("fold_residual", 1), ("wide_tiles", 1), ("conv_impl", 2),
+                        ("attn_impl", 1)):
         with pytest.raises(_lib.NopeError):
-            fresh.set_option(name, 1)
-    with pytest.raises(_lib.NopeError):
-        _lib.check(_lib.load().nope_ldm_set_impl(fresh._handle(), 0, 0))
+            fresh.set_option(name, value)
+    lib = _lib.load()
+    for name in ("nope_ldm_set_impl", "nope_ldm_sweep"):
+        assert not hasattr(lib, name), name
 
 
 # ---------------------------------------------------------------- production batch sizes

@@ -27,18 +27,7 @@ def test_new_entry_points_declared_bound_and_exported():
     assert _declared() == set(_lib.SIGNATURES)
     for n in NEW:
         assert n in _lib.SIGNATURES and hasattr(lib, n)
-    assert lib.nope_abi_version() == 2       # additions only
-
-
-def test_multi_query_signatures_extend_the_single_query_ones():
-    """the *_multi calls take the single-query arguments plus `int Q` right after the query pointer"""
-    from nope_b200 import _lib
-    S = _lib.SIGNATURES
-    for one, multi in (("nope_unet_sweep", "nope_unet_sweep_multi"), ("nope_ldm_sweep", "nope_ldm_sweep_multi")):
-        a, b = S[one][1], S[multi][1]
-        assert b[:6] + b[7:] == a and b[6] is C.c_int
-    a, b = S["nope_score_topk"][1], S["nope_score_topk_multi"][1]
-    assert b[:3] + b[5:] == a and b[3] is C.c_int and b[4] is C.c_int
+    assert lib.nope_abi_version() == 3
 
 
 def _fake():

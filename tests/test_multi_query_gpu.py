@@ -2,8 +2,9 @@
 nope_score_topk_multi and the Python forms above them).
 
 Pinned here: a Q-query call is bit-identical to Q one-query calls (each (hypothesis, query) score is summed
-in an order that does not depend on Q), Q = 1 is bit-identical to the single-query entry point, and the
-scores meet the same tolerances against the CPU oracle as the single-query path (tests/test_unet_gpu.py)."""
+in an order that does not depend on Q), a [B, 1, ...] query through the Python layer is bit-identical to a
+[B, C, 32, 32] query through the C ABI, and the scores meet the same tolerances against the CPU oracle as the
+single-query path (tests/test_unet_gpu.py)."""
 import ctypes as C
 
 import numpy as np
@@ -30,7 +31,7 @@ def multi_queries(g, Q=5):
 
 
 def _direct_sweep(u, rf, poses, qf, k):
-    """nope_unet_sweep (the single-query entry point) called directly through the C ABI"""
+    """nope_unet_sweep_multi with Q = 1 and a [B, C, 32, 32] query, called directly through the C ABI"""
     from nope_b200 import _lib
     lib = _lib.load()
     dev = u.device
@@ -41,9 +42,9 @@ def _direct_sweep(u, rf, poses, qf, k):
     topi = torch.empty((B, k), device=dev, dtype=torch.int64)
     u.reserve(min(u._chunk, B * N), B, B * N)
     with torch.cuda.device(dev):
-        _lib.check(lib.nope_unet_sweep(u._handle(), _lib.ptr(rf), _lib.ptr(poses), B, N, _lib.ptr(qf), None,
-                                       _lib.ptr(sim), k, _lib.ptr(topv), _lib.ptr(topi), 0,
-                                       C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        _lib.check(lib.nope_unet_sweep_multi(u._handle(), _lib.ptr(rf), _lib.ptr(poses), B, N, _lib.ptr(qf), 1,
+                                             None, _lib.ptr(sim), k, _lib.ptr(topv), _lib.ptr(topi), 0,
+                                             C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
     return sim, topv, topi
 
 

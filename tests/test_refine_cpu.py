@@ -157,7 +157,7 @@ def test_header_declares_and_lib_binds_the_new_calls():
     lib = _lib.load()
     for n in ("nope_pose_refine_propose", "nope_pose_refine_select"):
         assert n in _declared() and n in _lib.SIGNATURES and hasattr(lib, n)
-    assert _lib.EXPECTED_ABI == 2
+    assert _lib.EXPECTED_ABI == 3
 
 
 @pytest.mark.parametrize("R,keep,B,Q,needle", [(2, 0, 2, 1, "keep"), (2, 65, 2, 1, "keep"), (3, 2, 2, 1, "R")])

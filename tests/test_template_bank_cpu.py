@@ -236,7 +236,7 @@ def test_grouped_abi_is_declared_and_bound():
     from nope_b200 import _lib
     assert "nope_score_topk_grouped" in _lib.SIGNATURES
     assert hasattr(_lib.load(), "nope_score_topk_grouped")
-    assert _lib.load().nope_abi_version() == 2
+    assert _lib.load().nope_abi_version() == 3
 
 
 def test_grouped_abi_refusals():

@@ -139,7 +139,7 @@ def test_c_abi_refuses_bad_arguments():
         args = [1, V, 1, NF, 1, 1, 1, k.ctypes.data, F, P, H, W, znear, iters, 1, 1, 1, None, None]
         if null is not None:
             args[null] = None
-        return lib.nope_fit_translation(*args)
+        return lib.nope_fit_translation_occluded(*args[:7], None, *args[7:])     # occluders NULL
     for kw in (dict(F=0), dict(F=65536), dict(P=0), dict(P=65536), dict(H=0), dict(W=8193), dict(iters=-1),
                dict(znear=0.0), dict(znear=-1.0), dict(znear=math.inf), dict(k=K * [np.nan, 1, 1, 1]),
                dict(k=K * [1, 0, 1, 1]), dict(k=K * [1, 1, np.inf, 1]), dict(V=0), dict(NF=0), dict(null=0),

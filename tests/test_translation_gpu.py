@@ -1,7 +1,7 @@
-"""GPU: the translation fit (DESIGN.md section 18).  nope_fit_translation against the numpy oracle bit for bit on the
-same render_depth images after 0 ... 6 updates; the silhouette counts against render_depth's coverage; accuracy with
-the true rotation from initial_translation; edge cases (empty mask, a start off screen, batch composition, no host
-synchronisation); and eval_bop with t_est."""
+"""GPU: the translation fit (DESIGN.md section 18).  nope_fit_translation_occluded without occluders against the numpy
+oracle bit for bit on the same render_depth images after 0 ... 6 updates; the silhouette counts against render_depth's
+coverage; accuracy with the true rotation from initial_translation; edge cases (empty mask, a start off screen, batch
+composition, no host synchronisation); and eval_bop with t_est."""
 import math
 import os
 
@@ -88,7 +88,7 @@ def test_kernel_equals_oracle(name, P):
 
 
 def test_workspace_holds_the_final_render():
-    """nope_fit_translation leaves render_depth's image at the returned t in its workspace"""
+    """nope_fit_translation_occluded leaves render_depth's image at the returned t in its workspace"""
     from nope_b200 import _lib
     from nope_b200.translation import initial_translation
     from nope_b200.vsd import _stream
@@ -100,10 +100,10 @@ def test_workspace_holds_the_final_render():
     depth = torch.empty((6, H, W), device="cuda")
     t = torch.empty((2, 3, 3), device="cuda", dtype=torch.float64)
     iou = torch.empty((2, 3), device="cuda", dtype=torch.float64)
-    _lib.check(_lib.load().nope_fit_translation(
+    _lib.check(_lib.load().nope_fit_translation_occluded(
         _lib.ptr(mesh.vertices), mesh.vertices.shape[0], _lib.ptr(mesh.faces), mesh.num_faces, _lib.ptr(Rd),
-        _lib.ptr(t0), _lib.ptr(masks), K.ctypes.data, 2, 3, H, W, 0.05, 3, _lib.ptr(depth), _lib.ptr(t), _lib.ptr(iou),
-        None, _stream(torch.device("cuda"))))
+        _lib.ptr(t0), _lib.ptr(masks), None, K.ctypes.data, 2, 3, H, W, 0.05, 3, _lib.ptr(depth), _lib.ptr(t),
+        _lib.ptr(iou), None, _stream(torch.device("cuda"))))
     th = t.cpu().numpy()
     for f in range(2):
         for p in range(3):

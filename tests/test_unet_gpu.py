@@ -294,25 +294,23 @@ def test_bad_arguments_raise(gpu_model):
     with pytest.raises(NopeError):
         gpu_model.u_net.sweep(rf, torch.zeros(1, 3, 6), query_feat=rf, k=5)   # k > N
     # on an engine before finalize, where every option it has is accepted: convolutions other than the
-    # clustered kernel and the fuse_gn option do not exist
-    import ctypes as C
+    # clustered kernel, the fuse_gn option and the implementation switches do not exist
     from nope_b200 import _lib
     from nope_b200.encoder import FeatureExtractor
     from nope_b200.unet import UNet
     fresh = UNet(u_net_dim=192, rot_representation_dim=6, encoder=FeatureExtractor(descriptor_size=8),
                  device="cuda:0")
-    h = fresh._handle()
     for impl in ("tcgen05", "simt"):
         with pytest.raises(NopeError):
             fresh.set_conv_impl(impl)
-    with pytest.raises(NopeError):
-        _lib.check(_lib.load().nope_unet_set_conv_impl(h, 0))
-    with pytest.raises(NopeError):
-        fresh.set_option("fuse_gn", 0)
+    for name, value in (("fuse_gn", 0), ("conv_impl", 2), ("attn_impl", 1)):
+        with pytest.raises(NopeError):
+            fresh.set_option(name, value)
     fresh.set_conv_impl("tcgen05_2cta")
-    v = C.c_int()
-    _lib.check(_lib.load().nope_unet_get_option(h, b"conv_impl", C.byref(v)))
-    assert v.value == 2
+    lib = _lib.load()
+    for name in ("nope_unet_set_conv_impl", "nope_unet_get_option", "nope_unet_sweep", "nope_score_topk",
+                 "nope_fit_translation", "nope_refine_contour"):
+        assert not hasattr(lib, name), name
 
 
 def test_full_size_grid_properties(gpu_model):

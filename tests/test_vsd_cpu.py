@@ -161,7 +161,7 @@ def test_header_declares_and_lib_binds_the_new_calls():
     lib = _lib.load()
     for n in ("nope_render_depth", "nope_vsd_error"):
         assert n in _declared() and n in _lib.SIGNATURES and hasattr(lib, n)
-    assert lib.nope_abi_version() == 2
+    assert lib.nope_abi_version() == 3
 
 
 P = C.c_void_p(256)

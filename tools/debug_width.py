@@ -11,13 +11,11 @@ from nope_b200.encoder import FeatureExtractor
 from nope_b200.unet import UNet
 
 dim = int(sys.argv[1]) if len(sys.argv) > 1 else 64
-impl = sys.argv[2] if len(sys.argv) > 2 else "tcgen05_2cta"
-names = sys.argv[3].split(",") if len(sys.argv) > 3 else None
+names = sys.argv[2].split(",") if len(sys.argv) > 2 else None
 sd = weights.make_unet_state_dict(seed=3, u_net_dim=dim)
 unet = UNet(u_net_dim=dim, rot_representation_dim=6, encoder=FeatureExtractor(descriptor_size=8),
             pose_mlp_name="single_layer", device="cuda:0")
 unet.load_state_dict(sd)
-unet.set_conv_impl(impl)
 g = torch.Generator().manual_seed(dim)
 rf = torch.randn(1, 8, 32, 32, generator=g) * 1.5
 poses = torch.randn(3, 6, generator=g)
@@ -29,4 +27,4 @@ for name in names or ["init_conv", "downs.0.0", "downs.0.1", "downs.0.2", "downs
                       "ups.1.3", "ups.2.3", "ups.3.3", "final_res_block", "final_conv.0"]:
     got = unet.debug_tap(rf, poses, name).cpu()
     ref = taps[name]
-    print(f"{impl} dim={dim} {name:18s} rel_l2 {float((got - ref).norm() / ref.norm()):.3e}", flush=True)
+    print(f"dim={dim} {name:18s} rel_l2 {float((got - ref).norm() / ref.norm()):.3e}", flush=True)

@@ -10,12 +10,10 @@ from nope_b200.ldm import UNetModelPose
 from nope_b200.synth_weights import make_ldm_state_dict
 
 N = int(sys.argv[1]) if len(sys.argv) > 1 else 128
-attn = sys.argv[2] if len(sys.argv) > 2 else "tcgen05"
 m = UNetModelPose(device="cuda:0", chunk=N)
 t0 = time.time()
 m.load_state_dict(make_ldm_state_dict(seed=0))
 print(f"load {time.time() - t0:.1f}s", flush=True)
-m.set_impl(attn=attn)
 g = torch.Generator().manual_seed(0)
 ref = torch.randn(1, 4, 32, 32, generator=g).cuda()
 qry = torch.randn(1, 4, 32, 32, generator=g).cuda()
@@ -36,5 +34,5 @@ if os.environ.get("NOPE_PROFILE"):
     torch.cuda.synchronize()
     torch.cuda.profiler.stop()
 ms = e0.elapsed_time(e1) / reps
-print(f"LDM sweep N={N} attn={attn}: {ms:.2f} ms/sweep, {N / ms * 1e3:.0f} hyp/s, "
+print(f"LDM sweep N={N}: {ms:.2f} ms/sweep, {N / ms * 1e3:.0f} hyp/s, "
       f"{m.last_launch_count} launches, mem {torch.cuda.max_memory_allocated() / 2**30:.1f} GiB torch", flush=True)

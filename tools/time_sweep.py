@@ -1,8 +1,8 @@
 """Time the resident sweep (latents + poses in HBM, CUDA events on the current stream) for one or
-several engine configurations in ONE process, e.g.
-    python tools/time_sweep.py fp16 fp16:attn_impl=1 parity fp16_w2 --poses 642 --queries 1
-Each spec is precision[:option=value,...].  Prints one JSON line per spec (hyp/s, ms, parity vs the
-first spec's scores) -- a development aid, not the bench."""
+several engine precisions in ONE process, e.g.
+    python tools/time_sweep.py fp16 parity fp16_w2 --poses 642 --queries 1
+Prints one JSON line per precision (hyp/s, ms, parity vs the first one's scores) -- a development aid,
+not the bench."""
 import argparse
 import json
 import os
@@ -16,7 +16,7 @@ from nope_b200.model import build_model
 from nope_b200.poses import synthetic_pose_batch
 
 ap = argparse.ArgumentParser()
-ap.add_argument("specs", nargs="+")
+ap.add_argument("precisions", nargs="+")
 ap.add_argument("--poses", type=int, default=642)
 ap.add_argument("--queries", type=int, default=1)
 ap.add_argument("--chunk", type=int, default=642)
@@ -31,14 +31,8 @@ rf = (torch.randn(args.queries, 8, 32, 32, generator=g) * 1.5).cuda()
 qf = (torch.randn(args.queries, 8, 32, 32, generator=g) * 1.5).cuda()
 poses = poses.cuda()
 base = None
-for spec in args.specs:
-    prec, _, opts = spec.partition(":")
+for prec in args.precisions:
     model = build_model(device="cuda:0", chunk=args.chunk, precision=prec)
-    for kv in filter(None, opts.split(",")):
-        k, v = kv.split("=")
-        if k == "conv_impl":
-            continue
-        model.u_net.set_option(k, int(v))
     model.load_state_dict(sd)
     u = model.u_net
     run = lambda: u.sweep(rf, poses, query_feat=qf, want_emb=False, k=5)
@@ -52,7 +46,7 @@ for spec in args.specs:
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / args.steps
-    line = {"spec": spec, "ms": ms, "hyp_per_s": args.queries * args.poses / (ms * 1e-3),
+    line = {"precision": prec, "ms": ms, "hyp_per_s": args.queries * args.poses / (ms * 1e-3),
             "launches": u.last_launch_count, "top5": out["topi"][0].tolist(),
             "sim_crc": __import__("zlib").crc32(out["sim"].float().cpu().numpy().tobytes())}
     if base is None:
