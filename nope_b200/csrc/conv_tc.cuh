@@ -532,6 +532,14 @@ inline int make_weight_map(CUtensorMap* m, const void* base, int n_total, int k_
   uint32_t box[2] = {64, (uint32_t)bn};
   return make_tmap_f16(m, base, 2, dims, str, box);
 }
+// 3-D fp16 tensor map with 128-byte swizzle (the LDM attention's operands).
+inline int make_tmap3_f16(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d1, uint64_t d2,
+                          uint32_t b0, uint32_t b1) {
+  uint64_t dims[3] = {d0, d1, d2};
+  uint64_t str[2] = {d0 * 2, d0 * d1 * 2};
+  uint32_t box[3] = {b0, b1, 1};
+  return make_tmap_f16(m, base, 3, dims, str, box);
+}
 
 inline int pick_bn(int n_total) {
   if (n_total % 192 == 0) return 192;
@@ -546,7 +554,8 @@ inline bool conv_needs_extras(const ConvParams& p) {
 
 // Tensor maps of activation buffers, encoded once per (base, image capacity, lattice, C, H, W).  lattice < 0: the
 // plain NHWC map of geometry g (make_act_map); 0..3: the stride-2 sub-lattice (lattice >> 1, lattice & 1) of a
-// 2H x 2W tensor seen from g (make_unshuffle_map).  Call clear() whenever the buffers are reallocated.
+// 2H x 2W tensor seen from g (make_unshuffle_map).  get3: the 3-D maps of make_tmap3_f16, once per (base, dims).
+// Call clear() whenever the buffers are reallocated.
 class TmapCache {
  public:
   int get(const CUtensorMap** out, const void* base, int cap_img, int C, const TileGeom& g, int lattice) {
@@ -562,10 +571,22 @@ class TmapCache {
     *out = &it->second;
     return 0;
   }
-  void clear() { maps_.clear(); }
+  int get3(const CUtensorMap** out, const void* base, int d0, int d1, int d2, int b0, int b1) {
+    const auto key = std::make_tuple(base, d0, d1, d2);
+    auto it = maps3_.find(key);
+    if (it == maps3_.end()) {
+      CUtensorMap m;
+      if (make_tmap3_f16(&m, base, d0, d1, d2, b0, b1)) return -1;
+      it = maps3_.emplace(key, m).first;
+    }
+    *out = &it->second;
+    return 0;
+  }
+  void clear() { maps_.clear(); maps3_.clear(); }
 
  private:
   std::map<std::tuple<const void*, int, int, int, int, int>, CUtensorMap> maps_;
+  std::map<std::tuple<const void*, int, int, int>, CUtensorMap> maps3_;
 };
 
 // What a convolution layer of every engine holds.  K is the engine's GEMM depth (its weight layout decides whether

@@ -191,10 +191,10 @@ struct nope_encoder {
   std::map<std::string, nope::EncConv> convs;
   float *stem_w = nullptr, *stem_b = nullptr;
   nope::DeviceAllocs mem;             // weights, rot_stage
-  int cap = 0;
+  int cap = 0;                        // images the workspace holds
   nope::ActPair buf[5];
   float* proj_out = nullptr;
-  nope::DeviceAllocs ws_mem;          // workspace for cap images (ensure_workspace)
+  nope::WorkspaceSlab ws;
   nope::TmapCache tmaps;
   int64_t launches = 0;
   static constexpr int kChunk = 32;   // images per encode() call: the workspace holds this many
@@ -298,17 +298,16 @@ struct nope_encoder {
   }
 
   // ---------------------------------------------------------------- workspace
-  int ensure_workspace(int B) {
-    if (B <= cap) return 0;
-    NOPE_CUDA(cudaDeviceSynchronize());
-    ws_mem.release();
-    tmaps.clear();
-    cap = B;
-    const size_t n = (size_t)cap * 128 * 128 * 256;     // largest activation: layer1 output
-    for (auto& b : buf)
-      if (ws_mem.alloc(&b.hi, n) || (precision == 0 && ws_mem.alloc(&b.lo, n))) return -1;
-    return ws_mem.alloc(&proj_out, (size_t)cap * 1024 * 64);
+  size_t layout(nope::Bump& b, int c) {
+    const size_t n = (size_t)c * 128 * 128 * 256;     // largest activation: layer1 output
+    for (auto& a : buf) {
+      b.take(&a.hi, n);
+      if (precision == 0) b.take(&a.lo, n);
+    }
+    b.take(&proj_out, (size_t)c * 1024 * 64);
+    return b.off;
   }
+  int ensure_workspace(int B) { return B <= cap ? 0 : nope::grow_workspace(this, std::tie(cap), nullptr, B); }
 
   // out = [relu](conv(in) + bias [+ res]); Hin = input side; returns output side in *Hout
   int conv(const nope::EncConv& L, const nope::ActPair& in, int Hin, const nope::ActPair& out, int n_img,

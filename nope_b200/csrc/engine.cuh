@@ -10,8 +10,8 @@
 //
 // A sweep engine (engine_sweep, engine_debug_tap) also provides `int chunk`, `int64_t launches`, `DebugTap dtap`,
 // `float* score_partial` and `float* sim_buf`, and
-//   int ensure_workspace(int hyps, int refs, int scores, cudaStream_t)  sizes the workspace (and the score partials
-//       and similarity scratch of `scores` (reference, query, pose) triples) before a launch on the stream;
+//   int ensure_workspace(int hyps, int refs, int scores, cudaStream_t)  sizes the workspace (grow_workspace), score
+//       partials and similarity scratch of `scores` (reference, query, pose) triples included, before a launch;
 //   int prestage(const float* ref, int B, cudaStream_t)                  the pose-independent prefix per reference;
 //   int forward_chunk(poses, hyp0, n, N, query, out_emb, score_part, cudaStream_t, int Q);
 //   int rank(part, sim, B, N, Q, k, topv, topi, idx_base, cudaStream_t) the similarities and top-k from the partials.
@@ -21,6 +21,7 @@
 #include <algorithm>
 #include <map>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "common.cuh"
@@ -78,7 +79,7 @@ class StagedWeights {
   std::map<std::string, HostTensor> host_;
 };
 
-// Device allocations owned by an engine, freed by release() or with the owner.
+// Device allocations owned by an engine or a call, freed by release() or with the owner.
 class DeviceAllocs {
  public:
   DeviceAllocs() = default;
@@ -86,13 +87,14 @@ class DeviceAllocs {
   DeviceAllocs& operator=(const DeviceAllocs&) = delete;
   ~DeviceAllocs() { release(); }
 
+  // n elements; n == 0 still gets a distinct pointer
   template <typename T> int alloc(T** out, size_t n) {
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(out), n * sizeof(T)));
+    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(out), std::max<size_t>(n, 1) * sizeof(T)));
     ptrs_.push_back(*out);
     return 0;
   }
   template <typename T> int upload(T** out, const T* src, size_t n) {
-    if (alloc(out, std::max<size_t>(n, 1))) return -1;
+    if (alloc(out, n)) return -1;
     NOPE_CUDA(cudaMemcpy(*out, src, n * sizeof(T), cudaMemcpyHostToDevice));
     return 0;
   }
@@ -105,6 +107,66 @@ class DeviceAllocs {
  private:
   std::vector<void*> ptrs_;
 };
+
+// bump allocator over one device slab (base == nullptr: size computation only)
+struct Bump {
+  uint8_t* base = nullptr;
+  size_t off = 0;
+  template <typename T> void take(T** out, size_t n) {
+    off = (off + 255) & ~static_cast<size_t>(255);
+    if (base) *out = reinterpret_cast<T*>(base + off);     // size-only passes leave the engine untouched
+    off += n * sizeof(T);
+  }
+};
+
+// The slab a sweep or image engine's workspace lives in: owned and freed with the engine, or a caller's buffer
+// (`external`, nope_unet_set_workspace) that the engine never frees.
+struct WorkspaceSlab {
+  uint8_t* base = nullptr;
+  bool external = false;
+  WorkspaceSlab() = default;
+  WorkspaceSlab(const WorkspaceSlab&) = delete;
+  WorkspaceSlab& operator=(const WorkspaceSlab&) = delete;
+  ~WorkspaceSlab() { release(); }
+  void release() {
+    if (base && !external) cudaFree(base);
+    base = nullptr;
+    external = false;
+  }
+};
+
+// Moves the workspace of engine e to a new slab for the capacities c...  The engine provides `WorkspaceSlab ws`,
+// `TmapCache tmaps` and `size_t layout(Bump&, c...)`, which places every workspace buffer and returns the bytes they
+// span.  In order: a size pass; a device synchronisation, since launches may still use the old slab; the old slab
+// released and the tensor maps keyed by its pointers dropped; the new slab, `external` (a caller's buffer of at least
+// the size pass's bytes + 256) or one cudaMalloc; the assign pass; the capacity fields `caps` set to c...  After a
+// failure they are 0 and the slab is null, so the next call grows again instead of running on freed buffers, and the
+// runtime's last error is cleared so that later calls do not report it.
+template <typename E, typename... C>
+int grow_workspace(E* e, std::tuple<C&...> caps, void* external, C... c) {
+  caps = std::tuple<C...>();
+  Bump size;
+  const size_t bytes = e->layout(size, c...);
+  cudaError_t err = cudaDeviceSynchronize();
+  e->ws.release();
+  e->tmaps.clear();
+  if (err == cudaSuccess && !external) err = cudaMalloc(reinterpret_cast<void**>(&e->ws.base), bytes);
+  if (err != cudaSuccess) {
+    e->ws.base = nullptr;
+    cudaGetLastError();
+    return fail(std::string(E::kName) + ": workspace of " + std::to_string(bytes) + " bytes: " +
+                cudaGetErrorString(err));
+  }
+  if (external) {
+    e->ws.base = static_cast<uint8_t*>(external);
+    e->ws.external = true;
+  }
+  Bump b;
+  b.base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(e->ws.base) + 255) & ~static_cast<uintptr_t>(255));
+  e->layout(b, c...);
+  caps = std::tuple<C...>(c...);
+  return 0;
+}
 
 // The check of every *_create: `device` exists and is an sm_90 part; its SM count goes to *num_sms.
 inline int open_device(int device, int* num_sms) {

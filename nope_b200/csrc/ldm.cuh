@@ -82,9 +82,9 @@ struct nope_ldm {
   float *in_w = nullptr, *in_b = nullptr;
   nope::DeviceAllocs mem;                      // weights
 
-  // workspace (per chunk of `cap` hypotheses; `cap_ref` reference latents)
-  int cap = 0, cap_ref = 0;
-  std::vector<__half*> HS;                     // skip stack, one buffer per input block
+  // workspace (per chunk of `cap` hypotheses; `cap_ref` reference latents; `scores_cap` scored triples)
+  int cap = 0, cap_ref = 0, scores_cap = 0;
+  std::vector<__half*> HS;                     // skip stack, one buffer per input block (sized by build_plan)
   __half *XA = nullptr, *XB = nullptr, *XC = nullptr, *R = nullptr, *T1 = nullptr, *T2 = nullptr,
          *T3 = nullptr, *XN = nullptr, *PI = nullptr, *PJ = nullptr, *QKV = nullptr,
          *Vt = nullptr, *AO = nullptr, *GG = nullptr, *x0ref = nullptr, *Rref = nullptr, *Pref = nullptr;
@@ -93,21 +93,13 @@ struct nope_ldm {
   float* OF = nullptr;                          // out[2] result, fp32 [cap * S0 * S0][64]
   int* ref_of = nullptr;
   float* score_partial = nullptr;
-  size_t score_partial_cap = 0;
   float* sim_buf = nullptr;
-  size_t sim_buf_cap = 0;
-  nope::DeviceAllocs ws_mem;                   // workspace for cap hypotheses, cap_ref references (ensure_workspace)
+  nope::WorkspaceSlab ws;
   nope::TmapCache tmaps;
-  std::map<std::tuple<const void*, int, int, int>, CUtensorMap> tmaps3;
 
   // per-launch profile: record kind 0 = convolution / GEMM, 1 = attention
   nope::LaunchProfile prof;
   nope::DebugTap dtap;
-
-  ~nope_ldm() {
-    if (score_partial) cudaFree(score_partial);
-    if (sim_buf) cudaFree(sim_buf);
-  }
 
   // ------------------------------------------------------------------ plan + schema
   void build_plan() {
@@ -130,6 +122,7 @@ struct nope_ldm {
       }
     }
     mid_ch = ch;
+    HS.assign(inp.size(), nullptr);
     for (int level = (int)mult.size() - 1; level >= 0; --level)
       for (int i = 0; i <= nres; ++i) {
         const int ich = chans.back();
@@ -473,56 +466,41 @@ struct nope_ldm {
   }
 
   // ------------------------------------------------------------------ workspace
-  // Sizes the workspace for `need_cap` hypotheses and `need_ref` references, and the score partials and similarity
-  // scratch for `need_scores` (reference, query, pose) triples.  Each grows on demand only (a host synchronisation and
-  // cudaMalloc then).
-  int ensure_workspace(int need_cap, int need_ref, int need_scores, cudaStream_t st) {
-    const size_t scored = (size_t)need_scores, part = scored * nslab();
-    if (part > score_partial_cap) {
-      NOPE_CUDA(cudaStreamSynchronize(st));
-      if (score_partial) cudaFree(score_partial);
-      score_partial = nullptr;
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&score_partial), part * sizeof(float)));
-      score_partial_cap = part;
-    }
-    if (scored > sim_buf_cap) {
-      NOPE_CUDA(cudaStreamSynchronize(st));
-      if (sim_buf) cudaFree(sim_buf);
-      sim_buf = nullptr;
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&sim_buf), scored * sizeof(float)));
-      sim_buf_cap = scored;
-    }
-    if (need_cap <= cap && need_ref <= cap_ref) return 0;
-    NOPE_CUDA(cudaDeviceSynchronize());
-    ws_mem.release();
-    tmaps.clear();
-    tmaps3.clear();
-    cap = std::max(cap, need_cap);
-    cap_ref = std::max(cap_ref, need_ref);
-    const size_t c = (size_t)cap;
+  // layout(b) places every buffer for capacities (c hypotheses, r references, n_scores (reference, query, pose)
+  // triples of score partials and similarity scratch)
+  size_t layout(nope::Bump& b, int c_hyp, int c_ref, int n_scores) {
+    const size_t c = (size_t)c_hyp, r = (size_t)c_ref;
     const size_t u = (size_t)S0 * S0 * mc;        // one full-resolution base-width map
-    HS.assign(inp.size(), nullptr);
-    {
-      int S = S0;
-      for (size_t i = 0; i < inp.size(); ++i) {
-        if (inp[i].kind == 2) S /= 2;
-        if (ws_mem.alloc(&HS[i], c * S * S * inp[i].cout)) return -1;
-      }
+    int S = S0;
+    for (size_t i = 0; i < inp.size(); ++i) {
+      if (inp[i].kind == 2) S /= 2;
+      b.take(&HS[i], c * S * S * inp[i].cout);
     }
     // widest tensors: block outputs <= 2u (512 ch at 32^2 after the last upsample), ResBlock
     // inputs <= 3u (768 ch at 32^2), q|k|v 3u, V^T 1u, GEGLU output 4u
-    if (ws_mem.alloc(&XA, c * 2 * u) || ws_mem.alloc(&XB, c * 2 * u) || ws_mem.alloc(&XC, c * 2 * u) ||
-        ws_mem.alloc(&R, c * u) || ws_mem.alloc(&T1, c * 3 * u) || ws_mem.alloc(&T2, c * u) ||
-        ws_mem.alloc(&T3, c * u) || ws_mem.alloc(&XN, c * u) || ws_mem.alloc(&PI, c * u) || ws_mem.alloc(&PJ, c * u) ||
-        ws_mem.alloc(&QKV, c * 3 * u) || ws_mem.alloc(&Vt, c * u) || ws_mem.alloc(&AO, c * u) ||
-        ws_mem.alloc(&GG, c * 4 * u) || ws_mem.alloc(&x0ref, (size_t)cap_ref * u) ||
-        ws_mem.alloc(&Rref, (size_t)cap_ref * u) || ws_mem.alloc(&Pref, (size_t)cap_ref * u))
-      return -1;
+    for (__half** t : {&XA, &XB, &XC}) b.take(t, c * 2 * u);
+    b.take(&R, c * u);
+    b.take(&T1, c * 3 * u);
+    for (__half** t : {&T2, &T3, &XN, &PI, &PJ}) b.take(t, c * u);
+    b.take(&QKV, c * 3 * u);
+    for (__half** t : {&Vt, &AO}) b.take(t, c * u);
+    b.take(&GG, c * 4 * u);
+    for (__half** t : {&x0ref, &Rref, &Pref}) b.take(t, r * u);
     const size_t sts = (size_t)32 * 256;   // parts (<= 32) x octets (<= 256) per image
-    if (ws_mem.alloc(&S_in, c * sts) || ws_mem.alloc(&S_mid, c * sts) || ws_mem.alloc(&S_out, c * sts)) return -1;
-    if (ws_mem.alloc(&cb, c * (size_t)cb_width) || ws_mem.alloc(&ref_of, c) || ws_mem.alloc(&OF, c * S0 * S0 * 64))
-      return -1;
-    return 0;
+    for (float2** t : {&S_in, &S_mid, &S_out}) b.take(t, c * sts);
+    b.take(&cb, c * (size_t)cb_width);
+    b.take(&ref_of, c);
+    b.take(&OF, c * S0 * S0 * 64);
+    b.take(&score_partial, (size_t)n_scores * nslab());
+    b.take(&sim_buf, (size_t)n_scores);
+    return b.off;
+  }
+  // Sizes the workspace for `need_cap` hypotheses, `need_ref` references and `need_scores` scored triples.  It grows
+  // on demand only (a device synchronisation and cudaMalloc then).
+  int ensure_workspace(int need_cap, int need_ref, int need_scores, cudaStream_t) {
+    if (need_cap <= cap && need_ref <= cap_ref && need_scores <= scores_cap) return 0;
+    return nope::grow_workspace(this, std::tie(cap, cap_ref, scores_cap), nullptr, std::max(cap, need_cap),
+                                std::max(cap_ref, need_ref), std::max(scores_cap, need_scores));
   }
 
   // ------------------------------------------------------------------ op launchers
@@ -622,23 +600,12 @@ struct nope_ldm {
     ++launches;
     return 0;
   }
-  int get_map3(const CUtensorMap** out, const void* base, int d0, int d1, int d2, int b0, int b1) {
-    auto key = std::make_tuple(base, d0, d1, d2);
-    auto it = tmaps3.find(key);
-    if (it == tmaps3.end()) {
-      CUtensorMap m;
-      if (nope::make_tmap3_f16(&m, base, d0, d1, d2, b0, b1)) return -1;
-      it = tmaps3.emplace(key, m).first;
-    }
-    *out = &it->second;
-    return 0;
-  }
-  // self-attention core on qkv [n, ntok, 3C] -> out [n, ntok, C]
-  int attention(const __half* qkv, __half* out, int C, int ntok, int n, cudaStream_t st) {
+  // self-attention core on qkv [n, ntok, 3C] -> out [n, ntok, C]; vt [n, ntok, C] holds V^T
+  int attention(const __half* qkv, __half* vt, __half* out, int C, int ntok, int n, cudaStream_t st) {
     using namespace nope;
     const int Hh = C / 32;
     NOPE_CHECK(ntok % 64 == 0 && C % 64 == 0, "attention: tokens and channels must be multiples of 64");
-    ldm_attn_prep_kernel<<<dim3(ntok / 64, n), 256, 0, st>>>(qkv, Vt, ntok, C);
+    ldm_attn_prep_kernel<<<dim3(ntok / 64, n), 256, 0, st>>>(qkv, vt, ntok, C);
     NOPE_CUDA(cudaGetLastError());
     const float sl2e = 0.17677669529663687f * 1.4426950408889634f;   // 32^-1/2 * log2(e)
     const dim3 grid((unsigned)(n * Hh) * (unsigned)((ntok + 127) / 128));
@@ -653,9 +620,9 @@ struct nope_ldm {
     }
     AttnParams p;
     const CUtensorMap* m = nullptr;
-    if (get_map3(&m, qkv, 3 * C, ntok, n, 64, 128)) return -1;
+    if (tmaps.get3(&m, qkv, 3 * C, ntok, n, 64, 128)) return -1;
     p.qkmap = *m;
-    if (get_map3(&m, Vt, ntok, 32, n * Hh, 64, 32)) return -1;
+    if (tmaps.get3(&m, vt, ntok, 32, n * Hh, 64, 32)) return -1;
     p.vmap = *m;
     p.out = out; p.n = ntok; p.H = Hh; p.C = C; p.scale_log2e = sl2e;
     ldm_attn_tc_kernel<<<grid, 128, kAttnSmem, st>>>(p);
@@ -692,7 +659,7 @@ struct nope_ldm {
     if (conv(convs.at(p + ".proj_in"), XN, PI, S, n, st)) return -1;
     if (ln(norms.at(p + ".ln1"), PI, nullptr, nullptr, XN, C, S, n, st)) return -1;
     if (conv(convs.at(p + ".qkv"), XN, QKV, S, n, st)) return -1;
-    if (attention(QKV, AO, C, S * S, n, st)) return -1;
+    if (attention(QKV, Vt, AO, C, S * S, n, st)) return -1;
     return conv(convs.at(p + ".to_out"), AO, xs, S, n, st, nullptr, PI, C);
   }
   // st_post: x = attn2(norm2(x), context) + x -- the one-token cross-attention is the

@@ -42,19 +42,10 @@ namespace {
 
 constexpr int kAbiVersion = 3;
 
-struct Scratch {
-  std::vector<void*> p;
-  ~Scratch() { for (void* q : p) cudaFree(q); }
-  template <typename T> int get(T** out, size_t n) {
-    NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(out), std::max<size_t>(n, 1) * sizeof(T)));
-    p.push_back(*out);
-    return 0;
-  }
-};
-int to_nhwc(const float* x, __half** out, Scratch& s, int n, int C, int hw, cudaStream_t st,
+int to_nhwc(const float* x, __half** out, DeviceAllocs& s, int n, int C, int hw, cudaStream_t st,
             __half** out_lo = nullptr) {
-  if (s.get(out, (size_t)n * C * hw)) return -1;
-  if (out_lo && s.get(out_lo, (size_t)n * C * hw)) return -1;
+  if (s.alloc(out, (size_t)n * C * hw)) return -1;
+  if (out_lo && s.alloc(out_lo, (size_t)n * C * hw)) return -1;
   nchw_f32_to_nhwc_f16_kernel<<<ew_grid((long long)n * C * hw), 256, 0, st>>>(x, *out, n, C, hw,
                                                                               out_lo ? *out_lo : nullptr);
   NOPE_CUDA(cudaGetLastError());
@@ -1094,7 +1085,7 @@ namespace {
 // fp16 remainders at precision 2), the output buffer, the packed layer, and a UNet engine on the current device to
 // launch through.
 struct OpConv {
-  Scratch s;
+  DeviceAllocs s;
   nope_unet eng;
   ConvLayer L;
   Act in0, in1, out;
@@ -1113,7 +1104,7 @@ struct OpConv {
     if (x1 && to_nhwc(x1, &a1, s, n_img, C1, Hin * Hin, st, sp ? &a1l : nullptr)) return -1;
     in0 = Act(a0, C0, a0l);
     if (x1) in1 = Act(a1, C1, a1l);
-    if (s.get(&o, (size_t)n_img * H * W * Cout) || (sp && s.get(&ol, (size_t)n_img * H * W * Cout))) return -1;
+    if (s.alloc(&o, (size_t)n_img * H * W * Cout) || (sp && s.alloc(&ol, (size_t)n_img * H * W * Cout))) return -1;
     out = Act(o, Cout, ol);
     L.mode = mode;
     L.cin = C0 + (x1 ? C1 : 0);
@@ -1123,7 +1114,7 @@ struct OpConv {
     L.bn = pick_bn(Cout);
     L.bias = const_cast<float*>(bias);
     const int rows = mode == 3 ? 4 * Cout : Cout;
-    if (s.get(&L.w, (size_t)rows * L.Kp)) return -1;
+    if (s.alloc(&L.w, (size_t)rows * L.Kp)) return -1;
     if (pack_conv_weight(weight, L.w, Cout, L.cin, taps, mode == 3, L.Kp, 0, precision >= 1 ? L.K : 0, 0, st))
       return -1;
     if (make_weight_map(&L.wmap, L.w, rows, L.Kp, L.bn)) return -1;
@@ -1157,7 +1148,7 @@ int nope_op_conv_gn(int mode, const float* x0, int C0, const float* x1, int C1, 
   OpConv op;
   if (op.setup(mode, 2, 0, x0, C0, x1, C1, weight, bias, n_img, H, W, Cout, st)) return -1;
   float2* stats = nullptr;
-  if (op.s.get(&stats, (size_t)n_img * parts * noct)) return -1;
+  if (op.s.alloc(&stats, (size_t)n_img * parts * noct)) return -1;
   if (op.eng.conv(op.L, op.in0, op.in1, op.out, H, n_img, n_img, st, nullptr, stats)) return -1;
   // GroupNorm on the host, in double, from the epilogue's [img][parts][octet] partial sums alone: a group's sum and
   // sum of squares are the totals of its octets over all parts (the layout the LDM engine normalises from)
@@ -1227,7 +1218,7 @@ int nope_op_conv_gn_fused(int mode, int precision, const float* x0, int C0, cons
   float2* em = nullptr;
   const int eparts = nope_unet::fused_emit_parts(H, Cout);
   if (emit_out) {
-    if (op.s.get(&em, (size_t)n_img * eparts)) return -1;
+    if (op.s.alloc(&em, (size_t)n_img * eparts)) return -1;
     gs.emit = em;
   }
   if (op.eng.conv(op.L, op.in0, op.in1, op.out, H, n_img, n_img, st, &gs)) return -1;
@@ -1253,9 +1244,9 @@ int nope_op_linear_attention(int impl, const float* qkv, float* out, int n_img, 
   NOPE_CHECK(qkv && out, "null argument");
   NOPE_CHECK(impl == 1 || (impl == 0 && (H * W) % kBM == 0), "impl 0 (tensor cores) needs H*W % 128 == 0; impl 1 = CUDA cores");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  Scratch s;
+  DeviceAllocs s;
   __half *a = nullptr, *o = nullptr;
-  if (to_nhwc(qkv, &a, s, n_img, 384, H * W, st) || s.get(&o, (size_t)n_img * 128 * H * W)) return -1;
+  if (to_nhwc(qkv, &a, s, n_img, 384, H * W, st) || s.alloc(&o, (size_t)n_img * 128 * H * W)) return -1;
   if (impl == 0) {
     cudaDeviceProp prop;
     int dev = 0;
@@ -1274,9 +1265,9 @@ int nope_op_linear_attention(int impl, const float* qkv, float* out, int n_img, 
 int nope_op_attention(const float* qkv, float* out, int n_img, int H, int W, void* stream) {
   NOPE_CHECK(qkv && out && H * W <= 32, "bad argument (H*W must be <= 32)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  Scratch s;
+  DeviceAllocs s;
   __half *a = nullptr, *o = nullptr;
-  if (to_nhwc(qkv, &a, s, n_img, 384, H * W, st) || s.get(&o, (size_t)n_img * 128 * H * W)) return -1;
+  if (to_nhwc(qkv, &a, s, n_img, 384, H * W, st) || s.alloc(&o, (size_t)n_img * 128 * H * W)) return -1;
   midattn_kernel<<<n_img, 128, 0, st>>>(a, o, H * W);
   NOPE_CUDA(cudaGetLastError());
   if (to_nchw(o, out, n_img, 128, H * W, st)) return -1;
@@ -1287,9 +1278,9 @@ int nope_op_attention(const float* qkv, float* out, int n_img, int H, int W, voi
 int nope_op_upsample2x(const float* x, float* out, int n_img, int C, int H, int W, void* stream) {
   NOPE_CHECK(x && out && C % 8 == 0 && H == W, "bad argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  Scratch s;
+  DeviceAllocs s;
   __half *a = nullptr, *o = nullptr;
-  if (to_nhwc(x, &a, s, n_img, C, H * W, st) || s.get(&o, (size_t)n_img * C * H * W * 4)) return -1;
+  if (to_nhwc(x, &a, s, n_img, C, H * W, st) || s.alloc(&o, (size_t)n_img * C * H * W * 4)) return -1;
   upsample2x_kernel<<<ew_grid((long long)n_img * 4 * H * W * C / 8), 256, 0, st>>>(a, o, n_img, H, W, C);
   NOPE_CUDA(cudaGetLastError());
   if (to_nchw(o, out, n_img, C, 4 * H * W, st)) return -1;
@@ -1425,14 +1416,15 @@ int nope_op_mh_attention(const float* qkv, float* out, int n_img, int n_tok, int
   NOPE_CHECK(qkv && out && n_img >= 1 && n_tok >= 64 && n_tok % 64 == 0 && C % 64 == 0 && C >= 64,
              "bad arguments (n_tok and C must be multiples of 64)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  nope_ldm e;    // only the attention staging buffers are used; freed by the destructor
+  DeviceAllocs s;
+  nope_ldm e;    // launches the attention on the staging buffers in s
   const size_t tok = (size_t)n_img * n_tok;
-  __half *q16 = nullptr, *o16 = nullptr;
-  if (e.ws_mem.alloc(&q16, tok * 3 * C) || e.ws_mem.alloc(&o16, tok * C) || e.ws_mem.alloc(&e.Vt, tok * C)) return -1;
+  __half *q16 = nullptr, *vt = nullptr, *o16 = nullptr;
+  if (s.alloc(&q16, tok * 3 * C) || s.alloc(&o16, tok * C) || s.alloc(&vt, tok * C)) return -1;
   // [n_img, n_tok, 3C] fp32 is already token-major: a plain fp32 -> fp16 cast ("NCHW" with hw = 1)
   nchw_f32_to_nhwc_f16_kernel<<<ew_grid((long long)tok * 3 * C), 256, 0, st>>>(qkv, q16, (int)tok, 3 * C, 1);
   NOPE_CUDA(cudaGetLastError());
-  if (e.attention(q16, o16, C, n_tok, n_img, st)) return -1;
+  if (e.attention(q16, vt, o16, C, n_tok, n_img, st)) return -1;
   nhwc_f16_to_nchw_f32_kernel<<<ew_grid((long long)tok * C), 256, 0, st>>>(o16, out, (int)tok, C, 1);
   NOPE_CUDA(cudaGetLastError());
   NOPE_CUDA(cudaStreamSynchronize(st));

@@ -59,17 +59,6 @@ struct GnSpec {
   int pre_parts = 0;
 };
 
-// bump allocator over one device slab (base == nullptr: size computation only)
-struct Bump {
-  uint8_t* base = nullptr;
-  size_t off = 0;
-  template <typename T> void take(T** out, size_t n) {
-    off = (off + 255) & ~static_cast<size_t>(255);
-    if (base) *out = reinterpret_cast<T*>(base + off);     // size-only passes leave the engine untouched
-    off += n * sizeof(T);
-  }
-};
-
 struct UNetEngine {
   static constexpr const char* kName = "UNet";
   int dim = 0, Cl = 0, S0 = 0, rot_dim = 6, cemb = 0, device = 0, num_sms = 132;
@@ -96,10 +85,8 @@ struct UNetEngine {
   DeviceAllocs mem;  // every weight buffer
 
   // workspace: one slab, either caller-provided (nope_unet_set_workspace) or owned
-  int cap = 0, cap_ref = 0;
-  uint8_t* ws_base = nullptr;
-  size_t ws_bytes = 0;
-  bool ws_external = false;
+  int cap = 0, cap_ref = 0, scores_cap = 0;
+  WorkspaceSlab ws;
   bool ws_fresh = false;            // counters not zeroed yet
   Act sk[4][2];
   Act TB, TC, TD, XA, XB, RB;
@@ -120,9 +107,6 @@ struct UNetEngine {
   LaunchProfile prof;
   DebugTap dtap;
 
-  ~UNetEngine() {
-    if (ws_base && !ws_external) cudaFree(ws_base);
-  }
   bool split() const { return precision == 2 || precision == 4; }
   // precision 4: the residual stream, skip tensors and resampled maps keep their (hi, lo) pair, the tensor INSIDE a
   // ResnetBlock (block1's output h, consumed only by block2's convolution) is a single fp16 value -- block2 runs two
@@ -416,21 +400,14 @@ struct UNetEngine {
     Bump b;
     return layout(b, c_hyp, c_ref, n_scores) + 256;
   }
-  int scores_cap = 0;
   // no allocation when the slab fits (always, with a caller-provided one); otherwise the engine grows its own slab
   // (device synchronisation + cudaMalloc on growth only)
   int ensure_workspace(int need_cap, int need_ref, int need_scores, cudaStream_t st) {
     if (need_cap > cap || need_ref > cap_ref || need_scores > scores_cap) {
-      NOPE_CHECK(!ws_external, "the caller-provided workspace is too small for this sweep "
+      NOPE_CHECK(!ws.external, "the caller-provided workspace is too small for this sweep "
                                "(nope_unet_workspace_bytes / nope_unet_set_workspace)");
-      NOPE_CUDA(cudaDeviceSynchronize());
-      if (ws_base) cudaFree(ws_base);
-      ws_base = nullptr;
-      const int c = std::max(cap, need_cap), r = std::max(cap_ref, need_ref), sc = std::max(scores_cap, need_scores);
-      const size_t bytes = workspace_bytes(c, r, sc);
-      NOPE_CUDA(cudaMalloc(reinterpret_cast<void**>(&ws_base), bytes));
-      ws_bytes = bytes;
-      if (adopt(c, r, sc)) return -1;
+      if (adopt(nullptr, std::max(cap, need_cap), std::max(cap_ref, need_ref), std::max(scores_cap, need_scores)))
+        return -1;
     }
     // the tile-sync words of a fresh slab carry epoch 0, which no launch uses
     if (ws_fresh) {
@@ -439,26 +416,16 @@ struct UNetEngine {
     }
     return 0;
   }
-  int adopt(int c, int r, int sc) {
-    tmaps.clear();
-    cap = c; cap_ref = r; scores_cap = sc;
-    Bump b;
-    b.base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws_base) + 255) & ~static_cast<uintptr_t>(255));
-    layout(b, c, r, sc);
+  // the workspace in `external` (a caller's buffer), or in a slab of the engine's own when null
+  int adopt(void* external, int c, int r, int sc) {
+    if (grow_workspace(this, std::tie(cap, cap_ref, scores_cap), external, c, r, sc)) return -1;
     ws_fresh = true;
     return 0;
   }
   int set_workspace(void* ptr, size_t bytes, int c, int r, int sc) {
     NOPE_CHECK(ptr && c >= 1 && r >= 1, "bad workspace arguments");
     NOPE_CHECK(bytes >= workspace_bytes(c, r, sc), "workspace buffer smaller than nope_unet_workspace_bytes");
-    if (ws_base && !ws_external) {
-      NOPE_CUDA(cudaDeviceSynchronize());
-      cudaFree(ws_base);
-    }
-    ws_base = static_cast<uint8_t*>(ptr);
-    ws_bytes = bytes;
-    ws_external = true;
-    return adopt(c, r, sc);
+    return adopt(ptr, c, r, sc);
   }
 
   // ------------------------------------------------------------------ op launchers
