@@ -145,11 +145,6 @@ __global__ void enc_extract_kernel(const float* __restrict__ x, float* __restric
   }
 }
 
-// w: [cout][taps][3][cin] fp16: (W_hi | W_lo | W_hi) per tap; fp16 mode [cout][taps][cin].  K: the packed row length.
-struct EncConv : ConvLayerBase {
-  int cout_real = 0, k = 1, stride = 1;
-};
-
 struct ActPair {
   __half* hi = nullptr;
   __half* lo = nullptr;   // nullptr: a single fp16 tensor
@@ -180,121 +175,199 @@ inline void split_tap(ConvBuilder& b, int hi, int lo, int dy, int dx, int nch) {
   b.seg(lo, dy, dx, nch);
 }
 
-}  // namespace nope
+// A convolution of the template encoder and the VAE engines: packed weights [cout][K] fp16, K = taps x
+// (W_hi | W_lo | W_hi) x cin, then, for a convolution with a 1x1 shortcut, (S_hi | S_lo | S_hi) x cin_sc; in the
+// single-fp16 mode each tap holds W_hi alone: K = taps x cin (+ cin_sc).  cout is padded to 64 with zero rows.
+struct SplitConv : ConvLayerBase {
+  int cin_sc = 0, k = 1;
+};
 
-struct nope_encoder {
-  static constexpr const char* kName = "encoder";
-  int D = 8, device = 0, num_sms = 132;
+// What the template encoder and the VAE engines share: the handle's state, the split-precision convolutions, their
+// packing and their launch.  Every activation buffer holds `cap` images.
+struct SplitConvEngine {
+  int device = 0, num_sms = 132;
   int precision = 0;                  // 0: split (hi, lo) operands; 1: single fp16 (set before finalize)
   bool finalized = false;
-  nope::StagedWeights staged;
-  std::map<std::string, nope::EncConv> convs;
-  float *stem_w = nullptr, *stem_b = nullptr;
-  nope::DeviceAllocs mem;             // weights, rot_stage
-  int cap = 0;                        // images the workspace holds
-  nope::ActPair buf[5];
-  float* proj_out = nullptr;
-  nope::WorkspaceSlab ws;
-  nope::TmapCache tmaps;
+  StagedWeights staged;
+  std::map<std::string, SplitConv> convs;
+  DeviceAllocs mem;
+  TmapCache tmaps;
   int64_t launches = 0;
-  static constexpr int kChunk = 32;   // images per encode() call: the workspace holds this many
-  float* rot_stage = nullptr;         // kChunk rotated 256x256 crops (25 MB), allocated by the first rotated encode
-  size_t out_floats() const { return (size_t)D * 32 * 32; }   // per encoded image
+  int cap = 0;                        // images the workspace holds
 
-  // ---------------------------------------------------------------- schema (resnet.py:93-133)
-  void expect_bn(const std::string& p, int c) {
-    for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) staged.expect(p + s, {c});
-  }
-  void build_schema() {
-    staged.expect("backbone.conv1.weight", {64, 3, 7, 7});
-    expect_bn("backbone.bn1", 64);
-    int inplanes = 64;
-    const int planes[4] = {64, 128, 256, 512}, blocks[4] = {3, 4, 6, 3}, strides[4] = {1, 2, 2, 1};
-    for (int li = 0; li < 4; ++li)
-      for (int b = 0; b < blocks[li]; ++b) {
-        const std::string p = "backbone.layer" + std::to_string(li + 1) + "." + std::to_string(b);
-        staged.expect(p + ".conv1.weight", {planes[li], inplanes, 1, 1});
-        expect_bn(p + ".bn1", planes[li]);
-        staged.expect(p + ".conv2.weight", {planes[li], planes[li], 3, 3});
-        expect_bn(p + ".bn2", planes[li]);
-        staged.expect(p + ".conv3.weight", {planes[li] * 4, planes[li], 1, 1});
-        expect_bn(p + ".bn3", planes[li] * 4);
-        if (b == 0 && (strides[li] != 1 || inplanes != planes[li] * 4)) {
-          staged.expect(p + ".downsample.0.weight", {planes[li] * 4, inplanes, 1, 1});
-          expect_bn(p + ".downsample.1", planes[li] * 4);
-        }
-        inplanes = planes[li] * 4;
-      }
-    staged.expect("projector.1.weight", {256, 2048, 1, 1});
-    staged.expect("projector.3.weight", {D, 256, 1, 1});
-  }
-
-  // ---------------------------------------------------------------- weights
-  // fold eval-mode BN (eps 1e-5) into the conv in double, split into fp16 (hi, lo), pack; fp16 mode: hi only
-  int make_conv(const std::string& name, const std::string& wkey, const std::string& bnkey, int stride) {
-    using namespace nope;
-    const HostTensor& W = staged.at(wkey);
-    EncConv L;
-    L.cout_real = (int)W.shape[0];
-    L.cin = (int)W.shape[1];
-    L.k = (int)W.shape[2];
-    L.stride = stride;
-    L.cout = (L.cout_real + 63) / 64 * 64;
-    const int taps = L.k * L.k;
-    const int prods = tap_products(precision);
-    L.K = taps * prods * L.cin;
-    NOPE_CHECK(L.cin % 64 == 0, wkey + ": input channels must be a multiple of 64");
+  // W [cout_real][cin][k*k] and bias [cout_real] in float64 (any folding done), optional 1x1 shortcut
+  // Ws [cout_real][cin_sc] -> convs[name]
+  int pack_conv(const std::string& name, int cout_real, int cin, int k, const std::vector<double>& W,
+                const std::vector<double>& bias, int cin_sc = 0, const std::vector<double>* Ws = nullptr) {
+    SplitConv L;
+    L.cin = cin;
+    L.cin_sc = cin_sc;
+    L.k = k;
+    L.cout = (cout_real + 63) / 64 * 64;
+    const int taps = k * k, prods = tap_products(precision);
+    L.K = (taps * cin + cin_sc) * prods;
+    NOPE_CHECK(cin % 64 == 0 && cin_sc % 64 == 0, name + ": input channels must be a multiple of 64");
     L.bn = pick_bn(L.cout);
-    std::vector<double> scale(L.cout_real, 1.0), shift(L.cout_real, 0.0);
-    if (!bnkey.empty()) {
-      const auto &g = staged.at(bnkey + ".weight").data, &b = staged.at(bnkey + ".bias").data,
-                 &m = staged.at(bnkey + ".running_mean").data, &v = staged.at(bnkey + ".running_var").data;
-      for (int o = 0; o < L.cout_real; ++o) {
-        scale[o] = (double)g[o] / std::sqrt((double)v[o] + 1e-5);
-        shift[o] = (double)b[o] - (double)m[o] * scale[o];
-      }
-    }
     std::vector<__half> packed((size_t)L.cout * L.K, __float2half_rn(0.f));
-    for (int o = 0; o < L.cout_real; ++o)
-      for (int c = 0; c < L.cin; ++c)
+    for (int o = 0; o < cout_real; ++o) {
+      for (int c = 0; c < cin; ++c)
         for (int t = 0; t < taps; ++t)
-          put_split_weight(&packed[(size_t)o * L.K + (size_t)t * prods * L.cin + c], L.cin, prods,
-                           (float)((double)W.data[((size_t)o * L.cin + c) * taps + t] * scale[o]));
-    std::vector<float> bias(L.cout, 0.f);
-    for (int o = 0; o < L.cout_real; ++o) bias[o] = (float)shift[o];
-    if (mem.upload(&L.w, packed) || mem.upload(&L.bias, bias)) return -1;
+          put_split_weight(&packed[(size_t)o * L.K + (size_t)t * prods * cin + c], cin, prods,
+                           (float)W[((size_t)o * cin + c) * taps + t]);
+      for (int c = 0; c < cin_sc; ++c)
+        put_split_weight(&packed[(size_t)o * L.K + (size_t)taps * prods * cin + c], cin_sc, prods,
+                         (float)(*Ws)[(size_t)o * cin_sc + c]);
+    }
+    std::vector<float> b(L.cout, 0.f);
+    for (int o = 0; o < cout_real; ++o) b[o] = (float)bias[o];
+    if (mem.upload(&L.w, packed) || mem.upload(&L.bias, b)) return -1;
     if (make_weight_map(&L.wmap, L.w, L.cout, L.K, L.bn)) return -1;
     convs[name] = L;
     return 0;
   }
 
-  // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
-  int finalize() {
-    {  // stem: fold bn1 into conv1, keep fp32
-      const auto& W = staged.at("backbone.conv1.weight").data;
-      const auto &g = staged.at("backbone.bn1.weight").data, &b = staged.at("backbone.bn1.bias").data,
-                 &m = staged.at("backbone.bn1.running_mean").data, &v = staged.at("backbone.bn1.running_var").data;
-      std::vector<float> w(64 * 147), bias(64);
-      for (int o = 0; o < 64; ++o) {
-        const double s = (double)g[o] / std::sqrt((double)v[o] + 1e-5);
-        for (int i = 0; i < 147; ++i) w[o * 147 + i] = (float)((double)W[o * 147 + i] * s);
-        bias[o] = (float)((double)b[o] - (double)m[o] * s);
-      }
-      if (mem.upload(&stem_w, w) || mem.upload(&stem_b, bias)) return -1;
+  // out = [relu](conv(taps over the input pairs `in`) [+ 1x1 shortcut over the pair sc] + bias [+ res]); output
+  // H x H.  in: (hi, lo) base pointers of each input pair with their lattice (-1: plain NHWC of side H); a tap's lat
+  // is the index of its input pair; fp16 mode: the hi maps only.  K order: per tap A_hi W_hi, A_hi W_lo, A_lo W_hi,
+  // then the shortcut's segments.
+  int conv(const SplitConv& L, const std::vector<std::pair<ActPair, int>>& in, const std::vector<ConvTap>& taps,
+           const ActPair* sc, int H, int n, bool relu, const ActPair* res, __half* out_hi, __half* out_lo,
+           float* out_f32, cudaStream_t st) {
+    TileGeom g;
+    if (make_geom(H, H, &g)) return -1;
+    NOPE_CHECK(in.size() + (sc ? 1 : 0) <= (size_t)kMaxAMaps / 2, "conv: too many input maps");
+    ConvBuilder b(tmaps, g, cap);
+    ConvParams& p = b.p;
+    int mh[kMaxAMaps / 2], ml[kMaxAMaps / 2];
+    for (size_t i = 0; i < in.size(); ++i) {
+      mh[i] = b.map(in[i].first.hi, L.cin, in[i].second);
+      ml[i] = precision == 0 ? b.map(in[i].first.lo, L.cin, in[i].second) : -1;
     }
-    const int blocks[4] = {3, 4, 6, 3}, strides[4] = {1, 2, 2, 1};
+    for (const ConvTap& t : taps) split_tap(b, mh[t.lat], ml[t.lat], t.dy, t.dx, L.cin / 64);
+    if (sc) {
+      const int h = b.map(sc->hi, L.cin_sc), l = precision == 0 ? b.map(sc->lo, L.cin_sc) : -1;
+      split_tap(b, h, l, 0, 0, L.cin_sc / 64);
+    }
+    if (b.finish(L, out_hi, L.cout, n, 1)) return -1;
+    NOPE_CHECK(p.ksteps * 64 == L.K, "conv: segment table");
+    p.relu = relu ? 1 : 0;
+    p.res_hi = res ? res->hi : nullptr;
+    p.res_lo = res ? res->lo : nullptr;
+    p.out_lo = out_lo;
+    p.out_f32 = out_f32;
+    ++launches;
+    return launch_conv_tc2(p, L.bn, num_sms, st);
+  }
+};
+
+}  // namespace nope
+
+struct nope_encoder : nope::SplitConvEngine {
+  static constexpr const char* kName = "encoder";
+  enum { kStem, kBottleneck, kProjector };
+  int D = 8;
+  std::vector<nope::ImageModule> plan;
+  float *stem_w = nullptr, *stem_b = nullptr;
+  nope::ActPair buf[5];
+  float* proj_out = nullptr;
+  nope::WorkspaceSlab ws;
+  static constexpr int kChunk = 32;   // images per encode() call: the workspace holds this many
+  float* rot_stage = nullptr;         // kChunk rotated 256x256 crops (25 MB), allocated by the first rotated encode
+  size_t out_floats() const { return (size_t)D * 32 * 32; }   // per encoded image
+
+  // ---------------------------------------------------------------- plan + schema (resnet.py:93-133)
+  // the stem, the 16 bottlenecks "backbone.layer<l>.<b>" (conv2 and the downsample at stride Hi / Ho) and the projector
+  void build_plan() {
+    plan = {{"stem", kStem, 3, 256, 64, 128}};
+    const int planes[4] = {64, 128, 256, 512}, blocks[4] = {3, 4, 6, 3}, strides[4] = {1, 2, 2, 1};
+    int cin = 64, H = 128;
     for (int li = 0; li < 4; ++li)
       for (int b = 0; b < blocks[li]; ++b) {
-        const std::string p = "backbone.layer" + std::to_string(li + 1) + "." + std::to_string(b);
-        const int st = b == 0 ? strides[li] : 1;
-        if (make_conv(p + ".conv1", p + ".conv1.weight", p + ".bn1", 1)) return -1;
-        if (make_conv(p + ".conv2", p + ".conv2.weight", p + ".bn2", st)) return -1;   // resnet.py:62
-        if (make_conv(p + ".conv3", p + ".conv3.weight", p + ".bn3", 1)) return -1;
-        if (staged.has(p + ".downsample.0.weight"))
-          if (make_conv(p + ".down", p + ".downsample.0.weight", p + ".downsample.1", st)) return -1;
+        const int s = b == 0 ? strides[li] : 1;   // resnet.py:62
+        plan.push_back({"backbone.layer" + std::to_string(li + 1) + "." + std::to_string(b), kBottleneck, cin, H,
+                        planes[li] * 4, H / s});
+        cin = planes[li] * 4;
+        H /= s;
       }
-    if (make_conv("projector.1", "projector.1.weight", "", 1)) return -1;
-    return make_conv("projector.3", "projector.3.weight", "", 1);
+    plan.push_back({"projector", kProjector, 2048, 32, D, 32});
+  }
+  // a bottleneck that changes the side or the channels has a downsample on its shortcut
+  static bool has_down(const nope::ImageModule& m) { return m.Ci != m.Co || m.Hi != m.Ho; }
+
+  void expect_bn(const std::string& p, int c) {
+    for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) staged.expect(p + s, {c});
+  }
+  void build_schema() {
+    for (const nope::ImageModule& m : plan) {
+      const std::string& p = m.name;
+      if (m.kind == kStem) {
+        staged.expect("backbone.conv1.weight", {64, 3, 7, 7});
+        expect_bn("backbone.bn1", 64);
+      } else if (m.kind == kBottleneck) {
+        const int planes = m.Co / 4;
+        staged.expect(p + ".conv1.weight", {planes, m.Ci, 1, 1});
+        expect_bn(p + ".bn1", planes);
+        staged.expect(p + ".conv2.weight", {planes, planes, 3, 3});
+        expect_bn(p + ".bn2", planes);
+        staged.expect(p + ".conv3.weight", {m.Co, planes, 1, 1});
+        expect_bn(p + ".bn3", m.Co);
+        if (has_down(m)) {
+          staged.expect(p + ".downsample.0.weight", {m.Co, m.Ci, 1, 1});
+          expect_bn(p + ".downsample.1", m.Co);
+        }
+      } else {
+        staged.expect("projector.1.weight", {256, 2048, 1, 1});
+        staged.expect("projector.3.weight", {D, 256, 1, 1});
+      }
+    }
+  }
+
+  // ---------------------------------------------------------------- weights
+  // fold eval-mode BN (eps 1e-5) into the conv in double, then pack_conv; bnkey empty: no BN, no bias
+  int make_conv(const std::string& name, const std::string& wkey, const std::string& bnkey) {
+    const nope::HostTensor& W = staged.at(wkey);
+    const int cout = (int)W.shape[0], cin = (int)W.shape[1], k = (int)W.shape[2], taps = k * k;
+    std::vector<double> scale(cout, 1.0), shift(cout, 0.0);
+    if (!bnkey.empty()) {
+      const auto &g = staged.at(bnkey + ".weight").data, &b = staged.at(bnkey + ".bias").data,
+                 &m = staged.at(bnkey + ".running_mean").data, &v = staged.at(bnkey + ".running_var").data;
+      for (int o = 0; o < cout; ++o) {
+        scale[o] = (double)g[o] / std::sqrt((double)v[o] + 1e-5);
+        shift[o] = (double)b[o] - (double)m[o] * scale[o];
+      }
+    }
+    std::vector<double> w(W.data.size());
+    for (size_t i = 0; i < w.size(); ++i) w[i] = (double)W.data[i] * scale[i / ((size_t)cin * taps)];
+    return pack_conv(name, cout, cin, k, w, shift);
+  }
+
+  // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
+  int finalize() {
+    for (const nope::ImageModule& m : plan) {
+      const std::string& p = m.name;
+      if (m.kind == kStem) {  // fold bn1 into conv1, keep fp32
+        const auto& W = staged.at("backbone.conv1.weight").data;
+        const auto &g = staged.at("backbone.bn1.weight").data, &b = staged.at("backbone.bn1.bias").data,
+                   &mu = staged.at("backbone.bn1.running_mean").data, &v = staged.at("backbone.bn1.running_var").data;
+        std::vector<float> w(64 * 147), bias(64);
+        for (int o = 0; o < 64; ++o) {
+          const double s = (double)g[o] / std::sqrt((double)v[o] + 1e-5);
+          for (int i = 0; i < 147; ++i) w[o * 147 + i] = (float)((double)W[o * 147 + i] * s);
+          bias[o] = (float)((double)b[o] - (double)mu[o] * s);
+        }
+        if (mem.upload(&stem_w, w) || mem.upload(&stem_b, bias)) return -1;
+      } else if (m.kind == kBottleneck) {
+        if (make_conv(p + ".conv1", p + ".conv1.weight", p + ".bn1") ||
+            make_conv(p + ".conv2", p + ".conv2.weight", p + ".bn2") ||
+            make_conv(p + ".conv3", p + ".conv3.weight", p + ".bn3") ||
+            (has_down(m) && make_conv(p + ".down", p + ".downsample.0.weight", p + ".downsample.1")))
+          return -1;
+      } else if (make_conv("projector.1", "projector.1.weight", "") ||
+                 make_conv("projector.3", "projector.3.weight", "")) {
+        return -1;
+      }
+    }
+    return 0;
   }
 
   // ---------------------------------------------------------------- workspace
@@ -309,66 +382,40 @@ struct nope_encoder {
   }
   int ensure_workspace(int B) { return B <= cap ? 0 : nope::grow_workspace(this, std::tie(cap), nullptr, B); }
 
-  // out = [relu](conv(in) + bias [+ res]); Hin = input side; returns output side in *Hout
-  int conv(const nope::EncConv& L, const nope::ActPair& in, int Hin, const nope::ActPair& out, int n_img,
-           bool relu, const nope::ActPair* res, float* out_f32, cudaStream_t st) {
+  // out = [relu](conv(in) + bias [+ res]) of a 1x1 or 3x3 (pad 1) convolution at stride 1 or 2 over an input of side
+  // Hin; a stride-2 convolution reads its input as its four stride-2 sub-lattices (same trick as HardDownsample).
+  // out_f32: the fp32 output instead of out's lo half.
+  int conv_at(const nope::SplitConv& L, const nope::ActPair& in, int Hin, int stride, const nope::ActPair& out, int n,
+              bool relu, const nope::ActPair* res, float* out_f32, cudaStream_t st) {
     using namespace nope;
-    const int Ho = Hin / L.stride;
-    TileGeom g;
-    if (make_geom(Ho, Ho, &g)) return -1;
-    ConvBuilder b(tmaps, g, cap);
-    ConvParams& p = b.p;
-    // maps: hi then lo (fp16 mode: hi only), each as the four stride-2 lattices for a stride-2 convolution
-    const int n_lat = L.stride == 1 ? 1 : 4;
-    int mh[4] = {}, ml[4] = {-1, -1, -1, -1};
-    for (int t = 0; t < n_lat; ++t) mh[t] = b.map(in.hi, L.cin, L.stride == 1 ? -1 : t);
-    if (precision == 0)
-      for (int t = 0; t < n_lat; ++t) ml[t] = b.map(in.lo, L.cin, L.stride == 1 ? -1 : t);
+    std::vector<std::pair<ActPair, int>> src;
+    for (int t = 0; t < (stride == 1 ? 1 : 4); ++t) src.push_back({in, stride == 1 ? -1 : t});
+    std::vector<ConvTap> taps;
     for (int ky = 0; ky < L.k; ++ky)
       for (int kx = 0; kx < L.k; ++kx) {
         const int oy = L.k == 3 ? ky - 1 : 0, ox = L.k == 3 ? kx - 1 : 0;
-        const ConvTap t = L.stride == 1 ? ConvTap{0, oy, ox} : stride2_tap(oy, ox);
-        split_tap(b, mh[t.lat], ml[t.lat], t.dy, t.dx, L.cin / 64);
+        taps.push_back(stride == 1 ? ConvTap{0, oy, ox} : stride2_tap(oy, ox));
       }
-    if (b.finish(L, out.hi, L.cout, n_img, 1)) return -1;
-    NOPE_CHECK(p.ksteps * 64 == L.K, "encoder conv: segment table");
-    p.relu = relu ? 1 : 0;
-    p.res_hi = res ? res->hi : nullptr;
-    p.res_lo = res ? res->lo : nullptr;
-    p.out_lo = out_f32 ? nullptr : out.lo;
-    p.out_f32 = out_f32;
-    ++launches;
-    return launch_conv_tc2(p, L.bn, num_sms, st);
+    return conv(L, src, taps, nullptr, Hin / stride, n, relu, res, out.hi, out_f32 ? nullptr : out.lo, out_f32, st);
   }
 
-  // stem: images [B, 3, 256, 256] -> buf[0] (128 x 128 x 64)
-  int stem(const float* images, int B, cudaStream_t st) {
-    const long long npix = (long long)B * 128 * 128;
-    nope::enc_stem_kernel<<<(unsigned)((npix + 3) / 4), 256, 0, st>>>(images, stem_w, stem_b, buf[0].hi, buf[0].lo,
-                                                                      B, 256, 256);
-    NOPE_CUDA(cudaGetLastError());
-    ++launches;
-    return 0;
-  }
-
-  // bottleneck p (conv2 / downsample stride stv) on buf[cur] of side H -> buf[cur] (the new cur), side H / stv
-  int bottleneck(const std::string& p, int stv, int H, int B, int& cur, cudaStream_t st) {
+  // bottleneck m on buf[cur] -> buf[cur] (the new cur)
+  int bottleneck(const nope::ImageModule& m, int n, int& cur, cudaStream_t st) {
     using namespace nope;
     // free buffers: the four that are not `cur`
     int f[4], nf = 0;
     for (int i = 0; i < 5; ++i)
       if (i != cur) f[nf++] = i;
     const ActPair &x = buf[cur], &a = buf[f[0]], &bb = buf[f[1]], &r = buf[f[2]], &o = buf[f[3]];
-    if (conv(convs.at(p + ".conv1"), x, H, a, B, true, nullptr, nullptr, st)) return -1;
-    if (conv(convs.at(p + ".conv2"), a, H, bb, B, true, nullptr, nullptr, st)) return -1;
-    const int Ho = H / stv;
+    const int s = m.Hi / m.Ho;
+    if (conv_at(convs.at(m.name + ".conv1"), x, m.Hi, 1, a, n, true, nullptr, nullptr, st)) return -1;
+    if (conv_at(convs.at(m.name + ".conv2"), a, m.Hi, s, bb, n, true, nullptr, nullptr, st)) return -1;
     const ActPair* res = &x;
-    auto it = convs.find(p + ".down");
-    if (it != convs.end()) {
-      if (conv(it->second, x, H, r, B, false, nullptr, nullptr, st)) return -1;
+    if (has_down(m)) {
+      if (conv_at(convs.at(m.name + ".down"), x, m.Hi, s, r, n, false, nullptr, nullptr, st)) return -1;
       res = &r;
     }
-    if (conv(convs.at(p + ".conv3"), bb, Ho, o, B, true, res, nullptr, st)) return -1;
+    if (conv_at(convs.at(m.name + ".conv3"), bb, m.Ho, 1, o, n, true, res, nullptr, st)) return -1;
     cur = f[3];
     return 0;
   }
@@ -378,9 +425,9 @@ struct nope_encoder {
   int projector(int cur, int H, int B, float* out, cudaStream_t st) {
     using namespace nope;
     const int nxt = (cur + 1) % 5;
-    if (conv(convs.at("projector.1"), buf[cur], H, buf[nxt], B, true, nullptr, nullptr, st)) return -1;
+    if (conv_at(convs.at("projector.1"), buf[cur], H, 1, buf[nxt], B, true, nullptr, nullptr, st)) return -1;
     const int nx2 = (cur + 2) % 5;
-    if (conv(convs.at("projector.3"), buf[nxt], H, buf[nx2], B, false, nullptr, proj_out, st)) return -1;
+    if (conv_at(convs.at("projector.3"), buf[nxt], H, 1, buf[nx2], B, false, nullptr, proj_out, st)) return -1;
     enc_extract_kernel<<<ew_grid((long long)B * D * H * H), 256, 0, st>>>(proj_out, out, B, D, H * H,
                                                                           convs.at("projector.3").cout);
     NOPE_CUDA(cudaGetLastError());
@@ -388,73 +435,52 @@ struct nope_encoder {
     return 0;
   }
 
-  static constexpr int kBlocks[4] = {3, 4, 6, 3}, kStrides[4] = {1, 2, 2, 1};
-  static std::string block_name(int li, int b) {
-    return "backbone.layer" + std::to_string(li + 1) + "." + std::to_string(b);
+  // module m of n images: the stem on images [n, 3, 256, 256] -> buf[0]; a bottleneck on buf[cur] -> buf[cur] (the
+  // new cur); the projector on buf[cur] -> out [n, D, 32, 32]
+  int run(const nope::ImageModule& m, int n, int& cur, const float* images, float* out, cudaStream_t st) {
+    if (m.kind == kBottleneck) return bottleneck(m, n, cur, st);
+    if (m.kind == kProjector) return projector(cur, m.Hi, n, out, st);
+    const long long npix = (long long)n * 128 * 128;   // stem: 7x7 stride 2, 256 -> 128
+    nope::enc_stem_kernel<<<(unsigned)((npix + 3) / 4), 256, 0, st>>>(images, stem_w, stem_b, buf[0].hi, buf[0].lo,
+                                                                      n, 256, 256);
+    NOPE_CUDA(cudaGetLastError());
+    ++launches;
+    cur = 0;
+    return 0;
   }
 
   int encode(const float* images, int B, float* out, cudaStream_t st) {
     if (ensure_workspace(B)) return -1;
     launches = 0;
-    if (stem(images, B, st)) return -1;
-    int H = 128, cur = 0;   // buf[cur] holds the block input
-    for (int li = 0; li < 4; ++li)
-      for (int b = 0; b < kBlocks[li]; ++b) {
-        const int stv = b == 0 ? kStrides[li] : 1;
-        if (bottleneck(block_name(li, b), stv, H, B, cur, st)) return -1;
-        H /= stv;
-      }
-    return projector(cur, H, B, out, st);
+    int cur = 0;
+    for (const nope::ImageModule& m : plan)
+      if (run(m, B, cur, images, out, st)) return -1;
+    return 0;
   }
 
   // Runs one module on its own (nope_encoder_run_block): "stem" on images [n, 3, 256, 256], a bottleneck
   // "backbone.layer<l>.<b>" or "projector" on x [n, C, H, H] fp32 NCHW, staged as (hi, lo) into the block's input
-  // buffer -> out fp32 NCHW: hi + lo of the block's output pair, the projector's fp32 output.  *Co, *Ho: its shape.
+  // buffer -> out fp32 NCHW: hi + lo of the block's output pair, the projector's fp32 output.
   int run_block(const std::string& name, const float* x, int C, int H, int n, float* out, int64_t cap_floats,
                 cudaStream_t st) {
     using namespace nope;
-    int Ci = 0, Hi = 0, Co = 0, Ho = 0, stv = 1;
-    if (name == "stem") {
-      Ci = 3, Hi = 256, Co = 64, Ho = 128;
-    } else if (name == "projector") {
-      Ci = 2048, Hi = 32, Co = D, Ho = 32;
-    } else {
-      int h = 128;
-      for (int li = 0; li < 4 && !Ci; ++li)
-        for (int b = 0; b < kBlocks[li]; ++b) {
-          const int s = b == 0 ? kStrides[li] : 1;
-          if (name == block_name(li, b)) {
-            Ci = convs.at(name + ".conv1").cin, Hi = h, Co = convs.at(name + ".conv3").cout, Ho = h / s, stv = s;
-            break;
-          }
-          h /= s;
-        }
-      NOPE_CHECK(Ci, "run_block: unknown encoder module " + name);
-    }
-    if (check_block(name, kChunk, C, H, n, Ci, Hi, Co, Ho, cap_floats)) return -1;
+    const ImageModule* m = find_module(plan, name);
+    NOPE_CHECK(m, "run_block: unknown encoder module " + name);
+    if (check_block(*m, kChunk, C, H, n, cap_floats)) return -1;
     if (ensure_workspace(n)) return -1;
     launches = 0;
-    if (name == "stem") {
-      if (stem(x, n, st)) return -1;
-      to_nchw_pair(buf[0], out, n, Co, Ho, st);
-    } else {
+    if (m->kind != kStem) {
       nchw_f32_to_nhwc_f16_kernel<<<ew_grid((long long)n * C * H * H), 256, 0, st>>>(x, buf[0].hi, n, C, H * H,
                                                                                      buf[0].lo);
       NOPE_CUDA(cudaGetLastError());
-      int cur = 0;
-      if (name == "projector") {
-        if (projector(cur, H, n, out, st)) return -1;
-      } else {
-        if (bottleneck(name, stv, H, n, cur, st)) return -1;
-        to_nchw_pair(buf[cur], out, n, Co, Ho, st);
-      }
     }
+    int cur = 0;
+    if (run(*m, n, cur, x, out, st)) return -1;
+    if (m->kind != kProjector)
+      nhwc_f16_to_nchw_f32_kernel<<<ew_grid((long long)n * m->Co * m->Ho * m->Ho), 256, 0, st>>>(
+          buf[cur].hi, out, n, m->Co, m->Ho * m->Ho, buf[cur].lo);
     NOPE_CUDA(cudaGetLastError());
     NOPE_CUDA(cudaStreamSynchronize(st));
     return 0;
-  }
-  static void to_nchw_pair(const nope::ActPair& a, float* out, int n, int C, int H, cudaStream_t st) {
-    nope::nhwc_f16_to_nchw_f32_kernel<<<nope::ew_grid((long long)n * C * H * H), 256, 0, st>>>(a.hi, out, n, C, H * H,
-                                                                                               a.lo);
   }
 };

@@ -2,7 +2,8 @@
 // LDM) shares: the state_dict schema and the host copies staged against it until finalize, the device allocations
 // freed with the engine, the device check of every *_create, and the bodies of the *_load_tensor / *_finalize /
 // per-chunk C-ABI entry points.  The two sweep engines (UNet, LDM) also share the sweep driver, the debug tap and the
-// per-launch profile; the two image encoders share the rotated-encode loop and the run_block shape checks.
+// per-launch profile; the three image engines (template encoder, VAE encoder, VAE decoder) share the module entry of
+// their plans and the run_block argument checks, and the two image encoders the rotated-encode loop.
 //
 // An engine E provides: `static constexpr const char* kName` (the name its errors carry), `bool finalized`,
 // `int device`, `StagedWeights staged`, and `int finalize()` (packs the staged tensors; runs once every schema key
@@ -15,8 +16,10 @@
 //   int prestage(const float* ref, int B, cudaStream_t)                  the pose-independent prefix per reference;
 //   int forward_chunk(poses, hyp0, n, N, query, out_emb, score_part, cudaStream_t, int Q);
 //   int rank(part, sim, B, N, Q, k, topv, topi, idx_base, cudaStream_t) the similarities and top-k from the partials.
-// An image encoder (per_rotated_chunk) provides `kChunk`, `int64_t launches`, `DeviceAllocs mem`, `float* rot_stage`
-// and `int encode(const float*, int, float*, cudaStream_t)`.
+// An image engine derives from SplitConvEngine (encoder.cuh), which holds `launches`, `mem` and the split-precision
+// convolutions, and provides `kChunk` and `std::vector<ImageModule> plan`, built in forward order when the handle is
+// created; its schema, weight packing, forward pass and run_block all walk that plan.  An image encoder
+// (per_rotated_chunk) also provides `float* rot_stage` and `int encode(const float*, int, float*, cudaStream_t)`.
 #pragma once
 #include <algorithm>
 #include <map>
@@ -370,16 +373,25 @@ int per_rotated_chunk(E* e, int P, float* out, size_t out_per, cudaStream_t st, 
   return 0;
 }
 
-// The checks every *_run_block of an image engine makes once the module's input shape (Ci, Hi) and output shape
-// (Co, Ho) are known; Ci == 0: no such module.
-inline int check_block(const std::string& name, int chunk, int C, int H, int n, int Ci, int Hi, int Co, int Ho,
-                       int64_t cap_floats) {
-  NOPE_CHECK(Ci, "run_block: unknown module " + name);
+// One module of an image engine's plan: the name *_run_block takes, the engine's kind of module, and its input
+// [Ci, Hi, Hi] and output [Co, Ho, Ho] per image.  The plan lists the modules in forward order.
+struct ImageModule {
+  std::string name;
+  int kind, Ci, Hi, Co, Ho;
+};
+inline const ImageModule* find_module(const std::vector<ImageModule>& plan, const std::string& name) {
+  for (const ImageModule& m : plan)
+    if (m.name == name) return &m;
+  return nullptr;
+}
+
+// The checks every *_run_block of an image engine makes of its arguments against module m.
+inline int check_block(const ImageModule& m, int chunk, int C, int H, int n, int64_t cap_floats) {
   NOPE_CHECK(n >= 1 && n <= chunk, "run_block: n must be in [1, " + std::to_string(chunk) + "]");
-  NOPE_CHECK(C == Ci && H == Hi, "run_block: " + name + " takes [n, " + std::to_string(Ci) + ", " +
-                                     std::to_string(Hi) + ", " + std::to_string(Hi) + "] inputs, got C = " +
-                                     std::to_string(C) + ", H = " + std::to_string(H));
-  NOPE_CHECK(cap_floats >= (int64_t)n * Co * Ho * Ho, "run_block: output buffer too small");
+  NOPE_CHECK(C == m.Ci && H == m.Hi, "run_block: " + m.name + " takes [n, " + std::to_string(m.Ci) + ", " +
+                                         std::to_string(m.Hi) + ", " + std::to_string(m.Hi) + "] inputs, got C = " +
+                                         std::to_string(C) + ", H = " + std::to_string(H));
+  NOPE_CHECK(cap_floats >= (int64_t)n * m.Co * m.Ho * m.Ho, "run_block: output buffer too small");
   return 0;
 }
 

@@ -417,6 +417,7 @@ int nope_encoder_create(nope_encoder_t** out, int descriptor_size, int device) {
   if (open_device(device, &e->num_sms)) return -1;
   e->D = descriptor_size;
   e->device = device;
+  e->build_plan();
   e->build_schema();
   *out = e.release();
   return 0;
@@ -575,6 +576,7 @@ int nope_vae_create(nope_vae_t** out, int device) {
   auto v = std::make_unique<nope_vae>();
   if (open_device(device, &v->num_sms)) return -1;
   v->device = device;
+  v->build_plan();
   v->build_schema();
   *out = v.release();
   return 0;
@@ -618,6 +620,7 @@ int nope_vae_decoder_create(nope_vae_decoder_t** out, int device) {
   auto d = std::make_unique<nope_vae_decoder>();
   if (open_device(device, &d->num_sms)) return -1;
   d->device = device;
+  d->build_plan();
   d->build_schema();
   *out = d.release();
   return 0;

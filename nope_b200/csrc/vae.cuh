@@ -249,13 +249,6 @@ __global__ void __launch_bounds__(256) vae_softmax_kernel(float* __restrict__ s)
   for (int k = 0; k < 4; ++k) row[t + 256 * k] = __fdividef(v[k], sum);
 }
 
-// A convolution of the VAE: packed split-precision weights [cout][K] fp16, K = taps x (W_hi | W_lo | W_hi) x cin,
-// then, for a ResnetBlock2D conv2 with a 1x1 shortcut, (S_hi | S_lo | S_hi) x cin_sc; bias = b2 (+ b_shortcut).
-// In the single-fp16 mode each tap holds W_hi alone: K = taps x cin (+ cin_sc).
-struct VaeConv : ConvLayerBase {
-  int cin_sc = 0, k = 1;
-};
-
 struct VaeNorm {
   float* gamma = nullptr;
   float* beta = nullptr;
@@ -349,17 +342,13 @@ vae_dec_extract_kernel(const float* __restrict__ t, int ld, int cap, int n, floa
 }
 
 // ---------------------------------------------------------------- host side shared by the encoder and the decoder
-// The state_dict schema helpers, the split-precision weight packing, the workspace, and the launches of a
-// convolution, GroupNorm, ResnetBlock2D and the mid-block attention.  Every buffer holds `cap` images.
-struct VaeEngine {
-  const int cap;                              // images per pass
-  int device = 0, num_sms = 132;
-  int precision = 0;                          // 0: split (hi, lo) operands; 1: single fp16 (encoder, before finalize)
-  bool finalized = false;
-  StagedWeights staged;
-  std::map<std::string, VaeConv> convs;
+// The module kinds, the state_dict schema helpers, the workspace, the launches of a 3x3 convolution, GroupNorm,
+// ResnetBlock2D and the mid-block attention, the forward pass over the plan and run_block.  Every buffer holds `cap`
+// images (the engine's kChunk); mem also holds the workspace and rot_stage.
+struct VaeEngine : SplitConvEngine {
+  enum { kConvIn, kResnet, kDown, kUp, kAttention, kConvOut };
+  std::vector<ImageModule> plan;              // conv_in first, conv_out last
   std::map<std::string, VaeNorm> norms;
-  DeviceAllocs mem;                           // weights, workspace and rot_stage
   // workspace (alloc_workspace), each activation buffer sized for cap images of the widest level
   float* x32[2] = {nullptr, nullptr};         // residual stream, fp32
   ActPair xs[2];                              // residual stream, (hi, lo)
@@ -367,10 +356,43 @@ struct VaeEngine {
   float* t32 = nullptr;                       // conv1 / qkv / conv_out output, fp32
   double2* gn_part = nullptr;                 // GroupNorm partial sums
   float2* gn_stats = nullptr;                 // GroupNorm (mean, rstd)
-  TmapCache tmaps;
-  int64_t launches = 0;
 
-  explicit VaeEngine(int cap_) : cap(cap_) {}
+  explicit VaeEngine(int cap_) { cap = cap_; }
+
+  // module m of n inputs on the residual stream `cur` -> the new cur.  conv_in reads the raw inputs `in` (images or
+  // latents) and starts stream 0; conv_out leaves its fp32 output in t32 for extract_output.  The launches of
+  // conv_in and of extract_output are not counted (run_block reports neither; forward adds them).
+  virtual int run(const ImageModule& m, int n, int& cur, const float* in, cudaStream_t st) = 0;
+  // conv_out's output in t32 -> out, the engine's output layout
+  virtual int extract_output(int n, float* out, cudaStream_t st) = 0;
+
+  // n <= cap inputs through the plan -> out
+  int forward(const float* in, int n, float* out, cudaStream_t st) {
+    launches = 2;   // conv_in and extract_output
+    int cur = 0;
+    for (const ImageModule& m : plan)
+      if (run(m, n, cur, in, st)) return -1;
+    return extract_output(n, out, st);
+  }
+
+  // Runs one module of the forward pass on its own (nope_vae_run_block, nope_vae_decoder_run_block): x [n, C, H, H]
+  // fp32 NCHW (the raw inputs for conv_in) staged as the residual stream -> out: the fp32 stream after the module,
+  // out_pair (nullable): its (hi, lo) pair as hi + lo.  conv_out gives the engine's output and has no pair.
+  int run_block(const std::string& name, const float* x, int C, int H, int n, float* out, float* out_pair,
+                int64_t cap_floats, cudaStream_t st) {
+    const ImageModule* m = find_module(plan, name);
+    NOPE_CHECK(m, "run_block: unknown module " + name);
+    if (check_block(*m, cap, C, H, n, cap_floats)) return -1;
+    NOPE_CHECK(!out_pair || m->kind != kConvOut, "run_block: " + name + " has no (hi, lo) output");
+    launches = 0;
+    int cur = 0;
+    if (m->kind != kConvIn && stage_stream(x, C, H, n, st)) return -1;
+    if (run(*m, n, cur, x, st)) return -1;
+    if (m->kind == kConvOut ? extract_output(n, out, st) : extract_stream(cur, m->Co, m->Ho, n, out, out_pair, st))
+      return -1;
+    NOPE_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  }
 
   // ---------------------------------------------------------------- schema (diffusers AutoencoderKL, SD v1)
   void expect_norm(const std::string& p, int c) {
@@ -399,35 +421,6 @@ struct VaeEngine {
   // ---------------------------------------------------------------- weights
   const std::vector<float>& h(const std::string& k) const { return staged.at(k).data; }
 
-  // W [cout_real][cin][k*k], bias [cout_real] (float64), optional 1x1 shortcut Ws [cout_real][cin_sc] + its bias
-  int pack_conv(const std::string& name, int cout_real, int cin, int k, const std::vector<double>& W,
-                const std::vector<double>& bias, int cin_sc = 0, const std::vector<double>* Ws = nullptr) {
-    VaeConv L;
-    L.cin = cin;
-    L.cin_sc = cin_sc;
-    L.k = k;
-    L.cout = (cout_real + 63) / 64 * 64;
-    const int taps = k * k, prods = tap_products(precision);
-    L.K = (taps * cin + cin_sc) * prods;
-    NOPE_CHECK(cin % 64 == 0 && cin_sc % 64 == 0, name + ": input channels must be a multiple of 64");
-    L.bn = pick_bn(L.cout);
-    std::vector<__half> packed((size_t)L.cout * L.K, __float2half_rn(0.f));
-    for (int o = 0; o < cout_real; ++o) {
-      for (int c = 0; c < cin; ++c)
-        for (int t = 0; t < taps; ++t)
-          put_split_weight(&packed[(size_t)o * L.K + (size_t)t * prods * cin + c], cin, prods,
-                           (float)W[((size_t)o * cin + c) * taps + t]);
-      for (int c = 0; c < cin_sc; ++c)
-        put_split_weight(&packed[(size_t)o * L.K + (size_t)taps * prods * cin + c], cin_sc, prods,
-                         (float)(*Ws)[(size_t)o * cin_sc + c]);
-    }
-    std::vector<float> b(L.cout, 0.f);
-    for (int o = 0; o < cout_real; ++o) b[o] = (float)bias[o];
-    if (mem.upload(&L.w, packed) || mem.upload(&L.bias, b)) return -1;
-    if (make_weight_map(&L.wmap, L.w, L.cout, L.K, L.bn)) return -1;
-    convs[name] = L;
-    return 0;
-  }
   std::vector<double> dvec(const std::string& k) {
     const auto& v = h(k);
     return std::vector<double>(v.begin(), v.end());
@@ -483,47 +476,16 @@ struct VaeEngine {
   // offset of plane q of a parity-planar level-0 tensor with C channels
   size_t plane_off(int q, int C) const { return (size_t)q * cap * 128 * 128 * C; }
 
-  // out = conv(taps over the input pairs `in`) [+ shortcut taps over pair sc] + bias [+ res]; output H x H.
-  // in: (hi, lo) base pointers of each input pair with their lattice (-1: plain NHWC of side H); fp16 mode: hi only.
-  // A tap's lat is the index of its input pair.
-  int conv(const VaeConv& L, const std::vector<std::pair<ActPair, int>>& in, const std::vector<ConvTap>& taps,
-           int sc_pair, int H, int n, __half* out_hi, __half* out_lo, float* out_f32, const ActPair* res,
-           cudaStream_t st) {
-    TileGeom g;
-    if (make_geom(H, H, &g)) return -1;
-    NOPE_CHECK(in.size() <= (size_t)kMaxAMaps / 2, "vae conv: too many input maps");
-    ConvBuilder b(tmaps, g, cap);
-    ConvParams& p = b.p;
-    int mh[kMaxAMaps / 2], ml[kMaxAMaps / 2];
-    for (size_t i = 0; i < in.size(); ++i) {
-      const int C = (int)i == sc_pair ? L.cin_sc : L.cin;
-      mh[i] = b.map(in[i].first.hi, C, in[i].second);
-      ml[i] = precision == 0 ? b.map(in[i].first.lo, C, in[i].second) : -1;   // fp16 mode: the hi maps only
-    }
-    for (const ConvTap& t : taps) split_tap(b, mh[t.lat], ml[t.lat], t.dy, t.dx, L.cin / 64);
-    if (sc_pair >= 0) split_tap(b, mh[sc_pair], ml[sc_pair], 0, 0, L.cin_sc / 64);
-    if (b.finish(L, out_hi, L.cout, n, 1)) return -1;
-    NOPE_CHECK(p.ksteps * 64 == L.K, "vae conv: segment table");
-    p.res_hi = res ? res->hi : nullptr;
-    p.res_lo = res ? res->lo : nullptr;
-    p.out_lo = out_lo;
-    p.out_f32 = out_f32;
-    ++launches;
-    return launch_conv_tc2(p, L.bn, num_sms, st);
-  }
-
   // 3x3 pad-1 convolution at the current level.  Level 0 (parity-planar): one launch per output plane (py, px);
   // tap (oy, ox) of that plane reads input plane ((py + oy) & 1, (px + ox) & 1) at offset ((py + oy) >> 1, ...).
   // Output: out_f32 (+ (hi, lo) when out_lo), residual res (same layout) or the conv's 1x1 shortcut over sc.
-  int conv3(const VaeConv& L, const ActPair& in, int H, int n, const ActPair& out, bool want_lo, float* out_f32,
+  int conv3(const SplitConv& L, const ActPair& in, int H, int n, const ActPair& out, bool want_lo, float* out_f32,
             const ActPair* res, const ActPair* sc, cudaStream_t st) {
     std::vector<ConvTap> taps;
     if (H < 256) {
       for (int oy = -1; oy <= 1; ++oy)
         for (int ox = -1; ox <= 1; ++ox) taps.push_back(ConvTap{0, oy, ox});
-      std::vector<std::pair<ActPair, int>> src{{in, -1}};
-      if (sc) src.push_back({*sc, -1});
-      return conv(L, src, taps, sc ? 1 : -1, H, n, out.hi, want_lo ? out.lo : nullptr, out_f32, res, st);
+      return conv(L, {{in, -1}}, taps, sc, H, n, false, res, out.hi, want_lo ? out.lo : nullptr, out_f32, st);
     }
     NOPE_CHECK(!sc, "vae conv: no shortcut segments at the 256 x 256 level");
     std::vector<std::pair<ActPair, int>> src;
@@ -536,8 +498,8 @@ struct VaeEngine {
       const size_t o = plane_off(q, L.cout);
       ActPair r;
       if (res) r = act_at(*res, o);
-      if (conv(L, src, taps, -1, 128, n, out.hi + o, want_lo ? act_at(out, o).lo : nullptr, out_f32 + o,
-               res ? &r : nullptr, st))
+      if (conv(L, src, taps, nullptr, 128, n, false, res ? &r : nullptr, out.hi + o,
+               want_lo ? act_at(out, o).lo : nullptr, out_f32 + o, st))
         return -1;
     }
     return 0;
@@ -570,11 +532,11 @@ struct VaeEngine {
       // the 1x1 shortcut, one launch per plane, into x32[cur]'s memory (norm1 was its last reader)
       __half* s = reinterpret_cast<__half*>(x32[cur]);
       sres = ActPair{s, precision == 0 ? s + 4 * plane_off(1, cout) : nullptr};
-      const VaeConv& S = convs.at(p + ".conv_shortcut");
+      const SplitConv& S = convs.at(p + ".conv_shortcut");
       for (int q = 0; q < 4; ++q) {
         const size_t i = plane_off(q, cin), o = plane_off(q, cout);
-        if (conv(S, {{act_at(xs[cur], i), -1}}, {ConvTap{0, 0, 0}}, -1, 128, n, sres.hi + o, act_at(sres, o).lo,
-                 nullptr, nullptr, st))
+        if (conv(S, {{act_at(xs[cur], i), -1}}, {ConvTap{0, 0, 0}}, nullptr, 128, n, false, nullptr, sres.hi + o,
+                 act_at(sres, o).lo, nullptr, st))
           return -1;
       }
     }
@@ -594,8 +556,9 @@ struct VaeEngine {
     const int nxt = 1 - cur;
     if (group_norm(a + "group_norm", x32[cur], 512, 32, n, false, st)) return -1;
     // qkv [n * 1024, 1536] fp32 -> t32 (high halves into xs[nxt].hi, overwritten by proj_attn)
-    const VaeConv& qkv = convs.at(a + "qkv");
-    if (conv(qkv, {{nrm, -1}}, {ConvTap{0, 0, 0}}, -1, 32, n, xs[nxt].hi, nullptr, t32, nullptr, st)) return -1;
+    const SplitConv& qkv = convs.at(a + "qkv");
+    if (conv(qkv, {{nrm, -1}}, {ConvTap{0, 0, 0}}, nullptr, 32, n, false, nullptr, xs[nxt].hi, nullptr, t32, st))
+      return -1;
     // S = q k^T / sqrt(512) -> x32[nxt] (overwritten by proj_attn), softmax over keys in place
     float* S = x32[nxt];
     vae_attn_gemm_kernel<true, false><<<dim3(16, 16, n), 256, 0, st>>>(
@@ -611,8 +574,8 @@ struct VaeEngine {
     NOPE_CUDA(cudaGetLastError());
     launches += 3;
     // x + proj_attn(O)
-    if (conv(convs.at(a + "proj_attn"), {{nrm, -1}}, {ConvTap{0, 0, 0}}, -1, 32, n, xs[nxt].hi, xs[nxt].lo,
-             x32[nxt], &xs[cur], st))
+    if (conv(convs.at(a + "proj_attn"), {{nrm, -1}}, {ConvTap{0, 0, 0}}, nullptr, 32, n, false, &xs[cur], xs[nxt].hi,
+             xs[nxt].lo, x32[nxt], st))
       return -1;
     cur = nxt;
     return 0;
@@ -641,66 +604,91 @@ struct VaeEngine {
 
 }  // namespace nope
 
+
 // ---------------------------------------------------------------- encoder (DESIGN.md section 16)
-struct nope_vae : nope::VaeEngine {
+struct nope_vae final : nope::VaeEngine {
   static constexpr const char* kName = "VAE";
   static constexpr int kChunk = 16;           // images per pass: the workspace holds this many (~200 MB each)
-  static constexpr int kCh[4] = {128, 256, 512, 512};
   float *in_w = nullptr, *in_b = nullptr;
   float* rot_stage = nullptr;                 // kChunk rotated crops, allocated by the first rotated encode
   size_t out_floats() const { return 4 * 32 * 32; }   // per encoded image
 
   nope_vae() : VaeEngine(kChunk) {}
 
-  void build_schema() {
-    expect_conv("encoder.conv_in", 128, 3, 3);
-    int cin = 128;
+  void build_plan() {
+    const int ch[4] = {128, 256, 512, 512};
+    plan = {{"encoder.conv_in", kConvIn, 3, 256, 128, 256}};
+    int cin = 128, H = 256;
     for (int i = 0; i < 4; ++i) {
+      const std::string blk = "encoder.down_blocks." + std::to_string(i);
       for (int j = 0; j < 2; ++j) {
-        expect_resnet("encoder.down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), cin, kCh[i]);
-        cin = kCh[i];
+        plan.push_back({blk + ".resnets." + std::to_string(j), kResnet, cin, H, ch[i], H});
+        cin = ch[i];
       }
-      if (i < 3) expect_conv("encoder.down_blocks." + std::to_string(i) + ".downsamplers.0.conv", kCh[i], kCh[i], 3);
+      if (i < 3) {
+        plan.push_back({blk + ".downsamplers.0", kDown, cin, H, cin, H / 2});
+        H /= 2;
+      }
     }
-    for (int j = 0; j < 2; ++j) expect_resnet("encoder.mid_block.resnets." + std::to_string(j), 512, 512);
-    expect_attention("encoder.mid_block.attentions.0.");
-    expect_norm("encoder.conv_norm_out", 512);
-    expect_conv("encoder.conv_out", 8, 512, 3);
-    expect_conv("quant_conv", 8, 8, 1);
+    plan.push_back({"encoder.mid_block.resnets.0", kResnet, 512, 32, 512, 32});
+    plan.push_back({"encoder.mid_block.attentions.0", kAttention, 512, 32, 512, 32});
+    plan.push_back({"encoder.mid_block.resnets.1", kResnet, 512, 32, 512, 32});
+    // conv_norm_out + SiLU + conv_out + quant_conv's mean x 0.18215
+    plan.push_back({"encoder.conv_out", kConvOut, 512, 32, 4, 32});
+  }
+
+  void build_schema() {
+    for (const nope::ImageModule& m : plan) {
+      if (m.kind == kConvIn) {
+        expect_conv(m.name, m.Co, m.Ci, 3);
+      } else if (m.kind == kResnet) {
+        expect_resnet(m.name, m.Ci, m.Co);
+      } else if (m.kind == kDown) {
+        expect_conv(m.name + ".conv", m.Co, m.Ci, 3);
+      } else if (m.kind == kAttention) {
+        expect_attention(m.name + ".");
+      } else {
+        expect_norm("encoder.conv_norm_out", 512);
+        expect_conv("encoder.conv_out", 8, 512, 3);
+        expect_conv("quant_conv", 8, 8, 1);
+      }
+    }
+  }
+
+  // conv_out followed by quant_conv rows 0-3 (the mean) and the 0.18215 scale, folded in float64
+  int make_conv_out() {
+    const auto W = dvec("encoder.conv_out.weight"), b = dvec("encoder.conv_out.bias");
+    const auto Q = dvec("quant_conv.weight"), qb = dvec("quant_conv.bias");
+    constexpr double kScale = 0.18215;
+    std::vector<double> Wf((size_t)4 * 512 * 9, 0.0), bf(4, 0.0);
+    for (int o = 0; o < 4; ++o) {
+      double bo = qb[o];
+      for (int j = 0; j < 8; ++j) {
+        bo += Q[o * 8 + j] * b[j];
+        for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] += Q[o * 8 + j] * W[(size_t)j * 512 * 9 + i];
+      }
+      bf[o] = kScale * bo;
+      for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] *= kScale;
+    }
+    return pack_conv("conv_out", 4, 512, 3, Wf, bf);
   }
 
   // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
   int finalize() {
-    using namespace nope;
-    if (mem.upload(&in_w, h("encoder.conv_in.weight")) || mem.upload(&in_b, h("encoder.conv_in.bias"))) return -1;
-    int cin = 128;
-    for (int i = 0; i < 4; ++i) {
-      const std::string blk = "encoder.down_blocks." + std::to_string(i);
-      for (int j = 0; j < 2; ++j) {
-        if (make_resnet(blk + ".resnets." + std::to_string(j), cin, kCh[i])) return -1;
-        cin = kCh[i];
+    for (const nope::ImageModule& m : plan) {
+      int rc = 0;
+      if (m.kind == kConvIn) {
+        rc = mem.upload(&in_w, h(m.name + ".weight")) || mem.upload(&in_b, h(m.name + ".bias"));
+      } else if (m.kind == kResnet) {
+        rc = make_resnet(m.name, m.Ci, m.Co);
+      } else if (m.kind == kDown) {
+        rc = make_plain(m.name + ".conv", 3);
+      } else if (m.kind == kAttention) {
+        rc = make_attention(m.name + ".");
+      } else {
+        rc = make_norm("encoder.conv_norm_out") || make_conv_out();
       }
-      if (i < 3 && make_plain(blk + ".downsamplers.0.conv", 3)) return -1;
-    }
-    for (int j = 0; j < 2; ++j)
-      if (make_resnet("encoder.mid_block.resnets." + std::to_string(j), 512, 512)) return -1;
-    if (make_attention("encoder.mid_block.attentions.0.")) return -1;
-    if (make_norm("encoder.conv_norm_out")) return -1;
-    {  // conv_out followed by quant_conv rows 0-3 (the mean) and the 0.18215 scale, folded in float64
-      const auto W = dvec("encoder.conv_out.weight"), b = dvec("encoder.conv_out.bias");
-      const auto Q = dvec("quant_conv.weight"), qb = dvec("quant_conv.bias");
-      constexpr double kScale = 0.18215;
-      std::vector<double> Wf((size_t)4 * 512 * 9, 0.0), bf(4, 0.0);
-      for (int o = 0; o < 4; ++o) {
-        double bo = qb[o];
-        for (int j = 0; j < 8; ++j) {
-          bo += Q[o * 8 + j] * b[j];
-          for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] += Q[o * 8 + j] * W[(size_t)j * 512 * 9 + i];
-        }
-        bf[o] = kScale * bo;
-        for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] *= kScale;
-      }
-      if (pack_conv("conv_out", 4, 512, 3, Wf, bf)) return -1;
+      if (rc) return -1;
     }
     // workspace for kChunk images of the 256 x 256 x 128 level
     return alloc_workspace((size_t)kChunk * 256 * 256 * 128);
@@ -709,7 +697,7 @@ struct nope_vae : nope::VaeEngine {
   // Downsample2D: pad (0, 1, 0, 1) + 3x3 stride 2 from side 2H to H.  Tap (ky, kx) reads input (2y + ky, 2x + kx):
   // sub-lattice (ky & 1, kx & 1) at offset (ky >> 1, kx >> 1); the bottom / right zero padding is the TMA's
   // out-of-bounds fill of offset 1.  The 256 x 256 input's sub-lattices are its planes.
-  int downsample(const nope::VaeConv& L, const nope::ActPair& in, int Hin, int n, const nope::ActPair& out,
+  int downsample(const nope::SplitConv& L, const nope::ActPair& in, int Hin, int n, const nope::ActPair& out,
                  float* out_f32, cudaStream_t st) {
     using namespace nope;
     const int H = Hin / 2;
@@ -724,97 +712,39 @@ struct nope_vae : nope::VaeEngine {
     std::vector<ConvTap> taps;
     for (int ky = 0; ky < 3; ++ky)
       for (int kx = 0; kx < 3; ++kx) taps.push_back(stride2_tap(ky, kx));
-    return conv(L, src, taps, -1, H, n, out.hi, out.lo, out_f32, nullptr, st);
+    return conv(L, src, taps, nullptr, H, n, false, nullptr, out.hi, out.lo, out_f32, st);
+  }
+
+  int run(const nope::ImageModule& m, int n, int& cur, const float* images, cudaStream_t st) override {
+    using namespace nope;
+    switch (m.kind) {
+      case kConvIn:
+        vae_conv_in_kernel<<<n * 65536 / 2, 256, 0, st>>>(images, in_w, in_b, x32[0], xs[0].hi, xs[0].lo, n, cap);
+        NOPE_CUDA(cudaGetLastError());
+        cur = 0;
+        return 0;
+      case kResnet:
+        return resnet(m.name, m.Ci, m.Co, m.Hi, n, cur, st);
+      case kDown:
+        if (downsample(convs.at(m.name + ".conv"), xs[cur], m.Hi, n, xs[1 - cur], x32[1 - cur], st)) return -1;
+        cur = 1 - cur;
+        return 0;
+      case kAttention:
+        return attention(m.name + ".", n, cur, st);
+      default:
+        if (group_norm("encoder.conv_norm_out", x32[cur], 512, 32, n, true, st)) return -1;
+        return conv3(convs.at("conv_out"), nrm, 32, n, xs[1 - cur], false, t32, nullptr, nullptr, st);
+    }
+  }
+  int extract_output(int n, float* out, cudaStream_t st) override {
+    nope::enc_extract_kernel<<<nope::ew_grid((long long)n * 4 * 1024), 256, 0, st>>>(t32, out, n, 4, 1024,
+                                                                                     convs.at("conv_out").cout);
+    NOPE_CUDA(cudaGetLastError());
+    return 0;
   }
 
   // n <= kChunk images [n, 3, 256, 256] -> out [n, 4, 32, 32]
-  int encode(const float* images, int n, float* out, cudaStream_t st) {
-    using namespace nope;
-    launches = 0;
-    vae_conv_in_kernel<<<n * 65536 / 2, 256, 0, st>>>(images, in_w, in_b, x32[0], xs[0].hi, xs[0].lo, n, kChunk);
-    NOPE_CUDA(cudaGetLastError());
-    ++launches;
-    int cur = 0, H = 256, cin = 128;
-    for (int i = 0; i < 4; ++i) {
-      const std::string blk = "encoder.down_blocks." + std::to_string(i);
-      for (int j = 0; j < 2; ++j) {
-        if (resnet(blk + ".resnets." + std::to_string(j), cin, kCh[i], H, n, cur, st)) return -1;
-        cin = kCh[i];
-      }
-      if (i < 3) {
-        if (downsample(convs.at(blk + ".downsamplers.0.conv"), xs[cur], H, n, xs[1 - cur], x32[1 - cur], st))
-          return -1;
-        cur = 1 - cur;
-        H /= 2;
-      }
-    }
-    if (resnet("encoder.mid_block.resnets.0", 512, 512, 32, n, cur, st)) return -1;
-    if (attention("encoder.mid_block.attentions.0.", n, cur, st)) return -1;
-    if (resnet("encoder.mid_block.resnets.1", 512, 512, 32, n, cur, st)) return -1;
-    if (group_norm("encoder.conv_norm_out", x32[cur], 512, 32, n, true, st)) return -1;
-    const VaeConv& co = convs.at("conv_out");
-    if (conv3(co, nrm, 32, n, xs[1 - cur], false, t32, nullptr, nullptr, st)) return -1;
-    enc_extract_kernel<<<ew_grid((long long)n * 4 * 1024), 256, 0, st>>>(t32, out, n, 4, 1024, co.cout);
-    NOPE_CUDA(cudaGetLastError());
-    ++launches;
-    return 0;
-  }
-
-  // Runs one module of encode() on its own (nope_vae_run_block): x [n, C, H, H] fp32 NCHW (images for conv_in)
-  // staged as the residual stream -> out: the fp32 stream after the module, out_pair (nullable): its (hi, lo) pair
-  // as hi + lo.  "encoder.conv_out" is conv_norm_out + SiLU + conv_out + quant_conv's mean x 0.18215 and has no pair.
-  int run_block(const std::string& name, const float* x, int C, int H, int n, float* out, float* out_pair,
-                int64_t cap_floats, cudaStream_t st) {
-    using namespace nope;
-    enum { kResnet, kDown, kAttention, kIn, kOut } kind = kResnet;
-    int Ci = 0, Hi = 0, Co = 0, Ho = 0;
-    if (name == "encoder.conv_in") {
-      kind = kIn, Ci = 3, Hi = 256, Co = 128, Ho = 256;
-    } else if (name == "encoder.conv_out") {
-      kind = kOut, Ci = 512, Hi = 32, Co = 4, Ho = 32;
-    } else if (name == "encoder.mid_block.attentions.0") {
-      kind = kAttention, Ci = Co = 512, Hi = Ho = 32;
-    } else if (name == "encoder.mid_block.resnets.0" || name == "encoder.mid_block.resnets.1") {
-      Ci = Co = 512, Hi = Ho = 32;
-    } else {
-      int cin = 128;
-      for (int i = 0; i < 4; ++i) {
-        const std::string blk = "encoder.down_blocks." + std::to_string(i);
-        for (int j = 0; j < 2; ++j) {
-          if (name == blk + ".resnets." + std::to_string(j)) Ci = cin, Co = kCh[i], Hi = Ho = 256 >> i;
-          cin = kCh[i];
-        }
-        if (i < 3 && name == blk + ".downsamplers.0") kind = kDown, Ci = Co = kCh[i], Hi = 256 >> i, Ho = Hi / 2;
-      }
-    }
-    if (check_block(name, kChunk, C, H, n, Ci, Hi, Co, Ho, cap_floats)) return -1;
-    NOPE_CHECK(!out_pair || kind != kOut, "run_block: encoder.conv_out has no (hi, lo) output");
-    launches = 0;
-    int cur = 0;
-    if (kind == kIn) {
-      vae_conv_in_kernel<<<n * 65536 / 2, 256, 0, st>>>(x, in_w, in_b, x32[0], xs[0].hi, xs[0].lo, n, kChunk);
-      NOPE_CUDA(cudaGetLastError());
-    } else if (stage_stream(x, C, H, n, st)) {
-      return -1;
-    }
-    if (kind == kResnet) {
-      if (resnet(name, Ci, Co, H, n, cur, st)) return -1;
-    } else if (kind == kAttention) {
-      if (attention(name + ".", n, cur, st)) return -1;
-    } else if (kind == kDown) {
-      if (downsample(convs.at(name + ".conv"), xs[cur], H, n, xs[1 - cur], x32[1 - cur], st)) return -1;
-      cur = 1 - cur;
-    } else if (kind == kOut) {
-      if (group_norm("encoder.conv_norm_out", x32[cur], 512, 32, n, true, st)) return -1;
-      const VaeConv& co = convs.at("conv_out");
-      if (conv3(co, nrm, 32, n, xs[1 - cur], false, t32, nullptr, nullptr, st)) return -1;
-      enc_extract_kernel<<<ew_grid((long long)n * 4 * 1024), 256, 0, st>>>(t32, out, n, 4, 1024, co.cout);
-      NOPE_CUDA(cudaGetLastError());
-    }
-    if (kind != kOut && extract_stream(cur, Co, Ho, n, out, out_pair, st)) return -1;
-    NOPE_CUDA(cudaStreamSynchronize(st));
-    return 0;
-  }
+  int encode(const float* images, int n, float* out, cudaStream_t st) { return forward(images, n, out, st); }
 };
 
 // ---------------------------------------------------------------- decoder (DESIGN.md section 17)
@@ -822,34 +752,53 @@ struct nope_vae : nope::VaeEngine {
 // (4 -> 512); the mid block at 32 x 32; four up blocks of three ResnetBlock2D (512, 512, 256, 128 channels; blocks 0-2
 // end in Upsample2D, nearest x2 + 3x3 conv); GroupNorm(32) + SiLU and conv_out 3x3 (128 -> 3).  Up block 3 runs at
 // the parity-planar 256 x 256 level; the 64 x 64 and 128 x 128 levels are plain NHWC, as in the encoder.
-struct nope_vae_decoder : nope::VaeEngine {
+struct nope_vae_decoder final : nope::VaeEngine {
   static constexpr const char* kName = "VAE decoder";
   static constexpr int kChunk = 8;            // images per pass: 256 x 256 x 256 is 67 MB of fp32 per image
-  static constexpr int kCh[4] = {512, 512, 256, 128};
-  static constexpr const char* kAttn = "decoder.mid_block.attentions.0.";
   float *in_w = nullptr, *in_b = nullptr, *pq_w = nullptr, *pq_b = nullptr;
   size_t out_floats() const { return 3 * 256 * 256; }   // per decoded image
 
   nope_vae_decoder() : VaeEngine(kChunk) {}
 
-  static std::string up(int i) { return "decoder.up_blocks." + std::to_string(i); }
+  // "decoder.conv_in" is post_quant_conv with 1 / 0.18215, then conv_in, on latents [n, 4, 32, 32];
+  // "decoder.conv_out" is conv_norm_out + SiLU + conv_out, giving images [n, 3, 256, 256]
+  void build_plan() {
+    const int ch[4] = {512, 512, 256, 128};
+    plan = {{"decoder.conv_in", kConvIn, 4, 32, 512, 32}};
+    plan.push_back({"decoder.mid_block.resnets.0", kResnet, 512, 32, 512, 32});
+    plan.push_back({"decoder.mid_block.attentions.0", kAttention, 512, 32, 512, 32});
+    plan.push_back({"decoder.mid_block.resnets.1", kResnet, 512, 32, 512, 32});
+    int cin = 512, H = 32;
+    for (int i = 0; i < 4; ++i) {
+      const std::string blk = "decoder.up_blocks." + std::to_string(i);
+      for (int j = 0; j < 3; ++j) {
+        plan.push_back({blk + ".resnets." + std::to_string(j), kResnet, cin, H, ch[i], H});
+        cin = ch[i];
+      }
+      if (i < 3) {
+        plan.push_back({blk + ".upsamplers.0", kUp, cin, H, cin, 2 * H});
+        H *= 2;
+      }
+    }
+    plan.push_back({"decoder.conv_out", kConvOut, 128, 256, 3, 256});
+  }
 
   void build_schema() {
-    expect_conv("post_quant_conv", 4, 4, 1);
-    expect_conv("decoder.conv_in", 512, 4, 3);
-    expect_resnet("decoder.mid_block.resnets.0", 512, 512);
-    expect_attention(kAttn);
-    expect_resnet("decoder.mid_block.resnets.1", 512, 512);
-    int cin = 512;
-    for (int i = 0; i < 4; ++i) {
-      for (int j = 0; j < 3; ++j) {
-        expect_resnet(up(i) + ".resnets." + std::to_string(j), cin, kCh[i]);
-        cin = kCh[i];
+    for (const nope::ImageModule& m : plan) {
+      if (m.kind == kConvIn) {
+        expect_conv("post_quant_conv", 4, 4, 1);
+        expect_conv(m.name, m.Co, m.Ci, 3);
+      } else if (m.kind == kResnet) {
+        expect_resnet(m.name, m.Ci, m.Co);
+      } else if (m.kind == kAttention) {
+        expect_attention(m.name + ".");
+      } else if (m.kind == kUp) {
+        expect_conv(m.name + ".conv", m.Co, m.Ci, 3);
+      } else {
+        expect_norm("decoder.conv_norm_out", m.Ci);
+        expect_conv(m.name, m.Co, m.Ci, 3);
       }
-      if (i < 3) expect_conv(up(i) + ".upsamplers.0.conv", kCh[i], kCh[i], 3);
     }
-    expect_norm("decoder.conv_norm_out", 128);
-    expect_conv("decoder.conv_out", 3, 128, 3);
   }
 
   // Upsample2D's 3x3 kernel folded into one 2x2 kernel per output parity (py, px), in float64.  Output row 2 Y + py
@@ -874,26 +823,26 @@ struct nope_vae_decoder : nope::VaeEngine {
 
   // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
   int finalize() {
-    using namespace nope;
-    {  // post_quant_conv with the 1 / 0.18215 scale folded into its weight in float64; its bias stays separate
-      const auto W = dvec("post_quant_conv.weight");
-      std::vector<float> w(16);
-      for (int i = 0; i < 16; ++i) w[i] = (float)(W[i] / 0.18215);
-      if (mem.upload(&pq_w, w) || mem.upload(&pq_b, h("post_quant_conv.bias"))) return -1;
-    }
-    if (mem.upload(&in_w, h("decoder.conv_in.weight")) || mem.upload(&in_b, h("decoder.conv_in.bias"))) return -1;
-    if (make_resnet("decoder.mid_block.resnets.0", 512, 512) || make_attention(kAttn) ||
-        make_resnet("decoder.mid_block.resnets.1", 512, 512))
-      return -1;
-    int cin = 512;
-    for (int i = 0; i < 4; ++i) {
-      for (int j = 0; j < 3; ++j) {
-        if (make_resnet(up(i) + ".resnets." + std::to_string(j), cin, kCh[i], i == 3)) return -1;
-        cin = kCh[i];
+    for (const nope::ImageModule& m : plan) {
+      int rc = 0;
+      if (m.kind == kConvIn) {
+        // post_quant_conv with the 1 / 0.18215 scale folded into its weight in float64; its bias stays separate
+        const auto W = dvec("post_quant_conv.weight");
+        std::vector<float> w(16);
+        for (int i = 0; i < 16; ++i) w[i] = (float)(W[i] / 0.18215);
+        rc = mem.upload(&pq_w, w) || mem.upload(&pq_b, h("post_quant_conv.bias")) ||
+             mem.upload(&in_w, h(m.name + ".weight")) || mem.upload(&in_b, h(m.name + ".bias"));
+      } else if (m.kind == kResnet) {
+        rc = make_resnet(m.name, m.Ci, m.Co, m.Hi == 256);
+      } else if (m.kind == kAttention) {
+        rc = make_attention(m.name + ".");
+      } else if (m.kind == kUp) {
+        rc = make_upsample(m.name + ".conv", m.Co);
+      } else {
+        rc = make_norm("decoder.conv_norm_out") || make_plain(m.name, 3);
       }
-      if (i < 3 && make_upsample(up(i) + ".upsamplers.0.conv", kCh[i])) return -1;
+      if (rc) return -1;
     }
-    if (make_norm("decoder.conv_norm_out") || make_plain("decoder.conv_out", 3)) return -1;
     // workspace for kChunk images of the 256 x 256 x 256 level (the same 3.2 GB as the encoder's)
     return alloc_workspace((size_t)kChunk * 256 * 256 * 256);
   }
@@ -914,8 +863,8 @@ struct nope_vae_decoder : nope::VaeEngine {
       const size_t o = (size_t)q * cap * H * H * C;
       float* f = (planar ? x32[nxt] : t32) + o;
       const ActPair d = planar ? ActPair{xs[nxt].hi + o, xs[nxt].lo + o} : ActPair{nrm.hi + o, nrm.lo + o};
-      if (conv(convs.at(name + ".p" + std::to_string(q)), {{xs[cur], -1}}, taps, -1, H, n, d.hi, d.lo, f, nullptr,
-               st))
+      if (conv(convs.at(name + ".p" + std::to_string(q)), {{xs[cur], -1}}, taps, nullptr, H, n, false, nullptr, d.hi,
+               d.lo, f, st))
         return -1;
     }
     if (!planar) {
@@ -928,87 +877,33 @@ struct nope_vae_decoder : nope::VaeEngine {
     return 0;
   }
 
-  // n <= kChunk latents [n, 4, 32, 32] -> images out [n, 3, 256, 256] (unclamped)
-  int decode(const float* z, int n, float* out, cudaStream_t st) {
+  int run(const nope::ImageModule& m, int n, int& cur, const float* latents, cudaStream_t st) override {
     using namespace nope;
-    launches = 0;
-    vae_dec_conv_in_kernel<<<dim3(32, n, 2), 256, 0, st>>>(z, pq_w, pq_b, in_w, in_b, x32[0], xs[0].hi, xs[0].lo);
-    NOPE_CUDA(cudaGetLastError());
-    ++launches;
-    int cur = 0, H = 32, cin = 512;
-    if (resnet("decoder.mid_block.resnets.0", 512, 512, 32, n, cur, st) || attention(kAttn, n, cur, st) ||
-        resnet("decoder.mid_block.resnets.1", 512, 512, 32, n, cur, st))
-      return -1;
-    for (int i = 0; i < 4; ++i) {
-      for (int j = 0; j < 3; ++j) {
-        if (resnet(up(i) + ".resnets." + std::to_string(j), cin, kCh[i], H, n, cur, st)) return -1;
-        cin = kCh[i];
-      }
-      if (i < 3) {
-        if (upsample(up(i) + ".upsamplers.0.conv", kCh[i], H, n, cur, st)) return -1;
-        H *= 2;
-      }
+    switch (m.kind) {
+      case kConvIn:
+        vae_dec_conv_in_kernel<<<dim3(32, n, 2), 256, 0, st>>>(latents, pq_w, pq_b, in_w, in_b, x32[0], xs[0].hi,
+                                                               xs[0].lo);
+        NOPE_CUDA(cudaGetLastError());
+        cur = 0;
+        return 0;
+      case kResnet:
+        return resnet(m.name, m.Ci, m.Co, m.Hi, n, cur, st);
+      case kAttention:
+        return attention(m.name + ".", n, cur, st);
+      case kUp:
+        return upsample(m.name + ".conv", m.Co, m.Hi, n, cur, st);
+      default:
+        if (group_norm("decoder.conv_norm_out", x32[cur], 128, 256, n, true, st)) return -1;
+        return conv3(convs.at(m.name), nrm, 256, n, xs[1 - cur], false, t32, nullptr, nullptr, st);
     }
-    if (group_norm("decoder.conv_norm_out", x32[cur], 128, 256, n, true, st)) return -1;
-    const VaeConv& co = convs.at("decoder.conv_out");
-    if (conv3(co, nrm, 256, n, xs[1 - cur], false, t32, nullptr, nullptr, st)) return -1;
-    vae_dec_extract_kernel<<<ew_grid((long long)n * 3 * 65536), 256, 0, st>>>(t32, co.cout, cap, n, out);
+  }
+  int extract_output(int n, float* out, cudaStream_t st) override {
+    nope::vae_dec_extract_kernel<<<nope::ew_grid((long long)n * 3 * 65536), 256, 0, st>>>(
+        t32, convs.at("decoder.conv_out").cout, cap, n, out);
     NOPE_CUDA(cudaGetLastError());
-    ++launches;
     return 0;
   }
 
-  // Runs one module of decode() on its own (nope_vae_decoder_run_block), as nope_vae::run_block: "decoder.conv_in"
-  // (post_quant_conv with 1 / 0.18215, then conv_in) takes latents [n, 4, 32, 32]; "decoder.conv_out"
-  // (conv_norm_out + SiLU + conv_out) gives images [n, 3, 256, 256] and has no pair.
-  int run_block(const std::string& name, const float* x, int C, int H, int n, float* out, float* out_pair,
-                int64_t cap_floats, cudaStream_t st) {
-    using namespace nope;
-    enum { kResnet, kUp, kAttention, kIn, kOut } kind = kResnet;
-    int Ci = 0, Hi = 0, Co = 0, Ho = 0;
-    if (name == "decoder.conv_in") {
-      kind = kIn, Ci = 4, Hi = 32, Co = 512, Ho = 32;
-    } else if (name == "decoder.conv_out") {
-      kind = kOut, Ci = 128, Hi = 256, Co = 3, Ho = 256;
-    } else if (name + "." == kAttn) {
-      kind = kAttention, Ci = Co = 512, Hi = Ho = 32;
-    } else if (name == "decoder.mid_block.resnets.0" || name == "decoder.mid_block.resnets.1") {
-      Ci = Co = 512, Hi = Ho = 32;
-    } else {
-      int cin = 512;
-      for (int i = 0; i < 4; ++i) {
-        for (int j = 0; j < 3; ++j) {
-          if (name == up(i) + ".resnets." + std::to_string(j)) Ci = cin, Co = kCh[i], Hi = Ho = 32 << i;
-          cin = kCh[i];
-        }
-        if (i < 3 && name == up(i) + ".upsamplers.0") kind = kUp, Ci = Co = kCh[i], Hi = 32 << i, Ho = 2 * Hi;
-      }
-    }
-    if (check_block(name, kChunk, C, H, n, Ci, Hi, Co, Ho, cap_floats)) return -1;
-    NOPE_CHECK(!out_pair || kind != kOut, "run_block: decoder.conv_out has no (hi, lo) output");
-    launches = 0;
-    int cur = 0;
-    if (kind == kIn) {
-      vae_dec_conv_in_kernel<<<dim3(32, n, 2), 256, 0, st>>>(x, pq_w, pq_b, in_w, in_b, x32[0], xs[0].hi, xs[0].lo);
-      NOPE_CUDA(cudaGetLastError());
-    } else if (stage_stream(x, C, H, n, st)) {
-      return -1;
-    }
-    if (kind == kResnet) {
-      if (resnet(name, Ci, Co, H, n, cur, st)) return -1;
-    } else if (kind == kAttention) {
-      if (attention(kAttn, n, cur, st)) return -1;
-    } else if (kind == kUp) {
-      if (upsample(name + ".conv", Co, H, n, cur, st)) return -1;
-    } else if (kind == kOut) {
-      if (group_norm("decoder.conv_norm_out", x32[cur], 128, 256, n, true, st)) return -1;
-      const VaeConv& co = convs.at("decoder.conv_out");
-      if (conv3(co, nrm, 256, n, xs[1 - cur], false, t32, nullptr, nullptr, st)) return -1;
-      vae_dec_extract_kernel<<<ew_grid((long long)n * 3 * 65536), 256, 0, st>>>(t32, co.cout, cap, n, out);
-      NOPE_CUDA(cudaGetLastError());
-    }
-    if (kind != kOut && extract_stream(cur, Co, Ho, n, out, out_pair, st)) return -1;
-    NOPE_CUDA(cudaStreamSynchronize(st));
-    return 0;
-  }
+  // n <= kChunk latents [n, 4, 32, 32] -> images out [n, 3, 256, 256] (unclamped)
+  int decode(const float* z, int n, float* out, cudaStream_t st) { return forward(z, n, out, st); }
 };
