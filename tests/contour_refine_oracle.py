@@ -83,14 +83,32 @@ def contour(D):
     return out
 
 
-def accumulate(D, phi, K4, t, tau, rho):
+def visible(mask, occ):
+    """M' = M n U, bool: the mask's pixels outside the occluder mask occ (nonzero = something may be in front)"""
+    return (np.asarray(mask) != 0) & (np.asarray(occ) == 0)
+
+
+def known4(occ):
+    """bool [H, W]: the pixel and its four neighbours lie in U = not occ (the frame's border pixels are never contour
+    pixels)"""
+    u = np.asarray(occ) == 0
+    out = u.copy()
+    out[1:] &= u[:-1]
+    out[:-1] &= u[1:]
+    out[:, 1:] &= u[:, :-1]
+    out[:, :-1] &= u[:, 1:]
+    return out
+
+
+def accumulate(D, phi, K4, t, tau, rho, occ=None):
     """-> (int64 [29] sums, n_contour) of one render D [H, W] against the mask's phi [H, W] at the pixel tolerance tau:
-    the 21 entries of the upper triangle of J J^T row by row, the 6 of J e, e^2 and the pair count"""
+    the 21 entries of the upper triangle of J J^T row by row, the 6 of J e, e^2 and the pair count.  With an occluder
+    mask occ, a contour pixel is counted and paired only when it and its four neighbours lie in U (known4)."""
     D = np.asarray(D, dtype=np.float32).astype(np.float64)
     phi = np.asarray(phi, dtype=np.float64)
     tau, rho = np.float64(tau), np.float64(rho)
     fx, fy = np.float64(K4[0]), np.float64(K4[1])
-    cont = contour(D)
+    cont = contour(D) if occ is None else contour(D) & known4(occ)
     n_contour = int(cont.sum())
     r, c = np.nonzero(cont)
     e = phi[r, c] + 0.5
@@ -122,30 +140,35 @@ def solve(sums, R, t, tau, K4, rho):
     return dro.solve(sums, R, t, np.float64(tau) * kappa(t[2], K4), rho)
 
 
-def iou(D, mask):
-    """|S n M| / |S u M| of the render's silhouette and the mask; NaN for a mask without a contour"""
+def iou(D, mask, occ=None):
+    """|S n M| / |S u M| of the render's silhouette and the mask; NaN for a mask without a contour.  With an occluder
+    mask occ: |S' n M'| / |S' u M'| of both restricted to U."""
     m = np.asarray(mask) != 0
+    if occ is not None:
+        D, m = np.where(np.asarray(occ) != 0, 0, np.asarray(D)), visible(mask, occ)
     if not m.any() or m.all():
         return np.nan
     return to.iou(to.stats(np.asarray(D) > 0, m), to.stats(m))
 
 
-def refine(render, R, t, mask, K4, taus, rho, phi=None):
+def refine(render, R, t, mask, K4, taus, rho, phi=None, occ=None):
     """-> (R, t, fit [4] = (n_in, n_contour, rms, iou), sums [29]) after len(taus) - 1 updates of one hypothesis,
-    iteration i pairing at taus[i] times the mask's box size"""
+    iteration i pairing at taus[i] times the mask's box size.  Under an occluder mask occ, phi and the box size are
+    those of M' = visible(mask, occ), and accumulate and iou leave the occluded pixels out."""
     R = np.array(R, dtype=np.float64)
     t = np.array(t, dtype=np.float64)
-    phi = sdf(mask) if phi is None else phi
-    s = box_size(mask)
+    mv = mask if occ is None else visible(mask, occ)
+    phi = sdf(mv) if phi is None else phi
+    s = box_size(mv)
     iters = len(taus) - 1
     for i in range(iters):
         tau = np.float64(taus[i]) * s
-        sums, _ = accumulate(render(R, t), phi, K4, t, tau, rho)
+        sums, _ = accumulate(render(R, t), phi, K4, t, tau, rho, occ)
         R, t = solve(sums, R, t, tau, K4, rho)
     D = render(R, t)
     tau = np.float64(taus[iters]) * s
-    sums, nc = accumulate(D, phi, K4, t, tau, rho)
+    sums, nc = accumulate(D, phi, K4, t, tau, rho, occ)
     nin = float(int(sums[NSUMS - 1]))
     with np.errstate(invalid="ignore", divide="ignore"):
         rms = tau * np.sqrt(np.float64(dro.unfix(sums[NSUMS - 2])) / np.float64(nin))
-    return R, t, np.array([nin, float(nc), rms, iou(D, mask)]), sums
+    return R, t, np.array([nin, float(nc), rms, iou(D, mask, occ)]), sums

@@ -21,13 +21,8 @@ latent for encoder.conv_out)."""
 import torch
 import torch.nn.functional as F
 
-ENC_MODULES = (["stem"] + [f"backbone.layer{l}.{b}" for l, n in ((1, 3), (2, 4), (3, 6), (4, 3)) for b in range(n)]
-               + ["projector"])
-VAE_MODULES = (["encoder.conv_in"]
-               + [m for i in range(4) for m in [f"encoder.down_blocks.{i}.resnets.{j}" for j in range(2)]
-                  + ([f"encoder.down_blocks.{i}.downsamplers.0"] if i < 3 else [])]
-               + ["encoder.mid_block.resnets.0", "encoder.mid_block.attentions.0", "encoder.mid_block.resnets.1",
-                  "encoder.conv_out"])
+from _util import ENC_MODULES, VAE_MODULES, mixed_images
+
 _ATTN = "encoder.mid_block.attentions.0."
 
 
@@ -201,9 +196,7 @@ def predict(n_images=4, seed=70):
     sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
     from oracle import unet_oracle, vae_oracle, weights
     from nope_b200.synth_weights import make_vae_state_dict
-    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-    from test_vae_gpu import _crop_like, _uniform
-    x = torch.cat([_uniform(seed, n_images - n_images // 2), _crop_like(seed, n_images // 2)])
+    x = mixed_images(n_images, seed)
     out = {}
     full = weights.make_full_state_dict(seed=0)
     enc_sd = {k[len("encoder."):]: v for k, v in full.items()

@@ -32,6 +32,22 @@ def test_exports_match_header():
     assert set(names) == set(_lib.SIGNATURES), set(names) ^ set(_lib.SIGNATURES)
 
 
+# the entry points each feature added, by feature: every one is declared, bound and exported
+ENTRY_POINTS = ["nope_crop_frames", "nope_crop_camera", "nope_crop_rotate", "nope_render_depth", "nope_vsd_error",
+                "nope_pose_cells_expand", "nope_pose_cells_rank", "nope_pose_refine_propose", "nope_pose_refine_select",
+                "nope_inplane_rotate", "nope_encoder_encode_inplane", "nope_inplane_rotate_pairs",
+                "nope_encoder_encode_rotated", "nope_pose_refine_inplane_propose", "nope_pose_refine_inplane_select",
+                "nope_unet_sweep_multi", "nope_ldm_sweep_multi", "nope_score_topk_multi"]
+
+
+@pytest.mark.parametrize("name", ENTRY_POINTS)
+def test_entry_point_is_declared_bound_and_exported(name):
+    from nope_b200 import _lib
+    lib = _lib.load()
+    assert name in _declared() and name in _lib.SIGNATURES and hasattr(lib, name)
+    assert lib.nope_abi_version() == 3
+
+
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):
     from nope_b200 import _lib
     monkeypatch.setattr(_lib, "_lib", None)

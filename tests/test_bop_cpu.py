@@ -6,6 +6,7 @@ import math
 import numpy as np
 import pytest
 
+from _scenes import FLIPS
 from nope_b200 import bop
 from oracle import bop_oracle as bo
 from oracle import render_oracle as ro
@@ -24,7 +25,6 @@ def _pose(rng, z=400.0):
     return np.concatenate([_rot(rng), np.array([[rng.uniform(-30, 30)], [rng.uniform(-30, 30)], [z]])], axis=1)
 
 
-FLIPS = [np.diag([1.0, -1.0, -1.0, 1.0]), np.diag([-1.0, 1.0, -1.0, 1.0]), np.diag([-1.0, -1.0, 1.0, 1.0])]
 CYLINDER = {"diameter": 80.0, "symmetries_discrete": [np.diag([1.0, -1.0, -1.0, 1.0])],
             "symmetries_continuous": [{"axis": np.array([0.0, 0.0, 2.0]), "offset": np.array([1.0, -2.0, 0.0])}]}
 

@@ -9,13 +9,13 @@ import numpy as np
 import pytest
 import torch
 
+from _scenes import FLIPS, K4, tless_batch
+from _util import no_host_sync
 from oracle import bop_oracle as bo
 from oracle import render_oracle as ro
 
 pytestmark = pytest.mark.gpu
 
-K4 = np.array([1075.65091572, 1073.90347929, 360.0, 270.0])
-FLIPS = [np.diag([1.0, -1.0, -1.0, 1.0]), np.diag([-1.0, 1.0, -1.0, 1.0]), np.diag([-1.0, -1.0, 1.0, 1.0])]
 CYL = {"diameter": 80.0, "symmetries_discrete": [np.diag([1.0, -1.0, -1.0, 1.0])],
        "symmetries_continuous": [{"axis": np.array([0.0, 0.0, 1.0]), "offset": np.array([0.0, 0.0, 0.0])}]}
 
@@ -148,12 +148,8 @@ def test_pose_errors_bad_arguments_and_no_sync():
     pts, gt, est, K = _case(8, 100, 2, 2)
     args = (torch.from_numpy(pts).cuda(), torch.from_numpy(est[..., :3]).cuda(), torch.from_numpy(est[..., 3]).cuda(),
             torch.from_numpy(gt[..., :3]).cuda(), torch.from_numpy(gt[..., 3]).cuda())
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         ms, mp = pose_errors(*args, K, _syms(630))
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert np.array_equal(ms.cpu().numpy(), bo.pose_errors(pts, _syms(630), gt, est, K)[0])
     for k in (np.array([[np.nan, 1.0, 0, 0]] * 2), np.array([[0.0, 1.0, 0, 0]] * 2), np.ones((3, 4))):
         with pytest.raises(ValueError):
@@ -224,12 +220,8 @@ def test_multi_tau_bad_arguments_and_no_sync():
     from nope_b200 import _lib
     from nope_b200.vsd import vsd_errors
     dt, dg, de, K = _frames()
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         vsd_errors(dt, dg, de, K, tau=[10.0, 20.0])
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     for taus in ([], list(range(1, 18)), [1.0, 0.0], [np.nan]):
         with pytest.raises(ValueError):
             vsd_errors(dt, dg, de, K, tau=taus)
@@ -245,41 +237,6 @@ def test_multi_tau_bad_arguments_and_no_sync():
 
 
 # ------------------------------------------------------------------ eval_bop end to end
-def _tless_batch(tmp_path, B=3):
-    """as tests/test_vsd_gpu._tless_batch: a 60 x 40 x 30 box as obj_000001.ply, synthetic noisy depth PNGs"""
-    import cv2
-    from nope_b200.poses import icosphere_object_rotations, synthetic_pose_batch
-    from oracle import inputs
-    v, f = ro.box(60.0, 40.0, 30.0)
-    ply = tmp_path / "models"
-    ply.mkdir()
-    with open(ply / "obj_000001.ply", "w") as fh:
-        fh.write(f"ply\nformat ascii 1.0\nelement vertex {len(v)}\nproperty float x\nproperty float y\n"
-                 f"property float z\nelement face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
-        fh.writelines(" ".join(repr(float(x)) for x in p) + "\n" for p in v)
-        fh.writelines("3 " + " ".join(str(int(i)) for i in q) + "\n" for q in f)
-    (ply / "models_info.json").write_text(
-        '{"1": {"diameter": %r, "symmetries_discrete": [%s]}}'
-        % (float(np.linalg.norm([60.0, 40.0, 30.0])),
-           ", ".join("[" + ", ".join(repr(float(x)) for x in m.reshape(-1)) + "]" for m in FLIPS)))
-    rel = synthetic_pose_batch(42, B)[0]
-    tp = torch.from_numpy(icosphere_object_rotations(0)).float()[None].expand(B, -1, -1, -1).contiguous()
-    q, r = inputs.make_images(seed=3, batch=B)
-    K = torch.tensor([[150.0, 0.0, 48.2], [0.0, 151.0, 35.9], [0.0, 0.0, 1.0]], dtype=torch.float64)
-    gtR, paths = tp[torch.arange(B), torch.tensor([3, 17, 30])[:B]], []
-    trans = torch.tensor([[2.0, -3.0, 300.0], [-5.0, 1.0, 280.0], [0.0, 4.0, 320.0]])[:B, :, None]
-    for b in range(B):
-        T = np.eye(4)
-        T[:3, :3], T[:3, 3] = gtR[b].numpy(), trans[b, :, 0].numpy()
-        d = ro.render(v, f, T, K.numpy(), (72, 96))[0].numpy()
-        raw = np.round(d * 10.0 + np.random.default_rng(b).normal(0, 5.0, d.shape) * (d > 0)).clip(0).astype(np.uint16)
-        paths.append(str(tmp_path / f"depth_{b}.png"))
-        assert cv2.imwrite(paths[-1], raw)
-    return {"query": q, "reference": r, "gt_relativeR": rel[:, 0], "all_relativeR": rel, "template_poses": tp,
-            "query_pose": gtR, "query_translation": trans, "intrinsic": K[None].expand(B, 3, 3).contiguous(),
-            "depth_path": paths, "obj_id": torch.ones(B, dtype=torch.int64)}, str(ply)
-
-
 def _expected(batch, R, model):
     """the BOP scores from separate render_depth / vsd_errors / pose_errors / average_recall calls"""
     import cv2
@@ -317,7 +274,7 @@ def _expected(batch, R, model):
 def test_eval_bop_end_to_end(gpu_model, tmp_path, monkeypatch):
     from nope_b200 import bop
     from nope_b200 import vsd as V
-    batch, cad = _tless_batch(tmp_path)
+    batch, cad, _ = tless_batch(tmp_path, symmetries=FLIPS)
     model = gpu_model
     model.load_mesh(cad, obj_ids=[1])
     model.load_models_info(os.path.join(cad, "models_info.json"))
@@ -328,11 +285,8 @@ def test_eval_bop_end_to_end(gpu_model, tmp_path, monkeypatch):
     def strict(fn, name):
         def inner(*a, **kw):
             calls[name] += 1
-            torch.cuda.set_sync_debug_mode("error")
-            try:
+            with no_host_sync():
                 return fn(*a, **kw)
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
         return inner
     monkeypatch.setattr(V, "render_depth", strict(V.render_depth, "render"))
     monkeypatch.setattr(V, "vsd_errors", strict(V.vsd_errors, "vsd"))
@@ -375,7 +329,7 @@ def _vsd_inputs(batch, R, model):
 
 def test_eval_bop_with_refined_search(gpu_model, tmp_path):
     from nope_b200.inplane_refine import InplaneRefiner
-    batch, cad = _tless_batch(tmp_path)
+    batch, cad, _ = tless_batch(tmp_path, symmetries=FLIPS)
     model = gpu_model
     model.load_mesh(cad, obj_ids=[1])
     model.load_models_info(os.path.join(cad, "models_info.json"))

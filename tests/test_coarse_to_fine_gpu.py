@@ -5,6 +5,7 @@ top-`keep`, and the ranking is the exhaustive ranking restricted to that set."""
 import pytest
 import torch
 
+from _util import no_host_sync
 from oracle import hierarchy_oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -166,12 +167,8 @@ def test_search_does_not_synchronise(gpu_model, nested):
     qf = torch.randn(B, Q, 8, 32, 32, generator=g).cuda()
     rel = [nested["rel"][n] for n in (42, 162, 642)]
     ref_out = search(u, rf, qf, rel, nested["three"], keep=KEEP, k=K)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         out = search(u, rf, qf, rel, nested["three"], keep=KEEP, k=K)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     torch.cuda.synchronize()
     assert torch.equal(out["sim"], ref_out["sim"]) and torch.equal(out["topi"], ref_out["topi"])
     assert out["hypotheses"] == nested["three"].hypotheses(KEEP)

@@ -10,22 +10,11 @@ import pytest
 
 import contour_refine_oracle as cro
 import translation_oracle as to
+from _scenes import angle, rotvec
 from oracle import render_oracle as ro
 
 K4 = np.array([150.0, 151.0, 48.2, 35.9])                    # the 96 x 72 intrinsics of tests/test_bop_gpu.py
 SIZE = (72, 96)
-
-
-def _rotvec(w):
-    w = np.asarray(w, dtype=np.float64)
-    a = np.linalg.norm(w)
-    k = w / a
-    Kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
-    return np.eye(3) + math.sin(a) * Kx + (1 - math.cos(a)) * Kx @ Kx
-
-
-def _angle(Ra, Rb):
-    return math.degrees(2 * math.asin(min(1.0, np.linalg.norm(Ra - Rb) / (2 * math.sqrt(2)))))
 
 
 def _brute_force(mask):
@@ -140,9 +129,9 @@ def test_a_scale_about_the_origin_moves_z():
 
 def test_oracle_recovers_a_small_rotation():
     render, mask, rho = _setup(R_BOX, T_BOX)
-    R0 = _rotvec([0.03, -0.02, 0.025]) @ R_BOX
+    R0 = rotvec([0.03, -0.02, 0.025]) @ R_BOX
     R, t, fit, _ = cro.refine(render, R0, T_BOX, mask, K4, cro_default(), rho)
-    assert _angle(R, R_BOX) < 0.5 * _angle(R0, R_BOX), (_angle(R0, R_BOX), _angle(R, R_BOX))
+    assert angle(R, R_BOX) < 0.5 * angle(R0, R_BOX), (angle(R0, R_BOX), angle(R, R_BOX))
     assert fit[3] > 0.95
 
 

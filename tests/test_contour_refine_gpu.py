@@ -10,28 +10,24 @@ import pytest
 import torch
 
 import contour_refine_oracle as cro
-from test_depth_refine_gpu import H, K4, MESHES, W, _angle, _perturb, _render, _rot, _scene
+from _scenes import H, K4, W, angle, make_mesh, perturb, render, rot, scene, tless_batch
+from _util import no_host_sync
 
 pytestmark = pytest.mark.gpu
 
 TAUS = np.geomspace(0.15, 0.02, 7)
 
 
-def _mesh(name):
-    from nope_b200.vsd import Mesh
-    return Mesh(*MESHES[name]())
-
-
 def _masks_scene(mesh, seed, F, P, K=None, deg=5.0, mm=10.0):
     """(R_true, t_true, masks uint8 [F, H, W] on the GPU = the render at the true pose, R0, t0)"""
-    R_true, t_true, _, M, R0, t0 = _scene(mesh, seed, F, P, K=K, sensor=False, background=False, deg=deg, mm=mm)
+    R_true, t_true, _, M, R0, t0 = scene(mesh, seed, F, P, K=K, sensor=False, background=False, deg=deg, mm=mm)
     return R_true, t_true, M, R0, t0
 
 
 # ------------------------------------------------------------------ the signed distance field
 def test_mask_sdf_equals_oracle():
     from nope_b200.contour_refine import mask_sdf
-    mesh = _mesh("box")
+    mesh, _ = make_mesh("box")
     _, _, M, _, _ = _masks_scene(mesh, 5, 2, 1)
     got = mask_sdf(M).cpu().numpy()
     for f in range(2):
@@ -62,7 +58,7 @@ def test_kernel_equals_oracle(name, P):
     """R, t, the fit and the integer sums after 0 ... 6 updates equal the oracle's, which renders with render_depth at
     its own pose; frame 1 has a perturbed K"""
     from nope_b200.contour_refine import refine_pose_contour
-    mesh = _mesh(name)
+    mesh, _ = make_mesh(name)
     F = 2
     K = np.stack([K4, K4 * [1.0, 1.001, 1.02, 0.98]])
     _, _, M, R0, t0 = _masks_scene(mesh, 41 + P, F, P, K=K)
@@ -76,7 +72,7 @@ def test_kernel_equals_oracle(name, P):
         for p in range(P):
             R, t = R0[f, p], t0[f, p]
             for i in range(7):
-                D = _render(mesh, R, t, K[f]).cpu().numpy()
+                D = render(mesh, R, t, K[f]).cpu().numpy()
                 tau = TAUS[i] * s
                 sums, nc = cro.accumulate(D, phi, K[f], t, tau, rho)
                 assert np.array_equal(got[i][3][f, p], sums), (f, p, i, got[i][3][f, p] - sums)
@@ -93,7 +89,7 @@ def test_kernel_equals_oracle(name, P):
 def test_workspace_holds_the_final_render():
     from nope_b200 import _lib
     from nope_b200.vsd import _stream
-    mesh = _mesh("sphere")
+    mesh, _ = make_mesh("sphere")
     _, _, M, R0, t0 = _masks_scene(mesh, 3, 2, 3)
     K = np.repeat(K4[None], 2, axis=0)
     Rd, td = torch.from_numpy(R0).cuda().contiguous(), torch.from_numpy(t0).cuda().contiguous()
@@ -109,13 +105,13 @@ def test_workspace_holds_the_final_render():
     Rh, th = R.cpu().numpy(), t.cpu().numpy()
     for f in range(2):
         for p in range(3):
-            assert torch.equal(depth[3 * f + p], _render(mesh, Rh[f, p], th[f, p]))
+            assert torch.equal(depth[3 * f + p], render(mesh, Rh[f, p], th[f, p]))
 
 
 @pytest.mark.parametrize("name", ["box", "sphere", "soup"])
 def test_the_true_pose_stays_to_the_bit(name):
     from nope_b200.contour_refine import refine_pose_contour
-    mesh = _mesh(name)
+    mesh, _ = make_mesh(name)
     R_true, t_true, M, _, _ = _masks_scene(mesh, 7, 4, 1)
     R, t, fit, sums = refine_pose_contour(mesh, R_true, t_true, K4, M, return_sums=True)
     assert np.array_equal(R[:, 0].cpu().numpy(), R_true) and np.array_equal(t[:, 0].cpu().numpy(), t_true)
@@ -135,27 +131,22 @@ BOUNDS = {("box", "offset"): (1.0, 3.0, 0.95), ("box", "box fit"): (1.5, 4.5, 0.
           ("soup", "offset"): (0.5, 7.0, 0.6), ("soup", "box fit"): (0.5, 4.0, 0.9)}
 
 
-def _diameter(v):
-    v = np.asarray(v, dtype=np.float64)
-    return float(max(np.linalg.norm(v - p, axis=1).max() for p in v))
-
-
 @pytest.mark.parametrize("start", ["offset", "box fit"])
 @pytest.mark.parametrize("name", ["box", "sphere", "soup"])
 def test_accuracy_from_perturbed_starts(name, start):
     from nope_b200.contour_refine import refine_pose_contour
     from nope_b200.translation import estimate_translation
-    mesh = _mesh(name)
+    mesh, diameter = make_mesh(name)
     R_true, t_true, M, R0, t0 = _masks_scene(mesh, 100, 16, 1)
     if start == "box fit":
-        t0 = estimate_translation(mesh, R0, K4, M, diameter=_diameter(MESHES[name]()[0]))[0].cpu().numpy()
+        t0 = estimate_translation(mesh, R0, K4, M, diameter=diameter)[0].cpu().numpy()
     R, t, fit = refine_pose_contour(mesh, R0, t0, K4, M)
     R, t = R[:, 0].cpu().numpy(), t[:, 0].cpu().numpy()
     deg, mm, iou = BOUNDS[name, start]
     err_t = np.linalg.norm(t - t_true, axis=1)
     err_t0 = np.linalg.norm(t0[:, 0] - t_true, axis=1)
-    err_r = np.array([_angle(R[f], R_true[f]) for f in range(16)])
-    err_r0 = np.array([_angle(R0[f, 0], R_true[f]) for f in range(16)])
+    err_r = np.array([angle(R[f], R_true[f]) for f in range(16)])
+    err_r0 = np.array([angle(R0[f, 0], R_true[f]) for f in range(16)])
     assert np.median(err_t) <= mm, (err_t, err_t0)
     assert deg is None or np.median(err_r) <= deg, (err_r, err_r0)
     if name == "box":
@@ -166,7 +157,7 @@ def test_accuracy_from_perturbed_starts(name, start):
 # ------------------------------------------------------------------ batch independence and edge cases
 def test_batch_independence():
     from nope_b200.contour_refine import refine_pose_contour
-    mesh = _mesh("box")
+    mesh, _ = make_mesh("box")
     K = np.stack([K4 * [1, 1, 1 + 0.01 * f, 1] for f in range(3)])
     _, _, M, R0, t0 = _masks_scene(mesh, 21, 3, 4, K=K)
     R, t, fit = refine_pose_contour(mesh, R0, t0, K, M)
@@ -186,7 +177,7 @@ def test_batch_independence():
 
 def test_empty_and_full_masks_keep_the_pose():
     from nope_b200.contour_refine import refine_pose_contour
-    mesh = _mesh("box")
+    mesh, _ = make_mesh("box")
     _, _, M, R0, t0 = _masks_scene(mesh, 8, 3, 2)
     M[1] = 0
     M[2] = 1
@@ -201,18 +192,14 @@ def test_empty_and_full_masks_keep_the_pose():
 
 def test_no_host_synchronisation():
     from nope_b200.contour_refine import mask_sdf, refine_pose_contour
-    mesh = _mesh("box")
+    mesh, _ = make_mesh("box")
     _, _, M, R0, t0 = _masks_scene(mesh, 9, 2, 3)
     Rd, td = torch.from_numpy(R0).cuda(), torch.from_numpy(t0).cuda()
     K = np.repeat(K4[None], 2, axis=0)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         a = refine_pose_contour(mesh, Rd, td, K, M)
         b = refine_pose_contour(mesh, Rd.float(), td[:, 0], K, M.bool(), iters=2, tau=0.05)
         s = mask_sdf(M)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     c = refine_pose_contour(mesh, R0, t0, K, M.cpu())
     assert torch.equal(a[0], c[0]) and torch.equal(a[1], c[1])
     assert b[0].shape == (2, 3, 3, 3) and torch.isfinite(b[1]).all()
@@ -220,24 +207,15 @@ def test_no_host_synchronisation():
 
 
 # ------------------------------------------------------------------ PoseConditional.refine_contour and eval_bop
-def _batch(tmp_path):
-    from test_translation_gpu import _tless_batch
-    return _tless_batch(tmp_path)
-
-
-def _load(model, cad):
+def test_rerank_puts_the_true_rotation_first(gpu_model, tmp_path):
+    batch, cad, masks = tless_batch(tmp_path)
+    model = gpu_model
     model.load_mesh(cad, obj_ids=[1])
     model.load_models_info(os.path.join(cad, "models_info.json"))
-
-
-def test_rerank_puts_the_true_rotation_first(gpu_model, tmp_path):
-    batch, cad, masks = _batch(tmp_path)
-    model = gpu_model
-    _load(model, cad)
     B, k = 3, 5
     rng = np.random.default_rng(4)
     R_gt = batch["query_pose"].double().numpy()
-    R = np.stack([np.stack([_rot(rng) for _ in range(k)]) for _ in range(B)])
+    R = np.stack([np.stack([rot(rng) for _ in range(k)]) for _ in range(B)])
     for b in range(B):
         R[b, 3] = R_gt[b]
     t = batch["query_translation"][:, None, :, 0].expand(B, k, 3).double()
@@ -253,14 +231,15 @@ def test_rerank_puts_the_true_rotation_first(gpu_model, tmp_path):
 
 def test_eval_bop_at_refined_poses(gpu_model, tmp_path):
     """the median MSSD at poses refined from perturbed starts is lower than at the starts"""
-    batch, cad, masks = _batch(tmp_path)
+    batch, cad, masks = tless_batch(tmp_path)
     model = gpu_model
-    _load(model, cad)
+    model.load_mesh(cad, obj_ids=[1])
+    model.load_models_info(os.path.join(cad, "models_info.json"))
     B, k = 3, 4
     rng = np.random.default_rng(6)
     R_gt = batch["query_pose"].double().numpy()
     t_gt = batch["query_translation"][:, :, 0].double().numpy()
-    starts = [[_perturb(rng, R_gt[b], t_gt[b], 4.0, 6.0) for _ in range(k)] for b in range(B)]
+    starts = [[perturb(rng, R_gt[b], t_gt[b], 4.0, 6.0) for _ in range(k)] for b in range(B)]
     R0 = np.stack([np.stack([s[0] for s in row]) for row in starts])
     t0 = np.stack([np.stack([s[1] for s in row]) for row in starts])
     p0, p1 = tmp_path / "start.npz", tmp_path / "refined.npz"

@@ -13,8 +13,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from _util import log, max_rel, min_many_tile_pairs, pair_tiles, pick_bn, rounds, worst_block_rel_l2
-from test_ops_gpu import CONV_CASES, conv_reference, make_conv_case
+from _util import (CONV_CASES, conv_reference, log, make_conv_case, max_rel, min_many_tile_pairs, pair_tiles, pick_bn,
+                   rounds, worst_block_rel_l2)
 
 pytestmark = pytest.mark.gpu
 

@@ -1,18 +1,15 @@
 """CPU: full-frame crops without a device -- the numpy restatement of crop_warp_kernel (oracle/crop_oracle.py)
 against the live reference pipeline (PIL paste, cv2.warpPerspective, torchvision) and against the unmodified
 reference's crops (tests/golden/crop.npz), crop_transforms against the M the reference's crop_frame computes, the
-weight table, the coordinate association, and the ABI declaration, refusals and Python argument errors."""
+weight table, the coordinate association, and the ABI's refusals and Python argument errors."""
 import ctypes as C
 import os
-import re
 
 import numpy as np
 import pytest
 import torch
 
 from oracle import crop_oracle as co
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -177,19 +174,6 @@ def test_crop_transforms_batching_and_errors():
 
 
 # ------------------------------------------------------------------ ABI
-def _declared():
-    src = open(os.path.join(ROOT, "include", "nope_b200.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return set(re.findall(r"\b(nope_[a-z0-9_]+)\s*\(", src))
-
-
-def test_header_declares_and_lib_binds_crop():
-    from nope_b200 import _lib
-    lib = _lib.load()
-    assert "nope_crop_frames" in _declared() and "nope_crop_frames" in _lib.SIGNATURES
-    assert hasattr(lib, "nope_crop_frames") and lib.nope_abi_version() == 3
-
-
 P = C.c_void_p(256)
 _A = dict(fr=P, F=2, H=540, W=720, C=3, mk=None, fi=None, inv=P, B=2, S=256, o=P)
 

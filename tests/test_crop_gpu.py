@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+from _util import no_host_sync
 from oracle import crop_oracle as co
 from oracle import inputs
 
@@ -126,12 +127,8 @@ def test_no_host_synchronisation():
     inv = torch.eye(3, dtype=torch.float64, device="cuda").repeat(2, 1, 1)
     idx = torch.tensor([2, 0], device="cuda")
     crop_frames(frames, inv, 32, frame_idx=idx)                            # warm-up: library load
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         out = crop_frames(frames, inv, 32, frame_idx=idx)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert out.shape == (2, 3, 32, 32)
 
 

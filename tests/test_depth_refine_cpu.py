@@ -10,27 +10,11 @@ import torch
 
 import depth_refine_oracle as dro
 import translation_oracle as to
+from _scenes import angle, rotvec
 from oracle import render_oracle as ro
 
 K4 = np.array([150.0, 151.0, 48.2, 35.9])                    # the 96 x 72 intrinsics of tests/test_bop_gpu.py
 SIZE = (72, 96)
-
-
-def _rotvec(w):
-    """rotation matrix of the rotation vector w (radians)"""
-    w = np.asarray(w, dtype=np.float64)
-    a = np.linalg.norm(w)
-    if a == 0:
-        return np.eye(3)
-    k = w / a
-    Kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
-    return np.eye(3) + math.sin(a) * Kx + (1 - math.cos(a)) * Kx @ Kx
-
-
-def _angle(Ra, Rb):
-    """the angle of Ra Rb^T in degrees, from the chord |Ra - Rb|_F = 2 sqrt(2) sin(angle / 2): exactly 0 for equal
-    matrices, also for the slightly non-orthonormal float32-derived ones of look_pose"""
-    return math.degrees(2 * math.asin(min(1.0, np.linalg.norm(Ra - Rb) / (2 * math.sqrt(2)))))
 
 
 def _setup(v, f, R_true, t_true):
@@ -45,12 +29,12 @@ def test_oracle_recovers_a_small_motion_of_the_box():
     R_true = ro.look_pose(0.5, -0.4, 0.3)[:3, :3].astype(np.float64)
     t_true = np.array([4.0, -3.0, 330.0])
     render, S, rho = _setup(v, f, R_true, t_true)
-    R0 = _rotvec([0.03, -0.02, 0.025]) @ R_true
+    R0 = rotvec([0.03, -0.02, 0.025]) @ R_true
     t0 = t_true + [3.0, -2.0, 6.0]
     taus = np.geomspace(25.0, 2.0, 9)
     R, t, fit, sums = dro.refine(render, R0, t0, S, S > 0, K4, taus, rho)
-    assert _angle(R, R_true) < 0.1 and np.abs(t - t_true).max() < 0.1, (_angle(R, R_true), t - t_true)
-    assert _angle(R0, R_true) > 2.0
+    assert angle(R, R_true) < 0.1 and np.abs(t - t_true).max() < 0.1, (angle(R, R_true), t - t_true)
+    assert angle(R0, R_true) > 2.0
     assert fit[0] == sums[-1] > 100 and fit[1] == np.count_nonzero(S) and 0.5 < fit[3] <= 1.0 and fit[2] < 0.05
 
 
@@ -77,7 +61,7 @@ def test_oracle_does_not_slide_a_face_on_plane():
     R, t, fit, sums = dro.refine(render, R_true, t0, S, None, K4, np.geomspace(20.0, 2.0, 6), rho)
     assert np.abs(t[:2] - t0[:2]).max() < 1e-4, t - t0
     assert abs(t[2] - 400.0) < 1e-3
-    assert _angle(R, R_true) < 1e-3
+    assert angle(R, R_true) < 1e-3
     # the first update, from an exactly face-on render: the unobservable parameters do not move at all
     R1, t1, _, _ = dro.refine(render, R_true, t0, S, None, K4, [20.0, 20.0], rho)
     assert t1[0] == t0[0] and t1[1] == t0[1] and t1[2] != t0[2]
@@ -93,7 +77,7 @@ def test_oracle_does_not_turn_a_sphere():
     t0 = t_true + [4.0, -3.0, 8.0]
     R, t, fit, _ = dro.refine(render, R_true, t0, S, None, K4, np.geomspace(20.0, 2.0, 8), rho)
     assert np.abs(t - t_true).max() < 0.3, t - t_true
-    assert _angle(R, R_true) < 1.0
+    assert angle(R, R_true) < 1.0
 
 
 def test_fewer_than_six_pairs_keep_the_pose():

@@ -3,7 +3,6 @@ sums included, on the same render_depth images after 0 ... 6 updates; accuracy f
 depth (quantised to 0.1 mm, seeded noise and holes, a background plane behind the object); the true pose kept;
 batch independence; edge cases; no host synchronisation; `PoseConditional.refine_depth` with rerank, and eval_bop
 at refined poses."""
-import math
 import os
 
 import numpy as np
@@ -11,84 +10,10 @@ import pytest
 import torch
 
 import depth_refine_oracle as dro
-import translation_oracle as to
-from oracle import render_oracle as ro
+from _scenes import H, K4, W, angle, make_mesh, perturb, render, rot, scene, tless_batch
+from _util import no_host_sync
 
 pytestmark = pytest.mark.gpu
-
-K4 = np.array([1075.65091572, 1073.90347929, 360.0, 270.0])    # Primesense, as tools/vsd_time.py
-H, W = 540, 720
-MESHES = {"box": lambda: ro.box(), "sphere": lambda: ro.sphere(40.0, 2), "soup": lambda: ro.soup(64, seed=1)}
-
-
-def _mesh(name):
-    from nope_b200.vsd import Mesh
-    return Mesh(*MESHES[name]())
-
-
-def _rot(rng):
-    return ro.look_pose(*rng.uniform(-math.pi, math.pi, 3))[:3, :3].astype(np.float64)
-
-
-def _rotvec(w):
-    a = np.linalg.norm(w)
-    k = w / a
-    Kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
-    return np.eye(3) + math.sin(a) * Kx + (1 - math.cos(a)) * Kx @ Kx
-
-
-def _angle(Ra, Rb):
-    """the angle of Ra Rb^T in degrees, from the chord |Ra - Rb|_F = 2 sqrt(2) sin(angle / 2): exactly 0 for equal
-    matrices, also for the slightly non-orthonormal float32-derived ones of look_pose"""
-    return math.degrees(2 * math.asin(min(1.0, np.linalg.norm(Ra - Rb) / (2 * math.sqrt(2)))))
-
-
-def _render(mesh, R, t, K=K4):
-    from nope_b200.vsd import render_depth
-    return render_depth(mesh, torch.from_numpy(to.pose(R, t)), K, (H, W))[0]
-
-
-def _perturb(rng, R, t, deg=5.0, mm=10.0):
-    axis = rng.normal(size=3)
-    axis /= np.linalg.norm(axis)
-    d = rng.normal(size=3)
-    return _rotvec(axis * math.radians(rng.uniform(0.5, 1.0) * deg)) @ R, t + d / np.linalg.norm(d) * \
-        rng.uniform(0.5, 1.0) * mm
-
-
-def _scene(mesh, seed, F, P, K=None, sensor=True, background=True, deg=5.0, mm=10.0):
-    """F frames, a true pose each at 400 - 900 mm with the object inside the frame, and P perturbed hypotheses:
-    -> (R_true [F, 3, 3], t_true [F, 3], S float64 [F, H, W] on the GPU, masks uint8 [F, H, W], R0 [F, P, 3, 3],
-    t0 [F, P, 3]).  S is the render at the true pose; with `sensor` quantised to 0.1 mm after seeded noise
-    (sigma 0.5 mm) with 2 % seeded holes; with `background` merged by the minimum with a plane 40 mm behind it."""
-    rng = np.random.default_rng(seed)
-    K = np.repeat(K4[None], F, 0) if K is None else K
-    Rt, tt, S, M = [], [], [], []
-    while len(Rt) < F:
-        f = len(Rt)
-        R = _rot(rng)
-        z = rng.uniform(400.0, 900.0)
-        t = np.array([rng.uniform(-0.15, 0.15) * z, rng.uniform(-0.15, 0.15) * z, z])
-        d = _render(mesh, R, t, K[f]).double()
-        m = d > 0
-        rows, cols = m.any(1).nonzero(), m.any(0).nonzero()
-        if not m.any() or rows.min() == 0 or cols.min() == 0 or rows.max() == H - 1 or cols.max() == W - 1:
-            continue
-        if background:
-            d = torch.where(m, d, torch.full_like(d, z + 40.0))
-        if sensor:
-            g = torch.Generator(device=d.device).manual_seed(seed * 1000 + f)
-            d = d + 0.5 * torch.randn(d.shape, generator=g, device=d.device, dtype=torch.float64)
-            d = torch.round(d * 10.0) / 10.0
-            d = torch.where(torch.rand(d.shape, generator=g, device=d.device) < 0.02, torch.zeros_like(d), d)
-        Rt.append(R), tt.append(t), S.append(d), M.append(m.to(torch.uint8))
-    R0 = np.zeros((F, P, 3, 3))
-    t0 = np.zeros((F, P, 3))
-    for f in range(F):
-        for p in range(P):
-            R0[f, p], t0[f, p] = _perturb(rng, Rt[f], tt[f], deg, mm)
-    return np.stack(Rt), np.stack(tt), torch.stack(S), torch.stack(M), R0, t0
-
 
 TAUS = np.geomspace(20.0, 2.0, 7)
 
@@ -100,10 +25,10 @@ def test_kernel_equals_oracle(name, P):
     """R, t, the fit and the integer sums after 0 ... 6 updates equal the oracle's, which renders with render_depth at
     its own pose; frame 1 has a perturbed K; the P = 5 case uses masks"""
     from nope_b200.depth_refine import refine_pose_depth
-    mesh = _mesh(name)
+    mesh, _ = make_mesh(name)
     F = 2
     K = np.stack([K4, K4 * [1.0, 1.001, 1.02, 0.98]])
-    _, _, S, M, R0, t0 = _scene(mesh, 31 + P, F, P, K=K)
+    _, _, S, M, R0, t0 = scene(mesh, 31 + P, F, P, K=K)
     masks = M if P == 5 else None
     got = [refine_pose_depth(mesh, R0, t0, K, S, masks=masks, iters=i, tau=TAUS[:i + 1], return_sums=True)
            for i in range(7)]
@@ -117,7 +42,7 @@ def test_kernel_equals_oracle(name, P):
         for p in range(P):
             R, t = R0[f, p], t0[f, p]
             for i in range(7):
-                sums = dro.accumulate(_render(mesh, R, t, K[f]).cpu().numpy(), Sh[f], None if Mh is None else Mh[f],
+                sums = dro.accumulate(render(mesh, R, t, K[f]).cpu().numpy(), Sh[f], None if Mh is None else Mh[f],
                                       K[f], t, TAUS[i], rho)
                 assert np.array_equal(got[i][3][f, p], sums), (f, p, i, got[i][3][f, p] - sums)
                 assert np.array_equal(got[i][0][f, p], R) and np.array_equal(got[i][1][f, p], t), (f, p, i)
@@ -129,8 +54,8 @@ def test_kernel_equals_oracle(name, P):
 def test_workspace_holds_the_final_render():
     from nope_b200 import _lib
     from nope_b200.vsd import _stream
-    mesh = _mesh("sphere")
-    _, _, S, _, R0, t0 = _scene(mesh, 3, 2, 3)
+    mesh, _ = make_mesh("sphere")
+    _, _, S, _, R0, t0 = scene(mesh, 3, 2, 3)
     K = np.repeat(K4[None], 2, axis=0)
     Rd, td = torch.from_numpy(R0).cuda().contiguous(), torch.from_numpy(t0).cuda().contiguous()
     depth = torch.empty((6, H, W), device="cuda")
@@ -145,7 +70,7 @@ def test_workspace_holds_the_final_render():
     Rh, th = R.cpu().numpy(), t.cpu().numpy()
     for f in range(2):
         for p in range(3):
-            assert torch.equal(depth[3 * f + p], _render(mesh, Rh[f, p], th[f, p]))
+            assert torch.equal(depth[3 * f + p], render(mesh, Rh[f, p], th[f, p]))
 
 
 # ------------------------------------------------------------------ accuracy
@@ -163,15 +88,15 @@ BOUNDS = {"box": (0.2, 0.5, 0.5, 1.0), "sphere": (None, 0.1, 1.0, 0.1), "soup": 
 def test_accuracy_from_perturbed_starts(name):
     """sensor-like depth with a background plane, the mask, the default schedule"""
     from nope_b200.depth_refine import refine_pose_depth
-    mesh = _mesh(name)
-    R_true, t_true, S, M, R0, t0 = _scene(mesh, 100, 16, 1)
+    mesh, _ = make_mesh(name)
+    R_true, t_true, S, M, R0, t0 = scene(mesh, 100, 16, 1)
     R, t, fit = refine_pose_depth(mesh, R0, t0, K4, S, masks=M)
     R, t = R[:, 0].cpu().numpy(), t[:, 0].cpu().numpy()
     deg, mm, worse_deg, worse_mm = BOUNDS[name]
     err_t = np.linalg.norm(t - t_true, axis=1)
     err_t0 = np.linalg.norm(t0[:, 0] - t_true, axis=1)
-    err_r = np.array([_angle(R[f], R_true[f]) for f in range(16)])
-    err_r0 = np.array([_angle(R0[f, 0], R_true[f]) for f in range(16)])
+    err_r = np.array([angle(R[f], R_true[f]) for f in range(16)])
+    err_r0 = np.array([angle(R0[f, 0], R_true[f]) for f in range(16)])
     assert np.median(err_t) <= mm and (err_t <= err_t0 + worse_mm).all(), (err_t, err_t0)
     assert deg is None or np.median(err_r) <= deg, err_r
     assert (err_r <= err_r0 + worse_deg).all(), (err_r, err_r0)
@@ -181,12 +106,12 @@ def test_accuracy_from_perturbed_starts(name):
 @pytest.mark.parametrize("name", ["box", "sphere", "soup"])
 def test_the_true_pose_stays(name):
     from nope_b200.depth_refine import refine_pose_depth
-    mesh = _mesh(name)
-    R_true, t_true, S, _, _, _ = _scene(mesh, 7, 4, 1, sensor=False, background=False)
+    mesh, _ = make_mesh(name)
+    R_true, t_true, S, _, _, _ = scene(mesh, 7, 4, 1, sensor=False, background=False)
     R, t, fit = refine_pose_depth(mesh, R_true, t_true, K4, S)
     R, t = R[:, 0].cpu().numpy(), t[:, 0].cpu().numpy()
     assert np.abs(t - t_true).max() <= 1e-6
-    assert max(_angle(R[f], R_true[f]) for f in range(4)) <= 1e-6
+    assert max(angle(R[f], R_true[f]) for f in range(4)) <= 1e-6
     assert (fit["rms"] == 0).all()
 
 
@@ -194,9 +119,9 @@ def test_the_mask_keeps_the_background_out():
     """a background plane 40 mm behind the box, within the first tolerances: with the mask the fit is bit for bit the
     fit without a background; without the mask the plane's pixels count as valid"""
     from nope_b200.depth_refine import refine_pose_depth
-    mesh = _mesh("box")
-    R_true, t_true, S, M, R0, t0 = _scene(mesh, 55, 8, 1)
-    R_true2, t_true2, S2, M2, _, _ = _scene(mesh, 55, 8, 1, background=False)
+    mesh, _ = make_mesh("box")
+    R_true, t_true, S, M, R0, t0 = scene(mesh, 55, 8, 1)
+    R_true2, t_true2, S2, M2, _, _ = scene(mesh, 55, 8, 1, background=False)
     R, t, fit = refine_pose_depth(mesh, R0, t0, K4, S, masks=M)
     R2, t2, fit2 = refine_pose_depth(mesh, R0, t0, K4, S2, masks=M2)
     assert torch.equal(R, R2) and torch.equal(t, t2)                  # the mask hides the plane entirely
@@ -208,9 +133,9 @@ def test_the_mask_keeps_the_background_out():
 # ------------------------------------------------------------------ batch independence and edge cases
 def test_batch_independence():
     from nope_b200.depth_refine import refine_pose_depth
-    mesh = _mesh("sphere")
+    mesh, _ = make_mesh("sphere")
     K = np.stack([K4 * [1, 1, 1 + 0.01 * f, 1] for f in range(3)])
-    _, _, S, M, R0, t0 = _scene(mesh, 21, 3, 4, K=K)
+    _, _, S, M, R0, t0 = scene(mesh, 21, 3, 4, K=K)
     R, t, fit = refine_pose_depth(mesh, R0, t0, K, S, masks=M)
     for f in range(3):
         a, b, c = refine_pose_depth(mesh, R0[f:f + 1], t0[f:f + 1], K[f:f + 1], S[f:f + 1], masks=M[f:f + 1])
@@ -228,8 +153,8 @@ def test_batch_independence():
 
 def test_empty_mask_or_depth_keeps_the_pose():
     from nope_b200.depth_refine import refine_pose_depth
-    mesh = _mesh("box")
-    _, _, S, M, R0, t0 = _scene(mesh, 8, 3, 2)
+    mesh, _ = make_mesh("box")
+    _, _, S, M, R0, t0 = scene(mesh, 8, 3, 2)
     M[1] = 0
     S[2] = 0
     R, t, fit = refine_pose_depth(mesh, R0, t0, K4, S, masks=M)
@@ -243,41 +168,28 @@ def test_empty_mask_or_depth_keeps_the_pose():
 
 def test_no_host_synchronisation():
     from nope_b200.depth_refine import refine_pose_depth
-    mesh = _mesh("box")
-    _, _, S, M, R0, t0 = _scene(mesh, 9, 2, 3)
+    mesh, _ = make_mesh("box")
+    _, _, S, M, R0, t0 = scene(mesh, 9, 2, 3)
     Rd, td = torch.from_numpy(R0).cuda(), torch.from_numpy(t0).cuda()
     K = np.repeat(K4[None], 2, axis=0)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         a = refine_pose_depth(mesh, Rd, td, K, S, masks=M)
         b = refine_pose_depth(mesh, Rd.float(), td[:, 0], K, S.float(), masks=M.bool(), iters=2, tau=5.0)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     c = refine_pose_depth(mesh, R0, t0, K, S.cpu(), masks=M.cpu())
     assert torch.equal(a[0], c[0]) and torch.equal(a[1], c[1])
     assert b[0].shape == (2, 3, 3, 3) and torch.isfinite(b[1]).all()
 
 
 # ------------------------------------------------------------------ PoseConditional.refine_depth and eval_bop
-def _batch(tmp_path):
-    from test_translation_gpu import _tless_batch
-    return _tless_batch(tmp_path)
-
-
-def _load(model, cad):
+def test_rerank_puts_the_true_rotation_first(gpu_model, tmp_path):
+    batch, cad, masks = tless_batch(tmp_path)
+    model = gpu_model
     model.load_mesh(cad, obj_ids=[1])
     model.load_models_info(os.path.join(cad, "models_info.json"))
-
-
-def test_rerank_puts_the_true_rotation_first(gpu_model, tmp_path):
-    batch, cad, masks = _batch(tmp_path)
-    model = gpu_model
-    _load(model, cad)
     B, k = 3, 5
     rng = np.random.default_rng(4)
     R_gt = batch["query_pose"].double().numpy()
-    R = np.stack([np.stack([_rot(rng) for _ in range(k)]) for _ in range(B)])
+    R = np.stack([np.stack([rot(rng) for _ in range(k)]) for _ in range(B)])
     for b in range(B):
         R[b, 3] = R_gt[b]
     t = batch["query_translation"][:, None, :, 0].expand(B, k, 3).double()
@@ -294,14 +206,15 @@ def test_rerank_puts_the_true_rotation_first(gpu_model, tmp_path):
 def test_eval_bop_at_refined_poses(gpu_model, tmp_path):
     """MSSD at poses refined from perturbed starts is no worse than at the starts, row by row; refined from the truth,
     eval_bop gives the unrefined scores"""
-    batch, cad, masks = _batch(tmp_path)
+    batch, cad, masks = tless_batch(tmp_path)
     model = gpu_model
-    _load(model, cad)
+    model.load_mesh(cad, obj_ids=[1])
+    model.load_models_info(os.path.join(cad, "models_info.json"))
     B = 3
     rng = np.random.default_rng(6)
     R_gt = batch["query_pose"].double().numpy()
     t_gt = batch["query_translation"][:, :, 0].double().numpy()
-    R0, t0 = zip(*[_perturb(rng, R_gt[b], t_gt[b], 3.0, 4.0) for b in range(B)])
+    R0, t0 = zip(*[perturb(rng, R_gt[b], t_gt[b], 3.0, 4.0) for b in range(B)])
     R0, t0 = np.stack(R0)[:, None], np.stack(t0)[:, None]
     p0, p1 = tmp_path / "start.npz", tmp_path / "refined.npz"
     model.eval_bop(batch, "obj01", R_est=R0, t_est=t0, save_path=str(p0))

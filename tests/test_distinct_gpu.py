@@ -11,6 +11,8 @@ import pytest
 import torch
 
 import distinct_oracle as do
+from _scenes import FLIPS, tless_batch
+from _util import no_host_sync
 
 pytestmark = pytest.mark.gpu
 
@@ -206,12 +208,8 @@ def test_no_host_synchronisation(grids):
     R, _ = grids[2]
     rot = R[None].cuda()
     sim = torch.randn(B, Q, len(R), device="cuda")
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         score, idx = distinct_topk(sim, rot, 8, 20.0, [ENTRIES["flip"], ENTRIES["axis_flip"]])
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     s_o, i_o = _oracle(sim, rot, 8, 20.0, [ENTRIES["flip"], ENTRIES["axis_flip"]])
     assert np.array_equal(idx.cpu().numpy(), i_o) and np.array_equal(score.cpu().numpy(), s_o)
 
@@ -219,9 +217,8 @@ def test_no_host_synchronisation(grids):
 def test_select_distinct_end_to_end(gpu_model, tmp_path):
     """select_distinct -> estimate_translation -> eval_bop(R_est=, t_est=) on the synthetic T-LESS batch of the BOP
     tests (a box with three flips)"""
-    from test_bop_gpu import _tless_batch
     from nope_b200.distinct import distinct_topk
-    batch, cad = _tless_batch(tmp_path)
+    batch, cad, _ = tless_batch(tmp_path, symmetries=FLIPS)
     model = gpu_model
     model.load_mesh(cad, obj_ids=[1])
     model.load_models_info(os.path.join(cad, "models_info.json"))

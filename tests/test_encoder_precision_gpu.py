@@ -7,10 +7,9 @@ import math
 import pytest
 import torch
 
-from _util import log, rel_l2, worst_block_rel_l2
-from test_split_precision_blocks_gpu import (ENC_CHUNK, ENC_MODULES, SPLIT_BLOCK_TOL, VAE_CHUNK, VAE_MODULES, _run,
-                                             _skip_without_gpu, enc_sd, enc_taps, vae_sd, vae_taps)  # noqa: F401
-from test_vae_gpu import _crop_like, _uniform
+from _util import (ENC_CHUNK, ENC_MODULES, SPLIT_BLOCK_TOL, VAE_CHUNK, VAE_MODULES, crop_like_images, encoder_taps,
+                   encoder_weights, log, rel_l2, run_block, skip_without_gpu, uniform_images, vae_encoder_taps,
+                   worst_block_rel_l2)
 
 pytestmark = pytest.mark.gpu
 
@@ -42,8 +41,29 @@ def _module_gate(pred):
 
 
 @pytest.fixture(scope="module")
+def enc_sd(seeded_state_dict):
+    return encoder_weights(seeded_state_dict)
+
+
+@pytest.fixture(scope="module")
+def enc_taps(enc_sd):
+    return encoder_taps(enc_sd)
+
+
+@pytest.fixture(scope="module")
+def vae_sd():
+    from nope_b200.synth_weights import make_vae_state_dict
+    return make_vae_state_dict(seed=0, decoder=True)
+
+
+@pytest.fixture(scope="module")
+def vae_taps(vae_sd):
+    return vae_encoder_taps(vae_sd)
+
+
+@pytest.fixture(scope="module")
 def encoder16(enc_sd):
-    _skip_without_gpu()
+    skip_without_gpu()
     from nope_b200.encoder import FeatureExtractor
     fe = FeatureExtractor(descriptor_size=8, precision="fp16").cuda()
     fe.load_state_dict(enc_sd)
@@ -52,7 +72,7 @@ def encoder16(enc_sd):
 
 @pytest.fixture(scope="module")
 def encoder_split(enc_sd):
-    _skip_without_gpu()
+    skip_without_gpu()
     from nope_b200.encoder import FeatureExtractor
     fe = FeatureExtractor(descriptor_size=8).cuda()
     fe.load_state_dict(enc_sd)
@@ -61,14 +81,14 @@ def encoder_split(enc_sd):
 
 @pytest.fixture(scope="module")
 def vae16(vae_sd):
-    _skip_without_gpu()
+    skip_without_gpu()
     from nope_b200.vae import VAE_StableDiffusion
     return VAE_StableDiffusion(device="cuda:0", name="VAE", precision="fp16").load_state_dict(vae_sd)
 
 
 @pytest.fixture(scope="module")
 def vae_split(vae_sd):
-    _skip_without_gpu()
+    skip_without_gpu()
     from nope_b200.vae import VAE_StableDiffusion
     return VAE_StableDiffusion(device="cuda:0", name="VAE").load_state_dict(vae_sd)
 
@@ -76,7 +96,7 @@ def vae_split(vae_sd):
 # ------------------------------------------------------------------ 1. every module against the float64 oracle
 def _check_module16(engine, taps, name, n, pred, tag):
     x, ref = taps[name]
-    out, pair = _run(engine, name, x[:n].float())
+    out, pair = run_block(engine, name, x[:n].float())
     assert out.shape == ref[:n].shape
     e, img = worst_block_rel_l2(out, ref[:n])
     log("fp16_block", engine=tag, module=name, n=n, rel_l2=e, worst_image=img, predicted=pred, ratio=e / pred)
@@ -108,7 +128,7 @@ def test_vae_fp16_module_matches_the_float64_oracle(vae16, vae_taps, name, n):
 @pytest.mark.parametrize("engine", ["encoder", "vae"])
 def test_fp16_latents_match_the_prediction(engine, enc_sd, vae_sd, encoder16, encoder_split, vae16, vae_split):
     from oracle import unet_oracle, vae_oracle
-    x = torch.cat([_uniform(30, 2), _crop_like(30, 2)]).cuda()
+    x = torch.cat([uniform_images(30, 2), crop_like_images(30, 2)]).cuda()
     if engine == "encoder":
         ref = unet_oracle.encode_image({k: v.cuda().double() for k, v in enc_sd.items()}, x.double())
         z16, zs = encoder16.encode_image(x), encoder_split.encode_image(x)
@@ -128,7 +148,7 @@ def test_fp16_latents_match_the_prediction(engine, enc_sd, vae_sd, encoder16, en
 @pytest.mark.parametrize("engine,B", [("encoder", 33), ("vae", 17)])
 def test_fp16_latent_does_not_depend_on_the_batch(engine, B, encoder16, vae16):
     enc = encoder16 if engine == "encoder" else vae16
-    x = torch.cat([_uniform(40, B - B // 2), _crop_like(41, B // 2)]).cuda()
+    x = torch.cat([uniform_images(40, B - B // 2), crop_like_images(41, B // 2)]).cuda()
     z = enc.encode_image(x)
     for b in range(B):
         assert torch.equal(enc.encode_image(x[b:b + 1])[0], z[b]), b
@@ -139,7 +159,7 @@ def test_fp16_rotated_entry_points_equal_encode_of_the_rotated_batch(engine, enc
     from nope_b200.inplane import rotate_images
     from nope_b200.inplane_refine import rotate_pairs
     enc = encoder16 if engine == "encoder" else vae16
-    x = torch.cat([_crop_like(42, 2), _uniform(42, 1)]).cuda()
+    x = torch.cat([crop_like_images(42, 2), uniform_images(42, 1)]).cuda()
     A = 12                                                  # 36 pairs: crosses the chunk boundaries of both engines
     z = enc.encode_image_inplane(x, A)
     assert torch.equal(z.reshape(3 * A, *z.shape[2:]), enc.encode_image(rotate_images(x, A).reshape(3 * A, 3, 256, 256)))
@@ -196,7 +216,7 @@ def test_inplane_search_with_an_fp16_encoder(seeded_state_dict, enc_sd):
     between rank 1 and rank 2 exceeds twice the bound there"""
     from nope_b200.encoder import FeatureExtractor
     from nope_b200.model import build_model
-    _skip_without_gpu()
+    skip_without_gpu()
     Q, A = 16, 36
     model = build_model(device="cuda:0").load_state_dict(seeded_state_dict).eval()
     split = model.u_net.encoder
@@ -236,7 +256,7 @@ def test_inplane_search_with_an_fp16_encoder(seeded_state_dict, enc_sd):
 def test_split_and_fp16_engines_side_by_side(engine, enc_sd, vae_sd, encoder16, encoder_split, vae16, vae_split):
     from nope_b200.encoder import FeatureExtractor
     from nope_b200.vae import VAE_StableDiffusion
-    x = torch.cat([_uniform(50, 2), _crop_like(50, 3)]).cuda()
+    x = torch.cat([uniform_images(50, 2), crop_like_images(50, 3)]).cuda()
     if engine == "encoder":
         a, h = encoder_split, encoder16
         fresh = FeatureExtractor(descriptor_size=8).cuda()

@@ -5,45 +5,18 @@ engine against the hand-written chain of its stages; shared frames; host synchro
 nothing here says how accurate a trained model is on real frames."""
 import math
 import types
-import warnings
 
 import numpy as np
 import pytest
 import torch
 
 import crop_camera_oracle as cco
-from oracle import render_oracle as ro
+from _scenes import H, K3, W, inside, make_mesh, pose, rot, with_objects
+from _util import count_host_syncs, same_bits
 
 pytestmark = pytest.mark.gpu
 
-K3 = np.array([[1075.65091572, 0.0, 360.0], [0.0, 1073.90347929, 270.0], [0.0, 0.0, 1.0]])   # Primesense
-H, W = 540, 720
 S = 256
-MESHES = {"box": lambda: ro.box(), "sphere": lambda: ro.sphere(40.0, 2)}
-
-
-def _bits(x):
-    x = torch.as_tensor(x).detach().cpu().to(torch.float64).contiguous()
-    return x.view(torch.int64)
-
-
-def _same_bits(a, b):
-    return torch.equal(_bits(a), _bits(b))
-
-
-def _mesh(name):
-    from nope_b200.vsd import Mesh
-    v, f = MESHES[name]()
-    diameter = float(np.max(np.linalg.norm(v[:, None].astype(np.float64) - v[None], axis=2)))
-    return Mesh(v, f), diameter
-
-
-def _pose(R, t):
-    T = np.eye(4)
-    T[:3, :3], T[:3, 3] = R, t
-    return T
-
-
 def _scene(mesh, seed, n, corners=False):
     """n true poses with the object wholly inside the 720 x 540 frame, its centre anywhere in the frame (or within
     110 px of a frame corner), 400 ... 1200 mm deep -> (R [n, 3, 3], t [n, 3], masks uint8 0 / 255 [n, H, W] CUDA)"""
@@ -51,7 +24,7 @@ def _scene(mesh, seed, n, corners=False):
     rng = np.random.default_rng(seed)
     Rs, ts, ms = [], [], []
     while len(Rs) < n:
-        R = ro.look_pose(*rng.uniform(-math.pi, math.pi, 3))[:3, :3].astype(np.float64)
+        R = rot(rng)
         z = rng.uniform(700.0 if corners else 400.0, 1200.0)
         if corners:
             cu, cv = [(0, 0), (W, 0), (0, H), (W, H)][len(Rs) % 4]
@@ -59,9 +32,8 @@ def _scene(mesh, seed, n, corners=False):
         else:
             u, v = rng.uniform(0, W), rng.uniform(0, H)
         t = np.linalg.solve(K3, [u, v, 1.0]) * z
-        m = render_depth(mesh, torch.from_numpy(_pose(R, t)), K3, (H, W))[0] > 0
-        rows, cols = m.any(1).nonzero(), m.any(0).nonzero()
-        if len(rows) == 0 or rows.min() == 0 or cols.min() == 0 or rows.max() == H - 1 or cols.max() == W - 1:
+        m = render_depth(mesh, torch.from_numpy(pose(R, t)), K3, (H, W))[0] > 0
+        if not inside(m):
             continue
         Rs.append(R), ts.append(t), ms.append(m.to(torch.uint8) * 255)
     return np.stack(Rs), np.stack(ts), torch.stack(ms)
@@ -87,10 +59,10 @@ def test_crop_camera_and_rotate_equal_the_oracle(keep_inplane, F):
     Rv = crop_camera(torch.from_numpy(P).cuda(), keep_inplane)
     Rv_o = cco.crop_camera(P, keep_inplane)
     assert Rv.dtype == torch.float64 and Rv.shape == (F, 3, 3) and Rv.is_cuda
-    assert _same_bits(Rv, Rv_o)
+    assert same_bits(Rv, Rv_o)
     if F == 7:
         assert torch.equal(Rv[0].cpu(), torch.eye(3, dtype=torch.float64))
-    assert _same_bits(crop_camera(torch.from_numpy(P[0]).cuda(), keep_inplane), Rv_o[0])
+    assert same_bits(crop_camera(torch.from_numpy(P[0]).cuda(), keep_inplane), Rv_o[0])
     g = torch.Generator().manual_seed(F)
     for Pn in (1, 5, 36):
         Q, _ = torch.linalg.qr(torch.randn(F, Pn, 3, 3, generator=g, dtype=torch.float64))
@@ -99,14 +71,14 @@ def test_crop_camera_and_rotate_equal_the_oracle(keep_inplane, F):
             for fn, to_cam in ((to_camera, True), (to_crop, False)):
                 got = fn(R, Rv)
                 assert got.dtype == torch.float64 and got.shape == R.shape
-                assert _same_bits(got, cco.crop_rotate(Rv_o, R.double().cpu().numpy(), to_cam))
+                assert same_bits(got, cco.crop_rotate(Rv_o, R.double().cpu().numpy(), to_cam))
     # [F, 3, 3] input; out aliasing R through the C ABI
-    assert _same_bits(to_camera(Q[:, 0].cuda(), Rv), cco.crop_rotate(Rv_o, Q[:, :1].numpy(), True)[:, 0])
+    assert same_bits(to_camera(Q[:, 0].cuda(), Rv), cco.crop_rotate(Rv_o, Q[:, :1].numpy(), True)[:, 0])
     from nope_b200 import _lib
     for to_cam in (1, 0):
         R = Q.cuda().contiguous()
         _lib.check(_lib.load().nope_crop_rotate(_lib.ptr(Rv), F, _lib.ptr(R), 36, to_cam, _lib.ptr(R), None))
-        assert _same_bits(R, cco.crop_rotate(Rv_o, Q.numpy(), bool(to_cam)))
+        assert same_bits(R, cco.crop_rotate(Rv_o, Q.numpy(), bool(to_cam)))
 
 
 def test_round_trip_and_non_finite_rotations():
@@ -144,7 +116,7 @@ def test_crop_is_the_view_of_the_crop_camera(name, corners):
     without R_v (at (R, R_v t)) shows what the uncorrected rotation does."""
     from nope_b200.crop import crop_intrinsics, frame_crops
     from nope_b200.vsd import render_depth
-    mesh, d = _mesh(name)
+    mesh, d = make_mesh(name)
     n = 8
     R, t, masks = _scene(mesh, 5 + corners, n, corners)
     crops, t0, Rv, _ = frame_crops(_frames(masks), masks, K3, d)
@@ -157,7 +129,7 @@ def test_crop_is_the_view_of_the_crop_camera(name, corners):
     for b in range(n):
         tv = Rvh[b] @ t[b]
         for Rb, out in ((Rvh[b] @ R[b], ious), (R[b], raw)):
-            r = render_depth(mesh, torch.from_numpy(_pose(Rb, tv)), Kv[b], (S, S))[0].cpu() > 0
+            r = render_depth(mesh, torch.from_numpy(pose(Rb, tv)), Kv[b], (S, S))[0].cpu() > 0
             out.append(float((r & sil[b]).sum()) / float((r | sil[b]).sum()))
     tilt = [math.degrees(math.acos(min(1.0, (np.trace(Rvh[b]) - 1) / 2))) for b in range(n)]
     print(f"{name} corners={corners}: IoU min {min(ious):.4f}, without R_v min {min(raw):.4f}, "
@@ -174,25 +146,16 @@ def _detections(n=3, seed=7):
     """three detections of two objects (ids 91: box, 92: sphere) in two frames; detections 0 and 1 share frame 0
     -> (meshes {id: (mesh, d)}, ids, R [n, 3, 3], t [n, 3], masks, frames [2, H, W, 3], frame_idx)"""
     from nope_b200.vsd import render_depth
-    meshes = {91: _mesh("box"), 92: _mesh("sphere")}
+    meshes = {91: make_mesh("box"), 92: make_mesh("sphere")}
     ids = [91, 92, 91]
     rng = np.random.default_rng(seed)
     spots = [(150.0, 130.0, 700.0), (560.0, 380.0, 900.0), (400.0, 250.0, 600.0)]
-    R = np.stack([ro.look_pose(*rng.uniform(-math.pi, math.pi, 3))[:3, :3].astype(np.float64) for _ in ids])
+    R = np.stack([rot(rng) for _ in ids])
     t = np.stack([np.linalg.solve(K3, [u, v, 1.0]) * z for u, v, z in spots])
-    masks = torch.stack([(render_depth(meshes[i][0], torch.from_numpy(_pose(R[b], t[b])), K3, (H, W))[0] > 0)
+    masks = torch.stack([(render_depth(meshes[i][0], torch.from_numpy(pose(R[b], t[b])), K3, (H, W))[0] > 0)
                          .to(torch.uint8) * 255 for b, i in enumerate(ids)])
     frames = torch.stack([_frames(masks[0] | masks[1]), _frames(masks[2])])
     return meshes, ids, R, t, masks, frames, torch.tensor([0, 0, 1])
-
-
-def _with_objects(model, meshes):
-    from nope_b200 import bop
-    for i, (mesh, d) in meshes.items():
-        info = {"diameter": d, "symmetries_discrete": [], "symmetries_continuous": []}
-        model.tless_cad[i] = mesh
-        model.bop_models[i] = {"diameter": d, "symmetries": bop.symmetry_transformations(info), "info": info}
-    return model
 
 
 def test_frames_to_pose_with_the_true_crop_rotation():
@@ -203,7 +166,7 @@ def test_frames_to_pose_with_the_true_crop_rotation():
     from nope_b200.crop import frame_crops, to_crop
     from nope_b200.model import PoseConditional
     meshes, ids, R, t, masks, frames, fi = _detections()
-    model = _with_objects(PoseConditional(types.SimpleNamespace(device=torch.device("cuda", 0))), meshes)
+    model = with_objects(PoseConditional(types.SimpleNamespace(device=torch.device("cuda", 0))), meshes)
     d = np.array([meshes[i][1] for i in ids])
     _, t0, Rv, _ = frame_crops(frames, masks, K3, d, frame_idx=fi)
     k = 2
@@ -272,7 +235,7 @@ def _chain(model, meshes, ids, frames, masks, fi, sc, refine, refiner=None):
 def test_predict_pose_frames_equals_the_chain(gpu_model, engine_scene, refine, refined_search):
     from nope_b200.inplane_refine import InplaneRefiner
     meshes, ids, _, _, masks, frames, fi = _detections()
-    model = _with_objects(gpu_model, meshes)
+    model = with_objects(gpu_model, meshes)
     sc = engine_scene
     refiner = InplaneRefiner(sc["tp"], angles=6, steps=2) if refined_search else None
     out = model.predict_pose_frames(frames, masks, K3, ids, sc["ref"], sc["rel"], sc["tp"], angles=6, k=3,
@@ -287,41 +250,28 @@ def test_predict_pose_frames_equals_the_chain(gpu_model, engine_scene, refine, r
         assert torch.equal(out[key], dup[key]), key
 
 
-def _syncs(fn):
-    """(result, the host synchronisations torch's sync debug mode reports during fn())"""
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as w:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            out = fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    torch.cuda.synchronize()
-    return out, sum("called a synchronizing CUDA operation" in str(x.message) for x in w)
-
-
 def test_synchronisations(gpu_model, engine_scene):
     """predict_pose_frames synchronises as often as its stages do on their own, and frame_crops once (its copy of
     t0).  Sync debug mode sees synchronisation on the Python / torch side only."""
     from nope_b200 import translation
     from nope_b200.crop import frame_crops, to_camera
     meshes, ids, _, _, masks, frames, fi = _detections()
-    model = _with_objects(gpu_model, meshes)
+    model = with_objects(gpu_model, meshes)
     sc = engine_scene
     tp = sc["tp"].cuda()
     args = (frames, masks, K3, ids, sc["ref"], sc["rel"], tp)
     model.predict_pose_frames(*args, angles=6, k=3, frame_idx=fi)            # warm-up
-    _, n_all = _syncs(lambda: model.predict_pose_frames(*args, angles=6, k=3, frame_idx=fi))
+    _, n_all = count_host_syncs(lambda: model.predict_pose_frames(*args, angles=6, k=3, frame_idx=fi))
     d = np.array([meshes[i][1] for i in ids])
-    (crops, t0, Rv, _), n_crop = _syncs(lambda: frame_crops(frames, masks, K3, d, frame_idx=fi))
-    (R_crop, *_), n_search = _syncs(lambda: model.predict_pose_inplane(crops, sc["ref"], sc["rel"], tp, k=3, angles=6))
-    R, n_rot = _syncs(lambda: to_camera(R_crop, Rv))
+    (crops, t0, Rv, _), n_crop = count_host_syncs(lambda: frame_crops(frames, masks, K3, d, frame_idx=fi))
+    (R_crop, *_), n_search = count_host_syncs(lambda: model.predict_pose_inplane(crops, sc["ref"], sc["rel"], tp, k=3,
+                                                                                  angles=6))
+    R, n_rot = count_host_syncs(lambda: to_camera(R_crop, Rv))
     n_fit = 0
     for i in sorted(set(ids)):
         rows = torch.tensor([b for b, j in enumerate(ids) if j == i]).cuda()
-        _, n = _syncs(lambda: translation.estimate_translation(meshes[i][0], R[rows], K3[None].repeat(len(rows), 0),
-                                                               masks[rows], t_init=t0[rows]))
+        _, n = count_host_syncs(lambda: translation.estimate_translation(
+            meshes[i][0], R[rows], K3[None].repeat(len(rows), 0), masks[rows], t_init=t0[rows]))
         n_fit += n
     print(f"syncs: predict_pose_frames {n_all}, frame_crops {n_crop}, search {n_search}, to_camera {n_rot}, "
           f"fits {n_fit}")

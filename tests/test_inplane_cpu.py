@@ -1,10 +1,9 @@
 """CPU: the in-plane rotation search without a device -- the angle table, the pose rule against the reference's own
-in-plane helpers (tests/golden/inplane.npz), the pinhole identity behind it, the oracle's exact cases, the ABI
-declarations and refusals, and the Python argument errors."""
+in-plane helpers (tests/golden/inplane.npz), the pinhole identity behind it, the oracle's exact cases, the ABI's
+refusals, and the Python argument errors."""
 import ctypes as C
 import math
 import os
-import re
 import types
 
 import numpy as np
@@ -12,8 +11,6 @@ import pytest
 import torch
 
 from oracle import inplane_oracle as orc
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 # ------------------------------------------------------------------ convention
@@ -116,20 +113,6 @@ def test_oracle_bilinear_and_joint_topk():
 
 
 # ------------------------------------------------------------------ ABI
-def _declared():
-    src = open(os.path.join(ROOT, "include", "nope_b200.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return set(re.findall(r"\b(nope_[a-z0-9_]+)\s*\(", src))
-
-
-def test_header_declares_and_lib_binds_the_new_calls():
-    from nope_b200 import _lib
-    lib = _lib.load()
-    for n in ("nope_inplane_rotate", "nope_encoder_encode_inplane"):
-        assert n in _declared() and n in _lib.SIGNATURES and hasattr(lib, n)
-    assert _lib.EXPECTED_ABI == 3 and lib.nope_abi_version() == 3
-
-
 P = C.c_void_p(256)
 
 

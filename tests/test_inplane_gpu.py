@@ -8,6 +8,7 @@ import math
 import pytest
 import torch
 
+from _util import no_host_sync
 from oracle import inplane_oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -164,12 +165,8 @@ def test_search_does_not_synchronise(gpu_model, scene):
     q, r, rel = scene["q"], scene["r"], scene["rel"]
     tp = scene["tp"].cuda()
     first = gpu_model.predict_pose_inplane(q, r, rel, tp, k=K, angles=6)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         out = gpu_model.predict_pose_inplane(q, r, rel, tp, k=K, angles=6)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     torch.cuda.synchronize()
     for x, y in zip(out, first):
         assert torch.equal(x, y)

@@ -1,10 +1,8 @@
 """CPU: the joint roll and viewpoint refinement without a device -- the xy stencil and the step schedule, the torch
-oracle's propose / select conventions (and a whole refinement of a smooth synthetic score with it), the ABI
-declarations and refusals, and the Python argument errors."""
+oracle's propose / select conventions (and a whole refinement of a smooth synthetic score with it), the ABI's
+refusals, and the Python argument errors."""
 import ctypes as C
 import math
-import os
-import re
 import types
 
 import numpy as np
@@ -13,8 +11,6 @@ import torch
 
 from oracle import inplane_refine_oracle as orc
 from oracle import refine_oracle
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _angle(R):
@@ -179,24 +175,6 @@ def test_oracle_refinement_of_a_smooth_score_converges():
 
 
 # ------------------------------------------------------------------ ABI
-def _declared():
-    src = open(os.path.join(ROOT, "include", "nope_b200.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return set(re.findall(r"\b(nope_[a-z0-9_]+)\s*\(", src))
-
-
-NEW_CALLS = ("nope_inplane_rotate_pairs", "nope_encoder_encode_rotated", "nope_pose_refine_inplane_propose",
-             "nope_pose_refine_inplane_select")
-
-
-def test_header_declares_and_lib_binds_the_new_calls():
-    from nope_b200 import _lib
-    lib = _lib.load()
-    for n in NEW_CALLS:
-        assert n in _declared() and n in _lib.SIGNATURES and hasattr(lib, n)
-    assert _lib.EXPECTED_ABI == 3 and lib.nope_abi_version() == 3
-
-
 P = C.c_void_p(256)     # never dereferenced: every case below is refused before any CUDA call
 
 

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 import torch
 
+from _util import no_host_sync
 from oracle import inplane_oracle
 from oracle import inplane_refine_oracle as orc
 
@@ -257,12 +258,8 @@ def test_does_not_synchronise(gpu_model, grids, scene):
     caught here."""
     q, r, rel, ref = scene["q"], scene["r"], grids["rel"], grids["ref"]
     first = gpu_model.predict_pose_inplane_refined(q, r, rel, ref, k=K, keep=KEEP)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         out = gpu_model.predict_pose_inplane_refined(q, r, rel, ref, k=K, keep=KEEP)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     torch.cuda.synchronize()
     for x, y in zip(out, first):
         assert torch.equal(x, y)

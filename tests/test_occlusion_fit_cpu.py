@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+import contour_refine_oracle as cro
 import occlusion_fit_oracle as ofo
 import translation_oracle as to
 from oracle import render_oracle as ro
@@ -42,7 +43,7 @@ def test_the_true_pose_is_a_fixed_point_under_occlusion(shift):
     for occ in (O, O | Ob):
         t1, iou, _ = ofo.fit_translation(render, R, t, M, occ, K4, 3)
         assert np.abs(t1 - t).max() <= 1e-6 and iou == 1.0, (t1, t, iou)
-        R2, t2, fit, sums = ofo.refine_contour(render, R, t, M, occ, K4, TAUS, 40.0)
+        R2, t2, fit, sums = cro.refine(render, R, t, M, K4, TAUS, 40.0, occ=occ)
         assert np.array_equal(R2, R) and np.array_equal(t2, t) and fit[3] == 1.0, fit
         assert fit[0] >= 6 and fit[1] >= fit[0] and fit[2] == 0.0
     t1, iou, _ = to.fit(render, R, t, M, K4, 3)                  # the visible mask alone pulls the fit away
@@ -50,13 +51,12 @@ def test_the_true_pose_is_a_fixed_point_under_occlusion(shift):
 
 
 def test_an_all_zero_occluder_is_the_plain_fit():
-    import contour_refine_oracle as cro
     render, R, t, M, _, _ = _scene(10.0)
     zero = np.zeros_like(M)
     t0 = t + [2.0, -1.5, 12.0]
     a, b = ofo.fit_translation(render, R, t0, M, zero, K4, 3), to.fit(render, R, t0, M, K4, 3)
     assert np.array_equal(a[0], b[0]) and a[1] == b[1] and a[2] == b[2]
-    a, b = ofo.refine_contour(render, R, t0, M, zero, K4, TAUS, 40.0), cro.refine(render, R, t0, M, K4, TAUS, 40.0)
+    a, b = cro.refine(render, R, t0, M, K4, TAUS, 40.0, occ=zero), cro.refine(render, R, t0, M, K4, TAUS, 40.0)
     assert all(np.array_equal(x, y, equal_nan=True) for x, y in zip(a, b))
 
 
@@ -65,10 +65,10 @@ def test_contour_pixels_next_to_an_occluder_are_not_counted():
     D[2:7, 3:9] = 500.0
     occ = np.zeros((9, 12), np.uint8)
     occ[4, 9] = 1                                                 # right of the right edge's middle pixel
-    cont = ofo.cro.contour(D)
-    assert cont[4, 8] and ofo.known4(occ).sum() == 9 * 12 - 5
-    phi = ofo.cro.sdf(ofo.visible(D > 0, occ))
-    _, nc = ofo.accumulate(D, phi, K4, np.array([0.0, 0.0, 500.0]), 3.0, 40.0, occ)
+    cont = cro.contour(D)
+    assert cont[4, 8] and cro.known4(occ).sum() == 9 * 12 - 5
+    phi = cro.sdf(cro.visible(D > 0, occ))
+    _, nc = cro.accumulate(D, phi, K4, np.array([0.0, 0.0, 500.0]), 3.0, 40.0, occ)
     assert nc == cont.sum() - 1
 
 

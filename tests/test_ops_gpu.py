@@ -86,43 +86,6 @@ def test_upsample(dev):
     assert torch.equal(out.cpu(), F.interpolate(x, scale_factor=2, mode="nearest"))
 
 
-CONV_CASES = [
-    # n, C0, C1, Cout, S, mode
-    (2, 192, 0, 192, 32, "3x3"), (3, 192, 192, 192, 32, "3x3"), (3, 384, 192, 384, 16, "3x3"),
-    (5, 768, 384, 768, 8, "3x3"), (9, 1536, 768, 1536, 4, "3x3"), (2, 384, 0, 384, 16, "1x1"),
-    (3, 128, 0, 192, 32, "1x1"), (3, 192, 192, 192, 32, "1x1"), (2, 192, 0, 192, 16, "unshuffle"),
-    (5, 384, 0, 768, 4, "unshuffle"), (130, 768, 0, 12096, 1, "1x1"), (1, 64, 0, 64, 32, "3x3"),
-    (3, 384, 0, 192, 32, "upsample3x3"), (5, 768, 0, 384, 16, "upsample3x3"),
-    (7, 1536, 0, 768, 8, "upsample3x3"),
-]
-
-
-def conv_reference(x0, x1, w, b, mode):
-    x = x0 if x1 is None else torch.cat([x0, x1], dim=1)
-    if mode == "3x3":
-        return F.conv2d(x, w, b, padding=1)
-    if mode == "1x1":
-        return F.conv2d(x, w, b)
-    if mode == "upsample3x3":
-        return F.conv2d(F.interpolate(x, scale_factor=2, mode="nearest"), w, b, padding=1)
-    n, c, hh, ww = x.shape
-    x = x.reshape(n, c, hh // 2, 2, ww // 2, 2).permute(0, 1, 3, 5, 2, 4).reshape(n, c * 4, hh // 2, ww // 2)
-    return F.conv2d(x, w, b)
-
-
-def make_conv_case(n, C0, C1, Cout, S, mode, seed=0):
-    g = _g(seed + n + C0 + Cout + S)
-    cin = C0 + C1
-    sin = 2 * S if mode == "unshuffle" else (S // 2 if mode == "upsample3x3" else S)
-    x0 = h(torch.randn(n, C0, sin, sin, generator=g))
-    x1 = h(torch.randn(n, C1, sin, sin, generator=g)) if C1 else None
-    kk = {"3x3": 3, "1x1": 1, "unshuffle": 1, "upsample3x3": 3}[mode]
-    cw = cin * 4 if mode == "unshuffle" else cin
-    w = h(torch.randn(Cout, cw, kk, kk, generator=g) / (cw * kk * kk) ** 0.5)
-    b = 0.1 * torch.randn(Cout, generator=g)
-    return x0, x1, w, b
-
-
 @pytest.mark.parametrize("metric", ["l2", "cosine", "cosine_occlusion"])
 def test_score_topk(dev, metric):
     from nope_b200.model import score_topk

@@ -1,10 +1,8 @@
 """CPU: the off-grid pose refinement without a device -- the lattice stencil and the grid spacing it starts from,
 the torch oracle's propose / select conventions (and a whole refinement of a smooth synthetic score with it), the
-ABI declarations and refusals, and the Python argument errors."""
+ABI's refusals, and the Python argument errors."""
 import ctypes as C
 import math
-import os
-import re
 import types
 
 import numpy as np
@@ -12,8 +10,6 @@ import pytest
 import torch
 
 from oracle import refine_oracle as orc
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _angle(R):
@@ -146,20 +142,6 @@ def test_oracle_refinement_of_a_smooth_score_goes_below_the_grid():
 
 
 # ------------------------------------------------------------------ ABI
-def _declared():
-    src = open(os.path.join(ROOT, "include", "nope_b200.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return set(re.findall(r"\b(nope_[a-z0-9_]+)\s*\(", src))
-
-
-def test_header_declares_and_lib_binds_the_new_calls():
-    from nope_b200 import _lib
-    lib = _lib.load()
-    for n in ("nope_pose_refine_propose", "nope_pose_refine_select"):
-        assert n in _declared() and n in _lib.SIGNATURES and hasattr(lib, n)
-    assert _lib.EXPECTED_ABI == 3
-
-
 @pytest.mark.parametrize("R,keep,B,Q,needle", [(2, 0, 2, 1, "keep"), (2, 65, 2, 1, "keep"), (3, 2, 2, 1, "R")])
 def test_propose_rejects_bad_sizes(R, keep, B, Q, needle):
     from nope_b200 import _lib

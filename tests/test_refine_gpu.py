@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 import torch
 
+from _util import no_host_sync
 from oracle import refine_oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -209,12 +210,8 @@ def test_refine_does_not_synchronise(gpu_model, grids, feats):
     rel = grids["rel"][2]
     seeds = u.sweep(rf, rel, query_feat=qf, want_emb=False, k=KEEP)["topi"]
     first = refine(u, rf, qf, rel, seeds, grids["ref2"], k=K)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         out = refine(u, rf, qf, rel, seeds, grids["ref2"], k=K)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     torch.cuda.synchronize()
     assert torch.equal(out["score"], first["score"]) and torch.equal(out["D"], first["D"])
 

@@ -14,26 +14,11 @@ import ctypes as C
 import pytest
 import torch
 
-from _util import log, pair_tiles, pick_bn, rounds, worst_block_rel_l2
-from test_vae_gpu import _crop_like, _uniform
+from _util import (DEC_CHUNK, ENC_CHUNK, ENC_MODULES, SPLIT_BLOCK_TOL, VAE_CHUNK, VAE_MODULES, encoder_taps,
+                   encoder_weights, log, mixed_images, pair_tiles, pick_bn, rounds, run_block, skip_without_gpu,
+                   vae_encoder_taps, worst_block_rel_l2)
 
-# Worst per-image rel-L2 of one module against the float64 oracle.  Measured on an H100 80GB HBM3 at a 700 W power
-# limit, over every module at n = 1, 3 and the chunk: template encoder worst 1.29e-5 (projector), median 4.9e-6; VAE
-# encoder worst 1.70e-5 (down_blocks.2.downsamplers.0), median 8.6e-6; VAE decoder worst 1.71e-5
-# (mid_block.resnets.0), median 8.1e-6.  The error follows K (fp32 tensor-core accumulation over up to 13 824
-# products), above the ~1e-6 of the dropped A_lo W_lo term.  The gate is 2.6x the worst rather than 3x so that fp16
-# inputs (2.0-2.9e-4 on the SENSITIVE modules) miss it by at least 4x.
-SPLIT_BLOCK_TOL = 4.5e-5
 
-ENC_CHUNK, VAE_CHUNK, DEC_CHUNK = 32, 16, 8
-
-ENC_MODULES = (["stem"] + [f"backbone.layer{l}.{b}" for l, n in ((1, 3), (2, 4), (3, 6), (4, 3)) for b in range(n)]
-               + ["projector"])
-VAE_MODULES = (["encoder.conv_in"]
-               + [m for i in range(4) for m in [f"encoder.down_blocks.{i}.resnets.{j}" for j in range(2)]
-                  + ([f"encoder.down_blocks.{i}.downsamplers.0"] if i < 3 else [])]
-               + ["encoder.mid_block.resnets.0", "encoder.mid_block.attentions.0", "encoder.mid_block.resnets.1",
-                  "encoder.conv_out"])
 DEC_MODULES = (["decoder.conv_in", "decoder.mid_block.resnets.0", "decoder.mid_block.attentions.0",
                 "decoder.mid_block.resnets.1"]
                + [m for i in range(4) for m in [f"decoder.up_blocks.{i}.resnets.{j}" for j in range(3)]
@@ -107,24 +92,14 @@ def test_oracle_taps_chain_the_modules():
 
 
 # ------------------------------------------------------------------ GPU fixtures
-def _images(n, seed):
-    return torch.cat([_uniform(seed, n - n // 2), _crop_like(seed, n // 2)])
-
-
-def _skip_without_gpu():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-
-
 @pytest.fixture(scope="module")
 def enc_sd(seeded_state_dict):
-    return {k[len("encoder."):]: v for k, v in seeded_state_dict.items()
-            if k.startswith("encoder.backbone.") or k.startswith("encoder.projector.")}
+    return encoder_weights(seeded_state_dict)
 
 
 @pytest.fixture(scope="module")
 def encoder(enc_sd):
-    _skip_without_gpu()
+    skip_without_gpu()
     from nope_b200.encoder import FeatureExtractor
     fe = FeatureExtractor(descriptor_size=8).cuda()
     fe.load_state_dict(enc_sd)
@@ -133,12 +108,7 @@ def encoder(enc_sd):
 
 @pytest.fixture(scope="module")
 def enc_taps(enc_sd):
-    _skip_without_gpu()
-    from oracle import unet_oracle
-    taps = {}
-    unet_oracle.encode_image({k: v.cuda().double() for k, v in enc_sd.items()},
-                             _images(ENC_CHUNK, 70).cuda().double(), taps=taps)
-    return taps
+    return encoder_taps(enc_sd)
 
 
 @pytest.fixture(scope="module")
@@ -149,39 +119,28 @@ def vae_sd():
 
 @pytest.fixture(scope="module")
 def vae(vae_sd):
-    _skip_without_gpu()
+    skip_without_gpu()
     from nope_b200.vae import VAE_StableDiffusion
     return VAE_StableDiffusion(device="cuda:0", name="VAE").load_state_dict(vae_sd)
 
 
 @pytest.fixture(scope="module")
 def vae_taps(vae_sd):
-    _skip_without_gpu()
-    from oracle import vae_oracle
-    taps = {}
-    vae_oracle.encode(vae_sd, _images(VAE_CHUNK, 71).cuda().double(), taps=taps)
-    return taps
+    return vae_encoder_taps(vae_sd)
 
 
 @pytest.fixture(scope="module")
 def dec_taps(vae_sd, vae):
-    _skip_without_gpu()
+    skip_without_gpu()
     import vae_decoder_oracle
     taps = {}
-    vae_decoder_oracle.decode(vae_sd, vae.encode_image(_images(DEC_CHUNK, 72).cuda()).double(), taps=taps)
+    vae_decoder_oracle.decode(vae_sd, vae.encode_image(mixed_images(DEC_CHUNK, 72).cuda()).double(), taps=taps)
     return taps
-
-
-def _run(engine, name, x):
-    """-> (fp32 output, hi + lo of the pair or None)"""
-    if isinstance(engine, torch.nn.Module):
-        return engine.run_block(name, x), None
-    return engine.run_block(name, x, want_pair=not name.endswith("conv_out"))
 
 
 def _check_module(engine, taps, name, n, tag):
     x, ref = taps[name]
-    out, pair = _run(engine, name, x[:n].float())
+    out, pair = run_block(engine, name, x[:n].float())
     assert out.shape == ref[:n].shape
     e, img = worst_block_rel_l2(out, ref[:n])
     co, ho = ref.shape[1], ref.shape[2]
@@ -251,9 +210,9 @@ def test_the_gate_separates_split_precision_from_fp16(encoder, vae, enc_taps, va
         vae, dec_taps if name.startswith("decoder.") else vae_taps)
     x, ref = taps[name]
     n = 3
-    out, _ = _run(engine, name, x[:n].half().float())
+    out, _ = run_block(engine, name, x[:n].half().float())
     e, _ = worst_block_rel_l2(out, ref[:n])
-    exact, _ = worst_block_rel_l2(_run(engine, name, x[:n].float())[0], ref[:n])
+    exact, _ = worst_block_rel_l2(run_block(engine, name, x[:n].float())[0], ref[:n])
     log("split_block_fp16_input", module=name, rel_l2=e, split_rel_l2=exact, margin=e / SPLIT_BLOCK_TOL)
     assert e >= 4 * SPLIT_BLOCK_TOL, (name, e)
 

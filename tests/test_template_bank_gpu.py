@@ -4,14 +4,12 @@ against nope_score_topk_multi per detection, for every metric, with bank objects
 interleaved order; predict_pose_bank against retrieval_inplane and against the sweep path; the refined search against
 refine_inplane; predict_pose_frames(bank=) against its own chain; and its host synchronisations.  The weights are
 seeded: nothing here says how accurate a trained model is."""
-import math
-import warnings
-
 import numpy as np
 import pytest
 import torch
 
-from oracle import render_oracle as ro
+from _scenes import H, K3, W, make_mesh, pose, rot, with_objects
+from _util import count_host_syncs
 
 pytestmark = pytest.mark.gpu
 
@@ -200,50 +198,27 @@ def test_refined_search_equals_refine_inplane(request, scene):
 
 
 # ------------------------------------------------------------------ predict_pose_frames
-K3 = np.array([[1075.65091572, 0.0, 360.0], [0.0, 1073.90347929, 270.0], [0.0, 0.0, 1.0]])   # Primesense
-H, W = 540, 720
-
-
-def _pose(R, t):
-    T = np.eye(4)
-    T[:3, :3], T[:3, 3] = R, t
-    return T
-
-
 @pytest.fixture(scope="module")
 def frame_scene():
     """three detections of two objects (91: box, 92: sphere) in two frames, detections 0 and 1 in frame 0; a bank of
     objects 91, 92 and 93 (no detection) over the 42-pose grid"""
-    from nope_b200 import bop
     from nope_b200.poses import icosphere_object_rotations, synthetic_pose_batch
-    from nope_b200.vsd import Mesh, render_depth
+    from nope_b200.vsd import render_depth
     from oracle import inputs
-    meshes = {}
-    for i, (v, f) in ((91, ro.box()), (92, ro.sphere(40.0, 2))):
-        d = float(np.max(np.linalg.norm(v[:, None].astype(np.float64) - v[None], axis=2)))
-        meshes[i] = (Mesh(v, f), d)
+    meshes = {91: make_mesh("box"), 92: make_mesh("sphere")}
     ids = [91, 92, 91]
     rng = np.random.default_rng(7)
     spots = [(150.0, 130.0, 700.0), (560.0, 380.0, 900.0), (400.0, 250.0, 600.0)]
-    R = np.stack([ro.look_pose(*rng.uniform(-math.pi, math.pi, 3))[:3, :3].astype(np.float64) for _ in ids])
+    R = np.stack([rot(rng) for _ in ids])
     t = np.stack([np.linalg.solve(K3, [u, v, 1.0]) * z for u, v, z in spots])
-    masks = torch.stack([(render_depth(meshes[i][0], torch.from_numpy(_pose(R[b], t[b])), K3, (H, W))[0] > 0)
+    masks = torch.stack([(render_depth(meshes[i][0], torch.from_numpy(pose(R[b], t[b])), K3, (H, W))[0] > 0)
                          .to(torch.uint8) * 255 for b, i in enumerate(ids)])
     rgb = lambda m: m[..., None].expand(*m.shape, 3).contiguous()     # noqa: E731
     frames = torch.stack([rgb(masks[0] | masks[1]), rgb(masks[2])])
     _, ref = inputs.make_images(seed=4, batch=3)
-    infos = {i: {"diameter": d, "symmetries_discrete": [], "symmetries_continuous": []} for i, (_, d) in meshes.items()}
     return {"meshes": meshes, "ids": ids, "masks": masks, "frames": frames, "fi": torch.tensor([0, 0, 1]),
             "ref": ref.cuda(), "rel": synthetic_pose_batch(42, 3)[0].cuda(),
-            "tp": torch.from_numpy(icosphere_object_rotations(0)), "bank_ids": [91, 92, 93], "infos": infos,
-            "syms": {i: bop.symmetry_transformations(info) for i, info in infos.items()}}
-
-
-def _with_objects(model, fs):
-    for i, (mesh, d) in fs["meshes"].items():
-        model.tless_cad[i] = mesh
-        model.bop_models[i] = {"diameter": d, "symmetries": fs["syms"][i], "info": fs["infos"][i]}
-    return model
+            "tp": torch.from_numpy(icosphere_object_rotations(0)), "bank_ids": [91, 92, 93]}
 
 
 def _chain(model, fs, bank, refine, refiner, occluders):
@@ -281,7 +256,7 @@ def _chain(model, fs, bank, refine, refiner, occluders):
 def test_predict_pose_frames_with_a_bank_equals_the_chain(gpu_model, frame_scene, refine, refined_search, occluders):
     from nope_b200.inplane_refine import InplaneRefiner
     fs = frame_scene
-    model = _with_objects(gpu_model, fs)
+    model = with_objects(gpu_model, fs["meshes"])
     bank = model.build_template_bank(fs["bank_ids"], fs["ref"], fs["rel"], fs["tp"])
     refiner = InplaneRefiner(fs["tp"], angles=A, steps=2) if refined_search else None
     out = model.predict_pose_frames(fs["frames"], fs["masks"], K3, fs["ids"], angles=A, k=3, refiner=refiner,
@@ -291,23 +266,9 @@ def test_predict_pose_frames_with_a_bank_equals_the_chain(gpu_model, frame_scene
         assert torch.equal(out[key], ref[key]), key
 
 
-def _syncs(fn):
-    """(result, the host synchronisations torch's sync debug mode reports during fn())"""
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as w:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            out = fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    torch.cuda.synchronize()
-    return out, sum("called a synchronizing CUDA operation" in str(x.message) for x in w)
-
-
 def test_frames_with_a_bank_synchronise_no_more_than_with_references(gpu_model, frame_scene):
     fs = frame_scene
-    model = _with_objects(gpu_model, fs)
+    model = with_objects(gpu_model, fs["meshes"])
     bank = model.build_template_bank(fs["bank_ids"], fs["ref"], fs["rel"], fs["tp"])
     slots = [fs["bank_ids"].index(i) for i in fs["ids"]]
     tp = fs["tp"].cuda()
@@ -315,8 +276,10 @@ def test_frames_with_a_bank_synchronise_no_more_than_with_references(gpu_model, 
     triple = (fs["ref"][slots], fs["rel"][slots], tp)
     model.predict_pose_frames(*args, *triple, angles=A, k=3, frame_idx=fs["fi"])          # warm-up
     model.predict_pose_frames(*args, angles=A, k=3, frame_idx=fs["fi"], bank=bank)
-    _, n_triple = _syncs(lambda: model.predict_pose_frames(*args, *triple, angles=A, k=3, frame_idx=fs["fi"]))
-    out, n_bank = _syncs(lambda: model.predict_pose_frames(*args, angles=A, k=3, frame_idx=fs["fi"], bank=bank))
-    (R, n, a, sim), n_search = _syncs(lambda: model.predict_pose_bank(out["crops"], fs["ids"], bank, k=3, angles=A))
+    _, n_triple = count_host_syncs(lambda: model.predict_pose_frames(*args, *triple, angles=A, k=3, frame_idx=fs["fi"]))
+    out, n_bank = count_host_syncs(lambda: model.predict_pose_frames(*args, angles=A, k=3, frame_idx=fs["fi"],
+                                                                     bank=bank))
+    (R, n, a, sim), n_search = count_host_syncs(lambda: model.predict_pose_bank(out["crops"], fs["ids"], bank, k=3,
+                                                                                angles=A))
     print(f"syncs: with references {n_triple}, with the bank {n_bank}, predict_pose_bank alone {n_search}")
     assert n_bank <= n_triple and n_search == 0

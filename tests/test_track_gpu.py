@@ -4,20 +4,16 @@ track_pose_frames against the chain of its stages, with a bank and with referenc
 PoseTracker's searched, tracked, lost, new and dropped rows; and roll tracking over 48 frames through a stub engine
 whose templates do not depend on the pose.  The weights are seeded: nothing here says how well a trained model
 tracks."""
-import math
-import warnings
-
 import numpy as np
 import pytest
 import torch
 
 import track_oracle as to
-from oracle import render_oracle as ro
+from _scenes import H, K3, W, make_mesh, pose, rot, with_objects
+from _util import count_host_syncs, same_bits
 
 pytestmark = pytest.mark.gpu
 
-K3 = np.array([[1075.65091572, 0.0, 360.0], [0.0, 1073.90347929, 270.0], [0.0, 0.0, 1.0]])   # Primesense
-H, W = 540, 720
 A, KEEP, K = 6, 2, 3
 
 
@@ -32,11 +28,6 @@ def _seeds_raw(Rc, T):
     _lib.check(_lib.load().nope_track_seeds(_lib.ptr(rc), n, _lib.ptr(t), t.shape[0], _lib.ptr(D), _lib.ptr(seed),
                                             _lib.ptr(cs), None))
     return D.cpu().numpy(), seed.cpu().numpy(), cs.cpu().numpy()
-
-
-def _bits_equal(a, b):
-    a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
-    return a.dtype == b.dtype and a.shape == b.shape and np.array_equal(a.view(np.uint8), b.view(np.uint8))
 
 
 # ------------------------------------------------------------------ the seed kernel = the oracle
@@ -61,16 +52,16 @@ def test_seed_kernel_equals_the_oracle(level, Hn):
     want = to.track_seeds(Rc, grid)
     got = _seeds_raw(Rc, grid)
     for g, w in zip(got, want):
-        assert _bits_equal(g, w)
+        assert same_bits(g, w)
     ref = InplaneRefiner(grid, angles=36, steps=1)
     cen = seed_centres(torch.from_numpy(Rc).cuda()[None], ref)
     assert cen["D"].shape == (1, Hn, 3, 3) and cen["seed"].shape == (1, Hn) and cen["cossin"].shape == (1, Hn, 2)
     for name, w in zip(("D", "seed", "cossin"), want):
-        assert _bits_equal(cen[name][0].cpu().numpy(), w), name
+        assert same_bits(cen[name][0].cpu().numpy(), w), name
     # float32 priors are widened exactly
     cen32 = seed_centres(torch.from_numpy(Rc).float().cuda(), ref)
     for name, w in zip(("D", "seed", "cossin"), to.track_seeds(Rc.astype(np.float32).astype(np.float64), grid)):
-        assert _bits_equal(cen32[name].cpu().numpy(), w), name
+        assert same_bits(cen32[name].cpu().numpy(), w), name
     # ties and a NaN grid row
     T = grid.copy()
     T[-3:] = T[:3]
@@ -79,7 +70,7 @@ def test_seed_kernel_equals_the_oracle(level, Hn):
     want = to.track_seeds(Rt, T)
     assert want[1][-3] == 1 and want[1][-2] != 5 and want[1][-1] == 2
     for g, w in zip(_seeds_raw(Rt, T), want):
-        assert _bits_equal(g, w)
+        assert same_bits(g, w)
 
 
 # ------------------------------------------------------------------ refine_inplane with centres
@@ -149,39 +140,27 @@ def test_track_inplane_scores_and_seeds(gpu_model, grids, scene):
 
 
 # ------------------------------------------------------------------ track_pose_frames and PoseTracker
-def _pose(R, t):
-    T = np.eye(4)
-    T[:3, :3], T[:3, 3] = R, t
-    return T
-
-
 @pytest.fixture(scope="module")
 def frame_scene():
     """three detections of two objects (91: box, 92: sphere) in two frames, detections 0 and 1 in frame 0; a bank of
     objects 91, 92 and 93 (no detection) over the 42-pose grid"""
-    from nope_b200 import bop
     from nope_b200.poses import icosphere_object_rotations, synthetic_pose_batch
-    from nope_b200.vsd import Mesh, render_depth
+    from nope_b200.vsd import render_depth
     from oracle import inputs
-    meshes = {}
-    for i, (v, f) in ((91, ro.box()), (92, ro.sphere(40.0, 2))):
-        d = float(np.max(np.linalg.norm(v[:, None].astype(np.float64) - v[None], axis=2)))
-        meshes[i] = (Mesh(v, f), d)
+    meshes = {91: make_mesh("box"), 92: make_mesh("sphere")}
     ids = [91, 92, 91]
     rng = np.random.default_rng(8)
     spots = [(150.0, 130.0, 700.0), (560.0, 380.0, 900.0), (400.0, 250.0, 600.0)]
-    R = np.stack([ro.look_pose(*rng.uniform(-math.pi, math.pi, 3))[:3, :3].astype(np.float64) for _ in ids])
+    R = np.stack([rot(rng) for _ in ids])
     t = np.stack([np.linalg.solve(K3, [u, v, 1.0]) * z for u, v, z in spots])
-    masks = torch.stack([(render_depth(meshes[i][0], torch.from_numpy(_pose(R[b], t[b])), K3, (H, W))[0] > 0)
+    masks = torch.stack([(render_depth(meshes[i][0], torch.from_numpy(pose(R[b], t[b])), K3, (H, W))[0] > 0)
                          .to(torch.uint8) * 255 for b, i in enumerate(ids)])
     rgb = lambda m: m[..., None].expand(*m.shape, 3).contiguous()     # noqa: E731
     frames = torch.stack([rgb(masks[0] | masks[1]), rgb(masks[2])])
     _, ref = inputs.make_images(seed=4, batch=3)
-    infos = {i: {"diameter": d, "symmetries_discrete": [], "symmetries_continuous": []} for i, (_, d) in meshes.items()}
     return {"meshes": meshes, "ids": ids, "masks": masks, "frames": frames, "fi": torch.tensor([0, 0, 1]),
             "ref": ref.cuda(), "rel": synthetic_pose_batch(42, 3)[0].cuda(),
-            "tp": torch.from_numpy(icosphere_object_rotations(0)), "bank_ids": [91, 92, 93], "infos": infos,
-            "syms": {i: bop.symmetry_transformations(info) for i, info in infos.items()}}
+            "tp": torch.from_numpy(icosphere_object_rotations(0)), "bank_ids": [91, 92, 93]}
 
 
 @pytest.fixture(scope="module")
@@ -189,9 +168,7 @@ def tracked(gpu_model, frame_scene):
     """the model with the scene's objects, its bank and a refiner over the 42-pose grid"""
     from nope_b200.inplane_refine import InplaneRefiner
     fs = frame_scene
-    for i, (mesh, d) in fs["meshes"].items():
-        gpu_model.tless_cad[i] = mesh
-        gpu_model.bop_models[i] = {"diameter": d, "symmetries": fs["syms"][i], "info": fs["infos"][i]}
+    with_objects(gpu_model, fs["meshes"])
     bank = gpu_model.build_template_bank(fs["bank_ids"], fs["ref"], fs["rel"], fs["tp"])
     return gpu_model, bank, InplaneRefiner(fs["tp"], angles=A, steps=2)
 
@@ -252,20 +229,6 @@ def test_track_pose_frames_equals_the_chain(tracked, frame_scene, with_bank, ref
     assert set(out) == set(ref)
 
 
-def _syncs(fn):
-    """(result, the host synchronisations torch's sync debug mode reports during fn())"""
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as w:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            out = fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    torch.cuda.synchronize()
-    return out, sum("called a synchronizing CUDA operation" in str(x.message) for x in w)
-
-
 def test_synchronisations(tracked, frame_scene):
     """track_pose_frames synchronises as often as predict_pose_frames (with the bank and with references);
     PoseTracker.step with min_iou = 0 as often as track_pose_frames, and once more with the lost check"""
@@ -280,15 +243,15 @@ def test_synchronisations(tracked, frame_scene):
         search = lambda: model.predict_pose_frames(*args, k=K, refiner=refiner, frame_idx=fs["fi"], **src)  # noqa
         track = lambda: model.track_pose_frames(*args, prior, refiner, k=K, frame_idx=fs["fi"], **src)     # noqa
         search(), track()                                                                # warm-up
-        _, counts[f"search {name}"] = _syncs(search)
-        _, counts[f"track {name}"] = _syncs(track)
+        _, counts[f"search {name}"] = count_host_syncs(search)
+        _, counts[f"track {name}"] = count_host_syncs(track)
     tr0 = PoseTracker(model, bank, refiner, keep=KEEP, k=K, min_iou=0.0)
     tr1 = PoseTracker(model, bank, refiner, keep=KEEP, k=K, min_iou=1e-9)
     for tr in (tr0, tr1):
         tr.step(*args, [1, 2, 3], frame_idx=fs["fi"])
         tr.step(*args, [1, 2, 3], frame_idx=fs["fi"])                                    # warm-up of the tracked path
-    out0, counts["step min_iou=0"] = _syncs(lambda: tr0.step(*args, [1, 2, 3], frame_idx=fs["fi"]))
-    out1, counts["step min_iou>0"] = _syncs(lambda: tr1.step(*args, [1, 2, 3], frame_idx=fs["fi"]))
+    out0, counts["step min_iou=0"] = count_host_syncs(lambda: tr0.step(*args, [1, 2, 3], frame_idx=fs["fi"]))
+    out1, counts["step min_iou>0"] = count_host_syncs(lambda: tr1.step(*args, [1, 2, 3], frame_idx=fs["fi"]))
     print(f"syncs: {counts}")
     assert out0["tracked"].all() and out1["tracked"].all()
     assert counts["track bank"] == counts["search bank"]

@@ -10,50 +10,25 @@ import pytest
 import torch
 
 import translation_oracle as to
-from oracle import render_oracle as ro
+from _scenes import H, K4, W, inside, make_mesh, render, rot, tless_batch
+from _util import no_host_sync
 
 pytestmark = pytest.mark.gpu
 
-K4 = np.array([1075.65091572, 1073.90347929, 360.0, 270.0])    # Primesense, as tools/vsd_time.py
-H, W = 540, 720
-MESHES = {"box": lambda: ro.box(), "sphere": lambda: ro.sphere(40.0, 2), "soup": lambda: ro.soup(64, seed=1)}
-
-
-def _mesh(name):
-    from nope_b200.vsd import Mesh
-    v, f = MESHES[name]()
-    diameter = float(np.max(np.linalg.norm(v[:, None].astype(np.float64) - v[None], axis=2)))
-    return Mesh(v, f), diameter
-
-
-def _rot(rng):
-    return ro.look_pose(*rng.uniform(-math.pi, math.pi, 3))[:3, :3].astype(np.float64)
-
-
-def _render(mesh, R, t, K=K4):
-    from nope_b200.vsd import render_depth
-    return render_depth(mesh, torch.from_numpy(to.pose(R, t)), K, (H, W))[0]
-
-
-def _inside(mask):
-    n, _, r0, r1, c0, c1 = to.stats(mask)
-    return n > 0 and r0 > 0 and c0 > 0 and r1 < H - 1 and c1 < W - 1
-
-
-def _scene(mesh, seed, F, P, zlo=400.0, zhi=1200.0, inside=True):
+def _scene(mesh, seed, F, P, zlo=400.0, zhi=1200.0):
     """F frames: a true pose each (t at zlo ... zhi mm), its mask, and P rotation hypotheses (the first is the true
     one, the others random) -> (R_true [F, 3, 3], t_true [F, 3], masks uint8 [F, H, W] on the GPU, R [F, P, 3, 3])"""
     rng = np.random.default_rng(seed)
     Rt, tt, masks = [], [], []
     while len(Rt) < F:
-        R = _rot(rng)
+        R = rot(rng)
         z = rng.uniform(zlo, zhi)
         t = np.array([rng.uniform(-0.2, 0.2) * z, rng.uniform(-0.2, 0.2) * z, z])
-        m = _render(mesh, R, t) > 0
-        if inside and not _inside(m.cpu().numpy()):
+        m = render(mesh, R, t) > 0
+        if not inside(m):
             continue
         Rt.append(R), tt.append(t), masks.append(m.to(torch.uint8))
-    R = np.stack([np.stack([Rt[f]] + [_rot(rng) for _ in range(P - 1)]) for f in range(F)])
+    R = np.stack([np.stack([Rt[f]] + [rot(rng) for _ in range(P - 1)]) for f in range(F)])
     return np.stack(Rt), np.stack(tt), torch.stack(masks), R
 
 
@@ -64,7 +39,7 @@ def test_kernel_equals_oracle(name, P):
     """t and iou after 0 ... 6 updates equal the oracle's, which renders with render_depth at its own t; the kernel's
     silhouette counts equal render_depth's coverage at every step"""
     from nope_b200.translation import estimate_translation, initial_translation
-    mesh, diameter = _mesh(name)
+    mesh, diameter = make_mesh(name)
     F = 2
     _, _, masks, R = _scene(mesh, 11 + P, F, P)
     K = np.stack([K4 * [1, 1, 1, 1], K4 * [1.0, 1.001, 1.02, 0.98]])
@@ -79,7 +54,7 @@ def test_kernel_equals_oracle(name, P):
         for p in range(P):
             t = t0[f].cpu().numpy()
             for i in range(7):
-                d = _render(mesh, R[f, p], t, K[f]).cpu().numpy()
+                d = render(mesh, R[f, p], t, K[f]).cpu().numpy()
                 sil = to.stats(d > 0, mh[f])
                 assert tuple(got[i][2][f, p]) == sil, (f, p, i)
                 assert np.array_equal(got[i][0][f, p], t), (f, p, i, got[i][0][f, p], t)
@@ -92,7 +67,7 @@ def test_workspace_holds_the_final_render():
     from nope_b200 import _lib
     from nope_b200.translation import initial_translation
     from nope_b200.vsd import _stream
-    mesh, diameter = _mesh("sphere")
+    mesh, diameter = make_mesh("sphere")
     _, _, masks, R = _scene(mesh, 3, 2, 3)
     K = np.repeat(K4[None], 2, axis=0)
     t0 = initial_translation(masks, K, diameter)[:, None].expand(2, 3, 3).contiguous()
@@ -107,7 +82,7 @@ def test_workspace_holds_the_final_render():
     th = t.cpu().numpy()
     for f in range(2):
         for p in range(3):
-            assert torch.equal(depth[3 * f + p], _render(mesh, R[f, p], th[f, p]))
+            assert torch.equal(depth[3 * f + p], render(mesh, R[f, p], th[f, p]))
 
 
 # ------------------------------------------------------------------ accuracy with the true rotation
@@ -120,7 +95,7 @@ def test_accuracy_with_the_true_rotation(name, box_px, reproj_px):
     pixels under a sub-pixel move; it is held to its measured worst case (4.5 box pixels, 5.3 px; DESIGN.md
     section 18) with some room."""
     from nope_b200.translation import DEFAULT_ITERS, estimate_translation
-    mesh, diameter = _mesh(name)
+    mesh, diameter = make_mesh(name)
     R_true, t_true, masks, _ = _scene(mesh, 100, 32, 1)
     t, iou = estimate_translation(mesh, R_true, K4, masks, diameter=diameter)
     t, iou = t[:, 0].cpu().numpy(), iou[:, 0].cpu().numpy()
@@ -140,7 +115,7 @@ def test_accuracy_with_the_true_rotation(name, box_px, reproj_px):
 # ------------------------------------------------------------------ edge cases
 def test_empty_mask_and_a_start_off_screen():
     from nope_b200.translation import estimate_translation
-    mesh, diameter = _mesh("box")
+    mesh, diameter = make_mesh("box")
     _, t_true, masks, R = _scene(mesh, 7, 3, 2)
     masks[1] = 0
     t_init = np.repeat(t_true[:, None], 2, axis=1)
@@ -157,7 +132,7 @@ def test_empty_mask_and_a_start_off_screen():
 def test_batch_composition():
     """one frame alone equals the same frame inside a batch, and a hypothesis does not depend on its neighbours"""
     from nope_b200.translation import estimate_translation
-    mesh, diameter = _mesh("sphere")
+    mesh, diameter = make_mesh("sphere")
     _, _, masks, R = _scene(mesh, 21, 4, 5)
     K = np.stack([K4 * [1, 1, 1 + 0.01 * f, 1] for f in range(4)])
     t, iou = estimate_translation(mesh, R, K, masks, diameter=diameter, iters=4)
@@ -174,19 +149,15 @@ def test_batch_composition():
 
 def test_no_host_synchronisation():
     from nope_b200.translation import estimate_translation, initial_translation
-    mesh, diameter = _mesh("box")
+    mesh, diameter = make_mesh("box")
     _, t_true, masks, R = _scene(mesh, 9, 2, 3)
     Rd = torch.from_numpy(R).cuda()
     td = torch.from_numpy(t_true).cuda()
     K = np.repeat(K4[None], 2, axis=0)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         a = estimate_translation(mesh, Rd, K, masks, diameter=diameter)
         b = estimate_translation(mesh, Rd.float(), K, masks.bool(), t_init=td, iters=2)
         c = initial_translation(masks, K, diameter)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert torch.equal(a[0], estimate_translation(mesh, R, K, masks.cpu(), t_init=c.cpu())[0])
     assert b[0].shape == (2, 3, 3) and torch.isfinite(b[0]).all()
     with pytest.raises(ValueError):
@@ -200,42 +171,8 @@ def test_no_host_synchronisation():
 
 
 # ------------------------------------------------------------------ eval_bop with t_est
-def _tless_batch(tmp_path, B=3):
-    """as tests/test_bop_gpu._tless_batch, with no symmetries in models_info.json, plus each frame's mask (the box
-    rendered at the true pose)"""
-    import cv2
-    from nope_b200.poses import icosphere_object_rotations, synthetic_pose_batch
-    from oracle import inputs
-    v, f = ro.box(60.0, 40.0, 30.0)
-    ply = tmp_path / "models"
-    ply.mkdir()
-    with open(ply / "obj_000001.ply", "w") as fh:
-        fh.write(f"ply\nformat ascii 1.0\nelement vertex {len(v)}\nproperty float x\nproperty float y\n"
-                 f"property float z\nelement face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
-        fh.writelines(" ".join(repr(float(x)) for x in p) + "\n" for p in v)
-        fh.writelines("3 " + " ".join(str(int(i)) for i in q) + "\n" for q in f)
-    (ply / "models_info.json").write_text('{"1": {"diameter": %r}}' % float(np.linalg.norm([60.0, 40.0, 30.0])))
-    rel = synthetic_pose_batch(42, B)[0]
-    tp = torch.from_numpy(icosphere_object_rotations(0)).float()[None].expand(B, -1, -1, -1).contiguous()
-    q, r = inputs.make_images(seed=3, batch=B)
-    K = torch.tensor([[150.0, 0.0, 48.2], [0.0, 151.0, 35.9], [0.0, 0.0, 1.0]], dtype=torch.float64)
-    gtR, paths, masks = tp[torch.arange(B), torch.tensor([3, 17, 30])[:B]], [], []
-    trans = torch.tensor([[2.0, -3.0, 300.0], [-5.0, 1.0, 280.0], [0.0, 4.0, 320.0]])[:B, :, None]
-    for b in range(B):
-        T = np.eye(4)
-        T[:3, :3], T[:3, 3] = gtR[b].numpy(), trans[b, :, 0].numpy()
-        d = ro.render(v, f, T, K.numpy(), (72, 96))[0].numpy()
-        masks.append(d > 0)
-        raw = np.round(d * 10.0 + np.random.default_rng(b).normal(0, 5.0, d.shape) * (d > 0)).clip(0).astype(np.uint16)
-        paths.append(str(tmp_path / f"depth_{b}.png"))
-        assert cv2.imwrite(paths[-1], raw)
-    return {"query": q, "reference": r, "gt_relativeR": rel[:, 0], "all_relativeR": rel, "template_poses": tp,
-            "query_pose": gtR, "query_translation": trans, "intrinsic": K[None].expand(B, 3, 3).contiguous(),
-            "depth_path": paths, "obj_id": torch.ones(B, dtype=torch.int64)}, str(ply), torch.from_numpy(np.stack(masks))
-
-
 def test_eval_bop_with_estimated_translation(gpu_model, tmp_path):
-    batch, cad, masks = _tless_batch(tmp_path)
+    batch, cad, masks = tless_batch(tmp_path)
     model = gpu_model
     model.load_mesh(cad, obj_ids=[1])
     model.load_models_info(os.path.join(cad, "models_info.json"))

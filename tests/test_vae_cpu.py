@@ -10,17 +10,9 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from _util import SD15_CONFIG
 from nope_b200 import vae as V
 
-# diffusers' AutoencoderKL config.json of Stable Diffusion v1.5's VAE
-SD15_CONFIG = {
-    "_class_name": "AutoencoderKL", "_diffusers_version": "0.6.0", "act_fn": "silu",
-    "block_out_channels": [128, 256, 512, 512],
-    "down_block_types": ["DownEncoderBlock2D", "DownEncoderBlock2D", "DownEncoderBlock2D", "DownEncoderBlock2D"],
-    "in_channels": 3, "latent_channels": 4, "layers_per_block": 2, "norm_num_groups": 32, "out_channels": 3,
-    "sample_size": 512,
-    "up_block_types": ["UpDecoderBlock2D", "UpDecoderBlock2D", "UpDecoderBlock2D", "UpDecoderBlock2D"],
-}
 OTHER_VALUES = {
     "in_channels": [1, 4], "latent_channels": [8, 16], "block_out_channels": [[128, 256, 512], [64, 128, 256, 256]],
     "down_block_types": [["DownEncoderBlock2D"] * 3, ["AttnDownEncoderBlock2D"] * 4], "layers_per_block": [1, 3],

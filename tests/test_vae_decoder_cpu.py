@@ -11,7 +11,7 @@ import torch
 from nope_b200 import vae as V
 
 import vae_decoder_oracle as D
-from test_vae_cpu import SD15_CONFIG
+from _util import SD15_CONFIG
 
 
 @pytest.fixture(scope="module")

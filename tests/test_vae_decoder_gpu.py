@@ -7,8 +7,7 @@ import ctypes as C
 import pytest
 import torch
 
-from _util import log, rel_l2
-from test_vae_gpu import _crop_like, _uniform
+from _util import crop_like_images, log, no_host_sync, rel_l2, uniform_images
 
 import vae_decoder_oracle as D
 
@@ -56,12 +55,12 @@ def base_model(full_sd):
 
 def _latents(kind, B, vae, ldm_model):
     if kind == "uniform":
-        return vae.encode_image(_uniform(40 + B, B).cuda())
+        return vae.encode_image(uniform_images(40 + B, B).cuda())
     if kind == "crop":
-        return vae.encode_image(_crop_like(50 + B, B).cuda())
+        return vae.encode_image(crop_like_images(50 + B, B).cuda())
     from nope_b200.poses import synthetic_pose_batch
     rel = synthetic_pose_batch(42, B)[0][:, 7].cuda()
-    pred, _ = ldm_model.sample(_crop_like(60 + B, B).cuda(), rel)
+    pred, _ = ldm_model.sample(crop_like_images(60 + B, B).cuda(), rel)
     return pred
 
 
@@ -80,7 +79,7 @@ def test_images_match_the_float64_oracle(vae, full_sd, ldm_model, kind, B):
 
 
 def test_batch_invariance_across_chunks(vae):
-    z = torch.cat([vae.encode_image(_uniform(70, 9).cuda()), vae.encode_image(_crop_like(71, 8).cuda())])
+    z = torch.cat([vae.encode_image(uniform_images(70, 9).cuda()), vae.encode_image(crop_like_images(71, 8).cuda())])
     x = vae.decode_latent(z)                     # 17 latents: two full chunks and one
     for b in range(17):
         assert torch.equal(vae.decode_latent(z[b:b + 1])[0], x[b]), b
@@ -88,21 +87,17 @@ def test_batch_invariance_across_chunks(vae):
 
 def test_no_host_sync(vae, ldm_model):
     from nope_b200.poses import synthetic_pose_batch
-    z = vae.encode_image(_crop_like(80, 2).cuda())
-    r = _crop_like(81, 1).cuda()
+    z = vae.encode_image(crop_like_images(80, 2).cuda())
+    r = crop_like_images(81, 1).cuda()
     rel = synthetic_pose_batch(42, 1)[0].cuda()
     enc = ldm_model.u_net.encoder
     vae.decode_latent(z)                         # engines built outside the checked region
     ldm_model.sample(r, rel[:, 0])
     ldm_model.generate_templates(r, rel[:, :20])
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         vae.decode_latent(z)
         ldm_model.sample(r, rel[:, 0])
         ldm_model.generate_templates(r, rel[:, :20])
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     torch.cuda.synchronize()
     assert enc.has_decoder
 
@@ -113,7 +108,7 @@ def test_sample_and_generate_templates_decode(which, ldm_model, base_model):
     model = ldm_model if which == "ldm" else base_model
     enc = model.u_net.encoder
     assert enc.has_decoder
-    r = _crop_like(90, 2).cuda()
+    r = crop_like_images(90, 2).cuda()
     rel = synthetic_pose_batch(42, 2)[0].cuda()
     feat, rgb = model.sample(r, rel[:, 3])
     assert feat.shape == (2, 4, 32, 32) and rgb.shape == (2, 3, 256, 256)
@@ -134,7 +129,7 @@ def test_encoder_only_weights_return_none(which, full_sd):
     enc_only = {k: v for k, v in full_sd.items() if not (k.startswith("decoder.") or k.startswith("post_quant"))}
     model = _model(which, enc_only)
     assert not model.u_net.encoder.has_decoder
-    r = _crop_like(91, 1).cuda()
+    r = crop_like_images(91, 1).cuda()
     rel = synthetic_pose_batch(42, 1)[0].cuda()
     feat, rgb = model.sample(r, rel[:, 0])
     assert feat.shape == (1, 4, 32, 32) and rgb is None

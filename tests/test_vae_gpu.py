@@ -6,7 +6,8 @@ import math
 import pytest
 import torch
 
-from _util import log, rel_l2
+from _scenes import FLIPS, tless_batch
+from _util import crop_like_images, log, no_host_sync, rel_l2, uniform_images
 
 pytestmark = pytest.mark.gpu
 
@@ -25,27 +26,10 @@ def vae(vae_sd):
     return VAE_StableDiffusion(device="cuda:0", name="VAE").load_state_dict(vae_sd)
 
 
-def _uniform(seed, B):
-    g = torch.Generator().manual_seed(7000 + seed)
-    return torch.rand((B, 3, 256, 256), generator=g) * 2 - 1
-
-
-def _crop_like(seed, B):
-    """mostly -1 background with a textured object in the middle, as the model's crops are"""
-    g = torch.Generator().manual_seed(8000 + seed)
-    x = torch.full((B, 3, 256, 256), -1.0)
-    yy, xx = torch.meshgrid(torch.arange(256.0), torch.arange(256.0), indexing="ij")
-    for b in range(B):
-        cy, cx, r = (torch.rand(3, generator=g) * torch.tensor([60.0, 60.0, 40.0]) + torch.tensor([98.0, 98.0, 50.0]))
-        m = ((yy - cy) ** 2 + (xx - cx) ** 2) < r * r
-        x[b][:, m] = torch.rand((3, int(m.sum())), generator=g) * 1.6 - 0.8
-    return x
-
-
 @pytest.mark.parametrize("kind,B", [("uniform", 1), ("uniform", 3), ("crop", 1), ("crop", 3)])
 def test_latents_match_the_float64_oracle(vae, vae_sd, kind, B):
     from oracle import vae_oracle
-    x = (_uniform if kind == "uniform" else _crop_like)(B, B).cuda()
+    x = (uniform_images if kind == "uniform" else crop_like_images)(B, B).cuda()
     z = vae.encode_image(x)
     ref = vae_oracle.encode(vae_sd, x.double())
     e = rel_l2(z, ref)
@@ -55,7 +39,7 @@ def test_latents_match_the_float64_oracle(vae, vae_sd, kind, B):
 
 
 def test_batch_invariance_across_chunks(vae):
-    x = torch.cat([_uniform(5, 20), _crop_like(6, 13)]).cuda()       # 33 images: two full chunks and one
+    x = torch.cat([uniform_images(5, 20), crop_like_images(6, 13)]).cuda()       # 33 images: two full chunks and one
     z = vae.encode_image(x)
     for b in range(33):
         assert torch.equal(vae.encode_image(x[b:b + 1])[0], z[b]), b
@@ -63,7 +47,7 @@ def test_batch_invariance_across_chunks(vae):
 
 def test_encode_inplane_equals_materialised_rotations(vae):
     from nope_b200 import inplane
-    x = torch.cat([_crop_like(9, 2), _uniform(9, 1)]).cuda()
+    x = torch.cat([crop_like_images(9, 2), uniform_images(9, 1)]).cuda()
     A = 12                                                           # 36 pairs: crosses two chunk boundaries
     z = vae.encode_image_inplane(x, A)
     rot = inplane.rotate_images(x, A).reshape(3 * A, 3, 256, 256)
@@ -73,7 +57,7 @@ def test_encode_inplane_equals_materialised_rotations(vae):
 
 def test_encode_rotated_equals_materialised_rotations(vae):
     from nope_b200.inplane_refine import rotate_pairs
-    x = _crop_like(10, 3).cuda()
+    x = crop_like_images(10, 3).cuda()
     P = 19
     g = torch.Generator().manual_seed(11)
     idx = torch.randint(-1, 4, (P,), generator=g)                     # -1 and 3: out of range, all -1 crops
@@ -85,18 +69,14 @@ def test_encode_rotated_equals_materialised_rotations(vae):
 
 
 def test_no_host_sync(vae):
-    x = _crop_like(12, 2).cuda()
+    x = crop_like_images(12, 2).cuda()
     idx = torch.tensor([0, 1, 1], device="cuda")
     cs = torch.tensor([[1.0, 0.0], [0.0, 1.0], [0.6, 0.8]], device="cuda")
     vae.encode_image_inplane(x, 4)          # engine and the angle table's device copy made outside the checked region
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
+    with no_host_sync():
         vae.encode_image(x)
         vae.encode_image_inplane(x, 4)
         vae.encode_image_rotated(x, idx, cs)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     torch.cuda.synchronize()
 
 
@@ -104,7 +84,7 @@ def test_argument_checks(vae, vae_sd):
     import ctypes as C
     from nope_b200 import _lib
     from nope_b200.vae import VAE_StableDiffusion
-    x = _uniform(0, 1).cuda()
+    x = uniform_images(0, 1).cuda()
     with pytest.raises(_lib.NopeError):
         vae.encode_image(x.cpu())                                    # no CPU path
     with pytest.raises(_lib.NopeError):
@@ -173,7 +153,7 @@ def _poses(B, N=42):
 def test_ldm_predict_pose_from_images(ldm_model, vae_sd):
     from oracle import vae_oracle
     u = ldm_model.u_net
-    q, r = _crop_like(20, 2).cuda(), _crop_like(21, 2).cuda()
+    q, r = crop_like_images(20, 2).cuda(), crop_like_images(21, 2).cuda()
     rel, R = _poses(2)
     rel = rel.cuda()
     # one query per reference
@@ -203,7 +183,7 @@ def test_ldm_searches(ldm_model):
     from nope_b200.inplane_refine import InplaneRefiner
     from nope_b200.poses import icosphere_object_rotations, synthetic_pose_batch
     from nope_b200.refine import PoseRefiner
-    q, r = _crop_like(30, 1).cuda(), _crop_like(31, 1).cuda()
+    q, r = crop_like_images(30, 1).cuda(), crop_like_images(31, 1).cuda()
     R0, R1 = icosphere_object_rotations(0), icosphere_object_rotations(1)
     rel0, rel1 = synthetic_pose_batch(42, 1)[0].cuda(), synthetic_pose_batch(162, 1)[0].cuda()
     _, idx, sim = ldm_model.predict_pose(q, r, rel0, k=3)
@@ -222,7 +202,7 @@ def test_ldm_searches(ldm_model):
 
 def test_base_predict_pose_from_images(base_model):
     u = base_model.u_net
-    q, r = _crop_like(40, 2).cuda(), _crop_like(41, 2).cuda()
+    q, r = crop_like_images(40, 2).cuda(), crop_like_images(41, 2).cuda()
     rel, R = _poses(2)
     rel = rel.cuda()
     _, idx, sim = base_model.predict_pose(q, r, rel, R, k=5)
@@ -244,8 +224,7 @@ def test_test_step_on_a_synthetic_shapenet_batch(which, ldm_model, base_model):
 
 
 def test_eval_bop_with_the_ldm_model(ldm_model, tmp_path):
-    from test_bop_gpu import _tless_batch
-    batch, cad = _tless_batch(tmp_path)
+    batch, cad, _ = tless_batch(tmp_path, symmetries=FLIPS)
     ldm_model.load_mesh(cad, obj_ids=[1])
     ldm_model.load_models_info(cad + "/models_info.json")
     out = ldm_model.eval_bop(batch, "obj01")

@@ -9,20 +9,15 @@ import numpy as np
 import pytest
 import torch
 
+from _scenes import K3, tless_batch
+from _util import no_host_sync, same_bits
 from oracle import render_oracle as ro
 
 pytestmark = pytest.mark.gpu
 
-TLESS_K = np.array([[1075.65091572, 0.0, 360.0], [0.0, 1073.90347929, 270.0], [0.0, 0.0, 1.0]])   # Primesense, 720x540
-
-
 def _render(v, f, poses, K, size, znear=0.05):
     from nope_b200.vsd import Mesh, render_depth
     return render_depth(Mesh(v, f), torch.as_tensor(np.asarray(poses)), K, size, znear=znear).cpu()
-
-
-def _same_bits(a, b):
-    return torch.equal(a.view(torch.int32), torch.as_tensor(b).view(torch.int32))
 
 
 # ------------------------------------------------------------------ kernel vs oracle
@@ -42,7 +37,7 @@ def test_render_matches_oracle(mesh):
     out = _render(v, f, _POSES, _K_SMALL, (60, 80))
     ref = ro.render(v, f, _POSES, _K_SMALL, (60, 80))
     assert out.shape == (len(_POSES), 60, 80)
-    assert _same_bits(out, ref)
+    assert same_bits(out, ref)
     assert (out[0] > 0).any() and (out[2] == 0).all()
 
 
@@ -58,15 +53,15 @@ def test_render_full_cover_edges_through_samples_and_ties():
     pose = np.eye(4, dtype=np.float32)
     for faces in (f[:2], f[2:4], f[4:], f):
         out = _render(v, faces, pose[None], K, (12, 16))
-        assert _same_bits(out, ro.render(v, faces, pose, K, (12, 16)))
+        assert same_bits(out, ro.render(v, faces, pose, K, (12, 16)))
     assert (_render(v, f[:2], pose[None], K, (12, 16)) == 100.0).all()
 
 
 def test_render_tless_size_matches_oracle():
     v, f = ro.sphere(45.0, 2)
     poses = np.stack([ro.look_pose(0.3, 0.2, 0.1, t=(10, -15, 600)), ro.look_pose(-0.5, 0.9, 0.0, t=(-250, 120, 500))])
-    out = _render(v, f, poses, TLESS_K, (540, 720))
-    assert _same_bits(out, ro.render(v, f, poses, TLESS_K, (540, 720)))
+    out = _render(v, f, poses, K3, (540, 720))
+    assert same_bits(out, ro.render(v, f, poses, K3, (540, 720)))
     assert (out > 0).sum() > 1000
 
 
@@ -131,10 +126,10 @@ def test_winding_order_and_batch_independence():
     base = _render(v, f, poses, K, (72, 96))
     perm = np.random.default_rng(0).permutation(len(f))
     rolled = np.roll(f[perm], 1, axis=1)
-    assert _same_bits(_render(v, f[:, [0, 2, 1]], poses, K, (72, 96)), base)
-    assert _same_bits(_render(v, rolled, poses, K, (72, 96)), base)
+    assert same_bits(_render(v, f[:, [0, 2, 1]], poses, K, (72, 96)), base)
+    assert same_bits(_render(v, rolled, poses, K, (72, 96)), base)
     for p in (0, 3, 5):
-        assert _same_bits(_render(v, f, poses[p:p + 1], K, (72, 96)), base[p:p + 1])
+        assert same_bits(_render(v, f, poses[p:p + 1], K, (72, 96)), base[p:p + 1])
 
 
 def test_faces_out_of_range_are_skipped_by_the_kernel():
@@ -145,7 +140,7 @@ def test_faces_out_of_range_are_skipped_by_the_kernel():
     m.faces = torch.cat([m.faces, torch.tensor([[0, 1, 99], [-5, 1, 2]], dtype=torch.int32, device="cuda")])
     out = render_depth(m, ro.look_pose(0.3, 0.2, 0.0, t=(0, 0, 300)), _K_SMALL, (60, 80)).cpu()
     ref = ro.render(v, f, ro.look_pose(0.3, 0.2, 0.0, t=(0, 0, 300)), _K_SMALL, (60, 80))
-    assert _same_bits(out, ref)
+    assert same_bits(out, ref)
     assert (out > 0).any()
     m.faces = torch.tensor([[0, 1, 99], [-5, 1, 2], [2, 3, 8]], dtype=torch.int32, device="cuda")
     assert (render_depth(m, ro.look_pose(0.3, 0.2, 0.0, t=(0, 0, 300)), _K_SMALL, (60, 80)) == 0).all()
@@ -161,12 +156,12 @@ def _guard_case(v, f, drop, K, size, znear):
     f = np.asarray(f, dtype=np.int32)
     keep = [i for i in range(len(f)) if i not in drop]
     every = _render(v, f, pose, K, size, znear)[0]
-    assert _same_bits(every, ro.render(v, f, pose, K, size, znear)[0])
+    assert same_bits(every, ro.render(v, f, pose, K, size, znear)[0])
     kept = _render(v, f[keep], pose, K, size, znear)[0]
-    assert _same_bits(every, kept)
+    assert same_bits(every, kept)
     for i in range(len(f)):
         alone = _render(v, f[i:i + 1], pose, K, size, znear)[0]
-        assert _same_bits(alone, ro.render(v, f[i:i + 1], pose, K, size, znear)[0])
+        assert same_bits(alone, ro.render(v, f[i:i + 1], pose, K, size, znear)[0])
         assert ((alone > 0).sum() == 0) == (i in drop), i
     return every
 
@@ -260,16 +255,16 @@ def test_vsd_on_gpu_renders_matches_oracle():
     v, f = ro.sphere(45.0, 2)
     gt = ro.look_pose(0.3, 0.2, 0.1, t=(10, -15, 600))
     preds = np.stack([ro.look_pose(0.3 + d, 0.2 - d, 0.1, t=(10, -15, 600)) for d in (0.0, 0.05, 0.2, 0.6, 1.5)])
-    dg = _render(v, f, gt[None], TLESS_K, (540, 720))[0]
-    de = _render(v, f, preds, TLESS_K, (540, 720))
+    dg = _render(v, f, gt[None], K3, (540, 720))[0]
+    de = _render(v, f, preds, K3, (540, 720))
     rng = np.random.default_rng(1)
     dt = dg.double().numpy() + rng.normal(0, 2.0, dg.shape) * (dg.numpy() > 0)
     dt[rng.random(dt.shape) < 0.05] = 0
     dt = np.round(dt * 10) / 10.0
     for cost in ("step", "tlinear"):
-        out = vsd_errors(torch.from_numpy(dt)[None].cuda(), dg[None].cuda(), de[None].cuda(), TLESS_K[None],
+        out = vsd_errors(torch.from_numpy(dt)[None].cuda(), dg[None].cuda(), de[None].cuda(), K3[None],
                          cost_type=cost).cpu().numpy()[0]
-        ref = ro.vsd(dt, dg.numpy(), de.numpy(), TLESS_K, cost_type=cost)
+        ref = ro.vsd(dt, dg.numpy(), de.numpy(), K3, cost_type=cost)
         if cost == "step":
             assert np.array_equal(out, ref), (out, ref)
         else:
@@ -292,42 +287,10 @@ def test_vsd_empty_union_and_perfect_pose():
 
 
 # ------------------------------------------------------------------ eval_vsd / test_step end to end
-def _tless_batch(tmp_path, gpu_model, B=3):
-    import cv2
-    from nope_b200.poses import icosphere_object_rotations, synthetic_pose_batch
-    from oracle import inputs
-    v, f = ro.box(60.0, 40.0, 30.0)
-    ply = tmp_path / "models"
-    ply.mkdir()
-    with open(ply / "obj_000001.ply", "w") as fh:
-        fh.write(f"ply\nformat ascii 1.0\nelement vertex {len(v)}\nproperty float x\nproperty float y\n"
-                 f"property float z\nelement face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
-        fh.writelines(" ".join(repr(float(x)) for x in p) + "\n" for p in v)
-        fh.writelines("3 " + " ".join(str(int(i)) for i in q) + "\n" for q in f)
-    rel = synthetic_pose_batch(42, B)[0]
-    tp = torch.from_numpy(icosphere_object_rotations(0)).float()[None].expand(B, -1, -1, -1).contiguous()
-    N = tp.shape[1]
-    assert rel.shape[1] == N
-    q, r = inputs.make_images(seed=3, batch=B)
-    K = torch.tensor([[150.0, 0.0, 48.2], [0.0, 151.0, 35.9], [0.0, 0.0, 1.0]], dtype=torch.float64)
-    gtR, paths = tp[torch.arange(B), torch.tensor([3, 17, 30])[:B]], []
-    trans = torch.tensor([[2.0, -3.0, 300.0], [-5.0, 1.0, 280.0], [0.0, 4.0, 320.0]])[:B, :, None]
-    for b in range(B):
-        T = np.eye(4)
-        T[:3, :3], T[:3, 3] = gtR[b].numpy(), trans[b, :, 0].numpy()
-        d = ro.render(v, f, T, K.numpy(), (72, 96))[0].numpy()
-        raw = np.round(d * 10.0 + np.random.default_rng(b).normal(0, 5.0, d.shape) * (d > 0)).clip(0).astype(np.uint16)
-        paths.append(str(tmp_path / f"depth_{b}.png"))
-        assert cv2.imwrite(paths[-1], raw)
-    return {"query": q, "reference": r, "gt_relativeR": rel[:, 0], "all_relativeR": rel, "template_poses": tp,
-            "query_pose": gtR, "query_translation": trans, "intrinsic": K[None].expand(B, 3, 3).contiguous(),
-            "depth_path": paths, "obj_id": torch.ones(B, dtype=torch.int64)}, str(ply)
-
-
 def test_eval_vsd_end_to_end(gpu_model, tmp_path, monkeypatch):
     import cv2
     from nope_b200 import vsd as V
-    batch, cad = _tless_batch(tmp_path, gpu_model)
+    batch, cad, _ = tless_batch(tmp_path, models_info=False)
     B = batch["query"].shape[0]
     model = gpu_model
     model.load_mesh(cad, obj_ids=[1])
@@ -340,11 +303,8 @@ def test_eval_vsd_end_to_end(gpu_model, tmp_path, monkeypatch):
     def strict(fn, name):
         def inner(*a, **kw):
             calls[name] += 1
-            torch.cuda.set_sync_debug_mode("error")
-            try:
+            with no_host_sync():
                 return fn(*a, **kw)
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
         return inner
     monkeypatch.setattr(V, "render_depth", strict(render, "render"))
     monkeypatch.setattr(V, "vsd_errors", strict(vsd, "vsd"))

@@ -28,12 +28,12 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
+from _scenes import K4, angle, scene                                           # noqa: E402
 from nope_b200 import contour_refine                                           # noqa: E402
 from nope_b200.contour_refine import refine_pose_contour                       # noqa: E402
 from nope_b200.translation import estimate_translation                         # noqa: E402
 from nope_b200.vsd import Mesh                                                 # noqa: E402
 from oracle import render_oracle as ro                                         # noqa: E402
-from test_depth_refine_gpu import K4, _angle, _scene                           # noqa: E402
 from translation_time import card, timed, uv_sphere                            # noqa: E402
 
 SCHEDULES = [(0.15, 0.02), (0.3, 0.02), (0.15, 0.05), (0.08, 0.02)]
@@ -82,7 +82,7 @@ def accuracy_table():
     rows = []
     for name, (v, f) in meshes.items():
         mesh = Mesh(v, f)
-        R_true, t_true, _, M, R0, t0 = _scene(mesh, 100, 16, 1, sensor=False, background=False)
+        R_true, t_true, _, M, R0, t0 = scene(mesh, 100, 16, 1, sensor=False, background=False)
         tb, _ = estimate_translation(mesh, R0, K4, M, diameter=_diameter(v))
         for start, ts in (("offset", t0), ("box fit", tb.cpu().numpy())):
             for mname, masks in (("exact", M), ("+-1 px", _detector_masks(M))):
@@ -91,7 +91,7 @@ def accuracy_table():
                         R, t, fit = refine_pose_contour(mesh, R0, ts, K4, masks, iters=it,
                                                     tau=contour_refine.default_tau(it, a, b))
                         R, t = R[:, 0].cpu().numpy(), t[:, 0].cpu().numpy()
-                        er = np.array([_angle(R[i], R_true[i]) for i in range(16)])
+                        er = np.array([angle(R[i], R_true[i]) for i in range(16)])
                         et = np.linalg.norm(t - t_true, axis=1)
                         iou = fit["iou"][:, 0].cpu().numpy()
                         rows.append({"mesh": name, "start": start, "mask": mname, "tau": [a, b], "iters": it,
@@ -124,7 +124,7 @@ def main():
     for mname, (v, f) in meshes.items():
         mesh = Mesh(v, f)
         for F in (1, 16):
-            _, _, _, M, R0, t0 = _scene(mesh, 1, F, P, sensor=False, background=False)
+            _, _, _, M, R0, t0 = scene(mesh, 1, F, P, sensor=False, background=False)
             Rd, td = torch.from_numpy(R0).cuda(), torch.from_numpy(t0).cuda()
             call = lambda: refine_pose_contour(mesh, Rd, td, K4, M, iters=iters)   # noqa: E731
             ms = timed(call, a.reps)

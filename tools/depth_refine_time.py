@@ -28,11 +28,11 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
+from _scenes import K4, angle, scene                                           # noqa: E402
 from nope_b200 import depth_refine                                             # noqa: E402
 from nope_b200.depth_refine import refine_pose_depth                           # noqa: E402
 from nope_b200.vsd import Mesh                                                 # noqa: E402
 from oracle import render_oracle as ro                                         # noqa: E402
-from test_depth_refine_gpu import K4, _angle, _scene                           # noqa: E402
 from translation_time import card, timed, uv_sphere                            # noqa: E402
 
 SCHEDULES = [(0.25, 0.02), (0.5, 0.02), (0.5, 0.05), (1.0, 0.02)]
@@ -68,13 +68,13 @@ def accuracy_table():
         for name, (v, f) in meshes.items():
             mesh = Mesh(v, f)
             for noisy in (False, True):
-                R_true, t_true, S, M, R0, t0 = _scene(mesh, 100, 16, 1, sensor=noisy)
+                R_true, t_true, S, M, R0, t0 = scene(mesh, 100, 16, 1, sensor=noisy)
                 for a, b in SCHEDULES:
                     depth_refine.TAU_START, depth_refine.TAU_END = a, b
                     for it in ITERS:
                         R, t, fit = refine_pose_depth(mesh, R0, t0, K4, S, masks=M, iters=it)
                         R, t = R[:, 0].cpu().numpy(), t[:, 0].cpu().numpy()
-                        er = np.array([_angle(R[i], R_true[i]) for i in range(16)])
+                        er = np.array([angle(R[i], R_true[i]) for i in range(16)])
                         et = np.linalg.norm(t - t_true, axis=1)
                         sc = fit["score"][:, 0].cpu().numpy()
                         rows.append({"mesh": name, "noise": noisy, "tau": [a, b], "iters": it,
@@ -109,7 +109,7 @@ def main():
     for mname, (v, f) in meshes.items():
         mesh = Mesh(v, f)
         for F in (1, 16):
-            _, _, S, M, R0, t0 = _scene(mesh, 1, F, P)
+            _, _, S, M, R0, t0 = scene(mesh, 1, F, P)
             Rd, td = torch.from_numpy(R0).cuda(), torch.from_numpy(t0).cuda()
             call = lambda: refine_pose_depth(mesh, Rd, td, K4, S, masks=M, iters=iters)   # noqa: E731
             ms = timed(call, a.reps)

@@ -1,7 +1,7 @@
 """Measure the pose fits under occlusion (DESIGN.md section 24) at 720x540 with the Primesense intrinsics.
 
 --accuracy: 32 seeded scenes per mesh (box, icosphere) and occlusion level (a nearer sphere hiding 20, 40 or 60 % of
-the target's silhouette; tests/test_occlusion_fit_gpu.occluded_scene), with the visible mask M and the occluders O.
+the target's silhouette; tests/_scenes.occluded_scene), with the visible mask M and the occluders O.
 For the translation fit from initial_translation(M) at the true rotation: median / max |dz| in box pixels
 (|dz| sqrt(w h) / z, with the box of the whole silhouette) and the origin's reprojection error in px after 0 ... 6
 updates, with and without O.  For the contour refinement from starts 2.5 - 5 deg and 5 - 10 mm off: median / max
@@ -26,12 +26,11 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
+from _scenes import K4, accuracy, occluded_scene, perturb                      # noqa: E402
 from nope_b200.contour_refine import refine_pose_contour                       # noqa: E402
 from nope_b200.translation import DEFAULT_ITERS, estimate_translation          # noqa: E402
 from nope_b200.vsd import Mesh                                                 # noqa: E402
 from oracle import render_oracle as ro                                         # noqa: E402
-from test_depth_refine_gpu import _perturb                                     # noqa: E402
-from test_occlusion_fit_gpu import K4, accuracy, occluded_scene                # noqa: E402
 from translation_time import card, timed                                       # noqa: E402
 
 LEVELS = (0.2, 0.4, 0.6)
@@ -78,7 +77,7 @@ def main():
         for F in (1, 16):
             R_true, t_true, M, O, *_ = occluded_scene(mesh, 1, F, 0.4)
             rng = np.random.default_rng(2)
-            st = [[_perturb(rng, R_true[i], t_true[i]) for _ in range(P)] for i in range(F)]
+            st = [[perturb(rng, R_true[i], t_true[i]) for _ in range(P)] for i in range(F)]
             Rd = torch.from_numpy(np.array([[s[0] for s in r] for r in st])).cuda()
             td = torch.from_numpy(np.array([[s[1] for s in r] for r in st])).cuda()
             for occ_name, occ in (("no O", None), ("O", O)):
