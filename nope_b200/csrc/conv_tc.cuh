@@ -26,6 +26,7 @@
 #include <cstring>
 #include <map>
 #include <tuple>
+#include <vector>
 
 namespace nope {
 
@@ -589,15 +590,6 @@ class TmapCache {
   std::map<std::tuple<const void*, int, int, int>, CUtensorMap> maps3_;
 };
 
-// What a convolution layer of every engine holds.  K is the engine's GEMM depth (its weight layout decides whether
-// the W_lo columns are counted); each engine's layer adds its own extras.
-struct ConvLayerBase {
-  int cin = 0, cout = 0, K = 0, bn = 0;
-  __half* w = nullptr;     // packed fp16 weights, K-major
-  float* bias = nullptr;   // [cout] or nullptr
-  CUtensorMap wmap;        // weight box of bn rows
-};
-
 // One filter tap: activation lattice (0 for a plain map) and pixel offset.
 struct ConvTap {
   int lat, dy, dx;
@@ -609,6 +601,66 @@ inline ConvTap stride2_tap(int oy, int ox) {
   const int p1 = oy & 1, p2 = ox & 1;
   return ConvTap{p1 * 2 + p2, (oy - p1) / 2, (ox - p2) / 2};
 }
+// The k x k taps, row-major, of a convolution whose first tap reads input pixel (y + oy0, x + ox0) at stride 1 or
+// (2y + oy0, 2x + ox0) at stride 2.
+inline std::vector<ConvTap> conv_taps(int k, int stride, int oy0, int ox0) {
+  std::vector<ConvTap> taps;
+  for (int ky = 0; ky < k; ++ky)
+    for (int kx = 0; kx < k; ++kx)
+      taps.push_back(stride == 1 ? ConvTap{0, oy0 + ky, ox0 + kx} : stride2_tap(oy0 + ky, ox0 + kx));
+  return taps;
+}
+
+// A convolution layer of any engine.  Its weights are K-major fp16 rows, one per output channel (cout is padded to a
+// multiple of 64 with zero rows; the folded upsample has 4 cout rows, parity * cout + o): [W_hi (K) | W_lo (K)] when
+// the layer has a W_lo plane (the fp16 remainders W - fp16(W)), W_hi alone otherwise (bf16 in the UNet's bf16 mode).
+// The K columns of a plane are (tap, input channel) over the layer's taps, then any extra columns: a 1x1 shortcut or
+// skip, an identity residual.
+struct ConvLayer {
+  int cin = 0, cout = 0, K = 0, bn = 0;
+  bool wlo = false;                          // a W_lo plane follows at column K
+  int k = 1, stride = 1, oy0 = 0, ox0 = 0;   // the taps: conv_taps(k, stride, oy0, ox0)
+  bool up = false;                           // nearest-x2 upsample + 3x3 folded into four 2x2 parity kernels (n_par 4)
+  __half* w = nullptr;
+  float* bias = nullptr;                     // [cout] or nullptr
+  CUtensorMap wmap;                          // weight box of bn rows
+  // UNet: pre-norm folded into this (bias-free 1x1) layer: weights hold W diag(gamma); see GnFuse::pre_*
+  float* pre_w1 = nullptr;
+  float* pre_wb = nullptr;
+  // LDM
+  int skip_c = 0;        // channels of a folded 1x1 skip_connection / identity residual (extra K columns)
+  int k_alg = 0;         // K without identity-residual columns (algorithmic FLOP count)
+  bool geglu = false;    // rows permuted to (64 x | 64 gate) tiles; the epilogue emits x * gelu(gate)
+
+  int rows() const { return up ? 4 * cout : cout; }
+  int row_len() const { return wlo ? 2 * K : K; }
+  std::vector<ConvTap> taps() const { return conv_taps(k, stride, oy0, ox0); }
+};
+// A layer of the given taps (conv_taps) and upsample fold, its other fields unset.
+inline ConvLayer conv_shape(int k, int stride, int oy0, int ox0, bool up = false) {
+  ConvLayer L;
+  L.k = k;
+  L.stride = stride;
+  L.oy0 = oy0;
+  L.ox0 = ox0;
+  L.up = up;
+  return L;
+}
+// The shapes the UNet and LDM engines share: 3x3 pad 1, 1x1, pixel-unshuffle + 1x1 (HardDownsample: a 2x2 stride-2
+// convolution), nearest-x2 upsample + 3x3 folded into 2x2 kernels over the source, 3x3 stride 2 pad 1.
+inline ConvLayer conv3x3() { return conv_shape(3, 1, -1, -1); }
+inline ConvLayer conv1x1() { return conv_shape(1, 1, 0, 0); }
+inline ConvLayer conv_unshuffle() { return conv_shape(2, 2, 0, 0); }
+inline ConvLayer conv_upsample3x3() { return conv_shape(2, 1, -1, -1, true); }
+inline ConvLayer conv3x3_s2() { return conv_shape(3, 2, -1, -1); }
+
+// One input of a convolution as its K segments read it: its channels and the maps of its hi and lo halves for each
+// lattice a tap names (lo[0] < 0: the input carries no lo).
+struct ConvSrc {
+  int C = 0;
+  int hi[4] = {0, 0, 0, 0};
+  int lo[4] = {-1, -1, -1, -1};
+};
 
 // Builds the ConvParams of one launch.  The engine adds its activation maps and, in its accumulation order, the
 // K segments, then sets its epilogue fields around finish(), which fills everything that follows from the geometry,
@@ -633,6 +685,16 @@ struct ConvBuilder {
     p.amap[p.n_amaps] = *m;
     return p.n_amaps++;
   }
+  // the input (hi, lo) of C channels (lo == nullptr: none): its plain map, or with lattices == 4 its four stride-2
+  // sub-lattices
+  ConvSrc src(const void* hi, const void* lo, int C, int lattices = 1) {
+    ConvSrc s;
+    s.C = C;
+    for (int l = 0; l < lattices; ++l) s.hi[l] = map(hi, C, lattices == 4 ? l : -1);
+    if (lo)
+      for (int l = 0; l < lattices; ++l) s.lo[l] = map(lo, C, lattices == 4 ? l : -1);
+    return s;
+  }
   // appends a segment of nch 64-channel chunks (wcol1 as ConvSeg::wcol1)
   void seg(int map, int dy, int dx, int nch, int wcol1 = 0) {
     if (p.nseg >= kMaxSeg) {
@@ -642,9 +704,36 @@ struct ConvBuilder {
     p.seg[p.nseg++] = ConvSeg{(int16_t)map, (int16_t)dy, (int16_t)dx, (int16_t)nch, wcol1};
     p.ksteps += nch;
   }
+  // Appends the K segments of `taps` over the inputs `src` (a tap's lat picks each input's maps), whose W_hi columns
+  // start at `col` in (tap, input, channel) order, and returns the column after them.  Per tap, over its inputs:
+  // A_hi W_hi, then A_hi W_lo from the W_lo plane at column wlo_col (0: no W_lo plane), then A_lo W_hi for the inputs
+  // that carry lo.
+  int segs(const std::vector<ConvTap>& taps, const std::vector<ConvSrc>& src, int col, int wlo_col) {
+    for (const ConvTap& t : taps) {
+      int c = col;
+      for (const ConvSrc& s : src) {
+        seg(s.hi[t.lat], t.dy, t.dx, s.C / 64, c + 1);
+        c += s.C;
+      }
+      if (wlo_col) {
+        c = col;
+        for (const ConvSrc& s : src) {
+          seg(s.hi[t.lat], t.dy, t.dx, s.C / 64, wlo_col + c + 1);
+          c += s.C;
+        }
+      }
+      c = col;
+      for (const ConvSrc& s : src) {
+        if (s.lo[0] >= 0) seg(s.lo[t.lat], t.dy, t.dx, s.C / 64, c + 1);
+        c += s.C;
+      }
+      col = c;
+    }
+    return col;
+  }
   // n_par == 4: the folded upsample, whose output `out` (out_C channels) has 2H x 2W pixels and is stored through
   // its four parity sub-lattices
-  int finish(const ConvLayerBase& L, const void* out, int out_C, int n_img, int n_par) {
+  int finish(const ConvLayer& L, const void* out, int out_C, int n_img, int n_par) {
     if (err) return err;
     for (int i = p.n_amaps; i < kMaxAMaps; ++i) p.amap[i] = p.amap[0];   // never read: any valid descriptor
     p.bmap = L.wmap;

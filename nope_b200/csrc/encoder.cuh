@@ -152,76 +152,38 @@ struct ActPair {
 // the pair at element offset o of a (hi, lo) pair, keeping a null lo null
 inline ActPair act_at(const ActPair& a, size_t o) { return ActPair{a.hi + o, a.lo ? a.lo + o : nullptr}; }
 
-// the number of fp16 products per filter tap of a convolution: 3 in split precision (A_hi W_hi, A_hi W_lo,
-// A_lo W_hi), 1 in the single-fp16 mode
-inline int tap_products(int precision) { return precision == 0 ? 3 : 1; }
-
-// Weight w of one filter tap in the layout split_tap reads: dst[0] = W_hi = fp16(w); with 3 products also
-// dst[stride] = W_lo = fp16(w - W_hi) and dst[2 stride] = W_hi.
-inline void put_split_weight(__half* dst, int stride, int prods, float w) {
-  const __half hi = __float2half_rn(w);
-  dst[0] = hi;
-  if (prods == 1) return;
-  dst[stride] = __float2half_rn(w - __half2float(hi));
-  dst[2 * stride] = hi;
-}
-
-// The K segments of one filter tap over (W_hi | W_lo | W_hi) weight columns: A_hi W_hi, A_hi W_lo, A_lo W_hi from
-// the maps hi and lo; lo < 0 (single-fp16 mode): A_hi W_hi alone.
-inline void split_tap(ConvBuilder& b, int hi, int lo, int dy, int dx, int nch) {
-  b.seg(hi, dy, dx, nch);
-  if (lo < 0) return;
-  b.seg(hi, dy, dx, nch);
-  b.seg(lo, dy, dx, nch);
-}
-
-// A convolution of the template encoder and the VAE engines: packed weights [cout][K] fp16, K = taps x
-// (W_hi | W_lo | W_hi) x cin, then, for a convolution with a 1x1 shortcut, (S_hi | S_lo | S_hi) x cin_sc; in the
-// single-fp16 mode each tap holds W_hi alone: K = taps x cin (+ cin_sc).  cout is padded to 64 with zero rows.
-struct SplitConv : ConvLayerBase {
-  int cin_sc = 0, k = 1;
-};
-
-// What the template encoder and the VAE engines share: the handle's state, the split-precision convolutions, their
-// packing and their launch.  Every activation buffer holds `cap` images.
-struct SplitConvEngine {
+// What the template encoder and the VAE engines share: the handle's state, the convolution layers, their packing and
+// their launch.  Every activation buffer holds `cap` images.
+struct ImageEngine {
   int device = 0, num_sms = 132;
   int precision = 0;                  // 0: split (hi, lo) operands; 1: single fp16 (set before finalize)
   bool finalized = false;
   StagedWeights staged;
-  std::map<std::string, SplitConv> convs;
+  std::map<std::string, ConvLayer> convs;
   DeviceAllocs mem;
   TmapCache tmaps;
   int64_t launches = 0;
   int cap = 0;                        // images the workspace holds
 
-  // W [cout_real][cin][k*k] and bias [cout_real] in float64 (any folding done), optional 1x1 shortcut
-  // Ws [cout_real][cin_sc] -> convs[name]
-  int pack_conv(const std::string& name, int cout_real, int cin, int k, const std::vector<double>& W,
+  // L's taps, W [cout_real][cin][taps] and bias [cout_real] in float64 (any folding done), optional 1x1 shortcut
+  // Ws [cout_real][cin_sc] in the extra K columns -> convs[name].  Split precision packs the W_lo plane; cout is padded
+  // to 64 with zero rows.
+  int pack_conv(const std::string& name, ConvLayer L, int cout_real, int cin, const std::vector<double>& W,
                 const std::vector<double>& bias, int cin_sc = 0, const std::vector<double>* Ws = nullptr) {
-    SplitConv L;
+    const int taps = L.k * L.k;
     L.cin = cin;
-    L.cin_sc = cin_sc;
-    L.k = k;
     L.cout = (cout_real + 63) / 64 * 64;
-    const int taps = k * k, prods = tap_products(precision);
-    L.K = (taps * cin + cin_sc) * prods;
+    L.K = taps * cin + cin_sc;
+    L.wlo = precision == 0;
     NOPE_CHECK(cin % 64 == 0 && cin_sc % 64 == 0, name + ": input channels must be a multiple of 64");
-    L.bn = pick_bn(L.cout);
-    std::vector<__half> packed((size_t)L.cout * L.K, __float2half_rn(0.f));
-    for (int o = 0; o < cout_real; ++o) {
-      for (int c = 0; c < cin; ++c)
-        for (int t = 0; t < taps; ++t)
-          put_split_weight(&packed[(size_t)o * L.K + (size_t)t * prods * cin + c], cin, prods,
-                           (float)W[((size_t)o * cin + c) * taps + t]);
-      for (int c = 0; c < cin_sc; ++c)
-        put_split_weight(&packed[(size_t)o * L.K + (size_t)taps * prods * cin + c], cin_sc, prods,
-                         (float)(*Ws)[(size_t)o * cin_sc + c]);
-    }
+    const std::vector<float> w(W.begin(), W.end());
+    std::vector<float> ws;
+    if (Ws) ws.assign(Ws->begin(), Ws->end());
     std::vector<float> b(L.cout, 0.f);
     for (int o = 0; o < cout_real; ++o) b[o] = (float)bias[o];
-    if (mem.upload(&L.w, packed) || mem.upload(&L.bias, b)) return -1;
-    if (make_weight_map(&L.wmap, L.w, L.cout, L.K, L.bn)) return -1;
+    std::vector<WeightBlock> blocks{{w.data(), cout_real, cin, taps, 0, 0}};
+    if (cin_sc) blocks.push_back({ws.data(), cout_real, cin_sc, 1, 0, taps * cin});
+    if (pack_conv_layer(mem, L, blocks, b)) return -1;
     convs[name] = L;
     return 0;
   }
@@ -230,7 +192,7 @@ struct SplitConvEngine {
   // H x H.  in: (hi, lo) base pointers of each input pair with their lattice (-1: plain NHWC of side H); a tap's lat
   // is the index of its input pair; fp16 mode: the hi maps only.  K order: per tap A_hi W_hi, A_hi W_lo, A_lo W_hi,
   // then the shortcut's segments.
-  int conv(const SplitConv& L, const std::vector<std::pair<ActPair, int>>& in, const std::vector<ConvTap>& taps,
+  int conv(const ConvLayer& L, const std::vector<std::pair<ActPair, int>>& in, const std::vector<ConvTap>& taps,
            const ActPair* sc, int H, int n, bool relu, const ActPair* res, __half* out_hi, __half* out_lo,
            float* out_f32, cudaStream_t st) {
     TileGeom g;
@@ -238,18 +200,18 @@ struct SplitConvEngine {
     NOPE_CHECK(in.size() + (sc ? 1 : 0) <= (size_t)kMaxAMaps / 2, "conv: too many input maps");
     ConvBuilder b(tmaps, g, cap);
     ConvParams& p = b.p;
-    int mh[kMaxAMaps / 2], ml[kMaxAMaps / 2];
+    ConvSrc src;
+    src.C = L.cin;
     for (size_t i = 0; i < in.size(); ++i) {
-      mh[i] = b.map(in[i].first.hi, L.cin, in[i].second);
-      ml[i] = precision == 0 ? b.map(in[i].first.lo, L.cin, in[i].second) : -1;
+      src.hi[i] = b.map(in[i].first.hi, L.cin, in[i].second);
+      if (in[i].first.lo) src.lo[i] = b.map(in[i].first.lo, L.cin, in[i].second);
     }
-    for (const ConvTap& t : taps) split_tap(b, mh[t.lat], ml[t.lat], t.dy, t.dx, L.cin / 64);
-    if (sc) {
-      const int h = b.map(sc->hi, L.cin_sc), l = precision == 0 ? b.map(sc->lo, L.cin_sc) : -1;
-      split_tap(b, h, l, 0, 0, L.cin_sc / 64);
-    }
+    const int wlo_col = L.wlo ? L.K : 0;
+    int col = b.segs(taps, {src}, 0, wlo_col);
+    // the shortcut's channels are the W_hi columns past the taps
+    if (sc) col = b.segs({ConvTap{0, 0, 0}}, {b.src(sc->hi, sc->lo, L.K - col)}, col, wlo_col);
     if (b.finish(L, out_hi, L.cout, n, 1)) return -1;
-    NOPE_CHECK(p.ksteps * 64 == L.K, "conv: segment table");
+    NOPE_CHECK(col == L.K && p.ksteps * 64 == (L.wlo ? 3 : 1) * L.K, "conv: segment table");
     p.relu = relu ? 1 : 0;
     p.res_hi = res ? res->hi : nullptr;
     p.res_lo = res ? res->lo : nullptr;
@@ -262,7 +224,7 @@ struct SplitConvEngine {
 
 }  // namespace nope
 
-struct nope_encoder : nope::SplitConvEngine {
+struct nope_encoder : nope::ImageEngine {
   static constexpr const char* kName = "encoder";
   enum { kStem, kBottleneck, kProjector };
   int D = 8;
@@ -323,8 +285,9 @@ struct nope_encoder : nope::SplitConvEngine {
   }
 
   // ---------------------------------------------------------------- weights
-  // fold eval-mode BN (eps 1e-5) into the conv in double, then pack_conv; bnkey empty: no BN, no bias
-  int make_conv(const std::string& name, const std::string& wkey, const std::string& bnkey) {
+  // fold eval-mode BN (eps 1e-5) into the conv in double, then pack_conv (a 1x1 or 3x3 pad-1 convolution at input
+  // stride 1 or 2); bnkey empty: no BN, no bias
+  int make_conv(const std::string& name, const std::string& wkey, const std::string& bnkey, int stride = 1) {
     const nope::HostTensor& W = staged.at(wkey);
     const int cout = (int)W.shape[0], cin = (int)W.shape[1], k = (int)W.shape[2], taps = k * k;
     std::vector<double> scale(cout, 1.0), shift(cout, 0.0);
@@ -338,7 +301,7 @@ struct nope_encoder : nope::SplitConvEngine {
     }
     std::vector<double> w(W.data.size());
     for (size_t i = 0; i < w.size(); ++i) w[i] = (double)W.data[i] * scale[i / ((size_t)cin * taps)];
-    return pack_conv(name, cout, cin, k, w, shift);
+    return pack_conv(name, nope::conv_shape(k, stride, -(k / 2), -(k / 2)), cout, cin, w, shift);
   }
 
   // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
@@ -357,10 +320,11 @@ struct nope_encoder : nope::SplitConvEngine {
         }
         if (mem.upload(&stem_w, w) || mem.upload(&stem_b, bias)) return -1;
       } else if (m.kind == kBottleneck) {
+        const int s = m.Hi / m.Ho;
         if (make_conv(p + ".conv1", p + ".conv1.weight", p + ".bn1") ||
-            make_conv(p + ".conv2", p + ".conv2.weight", p + ".bn2") ||
+            make_conv(p + ".conv2", p + ".conv2.weight", p + ".bn2", s) ||
             make_conv(p + ".conv3", p + ".conv3.weight", p + ".bn3") ||
-            (has_down(m) && make_conv(p + ".down", p + ".downsample.0.weight", p + ".downsample.1")))
+            (has_down(m) && make_conv(p + ".down", p + ".downsample.0.weight", p + ".downsample.1", s)))
           return -1;
       } else if (make_conv("projector.1", "projector.1.weight", "") ||
                  make_conv("projector.3", "projector.3.weight", "")) {
@@ -382,21 +346,16 @@ struct nope_encoder : nope::SplitConvEngine {
   }
   int ensure_workspace(int B) { return B <= cap ? 0 : nope::grow_workspace(this, std::tie(cap), nullptr, B); }
 
-  // out = [relu](conv(in) + bias [+ res]) of a 1x1 or 3x3 (pad 1) convolution at stride 1 or 2 over an input of side
-  // Hin; a stride-2 convolution reads its input as its four stride-2 sub-lattices (same trick as HardDownsample).
-  // out_f32: the fp32 output instead of out's lo half.
-  int conv_at(const nope::SplitConv& L, const nope::ActPair& in, int Hin, int stride, const nope::ActPair& out, int n,
-              bool relu, const nope::ActPair* res, float* out_f32, cudaStream_t st) {
+  // out = [relu](conv(in) + bias [+ res]) of layer L over an input of side Hin; a stride-2 convolution reads its input
+  // as its four stride-2 sub-lattices (same trick as HardDownsample).  out_f32: the fp32 output instead of out's lo
+  // half.
+  int conv_at(const nope::ConvLayer& L, const nope::ActPair& in, int Hin, const nope::ActPair& out, int n, bool relu,
+              const nope::ActPair* res, float* out_f32, cudaStream_t st) {
     using namespace nope;
     std::vector<std::pair<ActPair, int>> src;
-    for (int t = 0; t < (stride == 1 ? 1 : 4); ++t) src.push_back({in, stride == 1 ? -1 : t});
-    std::vector<ConvTap> taps;
-    for (int ky = 0; ky < L.k; ++ky)
-      for (int kx = 0; kx < L.k; ++kx) {
-        const int oy = L.k == 3 ? ky - 1 : 0, ox = L.k == 3 ? kx - 1 : 0;
-        taps.push_back(stride == 1 ? ConvTap{0, oy, ox} : stride2_tap(oy, ox));
-      }
-    return conv(L, src, taps, nullptr, Hin / stride, n, relu, res, out.hi, out_f32 ? nullptr : out.lo, out_f32, st);
+    for (int t = 0; t < (L.stride == 1 ? 1 : 4); ++t) src.push_back({in, L.stride == 1 ? -1 : t});
+    return conv(L, src, L.taps(), nullptr, Hin / L.stride, n, relu, res, out.hi, out_f32 ? nullptr : out.lo, out_f32,
+                st);
   }
 
   // bottleneck m on buf[cur] -> buf[cur] (the new cur)
@@ -407,15 +366,14 @@ struct nope_encoder : nope::SplitConvEngine {
     for (int i = 0; i < 5; ++i)
       if (i != cur) f[nf++] = i;
     const ActPair &x = buf[cur], &a = buf[f[0]], &bb = buf[f[1]], &r = buf[f[2]], &o = buf[f[3]];
-    const int s = m.Hi / m.Ho;
-    if (conv_at(convs.at(m.name + ".conv1"), x, m.Hi, 1, a, n, true, nullptr, nullptr, st)) return -1;
-    if (conv_at(convs.at(m.name + ".conv2"), a, m.Hi, s, bb, n, true, nullptr, nullptr, st)) return -1;
+    if (conv_at(convs.at(m.name + ".conv1"), x, m.Hi, a, n, true, nullptr, nullptr, st)) return -1;
+    if (conv_at(convs.at(m.name + ".conv2"), a, m.Hi, bb, n, true, nullptr, nullptr, st)) return -1;
     const ActPair* res = &x;
     if (has_down(m)) {
-      if (conv_at(convs.at(m.name + ".down"), x, m.Hi, s, r, n, false, nullptr, nullptr, st)) return -1;
+      if (conv_at(convs.at(m.name + ".down"), x, m.Hi, r, n, false, nullptr, nullptr, st)) return -1;
       res = &r;
     }
-    if (conv_at(convs.at(m.name + ".conv3"), bb, m.Ho, 1, o, n, true, res, nullptr, st)) return -1;
+    if (conv_at(convs.at(m.name + ".conv3"), bb, m.Ho, o, n, true, res, nullptr, st)) return -1;
     cur = f[3];
     return 0;
   }
@@ -425,9 +383,9 @@ struct nope_encoder : nope::SplitConvEngine {
   int projector(int cur, int H, int B, float* out, cudaStream_t st) {
     using namespace nope;
     const int nxt = (cur + 1) % 5;
-    if (conv_at(convs.at("projector.1"), buf[cur], H, 1, buf[nxt], B, true, nullptr, nullptr, st)) return -1;
+    if (conv_at(convs.at("projector.1"), buf[cur], H, buf[nxt], B, true, nullptr, nullptr, st)) return -1;
     const int nx2 = (cur + 2) % 5;
-    if (conv_at(convs.at("projector.3"), buf[nxt], H, 1, buf[nx2], B, false, nullptr, proj_out, st)) return -1;
+    if (conv_at(convs.at("projector.3"), buf[nxt], H, buf[nx2], B, false, nullptr, proj_out, st)) return -1;
     enc_extract_kernel<<<ew_grid((long long)B * D * H * H), 256, 0, st>>>(proj_out, out, B, D, H * H,
                                                                           convs.at("projector.3").cout);
     NOPE_CUDA(cudaGetLastError());

@@ -16,8 +16,8 @@
 //   int prestage(const float* ref, int B, cudaStream_t)                  the pose-independent prefix per reference;
 //   int forward_chunk(poses, hyp0, n, N, query, out_emb, score_part, cudaStream_t, int Q);
 //   int rank(part, sim, B, N, Q, k, topv, topi, idx_base, cudaStream_t) the similarities and top-k from the partials.
-// An image engine derives from SplitConvEngine (encoder.cuh), which holds `launches`, `mem` and the split-precision
-// convolutions, and provides `kChunk` and `std::vector<ImageModule> plan`, built in forward order when the handle is
+// An image engine derives from ImageEngine (encoder.cuh), which holds `launches`, `mem` and the convolution
+// layers, and provides `kChunk` and `std::vector<ImageModule> plan`, built in forward order when the handle is
 // created; its schema, weight packing, forward pass and run_block all walk that plan.  An image encoder
 // (per_rotated_chunk) also provides `float* rot_stage` and `int encode(const float*, int, float*, cudaStream_t)`.
 #pragma once
@@ -28,6 +28,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "conv_tc.cuh"
 #include "kernels.cuh"
 #include "rank.cuh"
 
@@ -110,6 +111,31 @@ class DeviceAllocs {
  private:
   std::vector<void*> ptrs_;
 };
+
+// One block of a layer's weights: fp32 [rows][cin][taps] in host or device memory, placed at weight row `row` and
+// W_hi column `col` (its remainders at column K + col of the W_lo plane).  For the folded upsample it is the
+// [rows][cin][3][3] kernel, packed as 4 rows per output channel.
+struct WeightBlock {
+  const float* w;
+  int rows, cin, taps, row, col;
+};
+
+// Packs layer L, whose shape (cin, cout, K, wlo, taps, up) is set, from its weight blocks with pack_conv_weight (bf16:
+// the W_hi plane in bf16) into memory of `mem`; rows no block covers (the zero rows that pad cout) are zero.  Uploads
+// bias (cout values; empty: none) and encodes the weight map of bn rows (bn 0: pick_bn(cout)).
+inline int pack_conv_layer(DeviceAllocs& mem, ConvLayer& L, const std::vector<WeightBlock>& blocks,
+                           const std::vector<float>& bias, bool bf16 = false, cudaStream_t st = 0) {
+  if (!L.bn) L.bn = pick_bn(L.cout);
+  const size_t n = (size_t)L.rows() * L.row_len();
+  if (mem.alloc(&L.w, n)) return -1;
+  NOPE_CUDA(cudaMemsetAsync(L.w, 0, n * sizeof(__half), st));
+  for (const WeightBlock& b : blocks)
+    if (pack_conv_weight(b.w, L.w + (size_t)b.row * L.row_len(), b.rows, b.cin, b.taps, L.up, L.row_len(), b.col,
+                         L.wlo ? L.K : 0, bf16 ? 1 : 0, st))
+      return -1;
+  if (!bias.empty() && mem.upload(&L.bias, bias)) return -1;
+  return make_weight_map(&L.wmap, L.w, L.rows(), L.row_len(), L.bn);
+}
 
 // bump allocator over one device slab (base == nullptr: size computation only)
 struct Bump {

@@ -36,13 +36,6 @@
 
 namespace nope {
 
-// w: [rows][kp(K)] fp16; bn: the tile width of the clustered kernel (up to 256)
-struct LdmConv : ConvLayerBase {
-  int mode = 0;   // 0: 3x3 pad 1, 1: 1x1 / linear, 3: nearest-x2 + 3x3 (folded), 4: 3x3 stride 2 pad 1
-  int skip_c = 0;          // channels of a folded 1x1 skip_connection / identity residual (extra K columns)
-  int k_alg = 0;           // K without identity-residual columns (algorithmic FLOP count)
-  bool geglu = false;      // rows permuted to (64 x | 64 gate) tiles; the epilogue emits x * gelu(gate)
-};
 struct LdmNorm {
   float* gamma = nullptr;
   float* beta = nullptr;
@@ -64,9 +57,8 @@ struct nope_ldm {
   std::vector<int> mult{1, 2, 4};
   bool finalized = false;
   bool hoist = true;        // pose-independent prefix once per reference (prestage)
-  int precision = 0;        // 0: fp16 weights; 1: exact weights -- every packed row is [W_hi | W_lo] and the K loop
+  int precision = 0;        // 0: fp16 weights; 1: exact weights -- every layer has a W_lo plane and the K loop
                             // walks its segment list twice (A W_hi + A W_lo), 2x the MMA work (set before finalize)
-  int kp(int K) const { return precision ? 2 * K : K; }
   int chunk = 256;
   int64_t launches = 0;
 
@@ -74,7 +66,7 @@ struct nope_ldm {
   int mid_ch = 0;
 
   nope::StagedWeights staged;
-  std::map<std::string, nope::LdmConv> convs;
+  std::map<std::string, nope::ConvLayer> convs;
   std::map<std::string, nope::LdmNorm> norms;
   std::map<std::string, int> cb_off;   // transformer prefix -> offset in the cross-term vector
   int cb_width = 0;
@@ -226,37 +218,26 @@ struct nope_ldm {
 
   // ------------------------------------------------------------------ weights
   const HostTensor& H(const std::string& k) const { return staged.at(k); }
-  // dst[(row_off + o) * K + col_off + t * cin + c] = fp16(src[o][c][t])
-  int pack_into(__half* dst, int K, int row_off, int col_off, const HostTensor& t, int cout, int cin, int taps,
-                bool fold_up = false) {
-    NOPE_CHECK(t.data.size() == (size_t)cout * cin * (fold_up ? 9 : taps), "pack_into: size mismatch");
-    return nope::pack_conv_weight(t.data.data(), dst + (size_t)row_off * kp(K), cout, cin, taps, fold_up, kp(K),
-                                  col_off, precision ? K : 0, 0, 0);
-  }
-  int finish_conv(const std::string& name, nope::LdmConv& L, int rows, const std::vector<float>& bias) {
+  // packs layer L (shape, cin, cout, K and the LDM fields set) from its weight blocks -> convs[name]
+  int add_conv(const std::string& name, nope::ConvLayer L, const std::vector<nope::WeightBlock>& blocks,
+               const std::vector<float>& bias) {
     using namespace nope;
     if (L.k_alg == 0) L.k_alg = L.K;
+    L.wlo = precision != 0;
     L.bn = (!L.geglu && L.cout % 256 == 0) ? 256 : pick_bn(L.cout);
     NOPE_CHECK(L.bn != 0 && L.K % 64 == 0, name + ": channel counts must be multiples of 64");
-    if (!bias.empty() && mem.upload(&L.bias, bias)) return -1;
-    if (make_weight_map(&L.wmap, L.w, rows, kp(L.K), L.bn)) return -1;
+    if (pack_conv_layer(mem, L, blocks, bias)) return -1;
     convs[name] = L;
     return 0;
   }
-  int alloc_w(nope::LdmConv& L, int rows) { return mem.alloc(&L.w, (size_t)rows * kp(L.K)); }
-  // plain convolution / linear layer.  extra_bias (optional) is added to the bias.
-  int make_conv(const std::string& name, const std::string& wkey, const std::string& bkey, int mode,
+  // plain convolution / linear layer of the given shape.  extra_bias (optional) is added to the bias.
+  int make_conv(const std::string& name, const std::string& wkey, const std::string& bkey, nope::ConvLayer L,
                 const std::string& extra_bias = "") {
     const HostTensor& W = H(wkey);
-    nope::LdmConv L;
-    L.mode = mode;
     L.cout = (int)W.shape[0];
     L.cin = (int)W.shape[1];
-    const int taps = mode == 1 ? 1 : (mode == 3 ? 4 : 9);
+    const int taps = L.k * L.k;
     L.K = L.cin * taps;
-    const int rows = mode == 3 ? 4 * L.cout : L.cout;
-    if (alloc_w(L, rows)) return -1;
-    if (pack_into(L.w, L.K, 0, 0, W, L.cout, L.cin, taps, mode == 3)) return -1;
     std::vector<float> bias;
     if (!bkey.empty()) {
       bias = H(bkey).data;
@@ -265,7 +246,7 @@ struct nope_ldm {
         for (size_t i = 0; i < bias.size(); ++i) bias[i] += e[i];
       }
     }
-    return finish_conv(name, L, rows, bias);
+    return add_conv(name, L, {{W.data.data(), L.cout, L.cin, taps, 0, 0}}, bias);
   }
   // [c][c] identity as a host "weight": a residual add rides in the GEMM as one more K-segment
   // (out = W x + I r).  The product of an fp16 value with 1.0 is exact and accumulates in fp32, so
@@ -283,17 +264,15 @@ struct nope_ldm {
   // linear layer (1x1) whose output gets a residual of `cout` channels added
   int make_lin_res(const std::string& name, const std::string& wkey, const std::string& bkey) {
     const HostTensor& W = H(wkey);
-    nope::LdmConv L;
-    L.mode = 1;
+    nope::ConvLayer L = nope::conv1x1();
     L.cout = (int)W.shape[0];
     L.cin = (int)W.shape[1];
     L.skip_c = L.cout;
     L.K = L.cin + L.skip_c;
     L.k_alg = L.cin;
-    if (alloc_w(L, L.cout)) return -1;
-    if (pack_into(L.w, L.K, 0, 0, W, L.cout, L.cin, 1) || pack_into(L.w, L.K, 0, L.cin, identity(L.cout), L.cout, L.cout, 1))
-      return -1;
-    return finish_conv(name, L, L.cout, H(bkey).data);
+    const HostTensor I = identity(L.cout);
+    return add_conv(name, L, {{W.data.data(), L.cout, L.cin, 1, 0, 0}, {I.data.data(), L.cout, L.cout, 1, 0, L.cin}},
+                    H(bkey).data);
   }
   int make_norm(const std::string& name, const std::string& prefix) {
     nope::LdmNorm n;
@@ -307,11 +286,11 @@ struct nope_ldm {
     // ResBlock (ldm/openaimodel.py:217-286).  emb = 0, so emb_layers(emb) = Linear(SiLU(0)) =
     // emb_layers.1.bias: folded into the first convolution's bias.
     if (make_norm(p + ".n1", p + ".in_layers.0") || make_norm(p + ".n2", p + ".out_layers.0")) return -1;
-    if (make_conv(p + ".c1", p + ".in_layers.2.weight", p + ".in_layers.2.bias", 0, p + ".emb_layers.1.bias"))
+    if (make_conv(p + ".c1", p + ".in_layers.2.weight", p + ".in_layers.2.bias", nope::conv3x3(),
+                  p + ".emb_layers.1.bias"))
       return -1;
     const HostTensor& W2 = H(p + ".out_layers.3.weight");
-    nope::LdmConv L;
-    L.mode = 0;
+    nope::ConvLayer L = nope::conv3x3();
     L.cout = (int)W2.shape[0];
     L.cin = (int)W2.shape[1];
     std::vector<float> bias = H(p + ".out_layers.3.bias").data;
@@ -327,18 +306,17 @@ struct nope_ldm {
     if (id_skip) L.skip_c = L.cout;
     L.K = 9 * L.cin + L.skip_c;
     if (id_skip) L.k_alg = 9 * L.cin;
-    if (alloc_w(L, L.cout)) return -1;
-    if (pack_into(L.w, L.K, 0, 0, W2, L.cout, L.cin, 9)) return -1;
-    if (has_skip && pack_into(L.w, L.K, 0, 9 * L.cin, H(p + ".skip_connection.weight"), L.cout, L.skip_c, 1))
-      return -1;
-    if (id_skip && pack_into(L.w, L.K, 0, 9 * L.cin, identity(L.cout), L.cout, L.cout, 1)) return -1;
-    return finish_conv(p + ".c2", L, L.cout, bias);
+    // the skip's weights follow the 3x3's in the extra K columns
+    const HostTensor I = id_skip ? identity(L.cout) : HostTensor();
+    const float* ws = has_skip ? H(p + ".skip_connection.weight").data.data() : I.data.data();
+    return add_conv(p + ".c2", L, {{W2.data.data(), L.cout, L.cin, 9, 0, 0}, {ws, L.cout, L.skip_c, 1, 0, 9 * L.cin}},
+                    bias);
   }
   int make_st(const std::string& p) {
     const std::string t = p + ".transformer_blocks.0";
     const int c = (int)H(p + ".norm.weight").shape[0];
     if (make_norm(p + ".norm", p + ".norm")) return -1;
-    if (make_conv(p + ".proj_in", p + ".proj_in.weight", p + ".proj_in.bias", 1)) return -1;
+    if (make_conv(p + ".proj_in", p + ".proj_in.weight", p + ".proj_in.bias", nope::conv1x1())) return -1;
     if (make_lin_res(p + ".proj_out", p + ".proj_out.weight", p + ".proj_out.bias")) return -1;
     if (make_lin_res(p + ".to_out", t + ".attn1.to_out.0.weight", t + ".attn1.to_out.0.bias")) return -1;
     {  // the feed-forward projection with GEGLU fused into the epilogue: tile t of 128 rows =
@@ -358,30 +336,26 @@ struct nope_ldm {
                       Wp.data.begin() + (size_t)dst * c);
             bp[dst] = b[src];
           }
-      nope::LdmConv L;
-      L.mode = 1;
+      nope::ConvLayer L = nope::conv1x1();
       L.cin = c;
       L.cout = 2 * inner;
       L.K = c;
       L.geglu = true;
-      if (alloc_w(L, 2 * inner) || pack_into(L.w, c, 0, 0, Wp, 2 * inner, c, 1) ||
-          finish_conv(p + ".ff1g", L, 2 * inner, bp))
-        return -1;
+      if (add_conv(p + ".ff1g", L, {{Wp.data.data(), 2 * inner, c, 1, 0, 0}}, bp)) return -1;
       NOPE_CHECK(convs.at(p + ".ff1g").bn == 128, "GEGLU projection must tile by 128");
     }
     if (make_lin_res(p + ".ff2", t + ".ff.net.2.weight", t + ".ff.net.2.bias")) return -1;
     {  // q | k | v of the self-attention as one GEMM (no bias, ldm/attention.py:160-162)
-      nope::LdmConv L;
-      L.mode = 1;
+      nope::ConvLayer L = nope::conv1x1();
       L.cin = c;
       L.cout = 3 * c;
       L.K = c;
-      if (alloc_w(L, 3 * c)) return -1;
-      if (pack_into(L.w, c, 0, 0, H(t + ".attn1.to_q.weight"), c, c, 1) ||
-          pack_into(L.w, c, c, 0, H(t + ".attn1.to_k.weight"), c, c, 1) ||
-          pack_into(L.w, c, 2 * c, 0, H(t + ".attn1.to_v.weight"), c, c, 1))
+      if (add_conv(p + ".qkv", L,
+                   {{H(t + ".attn1.to_q.weight").data.data(), c, c, 1, 0, 0},
+                    {H(t + ".attn1.to_k.weight").data.data(), c, c, 1, c, 0},
+                    {H(t + ".attn1.to_v.weight").data.data(), c, c, 1, 2 * c, 0}},
+                   {}))
         return -1;
-      if (finish_conv(p + ".qkv", L, 3 * c, {})) return -1;
     }
     for (int n = 1; n <= 3; n += 2) {   // norm2 only feeds attn2's queries, which cancel (see below)
       nope::LdmNorm ln;
@@ -440,26 +414,26 @@ struct nope_ldm {
       std::copy(w.begin(), w.end(), W.data.begin());
       std::vector<float> bias(64, 0.f);
       std::copy(H("out.2.bias").data.begin(), H("out.2.bias").data.end(), bias.begin());
-      nope::LdmConv L;
-      L.mode = 0;
+      nope::ConvLayer L = nope::conv3x3();
       L.cout = 64;
       L.cin = mc;
       L.K = 9 * mc;
-      if (alloc_w(L, 64) || pack_into(L.w, L.K, 0, 0, W, 64, mc, 9) || finish_conv("out.2", L, 64, bias)) return -1;
+      if (add_conv("out.2", L, {{W.data.data(), 64, mc, 9, 0, 0}}, bias)) return -1;
     }
     for (size_t i = 1; i < inp.size(); ++i) {
       const std::string p = "input_blocks." + std::to_string(i);
       if (inp[i].kind == 1) {
         if (make_res(p + ".0") || make_st(p + ".1")) return -1;
       } else {
-        if (make_conv(p + ".0.op", p + ".0.op.weight", p + ".0.op.bias", 4)) return -1;
+        if (make_conv(p + ".0.op", p + ".0.op.weight", p + ".0.op.bias", nope::conv3x3_s2())) return -1;
       }
     }
     if (make_res("middle_block.0") || make_st("middle_block.1") || make_res("middle_block.2")) return -1;
     for (size_t i = 0; i < outp.size(); ++i) {
       const std::string p = "output_blocks." + std::to_string(i);
       if (make_res(p + ".0") || make_st(p + ".1")) return -1;
-      if (outp[i].up && make_conv(p + ".2.conv", p + ".2.conv.weight", p + ".2.conv.bias", 3)) return -1;
+      if (outp[i].up && make_conv(p + ".2.conv", p + ".2.conv.weight", p + ".2.conv.bias", nope::conv_upsample3x3()))
+        return -1;
     }
     if (make_norm("out.0", "out.0")) return -1;
     return make_cross();
@@ -505,57 +479,40 @@ struct nope_ldm {
 
   // ------------------------------------------------------------------ op launchers
   // out[n_img, So, So, cout] = conv(L, in) [+ 1x1 skip or identity residual over cat(sk0, sk1)] + bias
-  int conv(const nope::LdmConv& L, const __half* in, __half* out, int So, int n_img, cudaStream_t st,
+  int conv(const nope::ConvLayer& L, const __half* in, __half* out, int So, int n_img, cudaStream_t st,
            float2* stats = nullptr, const __half* sk0 = nullptr, int skc0 = 0,
            const __half* sk1 = nullptr, int skc1 = 0, float* out_f32 = nullptr) {
     using namespace nope;
     NOPE_CHECK(skc0 + skc1 == L.skip_c, "conv: skip channel mismatch");
-    NOPE_CHECK(!L.skip_c || ((L.mode == 0 || L.mode == 1) && sk0 && skc0 % 64 == 0 && skc1 % 64 == 0),
+    NOPE_CHECK(!L.skip_c || (!L.up && L.stride == 1 && sk0 && skc0 % 64 == 0 && skc1 % 64 == 0),
                "conv: bad skip sources");
-    NOPE_CHECK(!(stats && L.mode == 3), "upsample conv has no fused statistics");
+    NOPE_CHECK(!(stats && L.up), "upsample conv has no fused statistics");
     ++launches;
     TileGeom g;
-    if (make_geom(L.mode == 3 ? So / 2 : So, L.mode == 3 ? So / 2 : So, &g)) return -1;
+    if (make_geom(L.up ? So / 2 : So, L.up ? So / 2 : So, &g)) return -1;
     ConvBuilder b(tmaps, g, cap);
     ConvParams& p = b.p;
-    const int nch = L.cin / 64;
-    if (L.mode == 4) {
-      // in(2y + ky - 1, 2x + kx - 1) on the four stride-2 lattices of the 2So x 2So input
-      int m[4];
-      for (int t = 0; t < 4; ++t) m[t] = b.map(in, L.cin, t);
-      for (int ky = 0; ky < 3; ++ky)
-        for (int kx = 0; kx < 3; ++kx) {
-          const ConvTap t = stride2_tap(ky - 1, kx - 1);
-          b.seg(m[t.lat], t.dy, t.dx, nch);
-        }
-    } else {
-      const int m = b.map(in, L.cin);
-      if (L.mode == 3) {
-        for (int a = 0; a < 2; ++a)
-          for (int c = 0; c < 2; ++c) b.seg(m, a - 1, c - 1, nch);
-      } else {
-        const int taps = L.mode == 0 ? 9 : 1;
-        for (int t = 0; t < taps; ++t) b.seg(m, L.mode == 0 ? t / 3 - 1 : 0, L.mode == 0 ? t % 3 - 1 : 0, nch);
-      }
-    }
+    // a stride-2 convolution reads the four stride-2 lattices of its 2So x 2So input
+    int col = b.segs(L.taps(), {b.src(in, nullptr, L.cin, L.stride == 2 ? 4 : 1)}, 0, 0);
     if (L.skip_c) {
-      b.seg(b.map(sk0, skc0), 0, 0, skc0 / 64);
-      if (sk1) b.seg(b.map(sk1, skc1), 0, 0, skc1 / 64);
+      std::vector<ConvSrc> sk{b.src(sk0, nullptr, skc0)};
+      if (sk1) sk.push_back(b.src(sk1, nullptr, skc1));
+      col = b.segs({ConvTap{0, 0, 0}}, sk, col, 0);
     }
-    NOPE_CHECK(p.ksteps * 64 == L.K, "conv: K mismatch");
-    // exact weights: the same segments again over the W_lo columns (weight columns simply continue past K)
-    for (int i = 0, n = precision ? p.nseg : 0; i < n; ++i) {
+    NOPE_CHECK(col == L.K, "conv: K mismatch");
+    // exact weights: the same segments again over the W_lo plane
+    for (int i = 0, n = L.wlo ? p.nseg : 0; i < n; ++i) {
       const ConvSeg s = p.seg[i];
-      b.seg(s.map, s.dy, s.dx, s.nchunks, s.wcol1);
+      b.seg(s.map, s.dy, s.dx, s.nchunks, s.wcol1 + L.K);
     }
-    if (b.finish(L, out, L.geglu ? L.cout / 2 : L.cout, n_img, L.mode == 3 ? 4 : 1)) return -1;
+    if (b.finish(L, out, L.geglu ? L.cout / 2 : L.cout, n_img, L.up ? 4 : 1)) return -1;
     p.geglu = L.geglu ? 1 : 0;
     p.out_f32 = out_f32;
     p.stats = stats;
     if (prof.begin(st)) return -1;
     const int rc = launch_conv_tc2(p, L.bn, num_sms, st);
     // executed FLOPs (the folded upsample runs 4 parity GEMMs of K = 4 Cin over the source pixels)
-    const double fl = 2.0 * (double)n_img * g.H * g.W * (double)(L.mode == 3 ? 4 * L.cout : L.cout) * (double)L.k_alg;
+    const double fl = 2.0 * (double)n_img * g.H * g.W * (double)L.rows() * (double)L.k_alg;
     if (prof.end(st, {fl, fl, 0})) return -1;
     return rc;
   }
@@ -641,8 +598,8 @@ struct nope_ldm {
   // statistics of `out` in S_out (conv epilogue) for a following SpatialTransformer.norm.
   int resblock(const std::string& p, const __half* x0, int C0, const __half* x1, int C1, __half* out, int S, int n,
                cudaStream_t st) {
-    const nope::LdmConv& c1 = convs.at(p + ".c1");
-    const nope::LdmConv& c2 = convs.at(p + ".c2");
+    const nope::ConvLayer& c1 = convs.at(p + ".c1");
+    const nope::ConvLayer& c2 = convs.at(p + ".c2");
     NOPE_CHECK(c1.cin == C0 + C1, "resblock: channel mismatch");
     if (stats(x0, C0, x1, C1, S, n, S_in, st)) return -1;
     if (gn(norms.at(p + ".n1"), x0, C0, x1, C1, S_in, S, n, T1, true, 1e-5f, st)) return -1;

@@ -1100,8 +1100,10 @@ struct OpConv {
     NOPE_CHECK(H == W, "square images only");
     NOPE_CHECK(C0 % 64 == 0 && C1 % 64 == 0 && Cout % 64 == 0, "channels must be multiples of 64");
     const bool sp = precision == 2;
-    const int taps = mode == 0 ? 9 : (mode == 1 ? 1 : 4);
-    const int Hin = mode == 2 ? 2 * H : (mode == 3 ? H / 2 : H);
+    // the layer shape of each mode (nope_unet::prof_mode is its inverse)
+    const ConvLayer shapes[4] = {conv3x3(), conv1x1(), conv_unshuffle(), conv_upsample3x3()};
+    L = shapes[mode];
+    const int Hin = L.stride == 2 ? 2 * H : (L.up ? H / 2 : H);
     __half *a0 = nullptr, *a0l = nullptr, *a1 = nullptr, *a1l = nullptr, *o = nullptr, *ol = nullptr;
     if (to_nhwc(x0, &a0, s, n_img, C0, Hin * Hin, st, sp ? &a0l : nullptr)) return -1;
     if (x1 && to_nhwc(x1, &a1, s, n_img, C1, Hin * Hin, st, sp ? &a1l : nullptr)) return -1;
@@ -1109,18 +1111,12 @@ struct OpConv {
     if (x1) in1 = Act(a1, C1, a1l);
     if (s.alloc(&o, (size_t)n_img * H * W * Cout) || (sp && s.alloc(&ol, (size_t)n_img * H * W * Cout))) return -1;
     out = Act(o, Cout, ol);
-    L.mode = mode;
     L.cin = C0 + (x1 ? C1 : 0);
     L.cout = Cout;
-    L.K = L.cin * taps;
-    L.Kp = precision >= 1 ? 2 * L.K : L.K;
-    L.bn = pick_bn(Cout);
+    L.K = L.cin * L.k * L.k;
+    L.wlo = precision >= 1;
+    if (pack_conv_layer(s, L, {{weight, Cout, L.cin, L.k * L.k, 0, 0}}, {}, false, st)) return -1;
     L.bias = const_cast<float*>(bias);
-    const int rows = mode == 3 ? 4 * Cout : Cout;
-    if (s.alloc(&L.w, (size_t)rows * L.Kp)) return -1;
-    if (pack_conv_weight(weight, L.w, Cout, L.cin, taps, mode == 3, L.Kp, 0, precision >= 1 ? L.K : 0, 0, st))
-      return -1;
-    if (make_weight_map(&L.wmap, L.w, rows, L.Kp, L.bn)) return -1;
     eng.precision = precision;
     NOPE_CUDA(cudaGetDevice(&eng.device));
     NOPE_CUDA(cudaDeviceGetAttribute(&eng.num_sms, cudaDevAttrMultiProcessorCount, eng.device));
@@ -1401,9 +1397,9 @@ int nope_ldm_run_block(nope_ldm_t* m, const char* name, const float* x0, int C0,
     if (m->transformer(nm, m->XA, m->XC, C0, S, n, m->cb, st)) return -1;
     Co = C0;
   } else if (m->convs.count(nm)) {
-    const LdmConv& L = m->convs.at(nm);
-    NOPE_CHECK(x1 == nullptr && L.cin == C0 && (L.mode == 3 || L.mode == 4), "run_block: not a resample conv");
-    So = L.mode == 3 ? 2 * S : S / 2;
+    const ConvLayer& L = m->convs.at(nm);
+    NOPE_CHECK(x1 == nullptr && L.cin == C0 && (L.up || L.stride == 2), "run_block: not a resample conv");
+    So = L.up ? 2 * S : S / 2;
     if (m->conv(L, m->XA, m->XC, So, n, st)) return -1;
     Co = L.cout;
   } else {

@@ -22,15 +22,6 @@ namespace nope {
 
 constexpr int kHeadsHidden = 128;  // 4 heads x 32 (model_utils.py:368,394)
 
-// w: [rows][Kp] fp16, K = cin x taps
-struct ConvLayer : ConvLayerBase {
-  int mode = 0;  // 0: 3x3 pad1, 1: 1x1, 2: unshuffle+1x1, 3: nearest-x2 upsample + 3x3 (folded)
-  int Kp = 0;             // packed row length: K (fp16 weights) or 2K (W_hi | W_lo, precision >= 1)
-  // pre-norm folded into this (bias-free 1x1) layer: weights hold W diag(gamma); see GnFuse::pre_*
-  float* pre_w1 = nullptr;
-  float* pre_wb = nullptr;
-};
-
 struct NormLayer {
   float* gamma = nullptr;
   float* beta = nullptr;
@@ -102,8 +93,7 @@ struct UNetEngine {
 
   TmapCache tmaps;
 
-  // per-launch profile of the convolution kernel: records carry shape (GEMM resolution, mode 0 3x3 / 1 1x1 /
-  // 2 unshuffle / 3 folded upsample, Cout, K)
+  // per-launch profile of the convolution kernel: records carry shape (GEMM resolution, mode (prof_mode), Cout, K)
   LaunchProfile prof;
   DebugTap dtap;
 
@@ -193,32 +183,27 @@ struct UNetEngine {
 
   // ------------------------------------------------------------------ weights
   int upload_f32(const std::string& key, float** out) { return mem.upload(out, staged.at(key).data); }
-  // pack one conv weight (+ bias) into a ConvLayer.  mode 3 (nearest-x2 upsample + conv3x3,
-  // HardUpsample) first folds the 3x3 kernel into four 2x2 parity kernels (fold_upconv_kernel).
-  // precision >= 1 appends the fp16 remainders as a second K-block: rows are [W_hi (K) | W_lo (K)].
-  int make_conv(const std::string& name, const std::string& wkey, const std::string& bkey, int mode) {
+  // the code of L's shape in the profile's mode column (tools/conv_class_table.py reads it): 0 3x3, 1 1x1,
+  // 2 unshuffle, 3 folded upsample -- the mode ints of nope_op_conv*
+  static int prof_mode(const ConvLayer& L) { return L.up ? 3 : L.stride == 2 ? 2 : L.k == 3 ? 0 : 1; }
+
+  // pack one conv weight (+ bias) into a layer of the given shape (an unshuffle weight's input channel index is
+  // c * 4 + tap; an upsample's 3x3 kernel is folded into four 2x2 parity kernels).  The exact-weight precisions
+  // (1, 2, 4) add the W_lo plane: rows are [W_hi (K) | W_lo (K)].
+  int make_conv(const std::string& name, const std::string& wkey, const std::string& bkey, ConvLayer L) {
     const HostTensor& W = staged.at(wkey);
     const auto& sh = W.shape;
-    ConvLayer L;
-    L.mode = mode;
+    const int taps = L.k * L.k;
     L.cout = (int)sh[0];
-    const int rows = mode == 3 ? 4 * L.cout : L.cout;   // weight-matrix rows
-    const int taps = mode == 0 ? 9 : (mode == 1 ? 1 : 4);
-    L.cin = mode == 2 ? (int)sh[1] / 4 : (int)sh[1];
+    L.cin = L.stride == 2 ? (int)sh[1] / 4 : (int)sh[1];
     L.K = L.cin * taps;
-    const bool wlo = precision == 1 || precision == 2 || precision == 4;
-    L.Kp = wlo ? 2 * L.K : L.K;
+    L.wlo = precision == 1 || precision == 2 || precision == 4;
     NOPE_CHECK(L.cin % 64 == 0, wkey + ": input channels must be a multiple of 64");
-    L.bn = pick_bn(L.cout);
-    NOPE_CHECK(L.bn != 0, wkey + ": output channels must be a multiple of 64");
-    NOPE_CHECK(mode != 3 || (sh.size() == 4 && sh[2] == 3 && sh[3] == 3), wkey + ": expected a 3x3 kernel");
-    if (mem.alloc(&L.w, (size_t)rows * L.Kp)) return -1;
-    if (pack_conv_weight(W.data.data(), L.w, L.cout, L.cin, taps, mode == 3, L.Kp, 0, wlo ? L.K : 0, bf() ? 1 : 0, 0))
+    NOPE_CHECK(pick_bn(L.cout) != 0, wkey + ": output channels must be a multiple of 64");
+    NOPE_CHECK(!L.up || (sh.size() == 4 && sh[2] == 3 && sh[3] == 3), wkey + ": expected a 3x3 kernel");
+    if (pack_conv_layer(mem, L, {{W.data.data(), L.cout, L.cin, taps, 0, 0}},
+                        bkey.empty() ? std::vector<float>() : staged.at(bkey).data, bf()))
       return -1;
-    if (!bkey.empty()) {
-      if (upload_f32(bkey, &L.bias)) return -1;
-    }
-    if (make_weight_map(&L.wmap, L.w, rows, L.Kp, L.bn)) return -1;
     convs[name] = L;
     return 0;
   }
@@ -233,12 +218,12 @@ struct UNetEngine {
     return 0;
   }
   int make_resblock(const std::string& p) {
-    if (make_conv(p + ".block1", p + ".block1.proj.weight", p + ".block1.proj.bias", 0)) return -1;
-    if (make_conv(p + ".block2", p + ".block2.proj.weight", p + ".block2.proj.bias", 0)) return -1;
+    if (make_conv(p + ".block1", p + ".block1.proj.weight", p + ".block1.proj.bias", conv3x3())) return -1;
+    if (make_conv(p + ".block2", p + ".block2.proj.weight", p + ".block2.proj.bias", conv3x3())) return -1;
     if (make_norm(p + ".norm1", p + ".block1.norm", 8)) return -1;
     if (make_norm(p + ".norm2", p + ".block2.norm", 8)) return -1;
     if (staged.has(p + ".res_conv.weight"))
-      if (make_conv(p + ".res", p + ".res_conv.weight", p + ".res_conv.bias", 1)) return -1;
+      if (make_conv(p + ".res", p + ".res_conv.weight", p + ".res_conv.bias", conv1x1())) return -1;
     return 0;
   }
   // to_qkv with the PreNorm GroupNorm(1) folded in (model_utils.py:226-234, 399): packed weights
@@ -278,13 +263,13 @@ struct UNetEngine {
     }
     const std::string tmpkey = "__folded." + name;
     staged.put(tmpkey, std::move(Wf));
-    if (make_conv(name, tmpkey, "", 1)) return -1;
+    if (make_conv(name, tmpkey, "", conv1x1())) return -1;
     ConvLayer& L = convs[name];
     return mem.upload(&L.pre_w1, w1) || mem.upload(&L.pre_wb, wb) ? -1 : 0;
   }
   int make_linattn(const std::string& p) {
     if (make_qkv_folded(p + ".qkvf", p + ".fn.fn.to_qkv.weight", p + ".fn.norm")) return -1;
-    if (make_conv(p + ".out", p + ".fn.fn.to_out.0.weight", p + ".fn.fn.to_out.0.bias", 1)) return -1;
+    if (make_conv(p + ".out", p + ".fn.fn.to_out.0.weight", p + ".fn.fn.to_out.0.bias", conv1x1())) return -1;
     if (make_norm(p + ".outnorm", p + ".fn.fn.to_out.1", 1)) return -1;
     return 0;
   }
@@ -316,7 +301,7 @@ struct UNetEngine {
     tb.data = std::move(bias);
     staged.put("__poseproj.weight", std::move(tw));
     staged.put("__poseproj.bias", std::move(tb));
-    if (make_conv("__poseproj", "__poseproj.weight", "__poseproj.bias", 1)) return -1;
+    if (make_conv("__poseproj", "__poseproj.weight", "__poseproj.bias", conv1x1())) return -1;
     poseproj = convs["__poseproj"];
     return 0;
   }
@@ -331,22 +316,22 @@ struct UNetEngine {
       const std::string p = "downs." + std::to_string(i);
       if (make_resblock(p + ".0") || make_resblock(p + ".1") || make_linattn(p + ".2")) return -1;
       if (i < 3) {
-        if (make_conv(p + ".3", p + ".3.1.weight", p + ".3.1.bias", 2)) return -1;
+        if (make_conv(p + ".3", p + ".3.1.weight", p + ".3.1.bias", conv_unshuffle())) return -1;
       } else {
-        if (make_conv(p + ".3", p + ".3.weight", p + ".3.bias", 0)) return -1;
+        if (make_conv(p + ".3", p + ".3.weight", p + ".3.bias", conv3x3())) return -1;
       }
     }
     if (make_resblock("mid_block1") || make_resblock("mid_block2")) return -1;
     if (make_qkv_folded("mid_attn.qkvf", "mid_attn.fn.fn.to_qkv.weight", "mid_attn.fn.norm")) return -1;
-    if (make_conv("mid_attn.out", "mid_attn.fn.fn.to_out.weight", "mid_attn.fn.fn.to_out.bias", 1))
+    if (make_conv("mid_attn.out", "mid_attn.fn.fn.to_out.weight", "mid_attn.fn.fn.to_out.bias", conv1x1()))
       return -1;
     for (int j = 0; j < 4; ++j) {
       const std::string p = "ups." + std::to_string(j);
       if (make_resblock(p + ".0") || make_resblock(p + ".1") || make_linattn(p + ".2")) return -1;
       if (j < 3) {
-        if (make_conv(p + ".3", p + ".3.1.weight", p + ".3.1.bias", 3)) return -1;
+        if (make_conv(p + ".3", p + ".3.1.weight", p + ".3.1.bias", conv_upsample3x3())) return -1;
       } else {
-        if (make_conv(p + ".3", p + ".3.weight", p + ".3.bias", 0)) return -1;
+        if (make_conv(p + ".3", p + ".3.weight", p + ".3.bias", conv3x3())) return -1;
       }
     }
     if (make_resblock("final_res_block") || make_resblock("final_conv.0")) return -1;
@@ -430,63 +415,31 @@ struct UNetEngine {
 
   // ------------------------------------------------------------------ op launchers
   // out[n_img, So, So, cout] = conv(L, in0 (++ in1)).  The K loop walks, per filter tap and source
-  // tensor, up to three products: A_hi W_hi, A_hi W_lo (precision >= 1), A_lo W_hi (sources that
+  // tensor, up to three products: A_hi W_hi, A_hi W_lo (layers with a W_lo plane), A_lo W_hi (sources that
   // carry a remainder).  `gs` selects the fused GroupNorm epilogue; `stats` (plain epilogue only) receives the
   // GroupNorm partial sums of the output in the ConvParams::stats layout (nope_op_conv_gn checks them).
   int conv(const ConvLayer& L, const Act& in0, const Act& in1, const Act& out, int So, int n_img, int cap_img,
            cudaStream_t st, const GnSpec* gs = nullptr, float2* stats = nullptr) {
     const int c0 = in0.C, c1 = in1.hi ? in1.C : 0;
     NOPE_CHECK(c0 + c1 == L.cin, "conv: channel mismatch");
-    NOPE_CHECK(L.mode != 3 || (in1.hi == nullptr && So % 2 == 0), "upsample conv takes one source");
-    NOPE_CHECK(L.mode != 2 || in1.hi == nullptr, "unshuffle conv takes one source");
+    NOPE_CHECK(!L.up || (in1.hi == nullptr && So % 2 == 0), "upsample conv takes one source");
+    NOPE_CHECK(L.stride == 1 || in1.hi == nullptr, "unshuffle conv takes one source");
     ++launches;
     // the folded upsample's So is the OUTPUT side (2x the source side); tiles and input maps use the source geometry
-    const int Sg = L.mode == 3 ? So / 2 : So;
+    const int Sg = L.up ? So / 2 : So;
     TileGeom g;
     if (make_geom(Sg, Sg, &g)) return -1;
     ConvBuilder b(tmaps, g, cap_img);
     ConvParams& p = b.p;
-    ConvTap taps[9];
-    int n_taps = 0;
-    if (L.mode == 3) {
-      for (int a = 0; a < 2; ++a)
-        for (int c = 0; c < 2; ++c) taps[n_taps++] = ConvTap{0, a - 1, c - 1};
-    } else if (L.mode == 2) {
-      for (int t = 0; t < 4; ++t) taps[n_taps++] = stride2_tap(t >> 1, t & 1);
-    } else if (L.mode == 0) {
-      for (int t = 0; t < 9; ++t) taps[n_taps++] = ConvTap{0, t / 3 - 1, t % 3 - 1};
-    } else {
-      taps[n_taps++] = ConvTap{0, 0, 0};
-    }
-    // activation maps: in0 (hi, lo) per lattice, in1 (hi, lo)
-    const int n_lat = L.mode == 2 ? 4 : 1;
-    int h0[4] = {}, l0[4] = {}, h1 = 0, l1 = 0;
-    for (int lat = 0; lat < n_lat; ++lat) h0[lat] = b.map(in0.hi, c0, L.mode == 2 ? lat : -1);
-    if (in1.hi) h1 = b.map(in1.hi, c1);
-    if (in0.lo)
-      for (int lat = 0; lat < n_lat; ++lat) l0[lat] = b.map(in0.lo, c0, L.mode == 2 ? lat : -1);
-    const bool alo1 = in1.hi && in1.lo;
-    if (alo1) l1 = b.map(in1.lo, c1);
-    // per filter tap and source: A_hi W_hi, A_hi W_lo (packed rows carry W_lo at column K + ...), A_lo W_hi
-    const bool wlo = L.Kp > L.K;
-    for (int ti = 0; ti < n_taps; ++ti) {
-      const ConvTap& t = taps[ti];
-      const int wcol = ti * L.cin + 1;      // ConvSeg::wcol1 of the tap's first source
-      b.seg(h0[t.lat], t.dy, t.dx, c0 / 64, wcol);
-      if (in1.hi) b.seg(h1, t.dy, t.dx, c1 / 64, wcol + c0);
-      if (wlo) {
-        b.seg(h0[t.lat], t.dy, t.dx, c0 / 64, L.K + wcol);
-        if (in1.hi) b.seg(h1, t.dy, t.dx, c1 / 64, L.K + wcol + c0);
-      }
-      if (in0.lo) b.seg(l0[t.lat], t.dy, t.dx, c0 / 64, wcol);
-      if (alo1) b.seg(l1, t.dy, t.dx, c1 / 64, wcol + c0);
-    }
-    if (b.finish(L, out.hi, L.cout, n_img, L.mode == 3 ? 4 : 1)) return -1;
+    std::vector<ConvSrc> src{b.src(in0.hi, in0.lo, c0, L.stride == 2 ? 4 : 1)};
+    if (in1.hi) src.push_back(b.src(in1.hi, in1.lo, c1));
+    b.segs(L.taps(), src, 0, L.wlo ? L.K : 0);
+    if (b.finish(L, out.hi, L.cout, n_img, L.up ? 4 : 1)) return -1;
     p.bf16 = bf() ? 1 : 0;
     p.stats = stats;
-    NOPE_CHECK(!(stats && L.mode == 3), "fused statistics are not available on the upsample conv");
+    NOPE_CHECK(!(stats && L.up), "fused statistics are not available on the upsample conv");
     if (gs) {
-      NOPE_CHECK(L.mode != 3 && !stats, "fused GroupNorm epilogue: no upsample, no plain statistics");
+      NOPE_CHECK(!L.up && !stats, "fused GroupNorm epilogue: no upsample, no plain statistics");
       GnFuse& f = p.gn;
       const int hw = So * So;
       f.G = gs->norm ? gs->norm->G : 0;
@@ -530,7 +483,8 @@ struct UNetEngine {
       f.res_div = gs->res_div;
       f.res_base = gs->res_base;
       if (gs->pre_stats) {
-        NOPE_CHECK(!gs->norm && L.pre_w1 && L.pre_wb && L.mode == 1 && !L.bias, "pre-norm fold: bias-free 1x1 layer with folded weights");
+        NOPE_CHECK(!gs->norm && L.pre_w1 && L.pre_wb && L.k == 1 && L.stride == 1 && !L.bias,
+                   "pre-norm fold: bias-free 1x1 layer with folded weights");
         f.pre_stats = gs->pre_stats;
         f.pre_parts = gs->pre_parts;
         f.pre_inv_cnt = 1.0f / ((float)hw * (float)L.cin);
@@ -557,10 +511,10 @@ struct UNetEngine {
     };
     if (prof.begin(st)) return -1;
     const int rc = launch();
-    // executed FLOPs: mode 3 runs 4 parity GEMMs of K = 4 Cin over the source-resolution pixels;
+    // executed FLOPs: the folded upsample runs 4 parity GEMMs of K = 4 Cin over the source-resolution pixels;
     // the split-precision modes execute 2x / 3x the K-steps of the fp16 mode
     const double px = 2.0 * (double)n_img * So * So * (double)L.cout;
-    if (prof.end(st, {px * (double)p.ksteps * 64.0, px * (double)L.K, 0, make_int4(So, L.mode, L.cout, L.K)}))
+    if (prof.end(st, {px * (double)p.ksteps * 64.0, px * (double)L.K, 0, make_int4(So, prof_mode(L), L.cout, L.K)}))
       return -1;
     return rc;
   }

@@ -345,7 +345,7 @@ vae_dec_extract_kernel(const float* __restrict__ t, int ld, int cap, int n, floa
 // The module kinds, the state_dict schema helpers, the workspace, the launches of a 3x3 convolution, GroupNorm,
 // ResnetBlock2D and the mid-block attention, the forward pass over the plan and run_block.  Every buffer holds `cap`
 // images (the engine's kChunk); mem also holds the workspace and rot_stage.
-struct VaeEngine : SplitConvEngine {
+struct VaeEngine : ImageEngine {
   enum { kConvIn, kResnet, kDown, kUp, kAttention, kConvOut };
   std::vector<ImageModule> plan;              // conv_in first, conv_out last
   std::map<std::string, VaeNorm> norms;
@@ -425,9 +425,10 @@ struct VaeEngine : SplitConvEngine {
     const auto& v = h(k);
     return std::vector<double>(v.begin(), v.end());
   }
-  int make_plain(const std::string& name, int k) {
+  // a convolution with the taps of `shape` from its staged weight and bias
+  int make_plain(const std::string& name, const ConvLayer& shape) {
     const auto& s = staged.at(name + ".weight").shape;
-    return pack_conv(name, (int)s[0], (int)s[1], k, dvec(name + ".weight"), dvec(name + ".bias"));
+    return pack_conv(name, shape, (int)s[0], (int)s[1], dvec(name + ".weight"), dvec(name + ".bias"));
   }
   int make_norm(const std::string& name) {
     VaeNorm N;
@@ -439,14 +440,14 @@ struct VaeEngine : SplitConvEngine {
   // bias) whose (hi, lo) output is conv2's residual; elsewhere it rides in conv2 as extra K-segments.  Either way
   // the shortcut's bias is added to conv2's in float64.
   int make_resnet(const std::string& p, int cin, int cout, bool planar = false) {
-    if (make_norm(p + ".norm1") || make_norm(p + ".norm2") || make_plain(p + ".conv1", 3)) return -1;
+    if (make_norm(p + ".norm1") || make_norm(p + ".norm2") || make_plain(p + ".conv1", conv3x3())) return -1;
     std::vector<double> b = dvec(p + ".conv2.bias");
-    if (cin == cout) return pack_conv(p + ".conv2", cout, cout, 3, dvec(p + ".conv2.weight"), b);
+    if (cin == cout) return pack_conv(p + ".conv2", conv3x3(), cout, cout, dvec(p + ".conv2.weight"), b);
     const std::vector<double> ws = dvec(p + ".conv_shortcut.weight"), bs = dvec(p + ".conv_shortcut.bias");
     for (int o = 0; o < cout; ++o) b[o] += bs[o];
-    if (!planar) return pack_conv(p + ".conv2", cout, cout, 3, dvec(p + ".conv2.weight"), b, cin, &ws);
-    if (pack_conv(p + ".conv_shortcut", cout, cin, 1, ws, std::vector<double>(cout, 0.0))) return -1;
-    return pack_conv(p + ".conv2", cout, cout, 3, dvec(p + ".conv2.weight"), b);
+    if (!planar) return pack_conv(p + ".conv2", conv3x3(), cout, cout, dvec(p + ".conv2.weight"), b, cin, &ws);
+    if (pack_conv(p + ".conv_shortcut", conv1x1(), cout, cin, ws, std::vector<double>(cout, 0.0))) return -1;
+    return pack_conv(p + ".conv2", conv3x3(), cout, cout, dvec(p + ".conv2.weight"), b);
   }
   int make_attention(const std::string& a) {
     if (make_norm(a + "group_norm")) return -1;
@@ -457,9 +458,9 @@ struct VaeEngine : SplitConvEngine {
         W.insert(W.end(), w.begin(), w.end());
         b.insert(b.end(), bb.begin(), bb.end());
       }
-      if (pack_conv(a + "qkv", 1536, 512, 1, W, b)) return -1;
+      if (pack_conv(a + "qkv", conv1x1(), 1536, 512, W, b)) return -1;
     }
-    return pack_conv(a + "proj_attn", 512, 512, 1, dvec(a + "proj_attn.weight"), dvec(a + "proj_attn.bias"));
+    return pack_conv(a + "proj_attn", conv1x1(), 512, 512, dvec(a + "proj_attn.weight"), dvec(a + "proj_attn.bias"));
   }
 
   // workspace of E elements per activation buffer, allocated once so that no call allocates (or synchronises); the
@@ -479,26 +480,19 @@ struct VaeEngine : SplitConvEngine {
   // 3x3 pad-1 convolution at the current level.  Level 0 (parity-planar): one launch per output plane (py, px);
   // tap (oy, ox) of that plane reads input plane ((py + oy) & 1, (px + ox) & 1) at offset ((py + oy) >> 1, ...).
   // Output: out_f32 (+ (hi, lo) when out_lo), residual res (same layout) or the conv's 1x1 shortcut over sc.
-  int conv3(const SplitConv& L, const ActPair& in, int H, int n, const ActPair& out, bool want_lo, float* out_f32,
+  int conv3(const ConvLayer& L, const ActPair& in, int H, int n, const ActPair& out, bool want_lo, float* out_f32,
             const ActPair* res, const ActPair* sc, cudaStream_t st) {
-    std::vector<ConvTap> taps;
-    if (H < 256) {
-      for (int oy = -1; oy <= 1; ++oy)
-        for (int ox = -1; ox <= 1; ++ox) taps.push_back(ConvTap{0, oy, ox});
-      return conv(L, {{in, -1}}, taps, sc, H, n, false, res, out.hi, want_lo ? out.lo : nullptr, out_f32, st);
-    }
+    if (H < 256)
+      return conv(L, {{in, -1}}, L.taps(), sc, H, n, false, res, out.hi, want_lo ? out.lo : nullptr, out_f32, st);
     NOPE_CHECK(!sc, "vae conv: no shortcut segments at the 256 x 256 level");
     std::vector<std::pair<ActPair, int>> src;
     for (int q = 0; q < 4; ++q) src.push_back({act_at(in, plane_off(q, L.cin)), -1});
     for (int q = 0; q < 4; ++q) {
       const int py = q >> 1, px = q & 1;
-      taps.clear();
-      for (int oy = -1; oy <= 1; ++oy)
-        for (int ox = -1; ox <= 1; ++ox) taps.push_back(stride2_tap(py + oy, px + ox));
       const size_t o = plane_off(q, L.cout);
       ActPair r;
       if (res) r = act_at(*res, o);
-      if (conv(L, src, taps, nullptr, 128, n, false, res ? &r : nullptr, out.hi + o,
+      if (conv(L, src, conv_taps(3, 2, py - 1, px - 1), nullptr, 128, n, false, res ? &r : nullptr, out.hi + o,
                want_lo ? act_at(out, o).lo : nullptr, out_f32 + o, st))
         return -1;
     }
@@ -532,10 +526,10 @@ struct VaeEngine : SplitConvEngine {
       // the 1x1 shortcut, one launch per plane, into x32[cur]'s memory (norm1 was its last reader)
       __half* s = reinterpret_cast<__half*>(x32[cur]);
       sres = ActPair{s, precision == 0 ? s + 4 * plane_off(1, cout) : nullptr};
-      const SplitConv& S = convs.at(p + ".conv_shortcut");
+      const ConvLayer& S = convs.at(p + ".conv_shortcut");
       for (int q = 0; q < 4; ++q) {
         const size_t i = plane_off(q, cin), o = plane_off(q, cout);
-        if (conv(S, {{act_at(xs[cur], i), -1}}, {ConvTap{0, 0, 0}}, nullptr, 128, n, false, nullptr, sres.hi + o,
+        if (conv(S, {{act_at(xs[cur], i), -1}}, S.taps(), nullptr, 128, n, false, nullptr, sres.hi + o,
                  act_at(sres, o).lo, nullptr, st))
           return -1;
       }
@@ -556,8 +550,8 @@ struct VaeEngine : SplitConvEngine {
     const int nxt = 1 - cur;
     if (group_norm(a + "group_norm", x32[cur], 512, 32, n, false, st)) return -1;
     // qkv [n * 1024, 1536] fp32 -> t32 (high halves into xs[nxt].hi, overwritten by proj_attn)
-    const SplitConv& qkv = convs.at(a + "qkv");
-    if (conv(qkv, {{nrm, -1}}, {ConvTap{0, 0, 0}}, nullptr, 32, n, false, nullptr, xs[nxt].hi, nullptr, t32, st))
+    const ConvLayer& qkv = convs.at(a + "qkv");
+    if (conv(qkv, {{nrm, -1}}, qkv.taps(), nullptr, 32, n, false, nullptr, xs[nxt].hi, nullptr, t32, st))
       return -1;
     // S = q k^T / sqrt(512) -> x32[nxt] (overwritten by proj_attn), softmax over keys in place
     float* S = x32[nxt];
@@ -574,7 +568,8 @@ struct VaeEngine : SplitConvEngine {
     NOPE_CUDA(cudaGetLastError());
     launches += 3;
     // x + proj_attn(O)
-    if (conv(convs.at(a + "proj_attn"), {{nrm, -1}}, {ConvTap{0, 0, 0}}, nullptr, 32, n, false, &xs[cur], xs[nxt].hi,
+    const ConvLayer& proj = convs.at(a + "proj_attn");
+    if (conv(proj, {{nrm, -1}}, proj.taps(), nullptr, 32, n, false, &xs[cur], xs[nxt].hi,
              xs[nxt].lo, x32[nxt], st))
       return -1;
     cur = nxt;
@@ -670,7 +665,7 @@ struct nope_vae final : nope::VaeEngine {
       bf[o] = kScale * bo;
       for (size_t i = 0; i < (size_t)512 * 9; ++i) Wf[(size_t)o * 512 * 9 + i] *= kScale;
     }
-    return pack_conv("conv_out", 4, 512, 3, Wf, bf);
+    return pack_conv("conv_out", nope::conv3x3(), 4, 512, Wf, bf);
   }
 
   // packs the staged weights (nope::engine_finalize: every schema key is present, device selected)
@@ -682,7 +677,7 @@ struct nope_vae final : nope::VaeEngine {
       } else if (m.kind == kResnet) {
         rc = make_resnet(m.name, m.Ci, m.Co);
       } else if (m.kind == kDown) {
-        rc = make_plain(m.name + ".conv", 3);
+        rc = make_plain(m.name + ".conv", nope::conv_shape(3, 2, 0, 0));   // pad (0, 1): see downsample
       } else if (m.kind == kAttention) {
         rc = make_attention(m.name + ".");
       } else {
@@ -697,7 +692,7 @@ struct nope_vae final : nope::VaeEngine {
   // Downsample2D: pad (0, 1, 0, 1) + 3x3 stride 2 from side 2H to H.  Tap (ky, kx) reads input (2y + ky, 2x + kx):
   // sub-lattice (ky & 1, kx & 1) at offset (ky >> 1, kx >> 1); the bottom / right zero padding is the TMA's
   // out-of-bounds fill of offset 1.  The 256 x 256 input's sub-lattices are its planes.
-  int downsample(const nope::SplitConv& L, const nope::ActPair& in, int Hin, int n, const nope::ActPair& out,
+  int downsample(const nope::ConvLayer& L, const nope::ActPair& in, int Hin, int n, const nope::ActPair& out,
                  float* out_f32, cudaStream_t st) {
     using namespace nope;
     const int H = Hin / 2;
@@ -709,10 +704,7 @@ struct nope_vae final : nope::VaeEngine {
         src.push_back({in, q});
       }
     }
-    std::vector<ConvTap> taps;
-    for (int ky = 0; ky < 3; ++ky)
-      for (int kx = 0; kx < 3; ++kx) taps.push_back(stride2_tap(ky, kx));
-    return conv(L, src, taps, nullptr, H, n, false, nullptr, out.hi, out.lo, out_f32, st);
+    return conv(L, src, L.taps(), nullptr, H, n, false, nullptr, out.hi, out.lo, out_f32, st);
   }
 
   int run(const nope::ImageModule& m, int n, int& cur, const float* images, cudaStream_t st) override {
@@ -816,7 +808,7 @@ struct nope_vae_decoder final : nope::VaeEngine {
             const int a = fold_dy(py, ky) - py + 1, bb = fold_dy(px, kx) - px + 1;
             Wf[oc * 4 + a * 2 + bb] += W[oc * 9 + ky * 3 + kx];
           }
-      if (pack_conv(name + ".p" + std::to_string(q), C, C, 2, Wf, b)) return -1;
+      if (pack_conv(name + ".p" + std::to_string(q), nope::conv_shape(2, 1, py - 1, px - 1), C, C, Wf, b)) return -1;
     }
     return 0;
   }
@@ -839,7 +831,7 @@ struct nope_vae_decoder final : nope::VaeEngine {
       } else if (m.kind == kUp) {
         rc = make_upsample(m.name + ".conv", m.Co);
       } else {
-        rc = make_norm("decoder.conv_norm_out") || make_plain(m.name, 3);
+        rc = make_norm("decoder.conv_norm_out") || make_plain(m.name, nope::conv3x3());
       }
       if (rc) return -1;
     }
@@ -848,22 +840,19 @@ struct nope_vae_decoder final : nope::VaeEngine {
   }
 
   // Upsample2D from side H (residual stream `cur`, plain NHWC) to 2H -> 1 - cur.  One launch per output parity
-  // (py, px), four taps over the source; the zero padding one row / column past the source's edge is the TMA's
-  // out-of-bounds fill.  Into the 256 x 256 level the parity planes are that level's layout; below it they go to
-  // (t32, nrm) and are interleaved into plain NHWC.
+  // (py, px), the four taps of its layer over the source; the zero padding one row / column past the source's edge is
+  // the TMA's out-of-bounds fill.  Into the 256 x 256 level the parity planes are that level's layout; below it they go
+  // to (t32, nrm) and are interleaved into plain NHWC.
   int upsample(const std::string& name, int C, int H, int n, int& cur, cudaStream_t st) {
     using namespace nope;
     const int nxt = 1 - cur;
     const bool planar = 2 * H == 256;
     for (int q = 0; q < 4; ++q) {
-      const int py = q >> 1, px = q & 1;
-      std::vector<ConvTap> taps;
-      for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b) taps.push_back(ConvTap{0, py - 1 + a, px - 1 + b});
       const size_t o = (size_t)q * cap * H * H * C;
       float* f = (planar ? x32[nxt] : t32) + o;
       const ActPair d = planar ? ActPair{xs[nxt].hi + o, xs[nxt].lo + o} : ActPair{nrm.hi + o, nrm.lo + o};
-      if (conv(convs.at(name + ".p" + std::to_string(q)), {{xs[cur], -1}}, taps, nullptr, H, n, false, nullptr, d.hi,
+      const ConvLayer& L = convs.at(name + ".p" + std::to_string(q));
+      if (conv(L, {{xs[cur], -1}}, L.taps(), nullptr, H, n, false, nullptr, d.hi,
                d.lo, f, st))
         return -1;
     }
