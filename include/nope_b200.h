@@ -618,6 +618,52 @@ int nope_ldm_run_block(nope_ldm_t* m, const char* name, const float* x0, int C0,
  * qkv [n_img, n_tok, 3C] fp32 (q | k | v) -> out [n_img, n_tok, C] fp32, on the wgmma attention kernel. */
 int nope_op_mh_attention(const float* qkv, float* out, int n_img, int n_tok, int C, void* stream);
 
+/* ---- Searches under occlusion (DESIGN.md section 27) ----
+ * Pixels that an occluder may hide are left out of every score.  A detection's occluders become a crop-space mask,
+ * each rolled copy of the crop a visible map over the 32 x 32 latent grid, and the score entry points below score a
+ * row over its visible latent pixels only.  Each map argument is required; the entry points without one are those
+ * above, whose results do not change.  All five refuse their bad arguments before any CUDA call and none
+ * synchronises.
+ *
+ * nope_crop_hidden: occluders [B, H, W] uint8 (non-zero = something may hide the object there), inv_maps [B, 9] fp64
+ * (nope_crop_frames' maps), device -> out [B, S, S] uint8.  Crop pixel (x, y) is 1 when one of the four taps of its
+ * nope_crop_frames sample has a non-zero fixed-point weight, lies inside the frame and has a non-zero occluder, else
+ * 0.  Requires B in [1, 65535], H and W in [1, 16384], S = 8 * 32 = 256. */
+int nope_crop_hidden(const uint8_t* occluders, int H, int W, const double* inv_maps, int B, int S, uint8_t* out,
+                     void* stream);
+/* nope_latent_visibility: hidden [B, S, S] uint8 crop-space masks, pairs image_idx [P] int32 and cossin [P, 2] fp32
+ * (the pairs of nope_inplane_rotate_pairs), device -> out [P, 32, 32] uint8.  Pixel (x, y) of pair p's rolled copy
+ * is hidden when one of the taps of its nope_inplane_rotate_pairs sample -- (ix, iy), (ix + 1, iy) if fx > 0,
+ * (ix, iy + 1) if fy > 0, (ix + 1, iy + 1) if both -- lies inside the image and is hidden.  Latent pixel (i, j) is 0
+ * when its 8 x 8 block holds a hidden pixel, else 1; at roll (1, 0) the map is the 8 x 8 block-max of hidden,
+ * inverted.  An image index outside [0, B) gives an all-visible row.  The in-plane table form is this call with tiled
+ * pairs.  Requires B >= 1, S = 256, P in [1, 2^30). */
+int nope_latent_visibility(const uint8_t* hidden, int B, int S, const int32_t* image_idx, const float* cossin, int P,
+                           uint8_t* out, void* stream);
+/* nope_unet_sweep_visible / nope_ldm_sweep_visible: the arguments of nope_unet_sweep_multi / nope_ldm_sweep_multi
+ * plus query_visible [B, Q, hw] uint8 (device; non-zero = visible), the visible map of every (reference, query) row;
+ * query_feat / query_latent is required.  Row r with n_r visible latent pixels of hw scores, over its visible pixels
+ * only (a hidden pixel's term is skipped, so a non-finite hidden query value cannot reach the score):
+ *   l2: -(a f), a the sum of sqrt(sum_c (q - t)^4), f = hw / n_r rounded to fp32 once (1 when all are visible);
+ *   cosine: the three flattened sums; cosine_occlusion: the thresholded per-pixel cosines summed, over n_r.
+ * A row with n_r = 0 scores NaN at every pose, which ranks in nope_topk's order.  With every pixel visible the
+ * results are bit-identical to nope_*_sweep_multi.  The LDM engine scores l2 only, as in nope_ldm_sweep_multi. */
+int nope_unet_sweep_visible(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
+                            const float* query_feat, int Q, const uint8_t* query_visible, float* out_emb,
+                            float* out_sim, int k, float* out_topv, int64_t* out_topi, int64_t idx_base,
+                            void* stream);
+int nope_ldm_sweep_visible(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
+                           const float* query_latent, int Q, const uint8_t* query_visible, float* out_emb,
+                           float* out_sim, int k, float* out_topv, int64_t* out_topi, int64_t idx_base,
+                           void* stream);
+/* nope_score_topk_visible: nope_score_topk_grouped with visible [R, HW] uint8 (device), the visible map of every
+ * query row, scored as in nope_unet_sweep_visible; with every pixel visible the results are bit-identical to
+ * nope_score_topk_grouped.  Also refuses R * HW > INT32_MAX. */
+int nope_score_topk_visible(const float* query_feat, const float* emb, int R, int O, int N, int C, int HW,
+                            const int32_t* slots, const int32_t* row_off, int G, int A, const uint8_t* visible,
+                            int metric, float occlusion_threshold, int k, float* out_sim, float* out_topv,
+                            int64_t* out_topi, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

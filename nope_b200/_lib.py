@@ -129,6 +129,17 @@ SIGNATURES = {
     "nope_op_mh_attention": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "nope_unet_debug_tap": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_char_p, c_f32p,
                                       C.c_int64, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
+    "nope_crop_hidden": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                   C.c_void_p]),
+    "nope_latent_visibility": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_int, C.c_void_p,
+                                         C.c_void_p]),
+    "nope_unet_sweep_visible": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, C.c_void_p,
+                                          c_f32p, c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
+    "nope_ldm_sweep_visible": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, C.c_void_p,
+                                         c_f32p, c_f32p, C.c_int, c_f32p, c_i64p, C.c_int64, C.c_void_p]),
+    "nope_score_topk_visible": (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                          C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_int,
+                                          c_f32p, c_f32p, c_i64p, C.c_void_p]),
 }
 
 # the lifecycle entries of the five weight-holding engines: kind -> nope_<kind>_create's arguments after the out handle

@@ -243,11 +243,17 @@ class RowPlan:
         return x if self.inverse is None else x.index_select(0, self.inverse)
 
 
-def score_rows(bank, query, plan, metric, threshold, k):
+def score_rows(bank, query, plan, metric, threshold, k, visible=None):
     """nope_score_topk_grouped on the current stream: query [D, A, C, 32, 32] in the plan's group order against the
-    bank -> (sim [D, A, N], top [D, k] at a * N + n | None for k = 0), in group order"""
+    bank -> (sim [D, A, N], top [D, k] at a * N + n | None for k = 0), in group order.  visible [D, A, 32, 32] (the
+    rows' visible maps, DESIGN.md section 27): nope_score_topk_visible, each row scored over its visible pixels."""
     D, A, N = plan.D, plan.A, bank.num_poses
     dev = bank.device
+    if visible is not None:
+        from .visibility import score_visible
+        sim, top = score_visible(query.reshape(D * A, *query.shape[2:]), bank.templates, plan.gslots, plan.row_off,
+                                 A, visible.reshape(D * A, *visible.shape[2:]), metric, threshold, k)
+        return sim.view(D, A, N), top
     q = query.to(dev, torch.float32).contiguous()
     t = bank.templates
     sim = torch.empty((D, A, N), device=dev, dtype=torch.float32)

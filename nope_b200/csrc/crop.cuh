@@ -31,6 +31,49 @@ __device__ __forceinline__ int crop_fixed(double v) {
   return __double2int_rn(v);
 }
 
+// The sample of crop pixel (x, y) through the destination -> source map M [9]: the tap origin (sx, sy) and the
+// fixed-point bilinear weights wt of taps (sx, sy), (sx+1, sy), (sx, sy+1), (sx+1, sy+1).  crop_warp_kernel and
+// crop_hidden_kernel both sample through it.
+__device__ __forceinline__ void crop_sample(const double* __restrict__ M, int x, int y, int& sx, int& sy, int wt[4]) {
+  const int xb = x & ~(kCropBlockW - 1), x1 = x - xb;
+  const double m0 = __ldg(M), m1 = __ldg(M + 1), m2 = __ldg(M + 2), m3 = __ldg(M + 3), m4 = __ldg(M + 4),
+               m5 = __ldg(M + 5), m6 = __ldg(M + 6), m7 = __ldg(M + 7), m8 = __ldg(M + 8);
+  const double dxb = (double)xb, dy = (double)y, dx1 = (double)x1;
+  // block origin (M0 xb + M1 y) + M2, then + M0 x1: OpenCV's association
+  const double X0 = __dadd_rn(__dadd_rn(__dmul_rn(m0, dxb), __dmul_rn(m1, dy)), m2);
+  const double Y0 = __dadd_rn(__dadd_rn(__dmul_rn(m3, dxb), __dmul_rn(m4, dy)), m5);
+  const double W0 = __dadd_rn(__dadd_rn(__dmul_rn(m6, dxb), __dmul_rn(m7, dy)), m8);
+  double w = __dadd_rn(W0, __dmul_rn(m6, dx1));
+  w = w != 0.0 ? __ddiv_rn(32.0, w) : 0.0;
+  const int X = crop_fixed(__dmul_rn(__dadd_rn(X0, __dmul_rn(m0, dx1)), w));
+  const int Y = crop_fixed(__dmul_rn(__dadd_rn(Y0, __dmul_rn(m3, dx1)), w));
+  const int fx = X & 31, fy = Y & 31;
+  sx = X >> 5;
+  sy = Y >> 5;
+
+  // float32 1-D weights (1 - i/32, i/32), their product times 32768 rounded, the sum brought to 32768 through the
+  // largest (short) or smallest (over) one
+  const float ax = __fmul_rn((float)fx, 0.03125f), ay = __fmul_rn((float)fy, 0.03125f);
+  const float bx = __fsub_rn(1.f, ax), by = __fsub_rn(1.f, ay);
+  wt[0] = __float2int_rn(__fmul_rn(__fmul_rn(by, bx), 32768.f));
+  wt[1] = __float2int_rn(__fmul_rn(__fmul_rn(by, ax), 32768.f));
+  wt[2] = __float2int_rn(__fmul_rn(__fmul_rn(ay, bx), 32768.f));
+  wt[3] = __float2int_rn(__fmul_rn(__fmul_rn(ay, ax), 32768.f));
+  const int diff = wt[0] + wt[1] + wt[2] + wt[3] - 32768;
+  if (diff != 0) {
+    int hi = 0, lo = 0, whi = wt[0], wlo = wt[0];      // first largest / smallest, no indexed register array
+#pragma unroll
+    for (int k = 1; k < 4; ++k) {
+      if (wt[k] > whi) hi = k, whi = wt[k];
+      if (wt[k] < wlo) lo = k, wlo = wt[k];
+    }
+    const int at = diff < 0 ? hi : lo;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k == at) wt[k] -= diff;
+  }
+}
+
 template <int C>
 __global__ void __launch_bounds__(kCropThreads) crop_warp_kernel(
     const uint8_t* __restrict__ frames, int F, int H, int W, const uint8_t* __restrict__ masks,
@@ -48,42 +91,8 @@ __global__ void __launch_bounds__(kCropThreads) crop_warp_kernel(
     return;
   }
   const int y = p / S, x = p - y * S;
-  const int xb = x & ~(kCropBlockW - 1), x1 = x - xb;
-  const double* M = inv_maps + 9 * (size_t)b;
-  const double m0 = __ldg(M), m1 = __ldg(M + 1), m2 = __ldg(M + 2), m3 = __ldg(M + 3), m4 = __ldg(M + 4),
-               m5 = __ldg(M + 5), m6 = __ldg(M + 6), m7 = __ldg(M + 7), m8 = __ldg(M + 8);
-  const double dxb = (double)xb, dy = (double)y, dx1 = (double)x1;
-  // block origin (M0 xb + M1 y) + M2, then + M0 x1: OpenCV's association
-  const double X0 = __dadd_rn(__dadd_rn(__dmul_rn(m0, dxb), __dmul_rn(m1, dy)), m2);
-  const double Y0 = __dadd_rn(__dadd_rn(__dmul_rn(m3, dxb), __dmul_rn(m4, dy)), m5);
-  const double W0 = __dadd_rn(__dadd_rn(__dmul_rn(m6, dxb), __dmul_rn(m7, dy)), m8);
-  double w = __dadd_rn(W0, __dmul_rn(m6, dx1));
-  w = w != 0.0 ? __ddiv_rn(32.0, w) : 0.0;
-  const int X = crop_fixed(__dmul_rn(__dadd_rn(X0, __dmul_rn(m0, dx1)), w));
-  const int Y = crop_fixed(__dmul_rn(__dadd_rn(Y0, __dmul_rn(m3, dx1)), w));
-  const int sx = X >> 5, sy = Y >> 5, fx = X & 31, fy = Y & 31;
-
-  // bilinear weights of taps (sx, sy), (sx+1, sy), (sx, sy+1), (sx+1, sy+1): float32 1-D weights (1 - i/32, i/32),
-  // their product times 32768 rounded, the sum brought to 32768 through the largest (short) or smallest (over) one
-  const float ax = __fmul_rn((float)fx, 0.03125f), ay = __fmul_rn((float)fy, 0.03125f);
-  const float bx = __fsub_rn(1.f, ax), by = __fsub_rn(1.f, ay);
-  int wt[4] = {__float2int_rn(__fmul_rn(__fmul_rn(by, bx), 32768.f)),
-               __float2int_rn(__fmul_rn(__fmul_rn(by, ax), 32768.f)),
-               __float2int_rn(__fmul_rn(__fmul_rn(ay, bx), 32768.f)),
-               __float2int_rn(__fmul_rn(__fmul_rn(ay, ax), 32768.f))};
-  const int diff = wt[0] + wt[1] + wt[2] + wt[3] - 32768;
-  if (diff != 0) {
-    int hi = 0, lo = 0, whi = wt[0], wlo = wt[0];      // first largest / smallest, no indexed register array
-#pragma unroll
-    for (int k = 1; k < 4; ++k) {
-      if (wt[k] > whi) hi = k, whi = wt[k];
-      if (wt[k] < wlo) lo = k, wlo = wt[k];
-    }
-    const int at = diff < 0 ? hi : lo;
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      if (k == at) wt[k] -= diff;
-  }
+  int sx, sy, wt[4];
+  crop_sample(inv_maps + 9 * (size_t)b, x, y, sx, sy, wt);
 
   int acc0 = 0, acc1 = 0, acc2 = 0;
   const uint8_t* fr = frames + (size_t)f * H * W * C;
@@ -106,6 +115,29 @@ __global__ void __launch_bounds__(kCropThreads) crop_warp_kernel(
     // ToTensor (u / 255) then x * 2 - 1, each operation rounded on its own
     o[(size_t)c * SS] = __fsub_rn(__fmul_rn(__fdiv_rn((float)u, 255.f), 2.f), 1.f);
   }
+}
+
+// The crop-space hidden mask (DESIGN.md section 27): crop pixel (x, y) of detection b is 1 when a tap of its
+// crop_warp_kernel sample has a non-zero weight, lies inside the frame and is non-zero in occluders [B, H, W];
+// otherwise 0.  out [B, S, S]; one thread per crop pixel, grid (ceil(S * S / 256), B).
+__global__ void __launch_bounds__(kCropThreads) crop_hidden_kernel(
+    const uint8_t* __restrict__ occluders, int H, int W, const double* __restrict__ inv_maps, int S,
+    uint8_t* __restrict__ out) {
+  const int b = blockIdx.y;
+  const int p = blockIdx.x * kCropThreads + threadIdx.x;
+  const int SS = S * S;
+  if (p >= SS) return;
+  const int y = p / S, x = p - y * S;
+  int sx, sy, wt[4];
+  crop_sample(inv_maps + 9 * (size_t)b, x, y, sx, sy, wt);
+  const uint8_t* ob = occluders + (size_t)b * H * W;
+  bool hidden = false;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int tx = sx + (k & 1), ty = sy + (k >> 1);
+    if (wt[k] != 0 && tx >= 0 && tx < W && ty >= 0 && ty < H) hidden |= __ldg(ob + (size_t)ty * W + tx) != 0;
+  }
+  out[(size_t)b * SS + p] = hidden ? 1 : 0;
 }
 
 // ---------------------------------------------------------------------------------

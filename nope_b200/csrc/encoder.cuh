@@ -73,17 +73,28 @@ enc_stem_kernel(const float* __restrict__ x, const float* __restrict__ w, const 
 // quarter turns of a square image the fractions are 0 and the copy is an exact permutation.
 // The per-pixel body shared by both rotation kernels: pixel i = y * W + x of the copy of image src [3, H, W] rotated
 // by (c, s), written to dst[0], dst[hw], dst[2 hw].
-__device__ __forceinline__ void inplane_rotate_pixel(const float* __restrict__ src, float c, float s, int H, int W,
-                                                     int i, float* __restrict__ dst) {
-  const long long hw = (long long)H * W;
-  const int x = i % W, y = i / W;
+// The sample of pixel (x, y) of the copy rotated by (c, s): top-left tap (ix, iy) and fractions (fx, fy).
+// inplane_rotate_pixel and latent_visibility_kernel both sample through it.
+__device__ __forceinline__ void inplane_sample(float c, float s, int H, int W, int x, int y, int& ix, int& iy,
+                                               float& fx, float& fy) {
   const float cx = __fmul_rn((float)(W - 1), 0.5f), cy = __fmul_rn((float)(H - 1), 0.5f);
   const float dx = __fsub_rn((float)x, cx), dy = __fsub_rn((float)y, cy);
   const float sx = __fadd_rn(__fsub_rn(__fmul_rn(c, dx), __fmul_rn(s, dy)), cx);
   const float sy = __fadd_rn(__fadd_rn(__fmul_rn(s, dx), __fmul_rn(c, dy)), cy);
   const float x0 = floorf(sx), y0 = floorf(sy);
-  const float fx = __fsub_rn(sx, x0), fy = __fsub_rn(sy, y0);
-  const int ix = (int)x0, iy = (int)y0;
+  fx = __fsub_rn(sx, x0);
+  fy = __fsub_rn(sy, y0);
+  ix = (int)x0;
+  iy = (int)y0;
+}
+
+__device__ __forceinline__ void inplane_rotate_pixel(const float* __restrict__ src, float c, float s, int H, int W,
+                                                     int i, float* __restrict__ dst) {
+  const long long hw = (long long)H * W;
+  const int x = i % W, y = i / W;
+  int ix, iy;
+  float fx, fy;
+  inplane_sample(c, s, H, W, x, y, ix, iy, fx, fy);
   const bool in_x0 = ix >= 0 && ix < W, in_x1 = ix + 1 >= 0 && ix + 1 < W;
   const bool in_y0 = iy >= 0 && iy < H, in_y1 = iy + 1 >= 0 && iy + 1 < H;
 #pragma unroll
@@ -132,6 +143,46 @@ inplane_rotate_pairs_kernel(const float* __restrict__ img, int B, const int* __r
     return;
   }
   inplane_rotate_pixel(img + (long long)b * 3 * hw, cossin[2 * p], cossin[2 * p + 1], H, W, i, dst);
+}
+
+// Latent visibility of rolled copies (DESIGN.md section 27).  Pair p rolls crop-space mask image_idx[p] of hidden
+// [B, S, S] (uint8, non-zero = may be hidden) by (cossin[2p], cossin[2p + 1]) with inplane_rotate_pixel's sample:
+// pixel (x, y) of the copy is hidden when one of its taps (ix, iy), (ix + 1, iy) if fx > 0, (ix, iy + 1) if fy > 0,
+// (ix + 1, iy + 1) if both, lies inside the image and is hidden.  Latent pixel (i, j) of out [P, 32, 32] is 0 when
+// its 8 x 8 block holds a hidden pixel, otherwise 1.  An image index outside [0, B) gives an all-visible row.  One
+// CTA of 1024 threads per pair, thread (i, j) samples its block's 64 pixels (stopping at the first hidden one).
+// S = 8 * 32.
+constexpr int kVisSide = 32;                 // latent side of every visible map
+constexpr int kVisThreads = kVisSide * kVisSide;
+
+__global__ void __launch_bounds__(kVisThreads)
+latent_visibility_kernel(const uint8_t* __restrict__ hidden, int B, int S, const int* __restrict__ image_idx,
+                         const float* __restrict__ cossin, uint8_t* __restrict__ out) {
+  const int p = blockIdx.x, t = threadIdx.x;
+  const int li = t / kVisSide, lj = t - li * kVisSide;
+  const int b = image_idx[p];
+  uint8_t* o = out + (size_t)p * kVisThreads;
+  if (b < 0 || b >= B) {
+    o[t] = 1;
+    return;
+  }
+  const float c = cossin[2 * p], s = cossin[2 * p + 1];
+  const uint8_t* hb = hidden + (size_t)b * S * S;
+  const int blk = S / kVisSide;
+  bool any = false;
+  for (int dy = 0; dy < blk && !any; ++dy)
+    for (int dx = 0; dx < blk; ++dx) {
+      int ix, iy;
+      float fx, fy;
+      inplane_sample(c, s, S, S, lj * blk + dx, li * blk + dy, ix, iy, fx, fy);
+      const bool x0 = ix >= 0 && ix < S, y0 = iy >= 0 && iy < S;
+      const bool x1 = fx > 0.f && ix + 1 >= 0 && ix + 1 < S, y1 = fy > 0.f && iy + 1 >= 0 && iy + 1 < S;
+      const int r0 = iy * S + ix;          // read only where the tap lies inside the image
+      any |= (y0 && x0 && __ldg(hb + r0)) || (y0 && x1 && __ldg(hb + r0 + 1)) ||
+             (y1 && x0 && __ldg(hb + r0 + S)) || (y1 && x1 && __ldg(hb + r0 + S + 1));
+      if (any) break;
+    }
+  o[t] = any ? 0 : 1;
 }
 
 // [n_pix][ld] fp32 (first D columns valid) -> NCHW fp32 [B, D, hw]

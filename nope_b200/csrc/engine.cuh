@@ -14,8 +14,9 @@
 //   int ensure_workspace(int hyps, int refs, int scores, cudaStream_t)  sizes the workspace (grow_workspace), score
 //       partials and similarity scratch of `scores` (reference, query, pose) triples included, before a launch;
 //   int prestage(const float* ref, int B, cudaStream_t)                  the pose-independent prefix per reference;
-//   int forward_chunk(poses, hyp0, n, N, query, out_emb, score_part, cudaStream_t, int Q);
-//   int rank(part, sim, B, N, Q, k, topv, topi, idx_base, cudaStream_t) the similarities and top-k from the partials.
+//   int forward_chunk(poses, hyp0, n, N, query, out_emb, score_part, cudaStream_t, int Q, const uint8_t* vis);
+//   int rank(part, sim, B, N, Q, k, topv, topi, idx_base, cudaStream_t, vis) the similarities and top-k from the
+//       partials; vis (nullable) [B, Q, hw] the rows' visible maps (DESIGN.md section 27).
 // An image engine derives from ImageEngine (encoder.cuh), which holds `launches`, `mem` and the convolution
 // layers, and provides `kChunk` and `std::vector<ImageModule> plan`, built in forward order when the handle is
 // created; its schema, weight packing, forward pass and run_block all walk that plan.  An image encoder
@@ -331,10 +332,12 @@ struct LaunchProfile {
 
 // nope_unet_sweep_multi / nope_ldm_sweep_multi: the B references' N poses in chunks of the engine's `chunk`
 // hypotheses, each scored against its reference's Q queries, then ranked.  A sweep of a shape the engine has served
-// before makes no allocation and no host synchronisation.
+// before makes no allocation and no host synchronisation.  With vis (the *_sweep_visible entry points) each row
+// scores only its visible latent pixels.
 template <typename E>
 int engine_sweep(E* e, const float* ref, const float* poses, int B, int N, const float* query, int Q, float* out_emb,
-                 float* out_sim, int k, float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream) {
+                 float* out_sim, int k, float* out_topv, int64_t* out_topi, int64_t idx_base, void* stream,
+                 const uint8_t* vis = nullptr) {
   if (check_sweep(e, ref, poses, B, N, query, Q, out_sim, k, out_topv, out_topi)) return -1;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   NOPE_CUDA(cudaSetDevice(e->device));
@@ -346,10 +349,10 @@ int engine_sweep(E* e, const float* ref, const float* poses, int B, int N, const
   if (e->prestage(ref, B, st)) return -1;
   for (int h0 = 0; h0 < total; h0 += cap) {
     const int n = std::min(cap, total - h0);
-    if (e->forward_chunk(poses, h0, n, N, query, out_emb, part, st, Q)) return -1;
+    if (e->forward_chunk(poses, h0, n, N, query, out_emb, part, st, Q, vis)) return -1;
   }
   if (query && (out_sim || k > 0)) {
-    if (e->rank(part, out_sim ? out_sim : e->sim_buf, B, N, Q, k, out_topv, out_topi, idx_base, st)) return -1;
+    if (e->rank(part, out_sim ? out_sim : e->sim_buf, B, N, Q, k, out_topv, out_topi, idx_base, st, vis)) return -1;
     ++e->launches;
   }
   return 0;

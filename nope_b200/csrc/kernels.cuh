@@ -477,7 +477,8 @@ __global__ void upsample2x_kernel(const __half* __restrict__ x, __half* __restri
 // (model.py:260-262):  score[h] = -sum_p sqrt( sum_c (q[c,p] - e[c,p])^4 ).
 // x: [n_hyp, hw, C] fp16; w fp32 [Cl, C]; emb (optional) fp32 [n_hyp, Cl, hw] (NCHW);
 // query fp32 [B, Q, Cl, hw] (Q queries per reference; needed when partial is set);
-// partial (optional) [n_hyp, Q, nslab, kScoreParts] sums.
+// partial (optional) [n_hyp, Q, nslab, kScoreParts] sums.  With kVis the sums skip the pixels that the visible map
+// vis [B, Q, hw] of the (reference, query) row marks 0 (DESIGN.md section 27).
 // kFinalPPT pixels per thread, kFinalPix pixels per CTA.
 // ----------------------------------------------------------------------------
 constexpr int kFinalThreads = 128;
@@ -486,13 +487,14 @@ constexpr int kFinalPix = kFinalThreads * kFinalPPT;       // pixels per CTA (sl
 constexpr int kMaxLatent = 8;
 constexpr int kScoreParts = 3;     // partial sums per (hypothesis, pixel slab): metric-dependent
 
+template <bool kVis>
 __global__ void __launch_bounds__(kFinalThreads)
 final_conv_score_kernel(const __half* __restrict__ x, const float* __restrict__ w,
                         const float* __restrict__ bias, float* __restrict__ emb,
                         const float* __restrict__ query, const int* __restrict__ ref_of,
                         float* __restrict__ partial, int hw, int C, int Cl,
-                        const __half* __restrict__ x_lo = nullptr, int metric = 0, float occ_thr = 0.f,
-                        bool bf = false, int Q = 1) {
+                        const __half* __restrict__ x_lo, int metric, float occ_thr,
+                        bool bf, int Q, const uint8_t* __restrict__ vis) {
   pdl_sync();
   // weights transposed to [C][kMaxLatent] (zero beyond Cl): the 8 outputs of one input channel are two aligned 16-byte
   // broadcast loads, and every loaded weight serves the kFinalPPT pixels of the thread.  (With a [Cl][C] table and one
@@ -573,6 +575,7 @@ final_conv_score_kernel(const __half* __restrict__ x, const float* __restrict__ 
     for (int u = 0; u < kFinalPPT; ++u) {
       const int p = pix[u];
       if (p >= hw) continue;
+      if (kVis && !vis[(qrow0 + qi) * hw + p]) continue;
       const float* qp = query + (qrow0 + qi) * Cl * hw + p;     // coalesced: consecutive threads, consecutive pixels
       float s4 = 0.f, qe = 0.f, qq = 0.f, ee = 0.f;
 #pragma unroll

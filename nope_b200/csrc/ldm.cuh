@@ -663,9 +663,9 @@ struct nope_ldm {
   }
 
   // UNetModelPose.forward for hypotheses [hyp0, hyp0 + n) of the flattened (b, pose) list
-  // query [B, Q, Cl, hw]; score_part [B * N, Q, nslab]
+  // query [B, Q, Cl, hw]; score_part [B * N, Q, nslab]; vis (optional) [B, Q, hw] visible maps
   int forward_chunk(const float* poses, int hyp0, int n, int N, const float* query, float* out_emb,
-                    float* score_part, cudaStream_t st, int Q = 1) {
+                    float* score_part, cudaStream_t st, int Q = 1, const uint8_t* vis = nullptr) {
     using namespace nope;
     ref_of_kernel<<<(n + 255) / 256, 256, 0, st>>>(ref_of, hyp0, N, n);
     ++launches;
@@ -735,9 +735,9 @@ struct nope_ldm {
     const int hw = S * S;
     const int nslab = (hw + kFinalThreads - 1) / kFinalThreads;
     if (conv(convs.at("out.2"), T1, T2, S, n, st, nullptr, nullptr, 0, nullptr, 0, OF)) return -1;
-    ldm_score_kernel<<<dim3(nslab, n), kFinalThreads, 0, st>>>(
+    (vis ? ldm_score_kernel<true> : ldm_score_kernel<false>)<<<dim3(nslab, n), kFinalThreads, 0, st>>>(
         OF, out_emb ? out_emb + (size_t)hyp0 * Cl * hw : nullptr, query, ref_of,
-        score_part ? score_part + (size_t)hyp0 * Q * nslab : nullptr, hw, Cl, Q);
+        score_part ? score_part + (size_t)hyp0 * Q * nslab : nullptr, hw, Cl, Q, vis);
     NOPE_CUDA(cudaGetLastError());
     ++launches;
     return 0;
@@ -747,9 +747,14 @@ struct nope_ldm {
   int nslab() const { return (S0 * S0 + nope::kFinalThreads - 1) / nope::kFinalThreads; }
   // similarities (sim [B * Q, N]) and top-k of every (reference, query) row from the score partials
   int rank(const float* part, float* sim, int B, int N, int Q, int k, float* topv, int64_t* topi, int64_t idx_base,
-           cudaStream_t st) {
-    nope::sim_topk_kernel<<<B * Q, 256, 0, st>>>(part, nslab(), sim, N, k, topv, reinterpret_cast<long long*>(topi),
-                                                 (long long)idx_base, 1, 0, 1, Q);
+           cudaStream_t st, const uint8_t* vis = nullptr) {
+    if (vis)
+      nope::sim_topk_kernel<true><<<B * Q, 256, 0, st>>>(part, nslab(), sim, N, k, topv,
+                                                         reinterpret_cast<long long*>(topi), (long long)idx_base, 1, 0,
+                                                         S0 * S0, Q, vis);
+    else
+      nope::sim_topk_kernel<<<B * Q, 256, 0, st>>>(part, nslab(), sim, N, k, topv, reinterpret_cast<long long*>(topi),
+                                                   (long long)idx_base, 1, 0, 1, Q);
     NOPE_CUDA(cudaGetLastError());
     return 0;
   }

@@ -109,6 +109,38 @@ int stage_host_intrinsics(ScratchArena& arena, const double** dev, const double*
   arena.add(dev, 4 * (size_t)F, K);
   return 0;
 }
+
+// nope_score_topk_grouped and, with a visible map [R, HW], nope_score_topk_visible: the argument checks, one CTA per
+// (template n, group g) scoring slot slots[g]'s template n against the group's rows, then with k > 0 the joint top-k
+// over (row a, template n) of every A consecutive rows (sim viewed as [R / A, A * N]).
+int score_grouped(const float* query_feat, const float* emb, int R, int O, int N, int C, int HW, const int32_t* slots,
+                  const int32_t* row_off, int G, int A, const uint8_t* visible, int metric, float occlusion_threshold,
+                  int k, float* out_sim, float* out_topv, int64_t* out_topi, void* stream) {
+  NOPE_CHECK(query_feat && emb && slots && row_off && out_sim, "null argument");
+  NOPE_CHECK(R >= 1 && O >= 1 && N >= 1 && C >= 1 && HW >= 1, "bad arguments");
+  NOPE_CHECK(G >= 1 && G <= 65535, "G (row groups) must be in [1, 65535]");
+  NOPE_CHECK(A >= 1 && R % A == 0, "R (query rows) must be a multiple of A (rows per search row) >= 1");
+  NOPE_CHECK(O <= 65535 && (int64_t)R * N <= INT32_MAX, "too many templates or (query, template) pairs");
+  NOPE_CHECK(!visible || (int64_t)R * HW <= INT32_MAX, "R * HW (visible map entries) exceeds 2^31 - 1");
+  NOPE_CHECK(metric == NOPE_METRIC_L2 || metric == NOPE_METRIC_COSINE || metric == NOPE_METRIC_COSINE_OCC,
+             "unknown similarity metric (l2, cosine and cosine_occlusion exist)");
+  NOPE_CHECK(k >= 0 && k <= kMaxTopK && (int64_t)k <= (int64_t)A * N, "k must be in [0, min(64, A * N)]");
+  NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (visible)
+    score_kernel<true><<<dim3(N, G), 256, 0, st>>>(query_feat, emb, out_sim, N, C, HW, metric, occlusion_threshold, 0,
+                                                   slots, row_off, visible);
+  else
+    score_kernel<<<dim3(N, G), 256, 0, st>>>(query_feat, emb, out_sim, N, C, HW, metric, occlusion_threshold, 0,
+                                             slots, row_off);
+  NOPE_CUDA(cudaGetLastError());
+  if (k > 0) {
+    sim_topk_kernel<<<R / A, 256, 0, st>>>(nullptr, 0, out_sim, A * N, k, out_topv,
+                                           reinterpret_cast<long long*>(out_topi), 0LL);
+    NOPE_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
 }  // namespace
 
 // =============================================================================
@@ -265,27 +297,8 @@ int nope_score_topk_grouped(const float* query_feat, const float* emb, int R, in
                             const int32_t* slots, const int32_t* row_off, int G, int A, int metric,
                             float occlusion_threshold, int k, float* out_sim, float* out_topv, int64_t* out_topi,
                             void* stream) {
-  NOPE_CHECK(query_feat && emb && slots && row_off && out_sim, "null argument");
-  NOPE_CHECK(R >= 1 && O >= 1 && N >= 1 && C >= 1 && HW >= 1, "bad arguments");
-  NOPE_CHECK(G >= 1 && G <= 65535, "G (row groups) must be in [1, 65535]");
-  NOPE_CHECK(A >= 1 && R % A == 0, "R (query rows) must be a multiple of A (rows per search row) >= 1");
-  NOPE_CHECK(O <= 65535 && (int64_t)R * N <= INT32_MAX, "too many templates or (query, template) pairs");
-  NOPE_CHECK(metric == NOPE_METRIC_L2 || metric == NOPE_METRIC_COSINE || metric == NOPE_METRIC_COSINE_OCC,
-             "unknown similarity metric (l2, cosine and cosine_occlusion exist)");
-  NOPE_CHECK(k >= 0 && k <= kMaxTopK && (int64_t)k <= (int64_t)A * N, "k must be in [0, min(64, A * N)]");
-  NOPE_CHECK(k == 0 || (out_topv && out_topi), "top-k outputs missing");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // one CTA per (template n, group g): slot slots[g]'s template n against the group's rows
-  score_kernel<<<dim3(N, G), 256, 0, st>>>(query_feat, emb, out_sim, N, C, HW, metric, occlusion_threshold, 0,
-                                           slots, row_off);
-  NOPE_CUDA(cudaGetLastError());
-  if (k > 0) {
-    // the joint top-k over (row a, template n) of every A consecutive rows: sim viewed as [R / A, A * N]
-    sim_topk_kernel<<<R / A, 256, 0, st>>>(nullptr, 0, out_sim, A * N, k, out_topv,
-                                           reinterpret_cast<long long*>(out_topi), 0LL);
-    NOPE_CUDA(cudaGetLastError());
-  }
-  return 0;
+  return score_grouped(query_feat, emb, R, O, N, C, HW, slots, row_off, G, A, nullptr, metric, occlusion_threshold, k,
+                       out_sim, out_topv, out_topi, stream);
 }
 
 int nope_topk(float* sim, int B, int N, int k, float* out_topv, int64_t* out_topi, int64_t idx_base,
@@ -1428,6 +1441,60 @@ int nope_op_mh_attention(const float* qkv, float* out, int n_img, int n_tok, int
   NOPE_CUDA(cudaGetLastError());
   NOPE_CUDA(cudaStreamSynchronize(st));
   return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// searches under occlusion: visible latent maps and the scores over them (DESIGN.md section 27)
+// ---------------------------------------------------------------------------------
+int nope_crop_hidden(const uint8_t* occluders, int H, int W, const double* inv_maps, int B, int S, uint8_t* out,
+                     void* stream) {
+  NOPE_CHECK(occluders && inv_maps && out, "null argument");
+  NOPE_CHECK(B >= 1 && B <= 65535, "B must be in [1, 65535]");
+  NOPE_CHECK(H >= 1 && H <= kCropMaxSide && W >= 1 && W <= kCropMaxSide, "H and W must be in [1, 16384]");
+  NOPE_CHECK(S >= 8 && S % 8 == 0 && S / 8 == kVisSide, "S must be 8 * 32 = 256 (the latent grid is 32 x 32)");
+  crop_hidden_kernel<<<dim3((S * S + kCropThreads - 1) / kCropThreads, B), kCropThreads, 0,
+                       static_cast<cudaStream_t>(stream)>>>(occluders, H, W, inv_maps, S, out);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int nope_latent_visibility(const uint8_t* hidden, int B, int S, const int32_t* image_idx, const float* cossin, int P,
+                           uint8_t* out, void* stream) {
+  NOPE_CHECK(hidden && image_idx && cossin && out, "null argument");
+  NOPE_CHECK(B >= 1, "B must be >= 1");
+  NOPE_CHECK(S >= 8 && S % 8 == 0 && S / 8 == kVisSide, "S must be 8 * 32 = 256 (the latent grid is 32 x 32)");
+  NOPE_CHECK(P >= 1 && P <= INT32_MAX / 2, "P (pairs) must be in [1, 2^30)");
+  latent_visibility_kernel<<<P, kVisThreads, 0, static_cast<cudaStream_t>(stream)>>>(hidden, B, S, image_idx, cossin,
+                                                                                     out);
+  NOPE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int nope_unet_sweep_visible(nope_unet_t* u, const float* ref_feat, const float* poses, int B, int N,
+                            const float* query_feat, int Q, const uint8_t* query_visible, float* out_emb,
+                            float* out_sim, int k, float* out_topv, int64_t* out_topi, int64_t idx_base,
+                            void* stream) {
+  NOPE_CHECK(query_feat && query_visible, "null query or visible map");
+  return engine_sweep(u, ref_feat, poses, B, N, query_feat, Q, out_emb, out_sim, k, out_topv, out_topi, idx_base,
+                      stream, query_visible);
+}
+
+int nope_ldm_sweep_visible(nope_ldm_t* m, const float* ref_latent, const float* poses, int B, int N,
+                           const float* query_latent, int Q, const uint8_t* query_visible, float* out_emb,
+                           float* out_sim, int k, float* out_topv, int64_t* out_topi, int64_t idx_base,
+                           void* stream) {
+  NOPE_CHECK(query_latent && query_visible, "null query or visible map");
+  return engine_sweep(m, ref_latent, poses, B, N, query_latent, Q, out_emb, out_sim, k, out_topv, out_topi, idx_base,
+                      stream, query_visible);
+}
+
+int nope_score_topk_visible(const float* query_feat, const float* emb, int R, int O, int N, int C, int HW,
+                            const int32_t* slots, const int32_t* row_off, int G, int A, const uint8_t* visible,
+                            int metric, float occlusion_threshold, int k, float* out_sim, float* out_topv,
+                            int64_t* out_topi, void* stream) {
+  NOPE_CHECK(visible, "null visible map");
+  return score_grouped(query_feat, emb, R, O, N, C, HW, slots, row_off, G, A, visible, metric, occlusion_threshold, k,
+                       out_sim, out_topv, out_topi, stream);
 }
 
 }  // extern "C"

@@ -23,6 +23,16 @@ __device__ __forceinline__ float finish_score(int metric, float a, float b, floa
   return a / (float)hw;
 }
 
+// finish_score over the n visible pixels of hw (DESIGN.md section 27): "l2" -(a f) with f = hw / n rounded once
+// (f = 1 with every pixel visible), cosine from its sums over the visible pixels, the occlusion-aware cosine a / n;
+// NaN when no pixel is visible.
+__device__ __forceinline__ float finish_visible(int metric, float a, float b, float c, int n, int hw) {
+  if (n == 0) return __int_as_float(0x7fc00000);
+  if (metric == 0) return -(a * __fdiv_rn((float)hw, (float)n));
+  if (metric == 1) return finish_score(1, a, b, c, hw);
+  return a / (float)n;
+}
+
 // Standalone score of materialised embeddings (PoseConditional.retrieval, model.py:254-266):
 // emb fp32 [Bt, N, Cl, hw], query rows fp32 [Bt * rows, Cl, hw] -> sim [Bt * rows, N]: query row r is scored
 // against the templates of batch r / rows (the reference's broadcasting of query_feat against template_feat).
@@ -32,11 +42,15 @@ __device__ __forceinline__ float finish_score(int metric, float a, float b, floa
 // Grouped form (a template bank, DESIGN.md section 25): with slots [G] and row_off [G + 1] (device, both non-null),
 // blockIdx.y is a group g that reads template batch slots[g] and scores query rows [row_off[g], row_off[g + 1]);
 // `rows` is then unused.  With null pointers group b is template batch b and rows [b * rows, (b + 1) * rows).
+// With kVis, query row r scores only the pixels its visible map vis [rows, hw] marks non-zero (finish_visible).
+template <bool kVis = false>
 __global__ void __launch_bounds__(256)
 score_kernel(const float* __restrict__ query, const float* __restrict__ emb,
              float* __restrict__ sim, int N, int Cl, int hw, int metric, float occ_thr, int rows = 1,
-             const int* __restrict__ slots = nullptr, const int* __restrict__ row_off = nullptr) {
+             const int* __restrict__ slots = nullptr, const int* __restrict__ row_off = nullptr,
+             const uint8_t* __restrict__ vis = nullptr) {
   __shared__ float s_a[2][8], s_b[2][8], s_c[2][8];     // double-buffered across rows
+  __shared__ int s_n[2][8];
   const int n = blockIdx.x, b = blockIdx.y;
   const long long tb = slots ? slots[b] : b;
   const long long r0 = row_off ? row_off[b] : (long long)b * rows;
@@ -46,7 +60,12 @@ score_kernel(const float* __restrict__ query, const float* __restrict__ emb,
     const long long r = r0 + j;
     const float* q = query + r * Cl * hw;
     float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+    int nv = 0;
     for (int p = threadIdx.x; p < hw; p += blockDim.x) {
+      if (kVis) {
+        if (!vis[r * hw + p]) continue;
+        ++nv;
+      }
       if (metric == 0) {
         float s4 = 0.f;
         for (int c = 0; c < Cl; ++c) {
@@ -79,18 +98,24 @@ score_kernel(const float* __restrict__ query, const float* __restrict__ emb,
       a0 += __shfl_xor_sync(0xffffffffu, a0, o);
       a1 += __shfl_xor_sync(0xffffffffu, a1, o);
       a2 += __shfl_xor_sync(0xffffffffu, a2, o);
+      if (kVis) nv += __shfl_xor_sync(0xffffffffu, nv, o);
     }
     const int buf = j & 1;
     if ((threadIdx.x & 31) == 0) {
       s_a[buf][threadIdx.x >> 5] = a0;
       s_b[buf][threadIdx.x >> 5] = a1;
       s_c[buf][threadIdx.x >> 5] = a2;
+      if (kVis) s_n[buf][threadIdx.x >> 5] = nv;
     }
     __syncthreads();
     if (threadIdx.x == 0) {
       float t0 = 0.f, t1 = 0.f, t2 = 0.f;
-      for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { t0 += s_a[buf][i]; t1 += s_b[buf][i]; t2 += s_c[buf][i]; }
-      sim[r * N + n] = finish_score(metric, t0, t1, t2, hw);
+      int tn = 0;
+      for (int i = 0; i < (int)(blockDim.x >> 5); ++i) {
+        t0 += s_a[buf][i]; t1 += s_b[buf][i]; t2 += s_c[buf][i];
+        if (kVis) tn += s_n[buf][i];
+      }
+      sim[r * N + n] = kVis ? finish_visible(metric, t0, t1, t2, tn, hw) : finish_score(metric, t0, t1, t2, hw);
     }
   }
 }
@@ -210,24 +235,38 @@ struct ChosenListSel : TopkOut {
 // sim = -(sum of slab partials) and top-k (model.py:265 topk(k=5)); descending score,
 // ties -> lowest index, NaN last (ranks_before).  One CTA per row (b, q) of sim [B, Q, N]; partial is
 // [B, N, Q, nslab, nparts].
-// idx_base is added to the indices so a shard reports global pose indices.
+// idx_base is added to the indices so a shard reports global pose indices.  With kVis the partials cover only the
+// pixels the row's visible map vis [B * Q, hw] marks non-zero, and the row is finished over their count
+// (finish_visible).
 // ----------------------------------------------------------------------------
+template <bool kVis = false>
 __global__ void __launch_bounds__(256)
 sim_topk_kernel(const float* __restrict__ partial, int nslab, float* __restrict__ sim, int N,
                 int k, float* __restrict__ top_val, long long* __restrict__ top_idx,
-                long long idx_base, int nparts = 1, int metric = 0, int hw = 1, int Q = 1) {
+                long long idx_base, int nparts = 1, int metric = 0, int hw = 1, int Q = 1,
+                const uint8_t* __restrict__ vis = nullptr) {
   pdl_sync();
   __shared__ SelectSmem<256> sm;
+  __shared__ int s_nv;
   const int b = blockIdx.x;              // row b * Q + q
   float* srow = sim + (long long)b * N;
   if (partial) {
     const int bb = b / Q, qi = b - bb * Q;
+    int nv = 0;
+    if (kVis) {                          // the row's visible pixels: an integer sum, so any order gives the same count
+      if (threadIdx.x == 0) s_nv = 0;
+      __syncthreads();
+      for (int p = threadIdx.x; p < hw; p += blockDim.x) nv += vis[(long long)b * hw + p] != 0;
+      atomicAdd(&s_nv, nv);
+      __syncthreads();
+      nv = s_nv;
+    }
     for (int n = threadIdx.x; n < N; n += blockDim.x) {
       float t[3] = {0.f, 0.f, 0.f};
       const float* pp = partial + (((long long)bb * N + n) * Q + qi) * nslab * nparts;
       for (int s = 0; s < nslab; ++s)
         for (int q = 0; q < nparts; ++q) t[q] += pp[s * nparts + q];
-      srow[n] = finish_score(metric, t[0], t[1], t[2], hw);
+      srow[n] = kVis ? finish_visible(metric, t[0], t[1], t[2], nv, hw) : finish_score(metric, t[0], t[1], t[2], hw);
     }
     __syncthreads();
   }

@@ -621,9 +621,9 @@ struct UNetEngine {
   }
 
   // UNet.forward for hypotheses [hyp0, hyp0 + n) of the flattened (b, pose) list
-  // query_feat [B, Q, Cl, hw]; score_part [B * N, Q, nslab, kScoreParts]
+  // query_feat [B, Q, Cl, hw]; score_part [B * N, Q, nslab, kScoreParts]; vis (optional) [B, Q, hw] visible maps
   int forward_chunk(const float* poses, int hyp0, int n, int N, const float* query_feat,
-                    float* out_emb, float* score_part, cudaStream_t st, int Q = 1) {
+                    float* out_emb, float* score_part, cudaStream_t st, int Q = 1, const uint8_t* vis = nullptr) {
     const bool sp = split();
     auto A = [&](const Act& buf, int C) { return Act(buf.hi, C, sp ? buf.lo : nullptr); };
     ref_of_kernel<<<(n + 255) / 256, 256, 0, st>>>(ref_of, hyp0, N, n);
@@ -707,10 +707,11 @@ struct UNetEngine {
     if (tap("final_conv.0", A(curb, dim), dim, S, n, st)) return -1;
     const int hw = S * S;
     const int nslab = (hw + kFinalPix - 1) / kFinalPix;
-    NOPE_CUDA(launch_pdl(final_conv_score_kernel, dim3(nslab, n), dim3(kFinalThreads), (size_t)kMaxLatent * dim * sizeof(float),
+    NOPE_CUDA(launch_pdl(vis ? final_conv_score_kernel<true> : final_conv_score_kernel<false>, dim3(nslab, n),
+                         dim3(kFinalThreads), (size_t)kMaxLatent * dim * sizeof(float),
                          st, curb.hi, final_w, final_b, out_emb ? out_emb + (size_t)hyp0 * Cl * hw : nullptr, query_feat,
                          ref_of, score_part ? score_part + (size_t)hyp0 * Q * nslab * kScoreParts : nullptr, hw, dim,
-                         Cl, sp ? curb.lo : nullptr, metric, occ_threshold, bf(), Q));
+                         Cl, sp ? curb.lo : nullptr, metric, occ_threshold, bf(), Q, vis));
     ++launches;
     return 0;
   }
@@ -724,9 +725,10 @@ struct UNetEngine {
   int nslab() const { return (S0 * S0 + kFinalPix - 1) / kFinalPix; }
   // similarities (sim [B * Q, N]) and top-k of every (reference, query) row from the score partials
   int rank(const float* part, float* sim, int B, int N, int Q, int k, float* topv, int64_t* topi, int64_t idx_base,
-           cudaStream_t st) {
-    NOPE_CUDA(launch_pdl(sim_topk_kernel, dim3(B * Q), dim3(256), 0, st, part, nslab(), sim, N, k, topv,
-                         reinterpret_cast<long long*>(topi), (long long)idx_base, kScoreParts, metric, S0 * S0, Q));
+           cudaStream_t st, const uint8_t* vis = nullptr) {
+    NOPE_CUDA(launch_pdl(vis ? sim_topk_kernel<true> : sim_topk_kernel<false>, dim3(B * Q), dim3(256), 0, st, part,
+                         nslab(), sim, N, k, topv, reinterpret_cast<long long*>(topi), (long long)idx_base, kScoreParts,
+                         metric, S0 * S0, Q, vis));
     return 0;
   }
 };

@@ -187,7 +187,8 @@ def _check_seed_latents(seed_latents, shape):
         raise ValueError(f"seed_latents must be {shape}, got {tuple(seed_latents.shape)}")
 
 
-def refine_inplane(engine, encoder, ref_feat, query_images, all_relativeR, seeds, seed_latents, refiner, k=5):
+def refine_inplane(engine, encoder, ref_feat, query_images, all_relativeR, seeds, seed_latents, refiner, k=5,
+                   hidden=None):
     """Refine each (reference, query) row from its best (angle, pose) pairs, with any engine that has `sweep()`.
 
     ref_feat [B, C, 32, 32]; query_images [B, 3, 256, 256] or [B, Q, 3, 256, 256]; all_relativeR [B, N, 6], the grid
@@ -204,7 +205,9 @@ def refine_inplane(engine, encoder, ref_feat, query_images, all_relativeR, seeds
     Each step proposes keep * 9 poses and keep * 3 rolls per row, encodes the 2 * keep new rolled crops, sweeps all
     pairs with one reference row per (reference, query) and selects the next `keep` centres (the last step: k).
     Everything runs on the current stream with no host synchronisation (device copies of the refiner's constants
-    are made by the first call on a device)."""
+    are made by the first call on a device).  hidden [B(, Q), 256, 256] (uint8 or bool, the crops' masks of pixels
+    that may be hidden, DESIGN.md section 27): every step's pairs score over the visible map of their own roll, made
+    from the candidates' (cos, sin) by latent_visibility, so a kept roll and a fresh one use the same arithmetic."""
     centres = isinstance(seeds, dict)
     rest = tuple(ref_feat.shape[1:])
     if centres:
@@ -221,6 +224,9 @@ def refine_inplane(engine, encoder, ref_feat, query_images, all_relativeR, seeds
         raise ValueError(f"seeds must be two {lead + (keep,)} tensors, got {tuple(pose_idx.shape)} and "
                          f"{tuple(angle_idx.shape)}")
     _check_seed_latents(seed_latents, lead + (keep,) + rest)
+    if hidden is not None:
+        from .visibility import check_hidden, latent_visibility
+        hid = check_hidden(hidden, lead, "refine_inplane").to(dev)
     rows = ref_rows.shape[0]
     stencils, _, table = refiner._on(dev)
     rel = all_relativeR.to(dev, torch.float32).contiguous()
@@ -241,7 +247,12 @@ def refine_inplane(engine, encoder, ref_feat, query_images, all_relativeR, seeds
         fresh_idx = row_ix.to(torch.int32)[:, None].expand(rows, n * (ROLL - 1)).reshape(-1)
         fresh = encoder.encode_image_rotated(images, fresh_idx, fresh_cs).view(rows, n, ROLL - 1, *rest)
         qf = torch.cat([lat[:, :, None], fresh], dim=2).view(rows, n * ROLL, *rest)
-        sim = engine.sweep(ref_rows, cand["poses"], query_feat=qf, want_emb=False, want_sim=True, k=0)["sim"]
+        vis = {}                                   # query_visible= only with a mask: any sweep() serves without one
+        if hidden is not None:
+            pair_idx = row_ix.to(torch.int32)[:, None].expand(rows, n * ROLL).reshape(-1)
+            vis["query_visible"] = latent_visibility(hid, cand["cossin"].reshape(-1, 2), pair_idx).view(
+                rows, n * ROLL, 32, 32)
+        sim = engine.sweep(ref_rows, cand["poses"], query_feat=qf, want_emb=False, want_sim=True, k=0, **vis)["sim"]
         cur = select(sim, cand, refiner.thresholds[s], k if s == refiner.steps - 1 else keep)
         lat = qf[row_ix[:, None], cur["aslot"].long().clamp_min(0)]
     return {"D": cur["D"].view(*lead, k, 3, 3), "seed": cur["seed"].to(torch.int64).view(*lead, k),

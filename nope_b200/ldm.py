@@ -95,16 +95,16 @@ class UNetModelPose(SweepEngine):
             raise ValueError("UNetModelPose fuses the 'l2' similarity only")
 
     def sweep(self, ref_latent, poses, query_latent=None, want_emb=True, want_sim=None, k=0, idx_base=0,
-              query_feat=None, out=None):
+              query_feat=None, out=None, query_visible=None):
         """ref_latent [B,C,32,32], poses [B,N,6] (+ query_latent) -> dict(emb, sim, topv, topi).
         query_latent [B,C,32,32] gives sim [B,N] / topv, topi [B,k]; [B,Q,C,32,32] (Q queries per reference, one
         sweep) gives [B,Q,N] / [B,Q,k].
         `query_feat` is an alias of `query_latent` and `out` may carry preallocated `sim` / `topv` / `topi`
         tensors (the keywords nope_b200.unet.UNet.sweep and nope_b200.dist.ShardedSweep use), so the pose grid
-        shards across GPUs the same way."""
+        shards across GPUs the same way.  query_visible: the rows' visible maps, as in UNet.sweep."""
         if query_feat is not None:
             query_latent = query_feat
-        return super().sweep(ref_latent, poses, query_latent, want_emb, want_sim, k, idx_base, out)
+        return super().sweep(ref_latent, poses, query_latent, want_emb, want_sim, k, idx_base, out, query_visible)
 
     def predict_pose(self, query_latent, ref_latent, all_relativeR, template_poses, k=5):
         """Latent-space form of nope_b200.model.PoseConditional.predict_pose for this UNet:

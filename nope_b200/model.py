@@ -109,13 +109,20 @@ class PoseConditional:
 
     # ------------------------------------------------------------------ model.py:254-266
     @torch.no_grad()
-    def retrieval(self, query, template_feat, k=5):
+    def retrieval(self, query, template_feat, k=5, hidden=None):
         """-> (similarity, nearest_idx).  Query and template batches follow the reference's broadcasting
         (model.py:260-262): equal batches give [B,N]; templates [1,N,...] serve every query ([Bq,N]: templates
-        generated once, queries streamed); one query against [Bt,N,...] templates gives [Bt,N]."""
+        generated once, queries streamed); one query against [Bt,N,...] templates gives [Bt,N].  hidden [Bq, 256,
+        256] (uint8 or bool, non-zero = may be hidden by an occluder): each query scores only its visible latent
+        pixels (DESIGN.md section 27); None, or an all-zero mask, gives the scores without it bit for bit."""
         metric = self._metric()
+        hidden = self._hidden("retrieval", hidden, query.shape[:1])
         query_feat = self.u_net.encoder.encode_image(query.to(self.device), mode="mode")
-        return score_topk(query_feat, template_feat, k=k, metric=metric, threshold=self._occlusion_threshold())
+        vis = {}
+        if hidden is not None:
+            from .visibility import query_visible
+            vis["visible"] = query_visible(hidden.to(self.device), query.shape[:1], "retrieval")
+        return score_topk(query_feat, template_feat, k=k, metric=metric, threshold=self._occlusion_threshold(), **vis)
 
     def _occlusion_threshold(self):
         """`threshold` of the template encoder (OcclusionAwareSimilarity, base_template.py:67-75;
@@ -139,6 +146,19 @@ class PoseConditional:
             multi_query_form(query, reference)
         return metric, checked
 
+    def _hidden(self, name, hidden, lead):
+        """The refusals of a search's hidden= (DESIGN.md section 27), before any device work: model.dist set
+        (NotImplementedError; the searches under occlusion run on one device) and a mask that is not [*lead, 256,
+        256] uint8 or bool (ValueError).  -> hidden as given (None stays None)"""
+        if hidden is None:
+            return None
+        if self.dist is not None:
+            raise NotImplementedError(f"{name}(hidden=) does not shard across GPUs: it runs on one device (unset "
+                                      "model.dist)")
+        from .visibility import check_hidden
+        check_hidden(hidden, lead, name)
+        return hidden
+
     def _encode(self, query, reference, metric):
         """The metric set for the sweep's last layer, then queries and references through one encoder call over
         cat([flattened queries, references]).  -> (query latents in the query's form, reference latents)"""
@@ -151,7 +171,7 @@ class PoseConditional:
     # ------------------------------------------------------------------ model.py:313-357
     @torch.no_grad()
     def predict_pose(self, query, reference, all_relativeR, template_poses=None, k=5,
-                     return_templates=False):
+                     return_templates=False, hidden=None):
         """-> (R [B,k,3,3] | None, nearest_idx [B,k] int64, similarity [B,N]).  The scores and
         the ranking come out of the sweep's fused last layer; the [B,N,C,32,32] templates are
         only materialised when asked for.
@@ -160,13 +180,21 @@ class PoseConditional:
           query [B,Q,3,H,W] with reference [B,3,H,W] -> R [B,Q,k,3,3], nearest_idx [B,Q,k], similarity [B,Q,N];
           query [Q,3,H,W] with reference [1,3,H,W] and all_relativeR [1,N,6] -> [Q,k,3,3], [Q,k], [Q,N]
           (the reference's broadcasting of one template set against a query batch).
-        Query and reference images go through one encoder call, the templates through one sweep."""
+        Query and reference images go through one encoder call, the templates through one sweep.
+        hidden [..., 256, 256] (the query's leading shape; uint8 or bool, non-zero = may be hidden by an occluder):
+        every score leaves out the latent pixels those crop pixels reach (DESIGN.md section 27); None, or an all-zero
+        mask, gives the scores without it bit for bit."""
         metric, _ = self._checked(query, reference)
+        hidden = self._hidden("predict_pose", hidden, query.shape[:-3])
         query_feat, reference_feat = self._encode(query, reference, metric)
+        visible = None
+        if hidden is not None:
+            from .visibility import query_visible
+            visible = query_visible(hidden.to(self.device), query.shape[:-3], "predict_pose")
         # under sharding the templates are (local templates, lo, hi): each rank keeps only its slice
         return grid_search(self.u_net, reference_feat, query_feat, all_relativeR, template_poses, k=k,
                            return_templates=return_templates, dist=self.dist, metric=metric,
-                           threshold=self._occlusion_threshold())
+                           threshold=self._occlusion_threshold(), query_visible=visible)
 
     @torch.no_grad()
     def predict_pose_coarse_to_fine(self, query, reference, all_relativeR_levels, hierarchy, template_poses=None,
@@ -200,31 +228,40 @@ class PoseConditional:
         query_feat, reference_feat = self._encode(query, reference, metric)
         return refined_search(self.u_net, reference_feat, query_feat, all_relativeR, refiner, k=k, keep=keep)
 
-    def _inplane_sweep(self, query, reference, all_relativeR, metric, A, k):
+    def _inplane_sweep(self, query, reference, all_relativeR, metric, A, k, hidden=None):
         """The in-plane search's sweep (DESIGN.md section 11): the references encoded on their own, the A rotated
         copies of each of the B * Q queries by one encode_image_inplane call, one sweep with Q * A query rows per
         reference, and the top-k of each (reference, query) row jointly over (angle, pose).
         -> (sim [B, Q * A, N], top [B * Q, k] at a * N + n, query latents [B * Q, A, C, h, w], the flattened query
-        images [B * Q, 3, H, W] and the reference latents, on the device)"""
+        images [B * Q, 3, H, W] and the reference latents, on the device).  hidden: the queries' crop-space masks;
+        each rotated copy then scores over its own visible map."""
         enc = self.u_net.encoder
         self.u_net.set_metric(metric, self._occlusion_threshold())
         B, N = reference.shape[0], all_relativeR.shape[1]
         reference_feat = enc.encode_image(reference.to(self.device))
         images = query.reshape(-1, *query.shape[-3:]).to(self.device)
         query_feat = enc.encode_image_inplane(images, A)
+        visible = None
+        if hidden is not None:
+            from .visibility import latent_visibility_inplane
+            visible = latent_visibility_inplane(hidden.reshape(-1, *hidden.shape[-2:]).to(self.device), A)
+            visible = visible.view(B, -1, *visible.shape[2:])
+        vis = {} if visible is None else {"query_visible": visible}
         sim = self.u_net.sweep(reference_feat, all_relativeR, query_feat=query_feat.view(B, -1, *query_feat.shape[2:]),
-                               want_emb=False, want_sim=True, k=0)["sim"]
+                               want_emb=False, want_sim=True, k=0, **vis)["sim"]
         _, top = topk(sim.view(-1, A * N), k)
         return sim, top, query_feat, images, reference_feat
 
     @torch.no_grad()
-    def predict_pose_inplane(self, query, reference, all_relativeR, template_poses=None, k=5, angles=36):
+    def predict_pose_inplane(self, query, reference, all_relativeR, template_poses=None, k=5, angles=36,
+                             hidden=None):
         """predict_pose over pose x in-plane angle (nope_b200.inplane, DESIGN.md section 11): every query crop is
         rotated by the A = `angles` angles a * 360 / A and each rotated copy is scored against the same templates.
         -> (R [..., k, 3, 3] = Rz(alpha[angle_idx]) template_poses[nearest_idx] (float64) | None, nearest_idx [..., k],
         angle_idx [..., k], similarity [..., A, N]) in the query forms of predict_pose; the top-k runs jointly over
         (angle, pose), ties -> the lowest a * N + n.  One encoder call for the references, one encode_image_inplane
-        call for the queries, one sweep with Q * A query rows per reference.  angles = 1 is predict_pose."""
+        call for the queries, one sweep with Q * A query rows per reference.  angles = 1 is predict_pose.  hidden: as
+        in predict_pose; each rotated copy scores over the map of its own roll."""
         from .inplane import check_inplane_args, compose
 
         def check():
@@ -234,27 +271,30 @@ class PoseConditional:
             return check_inplane_args(angles, k, all_relativeR.shape[1])
 
         metric, (A, k) = self._checked(query, reference, "predict_pose_inplane", check)
-        sim, top, _, _, _ = self._inplane_sweep(query, reference, all_relativeR, metric, A, k)
+        hidden = self._hidden("predict_pose_inplane", hidden, query.shape[:-3])
+        sim, top, _, _, _ = self._inplane_sweep(query, reference, all_relativeR, metric, A, k, hidden)
         N, lead = all_relativeR.shape[1], tuple(query.shape[:-3])
         nearest, angle = (top % N).view(lead + (k,)), (top // N).view(lead + (k,))
         R = compose(template_poses, nearest, angle, A) if template_poses is not None else None
         return R, nearest, angle, sim.view(lead + (A, N))
 
     @torch.no_grad()
-    def predict_pose_inplane_refined(self, query, reference, all_relativeR, refiner, k=5, keep=2):
+    def predict_pose_inplane_refined(self, query, reference, all_relativeR, refiner, k=5, keep=2, hidden=None):
         """Roll and viewpoint between the bins and the grid poses (nope_b200.inplane_refine, DESIGN.md section 14):
         the in-plane search over the refiner's A angles seeds each (reference, query) row with its joint top-`keep`
         (angle, pose) pairs, and the refiner's steps refine the viewpoint on the template side and the roll on the
         query side.  refiner: an InplaneRefiner over the grid of all_relativeR [B, N, 6].
         -> (R [..., k, 3, 3] = Rz(rho) D template_poses[seed] (float64), seed [..., k], alpha_deg [..., k] =
         atan2(sin, cos) of the roll rho, score [..., k]) in the query forms of predict_pose; descending score, each
-        exactly the score a sweep of that pose against that rolled latent gives."""
+        exactly the score a sweep of that pose against that rolled latent gives.  hidden: as in predict_pose; the
+        search and every refinement step score over the visible maps of their rolls."""
         from .inplane_refine import check_inplane_refine_args, pose_rotations, refine_inplane, roll_degrees
         metric, _ = self._checked(
             query, reference, "predict_pose_inplane_refined",
             lambda: check_inplane_refine_args(refiner, all_relativeR, keep, k, reference.shape[0]))
+        hidden = self._hidden("predict_pose_inplane_refined", hidden, query.shape[:-3])
         _, top, query_feat, images, reference_feat = self._inplane_sweep(query, reference, all_relativeR, metric,
-                                                                         refiner.angles, keep)
+                                                                         refiner.angles, keep, hidden)
         N = refiner.num_poses
         pose_idx, angle_idx = top % N, top // N
         lat = query_feat[torch.arange(top.shape[0], device=top.device)[:, None], angle_idx]   # [B * Q, keep, C, h, w]
@@ -262,7 +302,8 @@ class PoseConditional:
         lead = tuple(query.shape[:-3])
         out = refine_inplane(self.u_net, self.u_net.encoder, reference_feat, images.view(*lead, *query.shape[-3:]),
                              all_relativeR, (pose_idx.view(*lead, keep), angle_idx.view(*lead, keep)),
-                             lat.view(*lead, keep, *lat.shape[2:]), refiner, k=k)
+                             lat.view(*lead, keep, *lat.shape[2:]), refiner, k=k,
+                             **({} if hidden is None else {"hidden": hidden.reshape(*lead, *hidden.shape[-2:])}))
         R = pose_rotations(out["D"], out["seed"], out["cossin"], refiner)
         seed, alpha, score = out["seed"], roll_degrees(out["cossin"]), out["score"]
         if squeeze:
@@ -270,11 +311,12 @@ class PoseConditional:
         return R, seed, alpha, score
 
     @torch.no_grad()
-    def retrieval_inplane(self, query, template_feat, k=5, angles=36):
+    def retrieval_inplane(self, query, template_feat, k=5, angles=36, hidden=None):
         """retrieval over pose x in-plane angle, for templates generated once and queries streamed: the A = `angles`
         rotated copies of every query image [Bq, 3, 256, 256] against template_feat [Bt, N, C, h, w], batches
         broadcast as in retrieval.  -> (similarity [rows, A, N], nearest_idx [rows, k], angle_idx [rows, k]); the
-        top-k runs jointly over (angle, pose), ties -> the lowest a * N + n."""
+        top-k runs jointly over (angle, pose), ties -> the lowest a * N + n.  hidden [Bq, 256, 256]: as in
+        predict_pose_inplane."""
         from .inplane import check_inplane_args
         if query.dim() != 4 or template_feat.dim() != 5:
             raise ValueError(f"query [B, 3, H, W] and template_feat [B, N, C, h, w] expected; got "
@@ -286,14 +328,25 @@ class PoseConditional:
         N = template_feat.shape[1]
         A, k = check_inplane_args(angles, k, N)
         metric = self._metric()
-        B, Q, _, rows = broadcast_batches(query.shape[0], template_feat.shape[0])
+        hidden = self._hidden("retrieval_inplane", hidden, query.shape[:1])
+        B, Q, Bt, rows = broadcast_batches(query.shape[0], template_feat.shape[0])
         dev = template_feat.device
         if dev.type != "cuda":
             raise _lib.NopeError("retrieval_inplane needs CUDA tensors (no CPU fallback)")
         q = enc.encode_image_inplane(query.to(dev), A)                                     # [Bq, A, C, h, w]
         q = q.reshape(-1, Q * A, *q.shape[2:]).expand(B, Q * A, *q.shape[2:]).contiguous()
-        sim, _, _ = _score_multi(q, template_feat.to(torch.float32).contiguous(), B, Q * A, metric,
-                                 self._occlusion_threshold())
+        t = template_feat.to(torch.float32).contiguous()
+        if hidden is None:
+            sim, _, _ = _score_multi(q, t, B, Q * A, metric, self._occlusion_threshold())
+        else:
+            # the broadcasting as groups: template batch g serves the B * Q * A / Bt rows that follow row_off[g]
+            from .visibility import latent_visibility_inplane, score_visible
+            vis = latent_visibility_inplane(hidden.to(dev), A)
+            vis = vis.reshape(-1, Q * A, *vis.shape[2:]).expand(B, Q * A, *vis.shape[2:]).reshape(-1, *vis.shape[2:])
+            slots = torch.arange(Bt, device=dev, dtype=torch.int32)
+            row_off = torch.arange(Bt + 1, device=dev, dtype=torch.int32) * (B * Q * A // Bt)
+            sim, _ = score_visible(q.view(-1, *q.shape[2:]), t, slots, row_off, A, vis, metric,
+                                   self._occlusion_threshold(), 0)
         _, flat = topk(sim.view(rows, A * N), k)
         return sim.view(rows, A, N), flat % N, flat // N
 
@@ -329,7 +382,7 @@ class PoseConditional:
             query, None, name, lambda: check_bank_search(bank, self.u_net, query.shape[0], obj_ids, angles, k))
         return metric, A, k, slots
 
-    def _bank_scores(self, query, bank, slots, metric, A, k):
+    def _bank_scores(self, query, bank, slots, metric, A, k, hidden=None):
         """the detections' crops grouped by slot, their A rotated copies encoded by one encode_image_inplane call and
         scored against the bank by one nope_score_topk_grouped call.  -> (plan, query latents, sim [D, A, N], top
         [D, k]), all in the plan's group order"""
@@ -337,32 +390,40 @@ class PoseConditional:
         plan = RowPlan(slots, A, bank.device)
         images = plan.grouped(query.to(self.device))
         lat = self.u_net.encoder.encode_image_inplane(images, A)
-        sim, top = score_rows(bank, lat, plan, metric, self._occlusion_threshold(), k)
+        visible = None
+        if hidden is not None:
+            from .visibility import latent_visibility_inplane
+            visible = latent_visibility_inplane(plan.grouped(hidden.to(self.device)), A)
+        vis = {} if visible is None else {"visible": visible}
+        sim, top = score_rows(bank, lat, plan, metric, self._occlusion_threshold(), k, **vis)
         return plan, lat, sim, top
 
     @torch.no_grad()
-    def predict_pose_bank(self, query, obj_ids, bank, k=5, angles=36):
+    def predict_pose_bank(self, query, obj_ids, bank, k=5, angles=36, hidden=None):
         """predict_pose_inplane against a template bank: query [D, 3, 256, 256], one crop per detection, obj_ids [D]
         (host) its objects, each held by `bank` (build_template_bank).  -> (R [D, k, 3, 3] = Rz(alpha[angle_idx])
         template_poses[nearest_idx] (float64), nearest_idx [D, k], angle_idx [D, k], similarity [D, A, N]) in the
         detections' order: what predict_pose_inplane returns for reference[slot], with each detection scored against
         its object's stored templates (the arithmetic of retrieval_inplane) instead of a sweep.  Detections of one
         object share each template read.  One encode_image_inplane call over all D crops, one scoring call, no host
-        synchronisation.  angles = 1 is the plain grid search.  Scores use the model's current metric."""
+        synchronisation.  angles = 1 is the plain grid search.  Scores use the model's current metric.  hidden
+        [D, 256, 256]: as in predict_pose_inplane, the scores of retrieval_inplane with the same hidden."""
         from .inplane import compose
         metric, A, k, slots = self._bank_query("predict_pose_bank", query, obj_ids, bank, angles, k)
-        plan, _, sim, top = self._bank_scores(query, bank, slots, metric, A, k)
+        hidden = self._hidden("predict_pose_bank", hidden, query.shape[:1])
+        plan, _, sim, top = self._bank_scores(query, bank, slots, metric, A, k, hidden)
         sim, top = plan.restore(sim), plan.restore(top)
         N = bank.num_poses
         nearest, angle = top % N, top // N
         return compose(bank.template_poses, nearest, angle, A), nearest, angle, sim
 
     @torch.no_grad()
-    def predict_pose_bank_refined(self, query, obj_ids, bank, refiner, k=5, keep=2):
+    def predict_pose_bank_refined(self, query, obj_ids, bank, refiner, k=5, keep=2, hidden=None):
         """predict_pose_inplane_refined against a template bank: the bank search over the refiner's angles seeds each
         detection with its joint top-`keep` (angle, pose) pairs, and refine_inplane continues from them with the
         detection's reference_latents[slot] and all_relativeR[slot].  refiner: an InplaneRefiner over the bank's grid.
-        -> (R [D, k, 3, 3], seed [D, k], alpha_deg [D, k], score [D, k]) as predict_pose_inplane_refined returns."""
+        -> (R [D, k, 3, 3], seed [D, k], alpha_deg [D, k], score [D, k]) as predict_pose_inplane_refined returns.
+        hidden [D, 256, 256]: as in predict_pose_inplane_refined."""
         from .inplane_refine import (InplaneRefiner, check_inplane_refine_args, pose_rotations, refine_inplane,
                                      roll_degrees)
         if not isinstance(refiner, InplaneRefiner):
@@ -371,7 +432,8 @@ class PoseConditional:
                                                keep)
         check_inplane_refine_args(refiner, bank.all_relativeR, keep, k)
         bank.check_grid(refiner.template_poses)
-        plan, lat, _, top = self._bank_scores(query, bank, slots, metric, A, keep)
+        hidden = self._hidden("predict_pose_bank_refined", hidden, query.shape[:1])
+        plan, lat, _, top = self._bank_scores(query, bank, slots, metric, A, keep, hidden)
         N = bank.num_poses
         pose_idx, angle_idx = top % N, top // N
         seed_lat = lat[torch.arange(plan.D, device=top.device)[:, None], angle_idx]     # [D, keep, C, h, w]
@@ -379,7 +441,8 @@ class PoseConditional:
         ref_feat = bank.reference_latents.index_select(0, plan.det_slots)
         rel = bank.all_relativeR.index_select(0, plan.det_slots)
         out = refine_inplane(self.u_net, self.u_net.encoder, ref_feat, query.to(self.device), rel,
-                             (pose_idx, angle_idx), seed_lat, refiner, k=k)
+                             (pose_idx, angle_idx), seed_lat, refiner, k=k, **({} if hidden is None else
+                                                                               {"hidden": hidden}))
         R = pose_rotations(out["D"], out["seed"], out["cossin"], refiner)
         return R, out["seed"], roll_degrees(out["cossin"]), out["score"]
 
@@ -722,7 +785,8 @@ class PoseConditional:
 
     @torch.no_grad()
     def predict_pose_frames(self, frames, masks, K, obj_ids, reference=None, all_relativeR=None, template_poses=None,
-                            angles=36, k=5, refiner=None, refine=None, frame_idx=None, occluders=None, bank=None):
+                            angles=36, k=5, refiner=None, refine=None, frame_idx=None, occluders=None, bank=None,
+                            occluded_search=False):
         """6D poses of B detections in camera frames (DESIGN.md section 23): `crop.frame_crops` cuts a keep_inplane
         crop around each mask's `initial_translation` t0, the in-plane search (`predict_pose_inplane`, or
         `predict_pose_inplane_refined` with a refiner) finds the rotation in the crop's camera, `crop.to_camera`
@@ -743,40 +807,55 @@ class PoseConditional:
                      and template_poses: the search is then predict_pose_bank (predict_pose_bank_refined with a
                      refiner), which scores each crop against its object's stored templates instead of sweeping the
                      reference (DESIGN.md section 25).  Give either the bank or reference and all_relativeR.
+          occluded_search  True: the search too leaves out what the occluders may hide -- its hidden= is
+                     crop_hidden of the occluders through each crop's map (DESIGN.md section 27); needs occluders.
+                     False is the search without them, bit for bit.
         -> {"R": float64 [B, k, 3, 3] in the real camera, "t": float64 [B, k, 3] mm, "score": the search's [B, k],
         "iou": the silhouette IoU [B, k], "R_crop": the search's rotations [B, k, 3, 3], "t0": [B, 3],
         "crops": [B, 3, 256, 256]}.  R and t go unchanged into eval_bop(R_est=, t_est=), refine_depth and
         select_distinct.  The only host synchronisation beyond the search's is frame_crops' copy of t0."""
         from .crop import frame_crops
-        ids = self._frame_ids("predict_pose_frames", masks, obj_ids, refine, occluders)
+        ids = self._frame_ids("predict_pose_frames", masks, obj_ids, refine, occluders, occluded_search)
         B = len(ids)
         self._frame_templates("predict_pose_frames", B, ids, bank, reference, all_relativeR, template_poses,
                               getattr(refiner, "angles", angles))
-        crops, t0, Rv, _ = frame_crops(frames, masks, K, self._diameters(ids), image_size=256, frame_idx=frame_idx)
+        crops, t0, Rv, inv_maps = frame_crops(frames, masks, K, self._diameters(ids), image_size=256,
+                                              frame_idx=frame_idx)
+        occ = {}                                   # the search's hidden=, passed only when there is one
+        if occluded_search:
+            occluders = self._frame_occluders("predict_pose_frames", frames, masks, frame_idx, occluders)
+            occ["hidden"] = self._crop_hidden(occluders, inv_maps)
         if bank is not None and refiner is None:
-            R_crop, nearest, angle, sim = self.predict_pose_bank(crops, ids, bank, k=k, angles=angles)
+            R_crop, nearest, angle, sim = self.predict_pose_bank(crops, ids, bank, k=k, angles=angles, **occ)
             N = sim.shape[-1]
             score = sim.reshape(B, -1).gather(1, angle * N + nearest)
         elif bank is not None:
-            R_crop, _, _, score = self.predict_pose_bank_refined(crops, ids, bank, refiner, k=k)
+            R_crop, _, _, score = self.predict_pose_bank_refined(crops, ids, bank, refiner, k=k, **occ)
         elif refiner is None:
             R_crop, nearest, angle, sim = self.predict_pose_inplane(crops, reference, all_relativeR, template_poses,
-                                                                    k=k, angles=angles)
+                                                                    k=k, angles=angles, **occ)
             N = sim.shape[-1]
             score = sim.reshape(B, -1).gather(1, angle * N + nearest)
         else:
-            R_crop, _, _, score = self.predict_pose_inplane_refined(crops, reference, all_relativeR, refiner, k=k)
+            R_crop, _, _, score = self.predict_pose_inplane_refined(crops, reference, all_relativeR, refiner, k=k,
+                                                                    **occ)
         return self._frame_fits("predict_pose_frames", frames, masks, K, ids, frame_idx, occluders, refine, R_crop,
                                 score, crops, t0, Rv)
 
-    def _frame_ids(self, name, masks, obj_ids, refine, occluders):
-        """The refusals of a pose from camera frames that do not depend on the search: refine, occluders, one obj_id
-        per mask and a mesh and models_info entry for each.  -> the ids (host ints)"""
+    def _frame_ids(self, name, masks, obj_ids, refine, occluders, occluded_search=False):
+        """The refusals of a pose from camera frames that do not depend on the search: refine, occluders (and
+        occluded_search without them, or with model.dist), one obj_id per mask and a mesh and models_info entry for
+        each.  -> the ids (host ints)"""
         import numpy as np
         if refine not in (None, "contour"):
             raise ValueError(f"refine must be None or 'contour', got {refine!r}")
         if isinstance(occluders, str) and occluders != "detections":
             raise ValueError(f"occluders must be None, a tensor or 'detections', got {occluders!r}")
+        if occluded_search and occluders is None:
+            raise ValueError(f"{name}: occluded_search=True needs occluders (a tensor or 'detections')")
+        if occluded_search and self.dist is not None:
+            raise NotImplementedError(f"{name}(occluded_search=True) does not shard across GPUs: it runs on one "
+                                      "device (unset model.dist)")
         ids = [int(i) for i in np.asarray(obj_ids.detach().cpu() if torch.is_tensor(obj_ids) else obj_ids)
                .reshape(-1).tolist()]
         B = len(ids)
@@ -804,6 +883,23 @@ class PoseConditional:
             raise ValueError(f"{name}: reference [1 | B, 3, 256, 256] with B = {B} expected, got "
                              f"{tuple(reference.shape)}")
 
+    def _frame_occluders(self, name, frames, masks, frame_idx, occluders):
+        """occluders as the fits take them: "detections" becomes crop.detection_occluders of the masks (on the
+        device), a tensor is checked against the masks' shape"""
+        from .crop import _tensor, detection_occluders
+        masks = _tensor(masks)
+        if isinstance(occluders, str):
+            from .bop import _to_dev
+            md = masks if masks.device.type == "cuda" else _to_dev(masks, self.device, masks.dtype)
+            occluders = detection_occluders(md, frame_idx, num_frames=_tensor(frames).shape[0])
+        return self._occluders(name, occluders, masks)
+
+    def _crop_hidden(self, occluders, inv_maps):
+        """the search's hidden= of occluders [B, H, W] through the crops' maps (crop_hidden)"""
+        from .crop import _to_device
+        from .visibility import crop_hidden
+        return crop_hidden(_to_device(self.device, occluders), inv_maps)
+
     def _diameters(self, ids):
         import numpy as np
         return np.array([self.bop_models[i]["diameter"] for i in ids], dtype=np.float64)
@@ -813,16 +909,12 @@ class PoseConditional:
         real camera, the occluders, the translation fit from t0 and, for refine="contour", the contour refinement.
         -> the dict of predict_pose_frames"""
         from . import contour_refine, translation
-        from .crop import _as_numpy, _tensor, detection_occluders, to_camera
+        from .crop import _as_numpy, _tensor, to_camera
         import numpy as np
         B = len(ids)
         R = to_camera(R_crop.to(self.device), Rv.to(self.device))
         masks = _tensor(masks)
-        if isinstance(occluders, str):
-            from .bop import _to_dev
-            md = masks if masks.device.type == "cuda" else _to_dev(masks, self.device, masks.dtype)
-            occluders = detection_occluders(md, frame_idx, num_frames=_tensor(frames).shape[0])
-        occluders = self._occluders(name, occluders, masks)
+        occluders = self._frame_occluders(name, frames, masks, frame_idx, occluders)
         Kh = torch.from_numpy(np.ascontiguousarray(np.broadcast_to(_as_numpy(K, "K").reshape(-1, 3, 3), (B, 3, 3))))
         kk = R.shape[1]
         t = torch.empty((B, kk, 3), device=self.device, dtype=torch.float64)
@@ -841,13 +933,15 @@ class PoseConditional:
 
     @torch.no_grad()
     def track_pose_frames(self, frames, masks, K, obj_ids, R_prior, refiner, bank=None, reference=None,
-                          all_relativeR=None, template_poses=None, k=5, refine=None, frame_idx=None, occluders=None):
+                          all_relativeR=None, template_poses=None, k=5, refine=None, frame_idx=None, occluders=None,
+                          occluded_search=False):
         """predict_pose_frames with the search replaced by a refinement from prior rotations (DESIGN.md section 26):
         R_prior [B, P, 3, 3] (1 <= P <= 16) in the real camera, e.g. the previous frame's R[:, :keep], is taken into
         each new crop's camera (crop.to_crop), mapped to refinement centres and refined by the refiner's steps
         (track.track_inplane), without the A rotated copies of a search.  refiner: an InplaneRefiner over the grid of
         the bank or of all_relativeR (template_poses, when given, must be that grid).  frames, masks, K, obj_ids, bank
-        or reference / all_relativeR, refine, frame_idx and occluders as predict_pose_frames takes them.
+        or reference / all_relativeR, refine, frame_idx, occluders and occluded_search as predict_pose_frames takes
+        them.
         -> predict_pose_frames' dict, "score" the refined score of each of the k poses.  Per detection it encodes P *
         (1 + 2 * steps) rotated crops and sweeps 9 * P * steps hypotheses; the host synchronises as often as in
         predict_pose_frames."""
@@ -859,7 +953,7 @@ class PoseConditional:
                                       "model.dist)")
         if not isinstance(refiner, InplaneRefiner):
             raise ValueError("refiner must be a nope_b200.inplane_refine.InplaneRefiner")
-        ids = self._frame_ids("track_pose_frames", masks, obj_ids, refine, occluders)
+        ids = self._frame_ids("track_pose_frames", masks, obj_ids, refine, occluders, occluded_search)
         B = len(ids)
         self._frame_templates("track_pose_frames", B, ids, bank, reference, all_relativeR, template_poses,
                               refiner.angles)
@@ -873,7 +967,12 @@ class PoseConditional:
                     torch.as_tensor(template_poses).detach().cpu().to(torch.float64), refiner.template_poses):
                 raise ValueError("track_pose_frames: template_poses is not the refiner's grid")
         metric = self._metric()
-        crops, t0, Rv, _ = frame_crops(frames, masks, K, self._diameters(ids), image_size=256, frame_idx=frame_idx)
+        crops, t0, Rv, inv_maps = frame_crops(frames, masks, K, self._diameters(ids), image_size=256,
+                                              frame_idx=frame_idx)
+        occ = {}
+        if occluded_search:
+            occluders = self._frame_occluders("track_pose_frames", frames, masks, frame_idx, occluders)
+            occ["hidden"] = self._crop_hidden(occluders, inv_maps)
         dev = self.device
         R_prior_crop = to_crop(R_prior.to(dev), Rv.to(dev))
         self.u_net.set_metric(metric, self._occlusion_threshold())
@@ -886,7 +985,7 @@ class PoseConditional:
             ref_feat = self.u_net.encoder.encode_image(reference.to(dev))
             ref_feat = ref_feat.expand(B, *ref_feat.shape[1:])
             rel = all_relativeR.to(dev).expand(B, *all_relativeR.shape[1:])
-        out = track_inplane(self.u_net, self.u_net.encoder, ref_feat, crops, rel, R_prior_crop, refiner, k=k)
+        out = track_inplane(self.u_net, self.u_net.encoder, ref_feat, crops, rel, R_prior_crop, refiner, k=k, **occ)
         R_crop = pose_rotations(out["D"], out["seed"], out["cossin"], refiner)
         return self._frame_fits("track_pose_frames", frames, masks, K, ids, frame_idx, occluders, refine, R_crop,
                                 out["score"], crops, t0, Rv)
@@ -986,10 +1085,11 @@ def broadcast_batches(bq, bt):
     raise ValueError(f"query batch {bq} and template batch {bt} do not broadcast (equal, or one of them 1)")
 
 
-def score_topk(query_feat, template_feat, k=5, metric="l2", idx_base=0, threshold=0.2):
+def score_topk(query_feat, template_feat, k=5, metric="l2", idx_base=0, threshold=0.2, visible=None):
     """similarity [B,N] and nearest_idx [B,k] of materialised templates
     (the arithmetic of model.py:260-265) on the GPU.  query_feat [Bq,C,h,w] and template_feat [Bt,N,C,h,w]
-    broadcast as in the reference (broadcast_batches): B = max(Bq, Bt)."""
+    broadcast as in the reference (broadcast_batches): B = max(Bq, Bt).  visible [Bq, 32, 32] (uint8 or bool,
+    DESIGN.md section 27): each query scores only the latent pixels its map marks non-zero."""
     check_metric(metric)
     if template_feat.dim() != 5 or query_feat.dim() != 4 or tuple(query_feat.shape[1:]) != tuple(template_feat.shape[2:]):
         raise ValueError(f"query_feat [B,C,h,w] and template_feat [B,N,C,h,w] expected; got "
@@ -1004,6 +1104,23 @@ def score_topk(query_feat, template_feat, k=5, metric="l2", idx_base=0, threshol
     q = query_feat.to(dev, torch.float32)
     if q.shape[0] != B * Q:
         q = q.expand(B * Q, *q.shape[1:])
+    if visible is not None:
+        from .visibility import score_visible
+        if visible.dtype not in (torch.uint8, torch.bool) or tuple(visible.shape) != (query_feat.shape[0], 32, 32):
+            raise ValueError(f"visible [{query_feat.shape[0]}, 32, 32] uint8 or bool expected, got "
+                             f"{tuple(visible.shape)} {visible.dtype}")
+        vis = visible.to(dev)
+        if vis.shape[0] != B * Q:
+            vis = vis.expand(B * Q, *vis.shape[1:])
+        Bt = template_feat.shape[0]
+        # the broadcasting as groups: template batch g serves rows [g * B * Q / Bt, (g + 1) * B * Q / Bt)
+        slots = torch.arange(Bt, device=dev, dtype=torch.int32)
+        row_off = torch.arange(Bt + 1, device=dev, dtype=torch.int32) * (B * Q // Bt)
+        sim, topi = score_visible(q.contiguous(), template_feat.to(torch.float32).contiguous(), slots, row_off, 1, vis,
+                                  metric, threshold, k)
+        if topi is None:
+            topi = torch.empty((B * Q, 0), device=dev, dtype=torch.int64)
+        return sim, (topi + idx_base if idx_base else topi)
     sim, _, topi = _score_multi(q.contiguous(), template_feat.to(torch.float32).contiguous(), B, Q, metric,
                                 threshold, k, idx_base)
     return sim, topi

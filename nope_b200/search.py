@@ -70,18 +70,22 @@ def _unsqueezed(squeeze, *xs):
 
 
 def grid_search(engine, ref_feat, query_feat, all_relativeR, template_poses=None, k=5, return_templates=False,
-                dist=None, metric="l2", threshold=0.2):
+                dist=None, metric="l2", threshold=0.2, query_visible=None):
     """The exhaustive search: one sweep of all_relativeR [B, N, 6] scores every query in its last layer.
     k is clamped to N.  dist: a nope_b200.dist.ShardedSweep to split the grid across GPUs (it selects the metric).
+    query_visible (the query's leading shape + [32, 32]): each query scores only its visible latent pixels.
     -> (R | None, nearest_idx, similarity[, templates]) in the query form of query_feat; under dist the templates are
     this rank's (local templates, lo, hi)."""
     query_feat, squeeze = multi_query_form(query_feat, ref_feat)
+    if query_visible is not None and squeeze:
+        query_visible = query_visible.unsqueeze(0)
     k = min(k, all_relativeR.shape[1])
     if dist is not None:
         sim, topi, emb = dist.sweep(engine, ref_feat, all_relativeR, query_feat, k=k, metric=metric,
                                     want_emb=return_templates, threshold=threshold)
     else:
-        out = engine.sweep(ref_feat, all_relativeR, query_feat=query_feat, want_emb=return_templates, k=k)
+        vis = {} if query_visible is None else {"query_visible": query_visible}
+        out = engine.sweep(ref_feat, all_relativeR, query_feat=query_feat, want_emb=return_templates, k=k, **vis)
         sim, topi, emb = out["sim"], out["topi"], out["emb"]
     sim, topi = _unsqueezed(squeeze, sim, topi)
     R = None if template_poses is None else lookup_rotations(template_poses, topi)

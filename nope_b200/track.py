@@ -61,14 +61,15 @@ def check_track_args(refiner, all_relativeR, R_prior_crop, k, B, refs=None):
     return P
 
 
-def track_inplane(engine, encoder, ref_feat, crops, all_relativeR, R_prior_crop, refiner, k=5):
+def track_inplane(engine, encoder, ref_feat, crops, all_relativeR, R_prior_crop, refiner, k=5, hidden=None):
     """Refine each crop's roll and viewpoint from prior rotations instead of a search, with any engine that has
     `sweep()`.  ref_feat [B, C, 32, 32], crops [B, 3, 256, 256], all_relativeR [B, N, 6] (the grid of `refiner`), one
     row per detection; R_prior_crop [B, P, 3, 3] (1 <= P <= 16), e.g. the previous frame's rotations in this frame's
     crop camera (crop.to_crop); encoder: a FeatureExtractor on the native engine.  The P priors of each row become
     centres (seed_centres), their latents come from one encode_image_rotated call, and refine_inplane continues from
     them.  -> refine_inplane's dict (D, seed, cossin, score, rel6d, latent [B, k, ...], hypotheses, crops).  Costs P
-    * (1 + 2 * steps) encodes and 9 * P * steps hypotheses per row; no host synchronisation."""
+    * (1 + 2 * steps) encodes and 9 * P * steps hypotheses per row; no host synchronisation.  hidden [B, 256, 256]:
+    the crops' masks of pixels that may be hidden, as refine_inplane takes them."""
     if crops.dim() != 4 or tuple(crops.shape[1:]) != (3, 256, 256):
         raise ValueError(f"crops [B, 3, 256, 256] expected, got {tuple(crops.shape)}")
     B = crops.shape[0]
@@ -81,7 +82,7 @@ def track_inplane(engine, encoder, ref_feat, crops, all_relativeR, R_prior_crop,
     idx = torch.arange(B, device=dev, dtype=torch.int32)[:, None].expand(B, P).reshape(-1)
     lat = encoder.encode_image_rotated(images, idx, cen["cossin"].reshape(B * P, 2))
     return refine_inplane(engine, encoder, ref_feat, images, all_relativeR, cen, lat.view(B, P, *lat.shape[1:]),
-                          refiner, k=k)
+                          refiner, k=k, **({} if hidden is None else {"hidden": hidden}))
 
 
 def _index(rows, device):
@@ -115,9 +116,12 @@ class PoseTracker:
     `min_iou` (or NaN) is lost: it is searched again in the same frame and its row replaced.  Reading the lost flags
     is one host read of the tracked rows' flags; min_iou = 0 turns the check off and removes that read.  The default
     0.5 is a guess that no real data has checked.  occluders: None or "detections" (each detection's occluders are
-    the other detections of its frame, as predict_pose_frames computes them, over all detections of the call)."""
+    the other detections of its frame, as predict_pose_frames computes them, over all detections of the call).
+    occluded_search: the searches and the tracking steps also leave out what those occluders may hide (DESIGN.md
+    section 27); it needs occluders="detections"."""
 
-    def __init__(self, model, bank, refiner, keep=2, k=5, min_iou=0.5, refine=None, occluders=None):
+    def __init__(self, model, bank, refiner, keep=2, k=5, min_iou=0.5, refine=None, occluders=None,
+                 occluded_search=False):
         from .bank import TemplateBank
         if model.dist is not None:
             raise NotImplementedError("PoseTracker does not shard across GPUs: it runs on one device (unset "
@@ -134,7 +138,10 @@ class PoseTracker:
             raise ValueError(f"refine must be None or 'contour', got {refine!r}")
         if occluders is not None and not (isinstance(occluders, str) and occluders == "detections"):
             raise ValueError(f"occluders must be None or 'detections', got {occluders!r}")
+        if occluded_search and occluders is None:
+            raise ValueError("occluded_search=True needs occluders='detections'")
         self.model, self.bank, self.refiner = model, bank, refiner
+        self._occluded = {"occluded_search": True} if occluded_search else {}
         self.keep, self.k, self.min_iou = int(keep), int(k), float(min_iou)
         self.refine, self.occluders = refine, occluders
         self.tracks = {}            # track id -> (obj_id, R [keep, 3, 3] float64 on the model's device)
@@ -147,7 +154,7 @@ class PoseTracker:
         return self.model.predict_pose_frames(
             frames, _rows(masks, rows, B), _rows(K, rows, B), [ids[b] for b in rows], k=self.k, refiner=self.refiner,
             refine=self.refine, frame_idx=_frame_rows(frame_idx, rows, B), occluders=_rows(occ, rows, B),
-            bank=self.bank)
+            bank=self.bank, **self._occluded)
 
     @torch.no_grad()
     def step(self, frames, masks, K, obj_ids, track_ids, frame_idx=None):
@@ -189,7 +196,7 @@ class PoseTracker:
             out = self.model.track_pose_frames(
                 frames, _rows(masks, known, B), Kh[known], [ids[b] for b in known], prior, self.refiner,
                 bank=self.bank, k=self.k, refine=self.refine, frame_idx=_frame_rows(fi, known, B),
-                occluders=_rows(occ, known, B))
+                occluders=_rows(occ, known, B), **self._occluded)
             lost = []
             if self.min_iou > 0:
                 ok = (out["iou"].amax(dim=1) >= self.min_iou).cpu().tolist()    # the one host read per frame

@@ -84,24 +84,40 @@ class SweepEngine:
         self._handle()
         self._native.call("profile", 1 if enable else 0)
 
-    def sweep(self, ref_feat, poses, query_feat=None, want_emb=True, want_sim=None, k=0, idx_base=0, out=None):
+    def sweep(self, ref_feat, poses, query_feat=None, want_emb=True, want_sim=None, k=0, idx_base=0, out=None,
+              query_visible=None):
         """ref_feat [B,C,32,32], poses [B,N,6] (+ query_feat [B,C,32,32]) ->
         dict(emb [B,N,C,32,32] | None, sim [B,N] | None, topv/topi [B,k] | None).
         query_feat may also be [B,Q,C,32,32]: Q queries per reference share the one sweep and
         sim is [B,Q,N], topv/topi [B,Q,k].
         `out` may carry preallocated contiguous `sim` / `topv` / `topi` tensors to write into (the
-        multi-GPU path points them into its all-gather record)."""
+        multi-GPU path points them into its all-gather record).
+        query_visible (uint8 or bool, the query's leading shape + [32, 32], DESIGN.md section 27): each row scores
+        only the latent pixels its map marks non-zero (nope_*_sweep_visible)."""
         if not self._native.finalized:
             raise _lib.NopeError("load_state_dict() must be called before the sweep")
         dev = self.device
+        if query_visible is not None and query_feat is None:
+            raise ValueError("query_visible needs query_feat")
         ref_feat, poses, query_feat, Q, emb, sim, topv, topi = stage_sweep(self, ref_feat, poses, query_feat,
                                                                            want_emb, want_sim, k, out)
         B, N = poses.shape[0], poses.shape[1]
+        if query_visible is not None:
+            lead = tuple(query_feat.shape[:-3])
+            if query_visible.dtype not in (torch.uint8, torch.bool) or tuple(query_visible.shape) != lead + (32, 32):
+                raise ValueError(f"query_visible {lead + (32, 32)} uint8 or bool expected, got "
+                                 f"{tuple(query_visible.shape)} {query_visible.dtype}")
+            query_visible = query_visible.to(dev).to(torch.uint8).contiguous()
         self._reserve(min(self._chunk, B * N), B, B * Q * N if query_feat is not None else 0)
         with torch.cuda.device(dev):
-            self._native.call("sweep_multi", _lib.ptr(ref_feat), _lib.ptr(poses), B, N, _lib.ptr(query_feat), Q,
-                              _lib.ptr(emb), _lib.ptr(sim), k, _lib.ptr(topv), _lib.ptr(topi), idx_base,
-                              _lib.stream(dev))
+            if query_visible is None:
+                self._native.call("sweep_multi", _lib.ptr(ref_feat), _lib.ptr(poses), B, N, _lib.ptr(query_feat), Q,
+                                  _lib.ptr(emb), _lib.ptr(sim), k, _lib.ptr(topv), _lib.ptr(topi), idx_base,
+                                  _lib.stream(dev))
+            else:
+                self._native.call("sweep_visible", _lib.ptr(ref_feat), _lib.ptr(poses), B, N, _lib.ptr(query_feat),
+                                  Q, _lib.ptr(query_visible), _lib.ptr(emb), _lib.ptr(sim), k, _lib.ptr(topv),
+                                  _lib.ptr(topi), idx_base, _lib.stream(dev))
         return {"emb": emb, "sim": sim, "topv": topv, "topi": topi}
 
     def __call__(self, x, pose):
